@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — the hot path of BASELINE.json's metric on synthetic corpora of the named shape.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload h1|h1c|v1|t1|v2] [--batch B]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload h1|h1c|v1|t1|v2] [--batch B] [--dump-outputs DIR]
     python bench.py --impl reference ...      # the CPU restatement (oracle) on the host cores
 
 A "step" = one pass of the hot path over one batch of B queries through the C ABI
@@ -13,8 +13,11 @@ query batches rotate through the timed loop (no step replays the previous step's
           K calls bracketed by barrier + device synchronize, max over ranks.
 Under torchrun (N>1) the corpus is sharded by document across ranks (strong scaling: the
 named corpus is fixed); one NCCL all-gather of per-shard top-k per batch, merged on device.
-The matrix (3.07 GB at 1M x 768) is far larger than L2 (126 MB), so no L2 flush is needed
-between iterations.
+The matrix (3.07 GB at 1M x 768) is far larger than the H100's L2 (50 MB), so no L2 flush is
+needed between iterations.
+--dump-outputs DIR: after the timed loop, the arrays the last timed step returned to its caller
+(doc ids, scores, hit counts, total matches; rank 0) are written as DIR/<name>.npy in float64 /
+float32.  The inputs are seeded, so two builds can be compared output for output.
 After the timed region (never inside it): parity of the timed queries against the CPU oracle
 (at every N: rank 0 runs the oracle on the UNSHARDED corpus and every rank's answer must be
 byte-identical to rank 0's), recall@10 against an fp64 evaluation on >= 1000 queries, the CPU
@@ -56,11 +59,8 @@ WORKLOADS = {
 # oc_timing.scan_variant (include/oramacore_b200.h OC_SCAN_*) -> (kernel, description)
 SCAN_VARIANTS = {
     0: ("emb_scan_kernel", "exact fp32 sweep"),
-    1: ("emb_gemm_kernel", "tcgen05 kind::tf32 on the fp32 rows + exact fp32 re-score"),
-    2: ("emb_gemm_pair_kernel", "tcgen05 cta_group::2 kind::tf32 on the fp32 rows + exact fp32 re-score"),
-    3: ("emb_gemm_cvt_kernel", "tcgen05 cta_group::2 kind::f16, fp32 rows streamed once and rounded to bf16 in the SM, + exact fp32 re-score"),
-    4: ("emb_gemm_kernel", "tcgen05 kind::f16 on the bf16 rows + exact fp32 re-score"),
-    5: ("emb_gemm_pair_kernel", "tcgen05 cta_group::2 kind::f16 on the bf16 rows + exact fp32 re-score"),
+    1: ("emb_gemm_kernel", "wgmma .tf32 on the fp32 rows + exact fp32 re-score"),
+    4: ("emb_gemm_kernel", "wgmma .bf16 on the bf16 rows + exact fp32 re-score"),
 }
 METRIC = {"h1": "hybrid_search_qps_at_recall10_ge_0.99_1Mx768", "h1c": "hybrid_search_qps_clustered_1Mx768"}
 
@@ -78,6 +78,8 @@ def parse():
     ap.add_argument("--recall-queries", type=int, default=1024, help="queries of the fp64 recall check")
     ap.add_argument("--no-cpu-baseline", action="store_true", help="skip oracle parity, recall and the CPU baseline")
     ap.add_argument("--no-extra", action="store_true", help="skip the configs[1] sub-result of the h1 line")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32 / float64)")
     return ap.parse_args()
 
 
@@ -85,11 +87,12 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p)), "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s — not measured
+    return {"hbm_gbs": 3350.0, "bf16_tflops_sustained": 989.0}, "fallback"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -287,6 +290,17 @@ def recall_hits(got_docs, exp_docs, exp_scores, got_scores):
     return hit, len(exp_docs)
 
 
+def dump_outputs(out_dir, res):
+    """The arrays one oc_search call hands its caller: doc ids (exact in float64 below 2^53), scores,
+    hits returned and total matches per query.  A few KB to a few MB: well under 64 MB at any batch."""
+    docs, scores, n, cnt = res
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "doc_ids.npy"), docs.astype(np.float64))
+    np.save(os.path.join(out_dir, "scores.npy"), scores.astype(np.float32))
+    np.save(os.path.join(out_dir, "n_hits.npy"), n.astype(np.float64))
+    np.save(os.path.join(out_dir, "count.npy"), cnt.astype(np.float64))
+
+
 def main():
     args = parse()
     w = dict(WORKLOADS[args.workload])
@@ -400,6 +414,8 @@ def main():
         if last[nb] is None:
             last[nb] = step(nb)
 
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last[(args.steps - 1) % N_BATCHES])
     dev_ms, scan_ms, bm_ms, fuse_ms, comm_ms, sweep_ms = (acc[k] for k in ("device_ms", "scan_ms", "bm25_ms", "fuse_ms", "comm_ms", "scan_sweep_ms"))
     ranks_agree = None
     if world > 1:
@@ -431,7 +447,7 @@ def main():
     pk, peak_src = peaks()
     peak = float(pk["hbm_gbs"])
     cfg = config_of(w, B, n_docs)
-    cfg.update({"parallelism": f"doc-shard x{world}", "l2_flush": "inputs larger than L2 (matrix >> 126 MB)"})
+    cfg.update({"parallelism": f"doc-shard x{world}", "l2_flush": "inputs larger than L2 (matrix >> 50 MB)"})
     line = {
         "metric": METRIC.get(args.workload, f"{w['mode']}_search_qps"),
         "value": value, "unit": "queries/s", "n_gpus": world, "steps": K, "warmup": n_warm,
@@ -445,10 +461,6 @@ def main():
         "stage_ms_per_step": {"scan": scan_ms / K, "scan_sweep_kernel": sweep_ms / K, "bm25": bm_ms / K, "fuse": fuse_ms / K, "comm": comm_ms / K},
     }
     # roofline of the dominant kernel
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tpath):
-        traffic = json.load(open(tpath)).get(args.workload)
     scan_bytes, scan_launches, postings = acc["scan_bytes"], acc["scan_launches"], acc["bm25_postings"]
     if w["dim"]:   # vector / hybrid: the matrix sweep is the dominant kernel (the fulltext stage overlaps it on the side stream)
         # dominant kernel = the sweep launch(es): CUDA events around those launches on the library's stream
@@ -463,26 +475,26 @@ def main():
                         "rows_rescored_exactly_per_query": acc["scan_rescored"] / K,
                         "tensor_tflops_per_gpu": tflops}
         if tensor_core and w.get("dtype") == "bf16" and B >= 512:
-            tpeak = float(pk.get("bf16_tflops_sustained", 1400.0))
+            tpeak = float(pk.get("bf16_tflops_sustained", 989.0))
             line["roofline_tensor"] = {"kernel": kname, "bound": "tensor", "achieved": tflops, "peak": tpeak,
                                        "unit": "TFLOP/s", "frac": tflops / tpeak,
                                        "peak_source": f"of {peak_src} (sustained)"}
         line["roofline"] = {"kernel": kname, "bound": "hbm", "achieved": ach, "peak": peak,
-                            "unit": "GB/s", "frac": ach / peak, "traffic": traffic, "peak_source": f"of {peak_src}",
+                            "unit": "GB/s", "frac": ach / peak, "peak_source": f"of {peak_src}",
                             "kernel_ms_per_launch": sweep_ms / max(scan_launches, 1), "launches_per_step": scan_launches / K,
                             "algorithmic_bytes_per_launch": scan_bytes / max(scan_launches, 1),
                             "batch_level_frac": (scan_bytes / max(scan_launches, 1) * K / 1e9) / (scan_ms * 1e-3) / peak}
     else:
         ach = (postings * 8 / 1e9) / (bm_ms * 1e-3)
         line["roofline"] = {"kernel": "bm25_warp_kernel (whole fulltext stage timed: plan + precompute + seed + scorer)", "bound": "hbm", "achieved": ach, "peak": peak,
-                            "unit": "GB/s", "frac": ach / peak, "traffic": traffic, "peak_source": f"of {peak_src}",
+                            "unit": "GB/s", "frac": ach / peak, "peak_source": f"of {peak_src}",
                             "postings_per_s": postings / (bm_ms * 1e-3)}
     if w["dim"] and w["vocab"] and postings:
         line["roofline_bm25"] = {"kernel": "bm25_warp_kernel (whole fulltext stage timed)", "bound": "hbm", "achieved": (postings * 8 / 1e9) / (bm_ms * 1e-3),
                                  "peak": peak, "unit": "GB/s", "frac": (postings * 8 / 1e9) / (bm_ms * 1e-3) / peak,
                                  "postings_per_s": postings / (bm_ms * 1e-3), "stage_ms": bm_ms / K,
                                  "note": "the fulltext stage runs on the side stream under the matrix sweep: its window includes the wait for "
-                                         "the SMs' shared memory the sweep holds (OC_SIDE_STREAM=0 times it alone: profiles/)"}
+                                         "the SMs' shared memory the sweep holds (OC_SIDE_STREAM=0 times it alone)"}
 
     def hits_of(raw, i):
         return ob.SearchHits(raw[0][i, :raw[2][i]].copy(), raw[1][i, :raw[2][i]].copy(), int(raw[3][i]))

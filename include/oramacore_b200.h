@@ -1,5 +1,5 @@
 /*
- * oramacore_b200.h — C ABI of the B200-native OramaCore search hot path.
+ * oramacore_b200.h — C ABI of the H100-native (sm_90a) OramaCore search hot path.
  *
  * The reference (oramasearch/oramacore @ 666ab48) has no plugin / FFI boundary for this
  * path: the seam is Rust-to-Rust (SURVEY.md §8b).  Each entry point below names the
@@ -7,7 +7,7 @@
  * pointers and sizes only; all `out_*` buffers are caller-allocated HOST memory; the
  * library owns every device allocation behind the opaque handles.  The shared library
  * (liboramacore_b200.so) is CUDA-only: there is no CPU fallback, every call fails with
- * OC_ERR_CUDA when no sm_100-class device is usable.
+ * OC_ERR_CUDA when no sm_90 device is usable.
  *
  * Status: 0 = OC_OK, <0 = error; text via oc_last_error() (thread-local, valid until the
  * next call on that thread).  Handles are Send+Sync: calls on one ctx are serialised
@@ -340,7 +340,7 @@ typedef struct {
     uint64_t scan_bytes;     /* algorithmic bytes swept by the scan kernels (rows x stride x elem) */
     uint64_t bm25_postings;  /* postings walked by the scorer (x8 B = algorithmic bytes)    */
     uint64_t h2d_bytes, d2h_bytes;
-    uint32_t scan_tensor_core;   /* 1 => the batched tcgen05 (tf32 select + exact re-score) scan ran */
+    uint32_t scan_tensor_core;   /* 1 => the batched wgmma (tf32/bf16 select + exact re-score) scan ran */
     uint32_t scan_unproven;      /* queries whose candidate buffers overflowed in the tensor-core scan and were
                                     re-run through the exact sweep (device_ms includes that re-run)     */
     uint32_t scan_variant;       /* OC_SCAN_*: which sweep kernel served the batch                      */
@@ -349,11 +349,8 @@ typedef struct {
     uint32_t scan_rescored;      /* rows re-scored in exact fp32 per query (batch average) by the tensor-core scan */
 } oc_timing;
 #define OC_SCAN_EXACT 0          /* emb_scan_kernel: exact fp32 sweep (B < 8, limit > 32, tiny stores)          */
-#define OC_SCAN_TC_TF32 1        /* emb_gemm_kernel: kind::tf32 on the fp32 rows, one CTA per SM               */
-#define OC_SCAN_TC_TF32_PAIR 2   /* emb_gemm_pair_kernel: same, CTA pairs (cta_group::2)                       */
-#define OC_SCAN_TC_CVT_PAIR 3    /* emb_gemm_cvt_kernel: fp32 rows rounded to bf16 in the SM, kind::f16, pairs */
-#define OC_SCAN_TC_BF16 4        /* emb_gemm_kernel on a bf16 store (kind::f16)                                */
-#define OC_SCAN_TC_BF16_PAIR 5   /* emb_gemm_pair_kernel on a bf16 store                                       */
+#define OC_SCAN_TC_TF32 1        /* emb_gemm_kernel: wgmma .tf32 on the fp32 rows, one CTA per SM and query group */
+#define OC_SCAN_TC_BF16 4        /* emb_gemm_kernel on a bf16 store (wgmma .bf16)                                */
 int oc_last_timing(oc_ctx *ctx, oc_timing *out);
 /* Total kernels this library has launched on ctx since oc_init. */
 uint64_t oc_launch_count(oc_ctx *ctx);

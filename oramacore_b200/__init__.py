@@ -1,4 +1,4 @@
-"""oramacore_b200 — B200-native (sm_100a) implementation of OramaCore's search hot path:
+"""oramacore_b200 — H100-native (sm_90a) implementation of OramaCore's search hot path:
 embedding scan + BM25F posting scorer + hybrid fusion/top-k behind the reference's
 search() surface (mode = fulltext | vector | hybrid).  CUDA only; no CPU fallback."""
 from .types import (FieldPostings, StringIndexData, TextQuery, SearchHits, MODE_FULLTEXT, MODE_VECTOR,

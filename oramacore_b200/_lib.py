@@ -1,7 +1,7 @@
 """ctypes binding of liboramacore_b200.so (the C ABI in include/oramacore_b200.h).
 
 The library is CUDA-only.  Loading succeeds on a CPU box (symbols resolve; used by the
-`not gpu` tests), every compute call fails loudly with OcError when no sm_100 device is
+`not gpu` tests), every compute call fails loudly with OcError when no sm_90 device is
 present — there is no CPU fallback anywhere in this package.
 """
 from __future__ import annotations
@@ -85,7 +85,7 @@ class Timing(C.Structure):
 
 
 def build(force: bool = False) -> str:
-    """Compile the shared library in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+    """Compile the shared library in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
     srcs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cu", ".cuh", ".h"))]
     srcs.append(os.path.join(_HERE, "..", "include", "oramacore_b200.h"))
     stale = (not os.path.exists(SO_PATH)) or any(os.path.getmtime(s) > os.path.getmtime(SO_PATH) for s in srcs)
@@ -105,7 +105,7 @@ def lib():
     if _lib is not None:
         return _lib
     if not os.path.exists(SO_PATH):
-        raise OcError(-2, f"{SO_PATH} is missing: run __graft_entry__.build() (nvcc, sm_100a). "
+        raise OcError(-2, f"{SO_PATH} is missing: run __graft_entry__.build() (nvcc, sm_90a). "
                           "There is no CPU fallback.")
     L = C.CDLL(SO_PATH)
     vp, u32, u64, f32, i32 = C.c_void_p, C.c_uint32, C.c_uint64, C.c_float, C.c_int

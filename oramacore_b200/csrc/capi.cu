@@ -1,5 +1,5 @@
 // capi.cu — host side of liboramacore_b200.so: the C ABI declared in
-// include/oramacore_b200.h over the sm_100a kernels (emb_scan.cuh, bm25.cuh, fuse.cuh).
+// include/oramacore_b200.h over the sm_90a kernels (emb_scan.cuh, bm25.cuh, fuse.cuh).
 // No torch, no CPU fallback: every entry point needs a live CUDA device.
 #include <cuda_runtime.h>
 
@@ -139,7 +139,6 @@ struct oc_ctx {
     cudaStream_t side = nullptr;      // descriptor upload + BM25 plan/precompute while the main stream sweeps the matrix
     cudaEvent_t ev_side = nullptr;
     bool sweep_timed = false;         // EV_SWEEP0/1 recorded in this call (tensor-core path)
-    uint32_t cvt_stages_default = 5;  // run_vector_stage: ring depth of the converting sweep when the caller has no preference
     bool rerun_timed = false;         // EV_RR0/1 recorded: flagged queries were re-run through the exact sweep
     bool side_dirty = false;          // work was queued on the side stream and not yet joined (an error path returned early)
     cudaDeviceProp prop{};
@@ -183,10 +182,10 @@ extern "C" int oc_init(int device_id, oc_ctx **out) {
     oc_ctx *c = new oc_ctx();
     c->device = device_id;
     CU(cudaGetDeviceProperties(&c->prop, device_id));
-    if (c->prop.major < 10) {
+    if (c->prop.major != 9 || c->prop.minor != 0) {   // sm_90a code (wgmma) runs on sm_90 devices only
         int mj = c->prop.major, mn = c->prop.minor;
         delete c;
-        return fail(OC_ERR_CUDA, "device sm_%d%d is not sm_100-class; kernels are built for sm_100a only", mj, mn);
+        return fail(OC_ERR_CUDA, "device sm_%d%d is not sm_90; kernels are built for sm_90a only", mj, mn);
     }
     CU(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
     CU(cudaStreamCreateWithFlags(&c->side, cudaStreamNonBlocking));
@@ -303,7 +302,6 @@ struct oc_emb {
     uint32_t esz = 4;            // element bytes
     float *inv_norm = nullptr;   // [cap] (NaN = tombstone)
     uint64_t *row_doc = nullptr; // [cap]
-    float *rho_x = nullptr;      // device scalar: max over rows of |x - bf16(x)| / |x| (fp32 stores; the sweep's error bound)
     uint64_t n_rows = 0, cap = 0, n_live = 0;
     std::unordered_multimap<uint64_t, uint64_t> doc_rows;  // doc -> rows (for delete)
 };
@@ -317,13 +315,6 @@ extern "C" int oc_emb_create(oc_ctx *c, uint32_t dim, int dtype, int rescale_e5,
     e->esz = dtype == OC_DTYPE_BF16 ? 2 : 4;
     e->stride = ((dim + 127) / 128) * 128;
     if (e->stride / 128 == 5 || e->stride / 128 == 7) e->stride += 128;  // instantiated widths: 1,2,3,4,6,8
-    {
-        std::lock_guard<std::mutex> g(c->mu);
-        if (cudaSetDevice(c->device) != cudaSuccess || cudaMalloc(&e->rho_x, 4) != cudaSuccess || cudaMemset(e->rho_x, 0, 4) != cudaSuccess) {
-            delete e;
-            return fail(OC_ERR_CUDA, "oc_emb_create: device allocation failed");
-        }
-    }
     *out = e;
     return OC_OK;
 }
@@ -332,7 +323,7 @@ extern "C" void oc_emb_destroy(oc_emb *e) {
     if (!e) return;
     cudaSetDevice(e->ctx->device);
     cudaStreamSynchronize(e->ctx->stream);
-    cudaFree(e->rows); cudaFree(e->inv_norm); cudaFree(e->row_doc); cudaFree(e->rho_x);
+    cudaFree(e->rows); cudaFree(e->inv_norm); cudaFree(e->row_doc);
     delete e;
 }
 
@@ -378,9 +369,8 @@ extern "C" int oc_emb_insert(oc_emb *e, const uint64_t *doc_ids, const void *row
     CU(cudaMemcpyAsync(e->row_doc + e->n_rows, doc_ids, n * sizeof(uint64_t), cudaMemcpyHostToDevice, c->stream));
     const uint64_t warps_per_block = 8;
     const uint64_t blocks = (n + warps_per_block - 1) / warps_per_block;
-    if (e->esz == 2) emb_inv_norm_kernel<bf16_t><<<(unsigned)blocks, 256, 0, c->stream>>>(e->rows, e->stride, e->n_rows, e->n_rows + n, e->inv_norm, nullptr);
-    else emb_inv_norm_kernel<float><<<(unsigned)blocks, 256, 0, c->stream>>>(e->rows, e->stride, e->n_rows, e->n_rows + n, e->inv_norm,
-                                                                             reinterpret_cast<unsigned int *>(e->rho_x));
+    if (e->esz == 2) emb_inv_norm_kernel<bf16_t><<<(unsigned)blocks, 256, 0, c->stream>>>(e->rows, e->stride, e->n_rows, e->n_rows + n, e->inv_norm);
+    else emb_inv_norm_kernel<float><<<(unsigned)blocks, 256, 0, c->stream>>>(e->rows, e->stride, e->n_rows, e->n_rows + n, e->inv_norm);
     launched(c);
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(c->stream));
@@ -516,9 +506,7 @@ static int run_exact_sweeps(oc_ctx *c, oc_emb *e, const float *inv_norm, const f
 typedef CUresult (*EncodeTiled_t)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
                                   const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-// sw64: bf16 matrix, 32-element (64-byte) boxes in the SWIZZLE_64B layout (operand of the converting sweep)
-static int make_tmap_2d(CUtensorMap *m, const void *base, uint64_t n_rows, uint32_t stride, uint32_t box_rows, bool bf16,
-                        bool sw64 = false) {
+static int make_tmap_2d(CUtensorMap *m, const void *base, uint64_t n_rows, uint32_t stride, uint32_t box_rows, bool bf16) {
     static EncodeTiled_t fn = nullptr;
     if (!fn) {
         void *f = nullptr;
@@ -529,17 +517,13 @@ static int make_tmap_2d(CUtensorMap *m, const void *base, uint64_t n_rows, uint3
     }
     cuuint64_t dims[2] = {stride, n_rows};
     cuuint64_t strides[1] = {cuuint64_t(stride) * (bf16 ? 2 : 4)};
-    cuuint32_t box[2] = {(bf16 && !sw64) ? 2 * GEMM_KB : GEMM_KB, box_rows};   // 128 bytes of K (64 when sw64)
+    cuuint32_t box[2] = {bf16 ? 2 * GEMM_KB : GEMM_KB, box_rows};   // 128 bytes of K
     cuuint32_t estr[2] = {1, 1};
-    // L2 promotion granule = the 128-byte box row: with 256 B every tile load also pulled the neighbouring
-    // K-block into L2, and the converting sweep re-fetched 17 % of the matrix from DRAM (ncu: 3.59 GB read
-    // vs 3.12 GB with 128 B; algorithmic 3.08 GB).  OC_TMA_PROMO=256|none: profiling switch.
-    const char *penv = getenv("OC_TMA_PROMO");
-    const CUtensorMapL2promotion promo = !penv ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B
-                                         : penv[0] == '2' ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B
-                                         : penv[0] == 'n' ? CU_TENSOR_MAP_L2_PROMOTION_NONE : CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
+    // L2 promotion granule = the 128-byte box row: a larger granule would also pull the neighbouring K-block
+    // of the row into L2, which another CTA's load may evict before it is used (extra DRAM reads)
+    const CUtensorMapL2promotion promo = CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
     CUresult r = fn(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void *>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, sw64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, promo,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, promo,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(OC_ERR_CUDA, "cuTensorMapEncodeTiled failed: %d", (int)r);
     return OC_OK;
@@ -590,78 +574,48 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
     CU(cudaEventRecord(c->ev[EV_SCAN0], c->stream));
     if (!use_gemm) return run_exact_sweeps(c, e, inv_norm, c->q_pad.as<float>(), c->q_inv.as<float>(), B, limit, similarity, out);
 
-    // ---------------- K2: tcgen05 batched scan ----------------
+    // ---------------- K2: wgmma batched scan ----------------
     const bool bf16 = e->esz == 2;
-    // NG = 2: one CTA serves two query groups against each staged X tile (one copy of X per 256 queries)
-    const int NG = n_qgroups >= 2 ? 2 : 1;
-    const uint32_t n_super = NG == 1 ? n_qgroups : (n_qgroups + 1) / 2;
-    // CTA pairs (cta_group::2): two SMs share one 256-query x 512-row tile (25 % less L2->SM traffic)
-    const char *penv = getenv("OC_GEMM_PAIR");
-    const uint32_t n_pairs = c->prop.multiProcessorCount / 2;
-    // default: fp32 stores only (there the pair feeds the converting sweep); for bf16 stores the pair kernel
-    // measured ~4 % slower than two groups per CTA on the tensor-bound 10M x 1024 workload (OC_GEMM_PAIR=1 forces it)
-    const bool pair_wanted = penv ? penv[0] == '1' : e->esz == 4;
-    const bool pair = NG == 2 && pair_wanted && !(penv && penv[0] == '0') && n_pairs >= n_super;
-    const uint32_t cpg = pair ? std::max<uint32_t>(1, n_pairs / n_super)
-                              : std::max<uint32_t>(1, c->prop.multiProcessorCount / n_super);
-    const uint32_t grid = pair ? 2 * cpg * n_super : cpg * n_super;
-    const uint32_t lists = (NG == 1 || pair) ? cpg * 2 : cpg;
-    if (lists > 512) return fail(OC_ERR_UNSUPPORTED, "%u candidate lists per query (> 512)", lists);
-    // fp32 store, pair path: convert the operands to bf16 inside the SM (kind::f16 at twice the tf32 rate)
-    const char *cenv = getenv("OC_GEMM_CVT");
-    const bool cvt = pair && !bf16 && !(cenv && cenv[0] == '0');
+    // one CTA per SM and query group; the merge gathers at most 512 lists per query
+    const uint32_t cpg = std::min<uint32_t>(512 / GEMM_LISTS_PER_CTA,
+                                            std::max<uint32_t>(1, c->prop.multiProcessorCount / n_qgroups));
+    const uint32_t grid = cpg * n_qgroups;
+    const uint32_t lists = cpg * GEMM_LISTS_PER_CTA;
     const uint32_t cap = GEMM_LIST_CAP;
-    const uint32_t Bpad2 = n_super * NG * GEMM_M;   // query rows the kernel may address (TMA zero-fills beyond the tensor)
     CUtensorMap tm_q, tm_x;
     const void *q_operand = c->q_pad.p;
-    if (bf16 || cvt) {   // the sweep's query operand in the store's dtype (the exact re-score keeps the fp32 query)
+    if (bf16) {   // the sweep's query operand in the store's dtype (the exact re-score keeps the fp32 query)
         OCTRY(c->q_bf16.ensure(size_t(Bpad) * e->stride * 2));
         const size_t nq_el = size_t(Bpad) * e->stride;
         f32_to_bf16_kernel<<<(unsigned)((nq_el + 255) / 256), 256, 0, c->stream>>>(c->q_pad.as<float>(), c->q_bf16.as<uint16_t>(), nq_el);
         launched(c);
         q_operand = c->q_bf16.p;
     }
-    OCTRY(make_tmap_2d(&tm_q, q_operand, Bpad, e->stride, GEMM_M, bf16 || cvt, cvt));
-    OCTRY(make_tmap_2d(&tm_x, e->rows, e->n_rows, e->stride, pair ? 128 : GEMM_N, bf16));
+    OCTRY(make_tmap_2d(&tm_q, q_operand, Bpad, e->stride, GEMM_M, bf16));
+    OCTRY(make_tmap_2d(&tm_x, e->rows, e->n_rows, e->stride, GEMM_N, bf16));
     OCTRY(c->g_thr.ensure(size_t(B) * 4));
     OCTRY(c->g_eps.ensure(size_t(B) * 4));
-    OCTRY(c->g_cand.ensure(size_t(Bpad2) * lists * cap * 8));
-    OCTRY(c->g_cnt.ensure(size_t(Bpad2) * lists * 4));
+    OCTRY(c->g_cand.ensure(size_t(Bpad) * lists * cap * 8));
+    OCTRY(c->g_cnt.ensure(size_t(Bpad) * lists * 4));
     OCTRY(c->g_ovf.ensure(size_t(B) * GEMM_OVF_CAP * 8));
     OCTRY(c->g_ovfcnt.ensure(size_t(B) * 4));
     OCTRY(c->g_resc.ensure(size_t(B) * 4));
     OCTRY(c->g_flag.ensure(B));
-    OCTRY(c->g_max.ensure(size_t(Bpad2) * lists * 4));
+    OCTRY(c->g_max.ensure(size_t(Bpad) * lists * 4));
     GemmParams gp{};
-    gp.n_rows = e->n_rows; gp.n_kblocks = e->stride / (bf16 ? 2 * GEMM_KB : GEMM_KB); gp.inv_norm = inv_norm; gp.n_queries = B;   // cvt: 32-element K-blocks too
+    gp.n_rows = e->n_rows; gp.n_kblocks = e->stride / (bf16 ? 2 * GEMM_KB : GEMM_KB); gp.inv_norm = inv_norm; gp.n_queries = B;
     gp.n_qgroups = n_qgroups; gp.ctas_per_group = cpg; gp.cap = cap; gp.lists_per_query = lists;
     gp.thr = c->g_thr.as<unsigned int>(); gp.eps_v = c->g_eps.as<float>(); gp.limit = limit; gp.cand = c->g_cand.as<uint64_t>(); gp.cand_cnt = c->g_cnt.as<uint32_t>();
     gp.gmax = c->g_max.as<float>();
     gp.ovf = c->g_ovf.as<uint64_t>(); gp.ovf_cnt = c->g_ovfcnt.as<uint32_t>(); gp.ovf_cap = GEMM_OVF_CAP;
-    // ring depth of the converting sweep: 5 stages alone on the SM; 4 stages (OC_CVT_STAGES=4) leave ~60 KB of shared
-    // memory so one CTA of the BM25 tile scorer (side stream) can co-reside and use the issue slots the HBM-bound sweep leaves idle
-    const char *stenv = getenv("OC_CVT_STAGES");
-    const uint32_t cvt_stages = (stenv && stenv[0] == '4') ? 4 : (stenv && stenv[0] == '5') ? 5 : c->cvt_stages_default;
-    if (smem_cfg_needed(c->device, (const void *)emb_gemm_cvt_kernel<5>, gemm_cvt_smem_bytes(5))) {   // all sweep variants at once
-        CU(cudaFuncSetAttribute(emb_gemm_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes(1)));
-        CU(cudaFuncSetAttribute(emb_gemm_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes(2)));
-        CU(cudaFuncSetAttribute(emb_gemm_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes(1)));
-        CU(cudaFuncSetAttribute(emb_gemm_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes(2)));
-        CU(cudaFuncSetAttribute(emb_gemm_pair_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_pair_smem_bytes()));
-        CU(cudaFuncSetAttribute(emb_gemm_pair_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_pair_smem_bytes()));
-        CU(cudaFuncSetAttribute(emb_gemm_cvt_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_cvt_smem_bytes(5)));
-        CU(cudaFuncSetAttribute(emb_gemm_cvt_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_cvt_smem_bytes(4)));
+    if (smem_cfg_needed(c->device, (const void *)emb_gemm_kernel<false>, gemm_smem_bytes())) {   // all sweep kernels at once
+        CU(cudaFuncSetAttribute(emb_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes()));
+        CU(cudaFuncSetAttribute(emb_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes()));
         CU(cudaFuncSetAttribute(emb_gemm_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_merge_smem_bytes()));
     }
     auto launch_gemm = [&]() -> int {
-        if (cvt && cvt_stages == 4) emb_gemm_cvt_kernel<4><<<grid, CVT_THREADS, gemm_cvt_smem_bytes(4), c->stream>>>(tm_q, tm_x, gp);
-        else if (cvt) emb_gemm_cvt_kernel<5><<<grid, CVT_THREADS, gemm_cvt_smem_bytes(5), c->stream>>>(tm_q, tm_x, gp);
-        else if (pair && !bf16) emb_gemm_pair_kernel<false><<<grid, GEMM_THREADS, gemm_pair_smem_bytes(), c->stream>>>(tm_q, tm_x, gp);
-        else if (pair) emb_gemm_pair_kernel<true><<<grid, GEMM_THREADS, gemm_pair_smem_bytes(), c->stream>>>(tm_q, tm_x, gp);
-        else if (NG == 1 && !bf16) emb_gemm_kernel<1, false><<<grid, GEMM_THREADS, gemm_smem_bytes(1), c->stream>>>(tm_q, tm_x, gp);
-        else if (NG == 1) emb_gemm_kernel<1, true><<<grid, GEMM_THREADS, gemm_smem_bytes(1), c->stream>>>(tm_q, tm_x, gp);
-        else if (!bf16) emb_gemm_kernel<2, false><<<grid, GEMM_THREADS, gemm_smem_bytes(2), c->stream>>>(tm_q, tm_x, gp);
-        else emb_gemm_kernel<2, true><<<grid, GEMM_THREADS, gemm_smem_bytes(2), c->stream>>>(tm_q, tm_x, gp);
+        if (bf16) emb_gemm_kernel<true><<<grid, GEMM_THREADS, gemm_smem_bytes(), c->stream>>>(tm_q, tm_x, gp);
+        else emb_gemm_kernel<false><<<grid, GEMM_THREADS, gemm_smem_bytes(), c->stream>>>(tm_q, tm_x, gp);
         launched(c, gp.max_mode == 0);   // the one-tile threshold pass is not counted as a sweep
         CU(cudaGetLastError());
         return OC_OK;
@@ -671,9 +625,8 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
     OCTRY(launch_gemm());
     GemmThrParams tp{};
     tp.gmax = c->g_max.as<float>(); tp.lists = lists; tp.limit = limit; tp.inv_qnorm = c->q_inv.as<float>();
-    tp.eps_const = (bf16 || cvt) ? GEMM_EPS_ACC : GEMM_EPS_TF32;
-    tp.rho_x = cvt ? e->rho_x : nullptr;                          // bf16 store: the rows are exact
-    tp.rho_q = (bf16 || cvt) ? c->q_rho.as<float>() : nullptr;
+    tp.eps_const = bf16 ? GEMM_EPS_ACC : GEMM_EPS_TF32;
+    tp.rho_q = bf16 ? c->q_rho.as<float>() : nullptr;             // bf16 store: the rows are exact, the query is rounded
     tp.thr = c->g_thr.as<unsigned int>(); tp.eps_v = c->g_eps.as<float>(); tp.ovf_cnt = c->g_ovfcnt.as<uint32_t>();
     gemm_thr_kernel<<<B, 256, 0, c->stream>>>(tp);
     launched(c);
@@ -698,7 +651,7 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
     // the overflow flags travel back with the results; oc_*search re-runs flagged queries (fix_unproven)
     c->gemm_pending = true; c->gemm_inv_norm = inv_norm;
     c->timing.scan_tensor_core = 1;
-    c->timing.scan_variant = cvt ? OC_SCAN_TC_CVT_PAIR : bf16 ? (pair ? OC_SCAN_TC_BF16_PAIR : OC_SCAN_TC_BF16) : (pair ? OC_SCAN_TC_TF32_PAIR : OC_SCAN_TC_TF32);
+    c->timing.scan_variant = bf16 ? OC_SCAN_TC_BF16 : OC_SCAN_TC_TF32;
     return OC_OK;
 }
 
@@ -2002,8 +1955,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     {   // smallest power-of-two key buffer that takes the candidates in one round (sort cost ~ capb log^2 capb)
         const uint64_t total = (has_ft ? uint64_t(n_tiles) * n_keep : 0) + (has_v ? vlimit : 0);
         // up to 16 K keys (128 KB) stay in shared memory and go through one radix select; the streaming bitonic path behind
-        // it cost 0.44 ms per batch on the 10M-document fulltext workload (1221 tiles x 10 candidate slots per query:
-        // profiles/r02_ncu_fuse_t1.md)
+        // it is for larger candidate sets (the 10M-document fulltext workload has 1221 tiles x 10 candidate slots per query)
         fp.capb = next_pow2((uint32_t)std::min<uint64_t>(16384, std::max<uint64_t>(total, 2 * n_keep)));
         fp.capb = std::max<uint32_t>(fp.capb, std::max<uint32_t>(64, next_pow2(2 * n_keep)));
     }

@@ -1,23 +1,23 @@
-// emb_gemm.cuh — K2: batched-query embedding scan on the 5th-gen tensor cores.
+// emb_gemm.cuh — K2: batched-query embedding scan on the Hopper tensor cores (wgmma).
 //
 // Same contract as K1 (EmbeddingFieldStorage::search, read/index/embedding_field.rs:250-278)
 // but for a BATCH of queries, where the distance computation is a true dense GEMM
 // S[q][r] = sum_k Q[q][k] * X[r][k] (north_star: "tensor cores used only when batched
 // queries make the distance a true dense GEMM").  One matrix sweep serves the whole batch.
 //
-//   * operands: fp32 rows straight from HBM, consumed by tcgen05.mma kind::tf32 (the tensor
-//     core reads the fp32 bits and drops the low 13 mantissa bits) — no converted copy of
-//     the store, algorithmic bytes = n_rows * stride * 4 per batch; bf16 stores use kind::f16;
-//   * CTA tile: M = 128 queries (A operand) x N = 256 rows (B operand), K-blocks of 128 bytes
-//     = one swizzle row; TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B) fills the shared-memory
-//     ring, a single thread issues the tcgen05.mma into 128-lane x 256-column fp32
-//     accumulators in TMEM (all 512 columns: NG=1 double-buffers one group's accumulator across
-//     tiles, NG=2 holds one accumulator per query group so two groups share each X tile);
-//   * epilogue: 8 warps, thread = TMEM lane = ONE QUERY: tcgen05.ld the scores of the tile,
-//     scale by the row's inverse norm, threshold-gated push into that query's private
-//     candidate buffer; the threshold is the query's running K'-th best, seeded by a one-tile
-//     threshold pass of the same kernel and shared across CTAs through an atomicMax'd global
-//     array (any subset's K'-th best bounds the global one);
+//   * operands: fp32 rows straight from HBM, consumed by wgmma .tf32 (the tensor core reads the
+//     fp32 bits and drops the low 13 mantissa bits) — no converted copy of the store, algorithmic
+//     bytes = n_rows * stride * 4 per batch; bf16 stores use wgmma .bf16;
+//   * CTA tile: M = 128 queries (A operand, two consumer warpgroups of 64) x N = 128 rows (B operand),
+//     K-blocks of 128 bytes = one swizzle row; one producer warp fills a 4-stage shared-memory ring
+//     with TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B) under full / empty mbarriers, each consumer
+//     warpgroup issues wgmma.mma_async m64n128 into 64 fp32 accumulator registers per thread;
+//   * epilogue, straight from the accumulator registers: a thread holds 2 queries x 32 rows of the
+//     tile (wgmma's D fragment), scales them by the rows' inverse norms and pushes every row whose
+//     approximate score clears the query's threshold into a private candidate list — one list per
+//     (query, CTA, lane % 4); the threshold is the query's running K'-th best, seeded by a one-tile
+//     threshold pass of the same kernel and shared across CTAs through an atomicMax'd global array
+//     (any subset's K'-th best bounds the global one);
 //   * the sweep's scores are only used to SELECT candidates.  The merge kernel re-scores the
 //     best K' candidates per query in exact fp32 with K1's arithmetic (bit-identical scores) and
 //     PROVES the answer: every non-candidate row has approx <= max(final threshold, K'-th
@@ -25,9 +25,7 @@
 //     when the limit-th exact score clears bound + eps the exact top-`limit` is inside the
 //     candidate set.  Queries that fail the proof are re-run through the exact K1 sweep by the
 //     host (rare).
-//   * variants in this file: emb_gemm_kernel<NG, BF16> (one CTA per SM), emb_gemm_pair_kernel
-//     (cta_group::2 CTA pairs), emb_gemm_cvt_kernel (pairs + fp32 -> bf16 conversion inside the
-//     SM: the default for fp32 stores at B > 128), gemm_tau_from_max_kernel, emb_gemm_merge_kernel.
+//   * kernels in this file: emb_gemm_kernel<BF16>, gemm_thr_kernel, emb_gemm_merge_kernel.
 #pragma once
 #include <cuda.h>
 
@@ -35,15 +33,16 @@
 
 namespace oc {
 
-constexpr uint32_t GEMM_EPI_WARPS = 8;  // two warps per TMEM lane quadrant, each takes half of the tile's rows
-constexpr int GEMM_THREADS = 64 + GEMM_EPI_WARPS * 32;   // warp0: TMA producer, warp1: MMA issuer, warps 2-9: epilogue
+constexpr uint32_t GEMM_CONSUMER_WG = 2;                          // warpgroups issuing wgmma, 64 queries each
+constexpr int GEMM_THREADS = GEMM_CONSUMER_WG * 128 + 32;         // warps 0-7: consumers, warp 8: TMA producer
 constexpr uint32_t GEMM_M = 128;       // queries per CTA
-constexpr uint32_t GEMM_N = 256;       // rows per tile
+constexpr uint32_t GEMM_N = 128;       // rows per tile
 constexpr uint32_t GEMM_KB = 32;       // fp32 elements per K-block (one 128 B swizzle row); bf16 rows: 64
 constexpr uint32_t GEMM_STAGES = 4;
 constexpr uint32_t GEMM_A_BYTES = GEMM_M * 128;   // 16 KB
-constexpr uint32_t GEMM_B_BYTES = GEMM_N * 128;   // 32 KB
+constexpr uint32_t GEMM_B_BYTES = GEMM_N * 128;   // 16 KB
 constexpr uint32_t GEMM_STAGE_BYTES = GEMM_A_BYTES + GEMM_B_BYTES;
+constexpr uint32_t GEMM_LISTS_PER_CTA = 4;        // candidate lists per (query, CTA): one per lane % 4 of the D fragment
 constexpr uint32_t GEMM_LIST_CAP = 128;           // entries of one (query, list) candidate buffer
 constexpr uint32_t GEMM_OVF_CAP = 2048;           // per-query spill area shared by its lists (global atomics; rare)
 constexpr uint32_t GEMM_MERGE_BUF = 4096;         // keys the merge kernel holds in shared memory
@@ -56,18 +55,16 @@ constexpr uint32_t GEMM_MAX_LIMIT = 128;          // largest `limit` the tensor-
 // rounding of the exact fp32 re-score it is compared with (<= 1024 x 2^-24, twice): GEMM_EPS_ACC.
 //   tf32: the tensor core drops the low 13 mantissa bits of both operands: rho <= 2^-10 each, worst case taken
 //         -> GEMM_EPS_TF32 (constant);
-//   bf16 operands (round to nearest, unit roundoff 2^-8): the worst case 2^-8 per operand is ~2.4x the actual
-//         residual norm of a rounded vector (errors are ~uniform in +-half an ulp), so the MEASURED residuals
-//         are used: rho_q per query (emb_prep_queries_kernel), rho_x = max over the rows of the store (kept by
-//         emb_inv_norm_kernel at insert; 0 for a bf16 store, whose rows are exact).  Typical: rho ~ 1.6e-3 each
-//         -> eps ~ 3.5e-3 instead of the worst-case 8.0e-3.
+//   bf16 store: the rows are exact bf16 values (rho_x = 0); the query is rounded to bf16 (unit roundoff 2^-8):
+//         the worst case 2^-8 is ~2.4x the actual residual norm of a rounded vector, so the MEASURED residual
+//         rho_q per query (emb_prep_queries_kernel) is used, capped at the worst case.
 constexpr float GEMM_EPS_ACC = 2.5e-4f;
 constexpr float GEMM_EPS_TF32 = 2.25e-3f;
 constexpr float GEMM_RHO_BF16_WORST = 3.90625e-3f;   // 2^-8: cap of a measured rho (a sound upper bound by itself)
 
 struct GemmParams {
     uint64_t n_rows;
-    uint32_t n_kblocks;        // stride / 32
+    uint32_t n_kblocks;        // stride / 32 (fp32) or stride / 64 (bf16)
     const float *inv_norm;     // [n_rows] (NaN => skipped)
     uint32_t n_queries;        // B (real queries)
     uint32_t n_qgroups;        // ceil(B / 128)
@@ -77,7 +74,7 @@ struct GemmParams {
                                // gemm_thr_kernel, raised with atomicMax whenever a list proves a better bound (see gemm_compact)
     const float *eps_v;        // [n_queries] error bound of the sweep's scores in the same units
     uint32_t limit;            // top-`limit` wanted
-    uint32_t lists_per_query;  // candidate lists per query (NG=1: 2 per row partition, NG=2: 1)
+    uint32_t lists_per_query;  // candidate lists per query: ctas_per_group * GEMM_LISTS_PER_CTA
     int max_mode;              // 1 => threshold pass: record each list's best approximate score, push nothing
     uint32_t tile_limit;       // max row tiles per CTA (0 = all); the threshold pass looks at one
     float *gmax;               // [n_qgroups*128][lists_per_query] best score per list (max_mode)
@@ -88,12 +85,12 @@ struct GemmParams {
     uint32_t ovf_cap;
 };
 
-__host__ __device__ inline size_t gemm_smem_bytes(int ng) {
-    const size_t ring = ng == 1 ? size_t(4) * (GEMM_A_BYTES + GEMM_B_BYTES) : size_t(3) * (2 * GEMM_A_BYTES + GEMM_B_BYTES);
-    return 1024 /*align slack*/ + ring + 2 * GEMM_N * 4 /*inv norms*/ + 256 /*barriers, tmem ptr*/;
+__host__ __device__ inline size_t gemm_smem_bytes() {
+    return 1024 /*align slack*/ + size_t(GEMM_STAGES) * GEMM_STAGE_BYTES + GEMM_CONSUMER_WG * 2 * GEMM_N * 4 /*inv norms*/
+           + 256 /*barriers*/;
 }
 
-// ---- tcgen05 / TMA PTX wrappers ------------------------------------------------------
+// ---- TMA / wgmma PTX wrappers ------------------------------------------------------
 __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, uint64_t *bar, int32_t c0, int32_t c1,
                                             uint64_t hint) {
     asm volatile(
@@ -102,79 +99,55 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, u
         "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
         : "memory");
 }
-// pulls a tile HBM -> L2 ahead of its TMA load (no shared memory, no barrier): the ring then only has to
-// cover L2 latency, not HBM latency
-__device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap *map, int32_t c0, int32_t c1) {
-    asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(reinterpret_cast<uint64_t>(map)),
-                 "r"(c0), "r"(c1)
-                 : "memory");
-}
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap *map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
+// K-major, SWIZZLE_128B shared-memory matrix descriptor of wgmma:
+// start>>4 [0,14) | LBO>>4 [16,30) = 1 (unused when swizzled) | SBO>>4 [32,46) = 1024/16 (8-row groups) | layout [62,64) = 1
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+    return uint64_t((smem_addr >> 4) & 0x3fffu) | (uint64_t(1) << 16) | (uint64_t(64) << 32) | (uint64_t(1) << 62);
 }
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::tf32, issued by one thread
-__device__ __forceinline__ void tc_mma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x 128] (+)= A[64 x K] * B[128 x K]^T, both K-major in shared memory; K = 8 (tf32) or 16 (bf16) = 32 bytes
+template <bool BF16>
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+#define OC_WGMMA_D                                                                                                             \
+    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, "   \
+    "%25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "    \
+    "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+#define OC_WGMMA_OPS                                                                                                           \
+    "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),    \
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),   \
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),   \
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),   \
+        "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),   \
+        "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),   \
+        "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+    if (BF16)
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %66, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " OC_WGMMA_D ", %64, %65, p, 1, 1, 0, 0;\n\t}"
+            : OC_WGMMA_OPS
+            : "l"(adesc), "l"(bdesc), "r"(accumulate));
+    else
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %66, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " OC_WGMMA_D ", %64, %65, p, 1, 1;\n\t}"
+            : OC_WGMMA_OPS
+            : "l"(adesc), "l"(bdesc), "r"(accumulate));
+#undef OC_WGMMA_D
+#undef OC_WGMMA_OPS
 }
-// same for bf16 operands (kind::f16, UMMA_K = 16 elements = 32 B)
-__device__ __forceinline__ void tc_mma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor layout):
-// start>>4 [0,14) | LBO>>4 [16,30) = 1 | SBO>>4 [32,46) = 1024/16 | version [46,48) = 1 | layout [61,64) = 2
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-    const uint32_t lo = ((smem_addr >> 4) & 0x3fffu) | (1u << 16);
-    const uint32_t hi = 64u | (1u << 14) | (2u << 29);
-    return (uint64_t(hi) << 32) | lo;
-}
-// instruction descriptor: D=f32 (1<<4), A=B=tf32 (2<<7, 2<<10), K-major both, N>>3 at [17,23), M>>4 at [24,29)
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(uint32_t m, uint32_t n) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
-// D=f32, A=B=bf16 (format 1)
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t m, uint32_t n) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 constexpr uint64_t TMA_EVICT_FIRST = 0x12F0000000000000ull;
 constexpr uint64_t TMA_EVICT_LAST = 0x14F0000000000000ull;
 
-// ---- the epilogue all sweep variants share: thread = TMEM lane = ONE QUERY --------------------------------
-// Reads n_chunks x 32 accumulator columns (rows rbase ..) of this thread's lane, scales by the rows' inverse
-// norms (inr: shared memory, warp-wide broadcast LDS.128) and gathers every row whose approximate score
-// clears the query's threshold into the thread's private list.  max_mode: only the best score is tracked
-// (threshold pass).
+// ---- the epilogue: one thread = 2 queries x 32 rows of the tile, one private list per query --------------------
 // The threshold only has to stay <= a_lim - 2 eps (a_lim = the limit-th best approximate score of the whole
 // store): the seed is a coarse sample bound, so when a list fills up the warp tightens it — the limit-th largest
 // score of ANY `limit` distinct rows bounds a_lim from below — drops what fell under the new threshold and shares
@@ -191,16 +164,17 @@ __device__ __noinline__ void gemm_spill(const GemmParams &p, uint32_t q, const u
         for (uint32_t i = 0; i < cnt; i++) p.ovf[size_t(q) * p.ovf_cap + base + i] = mybuf[i];
 }
 // Warp-cooperative tightening of the lists of the lanes in `need` (register-only: 4 keys per lane, cap <= 128).
-// For lane l: kth = limit-th largest score of its list (bitwise search on the order-preserving key, one
-// __reduce_add_sync per bit); thr_l = max(thr_l, kth - 2 eps_l); entries <= thr_l are dropped, the rest compacted
-// in place.  Returns, for the calling lane, its new (cnt, thr).
-__device__ __noinline__ void gemm_compact(const GemmParams &p, uint32_t need, uint32_t q_lane0, uint32_t lists, uint32_t my_list,
-                                          uint32_t lane, GemmEpi &e) {
+// Lane l owns list my_list of query my_q (both passed per lane).  For lane l: kth = limit-th largest score of its
+// list (bitwise search on the order-preserving key, one __reduce_add_sync per bit); thr_l = max(thr_l, kth - 2 eps_l);
+// entries <= thr_l are dropped, the rest compacted in place.  Returns, for the calling lane, its new (cnt, thr).
+__device__ __noinline__ void gemm_compact(const GemmParams &p, uint32_t need, uint32_t my_q, uint32_t my_list, uint32_t lane,
+                                          GemmEpi &e) {
     while (need) {
         const uint32_t l = __ffs(need) - 1;
         need &= need - 1;
-        const uint32_t lq = q_lane0 + l;
-        uint64_t *lbuf = p.cand + (size_t(lq) * lists + my_list) * p.cap;
+        const uint32_t lq = __shfl_sync(0xffffffffu, my_q, l);
+        const uint32_t llist = __shfl_sync(0xffffffffu, my_list, l);
+        uint64_t *lbuf = p.cand + (size_t(lq) * p.lists_per_query + llist) * p.cap;
         const uint32_t lcnt = __shfl_sync(0xffffffffu, e.cnt, l);
         float lthr = __shfl_sync(0xffffffffu, e.thr, l);
         __syncwarp();                                         // lane l's pushes are visible to the whole warp
@@ -246,621 +220,144 @@ __device__ __noinline__ void gemm_compact(const GemmParams &p, uint32_t need, ui
         __syncwarp();
     }
 }
-__device__ __forceinline__ void gemm_epilogue_tile(const GemmParams &p, uint32_t taddr, const float *inr, uint32_t n_chunks,
-                                                   uint32_t rbase, uint32_t q, uint32_t lists, uint32_t my_list,
-                                                   unsigned int thr_global, uint64_t *__restrict__ mybuf, GemmEpi &e) {
-    const float4 *inr4 = reinterpret_cast<const float4 *>(inr);
-    const uint32_t lane = threadIdx.x & 31;
-    if (thr_global) e.thr = fmaxf(e.thr, f32_unordered(thr_global));   // the query's threshold as raised by every CTA so far
-    for (uint32_t ch = 0; ch < n_chunks; ch++) {
-        uint32_t d[32];
-        tmem_ld32(taddr + ch * 32, d);
-        tmem_ld_wait();
-        float v[32];
-#pragma unroll
-        for (uint32_t j4 = 0; j4 < 8; j4++) {
-            const float4 w = inr4[ch * 8 + j4];          // LDS.128, warp-wide broadcast
-            v[4 * j4 + 0] = __uint_as_float(d[4 * j4 + 0]) * w.x;   // cos * |q|
-            v[4 * j4 + 1] = __uint_as_float(d[4 * j4 + 1]) * w.y;
-            v[4 * j4 + 2] = __uint_as_float(d[4 * j4 + 2]) * w.z;
-            v[4 * j4 + 3] = __uint_as_float(d[4 * j4 + 3]) * w.w;
-        }
-        if (p.max_mode) {
-#pragma unroll
-            for (uint32_t j = 0; j < 32; j++) e.best = fmaxf(e.best, v[j]);   // NaN (dead rows) ignored
-            continue;
-        }
-        uint32_t mask = 0;
-#pragma unroll
-        for (uint32_t j = 0; j < 32; j++) mask |= (v[j] > e.thr ? 1u : 0u) << j;   // NaN fails
-        if (mask) {   // rare once the threshold has tightened
-#pragma unroll
-            for (uint32_t j = 0; j < 32; j++)
-                if ((mask >> j) & 1u) { mybuf[e.cnt] = make_key(v[j], rbase + ch * 32 + j); e.cnt++; }
-        }
-        const uint32_t need = __ballot_sync(0xffffffffu, e.cnt + 32 > p.cap);
-        if (need) gemm_compact(p, need, q - lane, lists, my_list, lane, e);
-    }
-}
 
-// NG = query groups (of 128) handled by ONE CTA against each streamed row tile:
-//   NG=1: accumulator double-buffered across tiles (2 x 256 TMEM columns), 4 smem stages of 48 KB;
-//         several CTAs (one per group) walk the same rows.
-//   NG=2: both groups consume the SAME staged X tile (one copy of X per CTA instead of one per
-//         group: L2->SM traffic per 256 rows x 256 queries drops from 96 KB to 64 KB per K-block),
-//         one accumulator per group (2 x 256 columns), 3 stages of 64 KB; every CTA is a row partition.
-template <int NG, bool BF16>
+// One CTA = one query group (128 queries) x one row partition c of the store (tiles c, c + ctas_per_group, ...).
+// wgmma D fragment of m64n128 (per warpgroup): warp w holds rows [16w, 16w + 16); lane holds rows lane/4 and
+// lane/4 + 8, columns 8j + 2 (lane % 4) + {0, 1} for j = 0..15, in d[4j + 2h + {0, 1}] (h = row half).
+template <bool BF16>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_x, const GemmParams p) {
-    // SWIZZLE_128B tiles need 1024-byte alignment; every pointer below is derived from the
-    // __shared__ array itself so loads/stores stay in the shared address space (LDS/STS).
     extern __shared__ __align__(1024) uint8_t smem_gemm[];
-    constexpr uint32_t STAGES = NG == 1 ? 4 : 3;
-    constexpr uint32_t STAGE_BYTES = NG * GEMM_A_BYTES + GEMM_B_BYTES;
-    uint8_t *ring = smem_gemm;
-    float *inr_s = reinterpret_cast<float *>(smem_gemm + STAGES * STAGE_BYTES);   // [2][256]
-    uint64_t *bars = reinterpret_cast<uint64_t *>(inr_s + 2 * GEMM_N);
-    uint64_t *full = bars, *empty = bars + STAGES;
-    uint64_t *tfull = bars + 2 * STAGES, *tempty = tfull + 2;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(tempty + 2);
+    // SWIZZLE_128B tiles need 1024-byte alignment of the shared-memory address
+    uint8_t *ring = smem_gemm + ((1024u - (smem_u32(smem_gemm) & 1023u)) & 1023u);
+    float *inr_s = reinterpret_cast<float *>(ring + GEMM_STAGES * GEMM_STAGE_BYTES);   // [wg][2][GEMM_N]
+    uint64_t *bars = reinterpret_cast<uint64_t *>(inr_s + GEMM_CONSUMER_WG * 2 * GEMM_N);
+    uint64_t *full = bars, *empty = bars + GEMM_STAGES;
 
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // NG=1: blockIdx -> (query group g, row partition c); NG=2: every CTA is a row partition, groups 2*sg, 2*sg+1
-    const uint32_t n_super = NG == 1 ? p.n_qgroups : (p.n_qgroups + 1) / 2;
-    const uint32_t g0 = (blockIdx.x % n_super) * NG;   // first query group of this CTA
-    const uint32_t c = blockIdx.x / n_super;           // row partition
+    const uint32_t grp = blockIdx.x % p.n_qgroups;     // query group
+    const uint32_t c = blockIdx.x / p.n_qgroups;       // row partition
     const uint64_t n_tiles = (p.n_rows + GEMM_N - 1) / GEMM_N;
-    uint64_t my_tiles = (n_tiles > c) ? (n_tiles - c + p.ctas_per_group - 1) / p.ctas_per_group : 0;
-    if (p.tile_limit && my_tiles > p.tile_limit) my_tiles = p.tile_limit;
-    const uint32_t nkb = p.n_kblocks;
-    // threads that release an accumulator slot: NG=1 all 8 epilogue warps, NG=2 the 4 warps of that group
-    constexpr uint32_t TEMPTY_COUNT = NG == 1 ? GEMM_EPI_WARPS * 32 : GEMM_EPI_WARPS * 16;
-
-    if (threadIdx.x == 0) {
-        for (uint32_t s = 0; s < STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (uint32_t a = 0; a < 2; a++) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], TEMPTY_COUNT); }
-        fence_mbar_init();
-        tma_prefetch_desc(&tm_q);
-        tma_prefetch_desc(&tm_x);
-    }
-    if (warp == 1) {   // TMEM: all 512 columns (2 accumulators x 256 fp32 columns)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // ===================== TMA producer =====================
-        if (lane == 0) {
-            uint64_t n = 0;
-            for (uint64_t it = 0; it < my_tiles; it++) {
-                const uint64_t row0 = (c + it * p.ctas_per_group) * GEMM_N;
-                for (uint32_t kb = 0; kb < nkb; kb++, n++) {
-                    const uint32_t s = uint32_t(n % STAGES), ph = uint32_t((n / STAGES) & 1);
-                    mbar_wait(&empty[s], ph ^ 1);
-                    uint8_t *a_dst = ring + s * STAGE_BYTES, *b_dst = a_dst + NG * GEMM_A_BYTES;
-                    mbar_expect_tx(&full[s], STAGE_BYTES);
-#pragma unroll
-                    for (int gi = 0; gi < NG; gi++)   // rows past the padded query matrix are zero-filled by TMA
-                        tma_load_2d(a_dst + gi * GEMM_A_BYTES, &tm_q, &full[s], int32_t(kb * (BF16 ? 2 * GEMM_KB : GEMM_KB)),
-                                    int32_t((g0 + gi) * GEMM_M), TMA_EVICT_LAST);
-                    tma_load_2d(b_dst, &tm_x, &full[s], int32_t(kb * (BF16 ? 2 * GEMM_KB : GEMM_KB)), int32_t(row0), TMA_EVICT_FIRST);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (one thread) =====================
-        if (lane == 0) {
-            const uint32_t idesc = BF16 ? umma_idesc_bf16(GEMM_M, GEMM_N) : umma_idesc_tf32(GEMM_M, GEMM_N);
-            uint64_t n = 0;
-            for (uint64_t it = 0; it < my_tiles; it++) {
-                // accumulator slot and barrier phase: NG=1 alternates slots per tile; NG=2 uses slot = group every tile
-                const uint32_t slot1 = uint32_t(it & 1), ph1 = uint32_t((it >> 1) & 1), ph2 = uint32_t(it & 1);
-                if (NG == 1) { mbar_wait(&tempty[slot1], ph1 ^ 1); tc_fence_after(); }
-                for (uint32_t kb = 0; kb < nkb; kb++, n++) {
-                    const uint32_t s = uint32_t(n % STAGES), ph = uint32_t((n / STAGES) & 1);
-                    mbar_wait(&full[s], ph);
-                    tc_fence_after();
-                    const uint32_t a_addr = smem_u32(ring + s * STAGE_BYTES);
-                    const uint64_t bdesc = umma_desc_sw128(a_addr + NG * GEMM_A_BYTES);
-#pragma unroll
-                    for (int gi = 0; gi < NG; gi++) {
-                        if (NG == 2 && kb == 0) { mbar_wait(&tempty[gi], ph2 ^ 1); tc_fence_after(); }   // epilogue drained D_gi
-                        const uint32_t d_tmem = tmem_base + (NG == 1 ? slot1 : uint32_t(gi)) * GEMM_N;
-                        const uint64_t adesc = umma_desc_sw128(a_addr + gi * GEMM_A_BYTES);
-#pragma unroll
-                        for (uint32_t k = 0; k < 4; k++) {    // UMMA_K = 8 tf32 / 16 bf16 = 32 B: advance start address by 32 B
-                            if (BF16) tc_mma_bf16(d_tmem, adesc + k * 2, bdesc + k * 2, idesc, (kb | k) != 0);
-                            else tc_mma_tf32(d_tmem, adesc + k * 2, bdesc + k * 2, idesc, (kb | k) != 0);
-                        }
-                        if (NG == 2 && kb + 1 == nkb) tc_commit(&tfull[gi]);   // group gi's accumulator complete
-                    }
-                    tc_commit(&empty[s]);                  // frees the smem stage when these MMAs retire
-                }
-                if (NG == 1) tc_commit(&tfull[slot1]);     // accumulator complete -> epilogue
-            }
-        }
-    } else {
-        // ===================== epilogue: thread = TMEM lane = one query =====================
-        // NG=1: the two warps of a lane quadrant split the tile's 256 columns (rows) in halves;
-        // NG=2: they take one query group each and all 256 columns.
-        const uint32_t ew = warp - 2;                      // 0..7
-        const uint32_t quad = warp & 3;                    // TMEM lane quadrant this warp may access
-        const uint32_t sel = ew >> 2;                      // NG=1: column half, NG=2: group within the CTA
-        const uint32_t m = quad * 32 + lane;
-        const uint32_t grp = g0 + (NG == 2 ? sel : 0u);
-        const uint32_t q = grp * GEMM_M + m;
-        const bool live = q < p.n_queries;
-        const uint32_t et = ew * 32 + lane;                // 0..255 among epilogue threads
-        const uint32_t lists = p.lists_per_query;
-        const uint32_t my_list = NG == 1 ? c * 2 + sel : c;
-        uint64_t *__restrict__ mybuf = p.cand + (size_t(q) * lists + my_list) * p.cap;
-        GemmEpi e;
-        e.thr = live ? -INFINITY : INFINITY;               // refreshed from the query's global threshold before every tile
-        e.best = -INFINITY;                                // max_mode: best approximate score seen by this list
-        const uint32_t ncols = NG == 1 ? 128u : 256u, col0 = NG == 1 ? sel * 128u : 0u;
-        for (uint64_t it = 0; it < my_tiles; it++) {
-            const uint32_t slot = NG == 1 ? uint32_t(it & 1) : sel;
-            const uint32_t ph = NG == 1 ? uint32_t((it >> 1) & 1) : uint32_t(it & 1);
-            const uint64_t row0 = (c + it * p.ctas_per_group) * GEMM_N;
-            float *inr = inr_s + uint32_t(it & 1) * GEMM_N;
-            {
-                const uint64_t r = row0 + et;
-                inr[et] = r < p.n_rows ? __ldg(p.inv_norm + r) : __int_as_float(0x7fc00000);
-            }
-            // requested before the waits below, consumed after them: the L2 round trip hides behind the MMAs of this tile
-            const unsigned int tg = (live && !p.max_mode) ? *reinterpret_cast<volatile unsigned int *>(p.thr + q) : 0u;
-            named_bar_sync(1, GEMM_EPI_WARPS * 32);
-            mbar_wait(&tfull[slot], ph);
-            tc_fence_after();
-            gemm_epilogue_tile(p, tmem_base + ((quad * 32u) << 16) + slot * GEMM_N + col0, inr + col0, ncols / 32,
-                               uint32_t(row0) + col0, q, lists, my_list, tg, mybuf, e);
-            tc_fence_before();
-            mbar_arrive(&tempty[slot]);
-        }
-        if (p.max_mode) p.gmax[size_t(q) * lists + my_list] = live ? e.best : -INFINITY;
-        else if (grp < p.n_qgroups) p.cand_cnt[size_t(q) * lists + my_list] = live ? e.cnt : 0;
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-    }
-}
-
-// ---------------------------------------------------------------------------------------
-// CTA-pair variant (tcgen05 cta_group::2): the two SMs of a TPC run ONE 256-query x 512-row tile.
-// CTA r of the pair stages ITS 128 queries (A half) and ITS 128 rows of each of two 256-row B
-// tiles; the leader's MMAs (M = 256, N = 256) read both CTAs' shared memory, the accumulators
-// of CTA r hold queries [128r, 128r+128) x 512 rows (all 512 TMEM columns of both SMs).  Per
-// K-block a pair moves 32 KB of Q + 64 KB of X for 256 x 512 scores — 25 % less L2->SM traffic
-// than two independent NG=2 CTAs (2 x (32 + 32) KB), which is what bounds the fp32 sweep.
-// ---------------------------------------------------------------------------------------
-constexpr uint32_t PAIR_STAGES = 4;
-constexpr uint32_t PAIR_HALF_B = 128 * 128;                       // 128 rows x 128 B
-constexpr uint32_t PAIR_STAGE_BYTES = GEMM_A_BYTES + 2 * PAIR_HALF_B;   // 48 KB per CTA
-constexpr uint32_t PAIR_TILE_ROWS = 512;
-
-__host__ __device__ inline size_t gemm_pair_smem_bytes() {
-    return 1024 + size_t(PAIR_STAGES) * PAIR_STAGE_BYTES + 2 * PAIR_TILE_ROWS * 4 + 256;
-}
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    // default semantics (release at CTA scope): a cluster-scope release costs a MEMBAR.ALL.GPU per arrive;
-    // the data this orders is consumed by tcgen05 / the async proxy, which the tcgen05 / proxy fences cover
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t *bar, uint32_t parity) {
-    uint32_t ok = 0;
-    while (!ok)
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(ok)
-            : "r"(smem_u32(bar)), "r"(parity)
-            : "memory");
-}
-// TMA load issued by either CTA of the pair; the transaction bytes land on the LEADER's barrier
-__device__ __forceinline__ void tma_load_2d_pair(void *dst, const CUtensorMap *map, uint32_t leader_bar, int32_t c0, int32_t c1,
-                                                 uint64_t hint) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(dst)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(leader_bar), "r"(c0), "r"(c1), "l"(hint)
-        : "memory");
-}
-// arrives on the barrier at this offset in BOTH CTAs once all previously issued MMAs have retired
-__device__ __forceinline__ void tc_commit_pair(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(uint16_t(3))
-                 : "memory");
-}
-template <bool BF16>
-__device__ __forceinline__ void tc_mma_pair(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    const uint32_t z = 0;
-    if (BF16)
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n\t}" ::"r"(d_tmem),
-            "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(z)
-            : "memory");
-    else
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n\t}" ::"r"(d_tmem),
-            "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(z)
-            : "memory");
-}
-
-template <bool BF16>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-emb_gemm_pair_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_x, const GemmParams p) {
-    extern __shared__ __align__(1024) uint8_t smem_gemm[];
-    uint8_t *ring = smem_gemm;
-    float *inr_s = reinterpret_cast<float *>(smem_gemm + PAIR_STAGES * PAIR_STAGE_BYTES);   // [2][512]
-    uint64_t *bars = reinterpret_cast<uint64_t *>(inr_s + 2 * PAIR_TILE_ROWS);
-    uint64_t *full = bars, *empty = bars + PAIR_STAGES;       // full: used in the leader only
-    uint64_t *tfull = bars + 2 * PAIR_STAGES, *tempty = tfull + 2;   // tempty: used in the leader only
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(tempty + 2);
-
-    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const uint32_t cid = blockIdx.x >> 1;
-    const uint32_t n_super = (p.n_qgroups + 1) / 2;
-    const uint32_t grp = (cid % n_super) * 2 + rank;   // this CTA's query group (A half of the pair's M = 256)
-    const uint32_t c = cid / n_super;                  // the pair's row partition
-    const uint64_t n_tiles = (p.n_rows + PAIR_TILE_ROWS - 1) / PAIR_TILE_ROWS;
     uint64_t my_tiles = (n_tiles > c) ? (n_tiles - c + p.ctas_per_group - 1) / p.ctas_per_group : 0;
     if (p.tile_limit && my_tiles > p.tile_limit) my_tiles = p.tile_limit;
     const uint32_t nkb = p.n_kblocks;
     constexpr int32_t KSTEP = BF16 ? 2 * GEMM_KB : GEMM_KB;
 
     if (threadIdx.x == 0) {
-        for (uint32_t s = 0; s < PAIR_STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (uint32_t a = 0; a < 2; a++) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], 8); }   // 4 epilogue warps x 2 CTAs
+        for (uint32_t s = 0; s < GEMM_STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], GEMM_CONSUMER_WG * 4); }
         fence_mbar_init();
         tma_prefetch_desc(&tm_q);
         tma_prefetch_desc(&tm_x);
     }
-    if (warp == 1) {   // all 512 TMEM columns of both SMs
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    cluster_sync_all();   // the peer's barriers are initialised before any remote arrive / multicast commit
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
-        // ===================== TMA producer (both CTAs) =====================
+    if (warp == GEMM_CONSUMER_WG * 4) {
+        // ===================== TMA producer =====================
         if (lane == 0) {
             uint64_t n = 0;
             for (uint64_t it = 0; it < my_tiles; it++) {
-                const uint64_t row0 = (c + it * p.ctas_per_group) * PAIR_TILE_ROWS;
+                const uint64_t row0 = (c + it * p.ctas_per_group) * GEMM_N;
                 for (uint32_t kb = 0; kb < nkb; kb++, n++) {
-                    const uint32_t s = uint32_t(n % PAIR_STAGES), ph = uint32_t((n / PAIR_STAGES) & 1);
+                    const uint32_t s = uint32_t(n % GEMM_STAGES), ph = uint32_t((n / GEMM_STAGES) & 1);
                     mbar_wait(&empty[s], ph ^ 1);
-                    const uint32_t lbar = mapa_shared(smem_u32(&full[s]), 0);
-                    if (rank == 0) mbar_expect_tx(&full[s], 2 * PAIR_STAGE_BYTES);   // both CTAs' bytes
-                    uint8_t *a_dst = ring + s * PAIR_STAGE_BYTES;
-                    tma_load_2d_pair(a_dst, &tm_q, lbar, int32_t(kb) * KSTEP, int32_t(grp * GEMM_M), TMA_EVICT_LAST);
-#pragma unroll
-                    for (uint32_t j = 0; j < 2; j++)
-                        tma_load_2d_pair(a_dst + GEMM_A_BYTES + j * PAIR_HALF_B, &tm_x, lbar, int32_t(kb) * KSTEP,
-                                         int32_t(row0 + j * 256 + rank * 128), TMA_EVICT_FIRST);
+                    uint8_t *a_dst = ring + s * GEMM_STAGE_BYTES;
+                    mbar_expect_tx(&full[s], GEMM_STAGE_BYTES);
+                    // rows past the padded query matrix / the store are zero-filled by TMA
+                    tma_load_2d(a_dst, &tm_q, &full[s], int32_t(kb) * KSTEP, int32_t(grp * GEMM_M), TMA_EVICT_LAST);
+                    tma_load_2d(a_dst + GEMM_A_BYTES, &tm_x, &full[s], int32_t(kb) * KSTEP, int32_t(row0), TMA_EVICT_FIRST);
                 }
             }
         }
-        __syncwarp();
-    } else if (warp == 1) {
-        // ===================== MMA issuer (one thread of the leader CTA) =====================
-        if (rank == 0 && lane == 0) {
-            const uint32_t idesc = BF16 ? umma_idesc_bf16(256, 256) : umma_idesc_tf32(256, 256);
-            uint64_t n = 0;
-            for (uint64_t it = 0; it < my_tiles; it++) {
-                const uint32_t ph2 = uint32_t(it & 1);
-                for (uint32_t kb = 0; kb < nkb; kb++, n++) {
-                    const uint32_t s = uint32_t(n % PAIR_STAGES), ph = uint32_t((n / PAIR_STAGES) & 1);
-                    mbar_wait_cluster(&full[s], ph);
-                    tc_fence_after();
-                    const uint32_t a_addr = smem_u32(ring + s * PAIR_STAGE_BYTES);
-                    const uint64_t adesc = umma_desc_sw128(a_addr);
-#pragma unroll
-                    for (uint32_t j = 0; j < 2; j++) {
-                        if (kb == 0) { mbar_wait_cluster(&tempty[j], ph2 ^ 1); tc_fence_after(); }   // both CTAs drained D_j
-                        const uint64_t bdesc = umma_desc_sw128(a_addr + GEMM_A_BYTES + j * PAIR_HALF_B);
-#pragma unroll
-                        for (uint32_t k = 0; k < 4; k++)
-                            tc_mma_pair<BF16>(tmem_base + j * 256, adesc + k * 2, bdesc + k * 2, idesc, (kb | k) != 0);
-                        if (kb + 1 == nkb) tc_commit_pair(&tfull[j]);
-                    }
-                    tc_commit_pair(&empty[s]);   // frees this stage in both CTAs
-                }
-            }
-        }
-        __syncwarp();
-    } else {
-        // ===================== epilogue (both CTAs): thread = TMEM lane = one query =====================
-        const uint32_t ew = warp - 2, quad = warp & 3, sel = ew >> 2;   // sel = accumulator = 256-row half of the tile
-        const uint32_t m = quad * 32 + lane;
-        const uint32_t q = grp * GEMM_M + m;
-        const bool live = q < p.n_queries;
-        const uint32_t et = ew * 32 + lane;
-        const uint32_t lists = p.lists_per_query;
-        const uint32_t my_list = c * 2 + sel;
-        uint64_t *__restrict__ mybuf = p.cand + (size_t(q) * lists + my_list) * p.cap;
-        const uint32_t tempty_remote = mapa_shared(smem_u32(&tempty[sel]), 0);
-        GemmEpi e;
-        e.thr = live ? -INFINITY : INFINITY;
-        e.best = -INFINITY;
-        for (uint64_t it = 0; it < my_tiles; it++) {
-            const uint32_t ph = uint32_t(it & 1);
-            const uint64_t row0 = (c + it * p.ctas_per_group) * PAIR_TILE_ROWS;
-            float *inr = inr_s + uint32_t(it & 1) * PAIR_TILE_ROWS;
-#pragma unroll
-            for (uint32_t h = 0; h < 2; h++) {
-                const uint64_t r = row0 + et + h * 256;
-                inr[et + h * 256] = r < p.n_rows ? __ldg(p.inv_norm + r) : __int_as_float(0x7fc00000);
-            }
-            const unsigned int tg = (live && !p.max_mode) ? *reinterpret_cast<volatile unsigned int *>(p.thr + q) : 0u;
-            named_bar_sync(1, GEMM_EPI_WARPS * 32);
-            mbar_wait(&tfull[sel], ph);
-            tc_fence_after();
-            gemm_epilogue_tile(p, tmem_base + ((quad * 32u) << 16) + sel * 256, inr + sel * 256, 8, uint32_t(row0) + sel * 256, q,
-                               lists, my_list, tg, mybuf, e);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(tempty_remote);   // one arrival per warp on the leader's barrier
-        }
-        if (p.max_mode) p.gmax[size_t(q) * lists + my_list] = live ? e.best : -INFINITY;
-        else if (grp < p.n_qgroups) p.cand_cnt[size_t(q) * lists + my_list] = live ? e.cnt : 0;
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();   // no CTA leaves (or frees TMEM) while its peer can still touch its smem / barriers
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
+
+    // ===================== consumers: wgmma + epilogue =====================
+    const uint32_t wg = warp >> 2, t = threadIdx.x & 127;
+    const uint32_t lists = p.lists_per_query;
+    const uint32_t my_list = c * GEMM_LISTS_PER_CTA + (lane & 3);
+    uint32_t q[2];
+    bool live[2];
+    GemmEpi e[2];
+#pragma unroll
+    for (uint32_t h = 0; h < 2; h++) {
+        q[h] = grp * GEMM_M + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+        live[h] = q[h] < p.n_queries;
+        e[h].thr = live[h] ? -INFINITY : INFINITY;     // refreshed from the query's global threshold before every tile
+        e[h].best = -INFINITY;                         // max_mode: best approximate score seen by this list
     }
-}
-
-// ---------------------------------------------------------------------------------------
-// CTA-pair variant with IN-SM fp32 -> bf16 operand conversion (fp32 stores, B > 128).
-// At B = 256 the tf32 sweep is co-limited by the tensor pipe (tf32 runs at half the bf16 rate:
-// 2*256*n*d flop is ~0.54 ms of tf32 at the sustained rate vs 0.47 ms of HBM time).  Here the
-// fp32 rows still stream from HBM exactly once (TMA, 128-byte swizzle), four converter warps
-// round them to bf16 (cvt.rn) into a second ring laid out as the K-major SWIZZLE_64B UMMA
-// operand, and the MMAs run as kind::f16 at twice the tf32 rate, so the sweep is bound by HBM
-// alone.  Q is converted once per batch (f32_to_bf16_kernel) and arrives by TMA (SWIZZLE_64B).
-// Selection only: the merge re-scores in exact fp32; the proof uses eps = GEMM_EPS_BF16X2.
-//   per CTA: 5 stages x (32 KB fp32 X tile, converted IN PLACE into its first 16 KB, + 8 KB bf16 Q):
-//   a stage cycles TMA -> convert -> MMA -> free, so ~3 stages (96 KB) are in flight from HBM per SM.
-// ---------------------------------------------------------------------------------------
-constexpr uint32_t CVT_STAGES_DEFAULT = 5;               // ring depth: template parameter of the kernel (4 leaves room for a co-resident BM25 CTA)
-constexpr uint32_t CVT_PREFETCH = 0;                     // K-blocks (32 KB per CTA each) prefetched into L2 ahead of the ring
-constexpr uint32_t CVT_RAW_BYTES = 256 * 128;             // 256 rows x 32 fp32
-constexpr uint32_t CVT_XOP_BYTES = 256 * 64;              // 256 rows x 32 bf16 (two 128-row B tiles of 8 KB)
-constexpr uint32_t CVT_QOP_BYTES = 128 * 64;              // 128 queries x 32 bf16
-constexpr uint32_t CVT_STAGE_BYTES = CVT_RAW_BYTES + CVT_QOP_BYTES;   // 40 KB
-constexpr uint32_t CVT_WARPS = 4;
-constexpr int CVT_THREADS = GEMM_THREADS + CVT_WARPS * 32;   // warps 10-13 convert
-constexpr float GEMM_EPS_BF16X2 = 8.0e-3f;                // both operands rounded to bf16: 2*2^-8 + 2^-16 + accumulation
-
-__host__ __device__ inline size_t gemm_cvt_smem_bytes(uint32_t stages = CVT_STAGES_DEFAULT) {
-    return 1024 + size_t(stages) * CVT_STAGE_BYTES + 2 * PAIR_TILE_ROWS * 4 + 256;
-}
-// K-major SWIZZLE_64B descriptor: 64-byte rows, 8-row groups 512 B apart
-__device__ __forceinline__ uint64_t umma_desc_sw64(uint32_t smem_addr) {
-    const uint32_t lo = ((smem_addr >> 4) & 0x3fffu) | (1u << 16);
-    const uint32_t hi = 32u | (1u << 14) | (4u << 29);
-    return (uint64_t(hi) << 32) | lo;
-}
-__device__ __forceinline__ uint32_t pack_bf16x2_rn(float lo, float hi) {
-    uint32_t r;
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));   // first source -> upper half
-    return r;
-}
-
-template <uint32_t CVT_STAGES>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(CVT_THREADS, 1)
-emb_gemm_cvt_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_x, const GemmParams p) {
-    extern __shared__ __align__(1024) uint8_t smem_gemm[];
-    // stage: [0, 32 KB) fp32 X as landed ([2 tiles][128 rows][128 B], SW128) -> after conversion
-    //        [0, 16 KB) bf16 X ([2 tiles][128 rows][64 B], SW64); [32 KB, 40 KB) bf16 Q ([128][64 B], SW64)
-    uint8_t *ring = smem_gemm;
-    float *inr_s = reinterpret_cast<float *>(ring + CVT_STAGES * CVT_STAGE_BYTES);
-    uint64_t *bars = reinterpret_cast<uint64_t *>(inr_s + 2 * PAIR_TILE_ROWS);
-    uint64_t *raw_full = bars;                         // X tile landed (this CTA)
-    uint64_t *op_full = raw_full + CVT_STAGES;         // leader only: both CTAs converted + both Q tiles landed
-    uint64_t *empty = op_full + CVT_STAGES;            // MMAs that read the stage retired (multicast to both CTAs)
-    uint64_t *tfull = empty + CVT_STAGES, *tempty = tfull + 2;   // tempty: leader only
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(tempty + 2);
-
-    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const uint32_t cid = blockIdx.x >> 1;
-    const uint32_t n_super = (p.n_qgroups + 1) / 2;
-    const uint32_t grp = (cid % n_super) * 2 + rank;
-    const uint32_t c = cid / n_super;
-    const uint64_t n_tiles = (p.n_rows + PAIR_TILE_ROWS - 1) / PAIR_TILE_ROWS;
-    uint64_t my_tiles = (n_tiles > c) ? (n_tiles - c + p.ctas_per_group - 1) / p.ctas_per_group : 0;
-    if (p.tile_limit && my_tiles > p.tile_limit) my_tiles = p.tile_limit;
-    const uint32_t nkb = p.n_kblocks;   // K-blocks of 32 elements
-    const uint64_t n_blocks = my_tiles * nkb;
-
-    if (threadIdx.x == 0) {
-        for (uint32_t s = 0; s < CVT_STAGES; s++) {
-            mbar_init(&raw_full[s], 1);
-            mbar_init(&op_full[s], 1 + 2 * CVT_WARPS);   // leader's expect_tx arrive + one arrive per converter warp of both CTAs
-            mbar_init(&empty[s], 1);
+    float d[64];
+#pragma unroll
+    for (uint32_t i = 0; i < 64; i++) d[i] = 0.f;
+    uint64_t n = 0;
+    for (uint64_t it = 0; it < my_tiles; it++) {
+        const uint64_t row0 = (c + it * p.ctas_per_group) * GEMM_N;
+        float *inr = inr_s + (wg * 2 + uint32_t(it & 1)) * GEMM_N;
+        {
+            const uint64_t r = row0 + t;
+            inr[t] = r < p.n_rows ? __ldg(p.inv_norm + r) : __int_as_float(0x7fc00000);
         }
-        for (uint32_t a = 0; a < 2; a++) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], 8); }
-        fence_mbar_init();
-        tma_prefetch_desc(&tm_q);
-        tma_prefetch_desc(&tm_x);
+        // requested before the main loop, consumed after it: the L2 round trip hides behind the MMAs of this tile
+        unsigned int tg[2];
+#pragma unroll
+        for (uint32_t h = 0; h < 2; h++)
+            tg[h] = (live[h] && !p.max_mode) ? *reinterpret_cast<volatile unsigned int *>(p.thr + q[h]) : 0u;
+        uint32_t prev_s = 0;
+        for (uint32_t kb = 0; kb < nkb; kb++, n++) {
+            const uint32_t s = uint32_t(n % GEMM_STAGES), ph = uint32_t((n / GEMM_STAGES) & 1);
+            mbar_wait(&full[s], ph);
+            const uint32_t a_addr = smem_u32(ring + s * GEMM_STAGE_BYTES);
+            const uint64_t adesc = wgmma_desc_sw128(a_addr + wg * (GEMM_A_BYTES / 2));
+            const uint64_t bdesc = wgmma_desc_sw128(a_addr + GEMM_A_BYTES);
+            wgmma_fence();
+#pragma unroll
+            for (uint32_t k = 0; k < 4; k++)   // 32 B of K per instruction: advance the start address by 32 B (>> 4 = 2)
+                wgmma_m64n128<BF16>(d, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0);
+            wgmma_commit();
+            if (kb > 0) {                      // the previous K-block's MMAs have retired: free its stage
+                wgmma_wait<1>();
+                if (lane == 0) mbar_arrive(&empty[prev_s]);
+            }
+            prev_s = s;
+        }
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&empty[prev_s]);
+        named_bar_sync(1 + wg, 128);           // this warpgroup's inverse norms are in shared memory
+
+        const float2 *inr2 = reinterpret_cast<const float2 *>(inr);
+#pragma unroll
+        for (uint32_t h = 0; h < 2; h++) {
+            GemmEpi &E = e[h];
+            if (tg[h]) E.thr = fmaxf(E.thr, f32_unordered(tg[h]));   // the query's threshold as raised by every CTA so far
+            float v[32];
+#pragma unroll
+            for (uint32_t j = 0; j < 16; j++) {
+                const float2 w = inr2[4 * j + (lane & 3)];
+                v[2 * j + 0] = d[4 * j + 2 * h + 0] * w.x;   // cos * |q|
+                v[2 * j + 1] = d[4 * j + 2 * h + 1] * w.y;
+            }
+            if (p.max_mode) {
+#pragma unroll
+                for (uint32_t j = 0; j < 32; j++) E.best = fmaxf(E.best, v[j]);   // NaN (dead rows) ignored
+                continue;
+            }
+            uint32_t mask = 0;
+#pragma unroll
+            for (uint32_t j = 0; j < 32; j++) mask |= (v[j] > E.thr ? 1u : 0u) << j;   // NaN fails
+            if (mask) {   // rare once the threshold has tightened
+                uint64_t *mybuf = p.cand + (size_t(q[h]) * lists + my_list) * p.cap;
+                const uint32_t rb = uint32_t(row0) + 2 * (lane & 3);
+#pragma unroll
+                for (uint32_t j = 0; j < 32; j++)
+                    if ((mask >> j) & 1u) { mybuf[E.cnt] = make_key(v[j], rb + 8 * (j >> 1) + (j & 1)); E.cnt++; }
+            }
+            const uint32_t need = __ballot_sync(0xffffffffu, E.cnt + 32 > p.cap);
+            if (need) gemm_compact(p, need, q[h], my_list, lane, E);
+        }
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        // ===================== TMA producer (both CTAs): fp32 X tile + bf16 Q tile per stage =====================
-        if (lane == 0) {
-            uint64_t it = 0; uint32_t kb = 0;
-            uint64_t pit = 0; uint32_t pkb = 0; uint64_t pn = 0;   // L2 prefetch cursor, CVT_PREFETCH K-blocks ahead
-            for (uint64_t n = 0; n < n_blocks; n++) {
-                for (; pn < n_blocks && pn < n + CVT_PREFETCH; pn++) {
-                    const uint64_t prow0 = (c + pit * p.ctas_per_group) * PAIR_TILE_ROWS;
 #pragma unroll
-                    for (uint32_t j = 0; j < 2; j++)
-                        tma_prefetch_l2_2d(&tm_x, int32_t(pkb * GEMM_KB), int32_t(prow0 + j * 256 + rank * 128));
-                    if (++pkb == nkb) { pkb = 0; pit++; }
-                }
-                const uint64_t row0 = (c + it * p.ctas_per_group) * PAIR_TILE_ROWS;
-                const uint32_t s = uint32_t(n % CVT_STAGES), ph = uint32_t((n / CVT_STAGES) & 1);
-                mbar_wait(&empty[s], ph ^ 1);
-                uint8_t *st = ring + s * CVT_STAGE_BYTES;
-                mbar_expect_tx(&raw_full[s], CVT_RAW_BYTES);
-#pragma unroll
-                for (uint32_t j = 0; j < 2; j++)
-                    tma_load_2d(st + j * PAIR_HALF_B, &tm_x, &raw_full[s], int32_t(kb * GEMM_KB), int32_t(row0 + j * 256 + rank * 128),
-                                TMA_EVICT_FIRST);
-                if (rank == 0) mbar_expect_tx(&op_full[s], 2 * CVT_QOP_BYTES);
-                tma_load_2d_pair(st + CVT_RAW_BYTES, &tm_q, mapa_shared(smem_u32(&op_full[s]), 0), int32_t(kb * GEMM_KB),
-                                 int32_t(grp * GEMM_M), TMA_EVICT_LAST);
-                if (++kb == nkb) { kb = 0; it++; }
-            }
-        }
-        __syncwarp();
-    } else if (warp == 1) {
-        // ===================== MMA issuer (leader) =====================
-        if (rank == 0 && lane == 0) {
-            const uint32_t idesc = umma_idesc_bf16(256, 256);
-            uint64_t it = 0; uint32_t kb = 0;
-            for (uint64_t n = 0; n < n_blocks; n++) {
-                const uint32_t ph2 = uint32_t(it & 1);
-                const uint32_t s = uint32_t(n % CVT_STAGES), ph = uint32_t((n / CVT_STAGES) & 1);
-                mbar_wait_cluster(&op_full[s], ph);
-                tc_fence_after();
-                const uint32_t x_addr = smem_u32(ring + s * CVT_STAGE_BYTES);
-                const uint64_t adesc = umma_desc_sw64(x_addr + CVT_RAW_BYTES);
-#pragma unroll
-                for (uint32_t j = 0; j < 2; j++) {
-                    if (kb == 0) { mbar_wait_cluster(&tempty[j], ph2 ^ 1); tc_fence_after(); }
-                    const uint64_t bdesc = umma_desc_sw64(x_addr + j * (CVT_XOP_BYTES / 2));
-#pragma unroll
-                    for (uint32_t k = 0; k < 2; k++)   // UMMA_K = 16 bf16 = 32 B
-                        tc_mma_pair<true>(tmem_base + j * 256, adesc + k * 2, bdesc + k * 2, idesc, (kb | k) != 0);
-                    if (kb + 1 == nkb) tc_commit_pair(&tfull[j]);
-                }
-                tc_commit_pair(&empty[s]);
-                if (++kb == nkb) { kb = 0; it++; }
-            }
-        }
-        __syncwarp();
-    } else if (warp >= 2 + GEMM_EPI_WARPS) {
-        // ===================== converters (both CTAs): fp32 SW128 tile -> bf16 SW64 operand, in place =====================
-        const uint32_t t = threadIdx.x - (2 + GEMM_EPI_WARPS) * 32;   // 0..127
-        const uint32_t op_full_leader0 = mapa_shared(smem_u32(&op_full[0]), 0);
-        for (uint64_t n = 0; n < n_blocks; n++) {
-            const uint32_t s = uint32_t(n % CVT_STAGES), ph = uint32_t((n / CVT_STAGES) & 1);
-            uint8_t *st = ring + s * CVT_STAGE_BYTES;
-            mbar_wait(&raw_full[s], ph);
-            uint4 w[8];
-#pragma unroll
-            for (uint32_t i = 0; i < 8; i++) {
-                const uint32_t o = t + 128 * i;            // output 16-byte chunk: row = o / 4, chunk = o % 4
-                const uint32_t r = o >> 2, oc = o & 3;     // r in [0,256): B tile r / 128, row r % 128 (tiles are contiguous)
-                const uint8_t *rs = st + r * 128;
-                const uint32_t x7 = r & 7;
-                const float4 a = *reinterpret_cast<const float4 *>(rs + (((2 * oc) ^ x7) << 4));
-                const float4 b = *reinterpret_cast<const float4 *>(rs + (((2 * oc + 1) ^ x7) << 4));
-                w[i].x = pack_bf16x2_rn(a.x, a.y); w[i].y = pack_bf16x2_rn(a.z, a.w);
-                w[i].z = pack_bf16x2_rn(b.x, b.y); w[i].w = pack_bf16x2_rn(b.z, b.w);
-            }
-            named_bar_sync(2, CVT_WARPS * 32);   // every fp32 value is in registers before the tile is overwritten
-#pragma unroll
-            for (uint32_t i = 0; i < 8; i++) {
-                const uint32_t o = t + 128 * i;
-                const uint32_t r = o >> 2, oc = o & 3;
-                *reinterpret_cast<uint4 *>(st + r * 64 + ((oc ^ ((r >> 1) & 3)) << 4)) = w[i];
-            }
-            fence_proxy_async();   // generic-proxy writes -> visible to the tensor core's async-proxy reads
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(op_full_leader0 + s * 8);
-        }
-    } else {
-        // ===================== epilogue (both CTAs): thread = TMEM lane = one query =====================
-        const uint32_t ew = warp - 2, quad = warp & 3, sel = ew >> 2;
-        const uint32_t m = quad * 32 + lane;
-        const uint32_t q = grp * GEMM_M + m;
-        const bool live = q < p.n_queries;
-        const uint32_t et = ew * 32 + lane;
-        const uint32_t lists = p.lists_per_query;
-        const uint32_t my_list = c * 2 + sel;
-        uint64_t *__restrict__ mybuf = p.cand + (size_t(q) * lists + my_list) * p.cap;
-        const uint32_t tempty_remote = mapa_shared(smem_u32(&tempty[sel]), 0);
-        GemmEpi e;
-        e.thr = live ? -INFINITY : INFINITY;
-        e.best = -INFINITY;
-        for (uint64_t it = 0; it < my_tiles; it++) {
-            const uint32_t ph = uint32_t(it & 1);
-            const uint64_t row0 = (c + it * p.ctas_per_group) * PAIR_TILE_ROWS;
-            float *inr = inr_s + uint32_t(it & 1) * PAIR_TILE_ROWS;
-#pragma unroll
-            for (uint32_t h = 0; h < 2; h++) {
-                const uint64_t r = row0 + et + h * 256;
-                inr[et + h * 256] = r < p.n_rows ? __ldg(p.inv_norm + r) : __int_as_float(0x7fc00000);
-            }
-            const unsigned int tg = (live && !p.max_mode) ? *reinterpret_cast<volatile unsigned int *>(p.thr + q) : 0u;
-            named_bar_sync(1, GEMM_EPI_WARPS * 32);
-            mbar_wait(&tfull[sel], ph);
-            tc_fence_after();
-            gemm_epilogue_tile(p, tmem_base + ((quad * 32u) << 16) + sel * 256, inr + sel * 256, 8, uint32_t(row0) + sel * 256, q,
-                               lists, my_list, tg, mybuf, e);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(tempty_remote);   // one arrival per warp on the leader's barrier
-        }
-        if (p.max_mode) p.gmax[size_t(q) * lists + my_list] = live ? e.best : -INFINITY;
-        else if (grp < p.n_qgroups) p.cand_cnt[size_t(q) * lists + my_list] = live ? e.cnt : 0;
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    if (warp == 1) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
+    for (uint32_t h = 0; h < 2; h++) {
+        if (p.max_mode) p.gmax[size_t(q[h]) * lists + my_list] = live[h] ? e[h].best : -INFINITY;
+        else p.cand_cnt[size_t(q[h]) * lists + my_list] = live[h] ? e[h].cnt : 0;
     }
 }
 
@@ -1044,12 +541,11 @@ __global__ void __launch_bounds__(512, 2) emb_gemm_merge_kernel(const GemmMergeP
 // disjoint group of rows; the limit-th largest of those group maxima is attained by `limit` distinct rows,
 // hence a valid lower bound LB of the query's global limit-th best approximate score — in the same
 // arithmetic the sweep compares with.  The sweep gathers every row above thr = LB - 2 eps (see the merge).
-// eps (cosine) = eps_const + rho_x + rho_q + rho_x rho_q, scaled to the sweep's cos*|q| units.
+// eps (cosine) = eps_const + rho_q, scaled to the sweep's cos*|q| units (the rows enter the sweep exactly: rho_x = 0).
 struct GemmThrParams {
     const float *gmax; uint32_t lists, limit;
     const float *inv_qnorm;
     float eps_const;
-    const float *rho_x;       // device scalar: max relative bf16 residual norm over the store's rows, or NULL
     const float *rho_q;       // [B] relative bf16 residual norm of each query, or NULL
     unsigned int *thr;        // [B] out: seed threshold, order-preserving uint (atomicMax'ed by the sweep)
     float *eps_v;             // [B] out
@@ -1065,9 +561,8 @@ __global__ void __launch_bounds__(256) gemm_thr_kernel(const GemmThrParams p) {
     }
     group_bitonic_desc(keys, np2, tid, blockDim.x, 0);
     if (tid == 0) {
-        const float rx = p.rho_x ? fminf(*p.rho_x, GEMM_RHO_BF16_WORST) : 0.f;
         const float rq = p.rho_q ? fminf(p.rho_q[q], GEMM_RHO_BF16_WORST) : 0.f;
-        const float eps_cos = p.eps_const + rx + rq + rx * rq;
+        const float eps_cos = p.eps_const + rq;
         const float iqn = p.inv_qnorm[q];
         const float ev = iqn > 0.f ? __fdiv_ru(eps_cos, iqn) : INFINITY;
         float thr = -INFINITY;

@@ -213,32 +213,19 @@ __device__ __forceinline__ float bf16_round_f32(float x) {
     const uint32_t r = ((u & 0x7fffffffu) > 0x7f800000u) ? (u | 0x00400000u) : (u + 0x7fffu + ((u >> 16) & 1u));
     return __uint_as_float(r & 0xffff0000u);
 }
-// rho_max (optional, fp32 stores): running max over the rows of |x - bf16(x)| / |x|, the relative residual norm
-// of rounding the row to bf16 — the store-side term of the tensor-core sweep's error bound (emb_gemm.cuh).
-// Kept as the bits of a non-negative float (ordered like unsigned ints); padded 0.1 % for the fp32 sums.
 template <typename T>
-__global__ void emb_inv_norm_kernel(const void *rows, uint32_t stride, uint64_t row_begin, uint64_t row_end,
-                                    float *inv_norm, unsigned int *rho_max) {
+__global__ void emb_inv_norm_kernel(const void *rows, uint32_t stride, uint64_t row_begin, uint64_t row_end, float *inv_norm) {
     const uint64_t r = row_begin + (uint64_t(blockIdx.x) * blockDim.x + threadIdx.x) / 32;
     const uint32_t lane = threadIdx.x & 31;
     if (r >= row_end) return;
     const void *rp = static_cast<const uint8_t *>(rows) + r * stride * RowLoad<T>::ESZ;
-    float s = 0.f, sd = 0.f;
+    float s = 0.f;
     for (uint32_t j = lane; j < stride / 4; j += 32) {
         const float4 x = RowLoad<T>::ld(rp, j);
         s = fmaf(x.x, x.x, s); s = fmaf(x.y, x.y, s); s = fmaf(x.z, x.z, s); s = fmaf(x.w, x.w, s);
-        if (rho_max) {
-            const float a = x.x - bf16_round_f32(x.x), b = x.y - bf16_round_f32(x.y);
-            const float c = x.z - bf16_round_f32(x.z), d = x.w - bf16_round_f32(x.w);
-            sd = fmaf(a, a, sd); sd = fmaf(b, b, sd); sd = fmaf(c, c, sd); sd = fmaf(d, d, sd);
-        }
     }
     s = warp_sum(s);
-    if (rho_max) sd = warp_sum(sd);
-    if (lane == 0) {
-        inv_norm[r] = s > 0.f ? 1.0f / sqrtf(s) : 0.f;
-        if (rho_max && s > 0.f) atomicMax(rho_max, __float_as_uint(sqrtf(sd / s) * 1.001f));
-    }
+    if (lane == 0) inv_norm[r] = s > 0.f ? 1.0f / sqrtf(s) : 0.f;
 }
 
 // Query preparation: zero-pad to stride, 1/|q| and (optional) rho_q = |q - bf16(q)| / |q| (one warp per query).

@@ -1,5 +1,5 @@
 // oc_common.cuh — shared device helpers: ordered score keys, bitonic sorts, mbarrier /
-// bulk-copy (TMA 1-D) PTX wrappers.  sm_100a only.
+// bulk-copy (TMA 1-D) PTX wrappers.  sm_90a only.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

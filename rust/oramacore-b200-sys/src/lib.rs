@@ -1,4 +1,4 @@
-//! Bindings for `include/oramacore_b200.h` (C ABI of the B200-native search hot path) and safe
+//! Bindings for `include/oramacore_b200.h` (C ABI of the H100-native search hot path) and safe
 //! wrappers shaped like the reference types they replace:
 //!   * `EmbeddingField`  ~ `EmbeddingFieldStorage` (read/index/embedding_field.rs:29-34)
 //!   * `StringFields`    ~ the `StringFieldStorage` set of an Index (read/index/string_field.rs:32-36)

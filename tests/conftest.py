@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "oracle")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu on the GPU box)")
 
 
 @pytest.fixture(scope="session")

@@ -1,4 +1,4 @@
-"""K2 (tcgen05 batched scan: gather every row within 2*eps of the limit-th best approximate score, exact
+"""K2 (wgmma batched scan: gather every row within 2*eps of the limit-th best approximate score, exact
 re-score of those) against K1 (exact sweep) and the oracle.  The tensor-core path must return bit-identical
 hits to the exact path: the low-precision sweep only selects candidates; every returned score is
 re-computed with K1's fp32 arithmetic.  Includes the adversarial inputs for a selection scheme:
@@ -70,11 +70,12 @@ def test_gemm_path_with_filter_delete_and_zero_query(gpu_ctx, orc):
     emb.close()
 
 
+# `pair` (here and in test_bf16_store_parity) names the cases after the CTA-pair switch of the Blackwell kernels;
+# the H100 build has a single sweep kernel, so the value selects nothing and the cases keep their ids.
 @pytest.mark.parametrize("n,B,pair", [(120000, 64, "1"), (150001, 300, "1"), (150001, 300, "0"), (4100, 256, "1")])
-def test_gemm_equals_exact_sweep_bitwise(gpu_ctx, monkeypatch, n, B, pair):
-    """B <= 128: one query group per CTA; B > 128: CTA pairs (cta_group::2, OC_GEMM_PAIR=1, the
-    default) or two groups per CTA (OC_GEMM_PAIR=0) — all must equal the exact sweep bit for bit."""
-    monkeypatch.setenv("OC_GEMM_PAIR", pair)
+def test_gemm_equals_exact_sweep_bitwise(gpu_ctx, n, B, pair):
+    """B <= 128: one query group; B > 128: several query groups, each swept by its own CTAs (300: a partial
+    last group) — all must equal the exact sweep bit for bit."""
     dim = 768
     rows = synth.make_vectors(n, dim, seed=13)
     qv, _ = synth.make_vector_queries(rows, B, seed=14)
@@ -94,12 +95,10 @@ def test_gemm_equals_exact_sweep_bitwise(gpu_ctx, monkeypatch, n, B, pair):
 
 @pytest.mark.parametrize("n,dim,model,B,pair", [(30000, 1024, "BGELarge", 5, None), (30000, 1024, "BGELarge", 200, None),
                                                  (50000, 768, "BGEBase", 64, None), (20000, 384, "BGESmall", 130, None),
-                                                 (30000, 1024, "BGELarge", 200, "1")])   # "1": force the CTA-pair kernel
-def test_bf16_store_parity(gpu_ctx, orc, monkeypatch, n, dim, model, B, pair):
+                                                 (30000, 1024, "BGELarge", 200, "1")])
+def test_bf16_store_parity(gpu_ctx, orc, n, dim, model, B, pair):
     """OC_DTYPE_BF16 store (BASELINE configs[4] shape, reduced): rows are bf16 values; every score is
     exact fp32 arithmetic on those values, so the oracle runs on the bf16-rounded rows."""
-    if pair is not None:
-        monkeypatch.setenv("OC_GEMM_PAIR", pair)
     rows = ob.from_bf16(ob.to_bf16(synth.make_vectors(n, dim, seed=n + dim)))
     qv, planted = synth.make_vector_queries(rows, B, seed=n + 1)
     emb = ob.EmbeddingFieldStorage(gpu_ctx, model, dtype="bf16")

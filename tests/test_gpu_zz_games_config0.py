@@ -1,8 +1,8 @@
 """BASELINE configs[0] — "benches/fulltext_simple.rs on games.json (CPU-only reference, plumbing)":
 fulltext search over the 1512 game documents (fields title + description) for the bench's own query
 strings and a few game-domain ones.  The corpus travels as a derived fixture (committed postings +
-resolved query terms + the oracle's answers; tests/golden/make_games_fixture.py), because
-/root/reference does not exist on the GPU box."""
+resolved query terms + the oracle's answers; tests/golden/make_games_fixture.py), so that
+the test needs nothing outside the repository."""
 import os
 
 import numpy as np
@@ -37,11 +37,6 @@ def test_oracle_reproduces_the_committed_answers(orc):
     # shape of the plumbing case: "technology" matches 20 games, "the" almost all, an unknown term none
     assert int(oc[0]) == 20 and int(oc[-1]) == 1468 and int(oc[-2]) == 0
 
-
-# Written after this round's GPU budget was spent: it only uses API paths the other GPU parity tests
-# exercise (multi-field, multi-term tokens, df counted on device) and is expected to pass, but until it has
-# run once on a B200 it must not be able to turn the GPU tier red (the file also sorts last).  Remove the
-# marker when it shows up as XPASS.
 
 @pytest.mark.gpu
 def test_gpu_fulltext_on_the_games_corpus(gpu_ctx, orc):
