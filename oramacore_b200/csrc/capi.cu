@@ -23,6 +23,7 @@
 #include "emb_gemm.cuh"
 #include "emb_scan.cuh"
 #include "fuse.cuh"
+#include "tmap.cuh"
 #include "oramacore_b200.h"
 
 using namespace oc;
@@ -502,30 +503,10 @@ static int run_exact_sweeps(oc_ctx *c, oc_emb *e, const float *inv_norm, const f
     return OC_OK;
 }
 
-// ---- TMA descriptors (driver entry point fetched through the runtime: no -lcuda link)
-typedef CUresult (*EncodeTiled_t)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static int make_tmap_2d(CUtensorMap *m, const void *base, uint64_t n_rows, uint32_t stride, uint32_t box_rows, bool bf16) {
-    static EncodeTiled_t fn = nullptr;
-    if (!fn) {
-        void *f = nullptr;
-        cudaDriverEntryPointQueryResult qr;
-        CU(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &qr));
-        if (!f || qr != cudaDriverEntryPointSuccess) return fail(OC_ERR_CUDA, "cuTensorMapEncodeTiled unavailable");
-        fn = (EncodeTiled_t)f;
-    }
-    cuuint64_t dims[2] = {stride, n_rows};
-    cuuint64_t strides[1] = {cuuint64_t(stride) * (bf16 ? 2 : 4)};
-    cuuint32_t box[2] = {bf16 ? 2 * GEMM_KB : GEMM_KB, box_rows};   // 128 bytes of K
-    cuuint32_t estr[2] = {1, 1};
-    // L2 promotion granule = the 128-byte box row: a larger granule would also pull the neighbouring K-block
-    // of the row into L2, which another CTA's load may evict before it is used (extra DRAM reads)
-    const CUtensorMapL2promotion promo = CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
-    CUresult r = fn(m, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void *>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, promo,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(OC_ERR_CUDA, "cuTensorMapEncodeTiled failed: %d", (int)r);
+// ---- TMA descriptors (tmap.cuh)
+static int tmap_2d(CUtensorMap *m, const void *base, uint64_t n_rows, uint32_t stride, uint32_t box_rows, bool bf16) {
+    const TmapStatus s = make_tmap_2d(m, base, n_rows, stride, box_rows, bf16);
+    if (s.what) return fail(OC_ERR_CUDA, "%s failed: %d", s.what, s.code);
     return OC_OK;
 }
 
@@ -591,8 +572,8 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
         launched(c);
         q_operand = c->q_bf16.p;
     }
-    OCTRY(make_tmap_2d(&tm_q, q_operand, Bpad, e->stride, GEMM_M, bf16));
-    OCTRY(make_tmap_2d(&tm_x, e->rows, e->n_rows, e->stride, GEMM_N, bf16));
+    OCTRY(tmap_2d(&tm_q, q_operand, Bpad, e->stride, GEMM_M, bf16));
+    OCTRY(tmap_2d(&tm_x, e->rows, e->n_rows, e->stride, GEMM_N, bf16));
     OCTRY(c->g_thr.ensure(size_t(B) * 4));
     OCTRY(c->g_eps.ensure(size_t(B) * 4));
     OCTRY(c->g_cand.ensure(size_t(Bpad) * lists * cap * 8));

@@ -25,7 +25,8 @@
 //     when the limit-th exact score clears bound + eps the exact top-`limit` is inside the
 //     candidate set.  Queries that fail the proof are re-run through the exact K1 sweep by the
 //     host (rare).
-//   * kernels in this file: emb_gemm_kernel<BF16>, gemm_thr_kernel, emb_gemm_merge_kernel.
+//   * kernels in this file: emb_gemm_kernel<BF16>, gemm_thr_kernel, emb_gemm_merge_kernel.  emb_gemm_kernel<BF16, true>
+//     (score dump) is instantiated only by the kernel test harness (tests/kernels).
 #pragma once
 #include <cuda.h>
 
@@ -84,6 +85,13 @@ struct GemmParams {
     uint32_t *ovf_cnt;         // [n_queries] (may exceed ovf_cap: the merge then sends the query to the exact sweep)
     uint32_t ovf_cap;
 };
+// emb_gemm_kernel<BF16, DUMP = true> (test harness only): the epilogue writes every approximate score v of a live
+// (query, row) pair to dump[q * n_rows + row] instead of gathering candidates
+struct GemmDumpParams : GemmParams {
+    float *dump;               // [n_queries][n_rows]
+};
+template <bool DUMP> struct GemmKernelParams { using type = GemmParams; };
+template <> struct GemmKernelParams<true> { using type = GemmDumpParams; };
 
 __host__ __device__ inline size_t gemm_smem_bytes() {
     return 1024 /*align slack*/ + size_t(GEMM_STAGES) * GEMM_STAGE_BYTES + GEMM_CONSUMER_WG * 2 * GEMM_N * 4 /*inv norms*/
@@ -224,9 +232,10 @@ __device__ __noinline__ void gemm_compact(const GemmParams &p, uint32_t need, ui
 // One CTA = one query group (128 queries) x one row partition c of the store (tiles c, c + ctas_per_group, ...).
 // wgmma D fragment of m64n128 (per warpgroup): warp w holds rows [16w, 16w + 16); lane holds rows lane/4 and
 // lane/4 + 8, columns 8j + 2 (lane % 4) + {0, 1} for j = 0..15, in d[4j + 2h + {0, 1}] (h = row half).
-template <bool BF16>
+template <bool BF16, bool DUMP = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_x, const GemmParams p) {
+emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_x,
+                const typename GemmKernelParams<DUMP>::type p) {
     extern __shared__ __align__(1024) uint8_t smem_gemm[];
     // SWIZZLE_128B tiles need 1024-byte alignment of the shared-memory address
     uint8_t *ring = smem_gemm + ((1024u - (smem_u32(smem_gemm) & 1023u)) & 1023u);
@@ -300,7 +309,7 @@ emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         unsigned int tg[2];
 #pragma unroll
         for (uint32_t h = 0; h < 2; h++)
-            tg[h] = (live[h] && !p.max_mode) ? *reinterpret_cast<volatile unsigned int *>(p.thr + q[h]) : 0u;
+            tg[h] = (!DUMP && live[h] && !p.max_mode) ? *reinterpret_cast<volatile unsigned int *>(p.thr + q[h]) : 0u;
         uint32_t prev_s = 0;
         for (uint32_t kb = 0; kb < nkb; kb++, n++) {
             const uint32_t s = uint32_t(n % GEMM_STAGES), ph = uint32_t((n / GEMM_STAGES) & 1);
@@ -335,6 +344,15 @@ emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
                 v[2 * j + 0] = d[4 * j + 2 * h + 0] * w.x;   // cos * |q|
                 v[2 * j + 1] = d[4 * j + 2 * h + 1] * w.y;
             }
+            if constexpr (DUMP) {
+                const uint64_t rb = row0 + 2 * (lane & 3);
+#pragma unroll
+                for (uint32_t j = 0; j < 32; j++) {
+                    const uint64_t r = rb + 8 * (j >> 1) + (j & 1);
+                    if (live[h] && r < p.n_rows) p.dump[size_t(q[h]) * p.n_rows + r] = v[j];
+                }
+                continue;
+            }
             if (p.max_mode) {
 #pragma unroll
                 for (uint32_t j = 0; j < 32; j++) E.best = fmaxf(E.best, v[j]);   // NaN (dead rows) ignored
@@ -354,10 +372,12 @@ emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
             if (need) gemm_compact(p, need, q[h], my_list, lane, E);
         }
     }
+    if constexpr (!DUMP) {
 #pragma unroll
-    for (uint32_t h = 0; h < 2; h++) {
-        if (p.max_mode) p.gmax[size_t(q[h]) * lists + my_list] = live[h] ? e[h].best : -INFINITY;
-        else p.cand_cnt[size_t(q[h]) * lists + my_list] = live[h] ? e[h].cnt : 0;
+        for (uint32_t h = 0; h < 2; h++) {
+            if (p.max_mode) p.gmax[size_t(q[h]) * lists + my_list] = live[h] ? e[h].best : -INFINITY;
+            else p.cand_cnt[size_t(q[h]) * lists + my_list] = live[h] ? e[h].cnt : 0;
+        }
     }
 }
 
@@ -489,9 +509,7 @@ __global__ void __launch_bounds__(512, 2) emb_gemm_merge_kernel(const GemmMergeP
                 const float4 x = xr[j], y = qp[lane + 32 * j];
                 acc = fmaf(x.x, y.x, acc); acc = fmaf(x.y, y.y, acc); acc = fmaf(x.z, y.z, acc); acc = fmaf(x.w, y.w, acc);
             }
-        const float dot = warp_sum(acc);
-        const float cosv = dot * p.inv_norm[row] * iqn;
-        const float kf = -(1.0f - cosv);
+        const float kf = cos_rank_key(warp_sum(acc), p.inv_norm[row], iqn);
         __syncwarp();
         if (lane == 0) exact[i] = make_key(kf, row);
     }

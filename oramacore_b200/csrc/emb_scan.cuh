@@ -67,6 +67,14 @@ template <> struct RowLoad<bf16_t> {
     }
 };
 
+// Rank key of a row: -(cosine distance), distance = 1 - cos (embedding_field.rs:246-249), cos = dot * inv|x| * inv|q|.
+// The multiply by inv|q| is fused with the subtraction.  Spelled out so that every kernel that scores a row (K1 at
+// every QB, the K2 re-score) rounds identically: left to the compiler, the contraction depended on the surrounding
+// code, and K1 with QB = 1 scored the same row a few ulp apart from QB = 2 / 4 and from K2.
+__device__ __forceinline__ float cos_rank_key(float dot, float inr, float iqn) {
+    return -fmaf(-__fmul_rn(dot, inr), iqn, 1.0f);
+}
+
 template <int NCH, int QB, typename T>
 __global__ void __launch_bounds__(SCAN_THREADS, 1) emb_scan_kernel(const ScanParams p) {
     extern __shared__ __align__(16) uint8_t smem[];
@@ -165,10 +173,7 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) emb_scan_kernel(const ScanPar
             const float inr = sn[r];
 #pragma unroll
             for (int q = 0; q < QB; q++) {
-                const float dot = warp_sum(acc[q]);
-                const float cosv = dot * inr * iqn[q];
-                // rank key = -(cosine distance), distance = 1 - cos (embedding_field.rs:246-249)
-                const float kf = -(1.0f - cosv);
+                const float kf = cos_rank_key(warp_sum(acc[q]), inr, iqn[q]);
                 if (kf > tau[q]) {  // warp-uniform
                     if (cnt[q] == p.wcap) {
                         warp_bitonic_desc(mybuf[q], p.wcap, lane);
