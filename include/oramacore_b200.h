@@ -249,6 +249,39 @@ int oc_facets_add_number_field(oc_facets *f, uint64_t n, const double *values_so
 int oc_search_facets(oc_ctx *ctx, oc_emb *emb, oc_str *str, oc_facets *facets, const oc_search_params *p,
                      const oc_facet_req *reqs, uint32_t n_reqs, uint64_t *out_counts);
 
+/* ---- groups over the score map ------------------------------------------------------------------
+ * GroupContext::execute (read/index/group.rs) + sort_groups (read/sort.rs:129-230, the branch without sort_by).
+ * A group is one combination of variants, one variant per listed field: the Cartesian product of the fields'
+ * variants (generate_group_combinations), numbered mixed-radix over `fields` in the order given, the last field
+ * varying fastest; n_groups = the product of the fields' variant counts.  Variant index: for a bool or string_filter
+ * field the index it was registered with in oc_facets_add_field; for a number field the rank of its distinct value
+ * in ascending order (values equal under == are one value).  Every combination is a group, also when no document
+ * holds it.  A document listed under several variants of a field belongs to every matching group; ids >= the
+ * facets' nbits are ignored.  Built once on the host from the fields' device lists (setup, not the hot path) and
+ * kept on the device as one CSR of the groups, document ids ascending inside a group.  The handle does not refer to
+ * `facets` afterwards.  OC_ERR_UNSUPPORTED: more than 2^20 groups, or a group of more than 2^32 - 2 documents. */
+typedef struct oc_group_by oc_group_by;
+int oc_group_by_create(oc_facets *facets, const uint32_t *fields, uint32_t n_fields, oc_group_by **out,
+                       uint64_t *out_n_groups);
+void oc_group_by_destroy(oc_group_by *g);
+/* Hits and count exactly as oc_search with the same p; for query q and group g the top max_results documents of
+ * {d in group g : d is a key of q's score map}, by final score descending, ties by ascending document id, NaN scores
+ * dropped.  The score map is the one the hits come from: where-filter applied, uncommitted deletes excluded, OMC
+ * multipliers applied.  max_results in [0, OC_MAX_TOPK] (0: every group present and empty).
+ * p->limit == 0 is accepted here (not by oc_search): the hit arrays (out_doc_ids, out_scores, out_n; may be NULL) are
+ * not written, the vector stage gets depth 0 (limit_hint = 0: no vector launch), so a hybrid score map is the fulltext
+ * map alone and a vector-mode map is empty; out_count is written.
+ * out_group_doc_ids / out_group_scores: B x n_groups x max_results, best first; out_group_n: B x n_groups.
+ * Workspace: B x ceil(rows / 8192) x 8192 x 4 bytes of per-row scores on the device (1 GiB at B = 256 over 1M
+ * string rows), OC_ERR_OOM when it cannot be allocated: pass smaller batches.  B <= 65535.
+ * OC_ERR_UNSUPPORTED: p->sharded (hybrid normalisation and the vector set are global across shards),
+ * max_results > OC_MAX_TOPK.  OC_ERR_INVALID: a handle of another ctx.  A failed call writes nothing.
+ * Multi-index collections: run each index with limit' = limit + offset, vector_limit = limit as for oc_search, and
+ * merge the group arrays with oc_merge_results over n_queries = B x n_groups, limit' = max_results. */
+int oc_search_groups(oc_ctx *ctx, oc_emb *emb, oc_str *str, oc_group_by *groups, const oc_search_params *p,
+                     uint32_t max_results, uint64_t *out_doc_ids, float *out_scores, uint32_t *out_n, uint64_t *out_count,
+                     uint64_t *out_group_doc_ids, float *out_group_scores, uint32_t *out_group_n);
+
 /* ---- multi-index collections ---------------------------------------------------------------------
  * search_on_indexes runs every index of a collection into ONE score map (read/search.rs:304-338,
  * token_score.rs:472-499): document ids are unique per collection, so the per-index maps are disjoint; hybrid

@@ -165,6 +165,10 @@ struct Bm25Params {
     uint32_t cls_off[BM25_CLASSES];   // first item of each class
     uint32_t cls_nq[BM25_CLASSES];    // queries in the class
     uint32_t cls_q0[BM25_CLASSES];    // first perm entry of the class
+    // Group mode (the ROWFT instantiations of K3 / K3b; set together with matched_bits): out, [n_queries][n_tiles * TILE]
+    // raw fulltext score of every matched row, written where its matched bit is set — slots of unmatched rows are
+    // never written and must be read through the bitmap.  Last member so the other fields keep their offsets.
+    float *row_ft;
 };
 __host__ __device__ __forceinline__ void bm25_item_decode(const Bm25Params &p, const uint32_t k, uint32_t &tile, uint32_t &q) {
     if (!p.perm) { tile = k / p.n_queries; q = k % p.n_queries; return; }
@@ -297,7 +301,7 @@ __device__ inline void block_keep_top(uint64_t *buf, uint32_t count, uint32_t ca
 }
 
 // ---- the scorer: one CTA per (query, tile) ----
-template <bool MULTI, bool THRESH, bool OMC>
+template <bool MULTI, bool THRESH, bool OMC, bool ROWFT = false>
 __global__ void __launch_bounds__(BM25_THREADS) bm25_tile_kernel(const Bm25Params p) {
     extern __shared__ __align__(16) uint8_t smem[];
     float *score = reinterpret_cast<float *>(smem);
@@ -519,6 +523,7 @@ __global__ void __launch_bounds__(BM25_THREADS) bm25_tile_kernel(const Bm25Param
                     const bool present = s != 0.f;
                     matched += present ? 1u : 0u;
                     if (p.matched_bits && present) atomicOr(&s_mbits[(l0 + u) >> 5], 1u << ((l0 + u) & 31));
+                    if (ROWFT && present) p.row_ft[size_t(q) * p.n_tiles * BM25_TILE + row0 + l0 + u] = s;
                     lmax = fmaxf(lmax, s);
                     lmin = fminf(lmin, s);
                     float proxy = __fsub_rn(s, mh);
@@ -671,7 +676,7 @@ __global__ void __launch_bounds__(256) bm25_flatten_kernel(const Bm25Params p, I
     flat[gid] = it;
 }
 
-template <bool THRESH, bool OMC>
+template <bool THRESH, bool OMC, bool ROWFT = false>
 __global__ void __launch_bounds__(BM25_THREADS, 1024 / BM25_THREADS) bm25_tile2_kernel(const Bm25Params p, const ItemTok *flat, unsigned int *work_counter) {
     extern __shared__ __align__(16) uint8_t smem[];
     float *score = reinterpret_cast<float *>(smem);
@@ -880,6 +885,7 @@ __global__ void __launch_bounds__(BM25_THREADS, 1024 / BM25_THREADS) bm25_tile2_
         auto visit = [&](float s, uint32_t l) -> bool {   // one matched row
             matched++;
             if (want_bits) atomicOr(&s_mbits[l >> 5], 1u << (l & 31));
+            if (ROWFT) p.row_ft[size_t(q) * p.n_tiles * BM25_TILE + row0 + l] = s;
             lmax = fmaxf(lmax, s);
             lmin = fminf(lmin, s);
             return consider(s, l);

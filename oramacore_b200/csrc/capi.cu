@@ -23,6 +23,7 @@
 #include "emb_gemm.cuh"
 #include "emb_scan.cuh"
 #include "fuse.cuh"
+#include "group.cuh"
 #include "tmap.cuh"
 #include "oramacore_b200.h"
 
@@ -127,7 +128,7 @@ static bool is_pinned_host(const void *p) {
     return a.type == cudaMemoryTypeHost;
 }
 
-enum { EV_START, EV_H2D, EV_DEV, EV_D2H, EV_SCAN0, EV_SCAN1, EV_BM0, EV_BM1, EV_FUSE0, EV_FUSE1, EV_COMM0, EV_COMM1, EV_SWEEP0, EV_SWEEP1, EV_RR0, EV_RR1, EV_N };
+enum { EV_START, EV_H2D, EV_DEV, EV_D2H, EV_SCAN0, EV_SCAN1, EV_BM0, EV_BM1, EV_FUSE0, EV_FUSE1, EV_COMM0, EV_COMM1, EV_SWEEP0, EV_SWEEP1, EV_RR0, EV_RR1, EV_GRP0, EV_GRP1, EV_N };
 
 constexpr size_t P2P_WIN_BYTES = size_t(1) << 20;   // per (parity, source rank): a batch's records must fit (256 queries x 520 B = 133 KB)
 constexpr uint32_t P2P_MAX_Q = 4096;
@@ -153,6 +154,7 @@ struct oc_ctx {
     DevBuf seg, df_dev, row_ok, tau, cand_key, cand_ft, cand_cnt, tile_cnt, tile_max, tile_min, min_hint;
     DevBuf out_blob, shard_send, shard_recv, work_ctr, flat_desc, mbits, dbits, facet_req, facet_out;
     bool gemm_pending = false; const float *gemm_inv_norm = nullptr;
+    DevBuf row_ft, grp_vdoc, grp_vscore, grp_vn, grp_gmin, grp_den, grp_doc, grp_score, grp_n;   // oc_search_groups
     DevBuf q_bf16, q_rho, pre_post, dense_buf, g_thr, g_eps, g_ovf, g_ovfcnt, g_resc, g_cand, g_cnt, g_flag, g_max, r_qpad, r_qinv, r_map, r_doc, r_score, r_row, r_cnt, r_raw;
 
     HostBuf h_in, h_out, h_in0;   // h_in0 / in_blob0: query vectors + filter, uploaded before the descriptors
@@ -207,7 +209,8 @@ extern "C" void oc_shutdown(oc_ctx *c) {
                       &c->v_score, &c->v_row, &c->v_cnt, &c->v_srow, &c->v_ft, &c->v_present, &c->v_raw, &c->seg, &c->df_dev,
                       &c->row_ok, &c->tau, &c->cand_key, &c->cand_ft, &c->cand_cnt, &c->tile_cnt, &c->tile_max,
                       &c->tile_min, &c->min_hint, &c->out_blob, &c->shard_send, &c->shard_recv, &c->work_ctr, &c->flat_desc, &c->mbits, &c->dbits, &c->facet_req, &c->facet_out, &c->q_bf16, &c->q_rho, &c->pre_post, &c->dense_buf, &c->g_thr, &c->g_eps, &c->g_ovf, &c->g_ovfcnt, &c->g_resc, &c->g_cand, &c->g_cnt, &c->g_max,
-                      &c->g_flag, &c->r_qpad, &c->r_qinv, &c->r_map, &c->r_doc, &c->r_score, &c->r_row, &c->r_cnt, &c->r_raw};
+                      &c->g_flag, &c->r_qpad, &c->r_qinv, &c->r_map, &c->r_doc, &c->r_score, &c->r_row, &c->r_cnt, &c->r_raw,
+                      &c->row_ft, &c->grp_vdoc, &c->grp_vscore, &c->grp_vn, &c->grp_gmin, &c->grp_den, &c->grp_doc, &c->grp_score, &c->grp_n};
     for (DevBuf *b : bufs) b->release();
     c->h_in.release(); c->h_out.release();
     for (int i = 0; i < EV_N; i++) if (c->ev[i]) cudaEventDestroy(c->ev[i]);
@@ -1329,20 +1332,20 @@ static inline float host_idf(float total_documents, uint64_t corpus_df) {
     return log1pf(ratio);
 }
 
-template <bool MULTI, bool THRESH, bool OMC>
+template <bool MULTI, bool THRESH, bool OMC, bool ROWFT>
 static int launch_tile_t(oc_ctx *c, const Bm25Params &bp, uint32_t grid, size_t smem, cudaStream_t st) {
     // (static smem counts against the 227 KB cap)
-    if (smem_cfg_needed(c->device, (const void *)bm25_tile_kernel<MULTI, THRESH, OMC>, smem))
-        CU(cudaFuncSetAttribute(bm25_tile_kernel<MULTI, THRESH, OMC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    bm25_tile_kernel<MULTI, THRESH, OMC><<<grid, BM25_THREADS, smem, st>>>(bp);
+    if (smem_cfg_needed(c->device, (const void *)bm25_tile_kernel<MULTI, THRESH, OMC, ROWFT>, smem))
+        CU(cudaFuncSetAttribute(bm25_tile_kernel<MULTI, THRESH, OMC, ROWFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    bm25_tile_kernel<MULTI, THRESH, OMC, ROWFT><<<grid, BM25_THREADS, smem, st>>>(bp);
     launched(c);
     CU(cudaGetLastError());
     return OC_OK;
 }
-template <bool THRESH, bool OMC>
+template <bool THRESH, bool OMC, bool ROWFT>
 static int launch_tile2_t(oc_ctx *c, const Bm25Params &bp, size_t smem, cudaStream_t st, const ItemTok *flat, unsigned int *counter) {
-    if (smem_cfg_needed(c->device, (const void *)bm25_tile2_kernel<THRESH, OMC>, smem))
-        CU(cudaFuncSetAttribute(bm25_tile2_kernel<THRESH, OMC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (smem_cfg_needed(c->device, (const void *)bm25_tile2_kernel<THRESH, OMC, ROWFT>, smem))
+        CU(cudaFuncSetAttribute(bm25_tile2_kernel<THRESH, OMC, ROWFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     static std::mutex occ_mu;                         // occupancy per (device, shared-memory size): queried once
     static std::map<std::pair<int, size_t>, int> occ;
     int per_sm = 1;
@@ -1350,13 +1353,13 @@ static int launch_tile2_t(oc_ctx *c, const Bm25Params &bp, size_t smem, cudaStre
         std::lock_guard<std::mutex> g(occ_mu);
         auto it = occ.find(std::make_pair(c->device, smem));
         if (it == occ.end()) {
-            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bm25_tile2_kernel<THRESH, OMC>, BM25_THREADS, smem));
+            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bm25_tile2_kernel<THRESH, OMC, ROWFT>, BM25_THREADS, smem));
             occ[std::make_pair(c->device, smem)] = per_sm;
         } else per_sm = it->second;
     }
     const uint64_t items = uint64_t(bp.n_tiles) * bp.n_queries;
     const uint32_t grid = (uint32_t)std::min<uint64_t>(items, uint64_t(std::max(per_sm, 1)) * c->prop.multiProcessorCount);
-    bm25_tile2_kernel<THRESH, OMC><<<grid, BM25_THREADS, smem, st>>>(bp, flat, counter);
+    bm25_tile2_kernel<THRESH, OMC, ROWFT><<<grid, BM25_THREADS, smem, st>>>(bp, flat, counter);
     launched(c);
     CU(cudaGetLastError());
     return OC_OK;
@@ -1441,26 +1444,42 @@ static int launch_tile(oc_ctx *c, const Bm25Params &bp_in, uint32_t grid, bool m
         }
         const size_t smem = bm25_tile2_smem_bytes(thr, omc, bp.cap);
         const int sel = (thr ? 2 : 0) | (omc ? 1 : 0);
+        if (bp.row_ft) switch (sel) {   // group mode: the matched rows' scores too
+            case 0: return launch_tile2_t<false, false, true>(c, bp, smem, st, flat, counter);
+            case 1: return launch_tile2_t<false, true, true>(c, bp, smem, st, flat, counter);
+            case 2: return launch_tile2_t<true, false, true>(c, bp, smem, st, flat, counter);
+            default: return launch_tile2_t<true, true, true>(c, bp, smem, st, flat, counter);
+        }
         switch (sel) {
-            case 0: return launch_tile2_t<false, false>(c, bp, smem, st, flat, counter);
-            case 1: return launch_tile2_t<false, true>(c, bp, smem, st, flat, counter);
-            case 2: return launch_tile2_t<true, false>(c, bp, smem, st, flat, counter);
-            default: return launch_tile2_t<true, true>(c, bp, smem, st, flat, counter);
+            case 0: return launch_tile2_t<false, false, false>(c, bp, smem, st, flat, counter);
+            case 1: return launch_tile2_t<false, true, false>(c, bp, smem, st, flat, counter);
+            case 2: return launch_tile2_t<true, false, false>(c, bp, smem, st, flat, counter);
+            default: return launch_tile2_t<true, true, false>(c, bp, smem, st, flat, counter);
         }
     }
     Bm25Params bp = bp_in;
     bp.perm = nullptr;
     const size_t smem = bm25_smem_bytes(multi, thr, omc, bp.cap);
     const int sel = (multi ? 4 : 0) | (thr ? 2 : 0) | (omc ? 1 : 0);
+    if (bp.row_ft) switch (sel) {   // group mode: the matched rows' scores too
+        case 0: return launch_tile_t<false, false, false, true>(c, bp, grid, smem, st);
+        case 1: return launch_tile_t<false, false, true, true>(c, bp, grid, smem, st);
+        case 2: return launch_tile_t<false, true, false, true>(c, bp, grid, smem, st);
+        case 3: return launch_tile_t<false, true, true, true>(c, bp, grid, smem, st);
+        case 4: return launch_tile_t<true, false, false, true>(c, bp, grid, smem, st);
+        case 5: return launch_tile_t<true, false, true, true>(c, bp, grid, smem, st);
+        case 6: return launch_tile_t<true, true, false, true>(c, bp, grid, smem, st);
+        default: return launch_tile_t<true, true, true, true>(c, bp, grid, smem, st);
+    }
     switch (sel) {
-        case 0: return launch_tile_t<false, false, false>(c, bp, grid, smem, st);
-        case 1: return launch_tile_t<false, false, true>(c, bp, grid, smem, st);
-        case 2: return launch_tile_t<false, true, false>(c, bp, grid, smem, st);
-        case 3: return launch_tile_t<false, true, true>(c, bp, grid, smem, st);
-        case 4: return launch_tile_t<true, false, false>(c, bp, grid, smem, st);
-        case 5: return launch_tile_t<true, false, true>(c, bp, grid, smem, st);
-        case 6: return launch_tile_t<true, true, false>(c, bp, grid, smem, st);
-        default: return launch_tile_t<true, true, true>(c, bp, grid, smem, st);
+        case 0: return launch_tile_t<false, false, false, false>(c, bp, grid, smem, st);
+        case 1: return launch_tile_t<false, false, true, false>(c, bp, grid, smem, st);
+        case 2: return launch_tile_t<false, true, false, false>(c, bp, grid, smem, st);
+        case 3: return launch_tile_t<false, true, true, false>(c, bp, grid, smem, st);
+        case 4: return launch_tile_t<true, false, false, false>(c, bp, grid, smem, st);
+        case 5: return launch_tile_t<true, false, true, false>(c, bp, grid, smem, st);
+        case 6: return launch_tile_t<true, true, false, false>(c, bp, grid, smem, st);
+        default: return launch_tile_t<true, true, true, false>(c, bp, grid, smem, st);
     }
 }
 
@@ -1475,10 +1494,23 @@ struct FacetJob {   // oc_search_facets: count, per query, the matched documents
 };
 static int run_facets(oc_ctx *c, const FacetJob &fj, uint32_t B, bool has_ft, bool has_v, const StrSnap *S, uint32_t n_tiles,
                       uint32_t vlimit);
+struct GroupJob {   // oc_search_groups: the top max_results documents of every (query, group)
+    oc_group_by *g;
+    uint32_t max_results;
+    uint64_t *out_doc;      // [B][G][max_results]
+    float *out_score;
+    uint32_t *out_n;        // [B][G]
+};
+static int run_groups(oc_ctx *c, const GroupJob &gj, uint32_t B, int mode, const StrSnap *S, uint32_t n_tiles, uint32_t vlimit,
+                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc);
 
+// gj != NULL: oc_search_groups.  Then limit == 0 is allowed: the hits are not written (out_doc_ids / out_scores / out_n
+// may be NULL), the vector stage gets depth 0 and the fulltext stage runs with one candidate slot per tile.
 static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, uint64_t *out_doc_ids,
-                       float *out_scores, uint32_t *out_n, uint64_t *out_count, const FacetJob *fj) {
-    if (!c || !p || !out_doc_ids || !out_scores || !out_n || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
+                       float *out_scores, uint32_t *out_n, uint64_t *out_count, const FacetJob *fj, const GroupJob *gj = nullptr) {
+    if (!c || !p || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
+    const bool write_hits = !gj || p->limit > 0;
+    if (write_hits && (!out_doc_ids || !out_scores || !out_n)) return fail(OC_ERR_INVALID, "NULL argument");
     const uint32_t B = p->n_queries;
     if (B == 0) return OC_OK;
     const bool has_v = p->mode == OC_MODE_VECTOR || p->mode == OC_MODE_HYBRID;
@@ -1488,12 +1520,13 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     if (has_ft && (!str || !p->q_token_offsets)) return fail(OC_ERR_INVALID, "fulltext/hybrid mode needs str and tokens");
     if (emb && emb->ctx != c) return fail(OC_ERR_INVALID, "emb belongs to another ctx");
     if (str && str->ctx != c) return fail(OC_ERR_INVALID, "str belongs to another ctx");
-    if (p->limit == 0) return fail(OC_ERR_INVALID, "limit must be >= 1");
-    const uint64_t n_keep64 = uint64_t(p->limit) + p->offset;
+    if (p->limit == 0 && !gj) return fail(OC_ERR_INVALID, "limit must be >= 1");
+    const uint32_t limit = write_hits ? p->limit : 1;
+    const uint64_t n_keep64 = uint64_t(limit) + p->offset;
     if (n_keep64 > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "limit+offset %llu > %u", (unsigned long long)n_keep64, OC_MAX_TOPK);
     const uint32_t n_keep = (uint32_t)n_keep64;
     // limit_hint = limit, NOT limit+offset (search.rs:330-336); vector_limit lets a multi-index caller keep that depth
-    const uint32_t vlimit = p->vector_limit ? p->vector_limit : p->limit;
+    const uint32_t vlimit = !write_hits ? 0u : p->vector_limit ? p->vector_limit : limit;
     if (vlimit > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "vector_limit %u > %u", vlimit, OC_MAX_TOPK);
     if (p->sharded && !c->comm.ready()) return fail(OC_ERR_COMM, "sharded search without oc_comm_init");
 
@@ -1542,8 +1575,13 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         CU(cudaEventRecord(c->ev[EV_H2D], c->stream));
         h2d_early = pk0.total;
         if (filter_h) filter_dev = reinterpret_cast<const uint64_t *>(c->in_blob0.as<uint8_t>() + o_flt);
-        OCTRY(run_vector_stage(c, emb, reinterpret_cast<const float *>(c->in_blob0.as<uint8_t>() + o_qv), B, vlimit, p->similarity,
-                               filter_dev, filter_nbits));
+        if (vlimit) {
+            OCTRY(run_vector_stage(c, emb, reinterpret_cast<const float *>(c->in_blob0.as<uint8_t>() + o_qv), B, vlimit, p->similarity,
+                                   filter_dev, filter_nbits));
+        } else {   // limit_hint 0 (groups only): no vector hit
+            OCTRY(c->v_cnt.ensure(size_t(B) * 4));
+            CU(cudaMemsetAsync(c->v_cnt.p, 0, size_t(B) * 4, c->stream));
+        }
     }
 
     // ------------------------------------------------------------ host: descriptors
@@ -1787,7 +1825,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     Bm25Params bp{};
     float *min_hint_dev = nullptr;
     unsigned int *tile_counter = nullptr;
-    const size_t o_doc = 0, o_sc = size_t(B) * p->limit * 8, o_n = o_sc + size_t(B) * p->limit * 4;
+    const size_t o_doc = 0, o_sc = size_t(B) * limit * 8, o_n = o_sc + size_t(B) * limit * 4;
     const size_t o_cnt = (o_n + size_t(B) * 4 + 7) & ~size_t(7), o_min = o_cnt + size_t(B) * 8;
     const size_t o_gflag = o_min + size_t(B) * 4;                       // sharded: OR over the ranks of the per-query overflow flags
     const size_t out_bytes = o_gflag + ((size_t(B) + 3) & ~size_t(3));
@@ -1895,9 +1933,13 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
                 off += cls_nq[g] * n_tiles; q0 += cls_nq[g];
             }
         }
-        if (fj) {   // facets: the tile kernels also emit the bitmap of matched rows (every (query, tile) item writes its 256 words)
+        if (fj || gj) {   // facets / groups: the tile kernels also emit the bitmap of matched rows (every (query, tile) item writes its 256 words)
             OCTRY(c->mbits.ensure(size_t(B) * std::max<uint32_t>(n_tiles, 1) * (BM25_TILE / 32) * 4));
             bp.matched_bits = c->mbits.as<uint32_t>();
+        }
+        if (gj && n_tiles) {   // groups: and the raw score of each matched row
+            OCTRY(c->row_ft.ensure(size_t(B) * n_tiles * BM25_TILE * 4));
+            bp.row_ft = c->row_ft.as<float>();
         }
         if (n_tiles) OCTRY(launch_tile(c, bp, n_tiles * B, any_multi, thr, omc_tile, ps, max_tokens, tile_counter, need_df));
         CU(cudaEventRecord(c->ev[EV_BM1], ps));
@@ -1917,6 +1959,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         OCTRY(c->v_srow.ensure(size_t(B) * vlimit * 4));
         OCTRY(c->v_ft.ensure(size_t(B) * vlimit * 4));
         OCTRY(c->v_present.ensure(size_t(B) * vlimit));
+        if (vlimit) {
         map_docs_to_rows_kernel<<<(B * vlimit + 255) / 256, 256, 0, c->stream>>>(
             c->v_doc.as<uint64_t>(), c->v_cnt.as<uint32_t>(), vlimit, B, S->row_doc, S->n_rows, c->v_srow.as<uint32_t>());
         launched(c);
@@ -1928,11 +1971,12 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         bm25_point_kernel<<<(B * vlimit * 32 + 255) / 256, 256, 0, c->stream>>>(pp);
         launched(c);
         CU(cudaGetLastError());
+        }
     }
 
     // ------------------------------------------------------------ fusion + top-n (+ shard exchange)
     fp = FuseParams{};
-    fp.mode = p->mode; fp.n_tiles = n_tiles; fp.n_keep = n_keep; fp.limit = p->limit; fp.offset = p->offset;
+    fp.mode = p->mode; fp.n_tiles = n_tiles; fp.n_keep = n_keep; fp.limit = limit; fp.offset = p->offset;
     {   // smallest power-of-two key buffer that takes the candidates in one round (sort cost ~ capb log^2 capb)
         const uint64_t total = (has_ft ? uint64_t(n_tiles) * n_keep : 0) + (has_v ? vlimit : 0);
         // up to 16 K keys (128 KB) stay in shared memory and go through one radix select; the streaming bitonic path behind
@@ -1956,9 +2000,20 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     fp.out_doc = reinterpret_cast<uint64_t *>(dout + o_doc); fp.out_score = reinterpret_cast<float *>(dout + o_sc);
     fp.out_n = reinterpret_cast<uint32_t *>(dout + o_n); fp.out_count = reinterpret_cast<unsigned long long *>(dout + o_cnt);
     fp.out_min = reinterpret_cast<float *>(dout + o_min);
+    if (gj) {   // groups: K4 also exports the normalisation and the vector part of the score map
+        const uint32_t vs = std::max<uint32_t>(vlimit, 1);
+        OCTRY(c->grp_vdoc.ensure(size_t(B) * vs * 8));
+        OCTRY(c->grp_vscore.ensure(size_t(B) * vs * 4));
+        OCTRY(c->grp_vn.ensure(size_t(B) * 4));
+        OCTRY(c->grp_gmin.ensure(size_t(B) * 4));
+        OCTRY(c->grp_den.ensure(size_t(B) * 4));
+        fp.out_vdoc = c->grp_vdoc.as<uint64_t>(); fp.out_vscore = c->grp_vscore.as<float>(); fp.out_vn = c->grp_vn.as<uint32_t>();
+        fp.out_gmin = c->grp_gmin.as<float>(); fp.out_den = c->grp_den.as<float>();
+    }
     fuse_smem = size_t(fp.capb) * 8 + size_t(std::max<uint32_t>(32, next_pow2(n_keep))) * 8 + size_t(vlimit) * 8 + 64;
-    if (smem_cfg_needed(c->device, (const void *)fuse_topk_kernel, fuse_smem))
-        CU(cudaFuncSetAttribute(fuse_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fuse_smem));
+    if (smem_cfg_needed(c->device, gj ? (const void *)fuse_topk_kernel<true> : (const void *)fuse_topk_kernel<false>, fuse_smem))
+        CU(cudaFuncSetAttribute(gj ? (const void *)fuse_topk_kernel<true> : (const void *)fuse_topk_kernel<false>,
+                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fuse_smem));
 
     if (p->sharded && c->comm.world > 1) {
         CU(cudaEventRecord(c->ev[EV_FUSE0], c->stream));
@@ -1968,7 +2023,8 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         did_comm = true;
     } else {
         CU(cudaEventRecord(c->ev[EV_FUSE0], c->stream));
-        fuse_topk_kernel<<<B, 256, fuse_smem, c->stream>>>(fp);
+        if (gj) fuse_topk_kernel<true><<<B, 256, fuse_smem, c->stream>>>(fp);
+        else fuse_topk_kernel<<<B, 256, fuse_smem, c->stream>>>(fp);
         launched(c);
         CU(cudaGetLastError());
         CU(cudaEventRecord(c->ev[EV_FUSE1], c->stream));
@@ -2020,19 +2076,34 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
             CU(cudaMemsetAsync(c->tau.p, 0, size_t(B) * 8, c->stream));
             CU(cudaMemsetAsync(tile_counter, 0, 8, c->stream));
             OCTRY(launch_tile(c, bp, n_tiles * B, any_multi, thr, omc_tile, c->stream, max_tokens, tile_counter, need_df));
-            fuse_topk_kernel<<<B, 256, fuse_smem, c->stream>>>(fp);
+            if (gj) fuse_topk_kernel<true><<<B, 256, fuse_smem, c->stream>>>(fp);
+            else fuse_topk_kernel<<<B, 256, fuse_smem, c->stream>>>(fp);
             launched(c);
             CU(cudaMemcpyAsync(c->h_out.p, dout, out_bytes, cudaMemcpyDeviceToHost, c->stream));
             CU(cudaStreamSynchronize(c->stream));
         }
     }
     if (fj) OCTRY(run_facets(c, *fj, B, has_ft, has_v, S, n_tiles, vlimit));
+    if (gj) {
+        CU(cudaEventRecord(c->ev[EV_GRP0], c->stream));
+        OCTRY(run_groups(c, *gj, B, p->mode, S, n_tiles, vlimit, fp.omc_doc, fp.omc_mult, n_omc));
+        CU(cudaEventRecord(c->ev[EV_GRP1], c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+    }
     c->timing.d2h_bytes = out_bytes;
-    memcpy(out_doc_ids, h + o_doc, size_t(B) * p->limit * 8);
-    memcpy(out_scores, h + o_sc, size_t(B) * p->limit * 4);
-    memcpy(out_n, h + o_n, size_t(B) * 4);
+    if (write_hits) {
+        memcpy(out_doc_ids, h + o_doc, size_t(B) * limit * 8);
+        memcpy(out_scores, h + o_sc, size_t(B) * limit * 4);
+        memcpy(out_n, h + o_n, size_t(B) * 4);
+    }
     memcpy(out_count, h + o_cnt, size_t(B) * 8);
-    return finish_timing(c, has_v && emb->n_rows > 0, has_ft, true, did_comm);
+    OCTRY(finish_timing(c, has_v && vlimit && emb->n_rows > 0, has_ft, true, did_comm));
+    if (gj) {   // the group stage is device work of this call too
+        float ms = 0.f;
+        CU(cudaEventElapsedTime(&ms, c->ev[EV_GRP0], c->ev[EV_GRP1]));
+        c->timing.device_ms += ms;
+    }
+    return OC_OK;
 }
 
 extern "C" int oc_search(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, uint64_t *out_doc_ids,
@@ -2251,6 +2322,191 @@ extern "C" int oc_search_facets(oc_ctx *c, oc_emb *emb, oc_str *str, oc_facets *
     std::vector<uint32_t> n(B);
     FacetJob fj{facets, reqs, n_reqs, out_counts};
     return search_impl(c, emb, str, &q, docs.data(), scores.data(), n.data(), cnt.data(), &fj);
+}
+
+// ------------------------------------------------------------------------------------ groups
+// GroupContext::execute (read/index/group.rs) + sort_groups (read/sort.rs:129-230): the group CSR is built once on
+// the host; per call its documents are mapped to string rows and group_topk_kernel (group.cuh) runs one CTA per
+// (group, query) over the score map the search left on the device.
+struct oc_group_by {
+    oc_ctx *ctx;
+    uint32_t n_groups = 0;
+    uint64_t n_docs = 0;           // entries of the CSR (a document counts once per group it belongs to)
+    uint64_t *off = nullptr;       // device [n_groups + 1]
+    uint64_t *docs = nullptr;      // device [n_docs]
+    uint32_t *rows = nullptr;      // device [n_docs + 1]: string row of each entry, filled per call; rows[n_docs] = ~0
+};
+static void group_by_free(oc_group_by *g) {
+    cudaFree(g->off); cudaFree(g->docs); cudaFree(g->rows);
+    delete g;
+}
+extern "C" void oc_group_by_destroy(oc_group_by *g) {
+    if (!g) return;
+    {
+        std::lock_guard<std::mutex> lk(g->ctx->mu);
+        cudaSetDevice(g->ctx->device);
+        cudaStreamSynchronize(g->ctx->stream);
+    }
+    group_by_free(g);
+}
+extern "C" int oc_group_by_create(oc_facets *f, const uint32_t *fields, uint32_t n_fields, oc_group_by **out, uint64_t *out_n_groups) {
+    if (!f || !fields || n_fields == 0 || !out) return fail(OC_ERR_INVALID, "bad arguments");
+    oc_ctx *c = f->ctx;
+    constexpr uint64_t MAX_GROUPS = 1ull << 20, MAX_GROUP_DOCS = 0xfffffffeull;
+    // per field: its (document, variant index) pairs, sorted and unique
+    std::vector<std::vector<std::pair<uint64_t, uint32_t>>> dv(n_fields);
+    std::vector<uint64_t> nv(n_fields);
+    uint64_t G = 1;
+    {
+        std::lock_guard<std::mutex> lk(c->mu);
+        CU(cudaSetDevice(c->device));
+        for (uint32_t i = 0; i < n_fields; i++) {
+            if (fields[i] >= f->fields.size()) return fail(OC_ERR_INVALID, "group field %u: unknown field id %u", i, fields[i]);
+            const FacetField &fl = f->fields[fields[i]];
+            std::vector<uint64_t> docs(fl.n_docs);
+            if (fl.n_docs) CU(cudaMemcpy(docs.data(), fl.docs, fl.n_docs * 8, cudaMemcpyDeviceToHost));
+            auto &pairs = dv[i];
+            pairs.reserve(fl.n_docs);
+            if (fl.number) {   // variant = rank of the distinct value (values are ascending; == merges -0.0 and 0.0)
+                uint32_t v = 0;
+                for (uint64_t k = 0; k < fl.n_docs; k++) {
+                    if (k && !(fl.values[k] == fl.values[k - 1])) v++;
+                    if (docs[k] < f->nbits) pairs.emplace_back(docs[k], v);
+                }
+                nv[i] = fl.n_docs ? uint64_t(v) + 1 : 0;
+            } else {
+                nv[i] = fl.offsets.size() - 1;
+                for (uint32_t v = 0; v + 1 < fl.offsets.size(); v++)
+                    for (uint64_t k = fl.offsets[v]; k < fl.offsets[v + 1]; k++)
+                        if (docs[k] < f->nbits) pairs.emplace_back(docs[k], v);
+            }
+            std::sort(pairs.begin(), pairs.end());
+            pairs.erase(std::unique(pairs.begin(), pairs.end()), pairs.end());
+            G *= nv[i];
+            if (G > MAX_GROUPS) return fail(OC_ERR_UNSUPPORTED, "more than %llu groups", (unsigned long long)MAX_GROUPS);
+        }
+    }
+    // memberships (group, doc), walked in ascending document order so every group's list comes out ascending
+    std::vector<std::pair<uint32_t, uint64_t>> memb;
+    std::vector<uint64_t> cnt(G + 1, 0);
+    if (G) {
+        std::vector<std::pair<size_t, size_t>> rng(n_fields);   // this document's pairs in each field
+        std::vector<size_t> at(n_fields);
+        const auto &f0 = dv[0];
+        for (size_t a = 0; a < f0.size();) {
+            const uint64_t d = f0[a].first;
+            size_t b = a;
+            while (b < f0.size() && f0[b].first == d) b++;
+            rng[0] = {a, b};
+            bool all = true;
+            for (uint32_t i = 1; i < n_fields && all; i++) {
+                auto lo = std::lower_bound(dv[i].begin(), dv[i].end(), std::make_pair(d, 0u));
+                auto hi = std::upper_bound(lo, dv[i].end(), std::make_pair(d, 0xffffffffu));
+                rng[i] = {size_t(lo - dv[i].begin()), size_t(hi - dv[i].begin())};
+                all = hi != lo;
+            }
+            if (all) {   // every combination of this document's variants (odometer, last field fastest)
+                for (uint32_t i = 0; i < n_fields; i++) at[i] = rng[i].first;
+                for (;;) {
+                    uint64_t gid = 0;
+                    for (uint32_t i = 0; i < n_fields; i++) gid = gid * nv[i] + dv[i][at[i]].second;
+                    memb.emplace_back((uint32_t)gid, d);
+                    if (++cnt[gid + 1] > MAX_GROUP_DOCS)
+                        return fail(OC_ERR_UNSUPPORTED, "group %llu holds more than %llu documents", (unsigned long long)gid,
+                                    (unsigned long long)MAX_GROUP_DOCS);
+                    int i = int(n_fields) - 1;
+                    while (i >= 0 && ++at[i] == rng[i].second) { at[i] = rng[i].first; i--; }
+                    if (i < 0) break;
+                }
+            }
+            a = b;
+        }
+    }
+    for (uint64_t g = 0; g < G; g++) cnt[g + 1] += cnt[g];
+    std::vector<uint64_t> csr(memb.size());
+    {
+        std::vector<uint64_t> pos(cnt.begin(), cnt.end() - 1);
+        for (const auto &e : memb) csr[pos[e.first]++] = e.second;   // stable: documents stay ascending
+    }
+    oc_group_by *g = new oc_group_by();
+    g->ctx = c; g->n_groups = (uint32_t)G; g->n_docs = csr.size();
+    auto fail_free = [&](int code) { group_by_free(g); return code; };
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (cudaSetDevice(c->device) != cudaSuccess) return fail_free(fail(OC_ERR_CUDA, "cudaSetDevice failed"));
+    const uint32_t none = 0xffffffffu;
+    cudaError_t e = cudaMalloc(&g->off, (G + 1) * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&g->docs, std::max<size_t>(csr.size(), 1) * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&g->rows, (csr.size() + 1) * 4);
+    if (e == cudaSuccess) e = cudaMemcpy(g->off, cnt.data(), (G + 1) * 8, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && !csr.empty()) e = cudaMemcpy(g->docs, csr.data(), csr.size() * 8, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(g->rows + csr.size(), &none, 4, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess)
+        return fail_free(fail(e == cudaErrorMemoryAllocation ? OC_ERR_OOM : OC_ERR_CUDA, "group CSR upload: %s", cudaGetErrorString(e)));
+    *out = g;
+    if (out_n_groups) *out_n_groups = G;
+    return OC_OK;
+}
+
+static int run_groups(oc_ctx *c, const GroupJob &gj, uint32_t B, int mode, const StrSnap *S, uint32_t n_tiles, uint32_t vlimit,
+                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc) {
+    oc_group_by *g = gj.g;
+    const uint32_t G = g->n_groups, m = gj.max_results;
+    if (G == 0) return OC_OK;
+    const bool has_ft = mode != OC_MODE_VECTOR && n_tiles > 0;
+    if (has_ft && g->n_docs) {   // the CSR's documents -> string rows (identity, or a binary search over the ascending row_doc)
+        constexpr uint64_t CH = 1ull << 30;
+        for (uint64_t a = 0; a < g->n_docs; a += CH) {
+            const uint32_t len = (uint32_t)std::min<uint64_t>(CH, g->n_docs - a);
+            // counts = rows[n_docs] (~0): every entry of the chunk is mapped
+            map_docs_to_rows_kernel<<<(len + 255) / 256, 256, 0, c->stream>>>(g->docs + a, g->rows + g->n_docs, len, 1, S->row_doc,
+                                                                              S->n_rows, g->rows + a);
+            launched(c);
+            CU(cudaGetLastError());
+        }
+    }
+    const size_t n_out = size_t(B) * G * m;
+    OCTRY(c->grp_doc.ensure(std::max<size_t>(n_out, 1) * 8));
+    OCTRY(c->grp_score.ensure(std::max<size_t>(n_out, 1) * 4));
+    OCTRY(c->grp_n.ensure(size_t(B) * G * 4));
+    GroupParams gp{};
+    gp.n_groups = G; gp.max_results = m;
+    gp.kp2 = std::max<uint32_t>(32, next_pow2(m));
+    gp.vp2 = next_pow2(std::max<uint32_t>(vlimit, 1));
+    gp.g_off = g->off; gp.g_doc = g->docs; gp.g_row = has_ft ? g->rows : nullptr;
+    gp.has_ft = has_ft; gp.hybrid = mode == OC_MODE_HYBRID;
+    gp.mbits = c->mbits.as<uint32_t>(); gp.row_words = uint64_t(n_tiles) * (BM25_TILE / 32);
+    gp.row_ft = c->row_ft.as<float>();
+    gp.gmin = c->grp_gmin.as<float>(); gp.den = c->grp_den.as<float>();
+    gp.v_doc = c->grp_vdoc.as<uint64_t>(); gp.v_score = c->grp_vscore.as<float>(); gp.v_n = c->grp_vn.as<uint32_t>();
+    gp.v_stride = std::max<uint32_t>(vlimit, 1);
+    gp.omc_doc = omc_doc; gp.omc_mult = omc_mult; gp.n_omc = n_omc;
+    gp.out_doc = c->grp_doc.as<uint64_t>(); gp.out_score = c->grp_score.as<float>(); gp.out_n = c->grp_n.as<uint32_t>();
+    const size_t smem = (size_t(GROUP_BUF) + gp.kp2 + gp.vp2) * 8 + size_t(gp.vp2) * 4;
+    if (smem_cfg_needed(c->device, (const void *)group_topk_kernel, smem))
+        CU(cudaFuncSetAttribute(group_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    group_topk_kernel<<<dim3(G, B), GROUP_THREADS, smem, c->stream>>>(gp);
+    launched(c);
+    CU(cudaGetLastError());
+    if (n_out) {
+        CU(cudaMemcpyAsync(gj.out_doc, gp.out_doc, n_out * 8, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaMemcpyAsync(gj.out_score, gp.out_score, n_out * 4, cudaMemcpyDeviceToHost, c->stream));
+    }
+    CU(cudaMemcpyAsync(gj.out_n, gp.out_n, size_t(B) * G * 4, cudaMemcpyDeviceToHost, c->stream));
+    return OC_OK;
+}
+
+extern "C" int oc_search_groups(oc_ctx *c, oc_emb *emb, oc_str *str, oc_group_by *groups, const oc_search_params *p,
+                                uint32_t max_results, uint64_t *out_doc_ids, float *out_scores, uint32_t *out_n, uint64_t *out_count,
+                                uint64_t *out_group_doc_ids, float *out_group_scores, uint32_t *out_group_n) {
+    if (!c || !p || !groups || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
+    if (groups->n_groups && (!out_group_n || (max_results && (!out_group_doc_ids || !out_group_scores))))
+        return fail(OC_ERR_INVALID, "NULL group output");
+    if (groups->ctx != c) return fail(OC_ERR_INVALID, "group_by belongs to another ctx");
+    if (p->sharded) return fail(OC_ERR_UNSUPPORTED, "groups over a sharded search: hybrid normalisation and the vector set are global");
+    if (max_results > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "max_results %u > %u", max_results, OC_MAX_TOPK);
+    if (p->n_queries > 65535) return fail(OC_ERR_UNSUPPORTED, "groups: n_queries %u > 65535", p->n_queries);
+    GroupJob gj{groups, max_results, out_group_doc_ids, out_group_scores, out_group_n};
+    return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, &gj);
 }
 
 // ------------------------------------------------------------------------------------ micro-batching front

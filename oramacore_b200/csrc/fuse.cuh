@@ -44,20 +44,47 @@ struct FuseParams {
     uint32_t *out_n;
     unsigned long long *out_count;
     float *out_min;               // actual global min (rank-proxy validation), may be NULL
+    // group mode (oc_search_groups), all NULL otherwise: what the group kernel needs to score any document of the
+    // query's score map the way this kernel does
+    float *out_gmin, *out_den;    // [q] hybrid normalisation
+    uint64_t *out_vdoc;           // [q][v_stride] the unique vector hits (after the += merge) ...
+    float *out_vscore;            // ... with their final score (fused in hybrid mode, after OMC; NaN = dropped)
+    uint32_t *out_vn;             // [q]
 };
 
-__device__ __forceinline__ float omc_lookup(const FuseParams &p, uint64_t doc, bool *found) {
-    uint32_t lo = 0, hi = p.n_omc;
+__device__ __forceinline__ float omc_find(const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, uint64_t doc, bool *found) {
+    uint32_t lo = 0, hi = n_omc;
     while (lo < hi) {
         const uint32_t m = (lo + hi) >> 1;
-        if (p.omc_doc[m] < doc) lo = m + 1; else hi = m;
+        if (omc_doc[m] < doc) lo = m + 1; else hi = m;
     }
-    *found = lo < p.n_omc && p.omc_doc[lo] == doc;
-    return *found ? p.omc_mult[lo] : 1.0f;
+    *found = lo < n_omc && omc_doc[lo] == doc;
+    return *found ? omc_mult[lo] : 1.0f;
+}
+__device__ __forceinline__ float omc_lookup(const FuseParams &p, uint64_t doc, bool *found) {
+    return omc_find(p.omc_doc, p.omc_mult, p.n_omc, doc, found);
+}
+
+// The final score of a document of the fulltext map: (ft - min) / (max - min) in hybrid mode
+// (token_score.rs:393-422), then x its OMC multiplier if it has one (search.rs:39-48).  NaN = not a key.
+// Shared by K4 and the group kernel so both derive the same bits; doc_of() is only called with multipliers.
+template <typename DocOf>
+__device__ __forceinline__ float fused_ft_score(float ft, bool hybrid, float gmin, float den, const uint64_t *omc_doc,
+                                                const float *omc_mult, uint32_t n_omc, DocOf doc_of) {
+    float f = ft;
+    if (hybrid) f = __fdiv_rn(__fsub_rn(f, gmin), den);       // (v - min) / (max - min)
+    if (n_omc) {
+        bool found;
+        const float m = omc_find(omc_doc, omc_mult, n_omc, doc_of(), &found);
+        if (found) f = __fmul_rn(f, m);
+    }
+    return f;
 }
 
 constexpr uint32_t FUSE_MAX_V = OC_MAX_TOPK;
 
+// GROUPS: group mode, the out_gmin / out_den / out_v* exports are written
+template <bool GROUPS = false>
 __global__ void __launch_bounds__(256) fuse_topk_kernel(const FuseParams p) {
     extern __shared__ __align__(16) uint8_t smem[];
     uint64_t *buf = reinterpret_cast<uint64_t *>(smem);               // [capb]
@@ -120,6 +147,39 @@ __global__ void __launch_bounds__(256) fuse_topk_kernel(const FuseParams p) {
     // ---- candidate stream: tile candidates (minus vector-hit rows), then the vector hits
     const uint64_t n_ft_slots = has_ft ? uint64_t(p.n_tiles) * p.n_keep : 0;
     const uint64_t total = n_ft_slots + vc;
+    // final score of the unique vector hit j (NaN = dropped)
+    auto vhit_score = [&](uint32_t j) -> float {
+        float f;
+        if (hybrid) {
+            const size_t vs = size_t(q) * p.v_stride + j;
+            const float vn = __fdiv_rn(__fsub_rn(vsum[j], gmin), den);
+            const float fn = p.v_present[vs] ? __fdiv_rn(__fsub_rn(p.v_ft[vs], gmin), den) : 0.0f;
+            f = __fadd_rn(fn, vn);                                    // entry(k).or_default() += v
+        } else {
+            f = vsum[j];
+        }
+        if (p.n_omc) {
+            bool found;
+            const float m = omc_lookup(p, vdoc[j], &found);
+            if (found) f = __fmul_rn(f, m);
+        }
+        return f;
+    };
+    if (GROUPS) {   // group mode: export the vector part of the score map and the normalisation
+        uint32_t base = 0;
+        for (uint32_t j0 = 0; j0 < vc; j0 += blockDim.x) {   // block-uniform trip count (the scan has barriers)
+            const uint32_t j = j0 + tid;
+            const bool head = j < vc && vfirst[j];
+            uint32_t n_heads;
+            const uint32_t pos = base + block_exclusive_scan(head ? 1u : 0u, &n_heads);
+            if (head) {
+                p.out_vdoc[size_t(q) * p.v_stride + pos] = vdoc[j];
+                p.out_vscore[size_t(q) * p.v_stride + pos] = vhit_score(j);
+            }
+            base += n_heads;
+        }
+        if (tid == 0) { p.out_vn[q] = base; p.out_gmin[q] = gmin; p.out_den[q] = den; }
+    }
     auto load = [&](uint64_t i) -> uint64_t {
         if (i < n_ft_slots) {
             const uint32_t t = uint32_t(i / p.n_keep), k = uint32_t(i % p.n_keep);
@@ -129,34 +189,17 @@ __global__ void __launch_bounds__(256) fuse_topk_kernel(const FuseParams p) {
             if (hybrid)
                 for (uint32_t j = 0; j < vc; j++)
                     if (p.v_row[size_t(q) * p.v_stride + j] == row) return KEY_NONE;  // scored below
-            float f = p.cand_ft[s * p.n_keep + k];
-            if (hybrid) f = __fdiv_rn(__fsub_rn(f, gmin), den);       // (v - min) / (max - min)
-            if (p.n_omc) {
-                bool found;
-                const uint64_t doc = p.str_row_doc_ids ? p.str_row_doc_ids[row] : uint64_t(row);
-                const float m = omc_lookup(p, doc, &found);
-                if (found) f = __fmul_rn(f, m);
-            }
+            const float f = fused_ft_score(p.cand_ft[s * p.n_keep + k], hybrid, gmin, den, p.omc_doc, p.omc_mult, p.n_omc,
+                                           [&] { return p.str_row_doc_ids ? p.str_row_doc_ids[row] : uint64_t(row); });
             return f == f ? make_key(f, row) : KEY_NONE;              // NaN dropped (sort.rs:264-267)
         }
         const uint32_t j = uint32_t(i - n_ft_slots);
         if (!vfirst[j]) return KEY_NONE;
-        float f;
-        uint32_t idx;
+        const float f = vhit_score(j);
+        uint32_t idx = j;
         if (hybrid) {
             const size_t vs = size_t(q) * p.v_stride + j;
-            const float vn = __fdiv_rn(__fsub_rn(vsum[j], gmin), den);
-            const float fn = p.v_present[vs] ? __fdiv_rn(__fsub_rn(p.v_ft[vs], gmin), den) : 0.0f;
-            f = __fadd_rn(fn, vn);                                    // entry(k).or_default() += v
             idx = p.v_row[vs] != 0xffffffffu ? p.v_row[vs] : (0xfffffffeu - j);
-        } else {
-            f = vsum[j];
-            idx = j;
-        }
-        if (p.n_omc) {
-            bool found;
-            const float m = omc_lookup(p, vdoc[j], &found);
-            if (found) f = __fmul_rn(f, m);
         }
         return f == f ? make_key(f, idx) : KEY_NONE;
     };

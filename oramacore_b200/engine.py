@@ -360,7 +360,7 @@ class FacetStore:
         v, d = np.ascontiguousarray(v[o]), np.ascontiguousarray(d[o])
         fid = C.c_uint32()
         check(lib().oc_facets_add_number_field(self._h, v.shape[0], _p(v), _p(d), C.byref(fid)))
-        self.fields[name] = {"id": fid.value, "kind": "number"}
+        self.fields[name] = {"id": fid.value, "kind": "number", "values": np.unique(v)}   # distinct values, ascending
         return fid.value
 
     def close(self):
@@ -406,6 +406,69 @@ def search_facets(tsc: "TokenScoreContext", store: FacetStore, params: "TokenSco
             v["count"] = len(v["values"])
         res.append(r)
     return res
+
+
+class GroupBy:
+    """GroupByConfig.properties (types.rs:1367-1371) over the filter fields of a FacetStore (oc_group_by_*): one group per
+    combination of the fields' variants, last property varying fastest (generate_group_combinations, read/index/group.rs).
+    `values[g]` is group g's key: True / False for a bool field, the key for a string_filter field, the float value for a
+    number field (its distinct values, ascending)."""
+
+    def __init__(self, store: FacetStore, properties: Sequence[str]):
+        self.ctx, self.properties = store.ctx, list(properties)
+        fs = [store.fields[p] for p in self.properties]
+        ids = np.asarray([f["id"] for f in fs], np.uint32)
+        self._h, n = C.c_void_p(), C.c_uint64()
+        check(lib().oc_group_by_create(store._h, _p(ids), ids.shape[0], C.byref(self._h), C.byref(n)))
+        self.n_groups = int(n.value)
+        per_field = []
+        for f in fs:
+            if f["kind"] == "bool":
+                per_field.append([k == "true" for k in f["keys"]])
+            elif f["kind"] == "number":
+                per_field.append([float(x) for x in f["values"]])
+            else:
+                per_field.append(list(f["keys"]))
+        self.values: List[list] = [[]]
+        for vals in per_field:
+            self.values = [v + [x] for v in self.values for x in vals]
+        assert len(self.values) == self.n_groups
+
+    def close(self):
+        if self._h:
+            lib().oc_group_by_destroy(self._h)
+            self._h = None
+
+
+def search_groups_arrays(tsc: "TokenScoreContext", group_by: GroupBy, params: "TokenScoreParams", max_results: int = 1, texts=None,
+                         q_vecs: Optional[np.ndarray] = None):
+    """oc_search_groups as arrays: (docs [B,limit], scores, n [B], count [B], group docs [B,G,max_results], group scores,
+    group n [B,G])."""
+    sp, keep, B = tsc._build_params(params, texts, q_vecs)
+    L, G = params.limit_hint, group_by.n_groups
+    docs, scores = np.zeros((B, L), np.uint64), np.zeros((B, L), np.float32)
+    n, cnt = np.zeros(B, np.uint32), np.zeros(B, np.uint64)
+    gd, gs = np.zeros((B, G, max_results), np.uint64), np.zeros((B, G, max_results), np.float32)
+    gn = np.zeros((B, G), np.uint32)
+    check(lib().oc_search_groups(tsc.ctx._h, tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None, group_by._h,
+                                 C.byref(sp), int(max_results), _p(docs), _p(scores), _p(n), _p(cnt), _p(gd), _p(gs), _p(gn)))
+    return docs, scores, n, cnt, gd, gs, gn
+
+
+def search_groups(tsc: "TokenScoreContext", group_by: GroupBy, params: "TokenScoreParams", max_results: int = 1, texts=None,
+                  q_vecs: Optional[np.ndarray] = None):
+    """search() with groupBy (search.rs:415-429 + sort_groups, read/sort.rs:129-230): per query (hits, groups), groups a
+    list in group order of {"values": [...], "result": [(doc_id, score), ...]} (GroupedResult, types.rs:1375), the
+    top max_results documents of the group that are in the query's score map.  limit_hint 0 is allowed: no hits, and no
+    vector search (the reference's limit_hint = 0)."""
+    docs, scores, n, cnt, gd, gs, gn = search_groups_arrays(tsc, group_by, params, max_results, texts, q_vecs)
+    out = []
+    for q in range(cnt.shape[0]):
+        hits = SearchHits(docs[q, :n[q]].copy(), scores[q, :n[q]].copy(), int(cnt[q]))
+        groups = [{"values": list(group_by.values[g]),
+                   "result": [(int(gd[q, g, i]), float(gs[q, g, i])) for i in range(int(gn[q, g]))]} for g in range(group_by.n_groups)]
+        out.append((hits, groups))
+    return out
 
 
 def merge_index_results(per_index, limit: int, offset: int = 0) -> List[SearchHits]:

@@ -14,6 +14,7 @@ use std::ffi::{c_char, c_int, c_void, CStr};
 #[repr(C)] pub struct OcBatcher { _p: [u8; 0] }
 #[repr(C)] pub struct OcFilter { _p: [u8; 0] }
 #[repr(C)] pub struct OcFacets { _p: [u8; 0] }
+#[repr(C)] pub struct OcGroupBy { _p: [u8; 0] }
 #[repr(C)] pub struct OcDict { _p: [u8; 0] }
 #[repr(C)] pub struct OcResolved { _p: [u8; 0] }
 
@@ -126,6 +127,14 @@ extern "C" {
     pub fn oc_facets_add_number_field(f: *mut OcFacets, n: u64, values_sorted: *const f64, doc_ids: *const u64, out_field: *mut u32) -> c_int;
     pub fn oc_search_facets(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, f: *mut OcFacets, p: *const OcSearchParams,
                             reqs: *const OcFacetReq, n_reqs: u32, out_counts: *mut u64) -> c_int;
+    // groups over the score map (group.rs + sort_groups, sort.rs:129-230)
+    pub fn oc_group_by_create(f: *mut OcFacets, fields: *const u32, n_fields: u32, out: *mut *mut OcGroupBy,
+                              out_n_groups: *mut u64) -> c_int;
+    pub fn oc_group_by_destroy(g: *mut OcGroupBy);
+    pub fn oc_search_groups(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, g: *mut OcGroupBy, p: *const OcSearchParams,
+                            max_results: u32, out_doc_ids: *mut u64, out_scores: *mut f32, out_n: *mut u32,
+                            out_count: *mut u64, out_group_doc_ids: *mut u64, out_group_scores: *mut f32,
+                            out_group_n: *mut u32) -> c_int;
     /// search_on_indexes' union of the per-index maps (search.rs:304-338, 482-498), host side
     pub fn oc_merge_results(n_indexes: u32, n_queries: u32, limit: u32, offset: u32, in_stride: u32,
                             doc_ids: *const *const u64, scores: *const *const f32, n: *const *const u32,
