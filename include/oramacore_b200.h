@@ -294,6 +294,62 @@ int oc_merge_results(uint32_t n_indexes, uint32_t n_queries, uint32_t limit, uin
                      const uint64_t *const *counts, uint64_t *out_doc_ids /* B x limit */, float *out_scores,
                      uint32_t *out_n, uint64_t *out_count);
 
+/* ---- pin rules (promoted documents) ----------------------------------------------------------------
+ * Search::execute collects the consequences of the pin rules that match the query (read/search.rs:127-133,
+ * extract_pin_rules :257-281); sort_token_scores / sort_groups then splice their promote items into the ranking
+ * (apply_pin_rules_internal, read/sort.rs:285-391).  Rule matching stays on the host; per query the caller passes the
+ * promote items of the matched consequences, concatenated in the order extract_pin_rules leaves them.  Query q's items
+ * are [q_pin_offsets[q], q_pin_offsets[q+1]) of doc_ids / positions (and of the per-item outputs).  A query is ACTIVE
+ * when it has at least one item and apply != 0.  Deliberate deviation: a matched consequence with an empty promote list
+ * doubles top_count in the reference; here it is the same as no consequence.
+ * Active query, flat hits: take the top 2 x (limit + offset) of the score map (score desc, ties by ascending document id,
+ * NaN dropped); remove every document the query promotes; insert the items, stably sorted by position, one after the
+ * other at min(position, current length) with the document's score-map value (NaN stays NaN), or 0.0 when it is not a
+ * key of the map (no match, filtered out, deleted, under the threshold, in no store); then skip(offset).take(limit).
+ * So of equal positions the later item ends up in front, and a document promoted twice is inserted twice.  count is
+ * unchanged (promoted non-matching documents are not counted) and the vector stage keeps depth limit.  A query that is
+ * not active gets exactly oc_search's hits.  A promoted id with no stored document is dropped later by the caller's
+ * document fetch, as in search.rs:181-200. */
+typedef struct {
+    const uint32_t *q_pin_offsets;   /* B+1, monotone                                                      */
+    const uint64_t *doc_ids;         /* PromoteItem.doc_id of each item                                    */
+    const uint32_t *positions;       /* PromoteItem.position                                               */
+    int apply;                       /* 0: hits exactly as oc_search (no doubling, no splice): only the per-item
+                                        outputs are computed — the per-index call of a multi-index search   */
+} oc_pins;
+/* As oc_search, plus per item its score-map value (out_pin_scores, 0.0 when not a key) and whether the document is a
+ * key of the score map (out_pin_present, 1 / 0); both may be NULL.  pins may be NULL (no item).
+ * OC_ERR_UNSUPPORTED: p->sharded (scores and hybrid normalisation are global), an active query with
+ * 2 x (limit + offset) > OC_MAX_TOPK, a query with more than OC_MAX_TOPK items.  OC_ERR_INVALID: q_pin_offsets not
+ * monotone, a handle of another ctx.  A failed call writes nothing. */
+int oc_search_pinned(oc_ctx *ctx, oc_emb *emb, oc_str *str, const oc_search_params *p, const oc_pins *pins,
+                     uint64_t *out_doc_ids, float *out_scores, uint32_t *out_n, uint64_t *out_count,
+                     float *out_pin_scores, uint8_t *out_pin_present);
+/* oc_search_groups with pins (sort_groups + apply_pin_rules_to_group, read/sort.rs:129-230, 377-391).  The flat hits
+ * follow oc_search_pinned.  For an active query every group takes its top 2 x max_results, keeps the items whose
+ * document is a member of the group (the group's documents, whether or not they are keys of the score map), splices
+ * them as above and is NOT truncated afterwards: up to 2 x max_results + the query's member items.  A query that is not
+ * active keeps exactly oc_search_groups' top max_results.  out_group_doc_ids / out_group_scores:
+ * B x n_groups x group_stride; out_group_n: B x n_groups.  group_stride >= 2 x max_results + the most items of one query
+ * when some query is active, else >= max_results (OC_ERR_INVALID otherwise).  Refusals as oc_search_pinned and
+ * oc_search_groups, plus OC_ERR_UNSUPPORTED for an active query with 2 x max_results > OC_MAX_TOPK.  Multi-index
+ * grouped searches with pins are not supported: a promoted document's membership spans indexes. */
+int oc_search_groups_pinned(oc_ctx *ctx, oc_emb *emb, oc_str *str, oc_group_by *groups, const oc_search_params *p,
+                            uint32_t max_results, const oc_pins *pins, uint32_t group_stride, uint64_t *out_doc_ids,
+                            float *out_scores, uint32_t *out_n, uint64_t *out_count, uint64_t *out_group_doc_ids,
+                            float *out_group_scores, uint32_t *out_group_n);
+/* The multi-index union with pins (host, no device).  Run every index with oc_search_pinned, limit' = 2 x (limit +
+ * offset), offset' = 0, vector_limit = limit, apply = 0, and pass its hit lists (in_stride = limit'), counts and per-item
+ * outputs.  The per-index maps are disjoint, so a promoted document takes its score from the index where it is present,
+ * else 0.0.  An active query (pins->apply) gets the union's top 2 x (limit + offset), spliced, then skip/take; any
+ * other query exactly oc_merge_results' answer.  OC_ERR_INVALID: in_stride < 2 x (limit + offset) while a query is
+ * active, q_pin_offsets not monotone. */
+int oc_merge_pinned(uint32_t n_indexes, uint32_t n_queries, uint32_t limit, uint32_t offset, uint32_t in_stride,
+                    const uint64_t *const *doc_ids, const float *const *scores, const uint32_t *const *n,
+                    const uint64_t *const *counts, const oc_pins *pins, const float *const *pin_scores,
+                    const uint8_t *const *pin_present, uint64_t *out_doc_ids /* B x limit */, float *out_scores,
+                    uint32_t *out_n, uint64_t *out_count);
+
 /* ---- term dictionary and query-term resolution (host only; no device needed) ------------------------
  * The step the reference performs before the posting walk: TextParser::tokenize_and_stem(term) —
  * originals, plus stems unless `exact`, [""] when nothing is left (token_score.rs:196-209) — and the

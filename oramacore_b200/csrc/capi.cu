@@ -24,6 +24,7 @@
 #include "emb_scan.cuh"
 #include "fuse.cuh"
 #include "group.cuh"
+#include "pins.cuh"
 #include "tmap.cuh"
 #include "oramacore_b200.h"
 
@@ -155,6 +156,7 @@ struct oc_ctx {
     DevBuf out_blob, shard_send, shard_recv, work_ctr, flat_desc, mbits, dbits, facet_req, facet_out;
     bool gemm_pending = false; const float *gemm_inv_norm = nullptr;
     DevBuf row_ft, grp_vdoc, grp_vscore, grp_vn, grp_gmin, grp_den, grp_doc, grp_score, grp_n;   // oc_search_groups
+    DevBuf pin_row, pin_ft, pin_ftp, pin_score, pin_present, pin_top_doc, pin_top_score, pin_top_n, pin_gdoc, pin_gscore, pin_gn;   // pins
     DevBuf q_bf16, q_rho, pre_post, dense_buf, g_thr, g_eps, g_ovf, g_ovfcnt, g_resc, g_cand, g_cnt, g_flag, g_max, r_qpad, r_qinv, r_map, r_doc, r_score, r_row, r_cnt, r_raw;
 
     HostBuf h_in, h_out, h_in0;   // h_in0 / in_blob0: query vectors + filter, uploaded before the descriptors
@@ -210,7 +212,9 @@ extern "C" void oc_shutdown(oc_ctx *c) {
                       &c->row_ok, &c->tau, &c->cand_key, &c->cand_ft, &c->cand_cnt, &c->tile_cnt, &c->tile_max,
                       &c->tile_min, &c->min_hint, &c->out_blob, &c->shard_send, &c->shard_recv, &c->work_ctr, &c->flat_desc, &c->mbits, &c->dbits, &c->facet_req, &c->facet_out, &c->q_bf16, &c->q_rho, &c->pre_post, &c->dense_buf, &c->g_thr, &c->g_eps, &c->g_ovf, &c->g_ovfcnt, &c->g_resc, &c->g_cand, &c->g_cnt, &c->g_max,
                       &c->g_flag, &c->r_qpad, &c->r_qinv, &c->r_map, &c->r_doc, &c->r_score, &c->r_row, &c->r_cnt, &c->r_raw,
-                      &c->row_ft, &c->grp_vdoc, &c->grp_vscore, &c->grp_vn, &c->grp_gmin, &c->grp_den, &c->grp_doc, &c->grp_score, &c->grp_n};
+                      &c->row_ft, &c->grp_vdoc, &c->grp_vscore, &c->grp_vn, &c->grp_gmin, &c->grp_den, &c->grp_doc, &c->grp_score, &c->grp_n,
+                      &c->pin_row, &c->pin_ft, &c->pin_ftp, &c->pin_score, &c->pin_present, &c->pin_top_doc, &c->pin_top_score,
+                      &c->pin_top_n, &c->pin_gdoc, &c->pin_gscore, &c->pin_gn};
     for (DevBuf *b : bufs) b->release();
     c->h_in.release(); c->h_out.release();
     for (int i = 0; i < EV_N; i++) if (c->ev[i]) cudaEventDestroy(c->ev[i]);
@@ -1285,40 +1289,106 @@ extern "C" int oc_filter_read(const oc_filter *f, uint64_t *out_bits) {
 }
 
 // ------------------------------------------------------------------------------------ multi-index union (host)
+// k-way merge of query q's per-index lists, each sorted by (score desc, doc asc) (NaN never reaches a list): the first
+// `take` entries of the union, as (doc, score)
+static void merge_union_top(uint32_t n_indexes, uint32_t q, uint32_t in_stride, const uint64_t *const *doc_ids,
+                            const float *const *scores, const uint32_t *const *n, uint32_t take,
+                            std::vector<std::pair<uint64_t, float>> &out) {
+    std::vector<uint32_t> head(n_indexes, 0u);
+    out.clear();
+    while (out.size() < take) {
+        int best = -1;
+        for (uint32_t i = 0; i < n_indexes; i++) {
+            if (head[i] >= n[i][q]) continue;
+            if (best < 0) { best = (int)i; continue; }
+            const float sa = scores[i][size_t(q) * in_stride + head[i]], sb = scores[best][size_t(q) * in_stride + head[best]];
+            const uint64_t da = doc_ids[i][size_t(q) * in_stride + head[i]], db = doc_ids[best][size_t(q) * in_stride + head[best]];
+            if (sa > sb || (sa == sb && da < db)) best = (int)i;
+        }
+        if (best < 0) break;
+        out.emplace_back(doc_ids[best][size_t(q) * in_stride + head[best]], scores[best][size_t(q) * in_stride + head[best]]);
+        head[best]++;
+    }
+}
+// skip(offset).take(limit) of `top` into row q of the outputs (zero-padded)
+static void write_page(const std::vector<std::pair<uint64_t, float>> &top, uint32_t q, uint32_t limit, uint32_t offset,
+                       uint64_t *out_doc_ids, float *out_scores, uint32_t *out_n) {
+    uint32_t written = 0;
+    for (size_t i = offset; i < top.size() && written < limit; i++, written++) {
+        out_doc_ids[size_t(q) * limit + written] = top[i].first;
+        out_scores[size_t(q) * limit + written] = top[i].second;
+    }
+    for (uint32_t k = written; k < limit; k++) { out_doc_ids[size_t(q) * limit + k] = 0; out_scores[size_t(q) * limit + k] = 0.f; }
+    out_n[q] = written;
+}
+
 extern "C" int oc_merge_results(uint32_t n_indexes, uint32_t B, uint32_t limit, uint32_t offset, uint32_t in_stride,
                                 const uint64_t *const *doc_ids, const float *const *scores, const uint32_t *const *n,
                                 const uint64_t *const *counts, uint64_t *out_doc_ids, float *out_scores, uint32_t *out_n,
                                 uint64_t *out_count) {
     if (!doc_ids || !scores || !n || !counts || !out_doc_ids || !out_scores || !out_n || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
     if (limit == 0) return fail(OC_ERR_INVALID, "limit must be >= 1");
-    std::vector<uint32_t> head(n_indexes);
+    std::vector<std::pair<uint64_t, float>> top;
     for (uint32_t q = 0; q < B; q++) {
-        std::fill(head.begin(), head.end(), 0u);
         uint64_t cnt = 0;
         for (uint32_t i = 0; i < n_indexes; i++) {
             if (n[i][q] > in_stride) return fail(OC_ERR_INVALID, "index %u query %u: n > in_stride", i, q);
             cnt += counts[i][q];
         }
-        uint32_t taken = 0, written = 0;
-        while (written < limit) {   // k-way merge of lists already sorted by (score desc, doc asc); NaN never reaches a list
-            int best = -1;
-            for (uint32_t i = 0; i < n_indexes; i++) {
-                if (head[i] >= n[i][q]) continue;
-                if (best < 0) { best = (int)i; continue; }
-                const float sa = scores[i][size_t(q) * in_stride + head[i]], sb = scores[best][size_t(q) * in_stride + head[best]];
-                const uint64_t da = doc_ids[i][size_t(q) * in_stride + head[i]], db = doc_ids[best][size_t(q) * in_stride + head[best]];
-                if (sa > sb || (sa == sb && da < db)) best = (int)i;
+        merge_union_top(n_indexes, q, in_stride, doc_ids, scores, n, uint32_t(std::min<uint64_t>(uint64_t(limit) + offset, 0xffffffffu)), top);
+        write_page(top, q, limit, offset, out_doc_ids, out_scores, out_n);
+        out_count[q] = cnt;
+    }
+    return OC_OK;
+}
+
+// apply_pin_rules_internal (read/sort.rs:285-391) on the host: the union's top list of an active query, spliced
+extern "C" int oc_merge_pinned(uint32_t n_indexes, uint32_t B, uint32_t limit, uint32_t offset, uint32_t in_stride,
+                               const uint64_t *const *doc_ids, const float *const *scores, const uint32_t *const *n,
+                               const uint64_t *const *counts, const oc_pins *pins, const float *const *pin_scores,
+                               const uint8_t *const *pin_present, uint64_t *out_doc_ids, float *out_scores, uint32_t *out_n,
+                               uint64_t *out_count) {
+    if (!doc_ids || !scores || !n || !counts || !pins || !pins->q_pin_offsets || !out_doc_ids || !out_scores || !out_n || !out_count)
+        return fail(OC_ERR_INVALID, "NULL argument");
+    if (limit == 0) return fail(OC_ERR_INVALID, "limit must be >= 1");
+    const uint32_t *off = pins->q_pin_offsets;
+    const uint64_t top_pinned = (uint64_t(limit) + offset) * 2;
+    bool any = false;
+    for (uint32_t q = 0; q < B; q++) {   // everything is checked before anything is written
+        if (off[q + 1] < off[q]) return fail(OC_ERR_INVALID, "pins: q_pin_offsets is not monotone at query %u", q);
+        any = any || (pins->apply && off[q + 1] > off[q]);
+        for (uint32_t i = 0; i < n_indexes; i++)
+            if (n[i][q] > in_stride) return fail(OC_ERR_INVALID, "index %u query %u: n > in_stride", i, q);
+    }
+    if (any && (!pins->doc_ids || !pins->positions || !pin_scores || !pin_present)) return fail(OC_ERR_INVALID, "NULL pin argument");
+    if (any && in_stride < top_pinned)
+        return fail(OC_ERR_INVALID, "pins: in_stride %u < 2 x (limit+offset) %llu", in_stride, (unsigned long long)top_pinned);
+    std::vector<std::pair<uint64_t, float>> top;
+    std::vector<std::pair<uint32_t, uint32_t>> items;   // (position, item), sorted stably by position
+    std::vector<uint64_t> promoted;
+    for (uint32_t q = 0; q < B; q++) {
+        uint64_t cnt = 0;
+        for (uint32_t i = 0; i < n_indexes; i++) cnt += counts[i][q];
+        const bool active = pins->apply && off[q + 1] > off[q];
+        merge_union_top(n_indexes, q, in_stride, doc_ids, scores, n, uint32_t(active ? top_pinned : uint64_t(limit) + offset), top);
+        if (active) {
+            items.clear(); promoted.clear();
+            for (uint32_t j = off[q]; j < off[q + 1]; j++) { items.emplace_back(pins->positions[j], j); promoted.push_back(pins->doc_ids[j]); }
+            std::sort(promoted.begin(), promoted.end());
+            top.erase(std::remove_if(top.begin(), top.end(),
+                                     [&](const std::pair<uint64_t, float> &e) { return std::binary_search(promoted.begin(), promoted.end(), e.first); }),
+                      top.end());
+            std::stable_sort(items.begin(), items.end(), [](const std::pair<uint32_t, uint32_t> &a, const std::pair<uint32_t, uint32_t> &b) {
+                return a.first < b.first;
+            });
+            for (const auto &it : items) {
+                float s = 0.f;   // the disjoint maps: the score from the one index that holds the document, else 0.0
+                for (uint32_t i = 0; i < n_indexes; i++)
+                    if (pin_present[i][it.second]) { s = pin_scores[i][it.second]; break; }
+                top.insert(top.begin() + std::min<size_t>(it.first, top.size()), std::make_pair(pins->doc_ids[it.second], s));
             }
-            if (best < 0) break;
-            if (taken >= offset) {
-                out_doc_ids[size_t(q) * limit + written] = doc_ids[best][size_t(q) * in_stride + head[best]];
-                out_scores[size_t(q) * limit + written] = scores[best][size_t(q) * in_stride + head[best]];
-                written++;
-            }
-            taken++; head[best]++;
         }
-        for (uint32_t k = written; k < limit; k++) { out_doc_ids[size_t(q) * limit + k] = 0; out_scores[size_t(q) * limit + k] = 0.f; }
-        out_n[q] = written;
+        write_page(top, q, limit, offset, out_doc_ids, out_scores, out_n);
         out_count[q] = cnt;
     }
     return OC_OK;
@@ -1500,14 +1570,53 @@ struct GroupJob {   // oc_search_groups: the top max_results documents of every 
     uint64_t *out_doc;      // [B][G][max_results]
     float *out_score;
     uint32_t *out_n;        // [B][G]
+    uint32_t stride = 0;    // oc_search_groups_pinned: row stride of the group arrays ([B][G][stride])
 };
+struct PinJob {   // oc_search_pinned / oc_search_groups_pinned: the promote items, padded to `stride` slots per query
+    uint32_t stride = 0;                // most items of one query (0: no item in the batch)
+    bool splice = false;                // pins apply and some query has items: top lists at twice the depth + the splice
+    std::vector<uint64_t> doc;          // [B][stride]
+    std::vector<uint32_t> pos, cnt;     // [B][stride], [B]
+    const uint64_t *d_doc = nullptr;    // their device copies (set by search_impl)
+    const uint32_t *d_pos = nullptr, *d_cnt = nullptr;
+};
+// Checks and pads the items of pins (NULL: none).  Nothing is written on failure.
+static int pin_job_init(const oc_pins *pins, uint32_t B, PinJob &pj) {
+    if (!pins) return OC_OK;
+    const uint32_t *off = pins->q_pin_offsets;
+    if (!off) return fail(OC_ERR_INVALID, "pins: q_pin_offsets is NULL");
+    uint32_t most = 0;
+    for (uint32_t q = 0; q < B; q++) {
+        if (off[q + 1] < off[q]) return fail(OC_ERR_INVALID, "pins: q_pin_offsets is not monotone at query %u", q);
+        most = std::max(most, off[q + 1] - off[q]);
+    }
+    if (most > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "pins: a query has %u items > %u", most, OC_MAX_TOPK);
+    if (uint64_t(B) * most * 32 > 0x7fffffffull) return fail(OC_ERR_UNSUPPORTED, "pins: %u queries x %u items: pass smaller batches", B, most);
+    if (most && (!pins->doc_ids || !pins->positions)) return fail(OC_ERR_INVALID, "pins: doc_ids / positions are NULL");
+    pj.stride = most;
+    pj.splice = pins->apply && most > 0;
+    pj.doc.assign(size_t(B) * most, 0);
+    pj.pos.assign(size_t(B) * most, 0);
+    pj.cnt.assign(B, 0);
+    for (uint32_t q = 0; q < B; q++) {
+        pj.cnt[q] = off[q + 1] - off[q];
+        for (uint32_t j = 0; j < pj.cnt[q]; j++) {
+            pj.doc[size_t(q) * most + j] = pins->doc_ids[off[q] + j];
+            pj.pos[size_t(q) * most + j] = pins->positions[off[q] + j];
+        }
+    }
+    return OC_OK;
+}
 static int run_groups(oc_ctx *c, const GroupJob &gj, uint32_t B, int mode, const StrSnap *S, uint32_t n_tiles, uint32_t vlimit,
-                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc);
+                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, const PinJob *pj);
 
 // gj != NULL: oc_search_groups.  Then limit == 0 is allowed: the hits are not written (out_doc_ids / out_scores / out_n
 // may be NULL), the vector stage gets depth 0 and the fulltext stage runs with one candidate slot per tile.
+// pj != NULL: the pinned calls; the items' score-map values go to out_pin_scores / out_pin_present (may be NULL).
 static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, uint64_t *out_doc_ids,
-                       float *out_scores, uint32_t *out_n, uint64_t *out_count, const FacetJob *fj, const GroupJob *gj = nullptr) {
+                       float *out_scores, uint32_t *out_n, uint64_t *out_count, const FacetJob *fj, const GroupJob *gj = nullptr,
+                       PinJob *pj = nullptr, const oc_pins *pins = nullptr, float *out_pin_scores = nullptr,
+                       uint8_t *out_pin_present = nullptr) {
     if (!c || !p || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
     const bool write_hits = !gj || p->limit > 0;
     if (write_hits && (!out_doc_ids || !out_scores || !out_n)) return fail(OC_ERR_INVALID, "NULL argument");
@@ -1522,7 +1631,9 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     if (str && str->ctx != c) return fail(OC_ERR_INVALID, "str belongs to another ctx");
     if (p->limit == 0 && !gj) return fail(OC_ERR_INVALID, "limit must be >= 1");
     const uint32_t limit = write_hits ? p->limit : 1;
-    const uint64_t n_keep64 = uint64_t(limit) + p->offset;
+    // sort_token_scores with pins selects the top 2 * (limit + offset) (sort.rs:25-34); the vector depth stays limit
+    const bool pin_flat = pj && pj->splice && write_hits;
+    const uint64_t n_keep64 = (uint64_t(limit) + p->offset) * (pin_flat ? 2 : 1);
     if (n_keep64 > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "limit+offset %llu > %u", (unsigned long long)n_keep64, OC_MAX_TOPK);
     const uint32_t n_keep = (uint32_t)n_keep64;
     // limit_hint = limit, NOT limit+offset (search.rs:330-336); vector_limit lets a multi-index caller keep that depth
@@ -1803,6 +1914,10 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
             for (uint32_t q = 0; q < B; q++) if (nd_q[q] == nd) q_perm[at[cls_of(q)]++] = q;
     }
     const size_t o_perm = q_perm.empty() ? 0 : pk.add(q_perm.data(), q_perm.size() * 4);
+    const bool pin_items = pj && pj->stride;
+    const size_t o_pdoc = pin_items ? pk.add(pj->doc.data(), pj->doc.size() * 8) : 0;
+    const size_t o_ppos = pin_items ? pk.add(pj->pos.data(), pj->pos.size() * 4) : 0;
+    const size_t o_pcnt = pin_items ? pk.add(pj->cnt.data(), pj->cnt.size() * 4) : 0;
     // hybrid: the descriptors, the shared-contribution precompute, the filter bitmap and the (term, tile) plan do
     // not depend on the vector results: they run on the side stream while the main stream sweeps the matrix
     // (OC_SIDE_STREAM=0 disables it: the step gets ~2.5 % longer, the sweep itself ~4 % shorter — A/B switch)
@@ -1817,6 +1932,11 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     c->timing.h2d_bytes = h2d_early + pk.total;
     uint8_t *din = c->in_blob.as<uint8_t>();
     if (filter_h && !has_v) filter_dev = reinterpret_cast<const uint64_t *>(din + o_flt);
+    if (pin_items) {
+        pj->d_doc = reinterpret_cast<const uint64_t *>(din + o_pdoc);
+        pj->d_pos = reinterpret_cast<const uint32_t *>(din + o_ppos);
+        pj->d_cnt = reinterpret_cast<const uint32_t *>(din + o_pcnt);
+    }
 
     // ------------------------------------------------------------ fulltext stage + fusion (re-runnable)
     // arg-max selection (n_keep <= 32) needs no power-of-two buffer; the bitonic fallback does
@@ -1953,6 +2073,56 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     };
     if (has_ft) OCTRY(bm25_stage());
 
+    const bool exports = gj || pj;   // K4 exports the normalisation and the vector part of the score map
+    // pins, after K4: the score-map value of every promoted document, then (pin_flat) the splice into K4's top list
+    auto pin_tail = [&]() -> int {
+        if (!pin_items) return OC_OK;
+        const uint32_t ps = pj->stride;
+        const uint64_t nslot = uint64_t(B) * ps;
+        const unsigned warp_grid = (unsigned)((nslot * 32 + 255) / 256);
+        OCTRY(c->pin_score.ensure(nslot * 4));
+        OCTRY(c->pin_present.ensure(nslot));
+        if (has_ft) {   // the promoted documents' string rows and their fulltext scores (the hybrid lookups' kernels)
+            OCTRY(c->pin_row.ensure(nslot * 4));
+            OCTRY(c->pin_ft.ensure(nslot * 4));
+            OCTRY(c->pin_ftp.ensure(nslot));
+            map_docs_to_rows_kernel<<<(unsigned)((nslot + 255) / 256), 256, 0, c->stream>>>(
+                pj->d_doc, pj->d_cnt, ps, B, S->row_doc, S->n_rows, c->pin_row.as<uint32_t>());
+            launched(c);
+            PointParams pp{};
+            pp.terms = bp.terms; pp.tokens = bp.tokens; pp.queries = bp.queries;
+            pp.n_queries = B; pp.v_stride = ps; pp.v_row = c->pin_row.as<uint32_t>(); pp.row_ok_bits = row_ok;
+            pp.k = p->bm25_k; pp.threshold = thr ? 1 : 0;
+            pp.v_ft = c->pin_ft.as<float>(); pp.v_present = c->pin_ftp.as<uint8_t>();
+            bm25_point_kernel<<<warp_grid, 256, 0, c->stream>>>(pp);
+            launched(c);
+        }
+        PinScoreParams sp{};
+        sp.n_queries = B; sp.stride = ps; sp.doc = pj->d_doc; sp.cnt = pj->d_cnt;
+        sp.has_ft = has_ft; sp.hybrid = has_ft && has_v;
+        sp.ft = c->pin_ft.as<float>(); sp.ft_present = c->pin_ftp.as<uint8_t>();
+        sp.gmin = fp.out_gmin; sp.den = fp.out_den;
+        sp.v_doc = fp.out_vdoc; sp.v_score = fp.out_vscore; sp.v_n = fp.out_vn; sp.v_stride = std::max<uint32_t>(vlimit, 1);
+        sp.omc_doc = fp.omc_doc; sp.omc_mult = fp.omc_mult; sp.n_omc = n_omc;
+        sp.out_score = c->pin_score.as<float>(); sp.out_present = c->pin_present.as<uint8_t>();
+        pin_score_kernel<<<warp_grid, 256, 0, c->stream>>>(sp);
+        launched(c);
+        if (pin_flat) {
+            PinSpliceParams xp{};
+            xp.stride = ps; xp.kp2 = std::max<uint32_t>(32, next_pow2(ps));
+            xp.doc = pj->d_doc; xp.pos = pj->d_pos; xp.score = c->pin_score.as<float>(); xp.cnt = pj->d_cnt;
+            xp.n_top = n_keep; xp.limit = limit; xp.offset = p->offset;
+            xp.top_doc = c->pin_top_doc.as<uint64_t>(); xp.top_score = c->pin_top_score.as<float>(); xp.top_n = c->pin_top_n.as<uint32_t>();
+            xp.out_doc = reinterpret_cast<uint64_t *>(dout + o_doc); xp.out_score = reinterpret_cast<float *>(dout + o_sc);
+            xp.out_n = reinterpret_cast<uint32_t *>(dout + o_n);
+            const size_t smem = pin_splice_smem(xp.kp2, n_keep, limit + p->offset);
+            pin_splice_kernel<<<B, PIN_THREADS, smem, c->stream>>>(xp);
+            launched(c);
+        }
+        CU(cudaGetLastError());
+        return OC_OK;
+    };
+
     auto device_tail = [&]() -> int {
     if (has_ft && has_v) {
         // hybrid: vector hits -> string rows -> their fulltext scores (point lookups)
@@ -2000,7 +2170,14 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     fp.out_doc = reinterpret_cast<uint64_t *>(dout + o_doc); fp.out_score = reinterpret_cast<float *>(dout + o_sc);
     fp.out_n = reinterpret_cast<uint32_t *>(dout + o_n); fp.out_count = reinterpret_cast<unsigned long long *>(dout + o_cnt);
     fp.out_min = reinterpret_cast<float *>(dout + o_min);
-    if (gj) {   // groups: K4 also exports the normalisation and the vector part of the score map
+    if (pin_flat) {   // K4 keeps its whole top n_keep for the splice, which writes the hits
+        fp.limit = n_keep; fp.offset = 0;
+        OCTRY(c->pin_top_doc.ensure(size_t(B) * n_keep * 8));
+        OCTRY(c->pin_top_score.ensure(size_t(B) * n_keep * 4));
+        OCTRY(c->pin_top_n.ensure(size_t(B) * 4));
+        fp.out_doc = c->pin_top_doc.as<uint64_t>(); fp.out_score = c->pin_top_score.as<float>(); fp.out_n = c->pin_top_n.as<uint32_t>();
+    }
+    if (exports) {   // groups / pins: K4 also exports the normalisation and the vector part of the score map
         const uint32_t vs = std::max<uint32_t>(vlimit, 1);
         OCTRY(c->grp_vdoc.ensure(size_t(B) * vs * 8));
         OCTRY(c->grp_vscore.ensure(size_t(B) * vs * 4));
@@ -2011,8 +2188,8 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         fp.out_gmin = c->grp_gmin.as<float>(); fp.out_den = c->grp_den.as<float>();
     }
     fuse_smem = size_t(fp.capb) * 8 + size_t(std::max<uint32_t>(32, next_pow2(n_keep))) * 8 + size_t(vlimit) * 8 + 64;
-    if (smem_cfg_needed(c->device, gj ? (const void *)fuse_topk_kernel<true> : (const void *)fuse_topk_kernel<false>, fuse_smem))
-        CU(cudaFuncSetAttribute(gj ? (const void *)fuse_topk_kernel<true> : (const void *)fuse_topk_kernel<false>,
+    if (smem_cfg_needed(c->device, exports ? (const void *)fuse_topk_kernel<true> : (const void *)fuse_topk_kernel<false>, fuse_smem))
+        CU(cudaFuncSetAttribute(exports ? (const void *)fuse_topk_kernel<true> : (const void *)fuse_topk_kernel<false>,
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fuse_smem));
 
     if (p->sharded && c->comm.world > 1) {
@@ -2023,10 +2200,11 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         did_comm = true;
     } else {
         CU(cudaEventRecord(c->ev[EV_FUSE0], c->stream));
-        if (gj) fuse_topk_kernel<true><<<B, 256, fuse_smem, c->stream>>>(fp);
+        if (exports) fuse_topk_kernel<true><<<B, 256, fuse_smem, c->stream>>>(fp);
         else fuse_topk_kernel<<<B, 256, fuse_smem, c->stream>>>(fp);
         launched(c);
         CU(cudaGetLastError());
+        OCTRY(pin_tail());
         CU(cudaEventRecord(c->ev[EV_FUSE1], c->stream));
     }
     return OC_OK;
@@ -2076,9 +2254,10 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
             CU(cudaMemsetAsync(c->tau.p, 0, size_t(B) * 8, c->stream));
             CU(cudaMemsetAsync(tile_counter, 0, 8, c->stream));
             OCTRY(launch_tile(c, bp, n_tiles * B, any_multi, thr, omc_tile, c->stream, max_tokens, tile_counter, need_df));
-            if (gj) fuse_topk_kernel<true><<<B, 256, fuse_smem, c->stream>>>(fp);
+            if (exports) fuse_topk_kernel<true><<<B, 256, fuse_smem, c->stream>>>(fp);
             else fuse_topk_kernel<<<B, 256, fuse_smem, c->stream>>>(fp);
             launched(c);
+            OCTRY(pin_tail());
             CU(cudaMemcpyAsync(c->h_out.p, dout, out_bytes, cudaMemcpyDeviceToHost, c->stream));
             CU(cudaStreamSynchronize(c->stream));
         }
@@ -2086,8 +2265,17 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     if (fj) OCTRY(run_facets(c, *fj, B, has_ft, has_v, S, n_tiles, vlimit));
     if (gj) {
         CU(cudaEventRecord(c->ev[EV_GRP0], c->stream));
-        OCTRY(run_groups(c, *gj, B, p->mode, S, n_tiles, vlimit, fp.omc_doc, fp.omc_mult, n_omc));
+        OCTRY(run_groups(c, *gj, B, p->mode, S, n_tiles, vlimit, fp.omc_doc, fp.omc_mult, n_omc, pj));
         CU(cudaEventRecord(c->ev[EV_GRP1], c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+    }
+    std::vector<float> pin_sc;
+    std::vector<uint8_t> pin_pr;
+    if (pin_items && (out_pin_scores || out_pin_present)) {
+        pin_sc.resize(pj->doc.size());
+        pin_pr.resize(pj->doc.size());
+        CU(cudaMemcpyAsync(pin_sc.data(), c->pin_score.p, pin_sc.size() * 4, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaMemcpyAsync(pin_pr.data(), c->pin_present.p, pin_pr.size(), cudaMemcpyDeviceToHost, c->stream));
         CU(cudaStreamSynchronize(c->stream));
     }
     c->timing.d2h_bytes = out_bytes;
@@ -2097,6 +2285,13 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         memcpy(out_n, h + o_n, size_t(B) * 4);
     }
     memcpy(out_count, h + o_cnt, size_t(B) * 8);
+    if (!pin_sc.empty())
+        for (uint32_t q = 0; q < B; q++)
+            for (uint32_t j = 0; j < pj->cnt[q]; j++) {
+                const size_t i = size_t(pins->q_pin_offsets[q]) + j, s = size_t(q) * pj->stride + j;
+                if (out_pin_scores) out_pin_scores[i] = pin_sc[s];
+                if (out_pin_present) out_pin_present[i] = pin_pr[s];
+            }
     OCTRY(finish_timing(c, has_v && vlimit && emb->n_rows > 0, has_ft, true, did_comm));
     if (gj) {   // the group stage is device work of this call too
         float ms = 0.f;
@@ -2448,9 +2643,11 @@ extern "C" int oc_group_by_create(oc_facets *f, const uint32_t *fields, uint32_t
 }
 
 static int run_groups(oc_ctx *c, const GroupJob &gj, uint32_t B, int mode, const StrSnap *S, uint32_t n_tiles, uint32_t vlimit,
-                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc) {
+                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, const PinJob *pj) {
     oc_group_by *g = gj.g;
-    const uint32_t G = g->n_groups, m = gj.max_results;
+    // sort_groups with pins takes every group's top 2 * max_results (sort.rs:137-142)
+    const bool pin_grp = pj && pj->splice;
+    const uint32_t G = g->n_groups, m = gj.max_results * (pin_grp ? 2 : 1);
     if (G == 0) return OC_OK;
     const bool has_ft = mode != OC_MODE_VECTOR && n_tiles > 0;
     if (has_ft && g->n_docs) {   // the CSR's documents -> string rows (identity, or a binary search over the ascending row_doc)
@@ -2487,6 +2684,30 @@ static int run_groups(oc_ctx *c, const GroupJob &gj, uint32_t B, int mode, const
     group_topk_kernel<<<dim3(G, B), GROUP_THREADS, smem, c->stream>>>(gp);
     launched(c);
     CU(cudaGetLastError());
+    if (pj) {   // oc_search_groups_pinned: every group's list at the caller's stride, spliced for the queries with items
+        const size_t n_res = size_t(B) * G * gj.stride;
+        OCTRY(c->pin_gdoc.ensure(std::max<size_t>(n_res, 1) * 8));
+        OCTRY(c->pin_gscore.ensure(std::max<size_t>(n_res, 1) * 4));
+        OCTRY(c->pin_gn.ensure(size_t(B) * G * 4));
+        GroupPinParams xp{};
+        xp.n_groups = G; xp.max_results = gj.max_results; xp.stride = gj.stride; xp.n_top = m;
+        xp.kp2 = std::max<uint32_t>(32, next_pow2(pj->stride));
+        xp.g_off = g->off; xp.g_doc = g->docs;
+        xp.doc = pj->d_doc; xp.pos = pj->d_pos; xp.score = c->pin_score.as<float>();
+        xp.cnt = pin_grp ? pj->d_cnt : nullptr; xp.item_stride = pj->stride;
+        xp.top_doc = gp.out_doc; xp.top_score = gp.out_score; xp.top_n = gp.out_n;
+        xp.out_doc = c->pin_gdoc.as<uint64_t>(); xp.out_score = c->pin_gscore.as<float>(); xp.out_n = c->pin_gn.as<uint32_t>();
+        const size_t psmem = pin_splice_smem(xp.kp2, m, std::min<uint32_t>(gj.stride, m + pj->stride));
+        group_pin_splice_kernel<<<dim3(G, B), PIN_THREADS, psmem, c->stream>>>(xp);
+        launched(c);
+        CU(cudaGetLastError());
+        if (n_res) {
+            CU(cudaMemcpyAsync(gj.out_doc, xp.out_doc, n_res * 8, cudaMemcpyDeviceToHost, c->stream));
+            CU(cudaMemcpyAsync(gj.out_score, xp.out_score, n_res * 4, cudaMemcpyDeviceToHost, c->stream));
+        }
+        CU(cudaMemcpyAsync(gj.out_n, xp.out_n, size_t(B) * G * 4, cudaMemcpyDeviceToHost, c->stream));
+        return OC_OK;
+    }
     if (n_out) {
         CU(cudaMemcpyAsync(gj.out_doc, gp.out_doc, n_out * 8, cudaMemcpyDeviceToHost, c->stream));
         CU(cudaMemcpyAsync(gj.out_score, gp.out_score, n_out * 4, cudaMemcpyDeviceToHost, c->stream));
@@ -2507,6 +2728,48 @@ extern "C" int oc_search_groups(oc_ctx *c, oc_emb *emb, oc_str *str, oc_group_by
     if (p->n_queries > 65535) return fail(OC_ERR_UNSUPPORTED, "groups: n_queries %u > 65535", p->n_queries);
     GroupJob gj{groups, max_results, out_group_doc_ids, out_group_scores, out_group_n};
     return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, &gj);
+}
+
+// ------------------------------------------------------------------------------------ pin rules (pins.cuh)
+static int pins_check_flat(const oc_search_params *p, const PinJob &pj) {
+    if (p->sharded) return fail(OC_ERR_UNSUPPORTED, "pins over a sharded search: scores and the hybrid normalisation are global");
+    if (pj.splice && (uint64_t(p->limit) + p->offset) * 2 > OC_MAX_TOPK)
+        return fail(OC_ERR_UNSUPPORTED, "pins: 2 x (limit+offset) %llu > %u", (unsigned long long)(uint64_t(p->limit) + p->offset) * 2,
+                    OC_MAX_TOPK);
+    return OC_OK;
+}
+
+extern "C" int oc_search_pinned(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, const oc_pins *pins,
+                                uint64_t *out_doc_ids, float *out_scores, uint32_t *out_n, uint64_t *out_count,
+                                float *out_pin_scores, uint8_t *out_pin_present) {
+    if (!c || !p) return fail(OC_ERR_INVALID, "NULL argument");
+    PinJob pj;
+    OCTRY(pin_job_init(pins, p->n_queries, pj));
+    OCTRY(pins_check_flat(p, pj));
+    return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, nullptr, &pj, pins, out_pin_scores,
+                       out_pin_present);
+}
+
+extern "C" int oc_search_groups_pinned(oc_ctx *c, oc_emb *emb, oc_str *str, oc_group_by *groups, const oc_search_params *p,
+                                       uint32_t max_results, const oc_pins *pins, uint32_t group_stride, uint64_t *out_doc_ids,
+                                       float *out_scores, uint32_t *out_n, uint64_t *out_count, uint64_t *out_group_doc_ids,
+                                       float *out_group_scores, uint32_t *out_group_n) {
+    if (!c || !p || !groups || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
+    if (groups->n_groups && (!out_group_n || (group_stride && (!out_group_doc_ids || !out_group_scores))))
+        return fail(OC_ERR_INVALID, "NULL group output");
+    if (groups->ctx != c) return fail(OC_ERR_INVALID, "group_by belongs to another ctx");
+    if (max_results > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "max_results %u > %u", max_results, OC_MAX_TOPK);
+    if (p->n_queries > 65535) return fail(OC_ERR_UNSUPPORTED, "groups: n_queries %u > 65535", p->n_queries);
+    PinJob pj;
+    OCTRY(pin_job_init(pins, p->n_queries, pj));
+    OCTRY(pins_check_flat(p, pj));
+    if (pj.splice && 2 * max_results > OC_MAX_TOPK)
+        return fail(OC_ERR_UNSUPPORTED, "pins: 2 x max_results %u > %u", 2 * max_results, OC_MAX_TOPK);
+    const uint64_t need = pj.splice ? 2ull * max_results + pj.stride : max_results;
+    if (group_stride < need) return fail(OC_ERR_INVALID, "group_stride %u < %llu", group_stride, (unsigned long long)need);
+    GroupJob gj{groups, max_results, out_group_doc_ids, out_group_scores, out_group_n};
+    gj.stride = group_stride;
+    return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, &gj, &pj, pins);
 }
 
 // ------------------------------------------------------------------------------------ micro-batching front

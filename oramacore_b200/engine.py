@@ -20,7 +20,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import OcError, SearchParams, Timing, check, lib
-from .types import (BM25_B, BM25_K, MODE_FULLTEXT, MODE_HYBRID, MODE_VECTOR, SearchHits, StringIndexData,
+from .types import (BM25_B, BM25_K, MODE_FULLTEXT, MODE_HYBRID, MODE_VECTOR, PromoteItem, SearchHits, StringIndexData,
                     TextQuery)
 
 # Model::dimensions / rescale_score (python/embeddings.rs:52-92)
@@ -441,27 +441,39 @@ class GroupBy:
 
 
 def search_groups_arrays(tsc: "TokenScoreContext", group_by: GroupBy, params: "TokenScoreParams", max_results: int = 1, texts=None,
-                         q_vecs: Optional[np.ndarray] = None):
-    """oc_search_groups as arrays: (docs [B,limit], scores, n [B], count [B], group docs [B,G,max_results], group scores,
-    group n [B,G])."""
+                         q_vecs: Optional[np.ndarray] = None, promote=None):
+    """oc_search_groups as arrays: (docs [B,limit], scores, n [B], count [B], group docs [B,G,stride], group scores,
+    group n [B,G]); stride = max_results.  With `promote` (see search_pinned_arrays) the call is oc_search_groups_pinned:
+    a query with items gets pinned hits and every group's top 2 * max_results with its member items spliced in
+    (apply_pin_rules_to_group), stride = 2 * max_results + the most items of one query."""
     sp, keep, B = tsc._build_params(params, texts, q_vecs)
     L, G = params.limit_hint, group_by.n_groups
+    pins = None if promote is None else _pins(promote, B)
+    stride = max_results
+    if pins is not None and pins[1]:
+        stride = 2 * max_results + pins[1]
     docs, scores = np.zeros((B, L), np.uint64), np.zeros((B, L), np.float32)
     n, cnt = np.zeros(B, np.uint32), np.zeros(B, np.uint64)
-    gd, gs = np.zeros((B, G, max_results), np.uint64), np.zeros((B, G, max_results), np.float32)
+    gd, gs = np.zeros((B, G, stride), np.uint64), np.zeros((B, G, stride), np.float32)
     gn = np.zeros((B, G), np.uint32)
-    check(lib().oc_search_groups(tsc.ctx._h, tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None, group_by._h,
-                                 C.byref(sp), int(max_results), _p(docs), _p(scores), _p(n), _p(cnt), _p(gd), _p(gs), _p(gn)))
+    emb, strs = tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None
+    if pins is None:
+        check(lib().oc_search_groups(tsc.ctx._h, emb, strs, group_by._h, C.byref(sp), int(max_results), _p(docs), _p(scores), _p(n),
+                                     _p(cnt), _p(gd), _p(gs), _p(gn)))
+    else:
+        check(lib().oc_search_groups_pinned(tsc.ctx._h, emb, strs, group_by._h, C.byref(sp), int(max_results), C.byref(pins[0]),
+                                            int(stride), _p(docs), _p(scores), _p(n), _p(cnt), _p(gd), _p(gs), _p(gn)))
     return docs, scores, n, cnt, gd, gs, gn
 
 
 def search_groups(tsc: "TokenScoreContext", group_by: GroupBy, params: "TokenScoreParams", max_results: int = 1, texts=None,
-                  q_vecs: Optional[np.ndarray] = None):
+                  q_vecs: Optional[np.ndarray] = None, promote=None):
     """search() with groupBy (search.rs:415-429 + sort_groups, read/sort.rs:129-230): per query (hits, groups), groups a
     list in group order of {"values": [...], "result": [(doc_id, score), ...]} (GroupedResult, types.rs:1375), the
     top max_results documents of the group that are in the query's score map.  limit_hint 0 is allowed: no hits, and no
-    vector search (the reference's limit_hint = 0)."""
-    docs, scores, n, cnt, gd, gs, gn = search_groups_arrays(tsc, group_by, params, max_results, texts, q_vecs)
+    vector search (the reference's limit_hint = 0).  `promote`: the pin rules' promote items per query (see
+    search_pinned_arrays)."""
+    docs, scores, n, cnt, gd, gs, gn = search_groups_arrays(tsc, group_by, params, max_results, texts, q_vecs, promote)
     out = []
     for q in range(cnt.shape[0]):
         hits = SearchHits(docs[q, :n[q]].copy(), scores[q, :n[q]].copy(), int(cnt[q]))
@@ -469,6 +481,49 @@ def search_groups(tsc: "TokenScoreContext", group_by: GroupBy, params: "TokenSco
                    "result": [(int(gd[q, g, i]), float(gs[q, g, i])) for i in range(int(gn[q, g]))]} for g in range(group_by.n_groups)]
         out.append((hits, groups))
     return out
+
+
+def _pins(promote, B: int, apply: bool = True):
+    """oc_pins for B queries from `promote` (per query a sequence of PromoteItem or (doc_id, position) pairs, in the
+    order extract_pin_rules leaves the matched consequences' items).  Returns (struct, most items of one query, keep)."""
+    if len(promote) != B:
+        raise ValueError(f"promote has {len(promote)} entries for {B} queries")
+    items = [[(int(it.doc_id), int(it.position)) if isinstance(it, PromoteItem) else (int(it[0]), int(it[1])) for it in q]
+             for q in promote]
+    off = np.zeros(B + 1, np.uint32)
+    off[1:] = np.cumsum([len(q) for q in items])
+    flat = [it for q in items for it in q]
+    doc = np.ascontiguousarray([d for d, _ in flat] or [0], np.uint64)
+    pos = np.ascontiguousarray([p for _, p in flat] or [0], np.uint32)
+    pins = _lib.Pins(_p(off), _p(doc), _p(pos), 1 if apply else 0)
+    pins._keep = (off, doc, pos)
+    return pins, max((len(q) for q in items), default=0)
+
+
+def search_pinned_arrays(tsc: "TokenScoreContext", params: "TokenScoreParams", promote, texts=None,
+                         q_vecs: Optional[np.ndarray] = None, apply: bool = True):
+    """oc_search_pinned: search() with pin rules (sort_token_scores + apply_pin_rules, read/sort.rs:17-46, 285-391).
+    `promote`: per query the promote items (PromoteItem, or (doc_id, position)) of the consequences that matched it.
+    Returns (docs [B,limit], scores, n [B], count [B], pin scores [items], pin present [items]): per item, in the
+    concatenated order, the document's score-map value (0.0 when it is not a key) and whether it is a key.
+    apply=False: oc_search's hits, only the per-item values (the per-index call of merge_index_results_pinned)."""
+    sp, keep, B = tsc._build_params(params, texts, q_vecs)
+    pins, _ = _pins(promote, B, apply)
+    n_items = int(pins._keep[0][-1])
+    L = params.limit_hint
+    docs, scores = np.zeros((B, L), np.uint64), np.zeros((B, L), np.float32)
+    n, cnt = np.zeros(B, np.uint32), np.zeros(B, np.uint64)
+    ps, pp = np.zeros(max(n_items, 1), np.float32), np.zeros(max(n_items, 1), np.uint8)
+    check(lib().oc_search_pinned(tsc.ctx._h, tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None, C.byref(sp),
+                                 C.byref(pins), _p(docs), _p(scores), _p(n), _p(cnt), _p(ps), _p(pp)))
+    return docs, scores, n, cnt, ps[:n_items], pp[:n_items]
+
+
+def search_pinned(tsc: "TokenScoreContext", params: "TokenScoreParams", promote, texts=None,
+                  q_vecs: Optional[np.ndarray] = None) -> List[SearchHits]:
+    """search_pinned_arrays as one SearchHits per query."""
+    docs, scores, n, cnt, _, _ = search_pinned_arrays(tsc, params, promote, texts, q_vecs)
+    return [SearchHits(docs[i, :n[i]].copy(), scores[i, :n[i]].copy(), int(cnt[i])) for i in range(docs.shape[0])]
 
 
 def merge_index_results(per_index, limit: int, offset: int = 0) -> List[SearchHits]:
@@ -482,6 +537,22 @@ def merge_index_results(per_index, limit: int, offset: int = 0) -> List[SearchHi
     od, os_ = np.zeros((B, limit), np.uint64), np.zeros((B, limit), np.float32)
     on, oc = np.zeros(B, np.uint32), np.zeros(B, np.uint64)
     check(lib().oc_merge_results(k, B, limit, offset, stride, arr(0), arr(1), arr(2), arr(3), _p(od), _p(os_), _p(on), _p(oc)))
+    return [SearchHits(od[i, :on[i]].copy(), os_[i, :on[i]].copy(), int(oc[i])) for i in range(B)]
+
+
+def merge_index_results_pinned(per_index, promote, limit: int, offset: int = 0, apply: bool = True) -> List[SearchHits]:
+    """The multi-index union with pin rules (oc_merge_pinned, host): per_index = one (doc_ids [B, 2*(limit+offset)],
+    scores, n, count, pin scores, pin present) tuple per index, each from search_pinned_arrays with
+    limit' = 2 * (limit + offset), offset' = 0, vector_limit = limit, apply=False; `promote` as there."""
+    k = len(per_index)
+    B, stride = per_index[0][0].shape
+    keep = [[np.ascontiguousarray(a) for a in r] for r in per_index]
+    arr = lambda j: (C.c_void_p * k)(*[r[j].ctypes.data for r in keep])  # noqa: E731
+    pins, _ = _pins(promote, B, apply)
+    od, os_ = np.zeros((B, limit), np.uint64), np.zeros((B, limit), np.float32)
+    on, oc = np.zeros(B, np.uint32), np.zeros(B, np.uint64)
+    check(lib().oc_merge_pinned(k, B, limit, offset, stride, arr(0), arr(1), arr(2), arr(3), C.byref(pins), arr(4), arr(5),
+                                _p(od), _p(os_), _p(on), _p(oc)))
     return [SearchHits(od[i, :on[i]].copy(), os_[i, :on[i]].copy(), int(oc[i])) for i in range(B)]
 
 

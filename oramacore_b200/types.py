@@ -89,3 +89,10 @@ class SearchHits:
     doc_ids: np.ndarray   # uint64 [n]
     scores: np.ndarray    # float32 [n]
     count: int            # search.rs:482 — all matching documents
+
+
+@dataclass(frozen=True)
+class PromoteItem:
+    """oramacore_lib::pin_rules::PromoteItem: a pin rule's consequence places `doc_id` at `position`."""
+    doc_id: int
+    position: int

@@ -59,6 +59,15 @@ pub struct OcSearchParams {
 #[repr(C)]
 pub struct OcFacetReq { pub field: u32, pub variant: u32, pub from: f64, pub to: f64 }
 
+/// the promote items of the pin rules that matched each query (extract_pin_rules, search.rs:257-281)
+#[repr(C)]
+pub struct OcPins {
+    pub q_pin_offsets: *const u32,  // B+1
+    pub doc_ids: *const u64,        // PromoteItem.doc_id
+    pub positions: *const u32,      // PromoteItem.position
+    pub apply: c_int,               // 0: hits as oc_search, only the per-item score-map values
+}
+
 #[repr(C)]
 pub struct OcResolveParams {
     pub texts: *const *const c_char,
@@ -140,6 +149,19 @@ extern "C" {
                             doc_ids: *const *const u64, scores: *const *const f32, n: *const *const u32,
                             counts: *const *const u64, out_doc_ids: *mut u64, out_scores: *mut f32,
                             out_n: *mut u32, out_count: *mut u64) -> c_int;
+    // pin rules (apply_pin_rules / apply_pin_rules_to_group, sort.rs:285-391)
+    pub fn oc_search_pinned(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, p: *const OcSearchParams, pins: *const OcPins,
+                            out_doc_ids: *mut u64, out_scores: *mut f32, out_n: *mut u32, out_count: *mut u64,
+                            out_pin_scores: *mut f32, out_pin_present: *mut u8) -> c_int;
+    pub fn oc_search_groups_pinned(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, g: *mut OcGroupBy, p: *const OcSearchParams,
+                                   max_results: u32, pins: *const OcPins, group_stride: u32, out_doc_ids: *mut u64,
+                                   out_scores: *mut f32, out_n: *mut u32, out_count: *mut u64, out_group_doc_ids: *mut u64,
+                                   out_group_scores: *mut f32, out_group_n: *mut u32) -> c_int;
+    pub fn oc_merge_pinned(n_indexes: u32, n_queries: u32, limit: u32, offset: u32, in_stride: u32,
+                           doc_ids: *const *const u64, scores: *const *const f32, n: *const *const u32,
+                           counts: *const *const u64, pins: *const OcPins, pin_scores: *const *const f32,
+                           pin_present: *const *const u8, out_doc_ids: *mut u64, out_scores: *mut f32,
+                           out_n: *mut u32, out_count: *mut u64) -> c_int;
     // term dictionary + batch query resolution (tokenize_and_stem + FST expansion), host only
     pub fn oc_dict_create(n_fields: u32, out: *mut *mut OcDict) -> c_int;
     pub fn oc_dict_destroy(d: *mut OcDict);
