@@ -350,6 +350,76 @@ int oc_merge_pinned(uint32_t n_indexes, uint32_t n_queries, uint32_t limit, uint
                     const uint8_t *const *pin_present, uint64_t *out_doc_ids /* B x limit */, float *out_scores,
                     uint32_t *out_n, uint64_t *out_count);
 
+/* ---- sortBy: hits and groups in the order of a number, date or bool field --------------------------
+ * sort_token_scores / sort_groups with sort_by (read/sort.rs:17-46, 48-126, 147-201): the hits are the first
+ * top_count keys of the query's score map in field order, each with its score-map value; top_count = limit + offset,
+ * 2 x (limit + offset) for an ACTIVE pinned query (see oc_pins).  Then the pins are spliced (as oc_search_pinned) and
+ * skip(offset).take(limit).  The score map ("keys") is oc_search's: fulltext matches with the where-filter, uncommitted
+ * deletes and the threshold applied, plus the vector hits at depth limit; scores are final (hybrid fusion, OMC).
+ *   - count is unchanged (oc_search's), and a NaN score is KEPT: unlike score order, field order has no NotNan filter.
+ *   - A key with no value in the field never appears, so a page can hold fewer than min(limit, count - offset) hits.
+ *   - Order: by value (a number; a date as its i64 millisecond timestamp; a bool as 0 / 1, so false first in ASC).
+ * Deliberate deviations from the reference:
+ *   1. equal values: ascending document id, in both orders (the reference's order inside a value batch comes from an
+ *      un-vendored crate);
+ *   2. a document with several values (array field) is placed once, at its first value in the requested order: the
+ *      minimum for ASC, the maximum for DESC;
+ *   3. always a full page: the reference's single-index path stops collecting value batches once their total size,
+ *      counting documents that are not keys, reaches top_count, so its answer is a prefix of this one; its multi-index
+ *      path has no such cut and behaves as this library does everywhere;
+ *   4. the multi-index merge (oc_merge_sorted) compares the true values; the reference compares i32 / f32 keys and
+ *      clamps dates to the i32 range, which makes its cross-index date order effectively index order;
+ *   5. as oc_pins: a matched consequence with an empty promote list does not double top_count. */
+typedef struct oc_sort_field oc_sort_field;
+/* One (document, value) entry per value: documents may repeat (multi-valued fields).  A bool is 0 / 1, a date its
+ * millisecond timestamp; integers beyond 2^53 do not round-trip through the double and are not representable here.
+ * Ids >= nbits are ignored.  OC_ERR_INVALID: a NaN value, nbits == 0 or >= 2^32 - 1.  Sorted once on the host (setup,
+ * not the hot path); per order the device holds the documents in rank order (8 B each) and a rank per document id
+ * (4 x nbits bytes), plus a rank -> string row map rebuilt on the first sorted search after each oc_str_commit.  The
+ * handle is immutable: a changed field means a new handle. */
+int oc_sort_field_create(oc_ctx *ctx, uint64_t nbits, uint64_t n, const uint64_t *doc_ids, const double *values,
+                         oc_sort_field **out);
+void oc_sort_field_destroy(oc_sort_field *f);
+#define OC_SORT_ASC 0
+#define OC_SORT_DESC 1
+typedef struct {
+    const oc_sort_field *field;
+    int order;                       /* OC_SORT_ASC (the reference's default) or OC_SORT_DESC */
+} oc_sort;
+/* oc_search_pinned in field order.  out_doc_ids / out_scores / out_sort_values: B x limit; a hit's sort value is the
+ * value it was placed by, NaN for a promoted item (placed by its position); out_sort_values may be NULL.  out_n: hits written; out_count:
+ * oc_search's count.  pins may be NULL; out_pin_scores / out_pin_present as in oc_search_pinned (may be NULL).
+ * OC_ERR_UNSUPPORTED: p->sharded, limit + offset > OC_MAX_TOPK, an active query with 2 x (limit + offset) >
+ * OC_MAX_TOPK.  OC_ERR_INVALID: a bad order, a NULL sort or field, a handle of another ctx.  A failed call writes
+ * nothing. */
+int oc_search_sorted(oc_ctx *ctx, oc_emb *emb, oc_str *str, const oc_search_params *p, const oc_sort *sort,
+                     const oc_pins *pins, uint64_t *out_doc_ids, float *out_scores, double *out_sort_values,
+                     uint32_t *out_n, uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present);
+/* oc_search_groups_pinned in field order: per group the first max_results members that are keys, in field order (2 x
+ * max_results for an active query), with their score-map values (NaN kept), members with no value skipped; then the
+ * group's member items are spliced as in oc_search_groups_pinned.  The flat hits follow oc_search_sorted (not written
+ * when p->limit == 0).  group_stride follows oc_search_groups_pinned.  out_group_sort_values (B x n_groups x
+ * group_stride) may be NULL.  Refusals as oc_search_sorted and oc_search_groups_pinned.  Multi-index grouped sorting
+ * without pins: oc_merge_sorted over B x n_groups rows with limit = max_results. */
+int oc_search_groups_sorted(oc_ctx *ctx, oc_emb *emb, oc_str *str, oc_group_by *groups, const oc_search_params *p,
+                            uint32_t max_results, const oc_sort *sort, const oc_pins *pins, uint32_t group_stride,
+                            uint64_t *out_doc_ids, float *out_scores, double *out_sort_values, uint32_t *out_n,
+                            uint64_t *out_count, uint64_t *out_group_doc_ids, float *out_group_scores,
+                            double *out_group_sort_values, uint32_t *out_group_n);
+/* The multi-index union in field order (host, no device; MergeSortedIterator, read/sort.rs:491-559).  Run every index
+ * with oc_search_sorted, limit' = limit + offset (2 x (limit + offset) when pins apply, and then apply = 0),
+ * offset' = 0, vector_limit = limit, and pass its hits, sort values (in_stride = limit'), counts and per-item
+ * outputs.  The lists are merged by sort value in `order`; on equal values the index listed first wins.  count = the
+ * sum of the counts.  pins may be NULL; an active query is spliced as in oc_merge_pinned (a promoted item's sort
+ * value is NaN).  OC_ERR_INVALID: a bad order, n > in_stride, in_stride < 2 x (limit + offset) while a query is
+ * active, q_pin_offsets not monotone.  A failed call writes nothing. */
+int oc_merge_sorted(uint32_t n_indexes, uint32_t n_queries, uint32_t limit, uint32_t offset, uint32_t in_stride,
+                    int order, const uint64_t *const *doc_ids, const float *const *scores,
+                    const double *const *sort_values, const uint32_t *const *n, const uint64_t *const *counts,
+                    const oc_pins *pins, const float *const *pin_scores, const uint8_t *const *pin_present,
+                    uint64_t *out_doc_ids /* B x limit */, float *out_scores, double *out_sort_values,
+                    uint32_t *out_n, uint64_t *out_count);
+
 /* ---- term dictionary and query-term resolution (host only; no device needed) ------------------------
  * The step the reference performs before the posting walk: TextParser::tokenize_and_stem(term) —
  * originals, plus stems unless `exact`, [""] when nothing is left (token_score.rs:196-209) — and the

@@ -29,6 +29,7 @@ EXPORTED_SYMBOLS = [
     "oc_facets_create", "oc_facets_destroy", "oc_facets_add_field", "oc_facets_add_number_field", "oc_search_facets",
     "oc_group_by_create", "oc_group_by_destroy", "oc_search_groups",
     "oc_search_pinned", "oc_search_groups_pinned", "oc_merge_pinned",
+    "oc_sort_field_create", "oc_sort_field_destroy", "oc_search_sorted", "oc_search_groups_sorted", "oc_merge_sorted",
     "oc_dict_create", "oc_dict_destroy", "oc_dict_add_terms", "oc_dict_lookup", "oc_dict_size", "oc_dict_set_stemmer", "oc_stem_english",
     "oc_dict_resolve", "oc_resolved_arrays", "oc_resolved_fill", "oc_resolved_free",
 ]
@@ -67,6 +68,10 @@ class FacetReq(C.Structure):
 
 class Pins(C.Structure):
     _fields_ = [("q_pin_offsets", C.c_void_p), ("doc_ids", C.c_void_p), ("positions", C.c_void_p), ("apply", C.c_int)]
+
+
+class Sort(C.Structure):
+    _fields_ = [("field", C.c_void_p), ("order", C.c_int)]
 
 
 class ResolveParams(C.Structure):
@@ -175,6 +180,14 @@ def lib():
     L.oc_search_groups_pinned.argtypes = [vp, vp, vp, vp, C.POINTER(SearchParams), u32, C.POINTER(Pins), u32, vp, vp, vp, vp, vp, vp, vp]
     L.oc_merge_pinned.argtypes = [u32, u32, u32, u32, u32, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(Pins),
                                   C.POINTER(vp), C.POINTER(vp), vp, vp, vp, vp]
+    L.oc_sort_field_create.argtypes = [vp, u64, u64, vp, vp, C.POINTER(vp)]
+    L.oc_sort_field_destroy.argtypes = [vp]
+    L.oc_sort_field_destroy.restype = None
+    L.oc_search_sorted.argtypes = [vp, vp, vp, C.POINTER(SearchParams), C.POINTER(Sort), vp, vp, vp, vp, vp, vp, vp, vp]
+    L.oc_search_groups_sorted.argtypes = [vp, vp, vp, vp, C.POINTER(SearchParams), u32, C.POINTER(Sort), vp, u32, vp, vp, vp, vp,
+                                          vp, vp, vp, vp, vp]
+    L.oc_merge_sorted.argtypes = [u32, u32, u32, u32, u32, C.c_int, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp),
+                                  C.POINTER(vp), vp, C.POINTER(vp), C.POINTER(vp), vp, vp, vp, vp, vp]
     L.oc_dict_create.argtypes = [u32, C.POINTER(vp)]
     L.oc_dict_destroy.argtypes = [vp]
     L.oc_dict_destroy.restype = None

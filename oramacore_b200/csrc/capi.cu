@@ -8,6 +8,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <limits>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -25,6 +26,7 @@
 #include "fuse.cuh"
 #include "group.cuh"
 #include "pins.cuh"
+#include "sort.cuh"
 #include "tmap.cuh"
 #include "oramacore_b200.h"
 
@@ -157,6 +159,7 @@ struct oc_ctx {
     bool gemm_pending = false; const float *gemm_inv_norm = nullptr;
     DevBuf row_ft, grp_vdoc, grp_vscore, grp_vn, grp_gmin, grp_den, grp_doc, grp_score, grp_n;   // oc_search_groups
     DevBuf pin_row, pin_ft, pin_ftp, pin_score, pin_present, pin_top_doc, pin_top_score, pin_top_n, pin_gdoc, pin_gscore, pin_gn;   // pins
+    DevBuf srt_doc, srt_row, srt_n, srt_ft, srt_ftp, srt_score, srt_present, srt_zero;   // sortBy
     DevBuf q_bf16, q_rho, pre_post, dense_buf, g_thr, g_eps, g_ovf, g_ovfcnt, g_resc, g_cand, g_cnt, g_flag, g_max, r_qpad, r_qinv, r_map, r_doc, r_score, r_row, r_cnt, r_raw;
 
     HostBuf h_in, h_out, h_in0;   // h_in0 / in_blob0: query vectors + filter, uploaded before the descriptors
@@ -214,7 +217,8 @@ extern "C" void oc_shutdown(oc_ctx *c) {
                       &c->g_flag, &c->r_qpad, &c->r_qinv, &c->r_map, &c->r_doc, &c->r_score, &c->r_row, &c->r_cnt, &c->r_raw,
                       &c->row_ft, &c->grp_vdoc, &c->grp_vscore, &c->grp_vn, &c->grp_gmin, &c->grp_den, &c->grp_doc, &c->grp_score, &c->grp_n,
                       &c->pin_row, &c->pin_ft, &c->pin_ftp, &c->pin_score, &c->pin_present, &c->pin_top_doc, &c->pin_top_score,
-                      &c->pin_top_n, &c->pin_gdoc, &c->pin_gscore, &c->pin_gn};
+                      &c->pin_top_n, &c->pin_gdoc, &c->pin_gscore, &c->pin_gn,
+                      &c->srt_doc, &c->srt_row, &c->srt_n, &c->srt_ft, &c->srt_ftp, &c->srt_score, &c->srt_present, &c->srt_zero};
     for (DevBuf *b : bufs) b->release();
     c->h_in.release(); c->h_out.release();
     for (int i = 0; i < EV_N; i++) if (c->ev[i]) cudaEventDestroy(c->ev[i]);
@@ -1342,6 +1346,29 @@ extern "C" int oc_merge_results(uint32_t n_indexes, uint32_t B, uint32_t limit, 
     return OC_OK;
 }
 
+// apply_pin_rules_internal (read/sort.rs:285-391) on the host for query q: drop the promoted documents from top, then
+// insert the items, stably sorted by position, each with the score of the index that holds the document (else 0.0)
+static void splice_pins_host(std::vector<std::pair<uint64_t, float>> &top, const oc_pins *pins, uint32_t q, uint32_t n_indexes,
+                             const float *const *pin_scores, const uint8_t *const *pin_present) {
+    const uint32_t *off = pins->q_pin_offsets;
+    std::vector<std::pair<uint32_t, uint32_t>> items;   // (position, item), sorted stably by position
+    std::vector<uint64_t> promoted;
+    for (uint32_t j = off[q]; j < off[q + 1]; j++) { items.emplace_back(pins->positions[j], j); promoted.push_back(pins->doc_ids[j]); }
+    std::sort(promoted.begin(), promoted.end());
+    top.erase(std::remove_if(top.begin(), top.end(),
+                             [&](const std::pair<uint64_t, float> &e) { return std::binary_search(promoted.begin(), promoted.end(), e.first); }),
+              top.end());
+    std::stable_sort(items.begin(), items.end(), [](const std::pair<uint32_t, uint32_t> &a, const std::pair<uint32_t, uint32_t> &b) {
+        return a.first < b.first;
+    });
+    for (const auto &it : items) {
+        float s = 0.f;   // the disjoint maps: the score from the one index that holds the document, else 0.0
+        for (uint32_t i = 0; i < n_indexes; i++)
+            if (pin_present[i][it.second]) { s = pin_scores[i][it.second]; break; }
+        top.insert(top.begin() + std::min<size_t>(it.first, top.size()), std::make_pair(pins->doc_ids[it.second], s));
+    }
+}
+
 // apply_pin_rules_internal (read/sort.rs:285-391) on the host: the union's top list of an active query, spliced
 extern "C" int oc_merge_pinned(uint32_t n_indexes, uint32_t B, uint32_t limit, uint32_t offset, uint32_t in_stride,
                                const uint64_t *const *doc_ids, const float *const *scores, const uint32_t *const *n,
@@ -1364,32 +1391,82 @@ extern "C" int oc_merge_pinned(uint32_t n_indexes, uint32_t B, uint32_t limit, u
     if (any && in_stride < top_pinned)
         return fail(OC_ERR_INVALID, "pins: in_stride %u < 2 x (limit+offset) %llu", in_stride, (unsigned long long)top_pinned);
     std::vector<std::pair<uint64_t, float>> top;
-    std::vector<std::pair<uint32_t, uint32_t>> items;   // (position, item), sorted stably by position
-    std::vector<uint64_t> promoted;
     for (uint32_t q = 0; q < B; q++) {
         uint64_t cnt = 0;
         for (uint32_t i = 0; i < n_indexes; i++) cnt += counts[i][q];
         const bool active = pins->apply && off[q + 1] > off[q];
         merge_union_top(n_indexes, q, in_stride, doc_ids, scores, n, uint32_t(active ? top_pinned : uint64_t(limit) + offset), top);
-        if (active) {
-            items.clear(); promoted.clear();
-            for (uint32_t j = off[q]; j < off[q + 1]; j++) { items.emplace_back(pins->positions[j], j); promoted.push_back(pins->doc_ids[j]); }
-            std::sort(promoted.begin(), promoted.end());
-            top.erase(std::remove_if(top.begin(), top.end(),
-                                     [&](const std::pair<uint64_t, float> &e) { return std::binary_search(promoted.begin(), promoted.end(), e.first); }),
-                      top.end());
-            std::stable_sort(items.begin(), items.end(), [](const std::pair<uint32_t, uint32_t> &a, const std::pair<uint32_t, uint32_t> &b) {
-                return a.first < b.first;
-            });
-            for (const auto &it : items) {
-                float s = 0.f;   // the disjoint maps: the score from the one index that holds the document, else 0.0
-                for (uint32_t i = 0; i < n_indexes; i++)
-                    if (pin_present[i][it.second]) { s = pin_scores[i][it.second]; break; }
-                top.insert(top.begin() + std::min<size_t>(it.first, top.size()), std::make_pair(pins->doc_ids[it.second], s));
-            }
-        }
+        if (active) splice_pins_host(top, pins, q, n_indexes, pin_scores, pin_present);
         write_page(top, q, limit, offset, out_doc_ids, out_scores, out_n);
         out_count[q] = cnt;
+    }
+    return OC_OK;
+}
+
+// MergeSortedIterator (read/sort.rs:491-559) on the host: the per-index lists, each in field order, merged by sort value;
+// on equal values the index listed first wins (strict comparison), then pins and skip/take as oc_merge_pinned
+extern "C" int oc_merge_sorted(uint32_t n_indexes, uint32_t B, uint32_t limit, uint32_t offset, uint32_t in_stride, int order,
+                               const uint64_t *const *doc_ids, const float *const *scores, const double *const *sort_values,
+                               const uint32_t *const *n, const uint64_t *const *counts, const oc_pins *pins,
+                               const float *const *pin_scores, const uint8_t *const *pin_present, uint64_t *out_doc_ids,
+                               float *out_scores, double *out_sort_values, uint32_t *out_n, uint64_t *out_count) {
+    if (!doc_ids || !scores || !sort_values || !n || !counts || !out_doc_ids || !out_scores || !out_n || !out_count)
+        return fail(OC_ERR_INVALID, "NULL argument");
+    if (limit == 0) return fail(OC_ERR_INVALID, "limit must be >= 1");
+    if (order != OC_SORT_ASC && order != OC_SORT_DESC) return fail(OC_ERR_INVALID, "sort order %d is neither ASC nor DESC", order);
+    if (pins && !pins->q_pin_offsets) return fail(OC_ERR_INVALID, "pins: q_pin_offsets is NULL");
+    const uint32_t *off = pins ? pins->q_pin_offsets : nullptr;
+    const uint64_t top_plain = uint64_t(limit) + offset, top_pinned = top_plain * 2;
+    bool any = false;
+    for (uint32_t q = 0; q < B; q++) {   // everything is checked before anything is written
+        if (off && off[q + 1] < off[q]) return fail(OC_ERR_INVALID, "pins: q_pin_offsets is not monotone at query %u", q);
+        any = any || (off && pins->apply && off[q + 1] > off[q]);
+        for (uint32_t i = 0; i < n_indexes; i++)
+            if (n[i][q] > in_stride) return fail(OC_ERR_INVALID, "index %u query %u: n > in_stride", i, q);
+    }
+    if (any && (!pins->doc_ids || !pins->positions || !pin_scores || !pin_present)) return fail(OC_ERR_INVALID, "NULL pin argument");
+    if (any && in_stride < top_pinned)
+        return fail(OC_ERR_INVALID, "pins: in_stride %u < 2 x (limit+offset) %llu", in_stride, (unsigned long long)top_pinned);
+    std::vector<std::pair<uint64_t, float>> top;
+    std::vector<std::pair<uint64_t, double>> placed;   // (doc, sort value) of the merged entries, by doc
+    std::vector<uint32_t> head(n_indexes);
+    for (uint32_t q = 0; q < B; q++) {
+        uint64_t cnt = 0;
+        for (uint32_t i = 0; i < n_indexes; i++) cnt += counts[i][q];
+        const bool active = off && pins->apply && off[q + 1] > off[q];
+        const uint64_t take = active ? top_pinned : top_plain;
+        std::fill(head.begin(), head.end(), 0u);
+        top.clear(); placed.clear();
+        while (top.size() < take) {
+            int best = -1;
+            for (uint32_t i = 0; i < n_indexes; i++) {
+                if (head[i] >= n[i][q]) continue;
+                if (best < 0) { best = (int)i; continue; }
+                const double va = sort_values[i][size_t(q) * in_stride + head[i]], vb = sort_values[best][size_t(q) * in_stride + head[best]];
+                if (order == OC_SORT_ASC ? va < vb : va > vb) best = (int)i;
+            }
+            if (best < 0) break;
+            const size_t at = size_t(q) * in_stride + head[best];
+            top.emplace_back(doc_ids[best][at], scores[best][at]);
+            placed.emplace_back(doc_ids[best][at], sort_values[best][at]);
+            head[best]++;
+        }
+        if (active) splice_pins_host(top, pins, q, n_indexes, pin_scores, pin_present);
+        write_page(top, q, limit, offset, out_doc_ids, out_scores, out_n);
+        out_count[q] = cnt;
+        if (!out_sort_values) continue;
+        std::sort(placed.begin(), placed.end());
+        for (uint32_t k = 0; k < limit; k++) {
+            double v = 0.0;
+            if (k < out_n[q]) {
+                const uint64_t d = out_doc_ids[size_t(q) * limit + k];
+                bool promoted = false;
+                for (uint32_t j = active ? off[q] : 0; active && j < off[q + 1]; j++) promoted = promoted || pins->doc_ids[j] == d;
+                auto it = std::lower_bound(placed.begin(), placed.end(), std::make_pair(d, -std::numeric_limits<double>::infinity()));
+                v = (promoted || it == placed.end() || it->first != d) ? std::numeric_limits<double>::quiet_NaN() : it->second;
+            }
+            out_sort_values[size_t(q) * limit + k] = v;
+        }
     }
     return OC_OK;
 }
@@ -1607,16 +1684,78 @@ static int pin_job_init(const oc_pins *pins, uint32_t B, PinJob &pj) {
     }
     return OC_OK;
 }
+// ------------------------------------------------------------------------------------ sortBy (sort.cuh)
+// A sort field, per order: the documents in rank order (value, then ascending id; each document once, at its first
+// value in that order), the rank of every document id, and the string row of every rank for one snapshot of one string
+// store (rebuilt when a search sees another snapshot, i.e. after a commit).  Host copies give the outputs' sort values.
+struct SortOrder {
+    uint64_t n = 0;
+    uint64_t *rank_doc = nullptr;          // device [n]
+    uint32_t *doc_rank = nullptr;          // device [nbits], RANK_NONE = no value
+    uint32_t *rank_row = nullptr;          // device [n + 1]; rank_row[n] = RANK_NONE (the mapping kernel's count)
+    std::weak_ptr<StrSnap> rows_of;        // the snapshot rank_row maps to
+    std::vector<uint32_t> h_doc_rank;      // [nbits]
+    std::vector<double> h_value;           // [n] value of each rank
+};
+struct oc_sort_field {
+    oc_ctx *ctx;
+    uint64_t nbits;
+    SortOrder ord[2];                      // OC_SORT_ASC, OC_SORT_DESC
+};
+static void sort_field_free(oc_sort_field *f) {
+    for (SortOrder &o : f->ord) { cudaFree(o.rank_doc); cudaFree(o.doc_rank); cudaFree(o.rank_row); }
+    delete f;
+}
+struct SortJob {
+    oc_sort_field *f;
+    int order;
+    double *out_values;                    // B x limit, may be NULL
+    double *out_group_values;              // B x n_groups x group_stride, may be NULL
+    uint32_t n_groups;
+};
+static int sort_job_init(oc_ctx *c, const oc_sort *s, SortJob &sj) {
+    if (!s || !s->field) return fail(OC_ERR_INVALID, "NULL sort");
+    if (s->order != OC_SORT_ASC && s->order != OC_SORT_DESC) return fail(OC_ERR_INVALID, "sort order %d is neither ASC nor DESC", s->order);
+    if (s->field->ctx != c) return fail(OC_ERR_INVALID, "sort field belongs to another ctx");
+    sj.f = const_cast<oc_sort_field *>(s->field);   // only its per-snapshot row map is refreshed, under the ctx lock
+    sj.order = s->order;
+    return OC_OK;
+}
+// the value a listed document was placed by: NaN for a document the (active) query promotes, else its value
+static double sort_value_of(const SortJob &sj, const PinJob *pj, uint32_t q, uint64_t d) {
+    if (pj && pj->splice)
+        for (uint32_t j = 0; j < pj->cnt[q]; j++)
+            if (pj->doc[size_t(q) * pj->stride + j] == d) return std::numeric_limits<double>::quiet_NaN();
+    const SortOrder &o = sj.f->ord[sj.order];
+    const uint32_t r = d < sj.f->nbits ? o.h_doc_rank[d] : RANK_NONE;
+    return r == RANK_NONE ? std::numeric_limits<double>::quiet_NaN() : o.h_value[r];
+}
+// rank -> string row of snapshot S (kept until another snapshot is searched)
+static int sort_rows_for(oc_ctx *c, SortOrder &o, const std::shared_ptr<StrSnap> &snap) {
+    if (o.rows_of.lock() == snap) return OC_OK;
+    constexpr uint64_t CH = 1ull << 30;
+    for (uint64_t a = 0; a < o.n; a += CH) {
+        const uint32_t len = (uint32_t)std::min<uint64_t>(CH, o.n - a);
+        map_docs_to_rows_kernel<<<(len + 255) / 256, 256, 0, c->stream>>>(o.rank_doc + a, o.rank_row + o.n, len, 1, snap->row_doc,
+                                                                          snap->n_rows, o.rank_row + a);
+        launched(c);
+        CU(cudaGetLastError());
+    }
+    o.rows_of = snap;
+    return OC_OK;
+}
+
 static int run_groups(oc_ctx *c, const GroupJob &gj, uint32_t B, int mode, const StrSnap *S, uint32_t n_tiles, uint32_t vlimit,
-                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, const PinJob *pj);
+                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, const PinJob *pj, const SortJob *sj);
 
 // gj != NULL: oc_search_groups.  Then limit == 0 is allowed: the hits are not written (out_doc_ids / out_scores / out_n
 // may be NULL), the vector stage gets depth 0 and the fulltext stage runs with one candidate slot per tile.
 // pj != NULL: the pinned calls; the items' score-map values go to out_pin_scores / out_pin_present (may be NULL).
+// sj != NULL: the sorted calls (always with pj); the hits are the walk's in field order, K4's list only gives the count.
 static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, uint64_t *out_doc_ids,
                        float *out_scores, uint32_t *out_n, uint64_t *out_count, const FacetJob *fj, const GroupJob *gj = nullptr,
                        PinJob *pj = nullptr, const oc_pins *pins = nullptr, float *out_pin_scores = nullptr,
-                       uint8_t *out_pin_present = nullptr) {
+                       uint8_t *out_pin_present = nullptr, const SortJob *sj = nullptr) {
     if (!c || !p || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
     const bool write_hits = !gj || p->limit > 0;
     if (write_hits && (!out_doc_ids || !out_scores || !out_n)) return fail(OC_ERR_INVALID, "NULL argument");
@@ -1632,7 +1771,10 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     if (p->limit == 0 && !gj) return fail(OC_ERR_INVALID, "limit must be >= 1");
     const uint32_t limit = write_hits ? p->limit : 1;
     // sort_token_scores with pins selects the top 2 * (limit + offset) (sort.rs:25-34); the vector depth stays limit
-    const bool pin_flat = pj && pj->splice && write_hits;
+    const bool pin_flat = pj && pj->splice && write_hits && !sj;
+    const bool sort_flat = sj && write_hits;
+    // sort_token_scores with sort_by: top_count keys in field order, twice as many for an active pinned query
+    const uint32_t sort_top = sort_flat ? uint32_t((uint64_t(limit) + p->offset) * (pj->splice ? 2 : 1)) : 0u;
     const uint64_t n_keep64 = (uint64_t(limit) + p->offset) * (pin_flat ? 2 : 1);
     if (n_keep64 > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "limit+offset %llu > %u", (unsigned long long)n_keep64, OC_MAX_TOPK);
     const uint32_t n_keep = (uint32_t)n_keep64;
@@ -2053,7 +2195,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
                 off += cls_nq[g] * n_tiles; q0 += cls_nq[g];
             }
         }
-        if (fj || gj) {   // facets / groups: the tile kernels also emit the bitmap of matched rows (every (query, tile) item writes its 256 words)
+        if (fj || gj || sj) {   // facets / groups / sortBy: the tile kernels also emit the bitmap of matched rows (every (query, tile) item writes its 256 words)
             OCTRY(c->mbits.ensure(size_t(B) * std::max<uint32_t>(n_tiles, 1) * (BM25_TILE / 32) * 4));
             bp.matched_bits = c->mbits.as<uint32_t>();
         }
@@ -2073,7 +2215,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     };
     if (has_ft) OCTRY(bm25_stage());
 
-    const bool exports = gj || pj;   // K4 exports the normalisation and the vector part of the score map
+    const bool exports = gj || pj || sj;   // K4 exports the normalisation and the vector part of the score map
     // pins, after K4: the score-map value of every promoted document, then (pin_flat) the splice into K4's top list
     auto pin_tail = [&]() -> int {
         if (!pin_items) return OC_OK;
@@ -2119,6 +2261,71 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
             pin_splice_kernel<<<B, PIN_THREADS, smem, c->stream>>>(xp);
             launched(c);
         }
+        CU(cudaGetLastError());
+        return OC_OK;
+    };
+    // sortBy, after K4 and the pins' scores: the first sort_top keys in field order, scored like promoted documents,
+    // then paged with the pins spliced (pin_splice_kernel writes the hits over K4's)
+    auto sort_tail = [&]() -> int {
+        if (!sort_flat) return OC_OK;
+        SortOrder &so = sj->f->ord[sj->order];
+        const bool ft_map = has_ft && n_tiles > 0;
+        if (ft_map) OCTRY(sort_rows_for(c, so, snap));
+        const uint32_t top = sort_top;
+        const uint64_t nslot = uint64_t(B) * top;
+        const uint32_t vs = std::max<uint32_t>(vlimit, 1);
+        OCTRY(c->srt_doc.ensure(nslot * 8));
+        OCTRY(c->srt_row.ensure(nslot * 4));
+        OCTRY(c->srt_n.ensure(size_t(B) * 4));
+        OCTRY(c->srt_score.ensure(nslot * 4));
+        OCTRY(c->srt_present.ensure(nslot));
+        SortWalkParams wp{};
+        wp.n_ranks = so.n; wp.rank_row = ft_map ? so.rank_row : nullptr; wp.doc_rank = so.doc_rank; wp.nbits = sj->f->nbits;
+        wp.mbits = ft_map ? c->mbits.as<uint32_t>() : nullptr; wp.row_words = uint64_t(n_tiles) * (BM25_TILE / 32);
+        wp.v_doc = fp.out_vdoc; wp.v_n = fp.out_vn; wp.v_stride = vs;
+        wp.rank_doc = so.rank_doc; wp.top = top;
+        wp.out_doc = c->srt_doc.as<uint64_t>(); wp.out_row = c->srt_row.as<uint32_t>(); wp.out_n = c->srt_n.as<uint32_t>();
+        sort_walk_kernel<<<B, SORT_THREADS, size_t(vs) * 4, c->stream>>>(wp);
+        launched(c);
+        const unsigned warp_grid = (unsigned)((nslot * 32 + 255) / 256);
+        if (has_ft) {   // the selected rows' fulltext scores (RANK_NONE rows: vector hits without a row, empty slots)
+            OCTRY(c->srt_ft.ensure(nslot * 4));
+            OCTRY(c->srt_ftp.ensure(nslot));
+            PointParams pp{};
+            pp.terms = bp.terms; pp.tokens = bp.tokens; pp.queries = bp.queries;
+            pp.n_queries = B; pp.v_stride = top; pp.v_row = c->srt_row.as<uint32_t>(); pp.row_ok_bits = row_ok;
+            pp.k = p->bm25_k; pp.threshold = thr ? 1 : 0;
+            pp.v_ft = c->srt_ft.as<float>(); pp.v_present = c->srt_ftp.as<uint8_t>();
+            bm25_point_kernel<<<warp_grid, 256, 0, c->stream>>>(pp);
+            launched(c);
+        }
+        PinScoreParams sp{};
+        sp.n_queries = B; sp.stride = top; sp.doc = c->srt_doc.as<uint64_t>(); sp.cnt = c->srt_n.as<uint32_t>();
+        sp.has_ft = has_ft; sp.hybrid = has_ft && has_v;
+        sp.ft = c->srt_ft.as<float>(); sp.ft_present = c->srt_ftp.as<uint8_t>();
+        sp.gmin = fp.out_gmin; sp.den = fp.out_den;
+        sp.v_doc = fp.out_vdoc; sp.v_score = fp.out_vscore; sp.v_n = fp.out_vn; sp.v_stride = vs;
+        sp.omc_doc = fp.omc_doc; sp.omc_mult = fp.omc_mult; sp.n_omc = n_omc;
+        sp.out_score = c->srt_score.as<float>(); sp.out_present = c->srt_present.as<uint8_t>();
+        pin_score_kernel<<<warp_grid, 256, 0, c->stream>>>(sp);
+        launched(c);
+        PinSpliceParams xp{};
+        if (pj->splice) {
+            xp.stride = pj->stride; xp.kp2 = std::max<uint32_t>(32, next_pow2(pj->stride));
+            xp.doc = pj->d_doc; xp.pos = pj->d_pos; xp.score = c->pin_score.as<float>(); xp.cnt = pj->d_cnt;
+        } else {   // no item anywhere: every query takes the page of its list as it is
+            OCTRY(c->srt_zero.ensure(size_t(B) * 4));
+            CU(cudaMemsetAsync(c->srt_zero.p, 0, size_t(B) * 4, c->stream));
+            xp.stride = 0; xp.kp2 = 32;
+            xp.doc = c->srt_doc.as<uint64_t>(); xp.pos = c->srt_zero.as<uint32_t>(); xp.score = c->srt_score.as<float>();
+            xp.cnt = c->srt_zero.as<uint32_t>();
+        }
+        xp.n_top = top; xp.limit = limit; xp.offset = p->offset;
+        xp.top_doc = c->srt_doc.as<uint64_t>(); xp.top_score = c->srt_score.as<float>(); xp.top_n = c->srt_n.as<uint32_t>();
+        xp.out_doc = reinterpret_cast<uint64_t *>(dout + o_doc); xp.out_score = reinterpret_cast<float *>(dout + o_sc);
+        xp.out_n = reinterpret_cast<uint32_t *>(dout + o_n);
+        pin_splice_kernel<<<B, PIN_THREADS, pin_splice_smem(xp.kp2, top, limit + p->offset), c->stream>>>(xp);
+        launched(c);
         CU(cudaGetLastError());
         return OC_OK;
     };
@@ -2205,6 +2412,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         launched(c);
         CU(cudaGetLastError());
         OCTRY(pin_tail());
+        OCTRY(sort_tail());
         CU(cudaEventRecord(c->ev[EV_FUSE1], c->stream));
     }
     return OC_OK;
@@ -2258,6 +2466,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
             else fuse_topk_kernel<<<B, 256, fuse_smem, c->stream>>>(fp);
             launched(c);
             OCTRY(pin_tail());
+            OCTRY(sort_tail());
             CU(cudaMemcpyAsync(c->h_out.p, dout, out_bytes, cudaMemcpyDeviceToHost, c->stream));
             CU(cudaStreamSynchronize(c->stream));
         }
@@ -2265,7 +2474,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     if (fj) OCTRY(run_facets(c, *fj, B, has_ft, has_v, S, n_tiles, vlimit));
     if (gj) {
         CU(cudaEventRecord(c->ev[EV_GRP0], c->stream));
-        OCTRY(run_groups(c, *gj, B, p->mode, S, n_tiles, vlimit, fp.omc_doc, fp.omc_mult, n_omc, pj));
+        OCTRY(run_groups(c, *gj, B, p->mode, S, n_tiles, vlimit, fp.omc_doc, fp.omc_mult, n_omc, pj, sj));
         CU(cudaEventRecord(c->ev[EV_GRP1], c->stream));
         CU(cudaStreamSynchronize(c->stream));
     }
@@ -2285,6 +2494,21 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         memcpy(out_n, h + o_n, size_t(B) * 4);
     }
     memcpy(out_count, h + o_cnt, size_t(B) * 8);
+    if (sort_flat && sj->out_values)
+        for (uint32_t q = 0; q < B; q++)
+            for (uint32_t i = 0; i < limit; i++) {
+                const size_t o = size_t(q) * limit + i;
+                sj->out_values[o] = i < out_n[q] ? sort_value_of(*sj, pj, q, out_doc_ids[o]) : 0.0;
+            }
+    if (sj && gj && sj->out_group_values) {   // run_groups' copies are complete (synchronised above)
+        const uint32_t G = sj->n_groups;
+        for (uint32_t q = 0; q < B; q++)
+            for (uint32_t g = 0; g < G; g++)
+                for (uint32_t i = 0; i < gj->stride; i++) {
+                    const size_t o = (size_t(q) * G + g) * gj->stride + i;
+                    sj->out_group_values[o] = i < gj->out_n[size_t(q) * G + g] ? sort_value_of(*sj, pj, q, gj->out_doc[o]) : 0.0;
+                }
+    }
     if (!pin_sc.empty())
         for (uint32_t q = 0; q < B; q++)
             for (uint32_t j = 0; j < pj->cnt[q]; j++) {
@@ -2643,7 +2867,7 @@ extern "C" int oc_group_by_create(oc_facets *f, const uint32_t *fields, uint32_t
 }
 
 static int run_groups(oc_ctx *c, const GroupJob &gj, uint32_t B, int mode, const StrSnap *S, uint32_t n_tiles, uint32_t vlimit,
-                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, const PinJob *pj) {
+                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, const PinJob *pj, const SortJob *sj) {
     oc_group_by *g = gj.g;
     // sort_groups with pins takes every group's top 2 * max_results (sort.rs:137-142)
     const bool pin_grp = pj && pj->splice;
@@ -2678,10 +2902,13 @@ static int run_groups(oc_ctx *c, const GroupJob &gj, uint32_t B, int mode, const
     gp.v_stride = std::max<uint32_t>(vlimit, 1);
     gp.omc_doc = omc_doc; gp.omc_mult = omc_mult; gp.n_omc = n_omc;
     gp.out_doc = c->grp_doc.as<uint64_t>(); gp.out_score = c->grp_score.as<float>(); gp.out_n = c->grp_n.as<uint32_t>();
+    if (sj) { gp.doc_rank = sj->f->ord[sj->order].doc_rank; gp.rank_nbits = sj->f->nbits; }
+    const void *kern = sj ? (const void *)group_sort_topk_kernel : (const void *)group_topk_kernel;
     const size_t smem = (size_t(GROUP_BUF) + gp.kp2 + gp.vp2) * 8 + size_t(gp.vp2) * 4;
-    if (smem_cfg_needed(c->device, (const void *)group_topk_kernel, smem))
-        CU(cudaFuncSetAttribute(group_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    group_topk_kernel<<<dim3(G, B), GROUP_THREADS, smem, c->stream>>>(gp);
+    if (smem_cfg_needed(c->device, kern, smem))
+        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (sj) group_sort_topk_kernel<<<dim3(G, B), GROUP_THREADS, smem, c->stream>>>(gp);
+    else group_topk_kernel<<<dim3(G, B), GROUP_THREADS, smem, c->stream>>>(gp);
     launched(c);
     CU(cudaGetLastError());
     if (pj) {   // oc_search_groups_pinned: every group's list at the caller's stride, spliced for the queries with items
@@ -2770,6 +2997,103 @@ extern "C" int oc_search_groups_pinned(oc_ctx *c, oc_emb *emb, oc_str *str, oc_g
     GroupJob gj{groups, max_results, out_group_doc_ids, out_group_scores, out_group_n};
     gj.stride = group_stride;
     return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, &gj, &pj, pins);
+}
+
+// ------------------------------------------------------------------------------------ sortBy (sort.cuh)
+extern "C" int oc_sort_field_create(oc_ctx *c, uint64_t nbits, uint64_t n, const uint64_t *doc_ids, const double *values,
+                                    oc_sort_field **out) {
+    if (!c || !out || nbits == 0 || (n && (!doc_ids || !values))) return fail(OC_ERR_INVALID, "bad arguments");
+    if (nbits >= RANK_NONE) return fail(OC_ERR_INVALID, "nbits %llu >= 2^32 - 1", (unsigned long long)nbits);
+    std::vector<std::pair<double, uint64_t>> e;
+    e.reserve(n);
+    for (uint64_t i = 0; i < n; i++) {
+        if (values[i] != values[i]) return fail(OC_ERR_INVALID, "sort value %llu is NaN", (unsigned long long)i);
+        if (doc_ids[i] < nbits) e.emplace_back(values[i] + 0.0, doc_ids[i]);   // -0.0 ties with 0.0
+    }
+    oc_sort_field *f = new oc_sort_field();
+    f->ctx = c; f->nbits = nbits;
+    auto fail_free = [&](int code) { sort_field_free(f); return code; };
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (cudaSetDevice(c->device) != cudaSuccess) return fail_free(fail(OC_ERR_CUDA, "cudaSetDevice failed"));
+    std::vector<uint64_t> rank_doc;
+    for (int ord = OC_SORT_ASC; ord <= OC_SORT_DESC; ord++) {
+        // value in the requested order, ties by ascending id; a document keeps its first position
+        std::sort(e.begin(), e.end(), [ord](const std::pair<double, uint64_t> &a, const std::pair<double, uint64_t> &b) {
+            if (a.first != b.first) return ord == OC_SORT_ASC ? a.first < b.first : a.first > b.first;
+            return a.second < b.second;
+        });
+        SortOrder &o = f->ord[ord];
+        o.h_doc_rank.assign(nbits, RANK_NONE);
+        rank_doc.clear();
+        for (const auto &x : e)
+            if (o.h_doc_rank[x.second] == RANK_NONE) {
+                o.h_doc_rank[x.second] = (uint32_t)rank_doc.size();
+                rank_doc.push_back(x.second);
+                o.h_value.push_back(x.first);
+            }
+        o.n = rank_doc.size();
+        const uint32_t none = RANK_NONE;
+        cudaError_t err = cudaMalloc(&o.rank_doc, std::max<size_t>(o.n, 1) * 8);
+        if (err == cudaSuccess) err = cudaMalloc(&o.doc_rank, nbits * 4);
+        if (err == cudaSuccess) err = cudaMalloc(&o.rank_row, (o.n + 1) * 4);
+        if (err == cudaSuccess && o.n) err = cudaMemcpy(o.rank_doc, rank_doc.data(), o.n * 8, cudaMemcpyHostToDevice);
+        if (err == cudaSuccess) err = cudaMemcpy(o.doc_rank, o.h_doc_rank.data(), nbits * 4, cudaMemcpyHostToDevice);
+        if (err == cudaSuccess) err = cudaMemcpy(o.rank_row + o.n, &none, 4, cudaMemcpyHostToDevice);
+        if (err != cudaSuccess)
+            return fail_free(fail(err == cudaErrorMemoryAllocation ? OC_ERR_OOM : OC_ERR_CUDA, "sort field upload: %s", cudaGetErrorString(err)));
+    }
+    *out = f;
+    return OC_OK;
+}
+
+extern "C" void oc_sort_field_destroy(oc_sort_field *f) {
+    if (!f) return;
+    {
+        std::lock_guard<std::mutex> lk(f->ctx->mu);
+        cudaSetDevice(f->ctx->device);
+        cudaStreamSynchronize(f->ctx->stream);
+    }
+    sort_field_free(f);
+}
+
+extern "C" int oc_search_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, const oc_sort *sort,
+                                const oc_pins *pins, uint64_t *out_doc_ids, float *out_scores, double *out_sort_values,
+                                uint32_t *out_n, uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present) {
+    if (!c || !p) return fail(OC_ERR_INVALID, "NULL argument");
+    SortJob sj{};
+    OCTRY(sort_job_init(c, sort, sj));
+    sj.out_values = out_sort_values;
+    PinJob pj;
+    OCTRY(pin_job_init(pins, p->n_queries, pj));
+    OCTRY(pins_check_flat(p, pj));
+    return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, nullptr, &pj, pins, out_pin_scores,
+                       out_pin_present, &sj);
+}
+
+extern "C" int oc_search_groups_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, oc_group_by *groups, const oc_search_params *p,
+                                       uint32_t max_results, const oc_sort *sort, const oc_pins *pins, uint32_t group_stride,
+                                       uint64_t *out_doc_ids, float *out_scores, double *out_sort_values, uint32_t *out_n,
+                                       uint64_t *out_count, uint64_t *out_group_doc_ids, float *out_group_scores,
+                                       double *out_group_sort_values, uint32_t *out_group_n) {
+    if (!c || !p || !groups || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
+    if (groups->n_groups && (!out_group_n || (group_stride && (!out_group_doc_ids || !out_group_scores))))
+        return fail(OC_ERR_INVALID, "NULL group output");
+    if (groups->ctx != c) return fail(OC_ERR_INVALID, "group_by belongs to another ctx");
+    SortJob sj{};
+    OCTRY(sort_job_init(c, sort, sj));
+    sj.out_values = out_sort_values; sj.out_group_values = out_group_sort_values; sj.n_groups = groups->n_groups;
+    if (max_results > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "max_results %u > %u", max_results, OC_MAX_TOPK);
+    if (p->n_queries > 65535) return fail(OC_ERR_UNSUPPORTED, "groups: n_queries %u > 65535", p->n_queries);
+    PinJob pj;
+    OCTRY(pin_job_init(pins, p->n_queries, pj));
+    OCTRY(pins_check_flat(p, pj));
+    if (pj.splice && 2 * max_results > OC_MAX_TOPK)
+        return fail(OC_ERR_UNSUPPORTED, "pins: 2 x max_results %u > %u", 2 * max_results, OC_MAX_TOPK);
+    const uint64_t need = pj.splice ? 2ull * max_results + pj.stride : max_results;
+    if (group_stride < need) return fail(OC_ERR_INVALID, "group_stride %u < %llu", group_stride, (unsigned long long)need);
+    GroupJob gj{groups, max_results, out_group_doc_ids, out_group_scores, out_group_n};
+    gj.stride = group_stride;
+    return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, &gj, &pj, pins, nullptr, nullptr, &sj);
 }
 
 // ------------------------------------------------------------------------------------ micro-batching front

@@ -41,10 +41,16 @@ struct GroupParams {
     uint64_t *out_doc;              // [q][n_groups][max_results]
     float *out_score;
     uint32_t *out_n;                // [q][n_groups]
+    // group_sort_topk_kernel: the sort field's rank of each document id (0xffffffff = no value)
+    const uint32_t *doc_rank;
+    uint64_t rank_nbits;
 };
 
-// one CTA per (group, query): grid (n_groups, n_queries)
-__global__ void __launch_bounds__(GROUP_THREADS) group_topk_kernel(const GroupParams p) {
+// SORT = false: the top max_results members by score (score desc, ties by ascending id, NaN dropped).
+// SORT = true (sortBy, sort_groups with sort_by, read/sort.rs:147-166): the first max_results members in the sort
+// field's rank order; the key is the rank instead of the score, NaN scores are kept and members with no value skipped.
+template <bool SORT>
+__device__ __forceinline__ void group_topk_body(const GroupParams &p) {
     extern __shared__ __align__(16) uint8_t smem[];
     uint64_t *buf = reinterpret_cast<uint64_t *>(smem);   // [GROUP_BUF] candidate keys (score | position in group)
     uint64_t *sel = buf + GROUP_BUF;                       // [kp2]
@@ -89,8 +95,29 @@ __global__ void __launch_bounds__(GROUP_THREADS) group_topk_kernel(const GroupPa
     const uint32_t *mb = p.has_ft ? p.mbits + size_t(q) * p.row_words : nullptr;
     const float *rft = p.has_ft ? p.row_ft + size_t(q) * p.row_words * 32 : nullptr;
 
+    // sort: the i-th member's score-map value; *present = 0 when it is not a key
+    auto map_value = [&](uint64_t i, bool *present) -> float {
+        *present = true;
+        if (vc) {
+            const uint64_t d = gdoc[i];
+            uint32_t lo = 0, hi = vc;
+            while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (hdoc[mid] < d) lo = mid + 1; else hi = mid; }
+            if (lo < vc && hdoc[lo] == d) return hsc[lo];
+        }
+        const uint32_t row = p.has_ft ? grow[i] : 0xffffffffu;
+        if (row == 0xffffffffu || !((mb[row >> 5] >> (row & 31)) & 1u)) { *present = false; return 0.f; }
+        return fused_ft_score(rft[row], p.hybrid, gmin, den, p.omc_doc, p.omc_mult, p.n_omc, [&] { return gdoc[i]; });
+    };
     // rank key of the i-th document of the group, KEY_NONE when it is not a key of the score map (or scores NaN)
     auto load = [&](uint64_t i) -> uint64_t {
+        if constexpr (SORT) {   // larger key = smaller rank; ranks are unique, so the member index only decodes
+            const uint64_t d = gdoc[i];
+            const uint32_t r = d < p.rank_nbits ? p.doc_rank[d] : 0xffffffffu;
+            if (r == 0xffffffffu) return KEY_NONE;
+            bool present;
+            map_value(i, &present);
+            return present ? (uint64_t(0xffffffffu - r) << 32) | uint64_t(0xffffffffu - uint32_t(i)) : KEY_NONE;
+        }
         if (vc) {
             const uint64_t d = gdoc[i];
             uint32_t lo = 0, hi = vc;
@@ -145,11 +172,23 @@ __global__ void __launch_bounds__(GROUP_THREADS) group_topk_kernel(const GroupPa
     for (uint32_t i = tid; i < m; i += blockDim.x) {
         uint64_t doc = 0;
         float sc = 0.f;
-        if (i < kept) { doc = gdoc[key_idx(sel[i])]; sc = key_score(sel[i]); }
+        if (i < kept) {
+            doc = gdoc[key_idx(sel[i])];
+            if constexpr (SORT) {
+                bool present;
+                sc = map_value(key_idx(sel[i]), &present);   // NaN kept
+            } else {
+                sc = key_score(sel[i]);
+            }
+        }
         p.out_doc[og * m + i] = doc;
         p.out_score[og * m + i] = sc;
     }
     if (tid == 0) p.out_n[og] = kept;
 }
+
+// one CTA per (group, query): grid (n_groups, n_queries)
+__global__ void __launch_bounds__(GROUP_THREADS) group_topk_kernel(const GroupParams p) { group_topk_body<false>(p); }
+__global__ void __launch_bounds__(GROUP_THREADS) group_sort_topk_kernel(const GroupParams p) { group_topk_body<true>(p); }
 
 }  // namespace oc

@@ -14,14 +14,14 @@ from __future__ import annotations
 
 import ctypes as C
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Sequence
+from typing import Dict, List, Mapping, Optional, Sequence, Tuple
 
 import numpy as np
 
 from . import _lib
 from ._lib import OcError, SearchParams, Timing, check, lib
-from .types import (BM25_B, BM25_K, MODE_FULLTEXT, MODE_HYBRID, MODE_VECTOR, PromoteItem, SearchHits, StringIndexData,
-                    TextQuery)
+from .types import (BM25_B, BM25_K, MODE_FULLTEXT, MODE_HYBRID, MODE_VECTOR, InvalidSortField, PromoteItem, SearchHits,
+                    SortBy, SortFieldNotFound, StringIndexData, TextQuery)
 
 # Model::dimensions / rescale_score (python/embeddings.rs:52-92)
 MODEL_DIMS = {
@@ -441,11 +441,13 @@ class GroupBy:
 
 
 def search_groups_arrays(tsc: "TokenScoreContext", group_by: GroupBy, params: "TokenScoreParams", max_results: int = 1, texts=None,
-                         q_vecs: Optional[np.ndarray] = None, promote=None):
+                         q_vecs: Optional[np.ndarray] = None, promote=None, sort_by: Optional[Tuple["SortField", str]] = None):
     """oc_search_groups as arrays: (docs [B,limit], scores, n [B], count [B], group docs [B,G,stride], group scores,
     group n [B,G]); stride = max_results.  With `promote` (see search_pinned_arrays) the call is oc_search_groups_pinned:
     a query with items gets pinned hits and every group's top 2 * max_results with its member items spliced in
-    (apply_pin_rules_to_group), stride = 2 * max_results + the most items of one query."""
+    (apply_pin_rules_to_group), stride = 2 * max_results + the most items of one query.  With `sort_by` (a
+    (SortField, order) pair, see resolve_sort_by) the call is oc_search_groups_sorted: hits and groups in field order,
+    and two more arrays are returned, the hits' sort values [B,limit] and the groups' [B,G,stride]."""
     sp, keep, B = tsc._build_params(params, texts, q_vecs)
     L, G = params.limit_hint, group_by.n_groups
     pins = None if promote is None else _pins(promote, B)
@@ -457,6 +459,13 @@ def search_groups_arrays(tsc: "TokenScoreContext", group_by: GroupBy, params: "T
     gd, gs = np.zeros((B, G, stride), np.uint64), np.zeros((B, G, stride), np.float32)
     gn = np.zeros((B, G), np.uint32)
     emb, strs = tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None
+    if sort_by is not None:
+        srt = _sort(*sort_by)
+        sv, gsv = np.zeros((B, L), np.float64), np.zeros((B, G, stride), np.float64)
+        check(lib().oc_search_groups_sorted(tsc.ctx._h, emb, strs, group_by._h, C.byref(sp), int(max_results), C.byref(srt),
+                                            None if pins is None else C.byref(pins[0]), int(stride), _p(docs), _p(scores),
+                                            _p(sv), _p(n), _p(cnt), _p(gd), _p(gs), _p(gsv), _p(gn)))
+        return docs, scores, n, cnt, gd, gs, gn, sv, gsv
     if pins is None:
         check(lib().oc_search_groups(tsc.ctx._h, emb, strs, group_by._h, C.byref(sp), int(max_results), _p(docs), _p(scores), _p(n),
                                      _p(cnt), _p(gd), _p(gs), _p(gn)))
@@ -467,13 +476,14 @@ def search_groups_arrays(tsc: "TokenScoreContext", group_by: GroupBy, params: "T
 
 
 def search_groups(tsc: "TokenScoreContext", group_by: GroupBy, params: "TokenScoreParams", max_results: int = 1, texts=None,
-                  q_vecs: Optional[np.ndarray] = None, promote=None):
+                  q_vecs: Optional[np.ndarray] = None, promote=None, sort_by: Optional[Tuple["SortField", str]] = None):
     """search() with groupBy (search.rs:415-429 + sort_groups, read/sort.rs:129-230): per query (hits, groups), groups a
     list in group order of {"values": [...], "result": [(doc_id, score), ...]} (GroupedResult, types.rs:1375), the
     top max_results documents of the group that are in the query's score map.  limit_hint 0 is allowed: no hits, and no
     vector search (the reference's limit_hint = 0).  `promote`: the pin rules' promote items per query (see
-    search_pinned_arrays)."""
-    docs, scores, n, cnt, gd, gs, gn = search_groups_arrays(tsc, group_by, params, max_results, texts, q_vecs, promote)
+    search_pinned_arrays).  `sort_by`: a (SortField, order) pair; hits and group members then come in field order
+    (sort_groups with sort_by, read/sort.rs:147-166)."""
+    docs, scores, n, cnt, gd, gs, gn = search_groups_arrays(tsc, group_by, params, max_results, texts, q_vecs, promote, sort_by)[:7]
     out = []
     for q in range(cnt.shape[0]):
         hits = SearchHits(docs[q, :n[q]].copy(), scores[q, :n[q]].copy(), int(cnt[q]))
@@ -554,6 +564,115 @@ def merge_index_results_pinned(per_index, promote, limit: int, offset: int = 0, 
     check(lib().oc_merge_pinned(k, B, limit, offset, stride, arr(0), arr(1), arr(2), arr(3), C.byref(pins), arr(4), arr(5),
                                 _p(od), _p(os_), _p(on), _p(oc)))
     return [SearchHits(od[i, :on[i]].copy(), os_[i, :on[i]].copy(), int(oc[i])) for i in range(B)]
+
+
+class SortField:
+    """A number, date or bool filter field laid out for sortBy on the device (oc_sort_field_*): one (doc_id, value)
+    entry per value, so a multi-valued document repeats.  kind "number": any real value; "date": millisecond
+    timestamps (integers or numpy datetime64); "bool": False / True.  Integers beyond 2^53 and NaN are refused: the
+    values travel as doubles.  Immutable: build a new one when the field changes."""
+    KINDS = ("number", "date", "bool")
+
+    def __init__(self, ctx: Context, nbits: int, doc_ids, values, kind: str):
+        if kind not in self.KINDS:
+            raise ValueError(f"sort field kind {kind!r}: expected one of {self.KINDS}")
+        d = np.ascontiguousarray(np.asarray(doc_ids, np.uint64).reshape(-1))
+        v = np.asarray(values)
+        if kind == "date" and np.issubdtype(v.dtype, np.datetime64):
+            v = v.astype("datetime64[ms]").astype(np.int64)
+        if kind == "bool":
+            v = np.asarray(v, bool).astype(np.float64)
+        elif np.issubdtype(v.dtype, np.integer):
+            if v.size and int(np.max(np.abs(v.astype(object)))) > 2 ** 53:
+                raise ValueError("sort value beyond 2^53: it does not round-trip through a double")
+            v = v.astype(np.float64)
+        else:
+            v = v.astype(np.float64)
+        v = np.ascontiguousarray(v.reshape(-1))
+        if v.shape != d.shape:
+            raise ValueError(f"{d.shape[0]} doc ids for {v.shape[0]} values")
+        if np.isnan(v).any():
+            raise ValueError("sort value is NaN")
+        self.ctx, self.nbits, self.kind = ctx, int(nbits), kind
+        self._h = C.c_void_p()
+        check(lib().oc_sort_field_create(ctx._h, self.nbits, d.shape[0], _p(d), _p(v), C.byref(self._h)))
+
+    def close(self):
+        if self._h:
+            lib().oc_sort_field_destroy(self._h)
+            self._h = None
+
+
+_NOT_SORTABLE = {"string": "String", "string_filter": "StringFilter", "geopoint": "GeoPoint"}
+
+
+def resolve_sort_by(fields: Mapping[str, object], sort_by: SortBy) -> Tuple[SortField, str]:
+    """The index's field lookup of IndexSortContext::execute (read/index/sort.rs:186-265): `fields` maps every filter
+    property to its SortField, or to the kind name of a property that cannot be sorted ("string", "string_filter",
+    "geopoint").  Returns the (SortField, order) pair the sorted searches take.  Raises SortFieldNotFound(name) for an
+    unknown property and InvalidSortField(name, kind) for one that is not a number, date or bool field."""
+    if sort_by.order not in ("ASC", "DESC"):
+        raise ValueError(f"sort order {sort_by.order!r}: expected 'ASC' or 'DESC'")
+    if sort_by.property not in fields:
+        raise SortFieldNotFound(sort_by.property)
+    f = fields[sort_by.property]
+    if not isinstance(f, SortField):
+        raise InvalidSortField(sort_by.property, _NOT_SORTABLE.get(str(f), str(f)))
+    return f, sort_by.order
+
+
+def _sort(field: SortField, order: str = "ASC"):
+    if order not in ("ASC", "DESC"):
+        raise ValueError(f"sort order {order!r}: expected 'ASC' or 'DESC'")
+    return _lib.Sort(field._h, 0 if order == "ASC" else 1)
+
+
+def search_sorted_arrays(tsc: "TokenScoreContext", params: "TokenScoreParams", field: SortField, order: str = "ASC", promote=None,
+                         texts=None, q_vecs: Optional[np.ndarray] = None, apply: bool = True):
+    """oc_search_sorted: search() with sortBy (sort_token_scores with sort_by, read/sort.rs:17-46, 48-126): the first
+    limit + offset keys of the score map in field order, each with its score-map value (NaN kept), then pins and
+    skip/take.  `promote` as in search_pinned_arrays (None: no pin rule).  Returns (docs [B,limit], scores, sort values
+    [B,limit] (NaN for a promoted item), n [B], count [B], pin scores [items], pin present [items])."""
+    sp, keep, B = tsc._build_params(params, texts, q_vecs)
+    pins = None if promote is None else _pins(promote, B, apply)[0]
+    n_items = 0 if pins is None else int(pins._keep[0][-1])
+    L = params.limit_hint
+    docs, scores, sv = np.zeros((B, L), np.uint64), np.zeros((B, L), np.float32), np.zeros((B, L), np.float64)
+    n, cnt = np.zeros(B, np.uint32), np.zeros(B, np.uint64)
+    ps, pp = np.zeros(max(n_items, 1), np.float32), np.zeros(max(n_items, 1), np.uint8)
+    srt = _sort(field, order)
+    check(lib().oc_search_sorted(tsc.ctx._h, tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None, C.byref(sp),
+                                 C.byref(srt), None if pins is None else C.byref(pins), _p(docs), _p(scores), _p(sv), _p(n),
+                                 _p(cnt), _p(ps), _p(pp)))
+    return docs, scores, sv, n, cnt, ps[:n_items], pp[:n_items]
+
+
+def search_sorted(tsc: "TokenScoreContext", params: "TokenScoreParams", field: SortField, order: str = "ASC", promote=None,
+                  texts=None, q_vecs: Optional[np.ndarray] = None) -> List[SearchHits]:
+    """search_sorted_arrays as one SearchHits per query."""
+    docs, scores, _, n, cnt, _, _ = search_sorted_arrays(tsc, params, field, order, promote, texts, q_vecs)
+    return [SearchHits(docs[i, :n[i]].copy(), scores[i, :n[i]].copy(), int(cnt[i])) for i in range(docs.shape[0])]
+
+
+def merge_index_results_sorted(per_index, order: str, limit: int, offset: int = 0, promote=None, apply: bool = True):
+    """The multi-index union in field order (oc_merge_sorted, host; MergeSortedIterator, read/sort.rs:491-559):
+    per_index = one (doc_ids [B, limit'], scores, sort values, n, count[, pin scores, pin present]) tuple per index, each
+    from search_sorted_arrays with limit' = limit + offset (2 * (limit + offset) and apply=False with pins), offset' = 0,
+    vector_limit = limit.  On equal values the index listed first wins.  Returns (List[SearchHits], sort values
+    [B, limit])."""
+    k = len(per_index)
+    B, stride = per_index[0][0].shape
+    keep = [[np.ascontiguousarray(a) for a in r] for r in per_index]
+    arr = lambda j: (C.c_void_p * k)(*[r[j].ctypes.data for r in keep])  # noqa: E731
+    pins = None if promote is None else _pins(promote, B, apply)[0]
+    od, os_, ov = np.zeros((B, limit), np.uint64), np.zeros((B, limit), np.float32), np.zeros((B, limit), np.float64)
+    on, oc = np.zeros(B, np.uint32), np.zeros(B, np.uint64)
+    if order not in ("ASC", "DESC"):
+        raise ValueError(f"sort order {order!r}: expected 'ASC' or 'DESC'")
+    check(lib().oc_merge_sorted(k, B, limit, offset, stride, 0 if order == "ASC" else 1, arr(0), arr(1), arr(2), arr(3), arr(4),
+                                None if pins is None else C.byref(pins), arr(5) if pins is not None else None,
+                                arr(6) if pins is not None else None, _p(od), _p(os_), _p(ov), _p(on), _p(oc)))
+    return [SearchHits(od[i, :on[i]].copy(), os_[i, :on[i]].copy(), int(oc[i])) for i in range(B)], ov
 
 
 class TermDictionary:

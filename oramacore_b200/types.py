@@ -96,3 +96,28 @@ class PromoteItem:
     """oramacore_lib::pin_rules::PromoteItem: a pin rule's consequence places `doc_id` at `position`."""
     doc_id: int
     position: int
+
+
+@dataclass(frozen=True)
+class SortBy:
+    """SortBy (types.rs:1350-1357, 1403-1404): order the hits by a number, date or bool field; order "ASC" (the
+    default) or "DESC"."""
+    property: str
+    order: str = "ASC"
+
+
+class SortFieldNotFound(KeyError):
+    """ReadError::SortFieldNotFound: the sortBy property is not a filter field of the index."""
+
+    def __init__(self, name: str):
+        super().__init__(name)
+        self.name = name
+
+
+class InvalidSortField(ValueError):
+    """ReadError::InvalidSortField(name, kind): the sortBy property is a field that cannot be sorted by (string,
+    string_filter, geopoint); `kind` is the reference's FieldType name, e.g. "GeoPoint"."""
+
+    def __init__(self, name: str, kind: str):
+        super().__init__(name, kind)
+        self.name, self.kind = name, kind

@@ -15,6 +15,7 @@ use std::ffi::{c_char, c_int, c_void, CStr};
 #[repr(C)] pub struct OcFilter { _p: [u8; 0] }
 #[repr(C)] pub struct OcFacets { _p: [u8; 0] }
 #[repr(C)] pub struct OcGroupBy { _p: [u8; 0] }
+#[repr(C)] pub struct OcSortField { _p: [u8; 0] }
 #[repr(C)] pub struct OcDict { _p: [u8; 0] }
 #[repr(C)] pub struct OcResolved { _p: [u8; 0] }
 
@@ -66,6 +67,13 @@ pub struct OcPins {
     pub doc_ids: *const u64,        // PromoteItem.doc_id
     pub positions: *const u32,      // PromoteItem.position
     pub apply: c_int,               // 0: hits as oc_search, only the per-item score-map values
+}
+
+/// sortBy: a sort field handle and its order (OC_SORT_ASC = 0, OC_SORT_DESC = 1)
+#[repr(C)]
+pub struct OcSort {
+    pub field: *const OcSortField,
+    pub order: c_int,
 }
 
 #[repr(C)]
@@ -162,6 +170,23 @@ extern "C" {
                            counts: *const *const u64, pins: *const OcPins, pin_scores: *const *const f32,
                            pin_present: *const *const u8, out_doc_ids: *mut u64, out_scores: *mut f32,
                            out_n: *mut u32, out_count: *mut u64) -> c_int;
+    // sortBy (sort_token_scores / sort_groups with sort_by, MergeSortedIterator; sort.rs:17-201, 491-559)
+    pub fn oc_sort_field_create(ctx: *mut OcCtx, nbits: u64, n: u64, doc_ids: *const u64, values: *const f64,
+                                out: *mut *mut OcSortField) -> c_int;
+    pub fn oc_sort_field_destroy(f: *mut OcSortField);
+    pub fn oc_search_sorted(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, p: *const OcSearchParams, sort: *const OcSort,
+                            pins: *const OcPins, out_doc_ids: *mut u64, out_scores: *mut f32, out_sort_values: *mut f64,
+                            out_n: *mut u32, out_count: *mut u64, out_pin_scores: *mut f32, out_pin_present: *mut u8) -> c_int;
+    pub fn oc_search_groups_sorted(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, g: *mut OcGroupBy, p: *const OcSearchParams,
+                                   max_results: u32, sort: *const OcSort, pins: *const OcPins, group_stride: u32,
+                                   out_doc_ids: *mut u64, out_scores: *mut f32, out_sort_values: *mut f64, out_n: *mut u32,
+                                   out_count: *mut u64, out_group_doc_ids: *mut u64, out_group_scores: *mut f32,
+                                   out_group_sort_values: *mut f64, out_group_n: *mut u32) -> c_int;
+    pub fn oc_merge_sorted(n_indexes: u32, n_queries: u32, limit: u32, offset: u32, in_stride: u32, order: c_int,
+                           doc_ids: *const *const u64, scores: *const *const f32, sort_values: *const *const f64,
+                           n: *const *const u32, counts: *const *const u64, pins: *const OcPins,
+                           pin_scores: *const *const f32, pin_present: *const *const u8, out_doc_ids: *mut u64,
+                           out_scores: *mut f32, out_sort_values: *mut f64, out_n: *mut u32, out_count: *mut u64) -> c_int;
     // term dictionary + batch query resolution (tokenize_and_stem + FST expansion), host only
     pub fn oc_dict_create(n_fields: u32, out: *mut *mut OcDict) -> c_int;
     pub fn oc_dict_destroy(d: *mut OcDict);
