@@ -224,6 +224,41 @@ int oc_filter_count(const oc_filter *f, uint64_t *out);                       /*
 int oc_filter_read(const oc_filter *f, uint64_t *out_bits /* (nbits+63)/64 words */);
 void oc_filter_destroy(oc_filter *f);
 
+/* ---- geopoint where-filter leaves -----------------------------------------------------------------
+ * GeoPointFieldStorage::filter (read/index/geopoint_field.rs:179-229) for Filter::GeoPoint (read/index/filter.rs:125-139):
+ * the documents of a geopoint field with a point inside (or outside) a radius or a polygon, as an ordinary oc_filter
+ * over [0, nbits) of the field's ctx that combines with oc_filter_and / or / not and goes to any search as p->filter.
+ * Every query is one scan of the field's points on the device.
+ *   - Coordinates: degrees, latitude in [-90, 90], longitude in [-180, 180], both finite (FieldsGeoPoint::new refuses
+ *     anything else).  The reference widens its f32 API values to f64; the caller does the same before calling here.
+ *   - A field holds (document, point) entries; a document may have several points (GeoPointIndexedValue::Array).  A
+ *     document is in a leaf when AT LEAST ONE of its points satisfies the leaf's predicate, also for inside = 0, whose
+ *     predicate is "outside" (assumption).  A document with no point is in neither leaf.  Ids >= nbits are ignored.
+ * The geometry lives in the un-vendored oramacore_fields crate; this library assumes:
+ *   - radius: great-circle distance on a sphere of radius OC_GEO_EARTH_RADIUS_M; inside when d <= radius (boundary
+ *     included), outside when d > radius; radius >= pi x R puts every point inside.  Evaluated as the chord test
+ *     |u_p - u_c|^2 <= 4 sin^2(radius / 2R) on unit vectors, so points within ~1e-9 relative of the boundary may fall
+ *     on either side.  radius_m is value.to_meter(unit) computed in f32 and widened (types.rs:2159-2170).
+ *   - polygon: the even-odd ray-crossing test (PNPOLY) in planar (lon, lat) degrees over the edges (v[i-1], v[i]),
+ *     cyclic (closed implicitly; a repeated closing vertex is harmless), evaluated in f64 as
+ *     (yi > y) != (yj > y) && x < (xj - xi) * (y - yi) / (yj - yi) + xi, in that order, without FMA contraction.  Edges
+ *     are not geodesic and do not wrap at +-180.  "Outside" is the negation of the test for each point.
+ * OC_ERR_INVALID, creating nothing: invalid coordinates in the field or the query, a radius that is NaN, infinite or
+ * negative, fewer than 3 or more than OC_GEO_MAX_VERTICES vertices (the kernel stages them in shared memory). */
+#define OC_GEO_EARTH_RADIUS_M 6371000.0
+#define OC_GEO_MAX_VERTICES 2048u
+typedef struct oc_geo_field oc_geo_field;
+/* n entries (doc_ids[i], lat[i], lon[i]); n = 0 gives empty leaves.  Sorted by document id and kept on the device as
+ * 48 B per point (unit vector, lat / lon, id).  The handle is immutable: a changed field means a new handle. */
+int oc_geo_field_create(oc_ctx *ctx, uint64_t nbits, uint64_t n, const uint64_t *doc_ids, const double *lat,
+                        const double *lon, oc_geo_field **out);
+void oc_geo_field_destroy(oc_geo_field *g);
+/* GeoFilterOp::Radius / OutsideRadius: inside != 0 => points with d <= radius_m, else points with d > radius_m. */
+int oc_filter_geo_radius(const oc_geo_field *g, double lat, double lon, double radius_m, int inside, oc_filter **out);
+/* GeoFilterOp::Polygon / OutsidePolygon over the vertices (lat[k], lon[k]), k < n_vertices. */
+int oc_filter_geo_polygon(const oc_geo_field *g, const double *lat, const double *lon, uint32_t n_vertices, int inside,
+                          oc_filter **out);
+
 /* ---- facets over the score set ------------------------------------------------------------------
  * FacetContext::execute (read/index/facet.rs:147-209): for each requested variant of a filter field — bool
  * true / false (bool_field.rs:182-208), a number range [from, to], both ends inclusive (number_field.rs:368-387,

@@ -17,6 +17,8 @@ CSRC = os.path.join(_HERE, "csrc")
 OC_OK = 0
 OC_MAX_TOPK = 1024
 OC_COMM_ID_BYTES = 128
+OC_GEO_EARTH_RADIUS_M = 6371000.0
+OC_GEO_MAX_VERTICES = 2048
 
 EXPORTED_SYMBOLS = [
     "oc_last_error", "oc_version", "oc_abi_sizes", "oc_init", "oc_shutdown", "oc_device_info", "oc_comm_unique_id",
@@ -26,6 +28,7 @@ EXPORTED_SYMBOLS = [
     "oc_batcher_create", "oc_batcher_destroy", "oc_batcher_search", "oc_batcher_stats",
     "oc_filter_from_ids", "oc_filter_from_bits", "oc_filter_and", "oc_filter_or", "oc_filter_not", "oc_filter_count",
     "oc_filter_read", "oc_filter_destroy", "oc_merge_results",
+    "oc_geo_field_create", "oc_geo_field_destroy", "oc_filter_geo_radius", "oc_filter_geo_polygon",
     "oc_facets_create", "oc_facets_destroy", "oc_facets_add_field", "oc_facets_add_number_field", "oc_search_facets",
     "oc_group_by_create", "oc_group_by_destroy", "oc_search_groups",
     "oc_search_pinned", "oc_search_groups_pinned", "oc_merge_pinned",
@@ -165,6 +168,11 @@ def lib():
     L.oc_filter_read.argtypes = [vp, vp]
     L.oc_filter_destroy.argtypes = [vp]
     L.oc_filter_destroy.restype = None
+    L.oc_geo_field_create.argtypes = [vp, u64, u64, vp, vp, vp, C.POINTER(vp)]
+    L.oc_geo_field_destroy.argtypes = [vp]
+    L.oc_geo_field_destroy.restype = None
+    L.oc_filter_geo_radius.argtypes = [vp, C.c_double, C.c_double, C.c_double, i32, C.POINTER(vp)]
+    L.oc_filter_geo_polygon.argtypes = [vp, vp, vp, u32, i32, C.POINTER(vp)]
     L.oc_facets_create.argtypes = [vp, u64, C.POINTER(vp)]
     L.oc_facets_destroy.argtypes = [vp]
     L.oc_facets_destroy.restype = None

@@ -24,6 +24,7 @@
 #include "emb_gemm.cuh"
 #include "emb_scan.cuh"
 #include "fuse.cuh"
+#include "geo.cuh"
 #include "group.cuh"
 #include "pins.cuh"
 #include "sort.cuh"
@@ -3094,6 +3095,132 @@ extern "C" int oc_search_groups_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, oc_g
     GroupJob gj{groups, max_results, out_group_doc_ids, out_group_scores, out_group_n};
     gj.stride = group_stride;
     return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, &gj, &pj, pins, nullptr, nullptr, &sj);
+}
+
+// ------------------------------------------------------------------------------------ geopoint where-filter leaves (geo.cuh)
+static_assert(OC_GEO_MAX_VERTICES == GEO_MAX_VERTICES, "the header's vertex cap is the kernel's staging size");
+constexpr double GEO_PI = 3.14159265358979323846;
+
+struct oc_geo_field {
+    oc_ctx *ctx;
+    uint64_t nbits, n;
+    void *blob = nullptr;   // device: x, y, z, lat, lon (f64) then doc (u64), n entries each
+    GeoPoints pts() const {
+        const double *d = static_cast<const double *>(blob);
+        return GeoPoints{d, d + n, d + 2 * n, d + 3 * n, d + 4 * n, reinterpret_cast<const uint64_t *>(d + 5 * n), n};
+    }
+};
+
+static bool geo_valid(double lat, double lon) {
+    return std::isfinite(lat) && std::isfinite(lon) && lat >= -90.0 && lat <= 90.0 && lon >= -180.0 && lon <= 180.0;
+}
+static void geo_unit(double lat, double lon, double u[3]) {
+    const double la = lat * (GEO_PI / 180.0), lo = lon * (GEO_PI / 180.0);
+    u[0] = std::cos(la) * std::cos(lo); u[1] = std::cos(la) * std::sin(lo); u[2] = std::sin(la);
+}
+
+extern "C" int oc_geo_field_create(oc_ctx *c, uint64_t nbits, uint64_t n, const uint64_t *doc_ids, const double *lat,
+                                   const double *lon, oc_geo_field **out) {
+    if (!c || !out || (n && (!doc_ids || !lat || !lon))) return fail(OC_ERR_INVALID, "bad arguments");
+    for (uint64_t i = 0; i < n; i++)
+        if (!geo_valid(lat[i], lon[i]))
+            return fail(OC_ERR_INVALID, "geopoint %llu: invalid coordinates (%g, %g)", (unsigned long long)i, lat[i], lon[i]);
+    std::vector<uint64_t> order;
+    order.reserve(n);
+    for (uint64_t i = 0; i < n; i++) if (doc_ids[i] < nbits) order.push_back(i);
+    std::stable_sort(order.begin(), order.end(), [&](uint64_t a, uint64_t b) { return doc_ids[a] < doc_ids[b]; });
+    const uint64_t m = order.size();
+    std::vector<double> h(6 * m);
+    for (uint64_t k = 0; k < m; k++) {
+        const uint64_t i = order[k];
+        double u[3];
+        geo_unit(lat[i], lon[i], u);
+        h[k] = u[0]; h[m + k] = u[1]; h[2 * m + k] = u[2]; h[3 * m + k] = lat[i]; h[4 * m + k] = lon[i];
+        memcpy(&h[5 * m + k], &doc_ids[i], 8);
+    }
+    oc_geo_field *g = new oc_geo_field();
+    g->ctx = c; g->nbits = nbits; g->n = m;
+    std::lock_guard<std::mutex> lk(c->mu);
+    cudaError_t e = cudaSetDevice(c->device);
+    if (e == cudaSuccess && m) e = cudaMalloc(&g->blob, h.size() * 8);
+    if (e == cudaSuccess && m) e = cudaMemcpy(g->blob, h.data(), h.size() * 8, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        if (g->blob) cudaFree(g->blob);
+        delete g;
+        return fail(e == cudaErrorMemoryAllocation ? OC_ERR_OOM : OC_ERR_CUDA, "geo field upload: %s", cudaGetErrorString(e));
+    }
+    *out = g;
+    return OC_OK;
+}
+
+extern "C" void oc_geo_field_destroy(oc_geo_field *g) {
+    if (!g) return;
+    {
+        std::lock_guard<std::mutex> lk(g->ctx->mu);
+        cudaSetDevice(g->ctx->device);
+        cudaStreamSynchronize(g->ctx->stream);
+        if (g->blob) cudaFree(g->blob);
+    }
+    delete g;
+}
+
+// a zeroed leaf over [0, nbits) of g's ctx, filled by `launch` (called under the ctx lock when g has points)
+template <typename F>
+static int geo_leaf(const oc_geo_field *g, oc_filter **out, F &&launch) {
+    oc_ctx *c = g->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    CU(cudaSetDevice(c->device));
+    oc_filter *f = nullptr;
+    OCTRY(filter_alloc(c, g->nbits, &f));
+    auto fail_free = [&](int code) { cudaFree(f->bits); delete f; return code; };
+    cudaError_t e = cudaMemsetAsync(f->bits, 0, std::max<uint64_t>(f->words, 1) * 8, c->stream);
+    if (e == cudaSuccess && g->n) {
+        const int r = launch(c, reinterpret_cast<unsigned long long *>(f->bits),
+                             (unsigned)std::min<uint64_t>((g->n + GEO_THREADS - 1) / GEO_THREADS, uint64_t(c->prop.multiProcessorCount) * 8));
+        if (r != OC_OK) return fail_free(r);
+        launched(c);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e != cudaSuccess) return fail_free(fail(OC_ERR_CUDA, "geo filter: %s", cudaGetErrorString(e)));
+    *out = f;
+    return OC_OK;
+}
+
+extern "C" int oc_filter_geo_radius(const oc_geo_field *g, double lat, double lon, double radius_m, int inside, oc_filter **out) {
+    if (!g || !out) return fail(OC_ERR_INVALID, "NULL argument");
+    if (!geo_valid(lat, lon)) return fail(OC_ERR_INVALID, "radius centre: invalid coordinates (%g, %g)", lat, lon);
+    if (!(std::isfinite(radius_m) && radius_m >= 0.0)) return fail(OC_ERR_INVALID, "radius %g m: not finite and >= 0", radius_m);
+    double u[3];
+    geo_unit(lat, lon, u);
+    const double half = radius_m / (2.0 * OC_GEO_EARTH_RADIUS_M);   // half the central angle
+    const double s = std::sin(half);
+    const double thr = half >= GEO_PI / 2 ? std::numeric_limits<double>::infinity() : 4.0 * s * s;
+    return geo_leaf(g, out, [&](oc_ctx *c, unsigned long long *bits, unsigned grid) {
+        geo_radius_kernel<<<grid, GEO_THREADS, 0, c->stream>>>(g->pts(), u[0], u[1], u[2], thr, inside, bits);
+        return OC_OK;
+    });
+}
+
+extern "C" int oc_filter_geo_polygon(const oc_geo_field *g, const double *lat, const double *lon, uint32_t n_vertices,
+                                     int inside, oc_filter **out) {
+    if (!g || !out || (n_vertices && (!lat || !lon))) return fail(OC_ERR_INVALID, "NULL argument");
+    if (n_vertices < 3 || n_vertices > OC_GEO_MAX_VERTICES)
+        return fail(OC_ERR_INVALID, "polygon of %u vertices: 3 to %u are supported", n_vertices, OC_GEO_MAX_VERTICES);
+    double4 bb = make_double4(lon[0], lon[0], lat[0], lat[0]);
+    for (uint32_t k = 0; k < n_vertices; k++) {
+        if (!geo_valid(lat[k], lon[k])) return fail(OC_ERR_INVALID, "polygon vertex %u: invalid coordinates (%g, %g)", k, lat[k], lon[k]);
+        bb.x = std::min(bb.x, lon[k]); bb.y = std::max(bb.y, lon[k]); bb.z = std::min(bb.z, lat[k]); bb.w = std::max(bb.w, lat[k]);
+    }
+    bb.x -= GEO_BBOX_MARGIN; bb.y += GEO_BBOX_MARGIN;
+    return geo_leaf(g, out, [&](oc_ctx *c, unsigned long long *bits, unsigned grid) {
+        OCTRY(c->in_blob.ensure(size_t(2) * n_vertices * 8));
+        double *v = c->in_blob.as<double>();
+        CU(cudaMemcpyAsync(v, lon, size_t(n_vertices) * 8, cudaMemcpyHostToDevice, c->stream));
+        CU(cudaMemcpyAsync(v + n_vertices, lat, size_t(n_vertices) * 8, cudaMemcpyHostToDevice, c->stream));
+        geo_polygon_kernel<<<grid, GEO_THREADS, 0, c->stream>>>(g->pts(), v, v + n_vertices, n_vertices, bb, inside, bits);
+        return OC_OK;
+    });
 }
 
 // ------------------------------------------------------------------------------------ micro-batching front

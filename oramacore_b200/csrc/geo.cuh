@@ -1,0 +1,70 @@
+// geo.cuh — where-filter leaves on a geopoint field: the documents with a point inside / outside a radius or polygon.
+//
+// Replaces GeoPointFieldStorage::filter (read/index/geopoint_field.rs:179-229): a full scan of the field's points per
+// query.  A field holds its points sorted by document id, structure of arrays: the unit vector (x, y, z) of each point
+// (computed on the host), its latitude / longitude in degrees and its document id.  Each kernel runs one thread per
+// point, grid-stride, and sets the document's bit in a zeroed oc_filter bitmap when the leaf's predicate holds for that
+// point: a document is in the leaf when at least one of its points satisfies the predicate.
+//
+//   geo_radius_kernel   great-circle distance d <= r as a chord test: |u_p - u_c|^2 <= thr, thr = 4 sin^2(r / 2R) from
+//                       the host (+inf when r >= pi R).  Three subtractions and three multiply-adds per point.
+//   geo_polygon_kernel  even-odd ray crossing (PNPOLY) in planar (lon, lat) degrees against vertices staged in shared
+//                       memory, after a bounding-box pre-test.  The crossing test is evaluated with explicitly rounded
+//                       f64 operations in the order (xj - xi) * (y - yi) / (yj - yi) + xi, so no FMA contraction can
+//                       change a result.
+#pragma once
+#include <cstdint>
+
+namespace oc {
+
+constexpr uint32_t GEO_THREADS = 256;
+constexpr uint32_t GEO_MAX_VERTICES = 2048;   // OC_GEO_MAX_VERTICES: 2 x 2048 x 8 B = 32 KB of static shared memory
+// Widening of the polygon's lon bounds for the pre-test, in degrees.  A crossing abscissa over |lon| <= 180 carries an
+// error of a few ulp of 360 (~1e-13): any margin far above that and far below a meaningful distance is exact.
+constexpr double GEO_BBOX_MARGIN = 1e-9;
+
+struct GeoPoints {
+    const double *x, *y, *z;        // unit vector of each point
+    const double *lat, *lon;        // degrees
+    const uint64_t *doc;            // ascending; every id < the filter's nbits
+    uint64_t n;
+};
+
+__device__ __forceinline__ void geo_set(unsigned long long *bits, uint64_t d) {
+    atomicOr(bits + (d >> 6), 1ull << (d & 63));
+}
+
+__global__ void __launch_bounds__(GEO_THREADS) geo_radius_kernel(const GeoPoints g, double cx, double cy, double cz,
+                                                                 double thr, int inside, unsigned long long *bits) {
+    for (uint64_t i = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < g.n; i += uint64_t(gridDim.x) * blockDim.x) {
+        const double dx = g.x[i] - cx, dy = g.y[i] - cy, dz = g.z[i] - cz;
+        const bool in = dx * dx + dy * dy + dz * dz <= thr;
+        if (in == (inside != 0)) geo_set(bits, g.doc[i]);
+    }
+}
+
+// bbox = {lon_min, lon_max, lat_min, lat_max}.  A point below, above or left of the box crosses an even number of edges
+// and one right of it none, so the pre-test only skips points whose test is false.  The lon bounds are widened by the
+// host (GEO_BBOX_MARGIN) because a computed crossing abscissa may lie a few ulp outside [min(xi, xj), max(xi, xj)].
+__global__ void __launch_bounds__(GEO_THREADS) geo_polygon_kernel(const GeoPoints g, const double *vlon, const double *vlat,
+                                                                  uint32_t nv, double4 bbox, int inside,
+                                                                  unsigned long long *bits) {
+    __shared__ double sx[GEO_MAX_VERTICES], sy[GEO_MAX_VERTICES];
+    for (uint32_t k = threadIdx.x; k < nv; k += blockDim.x) { sx[k] = vlon[k]; sy[k] = vlat[k]; }
+    __syncthreads();
+    for (uint64_t i = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < g.n; i += uint64_t(gridDim.x) * blockDim.x) {
+        const double x = g.lon[i], y = g.lat[i];
+        bool in = false;
+        if (x >= bbox.x && x <= bbox.y && y >= bbox.z && y <= bbox.w) {
+            for (uint32_t k = 0, j = nv - 1; k < nv; j = k++) {
+                const double xi = sx[k], yi = sy[k], xj = sx[j], yj = sy[j];
+                if ((yi > y) != (yj > y) &&
+                    x < __dadd_rn(__ddiv_rn(__dmul_rn(__dadd_rn(xj, -xi), __dadd_rn(y, -yi)), __dadd_rn(yj, -yi)), xi))
+                    in = !in;
+            }
+        }
+        if (in == (inside != 0)) geo_set(bits, g.doc[i]);
+    }
+}
+
+}  // namespace oc

@@ -325,6 +325,83 @@ class DeviceFilter:
             self._h = None
 
 
+# GeoSearchRadiusValue::to_meter (types.rs:2159-2170): the value and the factor are f32, so is the product
+GEO_UNIT_TO_METER = {"cm": 0.01, "m": 1.0, "km": 1000.0, "ft": 0.3048, "yd": 0.9144, "mi": 1609.344}
+
+
+def geo_to_meter(value, unit: str = "m") -> float:
+    """value.to_meter(unit) in f32, widened to f64 as geo_search_filter_to_op does (geopoint_field.rs:200)."""
+    if unit not in GEO_UNIT_TO_METER:
+        raise ValueError(f"radius unit {unit!r}: expected one of {tuple(GEO_UNIT_TO_METER)}")
+    with np.errstate(over="ignore"):   # an f32 overflow is +inf, refused by the caller like any infinite radius
+        return float(np.float32(value) * np.float32(GEO_UNIT_TO_METER[unit]))
+
+
+def _geo_check(lat: float, lon: float, what: str):
+    if not (np.isfinite(lat) and np.isfinite(lon) and -90.0 <= lat <= 90.0 and -180.0 <= lon <= 180.0):
+        raise ValueError(f"{what}: invalid coordinates (lat {lat}, lon {lon})")
+
+
+def _api_coord(p) -> Tuple[float, float]:
+    """An API GeoPoint ({"lat", "lon"} or a (lat, lon) pair): f32 values widened to f64 (geopoint_field.rs:198, 216)."""
+    lat, lon = (p["lat"], p["lon"]) if isinstance(p, Mapping) else p
+    return float(np.float32(lat)), float(np.float32(lon))
+
+
+class GeoPointField:
+    """A geopoint filter field laid out for where-filter leaves on the device (oc_geo_field_*): one (doc_id, lat, lon)
+    entry per point, degrees, so a document with several points repeats.  The points are taken as f64, as
+    FilterGeoPoint2 carries them.  Ids >= nbits are ignored.  Immutable: build a new one when the field changes.
+    radius() / polygon() return a DeviceFilter over [0, nbits) that holds the documents with at least one point inside
+    (inside=True) or outside (inside=False); semantics and assumptions in include/oramacore_b200.h."""
+
+    def __init__(self, ctx: Context, nbits: int, doc_ids, lats, lons):
+        d = np.ascontiguousarray(np.asarray(doc_ids, np.uint64).reshape(-1))
+        la = np.ascontiguousarray(np.asarray(lats, np.float64).reshape(-1))
+        lo = np.ascontiguousarray(np.asarray(lons, np.float64).reshape(-1))
+        if not (d.shape == la.shape == lo.shape):
+            raise ValueError(f"{d.shape[0]} doc ids for {la.shape[0]} latitudes and {lo.shape[0]} longitudes")
+        bad = ~(np.isfinite(la) & np.isfinite(lo) & (np.abs(la) <= 90.0) & (np.abs(lo) <= 180.0))
+        if bad.any():
+            i = int(np.flatnonzero(bad)[0])
+            _geo_check(la[i], lo[i], f"geopoint {i}")
+        self.ctx, self.nbits, self.n = ctx, int(nbits), int(d.shape[0])
+        self._h = C.c_void_p()
+        check(lib().oc_geo_field_create(ctx._h, self.nbits, d.shape[0], _p(d), _p(la), _p(lo), C.byref(self._h)))
+
+    def radius(self, lat, lon, value, unit: str = "m", inside: bool = True) -> DeviceFilter:
+        """GeoSearchFilter::Radius: centre (lat, lon) as API f32 values, radius value.to_meter(unit) in f32."""
+        clat, clon = _api_coord((lat, lon))
+        _geo_check(clat, clon, "radius centre")
+        r = geo_to_meter(value, unit)
+        if not (np.isfinite(r) and r >= 0.0):
+            raise ValueError(f"radius {value} {unit}: must be finite and >= 0")
+        h = C.c_void_p()
+        check(lib().oc_filter_geo_radius(self._h, clat, clon, r, int(bool(inside)), C.byref(h)))
+        return DeviceFilter(self.ctx, h, self.nbits)
+
+    def polygon(self, coords, inside: bool = True) -> DeviceFilter:
+        """GeoSearchFilter::Polygon: `coords` = API GeoPoints ({"lat", "lon"} or (lat, lon) pairs), 3 to
+        OC_GEO_MAX_VERTICES of them."""
+        pts = [(p["lat"], p["lon"]) if isinstance(p, Mapping) else tuple(p) for p in coords]
+        if not 3 <= len(pts) <= _lib.OC_GEO_MAX_VERTICES:
+            raise ValueError(f"polygon of {len(pts)} vertices: 3 to {_lib.OC_GEO_MAX_VERTICES} are supported")
+        a = np.asarray(pts, np.float32).astype(np.float64)   # API f32 values, widened
+        la, lo = np.ascontiguousarray(a[:, 0]), np.ascontiguousarray(a[:, 1])
+        bad = ~(np.isfinite(la) & np.isfinite(lo) & (np.abs(la) <= 90.0) & (np.abs(lo) <= 180.0))
+        if bad.any():
+            k = int(np.flatnonzero(bad)[0])
+            _geo_check(la[k], lo[k], f"polygon vertex {k}")
+        h = C.c_void_p()
+        check(lib().oc_filter_geo_polygon(self._h, _p(la), _p(lo), len(pts), int(bool(inside)), C.byref(h)))
+        return DeviceFilter(self.ctx, h, self.nbits)
+
+    def close(self):
+        if self._h:
+            lib().oc_geo_field_destroy(self._h)
+            self._h = None
+
+
 class FacetStore:
     """The filter fields of one Index laid out for facet counting on the device (oc_facets_*): per field the
     variants' document lists — bool true/false (bool_field.rs:182-208), string_filter keys

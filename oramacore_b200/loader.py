@@ -5,6 +5,7 @@ The reference's read side is fed by `Index::update_data(IndexWriteOperation)` (r
       ScoreString2(field, IndexedValue{field_length: u16, terms: {term -> TermData{exact_positions, positions}}})
                                               -> StringFieldStorage::insert   (string_field.rs:155-177, mod.rs:1509-1515)
       FilterBool / FilterNumber / FilterString -> the filter fields the facets and filters read (mod.rs:1461-1497)
+      FilterGeoPoint2(field, Plain(point) | Array([points]))  -> the geopoint fields of the where-filter (mod.rs:1556-1565, 1678-1687)
   * `IndexEmbedding { data: field -> [(doc_id, vectors)] }` -> EmbeddingFieldStorage::insert (mod.rs:1688-1698)
   * `DeleteDocuments { doc_ids }` — uncommitted deletes, excluded from every search at once (mod.rs:1346-1427)
 and `commit` / `compact` lay the pending data out (`CURRENT` + `versions/<n>`, embedding_field.rs:91-95).
@@ -13,20 +14,21 @@ and `commit` / `compact` lay the pending data out (`CURRENT` + `versions/<n>`, e
 terms to stable term ids through the native dictionary (oc_dict_*), and drives the C ABI: oc_str_insert /
 oc_str_delete / oc_str_commit (snapshot swap: searches keep running on the previous version while a commit builds
 the next), oc_emb_insert / oc_emb_delete (live).  `refresh_facets()` lays the accumulated filter fields out for
-oc_search_facets.  tf of a term = number of positions (exact + stemmed), as StringStorage counts them."""
+oc_search_facets and rebuilds the geopoint field handles (`geo`, oc_geo_field_*).  tf of a term = number of positions (exact + stemmed), as StringStorage counts them."""
 from __future__ import annotations
 
 from typing import Dict, Iterable, List, Optional, Sequence
 
 import numpy as np
 
-from .engine import (Context, EmbeddingFieldStorage, FacetStore, StringFieldStorage, TermDictionary, TokenScoreContext)
+from .engine import (Context, EmbeddingFieldStorage, FacetStore, GeoPointField, StringFieldStorage, TermDictionary,
+                     TokenScoreContext)
 
 
 class IndexLoader:
     def __init__(self, ctx: Context, string_fields: Sequence[str], embedding_model: Optional[str] = None,
                  embedding_dim: Optional[int] = None, bool_fields: Sequence[str] = (), number_fields: Sequence[str] = (),
-                 string_filter_fields: Sequence[str] = ()):
+                 string_filter_fields: Sequence[str] = (), geopoint_fields: Sequence[str] = ()):
         self.ctx = ctx
         self.string_fields = list(string_fields)
         self.dict = TermDictionary(max(len(self.string_fields), 1))
@@ -35,10 +37,12 @@ class IndexLoader:
         self._bool = {f: ({}) for f in bool_fields}            # field -> {doc: bool}
         self._num = {f: ({}) for f in number_fields}           # field -> {doc: [numbers]}
         self._strf = {f: ({}) for f in string_filter_fields}   # field -> {doc: [keys]}
+        self._geo = {f: ({}) for f in geopoint_fields}         # field -> {doc: [(lat, lon)]}
         self.document_count = 0
         self.max_doc_id = -1
         self._deleted: set = set()
         self.facets: Optional[FacetStore] = None
+        self.geo: Dict[str, GeoPointField] = {}
 
     # ---- Index::update_data
     def apply(self, op: Dict) -> None:
@@ -63,6 +67,11 @@ class IndexLoader:
                     self._num[v["field"]].setdefault(d, []).append(float(v["value"]))
                 elif t == "FilterString":
                     self._strf[v["field"]].setdefault(d, []).append(str(v["value"]))
+                elif t == "FilterGeoPoint2":
+                    # GeoPointIndexedValue: {"Plain": {"lat", "lon"}} or {"Array": [{"lat", "lon"}, ...]}
+                    val = v["value"]
+                    pts = [val["Plain"]] if "Plain" in val else list(val["Array"])
+                    self._geo[v["field"]].setdefault(d, []).extend((float(p["lat"]), float(p["lon"])) for p in pts)
                 else:
                     raise ValueError(f"unsupported indexed value {t!r} (outside the search hot path)")
         elif kind == "IndexEmbedding":
@@ -78,7 +87,7 @@ class IndexLoader:
                 if d not in self._deleted:
                     self._deleted.add(d)
                     self.document_count -= 1
-                for m in list(self._bool.values()) + list(self._num.values()) + list(self._strf.values()):
+                for m in list(self._bool.values()) + list(self._num.values()) + list(self._strf.values()) + list(self._geo.values()):
                     m.pop(d, None)
         else:
             raise ValueError(f"unsupported operation {kind!r}")
@@ -89,13 +98,22 @@ class IndexLoader:
 
     def commit(self) -> None:
         """ReadSide::commit -> field compact(): publish the next snapshot of the string store (searches on the
-        previous one keep running meanwhile) and refresh the facet layout."""
+        previous one keep running meanwhile) and refresh the facet layout and the geopoint fields."""
         self.strs.commit()
         # N of the idf is Index::document_count (mod.rs:1460: +1 per Index op, also for documents without string fields)
         self.strs.set_global(max(self.document_count, 0))
         self.refresh_facets()
 
     def refresh_facets(self) -> None:
+        """Lay the filter fields out again: the facet store and one GeoPointField per geopoint field, both over
+        DocumentId [0, max_doc_id + 2).  Handles built earlier are closed."""
+        for g in self.geo.values():
+            g.close()
+        self.geo = {}
+        for f, m in self._geo.items():
+            docs = [d for d, ps in m.items() for _ in ps]
+            self.geo[f] = GeoPointField(self.ctx, self.max_doc_id + 2, docs, [p[0] for ps in m.values() for p in ps],
+                                        [p[1] for ps in m.values() for p in ps])
         if not (self._bool or self._num or self._strf):
             return
         if self.facets is not None:
@@ -123,6 +141,6 @@ class IndexLoader:
         return self.dict.resolve_batch(list(texts), **kw)
 
     def close(self):
-        for x in (self.facets, self.emb, self.strs, self.dict):
+        for x in [self.facets, self.emb, self.strs, self.dict] + list(self.geo.values()):
             if x is not None:
                 x.close()

@@ -16,6 +16,7 @@ use std::ffi::{c_char, c_int, c_void, CStr};
 #[repr(C)] pub struct OcFacets { _p: [u8; 0] }
 #[repr(C)] pub struct OcGroupBy { _p: [u8; 0] }
 #[repr(C)] pub struct OcSortField { _p: [u8; 0] }
+#[repr(C)] pub struct OcGeoField { _p: [u8; 0] }
 #[repr(C)] pub struct OcDict { _p: [u8; 0] }
 #[repr(C)] pub struct OcResolved { _p: [u8; 0] }
 
@@ -30,6 +31,9 @@ pub const OC_SHARDED: c_int = 1;
 pub const OC_SHARD_TOMBSTONES: c_int = 2;
 /// count corpus df across ranks instead of using replicated tables (a commit on a shard drops them)
 pub const OC_SHARD_COUNT_DF: c_int = 4;
+/// geopoint leaves: sphere radius of the great-circle distance (an assumption) and the polygon vertex cap
+pub const OC_GEO_EARTH_RADIUS_M: f64 = 6371000.0;
+pub const OC_GEO_MAX_VERTICES: u32 = 2048;
 
 #[repr(C)]
 pub struct OcSearchParams {
@@ -137,6 +141,14 @@ extern "C" {
     pub fn oc_filter_count(f: *const OcFilter, out: *mut u64) -> c_int;
     pub fn oc_filter_read(f: *const OcFilter, out_bits: *mut u64) -> c_int;
     pub fn oc_filter_destroy(f: *mut OcFilter);
+    // geopoint where-filter leaves (GeoPointFieldStorage::filter, geopoint_field.rs:179-229): an oc_filter over [0, nbits)
+    pub fn oc_geo_field_create(ctx: *mut OcCtx, nbits: u64, n: u64, doc_ids: *const u64, lat: *const f64, lon: *const f64,
+                               out: *mut *mut OcGeoField) -> c_int;
+    pub fn oc_geo_field_destroy(g: *mut OcGeoField);
+    pub fn oc_filter_geo_radius(g: *const OcGeoField, lat: f64, lon: f64, radius_m: f64, inside: c_int,
+                                out: *mut *mut OcFilter) -> c_int;
+    pub fn oc_filter_geo_polygon(g: *const OcGeoField, lat: *const f64, lon: *const f64, n_vertices: u32, inside: c_int,
+                                 out: *mut *mut OcFilter) -> c_int;
     // facets over the score set (facet.rs:147-209)
     pub fn oc_facets_create(ctx: *mut OcCtx, nbits: u64, out: *mut *mut OcFacets) -> c_int;
     pub fn oc_facets_destroy(f: *mut OcFacets);
