@@ -280,6 +280,30 @@ void oc_facets_destroy(oc_facets *f);
 int oc_facets_add_field(oc_facets *f, uint32_t n_variants, const uint64_t *variant_offsets /* n+1 */, const uint64_t *doc_ids,
                         uint32_t *out_field);
 int oc_facets_add_number_field(oc_facets *f, uint64_t n, const double *values_sorted, const uint64_t *doc_ids, uint32_t *out_field);
+
+/* where-filter leaves over a filter field of a facet store (read/index/filter.rs:49-124); the leaf's nbits is the store's.
+ * An ordinary oc_filter over the facets' ctx, for oc_filter_and / or / not and any search.  A document is in a leaf
+ * when AT LEAST ONE of its values passes.  The slice of the field is found by a binary search of the host copy of
+ * its values, then the device slice is scattered into a fresh bitmap: nothing is copied from the host, and an empty
+ * slice launches nothing.  Ids >= nbits are ignored.
+ *   - oc_filter_facet_variant: the documents of variant `variant` of a bool or string_filter field (bool_field.rs:163-166,
+ *     string_filter_field.rs:165-167).  Bool variants are 0 = true, 1 = false; a string_filter variant is one key.
+ *   - oc_filter_facet_range: the documents of a number field with a value v in the interval [lo, hi], compared as
+ *     f64 (IEEE: -0.0 == 0.0); OC_RANGE_LO_OPEN / OC_RANGE_HI_OPEN make that end open.  lo > hi is empty; +-inf are
+ *     allowed.  NumberFilter and DateFilter map onto it (number_field.rs:555-642, date_field.rs:271-280):
+ *     eq b = [b, b], gt b = (b, +inf], gte b = [b, +inf], lt b = [-inf, b), lte b = [-inf, b], between (a, b) = [a, b],
+ *     with the bound widened to f64 (a Number is I32 or F32; a date is its millisecond timestamp).  The reference keeps
+ *     integer and float values apart and converts F32 bounds for the integer values with ceil / floor and an EPSILON
+ *     test; for integer values |v| <= 2^53 that selects what this interval selects, except that a nonzero F32 bound
+ *     with |b| < 2^-52 counts as 0 there, so eq and lt / gt by such a bound differ from this interval at v = 0
+ *     (deliberate: the interval is the plain comparison with the given bound).
+ * OC_ERR_INVALID, creating nothing (*out untouched): NULL arguments, a field or variant out of range, a variant leaf on
+ * a number field or a range leaf on a bool / string_filter field, a NaN bound, unknown flag bits. */
+int oc_filter_facet_variant(const oc_facets *f, uint32_t field, uint32_t variant, oc_filter **out);
+#define OC_RANGE_LO_OPEN 1u
+#define OC_RANGE_HI_OPEN 2u
+int oc_filter_facet_range(const oc_facets *f, uint32_t field, double lo, double hi, uint32_t flags, oc_filter **out);
+
 /* out_counts: n_queries x n_reqs.  emb / str as for oc_search (the mode decides which are needed). */
 int oc_search_facets(oc_ctx *ctx, oc_emb *emb, oc_str *str, oc_facets *facets, const oc_search_params *p,
                      const oc_facet_req *reqs, uint32_t n_reqs, uint64_t *out_counts);

@@ -1,17 +1,18 @@
 """oramacore_b200 — H100-native (sm_90a) implementation of OramaCore's search hot path:
 embedding scan + BM25F posting scorer + hybrid fusion/top-k behind the reference's
 search() surface (mode = fulltext | vector | hybrid).  CUDA only; no CPU fallback."""
-from .types import (FieldPostings, InvalidSortField, PromoteItem, SortBy, SortFieldNotFound, StringIndexData, TextQuery, SearchHits, MODE_FULLTEXT, MODE_VECTOR,
+from .types import (FieldPostings, FilterFieldNotFound, InvalidSortField, PromoteItem, SortBy, SortFieldNotFound, StringIndexData, TextQuery, SearchHits, MODE_FULLTEXT, MODE_VECTOR,
                     MODE_HYBRID, BM25_B, BM25_K)
 from ._lib import OcError, build, lib, SO_PATH
 from .engine import (Context, DeviceFilter, FacetStore, GeoPointField, GroupBy, geo_to_meter, merge_index_results, merge_index_results_pinned, merge_index_results_sorted, resolve_sort_by,
                      search_facets, search_pinned, search_sorted, search_sorted_arrays, SortField,
                      search_pinned_arrays, search_groups, search_groups_arrays, EmbeddingFieldStorage, SearchBatcher, StringFieldStorage, TermDictionary, TextQueryBatch, TokenScoreContext, TokenScoreParams,
                      VectorSearchParams, from_bf16, pinned_empty, search, to_bf16)
+from .where import WhereFilter, evaluate_where, parse_where, where_keys
 
 __all__ = ["FieldPostings", "StringIndexData", "TextQuery", "SearchHits", "MODE_FULLTEXT", "MODE_VECTOR",
            "MODE_HYBRID", "BM25_B", "BM25_K", "OcError", "build", "lib", "SO_PATH", "Context", "DeviceFilter", "FacetStore", "GeoPointField", "GroupBy", "geo_to_meter", "merge_index_results", "merge_index_results_pinned", "PromoteItem",
-           "InvalidSortField", "SortBy", "SortFieldNotFound", "SortField", "merge_index_results_sorted", "resolve_sort_by",
+           "InvalidSortField", "FilterFieldNotFound", "WhereFilter", "evaluate_where", "parse_where", "where_keys", "SortBy", "SortFieldNotFound", "SortField", "merge_index_results_sorted", "resolve_sort_by",
            "search_sorted", "search_sorted_arrays",
            "search_facets", "search_pinned", "search_pinned_arrays", "search_groups", "search_groups_arrays",
            "EmbeddingFieldStorage", "SearchBatcher", "StringFieldStorage", "TermDictionary", "TextQueryBatch", "TokenScoreContext", "TokenScoreParams",

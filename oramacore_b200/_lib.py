@@ -19,6 +19,8 @@ OC_MAX_TOPK = 1024
 OC_COMM_ID_BYTES = 128
 OC_GEO_EARTH_RADIUS_M = 6371000.0
 OC_GEO_MAX_VERTICES = 2048
+OC_RANGE_LO_OPEN = 1
+OC_RANGE_HI_OPEN = 2
 
 EXPORTED_SYMBOLS = [
     "oc_last_error", "oc_version", "oc_abi_sizes", "oc_init", "oc_shutdown", "oc_device_info", "oc_comm_unique_id",
@@ -30,6 +32,7 @@ EXPORTED_SYMBOLS = [
     "oc_filter_read", "oc_filter_destroy", "oc_merge_results",
     "oc_geo_field_create", "oc_geo_field_destroy", "oc_filter_geo_radius", "oc_filter_geo_polygon",
     "oc_facets_create", "oc_facets_destroy", "oc_facets_add_field", "oc_facets_add_number_field", "oc_search_facets",
+    "oc_filter_facet_variant", "oc_filter_facet_range",
     "oc_group_by_create", "oc_group_by_destroy", "oc_search_groups",
     "oc_search_pinned", "oc_search_groups_pinned", "oc_merge_pinned",
     "oc_sort_field_create", "oc_sort_field_destroy", "oc_search_sorted", "oc_search_groups_sorted", "oc_merge_sorted",
@@ -178,6 +181,8 @@ def lib():
     L.oc_facets_destroy.restype = None
     L.oc_facets_add_field.argtypes = [vp, u32, vp, vp, C.POINTER(u32)]
     L.oc_facets_add_number_field.argtypes = [vp, u64, vp, vp, C.POINTER(u32)]
+    L.oc_filter_facet_variant.argtypes = [vp, u32, u32, C.POINTER(vp)]
+    L.oc_filter_facet_range.argtypes = [vp, u32, C.c_double, C.c_double, u32, C.POINTER(vp)]
     L.oc_search_facets.argtypes = [vp, vp, vp, vp, C.POINTER(SearchParams), C.POINTER(FacetReq), u32, vp]
     L.oc_group_by_create.argtypes = [vp, vp, u32, C.POINTER(vp), C.POINTER(u64)]
     L.oc_group_by_destroy.argtypes = [vp]

@@ -2602,6 +2602,65 @@ extern "C" int oc_facets_add_number_field(oc_facets *f, uint64_t n, const double
     return facets_add(f, std::move(fl), doc_ids, out_field);
 }
 
+// where-filter leaves over a filter field (read/index/filter.rs:49-124).  A leaf is one slice [lo, hi) of the field's
+// device document array, found on the host by `slice` (called under the ctx lock), scattered into a zeroed bitmap by
+// filter_scatter_ids_kernel: nothing is copied from the host and an empty slice launches nothing.
+template <typename F>
+static int facet_leaf(const oc_facets *f, uint32_t field, bool number, oc_filter **out, F &&slice) {
+    oc_ctx *c = f->ctx;
+    std::lock_guard<std::mutex> g(c->mu);
+    if (field >= f->fields.size()) return fail(OC_ERR_INVALID, "field %u: the store has %zu fields", field, f->fields.size());
+    const FacetField &fl = f->fields[field];
+    if (fl.number != number)
+        return fail(OC_ERR_INVALID, "field %u is a %s field", field, fl.number ? "number" : "bool / string_filter");
+    uint64_t lo = 0, hi = 0;
+    OCTRY(slice(fl, lo, hi));
+    CU(cudaSetDevice(c->device));
+    oc_filter *r = nullptr;
+    OCTRY(filter_alloc(c, f->nbits, &r));
+    cudaError_t e = cudaMemsetAsync(r->bits, 0, std::max<uint64_t>(r->words, 1) * 8, c->stream);
+    if (e == cudaSuccess && hi > lo) {
+        filter_scatter_ids_kernel<<<(unsigned)((hi - lo + 255) / 256), 256, 0, c->stream>>>(
+            fl.docs + lo, hi - lo, f->nbits, reinterpret_cast<unsigned long long *>(r->bits));
+        launched(c);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e != cudaSuccess) {
+        cudaFree(r->bits);
+        delete r;
+        return fail(OC_ERR_CUDA, "facet filter: %s", cudaGetErrorString(e));
+    }
+    *out = r;
+    return OC_OK;
+}
+
+extern "C" int oc_filter_facet_variant(const oc_facets *f, uint32_t field, uint32_t variant, oc_filter **out) {
+    if (!f || !out) return fail(OC_ERR_INVALID, "NULL argument");
+    return facet_leaf(f, field, false, out, [&](const FacetField &fl, uint64_t &lo, uint64_t &hi) {
+        if (variant + uint64_t(1) >= fl.offsets.size())
+            return fail(OC_ERR_INVALID, "variant %u: field %u has %zu variants", variant, field, fl.offsets.size() - 1);
+        lo = fl.offsets[variant];
+        hi = fl.offsets[variant + 1];
+        return int(OC_OK);
+    });
+}
+
+extern "C" int oc_filter_facet_range(const oc_facets *f, uint32_t field, double lo, double hi, uint32_t flags, oc_filter **out) {
+    if (!f || !out) return fail(OC_ERR_INVALID, "NULL argument");
+    if (std::isnan(lo) || std::isnan(hi)) return fail(OC_ERR_INVALID, "NaN range bound");
+    if (flags & ~(OC_RANGE_LO_OPEN | OC_RANGE_HI_OPEN)) return fail(OC_ERR_INVALID, "unknown range flags 0x%x", flags);
+    return facet_leaf(f, field, true, out, [&](const FacetField &fl, uint64_t &a, uint64_t &b) {
+        const auto &v = fl.values;   // ascending, no NaN
+        a = (flags & OC_RANGE_LO_OPEN) ? std::upper_bound(v.begin(), v.end(), lo) - v.begin()
+                                       : std::lower_bound(v.begin(), v.end(), lo) - v.begin();
+        b = (flags & OC_RANGE_HI_OPEN) ? std::lower_bound(v.begin(), v.end(), hi) - v.begin()
+                                       : std::upper_bound(v.begin(), v.end(), hi) - v.begin();
+        b = std::max(a, b);   // lo > hi: empty
+        return int(OC_OK);
+    });
+}
+
 // row bitmap -> DocumentId bitmap when rows are not document ids
 __global__ void facet_rows_to_docs_kernel(const uint32_t *row_bits, uint64_t row_stride_words, const uint64_t *row_doc, uint64_t n_rows,
                                           uint32_t *doc_bits, uint64_t doc_stride_words, uint64_t nbits) {

@@ -405,13 +405,49 @@ class GeoPointField:
 class FacetStore:
     """The filter fields of one Index laid out for facet counting on the device (oc_facets_*): per field the
     variants' document lists — bool true/false (bool_field.rs:182-208), string_filter keys
-    (string_filter_field.rs:175-193), number fields sorted by value so a range is a slice (number_field.rs:368-387)."""
+    (string_filter_field.rs:175-193), number and date fields sorted by value so a range is a slice
+    (number_field.rs:368-387).  `leaf()` turns a where-filter leaf on one of these fields into a DeviceFilter."""
 
     def __init__(self, ctx: Context, nbits: int):
         self.ctx, self.nbits = ctx, int(nbits)
         self._h = C.c_void_p()
         check(lib().oc_facets_create(ctx._h, self.nbits, C.byref(self._h)))
         self.fields: Dict[str, dict] = {}
+
+    def add_date_field(self, name: str, doc_ids, ms):
+        """A date field: one millisecond timestamp per (document, value), kept as a number field of kind "date".  The
+        doubles are exact: chrono's whole range is below 2^53 ms.  Dates have no facets and no groups
+        (group.rs:234-236)."""
+        fid = self.add_number_field(name, doc_ids, np.asarray(ms, np.int64).astype(np.float64))
+        self.fields[name]["kind"] = "date"
+        return fid
+
+    def leaf(self, name: str, flt) -> DeviceFilter:
+        """The documents of field `name` matched by the parsed where-filter leaf `flt` (where.Filter), as
+        calculate_filter_for_fields does (filter.rs:49-124): a bool or string_filter value is one variant (an unknown
+        key gives an empty leaf), a NumberFilter / DateFilter one value interval, compared in f64.  A filter of the
+        wrong kind for the field gives an empty leaf."""
+        from .where import DateFilter, NumberFilter
+        f = self.fields[name]
+        h = C.c_void_p()
+        kind = f["kind"]
+        if (kind == "bool" and isinstance(flt, bool)) or (kind == "string" and isinstance(flt, str)):
+            key = ("true" if flt else "false") if kind == "bool" else flt
+            if key not in f["variant"]:
+                return DeviceFilter.from_ids(self.ctx, [], self.nbits)
+            check(lib().oc_filter_facet_variant(self._h, f["id"], f["variant"][key], C.byref(h)))
+        elif (kind == "number" and isinstance(flt, NumberFilter)) or (kind == "date" and isinstance(flt, DateFilter)):
+            # eq / gt / gte / lt / lte / between (number_field.rs:555-642, date_field.rs:271-280) as [lo, hi] + open ends
+            b = flt.bounds()
+            if flt.op == "between":
+                lo, hi, flags = b[0], b[1], 0
+            else:
+                lo, hi, flags = {"eq": (b, b, 0), "gt": (b, np.inf, _lib.OC_RANGE_LO_OPEN), "gte": (b, np.inf, 0),
+                                 "lt": (-np.inf, b, _lib.OC_RANGE_HI_OPEN), "lte": (-np.inf, b, 0)}[flt.op]
+            check(lib().oc_filter_facet_range(self._h, f["id"], float(lo), float(hi), flags, C.byref(h)))
+        else:
+            return DeviceFilter.from_ids(self.ctx, [], self.nbits)
+        return DeviceFilter(self.ctx, h, self.nbits)
 
     def add_bool_field(self, name: str, true_docs, false_docs):
         return self._add_variants(name, "bool", {"true": true_docs, "false": false_docs})
@@ -427,7 +463,7 @@ class FacetStore:
         docs = np.ascontiguousarray(np.concatenate(lists) if lists else np.zeros(0, np.uint64))
         fid = C.c_uint32()
         check(lib().oc_facets_add_field(self._h, len(keys), _p(offs), _p(docs), C.byref(fid)))
-        self.fields[name] = {"id": fid.value, "kind": kind, "keys": keys}
+        self.fields[name] = {"id": fid.value, "kind": kind, "keys": keys, "variant": {k: i for i, k in enumerate(keys)}}
         return fid.value
 
     def add_number_field(self, name: str, doc_ids, values):
@@ -459,6 +495,8 @@ def search_facets(tsc: "TokenScoreContext", store: FacetStore, params: "TokenSco
     reqs, labels = [], []
     for name, d in facets.items():
         f = store.fields[name]
+        if f["kind"] == "date":
+            raise ValueError(f"{name!r} is a date field: dates have no facets")
         if f["kind"] == "number":
             for r in d["ranges"]:
                 reqs.append((f["id"], 0, float(r["from"]), float(r["to"])))
@@ -494,6 +532,9 @@ class GroupBy:
     def __init__(self, store: FacetStore, properties: Sequence[str]):
         self.ctx, self.properties = store.ctx, list(properties)
         fs = [store.fields[p] for p in self.properties]
+        for p, f in zip(self.properties, fs):
+            if f["kind"] == "date":
+                raise ValueError(f"{p!r} is a date field: groups on dates are refused (group.rs:234-236)")
         ids = np.asarray([f["id"] for f in fs], np.uint32)
         self._h, n = C.c_void_p(), C.c_uint64()
         check(lib().oc_group_by_create(store._h, _p(ids), ids.shape[0], C.byref(self._h), C.byref(n)))

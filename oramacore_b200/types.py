@@ -114,6 +114,14 @@ class SortFieldNotFound(KeyError):
         self.name = name
 
 
+class FilterFieldNotFound(KeyError):
+    """ReadError::FilterFieldNotFound: a key of the where-filter is not a filter field of any index (search.rs:435-449)."""
+
+    def __init__(self, name: str):
+        super().__init__(name)
+        self.name = name
+
+
 class InvalidSortField(ValueError):
     """ReadError::InvalidSortField(name, kind): the sortBy property is a field that cannot be sorted by (string,
     string_filter, geopoint); `kind` is the reference's FieldType name, e.g. "GeoPoint"."""

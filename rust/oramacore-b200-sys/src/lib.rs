@@ -34,6 +34,9 @@ pub const OC_SHARD_COUNT_DF: c_int = 4;
 /// geopoint leaves: sphere radius of the great-circle distance (an assumption) and the polygon vertex cap
 pub const OC_GEO_EARTH_RADIUS_M: f64 = 6371000.0;
 pub const OC_GEO_MAX_VERTICES: u32 = 2048;
+/// oc_filter_facet_range: open ends of the interval (closed when the flag is clear)
+pub const OC_RANGE_LO_OPEN: u32 = 1;
+pub const OC_RANGE_HI_OPEN: u32 = 2;
 
 #[repr(C)]
 pub struct OcSearchParams {
@@ -154,6 +157,9 @@ extern "C" {
     pub fn oc_facets_destroy(f: *mut OcFacets);
     pub fn oc_facets_add_field(f: *mut OcFacets, n_variants: u32, variant_offsets: *const u64, doc_ids: *const u64, out_field: *mut u32) -> c_int;
     pub fn oc_facets_add_number_field(f: *mut OcFacets, n: u64, values_sorted: *const f64, doc_ids: *const u64, out_field: *mut u32) -> c_int;
+    // where-filter leaves over a filter field (filter.rs:49-124): a variant's documents, or a number field's value interval
+    pub fn oc_filter_facet_variant(f: *const OcFacets, field: u32, variant: u32, out: *mut *mut OcFilter) -> c_int;
+    pub fn oc_filter_facet_range(f: *const OcFacets, field: u32, lo: f64, hi: f64, flags: u32, out: *mut *mut OcFilter) -> c_int;
     pub fn oc_search_facets(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, f: *mut OcFacets, p: *const OcSearchParams,
                             reqs: *const OcFacetReq, n_reqs: u32, out_counts: *mut u64) -> c_int;
     // groups over the score map (group.rs + sort_groups, sort.rs:129-230)
