@@ -200,10 +200,24 @@ typedef struct {
                                           union, oc_merge_results) asks for limit' = limit+offset, vector_limit = limit */
     const struct oc_filter *filter;    /* NULL, or a device-resident DocumentId bitmap (oc_filter_*): takes precedence
                                           over filter_bits and is not re-uploaded per call                           */
+    const struct oc_filter *const *q_filters;  /* NULL, or B entries: query b is filtered by q_filters[b] (NULL = none) */
 } oc_search_params;
 
 /* out_doc_ids/out_scores: B x limit (best first, after offset); out_n[b] hits written;
- * out_count[b] = all matching documents. emb may be NULL for fulltext, str NULL for vector. */
+ * out_count[b] = all matching documents. emb may be NULL for fulltext, str NULL for vector.
+ *
+ * Per-query where-filters (q_filters): every request of the reference carries its own where-filter
+ * (SearchParams.where_filter), evaluated per request and passed into that request's scoring.  With q_filters set,
+ * query b is scored exactly as if it were alone in an oc_search with p->filter = q_filters[b]: the vector stage,
+ * the fulltext stage with the corpus df counted under that query's filter (token_score.rs:262-275), hybrid fusion,
+ * OMC, count and offset / limit.  The result is byte-identical: same ids, same score bits, same count.
+ *   - Entries may repeat; the library deduplicates by handle and builds one row bitmap per distinct handle over each
+ *     store's rows (K distinct handles: K x rows / 8 bytes per store).  Each entry has its own nbits (ids >= nbits
+ *     do not pass).  All entries NULL: an unfiltered search; every entry the same handle: the p->filter path.
+ *   - OC_ERR_INVALID: q_filters together with filter or filter_bits, a handle of another ctx.
+ *     OC_ERR_UNSUPPORTED: sharded.  A refused call creates nothing and writes no output.
+ *   - oc_search_groups*, oc_search_pinned and oc_search_sorted refuse q_filters with OC_ERR_UNSUPPORTED;
+ *     oc_search_facets ignores it as it ignores filter (facets are scored without the where-filter). */
 int oc_search(oc_ctx *ctx, oc_emb *emb, oc_str *str, const oc_search_params *p,
               uint64_t *out_doc_ids, float *out_scores, uint32_t *out_n, uint64_t *out_count);
 
@@ -526,8 +540,11 @@ void oc_resolved_free(oc_resolved *r);
  * concurrent single-query oc_search calls: the first submitter of a group leads it, waits up to
  * max_wait_us (or until max_batch queries are in), runs ONE oc_search for the group and scatters
  * the per-query results to the blocked callers.  Coalesced: queries with the same (mode, limit,
- * offset, similarity, threshold, bm25_k, bm25_b), no filter, no OMC, not sharded; any other call
- * is passed straight to oc_search.  p->n_queries must be 1; outputs as for oc_search with B = 1. */
+ * offset, similarity, threshold, bm25_k, bm25_b, vector_limit), no host bitmap (filter_bits), no q_filters, no OMC,
+ * not sharded; a device filter (p->filter) is carried into the batch as that query's q_filters entry, so filtered
+ * and unfiltered requests share a batch.  Any other call is passed straight to oc_search, and a p->filter of
+ * another ctx is refused with OC_ERR_INVALID before it can join a batch.  p->n_queries must be 1; outputs as for
+ * oc_search with B = 1. */
 typedef struct oc_batcher oc_batcher;
 int oc_batcher_create(oc_ctx *ctx, oc_emb *emb, oc_str *str, uint32_t max_batch, uint32_t max_wait_us, oc_batcher **out);
 void oc_batcher_destroy(oc_batcher *b);

@@ -65,7 +65,8 @@ class SearchParams(C.Structure):
                 ("term_field", C.c_void_p), ("term_id", C.c_void_p), ("term_weight", C.c_void_p),
                 ("filter_bits", C.c_void_p), ("filter_nbits", C.c_uint64),
                 ("omc_doc_ids", C.c_void_p), ("omc_mult", C.c_void_p), ("n_omc", C.c_uint64),
-                ("sharded", C.c_int), ("vector_limit", C.c_uint32), ("filter", C.c_void_p)]
+                ("sharded", C.c_int), ("vector_limit", C.c_uint32), ("filter", C.c_void_p),
+                ("q_filters", C.c_void_p)]
 
 
 class FacetReq(C.Structure):

@@ -7,7 +7,9 @@
 // descriptors into ONE oc_search_params, runs it through `Exec` (oc_search in the library, a fake
 // in tests/batcher_test.cpp) and scatters the per-query results back to the waiting callers.
 // Only queries that can share a batch are coalesced: same (mode, limit, offset, similarity,
-// threshold, bm25_k, bm25_b), no filter, no OMC, not sharded; anything else runs directly.
+// threshold, bm25_k, bm25_b, vector_limit), no host bitmap (filter_bits), no q_filters, no OMC, not
+// sharded; anything else runs directly.  A device filter (p->filter) is per query: the merged batch
+// carries it as that query's q_filters entry, so filtered and unfiltered requests share a batch.
 #pragma once
 #include <atomic>
 #include <chrono>
@@ -34,7 +36,7 @@ inline BatchKey key_of(const oc_search_params *p) {
 // (unknown mode, missing store, NULL query arrays) is NOT batchable: it goes straight to the
 // executor so the caller gets oc_search's normal error instead of a merge that dereferences NULL.
 inline bool batchable(const oc_search_params *p, bool has_emb = true, bool has_str = true) {
-    if (p->n_queries != 1 || p->filter_bits || p->filter || p->n_omc != 0 || p->sharded) return false;
+    if (p->n_queries != 1 || p->filter_bits || p->q_filters || p->n_omc != 0 || p->sharded) return false;
     if (p->mode != OC_MODE_FULLTEXT && p->mode != OC_MODE_VECTOR && p->mode != OC_MODE_HYBRID) return false;
     const bool need_v = p->mode != OC_MODE_FULLTEXT, need_ft = p->mode != OC_MODE_VECTOR;
     if (need_v && (!has_emb || !p->q_vecs)) return false;
@@ -63,6 +65,7 @@ struct MergedBatch {
     std::vector<uint64_t> docs, count;
     std::vector<float> scores;
     std::vector<uint32_t> n;
+    std::vector<const oc_filter *> q_filters;   // [B] each query's p->filter, or empty when no query has one
 
     void build(const std::vector<BatchReq *> &reqs, uint32_t dim) {
         const oc_search_params *f = reqs[0]->p;
@@ -100,6 +103,15 @@ struct MergedBatch {
             p.term_id = term_id.empty() ? &zero_u : term_id.data();
             p.term_weight = term_weight.empty() ? &one_f : term_weight.data();
         }
+        q_filters.clear();
+        p.filter = nullptr; p.q_filters = nullptr;
+        for (uint32_t i = 0; i < B; i++)
+            if (reqs[i]->p->filter) {
+                q_filters.resize(B, nullptr);
+                for (uint32_t j = 0; j < B; j++) q_filters[j] = reqs[j]->p->filter;
+                p.q_filters = q_filters.data();
+                break;
+            }
         docs.assign(size_t(B) * f->limit, 0); scores.assign(size_t(B) * f->limit, 0.f);
         n.assign(B, 0); count.assign(B, 0);
     }

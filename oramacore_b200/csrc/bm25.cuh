@@ -169,7 +169,15 @@ struct Bm25Params {
     // raw fulltext score of every matched row, written where its matched bit is set — slots of unmatched rows are
     // never written and must be read through the bitmap.  Last member so the other fields keep their offsets.
     float *row_ft;
+    // per-query where-filters (oc_search_params.q_filters): NULL, or [n_queries] slot of each query in row_ok_bits, which
+    // then holds one bitmap of ok_words words per slot.  Only K3 and K3b read it (such a batch never runs K3c / K3d).
+    const uint32_t *q_ok_slot;
+    uint64_t ok_words;
 };
+// the row bitmap of query q (or of token t in the df pre-pass): the shared one, or its slot's
+__device__ __forceinline__ const uint32_t *row_ok_of(const uint32_t *bits, const uint32_t *slot, uint64_t words, uint32_t q) {
+    return (bits && slot) ? bits + size_t(slot[q]) * words : bits;
+}
 __host__ __device__ __forceinline__ void bm25_item_decode(const Bm25Params &p, const uint32_t k, uint32_t &tile, uint32_t &q) {
     if (!p.perm) { tile = k / p.n_queries; q = k % p.n_queries; return; }
     uint32_t g = 0;
@@ -230,6 +238,8 @@ struct DfParams {
     const uint32_t *seg;
     const uint32_t *row_ok_bits;
     unsigned int *df;  // [n_tokens]
+    const uint32_t *tok_ok_slot;   // NULL, or [n_tokens] slot of each token's query (per-query where-filters)
+    uint64_t ok_words;
 };
 __global__ void __launch_bounds__(BM25_THREADS) bm25_df_kernel(const DfParams p) {
     __shared__ uint8_t flag[BM25_TILE];
@@ -238,9 +248,10 @@ __global__ void __launch_bounds__(BM25_THREADS) bm25_df_kernel(const DfParams p)
     const uint32_t tile = blockIdx.x % p.n_tiles, tok = blockIdx.x / p.n_tiles;
     const uint32_t row0 = tile * BM25_TILE;
     const TokenDesc tk = p.tokens[tok];
+    const uint32_t *okq = row_ok_of(p.row_ok_bits, p.tok_ok_slot, p.ok_words, tok);
     for (uint32_t i = threadIdx.x; i < BM25_TILE / 4; i += blockDim.x) reinterpret_cast<uint32_t *>(flag)[i] = 0;
     for (uint32_t i = threadIdx.x; i < BM25_TILE / 32; i += blockDim.x)
-        okb[i] = p.row_ok_bits ? p.row_ok_bits[row0 / 32 + i] : 0xffffffffu;
+        okb[i] = okq ? okq[row0 / 32 + i] : 0xffffffffu;
     if (threadIdx.x == 0) s_sum = 0;
     __syncthreads();
     for (uint32_t e = tk.term_begin; e < tk.term_end; e++) {
@@ -327,8 +338,10 @@ __global__ void __launch_bounds__(BM25_THREADS) bm25_tile_kernel(const Bm25Param
         if (MULTI) reinterpret_cast<float4 *>(aux)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (THRESH) reinterpret_cast<uint4 *>(mask)[i] = make_uint4(0u, 0u, 0u, 0u);
     }
-    if (use_ok)
-        for (uint32_t i = tid; i < BM25_TILE / 32; i += BM25_THREADS) okb[i] = p.row_ok_bits[row0 / 32 + i];
+    if (use_ok) {
+        const uint32_t *okq = row_ok_of(p.row_ok_bits, p.q_ok_slot, p.ok_words, q);
+        for (uint32_t i = tid; i < BM25_TILE / 32; i += BM25_THREADS) okb[i] = okq[row0 / 32 + i];
+    }
     if (tid == 0) { s_cnt = 0; s_matched = 0; s_maxo = f32_ordered(0.f); s_mino = f32_ordered(0.f); s_tau = p.tau[q]; }
     if (p.matched_bits && tid < BM25_TILE / 32) s_mbits[tid] = 0u;
     __syncthreads();
@@ -748,8 +761,10 @@ __global__ void __launch_bounds__(BM25_THREADS, 1024 / BM25_THREADS) bm25_tile2_
             }
             if (tid == 0) s_ntok = ntok;
         }
-        if (use_ok)
-            for (uint32_t i = tid; i < BM25_TILE / 32; i += BM25_THREADS) okb[i] = p.row_ok_bits[row0 / 32 + i];
+        if (use_ok) {
+            const uint32_t *okq = row_ok_of(p.row_ok_bits, p.q_ok_slot, p.ok_words, q);
+            for (uint32_t i = tid; i < BM25_TILE / 32; i += BM25_THREADS) okb[i] = okq[row0 / 32 + i];
+        }
         if (!flat || use_ok) __syncthreads();
         const uint32_t ntok = s_ntok;
         // in flight during this item: the next item's descriptors and this query's running threshold
@@ -1543,6 +1558,8 @@ struct PointParams {
     float k;
     int threshold;
     float *v_ft; uint8_t *v_present;
+    const uint32_t *q_ok_slot;    // NULL, or [n_queries] slot of each query in row_ok_bits (per-query where-filters)
+    uint64_t ok_words;
 };
 __device__ __forceinline__ bool posting_find(const TermDesc &td, uint32_t row, uint32_t *payload) {
     const uint2 *pp = reinterpret_cast<const uint2 *>(td.ptr);
@@ -1561,7 +1578,7 @@ __global__ void __launch_bounds__(256) bm25_point_kernel(const PointParams p) {
     float score = 0.f;
     uint32_t mask = 0;
     bool ok = r != 0xffffffffu;
-    if (ok && p.row_ok_bits) ok = (p.row_ok_bits[r >> 5] >> (r & 31)) & 1u;
+    if (ok && p.row_ok_bits) ok = (row_ok_of(p.row_ok_bits, p.q_ok_slot, p.ok_words, q)[r >> 5] >> (r & 31)) & 1u;
     if (ok) {
         for (uint32_t t0 = qd.token_begin; t0 < qd.token_end; t0 += 32) {
             const uint32_t ti = t0 + lane;

@@ -162,6 +162,11 @@ struct oc_ctx {
     DevBuf pin_row, pin_ft, pin_ftp, pin_score, pin_present, pin_top_doc, pin_top_score, pin_top_n, pin_gdoc, pin_gscore, pin_gn;   // pins
     DevBuf srt_doc, srt_row, srt_n, srt_ft, srt_ftp, srt_score, srt_present, srt_zero;   // sortBy
     DevBuf q_bf16, q_rho, pre_post, dense_buf, g_thr, g_eps, g_ovf, g_ovfcnt, g_resc, g_cand, g_cnt, g_flag, g_max, r_qpad, r_qinv, r_map, r_doc, r_score, r_row, r_cnt, r_raw;
+    // per-query where-filters (q_filters): the embedding rows' bitmap of every distinct handle, and the slots of the
+    // queries the exact sweep re-runs; v_qslot / v_rowbits describe the vector stage of the current call (fix_unproven)
+    DevBuf e_rowbits, r_slot;
+    const uint32_t *v_rowbits = nullptr; uint64_t v_row_words = 0;
+    std::vector<uint32_t> v_qslot;
 
     HostBuf h_in, h_out, h_in0;   // h_in0 / in_blob0: query vectors + filter, uploaded before the descriptors
     OcComm comm;
@@ -219,7 +224,8 @@ extern "C" void oc_shutdown(oc_ctx *c) {
                       &c->row_ft, &c->grp_vdoc, &c->grp_vscore, &c->grp_vn, &c->grp_gmin, &c->grp_den, &c->grp_doc, &c->grp_score, &c->grp_n,
                       &c->pin_row, &c->pin_ft, &c->pin_ftp, &c->pin_score, &c->pin_present, &c->pin_top_doc, &c->pin_top_score,
                       &c->pin_top_n, &c->pin_gdoc, &c->pin_gscore, &c->pin_gn,
-                      &c->srt_doc, &c->srt_row, &c->srt_n, &c->srt_ft, &c->srt_ftp, &c->srt_score, &c->srt_present, &c->srt_zero};
+                      &c->srt_doc, &c->srt_row, &c->srt_n, &c->srt_ft, &c->srt_ftp, &c->srt_score, &c->srt_present, &c->srt_zero,
+                      &c->e_rowbits, &c->r_slot};
     for (DevBuf *b : bufs) b->release();
     c->h_in.release(); c->h_out.release();
     for (int i = 0; i < EV_N; i++) if (c->ev[i]) cudaEventDestroy(c->ev[i]);
@@ -478,8 +484,10 @@ static ScanPlan plan_scan(const oc_ctx *c, const oc_emb *e, uint32_t n_keep) {
 
 // ---- exact sweeps (K1) + merge for nq prepared queries; results into the given buffers
 struct VecOut { uint64_t *doc; float *score; uint32_t *row; uint32_t *cnt; float *raw; };
+// row_bits / q_slot: per-query where-filters (ScanParams), or NULL
 static int run_exact_sweeps(oc_ctx *c, oc_emb *e, const float *inv_norm, const float *qpad, const float *qinv,
-                            uint32_t nq, uint32_t limit, float similarity, const VecOut &o) {
+                            uint32_t nq, uint32_t limit, float similarity, const VecOut &o,
+                            const uint32_t *row_bits = nullptr, uint64_t row_words = 0, const uint32_t *q_slot = nullptr) {
     ScanPlan pl = plan_scan(c, e, limit);
     if (pl.n_stages < 2) return fail(OC_ERR_UNSUPPORTED, "limit %u leaves no shared memory for the scan ring", limit);
     OCTRY(c->scan_cand.ensure(size_t(nq) * pl.grid * limit * 8));
@@ -494,6 +502,7 @@ static int run_exact_sweeps(oc_ctx *c, oc_emb *e, const float *inv_norm, const f
         sp.n_keep = limit; sp.wcap = pl.wcap; sp.rows_per_stage = pl.rows_per_stage; sp.n_stages = pl.n_stages;
         sp.n_ctas_total = pl.grid;
         sp.cand = c->scan_cand.as<uint64_t>() + size_t(q0) * pl.grid * limit;
+        if (row_bits) { sp.row_bits = row_bits; sp.row_words = row_words; sp.q_slot = q_slot + q0; }
         const size_t smem = scan_smem_bytes(e->stride, pl.rows_per_stage, pl.n_stages, pl.wcap, qb, e->esz);
         if (qb == 4) OCTRY((launch_scan_d<4>(c, sp, pl.grid, smem, e->esz)));
         else if (qb == 2) OCTRY((launch_scan_d<2>(c, sp, pl.grid, smem, e->esz)));
@@ -524,10 +533,21 @@ static int tmap_2d(CUtensorMap *m, const void *base, uint64_t n_rows, uint32_t s
 
 static bool g_disable_gemm = false;   // OC_DISABLE_GEMM=1: force the exact sweep path (A/B testing)
 
+// Per-query where-filters of one search (oc_search_params.q_filters), deduplicated by handle.
+struct QFilterJob {
+    std::vector<RowsOkSlot> slots;     // the K distinct handles, then {NULL, 0}: the fulltext slot of unfiltered queries
+    std::vector<uint32_t> q_slot;      // [B] vector stage: index into slots, SLOT_NONE = unfiltered
+    std::vector<uint32_t> q_slot_ft;   // [B] fulltext stage: index into slots, K = unfiltered (tombstones only)
+    const RowsOkSlot *d_slots = nullptr;
+    const uint32_t *d_q_slot = nullptr, *d_q_slot_ft = nullptr;
+    uint32_t k() const { return (uint32_t)slots.size() - 1; }
+};
+
 // Runs prep + (tensor-core batched scan | exact sweeps) + merge for B queries already in device
 // memory (q_dev: B x dim).  Leaves hits in c->v_doc / v_score / v_row / v_cnt / v_raw ([B][limit]).
+// qf: per-query where-filters (device tables uploaded), or NULL.
 static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B, uint32_t limit, float similarity,
-                            const uint64_t *filter_dev, uint64_t filter_nbits) {
+                            const uint64_t *filter_dev, uint64_t filter_nbits, const QFilterJob *qf = nullptr) {
     OCTRY(c->v_doc.ensure(size_t(B) * limit * 8));
     OCTRY(c->v_score.ensure(size_t(B) * limit * 4));
     OCTRY(c->v_row.ensure(size_t(B) * limit * 4));
@@ -563,9 +583,23 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
         launched(c);
         inv_norm = c->eff_norm.as<float>();
     }
+    const uint32_t *row_bits = nullptr;
+    uint64_t row_words = 0;
+    if (qf) {   // one bitmap over the store's rows per distinct filter (whole 128-row tiles: K2 reads 4 words per tile)
+        row_words = (e->n_rows + GEMM_N - 1) / GEMM_N * (GEMM_N / 32);
+        OCTRY(c->e_rowbits.ensure(size_t(qf->k()) * row_words * 4));
+        rows_ok_kernel<<<dim3((unsigned)((row_words + 255) / 256), qf->k()), 256, 0, c->stream>>>(
+            e->row_doc, e->n_rows, nullptr, nullptr, 0, c->e_rowbits.as<uint32_t>(), row_words, qf->d_slots);
+        launched(c);
+        CU(cudaGetLastError());
+        row_bits = c->e_rowbits.as<uint32_t>();
+        c->v_rowbits = row_bits; c->v_row_words = row_words; c->v_qslot = qf->q_slot;
+    }
     VecOut out{c->v_doc.as<uint64_t>(), c->v_score.as<float>(), c->v_row.as<uint32_t>(), c->v_cnt.as<uint32_t>(), c->v_raw.as<float>()};
     CU(cudaEventRecord(c->ev[EV_SCAN0], c->stream));
-    if (!use_gemm) return run_exact_sweeps(c, e, inv_norm, c->q_pad.as<float>(), c->q_inv.as<float>(), B, limit, similarity, out);
+    if (!use_gemm)
+        return run_exact_sweeps(c, e, inv_norm, c->q_pad.as<float>(), c->q_inv.as<float>(), B, limit, similarity, out, row_bits,
+                                row_words, qf ? qf->d_q_slot : nullptr);
 
     // ---------------- K2: wgmma batched scan ----------------
     const bool bf16 = e->esz == 2;
@@ -601,6 +635,7 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
     gp.thr = c->g_thr.as<unsigned int>(); gp.eps_v = c->g_eps.as<float>(); gp.limit = limit; gp.cand = c->g_cand.as<uint64_t>(); gp.cand_cnt = c->g_cnt.as<uint32_t>();
     gp.gmax = c->g_max.as<float>();
     gp.ovf = c->g_ovf.as<uint64_t>(); gp.ovf_cnt = c->g_ovfcnt.as<uint32_t>(); gp.ovf_cap = GEMM_OVF_CAP;
+    if (qf) { gp.row_bits = row_bits; gp.row_words = row_words; gp.q_slot = qf->d_q_slot; }
     if (smem_cfg_needed(c->device, (const void *)emb_gemm_kernel<false>, gemm_smem_bytes())) {   // all sweep kernels at once
         CU(cudaFuncSetAttribute(emb_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes()));
         CU(cudaFuncSetAttribute(emb_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes()));
@@ -674,8 +709,15 @@ static int fix_unproven(oc_ctx *c, oc_emb *e, const uint8_t *flags, uint32_t B, 
         CU(cudaMemcpyAsync(c->r_qinv.as<float>() + i, c->q_inv.as<float>() + redo[i], 4, cudaMemcpyDeviceToDevice, c->stream));
     }
     CU(cudaMemcpyAsync(c->r_map.p, redo.data(), size_t(nr) * 4, cudaMemcpyHostToDevice, c->stream));
+    std::vector<uint32_t> rslot;   // per-query where-filters: each redone query keeps its own slot
+    if (c->v_rowbits) {
+        for (uint32_t q : redo) rslot.push_back(c->v_qslot[q]);
+        OCTRY(c->r_slot.ensure(size_t(nr) * 4));
+        CU(cudaMemcpyAsync(c->r_slot.p, rslot.data(), size_t(nr) * 4, cudaMemcpyHostToDevice, c->stream));
+    }
     VecOut ro{c->r_doc.as<uint64_t>(), c->r_score.as<float>(), c->r_row.as<uint32_t>(), c->r_cnt.as<uint32_t>(), c->r_raw.as<float>()};
-    OCTRY(run_exact_sweeps(c, e, inv_norm, c->r_qpad.as<float>(), c->r_qinv.as<float>(), nr, limit, similarity, ro));
+    OCTRY(run_exact_sweeps(c, e, inv_norm, c->r_qpad.as<float>(), c->r_qinv.as<float>(), nr, limit, similarity, ro, c->v_rowbits,
+                           c->v_row_words, c->v_rowbits ? c->r_slot.as<uint32_t>() : nullptr));
     scatter_rows_kernel<<<nr, 64, 0, c->stream>>>(c->r_map.as<uint32_t>(), nr, limit, ro.doc, ro.score, ro.row, ro.cnt, ro.raw,
                                                    out.doc, out.score, out.row, out.cnt, out.raw);
     launched(c);
@@ -686,6 +728,7 @@ static int fix_unproven(oc_ctx *c, oc_emb *e, const uint8_t *flags, uint32_t B, 
 
 static void begin_call(oc_ctx *c) {
     c->call_launches = 0; c->call_scan_launches = 0; c->gemm_pending = false; c->sweep_timed = false; c->rerun_timed = false;
+    c->v_rowbits = nullptr; c->v_row_words = 0;
     memset(&c->timing, 0, sizeof(c->timing));
 }
 static int finish_timing(oc_ctx *c, bool scan, bool bm, bool fuse, bool comm) {
@@ -1769,6 +1812,37 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     if (has_ft && (!str || !p->q_token_offsets)) return fail(OC_ERR_INVALID, "fulltext/hybrid mode needs str and tokens");
     if (emb && emb->ctx != c) return fail(OC_ERR_INVALID, "emb belongs to another ctx");
     if (str && str->ctx != c) return fail(OC_ERR_INVALID, "str belongs to another ctx");
+    // per-query where-filters: deduplicated by handle; all NULL = unfiltered, one handle for every query = p->filter
+    const oc_filter *batch_filter = p->filter;
+    QFilterJob qfj;
+    bool per_q = false;
+    if (p->q_filters) {
+        if (gj || pj || sj) return fail(OC_ERR_UNSUPPORTED, "q_filters: per-query filters are supported by oc_search only");
+        if (p->filter || p->filter_bits) return fail(OC_ERR_INVALID, "q_filters together with filter / filter_bits");
+        if (p->sharded) return fail(OC_ERR_UNSUPPORTED, "q_filters over a sharded search");
+        std::unordered_map<const oc_filter *, uint32_t> idx;
+        std::vector<const oc_filter *> distinct;
+        bool any_none = false;
+        qfj.q_slot.resize(B);
+        for (uint32_t b = 0; b < B; b++) {
+            const oc_filter *f = p->q_filters[b];
+            if (!f) { any_none = true; qfj.q_slot[b] = SLOT_NONE; continue; }
+            if (f->ctx != c) return fail(OC_ERR_INVALID, "q_filters[%u] belongs to another ctx", b);
+            auto it = idx.emplace(f, (uint32_t)distinct.size()).first;
+            if (it->second == distinct.size()) distinct.push_back(f);
+            qfj.q_slot[b] = it->second;
+        }
+        if (distinct.size() > 65535) return fail(OC_ERR_UNSUPPORTED, "q_filters: %zu distinct handles > 65535", distinct.size());
+        if (distinct.size() == 1 && !any_none) batch_filter = distinct[0];
+        else if (!distinct.empty()) {
+            per_q = true;
+            const uint32_t K = (uint32_t)distinct.size();
+            for (const oc_filter *f : distinct) qfj.slots.push_back(RowsOkSlot{f->bits, f->nbits});
+            qfj.slots.push_back(RowsOkSlot{nullptr, 0});
+            qfj.q_slot_ft.resize(B);
+            for (uint32_t b = 0; b < B; b++) qfj.q_slot_ft[b] = qfj.q_slot[b] == SLOT_NONE ? K : qfj.q_slot[b];
+        }
+    }
     if (p->limit == 0 && !gj) return fail(OC_ERR_INVALID, "limit must be >= 1");
     const uint32_t limit = write_hits ? p->limit : 1;
     // sort_token_scores with pins selects the top 2 * (limit + offset) (sort.rs:25-34); the vector depth stays limit
@@ -1813,25 +1887,39 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     };
     // ------------------------------------------------------------ vector stage first: the query vectors
     // (+ filter) go up alone and the matrix sweep starts; the host-side descriptor work below overlaps it
-    if (p->filter && p->filter->ctx != c) return fail(OC_ERR_INVALID, "filter belongs to another ctx");
-    const bool filter_h = !p->filter && p->filter_bits != nullptr;        // host bitmap: uploaded with this call
-    const bool filter = filter_h || p->filter != nullptr;
-    const uint64_t filter_nbits = p->filter ? p->filter->nbits : p->filter_nbits;
+    if (batch_filter && batch_filter->ctx != c) return fail(OC_ERR_INVALID, "filter belongs to another ctx");
+    const bool filter_h = !batch_filter && p->filter_bits != nullptr;     // host bitmap: uploaded with this call
+    const bool filter = filter_h || batch_filter != nullptr;
+    const uint64_t filter_nbits = batch_filter ? batch_filter->nbits : p->filter_nbits;
     const size_t fwords = filter_h ? (p->filter_nbits + 63) / 64 : 0;
-    const uint64_t *filter_dev = p->filter ? p->filter->bits : nullptr;
+    const uint64_t *filter_dev = batch_filter ? batch_filter->bits : nullptr;
+    // per-query filters: the slot tables travel with the first upload of the call
+    auto add_qf = [&](Packer &pk, size_t o[3]) {
+        o[0] = pk.add(qfj.slots.data(), qfj.slots.size() * sizeof(RowsOkSlot));
+        o[1] = pk.add(qfj.q_slot.data(), size_t(B) * 4);
+        o[2] = pk.add(qfj.q_slot_ft.data(), size_t(B) * 4);
+    };
+    auto bind_qf = [&](uint8_t *base, const size_t o[3]) {
+        qfj.d_slots = reinterpret_cast<const RowsOkSlot *>(base + o[0]);
+        qfj.d_q_slot = reinterpret_cast<const uint32_t *>(base + o[1]);
+        qfj.d_q_slot_ft = reinterpret_cast<const uint32_t *>(base + o[2]);
+    };
     size_t h2d_early = 0;
     if (has_v) {
         Packer pk0;
         const size_t o_qv = pk0.add(p->q_vecs, size_t(B) * emb->dim * 4, is_pinned_host(p->q_vecs));
         const size_t o_flt = filter_h ? pk0.add(p->filter_bits, fwords * 8) : 0;
+        size_t o_qf[3] = {0, 0, 0};
+        if (per_q) add_qf(pk0, o_qf);
         CU(cudaEventRecord(c->ev[EV_START], c->stream));
         OCTRY(upload(pk0, c->h_in0, c->in_blob0, c->stream));
         CU(cudaEventRecord(c->ev[EV_H2D], c->stream));
         h2d_early = pk0.total;
         if (filter_h) filter_dev = reinterpret_cast<const uint64_t *>(c->in_blob0.as<uint8_t>() + o_flt);
+        if (per_q) bind_qf(c->in_blob0.as<uint8_t>(), o_qf);
         if (vlimit) {
             OCTRY(run_vector_stage(c, emb, reinterpret_cast<const float *>(c->in_blob0.as<uint8_t>() + o_qv), B, vlimit, p->similarity,
-                                   filter_dev, filter_nbits));
+                                   filter_dev, filter_nbits, per_q ? &qfj : nullptr));
         } else {   // limit_hint 0 (groups only): no vector hit
             OCTRY(c->v_cnt.ensure(size_t(B) * 4));
             CU(cudaMemsetAsync(c->v_cnt.p, 0, size_t(B) * 4, c->stream));
@@ -1853,6 +1941,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     std::vector<TokenDesc> tokens;
     std::vector<QueryDesc> queries;
     std::vector<uint8_t> tok_need_df;
+    std::vector<uint32_t> tok_slot;     // per-query filters: the fulltext slot of each token's query
     std::vector<PreDesc> pre_descs;
     std::vector<uint2> pre_items;
     bool any_multi = false, need_df = false, derived_now = false;
@@ -1875,8 +1964,15 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
             }
         const float N = (float)S->document_count;  // token_score.rs:221
         queries.resize(B);
+        // Per-query filters are routed as a filtered batch is: df is counted on the device (need_df), so nothing is shared
+        // or dense and K3b / K3 score the batch, each (tile, query) item under its query's row bitmap.  A token keeps the
+        // idf its query would get alone: counted under the query's filter, or — single term, no filter, no tombstones —
+        // from the host's posting-list length (or corpus df table), as a plain oc_search does.  An unfiltered query runs
+        // under the tombstone-only row bitmap (slot K), so it scores exactly the rows it would score alone.
+        if (per_q) need_df = true;
         for (uint32_t q = 0; q < B; q++) {
             const uint32_t t0 = p->q_token_offsets[q], t1 = p->q_token_offsets[q + 1];
+            const bool q_filter = filter || (per_q && qfj.q_slot[q] != SLOT_NONE);
             QueryDesc qd{};
             qd.token_begin = (uint32_t)tokens.size();
             const uint32_t ntok = t1 - t0;
@@ -1908,12 +2004,13 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
                 tk.term_end = (uint32_t)terms.size();
                 const uint32_t nt = tk.term_end - tk.term_begin;
                 uint8_t need = 0;
-                if (nt == 1 && !filter && !tombs && !count_df) tk.idf = host_idf(N, std::max<uint64_t>(1, df_known));
+                if (nt == 1 && !q_filter && !tombs && !count_df) tk.idf = host_idf(N, std::max<uint64_t>(1, df_known));
                 else if (nt == 0) tk.idf = host_idf(N, 1);
                 else { need = 1; need_df = true; tk.idf = 0.f; }
                 if (nt != 1) { any_multi = any_multi || nt > 1; }
                 tokens.push_back(tk);
                 tok_need_df.push_back(need);
+                if (per_q) tok_slot.push_back(qfj.q_slot_ft[q]);
             }
             qd.token_end = (uint32_t)tokens.size();
             queries[q] = qd;
@@ -1921,8 +2018,9 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         if (df_local_only && !count_df)
             return fail(OC_ERR_INVALID, "sharded search: a field of this shard has no corpus-wide df table (dropped by a commit?): "
                                         "reload it or pass OC_SHARD_COUNT_DF on every rank");
-        // ---- batch-level sharing of per-posting contributions (single-term tokens with a host-known idf)
-        {
+        // ---- batch-level sharing of per-posting contributions (single-term tokens with a host-known idf); not with
+        // per-query filters: the precomputed contributions and dense arrays are masked by ONE row bitmap
+        if (!per_q) {
             struct U { uint32_t first_e; uint32_t uses; };
             struct K128 { uint64_t a, b; };            // (field, term) | (weight bits, idf bits)
             size_t cap_t = 64;
@@ -2033,6 +2131,9 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     const size_t o_omcm = n_omc ? pk.add(p->omc_mult, size_t(n_omc) * 4) : 0;
     const size_t o_omcr = omc_tile ? pk.add(omc_rows.data(), omc_rows.size() * 4) : 0;
     const size_t o_omcrm = omc_tile ? pk.add(omc_row_mult.data(), omc_row_mult.size() * 4) : 0;
+    size_t o_qf[3] = {0, 0, 0};
+    if (per_q && !has_v) add_qf(pk, o_qf);
+    const size_t o_tslot = (per_q && !tok_slot.empty()) ? pk.add(tok_slot.data(), tok_slot.size() * 4) : 0;
     // item order of the register-folded scorers (Bm25Params::perm): queries by their number of dense tokens, descending
     std::vector<uint32_t> q_perm;
     uint32_t cls_nq[BM25_CLASSES] = {0, 0, 0, 0, 0};
@@ -2075,6 +2176,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     c->timing.h2d_bytes = h2d_early + pk.total;
     uint8_t *din = c->in_blob.as<uint8_t>();
     if (filter_h && !has_v) filter_dev = reinterpret_cast<const uint64_t *>(din + o_flt);
+    if (per_q && !has_v) bind_qf(din, o_qf);
     if (pin_items) {
         pj->d_doc = reinterpret_cast<const uint64_t *>(din + o_pdoc);
         pj->d_pos = reinterpret_cast<const uint32_t *>(din + o_ppos);
@@ -2107,7 +2209,15 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         cudaStream_t ps = side ? c->side : c->stream;
         CU(cudaEventRecord(c->ev[EV_BM0], ps));
         const uint64_t ok_words = uint64_t(n_tiles) * (BM25_TILE / 32);
-        if (filter || tombs) {
+        if (per_q) {   // one row bitmap per distinct filter (tombstones AND filter), then the tombstone-only slot K
+            OCTRY(c->row_ok.ensure(std::max<uint64_t>(ok_words, 1) * qfj.slots.size() * 4));
+            if (ok_words) {
+                rows_ok_kernel<<<dim3((unsigned)((ok_words + 255) / 256), (unsigned)qfj.slots.size()), 256, 0, ps>>>(
+                    S->row_doc, S->n_rows, tombs ? S->alive : nullptr, nullptr, 0, c->row_ok.as<uint32_t>(), ok_words, qfj.d_slots);
+                launched(c);
+            }
+            row_ok = c->row_ok.as<uint32_t>();
+        } else if (filter || tombs) {
             OCTRY(c->row_ok.ensure(ok_words * 4));
             rows_ok_kernel<<<(unsigned)((ok_words + 255) / 256), 256, 0, ps>>>(
                 S->row_doc, S->n_rows, tombs ? S->alive : nullptr, filter_dev, filter_nbits,
@@ -2140,7 +2250,8 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
             dp.tokens = reinterpret_cast<const TokenDesc *>(din + o_tokens);
             dp.n_tokens = (uint32_t)ntok; dp.n_tiles = n_tiles; dp.seg = c->seg.as<uint32_t>();
             dp.row_ok_bits = row_ok; dp.df = c->df_dev.as<unsigned int>();
-            if (n_tiles) {
+            if (per_q) { dp.tok_ok_slot = reinterpret_cast<const uint32_t *>(din + o_tslot); dp.ok_words = ok_words; }
+            if (n_tiles && ntok) {
                 bm25_df_kernel<<<(unsigned)(uint64_t(n_tiles) * ntok), BM25_THREADS, 0, c->stream>>>(dp);
                 launched(c);
             }
@@ -2175,6 +2286,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         bp.n_queries = B; bp.n_tiles = n_tiles; bp.n_rows = S->n_rows;
         bp.k = p->bm25_k; bp.b = p->bm25_b;
         bp.row_ok_bits = row_ok;
+        if (per_q) { bp.q_ok_slot = qfj.d_q_slot_ft; bp.ok_words = ok_words; }
         bp.omc_row = omc_tile ? reinterpret_cast<const uint32_t *>(din + o_omcr) : nullptr;
         bp.omc_mult = omc_tile ? reinterpret_cast<const float *>(din + o_omcrm) : nullptr;
         bp.n_omc = (uint32_t)omc_rows.size();
@@ -2344,6 +2456,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         PointParams pp{};
         pp.terms = bp.terms; pp.tokens = bp.tokens; pp.queries = bp.queries;
         pp.n_queries = B; pp.v_stride = vlimit; pp.v_row = c->v_srow.as<uint32_t>(); pp.row_ok_bits = row_ok;
+        pp.q_ok_slot = per_q ? qfj.d_q_slot_ft : nullptr; pp.ok_words = uint64_t(n_tiles) * (BM25_TILE / 32);
         pp.k = p->bm25_k; pp.threshold = thr ? 1 : 0;
         pp.v_ft = c->v_ft.as<float>(); pp.v_present = c->v_present.as<uint8_t>();
         bm25_point_kernel<<<(B * vlimit * 32 + 255) / 256, 256, 0, c->stream>>>(pp);
@@ -2794,7 +2907,7 @@ extern "C" int oc_search_facets(oc_ctx *c, oc_emb *emb, oc_str *str, oc_facets *
     // the reference computes facets on the score map re-scored WITHOUT the where-filter (search.rs:361-396: only the
     // uncommitted deletes stay excluded), so that the counts do not collapse onto the selected category
     oc_search_params q = *p;
-    q.filter_bits = nullptr; q.filter_nbits = 0; q.filter = nullptr;
+    q.filter_bits = nullptr; q.filter_nbits = 0; q.filter = nullptr; q.q_filters = nullptr;
     const uint32_t B = p->n_queries;
     std::vector<uint64_t> docs(size_t(B) * p->limit), cnt(B);
     std::vector<float> scores(size_t(B) * p->limit);
@@ -3291,7 +3404,8 @@ struct OcSearchExec {
 };
 struct oc_batcher {
     ocb::Batcher<OcSearchExec> q;
-    oc_batcher(OcSearchExec x, uint32_t dim, uint32_t mb, uint32_t mw) : q(x, dim, mb, mw, x.e != nullptr, x.s != nullptr) {}
+    oc_ctx *ctx;
+    oc_batcher(OcSearchExec x, uint32_t dim, uint32_t mb, uint32_t mw) : q(x, dim, mb, mw, x.e != nullptr, x.s != nullptr), ctx(x.c) {}
 };
 extern "C" int oc_batcher_create(oc_ctx *c, oc_emb *emb, oc_str *str, uint32_t max_batch, uint32_t max_wait_us, oc_batcher **out) {
     if (!c || !out || (!emb && !str)) return fail(OC_ERR_INVALID, "bad arguments");
@@ -3305,6 +3419,8 @@ extern "C" int oc_batcher_search(oc_batcher *b, const oc_search_params *p, uint6
                                  uint32_t *out_n, uint64_t *out_count) {
     if (!b || !p || !out_doc_ids || !out_scores || !out_n || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
     if (p->n_queries != 1) return fail(OC_ERR_INVALID, "oc_batcher_search takes one query per call (n_queries = %u)", p->n_queries);
+    // a device filter joins a batch as that query's q_filters entry: one of another ctx would fail the whole batch
+    if (p->filter && p->filter->ctx != b->ctx) return fail(OC_ERR_INVALID, "filter belongs to another ctx");
     g_err[0] = 0;
     const int rc = b->q.submit(p, out_doc_ids, out_scores, out_n, out_count);
     // the batch ran on its leader's thread: that is where oc_last_error() holds the detail

@@ -84,7 +84,24 @@ struct GemmParams {
     uint64_t *ovf;             // [n_queries][ovf_cap] spill area: a full private list is appended here
     uint32_t *ovf_cnt;         // [n_queries] (may exceed ovf_cap: the merge then sends the query to the exact sweep)
     uint32_t ovf_cap;
+    // per-query where-filters (as ScanParams): NULL, or [n_slots][row_words] row bitmaps, row_words a multiple of 4
+    // covering every tile; query q keeps row r when q_slot[q] == SLOT_NONE or bit r of its slot is set
+    const uint32_t *row_bits;
+    uint64_t row_words;
+    const uint32_t *q_slot;    // [n_queries]
 };
+// The 32 rows a thread holds of a 128-row tile (rows row0 + 2 (lane & 3) + 8 (j >> 1) + (j & 1), j < 32) as bit j of a
+// mask, from the tile's 4 words of a row bitmap: word w gives bits 8w .. 8w + 7 (its bits 8m + 2 (lane & 3) + {0, 1}).
+__device__ __forceinline__ uint32_t gemm_tile_row_mask(const uint32_t *bits, uint32_t lane) {
+    const uint4 w = __ldg(reinterpret_cast<const uint4 *>(bits));
+    const uint32_t s = 2 * (lane & 3);
+    auto pick = [s](uint32_t x) {
+        x = (x >> s) & 0x03030303u;
+        x = (x | (x >> 6)) & 0x000f000fu;
+        return (x | (x >> 12)) & 0xffu;
+    };
+    return pick(w.x) | (pick(w.y) << 8) | (pick(w.z) << 16) | (pick(w.w) << 24);
+}
 // emb_gemm_kernel<BF16, DUMP = true> (test harness only): the epilogue writes every approximate score v of a live
 // (query, row) pair to dump[q * n_rows + row] instead of gathering candidates
 struct GemmDumpParams : GemmParams {
@@ -287,10 +304,12 @@ emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     uint32_t q[2];
     bool live[2];
     GemmEpi e[2];
+    uint32_t slot[2];
 #pragma unroll
     for (uint32_t h = 0; h < 2; h++) {
         q[h] = grp * GEMM_M + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
         live[h] = q[h] < p.n_queries;
+        slot[h] = (!DUMP && p.row_bits && live[h]) ? p.q_slot[q[h]] : SLOT_NONE;
         e[h].thr = live[h] ? -INFINITY : INFINITY;     // refreshed from the query's global threshold before every tile
         e[h].best = -INFINITY;                         // max_mode: best approximate score seen by this list
     }
@@ -354,13 +373,21 @@ emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
                 continue;
             }
             if (p.max_mode) {
+                // a row the query's own filter rejects must not raise its bound (it is NaN in a single-filter sweep)
+                const uint32_t ok = slot[h] == SLOT_NONE ? 0xffffffffu
+                                                         : gemm_tile_row_mask(p.row_bits + size_t(slot[h]) * p.row_words + row0 / 32, lane);
 #pragma unroll
-                for (uint32_t j = 0; j < 32; j++) E.best = fmaxf(E.best, v[j]);   // NaN (dead rows) ignored
+                for (uint32_t j = 0; j < 32; j++)
+                    if ((ok >> j) & 1u) E.best = fmaxf(E.best, v[j]);   // NaN (dead rows) ignored
                 continue;
             }
             uint32_t mask = 0;
 #pragma unroll
             for (uint32_t j = 0; j < 32; j++) mask |= (v[j] > E.thr ? 1u : 0u) << j;   // NaN fails
+            // per-query filter: only rows that already clear the threshold look at the bitmap (the common path of the
+            // sweep loads nothing more)
+            if (mask && slot[h] != SLOT_NONE)
+                mask &= gemm_tile_row_mask(p.row_bits + size_t(slot[h]) * p.row_words + row0 / 32, lane);
             if (mask) {   // rare once the threshold has tightened
                 uint64_t *mybuf = p.cand + (size_t(q[h]) * lists + my_list) * p.cap;
                 const uint32_t rb = uint32_t(row0) + 2 * (lane & 3);

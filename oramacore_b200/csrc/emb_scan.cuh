@@ -37,7 +37,16 @@ struct ScanParams {
     uint32_t n_stages;
     uint32_t n_ctas_total;    // candidate slots per query (>= gridDim.x)
     uint64_t *cand;           // [nq][n_ctas_total][n_keep] keys, KEY_NONE padded
+    // per-query where-filters (oc_search_params.q_filters): NULL, or [n_slots][row_words] row bitmaps; query q passes
+    // row r when q_slot[q] == SLOT_NONE or bit r of slot q_slot[q] is set
+    const uint32_t *row_bits;
+    uint64_t row_words;
+    const uint32_t *q_slot;   // [nq]
 };
+constexpr uint32_t SLOT_NONE = 0xffffffffu;
+__device__ __forceinline__ bool slot_row_ok(const uint32_t *row_bits, uint64_t row_words, uint32_t slot, uint64_t row) {
+    return slot == SLOT_NONE || ((__ldg(row_bits + size_t(slot) * row_words + (row >> 5)) >> (row & 31)) & 1u);
+}
 
 __host__ __device__ inline size_t scan_smem_bytes(uint32_t stride, uint32_t rows_per_stage,
                                                   uint32_t n_stages, uint32_t wcap, uint32_t qb, uint32_t esz = 4) {
@@ -174,7 +183,9 @@ __global__ void __launch_bounds__(SCAN_THREADS, 1) emb_scan_kernel(const ScanPar
 #pragma unroll
             for (int q = 0; q < QB; q++) {
                 const float kf = cos_rank_key(warp_sum(acc[q]), inr, iqn[q]);
-                if (kf > tau[q]) {  // warp-uniform
+                // warp-uniform; a row the query's own filter rejects is skipped here, where a NaN inverse norm would
+                // skip it in a single-filter sweep (slot and bit are only read for rows that clear the threshold)
+                if (kf > tau[q] && (!p.row_bits || slot_row_ok(p.row_bits, p.row_words, __ldg(p.q_slot + q), row0 + r))) {
                     if (cnt[q] == p.wcap) {
                         warp_bitonic_desc(mybuf[q], p.wcap, lane);
                         cnt[q] = p.n_keep;

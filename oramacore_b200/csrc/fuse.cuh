@@ -289,12 +289,21 @@ __global__ void map_docs_to_rows_kernel(const uint64_t *docs, const uint32_t *co
     out_rows[gid] = r;
 }
 
-// DocumentId bitmap -> row bitmap (alive AND filter); one thread per 32 rows.
+// One DocumentId bitmap of a per-query-filtered batch (oc_search_params.q_filters): bits == NULL => alive only.
+struct RowsOkSlot { const uint64_t *bits; uint64_t nbits; };
+
+// DocumentId bitmap -> row bitmap (alive AND filter); one thread per 32 rows.  slots != NULL: one bitmap per slot
+// blockIdx.y (filter = slots[y], output words [y * n_words, (y + 1) * n_words)), filter_bits is then unused.
 __global__ void rows_ok_kernel(const uint64_t *row_doc_ids, uint64_t n_rows, const uint32_t *alive_bits,
                                const uint64_t *filter_bits, uint64_t filter_nbits, uint32_t *out_bits,
-                               uint64_t n_words) {
+                               uint64_t n_words, const RowsOkSlot *slots = nullptr) {
     const uint64_t w = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x;
     if (w >= n_words) return;
+    if (slots) {
+        const RowsOkSlot s = slots[blockIdx.y];
+        filter_bits = s.bits; filter_nbits = s.nbits;
+        out_bits += uint64_t(blockIdx.y) * n_words;
+    }
     uint32_t bits = 0;
     for (uint32_t b = 0; b < 32; b++) {
         const uint64_t r = w * 32 + b;

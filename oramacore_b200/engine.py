@@ -928,6 +928,9 @@ class TokenScoreParams:
     filtered_doc_ids: Optional[np.ndarray] = None
     filter_nbits: int = 0
     device_filter: Optional["DeviceFilter"] = None   # device-resident bitmap (oc_filter_*); wins over filtered_doc_ids
+    # one entry per query (None = unfiltered): query b is scored as if alone with device_filter = device_filters[b]
+    # (oc_search_params.q_filters); not together with device_filter / filtered_doc_ids
+    device_filters: Optional[Sequence[Optional["DeviceFilter"]]] = None
     vector_limit: int = 0            # 0 => limit_hint (search.rs:330-336); see oc_search_params.vector_limit
     omc_doc_ids: Optional[np.ndarray] = None   # ascending
     omc_mult: Optional[np.ndarray] = None
@@ -987,6 +990,13 @@ class TokenScoreContext:
             sp.q_token_offsets, sp.token_term_offsets = _p(texts.q_token_offsets), _p(texts.token_term_offsets)
             sp.term_field, sp.term_id, sp.term_weight = _p(texts.term_field), _p(texts.term_id), _p(texts.term_weight)
         sp.vector_limit = int(params.vector_limit)
+        if params.device_filters is not None:
+            fl = list(params.device_filters)
+            if len(fl) != B:
+                raise ValueError(f"device_filters has {len(fl)} entries for {B} queries")
+            arr = (C.c_void_p * B)(*[None if f is None else f._h.value for f in fl])
+            keep += [arr, fl]   # the handles stay alive for the call
+            sp.q_filters = C.cast(arr, C.c_void_p)
         if params.device_filter is not None:
             keep.append(params.device_filter)
             sp.filter = params.device_filter._h
@@ -1018,7 +1028,10 @@ class SearchBatcher:
     """Micro-batching front (oc_batcher_*, csrc/batcher.h): many threads call search() with ONE query
     each — the way the reference's request tasks call TokenScoreContext::execute — and the library
     coalesces concurrent calls that share (mode, limit, offset, similarity, threshold) into one
-    batched oc_search.  ctypes releases the GIL while a caller is blocked in the library."""
+    batched oc_search.  A request's device_filter (its where-filter) travels with it into the batch as
+    that query's own filter, so filtered and unfiltered requests are coalesced together; requests with
+    filtered_doc_ids (a host bitmap), OMC multipliers or sharding run as their own oc_search.  ctypes
+    releases the GIL while a caller is blocked in the library."""
 
     def __init__(self, tsc: TokenScoreContext, max_batch: int = 256, max_wait_us: int = 200):
         self.tsc = tsc

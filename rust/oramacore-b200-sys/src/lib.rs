@@ -62,6 +62,7 @@ pub struct OcSearchParams {
     pub sharded: c_int,
     pub vector_limit: u32,          // 0 => limit (limit_hint of the vector stage, search.rs:330-336)
     pub filter: *const OcFilter,    // device-resident FilterResult bitmap; wins over filter_bits
+    pub q_filters: *const *const OcFilter,  // NULL, or B entries: query b's own filter (NULL = none); oc_search only
 }
 
 #[repr(C)]
