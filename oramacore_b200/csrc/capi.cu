@@ -567,8 +567,10 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
     const char *env = getenv("OC_DISABLE_GEMM");
     g_disable_gemm = env && env[0] == '1';
     // tensor-core scan: a batch (the distance is a true GEMM), a store large enough that the threshold pass sees
-    // at least `limit` row groups of <= 256 rows with data (its seeds are the limit-th largest group maximum; with
-    // fewer live groups the threshold degenerates to "gather everything" and the query falls back to the exact sweep)
+    // at least `limit` row groups with data (its seeds are the limit-th largest group maximum; with fewer live groups
+    // the threshold degenerates to "gather everything" and the query falls back to the exact sweep).  A group is the
+    // 64 rows one list sees of its CTA's first 256-row tile: n_rows >= 256 limit leaves >= limit full tiles, i.e.
+    // 4 min(ctas_per_group, limit) >= limit live groups whenever ctas_per_group >= limit / 4
     const bool use_gemm = !g_disable_gemm && B >= 8 && limit <= GEMM_MAX_LIMIT && e->n_rows >= std::max<uint64_t>(4096, uint64_t(limit) * 256);
     // (the prep kernel writes rows [0, B) whole, zero padded: only the rows of a partial last query group need clearing)
     if (use_gemm && Bpad != B) CU(cudaMemsetAsync(c->q_pad.as<float>() + size_t(B) * e->stride, 0, size_t(Bpad - B) * e->stride * 4, c->stream));
@@ -585,7 +587,7 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
     }
     const uint32_t *row_bits = nullptr;
     uint64_t row_words = 0;
-    if (qf) {   // one bitmap over the store's rows per distinct filter (whole 128-row tiles: K2 reads 4 words per tile)
+    if (qf) {   // one bitmap over the store's rows per distinct filter (whole 256-row tiles: K2 reads 8 words per tile)
         row_words = (e->n_rows + GEMM_N - 1) / GEMM_N * (GEMM_N / 32);
         OCTRY(c->e_rowbits.ensure(size_t(qf->k()) * row_words * 4));
         rows_ok_kernel<<<dim3((unsigned)((row_words + 255) / 256), qf->k()), 256, 0, c->stream>>>(
@@ -603,10 +605,44 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
 
     // ---------------- K2: wgmma batched scan ----------------
     const bool bf16 = e->esz == 2;
-    // one CTA per SM and query group; the merge gathers at most 512 lists per query
-    const uint32_t cpg = std::min<uint32_t>(512 / GEMM_LISTS_PER_CTA,
-                                            std::max<uint32_t>(1, c->prop.multiProcessorCount / n_qgroups));
+    const void *sweep_fn = bf16 ? (const void *)emb_gemm_kernel<true> : (const void *)emb_gemm_kernel<false>;
+    if (smem_cfg_needed(c->device, (const void *)emb_gemm_kernel<false>, gemm_smem_bytes())) {   // all sweep kernels at once
+        CU(cudaFuncSetAttribute(emb_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes()));
+        CU(cudaFuncSetAttribute(emb_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes()));
+        CU(cudaFuncSetAttribute(emb_gemm_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_merge_smem_bytes()));
+    }
+    // an even number of query groups runs in CTA pairs that share every row tile (emb_gemm.cuh)
+    const bool paired = n_qgroups % GEMM_CLUSTER == 0;
+    cudaLaunchAttribute cluster_attr{};
+    cluster_attr.id = cudaLaunchAttributeClusterDimension;
+    cluster_attr.val.clusterDim.x = paired ? GEMM_CLUSTER : 1;
+    cluster_attr.val.clusterDim.y = cluster_attr.val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg{};
+    cfg.blockDim = dim3(GEMM_THREADS);
+    cfg.dynamicSmemBytes = gemm_smem_bytes();
+    cfg.stream = c->stream;
+    cfg.attrs = &cluster_attr;
+    cfg.numAttrs = paired ? 1 : 0;
+    // one wave: one CTA per SM and query group, or as many pairs as can be resident at once (a GPC with an odd number
+    // of free SMs leaves one idle; a second wave would double the sweep); the merge gathers at most 512 lists per query
+    uint32_t resident = c->prop.multiProcessorCount;
+    if (paired) {
+        static std::mutex occ_mu;   // resident clusters per (device, kernel): queried once
+        static std::map<std::pair<int, const void *>, int> occ;
+        std::lock_guard<std::mutex> g(occ_mu);
+        auto it = occ.find(std::make_pair(c->device, sweep_fn));
+        int n_clusters = 0;
+        if (it == occ.end()) {
+            cfg.gridDim = dim3(GEMM_CLUSTER * c->prop.multiProcessorCount);
+            CU(cudaOccupancyMaxActiveClusters(&n_clusters, sweep_fn, &cfg));
+            occ[std::make_pair(c->device, sweep_fn)] = n_clusters;
+        } else n_clusters = it->second;
+        if (n_clusters < 1) return fail(OC_ERR_UNSUPPORTED, "no CTA pair of the K2 sweep fits on device %d", c->device);
+        resident = GEMM_CLUSTER * uint32_t(n_clusters);
+    }
+    const uint32_t cpg = std::min<uint32_t>(512 / GEMM_LISTS_PER_CTA, std::max<uint32_t>(1, resident / n_qgroups));
     const uint32_t grid = cpg * n_qgroups;
+    cfg.gridDim = dim3(grid);
     const uint32_t lists = cpg * GEMM_LISTS_PER_CTA;
     const uint32_t cap = GEMM_LIST_CAP;
     CUtensorMap tm_q, tm_x;
@@ -619,7 +655,7 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
         q_operand = c->q_bf16.p;
     }
     OCTRY(tmap_2d(&tm_q, q_operand, Bpad, e->stride, GEMM_M, bf16));
-    OCTRY(tmap_2d(&tm_x, e->rows, e->n_rows, e->stride, GEMM_N, bf16));
+    OCTRY(tmap_2d(&tm_x, e->rows, e->n_rows, e->stride, GEMM_N / (paired ? GEMM_CLUSTER : 1), bf16));   // a CTA's share of a tile
     OCTRY(c->g_thr.ensure(size_t(B) * 4));
     OCTRY(c->g_eps.ensure(size_t(B) * 4));
     OCTRY(c->g_cand.ensure(size_t(Bpad) * lists * cap * 8));
@@ -636,14 +672,9 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
     gp.gmax = c->g_max.as<float>();
     gp.ovf = c->g_ovf.as<uint64_t>(); gp.ovf_cnt = c->g_ovfcnt.as<uint32_t>(); gp.ovf_cap = GEMM_OVF_CAP;
     if (qf) { gp.row_bits = row_bits; gp.row_words = row_words; gp.q_slot = qf->d_q_slot; }
-    if (smem_cfg_needed(c->device, (const void *)emb_gemm_kernel<false>, gemm_smem_bytes())) {   // all sweep kernels at once
-        CU(cudaFuncSetAttribute(emb_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes()));
-        CU(cudaFuncSetAttribute(emb_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes()));
-        CU(cudaFuncSetAttribute(emb_gemm_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_merge_smem_bytes()));
-    }
     auto launch_gemm = [&]() -> int {
-        if (bf16) emb_gemm_kernel<true><<<grid, GEMM_THREADS, gemm_smem_bytes(), c->stream>>>(tm_q, tm_x, gp);
-        else emb_gemm_kernel<false><<<grid, GEMM_THREADS, gemm_smem_bytes(), c->stream>>>(tm_q, tm_x, gp);
+        if (bf16) CU(cudaLaunchKernelEx(&cfg, emb_gemm_kernel<true>, tm_q, tm_x, gp));
+        else CU(cudaLaunchKernelEx(&cfg, emb_gemm_kernel<false>, tm_q, tm_x, gp));
         launched(c, gp.max_mode == 0);   // the one-tile threshold pass is not counted as a sweep
         CU(cudaGetLastError());
         return OC_OK;

@@ -8,12 +8,19 @@
 //   * operands: fp32 rows straight from HBM, consumed by wgmma .tf32 (the tensor core reads the
 //     fp32 bits and drops the low 13 mantissa bits) — no converted copy of the store, algorithmic
 //     bytes = n_rows * stride * 4 per batch; bf16 stores use wgmma .bf16;
-//   * CTA tile: M = 128 queries (A operand, two consumer warpgroups of 64) x N = 128 rows (B operand),
+//   * CTA tile: M = 128 queries (A operand, two consumer warpgroups of 64) x N = 256 rows (B operand),
 //     K-blocks of 128 bytes = one swizzle row; one producer warp fills a 4-stage shared-memory ring
 //     with TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B) under full / empty mbarriers, each consumer
-//     warpgroup issues wgmma.mma_async m64n128 into 64 fp32 accumulator registers per thread;
-//   * epilogue, straight from the accumulator registers: a thread holds 2 queries x 32 rows of the
-//     tile (wgmma's D fragment), scales them by the rows' inverse norms and pushes every row whose
+//     warpgroup issues wgmma.mma_async m64n256 into 128 fp32 accumulator registers per thread;
+//   * CTA pairs: with an even number of query groups the sweep is launched in clusters of 2 CTAs, query
+//     groups 2i and 2i + 1 of the same row partition.  Each CTA loads one 128-row half of every row tile
+//     with TMA multicast into both CTAs' rings, so each row leaves L2 once per batch instead of once per
+//     query group; a stage is refilled only when the consumers of BOTH CTAs have released it.  Launched
+//     without a cluster (odd group counts, the kernel test harness) a CTA loads the whole tile itself;
+//     tm_x's box is GEMM_N / (cluster size) rows;
+//   * epilogue, straight from the accumulator registers: a thread holds 2 queries x 64 rows of the
+//     tile (wgmma's D fragment), taken in two halves of 32 rows (one per 128-row half of the tile),
+//     scales them by the rows' inverse norms and pushes every row whose
 //     approximate score clears the query's threshold into a private candidate list — one list per
 //     (query, CTA, lane % 4); the threshold is the query's running K'-th best, seeded by a one-tile
 //     threshold pass of the same kernel and shared across CTAs through an atomicMax'd global array
@@ -35,13 +42,18 @@
 namespace oc {
 
 constexpr uint32_t GEMM_CONSUMER_WG = 2;                          // warpgroups issuing wgmma, 64 queries each
-constexpr int GEMM_THREADS = GEMM_CONSUMER_WG * 128 + 32;         // warps 0-7: consumers, warp 8: TMA producer
+// warps 0-7: consumers, warps 8-11: the producer warpgroup (warp 8 issues the TMA loads).  A whole producer warpgroup
+// lets setmaxnreg move registers to the consumers: 168 per thread at launch (64K / 384), then 40 for the producers
+// and 232 for the consumers (128 accumulators + the epilogue)
+constexpr int GEMM_THREADS = (GEMM_CONSUMER_WG + 1) * 128;
+constexpr uint32_t GEMM_PRODUCER_REGS = 40, GEMM_CONSUMER_REGS = 232;
 constexpr uint32_t GEMM_M = 128;       // queries per CTA
-constexpr uint32_t GEMM_N = 128;       // rows per tile
+constexpr uint32_t GEMM_N = 256;       // rows per tile
 constexpr uint32_t GEMM_KB = 32;       // fp32 elements per K-block (one 128 B swizzle row); bf16 rows: 64
 constexpr uint32_t GEMM_STAGES = 4;
+constexpr uint32_t GEMM_CLUSTER = 2;   // CTAs of a paired launch (two query groups sharing each row tile)
 constexpr uint32_t GEMM_A_BYTES = GEMM_M * 128;   // 16 KB
-constexpr uint32_t GEMM_B_BYTES = GEMM_N * 128;   // 16 KB
+constexpr uint32_t GEMM_B_BYTES = GEMM_N * 128;   // 32 KB
 constexpr uint32_t GEMM_STAGE_BYTES = GEMM_A_BYTES + GEMM_B_BYTES;
 constexpr uint32_t GEMM_LISTS_PER_CTA = 4;        // candidate lists per (query, CTA): one per lane % 4 of the D fragment
 constexpr uint32_t GEMM_LIST_CAP = 128;           // entries of one (query, list) candidate buffer
@@ -90,8 +102,8 @@ struct GemmParams {
     uint64_t row_words;
     const uint32_t *q_slot;    // [n_queries]
 };
-// The 32 rows a thread holds of a 128-row tile (rows row0 + 2 (lane & 3) + 8 (j >> 1) + (j & 1), j < 32) as bit j of a
-// mask, from the tile's 4 words of a row bitmap: word w gives bits 8w .. 8w + 7 (its bits 8m + 2 (lane & 3) + {0, 1}).
+// The 32 rows a thread holds of a 128-row half tile (rows row0 + 2 (lane & 3) + 8 (j >> 1) + (j & 1), j < 32) as bit j
+// of a mask, from the half's 4 words of a row bitmap: word w gives bits 8w .. 8w + 7 (its bits 8m + 2 (lane & 3) + {0, 1}).
 __device__ __forceinline__ uint32_t gemm_tile_row_mask(const uint32_t *bits, uint32_t lane) {
     const uint4 w = __ldg(reinterpret_cast<const uint4 *>(bits));
     const uint32_t s = 2 * (lane & 3);
@@ -124,8 +136,46 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, u
         "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
         : "memory");
 }
+// the same box written to the same shared-memory offset of every CTA in cta_mask, each CTA's mbarrier at `bar`'s
+// offset receiving complete_tx of the box's bytes
+__device__ __forceinline__ void tma_load_2d_multicast(void *dst, const CUtensorMap *map, uint64_t *bar, int32_t c0, int32_t c1,
+                                                      uint16_t cta_mask, uint64_t hint) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
+        " [%0], [%1, {%3, %4}], [%2], %5, %6;" ::"r"(smem_u32(dst)),
+        "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask), "l"(hint)
+        : "memory");
+}
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap *map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
+}
+// ---- thread-block clusters (1 CTA when launched without a cluster) ----
+__device__ __forceinline__ uint32_t cluster_nctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
+    return r;
+}
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+// per-thread register budget of the calling warpgroup (all its warps execute the same one)
+template <uint32_t R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+// every thread of every CTA of the cluster (need not be warp-converged)
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// arrive on the mbarrier at `bar`'s shared-memory offset in CTA `cta` of the cluster.  Default (.cta) release scope:
+// what it orders is the arriving warp's wgmma reads of a stage, already complete (wgmma.wait_group), before the
+// partner's TMA overwrites it; .release.cluster would put a MEMBAR.GPU in front of every arrival of the K loop.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t *bar, uint32_t cta) {
+    asm volatile(
+        "{\n\t.reg .b32 ra;\n\t"
+        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+        "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)), "r"(cta)
+        : "memory");
 }
 // K-major, SWIZZLE_128B shared-memory matrix descriptor of wgmma:
 // start>>4 [0,14) | LBO>>4 [16,30) = 1 (unused when swizzled) | SBO>>4 [32,46) = 1024/16 (8-row groups) | layout [62,64) = 1
@@ -136,33 +186,45 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
-// D[64 x 128] (+)= A[64 x K] * B[128 x K]^T, both K-major in shared memory; K = 8 (tf32) or 16 (bf16) = 32 bytes
+// D[64 x 256] (+)= A[64 x K] * B[256 x K]^T, both K-major in shared memory; K = 8 (tf32) or 16 (bf16) = 32 bytes
 template <bool BF16>
-__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_m64n256(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
 #define OC_WGMMA_D                                                                                                             \
-    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, "   \
-    "%25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "    \
-    "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
+    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "         \
+    "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, "          \
+    "%46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, "          \
+    "%68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, "          \
+    "%90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, "          \
+    "%110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}"
 #define OC_WGMMA_OPS                                                                                                           \
-    "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),    \
-        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),   \
-        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),   \
-        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),   \
-        "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),   \
-        "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),   \
-        "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+    "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),               \
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),                 \
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),                \
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),                \
+        "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),                \
+        "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),                \
+        "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),                \
+        "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]),                \
+        "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]),                \
+        "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]),                \
+        "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]),                \
+        "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]),                \
+        "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]),           \
+        "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]),        \
+        "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]),        \
+        "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
     if (BF16)
         asm volatile(
             "{\n\t.reg .pred p;\n\t"
-            "setp.ne.b32 p, %66, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 " OC_WGMMA_D ", %64, %65, p, 1, 1, 0, 0;\n\t}"
+            "setp.ne.b32 p, %130, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 " OC_WGMMA_D ", %128, %129, p, 1, 1, 0, 0;\n\t}"
             : OC_WGMMA_OPS
             : "l"(adesc), "l"(bdesc), "r"(accumulate));
     else
         asm volatile(
             "{\n\t.reg .pred p;\n\t"
-            "setp.ne.b32 p, %66, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " OC_WGMMA_D ", %64, %65, p, 1, 1;\n\t}"
+            "setp.ne.b32 p, %130, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 " OC_WGMMA_D ", %128, %129, p, 1, 1;\n\t}"
             : OC_WGMMA_OPS
             : "l"(adesc), "l"(bdesc), "r"(accumulate));
 #undef OC_WGMMA_D
@@ -246,15 +308,30 @@ __device__ __noinline__ void gemm_compact(const GemmParams &p, uint32_t need, ui
     }
 }
 
+// Accumulator of the j-th of the 32 rows (rows 2 (lane & 3) + 8 (j >> 1) + (j & 1) of the 128-row half u of the tile)
+// a thread holds for its query h.
+__host__ __device__ constexpr uint32_t gemm_frag(uint32_t u, uint32_t h, uint32_t j) {
+    return 64 * u + 4 * (j >> 1) + 2 * h + (j & 1);
+}
+// A stage is free again once the consumer warps of every CTA it is loaded into have arrived on its `empty` barrier.
+__device__ __forceinline__ void gemm_release(uint64_t *empty, uint32_t csize) {
+    if (csize == 1) mbar_arrive(empty);
+    else
+        for (uint32_t r = 0; r < csize; r++) mbar_arrive_cluster(empty, r);
+}
+
 // One CTA = one query group (128 queries) x one row partition c of the store (tiles c, c + ctas_per_group, ...).
-// wgmma D fragment of m64n128 (per warpgroup): warp w holds rows [16w, 16w + 16); lane holds rows lane/4 and
-// lane/4 + 8, columns 8j + 2 (lane % 4) + {0, 1} for j = 0..15, in d[4j + 2h + {0, 1}] (h = row half).
+// The CTAs of a cluster (blockIdx.x 2i, 2i + 1; n_qgroups even) share c, hence the tiles and the stage sequence.
+// wgmma D fragment of m64n256 (per warpgroup): warp w holds rows [16w, 16w + 16); lane holds rows lane/4 and
+// lane/4 + 8, columns 8j + 2 (lane % 4) + {0, 1} for j = 0..31, in d[4j + 2h + {0, 1}] (h = row half); the
+// tile's 128-row half u is j = 16u .. 16u + 15.
 template <bool BF16, bool DUMP = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_x,
                 const typename GemmKernelParams<DUMP>::type p) {
     extern __shared__ __align__(1024) uint8_t smem_gemm[];
-    // SWIZZLE_128B tiles need 1024-byte alignment of the shared-memory address
+    // SWIZZLE_128B tiles need 1024-byte alignment of the shared-memory address (the same offset in every CTA: the
+    // multicast writes both CTAs of a pair at one offset)
     uint8_t *ring = smem_gemm + ((1024u - (smem_u32(smem_gemm) & 1023u)) & 1023u);
     float *inr_s = reinterpret_cast<float *>(ring + GEMM_STAGES * GEMM_STAGE_BYTES);   // [wg][2][GEMM_N]
     uint64_t *bars = reinterpret_cast<uint64_t *>(inr_s + GEMM_CONSUMER_WG * 2 * GEMM_N);
@@ -263,6 +340,7 @@ emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t grp = blockIdx.x % p.n_qgroups;     // query group
     const uint32_t c = blockIdx.x / p.n_qgroups;       // row partition
+    const uint32_t csize = cluster_nctarank();         // 1, or GEMM_CLUSTER for a paired launch
     const uint64_t n_tiles = (p.n_rows + GEMM_N - 1) / GEMM_N;
     uint64_t my_tiles = (n_tiles > c) ? (n_tiles - c + p.ctas_per_group - 1) / p.ctas_per_group : 0;
     if (p.tile_limit && my_tiles > p.tile_limit) my_tiles = p.tile_limit;
@@ -270,34 +348,48 @@ emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     constexpr int32_t KSTEP = BF16 ? 2 * GEMM_KB : GEMM_KB;
 
     if (threadIdx.x == 0) {
-        for (uint32_t s = 0; s < GEMM_STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], GEMM_CONSUMER_WG * 4); }
+        for (uint32_t s = 0; s < GEMM_STAGES; s++) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], GEMM_CONSUMER_WG * 4 * csize);
+        }
         fence_mbar_init();
         tma_prefetch_desc(&tm_q);
         tma_prefetch_desc(&tm_x);
     }
-    __syncthreads();
+    // the partner CTA multicasts into this CTA's ring and arrives on its barriers: both must be initialised first
+    if (csize > 1) cluster_sync();
+    else __syncthreads();
 
-    if (warp == GEMM_CONSUMER_WG * 4) {
+    if (warp >= GEMM_CONSUMER_WG * 4) {
         // ===================== TMA producer =====================
-        if (lane == 0) {
+        setmaxnreg_dec<GEMM_PRODUCER_REGS>();
+        if (warp == GEMM_CONSUMER_WG * 4 && lane == 0) {
+            // this CTA's share of the row tile: all of it, or one half multicast into both CTAs of the pair
+            const uint32_t crank = cluster_ctarank(), b_rows = GEMM_N / csize;
+            const uint16_t cta_mask = uint16_t((1u << csize) - 1u);
             uint64_t n = 0;
             for (uint64_t it = 0; it < my_tiles; it++) {
-                const uint64_t row0 = (c + it * p.ctas_per_group) * GEMM_N;
+                const uint64_t row0 = (c + it * p.ctas_per_group) * GEMM_N + crank * b_rows;
                 for (uint32_t kb = 0; kb < nkb; kb++, n++) {
                     const uint32_t s = uint32_t(n % GEMM_STAGES), ph = uint32_t((n / GEMM_STAGES) & 1);
                     mbar_wait(&empty[s], ph ^ 1);
                     uint8_t *a_dst = ring + s * GEMM_STAGE_BYTES;
-                    mbar_expect_tx(&full[s], GEMM_STAGE_BYTES);
+                    uint8_t *b_dst = a_dst + GEMM_A_BYTES + crank * b_rows * 128;
+                    mbar_expect_tx(&full[s], GEMM_STAGE_BYTES);   // the whole stage lands in every CTA
                     // rows past the padded query matrix / the store are zero-filled by TMA
                     tma_load_2d(a_dst, &tm_q, &full[s], int32_t(kb) * KSTEP, int32_t(grp * GEMM_M), TMA_EVICT_LAST);
-                    tma_load_2d(a_dst + GEMM_A_BYTES, &tm_x, &full[s], int32_t(kb) * KSTEP, int32_t(row0), TMA_EVICT_FIRST);
+                    if (csize == 1) tma_load_2d(b_dst, &tm_x, &full[s], int32_t(kb) * KSTEP, int32_t(row0), TMA_EVICT_FIRST);
+                    else tma_load_2d_multicast(b_dst, &tm_x, &full[s], int32_t(kb) * KSTEP, int32_t(row0), cta_mask, TMA_EVICT_FIRST);
                 }
             }
         }
+        // no CTA leaves while its partner may still write into its ring or arrive on its barriers
+        if (csize > 1) cluster_sync();
         return;
     }
 
     // ===================== consumers: wgmma + epilogue =====================
+    setmaxnreg_inc<GEMM_CONSUMER_REGS>();
     const uint32_t wg = warp >> 2, t = threadIdx.x & 127;
     const uint32_t lists = p.lists_per_query;
     const uint32_t my_list = c * GEMM_LISTS_PER_CTA + (lane & 3);
@@ -313,16 +405,17 @@ emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         e[h].thr = live[h] ? -INFINITY : INFINITY;     // refreshed from the query's global threshold before every tile
         e[h].best = -INFINITY;                         // max_mode: best approximate score seen by this list
     }
-    float d[64];
+    float d[128];
 #pragma unroll
-    for (uint32_t i = 0; i < 64; i++) d[i] = 0.f;
+    for (uint32_t i = 0; i < 128; i++) d[i] = 0.f;
     uint64_t n = 0;
     for (uint64_t it = 0; it < my_tiles; it++) {
         const uint64_t row0 = (c + it * p.ctas_per_group) * GEMM_N;
         float *inr = inr_s + (wg * 2 + uint32_t(it & 1)) * GEMM_N;
-        {
-            const uint64_t r = row0 + t;
-            inr[t] = r < p.n_rows ? __ldg(p.inv_norm + r) : __int_as_float(0x7fc00000);
+#pragma unroll
+        for (uint32_t i = t; i < GEMM_N; i += 128) {
+            const uint64_t r = row0 + i;
+            inr[i] = r < p.n_rows ? __ldg(p.inv_norm + r) : __int_as_float(0x7fc00000);
         }
         // requested before the main loop, consumed after it: the L2 round trip hides behind the MMAs of this tile
         unsigned int tg[2];
@@ -339,64 +432,70 @@ emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
             wgmma_fence();
 #pragma unroll
             for (uint32_t k = 0; k < 4; k++)   // 32 B of K per instruction: advance the start address by 32 B (>> 4 = 2)
-                wgmma_m64n128<BF16>(d, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0);
+                wgmma_m64n256<BF16>(d, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0);
             wgmma_commit();
             if (kb > 0) {                      // the previous K-block's MMAs have retired: free its stage
                 wgmma_wait<1>();
-                if (lane == 0) mbar_arrive(&empty[prev_s]);
+                if (lane == 0) gemm_release(&empty[prev_s], csize);
             }
             prev_s = s;
         }
         wgmma_wait<0>();
-        if (lane == 0) mbar_arrive(&empty[prev_s]);
+        if (lane == 0) gemm_release(&empty[prev_s], csize);
         named_bar_sync(1 + wg, 128);           // this warpgroup's inverse norms are in shared memory
 
-        const float2 *inr2 = reinterpret_cast<const float2 *>(inr);
+        // in 128-row halves of the tile: 32 rows per (thread, query) at a time keep v[] at 32 registers, and each
+        // half pushes at most 32 entries into a list between two list-full tests
 #pragma unroll
-        for (uint32_t h = 0; h < 2; h++) {
-            GemmEpi &E = e[h];
-            if (tg[h]) E.thr = fmaxf(E.thr, f32_unordered(tg[h]));   // the query's threshold as raised by every CTA so far
-            float v[32];
+        for (uint32_t u = 0; u < 2; u++) {
+            const uint64_t rowu = row0 + 128 * u;
+            const float2 *inr2 = reinterpret_cast<const float2 *>(inr + 128 * u);
 #pragma unroll
-            for (uint32_t j = 0; j < 16; j++) {
-                const float2 w = inr2[4 * j + (lane & 3)];
-                v[2 * j + 0] = d[4 * j + 2 * h + 0] * w.x;   // cos * |q|
-                v[2 * j + 1] = d[4 * j + 2 * h + 1] * w.y;
-            }
-            if constexpr (DUMP) {
-                const uint64_t rb = row0 + 2 * (lane & 3);
+            for (uint32_t h = 0; h < 2; h++) {
+                GemmEpi &E = e[h];
+                if (u == 0 && tg[h]) E.thr = fmaxf(E.thr, f32_unordered(tg[h]));   // the query's threshold as raised by every CTA so far
+                // scaled in place (the next tile's first wgmma overwrites the accumulators): no extra registers
 #pragma unroll
-                for (uint32_t j = 0; j < 32; j++) {
-                    const uint64_t r = rb + 8 * (j >> 1) + (j & 1);
-                    if (live[h] && r < p.n_rows) p.dump[size_t(q[h]) * p.n_rows + r] = v[j];
+                for (uint32_t j = 0; j < 16; j++) {
+                    const float2 w = inr2[4 * j + (lane & 3)];
+                    d[gemm_frag(u, h, 2 * j + 0)] *= w.x;   // cos * |q|
+                    d[gemm_frag(u, h, 2 * j + 1)] *= w.y;
                 }
-                continue;
-            }
-            if (p.max_mode) {
-                // a row the query's own filter rejects must not raise its bound (it is NaN in a single-filter sweep)
-                const uint32_t ok = slot[h] == SLOT_NONE ? 0xffffffffu
-                                                         : gemm_tile_row_mask(p.row_bits + size_t(slot[h]) * p.row_words + row0 / 32, lane);
+                if constexpr (DUMP) {
+                    const uint64_t rb = rowu + 2 * (lane & 3);
 #pragma unroll
-                for (uint32_t j = 0; j < 32; j++)
-                    if ((ok >> j) & 1u) E.best = fmaxf(E.best, v[j]);   // NaN (dead rows) ignored
-                continue;
-            }
-            uint32_t mask = 0;
+                    for (uint32_t j = 0; j < 32; j++) {
+                        const uint64_t r = rb + 8 * (j >> 1) + (j & 1);
+                        if (live[h] && r < p.n_rows) p.dump[size_t(q[h]) * p.n_rows + r] = d[gemm_frag(u, h, j)];
+                    }
+                    continue;
+                }
+                if (p.max_mode) {
+                    // a row the query's own filter rejects must not raise its bound (it is NaN in a single-filter sweep)
+                    const uint32_t ok = slot[h] == SLOT_NONE ? 0xffffffffu
+                                                             : gemm_tile_row_mask(p.row_bits + size_t(slot[h]) * p.row_words + rowu / 32, lane);
 #pragma unroll
-            for (uint32_t j = 0; j < 32; j++) mask |= (v[j] > E.thr ? 1u : 0u) << j;   // NaN fails
-            // per-query filter: only rows that already clear the threshold look at the bitmap (the common path of the
-            // sweep loads nothing more)
-            if (mask && slot[h] != SLOT_NONE)
-                mask &= gemm_tile_row_mask(p.row_bits + size_t(slot[h]) * p.row_words + row0 / 32, lane);
-            if (mask) {   // rare once the threshold has tightened
-                uint64_t *mybuf = p.cand + (size_t(q[h]) * lists + my_list) * p.cap;
-                const uint32_t rb = uint32_t(row0) + 2 * (lane & 3);
+                    for (uint32_t j = 0; j < 32; j++)
+                        if ((ok >> j) & 1u) E.best = fmaxf(E.best, d[gemm_frag(u, h, j)]);   // NaN (dead rows) ignored
+                    continue;
+                }
+                uint32_t mask = 0;
 #pragma unroll
-                for (uint32_t j = 0; j < 32; j++)
-                    if ((mask >> j) & 1u) { mybuf[E.cnt] = make_key(v[j], rb + 8 * (j >> 1) + (j & 1)); E.cnt++; }
+                for (uint32_t j = 0; j < 32; j++) mask |= (d[gemm_frag(u, h, j)] > E.thr ? 1u : 0u) << j;   // NaN fails
+                // per-query filter: only rows that already clear the threshold look at the bitmap (the common path of
+                // the sweep loads nothing more)
+                if (mask && slot[h] != SLOT_NONE)
+                    mask &= gemm_tile_row_mask(p.row_bits + size_t(slot[h]) * p.row_words + rowu / 32, lane);
+                if (mask) {   // rare once the threshold has tightened
+                    uint64_t *mybuf = p.cand + (size_t(q[h]) * lists + my_list) * p.cap;
+                    const uint32_t rb = uint32_t(rowu) + 2 * (lane & 3);
+#pragma unroll
+                    for (uint32_t j = 0; j < 32; j++)
+                        if ((mask >> j) & 1u) { mybuf[E.cnt] = make_key(d[gemm_frag(u, h, j)], rb + 8 * (j >> 1) + (j & 1)); E.cnt++; }
+                }
+                const uint32_t need = __ballot_sync(0xffffffffu, E.cnt + 32 > p.cap);
+                if (need) gemm_compact(p, need, q[h], my_list, lane, E);
             }
-            const uint32_t need = __ballot_sync(0xffffffffu, E.cnt + 32 > p.cap);
-            if (need) gemm_compact(p, need, q[h], my_list, lane, E);
         }
     }
     if constexpr (!DUMP) {
@@ -406,6 +505,7 @@ emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
             else p.cand_cnt[size_t(q[h]) * lists + my_list] = live[h] ? e[h].cnt : 0;
         }
     }
+    if (csize > 1) cluster_sync();
 }
 
 // ---------------------------------------------------------------------------------------
