@@ -216,6 +216,7 @@ typedef struct {
  *     do not pass).  All entries NULL: an unfiltered search; every entry the same handle: the p->filter path.
  *   - OC_ERR_INVALID: q_filters together with filter or filter_bits, a handle of another ctx.
  *     OC_ERR_UNSUPPORTED: sharded.  A refused call creates nothing and writes no output.
+ *   - oc_search_q_sorted takes q_filters together with a sort and pins per query;
  *   - oc_search_groups*, oc_search_pinned and oc_search_sorted refuse q_filters with OC_ERR_UNSUPPORTED;
  *     oc_search_facets ignores it as it ignores filter (facets are scored without the where-filter). */
 int oc_search(oc_ctx *ctx, oc_emb *emb, oc_str *str, const oc_search_params *p,
@@ -468,6 +469,19 @@ typedef struct {
 int oc_search_sorted(oc_ctx *ctx, oc_emb *emb, oc_str *str, const oc_search_params *p, const oc_sort *sort,
                      const oc_pins *pins, uint64_t *out_doc_ids, float *out_scores, double *out_sort_values,
                      uint32_t *out_n, uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present);
+/* One batch in which every query has its own sort, its own pins and (q_filters) its own where-filter: the batched form
+ * of Search::execute with a per-request sort_by and pin rules.  Query b's outputs (hits, scores, n, count, sort values
+ * and its items' pin scores / present flags) are exactly what it gets alone (B = 1) with its own filter and items:
+ *   - q_sorts[b].field != NULL: oc_search_sorted with q_sorts[b];
+ *   - q_sorts[b].field == NULL: oc_search_pinned (score order); its sort values are NaN, past out_n 0.0.
+ * So a batch whose entries all hold one sort, without q_filters, equals oc_search_sorted, and a batch of NULL fields
+ * equals oc_search_pinned.  q_sorts: B entries.  Outputs as oc_search_sorted; pins may be NULL.
+ * OC_ERR_INVALID: q_sorts NULL, a bad order in an entry with a field, a sort field, filter or store of another ctx,
+ * q_filters together with filter / filter_bits, q_pin_offsets not monotone.  OC_ERR_UNSUPPORTED: p->sharded, and the
+ * limit + offset limits of oc_search_sorted / oc_search_pinned.  A failed call writes nothing. */
+int oc_search_q_sorted(oc_ctx *ctx, oc_emb *emb, oc_str *str, const oc_search_params *p, const oc_sort *q_sorts,
+                       const oc_pins *pins, uint64_t *out_doc_ids, float *out_scores, double *out_sort_values,
+                       uint32_t *out_n, uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present);
 /* oc_search_groups_pinned in field order: per group the first max_results members that are keys, in field order (2 x
  * max_results for an active query), with their score-map values (NaN kept), members with no value skipped; then the
  * group's member items are spliced as in oc_search_groups_pinned.  The flat hits follow oc_search_sorted (not written
@@ -550,6 +564,19 @@ int oc_batcher_create(oc_ctx *ctx, oc_emb *emb, oc_str *str, uint32_t max_batch,
 void oc_batcher_destroy(oc_batcher *b);
 int oc_batcher_search(oc_batcher *b, const oc_search_params *p, uint64_t *out_doc_ids, float *out_scores,
                       uint32_t *out_n, uint64_t *out_count);
+/* oc_batcher_search with a sort and pin rules: one query, its sort (NULL: score order) and its items (pins may be NULL;
+ * q_pin_offsets has 2 entries).  Outputs as oc_search_q_sorted with B = 1: out_doc_ids / out_scores / out_sort_values
+ * hold limit entries (out_sort_values may be NULL), out_pin_scores / out_pin_present (may be NULL) item j at
+ * q_pin_offsets[0] + j.  Requests of both entry points share a
+ * batch when their (mode, limit, offset, similarity, threshold, bm25_k, bm25_b, vector_limit) match; a batch with no
+ * sort and no item runs as oc_search, any other as oc_search_q_sorted (the items concatenated in request order, each
+ * p->filter as its q_filters entry).  A sort field of another ctx, a bad order or malformed pins are refused with
+ * OC_ERR_INVALID before the request joins a batch.  A request the merged call could not take runs alone through
+ * oc_search_q_sorted and gets its normal error there: one oc_batcher_search would not coalesce, items with apply = 0,
+ * more than OC_MAX_TOPK items, or items with 2 x (limit + offset) > OC_MAX_TOPK. */
+int oc_batcher_search_sorted(oc_batcher *b, const oc_search_params *p, const oc_sort *sort, const oc_pins *pins,
+                             uint64_t *out_doc_ids, float *out_scores, double *out_sort_values, uint32_t *out_n,
+                             uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present);
 /* queries that went through a coalesced batch / number of batches / calls passed straight through */
 int oc_batcher_stats(oc_batcher *b, uint64_t *n_queries, uint64_t *n_batches, uint64_t *n_direct);
 

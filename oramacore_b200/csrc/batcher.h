@@ -10,11 +10,16 @@
 // threshold, bm25_k, bm25_b, vector_limit), no host bitmap (filter_bits), no q_filters, no OMC, not
 // sharded; anything else runs directly.  A device filter (p->filter) is per query: the merged batch
 // carries it as that query's q_filters entry, so filtered and unfiltered requests share a batch.
+// Requests of submit_sorted carry a sort (or score order) and pin items of their own and share batches with plain
+// requests: a batch with no sort and no item runs through `Exec` as before, any other through `SortedExec`
+// (oc_search_q_sorted) with the sorts and the items' CSR merged in request order.
 #pragma once
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
 #include <cstring>
+#include <limits>
 #include <mutex>
 #include <vector>
 
@@ -50,9 +55,38 @@ inline bool batchable(const oc_search_params *p, bool has_emb = true, bool has_s
     return true;
 }
 
+// The items of a one-query oc_pins (none for NULL); the library's checks of q_pin_offsets / doc_ids / positions.
+inline uint32_t pin_items(const oc_pins *pins) { return pins ? pins->q_pin_offsets[1] - pins->q_pin_offsets[0] : 0u; }
+// OC_OK, or OC_ERR_INVALID (with *why) for a request of submit_sorted the library would refuse for its own arguments:
+// it must not join, and fail, a batch.
+inline int check_sorted(const oc_sort *sort, const oc_pins *pins, const char **why) {
+    if (sort && sort->field && sort->order != OC_SORT_ASC && sort->order != OC_SORT_DESC) { *why = "sort order is neither ASC nor DESC"; return OC_ERR_INVALID; }
+    if (pins) {
+        if (!pins->q_pin_offsets) { *why = "pins: q_pin_offsets is NULL"; return OC_ERR_INVALID; }
+        if (pins->q_pin_offsets[1] < pins->q_pin_offsets[0]) { *why = "pins: q_pin_offsets is not monotone"; return OC_ERR_INVALID; }
+        if (pin_items(pins) && (!pins->doc_ids || !pins->positions)) { *why = "pins: doc_ids / positions are NULL"; return OC_ERR_INVALID; }
+    }
+    return OC_OK;
+}
+// Whether a request's items can join a merged oc_search_q_sorted without failing it.  apply = 0 with items (the
+// per-index call of a multi-index search) cannot share the merged apply = 1 CSR.  More than OC_MAX_TOPK items, or items
+// with 2 x (limit + offset) > OC_MAX_TOPK, make the library refuse the whole call with OC_ERR_UNSUPPORTED: such a
+// request runs alone and gets that error, and the requests it would have joined do not.
+inline bool pins_batchable(const oc_search_params *p, const oc_pins *pins) {
+    const uint32_t k = pin_items(pins);
+    if (!k) return true;
+    return pins->apply && k <= OC_MAX_TOPK && (uint64_t(p->limit) + p->offset) * 2 <= OC_MAX_TOPK;
+}
+
 struct BatchReq {
     const oc_search_params *p;
     uint64_t *docs; float *scores; uint32_t *n; uint64_t *count;
+    // submit_sorted only
+    const oc_sort *sort = nullptr;      // NULL or field NULL: score order
+    const oc_pins *pins = nullptr;      // this query's items, NULL: none
+    double *sort_values = nullptr;      // [limit]
+    float *pin_scores = nullptr;        // [items], may be NULL
+    uint8_t *pin_present = nullptr;
     int rc = 0;
     bool done = false;
 };
@@ -66,6 +100,15 @@ struct MergedBatch {
     std::vector<float> scores;
     std::vector<uint32_t> n;
     std::vector<const oc_filter *> q_filters;   // [B] each query's p->filter, or empty when no query has one
+    // a batch with a sort or an item: oc_search_q_sorted's arguments
+    bool sorted = false;
+    std::vector<oc_sort> q_sorts;               // [B]
+    std::vector<uint32_t> pin_off, pin_pos;     // [B + 1], [items]
+    std::vector<uint64_t> pin_doc;
+    oc_pins pins{};
+    std::vector<double> sort_values;            // [B][limit]
+    std::vector<float> pin_scores;              // [items]
+    std::vector<uint8_t> pin_present;
 
     void build(const std::vector<BatchReq *> &reqs, uint32_t dim) {
         const oc_search_params *f = reqs[0]->p;
@@ -114,6 +157,26 @@ struct MergedBatch {
             }
         docs.assign(size_t(B) * f->limit, 0); scores.assign(size_t(B) * f->limit, 0.f);
         n.assign(B, 0); count.assign(B, 0);
+        sorted = false;
+        for (uint32_t i = 0; i < B; i++) sorted = sorted || (reqs[i]->sort && reqs[i]->sort->field) || pin_items(reqs[i]->pins);
+        if (!sorted) return;
+        q_sorts.assign(B, oc_sort{nullptr, OC_SORT_ASC});
+        pin_off.assign(1, 0u); pin_doc.clear(); pin_pos.clear();
+        for (uint32_t i = 0; i < B; i++) {
+            const BatchReq *r = reqs[i];
+            if (r->sort) q_sorts[i] = *r->sort;
+            if (const uint32_t k = pin_items(r->pins)) {
+                const uint32_t o = r->pins->q_pin_offsets[0];
+                pin_doc.insert(pin_doc.end(), r->pins->doc_ids + o, r->pins->doc_ids + o + k);
+                pin_pos.insert(pin_pos.end(), r->pins->positions + o, r->pins->positions + o + k);
+            }
+            pin_off.push_back((uint32_t)pin_doc.size());
+        }
+        static const uint64_t zero_d = 0; static const uint32_t zero_p = 0;
+        pins = oc_pins{pin_off.data(), pin_doc.empty() ? &zero_d : pin_doc.data(), pin_pos.empty() ? &zero_p : pin_pos.data(), 1};
+        sort_values.assign(size_t(B) * f->limit, 0.0);
+        pin_scores.assign(std::max<size_t>(pin_doc.size(), 1), 0.f);
+        pin_present.assign(std::max<size_t>(pin_doc.size(), 1), 0);
     }
     void scatter(const std::vector<BatchReq *> &reqs, int rc) const {
         const uint32_t L = p.limit;
@@ -125,15 +188,36 @@ struct MergedBatch {
             memcpy(r->scores, scores.data() + i * L, size_t(L) * 4);
             *r->n = n[i];
             *r->count = count[i];
+            if (r->sort_values) {   // a batch run as oc_search: score order, NaN as oc_search_q_sorted writes it
+                if (sorted) memcpy(r->sort_values, sort_values.data() + i * L, size_t(L) * 8);
+                else for (uint32_t j = 0; j < L; j++) r->sort_values[j] = j < n[i] ? std::numeric_limits<double>::quiet_NaN() : 0.0;
+            }
+            if (sorted)   // the caller's item j is its entry q_pin_offsets[0] + j, as in a call of its own
+                for (uint32_t j = pin_off[i]; j < pin_off[i + 1]; j++) {
+                    const size_t o = r->pins->q_pin_offsets[0] + (j - pin_off[i]);
+                    if (r->pin_scores) r->pin_scores[o] = pin_scores[j];
+                    if (r->pin_present) r->pin_present[o] = pin_present[j];
+                }
         }
     }
 };
 
-template <class Exec>   // int Exec(const oc_search_params*, uint64_t* docs, float* scores, uint32_t* n, uint64_t* count)
+// The executor of a batcher that only takes submit(): it is never called.
+struct NoSortedExec {
+    int operator()(const oc_search_params *, const oc_sort *, const oc_pins *, uint64_t *, float *, double *, uint32_t *,
+                   uint64_t *, float *, uint8_t *) const { return OC_ERR_UNSUPPORTED; }
+};
+
+// int Exec(const oc_search_params*, uint64_t* docs, float* scores, uint32_t* n, uint64_t* count)
+// int SortedExec(const oc_search_params*, const oc_sort* q_sorts, const oc_pins*, uint64_t* docs, float* scores,
+//                double* sort_values, uint32_t* n, uint64_t* count, float* pin_scores, uint8_t* pin_present)
+template <class Exec, class SortedExec = NoSortedExec>
 class Batcher {
 public:
-    Batcher(Exec exec, uint32_t dim, uint32_t max_batch, uint32_t max_wait_us, bool has_emb = true, bool has_str = true)
-        : exec_(exec), dim_(dim), max_batch_(max_batch ? max_batch : 1), max_wait_us_(max_wait_us), has_emb_(has_emb), has_str_(has_str) {}
+    Batcher(Exec exec, uint32_t dim, uint32_t max_batch, uint32_t max_wait_us, bool has_emb = true, bool has_str = true,
+            SortedExec sexec = SortedExec())
+        : exec_(exec), sexec_(sexec), dim_(dim), max_batch_(max_batch ? max_batch : 1), max_wait_us_(max_wait_us), has_emb_(has_emb),
+          has_str_(has_str) {}
 
     int submit(const oc_search_params *p, uint64_t *docs, float *scores, uint32_t *n, uint64_t *count) {
         if (!batchable(p, has_emb_, has_str_) || max_batch_ == 1) {
@@ -141,6 +225,32 @@ public:
             return exec_(p, docs, scores, n, count);
         }
         BatchReq r{p, docs, scores, n, count};
+        return join(r);
+    }
+    // One query with its sort (NULL: score order) and pin items (NULL: none); pin outputs one per item.
+    int submit_sorted(const oc_search_params *p, const oc_sort *sort, const oc_pins *pins, uint64_t *docs, float *scores,
+                      double *sort_values, uint32_t *n, uint64_t *count, float *pin_scores, uint8_t *pin_present) {
+        const char *why = nullptr;
+        if (const int rc = check_sorted(sort, pins, &why)) return rc;
+        if (!batchable(p, has_emb_, has_str_) || max_batch_ == 1 || !pins_batchable(p, pins)) {
+            direct_++;
+            const oc_sort none{nullptr, OC_SORT_ASC};
+            return sexec_(p, sort ? sort : &none, pins, docs, scores, sort_values, n, count, pin_scores, pin_present);
+        }
+        BatchReq r{p, docs, scores, n, count};
+        r.sort = sort; r.pins = pins; r.sort_values = sort_values; r.pin_scores = pin_scores; r.pin_present = pin_present;
+        return join(r);
+    }
+    void stats(uint64_t *queries, uint64_t *batches, uint64_t *direct) {
+        std::lock_guard<std::mutex> g(mu_);
+        if (queries) *queries = queries_;
+        if (batches) *batches = batches_;
+        if (direct) *direct = direct_.load();
+    }
+
+private:
+    int join(BatchReq &r) {
+        const oc_search_params *p = r.p;
         std::unique_lock<std::mutex> lk(mu_);
         // one group collects at a time: wait while it is full or holds a different parameter tuple
         const BatchKey k = key_of(p);
@@ -159,7 +269,9 @@ public:
             lk.unlock();
             MergedBatch m;
             m.build(batch, dim_);
-            const int rc = exec_(&m.p, m.docs.data(), m.scores.data(), m.n.data(), m.count.data());
+            const int rc = m.sorted ? sexec_(&m.p, m.q_sorts.data(), &m.pins, m.docs.data(), m.scores.data(), m.sort_values.data(),
+                                             m.n.data(), m.count.data(), m.pin_scores.data(), m.pin_present.data())
+                                    : exec_(&m.p, m.docs.data(), m.scores.data(), m.n.data(), m.count.data());
             m.scatter(batch, rc);
             lk.lock();
             batches_++; queries_ += batch.size();
@@ -171,15 +283,9 @@ public:
         }
         return r.rc;
     }
-    void stats(uint64_t *queries, uint64_t *batches, uint64_t *direct) {
-        std::lock_guard<std::mutex> g(mu_);
-        if (queries) *queries = queries_;
-        if (batches) *batches = batches_;
-        if (direct) *direct = direct_.load();
-    }
 
-private:
     Exec exec_;
+    SortedExec sexec_;
     uint32_t dim_, max_batch_, max_wait_us_;
     bool has_emb_, has_str_;
     std::mutex mu_;

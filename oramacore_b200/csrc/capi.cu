@@ -1729,6 +1729,7 @@ struct PinJob {   // oc_search_pinned / oc_search_groups_pinned: the promote ite
     bool splice = false;                // pins apply and some query has items: top lists at twice the depth + the splice
     std::vector<uint64_t> doc;          // [B][stride]
     std::vector<uint32_t> pos, cnt;     // [B][stride], [B]
+    bool q_filters = false;             // oc_search_q_sorted: the batch may carry per-query filters
     const uint64_t *d_doc = nullptr;    // their device copies (set by search_impl)
     const uint32_t *d_pos = nullptr, *d_cnt = nullptr;
 };
@@ -1781,28 +1782,47 @@ static void sort_field_free(oc_sort_field *f) {
     for (SortOrder &o : f->ord) { cudaFree(o.rank_doc); cudaFree(o.doc_rank); cudaFree(o.rank_row); }
     delete f;
 }
+// The sorts of one batch: its distinct (field, order) pairs and, per query, the index of its pair or SORT_BY_SCORE
+// (oc_search_q_sorted: that query is oc_search_pinned's).  oc_search_sorted is the batch whose queries share entry 0.
 struct SortJob {
-    oc_sort_field *f;
-    int order;
-    double *out_values;                    // B x limit, may be NULL
-    double *out_group_values;              // B x n_groups x group_stride, may be NULL
-    uint32_t n_groups;
+    std::vector<oc_sort_field *> f;        // [entries]
+    std::vector<int> order;                // [entries]
+    std::vector<uint32_t> q_ent;           // [B]
+    bool by_score = false;                 // some query is in score order
+    double *out_values = nullptr;          // B x limit, may be NULL
+    double *out_group_values = nullptr;    // B x n_groups x group_stride, may be NULL
+    uint32_t n_groups = 0;
+    SortOrder &ord(uint32_t e) const { return f[e]->ord[order[e]]; }
 };
-static int sort_job_init(oc_ctx *c, const oc_sort *s, SortJob &sj) {
-    if (!s || !s->field) return fail(OC_ERR_INVALID, "NULL sort");
-    if (s->order != OC_SORT_ASC && s->order != OC_SORT_DESC) return fail(OC_ERR_INVALID, "sort order %d is neither ASC nor DESC", s->order);
-    if (s->field->ctx != c) return fail(OC_ERR_INVALID, "sort field belongs to another ctx");
-    sj.f = const_cast<oc_sort_field *>(s->field);   // only its per-snapshot row map is refreshed, under the ctx lock
-    sj.order = s->order;
+// Appends one query's sort (field NULL: score order).  Nothing is written on failure.
+static int sort_job_add(oc_ctx *c, const oc_sort &s, SortJob &sj) {
+    if (!s.field) { sj.q_ent.push_back(SORT_BY_SCORE); sj.by_score = true; return OC_OK; }
+    if (s.order != OC_SORT_ASC && s.order != OC_SORT_DESC) return fail(OC_ERR_INVALID, "sort order %d is neither ASC nor DESC", s.order);
+    if (s.field->ctx != c) return fail(OC_ERR_INVALID, "sort field belongs to another ctx");
+    oc_sort_field *f = const_cast<oc_sort_field *>(s.field);   // only its per-snapshot row map is refreshed, under the ctx lock
+    uint32_t e = 0;
+    while (e < sj.f.size() && !(sj.f[e] == f && sj.order[e] == s.order)) e++;
+    if (e == sj.f.size()) { sj.f.push_back(f); sj.order.push_back(s.order); }
+    sj.q_ent.push_back(e);
     return OC_OK;
 }
-// the value a listed document was placed by: NaN for a document the (active) query promotes, else its value
+// one sort for every query of the batch
+static int sort_job_init(oc_ctx *c, const oc_sort *s, uint32_t B, SortJob &sj) {
+    if (!s || !s->field) return fail(OC_ERR_INVALID, "NULL sort");
+    OCTRY(sort_job_add(c, *s, sj));
+    sj.q_ent.assign(B, 0);
+    return OC_OK;
+}
+// the value a listed document was placed by: NaN for a document the (active) query promotes or a query in score order,
+// else its value
 static double sort_value_of(const SortJob &sj, const PinJob *pj, uint32_t q, uint64_t d) {
+    const uint32_t e = sj.q_ent[q];
+    if (e == SORT_BY_SCORE) return std::numeric_limits<double>::quiet_NaN();
     if (pj && pj->splice)
         for (uint32_t j = 0; j < pj->cnt[q]; j++)
             if (pj->doc[size_t(q) * pj->stride + j] == d) return std::numeric_limits<double>::quiet_NaN();
-    const SortOrder &o = sj.f->ord[sj.order];
-    const uint32_t r = d < sj.f->nbits ? o.h_doc_rank[d] : RANK_NONE;
+    const SortOrder &o = sj.ord(e);
+    const uint32_t r = d < sj.f[e]->nbits ? o.h_doc_rank[d] : RANK_NONE;
     return r == RANK_NONE ? std::numeric_limits<double>::quiet_NaN() : o.h_value[r];
 }
 // rank -> string row of snapshot S (kept until another snapshot is searched)
@@ -1848,7 +1868,8 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     QFilterJob qfj;
     bool per_q = false;
     if (p->q_filters) {
-        if (gj || pj || sj) return fail(OC_ERR_UNSUPPORTED, "q_filters: per-query filters are supported by oc_search only");
+        if (gj || ((pj || sj) && !(pj && pj->q_filters)))
+            return fail(OC_ERR_UNSUPPORTED, "q_filters: per-query filters are supported by oc_search and oc_search_q_sorted only");
         if (p->filter || p->filter_bits) return fail(OC_ERR_INVALID, "q_filters together with filter / filter_bits");
         if (p->sharded) return fail(OC_ERR_UNSUPPORTED, "q_filters over a sharded search");
         std::unordered_map<const oc_filter *, uint32_t> idx;
@@ -1881,7 +1902,12 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     const bool sort_flat = sj && write_hits;
     // sort_token_scores with sort_by: top_count keys in field order, twice as many for an active pinned query
     const uint32_t sort_top = sort_flat ? uint32_t((uint64_t(limit) + p->offset) * (pj->splice ? 2 : 1)) : 0u;
-    const uint64_t n_keep64 = (uint64_t(limit) + p->offset) * (pin_flat ? 2 : 1);
+    // oc_search_q_sorted: the queries in score order take K4's list, spliced as pin_flat does
+    bool score_active = false;
+    if (sort_flat && sj->by_score && pj->splice)
+        for (uint32_t q = 0; q < B; q++) score_active = score_active || (sj->q_ent[q] == SORT_BY_SCORE && pj->cnt[q] > 0);
+    const bool k4_top = pin_flat || (sort_flat && sj->by_score);   // K4 writes its top n_keep (offset 0) for a splice
+    const uint64_t n_keep64 = (uint64_t(limit) + p->offset) * (pin_flat || score_active ? 2 : 1);
     if (n_keep64 > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "limit+offset %llu > %u", (unsigned long long)n_keep64, OC_MAX_TOPK);
     const uint32_t n_keep = (uint32_t)n_keep64;
     // limit_hint = limit, NOT limit+offset (search.rs:330-336); vector_limit lets a multi-index caller keep that depth
@@ -2193,6 +2219,27 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     const size_t o_pdoc = pin_items ? pk.add(pj->doc.data(), pj->doc.size() * 8) : 0;
     const size_t o_ppos = pin_items ? pk.add(pj->pos.data(), pj->pos.size() * 4) : 0;
     const size_t o_pcnt = pin_items ? pk.add(pj->cnt.data(), pj->cnt.size() * 4) : 0;
+    // sortBy: the batch's entries and each query's entry and top_count (doubled for an active query)
+    std::vector<SortEntry> s_ents;
+    std::vector<SortQuery> s_q;
+    std::vector<uint8_t> s_alt;
+    if (sort_flat) {
+        const bool ft_map = has_ft && n_tiles > 0;
+        for (uint32_t e = 0; e < sj->f.size(); e++) {
+            const SortOrder &o = sj->ord(e);
+            s_ents.push_back(SortEntry{o.n, ft_map ? o.rank_row : nullptr, o.doc_rank, sj->f[e]->nbits, o.rank_doc});
+        }
+        s_q.resize(B);
+        s_alt.resize(B);
+        for (uint32_t q = 0; q < B; q++) {
+            const bool active = pj->splice && pj->cnt[q] > 0;
+            s_q[q] = SortQuery{sj->q_ent[q], uint32_t((uint64_t(limit) + p->offset) * (active ? 2 : 1))};
+            s_alt[q] = sj->q_ent[q] == SORT_BY_SCORE;
+        }
+    }
+    const size_t o_sent = sort_flat ? pk.add(s_ents.data(), s_ents.size() * sizeof(SortEntry)) : 0;
+    const size_t o_sq = sort_flat ? pk.add(s_q.data(), s_q.size() * sizeof(SortQuery)) : 0;
+    const size_t o_salt = sort_flat && sj->by_score ? pk.add(s_alt.data(), s_alt.size()) : 0;
     // hybrid: the descriptors, the shared-contribution precompute, the filter bitmap and the (term, tile) plan do
     // not depend on the vector results: they run on the side stream while the main stream sweeps the matrix
     // (OC_SIDE_STREAM=0 disables it: the step gets ~2.5 % longer, the sweep itself ~4 % shorter — A/B switch)
@@ -2378,6 +2425,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
             PointParams pp{};
             pp.terms = bp.terms; pp.tokens = bp.tokens; pp.queries = bp.queries;
             pp.n_queries = B; pp.v_stride = ps; pp.v_row = c->pin_row.as<uint32_t>(); pp.row_ok_bits = row_ok;
+            pp.q_ok_slot = per_q ? qfj.d_q_slot_ft : nullptr; pp.ok_words = uint64_t(n_tiles) * (BM25_TILE / 32);
             pp.k = p->bm25_k; pp.threshold = thr ? 1 : 0;
             pp.v_ft = c->pin_ft.as<float>(); pp.v_present = c->pin_ftp.as<uint8_t>();
             bm25_point_kernel<<<warp_grid, 256, 0, c->stream>>>(pp);
@@ -2412,9 +2460,8 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     // then paged with the pins spliced (pin_splice_kernel writes the hits over K4's)
     auto sort_tail = [&]() -> int {
         if (!sort_flat) return OC_OK;
-        SortOrder &so = sj->f->ord[sj->order];
-        const bool ft_map = has_ft && n_tiles > 0;
-        if (ft_map) OCTRY(sort_rows_for(c, so, snap));
+        if (has_ft && n_tiles > 0)
+            for (uint32_t e = 0; e < sj->f.size(); e++) OCTRY(sort_rows_for(c, sj->ord(e), snap));
         const uint32_t top = sort_top;
         const uint64_t nslot = uint64_t(B) * top;
         const uint32_t vs = std::max<uint32_t>(vlimit, 1);
@@ -2424,10 +2471,10 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         OCTRY(c->srt_score.ensure(nslot * 4));
         OCTRY(c->srt_present.ensure(nslot));
         SortWalkParams wp{};
-        wp.n_ranks = so.n; wp.rank_row = ft_map ? so.rank_row : nullptr; wp.doc_rank = so.doc_rank; wp.nbits = sj->f->nbits;
-        wp.mbits = ft_map ? c->mbits.as<uint32_t>() : nullptr; wp.row_words = uint64_t(n_tiles) * (BM25_TILE / 32);
+        wp.ents = reinterpret_cast<const SortEntry *>(din + o_sent); wp.q = reinterpret_cast<const SortQuery *>(din + o_sq);
+        wp.mbits = has_ft && n_tiles > 0 ? c->mbits.as<uint32_t>() : nullptr; wp.row_words = uint64_t(n_tiles) * (BM25_TILE / 32);
         wp.v_doc = fp.out_vdoc; wp.v_n = fp.out_vn; wp.v_stride = vs;
-        wp.rank_doc = so.rank_doc; wp.top = top;
+        wp.top = top;
         wp.out_doc = c->srt_doc.as<uint64_t>(); wp.out_row = c->srt_row.as<uint32_t>(); wp.out_n = c->srt_n.as<uint32_t>();
         sort_walk_kernel<<<B, SORT_THREADS, size_t(vs) * 4, c->stream>>>(wp);
         launched(c);
@@ -2438,6 +2485,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
             PointParams pp{};
             pp.terms = bp.terms; pp.tokens = bp.tokens; pp.queries = bp.queries;
             pp.n_queries = B; pp.v_stride = top; pp.v_row = c->srt_row.as<uint32_t>(); pp.row_ok_bits = row_ok;
+            pp.q_ok_slot = per_q ? qfj.d_q_slot_ft : nullptr; pp.ok_words = uint64_t(n_tiles) * (BM25_TILE / 32);
             pp.k = p->bm25_k; pp.threshold = thr ? 1 : 0;
             pp.v_ft = c->srt_ft.as<float>(); pp.v_present = c->srt_ftp.as<uint8_t>();
             bm25_point_kernel<<<warp_grid, 256, 0, c->stream>>>(pp);
@@ -2468,7 +2516,12 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         xp.top_doc = c->srt_doc.as<uint64_t>(); xp.top_score = c->srt_score.as<float>(); xp.top_n = c->srt_n.as<uint32_t>();
         xp.out_doc = reinterpret_cast<uint64_t *>(dout + o_doc); xp.out_score = reinterpret_cast<float *>(dout + o_sc);
         xp.out_n = reinterpret_cast<uint32_t *>(dout + o_n);
-        pin_splice_kernel<<<B, PIN_THREADS, pin_splice_smem(xp.kp2, top, limit + p->offset), c->stream>>>(xp);
+        if (sj->by_score) {   // the queries in score order splice K4's top n_keep
+            xp.q_alt = din + o_salt; xp.alt_n_top = n_keep;
+            xp.alt_doc = c->pin_top_doc.as<uint64_t>(); xp.alt_score = c->pin_top_score.as<float>(); xp.alt_n = c->pin_top_n.as<uint32_t>();
+        }
+        pin_splice_kernel<<<B, PIN_THREADS, pin_splice_smem(xp.kp2, sj->by_score ? std::max(top, n_keep) : top, limit + p->offset),
+                            c->stream>>>(xp);
         launched(c);
         CU(cudaGetLastError());
         return OC_OK;
@@ -2522,7 +2575,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     fp.out_doc = reinterpret_cast<uint64_t *>(dout + o_doc); fp.out_score = reinterpret_cast<float *>(dout + o_sc);
     fp.out_n = reinterpret_cast<uint32_t *>(dout + o_n); fp.out_count = reinterpret_cast<unsigned long long *>(dout + o_cnt);
     fp.out_min = reinterpret_cast<float *>(dout + o_min);
-    if (pin_flat) {   // K4 keeps its whole top n_keep for the splice, which writes the hits
+    if (k4_top) {   // K4 keeps its whole top n_keep for the splice, which writes the hits
         fp.limit = n_keep; fp.offset = 0;
         OCTRY(c->pin_top_doc.ensure(size_t(B) * n_keep * 8));
         OCTRY(c->pin_top_score.ensure(size_t(B) * n_keep * 4));
@@ -3106,7 +3159,7 @@ static int run_groups(oc_ctx *c, const GroupJob &gj, uint32_t B, int mode, const
     gp.v_stride = std::max<uint32_t>(vlimit, 1);
     gp.omc_doc = omc_doc; gp.omc_mult = omc_mult; gp.n_omc = n_omc;
     gp.out_doc = c->grp_doc.as<uint64_t>(); gp.out_score = c->grp_score.as<float>(); gp.out_n = c->grp_n.as<uint32_t>();
-    if (sj) { gp.doc_rank = sj->f->ord[sj->order].doc_rank; gp.rank_nbits = sj->f->nbits; }
+    if (sj) { gp.doc_rank = sj->ord(0).doc_rank; gp.rank_nbits = sj->f[0]->nbits; }
     const void *kern = sj ? (const void *)group_sort_topk_kernel : (const void *)group_topk_kernel;
     const size_t smem = (size_t(GROUP_BUF) + gp.kp2 + gp.vp2) * 8 + size_t(gp.vp2) * 4;
     if (smem_cfg_needed(c->device, kern, smem))
@@ -3265,7 +3318,7 @@ extern "C" int oc_search_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_se
                                 uint32_t *out_n, uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present) {
     if (!c || !p) return fail(OC_ERR_INVALID, "NULL argument");
     SortJob sj{};
-    OCTRY(sort_job_init(c, sort, sj));
+    OCTRY(sort_job_init(c, sort, p->n_queries, sj));
     sj.out_values = out_sort_values;
     PinJob pj;
     OCTRY(pin_job_init(pins, p->n_queries, pj));
@@ -3284,7 +3337,7 @@ extern "C" int oc_search_groups_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, oc_g
         return fail(OC_ERR_INVALID, "NULL group output");
     if (groups->ctx != c) return fail(OC_ERR_INVALID, "group_by belongs to another ctx");
     SortJob sj{};
-    OCTRY(sort_job_init(c, sort, sj));
+    OCTRY(sort_job_init(c, sort, p->n_queries, sj));
     sj.out_values = out_sort_values; sj.out_group_values = out_group_sort_values; sj.n_groups = groups->n_groups;
     if (max_results > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "max_results %u > %u", max_results, OC_MAX_TOPK);
     if (p->n_queries > 65535) return fail(OC_ERR_UNSUPPORTED, "groups: n_queries %u > 65535", p->n_queries);
@@ -3298,6 +3351,32 @@ extern "C" int oc_search_groups_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, oc_g
     GroupJob gj{groups, max_results, out_group_doc_ids, out_group_scores, out_group_n};
     gj.stride = group_stride;
     return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, &gj, &pj, pins, nullptr, nullptr, &sj);
+}
+
+// One batch in which every query has its own sort (or score order), its own pins and, with q_filters, its own filter:
+// query b gets what it gets alone through oc_search_sorted (a sort) or oc_search_pinned (score order, sort values NaN).
+extern "C" int oc_search_q_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, const oc_sort *q_sorts,
+                                  const oc_pins *pins, uint64_t *out_doc_ids, float *out_scores, double *out_sort_values,
+                                  uint32_t *out_n, uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present) {
+    if (!c || !p || !q_sorts) return fail(OC_ERR_INVALID, "NULL argument");
+    SortJob sj{};
+    for (uint32_t b = 0; b < p->n_queries; b++) OCTRY(sort_job_add(c, q_sorts[b], sj));
+    sj.out_values = out_sort_values;
+    PinJob pj;
+    pj.q_filters = true;
+    OCTRY(pin_job_init(pins, p->n_queries, pj));
+    OCTRY(pins_check_flat(p, pj));
+    if (!sj.f.empty())
+        return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, nullptr, &pj, pins, out_pin_scores,
+                           out_pin_present, &sj);
+    // every query in score order: oc_search_pinned
+    OCTRY(search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, nullptr, &pj, pins, out_pin_scores,
+                      out_pin_present));
+    if (out_sort_values)
+        for (uint32_t q = 0; q < p->n_queries; q++)
+            for (uint32_t i = 0; i < p->limit; i++)
+                out_sort_values[size_t(q) * p->limit + i] = i < out_n[q] ? std::numeric_limits<double>::quiet_NaN() : 0.0;
+    return OC_OK;
 }
 
 // ------------------------------------------------------------------------------------ geopoint where-filter leaves (geo.cuh)
@@ -3433,10 +3512,18 @@ struct OcSearchExec {
         return oc_search(c, e, s, p, docs, scores, n, count);
     }
 };
+struct OcSortedExec {
+    oc_ctx *c; oc_emb *e; oc_str *s;
+    int operator()(const oc_search_params *p, const oc_sort *q_sorts, const oc_pins *pins, uint64_t *docs, float *scores,
+                   double *sort_values, uint32_t *n, uint64_t *count, float *pin_scores, uint8_t *pin_present) const {
+        return oc_search_q_sorted(c, e, s, p, q_sorts, pins, docs, scores, sort_values, n, count, pin_scores, pin_present);
+    }
+};
 struct oc_batcher {
-    ocb::Batcher<OcSearchExec> q;
+    ocb::Batcher<OcSearchExec, OcSortedExec> q;
     oc_ctx *ctx;
-    oc_batcher(OcSearchExec x, uint32_t dim, uint32_t mb, uint32_t mw) : q(x, dim, mb, mw, x.e != nullptr, x.s != nullptr), ctx(x.c) {}
+    oc_batcher(OcSearchExec x, uint32_t dim, uint32_t mb, uint32_t mw)
+        : q(x, dim, mb, mw, x.e != nullptr, x.s != nullptr, OcSortedExec{x.c, x.e, x.s}), ctx(x.c) {}
 };
 extern "C" int oc_batcher_create(oc_ctx *c, oc_emb *emb, oc_str *str, uint32_t max_batch, uint32_t max_wait_us, oc_batcher **out) {
     if (!c || !out || (!emb && !str)) return fail(OC_ERR_INVALID, "bad arguments");
@@ -3456,6 +3543,22 @@ extern "C" int oc_batcher_search(oc_batcher *b, const oc_search_params *p, uint6
     const int rc = b->q.submit(p, out_doc_ids, out_scores, out_n, out_count);
     // the batch ran on its leader's thread: that is where oc_last_error() holds the detail
     if (rc != OC_OK && g_err[0] == 0) return fail(rc, "the coalesced oc_search of this query's batch failed (detail on the leading caller's thread)");
+    return rc;
+}
+extern "C" int oc_batcher_search_sorted(oc_batcher *b, const oc_search_params *p, const oc_sort *sort, const oc_pins *pins,
+                                        uint64_t *out_doc_ids, float *out_scores, double *out_sort_values, uint32_t *out_n,
+                                        uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present) {
+    if (!b || !p || !out_doc_ids || !out_scores || !out_n || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
+    if (p->n_queries != 1) return fail(OC_ERR_INVALID, "oc_batcher_search_sorted takes one query per call (n_queries = %u)", p->n_queries);
+    // what would fail a whole batch is refused here, before the request joins one
+    if (p->filter && p->filter->ctx != b->ctx) return fail(OC_ERR_INVALID, "filter belongs to another ctx");
+    if (sort && sort->field && sort->field->ctx != b->ctx) return fail(OC_ERR_INVALID, "sort field belongs to another ctx");
+    const char *why = nullptr;
+    if (const int rc = ocb::check_sorted(sort, pins, &why)) return fail(rc, "%s", why);
+    g_err[0] = 0;
+    const int rc = b->q.submit_sorted(p, sort, pins, out_doc_ids, out_scores, out_sort_values, out_n, out_count, out_pin_scores,
+                                      out_pin_present);
+    if (rc != OC_OK && g_err[0] == 0) return fail(rc, "the coalesced search of this query's batch failed (detail on the leading caller's thread)");
     return rc;
 }
 extern "C" int oc_batcher_stats(oc_batcher *b, uint64_t *n_queries, uint64_t *n_batches, uint64_t *n_direct) {

@@ -8,8 +8,8 @@
 //                           exported (FuseParams::out_vdoc / out_vscore), any other document the point lookup of its
 //                           string row (bm25_point_kernel: same bits, presence under filter, tombstones and threshold)
 //                           through fused_ft_score; a document that is not a key scores 0.0 and is "not present".
-//   pin_splice_kernel       one CTA per query over K4's top 2 * (limit + offset): remove the promoted ids, insert the
-//                           items stably sorted by position, then skip(offset).take(limit).
+//   pin_splice_kernel       one CTA per query over K4's top 2 * (limit + offset) (or, sorted, the walk's list): remove
+//                           the promoted ids, insert the items stably sorted by position, then skip(offset).take(limit).
 //   group_pin_splice_kernel one CTA per (group, query) over group_topk_kernel's top 2 * max_results: the same splice
 //                           with the items restricted to the group's members, not truncated afterwards.
 #pragma once
@@ -175,6 +175,12 @@ struct PinSpliceParams {
     uint64_t *out_doc;              // [q][limit]
     float *out_score;
     uint32_t *out_n;                // [q]
+    // oc_search_q_sorted: the queries in score order (q_alt[q] != 0) take K4's list (alt_*) instead of the walk's
+    const uint8_t *q_alt;           // [q], NULL: every query takes top_*
+    uint32_t alt_n_top;
+    const uint64_t *alt_doc;        // [q][alt_n_top]
+    const float *alt_score;
+    const uint32_t *alt_n;          // [q]
 };
 
 // one CTA per query: the flat hits of sort_token_scores with pins, then skip(offset).take(limit); a query without items
@@ -182,8 +188,13 @@ struct PinSpliceParams {
 __global__ void __launch_bounds__(PIN_THREADS) pin_splice_kernel(const PinSpliceParams p) {
     extern __shared__ __align__(16) uint8_t smem[];
     const uint32_t q = blockIdx.x;
-    const size_t it = size_t(q) * p.stride, tp = size_t(q) * p.n_top, o = size_t(q) * p.limit;
-    const uint32_t n = pin_splice_block(p.top_doc + tp, p.top_score + tp, p.top_n[q], p.doc + it, p.pos + it, p.score + it,
+    const bool alt = p.q_alt && p.q_alt[q];
+    const uint32_t n_top = alt ? p.alt_n_top : p.n_top;
+    const uint64_t *top_doc = alt ? p.alt_doc : p.top_doc;
+    const float *top_score = alt ? p.alt_score : p.top_score;
+    const uint32_t top_n = alt ? p.alt_n[q] : p.top_n[q];
+    const size_t it = size_t(q) * p.stride, tp = size_t(q) * n_top, o = size_t(q) * p.limit;
+    const uint32_t n = pin_splice_block(top_doc + tp, top_score + tp, top_n, p.doc + it, p.pos + it, p.score + it,
                                         p.cnt[q], p.kp2, [](uint32_t) { return true; }, p.offset, p.limit,
                                         p.out_doc + o, p.out_score + o, smem);
     for (uint32_t i = n + threadIdx.x; i < p.limit; i += blockDim.x) { p.out_doc[o + i] = 0; p.out_score[o + i] = 0.f; }

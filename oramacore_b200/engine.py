@@ -772,6 +772,37 @@ def search_sorted(tsc: "TokenScoreContext", params: "TokenScoreParams", field: S
     return [SearchHits(docs[i, :n[i]].copy(), scores[i, :n[i]].copy(), int(cnt[i])) for i in range(docs.shape[0])]
 
 
+def _q_sorts(sorts, B: int):
+    """oc_sort[B] from `sorts`: per query a (SortField, order) pair, or None for score order."""
+    if len(sorts) != B:
+        raise ValueError(f"sorts has {len(sorts)} entries for {B} queries")
+    arr = (_lib.Sort * max(B, 1))()
+    for i, s in enumerate(sorts):
+        if s is not None:
+            arr[i] = _sort(s[0], s[1])
+    return arr
+
+
+def search_q_sorted_arrays(tsc: "TokenScoreContext", params: "TokenScoreParams", sorts, promote=None, texts=None,
+                           q_vecs: Optional[np.ndarray] = None):
+    """oc_search_q_sorted: one batch in which every query has its own sort and pin rules, and (params.device_filters)
+    its own where-filter.  `sorts[b]`: a (SortField, order) pair, or None for score order; `promote` as in
+    search_pinned_arrays.  Query b gets what search_sorted_arrays (a sort) or search_pinned_arrays (None; sort values
+    NaN) give it alone.  Returns what search_sorted_arrays returns."""
+    sp, keep, B = tsc._build_params(params, texts, q_vecs)
+    srt = _q_sorts(sorts, B)
+    pins = None if promote is None else _pins(promote, B)[0]
+    n_items = 0 if pins is None else int(pins._keep[0][-1])
+    L = params.limit_hint
+    docs, scores, sv = np.zeros((B, L), np.uint64), np.zeros((B, L), np.float32), np.zeros((B, L), np.float64)
+    n, cnt = np.zeros(B, np.uint32), np.zeros(B, np.uint64)
+    ps, pp = np.zeros(max(n_items, 1), np.float32), np.zeros(max(n_items, 1), np.uint8)
+    check(lib().oc_search_q_sorted(tsc.ctx._h, tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None, C.byref(sp),
+                                   srt, None if pins is None else C.byref(pins), _p(docs), _p(scores), _p(sv), _p(n),
+                                   _p(cnt), _p(ps), _p(pp)))
+    return docs, scores, sv, n, cnt, ps[:n_items], pp[:n_items]
+
+
 def merge_index_results_sorted(per_index, order: str, limit: int, offset: int = 0, promote=None, apply: bool = True):
     """The multi-index union in field order (oc_merge_sorted, host; MergeSortedIterator, read/sort.rs:491-559):
     per_index = one (doc_ids [B, limit'], scores, sort values, n, count[, pin scores, pin present]) tuple per index, each
@@ -1051,6 +1082,28 @@ class SearchBatcher:
         check(lib().oc_batcher_search(self._h, C.byref(sp), _p(docs), _p(scores), _p(n), _p(cnt)))
         k = int(n[0])
         return SearchHits(docs[:k].copy(), scores[:k].copy(), int(cnt[0]))
+
+    def search_sorted(self, params: TokenScoreParams, sort=None, promote=None, text: Optional[TextQuery] = None,
+                      q_vec: Optional[np.ndarray] = None):
+        """One query with its own sortBy (a (SortField, order) pair, None: score order) and pin rules (`promote`: its
+        promote items, None: no rule), coalesced with concurrent search() / search_sorted() calls.  Returns
+        (SearchHits, sort values [n], pin scores [items], pin present [items]) as search_q_sorted_arrays gives them for
+        this query alone."""
+        sp, keep, B = self.tsc._build_params(params, None if text is None else [text],
+                                             None if q_vec is None else np.asarray(q_vec, np.float32).reshape(1, -1))
+        assert B == 1
+        srt = None if sort is None else _sort(sort[0], sort[1])
+        pins = None if promote is None else _pins([promote], 1)[0]
+        n_items = 0 if pins is None else int(pins._keep[0][-1])
+        L = params.limit_hint
+        docs, scores, sv = np.zeros(L, np.uint64), np.zeros(L, np.float32), np.zeros(L, np.float64)
+        n, cnt = np.zeros(1, np.uint32), np.zeros(1, np.uint64)
+        ps, pp = np.zeros(max(n_items, 1), np.float32), np.zeros(max(n_items, 1), np.uint8)
+        check(lib().oc_batcher_search_sorted(self._h, C.byref(sp), None if srt is None else C.byref(srt),
+                                             None if pins is None else C.byref(pins), _p(docs), _p(scores), _p(sv), _p(n),
+                                             _p(cnt), _p(ps), _p(pp)))
+        k = int(n[0])
+        return SearchHits(docs[:k].copy(), scores[:k].copy(), int(cnt[0])), sv[:k].copy(), ps[:n_items], pp[:n_items]
 
     def stats(self) -> dict:
         q, b, d = C.c_uint64(), C.c_uint64(), C.c_uint64()

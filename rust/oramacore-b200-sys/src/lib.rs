@@ -130,6 +130,10 @@ extern "C" {
     pub fn oc_batcher_destroy(b: *mut OcBatcher);
     pub fn oc_batcher_search(b: *mut OcBatcher, p: *const OcSearchParams, out_doc_ids: *mut u64, out_scores: *mut f32,
                              out_n: *mut u32, out_count: *mut u64) -> c_int;
+    /// one query with its own sort (NULL: score order) and pin items, coalesced with oc_batcher_search calls
+    pub fn oc_batcher_search_sorted(b: *mut OcBatcher, p: *const OcSearchParams, sort: *const OcSort, pins: *const OcPins,
+                                    out_doc_ids: *mut u64, out_scores: *mut f32, out_sort_values: *mut f64, out_n: *mut u32,
+                                    out_count: *mut u64, out_pin_scores: *mut f32, out_pin_present: *mut u8) -> c_int;
     pub fn oc_batcher_stats(b: *mut OcBatcher, n_queries: *mut u64, n_batches: *mut u64, n_direct: *mut u64) -> c_int;
     pub fn oc_pinned_free(p: *mut c_void);
     pub fn oc_search(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, p: *const OcSearchParams,
@@ -196,6 +200,10 @@ extern "C" {
     pub fn oc_search_sorted(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, p: *const OcSearchParams, sort: *const OcSort,
                             pins: *const OcPins, out_doc_ids: *mut u64, out_scores: *mut f32, out_sort_values: *mut f64,
                             out_n: *mut u32, out_count: *mut u64, out_pin_scores: *mut f32, out_pin_present: *mut u8) -> c_int;
+    /// per query its own sort (q_sorts[b].field NULL: score order), pins and (q_filters) where-filter
+    pub fn oc_search_q_sorted(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, p: *const OcSearchParams, q_sorts: *const OcSort,
+                              pins: *const OcPins, out_doc_ids: *mut u64, out_scores: *mut f32, out_sort_values: *mut f64,
+                              out_n: *mut u32, out_count: *mut u64, out_pin_scores: *mut f32, out_pin_present: *mut u8) -> c_int;
     pub fn oc_search_groups_sorted(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, g: *mut OcGroupBy, p: *const OcSearchParams,
                                    max_results: u32, sort: *const OcSort, pins: *const OcPins, group_stride: u32,
                                    out_doc_ids: *mut u64, out_scores: *mut f32, out_sort_values: *mut f64, out_n: *mut u32,
