@@ -86,7 +86,11 @@ int oc_comm_p2p_import(oc_ctx *ctx, const uint8_t *handles);
 
 /* ---- embedding store ------------------------------------------------------------------
  * EmbeddingFieldStorage::new (embedding_field.rs:64-78): metric fixed = cosine;
- * rescale_e5 = Model::rescale_score for the E5 family (python/embeddings.rs:71-92). */
+ * rescale_e5 = Model::rescale_score for the E5 family (python/embeddings.rs:71-92).
+ * An OC_DTYPE_F32 store also keeps an fp16 copy of its rows (each row scaled by a power of two), the operand of the
+ * batched tensor-core sweep: 6 B per element in all instead of 4.  Scores are still exact fp32 arithmetic on the
+ * stored rows.  OC_EMB_F16=0 in the environment at creation keeps no copy (the sweep then reads the fp32 rows through
+ * tf32); if the copy cannot be allocated, the store drops it and is served the same way. */
 int oc_emb_create(oc_ctx *ctx, uint32_t dim, int dtype, int rescale_e5, oc_emb **out);
 void oc_emb_destroy(oc_emb *emb);
 int oc_emb_reserve(oc_emb *emb, uint64_t n_rows);
@@ -102,7 +106,7 @@ typedef struct {
     uint64_t num_rows;        /* incl. tombstones */
     uint32_t dimensions;
     int dtype;
-    uint64_t device_bytes;
+    uint64_t device_bytes;    /* rows, inverse norms, doc ids, and the fp16 copy with its row scales when kept */
 } oc_emb_info_t;
 int oc_emb_info(oc_emb *emb, oc_emb_info_t *out);
 
@@ -602,7 +606,7 @@ typedef struct {
     uint64_t scan_bytes;     /* algorithmic bytes swept by the scan kernels (rows x stride x elem) */
     uint64_t bm25_postings;  /* postings walked by the scorer (x8 B = algorithmic bytes)    */
     uint64_t h2d_bytes, d2h_bytes;
-    uint32_t scan_tensor_core;   /* 1 => the batched wgmma (tf32/bf16 select + exact re-score) scan ran */
+    uint32_t scan_tensor_core;   /* 1 => the batched wgmma (fp16/tf32/bf16 select + exact re-score) scan ran */
     uint32_t scan_unproven;      /* queries whose candidate buffers overflowed in the tensor-core scan and were
                                     re-run through the exact sweep (device_ms includes that re-run)     */
     uint32_t scan_variant;       /* OC_SCAN_*: which sweep kernel served the batch                      */
@@ -613,6 +617,7 @@ typedef struct {
 #define OC_SCAN_EXACT 0          /* emb_scan_kernel: exact fp32 sweep (B < 8, limit > 32, tiny stores)          */
 #define OC_SCAN_TC_TF32 1        /* emb_gemm_kernel: wgmma .tf32 on the fp32 rows, one CTA per SM and query group */
 #define OC_SCAN_TC_BF16 4        /* emb_gemm_kernel on a bf16 store (wgmma .bf16)                                */
+#define OC_SCAN_TC_F16 5         /* emb_gemm_kernel: wgmma .f16 on the fp16 copy of an fp32 store (OC_EMB_F16=0: tf32) */
 int oc_last_timing(oc_ctx *ctx, oc_timing *out);
 /* Total kernels this library has launched on ctx since oc_init. */
 uint64_t oc_launch_count(oc_ctx *ctx);

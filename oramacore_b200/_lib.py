@@ -21,6 +21,11 @@ OC_GEO_EARTH_RADIUS_M = 6371000.0
 OC_GEO_MAX_VERTICES = 2048
 OC_RANGE_LO_OPEN = 1
 OC_RANGE_HI_OPEN = 2
+# Timing.scan_variant: which embedding sweep served the last batch (include/oramacore_b200.h OC_SCAN_*)
+OC_SCAN_EXACT = 0
+OC_SCAN_TC_TF32 = 1
+OC_SCAN_TC_BF16 = 4
+OC_SCAN_TC_F16 = 5   # wgmma .f16 on the fp16 copy of an fp32 store; OC_EMB_F16=0 selects OC_SCAN_TC_TF32
 
 EXPORTED_SYMBOLS = [
     "oc_last_error", "oc_version", "oc_abi_sizes", "oc_init", "oc_shutdown", "oc_device_info", "oc_comm_unique_id",

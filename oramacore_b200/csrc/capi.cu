@@ -161,7 +161,7 @@ struct oc_ctx {
     DevBuf row_ft, grp_vdoc, grp_vscore, grp_vn, grp_gmin, grp_den, grp_doc, grp_score, grp_n;   // oc_search_groups
     DevBuf pin_row, pin_ft, pin_ftp, pin_score, pin_present, pin_top_doc, pin_top_score, pin_top_n, pin_gdoc, pin_gscore, pin_gn;   // pins
     DevBuf srt_doc, srt_row, srt_n, srt_ft, srt_ftp, srt_score, srt_present, srt_zero;   // sortBy
-    DevBuf q_bf16, q_rho, pre_post, dense_buf, g_thr, g_eps, g_ovf, g_ovfcnt, g_resc, g_cand, g_cnt, g_flag, g_max, r_qpad, r_qinv, r_map, r_doc, r_score, r_row, r_cnt, r_raw;
+    DevBuf q_bf16, q_f16, q_scale, q_rho, pre_post, dense_buf, g_thr, g_eps, g_ovf, g_ovfcnt, g_resc, g_cand, g_cnt, g_flag, g_max, r_qpad, r_qinv, r_map, r_doc, r_score, r_row, r_cnt, r_raw;
     // per-query where-filters (q_filters): the embedding rows' bitmap of every distinct handle, and the slots of the
     // queries the exact sweep re-runs; v_qslot / v_rowbits describe the vector stage of the current call (fix_unproven)
     DevBuf e_rowbits, r_slot;
@@ -219,7 +219,7 @@ extern "C" void oc_shutdown(oc_ctx *c) {
     DevBuf *bufs[] = {&c->in_blob, &c->q_pad, &c->q_inv, &c->eff_norm, &c->filter_dev, &c->scan_cand, &c->v_doc,
                       &c->v_score, &c->v_row, &c->v_cnt, &c->v_srow, &c->v_ft, &c->v_present, &c->v_raw, &c->seg, &c->df_dev,
                       &c->row_ok, &c->tau, &c->cand_key, &c->cand_ft, &c->cand_cnt, &c->tile_cnt, &c->tile_max,
-                      &c->tile_min, &c->min_hint, &c->out_blob, &c->shard_send, &c->shard_recv, &c->work_ctr, &c->flat_desc, &c->mbits, &c->dbits, &c->facet_req, &c->facet_out, &c->q_bf16, &c->q_rho, &c->pre_post, &c->dense_buf, &c->g_thr, &c->g_eps, &c->g_ovf, &c->g_ovfcnt, &c->g_resc, &c->g_cand, &c->g_cnt, &c->g_max,
+                      &c->tile_min, &c->min_hint, &c->out_blob, &c->shard_send, &c->shard_recv, &c->work_ctr, &c->flat_desc, &c->mbits, &c->dbits, &c->facet_req, &c->facet_out, &c->q_bf16, &c->q_f16, &c->q_scale, &c->q_rho, &c->pre_post, &c->dense_buf, &c->g_thr, &c->g_eps, &c->g_ovf, &c->g_ovfcnt, &c->g_resc, &c->g_cand, &c->g_cnt, &c->g_max,
                       &c->g_flag, &c->r_qpad, &c->r_qinv, &c->r_map, &c->r_doc, &c->r_score, &c->r_row, &c->r_cnt, &c->r_raw,
                       &c->row_ft, &c->grp_vdoc, &c->grp_vscore, &c->grp_vn, &c->grp_gmin, &c->grp_den, &c->grp_doc, &c->grp_score, &c->grp_n,
                       &c->pin_row, &c->pin_ft, &c->pin_ftp, &c->pin_score, &c->pin_present, &c->pin_top_doc, &c->pin_top_score,
@@ -321,9 +321,21 @@ struct oc_emb {
     uint32_t esz = 4;            // element bytes
     float *inv_norm = nullptr;   // [cap] (NaN = tombstone)
     uint64_t *row_doc = nullptr; // [cap]
+    // fp32 stores: the operand of the fp16 tensor-core sweep (emb_gemm.cuh, GEMM_F16).  f16 is false for bf16 stores,
+    // when OC_EMB_F16=0 at creation, and from the first time the copy could not be allocated on (the store is then
+    // swept through tf32)
+    bool f16 = false;
+    uint16_t *rows_f16 = nullptr; // [cap][stride] each row times 2^s, s putting its largest |x_i| in [2^14, 2^15)
+    float *row_scale = nullptr;   // [cap] 2^-s (NaN: a non-finite element)
     uint64_t n_rows = 0, cap = 0, n_live = 0;
     std::unordered_multimap<uint64_t, uint64_t> doc_rows;  // doc -> rows (for delete)
 };
+
+// OC_EMB_F16=0: no fp16 copy for stores created while it is set, and searches use the tf32 sweep (A/B testing)
+static bool env_emb_f16_off() {
+    const char *v = getenv("OC_EMB_F16");
+    return v && v[0] == '0';
+}
 
 extern "C" int oc_emb_create(oc_ctx *c, uint32_t dim, int dtype, int rescale_e5, oc_emb **out) {
     if (!c || !out) return fail(OC_ERR_INVALID, "NULL argument");
@@ -332,6 +344,7 @@ extern "C" int oc_emb_create(oc_ctx *c, uint32_t dim, int dtype, int rescale_e5,
     oc_emb *e = new oc_emb();
     e->ctx = c; e->dim = dim; e->dtype = dtype; e->e5 = rescale_e5 ? 1 : 0;
     e->esz = dtype == OC_DTYPE_BF16 ? 2 : 4;
+    e->f16 = dtype == OC_DTYPE_F32 && !env_emb_f16_off();
     e->stride = ((dim + 127) / 128) * 128;
     if (e->stride / 128 == 5 || e->stride / 128 == 7) e->stride += 128;  // instantiated widths: 1,2,3,4,6,8
     *out = e;
@@ -343,6 +356,7 @@ extern "C" void oc_emb_destroy(oc_emb *e) {
     cudaSetDevice(e->ctx->device);
     cudaStreamSynchronize(e->ctx->stream);
     cudaFree(e->rows); cudaFree(e->inv_norm); cudaFree(e->row_doc);
+    cudaFree(e->rows_f16); cudaFree(e->row_scale);
     delete e;
 }
 
@@ -355,14 +369,30 @@ static int emb_grow(oc_emb *e, uint64_t want_rows) {
     CU(cudaMalloc(&nr, ncap * e->stride * e->esz));
     CU(cudaMalloc(&nn, (ncap + 64) * sizeof(float)));
     CU(cudaMalloc(&nd, ncap * sizeof(uint64_t)));
+    uint16_t *nh = nullptr; float *ns = nullptr;
+    if (e->f16 && (cudaMalloc(&nh, ncap * e->stride * 2) != cudaSuccess || cudaMalloc(&ns, ncap * sizeof(float)) != cudaSuccess)) {
+        // no room for the fp16 copy: the store stays whole and is swept through tf32 from now on
+        (void)cudaGetLastError();
+        cudaFree(nh); cudaFree(ns); nh = nullptr; ns = nullptr;
+        cudaFree(e->rows_f16); cudaFree(e->row_scale); e->rows_f16 = nullptr; e->row_scale = nullptr;
+        e->f16 = false;
+    }
     if (e->n_rows) {
         CU(cudaMemcpyAsync(nr, e->rows, e->n_rows * e->stride * e->esz, cudaMemcpyDeviceToDevice, c->stream));
         CU(cudaMemcpyAsync(nn, e->inv_norm, e->n_rows * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
         CU(cudaMemcpyAsync(nd, e->row_doc, e->n_rows * sizeof(uint64_t), cudaMemcpyDeviceToDevice, c->stream));
+        if (nh) {
+            CU(cudaMemcpyAsync(nh, e->rows_f16, e->n_rows * e->stride * 2, cudaMemcpyDeviceToDevice, c->stream));
+            CU(cudaMemcpyAsync(ns, e->row_scale, e->n_rows * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
+        }
     }
     CU(cudaStreamSynchronize(c->stream));
     cudaFree(e->rows); cudaFree(e->inv_norm); cudaFree(e->row_doc);
     e->rows = nr; e->inv_norm = nn; e->row_doc = nd; e->cap = ncap;
+    if (nh) {
+        cudaFree(e->rows_f16); cudaFree(e->row_scale);
+        e->rows_f16 = nh; e->row_scale = ns;
+    }
     return OC_OK;
 }
 
@@ -391,6 +421,11 @@ extern "C" int oc_emb_insert(oc_emb *e, const uint64_t *doc_ids, const void *row
     if (e->esz == 2) emb_inv_norm_kernel<bf16_t><<<(unsigned)blocks, 256, 0, c->stream>>>(e->rows, e->stride, e->n_rows, e->n_rows + n, e->inv_norm);
     else emb_inv_norm_kernel<float><<<(unsigned)blocks, 256, 0, c->stream>>>(e->rows, e->stride, e->n_rows, e->n_rows + n, e->inv_norm);
     launched(c);
+    if (e->f16) {
+        emb_f16_rows_kernel<<<(unsigned)blocks, 256, 0, c->stream>>>(static_cast<const float *>(e->rows), e->stride, e->n_rows,
+                                                                     e->n_rows + n, e->rows_f16, e->row_scale);
+        launched(c);
+    }
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(c->stream));
     for (uint64_t i = 0; i < n; i++) e->doc_rows.emplace(doc_ids[i], e->n_rows + i);
@@ -429,6 +464,7 @@ extern "C" int oc_emb_info(oc_emb *e, oc_emb_info_t *out) {
     if (!e || !out) return fail(OC_ERR_INVALID, "NULL argument");
     out->num_embeddings = e->n_live; out->num_rows = e->n_rows; out->dimensions = e->dim; out->dtype = e->dtype;
     out->device_bytes = e->cap * (uint64_t(e->stride) * e->esz + 4 + 8);
+    if (e->f16) out->device_bytes += e->cap * (uint64_t(e->stride) * 2 + 4);
     return OC_OK;
 }
 
@@ -525,8 +561,8 @@ static int run_exact_sweeps(oc_ctx *c, oc_emb *e, const float *inv_norm, const f
 }
 
 // ---- TMA descriptors (tmap.cuh)
-static int tmap_2d(CUtensorMap *m, const void *base, uint64_t n_rows, uint32_t stride, uint32_t box_rows, bool bf16) {
-    const TmapStatus s = make_tmap_2d(m, base, n_rows, stride, box_rows, bf16);
+static int tmap_2d(CUtensorMap *m, const void *base, uint64_t n_rows, uint32_t stride, uint32_t box_rows, int op) {
+    const TmapStatus s = make_tmap_2d(m, base, n_rows, stride, box_rows, op);
     if (s.what) return fail(OC_ERR_CUDA, "%s failed: %d", s.what, s.code);
     return OC_OK;
 }
@@ -605,10 +641,16 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
 
     // ---------------- K2: wgmma batched scan ----------------
     const bool bf16 = e->esz == 2;
-    const void *sweep_fn = bf16 ? (const void *)emb_gemm_kernel<true> : (const void *)emb_gemm_kernel<false>;
-    if (smem_cfg_needed(c->device, (const void *)emb_gemm_kernel<false>, gemm_smem_bytes())) {   // all sweep kernels at once
-        CU(cudaFuncSetAttribute(emb_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes()));
-        CU(cudaFuncSetAttribute(emb_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes()));
+    // an fp32 store is swept through its fp16 copy when it has one (GEMM_F16), else through tf32 on the fp32 rows
+    const bool f16 = !bf16 && e->f16 && !env_emb_f16_off();
+    const int op = bf16 ? GEMM_BF16 : f16 ? GEMM_F16 : GEMM_TF32;
+    const void *sweep_fn = bf16  ? (const void *)emb_gemm_kernel<GEMM_BF16>
+                           : f16 ? (const void *)emb_gemm_kernel<GEMM_F16>
+                                 : (const void *)emb_gemm_kernel<GEMM_TF32>;
+    if (smem_cfg_needed(c->device, (const void *)emb_gemm_kernel<GEMM_TF32>, gemm_smem_bytes())) {   // all sweep kernels at once
+        CU(cudaFuncSetAttribute(emb_gemm_kernel<GEMM_TF32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes()));
+        CU(cudaFuncSetAttribute(emb_gemm_kernel<GEMM_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes()));
+        CU(cudaFuncSetAttribute(emb_gemm_kernel<GEMM_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes()));
         CU(cudaFuncSetAttribute(emb_gemm_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_merge_smem_bytes()));
     }
     // an even number of query groups runs in CTA pairs that share every row tile (emb_gemm.cuh)
@@ -653,9 +695,17 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
         f32_to_bf16_kernel<<<(unsigned)((nq_el + 255) / 256), 256, 0, c->stream>>>(c->q_pad.as<float>(), c->q_bf16.as<uint16_t>(), nq_el);
         launched(c);
         q_operand = c->q_bf16.p;
+    } else if (f16) {   // power-of-two scaled fp16 query; its scale turns eps into the sweep's units (gemm_thr_kernel)
+        OCTRY(c->q_f16.ensure(size_t(Bpad) * e->stride * 2));
+        OCTRY(c->q_scale.ensure(size_t(Bpad) * 4));
+        emb_f16_queries_kernel<<<(Bpad + 7) / 8, 256, 0, c->stream>>>(c->q_pad.as<float>(), e->stride, Bpad, c->q_f16.as<uint16_t>(),
+                                                                      c->q_scale.as<float>());
+        launched(c);
+        q_operand = c->q_f16.p;
     }
-    OCTRY(tmap_2d(&tm_q, q_operand, Bpad, e->stride, GEMM_M, bf16));
-    OCTRY(tmap_2d(&tm_x, e->rows, e->n_rows, e->stride, GEMM_N / (paired ? GEMM_CLUSTER : 1), bf16));   // a CTA's share of a tile
+    OCTRY(tmap_2d(&tm_q, q_operand, Bpad, e->stride, GEMM_M, op));
+    OCTRY(tmap_2d(&tm_x, f16 ? (const void *)e->rows_f16 : e->rows, e->n_rows, e->stride, GEMM_N / (paired ? GEMM_CLUSTER : 1),
+                  op));   // a CTA's share of a tile
     OCTRY(c->g_thr.ensure(size_t(B) * 4));
     OCTRY(c->g_eps.ensure(size_t(B) * 4));
     OCTRY(c->g_cand.ensure(size_t(Bpad) * lists * cap * 8));
@@ -666,15 +716,21 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
     OCTRY(c->g_flag.ensure(B));
     OCTRY(c->g_max.ensure(size_t(Bpad) * lists * 4));
     GemmParams gp{};
-    gp.n_rows = e->n_rows; gp.n_kblocks = e->stride / (bf16 ? 2 * GEMM_KB : GEMM_KB); gp.inv_norm = inv_norm; gp.n_queries = B;
+    gp.n_rows = e->n_rows; gp.n_kblocks = e->stride / (op == GEMM_TF32 ? GEMM_KB : 2 * GEMM_KB); gp.inv_norm = inv_norm; gp.n_queries = B;
     gp.n_qgroups = n_qgroups; gp.ctas_per_group = cpg; gp.cap = cap; gp.lists_per_query = lists;
     gp.thr = c->g_thr.as<unsigned int>(); gp.eps_v = c->g_eps.as<float>(); gp.limit = limit; gp.cand = c->g_cand.as<uint64_t>(); gp.cand_cnt = c->g_cnt.as<uint32_t>();
     gp.gmax = c->g_max.as<float>();
     gp.ovf = c->g_ovf.as<uint64_t>(); gp.ovf_cnt = c->g_ovfcnt.as<uint32_t>(); gp.ovf_cap = GEMM_OVF_CAP;
     if (qf) { gp.row_bits = row_bits; gp.row_words = row_words; gp.q_slot = qf->d_q_slot; }
     auto launch_gemm = [&]() -> int {
-        if (bf16) CU(cudaLaunchKernelEx(&cfg, emb_gemm_kernel<true>, tm_q, tm_x, gp));
-        else CU(cudaLaunchKernelEx(&cfg, emb_gemm_kernel<false>, tm_q, tm_x, gp));
+        if (bf16) CU(cudaLaunchKernelEx(&cfg, emb_gemm_kernel<GEMM_BF16>, tm_q, tm_x, gp));
+        else if (f16) {
+            GemmF16Params fp{};
+            static_cast<GemmParams &>(fp) = gp;
+            fp.row_scale = e->row_scale;
+            CU(cudaLaunchKernelEx(&cfg, emb_gemm_kernel<GEMM_F16>, tm_q, tm_x, fp));
+        }
+        else CU(cudaLaunchKernelEx(&cfg, emb_gemm_kernel<GEMM_TF32>, tm_q, tm_x, gp));
         launched(c, gp.max_mode == 0);   // the one-tile threshold pass is not counted as a sweep
         CU(cudaGetLastError());
         return OC_OK;
@@ -684,8 +740,9 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
     OCTRY(launch_gemm());
     GemmThrParams tp{};
     tp.gmax = c->g_max.as<float>(); tp.lists = lists; tp.limit = limit; tp.inv_qnorm = c->q_inv.as<float>();
-    tp.eps_const = bf16 ? GEMM_EPS_ACC : GEMM_EPS_TF32;
+    tp.eps_const = bf16 ? GEMM_EPS_ACC : f16 ? GEMM_EPS_F16 : GEMM_EPS_TF32;
     tp.rho_q = bf16 ? c->q_rho.as<float>() : nullptr;             // bf16 store: the rows are exact, the query is rounded
+    tp.q_scale = f16 ? c->q_scale.as<float>() : nullptr;
     tp.thr = c->g_thr.as<unsigned int>(); tp.eps_v = c->g_eps.as<float>(); tp.ovf_cnt = c->g_ovfcnt.as<uint32_t>();
     gemm_thr_kernel<<<B, 256, 0, c->stream>>>(tp);
     launched(c);
@@ -695,7 +752,8 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
     OCTRY(launch_gemm());
     CU(cudaEventRecord(c->ev[EV_SWEEP1], c->stream));
     c->sweep_timed = true;
-    c->timing.scan_bytes += e->n_rows * (uint64_t(e->stride) * e->esz + 4);
+    // the fp16 sweep reads the copy, the inverse norms and the row scales
+    c->timing.scan_bytes += f16 ? e->n_rows * (uint64_t(e->stride) * 2 + 4 + 4) : e->n_rows * (uint64_t(e->stride) * e->esz + 4);
     CU(cudaEventRecord(c->ev[EV_SCAN1], c->stream));
     GemmMergeParams mp{};
     mp.cand = gp.cand; mp.cand_cnt = gp.cand_cnt; mp.n_lists = lists; mp.cap = cap; mp.limit = limit;
@@ -710,7 +768,7 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
     // the overflow flags travel back with the results; oc_*search re-runs flagged queries (fix_unproven)
     c->gemm_pending = true; c->gemm_inv_norm = inv_norm;
     c->timing.scan_tensor_core = 1;
-    c->timing.scan_variant = bf16 ? OC_SCAN_TC_BF16 : OC_SCAN_TC_TF32;
+    c->timing.scan_variant = bf16 ? OC_SCAN_TC_BF16 : f16 ? OC_SCAN_TC_F16 : OC_SCAN_TC_TF32;
     return OC_OK;
 }
 

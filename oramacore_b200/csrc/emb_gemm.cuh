@@ -5,9 +5,11 @@
 // S[q][r] = sum_k Q[q][k] * X[r][k] (north_star: "tensor cores used only when batched
 // queries make the distance a true dense GEMM").  One matrix sweep serves the whole batch.
 //
-//   * operands: fp32 rows straight from HBM, consumed by wgmma .tf32 (the tensor core reads the
-//     fp32 bits and drops the low 13 mantissa bits) — no converted copy of the store, algorithmic
-//     bytes = n_rows * stride * 4 per batch; bf16 stores use wgmma .bf16;
+//   * operands (GemmOp): an fp32 store is swept through its fp16 copy (oc_emb.rows_f16: every row scaled by a power of
+//     two that puts its largest |x_i| in [2^14, 2^15), then rounded to nearest; the scale comes back exactly with the
+//     row's inverse norm) with wgmma .f16, algorithmic bytes = n_rows * (stride * 2 + 8) per batch; without the copy
+//     (OC_EMB_F16=0) the fp32 rows are read straight from HBM by wgmma .tf32 (the tensor core drops the low 13
+//     mantissa bits), n_rows * (stride * 4 + 4); bf16 stores use wgmma .bf16;
 //   * CTA tile: M = 128 queries (A operand, two consumer warpgroups of 64) x N = 256 rows (B operand),
 //     K-blocks of 128 bytes = one swizzle row; one producer warp fills a 4-stage shared-memory ring
 //     with TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B) under full / empty mbarriers, each consumer
@@ -32,10 +34,11 @@
 //     when the limit-th exact score clears bound + eps the exact top-`limit` is inside the
 //     candidate set.  Queries that fail the proof are re-run through the exact K1 sweep by the
 //     host (rare).
-//   * kernels in this file: emb_gemm_kernel<BF16>, gemm_thr_kernel, emb_gemm_merge_kernel.  emb_gemm_kernel<BF16, true>
+//   * kernels in this file: emb_gemm_kernel<OP>, gemm_thr_kernel, emb_gemm_merge_kernel.  emb_gemm_kernel<OP, true>
 //     (score dump) is instantiated only by the kernel test harness (tests/kernels).
 #pragma once
 #include <cuda.h>
+#include <cuda_fp16.h>
 
 #include "emb_scan.cuh"
 
@@ -49,7 +52,7 @@ constexpr int GEMM_THREADS = (GEMM_CONSUMER_WG + 1) * 128;
 constexpr uint32_t GEMM_PRODUCER_REGS = 40, GEMM_CONSUMER_REGS = 232;
 constexpr uint32_t GEMM_M = 128;       // queries per CTA
 constexpr uint32_t GEMM_N = 256;       // rows per tile
-constexpr uint32_t GEMM_KB = 32;       // fp32 elements per K-block (one 128 B swizzle row); bf16 rows: 64
+constexpr uint32_t GEMM_KB = 32;       // fp32 elements per K-block (one 128 B swizzle row); bf16 / fp16 rows: 64
 constexpr uint32_t GEMM_STAGES = 4;
 constexpr uint32_t GEMM_CLUSTER = 2;   // CTAs of a paired launch (two query groups sharing each row tile)
 constexpr uint32_t GEMM_A_BYTES = GEMM_M * 128;   // 16 KB
@@ -71,13 +74,26 @@ constexpr uint32_t GEMM_MAX_LIMIT = 128;          // largest `limit` the tensor-
 //   bf16 store: the rows are exact bf16 values (rho_x = 0); the query is rounded to bf16 (unit roundoff 2^-8):
 //         the worst case 2^-8 is ~2.4x the actual residual norm of a rounded vector, so the MEASURED residual
 //         rho_q per query (emb_prep_queries_kernel) is used, capped at the worst case.
+//   fp16 copy of an fp32 store: row and query are each scaled by a power of two (exact) that puts the largest |v_i| in
+//         [2^14, 2^15), then rounded to nearest fp16 (11 significant bits): rho <= 2^-11 for the normal components,
+//         and a component that lands in fp16's subnormal range is off by <= 2^-25 absolute, <= 2^-34 |v| over 1024
+//         of them: rho <= 2^-11 + 2^-34 per operand -> GEMM_EPS_F16 (constant).  The sweep's scores are then in
+//         units of cos * |q| * 2^e_q (the query's scale), and gemm_thr_kernel scales eps_v alike.
 constexpr float GEMM_EPS_ACC = 2.5e-4f;
 constexpr float GEMM_EPS_TF32 = 2.25e-3f;
+constexpr float GEMM_EPS_F16 = 1.25e-3f;
 constexpr float GEMM_RHO_BF16_WORST = 3.90625e-3f;   // 2^-8: cap of a measured rho (a sound upper bound by itself)
+
+// operand kind of the sweep (the template argument of emb_gemm_kernel)
+enum GemmOp : int {
+    GEMM_TF32 = 0,   // fp32 rows and query, wgmma .tf32, 32 elements per K-block
+    GEMM_BF16 = 1,   // bf16 store and bf16-rounded query, wgmma .bf16, 64 elements per K-block
+    GEMM_F16 = 2,    // power-of-two scaled fp16 copies of an fp32 store and of the query, wgmma .f16, 64 per K-block
+};
 
 struct GemmParams {
     uint64_t n_rows;
-    uint32_t n_kblocks;        // stride / 32 (fp32) or stride / 64 (bf16)
+    uint32_t n_kblocks;        // stride / 32 (tf32) or stride / 64 (bf16, fp16)
     const float *inv_norm;     // [n_rows] (NaN => skipped)
     uint32_t n_queries;        // B (real queries)
     uint32_t n_qgroups;        // ceil(B / 128)
@@ -102,6 +118,12 @@ struct GemmParams {
     uint64_t row_words;
     const uint32_t *q_slot;    // [n_queries]
 };
+// emb_gemm_kernel<GEMM_F16>: row_scale [n_rows] = the power of two that turns a row of the fp16 copy back into the stored
+// row (NaN for a row with a non-finite element), staged multiplied into the inverse norms.  (A field of its own type, so
+// that the tf32 and bf16 kernels keep their parameter block.)
+struct GemmF16Params : GemmParams {
+    const float *row_scale;
+};
 // The 32 rows a thread holds of a 128-row half tile (rows row0 + 2 (lane & 3) + 8 (j >> 1) + (j & 1), j < 32) as bit j
 // of a mask, from the half's 4 words of a row bitmap: word w gives bits 8w .. 8w + 7 (its bits 8m + 2 (lane & 3) + {0, 1}).
 __device__ __forceinline__ uint32_t gemm_tile_row_mask(const uint32_t *bits, uint32_t lane) {
@@ -114,13 +136,14 @@ __device__ __forceinline__ uint32_t gemm_tile_row_mask(const uint32_t *bits, uin
     };
     return pick(w.x) | (pick(w.y) << 8) | (pick(w.z) << 16) | (pick(w.w) << 24);
 }
-// emb_gemm_kernel<BF16, DUMP = true> (test harness only): the epilogue writes every approximate score v of a live
+// emb_gemm_kernel<OP, DUMP = true> (test harness only): the epilogue writes every approximate score v of a live
 // (query, row) pair to dump[q * n_rows + row] instead of gathering candidates
-struct GemmDumpParams : GemmParams {
+struct GemmDumpParams : GemmF16Params {
     float *dump;               // [n_queries][n_rows]
 };
-template <bool DUMP> struct GemmKernelParams { using type = GemmParams; };
-template <> struct GemmKernelParams<true> { using type = GemmDumpParams; };
+template <int OP, bool DUMP> struct GemmKernelParams { using type = GemmParams; };
+template <> struct GemmKernelParams<GEMM_F16, false> { using type = GemmF16Params; };
+template <int OP> struct GemmKernelParams<OP, true> { using type = GemmDumpParams; };
 
 __host__ __device__ inline size_t gemm_smem_bytes() {
     return 1024 /*align slack*/ + size_t(GEMM_STAGES) * GEMM_STAGE_BYTES + GEMM_CONSUMER_WG * 2 * GEMM_N * 4 /*inv norms*/
@@ -186,8 +209,8 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
-// D[64 x 256] (+)= A[64 x K] * B[256 x K]^T, both K-major in shared memory; K = 8 (tf32) or 16 (bf16) = 32 bytes
-template <bool BF16>
+// D[64 x 256] (+)= A[64 x K] * B[256 x K]^T, both K-major in shared memory; K = 8 (tf32) or 16 (bf16, fp16) = 32 bytes
+template <int OP>
 __device__ __forceinline__ void wgmma_m64n256(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
 #define OC_WGMMA_D                                                                                                             \
     "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "         \
@@ -213,11 +236,18 @@ __device__ __forceinline__ void wgmma_m64n256(float (&d)[128], uint64_t adesc, u
         "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]),        \
         "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]),        \
         "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
-    if (BF16)
+    if constexpr (OP == GEMM_BF16)
         asm volatile(
             "{\n\t.reg .pred p;\n\t"
             "setp.ne.b32 p, %130, 0;\n\t"
             "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 " OC_WGMMA_D ", %128, %129, p, 1, 1, 0, 0;\n\t}"
+            : OC_WGMMA_OPS
+            : "l"(adesc), "l"(bdesc), "r"(accumulate));
+    else if constexpr (OP == GEMM_F16)
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "setp.ne.b32 p, %130, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 " OC_WGMMA_D ", %128, %129, p, 1, 1, 0, 0;\n\t}"
             : OC_WGMMA_OPS
             : "l"(adesc), "l"(bdesc), "r"(accumulate));
     else
@@ -325,10 +355,10 @@ __device__ __forceinline__ void gemm_release(uint64_t *empty, uint32_t csize) {
 // wgmma D fragment of m64n256 (per warpgroup): warp w holds rows [16w, 16w + 16); lane holds rows lane/4 and
 // lane/4 + 8, columns 8j + 2 (lane % 4) + {0, 1} for j = 0..31, in d[4j + 2h + {0, 1}] (h = row half); the
 // tile's 128-row half u is j = 16u .. 16u + 15.
-template <bool BF16, bool DUMP = false>
+template <int OP, bool DUMP = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_x,
-                const typename GemmKernelParams<DUMP>::type p) {
+                const typename GemmKernelParams<OP, DUMP>::type p) {
     extern __shared__ __align__(1024) uint8_t smem_gemm[];
     // SWIZZLE_128B tiles need 1024-byte alignment of the shared-memory address (the same offset in every CTA: the
     // multicast writes both CTAs of a pair at one offset)
@@ -345,7 +375,7 @@ emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     uint64_t my_tiles = (n_tiles > c) ? (n_tiles - c + p.ctas_per_group - 1) / p.ctas_per_group : 0;
     if (p.tile_limit && my_tiles > p.tile_limit) my_tiles = p.tile_limit;
     const uint32_t nkb = p.n_kblocks;
-    constexpr int32_t KSTEP = BF16 ? 2 * GEMM_KB : GEMM_KB;
+    constexpr int32_t KSTEP = OP == GEMM_TF32 ? GEMM_KB : 2 * GEMM_KB;
 
     if (threadIdx.x == 0) {
         for (uint32_t s = 0; s < GEMM_STAGES; s++) {
@@ -415,7 +445,10 @@ emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 #pragma unroll
         for (uint32_t i = t; i < GEMM_N; i += 128) {
             const uint64_t r = row0 + i;
-            inr[i] = r < p.n_rows ? __ldg(p.inv_norm + r) : __int_as_float(0x7fc00000);
+            if constexpr (OP == GEMM_F16)   // row_scale is a power of two: the product is exact
+                inr[i] = r < p.n_rows ? __ldg(p.inv_norm + r) * __ldg(p.row_scale + r) : __int_as_float(0x7fc00000);
+            else
+                inr[i] = r < p.n_rows ? __ldg(p.inv_norm + r) : __int_as_float(0x7fc00000);
         }
         // requested before the main loop, consumed after it: the L2 round trip hides behind the MMAs of this tile
         unsigned int tg[2];
@@ -432,7 +465,7 @@ emb_gemm_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
             wgmma_fence();
 #pragma unroll
             for (uint32_t k = 0; k < 4; k++)   // 32 B of K per instruction: advance the start address by 32 B (>> 4 = 2)
-                wgmma_m64n256<BF16>(d, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0);
+                wgmma_m64n256<OP>(d, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0);
             wgmma_commit();
             if (kb > 0) {                      // the previous K-block's MMAs have retired: free its stage
                 wgmma_wait<1>();
@@ -686,7 +719,8 @@ __global__ void __launch_bounds__(512, 2) emb_gemm_merge_kernel(const GemmMergeP
 // disjoint group of rows; the limit-th largest of those group maxima is attained by `limit` distinct rows,
 // hence a valid lower bound LB of the query's global limit-th best approximate score — in the same
 // arithmetic the sweep compares with.  The sweep gathers every row above thr = LB - 2 eps (see the merge).
-// eps (cosine) = eps_const + rho_q, scaled to the sweep's cos*|q| units (the rows enter the sweep exactly: rho_x = 0).
+// eps (cosine) = eps_const + rho_q (bf16: the rows enter the sweep exactly, rho_x = 0), scaled to the sweep's cos*|q|
+// units (times 2^e_q for the fp16 sweep).
 struct GemmThrParams {
     const float *gmax; uint32_t lists, limit;
     const float *inv_qnorm;
@@ -695,6 +729,8 @@ struct GemmThrParams {
     unsigned int *thr;        // [B] out: seed threshold, order-preserving uint (atomicMax'ed by the sweep)
     float *eps_v;             // [B] out
     uint32_t *ovf_cnt;        // [B] reset here: the spill cursors of the sweep that follows
+    const float *q_scale;     // [B] GEMM_F16: the power of two 2^e_q the fp16 query was scaled by (the sweep's scores, hence
+                              // gmax and thr, are in cos*|q|*2^e_q units: eps_v is scaled alike), or NULL
 };
 __global__ void __launch_bounds__(256) gemm_thr_kernel(const GemmThrParams p) {
     __shared__ uint64_t keys[512];
@@ -709,7 +745,8 @@ __global__ void __launch_bounds__(256) gemm_thr_kernel(const GemmThrParams p) {
         const float rq = p.rho_q ? fminf(p.rho_q[q], GEMM_RHO_BF16_WORST) : 0.f;
         const float eps_cos = p.eps_const + rq;
         const float iqn = p.inv_qnorm[q];
-        const float ev = iqn > 0.f ? __fdiv_ru(eps_cos, iqn) : INFINITY;
+        float ev = iqn > 0.f ? __fdiv_ru(eps_cos, iqn) : INFINITY;
+        if (p.q_scale) ev *= p.q_scale[q];                     // a power of two: exact
         float thr = -INFINITY;
         if (n >= p.limit && keys[p.limit - 1] != KEY_NONE && ev < INFINITY) thr = key_score(keys[p.limit - 1]) - 2.0f * ev;
         p.thr[q] = f32_ordered(thr);
@@ -725,6 +762,46 @@ __global__ void f32_to_bf16_kernel(const float *in, uint16_t *out, size_t n) {
     const uint32_t u = __float_as_uint(in[i]);
     const uint32_t r = ((u & 0x7fffffffu) > 0x7f800000u) ? (u | 0x00400000u) : (u + 0x7fffu + ((u >> 16) & 1u));
     out[i] = uint16_t(r >> 16);
+}
+
+// ---- fp16 operands of the GEMM_F16 sweep ----
+// One warp: out[i] = fp16_rn(v[i] * 2^s) for i < n, s chosen so that the largest |v_i| * 2^s lies in [2^14, 2^15)
+// (the scaling is exact; nothing overflows, and rounding to nearest loses at most 2^-11 relative per component).
+// Returns s; 0 for an all-zero vector; F16_NONFINITE (and NaN in every element) when some v_i is inf or NaN.
+constexpr int F16_NONFINITE = -0x10000;
+__device__ __forceinline__ int f16_scaled_copy_warp(const float *v, uint32_t n, uint16_t *out, uint32_t lane) {
+    uint32_t mx = 0;   // largest |v_i| as bits: inf and NaN compare above every finite value
+    for (uint32_t j = lane; j < n; j += 32) mx = max(mx, __float_as_uint(v[j]) & 0x7fffffffu);
+    mx = __reduce_max_sync(0xffffffffu, mx);
+    if (mx >= 0x7f800000u) {
+        for (uint32_t j = lane; j < n; j += 32) out[j] = 0x7e00u;
+        return F16_NONFINITE;
+    }
+    int s = 0;
+    if (mx) {   // floor(log2 max|v_i|), subnormal maxima included
+        const int k = mx >= 0x00800000u ? int(mx >> 23) - 127 : (31 - __clz(int(mx))) - 149;
+        s = 14 - k;
+    }
+    for (uint32_t j = lane; j < n; j += 32) out[j] = __half_as_ushort(__float2half_rn(scalbnf(v[j], s)));
+    return s;
+}
+// Rows [row_begin, row_end) of an fp32 store -> their fp16 copy and row_scale = 2^-s (one warp per row).  A row with a
+// non-finite element gets a NaN scale, so its inverse norm in the sweep is NaN and the row is never gathered.
+__global__ void emb_f16_rows_kernel(const float *rows, uint32_t stride, uint64_t row_begin, uint64_t row_end,
+                                    uint16_t *rows_f16, float *row_scale) {
+    const uint64_t r = row_begin + (uint64_t(blockIdx.x) * blockDim.x + threadIdx.x) / 32;
+    if (r >= row_end) return;
+    const uint32_t lane = threadIdx.x & 31;
+    const int s = f16_scaled_copy_warp(rows + r * stride, stride, rows_f16 + r * stride, lane);
+    if (lane == 0) row_scale[r] = s == F16_NONFINITE ? __int_as_float(0x7fc00000) : scalbnf(1.0f, -s);
+}
+// Padded fp32 queries [nq][stride] -> the fp16 query operand and q_scale = 2^s (one warp per query).  A query with a
+// non-finite element keeps scale 1 and NaN operands: all its scores are NaN and nothing is gathered, as in the tf32 sweep.
+__global__ void emb_f16_queries_kernel(const float *q_pad, uint32_t stride, uint32_t nq, uint16_t *q_f16, float *q_scale) {
+    const uint32_t q = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x & 31;
+    if (q >= nq) return;
+    const int s = f16_scaled_copy_warp(q_pad + size_t(q) * stride, stride, q_f16 + size_t(q) * stride, lane);
+    if (lane == 0) q_scale[q] = s == F16_NONFINITE ? 1.0f : scalbnf(1.0f, s);
 }
 
 // copies the exact-path results of re-run queries into their slots of the batch outputs

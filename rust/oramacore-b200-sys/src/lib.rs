@@ -37,6 +37,12 @@ pub const OC_GEO_MAX_VERTICES: u32 = 2048;
 /// oc_filter_facet_range: open ends of the interval (closed when the flag is clear)
 pub const OC_RANGE_LO_OPEN: u32 = 1;
 pub const OC_RANGE_HI_OPEN: u32 = 2;
+/// `OcTiming::scan_variant`: which embedding sweep served the last batch
+pub const OC_SCAN_EXACT: u32 = 0;
+pub const OC_SCAN_TC_TF32: u32 = 1;
+pub const OC_SCAN_TC_BF16: u32 = 4;
+/// wgmma .f16 on the fp16 copy of an fp32 store (`OC_EMB_F16=0` selects `OC_SCAN_TC_TF32`)
+pub const OC_SCAN_TC_F16: u32 = 5;
 
 #[repr(C)]
 pub struct OcSearchParams {
