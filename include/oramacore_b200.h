@@ -220,7 +220,8 @@ typedef struct {
  *     do not pass).  All entries NULL: an unfiltered search; every entry the same handle: the p->filter path.
  *   - OC_ERR_INVALID: q_filters together with filter or filter_bits, a handle of another ctx.
  *     OC_ERR_UNSUPPORTED: sharded.  A refused call creates nothing and writes no output.
- *   - oc_search_q_sorted takes q_filters together with a sort and pins per query;
+ *   - oc_search_q_sorted takes q_filters together with a sort and pins per query, oc_search_q_groups together with
+ *     groups, a sort and pins per query;
  *   - oc_search_groups*, oc_search_pinned and oc_search_sorted refuse q_filters with OC_ERR_UNSUPPORTED;
  *     oc_search_facets ignores it as it ignores filter (facets are scored without the where-filter). */
 int oc_search(oc_ctx *ctx, oc_emb *emb, oc_str *str, const oc_search_params *p,
@@ -497,6 +498,40 @@ int oc_search_groups_sorted(oc_ctx *ctx, oc_emb *emb, oc_str *str, oc_group_by *
                             uint64_t *out_doc_ids, float *out_scores, double *out_sort_values, uint32_t *out_n,
                             uint64_t *out_count, uint64_t *out_group_doc_ids, float *out_group_scores,
                             double *out_group_sort_values, uint32_t *out_group_n);
+/* ---- per-query groups -------------------------------------------------------------------------------
+ * Every request of the reference carries its own groupBy (SearchParams.group_by: properties and max_results), together
+ * with its own where-filter, sortBy and pin rules.  oc_search_q_groups is the batched form: query b takes q_groups[b]
+ * and its items (pins), and, with q_filters, its own filter.  Query b's outputs — hits, scores, sort values, n, count,
+ * its items' pin scores / present flags, and its groups (ids, score bits, n, sort values) — are byte for byte what it
+ * gets alone (B = 1, p->filter = q_filters[b], its own items) from:
+ *   - groups NULL: oc_search_q_sorted with its sort (field NULL: score order);
+ *   - groups, score order, no item: oc_search_groups(max_results);
+ *   - groups, score order, items: oc_search_groups_pinned;
+ *   - groups, a sort: oc_search_groups_sorted.
+ * Group layout: query b's groups are the rows [G_b, G_b + n_groups(b)) of out_group_doc_ids / out_group_scores /
+ * out_group_sort_values (rows x group_stride) and out_group_n (rows), G_b = the sum of n_groups(b') over b' < b (0 for a
+ * query without groups).  Entries past a row's n are 0; the group sort values of a query in score order are NaN inside
+ * n.  group_stride >= 2 x max_results + its items for every ACTIVE query (see oc_pins) with groups, >= max_results for
+ * any other query with groups.  out_sort_values and out_group_sort_values may be NULL; the pin outputs may be NULL.
+ * p->limit == 0 is accepted when every query has groups (the hits are not written, as for oc_search_groups).
+ * Workspace: B x ceil(rows / 8192) x 8192 x 4 bytes of per-row scores for the whole batch, queries without groups
+ * included (as oc_search_groups); OC_ERR_OOM when it cannot be allocated: pass smaller batches.
+ * Refusals (nothing written): everything the four single calls refuse — OC_ERR_INVALID: q_groups NULL, a group_by,
+ * sort field, filter or store of another ctx, a bad order, group_stride below a query's need, q_pin_offsets not
+ * monotone, q_filters together with filter / filter_bits, p->limit == 0 with a query without groups; OC_ERR_UNSUPPORTED:
+ * p->sharded, max_results > OC_MAX_TOPK, an active query with 2 x max_results > OC_MAX_TOPK, the limit + offset limits of
+ * oc_search_q_sorted — and OC_ERR_UNSUPPORTED for 2^31 or more rows. */
+typedef struct {
+    const oc_group_by *groups;       /* NULL: this query has no groups                          */
+    uint32_t max_results;            /* per query, <= OC_MAX_TOPK                               */
+    oc_sort sort;                    /* field NULL: score order                                 */
+} oc_group_req;
+uint64_t oc_group_by_n_groups(const oc_group_by *g);   /* its n_groups (0 for NULL): lays out the group rows */
+int oc_search_q_groups(oc_ctx *ctx, oc_emb *emb, oc_str *str, const oc_search_params *p, const oc_group_req *q_groups,
+                       const oc_pins *pins, uint32_t group_stride, uint64_t *out_doc_ids, float *out_scores,
+                       double *out_sort_values, uint32_t *out_n, uint64_t *out_count, float *out_pin_scores,
+                       uint8_t *out_pin_present, uint64_t *out_group_doc_ids, float *out_group_scores,
+                       double *out_group_sort_values, uint32_t *out_group_n);
 /* The multi-index union in field order (host, no device; MergeSortedIterator, read/sort.rs:491-559).  Run every index
  * with oc_search_sorted, limit' = limit + offset (2 x (limit + offset) when pins apply, and then apply = 0),
  * offset' = 0, vector_limit = limit, and pass its hits, sort values (in_stride = limit'), counts and per-item
@@ -581,7 +616,22 @@ int oc_batcher_search(oc_batcher *b, const oc_search_params *p, uint64_t *out_do
 int oc_batcher_search_sorted(oc_batcher *b, const oc_search_params *p, const oc_sort *sort, const oc_pins *pins,
                              uint64_t *out_doc_ids, float *out_scores, double *out_sort_values, uint32_t *out_n,
                              uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present);
-/* queries that went through a coalesced batch / number of batches / calls passed straight through */
+/* oc_batcher_search_sorted with groupBy: one query, its oc_group_req, its items and group_stride; outputs as
+ * oc_search_q_groups with B = 1 (its groups are rows [0, n_groups)).  Grouped requests batch only with grouped requests
+ * of the same (mode, limit, offset, similarity, threshold, bm25_k, bm25_b, vector_limit); their handles, max_results,
+ * sorts, items and filters may differ.  The batch runs as one oc_search_q_groups at the largest stride of its requests,
+ * and each request's rows go back at its own group_stride.  Refused with OC_ERR_INVALID before joining a batch: a
+ * group_stride below the request's need, malformed pins, a bad order, a handle of another ctx.  A request the merged
+ * call would refuse (max_results > OC_MAX_TOPK, items with apply = 0, more than OC_MAX_TOPK items, items with
+ * 2 x (limit + offset) or 2 x max_results > OC_MAX_TOPK, no groups at limit 0) runs alone and gets its normal error.  A merged call
+ * that fails with OC_ERR_OOM (its row-score workspace) is split in halves and re-run, down to single requests. */
+int oc_batcher_search_groups(oc_batcher *b, const oc_search_params *p, const oc_group_req *req, const oc_pins *pins,
+                             uint32_t group_stride, uint64_t *out_doc_ids, float *out_scores, double *out_sort_values,
+                             uint32_t *out_n, uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present,
+                             uint64_t *out_group_doc_ids, float *out_group_scores, double *out_group_sort_values,
+                             uint32_t *out_group_n);
+/* queries that went through a coalesced batch (grouped ones included) / number of batches / calls passed straight
+ * through */
 int oc_batcher_stats(oc_batcher *b, uint64_t *n_queries, uint64_t *n_batches, uint64_t *n_direct);
 
 /* ---- pinned host buffers (optional) ----------------------------------------------------------

@@ -13,6 +13,9 @@
 // Requests of submit_sorted carry a sort (or score order) and pin items of their own and share batches with plain
 // requests: a batch with no sort and no item runs through `Exec` as before, any other through `SortedExec`
 // (oc_search_q_sorted) with the sorts and the items' CSR merged in request order.
+// Requests of submit_groups carry an oc_group_req and batch only with each other (the key's `grouped` bit): a batch runs
+// through `GroupedExec` (oc_search_q_groups) at the largest need of its requests as the group stride, and each request's
+// group rows go back at its own stride.  A merged call that runs out of device memory is split in halves and re-run.
 #pragma once
 #include <algorithm>
 #include <atomic>
@@ -29,8 +32,10 @@ namespace ocb {
 
 struct BatchKey {
     int mode; uint32_t limit, offset; float similarity, threshold, k, b; uint32_t vector_limit;
+    bool grouped = false;
     bool operator==(const BatchKey &o) const {
-        return mode == o.mode && limit == o.limit && offset == o.offset && vector_limit == o.vector_limit && memcmp(&similarity, &o.similarity, 4) == 0 &&
+        return mode == o.mode && limit == o.limit && offset == o.offset && vector_limit == o.vector_limit && grouped == o.grouped &&
+               memcmp(&similarity, &o.similarity, 4) == 0 &&
                memcmp(&threshold, &o.threshold, 4) == 0 && memcmp(&k, &o.k, 4) == 0 && memcmp(&b, &o.b, 4) == 0;
     }
 };
@@ -78,6 +83,19 @@ inline bool pins_batchable(const oc_search_params *p, const oc_pins *pins) {
     return pins->apply && k <= OC_MAX_TOPK && (uint64_t(p->limit) + p->offset) * 2 <= OC_MAX_TOPK;
 }
 
+// The group rows a request needs: 2 x max_results + its items when it is active, max_results otherwise, 0 without groups.
+inline uint64_t group_need(const oc_group_req *req, const oc_pins *pins) {
+    if (!req->groups) return 0;
+    const uint32_t k = pins && pins->apply ? pin_items(pins) : 0u;
+    return k ? 2ull * req->max_results + k : req->max_results;
+}
+// Whether a request of submit_groups can join a merged oc_search_q_groups without failing it (see pins_batchable).
+inline bool groups_batchable(const oc_search_params *p, const oc_group_req *req, const oc_pins *pins) {
+    if (!pins_batchable(p, pins)) return false;
+    if (!req->groups) return p->limit > 0;
+    return req->max_results <= OC_MAX_TOPK && (!pin_items(pins) || 2ull * req->max_results <= OC_MAX_TOPK);
+}
+
 struct BatchReq {
     const oc_search_params *p;
     uint64_t *docs; float *scores; uint32_t *n; uint64_t *count;
@@ -87,6 +105,15 @@ struct BatchReq {
     double *sort_values = nullptr;      // [limit]
     float *pin_scores = nullptr;        // [items], may be NULL
     uint8_t *pin_present = nullptr;
+    // submit_groups only
+    bool grouped = false;
+    const oc_group_req *greq = nullptr;
+    uint64_t n_groups = 0;              // its handle's n_groups (0 without groups)
+    uint32_t group_stride = 0;
+    uint64_t *g_doc = nullptr;          // [n_groups][group_stride]
+    float *g_score = nullptr;
+    double *g_values = nullptr;         // may be NULL
+    uint32_t *g_n = nullptr;            // [n_groups]
     int rc = 0;
     bool done = false;
 };
@@ -109,6 +136,15 @@ struct MergedBatch {
     std::vector<double> sort_values;            // [B][limit]
     std::vector<float> pin_scores;              // [items]
     std::vector<uint8_t> pin_present;
+    // a grouped batch: oc_search_q_groups' arguments, each request's rows from g_row[i]
+    bool grouped = false;
+    std::vector<oc_group_req> q_groups;         // [B]
+    std::vector<uint64_t> g_row;                // [B + 1]
+    uint32_t stride = 0;
+    std::vector<uint64_t> g_doc;                // [rows][stride]
+    std::vector<float> g_score;
+    std::vector<double> g_values;
+    std::vector<uint32_t> g_n;                  // [rows]
 
     void build(const std::vector<BatchReq *> &reqs, uint32_t dim) {
         const oc_search_params *f = reqs[0]->p;
@@ -157,7 +193,8 @@ struct MergedBatch {
             }
         docs.assign(size_t(B) * f->limit, 0); scores.assign(size_t(B) * f->limit, 0.f);
         n.assign(B, 0); count.assign(B, 0);
-        sorted = false;
+        grouped = reqs[0]->grouped;
+        sorted = grouped;
         for (uint32_t i = 0; i < B; i++) sorted = sorted || (reqs[i]->sort && reqs[i]->sort->field) || pin_items(reqs[i]->pins);
         if (!sorted) return;
         q_sorts.assign(B, oc_sort{nullptr, OC_SORT_ASC});
@@ -177,6 +214,20 @@ struct MergedBatch {
         sort_values.assign(size_t(B) * f->limit, 0.0);
         pin_scores.assign(std::max<size_t>(pin_doc.size(), 1), 0.f);
         pin_present.assign(std::max<size_t>(pin_doc.size(), 1), 0);
+        if (!grouped) return;
+        q_groups.resize(B);
+        g_row.assign(1, 0);
+        stride = 0;
+        for (uint32_t i = 0; i < B; i++) {
+            q_groups[i] = *reqs[i]->greq;
+            g_row.push_back(g_row.back() + reqs[i]->n_groups);
+            stride = std::max<uint32_t>(stride, (uint32_t)group_need(reqs[i]->greq, reqs[i]->pins));
+        }
+        const size_t rows = g_row.back();
+        g_doc.assign(std::max<size_t>(rows * stride, 1), 0);
+        g_score.assign(std::max<size_t>(rows * stride, 1), 0.f);
+        g_values.assign(std::max<size_t>(rows * stride, 1), 0.0);
+        g_n.assign(std::max<size_t>(rows, 1), 0);
     }
     void scatter(const std::vector<BatchReq *> &reqs, int rc) const {
         const uint32_t L = p.limit;
@@ -184,9 +235,11 @@ struct MergedBatch {
             BatchReq *r = reqs[i];
             r->rc = rc;
             if (rc != 0) continue;
-            memcpy(r->docs, docs.data() + i * L, size_t(L) * 8);
-            memcpy(r->scores, scores.data() + i * L, size_t(L) * 4);
-            *r->n = n[i];
+            if (L) {   // a grouped request at limit 0 gets no hits, as from a call of its own
+                memcpy(r->docs, docs.data() + i * L, size_t(L) * 8);
+                memcpy(r->scores, scores.data() + i * L, size_t(L) * 4);
+                *r->n = n[i];
+            }
             *r->count = count[i];
             if (r->sort_values) {   // a batch run as oc_search: score order, NaN as oc_search_q_sorted writes it
                 if (sorted) memcpy(r->sort_values, sort_values.data() + i * L, size_t(L) * 8);
@@ -198,6 +251,17 @@ struct MergedBatch {
                     if (r->pin_scores) r->pin_scores[o] = pin_scores[j];
                     if (r->pin_present) r->pin_present[o] = pin_present[j];
                 }
+            if (grouped)   // the request's rows at its own stride; past the merged stride its rows are 0, as past n
+                for (uint64_t g = 0; g < r->n_groups; g++) {
+                    const size_t src = (g_row[i] + g) * stride, dst = g * r->group_stride;
+                    const uint32_t w = std::min(stride, r->group_stride);
+                    for (uint32_t j = 0; j < r->group_stride; j++) {
+                        r->g_doc[dst + j] = j < w ? g_doc[src + j] : 0;
+                        r->g_score[dst + j] = j < w ? g_score[src + j] : 0.f;
+                        if (r->g_values) r->g_values[dst + j] = j < w ? g_values[src + j] : 0.0;
+                    }
+                    r->g_n[g] = g_n[g_row[i] + g];
+                }
         }
     }
 };
@@ -208,16 +272,27 @@ struct NoSortedExec {
                    uint64_t *, float *, uint8_t *) const { return OC_ERR_UNSUPPORTED; }
 };
 
+// The executor of a batcher that only takes submit() / submit_sorted(): it is never called.
+struct NoGroupedExec {
+    int operator()(const oc_search_params *, const oc_group_req *, const oc_pins *, uint32_t, uint64_t *, float *, double *,
+                   uint32_t *, uint64_t *, float *, uint8_t *, uint64_t *, float *, double *, uint32_t *) const {
+        return OC_ERR_UNSUPPORTED;
+    }
+};
+
 // int Exec(const oc_search_params*, uint64_t* docs, float* scores, uint32_t* n, uint64_t* count)
 // int SortedExec(const oc_search_params*, const oc_sort* q_sorts, const oc_pins*, uint64_t* docs, float* scores,
 //                double* sort_values, uint32_t* n, uint64_t* count, float* pin_scores, uint8_t* pin_present)
-template <class Exec, class SortedExec = NoSortedExec>
+// int GroupedExec(const oc_search_params*, const oc_group_req* q_groups, const oc_pins*, uint32_t group_stride,
+//                 uint64_t* docs, float* scores, double* sort_values, uint32_t* n, uint64_t* count, float* pin_scores,
+//                 uint8_t* pin_present, uint64_t* g_docs, float* g_scores, double* g_sort_values, uint32_t* g_n)
+template <class Exec, class SortedExec = NoSortedExec, class GroupedExec = NoGroupedExec>
 class Batcher {
 public:
     Batcher(Exec exec, uint32_t dim, uint32_t max_batch, uint32_t max_wait_us, bool has_emb = true, bool has_str = true,
-            SortedExec sexec = SortedExec())
-        : exec_(exec), sexec_(sexec), dim_(dim), max_batch_(max_batch ? max_batch : 1), max_wait_us_(max_wait_us), has_emb_(has_emb),
-          has_str_(has_str) {}
+            SortedExec sexec = SortedExec(), GroupedExec gexec = GroupedExec())
+        : exec_(exec), sexec_(sexec), gexec_(gexec), dim_(dim), max_batch_(max_batch ? max_batch : 1), max_wait_us_(max_wait_us),
+          has_emb_(has_emb), has_str_(has_str) {}
 
     int submit(const oc_search_params *p, uint64_t *docs, float *scores, uint32_t *n, uint64_t *count) {
         if (!batchable(p, has_emb_, has_str_) || max_batch_ == 1) {
@@ -241,6 +316,26 @@ public:
         r.sort = sort; r.pins = pins; r.sort_values = sort_values; r.pin_scores = pin_scores; r.pin_present = pin_present;
         return join(r);
     }
+    // One query with its oc_group_req (n_groups: its handle's, 0 without groups), items and group stride; outputs as
+    // oc_search_q_groups with B = 1.  OC_ERR_INVALID without joining: a stride below the request's need, a bad order,
+    // malformed pins.
+    int submit_groups(const oc_search_params *p, const oc_group_req *req, uint64_t n_groups, const oc_pins *pins,
+                      uint32_t group_stride, uint64_t *docs, float *scores, double *sort_values, uint32_t *n, uint64_t *count,
+                      float *pin_scores, uint8_t *pin_present, uint64_t *g_doc, float *g_score, double *g_values, uint32_t *g_n) {
+        const char *why = nullptr;
+        if (const int rc = check_sorted(&req->sort, pins, &why)) return rc;
+        if (group_stride < group_need(req, pins)) return OC_ERR_INVALID;
+        if (!batchable(p, has_emb_, has_str_) || max_batch_ == 1 || !groups_batchable(p, req, pins)) {
+            direct_++;
+            return gexec_(p, req, pins, group_stride, docs, scores, sort_values, n, count, pin_scores, pin_present, g_doc, g_score,
+                          g_values, g_n);
+        }
+        BatchReq r{p, docs, scores, n, count};
+        r.sort = &req->sort; r.pins = pins; r.sort_values = sort_values; r.pin_scores = pin_scores; r.pin_present = pin_present;
+        r.grouped = true; r.greq = req; r.n_groups = req->groups ? n_groups : 0; r.group_stride = group_stride;
+        r.g_doc = g_doc; r.g_score = g_score; r.g_values = g_values; r.g_n = g_n;
+        return join(r);
+    }
     void stats(uint64_t *queries, uint64_t *batches, uint64_t *direct) {
         std::lock_guard<std::mutex> g(mu_);
         if (queries) *queries = queries_;
@@ -253,7 +348,8 @@ private:
         const oc_search_params *p = r.p;
         std::unique_lock<std::mutex> lk(mu_);
         // one group collects at a time: wait while it is full or holds a different parameter tuple
-        const BatchKey k = key_of(p);
+        BatchKey k = key_of(p);
+        k.grouped = r.grouped;
         cv_slot_.wait(lk, [&] { return pending_.empty() || (pending_key_ == k && pending_.size() < max_batch_); });
         if (pending_.empty()) pending_key_ = k;
         pending_.push_back(&r);
@@ -267,12 +363,15 @@ private:
             leader_active_ = false;          // the next arrival leads the next group while this one runs
             cv_slot_.notify_all();
             lk.unlock();
-            MergedBatch m;
-            m.build(batch, dim_);
-            const int rc = m.sorted ? sexec_(&m.p, m.q_sorts.data(), &m.pins, m.docs.data(), m.scores.data(), m.sort_values.data(),
-                                             m.n.data(), m.count.data(), m.pin_scores.data(), m.pin_present.data())
-                                    : exec_(&m.p, m.docs.data(), m.scores.data(), m.n.data(), m.count.data());
-            m.scatter(batch, rc);
+            if (r.grouped) run_grouped(batch);
+            else {
+                MergedBatch m;
+                m.build(batch, dim_);
+                const int rc = m.sorted ? sexec_(&m.p, m.q_sorts.data(), &m.pins, m.docs.data(), m.scores.data(), m.sort_values.data(),
+                                                 m.n.data(), m.count.data(), m.pin_scores.data(), m.pin_present.data())
+                                        : exec_(&m.p, m.docs.data(), m.scores.data(), m.n.data(), m.count.data());
+                m.scatter(batch, rc);
+            }
             lk.lock();
             batches_++; queries_ += batch.size();
             for (BatchReq *b : batch) b->done = true;
@@ -283,9 +382,26 @@ private:
         }
         return r.rc;
     }
+    // One merged oc_search_q_groups; out of device memory (the row-score workspace grows with the batch), each half runs
+    // on its own, down to single requests, which then get the single call's answer.
+    void run_grouped(const std::vector<BatchReq *> &reqs) {
+        MergedBatch m;
+        m.build(reqs, dim_);
+        const int rc = gexec_(&m.p, m.q_groups.data(), &m.pins, m.stride, m.docs.data(), m.scores.data(), m.sort_values.data(),
+                              m.n.data(), m.count.data(), m.pin_scores.data(), m.pin_present.data(), m.g_doc.data(), m.g_score.data(),
+                              m.g_values.data(), m.g_n.data());
+        if (rc == OC_ERR_OOM && reqs.size() > 1) {
+            const size_t h = reqs.size() / 2;
+            run_grouped(std::vector<BatchReq *>(reqs.begin(), reqs.begin() + h));
+            run_grouped(std::vector<BatchReq *>(reqs.begin() + h, reqs.end()));
+            return;
+        }
+        m.scatter(reqs, rc);
+    }
 
     Exec exec_;
     SortedExec sexec_;
+    GroupedExec gexec_;
     uint32_t dim_, max_batch_, max_wait_us_;
     bool has_emb_, has_str_;
     std::mutex mu_;

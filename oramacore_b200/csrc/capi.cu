@@ -1774,13 +1774,35 @@ struct FacetJob {   // oc_search_facets: count, per query, the matched documents
 };
 static int run_facets(oc_ctx *c, const FacetJob &fj, uint32_t B, bool has_ft, bool has_v, const StrSnap *S, uint32_t n_tiles,
                       uint32_t vlimit);
-struct GroupJob {   // oc_search_groups: the top max_results documents of every (query, group)
-    oc_group_by *g;
-    uint32_t max_results;
-    uint64_t *out_doc;      // [B][G][max_results]
-    float *out_score;
-    uint32_t *out_n;        // [B][G]
-    uint32_t stride = 0;    // oc_search_groups_pinned: row stride of the group arrays ([B][G][stride])
+// A groupBy handle: the CSR of its groups, built once by oc_group_by_create (below).
+struct oc_group_by {
+    oc_ctx *ctx;
+    uint32_t n_groups = 0;
+    uint64_t n_docs = 0;           // entries of the CSR (a document counts once per group it belongs to)
+    uint64_t *off = nullptr;       // device [n_groups + 1]
+    uint64_t *docs = nullptr;      // device [n_docs]
+    uint32_t *rows = nullptr;      // device [n_docs + 1]: string row of each entry, filled per call; rows[n_docs] = ~0
+};
+// The grouped calls: per query its oc_group_by (or none) and max_results.  Query q's groups are the output rows
+// [q_row[q], q_row[q] + n_groups), each of `stride` entries.
+constexpr uint32_t GROUP_NONE = 0xffffffffu;
+struct GroupJob {
+    std::vector<oc_group_by *> h;           // the batch's distinct handles
+    std::vector<uint32_t> q_h;              // [B] index into h, GROUP_NONE: no groups
+    std::vector<uint32_t> q_m;              // [B] max_results
+    std::vector<uint32_t> q_row;            // [B]
+    uint32_t rows = 0;                      // sum of the queries' n_groups
+    uint32_t stride = 0;
+    uint64_t *out_doc = nullptr;            // [rows][stride]
+    float *out_score = nullptr;
+    uint32_t *out_n = nullptr;              // [rows]
+    double *out_values = nullptr;           // [rows][stride] sort values, may be NULL
+    // the work list (set by search_impl): spans of the score-order queries first, then those in field order
+    uint32_t n_spans = 0, n_score_spans = 0, n_score_items = 0, top = 0;
+    bool direct = false;                    // no splice and every depth == stride: the top lists are the outputs
+    const GroupHandle *d_hand = nullptr;
+    const GroupSpan *d_spans = nullptr;
+    const SortEntry *d_ents = nullptr;
 };
 struct PinJob {   // oc_search_pinned / oc_search_groups_pinned: the promote items, padded to `stride` slots per query
     uint32_t stride = 0;                // most items of one query (0: no item in the batch)
@@ -1848,8 +1870,6 @@ struct SortJob {
     std::vector<uint32_t> q_ent;           // [B]
     bool by_score = false;                 // some query is in score order
     double *out_values = nullptr;          // B x limit, may be NULL
-    double *out_group_values = nullptr;    // B x n_groups x group_stride, may be NULL
-    uint32_t n_groups = 0;
     SortOrder &ord(uint32_t e) const { return f[e]->ord[order[e]]; }
 };
 // Appends one query's sort (field NULL: score order).  Nothing is written on failure.
@@ -1898,15 +1918,15 @@ static int sort_rows_for(oc_ctx *c, SortOrder &o, const std::shared_ptr<StrSnap>
     return OC_OK;
 }
 
-static int run_groups(oc_ctx *c, const GroupJob &gj, uint32_t B, int mode, const StrSnap *S, uint32_t n_tiles, uint32_t vlimit,
-                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, const PinJob *pj, const SortJob *sj);
+static int run_groups(oc_ctx *c, const GroupJob &gj, int mode, const StrSnap *S, uint32_t n_tiles, uint32_t vlimit,
+                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, const PinJob &pj);
 
-// gj != NULL: oc_search_groups.  Then limit == 0 is allowed: the hits are not written (out_doc_ids / out_scores / out_n
+// gj != NULL: the grouped calls (always with pj).  Then limit == 0 is allowed: the hits are not written (out_doc_ids / out_scores / out_n
 // may be NULL), the vector stage gets depth 0 and the fulltext stage runs with one candidate slot per tile.
 // pj != NULL: the pinned calls; the items' score-map values go to out_pin_scores / out_pin_present (may be NULL).
 // sj != NULL: the sorted calls (always with pj); the hits are the walk's in field order, K4's list only gives the count.
 static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, uint64_t *out_doc_ids,
-                       float *out_scores, uint32_t *out_n, uint64_t *out_count, const FacetJob *fj, const GroupJob *gj = nullptr,
+                       float *out_scores, uint32_t *out_n, uint64_t *out_count, const FacetJob *fj, GroupJob *gj = nullptr,
                        PinJob *pj = nullptr, const oc_pins *pins = nullptr, float *out_pin_scores = nullptr,
                        uint8_t *out_pin_present = nullptr, const SortJob *sj = nullptr) {
     if (!c || !p || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
@@ -1926,8 +1946,9 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     QFilterJob qfj;
     bool per_q = false;
     if (p->q_filters) {
-        if (gj || ((pj || sj) && !(pj && pj->q_filters)))
-            return fail(OC_ERR_UNSUPPORTED, "q_filters: per-query filters are supported by oc_search and oc_search_q_sorted only");
+        if ((gj || pj || sj) && !(pj && pj->q_filters))
+            return fail(OC_ERR_UNSUPPORTED, "q_filters: per-query filters are supported by oc_search, oc_search_q_sorted and "
+                                            "oc_search_q_groups only");
         if (p->filter || p->filter_bits) return fail(OC_ERR_INVALID, "q_filters together with filter / filter_bits");
         if (p->sharded) return fail(OC_ERR_UNSUPPORTED, "q_filters over a sharded search");
         std::unordered_map<const oc_filter *, uint32_t> idx;
@@ -2281,12 +2302,12 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     std::vector<SortEntry> s_ents;
     std::vector<SortQuery> s_q;
     std::vector<uint8_t> s_alt;
-    if (sort_flat) {
-        const bool ft_map = has_ft && n_tiles > 0;
+    if (sj)
         for (uint32_t e = 0; e < sj->f.size(); e++) {
             const SortOrder &o = sj->ord(e);
-            s_ents.push_back(SortEntry{o.n, ft_map ? o.rank_row : nullptr, o.doc_rank, sj->f[e]->nbits, o.rank_doc});
+            s_ents.push_back(SortEntry{o.n, has_ft && n_tiles > 0 ? o.rank_row : nullptr, o.doc_rank, sj->f[e]->nbits, o.rank_doc});
         }
+    if (sort_flat) {
         s_q.resize(B);
         s_alt.resize(B);
         for (uint32_t q = 0; q < B; q++) {
@@ -2295,7 +2316,35 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
             s_alt[q] = sj->q_ent[q] == SORT_BY_SCORE;
         }
     }
-    const size_t o_sent = sort_flat ? pk.add(s_ents.data(), s_ents.size() * sizeof(SortEntry)) : 0;
+    const size_t o_sent = sj ? pk.add(s_ents.data(), s_ents.size() * sizeof(SortEntry)) : 0;
+    // groups: the batch's distinct handles and the work list of (query, group) items, one span per query with groups:
+    // the queries in score order first, then those in field order (one launch of group_topk_kernel /
+    // group_sort_topk_kernel each)
+    std::vector<GroupHandle> g_hand;
+    std::vector<GroupSpan> g_spans;
+    if (gj) {
+        for (const oc_group_by *g : gj->h) g_hand.push_back(GroupHandle{g->off, g->docs, has_ft && n_tiles > 0 ? g->rows : nullptr, g->n_groups});
+        uint32_t first = 0;
+        gj->top = 0;
+        gj->direct = !pj->splice;
+        for (int by_field = 0; by_field < 2; by_field++) {
+            for (uint32_t q = 0; q < B; q++) {
+                const uint32_t h = gj->q_h[q];
+                const uint32_t ent = sj ? sj->q_ent[q] : SORT_BY_SCORE;
+                if (h == GROUP_NONE || gj->h[h]->n_groups == 0 || (ent != SORT_BY_SCORE) != bool(by_field)) continue;
+                // sort_groups with pins takes every group's top 2 * max_results for an active query (sort.rs:137-142)
+                const uint32_t m = gj->q_m[q], depth = m * (pj->splice && pj->cnt[q] > 0 ? 2 : 1);
+                g_spans.push_back(GroupSpan{first, q, h, depth, m, ent, gj->q_row[q]});
+                first += gj->h[h]->n_groups;
+                gj->top = std::max(gj->top, depth);
+                gj->direct = gj->direct && depth == gj->stride;
+            }
+            if (!by_field) { gj->n_score_spans = (uint32_t)g_spans.size(); gj->n_score_items = first; }
+        }
+        gj->n_spans = (uint32_t)g_spans.size();
+    }
+    const size_t o_ghand = gj ? pk.add(g_hand.data(), g_hand.size() * sizeof(GroupHandle)) : 0;
+    const size_t o_gspan = gj ? pk.add(g_spans.data(), g_spans.size() * sizeof(GroupSpan)) : 0;
     const size_t o_sq = sort_flat ? pk.add(s_q.data(), s_q.size() * sizeof(SortQuery)) : 0;
     const size_t o_salt = sort_flat && sj->by_score ? pk.add(s_alt.data(), s_alt.size()) : 0;
     // hybrid: the descriptors, the shared-contribution precompute, the filter bitmap and the (term, tile) plan do
@@ -2313,6 +2362,11 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     uint8_t *din = c->in_blob.as<uint8_t>();
     if (filter_h && !has_v) filter_dev = reinterpret_cast<const uint64_t *>(din + o_flt);
     if (per_q && !has_v) bind_qf(din, o_qf);
+    if (gj) {
+        gj->d_hand = reinterpret_cast<const GroupHandle *>(din + o_ghand);
+        gj->d_spans = reinterpret_cast<const GroupSpan *>(din + o_gspan);
+        gj->d_ents = sj ? reinterpret_cast<const SortEntry *>(din + o_sent) : nullptr;
+    }
     if (pin_items) {
         pj->d_doc = reinterpret_cast<const uint64_t *>(din + o_pdoc);
         pj->d_pos = reinterpret_cast<const uint32_t *>(din + o_ppos);
@@ -2730,7 +2784,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     if (fj) OCTRY(run_facets(c, *fj, B, has_ft, has_v, S, n_tiles, vlimit));
     if (gj) {
         CU(cudaEventRecord(c->ev[EV_GRP0], c->stream));
-        OCTRY(run_groups(c, *gj, B, p->mode, S, n_tiles, vlimit, fp.omc_doc, fp.omc_mult, n_omc, pj, sj));
+        OCTRY(run_groups(c, *gj, p->mode, S, n_tiles, vlimit, fp.omc_doc, fp.omc_mult, n_omc, *pj));
         CU(cudaEventRecord(c->ev[EV_GRP1], c->stream));
         CU(cudaStreamSynchronize(c->stream));
     }
@@ -2756,15 +2810,17 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
                 const size_t o = size_t(q) * limit + i;
                 sj->out_values[o] = i < out_n[q] ? sort_value_of(*sj, pj, q, out_doc_ids[o]) : 0.0;
             }
-    if (sj && gj && sj->out_group_values) {   // run_groups' copies are complete (synchronised above)
-        const uint32_t G = sj->n_groups;
-        for (uint32_t q = 0; q < B; q++)
-            for (uint32_t g = 0; g < G; g++)
+    if (gj && gj->out_values)   // run_groups' copies are complete (synchronised above); score order: NaN
+        for (uint32_t q = 0; q < B; q++) {
+            if (gj->q_h[q] == GROUP_NONE) continue;
+            const uint32_t G = gj->h[gj->q_h[q]]->n_groups;
+            for (size_t r = gj->q_row[q]; r < size_t(gj->q_row[q]) + G; r++)
                 for (uint32_t i = 0; i < gj->stride; i++) {
-                    const size_t o = (size_t(q) * G + g) * gj->stride + i;
-                    sj->out_group_values[o] = i < gj->out_n[size_t(q) * G + g] ? sort_value_of(*sj, pj, q, gj->out_doc[o]) : 0.0;
+                    const size_t o = r * gj->stride + i;
+                    gj->out_values[o] = i >= gj->out_n[r] ? 0.0 : sj ? sort_value_of(*sj, pj, q, gj->out_doc[o])
+                                                                     : std::numeric_limits<double>::quiet_NaN();
                 }
-    }
+        }
     if (!pin_sc.empty())
         for (uint32_t q = 0; q < B; q++)
             for (uint32_t j = 0; j < pj->cnt[q]; j++) {
@@ -3061,15 +3117,7 @@ extern "C" int oc_search_facets(oc_ctx *c, oc_emb *emb, oc_str *str, oc_facets *
 // ------------------------------------------------------------------------------------ groups
 // GroupContext::execute (read/index/group.rs) + sort_groups (read/sort.rs:129-230): the group CSR is built once on
 // the host; per call its documents are mapped to string rows and group_topk_kernel (group.cuh) runs one CTA per
-// (group, query) over the score map the search left on the device.
-struct oc_group_by {
-    oc_ctx *ctx;
-    uint32_t n_groups = 0;
-    uint64_t n_docs = 0;           // entries of the CSR (a document counts once per group it belongs to)
-    uint64_t *off = nullptr;       // device [n_groups + 1]
-    uint64_t *docs = nullptr;      // device [n_docs]
-    uint32_t *rows = nullptr;      // device [n_docs + 1]: string row of each entry, filled per call; rows[n_docs] = ~0
-};
+// (query, group) over the score map the search left on the device.  struct oc_group_by is defined with GroupJob.
 static void group_by_free(oc_group_by *g) {
     cudaFree(g->off); cudaFree(g->docs); cudaFree(g->rows);
     delete g;
@@ -3181,34 +3229,32 @@ extern "C" int oc_group_by_create(oc_facets *f, const uint32_t *fields, uint32_t
     return OC_OK;
 }
 
-static int run_groups(oc_ctx *c, const GroupJob &gj, uint32_t B, int mode, const StrSnap *S, uint32_t n_tiles, uint32_t vlimit,
-                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, const PinJob *pj, const SortJob *sj) {
-    oc_group_by *g = gj.g;
-    // sort_groups with pins takes every group's top 2 * max_results (sort.rs:137-142)
-    const bool pin_grp = pj && pj->splice;
-    const uint32_t G = g->n_groups, m = gj.max_results * (pin_grp ? 2 : 1);
-    if (G == 0) return OC_OK;
+static int run_groups(oc_ctx *c, const GroupJob &gj, int mode, const StrSnap *S, uint32_t n_tiles, uint32_t vlimit,
+                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, const PinJob &pj) {
+    const uint32_t R = gj.rows, top = gj.top;
+    if (R == 0) return OC_OK;
     const bool has_ft = mode != OC_MODE_VECTOR && n_tiles > 0;
-    if (has_ft && g->n_docs) {   // the CSR's documents -> string rows (identity, or a binary search over the ascending row_doc)
-        constexpr uint64_t CH = 1ull << 30;
-        for (uint64_t a = 0; a < g->n_docs; a += CH) {
-            const uint32_t len = (uint32_t)std::min<uint64_t>(CH, g->n_docs - a);
-            // counts = rows[n_docs] (~0): every entry of the chunk is mapped
-            map_docs_to_rows_kernel<<<(len + 255) / 256, 256, 0, c->stream>>>(g->docs + a, g->rows + g->n_docs, len, 1, S->row_doc,
-                                                                              S->n_rows, g->rows + a);
-            launched(c);
-            CU(cudaGetLastError());
+    if (has_ft)   // each handle's documents -> string rows (identity, or a binary search over the ascending row_doc)
+        for (oc_group_by *g : gj.h) {
+            constexpr uint64_t CH = 1ull << 30;
+            for (uint64_t a = 0; a < g->n_docs; a += CH) {
+                const uint32_t len = (uint32_t)std::min<uint64_t>(CH, g->n_docs - a);
+                // counts = rows[n_docs] (~0): every entry of the chunk is mapped
+                map_docs_to_rows_kernel<<<(len + 255) / 256, 256, 0, c->stream>>>(g->docs + a, g->rows + g->n_docs, len, 1, S->row_doc,
+                                                                                  S->n_rows, g->rows + a);
+                launched(c);
+                CU(cudaGetLastError());
+            }
         }
-    }
-    const size_t n_out = size_t(B) * G * m;
+    const size_t n_out = size_t(R) * top;
     OCTRY(c->grp_doc.ensure(std::max<size_t>(n_out, 1) * 8));
     OCTRY(c->grp_score.ensure(std::max<size_t>(n_out, 1) * 4));
-    OCTRY(c->grp_n.ensure(size_t(B) * G * 4));
+    OCTRY(c->grp_n.ensure(size_t(R) * 4));
     GroupParams gp{};
-    gp.n_groups = G; gp.max_results = m;
-    gp.kp2 = std::max<uint32_t>(32, next_pow2(m));
+    gp.handles = gj.d_hand;
+    gp.top = top;
+    gp.kp2 = std::max<uint32_t>(32, next_pow2(top));
     gp.vp2 = next_pow2(std::max<uint32_t>(vlimit, 1));
-    gp.g_off = g->off; gp.g_doc = g->docs; gp.g_row = has_ft ? g->rows : nullptr;
     gp.has_ft = has_ft; gp.hybrid = mode == OC_MODE_HYBRID;
     gp.mbits = c->mbits.as<uint32_t>(); gp.row_words = uint64_t(n_tiles) * (BM25_TILE / 32);
     gp.row_ft = c->row_ft.as<float>();
@@ -3217,46 +3263,117 @@ static int run_groups(oc_ctx *c, const GroupJob &gj, uint32_t B, int mode, const
     gp.v_stride = std::max<uint32_t>(vlimit, 1);
     gp.omc_doc = omc_doc; gp.omc_mult = omc_mult; gp.n_omc = n_omc;
     gp.out_doc = c->grp_doc.as<uint64_t>(); gp.out_score = c->grp_score.as<float>(); gp.out_n = c->grp_n.as<uint32_t>();
-    if (sj) { gp.doc_rank = sj->ord(0).doc_rank; gp.rank_nbits = sj->f[0]->nbits; }
-    const void *kern = sj ? (const void *)group_sort_topk_kernel : (const void *)group_topk_kernel;
+    gp.ents = gj.d_ents;
     const size_t smem = (size_t(GROUP_BUF) + gp.kp2 + gp.vp2) * 8 + size_t(gp.vp2) * 4;
-    if (smem_cfg_needed(c->device, kern, smem))
-        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    if (sj) group_sort_topk_kernel<<<dim3(G, B), GROUP_THREADS, smem, c->stream>>>(gp);
-    else group_topk_kernel<<<dim3(G, B), GROUP_THREADS, smem, c->stream>>>(gp);
-    launched(c);
-    CU(cudaGetLastError());
-    if (pj) {   // oc_search_groups_pinned: every group's list at the caller's stride, spliced for the queries with items
-        const size_t n_res = size_t(B) * G * gj.stride;
-        OCTRY(c->pin_gdoc.ensure(std::max<size_t>(n_res, 1) * 8));
-        OCTRY(c->pin_gscore.ensure(std::max<size_t>(n_res, 1) * 4));
-        OCTRY(c->pin_gn.ensure(size_t(B) * G * 4));
-        GroupPinParams xp{};
-        xp.n_groups = G; xp.max_results = gj.max_results; xp.stride = gj.stride; xp.n_top = m;
-        xp.kp2 = std::max<uint32_t>(32, next_pow2(pj->stride));
-        xp.g_off = g->off; xp.g_doc = g->docs;
-        xp.doc = pj->d_doc; xp.pos = pj->d_pos; xp.score = c->pin_score.as<float>();
-        xp.cnt = pin_grp ? pj->d_cnt : nullptr; xp.item_stride = pj->stride;
-        xp.top_doc = gp.out_doc; xp.top_score = gp.out_score; xp.top_n = gp.out_n;
-        xp.out_doc = c->pin_gdoc.as<uint64_t>(); xp.out_score = c->pin_gscore.as<float>(); xp.out_n = c->pin_gn.as<uint32_t>();
-        const size_t psmem = pin_splice_smem(xp.kp2, m, std::min<uint32_t>(gj.stride, m + pj->stride));
-        group_pin_splice_kernel<<<dim3(G, B), PIN_THREADS, psmem, c->stream>>>(xp);
+    for (int by_field = 0; by_field < 2; by_field++) {   // score order, then field order: one launch per work list
+        const uint32_t s0 = by_field ? gj.n_score_spans : 0u, s1 = by_field ? gj.n_spans : gj.n_score_spans;
+        const uint32_t i0 = by_field ? gj.n_score_items : 0u, i1 = by_field ? R : gj.n_score_items;
+        if (i1 == i0) continue;
+        gp.spans = gj.d_spans + s0; gp.n_spans = s1 - s0; gp.item0 = i0;
+        const void *kern = by_field ? (const void *)group_sort_topk_kernel : (const void *)group_topk_kernel;
+        if (smem_cfg_needed(c->device, kern, smem))
+            CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        if (by_field) group_sort_topk_kernel<<<i1 - i0, GROUP_THREADS, smem, c->stream>>>(gp);
+        else group_topk_kernel<<<i1 - i0, GROUP_THREADS, smem, c->stream>>>(gp);
         launched(c);
         CU(cudaGetLastError());
-        if (n_res) {
-            CU(cudaMemcpyAsync(gj.out_doc, xp.out_doc, n_res * 8, cudaMemcpyDeviceToHost, c->stream));
-            CU(cudaMemcpyAsync(gj.out_score, xp.out_score, n_res * 4, cudaMemcpyDeviceToHost, c->stream));
-        }
-        CU(cudaMemcpyAsync(gj.out_n, xp.out_n, size_t(B) * G * 4, cudaMemcpyDeviceToHost, c->stream));
-        return OC_OK;
     }
-    if (n_out) {
-        CU(cudaMemcpyAsync(gj.out_doc, gp.out_doc, n_out * 8, cudaMemcpyDeviceToHost, c->stream));
-        CU(cudaMemcpyAsync(gj.out_score, gp.out_score, n_out * 4, cudaMemcpyDeviceToHost, c->stream));
+    const uint64_t *res_doc = gp.out_doc;
+    const float *res_score = gp.out_score;
+    const uint32_t *res_n = gp.out_n;
+    if (!gj.direct) {   // every list at the caller's stride, spliced for the queries with items
+        const size_t n_res = size_t(R) * gj.stride;
+        OCTRY(c->pin_gdoc.ensure(std::max<size_t>(n_res, 1) * 8));
+        OCTRY(c->pin_gscore.ensure(std::max<size_t>(n_res, 1) * 4));
+        OCTRY(c->pin_gn.ensure(size_t(R) * 4));
+        GroupPinParams xp{};
+        xp.handles = gj.d_hand; xp.spans = gj.d_spans; xp.n_spans = gj.n_spans;
+        xp.stride = gj.stride; xp.top = top;
+        xp.kp2 = std::max<uint32_t>(32, next_pow2(pj.stride));
+        xp.doc = pj.d_doc; xp.pos = pj.d_pos; xp.score = c->pin_score.as<float>();
+        xp.cnt = pj.splice ? pj.d_cnt : nullptr; xp.item_stride = pj.stride;
+        xp.top_doc = gp.out_doc; xp.top_score = gp.out_score; xp.top_n = gp.out_n;
+        xp.out_doc = c->pin_gdoc.as<uint64_t>(); xp.out_score = c->pin_gscore.as<float>(); xp.out_n = c->pin_gn.as<uint32_t>();
+        const size_t psmem = pin_splice_smem(xp.kp2, top, std::min<uint32_t>(gj.stride, top + pj.stride));
+        group_pin_splice_kernel<<<R, PIN_THREADS, psmem, c->stream>>>(xp);
+        launched(c);
+        CU(cudaGetLastError());
+        res_doc = xp.out_doc; res_score = xp.out_score; res_n = xp.out_n;
     }
-    CU(cudaMemcpyAsync(gj.out_n, gp.out_n, size_t(B) * G * 4, cudaMemcpyDeviceToHost, c->stream));
+    const size_t n_res = size_t(R) * gj.stride;
+    if (n_res) {
+        CU(cudaMemcpyAsync(gj.out_doc, res_doc, n_res * 8, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaMemcpyAsync(gj.out_score, res_score, n_res * 4, cudaMemcpyDeviceToHost, c->stream));
+    }
+    CU(cudaMemcpyAsync(gj.out_n, res_n, size_t(R) * 4, cudaMemcpyDeviceToHost, c->stream));
     return OC_OK;
 }
+
+static int pins_check_flat(const oc_search_params *p, const PinJob &pj) {
+    if (p->sharded) return fail(OC_ERR_UNSUPPORTED, "pins over a sharded search: scores and the hybrid normalisation are global");
+    if (pj.splice && (uint64_t(p->limit) + p->offset) * 2 > OC_MAX_TOPK)
+        return fail(OC_ERR_UNSUPPORTED, "pins: 2 x (limit+offset) %llu > %u", (unsigned long long)(uint64_t(p->limit) + p->offset) * 2,
+                    OC_MAX_TOPK);
+    return OC_OK;
+}
+
+// The one path of the grouped calls: query b takes q[b] (groups NULL: no groups) with its items and, per_query
+// (oc_search_q_groups), its q_filters entry; the flat hits follow oc_search_q_sorted.  The wrappers below pass one
+// request for every query.  Nothing is written on failure.
+static int groups_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, const oc_group_req *q, const oc_pins *pins,
+                       uint32_t group_stride, bool per_query, uint64_t *out_doc_ids, float *out_scores, double *out_sort_values,
+                       uint32_t *out_n, uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present,
+                       uint64_t *out_group_doc_ids, float *out_group_scores, double *out_group_sort_values, uint32_t *out_group_n) {
+    if (!c || !p || !q || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
+    const uint32_t B = p->n_queries;
+    SortJob sj{};
+    for (uint32_t b = 0; b < B; b++) OCTRY(sort_job_add(c, q[b].sort, sj));
+    sj.out_values = out_sort_values;
+    PinJob pj;
+    pj.q_filters = per_query;
+    OCTRY(pin_job_init(pins, B, pj));
+    OCTRY(pins_check_flat(p, pj));
+    GroupJob gj;
+    gj.q_h.assign(B, GROUP_NONE);
+    gj.q_m.assign(B, 0);
+    gj.q_row.assign(B, 0);
+    uint64_t rows = 0;
+    bool flat_only = false;   // some query has no groups: its hits are oc_search_q_sorted's, which needs limit >= 1
+    for (uint32_t b = 0; b < B; b++) {
+        const oc_group_by *g = q[b].groups;
+        if (!g) { flat_only = true; continue; }
+        if (g->ctx != c) return fail(OC_ERR_INVALID, "group_by of query %u belongs to another ctx", b);
+        const uint32_t m = q[b].max_results;
+        if (m > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "query %u: max_results %u > %u", b, m, OC_MAX_TOPK);
+        const bool active = pj.splice && pj.cnt[b] > 0;
+        if (active && 2 * m > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "query %u: pins: 2 x max_results %u > %u", b, 2 * m, OC_MAX_TOPK);
+        const uint64_t need = active ? 2ull * m + pj.cnt[b] : m;
+        if (group_stride < need)
+            return fail(OC_ERR_INVALID, "query %u: group_stride %u < %llu", b, group_stride, (unsigned long long)need);
+        uint32_t h = 0;
+        while (h < gj.h.size() && gj.h[h] != g) h++;
+        if (h == gj.h.size()) gj.h.push_back(const_cast<oc_group_by *>(g));   // only its per-call row map is refreshed, under the ctx lock
+        gj.q_h[b] = h; gj.q_m[b] = m; gj.q_row[b] = (uint32_t)rows;   // refused below past 2^31 rows
+        rows += g->n_groups;
+    }
+    if (flat_only && p->limit == 0) return fail(OC_ERR_INVALID, "limit must be >= 1 when a query has no groups");
+    // the work list is a 1-D grid of (query, group) items
+    if (rows > 0x7fffffffull) return fail(OC_ERR_UNSUPPORTED, "groups: %llu (query, group) rows >= 2^31", (unsigned long long)rows);
+    if (rows && (!out_group_n || (group_stride && (!out_group_doc_ids || !out_group_scores)))) return fail(OC_ERR_INVALID, "NULL group output");
+    gj.rows = (uint32_t)rows; gj.stride = group_stride;
+    gj.out_doc = out_group_doc_ids; gj.out_score = out_group_scores; gj.out_n = out_group_n; gj.out_values = out_group_sort_values;
+    // every query in score order: the flat hits are oc_search_pinned's (sort values NaN)
+    const SortJob *sjp = sj.f.empty() ? nullptr : &sj;
+    OCTRY(search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, &gj, &pj, pins, out_pin_scores,
+                      out_pin_present, sjp));
+    if (!sjp && out_sort_values && p->limit > 0)
+        for (uint32_t b = 0; b < B; b++)
+            for (uint32_t i = 0; i < p->limit; i++)
+                out_sort_values[size_t(b) * p->limit + i] = i < out_n[b] ? std::numeric_limits<double>::quiet_NaN() : 0.0;
+    return OC_OK;
+}
+
+extern "C" uint64_t oc_group_by_n_groups(const oc_group_by *g) { return g ? g->n_groups : 0; }
 
 extern "C" int oc_search_groups(oc_ctx *c, oc_emb *emb, oc_str *str, oc_group_by *groups, const oc_search_params *p,
                                 uint32_t max_results, uint64_t *out_doc_ids, float *out_scores, uint32_t *out_n, uint64_t *out_count,
@@ -3268,18 +3385,12 @@ extern "C" int oc_search_groups(oc_ctx *c, oc_emb *emb, oc_str *str, oc_group_by
     if (p->sharded) return fail(OC_ERR_UNSUPPORTED, "groups over a sharded search: hybrid normalisation and the vector set are global");
     if (max_results > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "max_results %u > %u", max_results, OC_MAX_TOPK);
     if (p->n_queries > 65535) return fail(OC_ERR_UNSUPPORTED, "groups: n_queries %u > 65535", p->n_queries);
-    GroupJob gj{groups, max_results, out_group_doc_ids, out_group_scores, out_group_n};
-    return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, &gj);
+    const std::vector<oc_group_req> req(p->n_queries, oc_group_req{groups, max_results, oc_sort{nullptr, OC_SORT_ASC}});
+    return groups_impl(c, emb, str, p, req.data(), nullptr, max_results, false, out_doc_ids, out_scores, nullptr, out_n, out_count,
+                       nullptr, nullptr, out_group_doc_ids, out_group_scores, nullptr, out_group_n);
 }
 
 // ------------------------------------------------------------------------------------ pin rules (pins.cuh)
-static int pins_check_flat(const oc_search_params *p, const PinJob &pj) {
-    if (p->sharded) return fail(OC_ERR_UNSUPPORTED, "pins over a sharded search: scores and the hybrid normalisation are global");
-    if (pj.splice && (uint64_t(p->limit) + p->offset) * 2 > OC_MAX_TOPK)
-        return fail(OC_ERR_UNSUPPORTED, "pins: 2 x (limit+offset) %llu > %u", (unsigned long long)(uint64_t(p->limit) + p->offset) * 2,
-                    OC_MAX_TOPK);
-    return OC_OK;
-}
 
 extern "C" int oc_search_pinned(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, const oc_pins *pins,
                                 uint64_t *out_doc_ids, float *out_scores, uint32_t *out_n, uint64_t *out_count,
@@ -3309,9 +3420,9 @@ extern "C" int oc_search_groups_pinned(oc_ctx *c, oc_emb *emb, oc_str *str, oc_g
         return fail(OC_ERR_UNSUPPORTED, "pins: 2 x max_results %u > %u", 2 * max_results, OC_MAX_TOPK);
     const uint64_t need = pj.splice ? 2ull * max_results + pj.stride : max_results;
     if (group_stride < need) return fail(OC_ERR_INVALID, "group_stride %u < %llu", group_stride, (unsigned long long)need);
-    GroupJob gj{groups, max_results, out_group_doc_ids, out_group_scores, out_group_n};
-    gj.stride = group_stride;
-    return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, &gj, &pj, pins);
+    const std::vector<oc_group_req> req(p->n_queries, oc_group_req{groups, max_results, oc_sort{nullptr, OC_SORT_ASC}});
+    return groups_impl(c, emb, str, p, req.data(), pins, group_stride, false, out_doc_ids, out_scores, nullptr, out_n, out_count,
+                       nullptr, nullptr, out_group_doc_ids, out_group_scores, nullptr, out_group_n);
 }
 
 // ------------------------------------------------------------------------------------ sortBy (sort.cuh)
@@ -3396,7 +3507,6 @@ extern "C" int oc_search_groups_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, oc_g
     if (groups->ctx != c) return fail(OC_ERR_INVALID, "group_by belongs to another ctx");
     SortJob sj{};
     OCTRY(sort_job_init(c, sort, p->n_queries, sj));
-    sj.out_values = out_sort_values; sj.out_group_values = out_group_sort_values; sj.n_groups = groups->n_groups;
     if (max_results > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "max_results %u > %u", max_results, OC_MAX_TOPK);
     if (p->n_queries > 65535) return fail(OC_ERR_UNSUPPORTED, "groups: n_queries %u > 65535", p->n_queries);
     PinJob pj;
@@ -3406,9 +3516,9 @@ extern "C" int oc_search_groups_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, oc_g
         return fail(OC_ERR_UNSUPPORTED, "pins: 2 x max_results %u > %u", 2 * max_results, OC_MAX_TOPK);
     const uint64_t need = pj.splice ? 2ull * max_results + pj.stride : max_results;
     if (group_stride < need) return fail(OC_ERR_INVALID, "group_stride %u < %llu", group_stride, (unsigned long long)need);
-    GroupJob gj{groups, max_results, out_group_doc_ids, out_group_scores, out_group_n};
-    gj.stride = group_stride;
-    return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, &gj, &pj, pins, nullptr, nullptr, &sj);
+    const std::vector<oc_group_req> req(p->n_queries, oc_group_req{groups, max_results, *sort});
+    return groups_impl(c, emb, str, p, req.data(), pins, group_stride, false, out_doc_ids, out_scores, out_sort_values, out_n,
+                       out_count, nullptr, nullptr, out_group_doc_ids, out_group_scores, out_group_sort_values, out_group_n);
 }
 
 // One batch in which every query has its own sort (or score order), its own pins and, with q_filters, its own filter:
@@ -3435,6 +3545,19 @@ extern "C" int oc_search_q_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_
             for (uint32_t i = 0; i < p->limit; i++)
                 out_sort_values[size_t(q) * p->limit + i] = i < out_n[q] ? std::numeric_limits<double>::quiet_NaN() : 0.0;
     return OC_OK;
+}
+
+// One batch in which every query has its own groups (or none), sort, pins and, with q_filters, filter: query b gets what
+// it gets alone through the grouped call or oc_search_q_sorted its request stands for.
+extern "C" int oc_search_q_groups(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, const oc_group_req *q_groups,
+                                  const oc_pins *pins, uint32_t group_stride, uint64_t *out_doc_ids, float *out_scores,
+                                  double *out_sort_values, uint32_t *out_n, uint64_t *out_count, float *out_pin_scores,
+                                  uint8_t *out_pin_present, uint64_t *out_group_doc_ids, float *out_group_scores,
+                                  double *out_group_sort_values, uint32_t *out_group_n) {
+    if (!c || !p || !q_groups) return fail(OC_ERR_INVALID, "NULL argument");
+    if (p->sharded) return fail(OC_ERR_UNSUPPORTED, "groups over a sharded search: hybrid normalisation and the vector set are global");
+    return groups_impl(c, emb, str, p, q_groups, pins, group_stride, true, out_doc_ids, out_scores, out_sort_values, out_n, out_count,
+                       out_pin_scores, out_pin_present, out_group_doc_ids, out_group_scores, out_group_sort_values, out_group_n);
 }
 
 // ------------------------------------------------------------------------------------ geopoint where-filter leaves (geo.cuh)
@@ -3577,11 +3700,20 @@ struct OcSortedExec {
         return oc_search_q_sorted(c, e, s, p, q_sorts, pins, docs, scores, sort_values, n, count, pin_scores, pin_present);
     }
 };
+struct OcGroupedExec {
+    oc_ctx *c; oc_emb *e; oc_str *s;
+    int operator()(const oc_search_params *p, const oc_group_req *q_groups, const oc_pins *pins, uint32_t group_stride, uint64_t *docs,
+                   float *scores, double *sort_values, uint32_t *n, uint64_t *count, float *pin_scores, uint8_t *pin_present,
+                   uint64_t *g_docs, float *g_scores, double *g_values, uint32_t *g_n) const {
+        return oc_search_q_groups(c, e, s, p, q_groups, pins, group_stride, docs, scores, sort_values, n, count, pin_scores, pin_present,
+                                  g_docs, g_scores, g_values, g_n);
+    }
+};
 struct oc_batcher {
-    ocb::Batcher<OcSearchExec, OcSortedExec> q;
+    ocb::Batcher<OcSearchExec, OcSortedExec, OcGroupedExec> q;
     oc_ctx *ctx;
     oc_batcher(OcSearchExec x, uint32_t dim, uint32_t mb, uint32_t mw)
-        : q(x, dim, mb, mw, x.e != nullptr, x.s != nullptr, OcSortedExec{x.c, x.e, x.s}), ctx(x.c) {}
+        : q(x, dim, mb, mw, x.e != nullptr, x.s != nullptr, OcSortedExec{x.c, x.e, x.s}, OcGroupedExec{x.c, x.e, x.s}), ctx(x.c) {}
 };
 extern "C" int oc_batcher_create(oc_ctx *c, oc_emb *emb, oc_str *str, uint32_t max_batch, uint32_t max_wait_us, oc_batcher **out) {
     if (!c || !out || (!emb && !str)) return fail(OC_ERR_INVALID, "bad arguments");
@@ -3617,6 +3749,32 @@ extern "C" int oc_batcher_search_sorted(oc_batcher *b, const oc_search_params *p
     const int rc = b->q.submit_sorted(p, sort, pins, out_doc_ids, out_scores, out_sort_values, out_n, out_count, out_pin_scores,
                                       out_pin_present);
     if (rc != OC_OK && g_err[0] == 0) return fail(rc, "the coalesced search of this query's batch failed (detail on the leading caller's thread)");
+    return rc;
+}
+extern "C" int oc_batcher_search_groups(oc_batcher *b, const oc_search_params *p, const oc_group_req *req, const oc_pins *pins,
+                                        uint32_t group_stride, uint64_t *out_doc_ids, float *out_scores, double *out_sort_values,
+                                        uint32_t *out_n, uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present,
+                                        uint64_t *out_group_doc_ids, float *out_group_scores, double *out_group_sort_values,
+                                        uint32_t *out_group_n) {
+    if (!b || !p || !req || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
+    if (p->limit && (!out_doc_ids || !out_scores || !out_n)) return fail(OC_ERR_INVALID, "NULL argument");
+    if (p->n_queries != 1) return fail(OC_ERR_INVALID, "oc_batcher_search_groups takes one query per call (n_queries = %u)", p->n_queries);
+    // what would fail a whole batch is refused here, before the request joins one
+    if (p->filter && p->filter->ctx != b->ctx) return fail(OC_ERR_INVALID, "filter belongs to another ctx");
+    if (req->sort.field && req->sort.field->ctx != b->ctx) return fail(OC_ERR_INVALID, "sort field belongs to another ctx");
+    if (req->groups && req->groups->ctx != b->ctx) return fail(OC_ERR_INVALID, "group_by belongs to another ctx");
+    const uint64_t n_groups = oc_group_by_n_groups(req->groups);
+    if (n_groups && (!out_group_n || (group_stride && (!out_group_doc_ids || !out_group_scores))))
+        return fail(OC_ERR_INVALID, "NULL group output");
+    const char *why = nullptr;
+    if (const int rc = ocb::check_sorted(&req->sort, pins, &why)) return fail(rc, "%s", why);
+    if (group_stride < ocb::group_need(req, pins))
+        return fail(OC_ERR_INVALID, "group_stride %u < %llu", group_stride, (unsigned long long)ocb::group_need(req, pins));
+    g_err[0] = 0;
+    const int rc = b->q.submit_groups(p, req, n_groups, pins, group_stride, out_doc_ids, out_scores, out_sort_values, out_n, out_count,
+                                      out_pin_scores, out_pin_present, out_group_doc_ids, out_group_scores, out_group_sort_values,
+                                      out_group_n);
+    if (rc != OC_OK && g_err[0] == 0) return fail(rc, "the coalesced grouped search of this query's batch failed (detail on the leading caller's thread)");
     return rc;
 }
 extern "C" int oc_batcher_stats(oc_batcher *b, uint64_t *n_queries, uint64_t *n_batches, uint64_t *n_direct) {

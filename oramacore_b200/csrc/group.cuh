@@ -18,12 +18,52 @@ constexpr uint32_t GROUP_THREADS = 256;
 constexpr uint32_t GROUP_CHUNK = GROUP_THREADS * 4;   // documents visited between two looks at the candidate buffer
 constexpr uint32_t GROUP_BUF = 2048;                  // candidate keys in shared memory: >= OC_MAX_TOPK + GROUP_CHUNK
 
-struct GroupParams {
-    uint32_t n_groups, max_results;
-    uint32_t kp2, vp2;              // selection scratch: max(32, next_pow2(max_results)); vector hits: next_pow2(v_stride)
+// One distinct (field, order) of a batch: its documents in rank order and the maps between ranks, ids and rows.  The
+// entries of sort_walk_kernel (sort.cuh); group_sort_topk_kernel takes the rank of each document id from them.
+struct SortEntry {
+    uint64_t n_ranks;               // documents with a value
+    const uint32_t *rank_row;       // [n_ranks] string row of each rank, RANK_NONE = none; NULL without a fulltext map
+    const uint32_t *doc_rank;       // [nbits] rank of each document id, RANK_NONE = no value
+    uint64_t nbits;
+    const uint64_t *rank_doc;       // [n_ranks]
+};
+
+// One distinct oc_group_by of a batch: its CSR.
+struct GroupHandle {
     const uint64_t *g_off;          // [n_groups + 1] group CSR
     const uint64_t *g_doc;          // document ids, ascending inside each group
     const uint32_t *g_row;          // string row of each entry (0xffffffff = none); NULL without a fulltext map
+    uint32_t n_groups;
+};
+// One query's groups in a work list of (query, group) items, one CTA each: items [first, first + n_groups of its
+// handle).  Query q's group g is output row row + g.
+struct GroupSpan {
+    uint32_t first;                 // its first item (the list's prefix sum of n_groups)
+    uint32_t q, h;                  // query, index into the handle table
+    uint32_t depth;                 // top list depth: max_results, 2 x max_results for an active pinned query
+    uint32_t max_results;
+    uint32_t ent;                   // group_sort_topk_kernel: index into the sort entries
+    uint32_t row;
+};
+// The span that holds `item`, the local-th of the list's n_items: the last one with first <= item (every span of a list
+// holds at least one item).  The first guess, local's share of the n spans, is exact when every span has as many items
+// (one handle for the whole list), so the common case costs one round of loads instead of a binary search.
+__device__ __forceinline__ GroupSpan group_span_of(const GroupSpan *s, uint32_t n, uint32_t item, uint32_t local, uint32_t n_items) {
+    uint32_t lo = uint32_t(uint64_t(local) * n / n_items);
+    const uint32_t next = lo + 1 < n ? s[lo + 1].first : 0xffffffffu;
+    if (s[lo].first <= item && item < next) return s[lo];
+    uint32_t hi = n;
+    lo = 0;
+    while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (s[mid].first <= item) lo = mid; else hi = mid; }
+    return s[lo];
+}
+
+struct GroupParams {
+    const GroupHandle *handles;
+    const GroupSpan *spans;         // this launch's work list: n_spans spans, items item0 + blockIdx.x
+    uint32_t n_spans, item0;
+    uint32_t top;                   // row stride of the top lists: the largest depth of the batch
+    uint32_t kp2, vp2;              // selection scratch: max(32, next_pow2(top)); vector hits: next_pow2(v_stride)
     // fulltext part of the score map (has_ft)
     bool has_ft, hybrid;
     const uint32_t *mbits;          // [q][row_words]
@@ -38,12 +78,11 @@ struct GroupParams {
     const uint64_t *omc_doc;
     const float *omc_mult;
     uint32_t n_omc;
-    uint64_t *out_doc;              // [q][n_groups][max_results]
+    uint64_t *out_doc;              // [row][top]
     float *out_score;
-    uint32_t *out_n;                // [q][n_groups]
-    // group_sort_topk_kernel: the sort field's rank of each document id (0xffffffff = no value)
-    const uint32_t *doc_rank;
-    uint64_t rank_nbits;
+    uint32_t *out_n;                // [row]
+    // group_sort_topk_kernel: the batch's sort entries (sort.cuh); a span's entry gives the rank of each document id
+    const SortEntry *ents;
 };
 
 // SORT = false: the top max_results members by score (score desc, ties by ascending id, NaN dropped).
@@ -58,16 +97,28 @@ __device__ __forceinline__ void group_topk_body(const GroupParams &p) {
     float *hsc = reinterpret_cast<float *>(hdoc + p.vp2);  // [vp2] their scores
     __shared__ uint32_t s_n;
     __shared__ unsigned long long s_tau;
-    const uint32_t g = blockIdx.x, q = blockIdx.y, tid = threadIdx.x;
-    const uint32_t m = p.max_results;
-    const size_t og = size_t(q) * p.n_groups + g;
-    if (m == 0) {
-        if (tid == 0) p.out_n[og] = 0;
+    // this CTA's span, with `first` turned into its group and `row` into its output row; read from shared memory
+    // wherever a value must outlive a call of block_select_largest (kept in registers, it would be saved to the stack
+    // around every call)
+    __shared__ GroupSpan s_sp;
+    const uint32_t tid = threadIdx.x;
+    if (tid == 0) {
+        const uint32_t item = p.item0 + blockIdx.x;
+        GroupSpan sp = group_span_of(p.spans, p.n_spans, item, blockIdx.x, gridDim.x);
+        sp.row += item - sp.first;
+        sp.first = item - sp.first;
+        s_sp = sp;
+    }
+    __syncthreads();
+    const GroupHandle gh = p.handles[s_sp.h];
+    const uint32_t g = s_sp.first, q = s_sp.q;
+    if (s_sp.depth == 0) {
+        if (tid == 0) p.out_n[s_sp.row] = 0;
         return;
     }
-    const uint64_t base = p.g_off[g], n = p.g_off[g + 1] - base;
-    const uint64_t *gdoc = p.g_doc + base;
-    const uint32_t *grow = p.g_row ? p.g_row + base : nullptr;
+    const uint64_t base = gh.g_off[g], n = gh.g_off[g + 1] - base;
+    const uint64_t *gdoc = gh.g_doc + base;
+    const uint32_t *grow = gh.g_row ? gh.g_row + base : nullptr;
 
     const uint32_t vc = p.v_n[q];
     if (vc) {   // bitonic sort of the query's hits by document id (ascending, padding last)
@@ -112,7 +163,8 @@ __device__ __forceinline__ void group_topk_body(const GroupParams &p) {
     auto load = [&](uint64_t i) -> uint64_t {
         if constexpr (SORT) {   // larger key = smaller rank; ranks are unique, so the member index only decodes
             const uint64_t d = gdoc[i];
-            const uint32_t r = d < p.rank_nbits ? p.doc_rank[d] : 0xffffffffu;
+            const SortEntry &e = p.ents[s_sp.ent];
+            const uint32_t r = d < e.nbits ? e.doc_rank[d] : 0xffffffffu;
             if (r == 0xffffffffu) return KEY_NONE;
             bool present;
             map_value(i, &present);
@@ -152,7 +204,7 @@ __device__ __forceinline__ void group_topk_body(const GroupParams &p) {
         const uint32_t cnt = s_n;   // snapshot, then barrier, so the branch is block-uniform
         __syncthreads();
         if (cnt + GROUP_CHUNK > GROUP_BUF && c0 + GROUP_CHUNK < n) {
-            const uint32_t kept = block_select_largest(buf, cnt, m, sel);
+            const uint32_t kept = block_select_largest(buf, cnt, s_sp.depth, sel);
             group_bitonic_desc(sel, p.kp2, tid, blockDim.x, 0);
             for (uint32_t i = tid; i < p.kp2; i += blockDim.x) {
                 if (i < kept) buf[i] = sel[i];
@@ -161,15 +213,16 @@ __device__ __forceinline__ void group_topk_body(const GroupParams &p) {
             __syncthreads();
             if (tid == 0) {
                 s_n = kept;
-                if (kept == m) s_tau = buf[m - 1];
+                if (kept == s_sp.depth) s_tau = buf[s_sp.depth - 1];
             }
             __syncthreads();
         }
     }
     const uint32_t cnt = s_n;
-    const uint32_t kept = block_select_largest(buf, cnt, m, sel);
+    const uint32_t kept = block_select_largest(buf, cnt, s_sp.depth, sel);
     group_bitonic_desc(sel, p.kp2, tid, blockDim.x, 0);
-    for (uint32_t i = tid; i < m; i += blockDim.x) {
+    const size_t og = s_sp.row;
+    for (uint32_t i = tid; i < s_sp.depth; i += blockDim.x) {
         uint64_t doc = 0;
         float sc = 0.f;
         if (i < kept) {
@@ -181,13 +234,13 @@ __device__ __forceinline__ void group_topk_body(const GroupParams &p) {
                 sc = key_score(sel[i]);
             }
         }
-        p.out_doc[og * m + i] = doc;
-        p.out_score[og * m + i] = sc;
+        p.out_doc[og * p.top + i] = doc;
+        p.out_score[og * p.top + i] = sc;
     }
     if (tid == 0) p.out_n[og] = kept;
 }
 
-// one CTA per (group, query): grid (n_groups, n_queries)
+// one CTA per (query, group) item of the work list: a 1-D grid over the list's items
 __global__ void __launch_bounds__(GROUP_THREADS) group_topk_kernel(const GroupParams p) { group_topk_body<false>(p); }
 __global__ void __launch_bounds__(GROUP_THREADS) group_sort_topk_kernel(const GroupParams p) { group_topk_body<true>(p); }
 

@@ -10,7 +10,7 @@
 //                           through fused_ft_score; a document that is not a key scores 0.0 and is "not present".
 //   pin_splice_kernel       one CTA per query over K4's top 2 * (limit + offset) (or, sorted, the walk's list): remove
 //                           the promoted ids, insert the items stably sorted by position, then skip(offset).take(limit).
-//   group_pin_splice_kernel one CTA per (group, query) over group_topk_kernel's top 2 * max_results: the same splice
+//   group_pin_splice_kernel one CTA per (query, group) over group_topk_kernel's top 2 * max_results: the same splice
 //                           with the items restricted to the group's members, not truncated afterwards.
 #pragma once
 #include "group.cuh"
@@ -202,31 +202,36 @@ __global__ void __launch_bounds__(PIN_THREADS) pin_splice_kernel(const PinSplice
 }
 
 struct GroupPinParams {
-    uint32_t n_groups, max_results, stride, n_top, kp2;   // n_top = group_topk_kernel's depth (2 * max_results)
-    const uint64_t *g_off, *g_doc;                        // group CSR, documents ascending inside a group
+    const GroupHandle *handles;
+    const GroupSpan *spans;                               // the whole batch's work list, items 0 .. n_items - 1
+    uint32_t n_spans;
+    uint32_t stride, top, kp2;                            // output row stride; group_topk_kernel's row stride
     const uint64_t *doc;                                  // [q][item_stride] items, as PinSpliceParams
     const uint32_t *pos;
     const float *score;
     const uint32_t *cnt;                                  // NULL: the pins do not apply (every list is the top max_results)
     uint32_t item_stride;
-    const uint64_t *top_doc;                              // [q][g][n_top]
+    const uint64_t *top_doc;                              // [row][top]
     const float *top_score;
-    const uint32_t *top_n;                                // [q][g]
-    uint64_t *out_doc;                                    // [q][g][stride]
+    const uint32_t *top_n;                                // [row]
+    uint64_t *out_doc;                                    // [row][stride]
     float *out_score;
-    uint32_t *out_n;                                      // [q][g]
+    uint32_t *out_n;                                      // [row]
 };
 
-// one CTA per (group, query): grid (n_groups, n_queries).  An active query splices the items whose document is a member
-// of the group into the group's top 2 * max_results and keeps the whole list; a query without items keeps the top
+// one CTA per (query, group) item of the work list.  An active query splices the items whose document is a member of
+// the group into the group's top 2 * max_results and keeps the whole list; a query without items keeps the top
 // max_results, exactly what group_topk_kernel computes at that depth.
 __global__ void __launch_bounds__(PIN_THREADS) group_pin_splice_kernel(const GroupPinParams p) {
     extern __shared__ __align__(16) uint8_t smem[];
-    const uint32_t g = blockIdx.x, q = blockIdx.y;
-    const size_t og = size_t(q) * p.n_groups + g, it = size_t(q) * p.item_stride;
+    const uint32_t item = blockIdx.x;
+    const GroupSpan sp = group_span_of(p.spans, p.n_spans, item, item, gridDim.x);
+    const GroupHandle gh = p.handles[sp.h];
+    const uint32_t g = item - sp.first, q = sp.q;
+    const size_t og = size_t(sp.row) + g, it = size_t(q) * p.item_stride;
     const uint32_t k = p.cnt ? p.cnt[q] : 0u;
-    const uint64_t gb = p.g_off[g], gn = p.g_off[g + 1] - gb;
-    const uint64_t *gdoc = p.g_doc + gb;
+    const uint64_t gb = gh.g_off[g], gn = gh.g_off[g + 1] - gb;
+    const uint64_t *gdoc = gh.g_doc + gb;
     const uint64_t *idoc = p.doc + it;
     auto member = [&](uint32_t j) {
         const uint64_t d = idoc[j];
@@ -234,8 +239,8 @@ __global__ void __launch_bounds__(PIN_THREADS) group_pin_splice_kernel(const Gro
         while (lo < hi) { const uint64_t mid = (lo + hi) >> 1; if (gdoc[mid] < d) lo = mid + 1; else hi = mid; }
         return lo < gn && gdoc[lo] == d;
     };
-    const uint32_t n = pin_splice_block(p.top_doc + og * p.n_top, p.top_score + og * p.n_top, p.top_n[og], idoc, p.pos + it,
-                                        p.score + it, k, p.kp2, member, 0, k ? p.stride : p.max_results,
+    const uint32_t n = pin_splice_block(p.top_doc + og * p.top, p.top_score + og * p.top, p.top_n[og], idoc, p.pos + it,
+                                        p.score + it, k, p.kp2, member, 0, k ? p.stride : sp.max_results,
                                         p.out_doc + og * p.stride, p.out_score + og * p.stride, smem);
     for (uint32_t i = n + threadIdx.x; i < p.stride; i += blockDim.x) { p.out_doc[og * p.stride + i] = 0; p.out_score[og * p.stride + i] = 0.f; }
     if (threadIdx.x == 0) p.out_n[og] = n;

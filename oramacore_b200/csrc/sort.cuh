@@ -23,14 +23,7 @@ constexpr uint32_t SORT_PER_THREAD = 4;                      // consecutive rank
 constexpr uint32_t SORT_CHUNK = SORT_THREADS * SORT_PER_THREAD;
 constexpr uint32_t RANK_NONE = 0xffffffffu;
 
-// One distinct (field, order) of a batch: its documents in rank order and the maps between ranks, ids and rows.
-struct SortEntry {
-    uint64_t n_ranks;               // documents with a value
-    const uint32_t *rank_row;       // [n_ranks] string row of each rank, RANK_NONE = none; NULL without a fulltext map
-    const uint32_t *doc_rank;       // [nbits] rank of each document id, RANK_NONE = no value
-    uint64_t nbits;
-    const uint64_t *rank_doc;       // [n_ranks]
-};
+// SortEntry (group.cuh): one distinct (field, order) of a batch.
 constexpr uint32_t SORT_BY_SCORE = 0xffffffffu;   // SortQuery::ent of a query in score order: no walk, no keys
 struct SortQuery {
     uint32_t ent;                   // index into SortWalkParams::ents, or SORT_BY_SCORE

@@ -803,6 +803,78 @@ def search_q_sorted_arrays(tsc: "TokenScoreContext", params: "TokenScoreParams",
     return docs, scores, sv, n, cnt, ps[:n_items], pp[:n_items]
 
 
+def _group_reqs(groups, B: int):
+    """oc_group_req[B] and the group row of each query from `groups`: per query None (no groups, score order) or a
+    (GroupBy or None, max_results[, (SortField, order)]) tuple."""
+    if len(groups) != B:
+        raise ValueError(f"groups has {len(groups)} entries for {B} queries")
+    arr = (_lib.GroupReq * max(B, 1))()
+    rows = np.zeros(B + 1, np.int64)
+    for i, g in enumerate(groups):
+        rows[i + 1] = rows[i]
+        if g is None:
+            continue
+        if g[0] is not None:
+            arr[i].groups, arr[i].max_results = g[0]._h, int(g[1])
+            rows[i + 1] += g[0].n_groups
+        if len(g) > 2 and g[2] is not None:
+            arr[i].sort = _sort(*g[2])
+    return arr, rows
+
+
+def _group_need(g, k: int) -> int:
+    """The group stride one request needs: 2 * max_results + its items when it has items, else max_results."""
+    if g is None or g[0] is None:
+        return 0
+    return 2 * int(g[1]) + k if k else int(g[1])
+
+
+def search_q_groups_arrays(tsc: "TokenScoreContext", params: "TokenScoreParams", groups, promote=None, texts=None,
+                           q_vecs: Optional[np.ndarray] = None, group_stride: Optional[int] = None):
+    """oc_search_q_groups: one batch in which every query has its own groupBy, sortBy and pin rules, and
+    (params.device_filters) its own where-filter.  `groups[b]`: None (no groups: the hits of search_q_sorted_arrays in
+    score order), or (GroupBy, max_results) or (GroupBy, max_results, (SortField, order)); `promote` as in
+    search_pinned_arrays.  (None, 0, (SortField, order)) is a query without groups in field order.  Query b gets what it
+    gets alone from search_groups_arrays (with its sort and items) or, without groups, search_q_sorted_arrays.  group_stride: default the largest need of the batch.  Returns (docs [B,limit],
+    scores, sort values [B,limit], n [B], count [B], pin scores [items], pin present [items], group docs [rows,stride],
+    group scores, group sort values [rows,stride], group n [rows], rows [B+1]): query b's groups are the rows
+    [rows[b], rows[b+1])."""
+    sp, keep, B = tsc._build_params(params, texts, q_vecs)
+    req, rows = _group_reqs(groups, B)
+    pins = None if promote is None else _pins(promote, B)[0]
+    n_items = 0 if pins is None else int(pins._keep[0][-1])
+    if group_stride is None:
+        k = [0] * B if promote is None else [len(x) for x in promote]
+        group_stride = max([0] + [_group_need(g, k[b]) for b, g in enumerate(groups)])
+    L, R, S = params.limit_hint, int(rows[-1]), int(group_stride)
+    docs, scores, sv = np.zeros((B, L), np.uint64), np.zeros((B, L), np.float32), np.zeros((B, L), np.float64)
+    n, cnt = np.zeros(B, np.uint32), np.zeros(B, np.uint64)
+    ps, pp = np.zeros(max(n_items, 1), np.float32), np.zeros(max(n_items, 1), np.uint8)
+    gd, gs, gsv = np.zeros((R, S), np.uint64), np.zeros((R, S), np.float32), np.zeros((R, S), np.float64)
+    gn = np.zeros(R, np.uint32)
+    check(lib().oc_search_q_groups(tsc.ctx._h, tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None, C.byref(sp),
+                                   req, None if pins is None else C.byref(pins), S, _p(docs), _p(scores), _p(sv), _p(n),
+                                   _p(cnt), _p(ps), _p(pp), _p(gd), _p(gs), _p(gsv), _p(gn)))
+    return docs, scores, sv, n, cnt, ps[:n_items], pp[:n_items], gd, gs, gsv, gn, rows
+
+
+def search_q_groups(tsc: "TokenScoreContext", params: "TokenScoreParams", groups, promote=None, texts=None,
+                    q_vecs: Optional[np.ndarray] = None):
+    """search_q_groups_arrays as search_groups returns it: per query (hits, groups), groups None for a query without
+    groupBy."""
+    docs, scores, _, n, cnt, _, _, gd, gs, _, gn, rows = search_q_groups_arrays(tsc, params, groups, promote, texts, q_vecs)
+    out = []
+    for q in range(cnt.shape[0]):
+        hits = SearchHits(docs[q, :n[q]].copy(), scores[q, :n[q]].copy(), int(cnt[q]))
+        res = None
+        if groups[q] is not None and groups[q][0] is not None:
+            gb = groups[q][0]
+            res = [{"values": list(gb.values[g]), "result": [(int(gd[r, i]), float(gs[r, i])) for i in range(int(gn[r]))]}
+                   for g, r in enumerate(range(int(rows[q]), int(rows[q + 1])))]
+        out.append((hits, res))
+    return out
+
+
 def merge_index_results_sorted(per_index, order: str, limit: int, offset: int = 0, promote=None, apply: bool = True):
     """The multi-index union in field order (oc_merge_sorted, host; MergeSortedIterator, read/sort.rs:491-559):
     per_index = one (doc_ids [B, limit'], scores, sort values, n, count[, pin scores, pin present]) tuple per index, each
@@ -1104,6 +1176,31 @@ class SearchBatcher:
                                              _p(cnt), _p(ps), _p(pp)))
         k = int(n[0])
         return SearchHits(docs[:k].copy(), scores[:k].copy(), int(cnt[0])), sv[:k].copy(), ps[:n_items], pp[:n_items]
+
+    def search_groups(self, params: TokenScoreParams, group=None, promote=None, text: Optional[TextQuery] = None,
+                      q_vec: Optional[np.ndarray] = None, group_stride: Optional[int] = None):
+        """One query with its own groupBy (`group`: None or (GroupBy, max_results[, (SortField, order)]), as an entry of
+        search_q_groups_arrays' `groups`) and pin rules, coalesced with concurrent search_groups() calls.  Returns (docs
+        [limit], scores, sort values [limit], n, count, pin scores [items], pin present [items], group docs
+        [n_groups, stride], group scores, group sort values, group n [n_groups]) as search_q_groups_arrays gives them for
+        this query alone."""
+        sp, keep, B = self.tsc._build_params(params, None if text is None else [text],
+                                             None if q_vec is None else np.asarray(q_vec, np.float32).reshape(1, -1))
+        assert B == 1
+        req, rows = _group_reqs([group], 1)
+        pins = None if promote is None else _pins([promote], 1)[0]
+        n_items = 0 if pins is None else int(pins._keep[0][-1])
+        if group_stride is None:
+            group_stride = _group_need(group, n_items)
+        L, G, S = params.limit_hint, int(rows[-1]), int(group_stride)
+        docs, scores, sv = np.zeros(L, np.uint64), np.zeros(L, np.float32), np.zeros(L, np.float64)
+        n, cnt = np.zeros(1, np.uint32), np.zeros(1, np.uint64)
+        ps, pp = np.zeros(max(n_items, 1), np.float32), np.zeros(max(n_items, 1), np.uint8)
+        gd, gs, gsv = np.zeros((G, S), np.uint64), np.zeros((G, S), np.float32), np.zeros((G, S), np.float64)
+        gn = np.zeros(G, np.uint32)
+        check(lib().oc_batcher_search_groups(self._h, C.byref(sp), req, None if pins is None else C.byref(pins), S, _p(docs),
+                                             _p(scores), _p(sv), _p(n), _p(cnt), _p(ps), _p(pp), _p(gd), _p(gs), _p(gsv), _p(gn)))
+        return docs, scores, sv, n[0], cnt[0], ps[:n_items], pp[:n_items], gd, gs, gsv, gn
 
     def stats(self) -> dict:
         q, b, d = C.c_uint64(), C.c_uint64(), C.c_uint64()

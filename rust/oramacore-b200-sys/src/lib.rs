@@ -90,6 +90,14 @@ pub struct OcSort {
     pub order: c_int,
 }
 
+/// one query's groupBy in oc_search_q_groups: its handle (NULL: no groups), max_results and sort (field NULL: score order)
+#[repr(C)]
+pub struct OcGroupReq {
+    pub groups: *const OcGroupBy,
+    pub max_results: u32,
+    pub sort: OcSort,
+}
+
 #[repr(C)]
 pub struct OcResolveParams {
     pub texts: *const *const c_char,
@@ -140,6 +148,11 @@ extern "C" {
     pub fn oc_batcher_search_sorted(b: *mut OcBatcher, p: *const OcSearchParams, sort: *const OcSort, pins: *const OcPins,
                                     out_doc_ids: *mut u64, out_scores: *mut f32, out_sort_values: *mut f64, out_n: *mut u32,
                                     out_count: *mut u64, out_pin_scores: *mut f32, out_pin_present: *mut u8) -> c_int;
+    pub fn oc_batcher_search_groups(b: *mut OcBatcher, p: *const OcSearchParams, req: *const OcGroupReq, pins: *const OcPins,
+                                    group_stride: u32, out_doc_ids: *mut u64, out_scores: *mut f32, out_sort_values: *mut f64,
+                                    out_n: *mut u32, out_count: *mut u64, out_pin_scores: *mut f32, out_pin_present: *mut u8,
+                                    out_group_doc_ids: *mut u64, out_group_scores: *mut f32, out_group_sort_values: *mut f64,
+                                    out_group_n: *mut u32) -> c_int;
     pub fn oc_batcher_stats(b: *mut OcBatcher, n_queries: *mut u64, n_batches: *mut u64, n_direct: *mut u64) -> c_int;
     pub fn oc_pinned_free(p: *mut c_void);
     pub fn oc_search(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, p: *const OcSearchParams,
@@ -215,6 +228,12 @@ extern "C" {
                                    out_doc_ids: *mut u64, out_scores: *mut f32, out_sort_values: *mut f64, out_n: *mut u32,
                                    out_count: *mut u64, out_group_doc_ids: *mut u64, out_group_scores: *mut f32,
                                    out_group_sort_values: *mut f64, out_group_n: *mut u32) -> c_int;
+    pub fn oc_group_by_n_groups(g: *const OcGroupBy) -> u64;
+    pub fn oc_search_q_groups(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, p: *const OcSearchParams, q_groups: *const OcGroupReq,
+                              pins: *const OcPins, group_stride: u32, out_doc_ids: *mut u64, out_scores: *mut f32,
+                              out_sort_values: *mut f64, out_n: *mut u32, out_count: *mut u64, out_pin_scores: *mut f32,
+                              out_pin_present: *mut u8, out_group_doc_ids: *mut u64, out_group_scores: *mut f32,
+                              out_group_sort_values: *mut f64, out_group_n: *mut u32) -> c_int;
     pub fn oc_merge_sorted(n_indexes: u32, n_queries: u32, limit: u32, offset: u32, in_stride: u32, order: c_int,
                            doc_ids: *const *const u64, scores: *const *const f32, sort_values: *const *const f64,
                            n: *const *const u32, counts: *const *const u64, pins: *const OcPins,
