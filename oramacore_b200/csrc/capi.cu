@@ -2151,6 +2151,9 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
             qd.token_end = (uint32_t)tokens.size();
             queries[q] = qd;
         }
+        // K3b holds a query's tokens in a BM25_MAX_TOK-entry shared table: a batch with a longer query goes to the
+        // accumulator kernel (K3), which walks any number of tokens, like a batch with multi-term tokens
+        if (max_tokens > BM25_MAX_TOK) any_multi = true;
         if (df_local_only && !count_df)
             return fail(OC_ERR_INVALID, "sharded search: a field of this shard has no corpus-wide df table (dropped by a commit?): "
                                         "reload it or pass OC_SHARD_COUNT_DF on every rank");
@@ -2704,7 +2707,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         fp.out_vdoc = c->grp_vdoc.as<uint64_t>(); fp.out_vscore = c->grp_vscore.as<float>(); fp.out_vn = c->grp_vn.as<uint32_t>();
         fp.out_gmin = c->grp_gmin.as<float>(); fp.out_den = c->grp_den.as<float>();
     }
-    fuse_smem = size_t(fp.capb) * 8 + size_t(std::max<uint32_t>(32, next_pow2(n_keep))) * 8 + size_t(vlimit) * 8 + 64;
+    fuse_smem = size_t(fp.capb) * 8 + size_t(std::max<uint32_t>(32, next_pow2(n_keep))) * 8 + size_t(vlimit) * 16 + 64;
     if (smem_cfg_needed(c->device, exports ? (const void *)fuse_topk_kernel<true> : (const void *)fuse_topk_kernel<false>, fuse_smem))
         CU(cudaFuncSetAttribute(exports ? (const void *)fuse_topk_kernel<true> : (const void *)fuse_topk_kernel<false>,
                                 cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fuse_smem));

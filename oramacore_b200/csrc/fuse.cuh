@@ -82,6 +82,7 @@ __device__ __forceinline__ float fused_ft_score(float ft, bool hybrid, float gmi
 }
 
 constexpr uint32_t FUSE_MAX_V = OC_MAX_TOPK;
+constexpr uint32_t FUSE_VONLY = 0xfffffffeu - FUSE_MAX_V;   // key index base of the hybrid vector hits without a string row
 
 // GROUPS: group mode, the out_gmin / out_den / out_v* exports are written
 template <bool GROUPS = false>
@@ -91,6 +92,8 @@ __global__ void __launch_bounds__(256) fuse_topk_kernel(const FuseParams p) {
     uint64_t *sel = buf + p.capb;                                     // [next_pow2(n_keep)] selection scratch
     float *vsum = reinterpret_cast<float *>(sel + max(32u, next_pow2(p.n_keep)));   // [v_stride] merged vector score
     uint32_t *vfirst = reinterpret_cast<uint32_t *>(vsum + p.v_stride); // [v_stride] 1 = unique head
+    uint32_t *vrank = vfirst + p.v_stride;                            // [v_stride] head j: rank of its doc id among the heads
+    uint32_t *vbyrank = vrank + p.v_stride;                           // [v_stride] rank -> head j
     __shared__ unsigned int s_maxo, s_mino;
     __shared__ unsigned long long s_count;
     const uint32_t q = blockIdx.x, tid = threadIdx.x;
@@ -110,6 +113,16 @@ __global__ void __launch_bounds__(256) fuse_topk_kernel(const FuseParams p) {
         vsum[j] = s;
         vfirst[j] = head ? 1u : 0u;
     }
+    __syncthreads();
+    // The key index of a vector hit is its doc id's rank among the unique hits, so that equal scores come out in doc id
+    // order as top_n breaks ties (sort.rs:260-279); the hit list itself is in (score, store row) order.
+    for (uint32_t j = tid; j < vc; j += blockDim.x)
+        if (vfirst[j]) {
+            uint32_t r = 0;
+            for (uint32_t i = 0; i < vc; i++) r += (vfirst[i] && vdoc[i] < vdoc[j]) ? 1u : 0u;
+            vrank[j] = r;
+            vbyrank[r] = j;
+        }
     __syncthreads();
 
     // ---- count and extrema
@@ -196,10 +209,10 @@ __global__ void __launch_bounds__(256) fuse_topk_kernel(const FuseParams p) {
         const uint32_t j = uint32_t(i - n_ft_slots);
         if (!vfirst[j]) return KEY_NONE;
         const float f = vhit_score(j);
-        uint32_t idx = j;
-        if (hybrid) {
+        uint32_t idx = vrank[j];
+        if (hybrid) {   // a hit without a string row sorts after every row on equal scores (its doc id has no row index)
             const size_t vs = size_t(q) * p.v_stride + j;
-            idx = p.v_row[vs] != 0xffffffffu ? p.v_row[vs] : (0xfffffffeu - j);
+            idx = p.v_row[vs] != 0xffffffffu ? p.v_row[vs] : (FUSE_VONLY + vrank[j]);
         }
         return f == f ? make_key(f, idx) : KEY_NONE;
     };
@@ -254,8 +267,8 @@ __global__ void __launch_bounds__(256) fuse_topk_kernel(const FuseParams p) {
             const uint64_t k = buf[p.offset + i];
             const uint32_t idx = key_idx(k);
             sc = key_score(k);
-            if (p.mode == OC_MODE_VECTOR) doc = vdoc[idx];
-            else if (hybrid && idx >= 0xfffffffeu - FUSE_MAX_V) doc = vdoc[0xfffffffeu - idx];
+            if (p.mode == OC_MODE_VECTOR) doc = vdoc[vbyrank[idx]];
+            else if (hybrid && idx >= FUSE_VONLY) doc = vdoc[vbyrank[idx - FUSE_VONLY]];
             else doc = p.str_row_doc_ids ? p.str_row_doc_ids[idx] : uint64_t(idx);
         }
         p.out_doc[size_t(q) * p.limit + i] = doc;
