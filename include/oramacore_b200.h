@@ -285,7 +285,8 @@ int oc_filter_geo_polygon(const oc_geo_field *g, const double *lat, const double
  * NumberFilter::Between), a string_filter key (string_filter_field.rs:175-193) — the number of the variant's
  * documents that are keys of the score map.  The store keeps, per field, the variants' document lists on the
  * device (number fields: documents sorted by value, so a range is a slice); a search in facet mode makes the tile
- * scorer emit the bitmap of matched documents (+ the vector hits) and one kernel counts every (query, variant).
+ * scorer emit the bitmap of matched documents (+ the vector hits) and one kernel counts every (query, variant): each
+ * distinct document slice is read once, against every query that asks for it.
  * As in the reference (search.rs:361-396) the score map is computed WITHOUT the where-filter (uncommitted deletes
  * stay excluded), so p->filter_bits / p->filter are ignored here: hits come from oc_search, facets from this call.
  * A document may be listed under several variants (array values).  nbits: DocumentId space [0, nbits). */
@@ -532,6 +533,29 @@ int oc_search_q_groups(oc_ctx *ctx, oc_emb *emb, oc_str *str, const oc_search_pa
                        double *out_sort_values, uint32_t *out_n, uint64_t *out_count, float *out_pin_scores,
                        uint8_t *out_pin_present, uint64_t *out_group_doc_ids, float *out_group_scores,
                        double *out_group_sort_values, uint32_t *out_group_n);
+/* ---- per-query facets --------------------------------------------------------------------------------
+ * oc_search_q_groups with each query's own facets (SearchParams.facets), in the same call.  facets: one store for the
+ * batch.  Query b's requests are facet_reqs[q_facet_offsets[b] .. q_facet_offsets[b + 1]) (an empty range: no facets);
+ * out_facet_counts has q_facet_offsets[B] entries, aligned with facet_reqs (entries before q_facet_offsets[0] are not
+ * written).  A request's kind follows its field: a variant of a bool / string_filter field, a range [from, to] of a
+ * number field.  q_groups may be NULL: no query has groups.  Byte for byte:
+ *   - query b's hits, scores, sort values, n, count, pin outputs and group rows are what oc_search_q_groups gives the same
+ *     batch without facets (and so what query b gets alone);
+ *   - query b's facet counts are what oc_search_facets gives it alone: B = 1, its own requests, its filter ignored.
+ * A query without a filter (no q_filters entry, no p->filter / filter_bits) counts on the matched documents of the main
+ * pass.  The queries with a filter and facets are re-scored without it, as the reference does (search.rs:361-396), in
+ * one more pass over just their sub-batch, without groups, sorts or pins.  p->limit == 0 is accepted when every query
+ * has groups or facets: the hits are not written, and both passes run the vector stage at depth 0 (limit_hint = limit).
+ * Refusals (nothing written): everything oc_search_q_groups refuses; OC_ERR_INVALID: facets of another ctx, NULL
+ * facets / q_facet_offsets, q_facet_offsets not monotone, an unknown field or variant, a NaN bound (oc_facets_check);
+ * OC_ERR_UNSUPPORTED: p->sharded. */
+int oc_facets_check(const oc_facets *f, const oc_facet_req *reqs, uint32_t n);   /* host only: OC_OK or OC_ERR_INVALID */
+int oc_search_q_facets(oc_ctx *ctx, oc_emb *emb, oc_str *str, const oc_search_params *p, const oc_group_req *q_groups,
+                       const oc_pins *pins, uint32_t group_stride, oc_facets *facets, const uint32_t *q_facet_offsets /* B+1 */,
+                       const oc_facet_req *facet_reqs, uint64_t *out_doc_ids, float *out_scores, double *out_sort_values,
+                       uint32_t *out_n, uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present,
+                       uint64_t *out_group_doc_ids, float *out_group_scores, double *out_group_sort_values,
+                       uint32_t *out_group_n, uint64_t *out_facet_counts);
 /* The multi-index union in field order (host, no device; MergeSortedIterator, read/sort.rs:491-559).  Run every index
  * with oc_search_sorted, limit' = limit + offset (2 x (limit + offset) when pins apply, and then apply = 0),
  * offset' = 0, vector_limit = limit, and pass its hits, sort values (in_stride = limit'), counts and per-item
@@ -630,6 +654,18 @@ int oc_batcher_search_groups(oc_batcher *b, const oc_search_params *p, const oc_
                              uint32_t *out_n, uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present,
                              uint64_t *out_group_doc_ids, float *out_group_scores, double *out_group_sort_values,
                              uint32_t *out_group_n);
+/* oc_batcher_search_groups with facets: one query, its facet store and n_facet_reqs requests, its oc_group_req or NULL (no
+ * groups), items and group_stride; outputs as oc_search_q_facets with B = 1 (out_facet_counts: n_facet_reqs entries).
+ * Faceted requests batch only with faceted requests of the same key and the same facet store; the batch runs as one
+ * oc_search_q_facets with the requests concatenated in request order, and each caller gets its own counts.  Refused with
+ * OC_ERR_INVALID before joining a batch: everything oc_batcher_search_groups refuses, facets of another ctx, and requests
+ * oc_facets_check refuses.  A merged call that fails with OC_ERR_OOM is split in halves and re-run. */
+int oc_batcher_search_faceted(oc_batcher *b, const oc_search_params *p, oc_facets *facets, const oc_facet_req *facet_reqs,
+                              uint32_t n_facet_reqs, const oc_group_req *req, const oc_pins *pins, uint32_t group_stride,
+                              uint64_t *out_doc_ids, float *out_scores, double *out_sort_values, uint32_t *out_n,
+                              uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present,
+                              uint64_t *out_group_doc_ids, float *out_group_scores, double *out_group_sort_values,
+                              uint32_t *out_group_n, uint64_t *out_facet_counts);
 /* queries that went through a coalesced batch (grouped ones included) / number of batches / calls passed straight
  * through */
 int oc_batcher_stats(oc_batcher *b, uint64_t *n_queries, uint64_t *n_batches, uint64_t *n_direct);

@@ -33,7 +33,7 @@ EXPORTED_SYMBOLS = [
     "oc_emb_info", "oc_emb_search", "oc_str_create", "oc_str_destroy", "oc_str_set_rows", "oc_str_load_field",
     "oc_str_insert", "oc_str_commit", "oc_str_delete", "oc_str_info", "oc_str_set_global", "oc_search", "oc_pinned_alloc", "oc_pinned_free", "oc_last_timing", "oc_launch_count",
     "oc_batcher_create", "oc_batcher_destroy", "oc_batcher_search", "oc_batcher_search_sorted", "oc_batcher_search_groups",
-    "oc_batcher_stats",
+    "oc_batcher_search_faceted", "oc_batcher_stats",
     "oc_filter_from_ids", "oc_filter_from_bits", "oc_filter_and", "oc_filter_or", "oc_filter_not", "oc_filter_count",
     "oc_filter_read", "oc_filter_destroy", "oc_merge_results",
     "oc_geo_field_create", "oc_geo_field_destroy", "oc_filter_geo_radius", "oc_filter_geo_polygon",
@@ -42,7 +42,7 @@ EXPORTED_SYMBOLS = [
     "oc_group_by_create", "oc_group_by_destroy", "oc_search_groups",
     "oc_search_pinned", "oc_search_groups_pinned", "oc_merge_pinned",
     "oc_sort_field_create", "oc_sort_field_destroy", "oc_search_sorted", "oc_search_q_sorted", "oc_search_groups_sorted", "oc_merge_sorted",
-    "oc_group_by_n_groups", "oc_search_q_groups",
+    "oc_group_by_n_groups", "oc_search_q_groups", "oc_facets_check", "oc_search_q_facets",
     "oc_dict_create", "oc_dict_destroy", "oc_dict_add_terms", "oc_dict_lookup", "oc_dict_size", "oc_dict_set_stemmer", "oc_stem_english",
     "oc_dict_resolve", "oc_resolved_arrays", "oc_resolved_fill", "oc_resolved_free",
 ]
@@ -175,6 +175,7 @@ def lib():
     L.oc_batcher_search.argtypes = [vp, C.POINTER(SearchParams), vp, vp, vp, vp]
     L.oc_batcher_search_sorted.argtypes = [vp, C.POINTER(SearchParams), vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.oc_batcher_search_groups.argtypes = [vp, C.POINTER(SearchParams), C.POINTER(GroupReq), vp, u32] + [vp] * 11
+    L.oc_batcher_search_faceted.argtypes = [vp, C.POINTER(SearchParams), vp, vp, u32, vp, vp, u32] + [vp] * 12
     L.oc_batcher_stats.argtypes = [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
     L.oc_filter_from_ids.argtypes = [vp, vp, u64, u64, C.POINTER(vp)]
     L.oc_filter_from_bits.argtypes = [vp, vp, u64, C.POINTER(vp)]
@@ -217,6 +218,8 @@ def lib():
     L.oc_group_by_n_groups.argtypes = [vp]
     L.oc_group_by_n_groups.restype = u64
     L.oc_search_q_groups.argtypes = [vp, vp, vp, C.POINTER(SearchParams), C.POINTER(GroupReq), vp, u32] + [vp] * 11
+    L.oc_facets_check.argtypes = [vp, vp, u32]
+    L.oc_search_q_facets.argtypes = [vp, vp, vp, C.POINTER(SearchParams), vp, vp, u32, vp, vp, vp] + [vp] * 12
     L.oc_merge_sorted.argtypes = [u32, u32, u32, u32, u32, C.c_int, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp),
                                   C.POINTER(vp), vp, C.POINTER(vp), C.POINTER(vp), vp, vp, vp, vp, vp]
     L.oc_dict_create.argtypes = [u32, C.POINTER(vp)]

@@ -16,6 +16,9 @@
 // Requests of submit_groups carry an oc_group_req and batch only with each other (the key's `grouped` bit): a batch runs
 // through `GroupedExec` (oc_search_q_groups) at the largest need of its requests as the group stride, and each request's
 // group rows go back at its own stride.  A merged call that runs out of device memory is split in halves and re-run.
+// Requests of submit_faceted carry a facet store, their facet requests and optionally an oc_group_req; they batch only
+// with faceted requests on the same store (the key's `faceted` bit and store) and run through `FacetedExec`
+// (oc_search_q_facets) with the facet requests concatenated in request order; the counts go back to each caller.
 #pragma once
 #include <algorithm>
 #include <atomic>
@@ -32,9 +35,11 @@ namespace ocb {
 
 struct BatchKey {
     int mode; uint32_t limit, offset; float similarity, threshold, k, b; uint32_t vector_limit;
-    bool grouped = false;
+    bool grouped = false, faceted = false;
+    const oc_facets *facets = nullptr;   // faceted requests batch only on the same store
     bool operator==(const BatchKey &o) const {
         return mode == o.mode && limit == o.limit && offset == o.offset && vector_limit == o.vector_limit && grouped == o.grouped &&
+               faceted == o.faceted && facets == o.facets &&
                memcmp(&similarity, &o.similarity, 4) == 0 &&
                memcmp(&threshold, &o.threshold, 4) == 0 && memcmp(&k, &o.k, 4) == 0 && memcmp(&b, &o.b, 4) == 0;
     }
@@ -95,6 +100,17 @@ inline bool groups_batchable(const oc_search_params *p, const oc_group_req *req,
     if (!req->groups) return p->limit > 0;
     return req->max_results <= OC_MAX_TOPK && (!pin_items(pins) || 2ull * req->max_results <= OC_MAX_TOPK);
 }
+// Whether a request of submit_faceted can join a merged oc_search_q_facets: as groups_batchable, except that a request
+// without groups but with facets may run at limit 0.
+inline bool faceted_batchable(const oc_search_params *p, const oc_group_req *req, const oc_pins *pins, uint32_t n_facets) {
+    if (!req->groups && p->limit == 0 && n_facets) return pins_batchable(p, pins);
+    return groups_batchable(p, req, pins);
+}
+// The request of a faceted query without groupBy.
+inline const oc_group_req *no_groups() {
+    static const oc_group_req none{nullptr, 0, oc_sort{nullptr, OC_SORT_ASC}};
+    return &none;
+}
 
 struct BatchReq {
     const oc_search_params *p;
@@ -114,6 +130,12 @@ struct BatchReq {
     float *g_score = nullptr;
     double *g_values = nullptr;         // may be NULL
     uint32_t *g_n = nullptr;            // [n_groups]
+    // submit_faceted only (also grouped)
+    bool faceted = false;
+    const oc_facets *facets = nullptr;
+    const oc_facet_req *f_reqs = nullptr;
+    uint32_t n_f = 0;
+    uint64_t *f_counts = nullptr;       // [n_f]
     int rc = 0;
     bool done = false;
 };
@@ -145,6 +167,11 @@ struct MergedBatch {
     std::vector<float> g_score;
     std::vector<double> g_values;
     std::vector<uint32_t> g_n;                  // [rows]
+    // a faceted batch (also grouped): oc_search_q_facets' requests, query i's at [f_off[i], f_off[i + 1])
+    bool faceted = false;
+    std::vector<uint32_t> f_off;                // [B + 1]
+    std::vector<oc_facet_req> f_reqs;
+    std::vector<uint64_t> f_counts;
 
     void build(const std::vector<BatchReq *> &reqs, uint32_t dim) {
         const oc_search_params *f = reqs[0]->p;
@@ -228,6 +255,15 @@ struct MergedBatch {
         g_score.assign(std::max<size_t>(rows * stride, 1), 0.f);
         g_values.assign(std::max<size_t>(rows * stride, 1), 0.0);
         g_n.assign(std::max<size_t>(rows, 1), 0);
+        faceted = reqs[0]->faceted;
+        if (!faceted) return;
+        f_off.assign(1, 0u); f_reqs.clear();
+        for (uint32_t i = 0; i < B; i++) {
+            f_reqs.insert(f_reqs.end(), reqs[i]->f_reqs, reqs[i]->f_reqs + reqs[i]->n_f);
+            f_off.push_back((uint32_t)f_reqs.size());
+        }
+        f_counts.assign(std::max<size_t>(f_reqs.size(), 1), 0);
+        if (f_reqs.empty()) f_reqs.resize(1);   // a non-NULL array for a batch without a request
     }
     void scatter(const std::vector<BatchReq *> &reqs, int rc) const {
         const uint32_t L = p.limit;
@@ -262,6 +298,8 @@ struct MergedBatch {
                     }
                     r->g_n[g] = g_n[g_row[i] + g];
                 }
+            if (faceted)
+                for (uint32_t j = f_off[i]; j < f_off[i + 1]; j++) r->f_counts[j - f_off[i]] = f_counts[j];
         }
     }
 };
@@ -280,18 +318,32 @@ struct NoGroupedExec {
     }
 };
 
+// The executor of a batcher that takes no submit_faceted(): it is never called.
+struct NoFacetedExec {
+    int operator()(const oc_search_params *, const oc_group_req *, const oc_pins *, uint32_t, const oc_facets *, const uint32_t *,
+                   const oc_facet_req *, uint64_t *, float *, double *, uint32_t *, uint64_t *, float *, uint8_t *, uint64_t *, float *,
+                   double *, uint32_t *, uint64_t *) const {
+        return OC_ERR_UNSUPPORTED;
+    }
+    int check(const oc_facets *, const oc_facet_req *, uint32_t) const { return OC_ERR_UNSUPPORTED; }
+};
+
 // int Exec(const oc_search_params*, uint64_t* docs, float* scores, uint32_t* n, uint64_t* count)
 // int SortedExec(const oc_search_params*, const oc_sort* q_sorts, const oc_pins*, uint64_t* docs, float* scores,
 //                double* sort_values, uint32_t* n, uint64_t* count, float* pin_scores, uint8_t* pin_present)
 // int GroupedExec(const oc_search_params*, const oc_group_req* q_groups, const oc_pins*, uint32_t group_stride,
 //                 uint64_t* docs, float* scores, double* sort_values, uint32_t* n, uint64_t* count, float* pin_scores,
 //                 uint8_t* pin_present, uint64_t* g_docs, float* g_scores, double* g_sort_values, uint32_t* g_n)
-template <class Exec, class SortedExec = NoSortedExec, class GroupedExec = NoGroupedExec>
+// int FacetedExec(const oc_search_params*, const oc_group_req* q_groups, const oc_pins*, uint32_t group_stride,
+//                 const oc_facets*, const uint32_t* q_facet_offsets, const oc_facet_req*, <GroupedExec's outputs>,
+//                 uint64_t* facet_counts)
+//     and int FacetedExec::check(const oc_facets*, const oc_facet_req*, uint32_t n): oc_facets_check
+template <class Exec, class SortedExec = NoSortedExec, class GroupedExec = NoGroupedExec, class FacetedExec = NoFacetedExec>
 class Batcher {
 public:
     Batcher(Exec exec, uint32_t dim, uint32_t max_batch, uint32_t max_wait_us, bool has_emb = true, bool has_str = true,
-            SortedExec sexec = SortedExec(), GroupedExec gexec = GroupedExec())
-        : exec_(exec), sexec_(sexec), gexec_(gexec), dim_(dim), max_batch_(max_batch ? max_batch : 1), max_wait_us_(max_wait_us),
+            SortedExec sexec = SortedExec(), GroupedExec gexec = GroupedExec(), FacetedExec fexec = FacetedExec())
+        : exec_(exec), sexec_(sexec), gexec_(gexec), fexec_(fexec), dim_(dim), max_batch_(max_batch ? max_batch : 1), max_wait_us_(max_wait_us),
           has_emb_(has_emb), has_str_(has_str) {}
 
     int submit(const oc_search_params *p, uint64_t *docs, float *scores, uint32_t *n, uint64_t *count) {
@@ -336,6 +388,31 @@ public:
         r.g_doc = g_doc; r.g_score = g_score; r.g_values = g_values; r.g_n = g_n;
         return join(r);
     }
+    // One query with its facet store and requests, its oc_group_req (NULL: no groups), items and group stride; outputs as
+    // oc_search_q_facets with B = 1.  OC_ERR_INVALID without joining: what submit_groups refuses, and requests the
+    // executor's check refuses.
+    int submit_faceted(const oc_search_params *p, const oc_facets *facets, const oc_facet_req *f_reqs, uint32_t n_f,
+                       const oc_group_req *req, uint64_t n_groups, const oc_pins *pins, uint32_t group_stride, uint64_t *docs,
+                       float *scores, double *sort_values, uint32_t *n, uint64_t *count, float *pin_scores, uint8_t *pin_present,
+                       uint64_t *g_doc, float *g_score, double *g_values, uint32_t *g_n, uint64_t *f_counts) {
+        if (!req) req = no_groups();
+        const char *why = nullptr;
+        if (const int rc = check_sorted(&req->sort, pins, &why)) return rc;
+        if (group_stride < group_need(req, pins)) return OC_ERR_INVALID;
+        if (const int rc = fexec_.check(facets, f_reqs, n_f)) return rc;
+        if (!batchable(p, has_emb_, has_str_) || max_batch_ == 1 || !faceted_batchable(p, req, pins, n_f)) {
+            direct_++;
+            const uint32_t off[2] = {0, n_f};
+            return fexec_(p, req, pins, group_stride, facets, off, f_reqs, docs, scores, sort_values, n, count, pin_scores, pin_present,
+                          g_doc, g_score, g_values, g_n, f_counts);
+        }
+        BatchReq r{p, docs, scores, n, count};
+        r.sort = &req->sort; r.pins = pins; r.sort_values = sort_values; r.pin_scores = pin_scores; r.pin_present = pin_present;
+        r.grouped = true; r.greq = req; r.n_groups = req->groups ? n_groups : 0; r.group_stride = group_stride;
+        r.g_doc = g_doc; r.g_score = g_score; r.g_values = g_values; r.g_n = g_n;
+        r.faceted = true; r.facets = facets; r.f_reqs = f_reqs; r.n_f = n_f; r.f_counts = f_counts;
+        return join(r);
+    }
     void stats(uint64_t *queries, uint64_t *batches, uint64_t *direct) {
         std::lock_guard<std::mutex> g(mu_);
         if (queries) *queries = queries_;
@@ -350,6 +427,8 @@ private:
         // one group collects at a time: wait while it is full or holds a different parameter tuple
         BatchKey k = key_of(p);
         k.grouped = r.grouped;
+        k.faceted = r.faceted;
+        k.facets = r.facets;
         cv_slot_.wait(lk, [&] { return pending_.empty() || (pending_key_ == k && pending_.size() < max_batch_); });
         if (pending_.empty()) pending_key_ = k;
         pending_.push_back(&r);
@@ -382,14 +461,18 @@ private:
         }
         return r.rc;
     }
-    // One merged oc_search_q_groups; out of device memory (the row-score workspace grows with the batch), each half runs
+    // One merged oc_search_q_groups (oc_search_q_facets for a faceted batch); out of device memory (the row-score workspace grows with the batch), each half runs
     // on its own, down to single requests, which then get the single call's answer.
     void run_grouped(const std::vector<BatchReq *> &reqs) {
         MergedBatch m;
         m.build(reqs, dim_);
-        const int rc = gexec_(&m.p, m.q_groups.data(), &m.pins, m.stride, m.docs.data(), m.scores.data(), m.sort_values.data(),
-                              m.n.data(), m.count.data(), m.pin_scores.data(), m.pin_present.data(), m.g_doc.data(), m.g_score.data(),
-                              m.g_values.data(), m.g_n.data());
+        const int rc = m.faceted
+            ? fexec_(&m.p, m.q_groups.data(), &m.pins, m.stride, reqs[0]->facets, m.f_off.data(), m.f_reqs.data(), m.docs.data(),
+                     m.scores.data(), m.sort_values.data(), m.n.data(), m.count.data(), m.pin_scores.data(), m.pin_present.data(),
+                     m.g_doc.data(), m.g_score.data(), m.g_values.data(), m.g_n.data(), m.f_counts.data())
+            : gexec_(&m.p, m.q_groups.data(), &m.pins, m.stride, m.docs.data(), m.scores.data(), m.sort_values.data(), m.n.data(),
+                     m.count.data(), m.pin_scores.data(), m.pin_present.data(), m.g_doc.data(), m.g_score.data(), m.g_values.data(),
+                     m.g_n.data());
         if (rc == OC_ERR_OOM && reqs.size() > 1) {
             const size_t h = reqs.size() / 2;
             run_grouped(std::vector<BatchReq *>(reqs.begin(), reqs.begin() + h));
@@ -402,6 +485,7 @@ private:
     Exec exec_;
     SortedExec sexec_;
     GroupedExec gexec_;
+    FacetedExec fexec_;
     uint32_t dim_, max_batch_, max_wait_us_;
     bool has_emb_, has_str_;
     std::mutex mu_;

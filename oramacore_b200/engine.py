@@ -483,44 +483,58 @@ class FacetStore:
 
 
 def _number_label(x) -> str:
-    return str(int(x)) if float(x) == int(x) else repr(float(x))
+    return str(int(x)) if np.isfinite(x) and float(x) == int(x) else repr(float(x))
 
 
-def search_facets(tsc: "TokenScoreContext", store: FacetStore, params: "TokenScoreParams", facets: Dict[str, dict], texts=None,
-                  q_vecs: Optional[np.ndarray] = None) -> List[Dict[str, dict]]:
-    """`facets` as in the reference's SearchParams: {"field": {"true": bool, "false": bool}} for a bool field,
-    {"field": {"ranges": [{"from": a, "to": b}, ...]}} for a number field, {"field": {}} for a string_filter field.
-    Returns, per query, {field: {"count": n_values, "values": {label: count}}} (FacetResult, types.rs:1508-1511;
-    number labels "from-to", number_field.rs:382).  The where-filter of `params` is ignored, as in search.rs:361-396."""
+def facet_requests(store: FacetStore, facets: Dict[str, dict]):
+    """The oc_facet_req tuples (field, variant, from, to) and (field name, label) pairs of one reference-style `facets`
+    map: {"field": {"true": bool, "false": bool}} for a bool field, {"field": {"ranges": [{"from": a, "to": b}, ...]}}
+    for a number field (labels "from-to", number_field.rs:382), {"field": {}} for a string_filter field (every key).
+    Date fields have no facets, and ranges only apply to number fields."""
     reqs, labels = [], []
     for name, d in facets.items():
         f = store.fields[name]
         if f["kind"] == "date":
             raise ValueError(f"{name!r} is a date field: dates have no facets")
         if f["kind"] == "number":
+            if "ranges" not in d:
+                raise ValueError(f"{name!r} is a number field: its facets are ranges")
             for r in d["ranges"]:
                 reqs.append((f["id"], 0, float(r["from"]), float(r["to"])))
                 labels.append((name, f"{_number_label(r['from'])}-{_number_label(r['to'])}"))
         else:
+            if "ranges" in d:
+                raise ValueError(f"{name!r} is a {f['kind']} field: ranges apply to number fields")
             for vi, key in enumerate(f["keys"]):
                 if f["kind"] == "bool" and not d.get(key, False):
                     continue
                 reqs.append((f["id"], vi, 0.0, 0.0))
                 labels.append((name, key))
+    return reqs, labels
+
+
+def _facet_result(counts, labels) -> Dict[str, dict]:
+    """FacetResult (types.rs:1508-1511) per field: {"count": n_values, "values": {label: count}}."""
+    r: Dict[str, dict] = {}
+    for j, (name, label) in enumerate(labels):
+        r.setdefault(name, {"count": 0, "values": {}})["values"][label] = int(counts[j])
+    for v in r.values():
+        v["count"] = len(v["values"])
+    return r
+
+
+def search_facets(tsc: "TokenScoreContext", store: FacetStore, params: "TokenScoreParams", facets: Dict[str, dict], texts=None,
+                  q_vecs: Optional[np.ndarray] = None) -> List[Dict[str, dict]]:
+    """`facets` as in the reference's SearchParams (see facet_requests), one map for every query.  Returns, per query,
+    {field: {"count": n_values, "values": {label: count}}}.  The where-filter of `params` is ignored, as in
+    search.rs:361-396."""
+    reqs, labels = facet_requests(store, facets)
     sp, keep, B = tsc._build_params(params, texts, q_vecs)
     arr = (_lib.FacetReq * len(reqs))(*[_lib.FacetReq(*r) for r in reqs])
     out = np.zeros((B, max(len(reqs), 1)), np.uint64)
     check(lib().oc_search_facets(tsc.ctx._h, tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None, store._h,
                                  C.byref(sp), arr, len(reqs), _p(out)))
-    res = []
-    for q in range(B):
-        r: Dict[str, dict] = {}
-        for j, (name, label) in enumerate(labels):
-            r.setdefault(name, {"count": 0, "values": {}})["values"][label] = int(out[q, j])
-        for v in r.values():
-            v["count"] = len(v["values"])
-        res.append(r)
-    return res
+    return [_facet_result(out[q], labels) for q in range(B)]
 
 
 class GroupBy:
@@ -875,6 +889,68 @@ def search_q_groups(tsc: "TokenScoreContext", params: "TokenScoreParams", groups
     return out
 
 
+def _q_facet_reqs(store: FacetStore, facets, B: int):
+    """oc_facet_req[] in query order, q_facet_offsets [B+1] and each query's labels, from one facets map (or None) per
+    query."""
+    if len(facets) != B:
+        raise ValueError(f"facets has {len(facets)} entries for {B} queries")
+    reqs, labels, off = [], [], np.zeros(B + 1, np.uint32)
+    for b, f in enumerate(facets):
+        r, lab = facet_requests(store, f) if f else ([], [])
+        reqs += r
+        labels.append(lab)
+        off[b + 1] = len(reqs)
+    arr = (_lib.FacetReq * max(len(reqs), 1))(*[_lib.FacetReq(*r) for r in reqs])
+    return arr, off, labels
+
+
+def search_q_facets_arrays(tsc: "TokenScoreContext", store: FacetStore, params: "TokenScoreParams", facets, groups=None,
+                           promote=None, texts=None, q_vecs: Optional[np.ndarray] = None, group_stride: Optional[int] = None):
+    """oc_search_q_facets: search_q_groups_arrays with each query's own facets (`facets[b]`: a reference-style map, see
+    facet_requests, or None) counted in the same call.  `groups` None: no query has groups.  Returns
+    search_q_groups_arrays' tuple followed by (facet counts [requests], q_facet_offsets [B+1], labels per query): query b's
+    counts are counts[off[b]:off[b+1]], what search_facets gives it alone (its where-filter ignored)."""
+    sp, keep, B = tsc._build_params(params, texts, q_vecs)
+    req, rows = _group_reqs(groups if groups is not None else [None] * B, B)
+    farr, foff, labels = _q_facet_reqs(store, facets, B)
+    pins = None if promote is None else _pins(promote, B)[0]
+    n_items = 0 if pins is None else int(pins._keep[0][-1])
+    if group_stride is None:
+        k = [0] * B if promote is None else [len(x) for x in promote]
+        group_stride = max([0] + [_group_need(g, k[b]) for b, g in enumerate(groups or [None] * B)])
+    L, R, S = params.limit_hint, int(rows[-1]), int(group_stride)
+    docs, scores, sv = np.zeros((B, L), np.uint64), np.zeros((B, L), np.float32), np.zeros((B, L), np.float64)
+    n, cnt = np.zeros(B, np.uint32), np.zeros(B, np.uint64)
+    ps, pp = np.zeros(max(n_items, 1), np.float32), np.zeros(max(n_items, 1), np.uint8)
+    gd, gs, gsv = np.zeros((R, S), np.uint64), np.zeros((R, S), np.float32), np.zeros((R, S), np.float64)
+    gn = np.zeros(R, np.uint32)
+    fc = np.zeros(max(int(foff[-1]), 1), np.uint64)
+    check(lib().oc_search_q_facets(tsc.ctx._h, tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None, C.byref(sp),
+                                   req, None if pins is None else C.byref(pins), S, store._h, _p(foff), farr, _p(docs),
+                                   _p(scores), _p(sv), _p(n), _p(cnt), _p(ps), _p(pp), _p(gd), _p(gs), _p(gsv), _p(gn), _p(fc)))
+    return (docs, scores, sv, n, cnt, ps[:n_items], pp[:n_items], gd, gs, gsv, gn, rows, fc[:int(foff[-1])], foff, labels)
+
+
+def search_q_facets(tsc: "TokenScoreContext", store: FacetStore, params: "TokenScoreParams", facets, groups=None, promote=None,
+                    texts=None, q_vecs: Optional[np.ndarray] = None):
+    """search_q_facets_arrays as search_q_groups returns it, plus the facets: per query (hits, groups, facets), groups
+    None without groupBy, facets None without facets, else {field: FacetResult}."""
+    got = search_q_facets_arrays(tsc, store, params, facets, groups, promote, texts, q_vecs)
+    docs, scores, n, cnt, gd, gs, gn, rows, fc, foff, labels = got[0], got[1], got[3], got[4], got[7], got[8], got[10], got[11], \
+        got[12], got[13], got[14]
+    out = []
+    for q in range(cnt.shape[0]):
+        hits = SearchHits(docs[q, :n[q]].copy(), scores[q, :n[q]].copy(), int(cnt[q]))
+        res = None
+        if groups is not None and groups[q] is not None and groups[q][0] is not None:
+            gb = groups[q][0]
+            res = [{"values": list(gb.values[g]), "result": [(int(gd[r, i]), float(gs[r, i])) for i in range(int(gn[r]))]}
+                   for g, r in enumerate(range(int(rows[q]), int(rows[q + 1])))]
+        fr = _facet_result(fc[foff[q]:foff[q + 1]], labels[q]) if facets[q] else None
+        out.append((hits, res, fr))
+    return out
+
+
 def merge_index_results_sorted(per_index, order: str, limit: int, offset: int = 0, promote=None, apply: bool = True):
     """The multi-index union in field order (oc_merge_sorted, host; MergeSortedIterator, read/sort.rs:491-559):
     per_index = one (doc_ids [B, limit'], scores, sort values, n, count[, pin scores, pin present]) tuple per index, each
@@ -1201,6 +1277,33 @@ class SearchBatcher:
         check(lib().oc_batcher_search_groups(self._h, C.byref(sp), req, None if pins is None else C.byref(pins), S, _p(docs),
                                              _p(scores), _p(sv), _p(n), _p(cnt), _p(ps), _p(pp), _p(gd), _p(gs), _p(gsv), _p(gn)))
         return docs, scores, sv, n[0], cnt[0], ps[:n_items], pp[:n_items], gd, gs, gsv, gn
+
+    def search_faceted(self, store: FacetStore, params: TokenScoreParams, facets, group=None, promote=None,
+                       text: Optional[TextQuery] = None, q_vec: Optional[np.ndarray] = None, group_stride: Optional[int] = None):
+        """One query with its own facets (a reference-style map, see facet_requests), groupBy (`group`, as for
+        search_groups, or None) and pin rules, coalesced with concurrent search_faceted() calls on the same store.
+        Returns search_groups()' tuple followed by the facet counts [requests] and their (field, label) pairs, as
+        search_q_facets_arrays gives them for this query alone."""
+        sp, keep, B = self.tsc._build_params(params, None if text is None else [text],
+                                             None if q_vec is None else np.asarray(q_vec, np.float32).reshape(1, -1))
+        assert B == 1
+        req, rows = _group_reqs([group], 1)
+        farr, foff, labels = _q_facet_reqs(store, [facets], 1)
+        pins = None if promote is None else _pins([promote], 1)[0]
+        n_items = 0 if pins is None else int(pins._keep[0][-1])
+        if group_stride is None:
+            group_stride = _group_need(group, n_items)
+        L, G, S, F = params.limit_hint, int(rows[-1]), int(group_stride), int(foff[-1])
+        docs, scores, sv = np.zeros(L, np.uint64), np.zeros(L, np.float32), np.zeros(L, np.float64)
+        n, cnt = np.zeros(1, np.uint32), np.zeros(1, np.uint64)
+        ps, pp = np.zeros(max(n_items, 1), np.float32), np.zeros(max(n_items, 1), np.uint8)
+        gd, gs, gsv = np.zeros((G, S), np.uint64), np.zeros((G, S), np.float32), np.zeros((G, S), np.float64)
+        gn = np.zeros(G, np.uint32)
+        fc = np.zeros(max(F, 1), np.uint64)
+        check(lib().oc_batcher_search_faceted(self._h, C.byref(sp), store._h, farr, F, None if group is None else req,
+                                              None if pins is None else C.byref(pins), S, _p(docs), _p(scores), _p(sv), _p(n),
+                                              _p(cnt), _p(ps), _p(pp), _p(gd), _p(gs), _p(gsv), _p(gn), _p(fc)))
+        return docs, scores, sv, n[0], cnt[0], ps[:n_items], pp[:n_items], gd, gs, gsv, gn, fc[:F], labels[0]
 
     def stats(self) -> dict:
         q, b, d = C.c_uint64(), C.c_uint64(), C.c_uint64()

@@ -153,6 +153,12 @@ extern "C" {
                                     out_n: *mut u32, out_count: *mut u64, out_pin_scores: *mut f32, out_pin_present: *mut u8,
                                     out_group_doc_ids: *mut u64, out_group_scores: *mut f32, out_group_sort_values: *mut f64,
                                     out_group_n: *mut u32) -> c_int;
+    pub fn oc_batcher_search_faceted(b: *mut OcBatcher, p: *const OcSearchParams, f: *mut OcFacets, facet_reqs: *const OcFacetReq,
+                                     n_facet_reqs: u32, req: *const OcGroupReq, pins: *const OcPins, group_stride: u32,
+                                     out_doc_ids: *mut u64, out_scores: *mut f32, out_sort_values: *mut f64, out_n: *mut u32,
+                                     out_count: *mut u64, out_pin_scores: *mut f32, out_pin_present: *mut u8,
+                                     out_group_doc_ids: *mut u64, out_group_scores: *mut f32, out_group_sort_values: *mut f64,
+                                     out_group_n: *mut u32, out_facet_counts: *mut u64) -> c_int;
     pub fn oc_batcher_stats(b: *mut OcBatcher, n_queries: *mut u64, n_batches: *mut u64, n_direct: *mut u64) -> c_int;
     pub fn oc_pinned_free(p: *mut c_void);
     pub fn oc_search(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, p: *const OcSearchParams,
@@ -234,6 +240,14 @@ extern "C" {
                               out_sort_values: *mut f64, out_n: *mut u32, out_count: *mut u64, out_pin_scores: *mut f32,
                               out_pin_present: *mut u8, out_group_doc_ids: *mut u64, out_group_scores: *mut f32,
                               out_group_sort_values: *mut f64, out_group_n: *mut u32) -> c_int;
+    // per-query facets in the batched grouped call
+    pub fn oc_facets_check(f: *const OcFacets, reqs: *const OcFacetReq, n: u32) -> c_int;
+    pub fn oc_search_q_facets(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, p: *const OcSearchParams, q_groups: *const OcGroupReq,
+                              pins: *const OcPins, group_stride: u32, f: *mut OcFacets, q_facet_offsets: *const u32,
+                              facet_reqs: *const OcFacetReq, out_doc_ids: *mut u64, out_scores: *mut f32, out_sort_values: *mut f64,
+                              out_n: *mut u32, out_count: *mut u64, out_pin_scores: *mut f32, out_pin_present: *mut u8,
+                              out_group_doc_ids: *mut u64, out_group_scores: *mut f32, out_group_sort_values: *mut f64,
+                              out_group_n: *mut u32, out_facet_counts: *mut u64) -> c_int;
     pub fn oc_merge_sorted(n_indexes: u32, n_queries: u32, limit: u32, offset: u32, in_stride: u32, order: c_int,
                            doc_ids: *const *const u64, scores: *const *const f32, sort_values: *const *const f64,
                            n: *const *const u32, counts: *const *const u64, pins: *const OcPins,
