@@ -74,9 +74,14 @@ static bool smem_cfg_needed(int device, const void *fn, size_t smem) {
 }
 
 // ------------------------------------------------------------------------------------ buffers
+// workspaces grow on demand and free themselves
 struct DevBuf {
     void *p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf &) = delete;
+    DevBuf &operator=(const DevBuf &) = delete;
+    ~DevBuf() { if (p) cudaFree(p); }
     int ensure(size_t bytes) {
         if (bytes <= cap) return OC_OK;
         if (p) cudaFree(p);
@@ -88,12 +93,15 @@ struct DevBuf {
         cap = want;
         return OC_OK;
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
     template <typename T> T *as() { return reinterpret_cast<T *>(p); }
 };
 struct HostBuf {  // pinned staging
     void *p = nullptr;
     size_t cap = 0;
+    HostBuf() = default;
+    HostBuf(const HostBuf &) = delete;
+    HostBuf &operator=(const HostBuf &) = delete;
+    ~HostBuf() { if (p) cudaFreeHost(p); }
     int ensure(size_t bytes) {
         if (bytes <= cap) return OC_OK;
         if (p) cudaFreeHost(p);
@@ -104,23 +112,30 @@ struct HostBuf {  // pinned staging
         cap = want;
         return OC_OK;
     }
-    void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
     template <typename T> T *as() { return reinterpret_cast<T *>(p); }
 };
 
+// an array's place in a packed upload; at(blob) is its device copy once the blob is up (NULL: never added)
+template <typename T> struct Slot {
+    size_t off = 0;
+    bool added = false;
+    const T *at(const DevBuf &blob) const {
+        return added ? reinterpret_cast<const T *>(static_cast<const uint8_t *>(blob.p) + off) : nullptr;
+    }
+};
 // lays several host arrays out in one pinned blob -> one H2D copy (sources are copied once,
 // straight into the pinned staging buffer)
 struct Packer {
     struct Seg { const void *src; size_t off, bytes; bool direct; };
     std::vector<Seg> segs;
     size_t total = 0;
-    // direct = the source already lives in pinned host memory (oc_pinned_alloc / cudaHostRegister):
-    // it is DMA'd straight from the caller's buffer instead of being staged
-    size_t add(const void *src, size_t bytes, bool direct = false) {
+    // n elements of src; direct = the source already lives in pinned host memory (oc_pinned_alloc /
+    // cudaHostRegister): it is DMA'd straight from the caller's buffer instead of being staged
+    template <typename T> Slot<T> add(const T *src, size_t n, bool direct = false) {
         const size_t off = (total + 255) & ~size_t(255);
-        segs.push_back({src, off, bytes, direct});
-        total = off + bytes;
-        return off;
+        segs.push_back({src, off, n * sizeof(T), direct});
+        total = off + n * sizeof(T);
+        return Slot<T>{off, true};
     }
     void fill(void *dst) const {
         for (const Seg &g : segs) if (g.bytes && g.src && !g.direct) memcpy(static_cast<uint8_t *>(dst) + g.off, g.src, g.bytes);
@@ -155,7 +170,7 @@ struct oc_ctx {
     uint32_t call_launches = 0, call_scan_launches = 0;
     // workspaces
     DevBuf in_blob, in_blob0, q_pad, q_inv, eff_norm, filter_dev, scan_cand, v_doc, v_score, v_row, v_cnt, v_srow, v_ft, v_present, v_raw;
-    DevBuf seg, df_dev, row_ok, tau, cand_key, cand_ft, cand_cnt, tile_cnt, tile_max, tile_min, min_hint;
+    DevBuf seg, df_dev, row_ok, tau, cand_key, cand_ft, cand_cnt, tile_cnt, tile_max, tile_min;
     DevBuf out_blob, shard_send, shard_recv, work_ctr, flat_desc, mbits, dbits, facet_out;
     bool gemm_pending = false; const float *gemm_inv_norm = nullptr;
     DevBuf row_ft, grp_vdoc, grp_vscore, grp_vn, grp_gmin, grp_den, grp_doc, grp_score, grp_n;   // oc_search_groups
@@ -178,6 +193,15 @@ struct oc_ctx {
         uint8_t *peer[16] = {};      // peer[rank] == local
         uint64_t seq = 0;            // exchanges done (all ranks run the same batches): parity = seq & 1
     } p2p;
+    ~oc_ctx() {   // the workspaces free themselves after this
+        for (int r = 0; r < 16; r++) if (p2p.ready && p2p.peer[r] && p2p.peer[r] != p2p.local) cudaIpcCloseMemHandle(p2p.peer[r]);
+        if (p2p.local) cudaFree(p2p.local);
+        comm.destroy();
+        for (int i = 0; i < EV_N; i++) if (ev[i]) cudaEventDestroy(ev[i]);
+        if (stream) cudaStreamDestroy(stream);
+        if (side) cudaStreamDestroy(side);
+        if (ev_side) cudaEventDestroy(ev_side);
+    }
 };
 
 static inline void launched(oc_ctx *c, bool scan = false) {
@@ -213,25 +237,6 @@ extern "C" void oc_shutdown(oc_ctx *c) {
     if (!c) return;
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
-    for (int r = 0; r < 16; r++) if (c->p2p.ready && c->p2p.peer[r] && c->p2p.peer[r] != c->p2p.local) cudaIpcCloseMemHandle(c->p2p.peer[r]);
-    if (c->p2p.local) cudaFree(c->p2p.local);
-    c->comm.destroy();
-    DevBuf *bufs[] = {&c->in_blob, &c->q_pad, &c->q_inv, &c->eff_norm, &c->filter_dev, &c->scan_cand, &c->v_doc,
-                      &c->v_score, &c->v_row, &c->v_cnt, &c->v_srow, &c->v_ft, &c->v_present, &c->v_raw, &c->seg, &c->df_dev,
-                      &c->row_ok, &c->tau, &c->cand_key, &c->cand_ft, &c->cand_cnt, &c->tile_cnt, &c->tile_max,
-                      &c->tile_min, &c->min_hint, &c->out_blob, &c->shard_send, &c->shard_recv, &c->work_ctr, &c->flat_desc, &c->mbits, &c->dbits, &c->facet_out, &c->q_bf16, &c->q_f16, &c->q_scale, &c->q_rho, &c->pre_post, &c->dense_buf, &c->g_thr, &c->g_eps, &c->g_ovf, &c->g_ovfcnt, &c->g_resc, &c->g_cand, &c->g_cnt, &c->g_max,
-                      &c->g_flag, &c->r_qpad, &c->r_qinv, &c->r_map, &c->r_doc, &c->r_score, &c->r_row, &c->r_cnt, &c->r_raw,
-                      &c->row_ft, &c->grp_vdoc, &c->grp_vscore, &c->grp_vn, &c->grp_gmin, &c->grp_den, &c->grp_doc, &c->grp_score, &c->grp_n,
-                      &c->pin_row, &c->pin_ft, &c->pin_ftp, &c->pin_score, &c->pin_present, &c->pin_top_doc, &c->pin_top_score,
-                      &c->pin_top_n, &c->pin_gdoc, &c->pin_gscore, &c->pin_gn,
-                      &c->srt_doc, &c->srt_row, &c->srt_n, &c->srt_ft, &c->srt_ftp, &c->srt_score, &c->srt_present, &c->srt_zero,
-                      &c->e_rowbits, &c->r_slot};
-    for (DevBuf *b : bufs) b->release();
-    c->h_in.release(); c->h_out.release();
-    for (int i = 0; i < EV_N; i++) if (c->ev[i]) cudaEventDestroy(c->ev[i]);
-    cudaStreamDestroy(c->stream);
-    if (c->side) cudaStreamDestroy(c->side);
-    if (c->ev_side) cudaEventDestroy(c->ev_side);
     delete c;
 }
 
@@ -1824,16 +1829,19 @@ struct GroupJob {
     const SortEntry *d_ents = nullptr;
 };
 struct PinJob {   // oc_search_pinned / oc_search_groups_pinned: the promote items, padded to `stride` slots per query
+    const oc_pins *pins = nullptr;      // the caller's items (NULL: none)
+    float *out_scores = nullptr;        // per item of pins: its score-map value and presence (each may be NULL)
+    uint8_t *out_present = nullptr;
     uint32_t stride = 0;                // most items of one query (0: no item in the batch)
     bool splice = false;                // pins apply and some query has items: top lists at twice the depth + the splice
     std::vector<uint64_t> doc;          // [B][stride]
     std::vector<uint32_t> pos, cnt;     // [B][stride], [B]
-    bool q_filters = false;             // oc_search_q_sorted: the batch may carry per-query filters
     const uint64_t *d_doc = nullptr;    // their device copies (set by search_impl)
     const uint32_t *d_pos = nullptr, *d_cnt = nullptr;
 };
 // Checks and pads the items of pins (NULL: none).  Nothing is written on failure.
 static int pin_job_init(const oc_pins *pins, uint32_t B, PinJob &pj) {
+    pj.pins = pins;
     if (!pins) return OC_OK;
     const uint32_t *off = pins->q_pin_offsets;
     if (!off) return fail(OC_ERR_INVALID, "pins: q_pin_offsets is NULL");
@@ -1888,7 +1896,6 @@ struct SortJob {
     std::vector<int> order;                // [entries]
     std::vector<uint32_t> q_ent;           // [B]
     bool by_score = false;                 // some query is in score order
-    double *out_values = nullptr;          // B x limit, may be NULL
     SortOrder &ord(uint32_t e) const { return f[e]->ord[order[e]]; }
 };
 // Appends one query's sort (field NULL: score order).  Nothing is written on failure.
@@ -1940,342 +1947,460 @@ static int sort_rows_for(oc_ctx *c, SortOrder &o, const std::shared_ptr<StrSnap>
 static int run_groups(oc_ctx *c, const GroupJob &gj, int mode, const StrSnap *S, uint32_t n_tiles, uint32_t vlimit,
                       const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, const PinJob &pj);
 
-// gj != NULL: the grouped calls (always with pj).  Then limit == 0 is allowed: the hits are not written (out_doc_ids / out_scores / out_n
-// may be NULL), the vector stage gets depth 0 and the fulltext stage runs with one candidate slot per tile.
-// pj != NULL: the pinned calls; the items' score-map values go to out_pin_scores / out_pin_present (may be NULL).
-// sj != NULL: the sorted calls (always with pj); the hits are the walk's in field order, K4's list only gives the count.
-static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, uint64_t *out_doc_ids,
-                       float *out_scores, uint32_t *out_n, uint64_t *out_count, const FacetJob *fj, GroupJob *gj = nullptr,
-                       PinJob *pj = nullptr, const oc_pins *pins = nullptr, float *out_pin_scores = nullptr,
-                       uint8_t *out_pin_present = nullptr, const SortJob *sj = nullptr) {
-    if (!c || !p || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
-    const bool write_hits = !(gj || (fj && fj->hits_optional)) || p->limit > 0;
-    if (write_hits && (!out_doc_ids || !out_scores || !out_n)) return fail(OC_ERR_INVALID, "NULL argument");
-    const uint32_t B = p->n_queries;
-    if (B == 0) return OC_OK;
-    const bool has_v = p->mode == OC_MODE_VECTOR || p->mode == OC_MODE_HYBRID;
-    const bool has_ft = p->mode == OC_MODE_FULLTEXT || p->mode == OC_MODE_HYBRID;
-    if (!has_v && !has_ft) return fail(OC_ERR_INVALID, "unknown mode %d", p->mode);
-    if (has_v && (!emb || !p->q_vecs)) return fail(OC_ERR_INVALID, "vector/hybrid mode needs emb and q_vecs");
-    if (has_ft && (!str || !p->q_token_offsets)) return fail(OC_ERR_INVALID, "fulltext/hybrid mode needs str and tokens");
-    if (emb && emb->ctx != c) return fail(OC_ERR_INVALID, "emb belongs to another ctx");
-    if (str && str->ctx != c) return fail(OC_ERR_INVALID, "str belongs to another ctx");
-    // per-query where-filters: deduplicated by handle; all NULL = unfiltered, one handle for every query = p->filter
-    const oc_filter *batch_filter = p->filter;
+// One search as an entry point asks for it.  fj: the facet counts.  gj: the grouped calls (always with pj); then
+// limit == 0 is allowed: the hits are not written (out_doc_ids / out_scores / out_n may be NULL), the vector stage gets
+// depth 0 and the fulltext stage runs with one candidate slot per tile.  pj: the pinned calls.  sj: the sorted calls
+// (always with pj); the hits are the walk's in field order, K4's list only gives the count.
+struct SearchReq {
+    const oc_search_params *p;
+    uint64_t *out_doc_ids; float *out_scores; uint32_t *out_n; uint64_t *out_count;
+    SearchReq(const oc_search_params *p_, uint64_t *doc, float *score, uint32_t *n, uint64_t *count)
+        : p(p_), out_doc_ids(doc), out_scores(score), out_n(n), out_count(count) {}
+    double *out_sort_values = nullptr;   // [B][limit] the hits' sort values (NaN in score order), may be NULL
+    const FacetJob *fj = nullptr;
+    GroupJob *gj = nullptr;
+    PinJob *pj = nullptr;
+    const SortJob *sj = nullptr;
+    bool q_filters_ok = false;           // the entry point takes per-query filters (p->q_filters)
+};
+
+// What one search derives once, filled in by the stages of search_impl in order.
+struct SearchCall {
+    oc_ctx *c; oc_emb *emb; oc_str *str;
+    const SearchReq &r;
+    const oc_search_params *p;
+    SearchCall(oc_ctx *c_, oc_emb *e, oc_str *s, const SearchReq &r_) : c(c_), emb(e), str(s), r(r_), p(r_.p) {}
+    // shape and path
+    uint32_t B = 0, limit = 0, n_keep = 0, vlimit = 0, cap = 0, sort_top = 0;
+    bool has_v = false, has_ft = false, per_q = false, facets = false, write_hits = false, pin_flat = false, sort_flat = false;
+    bool k4_top = false, exports = false, pin_items = false, side = false;
+    // inputs; filter_h: the filter is a host bitmap, uploaded with this call
+    std::shared_ptr<StrSnap> snap;
+    StrSnap *S = nullptr;
     QFilterJob qfj;
-    bool per_q = false;
-    if (p->q_filters) {
-        if ((gj || pj || sj) && !(pj && pj->q_filters))
-            return fail(OC_ERR_UNSUPPORTED, "q_filters: per-query filters are supported by oc_search, oc_search_q_sorted and "
-                                            "oc_search_q_groups only");
-        if (p->filter || p->filter_bits) return fail(OC_ERR_INVALID, "q_filters together with filter / filter_bits");
-        if (p->sharded) return fail(OC_ERR_UNSUPPORTED, "q_filters over a sharded search");
-        std::unordered_map<const oc_filter *, uint32_t> idx;
-        std::vector<const oc_filter *> distinct;
-        bool any_none = false;
-        qfj.q_slot.resize(B);
-        for (uint32_t b = 0; b < B; b++) {
-            const oc_filter *f = p->q_filters[b];
-            if (!f) { any_none = true; qfj.q_slot[b] = SLOT_NONE; continue; }
-            if (f->ctx != c) return fail(OC_ERR_INVALID, "q_filters[%u] belongs to another ctx", b);
-            auto it = idx.emplace(f, (uint32_t)distinct.size()).first;
-            if (it->second == distinct.size()) distinct.push_back(f);
-            qfj.q_slot[b] = it->second;
-        }
-        if (distinct.size() > 65535) return fail(OC_ERR_UNSUPPORTED, "q_filters: %zu distinct handles > 65535", distinct.size());
-        if (distinct.size() == 1 && !any_none) batch_filter = distinct[0];
-        else if (!distinct.empty()) {
-            per_q = true;
-            const uint32_t K = (uint32_t)distinct.size();
-            for (const oc_filter *f : distinct) qfj.slots.push_back(RowsOkSlot{f->bits, f->nbits});
-            qfj.slots.push_back(RowsOkSlot{nullptr, 0});
-            qfj.q_slot_ft.resize(B);
-            for (uint32_t b = 0; b < B; b++) qfj.q_slot_ft[b] = qfj.q_slot[b] == SLOT_NONE ? K : qfj.q_slot[b];
-        }
-    }
-    if (p->limit == 0 && write_hits) return fail(OC_ERR_INVALID, "limit must be >= 1");
-    const uint32_t limit = write_hits ? p->limit : 1;
-    // sort_token_scores with pins selects the top 2 * (limit + offset) (sort.rs:25-34); the vector depth stays limit
-    const bool pin_flat = pj && pj->splice && write_hits && !sj;
-    const bool sort_flat = sj && write_hits;
-    // sort_token_scores with sort_by: top_count keys in field order, twice as many for an active pinned query
-    const uint32_t sort_top = sort_flat ? uint32_t((uint64_t(limit) + p->offset) * (pj->splice ? 2 : 1)) : 0u;
-    // oc_search_q_sorted: the queries in score order take K4's list, spliced as pin_flat does
-    bool score_active = false;
-    if (sort_flat && sj->by_score && pj->splice)
-        for (uint32_t q = 0; q < B; q++) score_active = score_active || (sj->q_ent[q] == SORT_BY_SCORE && pj->cnt[q] > 0);
-    const bool k4_top = pin_flat || (sort_flat && sj->by_score);   // K4 writes its top n_keep (offset 0) for a splice
-    const uint64_t n_keep64 = (uint64_t(limit) + p->offset) * (pin_flat || score_active ? 2 : 1);
-    if (n_keep64 > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "limit+offset %llu > %u", (unsigned long long)n_keep64, OC_MAX_TOPK);
-    const uint32_t n_keep = (uint32_t)n_keep64;
-    // limit_hint = limit, NOT limit+offset (search.rs:330-336); vector_limit lets a multi-index caller keep that depth
-    const uint32_t vlimit = !write_hits ? 0u : p->vector_limit ? p->vector_limit : limit;
-    if (vlimit > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "vector_limit %u > %u", vlimit, OC_MAX_TOPK);
-    if (p->sharded && !c->comm.ready()) return fail(OC_ERR_COMM, "sharded search without oc_comm_init");
-
-    // the published snapshot of the string store: grabbed once, immutable for the whole call (a commit may
-    // publish the next version meanwhile); declared before the lock so a last reference dies outside it
-    std::shared_ptr<StrSnap> snap = str ? str_snapshot(str) : nullptr;
-    StrSnap *S = snap.get();
-    std::lock_guard<std::mutex> g(c->mu);
-    CU(cudaSetDevice(c->device));
-    // facets: the requests resolved to their distinct document slices (the work list goes up with the first upload)
-    const bool facets = fj && !fj->q.empty();
     FacetPlan fpl;
-    if (facets) OCTRY(facet_plan(*fj, fpl));
-    auto add_fpl = [&](Packer &pk, size_t o[2]) {
-        o[0] = pk.add(fpl.slices.data(), fpl.slices.size() * sizeof(FacetSliceDev));
-        o[1] = pk.add(fpl.pairs.data(), fpl.pairs.size() * sizeof(uint2));
-    };
-    auto bind_fpl = [&](uint8_t *base, const size_t o[2]) {
-        fpl.d_slices = reinterpret_cast<const FacetSliceDev *>(base + o[0]);
-        fpl.d_pairs = reinterpret_cast<const uint2 *>(base + o[1]);
-    };
-    begin_call(c);
-
-    // staged segments go in one copy per contiguous run; pinned caller buffers are DMA'd directly
-    auto upload = [&](const Packer &pk, HostBuf &hb, DevBuf &db, cudaStream_t st) -> int {
-        OCTRY(hb.ensure(pk.total + 256));
-        OCTRY(db.ensure(pk.total + 256));
-        pk.fill(hb.p);
-        size_t run0 = 0;
-        for (size_t i = 0; i <= pk.segs.size(); i++) {
-            const bool brk = i == pk.segs.size() || pk.segs[i].direct;
-            if (brk) {
-                const size_t end = i == pk.segs.size() ? pk.total : pk.segs[i].off;
-                if (end > run0) CU(cudaMemcpyAsync(db.as<uint8_t>() + run0, hb.as<uint8_t>() + run0, end - run0, cudaMemcpyHostToDevice, st));
-                if (i < pk.segs.size()) {
-                    CU(cudaMemcpyAsync(db.as<uint8_t>() + pk.segs[i].off, pk.segs[i].src, pk.segs[i].bytes, cudaMemcpyHostToDevice, st));
-                    run0 = pk.segs[i].off + pk.segs[i].bytes;
-                }
-            }
-        }
-        return OC_OK;
-    };
-    // ------------------------------------------------------------ vector stage first: the query vectors
-    // (+ filter) go up alone and the matrix sweep starts; the host-side descriptor work below overlaps it
-    if (batch_filter && batch_filter->ctx != c) return fail(OC_ERR_INVALID, "filter belongs to another ctx");
-    const bool filter_h = !batch_filter && p->filter_bits != nullptr;     // host bitmap: uploaded with this call
-    const bool filter = filter_h || batch_filter != nullptr;
-    const uint64_t filter_nbits = batch_filter ? batch_filter->nbits : p->filter_nbits;
-    const size_t fwords = filter_h ? (p->filter_nbits + 63) / 64 : 0;
-    const uint64_t *filter_dev = batch_filter ? batch_filter->bits : nullptr;
-    // per-query filters: the slot tables travel with the first upload of the call
-    auto add_qf = [&](Packer &pk, size_t o[3]) {
-        o[0] = pk.add(qfj.slots.data(), qfj.slots.size() * sizeof(RowsOkSlot));
-        o[1] = pk.add(qfj.q_slot.data(), size_t(B) * 4);
-        o[2] = pk.add(qfj.q_slot_ft.data(), size_t(B) * 4);
-    };
-    auto bind_qf = [&](uint8_t *base, const size_t o[3]) {
-        qfj.d_slots = reinterpret_cast<const RowsOkSlot *>(base + o[0]);
-        qfj.d_q_slot = reinterpret_cast<const uint32_t *>(base + o[1]);
-        qfj.d_q_slot_ft = reinterpret_cast<const uint32_t *>(base + o[2]);
-    };
-    size_t h2d_early = 0;
-    if (has_v) {
-        Packer pk0;
-        const size_t o_qv = pk0.add(p->q_vecs, size_t(B) * emb->dim * 4, is_pinned_host(p->q_vecs));
-        const size_t o_flt = filter_h ? pk0.add(p->filter_bits, fwords * 8) : 0;
-        size_t o_qf[3] = {0, 0, 0}, o_fpl[2] = {0, 0};
-        if (per_q) add_qf(pk0, o_qf);
-        if (facets) add_fpl(pk0, o_fpl);
-        CU(cudaEventRecord(c->ev[EV_START], c->stream));
-        OCTRY(upload(pk0, c->h_in0, c->in_blob0, c->stream));
-        CU(cudaEventRecord(c->ev[EV_H2D], c->stream));
-        h2d_early = pk0.total;
-        if (filter_h) filter_dev = reinterpret_cast<const uint64_t *>(c->in_blob0.as<uint8_t>() + o_flt);
-        if (per_q) bind_qf(c->in_blob0.as<uint8_t>(), o_qf);
-        if (facets) bind_fpl(c->in_blob0.as<uint8_t>(), o_fpl);
-        if (vlimit) {
-            OCTRY(run_vector_stage(c, emb, reinterpret_cast<const float *>(c->in_blob0.as<uint8_t>() + o_qv), B, vlimit, p->similarity,
-                                   filter_dev, filter_nbits, per_q ? &qfj : nullptr));
-        } else {   // limit_hint 0 (groups only): no vector hit
-            OCTRY(c->v_cnt.ensure(size_t(B) * 4));
-            CU(cudaMemsetAsync(c->v_cnt.p, 0, size_t(B) * 4, c->stream));
-        }
-    }
-
-    // ------------------------------------------------------------ host: descriptors
-    const bool multi_rank = p->sharded && c->comm.world > 1;
-    // sharded: every rank must take the same df decisions (they drive a collective), so the
-    // tombstone state is the caller's global flag (OC_SHARD_TOMBSTONES), not this shard's
-    const bool tombs_local = has_ft && S->n_deleted > 0;
-    if (multi_rank && tombs_local && !(p->sharded & OC_SHARD_TOMBSTONES))
-        return fail(OC_ERR_INVALID, "sharded search: this shard holds tombstones, set OC_SHARD_TOMBSTONES on every rank");
-    const bool tombs = has_ft && (multi_rank ? (p->sharded & OC_SHARD_TOMBSTONES) != 0 : tombs_local);
-    const uint32_t n_tiles = has_ft ? (uint32_t)((S->n_rows + BM25_TILE - 1) / BM25_TILE) : 0;
+    const oc_filter *batch_filter = nullptr;
+    bool filter_h = false, filter = false;
+    uint64_t filter_nbits = 0;
+    size_t fwords = 0;
+    const uint64_t *filter_dev = nullptr;
+    // fulltext descriptors.  max_tokens: tokens of the longest query; dense_bytes: the dense contribution arrays of the
+    // batch (zeroed before the precompute kernel fills them); term_key: (field << 32 | term id) of each expanded term;
+    // tok_slot: per-query filters, the fulltext slot of each token's query; q_perm: the register-folded scorers' item order
+    bool multi_rank = false, tombs = false, thr = false, count_df = false, any_multi = false, need_df = false, derived_now = false;
+    uint32_t n_tiles = 0, max_tokens = 0, cls_nq[BM25_CLASSES] = {0, 0, 0, 0, 0};
+    uint64_t dense_bytes = 0, postings_walked = 0;
     std::vector<TermDesc> terms;
-    std::vector<uint32_t> term_token;
-    std::vector<uint64_t> term_key;     // (field << 32 | term id) of each expanded term
     std::vector<TokenDesc> tokens;
     std::vector<QueryDesc> queries;
+    std::vector<uint64_t> term_key;
+    std::vector<uint32_t> term_token, tok_slot, q_perm;
     std::vector<uint8_t> tok_need_df;
-    std::vector<uint32_t> tok_slot;     // per-query filters: the fulltext slot of each token's query
     std::vector<PreDesc> pre_descs;
     std::vector<uint2> pre_items;
-    bool any_multi = false, need_df = false, derived_now = false;
-    uint32_t max_tokens = 0;    // tokens of the longest query of the batch
-    uint64_t dense_bytes = 0;   // dense contribution arrays of this batch (zeroed before the precompute kernel fills them)
-    // sharded: df comes from the replicated per-term table, or — OC_SHARD_COUNT_DF on every rank, e.g. after a
-    // commit dropped the table — from counting + all-reduce.  A shard-local list length is never a corpus df.
-    const bool count_df = multi_rank && (p->sharded & OC_SHARD_COUNT_DF) != 0;
-    bool df_local_only = false;
-    uint64_t postings_walked = 0;
-    const bool thr = p->threshold >= 0.0f;
-    if (has_ft) {
-        for (auto &f : S->fields)   // streamed posting format depends on (avg_field_len, b): derive once
-            if (f.n_post && f.b_cached != p->bm25_b) {
-                bm25_derive_postings_kernel<<<(unsigned)((f.n_post + 255) / 256), 256, 0, c->stream>>>(f.raw, f.n_post, f.avg_len, p->bm25_b, f.post);
-                launched(c);
-                CU(cudaGetLastError());
-                f.b_cached = p->bm25_b;
-                derived_now = true;   // queued on the main stream: this call keeps the BM25 prologue there too
-            }
-        const float N = (float)S->document_count;  // token_score.rs:221
-        queries.resize(B);
-        // Per-query filters are routed as a filtered batch is: df is counted on the device (need_df), so nothing is shared
-        // or dense and K3b / K3 score the batch, each (tile, query) item under its query's row bitmap.  A token keeps the
-        // idf its query would get alone: counted under the query's filter, or — single term, no filter, no tombstones —
-        // from the host's posting-list length (or corpus df table), as a plain oc_search does.  An unfiltered query runs
-        // under the tombstone-only row bitmap (slot K), so it scores exactly the rows it would score alone.
-        if (per_q) need_df = true;
-        for (uint32_t q = 0; q < B; q++) {
-            const uint32_t t0 = p->q_token_offsets[q], t1 = p->q_token_offsets[q + 1];
-            const bool q_filter = filter || (per_q && qfj.q_slot[q] != SLOT_NONE);
-            QueryDesc qd{};
-            qd.token_begin = (uint32_t)tokens.size();
-            const uint32_t ntok = t1 - t0;
-            max_tokens = std::max(max_tokens, ntok);
-            qd.required = thr ? (uint32_t)floorf((float)ntok * p->threshold) : 0;  // token_score.rs:211-218
-            qd.flags = thr ? QF_THRESHOLD : 0;
-            for (uint32_t t = t0; t < t1; t++) {
-                TokenDesc tk{};
-                tk.term_begin = (uint32_t)terms.size();
-                tk.bit = 1u << ((t - t0) & 31u);
-                uint64_t df_known = 0;
-                for (uint32_t e = p->token_term_offsets[t]; e < p->token_term_offsets[t + 1]; e++) {
-                    const uint32_t fi = p->term_field[e], ti = p->term_id[e];
-                    if (fi >= S->fields.size()) return fail(OC_ERR_INVALID, "term field %u out of range", fi);
-                    const StrField &f = S->fields[fi];
-                    if (ti >= f.n_terms) continue;  // unknown term: no postings
-                    TermDesc td{};
-                    td.ptr = f.post + f.term_offsets[ti];
-                    td.len = (uint32_t)(f.term_offsets[ti + 1] - f.term_offsets[ti]);
-                    td.weight = p->term_weight ? p->term_weight[e] : 1.0f;
-                    td.avg_len = f.avg_len;
-                    df_known = f.global_df.empty() ? td.len : f.global_df[ti];
-                    if (multi_rank && f.global_df.empty()) df_local_only = true;
-                    postings_walked += td.len;
-                    term_key.push_back((uint64_t(fi) << 32) | ti);
-                    terms.push_back(td);
-                    term_token.push_back((uint32_t)tokens.size());
-                }
-                tk.term_end = (uint32_t)terms.size();
-                const uint32_t nt = tk.term_end - tk.term_begin;
-                uint8_t need = 0;
-                if (nt == 1 && !q_filter && !tombs && !count_df) tk.idf = host_idf(N, std::max<uint64_t>(1, df_known));
-                else if (nt == 0) tk.idf = host_idf(N, 1);
-                else { need = 1; need_df = true; tk.idf = 0.f; }
-                if (nt != 1) { any_multi = any_multi || nt > 1; }
-                tokens.push_back(tk);
-                tok_need_df.push_back(need);
-                if (per_q) tok_slot.push_back(qfj.q_slot_ft[q]);
-            }
-            qd.token_end = (uint32_t)tokens.size();
-            queries[q] = qd;
-        }
-        // K3b holds a query's tokens in a BM25_MAX_TOK-entry shared table: a batch with a longer query goes to the
-        // accumulator kernel (K3), which walks any number of tokens, like a batch with multi-term tokens
-        if (max_tokens > BM25_MAX_TOK) any_multi = true;
-        if (df_local_only && !count_df)
-            return fail(OC_ERR_INVALID, "sharded search: a field of this shard has no corpus-wide df table (dropped by a commit?): "
-                                        "reload it or pass OC_SHARD_COUNT_DF on every rank");
-        // ---- batch-level sharing of per-posting contributions (single-term tokens with a host-known idf); not with
-        // per-query filters: the precomputed contributions and dense arrays are masked by ONE row bitmap
-        if (!per_q) {
-            struct U { uint32_t first_e; uint32_t uses; };
-            struct K128 { uint64_t a, b; };            // (field, term) | (weight bits, idf bits)
-            size_t cap_t = 64;
-            while (cap_t < tokens.size() * 2) cap_t <<= 1;
-            std::vector<K128> tab_k(cap_t);
-            std::vector<uint32_t> tab_v(cap_t, 0xffffffffu);   // open addressing, linear probing
-            std::vector<U> uniq;
-            std::vector<uint32_t> e_to_u(terms.size(), 0xffffffffu);
-            uint64_t walked = 0, distinct = 0;
-            for (size_t t = 0; t < tokens.size(); t++) {
-                const TokenDesc &tk = tokens[t];
-                if (tk.term_end - tk.term_begin != 1 || tok_need_df[t]) continue;
-                const uint32_t e = tk.term_begin;
-                if (terms[e].len < 64) continue;
-                uint32_t wb, ib;
-                memcpy(&wb, &terms[e].weight, 4); memcpy(&ib, &tk.idf, 4);
-                const K128 key{term_key[e], (uint64_t(wb) << 32) | ib};
-                uint64_t h = (key.a * 0x9E3779B97F4A7C15ull) ^ (key.b * 0xC2B2AE3D27D4EB4Full);
-                size_t slot = (h ^ (h >> 29)) & (cap_t - 1);
-                while (tab_v[slot] != 0xffffffffu && !(tab_k[slot].a == key.a && tab_k[slot].b == key.b)) slot = (slot + 1) & (cap_t - 1);
-                if (tab_v[slot] == 0xffffffffu) {
-                    tab_k[slot] = key; tab_v[slot] = (uint32_t)uniq.size();
-                    uniq.push_back({e, 0}); distinct += terms[e].len;
-                }
-                uniq[tab_v[slot]].uses++;
-                e_to_u[e] = tab_v[slot];
-                walked += terms[e].len;
-            }
-            const char *share_env = getenv("OC_BM25_SHARE");   // "off" / "force": A/B testing of the sharing pass
-            const bool share_off = share_env && !strcmp(share_env, "off"), share_force = share_env && !strcmp(share_env, "force");
-            // hot terms (a posting in at least every 16th row) go DENSE: their contributions are scattered once per batch
-            // into a float[rows] array and every (query, tile) item adds 8192 floats with 128-bit loads instead of
-            // walking ~thousands of postings (posting-centred kernel only: every token of the batch has <= 1 term)
-            const char *dense_env = getenv("OC_BM25_DENSE");
-            const char *t2_env = getenv("OC_BM25_TILE2");
-            const bool dense_on = !any_multi && !(dense_env && dense_env[0] == '0') && !share_off && !(t2_env && t2_env[0] == '0');
-            const uint64_t rows_pad = uint64_t(n_tiles) * BM25_TILE;
-            const uint64_t dense_min = std::max<uint64_t>(512, S->n_rows / 16);
-            std::vector<uint8_t> u_dense(uniq.size(), 0);
-            uint64_t n_dense = 0;
-            if (dense_on)
-                for (size_t u = 0; u < uniq.size(); u++)
-                    if (terms[uniq[u].first_e].len >= dense_min && (n_dense + 1) * rows_pad * 4 <= (size_t(8) << 30)) { u_dense[u] = 1; n_dense++; }
-            uint64_t walked_l = 0, distinct_l = 0;   // what is left for the list form
-            for (size_t e = 0; e < terms.size(); e++)
-                if (e_to_u[e] != 0xffffffffu && !u_dense[e_to_u[e]]) walked_l += terms[e].len;
-            for (size_t u = 0; u < uniq.size(); u++) if (!u_dense[u]) distinct_l += terms[uniq[u].first_e].len;
-            const bool lists = distinct_l && !share_off && (share_force || (walked_l >= 2 * distinct_l && walked_l >= (64u << 20))) &&
-                               distinct_l * 8 <= (size_t(6) << 30);
-            if (lists || n_dense) {
-                if (lists) OCTRY(c->pre_post.ensure(distinct_l * 8 + 64));
-                if (n_dense) OCTRY(c->dense_buf.ensure(n_dense * rows_pad * 4));
-                dense_bytes = n_dense * rows_pad * 4;
-                uint64_t off = 0, doff = 0;
-                std::vector<uint64_t> u_off(uniq.size());
-                std::vector<uint8_t> u_used(uniq.size(), 0);
-                for (size_t u = 0; u < uniq.size(); u++) {
-                    if (!u_dense[u] && !lists) continue;
-                    u_used[u] = 1;
-                    const TermDesc &td = terms[uniq[u].first_e];
-                    PreDesc pd{};
-                    pd.src = td.ptr; pd.len = td.len; pd.weight = td.weight;
-                    pd.idf = tokens[term_token[uniq[u].first_e]].idf;
-                    if (u_dense[u]) { u_off[u] = doff; pd.dense = c->dense_buf.as<float>() + doff; doff += rows_pad; }
-                    else { u_off[u] = off; pd.dst = c->pre_post.as<Posting>() + off; off += td.len; }
-                    const uint32_t pi = (uint32_t)pre_descs.size();
-                    pre_descs.push_back(pd);
-                    for (uint32_t ch = 0; ch * PRE_CHUNK < td.len; ch++) pre_items.push_back(make_uint2(pi, ch));
-                }
-                for (size_t e = 0; e < terms.size(); e++) {
-                    const uint32_t u = e_to_u[e];
-                    if (u == 0xffffffffu || !u_used[u]) continue;
-                    if (u_dense[u]) { terms[e].ptr = reinterpret_cast<const Posting *>(c->dense_buf.as<float>() + u_off[u]); terms[e].flags |= TD_DENSE; }
-                    else { terms[e].ptr = c->pre_post.as<Posting>() + u_off[u]; terms[e].flags |= TD_PRE; }
-                }
+    // OMC rows for the tile kernel (string rows, ascending)
+    uint32_t n_omc = 0;
+    bool omc_tile = false;
+    std::vector<uint32_t> omc_rows;
+    std::vector<float> omc_row_mult;
+    // sortBy entries and per-query walks, group handles and spans
+    std::vector<SortEntry> s_ents;
+    std::vector<SortQuery> s_q;
+    std::vector<uint8_t> s_alt;
+    std::vector<GroupHandle> g_hand;
+    std::vector<GroupSpan> g_spans;
+    // the two uploads: pk0 (vector modes: the query vectors, sent before the descriptors are built) and pk; `first` is
+    // the one the filter bitmap, the per-query filter tables and the facet work list ride in
+    Packer pk0, pk, *first = nullptr;
+    DevBuf *first_blob = nullptr;
+    Slot<uint64_t> s_flt, s_omcd;
+    Slot<uint32_t> s_qslot, s_qslot_ft, s_ttok, s_tslot, s_perm, s_omcr;
+    Slot<float> s_omcm, s_omcrm;
+    Slot<uint2> s_fpairs, s_pitems;
+    Slot<RowsOkSlot> s_qslots;
+    Slot<FacetSliceDev> s_fslices;
+    Slot<TermDesc> s_terms;
+    Slot<TokenDesc> s_tokens;
+    Slot<QueryDesc> s_queries;
+    Slot<PreDesc> s_pre;
+    Slot<SortEntry> s_sent;
+    Slot<SortQuery> s_sq;
+    Slot<uint8_t> s_salt;
+    // device state of the stages
+    Bm25Params bp{};
+    FuseParams fp{};
+    size_t fuse_smem = 0;
+    const uint32_t *row_ok = nullptr;
+    float *min_hint_dev = nullptr;
+    unsigned int *tile_counter = nullptr;
+    bool did_comm = false;
+    // the output blob: [doc B x limit][score B x limit][n B][count B][min B][gflag B]; the host copy adds [g_flag B][rescored B]
+    size_t o_sc = 0, o_n = 0, o_cnt = 0, o_min = 0, o_gflag = 0, out_bytes = 0, o_resc = 0;
+    uint8_t *dout = nullptr;
+    uint64_t *d_doc = nullptr;
+    float *d_score = nullptr;
+    uint32_t *d_n = nullptr;
+};
+
+// staged segments go in one copy per contiguous run; pinned caller buffers are DMA'd directly
+static int upload(const Packer &pk, HostBuf &hb, DevBuf &db, cudaStream_t st) {
+    OCTRY(hb.ensure(pk.total + 256));
+    OCTRY(db.ensure(pk.total + 256));
+    pk.fill(hb.p);
+    size_t run0 = 0;
+    for (size_t i = 0; i <= pk.segs.size(); i++) {
+        const bool brk = i == pk.segs.size() || pk.segs[i].direct;
+        if (brk) {
+            const size_t end = i == pk.segs.size() ? pk.total : pk.segs[i].off;
+            if (end > run0) CU(cudaMemcpyAsync(db.as<uint8_t>() + run0, hb.as<uint8_t>() + run0, end - run0, cudaMemcpyHostToDevice, st));
+            if (i < pk.segs.size()) {
+                CU(cudaMemcpyAsync(db.as<uint8_t>() + pk.segs[i].off, pk.segs[i].src, pk.segs[i].bytes, cudaMemcpyHostToDevice, st));
+                run0 = pk.segs[i].off + pk.segs[i].bytes;
             }
         }
     }
-    // OMC rows for the tile kernel (string rows, ascending)
-    std::vector<uint32_t> omc_rows; std::vector<float> omc_row_mult;
-    const uint32_t n_omc = (uint32_t)p->n_omc;
+    return OC_OK;
+}
+
+// per-query where-filters: deduplicated by handle; all NULL = unfiltered, one handle for every query = p->filter
+static int qfilter_plan(SearchCall &k) {
+    const oc_search_params *p = k.p; const uint32_t B = k.B;
+    QFilterJob &qfj = k.qfj;
+    if (!k.r.q_filters_ok)
+        return fail(OC_ERR_UNSUPPORTED, "q_filters: per-query filters are supported by oc_search, oc_search_q_sorted and "
+                                        "oc_search_q_groups only");
+    if (p->filter || p->filter_bits) return fail(OC_ERR_INVALID, "q_filters together with filter / filter_bits");
+    if (p->sharded) return fail(OC_ERR_UNSUPPORTED, "q_filters over a sharded search");
+    std::unordered_map<const oc_filter *, uint32_t> idx;
+    std::vector<const oc_filter *> distinct;
+    bool any_none = false;
+    qfj.q_slot.resize(B);
+    for (uint32_t b = 0; b < B; b++) {
+        const oc_filter *f = p->q_filters[b];
+        if (!f) { any_none = true; qfj.q_slot[b] = SLOT_NONE; continue; }
+        if (f->ctx != k.c) return fail(OC_ERR_INVALID, "q_filters[%u] belongs to another ctx", b);
+        auto it = idx.emplace(f, (uint32_t)distinct.size()).first;
+        if (it->second == distinct.size()) distinct.push_back(f);
+        qfj.q_slot[b] = it->second;
+    }
+    if (distinct.size() > 65535) return fail(OC_ERR_UNSUPPORTED, "q_filters: %zu distinct handles > 65535", distinct.size());
+    if (distinct.size() == 1 && !any_none) k.batch_filter = distinct[0];
+    else if (!distinct.empty()) {
+        k.per_q = true;
+        const uint32_t K = (uint32_t)distinct.size();
+        for (const oc_filter *f : distinct) qfj.slots.push_back(RowsOkSlot{f->bits, f->nbits});
+        qfj.slots.push_back(RowsOkSlot{nullptr, 0});
+        qfj.q_slot_ft.resize(B);
+        for (uint32_t b = 0; b < B; b++) qfj.q_slot_ft[b] = qfj.q_slot[b] == SLOT_NONE ? K : qfj.q_slot[b];
+    }
+    return OC_OK;
+}
+
+// The checks that need no device, and the call's shape and path.  B == 0 stops here.
+static int search_check(SearchCall &k) {
+    oc_ctx *c = k.c; const SearchReq &r = k.r;
+    const oc_search_params *p = r.p;
+    if (!c || !p || !r.out_count) return fail(OC_ERR_INVALID, "NULL argument");
+    k.write_hits = !(r.gj || (r.fj && r.fj->hits_optional)) || p->limit > 0;
+    if (k.write_hits && (!r.out_doc_ids || !r.out_scores || !r.out_n)) return fail(OC_ERR_INVALID, "NULL argument");
+    const uint32_t B = k.B = p->n_queries;
+    if (B == 0) return OC_OK;
+    k.has_v = p->mode == OC_MODE_VECTOR || p->mode == OC_MODE_HYBRID;
+    k.has_ft = p->mode == OC_MODE_FULLTEXT || p->mode == OC_MODE_HYBRID;
+    if (!k.has_v && !k.has_ft) return fail(OC_ERR_INVALID, "unknown mode %d", p->mode);
+    if (k.has_v && (!k.emb || !p->q_vecs)) return fail(OC_ERR_INVALID, "vector/hybrid mode needs emb and q_vecs");
+    if (k.has_ft && (!k.str || !p->q_token_offsets)) return fail(OC_ERR_INVALID, "fulltext/hybrid mode needs str and tokens");
+    if (k.emb && k.emb->ctx != c) return fail(OC_ERR_INVALID, "emb belongs to another ctx");
+    if (k.str && k.str->ctx != c) return fail(OC_ERR_INVALID, "str belongs to another ctx");
+    k.batch_filter = p->filter;
+    if (p->q_filters) OCTRY(qfilter_plan(k));
+    if (p->limit == 0 && k.write_hits) return fail(OC_ERR_INVALID, "limit must be >= 1");
+    const PinJob *pj = r.pj; const SortJob *sj = r.sj;
+    const uint32_t limit = k.limit = k.write_hits ? p->limit : 1;
+    // sort_token_scores with pins selects the top 2 * (limit + offset) (sort.rs:25-34); the vector depth stays limit
+    k.pin_flat = pj && pj->splice && k.write_hits && !sj;
+    k.sort_flat = sj && k.write_hits;
+    // sort_token_scores with sort_by: top_count keys in field order, twice as many for an active pinned query
+    k.sort_top = k.sort_flat ? uint32_t((uint64_t(limit) + p->offset) * (pj->splice ? 2 : 1)) : 0u;
+    // oc_search_q_sorted: the queries in score order take K4's list, spliced as pin_flat does
+    bool score_active = false;
+    if (k.sort_flat && sj->by_score && pj->splice)
+        for (uint32_t q = 0; q < B; q++) score_active = score_active || (sj->q_ent[q] == SORT_BY_SCORE && pj->cnt[q] > 0);
+    k.k4_top = k.pin_flat || (k.sort_flat && sj->by_score);   // K4 writes its top n_keep (offset 0) for a splice
+    const uint64_t n_keep64 = (uint64_t(limit) + p->offset) * (k.pin_flat || score_active ? 2 : 1);
+    if (n_keep64 > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "limit+offset %llu > %u", (unsigned long long)n_keep64, OC_MAX_TOPK);
+    k.n_keep = (uint32_t)n_keep64;
+    // limit_hint = limit, NOT limit+offset (search.rs:330-336); vector_limit lets a multi-index caller keep that depth
+    k.vlimit = !k.write_hits ? 0u : p->vector_limit ? p->vector_limit : limit;
+    if (k.vlimit > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "vector_limit %u > %u", k.vlimit, OC_MAX_TOPK);
+    if (p->sharded && !c->comm.ready()) return fail(OC_ERR_COMM, "sharded search without oc_comm_init");
+    k.exports = r.gj || pj || sj;   // K4 exports the normalisation and the vector part of the score map
+    k.pin_items = pj && pj->stride;
+    k.facets = r.fj && !r.fj->q.empty();
+    return OC_OK;
+}
+
+// per-query filters and the facet work list travel with the call's first upload
+static void add_first_tables(SearchCall &k) {
+    Packer &pk = *k.first;
+    if (k.per_q) {
+        k.s_qslots = pk.add(k.qfj.slots.data(), k.qfj.slots.size());
+        k.s_qslot = pk.add(k.qfj.q_slot.data(), k.B);
+        k.s_qslot_ft = pk.add(k.qfj.q_slot_ft.data(), k.B);
+    }
+    if (k.facets) {
+        k.s_fslices = pk.add(k.fpl.slices.data(), k.fpl.slices.size());
+        k.s_fpairs = pk.add(k.fpl.pairs.data(), k.fpl.pairs.size());
+    }
+}
+static void bind_first_tables(SearchCall &k) {
+    const DevBuf &b = *k.first_blob;
+    if (k.filter_h) k.filter_dev = k.s_flt.at(b);
+    k.qfj.d_slots = k.s_qslots.at(b);
+    k.qfj.d_q_slot = k.s_qslot.at(b);
+    k.qfj.d_q_slot_ft = k.s_qslot_ft.at(b);
+    k.fpl.d_slices = k.s_fslices.at(b);
+    k.fpl.d_pairs = k.s_fpairs.at(b);
+}
+
+// Vector stage first: the query vectors (+ filter) go up alone and the matrix sweep starts; the host-side descriptor
+// work of the next stages overlaps it.
+static int vector_first(SearchCall &k) {
+    oc_ctx *c = k.c; const oc_search_params *p = k.p;
+    const uint32_t B = k.B;
+    if (k.batch_filter && k.batch_filter->ctx != c) return fail(OC_ERR_INVALID, "filter belongs to another ctx");
+    k.filter_h = !k.batch_filter && p->filter_bits != nullptr;
+    k.filter = k.filter_h || k.batch_filter != nullptr;
+    k.filter_nbits = k.batch_filter ? k.batch_filter->nbits : p->filter_nbits;
+    k.fwords = k.filter_h ? (p->filter_nbits + 63) / 64 : 0;
+    k.filter_dev = k.batch_filter ? k.batch_filter->bits : nullptr;
+    k.first = k.has_v ? &k.pk0 : &k.pk;
+    k.first_blob = k.has_v ? &c->in_blob0 : &c->in_blob;
+    Slot<float> s_qv;
+    if (k.has_v) s_qv = k.pk0.add(p->q_vecs, size_t(B) * k.emb->dim, is_pinned_host(p->q_vecs));
+    if (k.filter_h) k.s_flt = k.first->add(p->filter_bits, k.fwords);
+    if (!k.has_v) return OC_OK;
+    add_first_tables(k);
+    CU(cudaEventRecord(c->ev[EV_START], c->stream));
+    OCTRY(upload(k.pk0, c->h_in0, c->in_blob0, c->stream));
+    CU(cudaEventRecord(c->ev[EV_H2D], c->stream));
+    bind_first_tables(k);
+    if (k.vlimit) {
+        OCTRY(run_vector_stage(c, k.emb, s_qv.at(c->in_blob0), B, k.vlimit, p->similarity, k.filter_dev, k.filter_nbits,
+                               k.per_q ? &k.qfj : nullptr));
+    } else {   // limit_hint 0 (groups only): no vector hit
+        OCTRY(c->v_cnt.ensure(size_t(B) * 4));
+        CU(cudaMemsetAsync(c->v_cnt.p, 0, size_t(B) * 4, c->stream));
+    }
+    return OC_OK;
+}
+
+// Batch-level sharing of per-posting contributions (single-term tokens with a host-known idf) and the dense form of
+// hot terms.  Not with per-query filters: the precomputed contributions and dense arrays are masked by ONE row bitmap.
+static int ft_share_dense(SearchCall &k) {
+    oc_ctx *c = k.c;
+    std::vector<TermDesc> &terms = k.terms;
+    const std::vector<TokenDesc> &tokens = k.tokens;
+    struct U { uint32_t first_e; uint32_t uses; };
+    struct K128 { uint64_t a, b; };            // (field, term) | (weight bits, idf bits)
+    size_t cap_t = 64;
+    while (cap_t < tokens.size() * 2) cap_t <<= 1;
+    std::vector<K128> tab_k(cap_t);
+    std::vector<uint32_t> tab_v(cap_t, 0xffffffffu);   // open addressing, linear probing
+    std::vector<U> uniq;
+    std::vector<uint32_t> e_to_u(terms.size(), 0xffffffffu);
+    uint64_t walked = 0, distinct = 0;
+    for (size_t t = 0; t < tokens.size(); t++) {
+        const TokenDesc &tk = tokens[t];
+        if (tk.term_end - tk.term_begin != 1 || k.tok_need_df[t]) continue;
+        const uint32_t e = tk.term_begin;
+        if (terms[e].len < 64) continue;
+        uint32_t wb, ib;
+        memcpy(&wb, &terms[e].weight, 4); memcpy(&ib, &tk.idf, 4);
+        const K128 key{k.term_key[e], (uint64_t(wb) << 32) | ib};
+        uint64_t h = (key.a * 0x9E3779B97F4A7C15ull) ^ (key.b * 0xC2B2AE3D27D4EB4Full);
+        size_t slot = (h ^ (h >> 29)) & (cap_t - 1);
+        while (tab_v[slot] != 0xffffffffu && !(tab_k[slot].a == key.a && tab_k[slot].b == key.b)) slot = (slot + 1) & (cap_t - 1);
+        if (tab_v[slot] == 0xffffffffu) {
+            tab_k[slot] = key; tab_v[slot] = (uint32_t)uniq.size();
+            uniq.push_back({e, 0}); distinct += terms[e].len;
+        }
+        uniq[tab_v[slot]].uses++;
+        e_to_u[e] = tab_v[slot];
+        walked += terms[e].len;
+    }
+    const char *share_env = getenv("OC_BM25_SHARE");   // "off" / "force": A/B testing of the sharing pass
+    const bool share_off = share_env && !strcmp(share_env, "off"), share_force = share_env && !strcmp(share_env, "force");
+    // hot terms (a posting in at least every 16th row) go DENSE: their contributions are scattered once per batch
+    // into a float[rows] array and every (query, tile) item adds 8192 floats with 128-bit loads instead of
+    // walking ~thousands of postings (posting-centred kernel only: every token of the batch has <= 1 term)
+    const char *dense_env = getenv("OC_BM25_DENSE");
+    const char *t2_env = getenv("OC_BM25_TILE2");
+    const bool dense_on = !k.any_multi && !(dense_env && dense_env[0] == '0') && !share_off && !(t2_env && t2_env[0] == '0');
+    const uint64_t rows_pad = uint64_t(k.n_tiles) * BM25_TILE;
+    const uint64_t dense_min = std::max<uint64_t>(512, k.S->n_rows / 16);
+    std::vector<uint8_t> u_dense(uniq.size(), 0);
+    uint64_t n_dense = 0;
+    if (dense_on)
+        for (size_t u = 0; u < uniq.size(); u++)
+            if (terms[uniq[u].first_e].len >= dense_min && (n_dense + 1) * rows_pad * 4 <= (size_t(8) << 30)) { u_dense[u] = 1; n_dense++; }
+    uint64_t walked_l = 0, distinct_l = 0;   // what is left for the list form
+    for (size_t e = 0; e < terms.size(); e++)
+        if (e_to_u[e] != 0xffffffffu && !u_dense[e_to_u[e]]) walked_l += terms[e].len;
+    for (size_t u = 0; u < uniq.size(); u++) if (!u_dense[u]) distinct_l += terms[uniq[u].first_e].len;
+    const bool lists = distinct_l && !share_off && (share_force || (walked_l >= 2 * distinct_l && walked_l >= (64u << 20))) &&
+                       distinct_l * 8 <= (size_t(6) << 30);
+    if (!lists && !n_dense) return OC_OK;
+    if (lists) OCTRY(c->pre_post.ensure(distinct_l * 8 + 64));
+    if (n_dense) OCTRY(c->dense_buf.ensure(n_dense * rows_pad * 4));
+    k.dense_bytes = n_dense * rows_pad * 4;
+    uint64_t off = 0, doff = 0;
+    std::vector<uint64_t> u_off(uniq.size());
+    std::vector<uint8_t> u_used(uniq.size(), 0);
+    for (size_t u = 0; u < uniq.size(); u++) {
+        if (!u_dense[u] && !lists) continue;
+        u_used[u] = 1;
+        const TermDesc &td = terms[uniq[u].first_e];
+        PreDesc pd{};
+        pd.src = td.ptr; pd.len = td.len; pd.weight = td.weight;
+        pd.idf = tokens[k.term_token[uniq[u].first_e]].idf;
+        if (u_dense[u]) { u_off[u] = doff; pd.dense = c->dense_buf.as<float>() + doff; doff += rows_pad; }
+        else { u_off[u] = off; pd.dst = c->pre_post.as<Posting>() + off; off += td.len; }
+        const uint32_t pi = (uint32_t)k.pre_descs.size();
+        k.pre_descs.push_back(pd);
+        for (uint32_t ch = 0; ch * PRE_CHUNK < td.len; ch++) k.pre_items.push_back(make_uint2(pi, ch));
+    }
+    for (size_t e = 0; e < terms.size(); e++) {
+        const uint32_t u = e_to_u[e];
+        if (u == 0xffffffffu || !u_used[u]) continue;
+        if (u_dense[u]) { terms[e].ptr = reinterpret_cast<const Posting *>(c->dense_buf.as<float>() + u_off[u]); terms[e].flags |= TD_DENSE; }
+        else { terms[e].ptr = c->pre_post.as<Posting>() + u_off[u]; terms[e].flags |= TD_PRE; }
+    }
+    return OC_OK;
+}
+
+// item order of the register-folded scorers (Bm25Params::perm): queries by their number of dense tokens, descending
+static void bm25_item_order(SearchCall &k) {
+    const uint32_t B = k.B;
+    std::vector<uint8_t> nd_q(B, 0);
+    for (uint32_t q = 0; q < B; q++) {
+        uint32_t nd = 0;
+        for (uint32_t t = k.queries[q].token_begin; t < k.queries[q].token_end; t++)
+            if (k.tokens[t].term_end > k.tokens[t].term_begin && (k.terms[k.tokens[t].term_begin].flags & TD_DENSE) &&
+                k.terms[k.tokens[t].term_begin].len)
+                nd++;
+        nd_q[q] = (uint8_t)std::min<uint32_t>(nd, BM25_CLASSES - 1);
+    }
+    // (used with OC_BM25_ORDER=1 only.)  TWO classes: every query with a dense token (one tile-major pass over the dense
+    // arrays: one class per dense-token count re-streamed those arrays once per class and cost the 10M-document
+    // workload 20 %), then the list-only queries, whose items are cheap and touch no dense array.  Inside the first
+    // class the queries are sorted by their number of dense tokens, descending.
+    auto cls_of = [&](uint32_t q) { return nd_q[q] ? 0u : BM25_CLASSES - 1; };
+    for (uint32_t q = 0; q < B; q++) k.cls_nq[cls_of(q)]++;
+    k.q_perm.resize(B);
+    uint32_t at[BM25_CLASSES], acc = 0;
+    for (uint32_t g = 0; g < BM25_CLASSES; g++) { at[g] = acc; acc += k.cls_nq[g]; }
+    for (int nd = BM25_CLASSES - 1; nd >= 0; nd--)
+        for (uint32_t q = 0; q < B; q++) if (nd_q[q] == nd) k.q_perm[at[cls_of(q)]++] = q;
+}
+
+// The fulltext descriptors: terms, tokens and queries, each token's idf where the host knows it, the sharing / dense
+// selection and the scorers' item order.
+static int ft_descriptors(SearchCall &k) {
+    oc_ctx *c = k.c; const oc_search_params *p = k.p;
+    const uint32_t B = k.B; StrSnap *S = k.S;
+    k.multi_rank = p->sharded && c->comm.world > 1;
+    // sharded: every rank must take the same df decisions (they drive a collective), so the
+    // tombstone state is the caller's global flag (OC_SHARD_TOMBSTONES), not this shard's
+    const bool tombs_local = k.has_ft && S->n_deleted > 0;
+    if (k.multi_rank && tombs_local && !(p->sharded & OC_SHARD_TOMBSTONES))
+        return fail(OC_ERR_INVALID, "sharded search: this shard holds tombstones, set OC_SHARD_TOMBSTONES on every rank");
+    k.tombs = k.has_ft && (k.multi_rank ? (p->sharded & OC_SHARD_TOMBSTONES) != 0 : tombs_local);
+    k.n_tiles = k.has_ft ? (uint32_t)((S->n_rows + BM25_TILE - 1) / BM25_TILE) : 0;
+    // sharded: df comes from the replicated per-term table, or — OC_SHARD_COUNT_DF on every rank, e.g. after a
+    // commit dropped the table — from counting + all-reduce.  A shard-local list length is never a corpus df.
+    k.count_df = k.multi_rank && (p->sharded & OC_SHARD_COUNT_DF) != 0;
+    k.thr = p->threshold >= 0.0f;
+    if (!k.has_ft) return OC_OK;
+    bool df_local_only = false;
+    for (auto &f : S->fields)   // streamed posting format depends on (avg_field_len, b): derive once
+        if (f.n_post && f.b_cached != p->bm25_b) {
+            bm25_derive_postings_kernel<<<(unsigned)((f.n_post + 255) / 256), 256, 0, c->stream>>>(f.raw, f.n_post, f.avg_len, p->bm25_b, f.post);
+            launched(c);
+            CU(cudaGetLastError());
+            f.b_cached = p->bm25_b;
+            k.derived_now = true;   // queued on the main stream: this call keeps the BM25 prologue there too
+        }
+    const float N = (float)S->document_count;  // token_score.rs:221
+    k.queries.resize(B);
+    // Per-query filters are routed as a filtered batch is: df is counted on the device (need_df), so nothing is shared
+    // or dense and K3b / K3 score the batch, each (tile, query) item under its query's row bitmap.  A token keeps the
+    // idf its query would get alone: counted under the query's filter, or — single term, no filter, no tombstones —
+    // from the host's posting-list length (or corpus df table), as a plain oc_search does.  An unfiltered query runs
+    // under the tombstone-only row bitmap (slot K), so it scores exactly the rows it would score alone.
+    if (k.per_q) k.need_df = true;
+    for (uint32_t q = 0; q < B; q++) {
+        const uint32_t t0 = p->q_token_offsets[q], t1 = p->q_token_offsets[q + 1];
+        const bool q_filter = k.filter || (k.per_q && k.qfj.q_slot[q] != SLOT_NONE);
+        QueryDesc qd{};
+        qd.token_begin = (uint32_t)k.tokens.size();
+        const uint32_t ntok = t1 - t0;
+        k.max_tokens = std::max(k.max_tokens, ntok);
+        qd.required = k.thr ? (uint32_t)floorf((float)ntok * p->threshold) : 0;  // token_score.rs:211-218
+        qd.flags = k.thr ? QF_THRESHOLD : 0;
+        for (uint32_t t = t0; t < t1; t++) {
+            TokenDesc tk{};
+            tk.term_begin = (uint32_t)k.terms.size();
+            tk.bit = 1u << ((t - t0) & 31u);
+            uint64_t df_known = 0;
+            for (uint32_t e = p->token_term_offsets[t]; e < p->token_term_offsets[t + 1]; e++) {
+                const uint32_t fi = p->term_field[e], ti = p->term_id[e];
+                if (fi >= S->fields.size()) return fail(OC_ERR_INVALID, "term field %u out of range", fi);
+                const StrField &f = S->fields[fi];
+                if (ti >= f.n_terms) continue;  // unknown term: no postings
+                TermDesc td{};
+                td.ptr = f.post + f.term_offsets[ti];
+                td.len = (uint32_t)(f.term_offsets[ti + 1] - f.term_offsets[ti]);
+                td.weight = p->term_weight ? p->term_weight[e] : 1.0f;
+                td.avg_len = f.avg_len;
+                df_known = f.global_df.empty() ? td.len : f.global_df[ti];
+                if (k.multi_rank && f.global_df.empty()) df_local_only = true;
+                k.postings_walked += td.len;
+                k.term_key.push_back((uint64_t(fi) << 32) | ti);
+                k.terms.push_back(td);
+                k.term_token.push_back((uint32_t)k.tokens.size());
+            }
+            tk.term_end = (uint32_t)k.terms.size();
+            const uint32_t nt = tk.term_end - tk.term_begin;
+            uint8_t need = 0;
+            if (nt == 1 && !q_filter && !k.tombs && !k.count_df) tk.idf = host_idf(N, std::max<uint64_t>(1, df_known));
+            else if (nt == 0) tk.idf = host_idf(N, 1);
+            else { need = 1; k.need_df = true; tk.idf = 0.f; }
+            if (nt != 1) { k.any_multi = k.any_multi || nt > 1; }
+            k.tokens.push_back(tk);
+            k.tok_need_df.push_back(need);
+            if (k.per_q) k.tok_slot.push_back(k.qfj.q_slot_ft[q]);
+        }
+        qd.token_end = (uint32_t)k.tokens.size();
+        k.queries[q] = qd;
+    }
+    // K3b holds a query's tokens in a BM25_MAX_TOK-entry shared table: a batch with a longer query goes to the
+    // accumulator kernel (K3), which walks any number of tokens, like a batch with multi-term tokens
+    if (k.max_tokens > BM25_MAX_TOK) k.any_multi = true;
+    if (df_local_only && !k.count_df)
+        return fail(OC_ERR_INVALID, "sharded search: a field of this shard has no corpus-wide df table (dropped by a commit?): "
+                                    "reload it or pass OC_SHARD_COUNT_DF on every rank");
+    if (!k.per_q) OCTRY(ft_share_dense(k));
+    if (!k.any_multi && k.max_tokens <= BM25_FLAT_TOK) bm25_item_order(k);
+    return OC_OK;
+}
+
+// OMC rows for the tile kernel: the documents' string rows, ascending
+static int omc_plan(SearchCall &k) {
+    const oc_search_params *p = k.p; const StrSnap *S = k.S;
+    const uint32_t n_omc = k.n_omc = (uint32_t)p->n_omc;
     if (n_omc && (!p->omc_doc_ids || !p->omc_mult)) return fail(OC_ERR_INVALID, "omc arrays are NULL");
-    if (n_omc && has_ft) {
+    if (n_omc && k.has_ft) {
         for (uint32_t i = 0; i < n_omc; i++) {
             if (i && p->omc_doc_ids[i] <= p->omc_doc_ids[i - 1]) return fail(OC_ERR_INVALID, "omc_doc_ids must be ascending");
             uint64_t r;
@@ -2285,431 +2410,430 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
                 if (it == S->row_doc_host.end() || *it != p->omc_doc_ids[i]) continue;
                 r = uint64_t(it - S->row_doc_host.begin());
             }
-            omc_rows.push_back((uint32_t)r); omc_row_mult.push_back(p->omc_mult[i]);
+            k.omc_rows.push_back((uint32_t)r); k.omc_row_mult.push_back(p->omc_mult[i]);
         }
     }
-    const bool omc_tile = !omc_rows.empty();
+    k.omc_tile = !k.omc_rows.empty();
+    return OC_OK;
+}
 
-    // ------------------------------------------------------------ H2D: descriptors in one packed blob
-    Packer pk;
-    const size_t o_flt = (filter_h && !has_v) ? pk.add(p->filter_bits, fwords * 8) : 0;
-    const size_t o_terms = has_ft ? pk.add(terms.data(), terms.size() * sizeof(TermDesc)) : 0;
-    const size_t o_tokens = has_ft ? pk.add(tokens.data(), tokens.size() * sizeof(TokenDesc)) : 0;
-    const size_t o_ttok = has_ft ? pk.add(term_token.data(), term_token.size() * 4) : 0;
-    const size_t o_pre = pre_descs.empty() ? 0 : pk.add(pre_descs.data(), pre_descs.size() * sizeof(PreDesc));
-    const size_t o_pitems = pre_items.empty() ? 0 : pk.add(pre_items.data(), pre_items.size() * sizeof(uint2));
-    const size_t o_queries = has_ft ? pk.add(queries.data(), queries.size() * sizeof(QueryDesc)) : 0;
-    const size_t o_omcd = n_omc ? pk.add(p->omc_doc_ids, size_t(n_omc) * 8) : 0;
-    const size_t o_omcm = n_omc ? pk.add(p->omc_mult, size_t(n_omc) * 4) : 0;
-    const size_t o_omcr = omc_tile ? pk.add(omc_rows.data(), omc_rows.size() * 4) : 0;
-    const size_t o_omcrm = omc_tile ? pk.add(omc_row_mult.data(), omc_row_mult.size() * 4) : 0;
-    size_t o_qf[3] = {0, 0, 0}, o_fpl[2] = {0, 0};
-    if (per_q && !has_v) add_qf(pk, o_qf);
-    if (facets && !has_v) add_fpl(pk, o_fpl);
-    const size_t o_tslot = (per_q && !tok_slot.empty()) ? pk.add(tok_slot.data(), tok_slot.size() * 4) : 0;
-    // item order of the register-folded scorers (Bm25Params::perm): queries by their number of dense tokens, descending
-    std::vector<uint32_t> q_perm;
-    uint32_t cls_nq[BM25_CLASSES] = {0, 0, 0, 0, 0};
-    if (has_ft && !any_multi && max_tokens <= BM25_FLAT_TOK) {
-        std::vector<uint8_t> nd_q(B, 0);
-        for (uint32_t q = 0; q < B; q++) {
-            uint32_t nd = 0;
-            for (uint32_t t = queries[q].token_begin; t < queries[q].token_end; t++)
-                if (tokens[t].term_end > tokens[t].term_begin && (terms[tokens[t].term_begin].flags & TD_DENSE) && terms[tokens[t].term_begin].len) nd++;
-            nd_q[q] = (uint8_t)std::min<uint32_t>(nd, BM25_CLASSES - 1);
-        }
-        // (used with OC_BM25_ORDER=1 only.)  TWO classes: every query with a dense token (one tile-major pass over the dense
-        // arrays: one class per dense-token count re-streamed those arrays once per class and cost the 10M-document
-        // workload 20 %), then the list-only queries, whose items are cheap and touch no dense array.  Inside the first
-        // class the queries are sorted by their number of dense tokens, descending.
-        auto cls_of = [&](uint32_t q) { return nd_q[q] ? 0u : BM25_CLASSES - 1; };
-        for (uint32_t q = 0; q < B; q++) cls_nq[cls_of(q)]++;
-        q_perm.resize(B);
-        uint32_t at[BM25_CLASSES], acc = 0;
-        for (uint32_t g = 0; g < BM25_CLASSES; g++) { at[g] = acc; acc += cls_nq[g]; }
-        for (int nd = BM25_CLASSES - 1; nd >= 0; nd--)
-            for (uint32_t q = 0; q < B; q++) if (nd_q[q] == nd) q_perm[at[cls_of(q)]++] = q;
-    }
-    const size_t o_perm = q_perm.empty() ? 0 : pk.add(q_perm.data(), q_perm.size() * 4);
-    const bool pin_items = pj && pj->stride;
-    const size_t o_pdoc = pin_items ? pk.add(pj->doc.data(), pj->doc.size() * 8) : 0;
-    const size_t o_ppos = pin_items ? pk.add(pj->pos.data(), pj->pos.size() * 4) : 0;
-    const size_t o_pcnt = pin_items ? pk.add(pj->cnt.data(), pj->cnt.size() * 4) : 0;
-    // sortBy: the batch's entries and each query's entry and top_count (doubled for an active query)
-    std::vector<SortEntry> s_ents;
-    std::vector<SortQuery> s_q;
-    std::vector<uint8_t> s_alt;
+// sortBy: the batch's entries and each query's entry and top_count (doubled for an active query).  Groups: the batch's
+// distinct handles and the work list of (query, group) items, one span per query with groups: the queries in score
+// order first, then those in field order (one launch of group_topk_kernel / group_sort_topk_kernel each).
+static void sort_group_plan(SearchCall &k) {
+    const SortJob *sj = k.r.sj; const PinJob *pj = k.r.pj;
+    GroupJob *gj = k.r.gj; const uint32_t B = k.B;
+    const bool rows = k.has_ft && k.n_tiles > 0;
     if (sj)
         for (uint32_t e = 0; e < sj->f.size(); e++) {
             const SortOrder &o = sj->ord(e);
-            s_ents.push_back(SortEntry{o.n, has_ft && n_tiles > 0 ? o.rank_row : nullptr, o.doc_rank, sj->f[e]->nbits, o.rank_doc});
+            k.s_ents.push_back(SortEntry{o.n, rows ? o.rank_row : nullptr, o.doc_rank, sj->f[e]->nbits, o.rank_doc});
         }
-    if (sort_flat) {
-        s_q.resize(B);
-        s_alt.resize(B);
+    if (k.sort_flat) {
+        k.s_q.resize(B);
+        k.s_alt.resize(B);
         for (uint32_t q = 0; q < B; q++) {
             const bool active = pj->splice && pj->cnt[q] > 0;
-            s_q[q] = SortQuery{sj->q_ent[q], uint32_t((uint64_t(limit) + p->offset) * (active ? 2 : 1))};
-            s_alt[q] = sj->q_ent[q] == SORT_BY_SCORE;
+            k.s_q[q] = SortQuery{sj->q_ent[q], uint32_t((uint64_t(k.limit) + k.p->offset) * (active ? 2 : 1))};
+            k.s_alt[q] = sj->q_ent[q] == SORT_BY_SCORE;
         }
     }
-    const size_t o_sent = sj ? pk.add(s_ents.data(), s_ents.size() * sizeof(SortEntry)) : 0;
-    // groups: the batch's distinct handles and the work list of (query, group) items, one span per query with groups:
-    // the queries in score order first, then those in field order (one launch of group_topk_kernel /
-    // group_sort_topk_kernel each)
-    std::vector<GroupHandle> g_hand;
-    std::vector<GroupSpan> g_spans;
+    if (!gj) return;
+    for (const oc_group_by *g : gj->h) k.g_hand.push_back(GroupHandle{g->off, g->docs, rows ? g->rows : nullptr, g->n_groups});
+    uint32_t first = 0;
+    gj->top = 0;
+    gj->direct = !pj->splice;
+    for (int by_field = 0; by_field < 2; by_field++) {
+        for (uint32_t q = 0; q < B; q++) {
+            const uint32_t h = gj->q_h[q];
+            const uint32_t ent = sj ? sj->q_ent[q] : SORT_BY_SCORE;
+            if (h == GROUP_NONE || gj->h[h]->n_groups == 0 || (ent != SORT_BY_SCORE) != bool(by_field)) continue;
+            // sort_groups with pins takes every group's top 2 * max_results for an active query (sort.rs:137-142)
+            const uint32_t m = gj->q_m[q], depth = m * (pj->splice && pj->cnt[q] > 0 ? 2 : 1);
+            k.g_spans.push_back(GroupSpan{first, q, h, depth, m, ent, gj->q_row[q]});
+            first += gj->h[h]->n_groups;
+            gj->top = std::max(gj->top, depth);
+            gj->direct = gj->direct && depth == gj->stride;
+        }
+        if (!by_field) { gj->n_score_spans = (uint32_t)k.g_spans.size(); gj->n_score_items = first; }
+    }
+    gj->n_spans = (uint32_t)k.g_spans.size();
+}
+
+// H2D: the descriptors in one packed blob (segment order is the upload's byte layout), then the output blob's layout.
+static int main_upload(SearchCall &k) {
+    oc_ctx *c = k.c; const oc_search_params *p = k.p;
+    const uint32_t B = k.B; const SortJob *sj = k.r.sj;
+    PinJob *pj = k.r.pj; GroupJob *gj = k.r.gj;
+    Packer &pk = k.pk;
+    if (k.has_ft) {
+        k.s_terms = pk.add(k.terms.data(), k.terms.size());
+        k.s_tokens = pk.add(k.tokens.data(), k.tokens.size());
+        k.s_ttok = pk.add(k.term_token.data(), k.term_token.size());
+    }
+    if (!k.pre_descs.empty()) k.s_pre = pk.add(k.pre_descs.data(), k.pre_descs.size());
+    if (!k.pre_items.empty()) k.s_pitems = pk.add(k.pre_items.data(), k.pre_items.size());
+    if (k.has_ft) k.s_queries = pk.add(k.queries.data(), k.queries.size());
+    if (k.n_omc) {
+        k.s_omcd = pk.add(p->omc_doc_ids, k.n_omc);
+        k.s_omcm = pk.add(p->omc_mult, k.n_omc);
+    }
+    if (k.omc_tile) {
+        k.s_omcr = pk.add(k.omc_rows.data(), k.omc_rows.size());
+        k.s_omcrm = pk.add(k.omc_row_mult.data(), k.omc_row_mult.size());
+    }
+    if (!k.has_v) add_first_tables(k);
+    if (k.per_q && !k.tok_slot.empty()) k.s_tslot = pk.add(k.tok_slot.data(), k.tok_slot.size());
+    if (!k.q_perm.empty()) k.s_perm = pk.add(k.q_perm.data(), k.q_perm.size());
+    Slot<uint64_t> s_pdoc;
+    Slot<uint32_t> s_ppos, s_pcnt;
+    if (k.pin_items) {
+        s_pdoc = pk.add(pj->doc.data(), pj->doc.size());
+        s_ppos = pk.add(pj->pos.data(), pj->pos.size());
+        s_pcnt = pk.add(pj->cnt.data(), pj->cnt.size());
+    }
+    if (sj) k.s_sent = pk.add(k.s_ents.data(), k.s_ents.size());
+    Slot<GroupHandle> s_ghand;
+    Slot<GroupSpan> s_gspan;
     if (gj) {
-        for (const oc_group_by *g : gj->h) g_hand.push_back(GroupHandle{g->off, g->docs, has_ft && n_tiles > 0 ? g->rows : nullptr, g->n_groups});
-        uint32_t first = 0;
-        gj->top = 0;
-        gj->direct = !pj->splice;
-        for (int by_field = 0; by_field < 2; by_field++) {
-            for (uint32_t q = 0; q < B; q++) {
-                const uint32_t h = gj->q_h[q];
-                const uint32_t ent = sj ? sj->q_ent[q] : SORT_BY_SCORE;
-                if (h == GROUP_NONE || gj->h[h]->n_groups == 0 || (ent != SORT_BY_SCORE) != bool(by_field)) continue;
-                // sort_groups with pins takes every group's top 2 * max_results for an active query (sort.rs:137-142)
-                const uint32_t m = gj->q_m[q], depth = m * (pj->splice && pj->cnt[q] > 0 ? 2 : 1);
-                g_spans.push_back(GroupSpan{first, q, h, depth, m, ent, gj->q_row[q]});
-                first += gj->h[h]->n_groups;
-                gj->top = std::max(gj->top, depth);
-                gj->direct = gj->direct && depth == gj->stride;
-            }
-            if (!by_field) { gj->n_score_spans = (uint32_t)g_spans.size(); gj->n_score_items = first; }
-        }
-        gj->n_spans = (uint32_t)g_spans.size();
+        s_ghand = pk.add(k.g_hand.data(), k.g_hand.size());
+        s_gspan = pk.add(k.g_spans.data(), k.g_spans.size());
     }
-    const size_t o_ghand = gj ? pk.add(g_hand.data(), g_hand.size() * sizeof(GroupHandle)) : 0;
-    const size_t o_gspan = gj ? pk.add(g_spans.data(), g_spans.size() * sizeof(GroupSpan)) : 0;
-    const size_t o_sq = sort_flat ? pk.add(s_q.data(), s_q.size() * sizeof(SortQuery)) : 0;
-    const size_t o_salt = sort_flat && sj->by_score ? pk.add(s_alt.data(), s_alt.size()) : 0;
+    if (k.sort_flat) k.s_sq = pk.add(k.s_q.data(), k.s_q.size());
+    if (k.sort_flat && sj->by_score) k.s_salt = pk.add(k.s_alt.data(), k.s_alt.size());
     // hybrid: the descriptors, the shared-contribution precompute, the filter bitmap and the (term, tile) plan do
     // not depend on the vector results: they run on the side stream while the main stream sweeps the matrix
     // (OC_SIDE_STREAM=0 disables it: the step gets ~2.5 % longer, the sweep itself ~4 % shorter — A/B switch)
     const char *senv = getenv("OC_SIDE_STREAM");
     // (single-GPU only for now: the sharded path was measured and validated without it)
-    const bool side = !(senv && senv[0] == '0') && has_v && has_ft && !need_df && !derived_now;
-    if (!has_v) CU(cudaEventRecord(c->ev[EV_START], c->stream));
+    k.side = !(senv && senv[0] == '0') && k.has_v && k.has_ft && !k.need_df && !k.derived_now;
+    if (!k.has_v) CU(cudaEventRecord(c->ev[EV_START], c->stream));
     if (c->side_dirty) { CU(cudaStreamSynchronize(c->side)); c->side_dirty = false; }   // leftover of a failed call
-    if (side) { CU(cudaStreamWaitEvent(c->side, c->ev[EV_H2D], 0)); c->side_dirty = true; }   // the filter bitmap went up with the query vectors
-    OCTRY(upload(pk, c->h_in, c->in_blob, side ? c->side : c->stream));
-    if (!has_v) CU(cudaEventRecord(c->ev[EV_H2D], c->stream));   // hybrid/vector: this copy rides inside the device window
-    c->timing.h2d_bytes = h2d_early + pk.total;
-    uint8_t *din = c->in_blob.as<uint8_t>();
-    if (filter_h && !has_v) filter_dev = reinterpret_cast<const uint64_t *>(din + o_flt);
-    if (per_q && !has_v) bind_qf(din, o_qf);
-    if (facets && !has_v) bind_fpl(din, o_fpl);
+    if (k.side) { CU(cudaStreamWaitEvent(c->side, c->ev[EV_H2D], 0)); c->side_dirty = true; }   // the filter bitmap went up with the query vectors
+    OCTRY(upload(pk, c->h_in, c->in_blob, k.side ? c->side : c->stream));
+    if (!k.has_v) CU(cudaEventRecord(c->ev[EV_H2D], c->stream));   // hybrid/vector: this copy rides inside the device window
+    c->timing.h2d_bytes = k.pk0.total + pk.total;
+    const DevBuf &din = c->in_blob;
+    if (!k.has_v) bind_first_tables(k);
     if (gj) {
-        gj->d_hand = reinterpret_cast<const GroupHandle *>(din + o_ghand);
-        gj->d_spans = reinterpret_cast<const GroupSpan *>(din + o_gspan);
-        gj->d_ents = sj ? reinterpret_cast<const SortEntry *>(din + o_sent) : nullptr;
+        gj->d_hand = s_ghand.at(din);
+        gj->d_spans = s_gspan.at(din);
+        gj->d_ents = k.s_sent.at(din);
     }
-    if (pin_items) {
-        pj->d_doc = reinterpret_cast<const uint64_t *>(din + o_pdoc);
-        pj->d_pos = reinterpret_cast<const uint32_t *>(din + o_ppos);
-        pj->d_cnt = reinterpret_cast<const uint32_t *>(din + o_pcnt);
+    if (k.pin_items) {
+        pj->d_doc = s_pdoc.at(din);
+        pj->d_pos = s_ppos.at(din);
+        pj->d_cnt = s_pcnt.at(din);
     }
-
-    // ------------------------------------------------------------ fulltext stage + fusion (re-runnable)
     // arg-max selection (n_keep <= 32) needs no power-of-two buffer; the bitonic fallback does
     // (also >= BM25_SPARSE_MAX: the sparse finish of the posting-centred kernel pushes at most that many candidates)
-    const uint32_t cap = n_keep <= 32 ? std::max<uint32_t>(n_keep + BM25_CHUNK, BM25_SPARSE_MAX) : next_pow2(std::max<uint32_t>(n_keep + BM25_CHUNK, BM25_SPARSE_MAX));
-    Bm25Params bp{};
-    float *min_hint_dev = nullptr;
-    unsigned int *tile_counter = nullptr;
-    const size_t o_doc = 0, o_sc = size_t(B) * limit * 8, o_n = o_sc + size_t(B) * limit * 4;
-    const size_t o_cnt = (o_n + size_t(B) * 4 + 7) & ~size_t(7), o_min = o_cnt + size_t(B) * 8;
-    const size_t o_gflag = o_min + size_t(B) * 4;                       // sharded: OR over the ranks of the per-query overflow flags
-    const size_t out_bytes = o_gflag + ((size_t(B) + 3) & ~size_t(3));
-    const size_t o_resc = out_bytes + ((size_t(B) + 3) & ~size_t(3));
-    OCTRY(c->out_blob.ensure(out_bytes));
-    OCTRY(c->h_out.ensure(o_resc + size_t(B) * 4));
-    uint8_t *dout = c->out_blob.as<uint8_t>();
-    FuseParams fp{};
-    size_t fuse_smem = 0;
-    bool did_comm = false;
-    // The fulltext stage does not depend on the vector stage (the vector hits' fulltext scores are point lookups
-    // afterwards): in hybrid mode it runs on the side stream, concurrently with the matrix sweep, and is joined
-    // before the lookups and the fusion.  It runs ONCE per call; device_tail (lookups + fusion) is re-runnable.
-    const uint32_t *row_ok = nullptr;
-    auto bm25_stage = [&]() -> int {
-        cudaStream_t ps = side ? c->side : c->stream;
-        CU(cudaEventRecord(c->ev[EV_BM0], ps));
-        const uint64_t ok_words = uint64_t(n_tiles) * (BM25_TILE / 32);
-        if (per_q) {   // one row bitmap per distinct filter (tombstones AND filter), then the tombstone-only slot K
-            OCTRY(c->row_ok.ensure(std::max<uint64_t>(ok_words, 1) * qfj.slots.size() * 4));
-            if (ok_words) {
-                rows_ok_kernel<<<dim3((unsigned)((ok_words + 255) / 256), (unsigned)qfj.slots.size()), 256, 0, ps>>>(
-                    S->row_doc, S->n_rows, tombs ? S->alive : nullptr, nullptr, 0, c->row_ok.as<uint32_t>(), ok_words, qfj.d_slots);
-                launched(c);
-            }
-            row_ok = c->row_ok.as<uint32_t>();
-        } else if (filter || tombs) {
-            OCTRY(c->row_ok.ensure(ok_words * 4));
-            rows_ok_kernel<<<(unsigned)((ok_words + 255) / 256), 256, 0, ps>>>(
-                S->row_doc, S->n_rows, tombs ? S->alive : nullptr, filter_dev, filter_nbits,
-                c->row_ok.as<uint32_t>(), ok_words);
-            launched(c);
-            row_ok = c->row_ok.as<uint32_t>();
-        }
-        if (!pre_items.empty()) {
-            if (dense_bytes) CU(cudaMemsetAsync(c->dense_buf.p, 0, dense_bytes, ps));
-            bm25_precompute_kernel<<<(unsigned)pre_items.size(), 256, 0, ps>>>(
-                reinterpret_cast<const PreDesc *>(din + o_pre), reinterpret_cast<const uint2 *>(din + o_pitems), p->bm25_k, row_ok);
-            launched(c);
-            CU(cudaGetLastError());
-        }
-        const size_t n_td = terms.size();
-        OCTRY(c->seg.ensure((n_td * (size_t(n_tiles) + 1) + 1) * 4));
-        if (n_td) {
-            const uint64_t work = uint64_t(n_td) * (n_tiles + 1);
-            bm25_plan_kernel<<<(unsigned)((work + 255) / 256), 256, 0, ps>>>(
-                reinterpret_cast<const TermDesc *>(din + o_terms), (uint32_t)n_td, n_tiles, c->seg.as<uint32_t>());
-            launched(c);
-        }
-        if (need_df) {   // (never on the side stream)
-            // corpus_df by counting (token_score.rs:262-275), then idf on the host
-            const size_t ntok = tokens.size();
-            OCTRY(c->df_dev.ensure(ntok * 4));
-            CU(cudaMemsetAsync(c->df_dev.p, 0, ntok * 4, c->stream));
-            DfParams dp{};
-            dp.terms = reinterpret_cast<const TermDesc *>(din + o_terms);
-            dp.tokens = reinterpret_cast<const TokenDesc *>(din + o_tokens);
-            dp.n_tokens = (uint32_t)ntok; dp.n_tiles = n_tiles; dp.seg = c->seg.as<uint32_t>();
-            dp.row_ok_bits = row_ok; dp.df = c->df_dev.as<unsigned int>();
-            if (per_q) { dp.tok_ok_slot = reinterpret_cast<const uint32_t *>(din + o_tslot); dp.ok_words = ok_words; }
-            if (n_tiles && ntok) {
-                bm25_df_kernel<<<(unsigned)(uint64_t(n_tiles) * ntok), BM25_THREADS, 0, c->stream>>>(dp);
-                launched(c);
-            }
-            if (multi_rank) {   // corpus df = sum of the shards' counts (disjoint documents)
-                std::string err;
-                if (!c->comm.all_reduce_sum_u32(c->df_dev.p, c->df_dev.p, ntok, c->stream, &err)) return fail(OC_ERR_COMM, "%s", err.c_str());
-            }
-            std::vector<uint32_t> dfh(ntok);
-            CU(cudaMemcpyAsync(dfh.data(), c->df_dev.p, ntok * 4, cudaMemcpyDeviceToHost, c->stream));
-            CU(cudaStreamSynchronize(c->stream));
-            const float N = (float)S->document_count;
-            for (size_t t = 0; t < ntok; t++)
-                if (tok_need_df[t]) tokens[t].idf = host_idf(N, std::max<uint32_t>(1u, dfh[t]));
-            CU(cudaMemcpyAsync(din + o_tokens, tokens.data(), ntok * sizeof(TokenDesc), cudaMemcpyHostToDevice, c->stream));
-        }
-        const size_t slots = size_t(B) * std::max<uint32_t>(n_tiles, 1);
-        OCTRY(c->tau.ensure(size_t(B) * 16 + 16));   // [tau B x 8][min_hint B x 8][work counter]: one memset
-        OCTRY(c->cand_key.ensure(slots * n_keep * 8));
-        OCTRY(c->cand_ft.ensure(slots * n_keep * 4));
-        OCTRY(c->cand_cnt.ensure(slots * 4));
-        OCTRY(c->tile_cnt.ensure(slots * 4));
-        OCTRY(c->tile_max.ensure(slots * 4));
-        OCTRY(c->tile_min.ensure(slots * 4));
-        min_hint_dev = reinterpret_cast<float *>(c->tau.as<uint8_t>() + size_t(B) * 8);
-        tile_counter = reinterpret_cast<unsigned int *>(c->tau.as<uint8_t>() + size_t(B) * 16);
-        CU(cudaMemsetAsync(c->tau.p, 0, size_t(B) * 16 + 16, ps));
-        bp.terms = reinterpret_cast<const TermDesc *>(din + o_terms);
-        bp.tokens = reinterpret_cast<const TokenDesc *>(din + o_tokens);
-        bp.queries = reinterpret_cast<const QueryDesc *>(din + o_queries);
-        bp.term_token = reinterpret_cast<const uint32_t *>(din + o_ttok);
-        bp.seg = c->seg.as<uint32_t>();
-        bp.n_queries = B; bp.n_tiles = n_tiles; bp.n_rows = S->n_rows;
-        bp.k = p->bm25_k; bp.b = p->bm25_b;
-        bp.row_ok_bits = row_ok;
-        if (per_q) { bp.q_ok_slot = qfj.d_q_slot_ft; bp.ok_words = ok_words; }
-        bp.omc_row = omc_tile ? reinterpret_cast<const uint32_t *>(din + o_omcr) : nullptr;
-        bp.omc_mult = omc_tile ? reinterpret_cast<const float *>(din + o_omcrm) : nullptr;
-        bp.n_omc = (uint32_t)omc_rows.size();
-        bp.v_row = nullptr;            // the hybrid lookups are point lookups (bm25_point_kernel)
-        bp.v_stride = vlimit;
-        bp.v_ft = nullptr; bp.v_present = nullptr;
-        bp.min_hint = min_hint_dev;
-        bp.n_keep = n_keep; bp.cap = cap;
-        bp.tau = c->tau.as<unsigned long long>();
-        bp.cand_key = c->cand_key.as<uint64_t>(); bp.cand_ft = c->cand_ft.as<float>();
-        bp.cand_cnt = c->cand_cnt.as<uint32_t>(); bp.tile_count = c->tile_cnt.as<uint32_t>();
-        bp.tile_max = c->tile_max.as<float>(); bp.tile_min = c->tile_min.as<float>();
-        bp.tile_first = 0;
-        if (!q_perm.empty()) {
-            bp.perm = reinterpret_cast<const uint32_t *>(din + o_perm);
-            uint32_t off = 0, q0 = 0;
-            for (uint32_t g = 0; g < BM25_CLASSES; g++) {
-                bp.cls_off[g] = off; bp.cls_nq[g] = cls_nq[g]; bp.cls_q0[g] = q0;
-                off += cls_nq[g] * n_tiles; q0 += cls_nq[g];
-            }
-        }
-        if (fj || gj || sj) {   // facets / groups / sortBy: the tile kernels also emit the bitmap of matched rows (every (query, tile) item writes its 256 words)
-            OCTRY(c->mbits.ensure(size_t(B) * std::max<uint32_t>(n_tiles, 1) * (BM25_TILE / 32) * 4));
-            bp.matched_bits = c->mbits.as<uint32_t>();
-        }
-        if (gj && n_tiles) {   // groups: and the raw score of each matched row
-            OCTRY(c->row_ft.ensure(size_t(B) * n_tiles * BM25_TILE * 4));
-            bp.row_ft = c->row_ft.as<float>();
-        }
-        if (n_tiles) OCTRY(launch_tile(c, bp, n_tiles * B, any_multi, thr, omc_tile, ps, max_tokens, tile_counter, need_df));
-        CU(cudaEventRecord(c->ev[EV_BM1], ps));
-        c->timing.bm25_postings = postings_walked;
-        if (side) {   // join: the lookups and the fusion need the vector hits (main stream) and the tiles (side stream)
-            CU(cudaEventRecord(c->ev_side, c->side));
-            CU(cudaStreamWaitEvent(c->stream, c->ev_side, 0));
-            c->side_dirty = false;
-        }
-        return OC_OK;
-    };
-    if (has_ft) OCTRY(bm25_stage());
+    const uint32_t n_keep = k.n_keep;
+    k.cap = n_keep <= 32 ? std::max<uint32_t>(n_keep + BM25_CHUNK, BM25_SPARSE_MAX)
+                         : next_pow2(std::max<uint32_t>(n_keep + BM25_CHUNK, BM25_SPARSE_MAX));
+    k.o_sc = size_t(B) * k.limit * 8;
+    k.o_n = k.o_sc + size_t(B) * k.limit * 4;
+    k.o_cnt = (k.o_n + size_t(B) * 4 + 7) & ~size_t(7);
+    k.o_min = k.o_cnt + size_t(B) * 8;
+    k.o_gflag = k.o_min + size_t(B) * 4;                       // sharded: OR over the ranks of the per-query overflow flags
+    k.out_bytes = k.o_gflag + ((size_t(B) + 3) & ~size_t(3));
+    k.o_resc = k.out_bytes + ((size_t(B) + 3) & ~size_t(3));
+    OCTRY(c->out_blob.ensure(k.out_bytes));
+    OCTRY(c->h_out.ensure(k.o_resc + size_t(B) * 4));
+    k.dout = c->out_blob.as<uint8_t>();
+    k.d_doc = c->out_blob.as<uint64_t>();
+    k.d_score = reinterpret_cast<float *>(k.dout + k.o_sc);
+    k.d_n = reinterpret_cast<uint32_t *>(k.dout + k.o_n);
+    return OC_OK;
+}
 
-    const bool exports = gj || pj || sj;   // K4 exports the normalisation and the vector part of the score map
-    // pins, after K4: the score-map value of every promoted document, then (pin_flat) the splice into K4's top list
-    auto pin_tail = [&]() -> int {
-        if (!pin_items) return OC_OK;
-        const uint32_t ps = pj->stride;
-        const uint64_t nslot = uint64_t(B) * ps;
-        const unsigned warp_grid = (unsigned)((nslot * 32 + 255) / 256);
-        OCTRY(c->pin_score.ensure(nslot * 4));
-        OCTRY(c->pin_present.ensure(nslot));
-        if (has_ft) {   // the promoted documents' string rows and their fulltext scores (the hybrid lookups' kernels)
-            OCTRY(c->pin_row.ensure(nslot * 4));
-            OCTRY(c->pin_ft.ensure(nslot * 4));
-            OCTRY(c->pin_ftp.ensure(nslot));
-            map_docs_to_rows_kernel<<<(unsigned)((nslot + 255) / 256), 256, 0, c->stream>>>(
-                pj->d_doc, pj->d_cnt, ps, B, S->row_doc, S->n_rows, c->pin_row.as<uint32_t>());
-            launched(c);
-            PointParams pp{};
-            pp.terms = bp.terms; pp.tokens = bp.tokens; pp.queries = bp.queries;
-            pp.n_queries = B; pp.v_stride = ps; pp.v_row = c->pin_row.as<uint32_t>(); pp.row_ok_bits = row_ok;
-            pp.q_ok_slot = per_q ? qfj.d_q_slot_ft : nullptr; pp.ok_words = uint64_t(n_tiles) * (BM25_TILE / 32);
-            pp.k = p->bm25_k; pp.threshold = thr ? 1 : 0;
-            pp.v_ft = c->pin_ft.as<float>(); pp.v_present = c->pin_ftp.as<uint8_t>();
-            bm25_point_kernel<<<warp_grid, 256, 0, c->stream>>>(pp);
+// The fulltext stage.  It does not depend on the vector stage (the vector hits' fulltext scores are point lookups
+// afterwards): in hybrid mode it runs on the side stream, concurrently with the matrix sweep, and is joined before the
+// lookups and the fusion.  It runs ONCE per call; device_tail (lookups + fusion) is re-runnable.
+static int bm25_stage(SearchCall &k) {
+    oc_ctx *c = k.c; const oc_search_params *p = k.p;
+    const uint32_t B = k.B, n_tiles = k.n_tiles, n_keep = k.n_keep; const StrSnap *S = k.S;
+    const DevBuf &din = c->in_blob; cudaStream_t ps = k.side ? c->side : c->stream;
+    CU(cudaEventRecord(c->ev[EV_BM0], ps));
+    const uint64_t ok_words = uint64_t(n_tiles) * (BM25_TILE / 32);
+    if (k.per_q) {   // one row bitmap per distinct filter (tombstones AND filter), then the tombstone-only slot K
+        OCTRY(c->row_ok.ensure(std::max<uint64_t>(ok_words, 1) * k.qfj.slots.size() * 4));
+        if (ok_words) {
+            rows_ok_kernel<<<dim3((unsigned)((ok_words + 255) / 256), (unsigned)k.qfj.slots.size()), 256, 0, ps>>>(
+                S->row_doc, S->n_rows, k.tombs ? S->alive : nullptr, nullptr, 0, c->row_ok.as<uint32_t>(), ok_words, k.qfj.d_slots);
             launched(c);
         }
-        PinScoreParams sp{};
-        sp.n_queries = B; sp.stride = ps; sp.doc = pj->d_doc; sp.cnt = pj->d_cnt;
-        sp.has_ft = has_ft; sp.hybrid = has_ft && has_v;
-        sp.ft = c->pin_ft.as<float>(); sp.ft_present = c->pin_ftp.as<uint8_t>();
-        sp.gmin = fp.out_gmin; sp.den = fp.out_den;
-        sp.v_doc = fp.out_vdoc; sp.v_score = fp.out_vscore; sp.v_n = fp.out_vn; sp.v_stride = std::max<uint32_t>(vlimit, 1);
-        sp.omc_doc = fp.omc_doc; sp.omc_mult = fp.omc_mult; sp.n_omc = n_omc;
-        sp.out_score = c->pin_score.as<float>(); sp.out_present = c->pin_present.as<uint8_t>();
-        pin_score_kernel<<<warp_grid, 256, 0, c->stream>>>(sp);
+        k.row_ok = c->row_ok.as<uint32_t>();
+    } else if (k.filter || k.tombs) {
+        OCTRY(c->row_ok.ensure(ok_words * 4));
+        rows_ok_kernel<<<(unsigned)((ok_words + 255) / 256), 256, 0, ps>>>(
+            S->row_doc, S->n_rows, k.tombs ? S->alive : nullptr, k.filter_dev, k.filter_nbits,
+            c->row_ok.as<uint32_t>(), ok_words);
         launched(c);
-        if (pin_flat) {
-            PinSpliceParams xp{};
-            xp.stride = ps; xp.kp2 = std::max<uint32_t>(32, next_pow2(ps));
-            xp.doc = pj->d_doc; xp.pos = pj->d_pos; xp.score = c->pin_score.as<float>(); xp.cnt = pj->d_cnt;
-            xp.n_top = n_keep; xp.limit = limit; xp.offset = p->offset;
-            xp.top_doc = c->pin_top_doc.as<uint64_t>(); xp.top_score = c->pin_top_score.as<float>(); xp.top_n = c->pin_top_n.as<uint32_t>();
-            xp.out_doc = reinterpret_cast<uint64_t *>(dout + o_doc); xp.out_score = reinterpret_cast<float *>(dout + o_sc);
-            xp.out_n = reinterpret_cast<uint32_t *>(dout + o_n);
-            const size_t smem = pin_splice_smem(xp.kp2, n_keep, limit + p->offset);
-            pin_splice_kernel<<<B, PIN_THREADS, smem, c->stream>>>(xp);
-            launched(c);
-        }
+        k.row_ok = c->row_ok.as<uint32_t>();
+    }
+    if (!k.pre_items.empty()) {
+        if (k.dense_bytes) CU(cudaMemsetAsync(c->dense_buf.p, 0, k.dense_bytes, ps));
+        bm25_precompute_kernel<<<(unsigned)k.pre_items.size(), 256, 0, ps>>>(k.s_pre.at(din), k.s_pitems.at(din), p->bm25_k, k.row_ok);
+        launched(c);
         CU(cudaGetLastError());
-        return OC_OK;
-    };
-    // sortBy, after K4 and the pins' scores: the first sort_top keys in field order, scored like promoted documents,
-    // then paged with the pins spliced (pin_splice_kernel writes the hits over K4's)
-    auto sort_tail = [&]() -> int {
-        if (!sort_flat) return OC_OK;
-        if (has_ft && n_tiles > 0)
-            for (uint32_t e = 0; e < sj->f.size(); e++) OCTRY(sort_rows_for(c, sj->ord(e), snap));
-        const uint32_t top = sort_top;
-        const uint64_t nslot = uint64_t(B) * top;
-        const uint32_t vs = std::max<uint32_t>(vlimit, 1);
-        OCTRY(c->srt_doc.ensure(nslot * 8));
-        OCTRY(c->srt_row.ensure(nslot * 4));
-        OCTRY(c->srt_n.ensure(size_t(B) * 4));
-        OCTRY(c->srt_score.ensure(nslot * 4));
-        OCTRY(c->srt_present.ensure(nslot));
-        SortWalkParams wp{};
-        wp.ents = reinterpret_cast<const SortEntry *>(din + o_sent); wp.q = reinterpret_cast<const SortQuery *>(din + o_sq);
-        wp.mbits = has_ft && n_tiles > 0 ? c->mbits.as<uint32_t>() : nullptr; wp.row_words = uint64_t(n_tiles) * (BM25_TILE / 32);
-        wp.v_doc = fp.out_vdoc; wp.v_n = fp.out_vn; wp.v_stride = vs;
-        wp.top = top;
-        wp.out_doc = c->srt_doc.as<uint64_t>(); wp.out_row = c->srt_row.as<uint32_t>(); wp.out_n = c->srt_n.as<uint32_t>();
-        sort_walk_kernel<<<B, SORT_THREADS, size_t(vs) * 4, c->stream>>>(wp);
+    }
+    const size_t n_td = k.terms.size();
+    OCTRY(c->seg.ensure((n_td * (size_t(n_tiles) + 1) + 1) * 4));
+    if (n_td) {
+        const uint64_t work = uint64_t(n_td) * (n_tiles + 1);
+        bm25_plan_kernel<<<(unsigned)((work + 255) / 256), 256, 0, ps>>>(k.s_terms.at(din), (uint32_t)n_td, n_tiles, c->seg.as<uint32_t>());
         launched(c);
-        const unsigned warp_grid = (unsigned)((nslot * 32 + 255) / 256);
-        if (has_ft) {   // the selected rows' fulltext scores (RANK_NONE rows: vector hits without a row, empty slots)
-            OCTRY(c->srt_ft.ensure(nslot * 4));
-            OCTRY(c->srt_ftp.ensure(nslot));
-            PointParams pp{};
-            pp.terms = bp.terms; pp.tokens = bp.tokens; pp.queries = bp.queries;
-            pp.n_queries = B; pp.v_stride = top; pp.v_row = c->srt_row.as<uint32_t>(); pp.row_ok_bits = row_ok;
-            pp.q_ok_slot = per_q ? qfj.d_q_slot_ft : nullptr; pp.ok_words = uint64_t(n_tiles) * (BM25_TILE / 32);
-            pp.k = p->bm25_k; pp.threshold = thr ? 1 : 0;
-            pp.v_ft = c->srt_ft.as<float>(); pp.v_present = c->srt_ftp.as<uint8_t>();
-            bm25_point_kernel<<<warp_grid, 256, 0, c->stream>>>(pp);
+    }
+    if (k.need_df) {   // (never on the side stream)
+        // corpus_df by counting (token_score.rs:262-275), then idf on the host
+        const size_t ntok = k.tokens.size();
+        OCTRY(c->df_dev.ensure(ntok * 4));
+        CU(cudaMemsetAsync(c->df_dev.p, 0, ntok * 4, c->stream));
+        DfParams dp{};
+        dp.terms = k.s_terms.at(din);
+        dp.tokens = k.s_tokens.at(din);
+        dp.n_tokens = (uint32_t)ntok; dp.n_tiles = n_tiles; dp.seg = c->seg.as<uint32_t>();
+        dp.row_ok_bits = k.row_ok; dp.df = c->df_dev.as<unsigned int>();
+        if (k.per_q) { dp.tok_ok_slot = k.s_tslot.at(din); dp.ok_words = ok_words; }
+        if (n_tiles && ntok) {
+            bm25_df_kernel<<<(unsigned)(uint64_t(n_tiles) * ntok), BM25_THREADS, 0, c->stream>>>(dp);
             launched(c);
         }
-        PinScoreParams sp{};
-        sp.n_queries = B; sp.stride = top; sp.doc = c->srt_doc.as<uint64_t>(); sp.cnt = c->srt_n.as<uint32_t>();
-        sp.has_ft = has_ft; sp.hybrid = has_ft && has_v;
-        sp.ft = c->srt_ft.as<float>(); sp.ft_present = c->srt_ftp.as<uint8_t>();
-        sp.gmin = fp.out_gmin; sp.den = fp.out_den;
-        sp.v_doc = fp.out_vdoc; sp.v_score = fp.out_vscore; sp.v_n = fp.out_vn; sp.v_stride = vs;
-        sp.omc_doc = fp.omc_doc; sp.omc_mult = fp.omc_mult; sp.n_omc = n_omc;
-        sp.out_score = c->srt_score.as<float>(); sp.out_present = c->srt_present.as<uint8_t>();
-        pin_score_kernel<<<warp_grid, 256, 0, c->stream>>>(sp);
+        if (k.multi_rank) {   // corpus df = sum of the shards' counts (disjoint documents)
+            std::string err;
+            if (!c->comm.all_reduce_sum_u32(c->df_dev.p, c->df_dev.p, ntok, c->stream, &err)) return fail(OC_ERR_COMM, "%s", err.c_str());
+        }
+        std::vector<uint32_t> dfh(ntok);
+        CU(cudaMemcpyAsync(dfh.data(), c->df_dev.p, ntok * 4, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        const float N = (float)S->document_count;
+        for (size_t t = 0; t < ntok; t++)
+            if (k.tok_need_df[t]) k.tokens[t].idf = host_idf(N, std::max<uint32_t>(1u, dfh[t]));
+        CU(cudaMemcpyAsync(const_cast<TokenDesc *>(k.s_tokens.at(din)), k.tokens.data(), ntok * sizeof(TokenDesc),
+                           cudaMemcpyHostToDevice, c->stream));
+    }
+    const size_t slots = size_t(B) * std::max<uint32_t>(n_tiles, 1);
+    OCTRY(c->tau.ensure(size_t(B) * 16 + 16));   // [tau B x 8][min_hint B x 8][work counter]: one memset
+    OCTRY(c->cand_key.ensure(slots * n_keep * 8));
+    OCTRY(c->cand_ft.ensure(slots * n_keep * 4));
+    OCTRY(c->cand_cnt.ensure(slots * 4));
+    OCTRY(c->tile_cnt.ensure(slots * 4));
+    OCTRY(c->tile_max.ensure(slots * 4));
+    OCTRY(c->tile_min.ensure(slots * 4));
+    k.min_hint_dev = reinterpret_cast<float *>(c->tau.as<uint8_t>() + size_t(B) * 8);
+    k.tile_counter = reinterpret_cast<unsigned int *>(c->tau.as<uint8_t>() + size_t(B) * 16);
+    CU(cudaMemsetAsync(c->tau.p, 0, size_t(B) * 16 + 16, ps));
+    Bm25Params &bp = k.bp;
+    bp.terms = k.s_terms.at(din);
+    bp.tokens = k.s_tokens.at(din);
+    bp.queries = k.s_queries.at(din);
+    bp.term_token = k.s_ttok.at(din);
+    bp.seg = c->seg.as<uint32_t>();
+    bp.n_queries = B; bp.n_tiles = n_tiles; bp.n_rows = S->n_rows;
+    bp.k = p->bm25_k; bp.b = p->bm25_b;
+    bp.row_ok_bits = k.row_ok;
+    if (k.per_q) { bp.q_ok_slot = k.qfj.d_q_slot_ft; bp.ok_words = ok_words; }
+    bp.omc_row = k.s_omcr.at(din);
+    bp.omc_mult = k.s_omcrm.at(din);
+    bp.n_omc = (uint32_t)k.omc_rows.size();
+    bp.v_row = nullptr;            // the hybrid lookups are point lookups (bm25_point_kernel)
+    bp.v_stride = k.vlimit;
+    bp.v_ft = nullptr; bp.v_present = nullptr;
+    bp.min_hint = k.min_hint_dev;
+    bp.n_keep = n_keep; bp.cap = k.cap;
+    bp.tau = c->tau.as<unsigned long long>();
+    bp.cand_key = c->cand_key.as<uint64_t>(); bp.cand_ft = c->cand_ft.as<float>();
+    bp.cand_cnt = c->cand_cnt.as<uint32_t>(); bp.tile_count = c->tile_cnt.as<uint32_t>();
+    bp.tile_max = c->tile_max.as<float>(); bp.tile_min = c->tile_min.as<float>();
+    bp.tile_first = 0;
+    if (!k.q_perm.empty()) {
+        bp.perm = k.s_perm.at(din);
+        uint32_t off = 0, q0 = 0;
+        for (uint32_t g = 0; g < BM25_CLASSES; g++) {
+            bp.cls_off[g] = off; bp.cls_nq[g] = k.cls_nq[g]; bp.cls_q0[g] = q0;
+            off += k.cls_nq[g] * n_tiles; q0 += k.cls_nq[g];
+        }
+    }
+    const SearchReq &r = k.r;
+    if (r.fj || r.gj || r.sj) {   // facets / groups / sortBy: the tile kernels also emit the bitmap of matched rows (every (query, tile) item writes its 256 words)
+        OCTRY(c->mbits.ensure(size_t(B) * std::max<uint32_t>(n_tiles, 1) * (BM25_TILE / 32) * 4));
+        bp.matched_bits = c->mbits.as<uint32_t>();
+    }
+    if (r.gj && n_tiles) {   // groups: and the raw score of each matched row
+        OCTRY(c->row_ft.ensure(size_t(B) * n_tiles * BM25_TILE * 4));
+        bp.row_ft = c->row_ft.as<float>();
+    }
+    if (n_tiles) OCTRY(launch_tile(c, bp, n_tiles * B, k.any_multi, k.thr, k.omc_tile, ps, k.max_tokens, k.tile_counter, k.need_df));
+    CU(cudaEventRecord(c->ev[EV_BM1], ps));
+    c->timing.bm25_postings = k.postings_walked;
+    if (k.side) {   // join: the lookups and the fusion need the vector hits (main stream) and the tiles (side stream)
+        CU(cudaEventRecord(c->ev_side, c->side));
+        CU(cudaStreamWaitEvent(c->stream, c->ev_side, 0));
+        c->side_dirty = false;
+    }
+    return OC_OK;
+}
+
+// The fulltext scores of n_slots string rows ([B][stride], RANK_NONE: none), by point lookups into the postings.
+static void point_lookup(SearchCall &k, const uint32_t *rows, uint32_t stride, float *out_ft, uint8_t *out_present, uint64_t n_slots) {
+    PointParams pp{};
+    pp.terms = k.bp.terms; pp.tokens = k.bp.tokens; pp.queries = k.bp.queries;
+    pp.n_queries = k.B; pp.v_stride = stride; pp.v_row = rows; pp.row_ok_bits = k.row_ok;
+    pp.q_ok_slot = k.per_q ? k.qfj.d_q_slot_ft : nullptr; pp.ok_words = uint64_t(k.n_tiles) * (BM25_TILE / 32);
+    pp.k = k.p->bm25_k; pp.threshold = k.thr ? 1 : 0;
+    pp.v_ft = out_ft; pp.v_present = out_present;
+    bm25_point_kernel<<<(unsigned)((n_slots * 32 + 255) / 256), 256, 0, k.c->stream>>>(pp);
+    launched(k.c);
+}
+
+// The score-map values of [B][stride] documents (cnt[q] per query), from K4's exports and their fulltext scores.
+static void pin_scores(SearchCall &k, uint32_t stride, const uint64_t *doc, const uint32_t *cnt, const float *ft,
+                       const uint8_t *ft_present, float *out_score, uint8_t *out_present) {
+    const FuseParams &fp = k.fp;
+    PinScoreParams sp{};
+    sp.n_queries = k.B; sp.stride = stride; sp.doc = doc; sp.cnt = cnt;
+    sp.has_ft = k.has_ft; sp.hybrid = k.has_ft && k.has_v;
+    sp.ft = ft; sp.ft_present = ft_present;
+    sp.gmin = fp.out_gmin; sp.den = fp.out_den;
+    sp.v_doc = fp.out_vdoc; sp.v_score = fp.out_vscore; sp.v_n = fp.out_vn; sp.v_stride = std::max<uint32_t>(k.vlimit, 1);
+    sp.omc_doc = fp.omc_doc; sp.omc_mult = fp.omc_mult; sp.n_omc = k.n_omc;
+    sp.out_score = out_score; sp.out_present = out_present;
+    pin_score_kernel<<<(unsigned)((uint64_t(k.B) * stride * 32 + 255) / 256), 256, 0, k.c->stream>>>(sp);
+    launched(k.c);
+}
+
+// pins, after K4: the score-map value of every promoted document, then (pin_flat) the splice into K4's top list
+static int pin_tail(SearchCall &k) {
+    if (!k.pin_items) return OC_OK;
+    oc_ctx *c = k.c; const PinJob *pj = k.r.pj;
+    const uint32_t B = k.B, ps = pj->stride;
+    const uint64_t nslot = uint64_t(B) * ps;
+    OCTRY(c->pin_score.ensure(nslot * 4));
+    OCTRY(c->pin_present.ensure(nslot));
+    if (k.has_ft) {   // the promoted documents' string rows and their fulltext scores (the hybrid lookups' kernels)
+        OCTRY(c->pin_row.ensure(nslot * 4));
+        OCTRY(c->pin_ft.ensure(nslot * 4));
+        OCTRY(c->pin_ftp.ensure(nslot));
+        map_docs_to_rows_kernel<<<(unsigned)((nslot + 255) / 256), 256, 0, c->stream>>>(
+            pj->d_doc, pj->d_cnt, ps, B, k.S->row_doc, k.S->n_rows, c->pin_row.as<uint32_t>());
         launched(c);
+        point_lookup(k, c->pin_row.as<uint32_t>(), ps, c->pin_ft.as<float>(), c->pin_ftp.as<uint8_t>(), nslot);
+    }
+    pin_scores(k, ps, pj->d_doc, pj->d_cnt, c->pin_ft.as<float>(), c->pin_ftp.as<uint8_t>(), c->pin_score.as<float>(),
+               c->pin_present.as<uint8_t>());
+    if (k.pin_flat) {
         PinSpliceParams xp{};
-        if (pj->splice) {
-            xp.stride = pj->stride; xp.kp2 = std::max<uint32_t>(32, next_pow2(pj->stride));
-            xp.doc = pj->d_doc; xp.pos = pj->d_pos; xp.score = c->pin_score.as<float>(); xp.cnt = pj->d_cnt;
-        } else {   // no item anywhere: every query takes the page of its list as it is
-            OCTRY(c->srt_zero.ensure(size_t(B) * 4));
-            CU(cudaMemsetAsync(c->srt_zero.p, 0, size_t(B) * 4, c->stream));
-            xp.stride = 0; xp.kp2 = 32;
-            xp.doc = c->srt_doc.as<uint64_t>(); xp.pos = c->srt_zero.as<uint32_t>(); xp.score = c->srt_score.as<float>();
-            xp.cnt = c->srt_zero.as<uint32_t>();
-        }
-        xp.n_top = top; xp.limit = limit; xp.offset = p->offset;
-        xp.top_doc = c->srt_doc.as<uint64_t>(); xp.top_score = c->srt_score.as<float>(); xp.top_n = c->srt_n.as<uint32_t>();
-        xp.out_doc = reinterpret_cast<uint64_t *>(dout + o_doc); xp.out_score = reinterpret_cast<float *>(dout + o_sc);
-        xp.out_n = reinterpret_cast<uint32_t *>(dout + o_n);
-        if (sj->by_score) {   // the queries in score order splice K4's top n_keep
-            xp.q_alt = din + o_salt; xp.alt_n_top = n_keep;
-            xp.alt_doc = c->pin_top_doc.as<uint64_t>(); xp.alt_score = c->pin_top_score.as<float>(); xp.alt_n = c->pin_top_n.as<uint32_t>();
-        }
-        pin_splice_kernel<<<B, PIN_THREADS, pin_splice_smem(xp.kp2, sj->by_score ? std::max(top, n_keep) : top, limit + p->offset),
-                            c->stream>>>(xp);
+        xp.stride = ps; xp.kp2 = std::max<uint32_t>(32, next_pow2(ps));
+        xp.doc = pj->d_doc; xp.pos = pj->d_pos; xp.score = c->pin_score.as<float>(); xp.cnt = pj->d_cnt;
+        xp.n_top = k.n_keep; xp.limit = k.limit; xp.offset = k.p->offset;
+        xp.top_doc = c->pin_top_doc.as<uint64_t>(); xp.top_score = c->pin_top_score.as<float>(); xp.top_n = c->pin_top_n.as<uint32_t>();
+        xp.out_doc = k.d_doc; xp.out_score = k.d_score; xp.out_n = k.d_n;
+        const size_t smem = pin_splice_smem(xp.kp2, k.n_keep, k.limit + k.p->offset);
+        pin_splice_kernel<<<B, PIN_THREADS, smem, c->stream>>>(xp);
         launched(c);
-        CU(cudaGetLastError());
-        return OC_OK;
-    };
+    }
+    CU(cudaGetLastError());
+    return OC_OK;
+}
 
-    auto device_tail = [&]() -> int {
+// sortBy, after K4 and the pins' scores: the first sort_top keys in field order, scored like promoted documents,
+// then paged with the pins spliced (pin_splice_kernel writes the hits over K4's)
+static int sort_tail(SearchCall &k) {
+    if (!k.sort_flat) return OC_OK;
+    oc_ctx *c = k.c; const SortJob *sj = k.r.sj;
+    const PinJob *pj = k.r.pj;
+    const uint32_t B = k.B, n_tiles = k.n_tiles, n_keep = k.n_keep, limit = k.limit, offset = k.p->offset;
+    const DevBuf &din = c->in_blob;
+    if (k.has_ft && n_tiles > 0)
+        for (uint32_t e = 0; e < sj->f.size(); e++) OCTRY(sort_rows_for(c, sj->ord(e), k.snap));
+    const uint32_t top = k.sort_top;
+    const uint64_t nslot = uint64_t(B) * top;
+    const uint32_t vs = std::max<uint32_t>(k.vlimit, 1);
+    OCTRY(c->srt_doc.ensure(nslot * 8));
+    OCTRY(c->srt_row.ensure(nslot * 4));
+    OCTRY(c->srt_n.ensure(size_t(B) * 4));
+    OCTRY(c->srt_score.ensure(nslot * 4));
+    OCTRY(c->srt_present.ensure(nslot));
+    SortWalkParams wp{};
+    wp.ents = k.s_sent.at(din); wp.q = k.s_sq.at(din);
+    wp.mbits = k.has_ft && n_tiles > 0 ? c->mbits.as<uint32_t>() : nullptr; wp.row_words = uint64_t(n_tiles) * (BM25_TILE / 32);
+    wp.v_doc = k.fp.out_vdoc; wp.v_n = k.fp.out_vn; wp.v_stride = vs;
+    wp.top = top;
+    wp.out_doc = c->srt_doc.as<uint64_t>(); wp.out_row = c->srt_row.as<uint32_t>(); wp.out_n = c->srt_n.as<uint32_t>();
+    sort_walk_kernel<<<B, SORT_THREADS, size_t(vs) * 4, c->stream>>>(wp);
+    launched(c);
+    if (k.has_ft) {   // the selected rows' fulltext scores (RANK_NONE rows: vector hits without a row, empty slots)
+        OCTRY(c->srt_ft.ensure(nslot * 4));
+        OCTRY(c->srt_ftp.ensure(nslot));
+        point_lookup(k, c->srt_row.as<uint32_t>(), top, c->srt_ft.as<float>(), c->srt_ftp.as<uint8_t>(), nslot);
+    }
+    pin_scores(k, top, c->srt_doc.as<uint64_t>(), c->srt_n.as<uint32_t>(), c->srt_ft.as<float>(), c->srt_ftp.as<uint8_t>(),
+               c->srt_score.as<float>(), c->srt_present.as<uint8_t>());
+    PinSpliceParams xp{};
+    if (pj->splice) {
+        xp.stride = pj->stride; xp.kp2 = std::max<uint32_t>(32, next_pow2(pj->stride));
+        xp.doc = pj->d_doc; xp.pos = pj->d_pos; xp.score = c->pin_score.as<float>(); xp.cnt = pj->d_cnt;
+    } else {   // no item anywhere: every query takes the page of its list as it is
+        OCTRY(c->srt_zero.ensure(size_t(B) * 4));
+        CU(cudaMemsetAsync(c->srt_zero.p, 0, size_t(B) * 4, c->stream));
+        xp.stride = 0; xp.kp2 = 32;
+        xp.doc = c->srt_doc.as<uint64_t>(); xp.pos = c->srt_zero.as<uint32_t>(); xp.score = c->srt_score.as<float>();
+        xp.cnt = c->srt_zero.as<uint32_t>();
+    }
+    xp.n_top = top; xp.limit = limit; xp.offset = offset;
+    xp.top_doc = c->srt_doc.as<uint64_t>(); xp.top_score = c->srt_score.as<float>(); xp.top_n = c->srt_n.as<uint32_t>();
+    xp.out_doc = k.d_doc; xp.out_score = k.d_score; xp.out_n = k.d_n;
+    if (sj->by_score) {   // the queries in score order splice K4's top n_keep
+        xp.q_alt = k.s_salt.at(din); xp.alt_n_top = n_keep;
+        xp.alt_doc = c->pin_top_doc.as<uint64_t>(); xp.alt_score = c->pin_top_score.as<float>(); xp.alt_n = c->pin_top_n.as<uint32_t>();
+    }
+    pin_splice_kernel<<<B, PIN_THREADS, pin_splice_smem(xp.kp2, sj->by_score ? std::max(top, n_keep) : top, limit + offset),
+                        c->stream>>>(xp);
+    launched(c);
+    CU(cudaGetLastError());
+    return OC_OK;
+}
+
+// K4 (fusion + top-n), then the pins and the sortBy walk that read its exports
+static int fuse_and_tails(SearchCall &k) {
+    void (*fuse)(const FuseParams) = k.exports ? fuse_topk_kernel<true> : fuse_topk_kernel<false>;
+    fuse<<<k.B, 256, k.fuse_smem, k.c->stream>>>(k.fp);
+    launched(k.c);
+    CU(cudaGetLastError());
+    OCTRY(pin_tail(k));
+    return sort_tail(k);
+}
+
+// The hybrid lookups, the fusion and what follows it (+ the shard exchange).  Re-runnable.
+static int device_tail(SearchCall &k) {
+    oc_ctx *c = k.c; const oc_search_params *p = k.p;
+    const uint32_t B = k.B, vlimit = k.vlimit, n_keep = k.n_keep; const bool has_ft = k.has_ft, has_v = k.has_v;
+    const StrSnap *S = k.S;
     if (has_ft && has_v) {
         // hybrid: vector hits -> string rows -> their fulltext scores (point lookups)
         OCTRY(c->v_srow.ensure(size_t(B) * vlimit * 4));
         OCTRY(c->v_ft.ensure(size_t(B) * vlimit * 4));
         OCTRY(c->v_present.ensure(size_t(B) * vlimit));
         if (vlimit) {
-        map_docs_to_rows_kernel<<<(B * vlimit + 255) / 256, 256, 0, c->stream>>>(
-            c->v_doc.as<uint64_t>(), c->v_cnt.as<uint32_t>(), vlimit, B, S->row_doc, S->n_rows, c->v_srow.as<uint32_t>());
-        launched(c);
-        PointParams pp{};
-        pp.terms = bp.terms; pp.tokens = bp.tokens; pp.queries = bp.queries;
-        pp.n_queries = B; pp.v_stride = vlimit; pp.v_row = c->v_srow.as<uint32_t>(); pp.row_ok_bits = row_ok;
-        pp.q_ok_slot = per_q ? qfj.d_q_slot_ft : nullptr; pp.ok_words = uint64_t(n_tiles) * (BM25_TILE / 32);
-        pp.k = p->bm25_k; pp.threshold = thr ? 1 : 0;
-        pp.v_ft = c->v_ft.as<float>(); pp.v_present = c->v_present.as<uint8_t>();
-        bm25_point_kernel<<<(B * vlimit * 32 + 255) / 256, 256, 0, c->stream>>>(pp);
-        launched(c);
-        CU(cudaGetLastError());
+            map_docs_to_rows_kernel<<<(B * vlimit + 255) / 256, 256, 0, c->stream>>>(
+                c->v_doc.as<uint64_t>(), c->v_cnt.as<uint32_t>(), vlimit, B, S->row_doc, S->n_rows, c->v_srow.as<uint32_t>());
+            launched(c);
+            point_lookup(k, c->v_srow.as<uint32_t>(), vlimit, c->v_ft.as<float>(), c->v_present.as<uint8_t>(), uint64_t(B) * vlimit);
+            CU(cudaGetLastError());
         }
     }
-
-    // ------------------------------------------------------------ fusion + top-n (+ shard exchange)
+    FuseParams &fp = k.fp;
     fp = FuseParams{};
-    fp.mode = p->mode; fp.n_tiles = n_tiles; fp.n_keep = n_keep; fp.limit = limit; fp.offset = p->offset;
+    fp.mode = p->mode; fp.n_tiles = k.n_tiles; fp.n_keep = n_keep; fp.limit = k.limit; fp.offset = p->offset;
     {   // smallest power-of-two key buffer that takes the candidates in one round (sort cost ~ capb log^2 capb)
-        const uint64_t total = (has_ft ? uint64_t(n_tiles) * n_keep : 0) + (has_v ? vlimit : 0);
+        const uint64_t total = (has_ft ? uint64_t(k.n_tiles) * n_keep : 0) + (has_v ? vlimit : 0);
         // up to 16 K keys (128 KB) stay in shared memory and go through one radix select; the streaming bitonic path behind
         // it is for larger candidate sets (the 10M-document fulltext workload has 1221 tiles x 10 candidate slots per query)
         fp.capb = next_pow2((uint32_t)std::min<uint64_t>(16384, std::max<uint64_t>(total, 2 * n_keep)));
         fp.capb = std::max<uint32_t>(fp.capb, std::max<uint32_t>(64, next_pow2(2 * n_keep)));
     }
     if (has_ft) {
+        const Bm25Params &bp = k.bp;
         fp.cand_key = bp.cand_key; fp.cand_ft = bp.cand_ft; fp.cand_cnt = bp.cand_cnt; fp.tile_count = bp.tile_count;
         fp.tile_max = bp.tile_max; fp.tile_min = bp.tile_min; fp.str_row_doc_ids = S->row_doc;
     }
@@ -2719,20 +2843,20 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         fp.v_ft = c->v_ft.as<float>(); fp.v_present = c->v_present.as<uint8_t>();
     }
     fp.v_stride = vlimit;
-    fp.omc_doc = n_omc ? reinterpret_cast<const uint64_t *>(din + o_omcd) : nullptr;
-    fp.omc_mult = n_omc ? reinterpret_cast<const float *>(din + o_omcm) : nullptr;
-    fp.n_omc = n_omc;
-    fp.out_doc = reinterpret_cast<uint64_t *>(dout + o_doc); fp.out_score = reinterpret_cast<float *>(dout + o_sc);
-    fp.out_n = reinterpret_cast<uint32_t *>(dout + o_n); fp.out_count = reinterpret_cast<unsigned long long *>(dout + o_cnt);
-    fp.out_min = reinterpret_cast<float *>(dout + o_min);
-    if (k4_top) {   // K4 keeps its whole top n_keep for the splice, which writes the hits
+    fp.omc_doc = k.s_omcd.at(c->in_blob);
+    fp.omc_mult = k.s_omcm.at(c->in_blob);
+    fp.n_omc = k.n_omc;
+    fp.out_doc = k.d_doc; fp.out_score = k.d_score; fp.out_n = k.d_n;
+    fp.out_count = reinterpret_cast<unsigned long long *>(k.dout + k.o_cnt);
+    fp.out_min = reinterpret_cast<float *>(k.dout + k.o_min);
+    if (k.k4_top) {   // K4 keeps its whole top n_keep for the splice, which writes the hits
         fp.limit = n_keep; fp.offset = 0;
         OCTRY(c->pin_top_doc.ensure(size_t(B) * n_keep * 8));
         OCTRY(c->pin_top_score.ensure(size_t(B) * n_keep * 4));
         OCTRY(c->pin_top_n.ensure(size_t(B) * 4));
         fp.out_doc = c->pin_top_doc.as<uint64_t>(); fp.out_score = c->pin_top_score.as<float>(); fp.out_n = c->pin_top_n.as<uint32_t>();
     }
-    if (exports) {   // groups / pins: K4 also exports the normalisation and the vector part of the score map
+    if (k.exports) {   // groups / pins: K4 also exports the normalisation and the vector part of the score map
         const uint32_t vs = std::max<uint32_t>(vlimit, 1);
         OCTRY(c->grp_vdoc.ensure(size_t(B) * vs * 8));
         OCTRY(c->grp_vscore.ensure(size_t(B) * vs * 4));
@@ -2742,36 +2866,32 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         fp.out_vdoc = c->grp_vdoc.as<uint64_t>(); fp.out_vscore = c->grp_vscore.as<float>(); fp.out_vn = c->grp_vn.as<uint32_t>();
         fp.out_gmin = c->grp_gmin.as<float>(); fp.out_den = c->grp_den.as<float>();
     }
-    fuse_smem = size_t(fp.capb) * 8 + size_t(std::max<uint32_t>(32, next_pow2(n_keep))) * 8 + size_t(vlimit) * 16 + 64;
-    if (smem_cfg_needed(c->device, exports ? (const void *)fuse_topk_kernel<true> : (const void *)fuse_topk_kernel<false>, fuse_smem))
-        CU(cudaFuncSetAttribute(exports ? (const void *)fuse_topk_kernel<true> : (const void *)fuse_topk_kernel<false>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fuse_smem));
-
+    k.fuse_smem = size_t(fp.capb) * 8 + size_t(std::max<uint32_t>(32, next_pow2(n_keep))) * 8 + size_t(vlimit) * 16 + 64;
+    const void *fuse = k.exports ? (const void *)fuse_topk_kernel<true> : (const void *)fuse_topk_kernel<false>;
+    if (smem_cfg_needed(c->device, fuse, k.fuse_smem))
+        CU(cudaFuncSetAttribute(fuse, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k.fuse_smem));
+    CU(cudaEventRecord(c->ev[EV_FUSE0], c->stream));
     if (p->sharded && c->comm.world > 1) {
-        CU(cudaEventRecord(c->ev[EV_FUSE0], c->stream));
-        OCTRY(run_sharded_merge(c, p, fp, has_ft ? (uint32_t)S->n_rows : 0, has_v ? (uint32_t)emb->n_rows : 0, B,
-                                (has_v && c->gemm_pending) ? c->g_flag.as<uint8_t>() : nullptr, dout + o_gflag));
-        CU(cudaEventRecord(c->ev[EV_FUSE1], c->stream));
-        did_comm = true;
+        OCTRY(run_sharded_merge(c, p, fp, has_ft ? (uint32_t)S->n_rows : 0, has_v ? (uint32_t)k.emb->n_rows : 0, B,
+                                (has_v && c->gemm_pending) ? c->g_flag.as<uint8_t>() : nullptr, k.dout + k.o_gflag));
+        k.did_comm = true;
     } else {
-        CU(cudaEventRecord(c->ev[EV_FUSE0], c->stream));
-        if (exports) fuse_topk_kernel<true><<<B, 256, fuse_smem, c->stream>>>(fp);
-        else fuse_topk_kernel<<<B, 256, fuse_smem, c->stream>>>(fp);
-        launched(c);
-        CU(cudaGetLastError());
-        OCTRY(pin_tail());
-        OCTRY(sort_tail());
-        CU(cudaEventRecord(c->ev[EV_FUSE1], c->stream));
+        OCTRY(fuse_and_tails(k));
     }
+    CU(cudaEventRecord(c->ev[EV_FUSE1], c->stream));
     return OC_OK;
-    };   // device_tail
-    OCTRY(device_tail());
+}
+
+// The results (and the tensor-core scan's overflow flags) to the host, then the re-runs they ask for: the tensor-core
+// scan's overflowed queries, and the hybrid rank proxy.
+static int rerun_checks(SearchCall &k) {
+    oc_ctx *c = k.c; const oc_search_params *p = k.p;
+    const uint32_t B = k.B; uint8_t *h = c->h_out.as<uint8_t>();
     CU(cudaEventRecord(c->ev[EV_DEV], c->stream));
-    uint8_t *h = c->h_out.as<uint8_t>();
-    CU(cudaMemcpyAsync(h, dout, out_bytes, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaMemcpyAsync(h, k.dout, k.out_bytes, cudaMemcpyDeviceToHost, c->stream));
     if (c->gemm_pending) {
-        CU(cudaMemcpyAsync(h + out_bytes, c->g_flag.p, B, cudaMemcpyDeviceToHost, c->stream));
-        CU(cudaMemcpyAsync(h + o_resc, c->g_resc.p, size_t(B) * 4, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaMemcpyAsync(h + k.out_bytes, c->g_flag.p, k.B, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaMemcpyAsync(h + k.o_resc, c->g_resc.p, size_t(k.B) * 4, cudaMemcpyDeviceToHost, c->stream));
     }
     CU(cudaEventRecord(c->ev[EV_D2H], c->stream));
     CU(cudaStreamSynchronize(c->stream));
@@ -2780,93 +2900,101 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
         // taken on the flags all ranks exchanged inside the shard records (no host sync before the collective),
         // by every rank — also one whose own shard was served by the exact sweep
         bool rerun = false;
-        if (did_comm && has_v) for (uint32_t q = 0; q < B; q++) rerun = rerun || h[o_gflag + q] != 0;
+        if (k.did_comm && k.has_v) for (uint32_t q = 0; q < B; q++) rerun = rerun || h[k.o_gflag + q] != 0;
         uint32_t redone = 0;
         if (c->gemm_pending || rerun) CU(cudaEventRecord(c->ev[EV_RR0], c->stream));
         if (c->gemm_pending) {
             uint64_t resc = 0;
-            for (uint32_t q = 0; q < B; q++) resc += reinterpret_cast<const uint32_t *>(h + o_resc)[q];
+            for (uint32_t q = 0; q < B; q++) resc += reinterpret_cast<const uint32_t *>(h + k.o_resc)[q];
             c->timing.scan_rescored = (uint32_t)(resc / B);
-            OCTRY(fix_unproven(c, emb, h + out_bytes, B, vlimit, p->similarity, &redone));
+            OCTRY(fix_unproven(c, k.emb, h + k.out_bytes, B, k.vlimit, p->similarity, &redone));
         }
         if (redone || rerun) {
             c->gemm_pending = false;
-            OCTRY(device_tail());
-            CU(cudaMemcpyAsync(h, dout, out_bytes, cudaMemcpyDeviceToHost, c->stream));
+            OCTRY(device_tail(k));
+            CU(cudaMemcpyAsync(h, k.dout, k.out_bytes, cudaMemcpyDeviceToHost, c->stream));
             CU(cudaEventRecord(c->ev[EV_RR1], c->stream));
             c->rerun_timed = true;
             CU(cudaStreamSynchronize(c->stream));
         }
     }
-
     // rank-proxy validation: with OMC multipliers the tile ranking assumed min == min_hint (0);
     // a negative global min changes the order of (ft - min) * omc -> rerun with the real min.
-    if (!did_comm && p->mode == OC_MODE_HYBRID && omc_tile && n_tiles) {
-        const float *mins = reinterpret_cast<const float *>(h + o_min);
+    // The hybrid point lookups do not depend on the tiles: they are not redone.
+    if (!k.did_comm && p->mode == OC_MODE_HYBRID && k.omc_tile && k.n_tiles) {
+        const float *mins = reinterpret_cast<const float *>(h + k.o_min);
         bool redo = false;
         for (uint32_t q = 0; q < B; q++) redo = redo || mins[q] < 0.f;
         if (redo) {
-            CU(cudaMemcpyAsync(min_hint_dev, mins, size_t(B) * 4, cudaMemcpyHostToDevice, c->stream));
+            CU(cudaMemcpyAsync(k.min_hint_dev, mins, size_t(B) * 4, cudaMemcpyHostToDevice, c->stream));
             CU(cudaMemsetAsync(c->tau.p, 0, size_t(B) * 8, c->stream));
-            CU(cudaMemsetAsync(tile_counter, 0, 8, c->stream));
-            OCTRY(launch_tile(c, bp, n_tiles * B, any_multi, thr, omc_tile, c->stream, max_tokens, tile_counter, need_df));
-            if (exports) fuse_topk_kernel<true><<<B, 256, fuse_smem, c->stream>>>(fp);
-            else fuse_topk_kernel<<<B, 256, fuse_smem, c->stream>>>(fp);
-            launched(c);
-            OCTRY(pin_tail());
-            OCTRY(sort_tail());
-            CU(cudaMemcpyAsync(c->h_out.p, dout, out_bytes, cudaMemcpyDeviceToHost, c->stream));
+            CU(cudaMemsetAsync(k.tile_counter, 0, 8, c->stream));
+            OCTRY(launch_tile(c, k.bp, k.n_tiles * B, k.any_multi, k.thr, k.omc_tile, c->stream, k.max_tokens, k.tile_counter, k.need_df));
+            OCTRY(fuse_and_tails(k));
+            CU(cudaMemcpyAsync(h, k.dout, k.out_bytes, cudaMemcpyDeviceToHost, c->stream));
             CU(cudaStreamSynchronize(c->stream));
         }
     }
-    if (facets) OCTRY(run_facets(c, *fj, fpl, B, has_ft, has_v, S, n_tiles, vlimit));
+    return OC_OK;
+}
+
+// the value a listed document was placed by: its sort value, NaN in score order
+static double value_of(const SearchCall &k, uint32_t q, uint64_t d) {
+    return k.r.sj ? sort_value_of(*k.r.sj, k.r.pj, q, d) : std::numeric_limits<double>::quiet_NaN();
+}
+
+// Facets and groups (on the final score map), then every output to the caller, and the call's timing.
+static int copy_out(SearchCall &k) {
+    oc_ctx *c = k.c; const SearchReq &r = k.r;
+    const PinJob *pj = r.pj; GroupJob *gj = r.gj;
+    const uint32_t B = k.B, limit = k.limit; const uint8_t *h = c->h_out.as<uint8_t>();
+    if (k.facets) OCTRY(run_facets(c, *r.fj, k.fpl, B, k.has_ft, k.has_v, k.S, k.n_tiles, k.vlimit));
     if (gj) {
         CU(cudaEventRecord(c->ev[EV_GRP0], c->stream));
-        OCTRY(run_groups(c, *gj, p->mode, S, n_tiles, vlimit, fp.omc_doc, fp.omc_mult, n_omc, *pj));
+        OCTRY(run_groups(c, *gj, k.p->mode, k.S, k.n_tiles, k.vlimit, k.fp.omc_doc, k.fp.omc_mult, k.n_omc, *pj));
         CU(cudaEventRecord(c->ev[EV_GRP1], c->stream));
         CU(cudaStreamSynchronize(c->stream));
     }
     std::vector<float> pin_sc;
     std::vector<uint8_t> pin_pr;
-    if (pin_items && (out_pin_scores || out_pin_present)) {
+    if (k.pin_items && (pj->out_scores || pj->out_present)) {
         pin_sc.resize(pj->doc.size());
         pin_pr.resize(pj->doc.size());
         CU(cudaMemcpyAsync(pin_sc.data(), c->pin_score.p, pin_sc.size() * 4, cudaMemcpyDeviceToHost, c->stream));
         CU(cudaMemcpyAsync(pin_pr.data(), c->pin_present.p, pin_pr.size(), cudaMemcpyDeviceToHost, c->stream));
         CU(cudaStreamSynchronize(c->stream));
     }
-    c->timing.d2h_bytes = out_bytes;
-    if (write_hits) {
-        memcpy(out_doc_ids, h + o_doc, size_t(B) * limit * 8);
-        memcpy(out_scores, h + o_sc, size_t(B) * limit * 4);
-        memcpy(out_n, h + o_n, size_t(B) * 4);
+    c->timing.d2h_bytes = k.out_bytes;
+    if (k.write_hits) {
+        memcpy(r.out_doc_ids, h, size_t(B) * limit * 8);
+        memcpy(r.out_scores, h + k.o_sc, size_t(B) * limit * 4);
+        memcpy(r.out_n, h + k.o_n, size_t(B) * 4);
     }
-    memcpy(out_count, h + o_cnt, size_t(B) * 8);
-    if (sort_flat && sj->out_values)
+    memcpy(r.out_count, h + k.o_cnt, size_t(B) * 8);
+    if (k.write_hits && r.out_sort_values)
         for (uint32_t q = 0; q < B; q++)
             for (uint32_t i = 0; i < limit; i++) {
                 const size_t o = size_t(q) * limit + i;
-                sj->out_values[o] = i < out_n[q] ? sort_value_of(*sj, pj, q, out_doc_ids[o]) : 0.0;
+                r.out_sort_values[o] = i < r.out_n[q] ? value_of(k, q, r.out_doc_ids[o]) : 0.0;
             }
-    if (gj && gj->out_values)   // run_groups' copies are complete (synchronised above); score order: NaN
+    if (gj && gj->out_values)   // run_groups' copies are complete (synchronised above)
         for (uint32_t q = 0; q < B; q++) {
             if (gj->q_h[q] == GROUP_NONE) continue;
             const uint32_t G = gj->h[gj->q_h[q]]->n_groups;
-            for (size_t r = gj->q_row[q]; r < size_t(gj->q_row[q]) + G; r++)
+            for (size_t row = gj->q_row[q]; row < size_t(gj->q_row[q]) + G; row++)
                 for (uint32_t i = 0; i < gj->stride; i++) {
-                    const size_t o = r * gj->stride + i;
-                    gj->out_values[o] = i >= gj->out_n[r] ? 0.0 : sj ? sort_value_of(*sj, pj, q, gj->out_doc[o])
-                                                                     : std::numeric_limits<double>::quiet_NaN();
+                    const size_t o = row * gj->stride + i;
+                    gj->out_values[o] = i < gj->out_n[row] ? value_of(k, q, gj->out_doc[o]) : 0.0;
                 }
         }
     if (!pin_sc.empty())
         for (uint32_t q = 0; q < B; q++)
             for (uint32_t j = 0; j < pj->cnt[q]; j++) {
-                const size_t i = size_t(pins->q_pin_offsets[q]) + j, s = size_t(q) * pj->stride + j;
-                if (out_pin_scores) out_pin_scores[i] = pin_sc[s];
-                if (out_pin_present) out_pin_present[i] = pin_pr[s];
+                const size_t i = size_t(pj->pins->q_pin_offsets[q]) + j, s = size_t(q) * pj->stride + j;
+                if (pj->out_scores) pj->out_scores[i] = pin_sc[s];
+                if (pj->out_present) pj->out_present[i] = pin_pr[s];
             }
-    OCTRY(finish_timing(c, has_v && vlimit && emb->n_rows > 0, has_ft, true, did_comm));
+    OCTRY(finish_timing(c, k.has_v && k.vlimit && k.emb->n_rows > 0, k.has_ft, true, k.did_comm));
     if (gj) {   // the group stage is device work of this call too
         float ms = 0.f;
         CU(cudaEventElapsedTime(&ms, c->ev[EV_GRP0], c->ev[EV_GRP1]));
@@ -2875,9 +3003,35 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     return OC_OK;
 }
 
+static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const SearchReq &r) {
+    SearchCall k(c, emb, str, r);
+    OCTRY(search_check(k));
+    if (k.B == 0) return OC_OK;
+    // the published snapshot of the string store: grabbed once, immutable for the whole call (a commit may
+    // publish the next version meanwhile); taken before the lock so a last reference dies outside it
+    k.snap = str ? str_snapshot(str) : nullptr;
+    k.S = k.snap.get();
+    std::lock_guard<std::mutex> g(c->mu);
+    CU(cudaSetDevice(c->device));
+    // facets: the requests resolved to their distinct document slices (the work list goes up with the first upload)
+    if (k.facets) OCTRY(facet_plan(*r.fj, k.fpl));
+    begin_call(c);
+    OCTRY(vector_first(k));
+    OCTRY(ft_descriptors(k));
+    OCTRY(omc_plan(k));
+    sort_group_plan(k);
+    OCTRY(main_upload(k));
+    if (k.has_ft) OCTRY(bm25_stage(k));
+    OCTRY(device_tail(k));
+    OCTRY(rerun_checks(k));
+    return copy_out(k);
+}
+
 extern "C" int oc_search(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, uint64_t *out_doc_ids,
                          float *out_scores, uint32_t *out_n, uint64_t *out_count) {
-    return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr);
+    SearchReq r(p, out_doc_ids, out_scores, out_n, out_count);
+    r.q_filters_ok = true;
+    return search_impl(c, emb, str, r);
 }
 
 // ------------------------------------------------------------------------------------ facets
@@ -3188,7 +3342,10 @@ static int facets_unfiltered(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_searc
     std::vector<uint64_t> docs(size_t(B) * p->limit), cnt(B);
     std::vector<float> scores(size_t(B) * p->limit);
     std::vector<uint32_t> n(B);
-    return search_impl(c, emb, str, &q, docs.data(), scores.data(), n.data(), cnt.data(), &fj);
+    SearchReq r(&q, docs.data(), scores.data(), n.data(), cnt.data());
+    r.fj = &fj;
+    r.q_filters_ok = true;
+    return search_impl(c, emb, str, r);
 }
 
 extern "C" int oc_search_facets(oc_ctx *c, oc_emb *emb, oc_str *str, oc_facets *facets, const oc_search_params *p,
@@ -3428,11 +3585,10 @@ static int groups_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     const uint32_t B = p->n_queries;
     SortJob sj{};
     for (uint32_t b = 0; b < B; b++) OCTRY(sort_job_add(c, q[b].sort, sj));
-    sj.out_values = out_sort_values;
     PinJob pj;
-    pj.q_filters = per_query;
     OCTRY(pin_job_init(pins, B, pj));
     OCTRY(pins_check_flat(p, pj));
+    pj.out_scores = out_pin_scores; pj.out_present = out_pin_present;
     GroupJob gj;
     gj.q_h.assign(B, GROUP_NONE);
     gj.q_m.assign(B, 0);
@@ -3462,15 +3618,27 @@ static int groups_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     if (rows && (!out_group_n || (group_stride && (!out_group_doc_ids || !out_group_scores)))) return fail(OC_ERR_INVALID, "NULL group output");
     gj.rows = (uint32_t)rows; gj.stride = group_stride;
     gj.out_doc = out_group_doc_ids; gj.out_score = out_group_scores; gj.out_n = out_group_n; gj.out_values = out_group_sort_values;
-    // every query in score order: the flat hits are oc_search_pinned's (sort values NaN)
-    const SortJob *sjp = sj.f.empty() ? nullptr : &sj;
-    OCTRY(search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, fj, &gj, &pj, pins, out_pin_scores,
-                      out_pin_present, sjp));
-    if (!sjp && out_sort_values && p->limit > 0)
-        for (uint32_t b = 0; b < B; b++)
-            for (uint32_t i = 0; i < p->limit; i++)
-                out_sort_values[size_t(b) * p->limit + i] = i < out_n[b] ? std::numeric_limits<double>::quiet_NaN() : 0.0;
-    return OC_OK;
+    SearchReq r(p, out_doc_ids, out_scores, out_n, out_count);
+    r.out_sort_values = out_sort_values; r.fj = fj; r.gj = &gj; r.pj = &pj;
+    r.sj = sj.f.empty() ? nullptr : &sj;   // every query in score order: the flat hits are oc_search_pinned's
+    r.q_filters_ok = per_query;
+    return search_impl(c, emb, str, r);
+}
+
+// oc_search_pinned, oc_search_sorted and oc_search_q_sorted: the flat hits with the items of pins, in field order where
+// sj has a sort (else in score order: oc_search_pinned's hits, sort values NaN).  Nothing is written on failure.
+static int sorted_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, const SortJob &sj, const oc_pins *pins,
+                       bool q_filters_ok, uint64_t *out_doc_ids, float *out_scores, double *out_sort_values, uint32_t *out_n,
+                       uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present) {
+    PinJob pj;
+    OCTRY(pin_job_init(pins, p->n_queries, pj));
+    OCTRY(pins_check_flat(p, pj));
+    pj.out_scores = out_pin_scores; pj.out_present = out_pin_present;
+    SearchReq r(p, out_doc_ids, out_scores, out_n, out_count);
+    r.out_sort_values = out_sort_values; r.pj = &pj;
+    r.sj = sj.f.empty() ? nullptr : &sj;
+    r.q_filters_ok = q_filters_ok;
+    return search_impl(c, emb, str, r);
 }
 
 extern "C" uint64_t oc_group_by_n_groups(const oc_group_by *g) { return g ? g->n_groups : 0; }
@@ -3481,9 +3649,7 @@ extern "C" int oc_search_groups(oc_ctx *c, oc_emb *emb, oc_str *str, oc_group_by
     if (!c || !p || !groups || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
     if (groups->n_groups && (!out_group_n || (max_results && (!out_group_doc_ids || !out_group_scores))))
         return fail(OC_ERR_INVALID, "NULL group output");
-    if (groups->ctx != c) return fail(OC_ERR_INVALID, "group_by belongs to another ctx");
     if (p->sharded) return fail(OC_ERR_UNSUPPORTED, "groups over a sharded search: hybrid normalisation and the vector set are global");
-    if (max_results > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "max_results %u > %u", max_results, OC_MAX_TOPK);
     if (p->n_queries > 65535) return fail(OC_ERR_UNSUPPORTED, "groups: n_queries %u > 65535", p->n_queries);
     const std::vector<oc_group_req> req(p->n_queries, oc_group_req{groups, max_results, oc_sort{nullptr, OC_SORT_ASC}});
     return groups_impl(c, emb, str, p, req.data(), nullptr, max_results, false, out_doc_ids, out_scores, nullptr, out_n, out_count,
@@ -3496,10 +3662,7 @@ extern "C" int oc_search_pinned(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_se
                                 uint64_t *out_doc_ids, float *out_scores, uint32_t *out_n, uint64_t *out_count,
                                 float *out_pin_scores, uint8_t *out_pin_present) {
     if (!c || !p) return fail(OC_ERR_INVALID, "NULL argument");
-    PinJob pj;
-    OCTRY(pin_job_init(pins, p->n_queries, pj));
-    OCTRY(pins_check_flat(p, pj));
-    return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, nullptr, &pj, pins, out_pin_scores,
+    return sorted_impl(c, emb, str, p, SortJob{}, pins, false, out_doc_ids, out_scores, nullptr, out_n, out_count, out_pin_scores,
                        out_pin_present);
 }
 
@@ -3510,16 +3673,7 @@ extern "C" int oc_search_groups_pinned(oc_ctx *c, oc_emb *emb, oc_str *str, oc_g
     if (!c || !p || !groups || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
     if (groups->n_groups && (!out_group_n || (group_stride && (!out_group_doc_ids || !out_group_scores))))
         return fail(OC_ERR_INVALID, "NULL group output");
-    if (groups->ctx != c) return fail(OC_ERR_INVALID, "group_by belongs to another ctx");
-    if (max_results > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "max_results %u > %u", max_results, OC_MAX_TOPK);
     if (p->n_queries > 65535) return fail(OC_ERR_UNSUPPORTED, "groups: n_queries %u > 65535", p->n_queries);
-    PinJob pj;
-    OCTRY(pin_job_init(pins, p->n_queries, pj));
-    OCTRY(pins_check_flat(p, pj));
-    if (pj.splice && 2 * max_results > OC_MAX_TOPK)
-        return fail(OC_ERR_UNSUPPORTED, "pins: 2 x max_results %u > %u", 2 * max_results, OC_MAX_TOPK);
-    const uint64_t need = pj.splice ? 2ull * max_results + pj.stride : max_results;
-    if (group_stride < need) return fail(OC_ERR_INVALID, "group_stride %u < %llu", group_stride, (unsigned long long)need);
     const std::vector<oc_group_req> req(p->n_queries, oc_group_req{groups, max_results, oc_sort{nullptr, OC_SORT_ASC}});
     return groups_impl(c, emb, str, p, req.data(), pins, group_stride, false, out_doc_ids, out_scores, nullptr, out_n, out_count,
                        nullptr, nullptr, out_group_doc_ids, out_group_scores, nullptr, out_group_n);
@@ -3588,12 +3742,8 @@ extern "C" int oc_search_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_se
     if (!c || !p) return fail(OC_ERR_INVALID, "NULL argument");
     SortJob sj{};
     OCTRY(sort_job_init(c, sort, p->n_queries, sj));
-    sj.out_values = out_sort_values;
-    PinJob pj;
-    OCTRY(pin_job_init(pins, p->n_queries, pj));
-    OCTRY(pins_check_flat(p, pj));
-    return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, nullptr, &pj, pins, out_pin_scores,
-                       out_pin_present, &sj);
+    return sorted_impl(c, emb, str, p, sj, pins, false, out_doc_ids, out_scores, out_sort_values, out_n, out_count, out_pin_scores,
+                       out_pin_present);
 }
 
 extern "C" int oc_search_groups_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, oc_group_by *groups, const oc_search_params *p,
@@ -3604,18 +3754,8 @@ extern "C" int oc_search_groups_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, oc_g
     if (!c || !p || !groups || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
     if (groups->n_groups && (!out_group_n || (group_stride && (!out_group_doc_ids || !out_group_scores))))
         return fail(OC_ERR_INVALID, "NULL group output");
-    if (groups->ctx != c) return fail(OC_ERR_INVALID, "group_by belongs to another ctx");
-    SortJob sj{};
-    OCTRY(sort_job_init(c, sort, p->n_queries, sj));
-    if (max_results > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "max_results %u > %u", max_results, OC_MAX_TOPK);
+    if (!sort || !sort->field) return fail(OC_ERR_INVALID, "NULL sort");   // (a NULL field is score order in a request)
     if (p->n_queries > 65535) return fail(OC_ERR_UNSUPPORTED, "groups: n_queries %u > 65535", p->n_queries);
-    PinJob pj;
-    OCTRY(pin_job_init(pins, p->n_queries, pj));
-    OCTRY(pins_check_flat(p, pj));
-    if (pj.splice && 2 * max_results > OC_MAX_TOPK)
-        return fail(OC_ERR_UNSUPPORTED, "pins: 2 x max_results %u > %u", 2 * max_results, OC_MAX_TOPK);
-    const uint64_t need = pj.splice ? 2ull * max_results + pj.stride : max_results;
-    if (group_stride < need) return fail(OC_ERR_INVALID, "group_stride %u < %llu", group_stride, (unsigned long long)need);
     const std::vector<oc_group_req> req(p->n_queries, oc_group_req{groups, max_results, *sort});
     return groups_impl(c, emb, str, p, req.data(), pins, group_stride, false, out_doc_ids, out_scores, out_sort_values, out_n,
                        out_count, nullptr, nullptr, out_group_doc_ids, out_group_scores, out_group_sort_values, out_group_n);
@@ -3629,22 +3769,8 @@ extern "C" int oc_search_q_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_
     if (!c || !p || !q_sorts) return fail(OC_ERR_INVALID, "NULL argument");
     SortJob sj{};
     for (uint32_t b = 0; b < p->n_queries; b++) OCTRY(sort_job_add(c, q_sorts[b], sj));
-    sj.out_values = out_sort_values;
-    PinJob pj;
-    pj.q_filters = true;
-    OCTRY(pin_job_init(pins, p->n_queries, pj));
-    OCTRY(pins_check_flat(p, pj));
-    if (!sj.f.empty())
-        return search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, nullptr, &pj, pins, out_pin_scores,
-                           out_pin_present, &sj);
-    // every query in score order: oc_search_pinned
-    OCTRY(search_impl(c, emb, str, p, out_doc_ids, out_scores, out_n, out_count, nullptr, nullptr, &pj, pins, out_pin_scores,
-                      out_pin_present));
-    if (out_sort_values)
-        for (uint32_t q = 0; q < p->n_queries; q++)
-            for (uint32_t i = 0; i < p->limit; i++)
-                out_sort_values[size_t(q) * p->limit + i] = i < out_n[q] ? std::numeric_limits<double>::quiet_NaN() : 0.0;
-    return OC_OK;
+    return sorted_impl(c, emb, str, p, sj, pins, true, out_doc_ids, out_scores, out_sort_values, out_n, out_count, out_pin_scores,
+                       out_pin_present);
 }
 
 // One batch in which every query has its own groups (or none), sort, pins and, with q_filters, filter: query b gets what
