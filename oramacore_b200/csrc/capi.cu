@@ -3986,82 +3986,75 @@ extern "C" int oc_filter_geo_polygon(const oc_geo_field *g, const double *lat, c
 }
 
 // ------------------------------------------------------------------------------------ micro-batching front
-struct OcSearchExec {
+struct OcExec {
     oc_ctx *c; oc_emb *e; oc_str *s;
-    int operator()(const oc_search_params *p, uint64_t *docs, float *scores, uint32_t *n, uint64_t *count) const {
-        return oc_search(c, e, s, p, docs, scores, n, count);
-    }
-};
-struct OcSortedExec {
-    oc_ctx *c; oc_emb *e; oc_str *s;
-    int operator()(const oc_search_params *p, const oc_sort *q_sorts, const oc_pins *pins, uint64_t *docs, float *scores,
-                   double *sort_values, uint32_t *n, uint64_t *count, float *pin_scores, uint8_t *pin_present) const {
-        return oc_search_q_sorted(c, e, s, p, q_sorts, pins, docs, scores, sort_values, n, count, pin_scores, pin_present);
-    }
-};
-struct OcGroupedExec {
-    oc_ctx *c; oc_emb *e; oc_str *s;
-    int operator()(const oc_search_params *p, const oc_group_req *q_groups, const oc_pins *pins, uint32_t group_stride, uint64_t *docs,
-                   float *scores, double *sort_values, uint32_t *n, uint64_t *count, float *pin_scores, uint8_t *pin_present,
-                   uint64_t *g_docs, float *g_scores, double *g_values, uint32_t *g_n) const {
-        return oc_search_q_groups(c, e, s, p, q_groups, pins, group_stride, docs, scores, sort_values, n, count, pin_scores, pin_present,
-                                  g_docs, g_scores, g_values, g_n);
-    }
-};
-struct OcFacetedExec {
-    oc_ctx *c; oc_emb *e; oc_str *s;
-    int operator()(const oc_search_params *p, const oc_group_req *q_groups, const oc_pins *pins, uint32_t group_stride,
-                   const oc_facets *facets, const uint32_t *q_facet_offsets, const oc_facet_req *facet_reqs, uint64_t *docs,
-                   float *scores, double *sort_values, uint32_t *n, uint64_t *count, float *pin_scores, uint8_t *pin_present,
-                   uint64_t *g_docs, float *g_scores, double *g_values, uint32_t *g_n, uint64_t *f_counts) const {
-        return oc_search_q_facets(c, e, s, p, q_groups, pins, group_stride, const_cast<oc_facets *>(facets), q_facet_offsets,
-                                  facet_reqs, docs, scores, sort_values, n, count, pin_scores, pin_present, g_docs, g_scores, g_values,
-                                  g_n, f_counts);
+    int operator()(const ocb::Call &k) const {
+        switch (k.kind) {
+        case ocb::PLAIN: return oc_search(c, e, s, k.p, k.docs, k.scores, k.n, k.count);
+        case ocb::SORTED:
+            return oc_search_q_sorted(c, e, s, k.p, k.q_sorts, k.pins, k.docs, k.scores, k.sort_values, k.n, k.count, k.pin_scores,
+                                      k.pin_present);
+        case ocb::GROUPED:
+            return oc_search_q_groups(c, e, s, k.p, k.q_groups, k.pins, k.group_stride, k.docs, k.scores, k.sort_values, k.n, k.count,
+                                      k.pin_scores, k.pin_present, k.g_docs, k.g_scores, k.g_values, k.g_n);
+        case ocb::FACETED:
+            return oc_search_q_facets(c, e, s, k.p, k.q_groups, k.pins, k.group_stride, k.facets, k.q_facet_offsets, k.facet_reqs,
+                                      k.docs, k.scores, k.sort_values, k.n, k.count, k.pin_scores, k.pin_present, k.g_docs,
+                                      k.g_scores, k.g_values, k.g_n, k.f_counts);
+        }
+        return fail(OC_ERR_INVALID, "unknown call kind %d", (int)k.kind);
     }
     int check(const oc_facets *f, const oc_facet_req *reqs, uint32_t n) const { return oc_facets_check(f, reqs, n); }
 };
 struct oc_batcher {
-    ocb::Batcher<OcSearchExec, OcSortedExec, OcGroupedExec, OcFacetedExec> q;
+    ocb::Batcher<OcExec> q;
     oc_ctx *ctx;
-    oc_batcher(OcSearchExec x, uint32_t dim, uint32_t mb, uint32_t mw)
-        : q(x, dim, mb, mw, x.e != nullptr, x.s != nullptr, OcSortedExec{x.c, x.e, x.s}, OcGroupedExec{x.c, x.e, x.s},
-            OcFacetedExec{x.c, x.e, x.s}), ctx(x.c) {}
+    oc_batcher(OcExec x, uint32_t dim, uint32_t mb, uint32_t mw) : q(x, dim, mb, mw, x.e != nullptr, x.s != nullptr), ctx(x.c) {}
 };
 extern "C" int oc_batcher_create(oc_ctx *c, oc_emb *emb, oc_str *str, uint32_t max_batch, uint32_t max_wait_us, oc_batcher **out) {
     if (!c || !out || (!emb && !str)) return fail(OC_ERR_INVALID, "bad arguments");
     if ((emb && emb->ctx != c) || (str && str->ctx != c)) return fail(OC_ERR_INVALID, "store belongs to another ctx");
     if (max_batch == 0 || max_batch > 4096) return fail(OC_ERR_INVALID, "max_batch %u outside 1..4096", max_batch);
-    *out = new oc_batcher(OcSearchExec{c, emb, str}, emb ? emb->dim : 0, max_batch, max_wait_us);
+    *out = new oc_batcher(OcExec{c, emb, str}, emb ? emb->dim : 0, max_batch, max_wait_us);
     return OC_OK;
 }
 extern "C" void oc_batcher_destroy(oc_batcher *b) { delete b; }
+// The rest of every oc_batcher_search* call once its NULL arguments are checked.  What would fail a whole batch is
+// refused here, before the request joins one: a handle of another ctx (a device filter joins as that query's q_filters
+// entry), a NULL group output, and what submit refuses.
+static int batcher_submit(oc_batcher *b, ocb::Request &r, const char *name) {
+    const ocb::Call &k = r.call;
+    if (k.p->n_queries != 1) return fail(OC_ERR_INVALID, "%s takes one query per call (n_queries = %u)", name, k.p->n_queries);
+    const oc_sort *sort = ocb::sort_of(k);
+    if (k.facets && k.facets->ctx != b->ctx) return fail(OC_ERR_INVALID, "facets belong to another ctx");
+    if (k.p->filter && k.p->filter->ctx != b->ctx) return fail(OC_ERR_INVALID, "filter belongs to another ctx");
+    if (sort && sort->field && sort->field->ctx != b->ctx) return fail(OC_ERR_INVALID, "sort field belongs to another ctx");
+    if (k.q_groups) {
+        if (k.q_groups->groups && k.q_groups->groups->ctx != b->ctx) return fail(OC_ERR_INVALID, "group_by belongs to another ctx");
+        r.n_groups = oc_group_by_n_groups(k.q_groups->groups);
+        if (r.n_groups && (!k.g_n || (k.group_stride && (!k.g_docs || !k.g_scores)))) return fail(OC_ERR_INVALID, "NULL group output");
+    }
+    g_err[0] = 0;
+    const char *why = nullptr;
+    const int rc = b->q.submit(r, &why);
+    if (rc != OC_OK && why) return fail(rc, "%s", why);
+    // the batch ran on its leader's thread: that is where oc_last_error() holds the detail
+    if (rc != OC_OK && g_err[0] == 0) return fail(rc, "the coalesced search of this query's batch failed (detail on the leading caller's thread)");
+    return rc;
+}
 extern "C" int oc_batcher_search(oc_batcher *b, const oc_search_params *p, uint64_t *out_doc_ids, float *out_scores,
                                  uint32_t *out_n, uint64_t *out_count) {
     if (!b || !p || !out_doc_ids || !out_scores || !out_n || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
-    if (p->n_queries != 1) return fail(OC_ERR_INVALID, "oc_batcher_search takes one query per call (n_queries = %u)", p->n_queries);
-    // a device filter joins a batch as that query's q_filters entry: one of another ctx would fail the whole batch
-    if (p->filter && p->filter->ctx != b->ctx) return fail(OC_ERR_INVALID, "filter belongs to another ctx");
-    g_err[0] = 0;
-    const int rc = b->q.submit(p, out_doc_ids, out_scores, out_n, out_count);
-    // the batch ran on its leader's thread: that is where oc_last_error() holds the detail
-    if (rc != OC_OK && g_err[0] == 0) return fail(rc, "the coalesced oc_search of this query's batch failed (detail on the leading caller's thread)");
-    return rc;
+    ocb::Request r{{ocb::PLAIN, p, out_doc_ids, out_scores, out_n, out_count}};
+    return batcher_submit(b, r, "oc_batcher_search");
 }
 extern "C" int oc_batcher_search_sorted(oc_batcher *b, const oc_search_params *p, const oc_sort *sort, const oc_pins *pins,
                                         uint64_t *out_doc_ids, float *out_scores, double *out_sort_values, uint32_t *out_n,
                                         uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present) {
     if (!b || !p || !out_doc_ids || !out_scores || !out_n || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
-    if (p->n_queries != 1) return fail(OC_ERR_INVALID, "oc_batcher_search_sorted takes one query per call (n_queries = %u)", p->n_queries);
-    // what would fail a whole batch is refused here, before the request joins one
-    if (p->filter && p->filter->ctx != b->ctx) return fail(OC_ERR_INVALID, "filter belongs to another ctx");
-    if (sort && sort->field && sort->field->ctx != b->ctx) return fail(OC_ERR_INVALID, "sort field belongs to another ctx");
-    const char *why = nullptr;
-    if (const int rc = ocb::check_sorted(sort, pins, &why)) return fail(rc, "%s", why);
-    g_err[0] = 0;
-    const int rc = b->q.submit_sorted(p, sort, pins, out_doc_ids, out_scores, out_sort_values, out_n, out_count, out_pin_scores,
-                                      out_pin_present);
-    if (rc != OC_OK && g_err[0] == 0) return fail(rc, "the coalesced search of this query's batch failed (detail on the leading caller's thread)");
-    return rc;
+    ocb::Request r{{ocb::SORTED, p, out_doc_ids, out_scores, out_n, out_count, out_sort_values, out_pin_scores, out_pin_present, pins,
+                    sort ? sort : ocb::score_order()}};
+    return batcher_submit(b, r, "oc_batcher_search_sorted");
 }
 extern "C" int oc_batcher_search_groups(oc_batcher *b, const oc_search_params *p, const oc_group_req *req, const oc_pins *pins,
                                         uint32_t group_stride, uint64_t *out_doc_ids, float *out_scores, double *out_sort_values,
@@ -4070,24 +4063,9 @@ extern "C" int oc_batcher_search_groups(oc_batcher *b, const oc_search_params *p
                                         uint32_t *out_group_n) {
     if (!b || !p || !req || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
     if (p->limit && (!out_doc_ids || !out_scores || !out_n)) return fail(OC_ERR_INVALID, "NULL argument");
-    if (p->n_queries != 1) return fail(OC_ERR_INVALID, "oc_batcher_search_groups takes one query per call (n_queries = %u)", p->n_queries);
-    // what would fail a whole batch is refused here, before the request joins one
-    if (p->filter && p->filter->ctx != b->ctx) return fail(OC_ERR_INVALID, "filter belongs to another ctx");
-    if (req->sort.field && req->sort.field->ctx != b->ctx) return fail(OC_ERR_INVALID, "sort field belongs to another ctx");
-    if (req->groups && req->groups->ctx != b->ctx) return fail(OC_ERR_INVALID, "group_by belongs to another ctx");
-    const uint64_t n_groups = oc_group_by_n_groups(req->groups);
-    if (n_groups && (!out_group_n || (group_stride && (!out_group_doc_ids || !out_group_scores))))
-        return fail(OC_ERR_INVALID, "NULL group output");
-    const char *why = nullptr;
-    if (const int rc = ocb::check_sorted(&req->sort, pins, &why)) return fail(rc, "%s", why);
-    if (group_stride < ocb::group_need(req, pins))
-        return fail(OC_ERR_INVALID, "group_stride %u < %llu", group_stride, (unsigned long long)ocb::group_need(req, pins));
-    g_err[0] = 0;
-    const int rc = b->q.submit_groups(p, req, n_groups, pins, group_stride, out_doc_ids, out_scores, out_sort_values, out_n, out_count,
-                                      out_pin_scores, out_pin_present, out_group_doc_ids, out_group_scores, out_group_sort_values,
-                                      out_group_n);
-    if (rc != OC_OK && g_err[0] == 0) return fail(rc, "the coalesced grouped search of this query's batch failed (detail on the leading caller's thread)");
-    return rc;
+    ocb::Request r{{ocb::GROUPED, p, out_doc_ids, out_scores, out_n, out_count, out_sort_values, out_pin_scores, out_pin_present, pins,
+                    nullptr, req, group_stride, out_group_doc_ids, out_group_scores, out_group_sort_values, out_group_n}};
+    return batcher_submit(b, r, "oc_batcher_search_groups");
 }
 extern "C" int oc_batcher_search_faceted(oc_batcher *b, const oc_search_params *p, oc_facets *facets, const oc_facet_req *facet_reqs,
                                          uint32_t n_facet_reqs, const oc_group_req *req, const oc_pins *pins, uint32_t group_stride,
@@ -4098,26 +4076,11 @@ extern "C" int oc_batcher_search_faceted(oc_batcher *b, const oc_search_params *
     if (!b || !p || !facets || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
     if (p->limit && (!out_doc_ids || !out_scores || !out_n)) return fail(OC_ERR_INVALID, "NULL argument");
     if (n_facet_reqs && (!facet_reqs || !out_facet_counts)) return fail(OC_ERR_INVALID, "NULL facet requests / counts");
-    if (p->n_queries != 1) return fail(OC_ERR_INVALID, "oc_batcher_search_faceted takes one query per call (n_queries = %u)", p->n_queries);
-    // what would fail a whole batch is refused here, before the request joins one
-    if (facets->ctx != b->ctx) return fail(OC_ERR_INVALID, "facets belong to another ctx");
-    if (p->filter && p->filter->ctx != b->ctx) return fail(OC_ERR_INVALID, "filter belongs to another ctx");
-    const oc_group_req *r = req ? req : ocb::no_groups();
-    if (r->sort.field && r->sort.field->ctx != b->ctx) return fail(OC_ERR_INVALID, "sort field belongs to another ctx");
-    if (r->groups && r->groups->ctx != b->ctx) return fail(OC_ERR_INVALID, "group_by belongs to another ctx");
-    const uint64_t n_groups = oc_group_by_n_groups(r->groups);
-    if (n_groups && (!out_group_n || (group_stride && (!out_group_doc_ids || !out_group_scores))))
-        return fail(OC_ERR_INVALID, "NULL group output");
-    const char *why = nullptr;
-    if (const int rc = ocb::check_sorted(&r->sort, pins, &why)) return fail(rc, "%s", why);
-    if (group_stride < ocb::group_need(r, pins))
-        return fail(OC_ERR_INVALID, "group_stride %u < %llu", group_stride, (unsigned long long)ocb::group_need(r, pins));
-    g_err[0] = 0;
-    const int rc = b->q.submit_faceted(p, facets, facet_reqs, n_facet_reqs, r, n_groups, pins, group_stride, out_doc_ids, out_scores,
-                                       out_sort_values, out_n, out_count, out_pin_scores, out_pin_present, out_group_doc_ids,
-                                       out_group_scores, out_group_sort_values, out_group_n, out_facet_counts);
-    if (rc != OC_OK && g_err[0] == 0) return fail(rc, "the coalesced faceted search of this query's batch failed (detail on the leading caller's thread)");
-    return rc;
+    ocb::Request r{{ocb::FACETED, p, out_doc_ids, out_scores, out_n, out_count, out_sort_values, out_pin_scores, out_pin_present, pins,
+                    nullptr, req ? req : ocb::no_groups(), group_stride, out_group_doc_ids, out_group_scores, out_group_sort_values,
+                    out_group_n, facets, nullptr, facet_reqs, out_facet_counts}, 0, {0, n_facet_reqs}};
+    r.call.q_facet_offsets = r.f_off;
+    return batcher_submit(b, r, "oc_batcher_search_faceted");
 }
 extern "C" int oc_batcher_stats(oc_batcher *b, uint64_t *n_queries, uint64_t *n_batches, uint64_t *n_direct) {
     if (!b) return fail(OC_ERR_INVALID, "NULL argument");

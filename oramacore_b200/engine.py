@@ -843,6 +843,14 @@ def _group_need(g, k: int) -> int:
     return 2 * int(g[1]) + k if k else int(g[1])
 
 
+def _q_outputs(B: int, L: int, n_items: int, R: int, S: int):
+    """Zeroed outputs of oc_search_q_groups: docs, scores, sort values [B,L], n, count [B], pin scores, pin present
+    [max(items, 1)], group docs, group scores, group sort values [R,S], group n [R]."""
+    return (np.zeros((B, L), np.uint64), np.zeros((B, L), np.float32), np.zeros((B, L), np.float64), np.zeros(B, np.uint32),
+            np.zeros(B, np.uint64), np.zeros(max(n_items, 1), np.float32), np.zeros(max(n_items, 1), np.uint8),
+            np.zeros((R, S), np.uint64), np.zeros((R, S), np.float32), np.zeros((R, S), np.float64), np.zeros(R, np.uint32))
+
+
 def search_q_groups_arrays(tsc: "TokenScoreContext", params: "TokenScoreParams", groups, promote=None, texts=None,
                            q_vecs: Optional[np.ndarray] = None, group_stride: Optional[int] = None):
     """oc_search_q_groups: one batch in which every query has its own groupBy, sortBy and pin rules, and
@@ -861,11 +869,7 @@ def search_q_groups_arrays(tsc: "TokenScoreContext", params: "TokenScoreParams",
         k = [0] * B if promote is None else [len(x) for x in promote]
         group_stride = max([0] + [_group_need(g, k[b]) for b, g in enumerate(groups)])
     L, R, S = params.limit_hint, int(rows[-1]), int(group_stride)
-    docs, scores, sv = np.zeros((B, L), np.uint64), np.zeros((B, L), np.float32), np.zeros((B, L), np.float64)
-    n, cnt = np.zeros(B, np.uint32), np.zeros(B, np.uint64)
-    ps, pp = np.zeros(max(n_items, 1), np.float32), np.zeros(max(n_items, 1), np.uint8)
-    gd, gs, gsv = np.zeros((R, S), np.uint64), np.zeros((R, S), np.float32), np.zeros((R, S), np.float64)
-    gn = np.zeros(R, np.uint32)
+    docs, scores, sv, n, cnt, ps, pp, gd, gs, gsv, gn = _q_outputs(B, L, n_items, R, S)
     check(lib().oc_search_q_groups(tsc.ctx._h, tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None, C.byref(sp),
                                    req, None if pins is None else C.byref(pins), S, _p(docs), _p(scores), _p(sv), _p(n),
                                    _p(cnt), _p(ps), _p(pp), _p(gd), _p(gs), _p(gsv), _p(gn)))
@@ -919,11 +923,7 @@ def search_q_facets_arrays(tsc: "TokenScoreContext", store: FacetStore, params: 
         k = [0] * B if promote is None else [len(x) for x in promote]
         group_stride = max([0] + [_group_need(g, k[b]) for b, g in enumerate(groups or [None] * B)])
     L, R, S = params.limit_hint, int(rows[-1]), int(group_stride)
-    docs, scores, sv = np.zeros((B, L), np.uint64), np.zeros((B, L), np.float32), np.zeros((B, L), np.float64)
-    n, cnt = np.zeros(B, np.uint32), np.zeros(B, np.uint64)
-    ps, pp = np.zeros(max(n_items, 1), np.float32), np.zeros(max(n_items, 1), np.uint8)
-    gd, gs, gsv = np.zeros((R, S), np.uint64), np.zeros((R, S), np.float32), np.zeros((R, S), np.float64)
-    gn = np.zeros(R, np.uint32)
+    docs, scores, sv, n, cnt, ps, pp, gd, gs, gsv, gn = _q_outputs(B, L, n_items, R, S)
     fc = np.zeros(max(int(foff[-1]), 1), np.uint64)
     check(lib().oc_search_q_facets(tsc.ctx._h, tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None, C.byref(sp),
                                    req, None if pins is None else C.byref(pins), S, store._h, _p(foff), farr, _p(docs),
@@ -1219,11 +1219,16 @@ class SearchBatcher:
                                       int(max_batch), int(max_wait_us), C.byref(h)))
         self._h = h
 
-    def search(self, params: TokenScoreParams, text: Optional[TextQuery] = None,
-               q_vec: Optional[np.ndarray] = None) -> SearchHits:
+    def _params(self, params: TokenScoreParams, text: Optional[TextQuery], q_vec: Optional[np.ndarray]):
+        """oc_search_params of one query and the arrays they point into."""
         sp, keep, B = self.tsc._build_params(params, None if text is None else [text],
                                              None if q_vec is None else np.asarray(q_vec, np.float32).reshape(1, -1))
         assert B == 1
+        return sp, keep
+
+    def search(self, params: TokenScoreParams, text: Optional[TextQuery] = None,
+               q_vec: Optional[np.ndarray] = None) -> SearchHits:
+        sp, keep = self._params(params, text, q_vec)
         L = params.limit_hint
         docs, scores = np.empty(L, np.uint64), np.empty(L, np.float32)
         n, cnt = np.zeros(1, np.uint32), np.zeros(1, np.uint64)
@@ -1237,9 +1242,7 @@ class SearchBatcher:
         promote items, None: no rule), coalesced with concurrent search() / search_sorted() calls.  Returns
         (SearchHits, sort values [n], pin scores [items], pin present [items]) as search_q_sorted_arrays gives them for
         this query alone."""
-        sp, keep, B = self.tsc._build_params(params, None if text is None else [text],
-                                             None if q_vec is None else np.asarray(q_vec, np.float32).reshape(1, -1))
-        assert B == 1
+        sp, keep = self._params(params, text, q_vec)
         srt = None if sort is None else _sort(sort[0], sort[1])
         pins = None if promote is None else _pins([promote], 1)[0]
         n_items = 0 if pins is None else int(pins._keep[0][-1])
@@ -1260,23 +1263,17 @@ class SearchBatcher:
         [limit], scores, sort values [limit], n, count, pin scores [items], pin present [items], group docs
         [n_groups, stride], group scores, group sort values, group n [n_groups]) as search_q_groups_arrays gives them for
         this query alone."""
-        sp, keep, B = self.tsc._build_params(params, None if text is None else [text],
-                                             None if q_vec is None else np.asarray(q_vec, np.float32).reshape(1, -1))
-        assert B == 1
+        sp, keep = self._params(params, text, q_vec)
         req, rows = _group_reqs([group], 1)
         pins = None if promote is None else _pins([promote], 1)[0]
         n_items = 0 if pins is None else int(pins._keep[0][-1])
         if group_stride is None:
             group_stride = _group_need(group, n_items)
-        L, G, S = params.limit_hint, int(rows[-1]), int(group_stride)
-        docs, scores, sv = np.zeros(L, np.uint64), np.zeros(L, np.float32), np.zeros(L, np.float64)
-        n, cnt = np.zeros(1, np.uint32), np.zeros(1, np.uint64)
-        ps, pp = np.zeros(max(n_items, 1), np.float32), np.zeros(max(n_items, 1), np.uint8)
-        gd, gs, gsv = np.zeros((G, S), np.uint64), np.zeros((G, S), np.float32), np.zeros((G, S), np.float64)
-        gn = np.zeros(G, np.uint32)
+        S = int(group_stride)
+        docs, scores, sv, n, cnt, ps, pp, gd, gs, gsv, gn = _q_outputs(1, params.limit_hint, n_items, int(rows[-1]), S)
         check(lib().oc_batcher_search_groups(self._h, C.byref(sp), req, None if pins is None else C.byref(pins), S, _p(docs),
                                              _p(scores), _p(sv), _p(n), _p(cnt), _p(ps), _p(pp), _p(gd), _p(gs), _p(gsv), _p(gn)))
-        return docs, scores, sv, n[0], cnt[0], ps[:n_items], pp[:n_items], gd, gs, gsv, gn
+        return docs[0], scores[0], sv[0], n[0], cnt[0], ps[:n_items], pp[:n_items], gd, gs, gsv, gn
 
     def search_faceted(self, store: FacetStore, params: TokenScoreParams, facets, group=None, promote=None,
                        text: Optional[TextQuery] = None, q_vec: Optional[np.ndarray] = None, group_stride: Optional[int] = None):
@@ -1284,26 +1281,20 @@ class SearchBatcher:
         search_groups, or None) and pin rules, coalesced with concurrent search_faceted() calls on the same store.
         Returns search_groups()' tuple followed by the facet counts [requests] and their (field, label) pairs, as
         search_q_facets_arrays gives them for this query alone."""
-        sp, keep, B = self.tsc._build_params(params, None if text is None else [text],
-                                             None if q_vec is None else np.asarray(q_vec, np.float32).reshape(1, -1))
-        assert B == 1
+        sp, keep = self._params(params, text, q_vec)
         req, rows = _group_reqs([group], 1)
         farr, foff, labels = _q_facet_reqs(store, [facets], 1)
         pins = None if promote is None else _pins([promote], 1)[0]
         n_items = 0 if pins is None else int(pins._keep[0][-1])
         if group_stride is None:
             group_stride = _group_need(group, n_items)
-        L, G, S, F = params.limit_hint, int(rows[-1]), int(group_stride), int(foff[-1])
-        docs, scores, sv = np.zeros(L, np.uint64), np.zeros(L, np.float32), np.zeros(L, np.float64)
-        n, cnt = np.zeros(1, np.uint32), np.zeros(1, np.uint64)
-        ps, pp = np.zeros(max(n_items, 1), np.float32), np.zeros(max(n_items, 1), np.uint8)
-        gd, gs, gsv = np.zeros((G, S), np.uint64), np.zeros((G, S), np.float32), np.zeros((G, S), np.float64)
-        gn = np.zeros(G, np.uint32)
+        S, F = int(group_stride), int(foff[-1])
+        docs, scores, sv, n, cnt, ps, pp, gd, gs, gsv, gn = _q_outputs(1, params.limit_hint, n_items, int(rows[-1]), S)
         fc = np.zeros(max(F, 1), np.uint64)
         check(lib().oc_batcher_search_faceted(self._h, C.byref(sp), store._h, farr, F, None if group is None else req,
                                               None if pins is None else C.byref(pins), S, _p(docs), _p(scores), _p(sv), _p(n),
                                               _p(cnt), _p(ps), _p(pp), _p(gd), _p(gs), _p(gsv), _p(gn), _p(fc)))
-        return docs, scores, sv, n[0], cnt[0], ps[:n_items], pp[:n_items], gd, gs, gsv, gn, fc[:F], labels[0]
+        return docs[0], scores[0], sv[0], n[0], cnt[0], ps[:n_items], pp[:n_items], gd, gs, gsv, gn, fc[:F], labels[0]
 
     def stats(self) -> dict:
         q, b, d = C.c_uint64(), C.c_uint64(), C.c_uint64()

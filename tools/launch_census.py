@@ -1,7 +1,10 @@
 """Launch census: a fixed matrix of calls through every public search entry point, on small seeded stores.
 
 Per call it prints one line: the return code, the oc_launch_count() delta, oc_last_timing's h2d_bytes / d2h_bytes
-and a sha256 of every output array.  Two builds that do the same device work print the same lines, so a host-side
+and a sha256 of every output array.  Then every oc_batcher_search* function runs rounds of B single-query requests,
+direct (max_batch = 1) and merged into one call, and mixed rounds (plain, plain with sorted / pinned, grouped) on each
+filter variant; per request it prints the return code and output digest, per round the same counters and the
+oc_batcher_stats delta.  Two builds that do the same device work print the same lines, so a host-side
 change is checked by running this under OC_SO_PATH for each build and diffing the two outputs:
 
     OC_SO_PATH=/path/to/parent/liboramacore_b200.so python tools/launch_census.py > parent.txt
@@ -14,6 +17,8 @@ import hashlib
 import itertools
 import os
 import sys
+import threading
+import time
 
 import numpy as np
 
@@ -146,6 +151,58 @@ def main():
         return rc, d, s, n, c, gd, gs, gn, sv, gsv
     run("refuse groups n_queries", lambda: raw_groups(70000, False))
     run("refuse groups_sorted NULL sort", lambda: raw_groups(B, True))
+
+    # oc_batcher: one round of B requests.  Per request: rc and output digest; per round: the launch delta, the last
+    # call's h2d / d2h bytes and the stats delta.  A merged round starts its requests 30 ms apart from B threads into a
+    # batcher that waits for all B, so each round is one merged call with the requests in index order.
+    q_flt = [f_a, None, f_b, f_a, None, f_b]
+
+    def bparams(mode, flt, i):
+        kw = {"device_filter": f_a} if flt == "filter" else {"device_filter": q_flt[i]} if flt == "q_filters" else \
+            {"filtered_doc_ids": host_bits, "filter_nbits": N} if flt == "bits" else {}
+        return ob.TokenScoreParams(mode=MODES[mode], limit_hint=8, offset=1, similarity=0.0, **kw)
+
+    bcalls = {
+        "search": lambda bat, p, i: bat.search(p, texts[i], qv[i]),
+        "search_sorted": lambda bat, p, i: bat.search_sorted(p, sorts[i], promote[i], texts[i], qv[i]),
+        "search_groups": lambda bat, p, i: bat.search_groups(p, qgroups[i], promote[i], texts[i], qv[i]),
+        "search_faceted": lambda bat, p, i: bat.search_faceted(store, p, facets[i], qgroups[i], promote[i], texts[i], qv[i]),
+    }
+
+    def batcher_round(name, max_batch, mode, flt, fns):
+        bat = ob.SearchBatcher(tsc, max_batch=max_batch, max_wait_us=5_000_000)
+        outs = [None] * B
+
+        def one(i):
+            if max_batch > 1 and flt != "bits":
+                time.sleep(0.03 * i)
+            try:
+                outs[i] = (0, bcalls[fns[i]](bat, bparams(mode, flt, i), i))
+            except ob.OcError as e:
+                outs[i] = (e.code, ())
+
+        before = ctx.launch_count()
+        if max_batch == 1 or flt == "bits":   # every request runs directly: one at a time, so the last call is request B-1
+            for i in range(B):
+                one(i)
+        else:
+            th = [threading.Thread(target=one, args=(i,)) for i in range(B)]
+            for t in th:
+                t.start()
+            for t in th:
+                t.join()
+        t, s = ctx.last_timing(), bat.stats()
+        bat.close()
+        for i, (rc, out) in enumerate(outs):
+            print(f"batcher {name} req{i} {fns[i]} rc={rc} out={digest(out if isinstance(out, tuple) else [out])}", flush=True)
+        print(f"batcher {name} launches={ctx.launch_count() - before} h2d={t['h2d_bytes']} d2h={t['d2h_bytes']} "
+              f"queries={s['queries']} batches={s['batches']} direct={s['direct']}", flush=True)
+
+    for fn, mode, (case, mb) in itertools.product(bcalls, MODES, [("direct", 1), ("merged", B)]):
+        batcher_round(f"{fn} {mode} {case}", mb, mode, "none", [fn] * B)
+    mixes = {"plain": ["search"] * B, "plain+sorted": ["search", "search_sorted"] * (B // 2), "grouped": ["search_groups"] * B}
+    for mix, mode, flt in itertools.product(mixes, MODES, ["none", "filter", "bits", "q_filters"]):
+        batcher_round(f"mix {mix} {mode} {flt}", B, mode, flt, mixes[mix])
 
 
 if __name__ == "__main__":
