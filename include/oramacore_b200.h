@@ -205,7 +205,19 @@ typedef struct {
     const struct oc_filter *filter;    /* NULL, or a device-resident DocumentId bitmap (oc_filter_*): takes precedence
                                           over filter_bits and is not re-uploaded per call                           */
     const struct oc_filter *const *q_filters;  /* NULL, or B entries: query b is filtered by q_filters[b] (NULL = none) */
+    const struct oc_query_params *q_params;    /* NULL, or B entries: query b's own mode, limit, offset, similarity,
+                                                  threshold and vector_limit (see below)                          */
 } oc_search_params;
+
+/* One query's scalar parameters (SearchParams, types.rs:1381-1409, with FulltextMode / VectorMode / HybridMode,
+ * types.rs:837-912): the fields of oc_search_params with the same names, for one query. */
+typedef struct oc_query_params {
+    int mode;              /* OC_MODE_*                                      */
+    uint32_t limit, offset;
+    float similarity;      /* vector / hybrid                                */
+    float threshold;       /* < 0 => None                                    */
+    uint32_t vector_limit; /* 0 => limit (as oc_search_params.vector_limit)  */
+} oc_query_params;
 
 /* out_doc_ids/out_scores: B x limit (best first, after offset); out_n[b] hits written;
  * out_count[b] = all matching documents. emb may be NULL for fulltext, str NULL for vector.
@@ -223,7 +235,28 @@ typedef struct {
  *   - oc_search_q_sorted takes q_filters together with a sort and pins per query, oc_search_q_groups together with
  *     groups, a sort and pins per query;
  *   - oc_search_groups*, oc_search_pinned and oc_search_sorted refuse q_filters with OC_ERR_UNSUPPORTED;
- *     oc_search_facets ignores it as it ignores filter (facets are scored without the where-filter). */
+ *     oc_search_facets ignores it as it ignores filter (facets are scored without the where-filter).
+ *
+ * Per-query parameters (q_params): every request of the reference sets its own mode, limit, offset, similarity and
+ * threshold.  With q_params set, query b's outputs — ids, score bits, n, count, and in the calls below its sort values,
+ * pin scores / present flags, group rows and facet counts — are byte for byte what it gets alone: B = 1 with
+ * p->mode / limit / offset / similarity / threshold / vector_limit taken from q_params[b], together with its own
+ * filter, sort, items, groups and facets.  So a batch whose entries all equal p's scalars gives the plain call's
+ * outputs.  Taken by oc_search, oc_search_q_sorted, oc_search_q_groups and oc_search_q_facets.
+ *   - Layout: p->limit is the row stride of the hit arrays (out_doc_ids, out_scores, out_sort_values) and must be at
+ *     least every entry's limit; entries past out_n[b] are 0.  p->mode, offset, similarity, threshold and
+ *     vector_limit are ignored; bm25_k, bm25_b, OMC, filter / filter_bits / q_filters and sharded stay batch-wide.
+ *   - Inputs: emb and q_vecs are needed when some entry has a vector part (q_vecs keeps B rows; the rows of fulltext
+ *     entries are not read), str and q_token_offsets when some entry has a text part (the token ranges of vector
+ *     entries are ignored).
+ *   - Refusals (nothing written): every check a query's scalars get alone applies to its entry (unknown mode, limit 0
+ *     where the entry point refuses it, the limit + offset, 2 x (limit + offset) and vector_limit bounds, a missing
+ *     store or array for its mode); OC_ERR_INVALID: an entry's limit above p->limit; OC_ERR_UNSUPPORTED: p->sharded,
+ *     and q_params given to oc_search_pinned, oc_search_sorted, oc_search_groups* or oc_search_facets.
+ *   - Cost: one sweep of the embedding store serves the entries with a vector part, at their largest depth; the
+ *     fulltext stage keeps every query's candidates at the largest limit + offset.  One entry with a threshold routes
+ *     the batch's fulltext stage to the threshold scorer, one vector depth above 128 the vector sweep to the exact
+ *     path. */
 int oc_search(oc_ctx *ctx, oc_emb *emb, oc_str *str, const oc_search_params *p,
               uint64_t *out_doc_ids, float *out_scores, uint32_t *out_n, uint64_t *out_count);
 
@@ -621,9 +654,20 @@ void oc_resolved_free(oc_resolved *r);
  * not sharded; a device filter (p->filter) is carried into the batch as that query's q_filters entry, so filtered
  * and unfiltered requests share a batch.  Any other call is passed straight to oc_search, and a p->filter of
  * another ctx is refused with OC_ERR_INVALID before it can join a batch.  p->n_queries must be 1; outputs as for
- * oc_search with B = 1. */
+ * oc_search with B = 1.  A query with its own q_params runs directly.
+ * oc_batcher_create2 with flags OC_BATCHER_MIXED: the key drops mode, limit, offset, similarity, threshold and
+ * vector_limit.  The merged call carries each request's scalars as its q_params entry (row stride = the largest
+ * limit) and every caller gets its hits at its own limit, byte for byte what it gets alone.  The key keeps bm25_k,
+ * bm25_b, the class (flat / grouped / faceted on one store), the OMC arrays (requests with identical omc_doc_ids,
+ * omc_mult, n_omc batch; OMC no longer sends a request straight to oc_search) and two route flags: whether the query
+ * has a threshold (text part), and whether its vector depth exceeds the tensor-core sweep's 128.  A request whose
+ * limit + offset or vector depth the library refuses, or a flat request at limit 0, runs directly.
+ * oc_batcher_create == oc_batcher_create2 with flags 0.  OC_ERR_INVALID: unknown flag bits. */
 typedef struct oc_batcher oc_batcher;
+#define OC_BATCHER_MIXED 1u
 int oc_batcher_create(oc_ctx *ctx, oc_emb *emb, oc_str *str, uint32_t max_batch, uint32_t max_wait_us, oc_batcher **out);
+int oc_batcher_create2(oc_ctx *ctx, oc_emb *emb, oc_str *str, uint32_t max_batch, uint32_t max_wait_us, uint32_t flags,
+                       oc_batcher **out);
 void oc_batcher_destroy(oc_batcher *b);
 int oc_batcher_search(oc_batcher *b, const oc_search_params *p, uint64_t *out_doc_ids, float *out_scores,
                       uint32_t *out_n, uint64_t *out_count);

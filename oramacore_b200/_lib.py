@@ -26,13 +26,14 @@ OC_SCAN_EXACT = 0
 OC_SCAN_TC_TF32 = 1
 OC_SCAN_TC_BF16 = 4
 OC_SCAN_TC_F16 = 5   # wgmma .f16 on the fp16 copy of an fp32 store; OC_EMB_F16=0 selects OC_SCAN_TC_TF32
+OC_BATCHER_MIXED = 1   # oc_batcher_create2: requests with different scalars share a batch
 
 EXPORTED_SYMBOLS = [
     "oc_last_error", "oc_version", "oc_abi_sizes", "oc_init", "oc_shutdown", "oc_device_info", "oc_comm_unique_id",
     "oc_comm_init", "oc_comm_p2p_export", "oc_comm_p2p_import", "oc_emb_create", "oc_emb_destroy", "oc_emb_reserve", "oc_emb_insert", "oc_emb_delete",
     "oc_emb_info", "oc_emb_search", "oc_str_create", "oc_str_destroy", "oc_str_set_rows", "oc_str_load_field",
     "oc_str_insert", "oc_str_commit", "oc_str_delete", "oc_str_info", "oc_str_set_global", "oc_search", "oc_pinned_alloc", "oc_pinned_free", "oc_last_timing", "oc_launch_count",
-    "oc_batcher_create", "oc_batcher_destroy", "oc_batcher_search", "oc_batcher_search_sorted", "oc_batcher_search_groups",
+    "oc_batcher_create", "oc_batcher_create2", "oc_batcher_destroy", "oc_batcher_search", "oc_batcher_search_sorted", "oc_batcher_search_groups",
     "oc_batcher_search_faceted", "oc_batcher_stats",
     "oc_filter_from_ids", "oc_filter_from_bits", "oc_filter_and", "oc_filter_or", "oc_filter_not", "oc_filter_count",
     "oc_filter_read", "oc_filter_destroy", "oc_merge_results",
@@ -73,7 +74,12 @@ class SearchParams(C.Structure):
                 ("filter_bits", C.c_void_p), ("filter_nbits", C.c_uint64),
                 ("omc_doc_ids", C.c_void_p), ("omc_mult", C.c_void_p), ("n_omc", C.c_uint64),
                 ("sharded", C.c_int), ("vector_limit", C.c_uint32), ("filter", C.c_void_p),
-                ("q_filters", C.c_void_p)]
+                ("q_filters", C.c_void_p), ("q_params", C.c_void_p)]
+
+
+class QueryParams(C.Structure):   # oc_query_params: one entry of SearchParams.q_params
+    _fields_ = [("mode", C.c_int), ("limit", C.c_uint32), ("offset", C.c_uint32), ("similarity", C.c_float),
+                ("threshold", C.c_float), ("vector_limit", C.c_uint32)]
 
 
 class FacetReq(C.Structure):
@@ -170,6 +176,7 @@ def lib():
     L.oc_str_info.argtypes = [vp, C.POINTER(StrInfo)]
     L.oc_search.argtypes = [vp, vp, vp, C.POINTER(SearchParams), vp, vp, vp, vp]
     L.oc_batcher_create.argtypes = [vp, vp, vp, u32, u32, C.POINTER(vp)]
+    L.oc_batcher_create2.argtypes = [vp, vp, vp, u32, u32, u32, C.POINTER(vp)]
     L.oc_batcher_destroy.argtypes = [vp]
     L.oc_batcher_destroy.restype = None
     L.oc_batcher_search.argtypes = [vp, C.POINTER(SearchParams), vp, vp, vp, vp]

@@ -11,6 +11,11 @@
 // its q_filters entry.  A request the merged call could not take (batchable and the *_batchable predicates) runs
 // directly, alone; one the library would refuse for its own arguments is refused before it joins.  A merged grouped or
 // faceted call that runs out of device memory is split in halves and re-run.
+// Mixed batcher (OC_BATCHER_MIXED): the key drops (mode, limit, offset, similarity, threshold, vector_limit); requests
+// that differ in them share a batch, each carrying its scalars as its q_params entry of the merged call, whose limit
+// (the hits' row stride) is the batch's largest.  The key keeps bm25_k, bm25_b, the class, the OMC arrays (requests on
+// one index share them, so they batch) and two route flags, each of which would move a whole batch to a slower kernel:
+// "has a threshold" (the threshold scorer) and "vector depth above the tensor-core limit" (the exact sweep).
 #pragma once
 #include <algorithm>
 #include <atomic>
@@ -70,26 +75,49 @@ inline const oc_group_req *no_groups() {
     return &none;
 }
 
+// Largest vector depth the tensor-core sweep serves (emb_gemm.cuh GEMM_MAX_LIMIT): a deeper query sends the vector
+// sub-batch of its call to the exact sweep.
+constexpr uint32_t TC_MAX_DEPTH = 128;
+
 struct BatchKey {
     int mode; uint32_t limit, offset; float similarity, threshold, k, b; uint32_t vector_limit;
     Kind cls;                            // PLAIN for the flat class, GROUPED or FACETED
     const oc_facets *facets;             // faceted requests batch only on the same store
+    // mixed batcher: the scalars above are 0; the route flags and the OMC arrays take their place
+    bool thr, deep;
+    const uint64_t *omc_doc; const float *omc_mult; uint64_t n_omc;
     bool operator==(const BatchKey &o) const {
         return mode == o.mode && limit == o.limit && offset == o.offset && vector_limit == o.vector_limit && cls == o.cls &&
                facets == o.facets && memcmp(&similarity, &o.similarity, 4) == 0 && memcmp(&threshold, &o.threshold, 4) == 0 &&
-               memcmp(&k, &o.k, 4) == 0 && memcmp(&b, &o.b, 4) == 0;
+               memcmp(&k, &o.k, 4) == 0 && memcmp(&b, &o.b, 4) == 0 && thr == o.thr && deep == o.deep && omc_doc == o.omc_doc &&
+               omc_mult == o.omc_mult && n_omc == o.n_omc;
     }
 };
-inline BatchKey key_of(const Call &c) {
+// The vector depth of a query alone (0 without a vector part): vector_limit, else limit.
+inline uint32_t vector_depth(const oc_search_params *p) {
+    return p->mode == OC_MODE_FULLTEXT ? 0u : p->vector_limit ? p->vector_limit : p->limit;
+}
+inline BatchKey key_of(const Call &c, bool mixed = false) {
     const oc_search_params *p = c.p;
+    const Kind cls = c.kind == SORTED ? PLAIN : c.kind;
+    if (mixed)
+        return BatchKey{0, 0, 0, 0.f, 0.f, p->bm25_k, p->bm25_b, 0, cls, c.facets,
+                        p->mode != OC_MODE_VECTOR && p->threshold >= 0.0f, vector_depth(p) > TC_MAX_DEPTH,
+                        p->n_omc ? p->omc_doc_ids : nullptr, p->n_omc ? p->omc_mult : nullptr, p->n_omc};
     return BatchKey{p->mode, p->limit, p->offset, p->similarity, p->threshold, p->bm25_k, p->bm25_b, p->vector_limit,
-                    c.kind == SORTED ? PLAIN : c.kind, c.facets};
+                    cls, c.facets, false, false, nullptr, nullptr, 0};
 }
 // has_emb / has_str: the stores the batcher was created with.  A call that oc_search would reject
 // (unknown mode, missing store, NULL query arrays) is NOT batchable: it goes straight to the
 // executor so the caller gets oc_search's normal error instead of a merge that dereferences NULL.
-inline bool batchable(const oc_search_params *p, bool has_emb = true, bool has_str = true) {
-    if (p->n_queries != 1 || p->filter_bits || p->q_filters || p->n_omc != 0 || p->sharded) return false;
+// A request with its own q_params runs directly (the merged call's q_params are the requests' scalars).  mixed: OMC
+// arrays join the key instead of keeping the request out; the scalars must pass the library's bounds, which a batch
+// of equal scalars would otherwise refuse for all of its requests alike.
+inline bool batchable(const oc_search_params *p, bool has_emb = true, bool has_str = true, bool mixed = false) {
+    if (p->n_queries != 1 || p->filter_bits || p->q_filters || p->q_params || (p->n_omc != 0 && !mixed) || p->sharded) return false;
+    if (mixed && (uint64_t(p->limit) + p->offset > OC_MAX_TOPK || (p->limit && (p->vector_limit ? p->vector_limit : p->limit) > OC_MAX_TOPK)))
+        return false;
+    if (mixed && p->n_omc && (!p->omc_doc_ids || !p->omc_mult)) return false;
     if (p->mode != OC_MODE_FULLTEXT && p->mode != OC_MODE_VECTOR && p->mode != OC_MODE_HYBRID) return false;
     const bool need_v = p->mode != OC_MODE_FULLTEXT, need_ft = p->mode != OC_MODE_VECTOR;
     if (need_v && (!has_emb || !p->q_vecs)) return false;
@@ -151,6 +179,7 @@ struct MergedBatch {
     std::vector<float> scores;
     std::vector<uint32_t> n;
     std::vector<const oc_filter *> q_filters;   // [B] each query's p->filter, or empty when no query has one
+    std::vector<oc_query_params> q_params;      // [B] mixed: each query's scalars
     // sort values and items (all but PLAIN)
     std::vector<oc_sort> q_sorts;               // [B] (SORTED)
     std::vector<uint32_t> pin_off, pin_pos;     // [B + 1], [items]
@@ -171,15 +200,16 @@ struct MergedBatch {
     std::vector<oc_facet_req> f_reqs;
     std::vector<uint64_t> f_counts;
 
-    void build(const std::vector<Request *> &reqs, uint32_t dim) {
+    void build(const std::vector<Request *> &reqs, uint32_t dim, bool mixed = false) {
         const Call &f = reqs[0]->call;
-        const uint32_t B = (uint32_t)reqs.size(), L = f.p->limit;
+        const uint32_t B = (uint32_t)reqs.size();
         Kind kind = f.kind == SORTED ? PLAIN : f.kind;
         for (const Request *r : reqs) {
             const oc_sort *s = sort_of(r->call);
             if (kind == PLAIN && ((s && s->field) || pin_items(r->call.pins))) kind = SORTED;
         }
-        build_hits(reqs, dim);
+        build_hits(reqs, dim, mixed);
+        const uint32_t L = p.limit;
         call = Call{kind, &p, docs.data(), scores.data(), n.data(), count.data()};
         if (kind != PLAIN) build_pins(reqs, L);
         if (kind == SORTED) {
@@ -190,21 +220,41 @@ struct MergedBatch {
         if (kind == GROUPED || kind == FACETED) build_groups(reqs);
         if (kind == FACETED) build_facets(reqs);
     }
-    void build_hits(const std::vector<Request *> &reqs, uint32_t dim) {
+    // mixed: every query's scalars go into q_params; the merged limit is the largest (the row stride), the vectors of
+    // the queries without a vector part are zero rows (not read) and those without a text part have no token
+    void build_hits(const std::vector<Request *> &reqs, uint32_t dim, bool mixed) {
         const oc_search_params *f = reqs[0]->call.p;
         const uint32_t B = (uint32_t)reqs.size();
         p = *f;
         p.n_queries = B;
-        if (f->mode != OC_MODE_FULLTEXT) {
-            q_vecs.resize(size_t(B) * dim);
-            for (uint32_t i = 0; i < B; i++) memcpy(q_vecs.data() + size_t(i) * dim, reqs[i]->call.p->q_vecs, size_t(dim) * 4);
+        bool any_v = f->mode != OC_MODE_FULLTEXT, any_ft = f->mode != OC_MODE_VECTOR;
+        if (mixed) {
+            p.limit = 0;
+            any_v = any_ft = false;
+            for (const Request *req : reqs) {
+                const oc_search_params *r = req->call.p;
+                q_params.push_back(oc_query_params{r->mode, r->limit, r->offset, r->similarity, r->threshold, r->vector_limit});
+                p.limit = std::max(p.limit, r->limit);
+                any_v = any_v || r->mode != OC_MODE_FULLTEXT;
+                any_ft = any_ft || r->mode != OC_MODE_VECTOR;
+            }
+            p.q_params = q_params.data();
+            p.mode = any_v && any_ft ? OC_MODE_HYBRID : any_v ? OC_MODE_VECTOR : OC_MODE_FULLTEXT;
+            p.q_vecs = nullptr; p.q_token_offsets = nullptr;
+        }
+        if (any_v) {
+            q_vecs.assign(size_t(B) * dim, 0.f);
+            for (uint32_t i = 0; i < B; i++)
+                if (reqs[i]->call.p->mode != OC_MODE_FULLTEXT)
+                    memcpy(q_vecs.data() + size_t(i) * dim, reqs[i]->call.p->q_vecs, size_t(dim) * 4);
             p.q_vecs = q_vecs.data();
         }
-        if (f->mode != OC_MODE_VECTOR) {
+        if (any_ft) {
             q_token_offsets.assign(1, 0u);
             token_term_offsets.assign(1, 0u);
             for (const Request *req : reqs) {
                 const oc_search_params *r = req->call.p;
+                if (r->mode == OC_MODE_VECTOR) { q_token_offsets.push_back(q_token_offsets.back()); continue; }
                 const uint32_t t0 = r->q_token_offsets[0], t1 = r->q_token_offsets[1];
                 for (uint32_t t = t0; t < t1; t++) {
                     const uint32_t e0 = r->token_term_offsets[t], e1 = r->token_term_offsets[t + 1];
@@ -232,7 +282,7 @@ struct MergedBatch {
                 p.q_filters = q_filters.data();
                 break;
             }
-        docs.assign(size_t(B) * f->limit, 0); scores.assign(size_t(B) * f->limit, 0.f);
+        docs.assign(size_t(B) * p.limit, 0); scores.assign(size_t(B) * p.limit, 0.f);
         n.assign(B, 0); count.assign(B, 0);
     }
     void build_pins(const std::vector<Request *> &reqs, uint32_t L) {
@@ -286,15 +336,16 @@ struct MergedBatch {
             reqs[i]->rc = rc;
             if (rc != 0) continue;
             const Call &o = reqs[i]->call;
-            if (L) {   // a request at limit 0 gets no hits, as from a call of its own
-                memcpy(o.docs, docs.data() + i * L, size_t(L) * 8);
-                memcpy(o.scores, scores.data() + i * L, size_t(L) * 4);
+            const uint32_t Li = o.p->limit;   // the request's own row: the first Li entries of its row of L (mixed: L >= Li)
+            if (Li) {   // a request at limit 0 gets no hits, as from a call of its own
+                memcpy(o.docs, docs.data() + i * L, size_t(Li) * 8);
+                memcpy(o.scores, scores.data() + i * L, size_t(Li) * 4);
                 *o.n = n[i];
             }
             *o.count = count[i];
             if (o.sort_values) {   // a batch run as oc_search: score order, NaN as oc_search_q_sorted writes it
-                if (call.kind != PLAIN) memcpy(o.sort_values, sort_values.data() + i * L, size_t(L) * 8);
-                else for (uint32_t j = 0; j < L; j++) o.sort_values[j] = j < n[i] ? std::numeric_limits<double>::quiet_NaN() : 0.0;
+                if (call.kind != PLAIN) memcpy(o.sort_values, sort_values.data() + i * L, size_t(Li) * 8);
+                else for (uint32_t j = 0; j < Li; j++) o.sort_values[j] = j < n[i] ? std::numeric_limits<double>::quiet_NaN() : 0.0;
             }
             if (call.kind != PLAIN)   // the caller's item j is its entry q_pin_offsets[0] + j, as in a call of its own
                 for (uint32_t j = pin_off[i]; j < pin_off[i + 1]; j++) {
@@ -324,9 +375,10 @@ struct MergedBatch {
 template <class Exec>
 class Batcher {
 public:
-    Batcher(Exec exec, uint32_t dim, uint32_t max_batch, uint32_t max_wait_us, bool has_emb = true, bool has_str = true)
+    Batcher(Exec exec, uint32_t dim, uint32_t max_batch, uint32_t max_wait_us, bool has_emb = true, bool has_str = true,
+            bool mixed = false)
         : exec_(exec), dim_(dim), max_batch_(max_batch ? max_batch : 1), max_wait_us_(max_wait_us), has_emb_(has_emb),
-          has_str_(has_str) {}
+          has_str_(has_str), mixed_(mixed) {}
 
     // Runs r (n_groups set for a grouped or faceted request) directly or in a batch and returns its code.  A request
     // the library would refuse for its own arguments gets OC_ERR_INVALID (with *why; a refusal of the facet check sets
@@ -340,7 +392,9 @@ public:
         }
         if (c.kind == FACETED)
             if (const int rc = exec_.check(c.facets, c.facet_reqs, n_facets(c))) return rc;
-        bool merge = max_batch_ > 1 && batchable(c.p, has_emb_, has_str_);
+        bool merge = max_batch_ > 1 && batchable(c.p, has_emb_, has_str_, mixed_);
+        // mixed: a flat request at limit 0 would make the library refuse the merged call of every request with it
+        if (mixed_ && !c.q_groups && c.p->limit == 0) merge = false;
         if (c.kind == SORTED) merge = merge && pins_batchable(c.p, c.pins);
         if (c.q_groups) merge = merge && groups_batchable(c.p, c.q_groups, c.pins, n_facets(c));
         if (!merge) {
@@ -360,7 +414,7 @@ private:
     int join(Request &r) {
         std::unique_lock<std::mutex> lk(mu_);
         // one group collects at a time: wait while it is full or holds a different key
-        const BatchKey k = key_of(r.call);
+        const BatchKey k = key_of(r.call, mixed_);
         cv_slot_.wait(lk, [&] { return pending_.empty() || (pending_key_ == k && pending_.size() < max_batch_); });
         if (pending_.empty()) pending_key_ = k;
         pending_.push_back(&r);
@@ -389,7 +443,7 @@ private:
     // batch) is split in halves, down to single requests, which then get the single call's answer.
     void run(const std::vector<Request *> &reqs) {
         MergedBatch m;
-        m.build(reqs, dim_);
+        m.build(reqs, dim_, mixed_);
         const int rc = exec_(m.call);
         if (rc == OC_ERR_OOM && m.call.q_groups && reqs.size() > 1) {
             const size_t h = reqs.size() / 2;
@@ -402,7 +456,7 @@ private:
 
     Exec exec_;
     uint32_t dim_, max_batch_, max_wait_us_;
-    bool has_emb_, has_str_;
+    bool has_emb_, has_str_, mixed_;
     std::mutex mu_;
     std::condition_variable cv_slot_, cv_leader_, cv_done_;
     std::vector<Request *> pending_;

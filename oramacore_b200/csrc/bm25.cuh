@@ -1620,7 +1620,9 @@ __global__ void __launch_bounds__(256) bm25_point_kernel(const PointParams p) {
         }
     }
     if (lane == 0) {
-        const bool present = ok && (p.threshold ? (mask != 0u && uint32_t(__popc(mask)) >= qd.required) : score != 0.f);
+        // the query's own threshold mode (a batch with per-query parameters mixes queries with and without one)
+        const bool thr = p.threshold && (qd.flags & QF_THRESHOLD);
+        const bool present = ok && (thr ? (mask != 0u && uint32_t(__popc(mask)) >= qd.required) : score != 0.f);
         p.v_ft[wid] = present ? score : 0.f;
         p.v_present[wid] = present ? 1 : 0;
     }

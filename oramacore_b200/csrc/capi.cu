@@ -182,6 +182,12 @@ struct oc_ctx {
     DevBuf e_rowbits, r_slot;
     const uint32_t *v_rowbits = nullptr; uint64_t v_row_words = 0;
     std::vector<uint32_t> v_qslot;
+    // per-query parameters (q_params): the vector stage sweeps the sub-batch of queries with a vector part, each cut to
+    // its own depth (v_qlim) and similarity (v_qsim); v_qmap: the batch query of each sub-batch query (empty: the
+    // whole batch).  vq_*: the sub-batch's hits before they are scattered to their queries' rows.
+    std::vector<uint32_t> v_qlim, v_qmap;
+    std::vector<float> v_qsim;
+    DevBuf vq_doc, vq_score, vq_row, vq_cnt, vq_raw, r_lim, r_sim;
 
     HostBuf h_in, h_out, h_in0;   // h_in0 / in_blob0: query vectors + filter, uploaded before the descriptors
     OcComm comm;
@@ -526,9 +532,11 @@ static ScanPlan plan_scan(const oc_ctx *c, const oc_emb *e, uint32_t n_keep) {
 // ---- exact sweeps (K1) + merge for nq prepared queries; results into the given buffers
 struct VecOut { uint64_t *doc; float *score; uint32_t *row; uint32_t *cnt; float *raw; };
 // row_bits / q_slot: per-query where-filters (ScanParams), or NULL
+// q_lim / q_sim: per-query depth and similarity (ScanMergeParams), or NULL
 static int run_exact_sweeps(oc_ctx *c, oc_emb *e, const float *inv_norm, const float *qpad, const float *qinv,
                             uint32_t nq, uint32_t limit, float similarity, const VecOut &o,
-                            const uint32_t *row_bits = nullptr, uint64_t row_words = 0, const uint32_t *q_slot = nullptr) {
+                            const uint32_t *row_bits = nullptr, uint64_t row_words = 0, const uint32_t *q_slot = nullptr,
+                            const uint32_t *q_lim = nullptr, const float *q_sim = nullptr) {
     ScanPlan pl = plan_scan(c, e, limit);
     if (pl.n_stages < 2) return fail(OC_ERR_UNSUPPORTED, "limit %u leaves no shared memory for the scan ring", limit);
     OCTRY(c->scan_cand.ensure(size_t(nq) * pl.grid * limit * 8));
@@ -557,6 +565,7 @@ static int run_exact_sweeps(oc_ctx *c, oc_emb *e, const float *inv_norm, const f
     mp.capb = std::max<uint32_t>(2048, next_pow2(2 * limit));
     mp.row_doc_ids = e->row_doc; mp.rescale_e5 = e->e5; mp.similarity = similarity;
     mp.out_doc = o.doc; mp.out_score = o.score; mp.out_row = o.row; mp.out_count = o.cnt; mp.out_raw = o.raw;
+    mp.q_limit = q_lim; mp.q_sim = q_sim;
     if (smem_cfg_needed(c->device, (const void *)emb_scan_merge_kernel, size_t(mp.capb) * 8))
         CU(cudaFuncSetAttribute(emb_scan_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(mp.capb * 8)));
     emb_scan_merge_kernel<<<nq, 256, mp.capb * 8, c->stream>>>(mp);
@@ -586,9 +595,11 @@ struct QFilterJob {
 
 // Runs prep + (tensor-core batched scan | exact sweeps) + merge for B queries already in device
 // memory (q_dev: B x dim).  Leaves hits in c->v_doc / v_score / v_row / v_cnt / v_raw ([B][limit]).
-// qf: per-query where-filters (device tables uploaded), or NULL.
+// qf: per-query where-filters (device tables uploaded), or NULL.  q_lim / q_sim: per-query depth (<= limit) and
+// similarity, or NULL.
 static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B, uint32_t limit, float similarity,
-                            const uint64_t *filter_dev, uint64_t filter_nbits, const QFilterJob *qf = nullptr) {
+                            const uint64_t *filter_dev, uint64_t filter_nbits, const QFilterJob *qf = nullptr,
+                            const uint32_t *q_lim = nullptr, const float *q_sim = nullptr) {
     OCTRY(c->v_doc.ensure(size_t(B) * limit * 8));
     OCTRY(c->v_score.ensure(size_t(B) * limit * 4));
     OCTRY(c->v_row.ensure(size_t(B) * limit * 4));
@@ -642,7 +653,7 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
     CU(cudaEventRecord(c->ev[EV_SCAN0], c->stream));
     if (!use_gemm)
         return run_exact_sweeps(c, e, inv_norm, c->q_pad.as<float>(), c->q_inv.as<float>(), B, limit, similarity, out, row_bits,
-                                row_words, qf ? qf->d_q_slot : nullptr);
+                                row_words, qf ? qf->d_q_slot : nullptr, q_lim, q_sim);
 
     // ---------------- K2: wgmma batched scan ----------------
     const bool bf16 = e->esz == 2;
@@ -767,6 +778,7 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
     mp.inv_qnorm = c->q_inv.as<float>(); mp.row_doc_ids = e->row_doc; mp.rescale_e5 = e->e5; mp.similarity = similarity;
     mp.out_doc = out.doc; mp.out_score = out.score; mp.out_row = out.row; mp.out_count = out.cnt; mp.out_raw = out.raw;
     mp.out_unproven = c->g_flag.as<uint8_t>(); mp.out_rescored = c->g_resc.as<uint32_t>();
+    mp.q_limit = q_lim; mp.q_sim = q_sim;
     emb_gemm_merge_kernel<<<B, 512, gemm_merge_smem_bytes(), c->stream>>>(mp);
     launched(c);
     CU(cudaGetLastError());
@@ -802,16 +814,29 @@ static int fix_unproven(oc_ctx *c, oc_emb *e, const uint8_t *flags, uint32_t B, 
                            size_t(e->stride) * 4, cudaMemcpyDeviceToDevice, c->stream));
         CU(cudaMemcpyAsync(c->r_qinv.as<float>() + i, c->q_inv.as<float>() + redo[i], 4, cudaMemcpyDeviceToDevice, c->stream));
     }
-    CU(cudaMemcpyAsync(c->r_map.p, redo.data(), size_t(nr) * 4, cudaMemcpyHostToDevice, c->stream));
+    // the slot a redone query's result goes to: its batch row (a sub-batch of per-query parameters scattered its hits there)
+    std::vector<uint32_t> rmap(redo);
+    if (!c->v_qmap.empty()) for (uint32_t &q : rmap) q = c->v_qmap[q];
+    CU(cudaMemcpyAsync(c->r_map.p, rmap.data(), size_t(nr) * 4, cudaMemcpyHostToDevice, c->stream));
     std::vector<uint32_t> rslot;   // per-query where-filters: each redone query keeps its own slot
     if (c->v_rowbits) {
         for (uint32_t q : redo) rslot.push_back(c->v_qslot[q]);
         OCTRY(c->r_slot.ensure(size_t(nr) * 4));
         CU(cudaMemcpyAsync(c->r_slot.p, rslot.data(), size_t(nr) * 4, cudaMemcpyHostToDevice, c->stream));
     }
+    std::vector<uint32_t> rlim;    // per-query parameters: each redone query keeps its own depth and similarity
+    std::vector<float> rsim;
+    if (!c->v_qlim.empty()) {
+        for (uint32_t q : redo) { rlim.push_back(c->v_qlim[q]); rsim.push_back(c->v_qsim[q]); }
+        OCTRY(c->r_lim.ensure(size_t(nr) * 4));
+        OCTRY(c->r_sim.ensure(size_t(nr) * 4));
+        CU(cudaMemcpyAsync(c->r_lim.p, rlim.data(), size_t(nr) * 4, cudaMemcpyHostToDevice, c->stream));
+        CU(cudaMemcpyAsync(c->r_sim.p, rsim.data(), size_t(nr) * 4, cudaMemcpyHostToDevice, c->stream));
+    }
     VecOut ro{c->r_doc.as<uint64_t>(), c->r_score.as<float>(), c->r_row.as<uint32_t>(), c->r_cnt.as<uint32_t>(), c->r_raw.as<float>()};
     OCTRY(run_exact_sweeps(c, e, inv_norm, c->r_qpad.as<float>(), c->r_qinv.as<float>(), nr, limit, similarity, ro, c->v_rowbits,
-                           c->v_row_words, c->v_rowbits ? c->r_slot.as<uint32_t>() : nullptr));
+                           c->v_row_words, c->v_rowbits ? c->r_slot.as<uint32_t>() : nullptr,
+                           rlim.empty() ? nullptr : c->r_lim.as<uint32_t>(), rsim.empty() ? nullptr : c->r_sim.as<float>()));
     scatter_rows_kernel<<<nr, 64, 0, c->stream>>>(c->r_map.as<uint32_t>(), nr, limit, ro.doc, ro.score, ro.row, ro.cnt, ro.raw,
                                                    out.doc, out.score, out.row, out.cnt, out.raw);
     launched(c);
@@ -823,6 +848,7 @@ static int fix_unproven(oc_ctx *c, oc_emb *e, const uint8_t *flags, uint32_t B, 
 static void begin_call(oc_ctx *c) {
     c->call_launches = 0; c->call_scan_launches = 0; c->gemm_pending = false; c->sweep_timed = false; c->rerun_timed = false;
     c->v_rowbits = nullptr; c->v_row_words = 0;
+    c->v_qlim.clear(); c->v_qsim.clear(); c->v_qmap.clear();
     memset(&c->timing, 0, sizeof(c->timing));
 }
 static int finish_timing(oc_ctx *c, bool scan, bool bm, bool fuse, bool comm) {
@@ -1945,7 +1971,7 @@ static int sort_rows_for(oc_ctx *c, SortOrder &o, const std::shared_ptr<StrSnap>
 }
 
 static int run_groups(oc_ctx *c, const GroupJob &gj, int mode, const StrSnap *S, uint32_t n_tiles, uint32_t vlimit,
-                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, const PinJob &pj);
+                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, const PinJob &pj, const QueryPlan *q_plan);
 
 // One search as an entry point asks for it.  fj: the facet counts.  gj: the grouped calls (always with pj); then
 // limit == 0 is allowed: the hits are not written (out_doc_ids / out_scores / out_n may be NULL), the vector stage gets
@@ -1962,6 +1988,7 @@ struct SearchReq {
     PinJob *pj = nullptr;
     const SortJob *sj = nullptr;
     bool q_filters_ok = false;           // the entry point takes per-query filters (p->q_filters)
+    bool q_params_ok = false;            // ... and per-query parameters (p->q_params)
 };
 
 // What one search derives once, filled in by the stages of search_impl in order.
@@ -1970,8 +1997,23 @@ struct SearchCall {
     const SearchReq &r;
     const oc_search_params *p;
     SearchCall(oc_ctx *c_, oc_emb *e, oc_str *s, const SearchReq &r_) : c(c_), emb(e), str(s), r(r_), p(r_.p) {}
-    // shape and path
+    // shape and path.  mode: p->mode, or with per-query parameters the union of the entries' parts
     uint32_t B = 0, limit = 0, n_keep = 0, vlimit = 0, cap = 0, sort_top = 0;
+    int mode = OC_MODE_FULLTEXT;
+    // per-query parameters (p->q_params): K4's plan and the page of each query, the largest offset + limit, and the
+    // sub-batch of queries with a vector part with each one's depth and similarity (v_rows: their packed vectors,
+    // vqf: their filter slots, when the sub-batch is not the whole batch).  Bv: the queries the vector stage sweeps.
+    bool qp = false;
+    uint32_t page_max = 0, Bv = 0;
+    std::vector<QueryPlan> q_plan;
+    std::vector<uint2> q_page;
+    std::vector<uint32_t> v_sub, v_lim;
+    std::vector<float> v_sim, v_rows;
+    QFilterJob vqf;
+    Slot<QueryPlan> s_plan;
+    Slot<uint2> s_page;
+    Slot<uint32_t> s_vsub, s_vlim, s_vqslot;
+    Slot<float> s_vsim;
     bool has_v = false, has_ft = false, per_q = false, facets = false, write_hits = false, pin_flat = false, sort_flat = false;
     bool k4_top = false, exports = false, pin_items = false, side = false;
     // inputs; filter_h: the filter is a host bitmap, uploaded with this call
@@ -2096,6 +2138,47 @@ static int qfilter_plan(SearchCall &k) {
     return OC_OK;
 }
 
+// Per-query parameters: each entry gets the checks its scalars get alone, and the table of what every stage does for it.
+// The batch runs at the largest depths: n_keep = the largest (limit + offset) x (2 for an active pinned query), the
+// vector depth = the largest of the vector entries' own depths, sort_top = the largest top_count.
+static int qparams_plan(SearchCall &k) {
+    const SearchReq &r = k.r; const oc_search_params *p = k.p;
+    const PinJob *pj = r.pj;
+    const bool limit0_ok = r.gj || (r.fj && r.fj->hits_optional);   // (oc_search_q_groups checks the queries without groups)
+    k.q_page.resize(k.B);
+    k.sort_top = 0;
+    for (uint32_t b = 0; b < k.B; b++) {
+        const oc_query_params &e = p->q_params[b];
+        if (e.limit > p->limit) return fail(OC_ERR_INVALID, "q_params[%u]: limit %u > p->limit %u (the row stride)", b, e.limit, p->limit);
+        if (e.limit == 0 && !limit0_ok) return fail(OC_ERR_INVALID, "q_params[%u]: limit must be >= 1", b);
+        const bool hits = k.write_hits && e.limit > 0;   // as alone: limit 0 writes no hit and gives the vector stage depth 0
+        const uint32_t lim = hits ? e.limit : 1;
+        const bool active = pj && pj->splice && pj->cnt[b] > 0;
+        if (active && (uint64_t(e.limit) + e.offset) * 2 > OC_MAX_TOPK)
+            return fail(OC_ERR_UNSUPPORTED, "q_params[%u]: pins: 2 x (limit+offset) %llu > %u", b,
+                        (unsigned long long)(uint64_t(e.limit) + e.offset) * 2, OC_MAX_TOPK);
+        const uint64_t nk = (uint64_t(lim) + e.offset) * (active && hits ? 2 : 1);
+        if (nk > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "q_params[%u]: limit+offset %llu > %u", b, (unsigned long long)nk, OC_MAX_TOPK);
+        const uint32_t vl = !hits ? 0u : e.vector_limit ? e.vector_limit : e.limit;
+        if (vl > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "q_params[%u]: vector_limit %u > %u", b, vl, OC_MAX_TOPK);
+        const uint32_t page_lim = hits ? e.limit : 0u;
+        k.q_page[b] = make_uint2(e.offset, page_lim);
+        QueryPlan &qp = k.q_plan[b];
+        qp.n_keep = (uint32_t)nk;
+        qp.limit = k.k4_top ? qp.n_keep : page_lim;     // a splice pages K4's whole top n_keep afterwards
+        qp.offset = k.k4_top ? 0u : e.offset;
+        k.n_keep = std::max(k.n_keep, qp.n_keep);
+        k.page_max = std::max(k.page_max, e.offset + page_lim);
+        if (k.sort_flat) k.sort_top = std::max(k.sort_top, uint32_t((uint64_t(page_lim) + e.offset) * (active ? 2 : 1)));
+        if (qp.mode != OC_MODE_FULLTEXT) {
+            k.v_sub.push_back(b); k.v_lim.push_back(vl); k.v_sim.push_back(e.similarity);
+            k.vlimit = std::max(k.vlimit, vl);
+        }
+    }
+    if (k.sort_flat) k.sort_top = std::max(k.sort_top, 1u);
+    return OC_OK;
+}
+
 // The checks that need no device, and the call's shape and path.  B == 0 stops here.
 static int search_check(SearchCall &k) {
     oc_ctx *c = k.c; const SearchReq &r = k.r;
@@ -2104,10 +2187,29 @@ static int search_check(SearchCall &k) {
     k.write_hits = !(r.gj || (r.fj && r.fj->hits_optional)) || p->limit > 0;
     if (k.write_hits && (!r.out_doc_ids || !r.out_scores || !r.out_n)) return fail(OC_ERR_INVALID, "NULL argument");
     const uint32_t B = k.B = p->n_queries;
+    k.qp = p->q_params != nullptr;
+    if (k.qp && !r.q_params_ok)
+        return fail(OC_ERR_UNSUPPORTED, "q_params: per-query parameters are supported by oc_search, oc_search_q_sorted, "
+                                        "oc_search_q_groups and oc_search_q_facets only");
+    if (k.qp && p->sharded) return fail(OC_ERR_UNSUPPORTED, "q_params over a sharded search");
     if (B == 0) return OC_OK;
-    k.has_v = p->mode == OC_MODE_VECTOR || p->mode == OC_MODE_HYBRID;
-    k.has_ft = p->mode == OC_MODE_FULLTEXT || p->mode == OC_MODE_HYBRID;
-    if (!k.has_v && !k.has_ft) return fail(OC_ERR_INVALID, "unknown mode %d", p->mode);
+    if (k.qp) {   // each entry's mode; the batch has the union of their parts
+        k.q_plan.resize(B);
+        for (uint32_t b = 0; b < B; b++) {
+            const int m = p->q_params[b].mode;
+            if (m != OC_MODE_FULLTEXT && m != OC_MODE_VECTOR && m != OC_MODE_HYBRID)
+                return fail(OC_ERR_INVALID, "q_params[%u]: unknown mode %d", b, m);
+            k.q_plan[b].mode = m;
+            k.has_v = k.has_v || m != OC_MODE_FULLTEXT;
+            k.has_ft = k.has_ft || m != OC_MODE_VECTOR;
+        }
+        k.mode = k.has_v && k.has_ft ? OC_MODE_HYBRID : k.has_v ? OC_MODE_VECTOR : OC_MODE_FULLTEXT;
+    } else {
+        k.has_v = p->mode == OC_MODE_VECTOR || p->mode == OC_MODE_HYBRID;
+        k.has_ft = p->mode == OC_MODE_FULLTEXT || p->mode == OC_MODE_HYBRID;
+        if (!k.has_v && !k.has_ft) return fail(OC_ERR_INVALID, "unknown mode %d", p->mode);
+        k.mode = p->mode;
+    }
     if (k.has_v && (!k.emb || !p->q_vecs)) return fail(OC_ERR_INVALID, "vector/hybrid mode needs emb and q_vecs");
     if (k.has_ft && (!k.str || !p->q_token_offsets)) return fail(OC_ERR_INVALID, "fulltext/hybrid mode needs str and tokens");
     if (k.emb && k.emb->ctx != c) return fail(OC_ERR_INVALID, "emb belongs to another ctx");
@@ -2127,12 +2229,16 @@ static int search_check(SearchCall &k) {
     if (k.sort_flat && sj->by_score && pj->splice)
         for (uint32_t q = 0; q < B; q++) score_active = score_active || (sj->q_ent[q] == SORT_BY_SCORE && pj->cnt[q] > 0);
     k.k4_top = k.pin_flat || (k.sort_flat && sj->by_score);   // K4 writes its top n_keep (offset 0) for a splice
-    const uint64_t n_keep64 = (uint64_t(limit) + p->offset) * (k.pin_flat || score_active ? 2 : 1);
-    if (n_keep64 > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "limit+offset %llu > %u", (unsigned long long)n_keep64, OC_MAX_TOPK);
-    k.n_keep = (uint32_t)n_keep64;
-    // limit_hint = limit, NOT limit+offset (search.rs:330-336); vector_limit lets a multi-index caller keep that depth
-    k.vlimit = !k.write_hits ? 0u : p->vector_limit ? p->vector_limit : limit;
-    if (k.vlimit > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "vector_limit %u > %u", k.vlimit, OC_MAX_TOPK);
+    if (k.qp) {
+        OCTRY(qparams_plan(k));
+    } else {
+        const uint64_t n_keep64 = (uint64_t(limit) + p->offset) * (k.pin_flat || score_active ? 2 : 1);
+        if (n_keep64 > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "limit+offset %llu > %u", (unsigned long long)n_keep64, OC_MAX_TOPK);
+        k.n_keep = (uint32_t)n_keep64;
+        // limit_hint = limit, NOT limit+offset (search.rs:330-336); vector_limit lets a multi-index caller keep that depth
+        k.vlimit = !k.write_hits ? 0u : p->vector_limit ? p->vector_limit : limit;
+        if (k.vlimit > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "vector_limit %u > %u", k.vlimit, OC_MAX_TOPK);
+    }
     if (p->sharded && !c->comm.ready()) return fail(OC_ERR_COMM, "sharded search without oc_comm_init");
     k.exports = r.gj || pj || sj;   // K4 exports the normalisation and the vector part of the score map
     k.pin_items = pj && pj->stride;
@@ -2163,6 +2269,32 @@ static void bind_first_tables(SearchCall &k) {
     k.fpl.d_pairs = k.s_fpairs.at(b);
 }
 
+static void swap_buf(DevBuf &a, DevBuf &b) { std::swap(a.p, b.p); std::swap(a.cap, b.cap); }
+
+// The sub-batch's vector hits ([Bv][vlimit] in c->v_*) to their queries' rows of [B][vlimit]; a query without a vector
+// part gets no hit.  The buffers are swapped afterwards, so every later stage reads c->v_* in the batch's layout, and
+// fix_unproven patches the batch rows through c->v_qmap.
+static int scatter_sub_hits(SearchCall &k) {
+    oc_ctx *c = k.c;
+    const size_t n = size_t(k.B) * k.vlimit;
+    OCTRY(c->vq_doc.ensure(n * 8));
+    OCTRY(c->vq_score.ensure(n * 4));
+    OCTRY(c->vq_row.ensure(n * 4));
+    OCTRY(c->vq_cnt.ensure(size_t(k.B) * 4));
+    OCTRY(c->vq_raw.ensure(n * 4));
+    CU(cudaMemsetAsync(c->vq_cnt.p, 0, size_t(k.B) * 4, c->stream));
+    scatter_rows_kernel<<<k.Bv, 64, 0, c->stream>>>(k.s_vsub.at(c->in_blob0), k.Bv, k.vlimit, c->v_doc.as<uint64_t>(), c->v_score.as<float>(),
+                                                    c->v_row.as<uint32_t>(), c->v_cnt.as<uint32_t>(), c->v_raw.as<float>(),
+                                                    c->vq_doc.as<uint64_t>(), c->vq_score.as<float>(), c->vq_row.as<uint32_t>(),
+                                                    c->vq_cnt.as<uint32_t>(), c->vq_raw.as<float>());
+    launched(c);
+    CU(cudaGetLastError());
+    swap_buf(c->v_doc, c->vq_doc); swap_buf(c->v_score, c->vq_score); swap_buf(c->v_row, c->vq_row);
+    swap_buf(c->v_cnt, c->vq_cnt); swap_buf(c->v_raw, c->vq_raw);
+    c->v_qmap = k.v_sub;
+    return OC_OK;
+}
+
 // Vector stage first: the query vectors (+ filter) go up alone and the matrix sweep starts; the host-side descriptor
 // work of the next stages overlaps it.
 static int vector_first(SearchCall &k) {
@@ -2176,18 +2308,47 @@ static int vector_first(SearchCall &k) {
     k.filter_dev = k.batch_filter ? k.batch_filter->bits : nullptr;
     k.first = k.has_v ? &k.pk0 : &k.pk;
     k.first_blob = k.has_v ? &c->in_blob0 : &c->in_blob;
+    // per-query parameters: the vector stage sweeps the sub-batch of queries with a vector part (their rows packed when it
+    // is not the whole batch), each with its own depth and similarity
+    k.Bv = k.qp ? (uint32_t)k.v_sub.size() : B;
+    const bool sub = k.Bv < B;
     Slot<float> s_qv;
-    if (k.has_v) s_qv = k.pk0.add(p->q_vecs, size_t(B) * k.emb->dim, is_pinned_host(p->q_vecs));
+    if (k.has_v && sub) {
+        const size_t dim = k.emb->dim;
+        k.v_rows.resize(size_t(k.Bv) * dim);
+        for (uint32_t i = 0; i < k.Bv; i++) memcpy(k.v_rows.data() + i * dim, p->q_vecs + size_t(k.v_sub[i]) * dim, dim * 4);
+        s_qv = k.pk0.add(k.v_rows.data(), k.v_rows.size());
+    } else if (k.has_v) {
+        s_qv = k.pk0.add(p->q_vecs, size_t(B) * k.emb->dim, is_pinned_host(p->q_vecs));
+    }
     if (k.filter_h) k.s_flt = k.first->add(p->filter_bits, k.fwords);
     if (!k.has_v) return OC_OK;
     add_first_tables(k);
+    if (k.qp) {
+        k.s_vlim = k.pk0.add(k.v_lim.data(), k.Bv);
+        k.s_vsim = k.pk0.add(k.v_sim.data(), k.Bv);
+        if (sub) k.s_vsub = k.pk0.add(k.v_sub.data(), k.Bv);
+        if (sub && k.per_q) {   // the sub-batch's filter slots
+            for (uint32_t b : k.v_sub) k.vqf.q_slot.push_back(k.qfj.q_slot[b]);
+            k.s_vqslot = k.pk0.add(k.vqf.q_slot.data(), k.Bv);
+        }
+    }
     CU(cudaEventRecord(c->ev[EV_START], c->stream));
     OCTRY(upload(k.pk0, c->h_in0, c->in_blob0, c->stream));
     CU(cudaEventRecord(c->ev[EV_H2D], c->stream));
     bind_first_tables(k);
     if (k.vlimit) {
-        OCTRY(run_vector_stage(c, k.emb, s_qv.at(c->in_blob0), B, k.vlimit, p->similarity, k.filter_dev, k.filter_nbits,
-                               k.per_q ? &k.qfj : nullptr));
+        const QFilterJob *qf = k.per_q ? &k.qfj : nullptr;
+        if (sub && k.per_q) {
+            k.vqf.slots = k.qfj.slots;
+            k.vqf.d_slots = k.qfj.d_slots;
+            k.vqf.d_q_slot = k.s_vqslot.at(c->in_blob0);
+            qf = &k.vqf;
+        }
+        OCTRY(run_vector_stage(c, k.emb, s_qv.at(c->in_blob0), k.Bv, k.vlimit, p->similarity, k.filter_dev, k.filter_nbits, qf,
+                               k.s_vlim.at(c->in_blob0), k.s_vsim.at(c->in_blob0)));
+        if (k.qp) { c->v_qlim = k.v_lim; c->v_qsim = k.v_sim; }
+        if (sub) OCTRY(scatter_sub_hits(k));
     } else {   // limit_hint 0 (groups only): no vector hit
         OCTRY(c->v_cnt.ensure(size_t(B) * 4));
         CU(cudaMemsetAsync(c->v_cnt.p, 0, size_t(B) * 4, c->stream));
@@ -2321,6 +2482,10 @@ static int ft_descriptors(SearchCall &k) {
     // commit dropped the table — from counting + all-reduce.  A shard-local list length is never a corpus df.
     k.count_df = k.multi_rank && (p->sharded & OC_SHARD_COUNT_DF) != 0;
     k.thr = p->threshold >= 0.0f;
+    if (k.qp) {   // per-query parameters: the threshold scorer when some query with a text part has a threshold
+        k.thr = false;
+        for (uint32_t q = 0; q < B; q++) k.thr = k.thr || (k.q_plan[q].mode != OC_MODE_VECTOR && p->q_params[q].threshold >= 0.0f);
+    }
     if (!k.has_ft) return OC_OK;
     bool df_local_only = false;
     for (auto &f : S->fields)   // streamed posting format depends on (avg_field_len, b): derive once
@@ -2340,14 +2505,18 @@ static int ft_descriptors(SearchCall &k) {
     // under the tombstone-only row bitmap (slot K), so it scores exactly the rows it would score alone.
     if (k.per_q) k.need_df = true;
     for (uint32_t q = 0; q < B; q++) {
-        const uint32_t t0 = p->q_token_offsets[q], t1 = p->q_token_offsets[q + 1];
+        // per-query parameters: a vector query has no token, a query's threshold is its own
+        const bool text = !k.qp || k.q_plan[q].mode != OC_MODE_VECTOR;
+        const uint32_t t0 = text ? p->q_token_offsets[q] : 0, t1 = text ? p->q_token_offsets[q + 1] : 0;
+        const float threshold = k.qp ? p->q_params[q].threshold : p->threshold;
+        const bool thr = k.qp ? text && threshold >= 0.0f : k.thr;
         const bool q_filter = k.filter || (k.per_q && k.qfj.q_slot[q] != SLOT_NONE);
         QueryDesc qd{};
         qd.token_begin = (uint32_t)k.tokens.size();
         const uint32_t ntok = t1 - t0;
         k.max_tokens = std::max(k.max_tokens, ntok);
-        qd.required = k.thr ? (uint32_t)floorf((float)ntok * p->threshold) : 0;  // token_score.rs:211-218
-        qd.flags = k.thr ? QF_THRESHOLD : 0;
+        qd.required = thr ? (uint32_t)floorf((float)ntok * threshold) : 0;  // token_score.rs:211-218
+        qd.flags = thr ? QF_THRESHOLD : 0;
         for (uint32_t t = t0; t < t1; t++) {
             TokenDesc tk{};
             tk.term_begin = (uint32_t)k.terms.size();
@@ -2434,7 +2603,8 @@ static void sort_group_plan(SearchCall &k) {
         k.s_alt.resize(B);
         for (uint32_t q = 0; q < B; q++) {
             const bool active = pj->splice && pj->cnt[q] > 0;
-            k.s_q[q] = SortQuery{sj->q_ent[q], uint32_t((uint64_t(k.limit) + k.p->offset) * (active ? 2 : 1))};
+            const uint64_t page = k.qp ? uint64_t(k.q_page[q].y) + k.q_page[q].x : uint64_t(k.limit) + k.p->offset;
+            k.s_q[q] = SortQuery{sj->q_ent[q], uint32_t(page * (active ? 2 : 1))};
             k.s_alt[q] = sj->q_ent[q] == SORT_BY_SCORE;
         }
     }
@@ -2501,6 +2671,10 @@ static int main_upload(SearchCall &k) {
     }
     if (k.sort_flat) k.s_sq = pk.add(k.s_q.data(), k.s_q.size());
     if (k.sort_flat && sj->by_score) k.s_salt = pk.add(k.s_alt.data(), k.s_alt.size());
+    if (k.qp) {
+        k.s_plan = pk.add(k.q_plan.data(), B);
+        k.s_page = pk.add(k.q_page.data(), B);
+    }
     // hybrid: the descriptors, the shared-contribution precompute, the filter bitmap and the (term, tile) plan do
     // not depend on the vector results: they run on the side stream while the main stream sweeps the matrix
     // (OC_SIDE_STREAM=0 disables it: the step gets ~2.5 % longer, the sweep itself ~4 % shorter — A/B switch)
@@ -2698,6 +2872,7 @@ static void pin_scores(SearchCall &k, uint32_t stride, const uint64_t *doc, cons
     sp.v_doc = fp.out_vdoc; sp.v_score = fp.out_vscore; sp.v_n = fp.out_vn; sp.v_stride = std::max<uint32_t>(k.vlimit, 1);
     sp.omc_doc = fp.omc_doc; sp.omc_mult = fp.omc_mult; sp.n_omc = k.n_omc;
     sp.out_score = out_score; sp.out_present = out_present;
+    sp.q_plan = k.s_plan.at(k.c->in_blob);
     pin_score_kernel<<<(unsigned)((uint64_t(k.B) * stride * 32 + 255) / 256), 256, 0, k.c->stream>>>(sp);
     launched(k.c);
 }
@@ -2728,7 +2903,8 @@ static int pin_tail(SearchCall &k) {
         xp.n_top = k.n_keep; xp.limit = k.limit; xp.offset = k.p->offset;
         xp.top_doc = c->pin_top_doc.as<uint64_t>(); xp.top_score = c->pin_top_score.as<float>(); xp.top_n = c->pin_top_n.as<uint32_t>();
         xp.out_doc = k.d_doc; xp.out_score = k.d_score; xp.out_n = k.d_n;
-        const size_t smem = pin_splice_smem(xp.kp2, k.n_keep, k.limit + k.p->offset);
+        xp.q_page = k.s_page.at(c->in_blob);
+        const size_t smem = pin_splice_smem(xp.kp2, k.n_keep, k.qp ? k.page_max : k.limit + k.p->offset);
         pin_splice_kernel<<<B, PIN_THREADS, smem, c->stream>>>(xp);
         launched(c);
     }
@@ -2787,7 +2963,8 @@ static int sort_tail(SearchCall &k) {
         xp.q_alt = k.s_salt.at(din); xp.alt_n_top = n_keep;
         xp.alt_doc = c->pin_top_doc.as<uint64_t>(); xp.alt_score = c->pin_top_score.as<float>(); xp.alt_n = c->pin_top_n.as<uint32_t>();
     }
-    pin_splice_kernel<<<B, PIN_THREADS, pin_splice_smem(xp.kp2, sj->by_score ? std::max(top, n_keep) : top, limit + offset),
+    xp.q_page = k.s_page.at(din);
+    pin_splice_kernel<<<B, PIN_THREADS, pin_splice_smem(xp.kp2, sj->by_score ? std::max(top, n_keep) : top, k.qp ? k.page_max : limit + offset),
                         c->stream>>>(xp);
     launched(c);
     CU(cudaGetLastError());
@@ -2824,7 +3001,8 @@ static int device_tail(SearchCall &k) {
     }
     FuseParams &fp = k.fp;
     fp = FuseParams{};
-    fp.mode = p->mode; fp.n_tiles = k.n_tiles; fp.n_keep = n_keep; fp.limit = k.limit; fp.offset = p->offset;
+    fp.mode = k.mode; fp.n_tiles = k.n_tiles; fp.n_keep = n_keep; fp.limit = k.limit; fp.offset = p->offset;
+    fp.q_plan = k.s_plan.at(c->in_blob);
     {   // smallest power-of-two key buffer that takes the candidates in one round (sort cost ~ capb log^2 capb)
         const uint64_t total = (has_ft ? uint64_t(k.n_tiles) * n_keep : 0) + (has_v ? vlimit : 0);
         // up to 16 K keys (128 KB) stay in shared memory and go through one radix select; the streaming bitonic path behind
@@ -2889,9 +3067,9 @@ static int rerun_checks(SearchCall &k) {
     const uint32_t B = k.B; uint8_t *h = c->h_out.as<uint8_t>();
     CU(cudaEventRecord(c->ev[EV_DEV], c->stream));
     CU(cudaMemcpyAsync(h, k.dout, k.out_bytes, cudaMemcpyDeviceToHost, c->stream));
-    if (c->gemm_pending) {
-        CU(cudaMemcpyAsync(h + k.out_bytes, c->g_flag.p, k.B, cudaMemcpyDeviceToHost, c->stream));
-        CU(cudaMemcpyAsync(h + k.o_resc, c->g_resc.p, size_t(k.B) * 4, cudaMemcpyDeviceToHost, c->stream));
+    if (c->gemm_pending) {   // (per the Bv queries the vector stage swept)
+        CU(cudaMemcpyAsync(h + k.out_bytes, c->g_flag.p, k.Bv, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaMemcpyAsync(h + k.o_resc, c->g_resc.p, size_t(k.Bv) * 4, cudaMemcpyDeviceToHost, c->stream));
     }
     CU(cudaEventRecord(c->ev[EV_D2H], c->stream));
     CU(cudaStreamSynchronize(c->stream));
@@ -2904,10 +3082,11 @@ static int rerun_checks(SearchCall &k) {
         uint32_t redone = 0;
         if (c->gemm_pending || rerun) CU(cudaEventRecord(c->ev[EV_RR0], c->stream));
         if (c->gemm_pending) {
+            const uint32_t Bv = k.Bv;
             uint64_t resc = 0;
-            for (uint32_t q = 0; q < B; q++) resc += reinterpret_cast<const uint32_t *>(h + k.o_resc)[q];
-            c->timing.scan_rescored = (uint32_t)(resc / B);
-            OCTRY(fix_unproven(c, k.emb, h + k.out_bytes, B, k.vlimit, p->similarity, &redone));
+            for (uint32_t q = 0; q < Bv; q++) resc += reinterpret_cast<const uint32_t *>(h + k.o_resc)[q];
+            c->timing.scan_rescored = (uint32_t)(resc / Bv);
+            OCTRY(fix_unproven(c, k.emb, h + k.out_bytes, Bv, k.vlimit, p->similarity, &redone));
         }
         if (redone || rerun) {
             c->gemm_pending = false;
@@ -2921,8 +3100,14 @@ static int rerun_checks(SearchCall &k) {
     // rank-proxy validation: with OMC multipliers the tile ranking assumed min == min_hint (0);
     // a negative global min changes the order of (ft - min) * omc -> rerun with the real min.
     // The hybrid point lookups do not depend on the tiles: they are not redone.
-    if (!k.did_comm && p->mode == OC_MODE_HYBRID && k.omc_tile && k.n_tiles) {
+    if (!k.did_comm && k.mode == OC_MODE_HYBRID && k.omc_tile && k.n_tiles) {
         const float *mins = reinterpret_cast<const float *>(h + k.o_min);
+        std::vector<float> hyb_mins;   // per-query parameters: only the hybrid queries rank by (ft - min)
+        if (k.qp) {
+            hyb_mins.assign(mins, mins + B);
+            for (uint32_t q = 0; q < B; q++) if (k.q_plan[q].mode != OC_MODE_HYBRID) hyb_mins[q] = 0.f;
+            mins = hyb_mins.data();
+        }
         bool redo = false;
         for (uint32_t q = 0; q < B; q++) redo = redo || mins[q] < 0.f;
         if (redo) {
@@ -2951,7 +3136,7 @@ static int copy_out(SearchCall &k) {
     if (k.facets) OCTRY(run_facets(c, *r.fj, k.fpl, B, k.has_ft, k.has_v, k.S, k.n_tiles, k.vlimit));
     if (gj) {
         CU(cudaEventRecord(c->ev[EV_GRP0], c->stream));
-        OCTRY(run_groups(c, *gj, k.p->mode, k.S, k.n_tiles, k.vlimit, k.fp.omc_doc, k.fp.omc_mult, k.n_omc, *pj));
+        OCTRY(run_groups(c, *gj, k.mode, k.S, k.n_tiles, k.vlimit, k.fp.omc_doc, k.fp.omc_mult, k.n_omc, *pj, k.s_plan.at(c->in_blob)));
         CU(cudaEventRecord(c->ev[EV_GRP1], c->stream));
         CU(cudaStreamSynchronize(c->stream));
     }
@@ -3030,7 +3215,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const SearchReq &r) 
 extern "C" int oc_search(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, uint64_t *out_doc_ids,
                          float *out_scores, uint32_t *out_n, uint64_t *out_count) {
     SearchReq r(p, out_doc_ids, out_scores, out_n, out_count);
-    r.q_filters_ok = true;
+    r.q_filters_ok = r.q_params_ok = true;
     return search_impl(c, emb, str, r);
 }
 
@@ -3335,7 +3520,8 @@ static int run_facets(oc_ctx *c, const FacetJob &fj, const FacetPlan &pl, uint32
 // The facet pass the reference runs for a request: the score map re-scored WITHOUT the where-filter (search.rs:361-396:
 // only the uncommitted deletes stay excluded, and stores tombstone deletes at once), so that the counts do not collapse
 // onto the selected category.  The hits of this pass are dropped.
-static int facets_unfiltered(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, FacetJob &fj) {
+// q_params_ok: the sub-batch pass of oc_search_q_facets (oc_search_facets takes one set of scalars).
+static int facets_unfiltered(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, FacetJob &fj, bool q_params_ok) {
     oc_search_params q = *p;
     q.filter_bits = nullptr; q.filter_nbits = 0; q.filter = nullptr; q.q_filters = nullptr;
     const uint32_t B = p->n_queries;
@@ -3345,6 +3531,7 @@ static int facets_unfiltered(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_searc
     SearchReq r(&q, docs.data(), scores.data(), n.data(), cnt.data());
     r.fj = &fj;
     r.q_filters_ok = true;
+    r.q_params_ok = q_params_ok;
     return search_impl(c, emb, str, r);
 }
 
@@ -3359,7 +3546,7 @@ extern "C" int oc_search_facets(oc_ctx *c, oc_emb *emb, oc_str *str, oc_facets *
     fj.fc = facets; fj.reqs = reqs; fj.out_counts = out_counts;
     for (uint32_t q = 0; q < B; q++)
         for (uint32_t r = 0; r < n_reqs; r++) { fj.q.push_back(q); fj.r.push_back(r); fj.o.push_back(size_t(q) * n_reqs + r); }
-    return facets_unfiltered(c, emb, str, p, fj);
+    return facets_unfiltered(c, emb, str, p, fj, false);
 }
 
 extern "C" int oc_facets_check(const oc_facets *f, const oc_facet_req *reqs, uint32_t n) {
@@ -3485,8 +3672,9 @@ extern "C" int oc_group_by_create(oc_facets *f, const uint32_t *fields, uint32_t
     return OC_OK;
 }
 
+// mode: the batch's (with per-query parameters, q_plan gives each query's own)
 static int run_groups(oc_ctx *c, const GroupJob &gj, int mode, const StrSnap *S, uint32_t n_tiles, uint32_t vlimit,
-                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, const PinJob &pj) {
+                      const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, const PinJob &pj, const QueryPlan *q_plan) {
     const uint32_t R = gj.rows, top = gj.top;
     if (R == 0) return OC_OK;
     const bool has_ft = mode != OC_MODE_VECTOR && n_tiles > 0;
@@ -3520,6 +3708,7 @@ static int run_groups(oc_ctx *c, const GroupJob &gj, int mode, const StrSnap *S,
     gp.omc_doc = omc_doc; gp.omc_mult = omc_mult; gp.n_omc = n_omc;
     gp.out_doc = c->grp_doc.as<uint64_t>(); gp.out_score = c->grp_score.as<float>(); gp.out_n = c->grp_n.as<uint32_t>();
     gp.ents = gj.d_ents;
+    gp.q_plan = q_plan;
     const size_t smem = (size_t(GROUP_BUF) + gp.kp2 + gp.vp2) * 8 + size_t(gp.vp2) * 4;
     for (int by_field = 0; by_field < 2; by_field++) {   // score order, then field order: one launch per work list
         const uint32_t s0 = by_field ? gj.n_score_spans : 0u, s1 = by_field ? gj.n_spans : gj.n_score_spans;
@@ -3567,7 +3756,7 @@ static int run_groups(oc_ctx *c, const GroupJob &gj, int mode, const StrSnap *S,
 
 static int pins_check_flat(const oc_search_params *p, const PinJob &pj) {
     if (p->sharded) return fail(OC_ERR_UNSUPPORTED, "pins over a sharded search: scores and the hybrid normalisation are global");
-    if (pj.splice && (uint64_t(p->limit) + p->offset) * 2 > OC_MAX_TOPK)
+    if (pj.splice && !p->q_params && (uint64_t(p->limit) + p->offset) * 2 > OC_MAX_TOPK)   // (q_params: per query, qparams_plan)
         return fail(OC_ERR_UNSUPPORTED, "pins: 2 x (limit+offset) %llu > %u", (unsigned long long)(uint64_t(p->limit) + p->offset) * 2,
                     OC_MAX_TOPK);
     return OC_OK;
@@ -3597,7 +3786,13 @@ static int groups_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     bool flat_only = false;   // some query has neither groups nor facets: its hits are oc_search_q_sorted's, which needs limit >= 1
     for (uint32_t b = 0; b < B; b++) {
         const oc_group_by *g = q[b].groups;
-        if (!g) { flat_only = flat_only || !(fj && fj->q_off[b + 1] > fj->q_off[b]); continue; }
+        if (!g) {
+            const bool flat = !(fj && fj->q_off[b + 1] > fj->q_off[b]);
+            if (flat && p->q_params && p->q_params[b].limit == 0)
+                return fail(OC_ERR_INVALID, "q_params[%u]: limit must be >= 1 when the query has no groups%s", b, fj ? " and no facets" : "");
+            flat_only = flat_only || flat;
+            continue;
+        }
         if (g->ctx != c) return fail(OC_ERR_INVALID, "group_by of query %u belongs to another ctx", b);
         const uint32_t m = q[b].max_results;
         if (m > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "query %u: max_results %u > %u", b, m, OC_MAX_TOPK);
@@ -3621,7 +3816,7 @@ static int groups_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     SearchReq r(p, out_doc_ids, out_scores, out_n, out_count);
     r.out_sort_values = out_sort_values; r.fj = fj; r.gj = &gj; r.pj = &pj;
     r.sj = sj.f.empty() ? nullptr : &sj;   // every query in score order: the flat hits are oc_search_pinned's
-    r.q_filters_ok = per_query;
+    r.q_filters_ok = r.q_params_ok = per_query;
     return search_impl(c, emb, str, r);
 }
 
@@ -3637,7 +3832,7 @@ static int sorted_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     SearchReq r(p, out_doc_ids, out_scores, out_n, out_count);
     r.out_sort_values = out_sort_values; r.pj = &pj;
     r.sj = sj.f.empty() ? nullptr : &sj;
-    r.q_filters_ok = q_filters_ok;
+    r.q_filters_ok = r.q_params_ok = q_filters_ok;
     return search_impl(c, emb, str, r);
 }
 
@@ -3834,14 +4029,30 @@ extern "C" int oc_search_q_facets(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_
     std::vector<float> vecs;
     std::vector<uint32_t> q_tok{0}, tok_term{0}, t_field, t_id;
     std::vector<float> t_weight;
-    if (p->mode != OC_MODE_FULLTEXT) {
+    // per-query parameters: the sub-batch's entries; a vector entry's row and a text entry's tokens are the ones read
+    std::vector<oc_query_params> sub_qp;
+    bool sub_v = p->mode != OC_MODE_FULLTEXT, sub_ft = p->mode != OC_MODE_VECTOR;
+    if (p->q_params) {
+        sub_v = sub_ft = false;
+        for (uint32_t b : sub) {
+            sub_qp.push_back(p->q_params[b]);
+            sub_v = sub_v || p->q_params[b].mode != OC_MODE_FULLTEXT;
+            sub_ft = sub_ft || p->q_params[b].mode != OC_MODE_VECTOR;
+        }
+        q.q_params = sub_qp.data();
+    }
+    auto text_of = [&](uint32_t b) { return !p->q_params || p->q_params[b].mode != OC_MODE_VECTOR; };
+    if (sub_v && emb && p->q_vecs) {
         const size_t dim = emb->dim;
         vecs.resize(size_t(S) * dim);
-        for (uint32_t s = 0; s < S; s++) memcpy(vecs.data() + size_t(s) * dim, p->q_vecs + size_t(sub[s]) * dim, dim * 4);
+        for (uint32_t s = 0; s < S; s++)
+            if (!p->q_params || p->q_params[sub[s]].mode != OC_MODE_FULLTEXT)
+                memcpy(vecs.data() + size_t(s) * dim, p->q_vecs + size_t(sub[s]) * dim, dim * 4);
         q.q_vecs = vecs.data();
     }
-    if (p->mode != OC_MODE_VECTOR) {
+    if (sub_ft && p->q_token_offsets) {
         for (uint32_t b : sub) {
+            if (!text_of(b)) { q_tok.push_back((uint32_t)tok_term.size() - 1); continue; }
             for (uint32_t t = p->q_token_offsets[b]; t < p->q_token_offsets[b + 1]; t++) {
                 for (uint32_t e = p->token_term_offsets[t]; e < p->token_term_offsets[t + 1]; e++) {
                     t_field.push_back(p->term_field[e]);
@@ -3856,7 +4067,7 @@ extern "C" int oc_search_q_facets(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_
         q.q_token_offsets = q_tok.data(); q.token_term_offsets = tok_term.data();
         q.term_field = t_field.data(); q.term_id = t_id.data(); q.term_weight = t_weight.data();
     }
-    return facets_unfiltered(c, emb, str, &q, fj);
+    return facets_unfiltered(c, emb, str, &q, fj, true);
 }
 
 // ------------------------------------------------------------------------------------ geopoint where-filter leaves (geo.cuh)
@@ -4009,14 +4220,20 @@ struct OcExec {
 struct oc_batcher {
     ocb::Batcher<OcExec> q;
     oc_ctx *ctx;
-    oc_batcher(OcExec x, uint32_t dim, uint32_t mb, uint32_t mw) : q(x, dim, mb, mw, x.e != nullptr, x.s != nullptr), ctx(x.c) {}
+    oc_batcher(OcExec x, uint32_t dim, uint32_t mb, uint32_t mw, bool mixed)
+        : q(x, dim, mb, mw, x.e != nullptr, x.s != nullptr, mixed), ctx(x.c) {}
 };
-extern "C" int oc_batcher_create(oc_ctx *c, oc_emb *emb, oc_str *str, uint32_t max_batch, uint32_t max_wait_us, oc_batcher **out) {
+extern "C" int oc_batcher_create2(oc_ctx *c, oc_emb *emb, oc_str *str, uint32_t max_batch, uint32_t max_wait_us, uint32_t flags,
+                                  oc_batcher **out) {
     if (!c || !out || (!emb && !str)) return fail(OC_ERR_INVALID, "bad arguments");
     if ((emb && emb->ctx != c) || (str && str->ctx != c)) return fail(OC_ERR_INVALID, "store belongs to another ctx");
     if (max_batch == 0 || max_batch > 4096) return fail(OC_ERR_INVALID, "max_batch %u outside 1..4096", max_batch);
-    *out = new oc_batcher(OcExec{c, emb, str}, emb ? emb->dim : 0, max_batch, max_wait_us);
+    if (flags & ~uint32_t(OC_BATCHER_MIXED)) return fail(OC_ERR_INVALID, "unknown batcher flags 0x%x", flags);
+    *out = new oc_batcher(OcExec{c, emb, str}, emb ? emb->dim : 0, max_batch, max_wait_us, (flags & OC_BATCHER_MIXED) != 0);
     return OC_OK;
+}
+extern "C" int oc_batcher_create(oc_ctx *c, oc_emb *emb, oc_str *str, uint32_t max_batch, uint32_t max_wait_us, oc_batcher **out) {
+    return oc_batcher_create2(c, emb, str, max_batch, max_wait_us, 0, out);
 }
 extern "C" void oc_batcher_destroy(oc_batcher *b) { delete b; }
 // The rest of every oc_batcher_search* call once its NULL arguments are checked.  What would fail a whole batch is

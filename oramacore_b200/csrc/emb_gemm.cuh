@@ -571,6 +571,8 @@ struct GemmMergeParams {
     uint64_t *out_doc; float *out_score; uint32_t *out_row; uint32_t *out_count; float *out_raw;
     uint8_t *out_unproven;       // [B] 1 => host must re-run this query through the exact sweep
     uint32_t *out_rescored;      // [B] rows re-scored exactly (diagnostics), may be NULL
+    const uint32_t *q_limit;     // NULL, or [B] each query's own depth (<= limit): its list is cut there ...
+    const float *q_sim;          // ... before its own similarity test (NULL: similarity)
 };
 __host__ __device__ inline size_t gemm_merge_smem_bytes() { return size_t(GEMM_MERGE_BUF + GEMM_MAX_RESCORE + GEMM_MAX_LIMIT) * 8; }
 
@@ -688,15 +690,17 @@ __global__ void __launch_bounds__(512, 2) emb_gemm_merge_kernel(const GemmMergeP
         for (uint32_t i = tid; i < GEMM_MAX_LIMIT; i += blockDim.x) exact[i] = sel[i];
         __syncthreads();
     }
+    const uint32_t n_mine = p.q_limit ? min(n_top, p.q_limit[q]) : n_top;
+    const float similarity = p.q_sim ? p.q_sim[q] : p.similarity;
     for (uint32_t i = tid; i < p.limit; i += blockDim.x) {
         uint64_t doc = 0; float score = 0.f, raw = 0.f; uint32_t row = 0xffffffffu;
-        if (i < n_top) {
+        if (i < n_mine) {
             const uint64_t k = exact[i];
             const uint32_t r = key_idx(k);
             const float distance = -key_score(k);
             const float sim = 1.0f - distance;
             const float sc = rescale_score(sim, p.rescale_e5);
-            if (sc >= p.similarity) {
+            if (sc >= similarity) {
                 doc = p.row_doc_ids ? p.row_doc_ids[r] : uint64_t(r);
                 score = sc; row = r; raw = key_score(k);
                 atomicAdd(&s_cnt, 1u);

@@ -320,6 +320,10 @@ struct ScanMergeParams {
     uint32_t *out_row;   // [nq][limit] (row index, for hybrid fusion); may be NULL
     uint32_t *out_count; // [nq]
     float *out_raw;      // [nq][limit] rank key (-distance) of each kept hit; may be NULL
+    // per-query parameters: NULL, or [nq] each query's own depth (<= limit) and similarity.  A query's top-L is the
+    // first L entries of its top-limit list (keys are unique), so the list is cut before the similarity test.
+    const uint32_t *q_limit;
+    const float *q_sim;
 };
 
 // Model::rescale_score (python/embeddings.rs:71-92)
@@ -370,6 +374,8 @@ __global__ void __launch_bounds__(256) emb_scan_merge_kernel(const ScanMergePara
     __shared__ uint32_t s_cnt;
     if (threadIdx.x == 0) s_cnt = 0;
     __syncthreads();
+    if (p.q_limit) got = min(got, p.q_limit[q]);
+    const float similarity = p.q_sim ? p.q_sim[q] : p.similarity;
     for (uint32_t i = threadIdx.x; i < p.limit; i += blockDim.x) {
         uint64_t doc = 0; float score = 0.f; uint32_t row = 0xffffffffu;
         if (i < got) {
@@ -378,7 +384,7 @@ __global__ void __launch_bounds__(256) emb_scan_merge_kernel(const ScanMergePara
             const float distance = -key_score(k);
             const float sim = 1.0f - distance;                 // embedding_field.rs:270
             score = rescale_score(sim, p.rescale_e5);          // :271
-            if (score >= p.similarity) {                       // :272 (kept hits form a prefix)
+            if (score >= similarity) {                         // :272 (kept hits form a prefix)
                 doc = p.row_doc_ids ? p.row_doc_ids[row] : uint64_t(row);
                 atomicAdd(&s_cnt, 1u);
             } else {

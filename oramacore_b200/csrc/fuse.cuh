@@ -14,6 +14,14 @@
 
 namespace oc {
 
+// One query's own scalars in a batch with per-query parameters (oc_search_params.q_params): what K4 selects for it and
+// how the group and pin kernels score its map.  limit / offset: K4's page (the whole top n_keep, offset 0, when a
+// splice pages it afterwards).
+struct QueryPlan {
+    int mode;
+    uint32_t limit, offset, n_keep;
+};
+
 struct FuseParams {
     int mode;                     // OC_MODE_*
     uint32_t n_tiles, n_keep;     // n_keep = limit + offset
@@ -50,6 +58,9 @@ struct FuseParams {
     uint64_t *out_vdoc;           // [q][v_stride] the unique vector hits (after the += merge) ...
     float *out_vscore;            // ... with their final score (fused in hybrid mode, after OMC; NaN = dropped)
     uint32_t *out_vn;             // [q]
+    // per-query parameters: NULL, or [q] each query's mode, page and n_keep.  Then mode is the batch's (the union of
+    // its parts), n_keep the candidate stride of the tiles and limit the row stride of the outputs.
+    const QueryPlan *q_plan;
 };
 
 __device__ __forceinline__ float omc_find(const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, uint64_t doc, bool *found) {
@@ -97,8 +108,13 @@ __global__ void __launch_bounds__(256) fuse_topk_kernel(const FuseParams p) {
     __shared__ unsigned int s_maxo, s_mino;
     __shared__ unsigned long long s_count;
     const uint32_t q = blockIdx.x, tid = threadIdx.x;
-    const bool has_ft = p.mode != OC_MODE_VECTOR;
-    const bool has_v = p.mode != OC_MODE_FULLTEXT;
+    // this query's mode, page and n_keep: its entry of the per-query plan, else the batch's scalars
+    const QueryPlan *pl = p.q_plan ? p.q_plan + q : nullptr;
+    const int qmode = pl ? __ldg(&pl->mode) : p.mode;
+    const uint32_t q_limit = pl ? __ldg(&pl->limit) : p.limit, q_offset = pl ? __ldg(&pl->offset) : p.offset;
+    const uint32_t q_keep = pl ? __ldg(&pl->n_keep) : p.n_keep;
+    const bool has_ft = qmode != OC_MODE_VECTOR;
+    const bool has_v = qmode != OC_MODE_FULLTEXT;
     const uint32_t vc = has_v ? p.v_count[q] : 0;
     const uint64_t *vdoc = has_v ? p.v_doc + size_t(q) * p.v_stride : nullptr;
     const float *vscore = has_v ? p.v_score + size_t(q) * p.v_stride : nullptr;
@@ -236,12 +252,12 @@ __global__ void __launch_bounds__(256) fuse_topk_kernel(const FuseParams p) {
                 }
             for (uint32_t j = tid; j < vc; j += blockDim.x) buf[n_valid_ft + j] = load(n_ft_slots + j);
             const uint32_t np2 = max(32u, next_pow2(n_all));
-            const uint32_t kp2 = max(32u, next_pow2(p.n_keep));
+            const uint32_t kp2 = max(32u, next_pow2(q_keep));
             if (np2 > 2 * kp2) {
                 // many more candidates than needed: radix-select the n_keep best, sort only those
                 for (uint32_t i = tid; i < kp2; i += blockDim.x) sel[i] = KEY_NONE;
                 __syncthreads();
-                block_select_largest(buf, n_all, p.n_keep, sel);
+                block_select_largest(buf, n_all, q_keep, sel);
                 group_bitonic_desc(sel, kp2, tid, blockDim.x, 0);
                 for (uint32_t i = tid; i < kp2; i += blockDim.x) buf[i] = sel[i];
                 __syncthreads();
@@ -249,25 +265,25 @@ __global__ void __launch_bounds__(256) fuse_topk_kernel(const FuseParams p) {
                 for (uint32_t i = n_all + tid; i < np2; i += blockDim.x) buf[i] = KEY_NONE;
                 group_bitonic_desc(buf, np2, tid, blockDim.x, 0);
             }
-            uint32_t real = min(n_all, p.n_keep);
+            uint32_t real = min(n_all, q_keep);
             __shared__ uint32_t s_real2;
             if (tid == 0) { while (real > 0 && buf[real - 1] == KEY_NONE) real--; s_real2 = real; }
             __syncthreads();
             got = s_real2;
         } else {
-            got = block_topn_stream(buf, p.capb, p.n_keep, total, load);
+            got = block_topn_stream(buf, p.capb, q_keep, total, load);
         }
     }
 
-    // ---- skip(offset).take(limit)
-    const uint32_t n_out = got > p.offset ? min(p.limit, got - p.offset) : 0;
+    // ---- skip(offset).take(limit); rows of p.limit entries
+    const uint32_t n_out = got > q_offset ? min(q_limit, got - q_offset) : 0;
     for (uint32_t i = tid; i < p.limit; i += blockDim.x) {
         uint64_t doc = 0; float sc = 0.f;
         if (i < n_out) {
-            const uint64_t k = buf[p.offset + i];
+            const uint64_t k = buf[q_offset + i];
             const uint32_t idx = key_idx(k);
             sc = key_score(k);
-            if (p.mode == OC_MODE_VECTOR) doc = vdoc[vbyrank[idx]];
+            if (qmode == OC_MODE_VECTOR) doc = vdoc[vbyrank[idx]];
             else if (hybrid && idx >= FUSE_VONLY) doc = vdoc[vbyrank[idx - FUSE_VONLY]];
             else doc = p.str_row_doc_ids ? p.str_row_doc_ids[idx] : uint64_t(idx);
         }

@@ -83,6 +83,7 @@ struct GroupParams {
     uint32_t *out_n;                // [row]
     // group_sort_topk_kernel: the batch's sort entries (sort.cuh); a span's entry gives the rank of each document id
     const SortEntry *ents;
+    const QueryPlan *q_plan;        // NULL, or [q]: a query is hybrid when hybrid is set and its own mode is
 };
 
 // SORT = false: the top max_results members by score (score desc, ties by ascending id, NaN dropped).
@@ -143,6 +144,7 @@ __device__ __forceinline__ void group_topk_body(const GroupParams &p) {
             }
     }
     const float gmin = p.has_ft ? p.gmin[q] : 0.f, den = p.has_ft ? p.den[q] : 0.f;
+    const bool hybrid = p.hybrid && (!p.q_plan || p.q_plan[q].mode == OC_MODE_HYBRID);
     const uint32_t *mb = p.has_ft ? p.mbits + size_t(q) * p.row_words : nullptr;
     const float *rft = p.has_ft ? p.row_ft + size_t(q) * p.row_words * 32 : nullptr;
 
@@ -157,7 +159,7 @@ __device__ __forceinline__ void group_topk_body(const GroupParams &p) {
         }
         const uint32_t row = p.has_ft ? grow[i] : 0xffffffffu;
         if (row == 0xffffffffu || !((mb[row >> 5] >> (row & 31)) & 1u)) { *present = false; return 0.f; }
-        return fused_ft_score(rft[row], p.hybrid, gmin, den, p.omc_doc, p.omc_mult, p.n_omc, [&] { return gdoc[i]; });
+        return fused_ft_score(rft[row], hybrid, gmin, den, p.omc_doc, p.omc_mult, p.n_omc, [&] { return gdoc[i]; });
     };
     // rank key of the i-th document of the group, KEY_NONE when it is not a key of the score map (or scores NaN)
     auto load = [&](uint64_t i) -> uint64_t {
@@ -182,7 +184,7 @@ __device__ __forceinline__ void group_topk_body(const GroupParams &p) {
         if (!p.has_ft) return KEY_NONE;
         const uint32_t row = grow[i];
         if (row == 0xffffffffu || !((mb[row >> 5] >> (row & 31)) & 1u)) return KEY_NONE;
-        const float f = fused_ft_score(rft[row], p.hybrid, gmin, den, p.omc_doc, p.omc_mult, p.n_omc, [&] { return gdoc[i]; });
+        const float f = fused_ft_score(rft[row], hybrid, gmin, den, p.omc_doc, p.omc_mult, p.n_omc, [&] { return gdoc[i]; });
         return f == f ? make_key(f, uint32_t(i)) : KEY_NONE;   // NaN dropped (NotNan, sort.rs:205-209)
     };
 

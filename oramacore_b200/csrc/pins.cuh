@@ -36,6 +36,7 @@ struct PinScoreParams {
     uint32_t n_omc;
     float *out_score;               // [q][stride] score-map value, 0.0 when not a key
     uint8_t *out_present;           // [q][stride] 1 = the document is a key of the score map
+    const QueryPlan *q_plan;        // NULL, or [q]: a query is hybrid when hybrid is set and its own mode is
 };
 
 // one warp per (query, item slot)
@@ -60,7 +61,8 @@ __global__ void __launch_bounds__(256) pin_score_kernel(const PinScoreParams p) 
         s = p.v_score[size_t(q) * p.v_stride + hit];
         present = 1;
     } else if (p.has_ft && p.ft_present[wid]) {
-        s = fused_ft_score(p.ft[wid], p.hybrid, p.gmin[q], p.den[q], p.omc_doc, p.omc_mult, p.n_omc, [&] { return d; });
+        const bool hybrid = p.hybrid && (!p.q_plan || p.q_plan[q].mode == OC_MODE_HYBRID);
+        s = fused_ft_score(p.ft[wid], hybrid, p.gmin[q], p.den[q], p.omc_doc, p.omc_mult, p.n_omc, [&] { return d; });
         present = 1;
     }
     p.out_score[wid] = s;   // NaN stays NaN: it is still the map's value
@@ -181,6 +183,7 @@ struct PinSpliceParams {
     const uint64_t *alt_doc;        // [q][alt_n_top]
     const float *alt_score;
     const uint32_t *alt_n;          // [q]
+    const uint2 *q_page;            // NULL, or [q] each query's own (offset, limit); limit is then the output row stride
 };
 
 // one CTA per query: the flat hits of sort_token_scores with pins, then skip(offset).take(limit); a query without items
@@ -193,9 +196,10 @@ __global__ void __launch_bounds__(PIN_THREADS) pin_splice_kernel(const PinSplice
     const uint64_t *top_doc = alt ? p.alt_doc : p.top_doc;
     const float *top_score = alt ? p.alt_score : p.top_score;
     const uint32_t top_n = alt ? p.alt_n[q] : p.top_n[q];
+    const uint2 page = p.q_page ? p.q_page[q] : make_uint2(p.offset, p.limit);
     const size_t it = size_t(q) * p.stride, tp = size_t(q) * n_top, o = size_t(q) * p.limit;
     const uint32_t n = pin_splice_block(top_doc + tp, top_score + tp, top_n, p.doc + it, p.pos + it, p.score + it,
-                                        p.cnt[q], p.kp2, [](uint32_t) { return true; }, p.offset, p.limit,
+                                        p.cnt[q], p.kp2, [](uint32_t) { return true; }, page.x, page.y,
                                         p.out_doc + o, p.out_score + o, smem);
     for (uint32_t i = n + threadIdx.x; i < p.limit; i += blockDim.x) { p.out_doc[o + i] = 0; p.out_score[o + i] = 0.f; }
     if (threadIdx.x == 0) p.out_n[q] = n;

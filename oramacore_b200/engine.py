@@ -807,7 +807,7 @@ def search_q_sorted_arrays(tsc: "TokenScoreContext", params: "TokenScoreParams",
     srt = _q_sorts(sorts, B)
     pins = None if promote is None else _pins(promote, B)[0]
     n_items = 0 if pins is None else int(pins._keep[0][-1])
-    L = params.limit_hint
+    L = _stride(params)
     docs, scores, sv = np.zeros((B, L), np.uint64), np.zeros((B, L), np.float32), np.zeros((B, L), np.float64)
     n, cnt = np.zeros(B, np.uint32), np.zeros(B, np.uint64)
     ps, pp = np.zeros(max(n_items, 1), np.float32), np.zeros(max(n_items, 1), np.uint8)
@@ -868,7 +868,7 @@ def search_q_groups_arrays(tsc: "TokenScoreContext", params: "TokenScoreParams",
     if group_stride is None:
         k = [0] * B if promote is None else [len(x) for x in promote]
         group_stride = max([0] + [_group_need(g, k[b]) for b, g in enumerate(groups)])
-    L, R, S = params.limit_hint, int(rows[-1]), int(group_stride)
+    L, R, S = _stride(params), int(rows[-1]), int(group_stride)
     docs, scores, sv, n, cnt, ps, pp, gd, gs, gsv, gn = _q_outputs(B, L, n_items, R, S)
     check(lib().oc_search_q_groups(tsc.ctx._h, tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None, C.byref(sp),
                                    req, None if pins is None else C.byref(pins), S, _p(docs), _p(scores), _p(sv), _p(n),
@@ -922,7 +922,7 @@ def search_q_facets_arrays(tsc: "TokenScoreContext", store: FacetStore, params: 
     if group_stride is None:
         k = [0] * B if promote is None else [len(x) for x in promote]
         group_stride = max([0] + [_group_need(g, k[b]) for b, g in enumerate(groups or [None] * B)])
-    L, R, S = params.limit_hint, int(rows[-1]), int(group_stride)
+    L, R, S = _stride(params), int(rows[-1]), int(group_stride)
     docs, scores, sv, n, cnt, ps, pp, gd, gs, gsv, gn = _q_outputs(B, L, n_items, R, S)
     fc = np.zeros(max(int(foff[-1]), 1), np.uint64)
     check(lib().oc_search_q_facets(tsc.ctx._h, tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None, C.byref(sp),
@@ -1096,6 +1096,18 @@ class TextQueryBatch:
 
 
 @dataclass
+class QueryParams:
+    """One query's own scalars in a batch (oc_query_params; SearchParams, types.rs:1381-1409): the TokenScoreParams
+    fields of the same meaning, for one query."""
+    mode: int
+    limit: int = 10
+    offset: int = 0
+    similarity: float = 0.7
+    threshold: Optional[float] = None
+    vector_limit: int = 0            # 0 => limit
+
+
+@dataclass
 class TokenScoreParams:
     """token_score.rs:31-41 (mode already resolved; boost/properties are folded into the
     resolved TextQuery by the host-side term resolution)."""
@@ -1116,6 +1128,22 @@ class TokenScoreParams:
     sharded: bool = False
     shard_tombstones: bool = False   # OC_SHARD_TOMBSTONES: some rank's string store holds uncommitted deletes
     shard_count_df: bool = False     # OC_SHARD_COUNT_DF: some rank's store lacks the corpus-wide df tables
+    # one entry per query (oc_search_params.q_params): query b takes its mode, limit, offset, similarity, threshold and
+    # vector_limit from query_params[b], and the fields above of those names are ignored; the hit arrays are sized by
+    # the largest limit (_stride)
+    query_params: Optional[Sequence[QueryParams]] = None
+
+
+def _stride(params: TokenScoreParams) -> int:
+    """The row stride of the hit arrays: limit_hint, or with query_params the largest entry's limit."""
+    if params.query_params is None:
+        return params.limit_hint
+    return max([0] + [int(q.limit) for q in params.query_params])
+
+
+def _modes(params: TokenScoreParams):
+    """The modes of a batch: params.mode, or each entry's."""
+    return {params.mode} if params.query_params is None else {int(q.mode) for q in params.query_params}
 
 
 class TokenScoreContext:
@@ -1139,8 +1167,8 @@ class TokenScoreContext:
         `texts` is a sequence of TextQuery or a pre-packed TextQueryBatch (term resolution happens
         before the hot path in the reference as well: token_score.rs:196-209)."""
         sp, keep, B = self._build_params(params, texts, q_vecs)
-        docs = np.empty((B, params.limit_hint), np.uint64)
-        scores = np.empty((B, params.limit_hint), np.float32)
+        docs = np.empty((B, _stride(params)), np.uint64)
+        scores = np.empty((B, _stride(params)), np.float32)
         n = np.empty(B, np.uint32)
         cnt = np.empty(B, np.uint64)
         check(lib().oc_search(self.ctx._h, self.emb._h if self.emb else None, self.str._h if self.str else None,
@@ -1160,11 +1188,22 @@ class TokenScoreContext:
         sp.threshold = -1.0 if params.threshold is None else params.threshold
         sp.bm25_k, sp.bm25_b = BM25_K, BM25_B
         keep = []
-        if params.mode in (MODE_VECTOR, MODE_HYBRID):
+        modes = _modes(params)
+        if params.query_params is not None:
+            qps = list(params.query_params)
+            if len(qps) != B:
+                raise ValueError(f"query_params has {len(qps)} entries for {B} queries")
+            arr = (_lib.QueryParams * max(B, 1))(*[_lib.QueryParams(int(q.mode), int(q.limit), int(q.offset), float(q.similarity),
+                                                                    -1.0 if q.threshold is None else float(q.threshold),
+                                                                    int(q.vector_limit)) for q in qps])
+            keep.append(arr)
+            sp.q_params = C.cast(arr, C.c_void_p)
+            sp.limit = _stride(params)
+        if modes & {MODE_VECTOR, MODE_HYBRID}:
             qv = np.ascontiguousarray(q_vecs, np.float32).reshape(B, self.emb.dim)
             keep.append(qv)
             sp.q_vecs = _p(qv)
-        if params.mode in (MODE_FULLTEXT, MODE_HYBRID):
+        if modes & {MODE_FULLTEXT, MODE_HYBRID}:
             keep.append(texts)
             sp.q_token_offsets, sp.token_term_offsets = _p(texts.q_token_offsets), _p(texts.token_term_offsets)
             sp.term_field, sp.term_id, sp.term_weight = _p(texts.term_field), _p(texts.term_id), _p(texts.term_weight)
@@ -1210,17 +1249,24 @@ class SearchBatcher:
     batched oc_search.  A request's device_filter (its where-filter) travels with it into the batch as
     that query's own filter, so filtered and unfiltered requests are coalesced together; requests with
     filtered_doc_ids (a host bitmap), OMC multipliers or sharding run as their own oc_search.  ctypes
-    releases the GIL while a caller is blocked in the library."""
+    releases the GIL while a caller is blocked in the library.
+    mixed=True (OC_BATCHER_MIXED): calls that differ in mode, limit, offset, similarity, threshold or vector_limit
+    share a batch too (each request's scalars become its q_params entry), and so do calls with the same OMC arrays;
+    each caller still gets what it gets alone."""
 
-    def __init__(self, tsc: TokenScoreContext, max_batch: int = 256, max_wait_us: int = 200):
+    def __init__(self, tsc: TokenScoreContext, max_batch: int = 256, max_wait_us: int = 200, mixed: bool = False):
         self.tsc = tsc
         h = C.c_void_p()
-        check(lib().oc_batcher_create(tsc.ctx._h, tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None,
-                                      int(max_batch), int(max_wait_us), C.byref(h)))
+        check(lib().oc_batcher_create2(tsc.ctx._h, tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None,
+                                       int(max_batch), int(max_wait_us), _lib.OC_BATCHER_MIXED if mixed else 0, C.byref(h)))
         self._h = h
 
     def _params(self, params: TokenScoreParams, text: Optional[TextQuery], q_vec: Optional[np.ndarray]):
-        """oc_search_params of one query and the arrays they point into."""
+        """oc_search_params of one query and the arrays they point into.  A request is one query with its scalars in
+        TokenScoreParams' own fields: query_params (a batch's per-query scalars) is refused."""
+        if params.query_params is not None:
+            raise ValueError("SearchBatcher takes one query per call: set mode / limit_hint / offset / similarity / "
+                             "threshold / vector_limit, not query_params")
         sp, keep, B = self.tsc._build_params(params, None if text is None else [text],
                                              None if q_vec is None else np.asarray(q_vec, np.float32).reshape(1, -1))
         assert B == 1

@@ -43,6 +43,7 @@ pub const OC_SCAN_TC_TF32: u32 = 1;
 pub const OC_SCAN_TC_BF16: u32 = 4;
 /// wgmma .f16 on the fp16 copy of an fp32 store (`OC_EMB_F16=0` selects `OC_SCAN_TC_TF32`)
 pub const OC_SCAN_TC_F16: u32 = 5;
+pub const OC_BATCHER_MIXED: u32 = 1;
 
 #[repr(C)]
 pub struct OcSearchParams {
@@ -69,6 +70,20 @@ pub struct OcSearchParams {
     pub vector_limit: u32,          // 0 => limit (limit_hint of the vector stage, search.rs:330-336)
     pub filter: *const OcFilter,    // device-resident FilterResult bitmap; wins over filter_bits
     pub q_filters: *const *const OcFilter,  // NULL, or B entries: query b's own filter (NULL = none); oc_search only
+    pub q_params: *const OcQueryParams,     // NULL, or B entries: query b's own mode / limit / offset / similarity /
+                                            // threshold / vector_limit; `limit` is then the hit arrays' row stride
+}
+
+/// One query's scalars (oc_query_params), the entry of OcSearchParams::q_params.
+#[repr(C)]
+#[derive(Clone, Copy, Debug)]
+pub struct OcQueryParams {
+    pub mode: c_int,
+    pub limit: u32,
+    pub offset: u32,
+    pub similarity: f32,
+    pub threshold: f32,     // < 0 => None
+    pub vector_limit: u32,  // 0 => limit
 }
 
 #[repr(C)]
@@ -141,6 +156,9 @@ extern "C" {
     /// micro-batching front: one query per call from many threads, coalesced into batched `oc_search`
     pub fn oc_batcher_create(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, max_batch: u32, max_wait_us: u32,
                              out: *mut *mut OcBatcher) -> c_int;
+    /// flags: 0 or OC_BATCHER_MIXED (requests with different mode / limit / offset / similarity / threshold share a batch)
+    pub fn oc_batcher_create2(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, max_batch: u32, max_wait_us: u32, flags: u32,
+                              out: *mut *mut OcBatcher) -> c_int;
     pub fn oc_batcher_destroy(b: *mut OcBatcher);
     pub fn oc_batcher_search(b: *mut OcBatcher, p: *const OcSearchParams, out_doc_ids: *mut u64, out_scores: *mut f32,
                              out_n: *mut u32, out_count: *mut u64) -> c_int;
