@@ -207,6 +207,8 @@ typedef struct {
     const struct oc_filter *const *q_filters;  /* NULL, or B entries: query b is filtered by q_filters[b] (NULL = none) */
     const struct oc_query_params *q_params;    /* NULL, or B entries: query b's own mode, limit, offset, similarity,
                                                   threshold and vector_limit (see below)                          */
+    const struct oc_where *q_where;            /* NULL, or query b's where-clause as a program, evaluated inside the
+                                                  call (see "where programs" below); same meaning as q_filters     */
 } oc_search_params;
 
 /* One query's scalar parameters (SearchParams, types.rs:1381-1409, with FulltextMode / VectorMode / HybridMode,
@@ -357,6 +359,65 @@ int oc_filter_facet_variant(const oc_facets *f, uint32_t field, uint32_t variant
 #define OC_RANGE_LO_OPEN 1u
 #define OC_RANGE_HI_OPEN 2u
 int oc_filter_facet_range(const oc_facets *f, uint32_t field, double lo, double hi, uint32_t flags, oc_filter **out);
+
+/* ---- where programs ------------------------------------------------------------------------------
+ * A where-clause as a postfix program over the leaves above, evaluated inside a search call (oc_search_params.q_where)
+ * instead of through one oc_filter_* call per leaf and per And / Or / Not.  Query b's program is
+ * nodes[q_node_offsets[b] .. q_node_offsets[b + 1]); an empty range leaves the query unfiltered.  Each node pushes one
+ * bitmap over [0, nbits) or combines the top of the stack:
+ *   OC_WHERE_NONE         the empty set
+ *   OC_WHERE_VARIANT      oc_filter_facet_variant(src = oc_facets *, field, arg = variant)
+ *   OC_WHERE_RANGE        oc_filter_facet_range(src = oc_facets *, field, a = lo, b = hi, arg = OC_RANGE_* flags)
+ *   OC_WHERE_GEO_RADIUS   oc_filter_geo_radius(src = oc_geo_field *, a = lat, b = lon, c = radius_m, arg = inside)
+ *   OC_WHERE_GEO_POLYGON  oc_filter_geo_polygon(src = oc_geo_field *, vertex_lat / vertex_lon [first_vertex ..
+ *                         first_vertex + n_vertices), arg = inside)
+ *   OC_WHERE_FILTER       an existing handle (src = oc_filter *), e.g. NOT(uncommitted deletes), built once per commit
+ *   OC_WHERE_AND / OR     pops arg >= 2 values, pushes their And / Or
+ *   OC_WHERE_NOT          pops one value, pushes its complement within [0, nbits) (as oc_filter_not)
+ * A program ends with exactly one value on the stack.  Query b's outputs are byte for byte those it gets with
+ * q_filters[b] = the handle that oc_filter_* build from the same leaves and combinators.
+ * Cost: the call plans on the host (identical leaves and identical programs of the batch are evaluated once; variant and
+ * range leaves are resolved to document slices by binary search), then a fixed number of launches on the call's stream:
+ * one scatter for every facet leaf, one for every geo leaf, one evaluation of every program, and no synchronise.  The
+ * leaf and result bitmaps live in a ctx workspace of (distinct leaves + distinct programs) x nbits / 8 bytes (a program
+ * of one leaf or one FILTER takes no result bitmap), kept between calls; OC_ERR_OOM when it cannot be allocated.
+ * Checks (OC_ERR_INVALID unless noted; a refused call writes nothing): every check of the leaf call the node stands
+ * for; a store or handle of another ctx; a store, or a handle combined with other values, whose nbits differs from
+ * oc_where.nbits (a program of one FILTER node takes the handle as it is, as a q_filters entry would); an unknown op;
+ * stack underflow; a program that does not end with one value; an arity below 2; more than OC_WHERE_MAX_NODES nodes or
+ * a stack deeper than OC_WHERE_MAX_DEPTH in one program; q_where together with filter, filter_bits or q_filters.
+ * Entry points: those that take q_filters take q_where (a query with a program counts as filtered there); those that
+ * refuse q_filters refuse q_where with the same code; a sharded call refuses it with OC_ERR_UNSUPPORTED. */
+#define OC_WHERE_NONE 0u
+#define OC_WHERE_VARIANT 1u
+#define OC_WHERE_RANGE 2u
+#define OC_WHERE_GEO_RADIUS 3u
+#define OC_WHERE_GEO_POLYGON 4u
+#define OC_WHERE_FILTER 5u
+#define OC_WHERE_AND 6u
+#define OC_WHERE_OR 7u
+#define OC_WHERE_NOT 8u
+#define OC_WHERE_MAX_NODES 4096u   /* nodes of one query's program                  */
+#define OC_WHERE_MAX_DEPTH 32u     /* values on the stack of one program at a time  */
+typedef struct oc_where_node {
+    uint32_t op;             /* OC_WHERE_*                                                               */
+    uint32_t field;          /* VARIANT / RANGE: the store's field                                       */
+    uint32_t arg;            /* VARIANT: variant; RANGE: flags; GEO_*: inside; AND / OR: arity           */
+    uint32_t first_vertex;   /* GEO_POLYGON: index into vertex_lat / vertex_lon                          */
+    uint32_t n_vertices;     /* GEO_POLYGON                                                              */
+    double a, b, c;          /* RANGE: lo, hi; GEO_RADIUS: lat, lon, radius_m                            */
+    const void *src;         /* VARIANT / RANGE: oc_facets *; GEO_*: oc_geo_field *; FILTER: oc_filter * */
+} oc_where_node;
+typedef struct oc_where {
+    uint64_t nbits;                   /* DocumentId space of every leaf                      */
+    const uint32_t *q_node_offsets;   /* B + 1                                                */
+    const oc_where_node *nodes;
+    const double *vertex_lat, *vertex_lon;   /* polygon vertices (NULL when no polygon)       */
+} oc_where;
+/* Host only: the checks above over queries [0, n_queries), as oc_facets_check.  OC_OK or the code a search would give. */
+int oc_where_check(const oc_where *w, uint32_t n_queries);
+/* One query's program as an ordinary handle over [0, w->nbits), in one call with one synchronise. */
+int oc_filter_from_where(oc_ctx *ctx, const oc_where *w, uint32_t query, oc_filter **out);
 
 /* out_counts: n_queries x n_reqs.  emb / str as for oc_search (the mode decides which are needed). */
 int oc_search_facets(oc_ctx *ctx, oc_emb *emb, oc_str *str, oc_facets *facets, const oc_search_params *p,
@@ -655,6 +716,13 @@ void oc_resolved_free(oc_resolved *r);
  * and unfiltered requests share a batch.  Any other call is passed straight to oc_search, and a p->filter of
  * another ctx is refused with OC_ERR_INVALID before it can join a batch.  p->n_queries must be 1; outputs as for
  * oc_search with B = 1.  A query with its own q_params runs directly.
+ * A request may carry its where-clause as a one-query program (p->q_where, not together with p->filter): when some
+ * request of a merged call has one, the call carries q_where with the requests' nodes concatenated (polygon vertices
+ * copied after the previous requests' ones), a p->filter request as a one-node OC_WHERE_FILTER program and an
+ * unfiltered request as an empty range; a merged call without programs carries q_filters as above.  A program the
+ * library would refuse (every check of a where program, with the batcher's ctx as the ctx its stores and handles must
+ * belong to) is refused with that error before the request joins a batch; programs over different nbits are not merged.
+ * A merged call with programs that fails with OC_ERR_OOM (its bitmap workspace) is split in halves and re-run.
  * oc_batcher_create2 with flags OC_BATCHER_MIXED: the key drops mode, limit, offset, similarity, threshold and
  * vector_limit.  The merged call carries each request's scalars as its q_params entry (row stride = the largest
  * limit) and every caller gets its hits at its own limit, byte for byte what it gets alone.  The key keeps bm25_k,

@@ -27,6 +27,11 @@ OC_SCAN_TC_TF32 = 1
 OC_SCAN_TC_BF16 = 4
 OC_SCAN_TC_F16 = 5   # wgmma .f16 on the fp16 copy of an fp32 store; OC_EMB_F16=0 selects OC_SCAN_TC_TF32
 OC_BATCHER_MIXED = 1   # oc_batcher_create2: requests with different scalars share a batch
+# where-program node ops (oc_where_node.op) and bounds
+OC_WHERE_NONE, OC_WHERE_VARIANT, OC_WHERE_RANGE, OC_WHERE_GEO_RADIUS, OC_WHERE_GEO_POLYGON = 0, 1, 2, 3, 4
+OC_WHERE_FILTER, OC_WHERE_AND, OC_WHERE_OR, OC_WHERE_NOT = 5, 6, 7, 8
+OC_WHERE_MAX_NODES = 4096
+OC_WHERE_MAX_DEPTH = 32
 
 EXPORTED_SYMBOLS = [
     "oc_last_error", "oc_version", "oc_abi_sizes", "oc_init", "oc_shutdown", "oc_device_info", "oc_comm_unique_id",
@@ -39,7 +44,7 @@ EXPORTED_SYMBOLS = [
     "oc_filter_read", "oc_filter_destroy", "oc_merge_results",
     "oc_geo_field_create", "oc_geo_field_destroy", "oc_filter_geo_radius", "oc_filter_geo_polygon",
     "oc_facets_create", "oc_facets_destroy", "oc_facets_add_field", "oc_facets_add_number_field", "oc_search_facets",
-    "oc_filter_facet_variant", "oc_filter_facet_range",
+    "oc_filter_facet_variant", "oc_filter_facet_range", "oc_where_check", "oc_filter_from_where",
     "oc_group_by_create", "oc_group_by_destroy", "oc_search_groups",
     "oc_search_pinned", "oc_search_groups_pinned", "oc_merge_pinned",
     "oc_sort_field_create", "oc_sort_field_destroy", "oc_search_sorted", "oc_search_q_sorted", "oc_search_groups_sorted", "oc_merge_sorted",
@@ -74,12 +79,22 @@ class SearchParams(C.Structure):
                 ("filter_bits", C.c_void_p), ("filter_nbits", C.c_uint64),
                 ("omc_doc_ids", C.c_void_p), ("omc_mult", C.c_void_p), ("n_omc", C.c_uint64),
                 ("sharded", C.c_int), ("vector_limit", C.c_uint32), ("filter", C.c_void_p),
-                ("q_filters", C.c_void_p), ("q_params", C.c_void_p)]
+                ("q_filters", C.c_void_p), ("q_params", C.c_void_p), ("q_where", C.c_void_p)]
 
 
 class QueryParams(C.Structure):   # oc_query_params: one entry of SearchParams.q_params
     _fields_ = [("mode", C.c_int), ("limit", C.c_uint32), ("offset", C.c_uint32), ("similarity", C.c_float),
                 ("threshold", C.c_float), ("vector_limit", C.c_uint32)]
+
+
+class WhereNode(C.Structure):   # oc_where_node: one node of a where program
+    _fields_ = [("op", C.c_uint32), ("field", C.c_uint32), ("arg", C.c_uint32), ("first_vertex", C.c_uint32),
+                ("n_vertices", C.c_uint32), ("a", C.c_double), ("b", C.c_double), ("c", C.c_double), ("src", C.c_void_p)]
+
+
+class Where(C.Structure):   # oc_where: the programs of a batch (SearchParams.q_where)
+    _fields_ = [("nbits", C.c_uint64), ("q_node_offsets", C.c_void_p), ("nodes", C.c_void_p), ("vertex_lat", C.c_void_p),
+                ("vertex_lon", C.c_void_p)]
 
 
 class FacetReq(C.Structure):
@@ -205,6 +220,8 @@ def lib():
     L.oc_facets_add_number_field.argtypes = [vp, u64, vp, vp, C.POINTER(u32)]
     L.oc_filter_facet_variant.argtypes = [vp, u32, u32, C.POINTER(vp)]
     L.oc_filter_facet_range.argtypes = [vp, u32, C.c_double, C.c_double, u32, C.POINTER(vp)]
+    L.oc_where_check.argtypes = [C.POINTER(Where), u32]
+    L.oc_filter_from_where.argtypes = [vp, C.POINTER(Where), u32, C.POINTER(vp)]
     L.oc_search_facets.argtypes = [vp, vp, vp, vp, C.POINTER(SearchParams), C.POINTER(FacetReq), u32, vp]
     L.oc_group_by_create.argtypes = [vp, vp, u32, C.POINTER(vp), C.POINTER(u64)]
     L.oc_group_by_destroy.argtypes = [vp]

@@ -115,6 +115,7 @@ inline BatchKey key_of(const Call &c, bool mixed = false) {
 // of equal scalars would otherwise refuse for all of its requests alike.
 inline bool batchable(const oc_search_params *p, bool has_emb = true, bool has_str = true, bool mixed = false) {
     if (p->n_queries != 1 || p->filter_bits || p->q_filters || p->q_params || (p->n_omc != 0 && !mixed) || p->sharded) return false;
+    if (p->q_where && p->filter) return false;
     if (mixed && (uint64_t(p->limit) + p->offset > OC_MAX_TOPK || (p->limit && (p->vector_limit ? p->vector_limit : p->limit) > OC_MAX_TOPK)))
         return false;
     if (mixed && p->n_omc && (!p->omc_doc_ids || !p->omc_mult)) return false;
@@ -179,6 +180,12 @@ struct MergedBatch {
     std::vector<float> scores;
     std::vector<uint32_t> n;
     std::vector<const oc_filter *> q_filters;   // [B] each query's p->filter, or empty when no query has one
+    // when some query has a where program: each query's program (its p->filter as one FILTER node), polygon vertices
+    // copied after the previous queries' ones
+    oc_where where{};
+    std::vector<uint32_t> w_off;                // [B + 1]
+    std::vector<oc_where_node> w_nodes;
+    std::vector<double> w_lat, w_lon;
     std::vector<oc_query_params> q_params;      // [B] mixed: each query's scalars
     // sort values and items (all but PLAIN)
     std::vector<oc_sort> q_sorts;               // [B] (SORTED)
@@ -275,15 +282,56 @@ struct MergedBatch {
             p.term_id = term_id.empty() ? &zero_u : term_id.data();
             p.term_weight = term_weight.empty() ? &one_f : term_weight.data();
         }
-        p.filter = nullptr; p.q_filters = nullptr;
+        p.filter = nullptr; p.q_filters = nullptr; p.q_where = nullptr;
+        if (std::any_of(reqs.begin(), reqs.end(), [](const Request *r) { return r->call.p->q_where != nullptr; })) {
+            build_where(reqs);
+            return;
+        }
         for (const Request *r : reqs)
             if (r->call.p->filter) {
                 for (const Request *q : reqs) q_filters.push_back(q->call.p->filter);
                 p.q_filters = q_filters.data();
                 break;
             }
+        alloc_hits(B);
+    }
+    void alloc_hits(uint32_t B) {
         docs.assign(size_t(B) * p.limit, 0); scores.assign(size_t(B) * p.limit, 0.f);
         n.assign(B, 0); count.assign(B, 0);
+    }
+    // the requests' programs concatenated (nbits: the first program's; run() keeps other sizes out of one batch)
+    void build_where(const std::vector<Request *> &reqs) {
+        w_off.assign(1, 0u);
+        bool first = true;
+        for (const Request *r : reqs) {
+            const oc_search_params *rp = r->call.p;
+            if (const oc_where *w = rp->q_where) {
+                if (first) where.nbits = w->nbits;
+                first = false;
+                for (uint32_t i = w->q_node_offsets[0]; i < w->q_node_offsets[1]; i++) {
+                    oc_where_node nd = w->nodes[i];
+                    if (nd.op == OC_WHERE_GEO_POLYGON) {
+                        const uint32_t fv = nd.first_vertex;
+                        nd.first_vertex = (uint32_t)w_lat.size();
+                        w_lat.insert(w_lat.end(), w->vertex_lat + fv, w->vertex_lat + fv + nd.n_vertices);
+                        w_lon.insert(w_lon.end(), w->vertex_lon + fv, w->vertex_lon + fv + nd.n_vertices);
+                    }
+                    w_nodes.push_back(nd);
+                }
+            } else if (rp->filter) {
+                oc_where_node nd{};
+                nd.op = OC_WHERE_FILTER;
+                nd.src = rp->filter;
+                w_nodes.push_back(nd);
+            }
+            w_off.push_back((uint32_t)w_nodes.size());
+        }
+        where.q_node_offsets = w_off.data();
+        where.nodes = w_nodes.empty() ? nullptr : w_nodes.data();
+        where.vertex_lat = w_lat.empty() ? nullptr : w_lat.data();
+        where.vertex_lon = w_lon.empty() ? nullptr : w_lon.data();
+        p.q_where = &where;
+        alloc_hits((uint32_t)reqs.size());
     }
     void build_pins(const std::vector<Request *> &reqs, uint32_t L) {
         pin_off.assign(1, 0u);
@@ -439,13 +487,25 @@ private:
         }
         return r.rc;
     }
-    // One merged call.  A grouped or faceted one that runs out of device memory (the row-score workspace grows with the
-    // batch) is split in halves, down to single requests, which then get the single call's answer.
+    // One merged call.  A grouped or faceted one, or one with where programs, that runs out of device memory (the
+    // row-score and bitmap workspaces grow with the batch) is split in halves, down to single requests, which then get
+    // the single call's answer.  Programs over different DocumentId spaces cannot share a call: such a batch runs one
+    // request per call.
     void run(const std::vector<Request *> &reqs) {
+        const oc_where *w0 = nullptr;
+        for (const Request *r : reqs) {
+            const oc_where *w = r->call.p->q_where;
+            if (!w) continue;
+            if (w0 && w->nbits != w0->nbits && reqs.size() > 1) {
+                for (Request *q : reqs) run(std::vector<Request *>{q});
+                return;
+            }
+            w0 = w0 ? w0 : w;
+        }
         MergedBatch m;
         m.build(reqs, dim_, mixed_);
         const int rc = exec_(m.call);
-        if (rc == OC_ERR_OOM && m.call.q_groups && reqs.size() > 1) {
+        if (rc == OC_ERR_OOM && (m.call.q_groups || m.p.q_where) && reqs.size() > 1) {
             const size_t h = reqs.size() / 2;
             run(std::vector<Request *>(reqs.begin(), reqs.begin() + h));
             run(std::vector<Request *>(reqs.begin() + h, reqs.end()));

@@ -29,6 +29,7 @@
 #include "pins.cuh"
 #include "sort.cuh"
 #include "tmap.cuh"
+#include "where.cuh"
 #include "oramacore_b200.h"
 
 using namespace oc;
@@ -188,6 +189,9 @@ struct oc_ctx {
     std::vector<uint32_t> v_qlim, v_qmap;
     std::vector<float> v_qsim;
     DevBuf vq_doc, vq_score, vq_row, vq_cnt, vq_raw, r_lim, r_sim;
+    // where programs (q_where): the leaf and result bitmaps of the call, and its plan tables (h_where: their staging)
+    DevBuf w_bits, w_blob;
+    HostBuf h_where;
 
     HostBuf h_in, h_out, h_in0;   // h_in0 / in_blob0: query vectors + filter, uploaded before the descriptors
     OcComm comm;
@@ -2020,6 +2024,9 @@ struct SearchCall {
     std::shared_ptr<StrSnap> snap;
     StrSnap *S = nullptr;
     QFilterJob qfj;
+    // where programs (p->q_where): a handle over each distinct result bitmap in c->w_bits, and each query's handle
+    std::vector<oc_filter> w_handles;
+    std::vector<const oc_filter *> w_qf;
     FacetPlan fpl;
     const oc_filter *batch_filter = nullptr;
     bool filter_h = false, filter = false;
@@ -2105,20 +2112,26 @@ static int upload(const Packer &pk, HostBuf &hb, DevBuf &db, cudaStream_t st) {
 }
 
 // per-query where-filters: deduplicated by handle; all NULL = unfiltered, one handle for every query = p->filter
+static int qfilter_slots(SearchCall &k, const oc_filter *const *q_filters);
 static int qfilter_plan(SearchCall &k) {
-    const oc_search_params *p = k.p; const uint32_t B = k.B;
-    QFilterJob &qfj = k.qfj;
+    const oc_search_params *p = k.p;
     if (!k.r.q_filters_ok)
         return fail(OC_ERR_UNSUPPORTED, "q_filters: per-query filters are supported by oc_search, oc_search_q_sorted and "
                                         "oc_search_q_groups only");
     if (p->filter || p->filter_bits) return fail(OC_ERR_INVALID, "q_filters together with filter / filter_bits");
     if (p->sharded) return fail(OC_ERR_UNSUPPORTED, "q_filters over a sharded search");
+    return qfilter_slots(k, p->q_filters);
+}
+// the slots of the per-query filter handles q_filters[B] (p->q_filters, or the results of the call's where programs)
+static int qfilter_slots(SearchCall &k, const oc_filter *const *q_filters) {
+    const uint32_t B = k.B;
+    QFilterJob &qfj = k.qfj;
     std::unordered_map<const oc_filter *, uint32_t> idx;
     std::vector<const oc_filter *> distinct;
     bool any_none = false;
     qfj.q_slot.resize(B);
     for (uint32_t b = 0; b < B; b++) {
-        const oc_filter *f = p->q_filters[b];
+        const oc_filter *f = q_filters[b];
         if (!f) { any_none = true; qfj.q_slot[b] = SLOT_NONE; continue; }
         if (f->ctx != k.c) return fail(OC_ERR_INVALID, "q_filters[%u] belongs to another ctx", b);
         auto it = idx.emplace(f, (uint32_t)distinct.size()).first;
@@ -2215,6 +2228,14 @@ static int search_check(SearchCall &k) {
     if (k.emb && k.emb->ctx != c) return fail(OC_ERR_INVALID, "emb belongs to another ctx");
     if (k.str && k.str->ctx != c) return fail(OC_ERR_INVALID, "str belongs to another ctx");
     k.batch_filter = p->filter;
+    if (p->q_where) {   // the programs themselves are checked and planned under the ctx lock (where_stage)
+        if (!r.q_filters_ok)
+            return fail(OC_ERR_UNSUPPORTED, "q_where: per-query where programs are supported by oc_search, oc_search_q_sorted, "
+                                            "oc_search_q_groups and oc_search_q_facets only");
+        if (p->filter || p->filter_bits || p->q_filters) return fail(OC_ERR_INVALID, "q_where together with filter / filter_bits / q_filters");
+        if (p->sharded) return fail(OC_ERR_UNSUPPORTED, "q_where over a sharded search");
+        if (!p->q_where->q_node_offsets) return fail(OC_ERR_INVALID, "q_where: q_node_offsets is NULL");
+    }
     if (p->q_filters) OCTRY(qfilter_plan(k));
     if (p->limit == 0 && k.write_hits) return fail(OC_ERR_INVALID, "limit must be >= 1");
     const PinJob *pj = r.pj; const SortJob *sj = r.sj;
@@ -3188,6 +3209,8 @@ static int copy_out(SearchCall &k) {
     return OC_OK;
 }
 
+static int where_stage(SearchCall &k);
+
 static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const SearchReq &r) {
     SearchCall k(c, emb, str, r);
     OCTRY(search_check(k));
@@ -3201,6 +3224,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const SearchReq &r) 
     // facets: the requests resolved to their distinct document slices (the work list goes up with the first upload)
     if (k.facets) OCTRY(facet_plan(*r.fj, k.fpl));
     begin_call(c);
+    if (k.p->q_where) OCTRY(where_stage(k));
     OCTRY(vector_first(k));
     OCTRY(ft_descriptors(k));
     OCTRY(omc_plan(k));
@@ -3523,7 +3547,7 @@ static int run_facets(oc_ctx *c, const FacetJob &fj, const FacetPlan &pl, uint32
 // q_params_ok: the sub-batch pass of oc_search_q_facets (oc_search_facets takes one set of scalars).
 static int facets_unfiltered(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, FacetJob &fj, bool q_params_ok) {
     oc_search_params q = *p;
-    q.filter_bits = nullptr; q.filter_nbits = 0; q.filter = nullptr; q.q_filters = nullptr;
+    q.filter_bits = nullptr; q.filter_nbits = 0; q.filter = nullptr; q.q_filters = nullptr; q.q_where = nullptr;
     const uint32_t B = p->n_queries;
     std::vector<uint64_t> docs(size_t(B) * p->limit), cnt(B);
     std::vector<float> scores(size_t(B) * p->limit);
@@ -4013,7 +4037,8 @@ extern "C" int oc_search_q_facets(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_
     std::vector<uint32_t> sub;
     for (uint32_t b = 0; b < B; b++) {
         if (off[b + 1] == off[b]) continue;
-        const bool filtered = all_filtered || (p->q_filters && p->q_filters[b]);
+        const bool filtered = all_filtered || (p->q_filters && p->q_filters[b]) ||
+                              (p->q_where && p->q_where->q_node_offsets && p->q_where->q_node_offsets[b + 1] > p->q_where->q_node_offsets[b]);
         if (filtered) sub.push_back(b);
         FacetJob &j = filtered ? fj : mj;
         const uint32_t row = filtered ? (uint32_t)sub.size() - 1 : b;
@@ -4196,6 +4221,310 @@ extern "C" int oc_filter_geo_polygon(const oc_geo_field *g, const double *lat, c
     });
 }
 
+// ------------------------------------------------------------------------------------ where programs (where.cuh)
+// The where programs of queries [q0, q0 + n), planned on the host: their distinct leaves (keyed on store, field and
+// parameters, facet leaves on their resolved slice), their distinct programs of more than one node (keyed on content),
+// and the bitmap each query is filtered by.  Workspace slots: the leaves that need a bitmap, then the programs.
+struct WherePlan {
+    uint64_t nbits = 0, words = 0;
+    std::vector<const oc_filter *> leaf_h;   // per distinct leaf: its handle (FILTER), else NULL
+    std::vector<uint32_t> leaf_slot;          // per distinct leaf: its workspace slot (not FILTER)
+    uint32_t n_leaf_slots = 0;
+    std::vector<WhereSlice> slices;           // .bits holds the slot until where_run
+    std::vector<WhereGeo> geo;                // .bits holds the slot, .vlon the vertex offset until where_run
+    std::vector<double> verts;                // polygon vertices: lon[nv] then lat[nv] per polygon leaf
+    uint64_t total = 0;                       // ids of all slices
+    std::vector<WhereOp> ops;
+    std::vector<WhereProg> progs;             // .out is set by where_run
+    // per query: UINT32_MAX unfiltered, else its result: a leaf index (a program of one node) or leaves + program index
+    std::vector<uint32_t> q_res;
+};
+static uint64_t dbits(double x) { uint64_t u; memcpy(&u, &x, 8); return u; }
+
+// Checks queries [q0, q0 + n) of w (c: the ctx they must belong to, NULL: the ctx of the first store or handle, taken
+// from *c_out) and, with pl, plans them.  Called with the stores' ctx lock held.
+static int where_plan(const oc_where *w, uint32_t q0, uint32_t n, const oc_ctx *c, WherePlan *pl) {
+    constexpr uint32_t PROG_BIT = 1u << 31;
+    if (!w || !w->q_node_offsets) return fail(OC_ERR_INVALID, "q_where: NULL argument");
+    const uint32_t *off = w->q_node_offsets;
+    for (uint32_t b = q0; b < q0 + n; b++) {
+        if (off[b + 1] < off[b]) return fail(OC_ERR_INVALID, "q_where: q_node_offsets is not monotone at query %u", b);
+        if (off[b + 1] > off[b] && !w->nodes) return fail(OC_ERR_INVALID, "q_where: nodes is NULL");
+    }
+    std::map<std::vector<uint64_t>, uint32_t> leaf_idx, prog_idx;
+    if (pl) { pl->nbits = w->nbits; pl->words = (w->nbits + 63) / 64; pl->q_res.assign(n, UINT32_MAX); }
+    auto same_ctx = [&](const oc_ctx *x) { if (!c) c = x; return x == c; };
+    for (uint32_t b = q0; b < q0 + n; b++) {
+        const uint32_t len = off[b + 1] - off[b];
+        if (len == 0) continue;
+        if (len > OC_WHERE_MAX_NODES) return fail(OC_ERR_INVALID, "q_where[%u]: %u nodes > %u", b, len, OC_WHERE_MAX_NODES);
+        std::vector<uint64_t> prog;   // (WHERE_PUSH, leaf) / (op, arity) pairs
+        uint32_t sp = 0;
+        for (uint32_t i = 0; i < len; i++) {
+            const oc_where_node &nd = w->nodes[off[b] + i];
+            std::vector<uint64_t> key;
+            const oc_filter *h = nullptr;
+            const FacetField *ff = nullptr; uint64_t lo = 0, hi = 0;
+            const oc_geo_field *g = nullptr;
+            double u[3] = {0, 0, 0}, thr = 0; double4 bb{};
+            switch (nd.op) {
+            case OC_WHERE_NONE: key = {0}; break;
+            case OC_WHERE_VARIANT: case OC_WHERE_RANGE: {
+                const oc_facets *f = static_cast<const oc_facets *>(nd.src);
+                const bool number = nd.op == OC_WHERE_RANGE;
+                if (!f) return fail(OC_ERR_INVALID, "q_where[%u] node %u: NULL facet store", b, i);
+                if (!same_ctx(f->ctx)) return fail(OC_ERR_INVALID, "q_where[%u] node %u: facet store of another ctx", b, i);
+                if (f->nbits != w->nbits)
+                    return fail(OC_ERR_INVALID, "q_where[%u] node %u: store nbits %llu != %llu", b, i, (unsigned long long)f->nbits,
+                                (unsigned long long)w->nbits);
+                if (number && (std::isnan(nd.a) || std::isnan(nd.b))) return fail(OC_ERR_INVALID, "q_where[%u] node %u: NaN range bound", b, i);
+                if (number && (nd.arg & ~(OC_RANGE_LO_OPEN | OC_RANGE_HI_OPEN)))
+                    return fail(OC_ERR_INVALID, "q_where[%u] node %u: unknown range flags 0x%x", b, i, nd.arg);
+                if (nd.field >= f->fields.size())
+                    return fail(OC_ERR_INVALID, "q_where[%u] node %u: field %u: the store has %zu fields", b, i, nd.field, f->fields.size());
+                ff = &f->fields[nd.field];
+                if (ff->number != number)
+                    return fail(OC_ERR_INVALID, "q_where[%u] node %u: field %u is a %s field", b, i, nd.field,
+                                ff->number ? "number" : "bool / string_filter");
+                if (!number) {   // the slices oc_filter_facet_variant / _range take
+                    if (nd.arg + uint64_t(1) >= ff->offsets.size())
+                        return fail(OC_ERR_INVALID, "q_where[%u] node %u: variant %u: field %u has %zu variants", b, i, nd.arg, nd.field,
+                                    ff->offsets.size() - 1);
+                    lo = ff->offsets[nd.arg]; hi = ff->offsets[nd.arg + 1];
+                } else {
+                    const auto &v = ff->values;
+                    lo = (nd.arg & OC_RANGE_LO_OPEN) ? std::upper_bound(v.begin(), v.end(), nd.a) - v.begin()
+                                                     : std::lower_bound(v.begin(), v.end(), nd.a) - v.begin();
+                    hi = (nd.arg & OC_RANGE_HI_OPEN) ? std::lower_bound(v.begin(), v.end(), nd.b) - v.begin()
+                                                     : std::upper_bound(v.begin(), v.end(), nd.b) - v.begin();
+                    hi = std::max(lo, hi);
+                }
+                key = hi > lo ? std::vector<uint64_t>{1, uint64_t(uintptr_t(ff->docs)), lo, hi} : std::vector<uint64_t>{0};
+                break;
+            }
+            case OC_WHERE_GEO_RADIUS: case OC_WHERE_GEO_POLYGON: {
+                g = static_cast<const oc_geo_field *>(nd.src);
+                if (!g) return fail(OC_ERR_INVALID, "q_where[%u] node %u: NULL geo field", b, i);
+                if (!same_ctx(g->ctx)) return fail(OC_ERR_INVALID, "q_where[%u] node %u: geo field of another ctx", b, i);
+                if (g->nbits != w->nbits)
+                    return fail(OC_ERR_INVALID, "q_where[%u] node %u: geo field nbits %llu != %llu", b, i, (unsigned long long)g->nbits,
+                                (unsigned long long)w->nbits);
+                const uint64_t inside = nd.arg != 0;
+                if (nd.op == OC_WHERE_GEO_RADIUS) {   // oc_filter_geo_radius's checks and threshold
+                    if (!geo_valid(nd.a, nd.b)) return fail(OC_ERR_INVALID, "q_where[%u] node %u: radius centre: invalid coordinates (%g, %g)", b, i, nd.a, nd.b);
+                    if (!(std::isfinite(nd.c) && nd.c >= 0.0)) return fail(OC_ERR_INVALID, "q_where[%u] node %u: radius %g m: not finite and >= 0", b, i, nd.c);
+                    geo_unit(nd.a, nd.b, u);
+                    const double half = nd.c / (2.0 * OC_GEO_EARTH_RADIUS_M);
+                    const double s = std::sin(half);
+                    thr = half >= GEO_PI / 2 ? std::numeric_limits<double>::infinity() : 4.0 * s * s;
+                    key = {2, uint64_t(uintptr_t(g)), dbits(u[0]), dbits(u[1]), dbits(u[2]), dbits(thr), inside};
+                } else {   // oc_filter_geo_polygon's checks and bounding box
+                    const uint32_t nv = nd.n_vertices;
+                    if (nv < 3 || nv > OC_GEO_MAX_VERTICES)
+                        return fail(OC_ERR_INVALID, "q_where[%u] node %u: polygon of %u vertices: 3 to %u are supported", b, i, nv, OC_GEO_MAX_VERTICES);
+                    if (!w->vertex_lat || !w->vertex_lon) return fail(OC_ERR_INVALID, "q_where[%u] node %u: NULL vertices", b, i);
+                    const double *la = w->vertex_lat + nd.first_vertex, *ln = w->vertex_lon + nd.first_vertex;
+                    bb = make_double4(ln[0], ln[0], la[0], la[0]);
+                    key = {3, uint64_t(uintptr_t(g)), inside, nv};
+                    for (uint32_t v = 0; v < nv; v++) {
+                        if (!geo_valid(la[v], ln[v]))
+                            return fail(OC_ERR_INVALID, "q_where[%u] node %u: polygon vertex %u: invalid coordinates (%g, %g)", b, i, v, la[v], ln[v]);
+                        bb.x = std::min(bb.x, ln[v]); bb.y = std::max(bb.y, ln[v]); bb.z = std::min(bb.z, la[v]); bb.w = std::max(bb.w, la[v]);
+                        key.push_back(dbits(la[v])); key.push_back(dbits(ln[v]));
+                    }
+                    bb.x -= GEO_BBOX_MARGIN; bb.y += GEO_BBOX_MARGIN;
+                }
+                if (g->n == 0) key = {0};   // no point: an empty leaf, as the leaf call's zeroed bitmap
+                break;
+            }
+            case OC_WHERE_FILTER:
+                h = static_cast<const oc_filter *>(nd.src);
+                if (!h) return fail(OC_ERR_INVALID, "q_where[%u] node %u: NULL filter", b, i);
+                if (!same_ctx(h->ctx)) return fail(OC_ERR_INVALID, "q_where[%u] node %u: filter of another ctx", b, i);
+                if (len > 1 && h->nbits != w->nbits)
+                    return fail(OC_ERR_INVALID, "q_where[%u] node %u: filter nbits %llu != %llu", b, i, (unsigned long long)h->nbits,
+                                (unsigned long long)w->nbits);
+                key = {4, uint64_t(uintptr_t(h))};
+                break;
+            case OC_WHERE_AND: case OC_WHERE_OR: case OC_WHERE_NOT: {
+                const uint32_t ar = nd.op == OC_WHERE_NOT ? 1u : nd.arg;
+                if (nd.op != OC_WHERE_NOT && ar < 2) return fail(OC_ERR_INVALID, "q_where[%u] node %u: arity %u < 2", b, i, ar);
+                if (sp < ar) return fail(OC_ERR_INVALID, "q_where[%u] node %u: stack underflow", b, i);
+                sp -= ar - 1;
+                prog.push_back(uint64_t(nd.op) << 32 | ar);
+                continue;
+            }
+            default: return fail(OC_ERR_INVALID, "q_where[%u] node %u: unknown op %u", b, i, nd.op);
+            }
+            if (++sp > OC_WHERE_MAX_DEPTH) return fail(OC_ERR_INVALID, "q_where[%u]: stack deeper than %u", b, OC_WHERE_MAX_DEPTH);
+            if (!pl) continue;
+            auto it = leaf_idx.emplace(key, (uint32_t)pl->leaf_h.size()).first;
+            if (it->second == pl->leaf_h.size()) {   // a new leaf
+                pl->leaf_h.push_back(h);
+                pl->leaf_slot.push_back(h ? UINT32_MAX : pl->n_leaf_slots++);
+                const uint32_t slot = pl->leaf_slot.back();
+                if (key[0] == 1) {
+                    pl->slices.push_back(WhereSlice{ff->docs + lo, pl->total, reinterpret_cast<unsigned long long *>(uintptr_t(slot))});
+                    pl->total += hi - lo;
+                } else if (key[0] == 2 || key[0] == 3) {
+                    WhereGeo L{};
+                    L.g = g->pts(); L.cx = u[0]; L.cy = u[1]; L.cz = u[2]; L.thr = thr; L.bbox = bb; L.inside = nd.arg != 0;
+                    L.bits = reinterpret_cast<unsigned long long *>(uintptr_t(slot));
+                    if (key[0] == 3) {
+                        L.nv = nd.n_vertices;
+                        L.vlon = reinterpret_cast<const double *>(uintptr_t(pl->verts.size()));
+                        pl->verts.insert(pl->verts.end(), w->vertex_lon + nd.first_vertex, w->vertex_lon + nd.first_vertex + L.nv);
+                        pl->verts.insert(pl->verts.end(), w->vertex_lat + nd.first_vertex, w->vertex_lat + nd.first_vertex + L.nv);
+                    }
+                    pl->geo.push_back(L);
+                }
+            }
+            prog.push_back(uint64_t(WHERE_PUSH) << 32 | it->second);
+        }
+        if (sp != 1) return fail(OC_ERR_INVALID, "q_where[%u]: the program leaves %u values, not 1", b, sp);
+        if (!pl) continue;
+        if (prog.size() == 1) { pl->q_res[b - q0] = uint32_t(prog[0]); continue; }   // one leaf: its bitmap
+        auto it = prog_idx.emplace(prog, (uint32_t)pl->progs.size()).first;
+        if (it->second == pl->progs.size()) {
+            pl->progs.push_back(WhereProg{(uint32_t)pl->ops.size(), (uint32_t)prog.size(), nullptr});
+            for (uint64_t o : prog) pl->ops.push_back(WhereOp{uint32_t(o >> 32), uint32_t(o)});
+        }
+        pl->q_res[b - q0] = PROG_BIT | it->second;   // numbered after the leaves below, once their count is known
+    }
+    if (pl)
+        for (uint32_t &r : pl->q_res)
+            if (r != UINT32_MAX && (r & PROG_BIT)) r = (uint32_t)pl->leaf_h.size() + (r & ~PROG_BIT);
+    return OC_OK;
+}
+
+// Uploads the plan and materialises every leaf and program on c->stream: one zeroing of the leaf bitmaps, then at most
+// one launch each of where_scatter_kernel, where_geo_kernel and where_eval_kernel.  bits[r] afterwards: the bitmap of
+// result r (a leaf, then the programs) as q_res numbers them.
+static int where_run(oc_ctx *c, WherePlan &pl, std::vector<const uint64_t *> &bits) {
+    const uint64_t words = pl.words;
+    const uint32_t n_slots = pl.n_leaf_slots + (uint32_t)pl.progs.size();
+    OCTRY(c->w_bits.ensure(std::max<size_t>(size_t(n_slots) * words * 8, 8)));
+    uint64_t *ws = c->w_bits.as<uint64_t>();
+    auto slot_bits = [&](uint32_t s) { return reinterpret_cast<unsigned long long *>(ws + size_t(s) * words); };
+    std::vector<const unsigned long long *> leaf_ptr(pl.leaf_h.size());
+    bits.resize(pl.leaf_h.size() + pl.progs.size());
+    for (size_t i = 0; i < pl.leaf_h.size(); i++) {
+        leaf_ptr[i] = pl.leaf_h[i] ? reinterpret_cast<const unsigned long long *>(pl.leaf_h[i]->bits) : slot_bits(pl.leaf_slot[i]);
+        bits[i] = reinterpret_cast<const uint64_t *>(leaf_ptr[i]);
+    }
+    for (size_t p = 0; p < pl.progs.size(); p++) {
+        pl.progs[p].out = slot_bits(pl.n_leaf_slots + (uint32_t)p);
+        bits[pl.leaf_h.size() + p] = reinterpret_cast<const uint64_t *>(pl.progs[p].out);
+    }
+    if (words == 0) return OC_OK;
+    Packer pk;
+    const Slot<double> s_v = pk.add(pl.verts.data(), pl.verts.size());
+    const Slot<WhereSlice> s_s = pk.add(pl.slices.data(), pl.slices.size());
+    const Slot<WhereGeo> s_g = pk.add(pl.geo.data(), pl.geo.size());
+    const Slot<WhereOp> s_o = pk.add(pl.ops.data(), pl.ops.size());
+    const Slot<WhereProg> s_p = pk.add(pl.progs.data(), pl.progs.size());
+    const Slot<const unsigned long long *> s_l = pk.add(leaf_ptr.data(), leaf_ptr.size());
+    OCTRY(c->w_blob.ensure(pk.total + 256));   // device addresses of the vertices are known from here on
+    const double *dv = s_v.at(c->w_blob);
+    for (WhereSlice &s : pl.slices) s.bits = slot_bits((uint32_t)uintptr_t(s.bits));
+    for (WhereGeo &L : pl.geo) {
+        L.bits = slot_bits((uint32_t)uintptr_t(L.bits));
+        if (L.nv) { L.vlon = dv + uintptr_t(L.vlon); L.vlat = L.vlon + L.nv; }
+    }
+    OCTRY(upload(pk, c->h_where, c->w_blob, c->stream));
+    if (pl.n_leaf_slots) CU(cudaMemsetAsync(ws, 0, size_t(pl.n_leaf_slots) * words * 8, c->stream));
+    if (pl.total) {
+        where_scatter_kernel<<<(unsigned)std::min<uint64_t>((pl.total + 255) / 256, uint64_t(c->prop.multiProcessorCount) * 16), 256, 0,
+                               c->stream>>>(s_s.at(c->w_blob), (uint32_t)pl.slices.size(), pl.total, pl.nbits);
+        launched(c);
+        CU(cudaGetLastError());
+    }
+    if (!pl.geo.empty()) {
+        uint64_t most = 0;
+        for (const WhereGeo &L : pl.geo) most = std::max(most, L.g.n);
+        // blocks per leaf; the flat grid stays below 2^31 blocks however many leaves there are (a grid-stride loop covers
+        // the points)
+        const uint64_t n_geo = pl.geo.size();
+        const uint32_t gx = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>({(most + GEO_THREADS - 1) / GEO_THREADS,
+                                                                                  uint64_t(c->prop.multiProcessorCount) * 8,
+                                                                                  uint64_t(INT32_MAX) / n_geo}));
+        where_geo_kernel<<<(unsigned)(gx * n_geo), GEO_THREADS, 0, c->stream>>>(s_g.at(c->w_blob), gx);
+        launched(c);
+        CU(cudaGetLastError());
+    }
+    if (!pl.progs.empty()) {
+        where_eval_kernel<<<dim3((unsigned)((words + 255) / 256), (unsigned)pl.progs.size()), 256, 0, c->stream>>>(
+            s_o.at(c->w_blob), s_p.at(c->w_blob), s_l.at(c->w_blob), words, pl.nbits);
+        launched(c);
+        CU(cudaGetLastError());
+    }
+    return OC_OK;
+}
+
+// The where programs of a search: planned and evaluated on the call's stream, then handed to the q_filters machinery as
+// one handle per distinct result bitmap (a FILTER leaf is its own handle).
+static int where_stage(SearchCall &k) {
+    oc_ctx *c = k.c;
+    if (k.B > 65535) return fail(OC_ERR_UNSUPPORTED, "q_where: n_queries %u > 65535", k.B);
+    WherePlan pl;
+    OCTRY(where_plan(k.p->q_where, 0, k.B, c, &pl));
+    std::vector<const uint64_t *> bits;
+    OCTRY(where_run(c, pl, bits));
+    k.w_handles.resize(bits.size());
+    k.w_qf.assign(k.B, nullptr);
+    for (uint32_t b = 0; b < k.B; b++) {
+        const uint32_t r = pl.q_res[b];
+        if (r == UINT32_MAX) continue;
+        if (r < pl.leaf_h.size() && pl.leaf_h[r]) { k.w_qf[b] = pl.leaf_h[r]; continue; }
+        oc_filter &h = k.w_handles[r];
+        h.ctx = c; h.nbits = pl.nbits; h.words = pl.words; h.bits = const_cast<uint64_t *>(bits[r]);
+        k.w_qf[b] = &h;
+    }
+    return qfilter_slots(k, k.w_qf.data());
+}
+
+extern "C" int oc_where_check(const oc_where *w, uint32_t n_queries) {
+    if (!w || !w->q_node_offsets) return fail(OC_ERR_INVALID, "NULL argument");
+    // the stores' fields are read under their ctx lock: the ctx of the program's first store or handle
+    const oc_ctx *c = nullptr;
+    for (uint32_t i = w->q_node_offsets[0]; w->nodes && i < w->q_node_offsets[n_queries] && !c; i++) {
+        const oc_where_node &nd = w->nodes[i];
+        if (!nd.src) continue;
+        if (nd.op == OC_WHERE_VARIANT || nd.op == OC_WHERE_RANGE) c = static_cast<const oc_facets *>(nd.src)->ctx;
+        else if (nd.op == OC_WHERE_GEO_RADIUS || nd.op == OC_WHERE_GEO_POLYGON) c = static_cast<const oc_geo_field *>(nd.src)->ctx;
+        else if (nd.op == OC_WHERE_FILTER) c = static_cast<const oc_filter *>(nd.src)->ctx;
+    }
+    if (!c) return where_plan(w, 0, n_queries, nullptr, nullptr);
+    std::lock_guard<std::mutex> g(const_cast<oc_ctx *>(c)->mu);
+    return where_plan(w, 0, n_queries, c, nullptr);
+}
+
+extern "C" int oc_filter_from_where(oc_ctx *c, const oc_where *w, uint32_t query, oc_filter **out) {
+    if (!c || !w || !w->q_node_offsets || !out) return fail(OC_ERR_INVALID, "NULL argument");
+    if (w->q_node_offsets[query + 1] <= w->q_node_offsets[query]) return fail(OC_ERR_INVALID, "q_where[%u]: no program", query);
+    std::lock_guard<std::mutex> g(c->mu);
+    CU(cudaSetDevice(c->device));
+    WherePlan pl;
+    OCTRY(where_plan(w, query, 1, c, &pl));
+    const uint32_t r = pl.q_res[0];
+    const oc_filter *h = r < pl.leaf_h.size() ? pl.leaf_h[r] : nullptr;
+    oc_filter *f = nullptr;
+    OCTRY(filter_alloc(c, h ? h->nbits : pl.nbits, &f));
+    std::vector<const uint64_t *> bits;
+    int rc = where_run(c, pl, bits);
+    cudaError_t e = cudaSuccess;
+    if (rc == OC_OK && f->words) e = cudaMemcpyAsync(f->bits, bits[r], f->words * 8, cudaMemcpyDeviceToDevice, c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (rc == OC_OK && e != cudaSuccess) rc = fail(OC_ERR_CUDA, "oc_filter_from_where: %s", cudaGetErrorString(e));
+    if (rc != OC_OK) {
+        cudaFree(f->bits);
+        delete f;
+        return rc;
+    }
+    *out = f;
+    return OC_OK;
+}
+
 // ------------------------------------------------------------------------------------ micro-batching front
 struct OcExec {
     oc_ctx *c; oc_emb *e; oc_str *s;
@@ -4238,13 +4567,18 @@ extern "C" int oc_batcher_create(oc_ctx *c, oc_emb *emb, oc_str *str, uint32_t m
 extern "C" void oc_batcher_destroy(oc_batcher *b) { delete b; }
 // The rest of every oc_batcher_search* call once its NULL arguments are checked.  What would fail a whole batch is
 // refused here, before the request joins one: a handle of another ctx (a device filter joins as that query's q_filters
-// entry), a NULL group output, and what submit refuses.
+// entry), a where program the library would refuse (where_plan's checks against the batcher's ctx, so also a store or
+// handle of another ctx), a NULL group output, and what submit refuses.
 static int batcher_submit(oc_batcher *b, ocb::Request &r, const char *name) {
     const ocb::Call &k = r.call;
     if (k.p->n_queries != 1) return fail(OC_ERR_INVALID, "%s takes one query per call (n_queries = %u)", name, k.p->n_queries);
     const oc_sort *sort = ocb::sort_of(k);
     if (k.facets && k.facets->ctx != b->ctx) return fail(OC_ERR_INVALID, "facets belong to another ctx");
     if (k.p->filter && k.p->filter->ctx != b->ctx) return fail(OC_ERR_INVALID, "filter belongs to another ctx");
+    if (k.p->q_where) {   // a program with a store or handle of another ctx (or any other refusal) fails here, alone
+        std::lock_guard<std::mutex> g(b->ctx->mu);
+        OCTRY(where_plan(k.p->q_where, 0, 1, b->ctx, nullptr));
+    }
     if (sort && sort->field && sort->field->ctx != b->ctx) return fail(OC_ERR_INVALID, "sort field belongs to another ctx");
     if (k.q_groups) {
         if (k.q_groups->groups && k.q_groups->groups->ctx != b->ctx) return fail(OC_ERR_INVALID, "group_by belongs to another ctx");

@@ -34,18 +34,36 @@ __device__ __forceinline__ void geo_set(unsigned long long *bits, uint64_t d) {
     atomicOr(bits + (d >> 6), 1ull << (d & 63));
 }
 
-__global__ void __launch_bounds__(GEO_THREADS) geo_radius_kernel(const GeoPoints g, double cx, double cy, double cz,
-                                                                 double thr, int inside, unsigned long long *bits) {
-    for (uint64_t i = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < g.n; i += uint64_t(gridDim.x) * blockDim.x) {
-        const double dx = g.x[i] - cx, dy = g.y[i] - cy, dz = g.z[i] - cz;
-        const bool in = dx * dx + dy * dy + dz * dz <= thr;
-        if (in == (inside != 0)) geo_set(bits, g.doc[i]);
-    }
+// The per-point tests, shared by these kernels and where_geo_kernel (where.cuh) so both give the same bits.
+__device__ __forceinline__ bool geo_in_radius(double x, double y, double z, double cx, double cy, double cz, double thr) {
+    const double dx = x - cx, dy = y - cy, dz = z - cz;
+    return dx * dx + dy * dy + dz * dz <= thr;
 }
 
 // bbox = {lon_min, lon_max, lat_min, lat_max}.  A point below, above or left of the box crosses an even number of edges
 // and one right of it none, so the pre-test only skips points whose test is false.  The lon bounds are widened by the
 // host (GEO_BBOX_MARGIN) because a computed crossing abscissa may lie a few ulp outside [min(xi, xj), max(xi, xj)].
+__device__ __forceinline__ bool geo_in_polygon(double x, double y, const double *sx, const double *sy, uint32_t nv, double4 bbox) {
+    bool in = false;
+    if (x >= bbox.x && x <= bbox.y && y >= bbox.z && y <= bbox.w) {
+        for (uint32_t k = 0, j = nv - 1; k < nv; j = k++) {
+            const double xi = sx[k], yi = sy[k], xj = sx[j], yj = sy[j];
+            if ((yi > y) != (yj > y) &&
+                x < __dadd_rn(__ddiv_rn(__dmul_rn(__dadd_rn(xj, -xi), __dadd_rn(y, -yi)), __dadd_rn(yj, -yi)), xi))
+                in = !in;
+        }
+    }
+    return in;
+}
+
+__global__ void __launch_bounds__(GEO_THREADS) geo_radius_kernel(const GeoPoints g, double cx, double cy, double cz,
+                                                                 double thr, int inside, unsigned long long *bits) {
+    for (uint64_t i = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < g.n; i += uint64_t(gridDim.x) * blockDim.x) {
+        const bool in = geo_in_radius(g.x[i], g.y[i], g.z[i], cx, cy, cz, thr);
+        if (in == (inside != 0)) geo_set(bits, g.doc[i]);
+    }
+}
+
 __global__ void __launch_bounds__(GEO_THREADS) geo_polygon_kernel(const GeoPoints g, const double *vlon, const double *vlat,
                                                                   uint32_t nv, double4 bbox, int inside,
                                                                   unsigned long long *bits) {
@@ -53,16 +71,7 @@ __global__ void __launch_bounds__(GEO_THREADS) geo_polygon_kernel(const GeoPoint
     for (uint32_t k = threadIdx.x; k < nv; k += blockDim.x) { sx[k] = vlon[k]; sy[k] = vlat[k]; }
     __syncthreads();
     for (uint64_t i = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < g.n; i += uint64_t(gridDim.x) * blockDim.x) {
-        const double x = g.lon[i], y = g.lat[i];
-        bool in = false;
-        if (x >= bbox.x && x <= bbox.y && y >= bbox.z && y <= bbox.w) {
-            for (uint32_t k = 0, j = nv - 1; k < nv; j = k++) {
-                const double xi = sx[k], yi = sy[k], xj = sx[j], yj = sy[j];
-                if ((yi > y) != (yj > y) &&
-                    x < __dadd_rn(__ddiv_rn(__dmul_rn(__dadd_rn(xj, -xi), __dadd_rn(y, -yi)), __dadd_rn(yj, -yi)), xi))
-                    in = !in;
-            }
-        }
+        const bool in = geo_in_polygon(g.lon[i], g.lat[i], sx, sy, nv, bbox);
         if (in == (inside != 0)) geo_set(bits, g.doc[i]);
     }
 }

@@ -371,18 +371,32 @@ class GeoPointField:
 
     def radius(self, lat, lon, value, unit: str = "m", inside: bool = True) -> DeviceFilter:
         """GeoSearchFilter::Radius: centre (lat, lon) as API f32 values, radius value.to_meter(unit) in f32."""
+        clat, clon, r = self.radius_args(lat, lon, value, unit)
+        h = C.c_void_p()
+        check(lib().oc_filter_geo_radius(self._h, clat, clon, r, int(bool(inside)), C.byref(h)))
+        return DeviceFilter(self.ctx, h, self.nbits)
+
+    @staticmethod
+    def radius_args(lat, lon, value, unit: str = "m"):
+        """The checked (lat, lon, radius_m) radius() passes to the library."""
         clat, clon = _api_coord((lat, lon))
         _geo_check(clat, clon, "radius centre")
         r = geo_to_meter(value, unit)
         if not (np.isfinite(r) and r >= 0.0):
             raise ValueError(f"radius {value} {unit}: must be finite and >= 0")
-        h = C.c_void_p()
-        check(lib().oc_filter_geo_radius(self._h, clat, clon, r, int(bool(inside)), C.byref(h)))
-        return DeviceFilter(self.ctx, h, self.nbits)
+        return clat, clon, r
 
     def polygon(self, coords, inside: bool = True) -> DeviceFilter:
         """GeoSearchFilter::Polygon: `coords` = API GeoPoints ({"lat", "lon"} or (lat, lon) pairs), 3 to
         OC_GEO_MAX_VERTICES of them."""
+        la, lo = self.polygon_args(coords)
+        h = C.c_void_p()
+        check(lib().oc_filter_geo_polygon(self._h, _p(la), _p(lo), la.shape[0], int(bool(inside)), C.byref(h)))
+        return DeviceFilter(self.ctx, h, self.nbits)
+
+    @staticmethod
+    def polygon_args(coords):
+        """The checked vertex latitudes and longitudes (f64 arrays) polygon() passes to the library."""
         pts = [(p["lat"], p["lon"]) if isinstance(p, Mapping) else tuple(p) for p in coords]
         if not 3 <= len(pts) <= _lib.OC_GEO_MAX_VERTICES:
             raise ValueError(f"polygon of {len(pts)} vertices: 3 to {_lib.OC_GEO_MAX_VERTICES} are supported")
@@ -392,9 +406,7 @@ class GeoPointField:
         if bad.any():
             k = int(np.flatnonzero(bad)[0])
             _geo_check(la[k], lo[k], f"polygon vertex {k}")
-        h = C.c_void_p()
-        check(lib().oc_filter_geo_polygon(self._h, _p(la), _p(lo), len(pts), int(bool(inside)), C.byref(h)))
-        return DeviceFilter(self.ctx, h, self.nbits)
+        return la, lo
 
     def close(self):
         if self._h:
@@ -427,16 +439,28 @@ class FacetStore:
         calculate_filter_for_fields does (filter.rs:49-124): a bool or string_filter value is one variant (an unknown
         key gives an empty leaf), a NumberFilter / DateFilter one value interval, compared in f64.  A filter of the
         wrong kind for the field gives an empty leaf."""
+        spec = self.leaf_args(name, flt)
+        if spec is None:
+            return DeviceFilter.from_ids(self.ctx, [], self.nbits)
+        h = C.c_void_p()
+        if spec[0] == "variant":
+            check(lib().oc_filter_facet_variant(self._h, spec[1], spec[2], C.byref(h)))
+        else:
+            check(lib().oc_filter_facet_range(self._h, spec[1], spec[2], spec[3], spec[4], C.byref(h)))
+        return DeviceFilter(self.ctx, h, self.nbits)
+
+    def leaf_args(self, name: str, flt):
+        """What leaf() asks of the library: ("variant", field id, variant), ("range", field id, lo, hi, flags), or None
+        for an empty leaf."""
         from .where import DateFilter, NumberFilter
         f = self.fields[name]
-        h = C.c_void_p()
         kind = f["kind"]
         if (kind == "bool" and isinstance(flt, bool)) or (kind == "string" and isinstance(flt, str)):
             key = ("true" if flt else "false") if kind == "bool" else flt
             if key not in f["variant"]:
-                return DeviceFilter.from_ids(self.ctx, [], self.nbits)
-            check(lib().oc_filter_facet_variant(self._h, f["id"], f["variant"][key], C.byref(h)))
-        elif (kind == "number" and isinstance(flt, NumberFilter)) or (kind == "date" and isinstance(flt, DateFilter)):
+                return None
+            return "variant", f["id"], f["variant"][key]
+        if (kind == "number" and isinstance(flt, NumberFilter)) or (kind == "date" and isinstance(flt, DateFilter)):
             # eq / gt / gte / lt / lte / between (number_field.rs:555-642, date_field.rs:271-280) as [lo, hi] + open ends
             b = flt.bounds()
             if flt.op == "between":
@@ -444,10 +468,8 @@ class FacetStore:
             else:
                 lo, hi, flags = {"eq": (b, b, 0), "gt": (b, np.inf, _lib.OC_RANGE_LO_OPEN), "gte": (b, np.inf, 0),
                                  "lt": (-np.inf, b, _lib.OC_RANGE_HI_OPEN), "lte": (-np.inf, b, 0)}[flt.op]
-            check(lib().oc_filter_facet_range(self._h, f["id"], float(lo), float(hi), flags, C.byref(h)))
-        else:
-            return DeviceFilter.from_ids(self.ctx, [], self.nbits)
-        return DeviceFilter(self.ctx, h, self.nbits)
+            return "range", f["id"], float(lo), float(hi), flags
+        return None
 
     def add_bool_field(self, name: str, true_docs, false_docs):
         return self._add_variants(name, "bool", {"true": true_docs, "false": false_docs})
@@ -1122,6 +1144,10 @@ class TokenScoreParams:
     # one entry per query (None = unfiltered): query b is scored as if alone with device_filter = device_filters[b]
     # (oc_search_params.q_filters); not together with device_filter / filtered_doc_ids
     device_filters: Optional[Sequence[Optional["DeviceFilter"]]] = None
+    # one entry per query (None = unfiltered): query b's where-clause as a program (where.WhereProgram, e.g. from
+    # IndexLoader.where_program), evaluated inside the search call (oc_search_params.q_where); the same results as
+    # device_filters holding the handles the programs stand for, and not together with them or device_filter
+    where_programs: Optional[Sequence[Optional[object]]] = None
     vector_limit: int = 0            # 0 => limit_hint (search.rs:330-336); see oc_search_params.vector_limit
     omc_doc_ids: Optional[np.ndarray] = None   # ascending
     omc_mult: Optional[np.ndarray] = None
@@ -1215,6 +1241,15 @@ class TokenScoreContext:
             arr = (C.c_void_p * B)(*[None if f is None else f._h.value for f in fl])
             keep += [arr, fl]   # the handles stay alive for the call
             sp.q_filters = C.cast(arr, C.c_void_p)
+        if params.where_programs is not None:
+            from .where import pack_programs
+            wl = list(params.where_programs)
+            if len(wl) != B:
+                raise ValueError(f"where_programs has {len(wl)} entries for {B} queries")
+            if any(w is not None for w in wl):
+                w, wkeep = pack_programs(wl)
+                keep += [w, wkeep]
+                sp.q_where = C.cast(C.pointer(w), C.c_void_p)
         if params.device_filter is not None:
             keep.append(params.device_filter)
             sp.filter = params.device_filter._h

@@ -26,7 +26,7 @@ import numpy as np
 
 from .engine import (Context, DeviceFilter, EmbeddingFieldStorage, FacetStore, GeoPointField, StringFieldStorage,
                      TermDictionary, TokenScoreContext)
-from .where import WhereFilter, check_where_keys, evaluate_where, parse_where
+from .where import WhereFilter, WhereProgram, check_where_keys, compile_where, evaluate_where, parse_where
 
 _F64_INT_MAX = 1 << 53   # I64 values beyond +-2^53 would not survive the trip through a double
 
@@ -63,6 +63,8 @@ class IndexLoader:
         self.facets: Optional[FacetStore] = None
         self.geo: Dict[str, GeoPointField] = {}
         self.nbits = 1                                         # DocumentId space of `facets` and `geo`
+        self._live: Optional[DeviceFilter] = None              # NOT(uncommitted deletes) of where_program, built once
+        self._retired: List[DeviceFilter] = []                 # earlier ones, which programs may still point at
 
     # ---- Index::update_data
     def apply(self, op: Dict) -> None:
@@ -72,7 +74,9 @@ class IndexLoader:
             self.document_count += 1
             self.max_doc_id = max(self.max_doc_id, d)
             self._deleted.discard(d)
-            self._uncommitted_deleted.discard(d)
+            if d in self._uncommitted_deleted:
+                self._uncommitted_deleted.discard(d)
+                self._retire_live()
             for v in op["indexed_values"]:
                 t = v["type"]
                 if t == "ScoreString2":
@@ -126,6 +130,7 @@ class IndexLoader:
                 self._uncommitted_deleted.add(d)
                 for m in list(self._bool.values()) + list(self._num.values()) + list(self._strf.values()) + list(self._geo.values()) + list(self._date.values()):
                     m.pop(d, None)
+            self._retire_live()
         else:
             raise ValueError(f"unsupported operation {kind!r}")
 
@@ -148,6 +153,10 @@ class IndexLoader:
         for g in self.geo.values():
             g.close()
         self.geo = {}
+        self._retire_live()       # nbits changes: the deletes handle is rebuilt over the new DocumentId space
+        for f in self._retired:   # programs built before now point at the closed facet store and fields as well
+            f.close()
+        self._retired = []
         self.nbits = self.max_doc_id + 2
         for f, m in self._geo.items():
             docs = [d for d, ps in m.items() for _ in ps]
@@ -188,6 +197,25 @@ class IndexLoader:
         check_where_keys(w, [self.filter_fields()])
         return evaluate_where(w, self.facets, self.geo, self.nbits, sorted(self._uncommitted_deleted), ctx=self.ctx)
 
+    def where_program(self, where) -> Optional[WhereProgram]:
+        """The counterpart of where_filter: the same clause as a program for TokenScoreParams.where_programs, which the
+        search call evaluates itself.  Nothing runs on the device here except, once per set of uncommitted deletes, the
+        NOT(deletes) handle the program carries.  A program is valid until the next refresh_facets() / commit()."""
+        w = where if isinstance(where, WhereFilter) else parse_where(where)
+        check_where_keys(w, [self.filter_fields()])
+        if self._uncommitted_deleted and self._live is None:
+            dele = DeviceFilter.from_ids(self.ctx, sorted(self._uncommitted_deleted), self.nbits)
+            try:
+                self._live = ~dele
+            finally:
+                dele.close()
+        return compile_where(w, self.facets, self.geo, self.nbits, self._live)
+
+    def _retire_live(self) -> None:
+        if self._live is not None:
+            self._retired.append(self._live)
+            self._live = None
+
     def context(self) -> TokenScoreContext:
         return TokenScoreContext(self.ctx, self.emb, self.strs)
 
@@ -196,6 +224,6 @@ class IndexLoader:
         return self.dict.resolve_batch(list(texts), **kw)
 
     def close(self):
-        for x in [self.facets, self.emb, self.strs, self.dict] + list(self.geo.values()):
+        for x in [self.facets, self.emb, self.strs, self.dict, self._live] + list(self.geo.values()) + self._retired:
             if x is not None:
                 x.close()

@@ -35,7 +35,9 @@ Assumptions and deliberate differences (the oramacore_fields source is not avail
     (tests/test_where_host.py shows this is the only difference).
   * The reference raises FilterFieldNotFound only when the search found nothing (search.rs:435-449); IndexLoader
     .where_filter checks the keys before any device work, so a clause naming an unknown field is always refused.
-  * Bitmaps are exact, where the reference's sets may be Bloom-backed."""
+  * Bitmaps are exact, where the reference's sets may be Bloom-backed.
+compile_where(...) applies the same tree rules (one `_node` walk, one `_top_level` rule) to build the postfix program a
+search call evaluates itself (oc_search_params.q_where): no device call per request, and the same bitmap."""
 from __future__ import annotations
 
 import math
@@ -43,8 +45,12 @@ import re
 from dataclasses import dataclass, field
 from typing import Dict, List, Mapping, Optional, Sequence, Tuple, Union
 
+import ctypes as C
+
 import numpy as np
 
+from . import _lib
+from ._lib import check
 from .engine import Context, DeviceFilter, FacetStore, GeoPointField
 from .types import FilterFieldNotFound
 
@@ -293,17 +299,67 @@ def check_where_keys(w: WhereFilter, filter_fields_per_index: Sequence[Sequence[
 
 
 # ---------------------------------------------------------------- evaluation
-class _Eval:
-    """calculate_filter (filter.rs:176-287) over one index.  Every handle made while a tree is evaluated is kept in
+def _node(b, w: WhereFilter):
+    """The tree rules of calculate_filter (filter.rs:176-287) over a builder `b` (has / leaf / empty / and_ / or_ / not_):
+    the AND of the node's field leaves, of each `and` child, of the OR of its `or` children and of NOT its `not` child.
+    A key that is not a filter field makes the node empty (leaves after it are never built); `or: []` and a node with
+    no parts are empty."""
+    parts = []
+    for k, flt in w.filter_on_fields:
+        if not b.has(k):
+            return b.empty()
+        parts.append(b.leaf(k, flt))
+    parts += [_node(b, c) for c in w.and_ or []]
+    if w.or_ is not None:
+        if not w.or_:
+            return b.empty()
+        parts.append(b.or_([_node(b, c) for c in w.or_]))
+    if w.not_ is not None:
+        parts.append(b.not_(_node(b, w.not_)))
+    return b.and_(parts) if parts else b.empty()
+
+
+def _top_level(w: WhereFilter, has_deletes: bool) -> str:
+    """execute_filter's top level (filter.rs:344-392): "none" (no filter), "live" (NOT deletes), "tree" or
+    "tree_and_live"."""
+    if w.is_empty():
+        return "live" if has_deletes else "none"
+    return "tree_and_live" if has_deletes else "tree"
+
+
+class _Builder:
+    """What both builders of `_node` share: which keys are filter fields of the index, and which leaf a (key, filter)
+    pair is.  A subclass builds its values: facet_leaf, radius, polygon, empty, and_, or_, not_."""
+
+    def __init__(self, facets, geo_fields):
+        self.facets, self.geo = facets, geo_fields
+
+    def has(self, key) -> bool:
+        return key in self.geo or (self.facets is not None and key in self.facets.fields)
+
+    def leaf(self, key, flt):
+        if key not in self.geo:
+            return self.facet_leaf(key, flt)
+        g = self.geo[key]
+        if isinstance(flt, GeoRadius):
+            return self.radius(g, flt)
+        if isinstance(flt, GeoPolygon):
+            return self.polygon(g, flt)
+        return self.empty()   # wrong kind for a geopoint field
+
+
+class _Eval(_Builder):
+    """The tree rules building device handles over one index.  Every handle made while a tree is evaluated is kept in
     `owned` and closed when the evaluation ends, except the result."""
 
     def __init__(self, ctx, facets, geo_fields, nbits):
-        self.ctx, self.facets, self.geo, self.nbits = ctx, facets, geo_fields, nbits
+        super().__init__(facets, geo_fields)
+        self.ctx, self.nbits = ctx, nbits
         self.owned: List[DeviceFilter] = []
 
     def evaluate(self, w: WhereFilter) -> DeviceFilter:
         try:
-            res = self.node(w)
+            res = _node(self, w)
             self.owned.remove(res)
             return res
         finally:
@@ -314,18 +370,17 @@ class _Eval:
         self.owned.append(f)
         return f
 
-    def has(self, key) -> bool:
-        return key in self.geo or (self.facets is not None and key in self.facets.fields)
+    def facet_leaf(self, key, flt) -> DeviceFilter:
+        return self.keep(self.facets.leaf(key, flt))
 
-    def leaf(self, key, flt) -> DeviceFilter:
-        if key not in self.geo:
-            return self.facets.leaf(key, flt)
-        g = self.geo[key]
-        if isinstance(flt, GeoRadius):
-            return g.radius(flt.lat, flt.lon, flt.value, flt.unit, flt.inside)
-        if isinstance(flt, GeoPolygon):
-            return g.polygon(flt.coordinates, flt.inside)
-        return DeviceFilter.from_ids(self.ctx, [], self.nbits)   # wrong kind for a geopoint field
+    def radius(self, g, flt) -> DeviceFilter:
+        return self.keep(g.radius(flt.lat, flt.lon, flt.value, flt.unit, flt.inside))
+
+    def polygon(self, g, flt) -> DeviceFilter:
+        return self.keep(g.polygon(flt.coordinates, flt.inside))
+
+    def empty(self) -> DeviceFilter:
+        return self.keep(DeviceFilter.from_ids(self.ctx, [], self.nbits))
 
     def fold(self, parts: List[DeviceFilter], op) -> DeviceFilter:
         acc = parts[0]
@@ -333,21 +388,14 @@ class _Eval:
             acc = self.keep(op(acc, p))
         return acc
 
-    def node(self, w: WhereFilter) -> DeviceFilter:
-        empty = lambda: self.keep(DeviceFilter.from_ids(self.ctx, [], self.nbits))  # noqa: E731
-        parts = []
-        for k, flt in w.filter_on_fields:
-            if not self.has(k):
-                return empty()
-            parts.append(self.keep(self.leaf(k, flt)))
-        parts += [self.node(c) for c in w.and_ or []]
-        if w.or_ is not None:
-            if not w.or_:
-                return empty()
-            parts.append(self.fold([self.node(c) for c in w.or_], DeviceFilter.__or__))
-        if w.not_ is not None:
-            parts.append(self.keep(~self.node(w.not_)))
-        return self.fold(parts, DeviceFilter.__and__) if parts else empty()
+    def and_(self, parts):
+        return self.fold(parts, DeviceFilter.__and__)
+
+    def or_(self, parts):
+        return self.fold(parts, DeviceFilter.__or__)
+
+    def not_(self, x):
+        return self.keep(~x)
 
 
 def evaluate_where(w: WhereFilter, facets: Optional[FacetStore], geo_fields: Mapping[str, GeoPointField], nbits: int,
@@ -359,7 +407,8 @@ def evaluate_where(w: WhereFilter, facets: Optional[FacetStore], geo_fields: Map
     if ctx is None:
         raise ValueError("evaluate_where: no context (pass ctx= for an index without filter fields)")
     deleted = sorted({int(d) for d in uncommitted_deleted})
-    if w.is_empty() and not deleted:
+    top = _top_level(w, bool(deleted))
+    if top == "none":
         return None
     live = None
     if deleted:
@@ -368,7 +417,7 @@ def evaluate_where(w: WhereFilter, facets: Optional[FacetStore], geo_fields: Map
             live = ~dele
         finally:
             dele.close()
-    if w.is_empty():
+    if top == "live":
         return live
     tree = _Eval(ctx, facets, dict(geo_fields), int(nbits)).evaluate(w)
     if live is None:
@@ -378,3 +427,112 @@ def evaluate_where(w: WhereFilter, facets: Optional[FacetStore], geo_fields: Map
     finally:
         tree.close()
         live.close()
+
+
+# ---------------------------------------------------------------- programs (oc_search_params.q_where)
+@dataclass
+class WhereProgram:
+    """A where-clause compiled to the library's postfix program (include/oramacore_b200.h "where programs"): `nodes` are
+    (op, field, arg, a, b, c, src, vertices) tuples, vertices = (lats, lons) for a polygon else None.  `keep` holds the
+    handles the program points at (the deletes handle), `nbits` the DocumentId space of its leaves."""
+    nbits: int
+    nodes: List[tuple] = field(default_factory=list)
+    keep: list = field(default_factory=list)
+
+
+def _n(op, field_=0, arg=0, a=0.0, b=0.0, c=0.0, src=None, verts=None):
+    return (op, field_, arg, a, b, c, src, verts)
+
+
+class _Compile(_Builder):
+    """The tree rules building a postfix program; a value is the node list that pushes it."""
+
+    def empty(self):
+        return [_n(_lib.OC_WHERE_NONE)]
+
+    def facet_leaf(self, key, flt):
+        spec = self.facets.leaf_args(key, flt)
+        if spec is None:
+            return self.empty()
+        src = self.facets._h.value
+        if spec[0] == "variant":
+            return [_n(_lib.OC_WHERE_VARIANT, spec[1], spec[2], src=src)]
+        return [_n(_lib.OC_WHERE_RANGE, spec[1], spec[4], spec[2], spec[3], src=src)]
+
+    def radius(self, g, flt):
+        lat, lon, r = g.radius_args(flt.lat, flt.lon, flt.value, flt.unit)
+        return [_n(_lib.OC_WHERE_GEO_RADIUS, 0, int(bool(flt.inside)), lat, lon, r, src=g._h.value)]
+
+    def polygon(self, g, flt):
+        la, lo = g.polygon_args(flt.coordinates)
+        return [_n(_lib.OC_WHERE_GEO_POLYGON, 0, int(bool(flt.inside)), src=g._h.value, verts=(la, lo))]
+
+    def _nary(self, parts, op):
+        if len(parts) == 1:
+            return parts[0]
+        return [x for p in parts for x in p] + [_n(op, arg=len(parts))]
+
+    def and_(self, parts):
+        return self._nary(parts, _lib.OC_WHERE_AND)
+
+    def or_(self, parts):
+        return self._nary(parts, _lib.OC_WHERE_OR)
+
+    def not_(self, x):
+        return x + [_n(_lib.OC_WHERE_NOT)]
+
+
+def compile_where(w: WhereFilter, facets: Optional[FacetStore], geo_fields: Mapping[str, GeoPointField], nbits: int,
+                  live: Optional[DeviceFilter] = None) -> Optional[WhereProgram]:
+    """The program of evaluate_where(w, ...): None when nothing is filtered.  `live` is the NOT(uncommitted deletes)
+    handle (None without deletes), passed as a FILTER node; leaves are checked as their leaf calls check them."""
+    top = _top_level(w, live is not None)
+    if top == "none":
+        return None
+    prog = WhereProgram(int(nbits))
+    if top != "live":
+        prog.nodes = _node(_Compile(facets, dict(geo_fields)), w)
+    if live is not None:
+        prog.keep.append(live)
+        prog.nodes = prog.nodes + [_n(_lib.OC_WHERE_FILTER, src=live._h.value)]
+        if top == "tree_and_live":
+            prog.nodes.append(_n(_lib.OC_WHERE_AND, arg=2))
+    return prog
+
+
+def pack_programs(programs: Sequence[Optional[WhereProgram]]):
+    """The oc_where of a batch (query b: programs[b], None = unfiltered) and the arrays it points into."""
+    progs = [p for p in programs if p is not None]
+    if not progs:
+        raise ValueError("pack_programs: no program")
+    nbits = progs[0].nbits
+    offs, nodes, vlat, vlon, keep = [0], [], [], [], []
+    for p in programs:
+        if p is not None:
+            if p.nbits != nbits:
+                raise ValueError(f"where programs over {p.nbits} and {nbits} documents in one batch")
+            keep.append(p)
+            for (op, fl, arg, a, b, c, src, verts) in p.nodes:
+                first, nv = 0, 0
+                if verts is not None:
+                    first, nv = len(vlat), len(verts[0])
+                    vlat.extend(verts[0]); vlon.extend(verts[1])
+                nodes.append(_lib.WhereNode(op, fl, arg, first, nv, a, b, c, src))
+        offs.append(len(nodes))
+    off_a = np.asarray(offs, np.uint32)
+    node_a = (_lib.WhereNode * max(len(nodes), 1))(*nodes)
+    la, lo = np.asarray(vlat, np.float64), np.asarray(vlon, np.float64)
+    w = _lib.Where(nbits, off_a.ctypes.data, C.cast(node_a, C.c_void_p).value, la.ctypes.data if len(la) else None,
+                   lo.ctypes.data if len(lo) else None)
+    return w, [off_a, node_a, la, lo, keep]
+
+
+def filter_from_program(ctx: Context, prog: WhereProgram) -> DeviceFilter:
+    """oc_filter_from_where: the program's bitmap as an ordinary handle, in one call."""
+    w, keep = pack_programs([prog])
+    h = C.c_void_p()
+    check(_lib.lib().oc_filter_from_where(ctx._h, C.byref(w), 0, C.byref(h)))
+    nbits = prog.nbits
+    if len(prog.nodes) == 1 and prog.nodes[0][0] == _lib.OC_WHERE_FILTER:
+        nbits = prog.keep[0].nbits   # a lone handle is taken as it is
+    return DeviceFilter(ctx, h, nbits)

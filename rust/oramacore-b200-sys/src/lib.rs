@@ -72,6 +72,46 @@ pub struct OcSearchParams {
     pub q_filters: *const *const OcFilter,  // NULL, or B entries: query b's own filter (NULL = none); oc_search only
     pub q_params: *const OcQueryParams,     // NULL, or B entries: query b's own mode / limit / offset / similarity /
                                             // threshold / vector_limit; `limit` is then the hit arrays' row stride
+    pub q_where: *const OcWhere,            // NULL, or each query's where-clause as a program, evaluated in the call
+}
+
+/// Where-program node ops (oc_where_node.op) and bounds.
+pub const OC_WHERE_NONE: u32 = 0;
+pub const OC_WHERE_VARIANT: u32 = 1;
+pub const OC_WHERE_RANGE: u32 = 2;
+pub const OC_WHERE_GEO_RADIUS: u32 = 3;
+pub const OC_WHERE_GEO_POLYGON: u32 = 4;
+pub const OC_WHERE_FILTER: u32 = 5;
+pub const OC_WHERE_AND: u32 = 6;
+pub const OC_WHERE_OR: u32 = 7;
+pub const OC_WHERE_NOT: u32 = 8;
+pub const OC_WHERE_MAX_NODES: u32 = 4096;
+pub const OC_WHERE_MAX_DEPTH: u32 = 32;
+
+/// One node of a where program (oc_where_node): a leaf (src = the facet store, geo field or filter handle), or
+/// AND / OR (arg = arity) / NOT over the values on the stack.
+#[repr(C)]
+#[derive(Clone, Copy, Debug)]
+pub struct OcWhereNode {
+    pub op: u32,
+    pub field: u32,
+    pub arg: u32,            // VARIANT: variant; RANGE: flags; GEO_*: inside; AND / OR: arity
+    pub first_vertex: u32,   // GEO_POLYGON
+    pub n_vertices: u32,
+    pub a: f64,              // RANGE: lo, hi; GEO_RADIUS: lat, lon, radius_m
+    pub b: f64,
+    pub c: f64,
+    pub src: *const c_void,
+}
+
+/// The programs of a batch (oc_where): query b's nodes are nodes[q_node_offsets[b] .. q_node_offsets[b + 1]).
+#[repr(C)]
+pub struct OcWhere {
+    pub nbits: u64,
+    pub q_node_offsets: *const u32,
+    pub nodes: *const OcWhereNode,
+    pub vertex_lat: *const f64,
+    pub vertex_lon: *const f64,
 }
 
 /// One query's scalars (oc_query_params), the entry of OcSearchParams::q_params.
@@ -200,6 +240,9 @@ extern "C" {
                                 out: *mut *mut OcFilter) -> c_int;
     pub fn oc_filter_geo_polygon(g: *const OcGeoField, lat: *const f64, lon: *const f64, n_vertices: u32, inside: c_int,
                                  out: *mut *mut OcFilter) -> c_int;
+    // where programs: host-only checks, and one query's program as a handle in one call
+    pub fn oc_where_check(w: *const OcWhere, n_queries: u32) -> c_int;
+    pub fn oc_filter_from_where(ctx: *mut OcCtx, w: *const OcWhere, query: u32, out: *mut *mut OcFilter) -> c_int;
     // facets over the score set (facet.rs:147-209)
     pub fn oc_facets_create(ctx: *mut OcCtx, nbits: u64, out: *mut *mut OcFacets) -> c_int;
     pub fn oc_facets_destroy(f: *mut OcFacets);
