@@ -110,6 +110,30 @@ typedef struct {
 } oc_emb_info_t;
 int oc_emb_info(oc_emb *emb, oc_emb_info_t *out);
 
+/* == EmbeddingFieldStorage compact() as Index::commit runs it (index/mod.rs:583-590): removes the rows oc_emb_delete
+ * tombstoned, on the device and in place.  Live rows keep their relative order, so every search returns the ids,
+ * score bits, counts and tie order it returned before; what changes is num_rows (== num_embeddings afterwards), the
+ * bytes a sweep reads, and the room left for inserts.  The rows move through a staging window: the extra device
+ * memory (workspace_bytes) is the window (32 MiB) plus a quarter byte per row of the store, each rounded up by a
+ * quarter, never a second copy of the matrix; it is a ctx workspace, allocated for the call and freed at its end.  Rows below the first dead row are neither moved
+ * nor read, and a store without dead rows launches nothing.
+ * OC_EMB_COMPACT_SHRINK also gives the capacity beyond num_rows (rounded up to 64 rows) back by moving the store into
+ * a smaller allocation; when that allocation cannot be made the store stays compacted at its old capacity and the
+ * call still succeeds (device_bytes_after == device_bytes_before).  Without the flag the capacity is kept.
+ * Runs under the ctx lock on the ctx stream and returns when the stream is idle; searches on the ctx serialise with
+ * it.  A failure before the first row moves (OC_ERR_OOM for the workspace) leaves the store as it was.  There is no
+ * rollback once rows move: the call then finishes or returns OC_ERR_CUDA, after which the store must be destroyed.
+ * OC_ERR_INVALID: NULL store, unknown flag bits.  `out` may be NULL. */
+#define OC_EMB_COMPACT_SHRINK 1u
+typedef struct {
+    uint64_t rows_before, rows_after;      /* num_rows before / after (after == num_embeddings)       */
+    uint64_t rows_moved;                   /* live rows whose index changed                             */
+    uint64_t device_bytes_before, device_bytes_after;   /* as oc_emb_info reports them                 */
+    uint64_t workspace_bytes;              /* extra device memory the call held (0 when nothing ran)    */
+    float device_ms;                       /* CUDA-event time of the device work, 0 when nothing ran    */
+} oc_emb_compact_t;
+int oc_emb_compact(oc_emb *emb, uint32_t flags, oc_emb_compact_t *out);
+
 /* EmbeddingFieldStorage::search (embedding_field.rs:250-278) for B targets at once:
  * exact top-`limit` by cosine distance (== storage.search(target, limit, None) :255-266),
  * then similarity = 1 - distance, rescale, keep score >= similarity (:268-276).

@@ -26,6 +26,7 @@ OC_SCAN_EXACT = 0
 OC_SCAN_TC_TF32 = 1
 OC_SCAN_TC_BF16 = 4
 OC_SCAN_TC_F16 = 5   # wgmma .f16 on the fp16 copy of an fp32 store; OC_EMB_F16=0 selects OC_SCAN_TC_TF32
+OC_EMB_COMPACT_SHRINK = 1   # oc_emb_compact: also give the capacity beyond num_rows back
 OC_BATCHER_MIXED = 1   # oc_batcher_create2: requests with different scalars share a batch
 # where-program node ops (oc_where_node.op) and bounds
 OC_WHERE_NONE, OC_WHERE_VARIANT, OC_WHERE_RANGE, OC_WHERE_GEO_RADIUS, OC_WHERE_GEO_POLYGON = 0, 1, 2, 3, 4
@@ -35,7 +36,7 @@ OC_WHERE_MAX_DEPTH = 32
 
 EXPORTED_SYMBOLS = [
     "oc_last_error", "oc_version", "oc_abi_sizes", "oc_init", "oc_shutdown", "oc_device_info", "oc_comm_unique_id",
-    "oc_comm_init", "oc_comm_p2p_export", "oc_comm_p2p_import", "oc_emb_create", "oc_emb_destroy", "oc_emb_reserve", "oc_emb_insert", "oc_emb_delete",
+    "oc_comm_init", "oc_comm_p2p_export", "oc_comm_p2p_import", "oc_emb_create", "oc_emb_destroy", "oc_emb_reserve", "oc_emb_insert", "oc_emb_delete", "oc_emb_compact",
     "oc_emb_info", "oc_emb_search", "oc_str_create", "oc_str_destroy", "oc_str_set_rows", "oc_str_load_field",
     "oc_str_insert", "oc_str_commit", "oc_str_delete", "oc_str_info", "oc_str_set_global", "oc_search", "oc_pinned_alloc", "oc_pinned_free", "oc_last_timing", "oc_launch_count",
     "oc_batcher_create", "oc_batcher_create2", "oc_batcher_destroy", "oc_batcher_search", "oc_batcher_search_sorted", "oc_batcher_search_groups",
@@ -63,6 +64,15 @@ class OcError(RuntimeError):
 class EmbInfo(C.Structure):
     _fields_ = [("num_embeddings", C.c_uint64), ("num_rows", C.c_uint64), ("dimensions", C.c_uint32),
                 ("dtype", C.c_int), ("device_bytes", C.c_uint64)]
+
+
+class EmbCompact(C.Structure):   # oc_emb_compact_t
+    _fields_ = [("rows_before", C.c_uint64), ("rows_after", C.c_uint64), ("rows_moved", C.c_uint64),
+                ("device_bytes_before", C.c_uint64), ("device_bytes_after", C.c_uint64), ("workspace_bytes", C.c_uint64),
+                ("device_ms", C.c_float)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
 
 
 class StrInfo(C.Structure):
@@ -178,6 +188,7 @@ def lib():
     L.oc_emb_insert.argtypes = [vp, vp, vp, u64]
     L.oc_emb_delete.argtypes = [vp, vp, u64]
     L.oc_emb_info.argtypes = [vp, C.POINTER(EmbInfo)]
+    L.oc_emb_compact.argtypes = [vp, u32, C.POINTER(EmbCompact)]
     L.oc_emb_search.argtypes = [vp, vp, u32, u32, f32, vp, u64, vp, vp, vp]
     L.oc_str_create.argtypes = [vp, u32, C.POINTER(vp)]
     L.oc_str_destroy.argtypes = [vp]

@@ -21,6 +21,7 @@
 #include "comm.h"
 #include "dict.h"
 #include "stem_en.h"
+#include "emb_compact.cuh"
 #include "emb_gemm.cuh"
 #include "emb_scan.cuh"
 #include "fuse.cuh"
@@ -94,6 +95,7 @@ struct DevBuf {
         cap = want;
         return OC_OK;
     }
+    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }   // a large workspace of a rare call goes back at once
     template <typename T> T *as() { return reinterpret_cast<T *>(p); }
 };
 struct HostBuf {  // pinned staging
@@ -192,6 +194,9 @@ struct oc_ctx {
     // where programs (q_where): the leaf and result bitmaps of the call, and its plan tables (h_where: their staging)
     DevBuf w_bits, w_blob;
     HostBuf h_where;
+    // oc_emb_compact: the dead-row bitmap with its scan, and the staging window the rows move through (held for the
+    // call only: a compaction is rare and its window is large)
+    DevBuf cmp_scan, cmp_stage;
 
     HostBuf h_in, h_out, h_in0;   // h_in0 / in_blob0: query vectors + filter, uploaded before the descriptors
     OcComm comm;
@@ -344,6 +349,7 @@ struct oc_emb {
     float *row_scale = nullptr;   // [cap] 2^-s (NaN: a non-finite element)
     uint64_t n_rows = 0, cap = 0, n_live = 0;
     std::unordered_multimap<uint64_t, uint64_t> doc_rows;  // doc -> rows (for delete)
+    std::vector<uint64_t> dead;   // the rows tombstoned since the last compaction (n_rows - n_live of them), unsorted
 };
 
 // OC_EMB_F16=0: no fp16 copy for stores created while it is set, and searches use the tf32 sweep (A/B testing)
@@ -375,33 +381,40 @@ extern "C" void oc_emb_destroy(oc_emb *e) {
     delete e;
 }
 
-static int emb_grow(oc_emb *e, uint64_t want_rows) {
-    if (want_rows <= e->cap) return OC_OK;
+// Moves the store into fresh allocations of ncap >= n_rows rows.  An fp16 copy that finds no room is dropped (the
+// store stays whole and is swept through tf32 from now on) unless keep_f16: then the call fails and changes nothing.
+static int emb_realloc(oc_emb *e, uint64_t ncap, bool keep_f16) {
     oc_ctx *c = e->ctx;
-    uint64_t ncap = std::max<uint64_t>(want_rows, e->cap + e->cap / 2);
-    ncap = (ncap + 63) / 64 * 64;
     void *nr = nullptr; float *nn = nullptr; uint64_t *nd = nullptr;
-    CU(cudaMalloc(&nr, ncap * e->stride * e->esz));
-    CU(cudaMalloc(&nn, (ncap + 64) * sizeof(float)));
-    CU(cudaMalloc(&nd, ncap * sizeof(uint64_t)));
     uint16_t *nh = nullptr; float *ns = nullptr;
-    if (e->f16 && (cudaMalloc(&nh, ncap * e->stride * 2) != cudaSuccess || cudaMalloc(&ns, ncap * sizeof(float)) != cudaSuccess)) {
-        // no room for the fp16 copy: the store stays whole and is swept through tf32 from now on
+    auto undo = [&](int rc) { cudaFree(nr); cudaFree(nn); cudaFree(nd); cudaFree(nh); cudaFree(ns); return rc; };
+    if (cudaMalloc(&nr, ncap * e->stride * e->esz) != cudaSuccess || cudaMalloc(&nn, (ncap + 64) * sizeof(float)) != cudaSuccess ||
+        cudaMalloc(&nd, ncap * sizeof(uint64_t)) != cudaSuccess) {
         (void)cudaGetLastError();
+        return undo(fail(OC_ERR_OOM, "embedding store: no room for %llu rows", (unsigned long long)ncap));
+    }
+    if (e->f16 && (cudaMalloc(&nh, ncap * e->stride * 2) != cudaSuccess || cudaMalloc(&ns, ncap * sizeof(float)) != cudaSuccess)) {
+        (void)cudaGetLastError();
+        if (keep_f16) return undo(fail(OC_ERR_OOM, "embedding store: no room for the fp16 copy of %llu rows", (unsigned long long)ncap));
         cudaFree(nh); cudaFree(ns); nh = nullptr; ns = nullptr;
         cudaFree(e->rows_f16); cudaFree(e->row_scale); e->rows_f16 = nullptr; e->row_scale = nullptr;
         e->f16 = false;
     }
+    cudaError_t ce = cudaSuccess;
+    auto copy = [&](void *dst, const void *src, size_t bytes) {
+        if (ce == cudaSuccess) ce = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, c->stream);
+    };
     if (e->n_rows) {
-        CU(cudaMemcpyAsync(nr, e->rows, e->n_rows * e->stride * e->esz, cudaMemcpyDeviceToDevice, c->stream));
-        CU(cudaMemcpyAsync(nn, e->inv_norm, e->n_rows * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
-        CU(cudaMemcpyAsync(nd, e->row_doc, e->n_rows * sizeof(uint64_t), cudaMemcpyDeviceToDevice, c->stream));
+        copy(nr, e->rows, e->n_rows * e->stride * e->esz);
+        copy(nn, e->inv_norm, e->n_rows * sizeof(float));
+        copy(nd, e->row_doc, e->n_rows * sizeof(uint64_t));
         if (nh) {
-            CU(cudaMemcpyAsync(nh, e->rows_f16, e->n_rows * e->stride * 2, cudaMemcpyDeviceToDevice, c->stream));
-            CU(cudaMemcpyAsync(ns, e->row_scale, e->n_rows * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
+            copy(nh, e->rows_f16, e->n_rows * e->stride * 2);
+            copy(ns, e->row_scale, e->n_rows * sizeof(float));
         }
     }
-    CU(cudaStreamSynchronize(c->stream));
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(c->stream);
+    if (ce != cudaSuccess) return undo(fail(OC_ERR_CUDA, "embedding store: copy to the new allocation: %s", cudaGetErrorString(ce)));
     cudaFree(e->rows); cudaFree(e->inv_norm); cudaFree(e->row_doc);
     e->rows = nr; e->inv_norm = nn; e->row_doc = nd; e->cap = ncap;
     if (nh) {
@@ -409,6 +422,14 @@ static int emb_grow(oc_emb *e, uint64_t want_rows) {
         e->rows_f16 = nh; e->row_scale = ns;
     }
     return OC_OK;
+}
+
+// the capacity a store grown from empty to want_rows rows gets
+static uint64_t emb_round_cap(uint64_t want_rows) { return (want_rows + 63) / 64 * 64; }
+
+static int emb_grow(oc_emb *e, uint64_t want_rows) {
+    if (want_rows <= e->cap) return OC_OK;
+    return emb_realloc(e, emb_round_cap(std::max<uint64_t>(want_rows, e->cap + e->cap / 2)), false);
 }
 
 extern "C" int oc_emb_reserve(oc_emb *e, uint64_t n_rows) {
@@ -472,6 +493,7 @@ extern "C" int oc_emb_delete(oc_emb *e, const uint64_t *doc_ids, uint64_t n) {
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(c->stream));
     e->n_live -= rows.size();
+    e->dead.insert(e->dead.end(), rows.begin(), rows.end());
     return OC_OK;
 }
 
@@ -480,6 +502,132 @@ extern "C" int oc_emb_info(oc_emb *e, oc_emb_info_t *out) {
     out->num_embeddings = e->n_live; out->num_rows = e->n_rows; out->dimensions = e->dim; out->dtype = e->dtype;
     out->device_bytes = e->cap * (uint64_t(e->stride) * e->esz + 4 + 8);
     if (e->f16) out->device_bytes += e->cap * (uint64_t(e->stride) * 2 + 4);
+    return OC_OK;
+}
+
+// ---- compaction (emb_compact.cuh)
+// OC_EMB_COMPACT_WINDOW=<bytes>: the staging window of oc_emb_compact (tests use a small one to span many windows)
+static size_t compact_window_bytes() {
+    const char *v = getenv("OC_EMB_COMPACT_WINDOW");
+    const unsigned long long b = v ? strtoull(v, nullptr, 10) : 0;
+    return b ? (size_t)std::min<unsigned long long>(b, 128ull << 20) : size_t(32) << 20;
+}
+
+extern "C" int oc_emb_compact(oc_emb *e, uint32_t flags, oc_emb_compact_t *out) {
+    if (!e) return fail(OC_ERR_INVALID, "emb is NULL");
+    if (flags & ~OC_EMB_COMPACT_SHRINK) return fail(OC_ERR_INVALID, "oc_emb_compact: unknown flags 0x%x", flags);
+    oc_ctx *c = e->ctx;
+    std::lock_guard<std::mutex> g(c->mu);
+    CU(cudaSetDevice(c->device));
+    struct Release {   // every way out of the call gives the workspace back
+        oc_ctx *c;
+        ~Release() { cudaStreamSynchronize(c->stream); c->cmp_scan.release(); c->cmp_stage.release(); }
+    } release{c};
+    oc_emb_compact_t st{};
+    oc_emb_info_t inf{};
+    oc_emb_info(e, &inf);
+    st.rows_before = st.rows_after = e->n_rows;
+    st.device_bytes_before = st.device_bytes_after = inf.device_bytes;
+    if (!e->dead.empty()) {
+        std::vector<uint64_t> &dead = e->dead;
+        std::sort(dead.begin(), dead.end());
+        const uint64_t n = e->n_rows, first = dead[0];
+        const uint64_t n_words = (n + 31) / 32, n_blocks = (n_words + COMPACT_SCAN_WORDS - 1) / COMPACT_SCAN_WORDS;
+        std::vector<uint32_t> bits(n_words, 0);
+        for (uint64_t r : dead) bits[r >> 5] |= 1u << (r & 31);
+        // row windows of the matrix (W rows) and of the per-row arrays (16 B per row: Ws rows), one staging buffer
+        const size_t win = compact_window_bytes(), row_bytes = size_t(e->stride) * e->esz;
+        const uint64_t W = std::max<uint64_t>(1, win / row_bytes), Ws = std::max<uint64_t>(1, win / 16);
+        const size_t stage_bytes = std::max<size_t>(std::min<uint64_t>(W, n - first) * row_bytes, std::min<uint64_t>(Ws, n - first) * 16);
+        const size_t o_pre = (n_words * 4 + 255) & ~size_t(255), o_blk = o_pre * 2;
+        // everything that can fail for want of memory happens before the first row moves
+        OCTRY(c->cmp_scan.ensure(o_blk + n_blocks * 4));
+        OCTRY(c->cmp_stage.ensure(stage_bytes));
+        st.workspace_bytes = c->cmp_scan.cap + c->cmp_stage.cap;
+        uint32_t *d_bits = c->cmp_scan.as<uint32_t>(), *d_pre = d_bits + o_pre / 4, *d_blk = d_bits + o_blk / 4;
+        CU(cudaMemcpyAsync(d_bits, bits.data(), n_words * 4, cudaMemcpyHostToDevice, c->stream));
+        CU(cudaEventRecord(c->ev[EV_START], c->stream));
+        compact_scan_words_kernel<<<(unsigned)n_blocks, COMPACT_SCAN_WORDS, 0, c->stream>>>(d_bits, n_words, d_pre, d_blk);
+        launched(c);
+        compact_scan_blocks_kernel<<<1, COMPACT_SCAN_WORDS, 0, c->stream>>>(d_blk, (uint32_t)n_blocks);
+        launched(c);
+        CU(cudaGetLastError());
+        const unsigned max_grid = (unsigned)c->prop.multiProcessorCount * 8;
+        auto grid_for = [&](uint64_t items, uint64_t per_block) {
+            return (unsigned)std::min<uint64_t>(max_grid, std::max<uint64_t>(1, (items + per_block - 1) / per_block));
+        };
+        auto dead_below = [&](uint64_t r) { return uint64_t(std::lower_bound(dead.begin(), dead.end(), r) - dead.begin()); };
+        // Windows of source rows [a, b) in ascending order on one stream, starting at the first dead row (the rows
+        // below it keep their place).  A window's live rows go to [dst, dst + live) with dst = a - dead_below(a) <= a
+        // and live <= b - a, so the store ends at or below b: it overwrites only rows of this window, which the
+        // gather before it has read in full, and rows of earlier windows, which have been stored already.  Nothing of
+        // a later window is touched before its own gather reads it.
+        auto move = [&](uint64_t w_rows, auto &&gather, auto &&store) -> int {
+            for (uint64_t a = first; a < n; a += w_rows) {
+                const uint64_t b = std::min(n, a + w_rows), below = dead_below(a), live = (b - a) - (dead_below(b) - below);
+                if (!live) continue;
+                gather(a, b, a - below);
+                store(a - below, live);
+                CU(cudaGetLastError());
+            }
+            return OC_OK;
+        };
+        auto move_rows = [&](void *rows, uint32_t esz) -> int {   // the matrix or its fp16 copy, same stride
+            const uint64_t row_vec = uint64_t(e->stride) * esz / 16;
+            return move(W,
+                [&](uint64_t a, uint64_t b, uint64_t dst) {
+                    const unsigned grid = grid_for(b - a, COMPACT_THREADS / 32);
+                    if (esz == 2) compact_gather_kernel<2><<<grid, COMPACT_THREADS, 0, c->stream>>>(
+                        rows, e->stride, a, b, dst, d_bits, d_pre, d_blk, c->cmp_stage.as<uint4>());
+                    else compact_gather_kernel<4><<<grid, COMPACT_THREADS, 0, c->stream>>>(
+                        rows, e->stride, a, b, dst, d_bits, d_pre, d_blk, c->cmp_stage.as<uint4>());
+                    launched(c);
+                },
+                [&](uint64_t dst, uint64_t live) {
+                    compact_store_kernel<<<grid_for(live * row_vec, COMPACT_THREADS * 4), COMPACT_THREADS, 0, c->stream>>>(
+                        c->cmp_stage.as<uint4>(), static_cast<uint4 *>(rows) + dst * row_vec, live * row_vec);
+                    launched(c);
+                });
+        };
+        OCTRY(move_rows(e->rows, e->esz));
+        if (e->f16) OCTRY(move_rows(e->rows_f16, 2));
+        const uint64_t ws_rows = std::min<uint64_t>(Ws, n - first);
+        uint64_t *st_doc = c->cmp_stage.as<uint64_t>();
+        float *st_inv = reinterpret_cast<float *>(st_doc + ws_rows), *st_scale = e->f16 ? st_inv + ws_rows : nullptr;
+        float *row_scale = e->f16 ? e->row_scale : nullptr;
+        OCTRY(move(Ws,
+            [&](uint64_t a, uint64_t b, uint64_t dst) {
+                compact_small_gather_kernel<<<(unsigned)((b - a + COMPACT_THREADS - 1) / COMPACT_THREADS), COMPACT_THREADS, 0, c->stream>>>(
+                    e->inv_norm, e->row_doc, row_scale, a, b, dst, d_bits, d_pre, d_blk, st_doc, st_inv, st_scale);
+                launched(c);
+            },
+            [&](uint64_t dst, uint64_t live) {
+                compact_small_store_kernel<<<(unsigned)((live + COMPACT_THREADS - 1) / COMPACT_THREADS), COMPACT_THREADS, 0, c->stream>>>(
+                    st_doc, st_inv, st_scale, live, e->row_doc + dst, e->inv_norm + dst, row_scale ? row_scale + dst : nullptr);
+                launched(c);
+            }));
+        CU(cudaEventRecord(c->ev[EV_DEV], c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        cudaEventElapsedTime(&st.device_ms, c->ev[EV_START], c->ev[EV_DEV]);
+        for (auto &dr : e->doc_rows) dr.second -= dead_below(dr.second);
+        st.rows_moved = e->n_live - first;
+        e->n_rows = e->n_live;
+        dead.clear();
+        st.rows_after = e->n_rows;
+    }
+    if ((flags & OC_EMB_COMPACT_SHRINK) && e->cap > emb_round_cap(e->n_rows)) {
+        if (e->n_rows == 0) {
+            CU(cudaStreamSynchronize(c->stream));
+            cudaFree(e->rows); cudaFree(e->inv_norm); cudaFree(e->row_doc); cudaFree(e->rows_f16); cudaFree(e->row_scale);
+            e->rows = nullptr; e->inv_norm = nullptr; e->row_doc = nullptr; e->rows_f16 = nullptr; e->row_scale = nullptr;
+            e->cap = 0;
+        } else if (emb_realloc(e, emb_round_cap(e->n_rows), true) == OC_ERR_CUDA) {
+            return OC_ERR_CUDA;   // (no room for the smaller allocation: the store stays compacted at its old capacity)
+        }
+        oc_emb_info(e, &inf);
+        st.device_bytes_after = inf.device_bytes;
+    }
+    if (out) *out = st;
     return OC_OK;
 }
 

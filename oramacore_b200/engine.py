@@ -165,6 +165,14 @@ class EmbeddingFieldStorage:
         d = np.ascontiguousarray(np.atleast_1d(np.asarray(doc_id, np.uint64)).ravel())
         check(lib().oc_emb_delete(self._h, _p(d), int(d.shape[0])))
 
+    def compact(self, shrink: bool = False) -> dict:
+        """compact() as Index::commit runs it (index/mod.rs:583-590): drop the deleted rows on the device, in place and
+        order-preserving, so that searches return what they returned before.  shrink=True also gives the capacity
+        beyond num_rows back.  Returns the call's statistics (oc_emb_compact_t)."""
+        st = _lib.EmbCompact()
+        check(lib().oc_emb_compact(self._h, _lib.OC_EMB_COMPACT_SHRINK if shrink else 0, C.byref(st)))
+        return st.as_dict()
+
     def info(self) -> dict:
         i = _lib.EmbInfo()
         check(lib().oc_emb_info(self._h, C.byref(i)))

@@ -15,7 +15,7 @@ and `commit` / `compact` lay the pending data out (`CURRENT` + `versions/<n>`, e
 `IndexLoader.apply(op)` takes the same operations as plain dicts (the JSON shape of the reference's enum), resolves
 terms to stable term ids through the native dictionary (oc_dict_*), and drives the C ABI: oc_str_insert /
 oc_str_delete / oc_str_commit (snapshot swap: searches keep running on the previous version while a commit builds
-the next), oc_emb_insert / oc_emb_delete (live).  `refresh_facets()` lays the accumulated filter fields out for
+the next), oc_emb_insert / oc_emb_delete (live) and oc_emb_compact at commit.  `refresh_facets()` lays the accumulated filter fields out for
 oc_search_facets and rebuilds the geopoint field handles (`geo`, oc_geo_field_*); `where_filter(where)` evaluates a
 where-clause over them (where.py).  tf of a term = number of positions (exact + stemmed), as StringStorage counts them."""
 from __future__ import annotations
@@ -140,8 +140,11 @@ class IndexLoader:
 
     def commit(self) -> None:
         """ReadSide::commit -> field compact(): publish the next snapshot of the string store (searches on the
-        previous one keep running meanwhile) and refresh the facet layout and the geopoint fields."""
+        previous one keep running meanwhile), drop the deleted rows of the embedding store (index/mod.rs:583-590) and
+        refresh the facet layout and the geopoint fields."""
         self.strs.commit()
+        if self.emb is not None:
+            self.emb.compact()
         # N of the idf is Index::document_count (mod.rs:1460: +1 per Index op, also for documents without string fields)
         self.strs.set_global(max(self.document_count, 0))
         self._uncommitted_deleted.clear()

@@ -25,6 +25,20 @@ pub const OC_MODE_VECTOR: c_int = 1;
 pub const OC_MODE_HYBRID: c_int = 2;
 pub const OC_DTYPE_F32: c_int = 0;
 pub const OC_DTYPE_BF16: c_int = 1;
+/// `oc_emb_compact` flag: also give the capacity beyond `num_rows` back.
+pub const OC_EMB_COMPACT_SHRINK: u32 = 1;
+/// Statistics of one `oc_emb_compact` call (`oc_emb_compact_t`).
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct OcEmbCompact {
+    pub rows_before: u64,
+    pub rows_after: u64,
+    pub rows_moved: u64,
+    pub device_bytes_before: u64,
+    pub device_bytes_after: u64,
+    pub workspace_bytes: u64,
+    pub device_ms: f32,
+}
 /// `OcSearchParams::sharded`: merge across `oc_comm` ranks; add `OC_SHARD_TOMBSTONES` on every rank while
 /// any rank's string store holds uncommitted deletes (the df all-reduce must be entered by all ranks).
 pub const OC_SHARDED: c_int = 1;
@@ -176,6 +190,7 @@ extern "C" {
     pub fn oc_emb_destroy(emb: *mut OcEmb);
     pub fn oc_emb_insert(emb: *mut OcEmb, doc_ids: *const u64, rows: *const c_void, n: u64) -> c_int;
     pub fn oc_emb_delete(emb: *mut OcEmb, doc_ids: *const u64, n: u64) -> c_int;
+    pub fn oc_emb_compact(emb: *mut OcEmb, flags: u32, out: *mut OcEmbCompact) -> c_int;
     pub fn oc_emb_search(emb: *mut OcEmb, queries: *const f32, b: u32, limit: u32, similarity: f32,
                          filter_bits: *const u64, filter_nbits: u64, out_doc_ids: *mut u64,
                          out_scores: *mut f32, out_counts: *mut u32) -> c_int;
@@ -366,6 +381,12 @@ impl EmbeddingField {
     }
     /// delete(DocumentId)  (embedding_field.rs:240-242)
     pub fn delete(&self, doc_id: u64) -> anyhow::Result<()> { check(unsafe { oc_emb_delete(self.h, &doc_id, 1) }) }
+    /// compact() as Index::commit runs it (index/mod.rs:583-590): drops the deleted rows on the device, in place
+    pub fn compact(&self, shrink: bool) -> anyhow::Result<OcEmbCompact> {
+        let mut st = OcEmbCompact::default();
+        check(unsafe { oc_emb_compact(self.h, if shrink { OC_EMB_COMPACT_SHRINK } else { 0 }, &mut st) })?;
+        Ok(st)
+    }
     /// search(&VectorSearchParams, &mut HashMap)  (embedding_field.rs:250-278): `output[doc] += score`
     pub fn search(&self, target: &[f32], similarity: f32, limit: usize, filter: Option<(&[u64], u64)>,
                   output: &mut std::collections::HashMap<u64, f32>) -> anyhow::Result<()> {
