@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -19,6 +20,7 @@
 
 #include "bm25.cuh"
 #include "comm.h"
+#include "dense_cache.h"
 #include "dict.h"
 #include "stem_en.h"
 #include "emb_compact.cuh"
@@ -197,6 +199,8 @@ struct oc_ctx {
     // oc_emb_compact: the dead-row bitmap with its scan, and the staging window the rows move through (held for the
     // call only: a compaction is rare and its window is large)
     DevBuf cmp_scan, cmp_stage;
+    // the dense contribution arrays of hot terms, kept across calls (dense_cache.h)
+    DenseCache dense_cache;
 
     HostBuf h_in, h_out, h_in0;   // h_in0 / in_blob0: query vectors + filter, uploaded before the descriptors
     OcComm comm;
@@ -212,6 +216,7 @@ struct oc_ctx {
         for (int r = 0; r < 16; r++) if (p2p.ready && p2p.peer[r] && p2p.peer[r] != p2p.local) cudaIpcCloseMemHandle(p2p.peer[r]);
         if (p2p.local) cudaFree(p2p.local);
         comm.destroy();
+        if (stream) { dense_cache.clear(stream); cudaStreamSynchronize(stream); }
         for (int i = 0; i < EV_N; i++) if (ev[i]) cudaEventDestroy(ev[i]);
         if (stream) cudaStreamDestroy(stream);
         if (side) cudaStreamDestroy(side);
@@ -1100,9 +1105,16 @@ struct StrField {
     uint64_t n_post = 0;
     std::vector<PostingRaw> host_post;   // host copy of the committed postings (term-major), kept for oc_str_commit
 };
+// a process-wide identity per snapshot state: a new snapshot takes one, and so does every change made to a published
+// snapshot in place (a field load, corpus-wide values, tombstones).  Keys the dense-array cache (dense_cache.h).
+static uint64_t next_snap_ident() {
+    static std::atomic<uint64_t> n{0};
+    return ++n;
+}
 struct StrSnap {
     int device = 0;
     uint64_t version = 0;
+    uint64_t ident = next_snap_ident();
     std::vector<StrField> fields;
     uint64_t n_rows = 0, document_count = 0;
     std::vector<uint64_t> row_doc_host;  // empty => identity
@@ -1205,6 +1217,7 @@ extern "C" int oc_str_set_global(oc_str *s, uint64_t document_count, const float
     std::lock_guard<std::mutex> g(c->mu);
     std::lock_guard<std::mutex> g2(s->mu);
     StrSnap &S = *s->cur;
+    S.ident = next_snap_ident();
     S.document_count = document_count;
     if (avg_field_len)
         for (size_t i = 0; i < S.fields.size(); i++)
@@ -1225,6 +1238,7 @@ extern "C" int oc_str_load_field(oc_str *s, uint32_t field, float avg_field_len,
     StrSnap &S = *snap;
     if (field >= S.fields.size()) return fail(OC_ERR_INVALID, "field %u out of range", field);
     StrField &f = S.fields[field];
+    S.ident = next_snap_ident();
     cudaFree(f.post); f.post = nullptr; cudaFree(f.raw); f.raw = nullptr; f.b_cached = -1.f;
     const uint64_t np = term_offsets[n_terms];
     if (np && (!post_row || !post_tf || !post_len)) return fail(OC_ERR_INVALID, "posting arrays are NULL");
@@ -1253,6 +1267,7 @@ extern "C" int oc_str_load_field(oc_str *s, uint32_t field, float avg_field_len,
 // tombstones `rows` of snapshot S (host bitmap + device copy on stream st)
 static int snap_tombstone(StrSnap &S, const std::vector<uint64_t> &rows, cudaStream_t st) {
     if (rows.empty() || S.n_rows == 0) return OC_OK;
+    S.ident = next_snap_ident();
     const uint64_t words = (S.n_rows + BM25_TILE - 1) / BM25_TILE * (BM25_TILE / 32);
     if (S.alive_host.empty()) {
         S.alive_host.assign(words, 0xffffffffu);
@@ -2182,11 +2197,15 @@ struct SearchCall {
     size_t fwords = 0;
     const uint64_t *filter_dev = nullptr;
     // fulltext descriptors.  max_tokens: tokens of the longest query; dense_bytes: the dense contribution arrays of the
-    // batch (zeroed before the precompute kernel fills them); term_key: (field << 32 | term id) of each expanded term;
+    // batch in c->dense_buf, dense_new: those built into the ctx's dense-array cache (both zeroed before the precompute
+    // kernel fills them); dense_seen: the snapshots the cache's sweep looked at (released after the ctx lock);
+    // term_key: (field << 32 | term id) of each expanded term;
     // tok_slot: per-query filters, the fulltext slot of each token's query; q_perm: the register-folded scorers' item order
     bool multi_rank = false, tombs = false, thr = false, count_df = false, any_multi = false, need_df = false, derived_now = false;
     uint32_t n_tiles = 0, max_tokens = 0, cls_nq[BM25_CLASSES] = {0, 0, 0, 0, 0};
     uint64_t dense_bytes = 0, postings_walked = 0;
+    std::vector<DenseEntry *> dense_new;
+    std::vector<std::shared_ptr<StrSnap>> dense_seen;
     std::vector<TermDesc> terms;
     std::vector<TokenDesc> tokens;
     std::vector<QueryDesc> queries;
@@ -2525,14 +2544,65 @@ static int vector_first(SearchCall &k) {
     return OC_OK;
 }
 
+// OC_BM25_DENSE_CACHE_MB (default 2048, enough for the hot terms of a 10M-row store): the device memory a ctx keeps
+// dense arrays of hot terms in across calls; 0 builds every call's arrays from scratch into c->dense_buf
+static uint64_t dense_cache_budget() {
+    const char *v = getenv("OC_BM25_DENSE_CACHE_MB");
+    return (v && *v ? strtoull(v, nullptr, 10) : 2048ull) << 20;
+}
+
+// Frees the kept arrays no call can read any more: their snapshot is gone or has changed (its ident moved on), or the
+// call that was to build them failed first.  The snapshots looked at are held by the call until it has left the ctx
+// lock, so a last reference never frees a snapshot under it.
+static void dense_cache_sweep(SearchCall &k) {
+    oc_ctx *c = k.c; DenseCache &dc = c->dense_cache;
+    cudaStream_t ps = k.side ? c->side : c->stream;
+    for (auto it = dc.map.begin(); it != dc.map.end();) {
+        std::shared_ptr<StrSnap> s = it->second.snap.lock();
+        const bool live = s && s->ident == it->first.snap && it->second.ready;
+        if (s) k.dense_seen.push_back(std::move(s));
+        it = live ? std::next(it) : dc.drop(it, ps);
+    }
+}
+
+// The kept array of each of the call's dense terms (keys[i], `bytes` each).  A hit is read as it is (arr[i], build[i]
+// = 0).  A miss gets a new array that this call builds (build[i] = 1) while the budget allows, evicting the least
+// recently used arrays this call does not read.  arr[i] = NULL: the term's array goes in c->dense_buf, as every one
+// does when a row bitmap masks the call's arrays (filter, tombstones, df counted on the device) or the budget is 0.
+static void dense_cache_bind(SearchCall &k, const std::vector<DenseKey> &keys, uint64_t bytes, std::vector<float *> &arr,
+                             std::vector<uint8_t> &build) {
+    oc_ctx *c = k.c; DenseCache &dc = c->dense_cache;
+    cudaStream_t ps = k.side ? c->side : c->stream;
+    const uint64_t budget = dense_cache_budget();
+    arr.assign(keys.size(), nullptr);
+    build.assign(keys.size(), 0);
+    if (!budget || k.filter || k.tombs || k.need_df) return;
+    dc.tick++;
+    dc.in_call = 0;
+    for (size_t i = 0; i < keys.size(); i++) {
+        auto it = dc.map.find(keys[i]);
+        if (it != dc.map.end()) { it->second.last_use = dc.tick; dc.in_call += bytes; arr[i] = it->second.p; continue; }
+        if (dc.in_call + bytes > budget) continue;
+        while (dc.used + bytes > budget && dc.evict_one(ps)) {}
+        float *p = nullptr;
+        if (cudaMallocAsync(reinterpret_cast<void **>(&p), bytes, ps) != cudaSuccess) { cudaGetLastError(); continue; }   // device full: c->dense_buf
+        DenseEntry &e = dc.map[keys[i]];
+        e.p = p; e.bytes = bytes; e.last_use = dc.tick; e.snap = k.snap;
+        dc.used += bytes; dc.in_call += bytes;
+        arr[i] = p; build[i] = 1;
+        k.dense_new.push_back(&e);
+    }
+}
+
 // Batch-level sharing of per-posting contributions (single-term tokens with a host-known idf) and the dense form of
 // hot terms.  Not with per-query filters: the precomputed contributions and dense arrays are masked by ONE row bitmap.
 static int ft_share_dense(SearchCall &k) {
     oc_ctx *c = k.c;
+    if (!c->dense_cache.map.empty()) dense_cache_sweep(k);
     std::vector<TermDesc> &terms = k.terms;
     const std::vector<TokenDesc> &tokens = k.tokens;
-    struct U { uint32_t first_e; uint32_t uses; };
     struct K128 { uint64_t a, b; };            // (field, term) | (weight bits, idf bits)
+    struct U { uint32_t first_e; uint32_t uses; K128 key; };
     size_t cap_t = 64;
     while (cap_t < tokens.size() * 2) cap_t <<= 1;
     std::vector<K128> tab_k(cap_t);
@@ -2553,7 +2623,7 @@ static int ft_share_dense(SearchCall &k) {
         while (tab_v[slot] != 0xffffffffu && !(tab_k[slot].a == key.a && tab_k[slot].b == key.b)) slot = (slot + 1) & (cap_t - 1);
         if (tab_v[slot] == 0xffffffffu) {
             tab_k[slot] = key; tab_v[slot] = (uint32_t)uniq.size();
-            uniq.push_back({e, 0}); distinct += terms[e].len;
+            uniq.push_back({e, 0, key}); distinct += terms[e].len;
         }
         uniq[tab_v[slot]].uses++;
         e_to_u[e] = tab_v[slot];
@@ -2581,20 +2651,43 @@ static int ft_share_dense(SearchCall &k) {
     const bool lists = distinct_l && !share_off && (share_force || (walked_l >= 2 * distinct_l && walked_l >= (64u << 20))) &&
                        distinct_l * 8 <= (size_t(6) << 30);
     if (!lists && !n_dense) return OC_OK;
+    // each dense term's array: a kept one of the ctx's cache (read as it is on a hit, built by this call on a miss), or
+    // one in this call's c->dense_buf
+    std::vector<float *> u_arr(uniq.size(), nullptr);
+    std::vector<uint8_t> u_kept(uniq.size(), 0);
+    if (n_dense) {
+        std::vector<DenseKey> keys;
+        std::vector<uint32_t> key_u;
+        uint32_t kb, bb;
+        memcpy(&kb, &k.p->bm25_k, 4); memcpy(&bb, &k.p->bm25_b, 4);
+        for (size_t u = 0; u < uniq.size(); u++)
+            if (u_dense[u]) {
+                keys.push_back(DenseKey{k.S->ident, uniq[u].key.a, uint32_t(uniq[u].key.b >> 32), uint32_t(uniq[u].key.b), kb, bb});
+                key_u.push_back((uint32_t)u);
+            }
+        std::vector<float *> arr;
+        std::vector<uint8_t> build;
+        dense_cache_bind(k, keys, rows_pad * 4, arr, build);
+        for (size_t i = 0; i < keys.size(); i++) { u_arr[key_u[i]] = arr[i]; u_kept[key_u[i]] = arr[i] && !build[i]; }
+    }
+    uint64_t n_buf = 0;
+    for (size_t u = 0; u < uniq.size(); u++) n_buf += u_dense[u] && !u_arr[u];
     if (lists) OCTRY(c->pre_post.ensure(distinct_l * 8 + 64));
-    if (n_dense) OCTRY(c->dense_buf.ensure(n_dense * rows_pad * 4));
-    k.dense_bytes = n_dense * rows_pad * 4;
+    if (n_buf) OCTRY(c->dense_buf.ensure(n_buf * rows_pad * 4));
+    k.dense_bytes = n_buf * rows_pad * 4;
     uint64_t off = 0, doff = 0;
     std::vector<uint64_t> u_off(uniq.size());
     std::vector<uint8_t> u_used(uniq.size(), 0);
     for (size_t u = 0; u < uniq.size(); u++) {
         if (!u_dense[u] && !lists) continue;
         u_used[u] = 1;
+        if (u_dense[u] && !u_arr[u]) { u_arr[u] = c->dense_buf.as<float>() + doff; doff += rows_pad; }
+        if (u_kept[u]) continue;   // a cache hit: nothing to build
         const TermDesc &td = terms[uniq[u].first_e];
         PreDesc pd{};
         pd.src = td.ptr; pd.len = td.len; pd.weight = td.weight;
         pd.idf = tokens[k.term_token[uniq[u].first_e]].idf;
-        if (u_dense[u]) { u_off[u] = doff; pd.dense = c->dense_buf.as<float>() + doff; doff += rows_pad; }
+        if (u_dense[u]) pd.dense = u_arr[u];
         else { u_off[u] = off; pd.dst = c->pre_post.as<Posting>() + off; off += td.len; }
         const uint32_t pi = (uint32_t)k.pre_descs.size();
         k.pre_descs.push_back(pd);
@@ -2603,7 +2696,7 @@ static int ft_share_dense(SearchCall &k) {
     for (size_t e = 0; e < terms.size(); e++) {
         const uint32_t u = e_to_u[e];
         if (u == 0xffffffffu || !u_used[u]) continue;
-        if (u_dense[u]) { terms[e].ptr = reinterpret_cast<const Posting *>(c->dense_buf.as<float>() + u_off[u]); terms[e].flags |= TD_DENSE; }
+        if (u_dense[u]) { terms[e].ptr = reinterpret_cast<const Posting *>(u_arr[u]); terms[e].flags |= TD_DENSE; }
         else { terms[e].ptr = c->pre_post.as<Posting>() + u_off[u]; terms[e].flags |= TD_PRE; }
     }
     return OC_OK;
@@ -2634,8 +2727,7 @@ static void bm25_item_order(SearchCall &k) {
         for (uint32_t q = 0; q < B; q++) if (nd_q[q] == nd) k.q_perm[at[cls_of(q)]++] = q;
 }
 
-// The fulltext descriptors: terms, tokens and queries, each token's idf where the host knows it, the sharing / dense
-// selection and the scorers' item order.
+// The fulltext descriptors: terms, tokens and queries, and each token's idf where the host knows it.
 static int ft_descriptors(SearchCall &k) {
     oc_ctx *c = k.c; const oc_search_params *p = k.p;
     const uint32_t B = k.B; StrSnap *S = k.S;
@@ -2728,6 +2820,26 @@ static int ft_descriptors(SearchCall &k) {
     if (df_local_only && !k.count_df)
         return fail(OC_ERR_INVALID, "sharded search: a field of this shard has no corpus-wide df table (dropped by a commit?): "
                                     "reload it or pass OC_SHARD_COUNT_DF on every rank");
+    return OC_OK;
+}
+
+// The stream of the fulltext stage.  Hybrid: the descriptors, the shared-contribution precompute, the filter bitmap
+// and the (term, tile) plan do not depend on the vector results: they run on the side stream while the main stream
+// sweeps the matrix (OC_SIDE_STREAM=0 disables it: the step gets ~2.5 % longer, the sweep itself ~4 % shorter — A/B
+// switch).  Chosen before the dense arrays are: kept arrays are allocated and freed on it.
+static int ft_stream(SearchCall &k) {
+    oc_ctx *c = k.c;
+    const char *senv = getenv("OC_SIDE_STREAM");
+    // (single-GPU only for now: the sharded path was measured and validated without it)
+    k.side = !(senv && senv[0] == '0') && k.has_v && k.has_ft && !k.need_df && !k.derived_now;
+    if (c->side_dirty) { CU(cudaStreamSynchronize(c->side)); c->side_dirty = false; }   // leftover of a failed call
+    if (k.side) { CU(cudaStreamWaitEvent(c->side, c->ev[EV_H2D], 0)); c->side_dirty = true; }   // the filter bitmap went up with the query vectors
+    return OC_OK;
+}
+
+// The sharing / dense selection and the scorers' item order.
+static int ft_share(SearchCall &k) {
+    if (!k.has_ft) return OC_OK;
     if (!k.per_q) OCTRY(ft_share_dense(k));
     if (!k.any_multi && k.max_tokens <= BM25_FLAT_TOK) bm25_item_order(k);
     return OC_OK;
@@ -2844,15 +2956,8 @@ static int main_upload(SearchCall &k) {
         k.s_plan = pk.add(k.q_plan.data(), B);
         k.s_page = pk.add(k.q_page.data(), B);
     }
-    // hybrid: the descriptors, the shared-contribution precompute, the filter bitmap and the (term, tile) plan do
-    // not depend on the vector results: they run on the side stream while the main stream sweeps the matrix
-    // (OC_SIDE_STREAM=0 disables it: the step gets ~2.5 % longer, the sweep itself ~4 % shorter — A/B switch)
-    const char *senv = getenv("OC_SIDE_STREAM");
-    // (single-GPU only for now: the sharded path was measured and validated without it)
-    k.side = !(senv && senv[0] == '0') && k.has_v && k.has_ft && !k.need_df && !k.derived_now;
+    // (the stream of the fulltext stage, k.side, was chosen by ft_stream)
     if (!k.has_v) CU(cudaEventRecord(c->ev[EV_START], c->stream));
-    if (c->side_dirty) { CU(cudaStreamSynchronize(c->side)); c->side_dirty = false; }   // leftover of a failed call
-    if (k.side) { CU(cudaStreamWaitEvent(c->side, c->ev[EV_H2D], 0)); c->side_dirty = true; }   // the filter bitmap went up with the query vectors
     OCTRY(upload(pk, c->h_in, c->in_blob, k.side ? c->side : c->stream));
     if (!k.has_v) CU(cudaEventRecord(c->ev[EV_H2D], c->stream));   // hybrid/vector: this copy rides inside the device window
     c->timing.h2d_bytes = k.pk0.total + pk.total;
@@ -2916,9 +3021,11 @@ static int bm25_stage(SearchCall &k) {
     }
     if (!k.pre_items.empty()) {
         if (k.dense_bytes) CU(cudaMemsetAsync(c->dense_buf.p, 0, k.dense_bytes, ps));
+        for (const DenseEntry *e : k.dense_new) CU(cudaMemsetAsync(e->p, 0, e->bytes, ps));
         bm25_precompute_kernel<<<(unsigned)k.pre_items.size(), 256, 0, ps>>>(k.s_pre.at(din), k.s_pitems.at(din), p->bm25_k, k.row_ok);
         launched(c);
         CU(cudaGetLastError());
+        for (DenseEntry *e : k.dense_new) e->ready = true;   // later calls may read them (after this stream's work)
     }
     const size_t n_td = k.terms.size();
     OCTRY(c->seg.ensure((n_td * (size_t(n_tiles) + 1) + 1) * 4));
@@ -3375,6 +3482,8 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const SearchReq &r) 
     if (k.p->q_where) OCTRY(where_stage(k));
     OCTRY(vector_first(k));
     OCTRY(ft_descriptors(k));
+    OCTRY(ft_stream(k));
+    OCTRY(ft_share(k));
     OCTRY(omc_plan(k));
     sort_group_plan(k);
     OCTRY(main_upload(k));
