@@ -74,6 +74,13 @@ int oc_device_info(oc_ctx *ctx, int *sm_count, size_t *hbm_bytes, char *name, si
 #define OC_COMM_ID_BYTES 128
 int oc_comm_unique_id(uint8_t out_id[OC_COMM_ID_BYTES]);
 int oc_comm_init(oc_ctx *ctx, int world_size, int rank, const uint8_t id[OC_COMM_ID_BYTES]);
+/* In-process group: ctxs[r] becomes rank r of `world` ranks (1..16 distinct contexts of this process, e.g. several
+ * on one GPU, which NCCL refuses).  The collectives of a sharded oc_search then run on the calling threads through
+ * host memory: each rank drains its own stream, copies its bytes to the host, waits for the other ranks (host
+ * condition variable, fixed timeout) and copies the result back.  Every rank calls oc_search on its own thread.
+ * Ranks that call different collectives (kind or size) all get OC_ERR_COMM and the group stays usable; a timeout,
+ * or an oc_shutdown of one of the contexts, fails every later collective of the group. */
+int oc_comm_init_local(oc_ctx *const *ctxs, int world);
 /* Optional: direct NVLink exchange of the per-shard top-k records instead of the NCCL all-gather.  After
  * oc_comm_init every rank exports the CUDA-IPC handle of its receive window, the host runtime all-gathers the
  * blobs (world x OC_P2P_HANDLE_BYTES, rank order) and every rank imports them.  From then on the pack kernel of a

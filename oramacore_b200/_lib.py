@@ -36,7 +36,7 @@ OC_WHERE_MAX_DEPTH = 32
 
 EXPORTED_SYMBOLS = [
     "oc_last_error", "oc_version", "oc_abi_sizes", "oc_init", "oc_shutdown", "oc_device_info", "oc_comm_unique_id",
-    "oc_comm_init", "oc_comm_p2p_export", "oc_comm_p2p_import", "oc_emb_create", "oc_emb_destroy", "oc_emb_reserve", "oc_emb_insert", "oc_emb_delete", "oc_emb_compact",
+    "oc_comm_init", "oc_comm_init_local", "oc_comm_p2p_export", "oc_comm_p2p_import", "oc_emb_create", "oc_emb_destroy", "oc_emb_reserve", "oc_emb_insert", "oc_emb_delete", "oc_emb_compact",
     "oc_emb_info", "oc_emb_search", "oc_str_create", "oc_str_destroy", "oc_str_set_rows", "oc_str_load_field",
     "oc_str_insert", "oc_str_commit", "oc_str_delete", "oc_str_info", "oc_str_set_global", "oc_search", "oc_pinned_alloc", "oc_pinned_free", "oc_last_timing", "oc_launch_count",
     "oc_batcher_create", "oc_batcher_create2", "oc_batcher_destroy", "oc_batcher_search", "oc_batcher_search_sorted", "oc_batcher_search_groups",
@@ -179,6 +179,7 @@ def lib():
     L.oc_device_info.argtypes = [vp, C.POINTER(i32), C.POINTER(C.c_size_t), C.c_char_p, C.c_size_t]
     L.oc_comm_unique_id.argtypes = [vp]
     L.oc_comm_init.argtypes = [vp, i32, i32, vp]
+    L.oc_comm_init_local.argtypes = [vp, i32]
     L.oc_comm_p2p_export.argtypes = [vp, vp]
     L.oc_comm_p2p_import.argtypes = [vp, vp]
     L.oc_emb_create.argtypes = [vp, u32, i32, i32, C.POINTER(vp)]

@@ -66,15 +66,17 @@ extern "C" void oc_abi_sizes(size_t out[4]) {
 }
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is per (device, function): remember what was configured
-// per device so several contexts on different GPUs in one process each get their kernels configured
-static bool smem_cfg_needed(int device, const void *fn, size_t smem) {
+// per device so several contexts on different GPUs in one process each get their kernels configured.  The attribute
+// is set under the lock: a context sharing the device with another must not launch before the size it relies on is set.
+static cudaError_t smem_cfg(int device, const void *fn, size_t smem) {
     static std::mutex mu;
     static std::map<std::pair<int, const void *>, size_t> done;
     std::lock_guard<std::mutex> g(mu);
     size_t &v = done[std::make_pair(device, fn)];
-    if (smem <= v) return false;
-    v = smem;
-    return true;
+    if (smem <= v) return cudaSuccess;
+    const cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) v = smem;
+    return e;
 }
 
 // ------------------------------------------------------------------------------------ buffers
@@ -158,6 +160,7 @@ constexpr size_t P2P_WIN_BYTES = size_t(1) << 20;   // per (parity, source rank)
 constexpr uint32_t P2P_MAX_Q = 4096;
 constexpr size_t P2P_FLAG_BYTES = size_t(2) * P2P_MAX_Q * 4;
 constexpr uint32_t P2P_MAX_WORLD = 16;
+constexpr uint32_t LOCAL_MAX_WORLD = 16;   // oc_comm_init_local: = SHARD_MAX_WORLD (shard.cuh), the merge's largest world
 
 struct oc_ctx {
     int device = 0;
@@ -296,6 +299,20 @@ extern "C" int oc_comm_init(oc_ctx *c, int world, int rank, const uint8_t id[OC_
     if (!c->comm.init(world, rank, id, &err)) return fail(OC_ERR_COMM, "%s", err.c_str());
     return OC_OK;
 }
+extern "C" int oc_comm_init_local(oc_ctx *const *ctxs, int world) {
+    if (!ctxs || world < 1 || world > (int)LOCAL_MAX_WORLD) return fail(OC_ERR_INVALID, "oc_comm_init_local: 1..%u contexts", LOCAL_MAX_WORLD);
+    for (int r = 0; r < world; r++) {
+        if (!ctxs[r]) return fail(OC_ERR_INVALID, "oc_comm_init_local: ctxs[%d] is NULL", r);
+        for (int s = 0; s < r; s++)
+            if (ctxs[s] == ctxs[r]) return fail(OC_ERR_INVALID, "oc_comm_init_local: ctxs[%d] == ctxs[%d]", s, r);
+    }
+    auto g = std::make_shared<LocalGroup>(world);
+    for (int r = 0; r < world; r++) {
+        std::lock_guard<std::mutex> lk(ctxs[r]->mu);
+        ctxs[r]->comm.init_local(g, r);
+    }
+    return OC_OK;
+}
 
 // Direct NVLink exchange: rank r exports the IPC handle of its window, the host runtime all-gathers the blobs (like
 // the NCCL unique id) and every rank maps all peers' windows.  Afterwards the sharded oc_search stores each query's
@@ -303,6 +320,7 @@ extern "C" int oc_comm_init(oc_ctx *c, int world, int rank, const uint8_t id[OC_
 // counters — no library collective on the data path (ncclAllGather stays the fallback for batches larger than a window).
 extern "C" int oc_comm_p2p_export(oc_ctx *c, uint8_t out[OC_P2P_HANDLE_BYTES]) {
     if (!c || !out) return fail(OC_ERR_INVALID, "NULL argument");
+    if (c->comm.local) return fail(OC_ERR_INVALID, "oc_comm_p2p_export: the ranks of a local group exchange through the host");
     if (c->comm.world < 2 || c->comm.world > (int)P2P_MAX_WORLD) return fail(OC_ERR_INVALID, "oc_comm_init first (2..%u ranks)", P2P_MAX_WORLD);
     std::lock_guard<std::mutex> g(c->mu);
     CU(cudaSetDevice(c->device));
@@ -639,8 +657,7 @@ extern "C" int oc_emb_compact(oc_emb *e, uint32_t flags, oc_emb_compact_t *out) 
 // ---- scan launch plumbing
 template <int NCH, int QB, typename T>
 static int launch_scan_t(oc_ctx *c, const ScanParams &sp, uint32_t grid, size_t smem) {
-    if (smem_cfg_needed(c->device, (const void *)emb_scan_kernel<NCH, QB, T>, smem))
-        CU(cudaFuncSetAttribute(emb_scan_kernel<NCH, QB, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CU(smem_cfg(c->device, (const void *)emb_scan_kernel<NCH, QB, T>, smem));
     emb_scan_kernel<NCH, QB, T><<<grid, SCAN_THREADS, smem, c->stream>>>(sp);
     launched(c, true);
     CU(cudaGetLastError());
@@ -723,8 +740,7 @@ static int run_exact_sweeps(oc_ctx *c, oc_emb *e, const float *inv_norm, const f
     mp.row_doc_ids = e->row_doc; mp.rescale_e5 = e->e5; mp.similarity = similarity;
     mp.out_doc = o.doc; mp.out_score = o.score; mp.out_row = o.row; mp.out_count = o.cnt; mp.out_raw = o.raw;
     mp.q_limit = q_lim; mp.q_sim = q_sim;
-    if (smem_cfg_needed(c->device, (const void *)emb_scan_merge_kernel, size_t(mp.capb) * 8))
-        CU(cudaFuncSetAttribute(emb_scan_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(mp.capb * 8)));
+    CU(smem_cfg(c->device, (const void *)emb_scan_merge_kernel, size_t(mp.capb) * 8));
     emb_scan_merge_kernel<<<nq, 256, mp.capb * 8, c->stream>>>(mp);
     launched(c);
     CU(cudaGetLastError());
@@ -820,12 +836,8 @@ static int run_vector_stage(oc_ctx *c, oc_emb *e, const float *q_dev, uint32_t B
     const void *sweep_fn = bf16  ? (const void *)emb_gemm_kernel<GEMM_BF16>
                            : f16 ? (const void *)emb_gemm_kernel<GEMM_F16>
                                  : (const void *)emb_gemm_kernel<GEMM_TF32>;
-    if (smem_cfg_needed(c->device, (const void *)emb_gemm_kernel<GEMM_TF32>, gemm_smem_bytes())) {   // all sweep kernels at once
-        CU(cudaFuncSetAttribute(emb_gemm_kernel<GEMM_TF32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes()));
-        CU(cudaFuncSetAttribute(emb_gemm_kernel<GEMM_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes()));
-        CU(cudaFuncSetAttribute(emb_gemm_kernel<GEMM_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_smem_bytes()));
-        CU(cudaFuncSetAttribute(emb_gemm_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gemm_merge_smem_bytes()));
-    }
+    CU(smem_cfg(c->device, sweep_fn, gemm_smem_bytes()));
+    CU(smem_cfg(c->device, (const void *)emb_gemm_merge_kernel, gemm_merge_smem_bytes()));
     // an even number of query groups runs in CTA pairs that share every row tile (emb_gemm.cuh)
     const bool paired = n_qgroups % GEMM_CLUSTER == 0;
     cudaLaunchAttribute cluster_attr{};
@@ -1813,8 +1825,7 @@ static inline float host_idf(float total_documents, uint64_t corpus_df) {
 template <bool MULTI, bool THRESH, bool OMC, bool ROWFT>
 static int launch_tile_t(oc_ctx *c, const Bm25Params &bp, uint32_t grid, size_t smem, cudaStream_t st) {
     // (static smem counts against the 227 KB cap)
-    if (smem_cfg_needed(c->device, (const void *)bm25_tile_kernel<MULTI, THRESH, OMC, ROWFT>, smem))
-        CU(cudaFuncSetAttribute(bm25_tile_kernel<MULTI, THRESH, OMC, ROWFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CU(smem_cfg(c->device, (const void *)bm25_tile_kernel<MULTI, THRESH, OMC, ROWFT>, smem));
     bm25_tile_kernel<MULTI, THRESH, OMC, ROWFT><<<grid, BM25_THREADS, smem, st>>>(bp);
     launched(c);
     CU(cudaGetLastError());
@@ -1822,8 +1833,7 @@ static int launch_tile_t(oc_ctx *c, const Bm25Params &bp, uint32_t grid, size_t 
 }
 template <bool THRESH, bool OMC, bool ROWFT>
 static int launch_tile2_t(oc_ctx *c, const Bm25Params &bp, size_t smem, cudaStream_t st, const ItemTok *flat, unsigned int *counter) {
-    if (smem_cfg_needed(c->device, (const void *)bm25_tile2_kernel<THRESH, OMC, ROWFT>, smem))
-        CU(cudaFuncSetAttribute(bm25_tile2_kernel<THRESH, OMC, ROWFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CU(smem_cfg(c->device, (const void *)bm25_tile2_kernel<THRESH, OMC, ROWFT>, smem));
     static std::mutex occ_mu;                         // occupancy per (device, shared-memory size): queried once
     static std::map<std::pair<int, size_t>, int> occ;
     int per_sm = 1;
@@ -1873,8 +1883,7 @@ static int launch_tile(oc_ctx *c, const Bm25Params &bp_in, uint32_t grid, bool m
         if (use3) {
             // plain queries: the register-folded scorer (no accumulator arrays)
             const size_t smem3 = bm25_tile3_smem_bytes(bp.cap);
-            if (smem_cfg_needed(c->device, (const void *)bm25_tile3_kernel, smem3))
-                CU(cudaFuncSetAttribute(bm25_tile3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3));
+            CU(smem_cfg(c->device, (const void *)bm25_tile3_kernel, smem3));
             static std::mutex occ3_mu;
             static std::map<std::pair<int, size_t>, int> occ3;
             int per_sm = 1;
@@ -1896,8 +1905,7 @@ static int launch_tile(oc_ctx *c, const Bm25Params &bp_in, uint32_t grid, bool m
             const char *wenv = getenv("OC_BM25_WARP");
             if (bp.n_keep <= 32 && !(wenv && wenv[0] == '0')) {   // a warp per item: no block barriers
                 const size_t smemw = size_t(BW_WARPS) * sizeof(WarpScratch);
-                if (smem_cfg_needed(c->device, (const void *)bm25_warp_kernel, smemw))
-                    CU(cudaFuncSetAttribute(bm25_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemw));
+                CU(smem_cfg(c->device, (const void *)bm25_warp_kernel, smemw));
                 static std::mutex occw_mu;
                 static std::map<int, int> occw;
                 int pw = 1;
@@ -3012,11 +3020,13 @@ static int bm25_stage(SearchCall &k) {
         }
         k.row_ok = c->row_ok.as<uint32_t>();
     } else if (k.filter || k.tombs) {
-        OCTRY(c->row_ok.ensure(ok_words * 4));
-        rows_ok_kernel<<<(unsigned)((ok_words + 255) / 256), 256, 0, ps>>>(
-            S->row_doc, S->n_rows, k.tombs ? S->alive : nullptr, k.filter_dev, k.filter_nbits,
-            c->row_ok.as<uint32_t>(), ok_words);
-        launched(c);
+        OCTRY(c->row_ok.ensure(std::max<uint64_t>(ok_words, 1) * 4));
+        if (ok_words) {   // (a shard without string rows still takes part in the df all-reduce below)
+            rows_ok_kernel<<<(unsigned)((ok_words + 255) / 256), 256, 0, ps>>>(
+                S->row_doc, S->n_rows, k.tombs ? S->alive : nullptr, k.filter_dev, k.filter_nbits,
+                c->row_ok.as<uint32_t>(), ok_words);
+            launched(c);
+        }
         k.row_ok = c->row_ok.as<uint32_t>();
     }
     if (!k.pre_items.empty()) {
@@ -3257,6 +3267,17 @@ static int fuse_and_tails(SearchCall &k) {
     return sort_tail(k);
 }
 
+// K4 and its tails, or on a sharded search the pack, the exchange of the shard records and the merge
+static int fuse_or_merge(SearchCall &k) {
+    oc_ctx *c = k.c;
+    if (!(k.p->sharded && c->comm.world > 1)) return fuse_and_tails(k);
+    const bool has_v = k.has_v;
+    OCTRY(run_sharded_merge(c, k.p, k.fp, k.has_ft ? (uint32_t)k.S->n_rows : 0, has_v ? (uint32_t)k.emb->n_rows : 0, k.B,
+                            (has_v && c->gemm_pending) ? c->g_flag.as<uint8_t>() : nullptr, k.dout + k.o_gflag));
+    k.did_comm = true;
+    return OC_OK;
+}
+
 // The hybrid lookups, the fusion and what follows it (+ the shard exchange).  Re-runnable.
 static int device_tail(SearchCall &k) {
     oc_ctx *c = k.c; const oc_search_params *p = k.p;
@@ -3322,16 +3343,9 @@ static int device_tail(SearchCall &k) {
     }
     k.fuse_smem = size_t(fp.capb) * 8 + size_t(std::max<uint32_t>(32, next_pow2(n_keep))) * 8 + size_t(vlimit) * 16 + 64;
     const void *fuse = k.exports ? (const void *)fuse_topk_kernel<true> : (const void *)fuse_topk_kernel<false>;
-    if (smem_cfg_needed(c->device, fuse, k.fuse_smem))
-        CU(cudaFuncSetAttribute(fuse, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k.fuse_smem));
+    CU(smem_cfg(c->device, fuse, k.fuse_smem));
     CU(cudaEventRecord(c->ev[EV_FUSE0], c->stream));
-    if (p->sharded && c->comm.world > 1) {
-        OCTRY(run_sharded_merge(c, p, fp, has_ft ? (uint32_t)S->n_rows : 0, has_v ? (uint32_t)k.emb->n_rows : 0, B,
-                                (has_v && c->gemm_pending) ? c->g_flag.as<uint8_t>() : nullptr, k.dout + k.o_gflag));
-        k.did_comm = true;
-    } else {
-        OCTRY(fuse_and_tails(k));
-    }
+    OCTRY(fuse_or_merge(k));
     CU(cudaEventRecord(c->ev[EV_FUSE1], c->stream));
     return OC_OK;
 }
@@ -3376,7 +3390,11 @@ static int rerun_checks(SearchCall &k) {
     // rank-proxy validation: with OMC multipliers the tile ranking assumed min == min_hint (0);
     // a negative global min changes the order of (ft - min) * omc -> rerun with the real min.
     // The hybrid point lookups do not depend on the tiles: they are not redone.
-    if (!k.did_comm && k.mode == OC_MODE_HYBRID && k.omc_tile && k.n_tiles) {
+    // Sharded: the re-run re-enters the collective, so every rank decides on what all ranks share — the merged min,
+    // the batch's mode and whether it carries OMC — never on its own shard's OMC rows or tiles.  A rank whose shard
+    // has neither re-launches no tile, but packs, exchanges and merges again.
+    const bool proxy = k.mode == OC_MODE_HYBRID && (k.did_comm ? k.n_omc > 0 : k.omc_tile && k.n_tiles);
+    if (proxy) {
         const float *mins = reinterpret_cast<const float *>(h + k.o_min);
         std::vector<float> hyb_mins;   // per-query parameters: only the hybrid queries rank by (ft - min)
         if (k.qp) {
@@ -3387,11 +3405,13 @@ static int rerun_checks(SearchCall &k) {
         bool redo = false;
         for (uint32_t q = 0; q < B; q++) redo = redo || mins[q] < 0.f;
         if (redo) {
-            CU(cudaMemcpyAsync(k.min_hint_dev, mins, size_t(B) * 4, cudaMemcpyHostToDevice, c->stream));
-            CU(cudaMemsetAsync(c->tau.p, 0, size_t(B) * 8, c->stream));
-            CU(cudaMemsetAsync(k.tile_counter, 0, 8, c->stream));
-            OCTRY(launch_tile(c, k.bp, k.n_tiles * B, k.any_multi, k.thr, k.omc_tile, c->stream, k.max_tokens, k.tile_counter, k.need_df));
-            OCTRY(fuse_and_tails(k));
+            if (k.omc_tile && k.n_tiles) {
+                CU(cudaMemcpyAsync(k.min_hint_dev, mins, size_t(B) * 4, cudaMemcpyHostToDevice, c->stream));
+                CU(cudaMemsetAsync(c->tau.p, 0, size_t(B) * 8, c->stream));
+                CU(cudaMemsetAsync(k.tile_counter, 0, 8, c->stream));
+                OCTRY(launch_tile(c, k.bp, k.n_tiles * B, k.any_multi, k.thr, k.omc_tile, c->stream, k.max_tokens, k.tile_counter, k.need_df));
+            }
+            OCTRY(fuse_or_merge(k));
             CU(cudaMemcpyAsync(h, k.dout, k.out_bytes, cudaMemcpyDeviceToHost, c->stream));
             CU(cudaStreamSynchronize(c->stream));
         }
@@ -3997,8 +4017,7 @@ static int run_groups(oc_ctx *c, const GroupJob &gj, int mode, const StrSnap *S,
         if (i1 == i0) continue;
         gp.spans = gj.d_spans + s0; gp.n_spans = s1 - s0; gp.item0 = i0;
         const void *kern = by_field ? (const void *)group_sort_topk_kernel : (const void *)group_topk_kernel;
-        if (smem_cfg_needed(c->device, kern, smem))
-            CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CU(smem_cfg(c->device, kern, smem));
         if (by_field) group_sort_topk_kernel<<<i1 - i0, GROUP_THREADS, smem, c->stream>>>(gp);
         else group_topk_kernel<<<i1 - i0, GROUP_THREADS, smem, c->stream>>>(gp);
         launched(c);

@@ -3,6 +3,8 @@
 // (filters / multi-term tokens / tombstones), an all-reduce of the per-token df counters.  libnccl is bound with
 // dlopen/dlsym (no link-time dependency, no header needed): the torch-bundled
 // libnccl.so.2 already mapped into a torchrun worker is reused, else the system one.
+// A second transport joins several contexts of one process (oc_comm_init_local, e.g. ranks sharing one GPU): the
+// same collectives through host memory (comm_local.h), each rank on its own thread.
 #pragma once
 #include <cuda_runtime.h>
 #include <dlfcn.h>
@@ -10,7 +12,11 @@
 
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <string>
+#include <vector>
+
+#include "comm_local.h"
 
 struct OcComm {
     typedef struct { char internal[128]; } UniqueId;   // ncclUniqueId
@@ -80,21 +86,59 @@ struct OcComm {
         world = world_size; rank = my_rank;
         return true;
     }
-    bool ready() const { return comm != nullptr || world == 1; }
+    // in-process group: this rank's view of it and its host staging buffers
+    std::shared_ptr<LocalGroup> local;
+    std::vector<uint8_t> h_send, h_recv;
+
+    void init_local(std::shared_ptr<LocalGroup> g, int my_rank) {
+        destroy();
+        local = std::move(g); world = local->world(); rank = my_rank;
+    }
+    bool ready() const { return comm != nullptr || local != nullptr || world == 1; }
     // bytes per rank; ncclInt8 = 0
     bool all_gather(const void *send, void *recv, size_t bytes, cudaStream_t s, std::string *err) {
+        if (local) {
+            h_send.resize(bytes); h_recv.resize(bytes * world);
+            if (!to_host(h_send.data(), send, bytes, s, err)) return false;
+            if (!local->all_gather(rank, h_send.data(), h_recv.data(), bytes, err)) return false;
+            return to_device(recv, h_recv.data(), bytes * world, s, err);
+        }
         int rc = api().AllGather(send, recv, bytes, /*ncclInt8*/ 0, comm, s);
         if (rc != 0) { if (err) *err = "ncclAllGather: " + estr(rc); return false; }
         return true;
     }
     // in-place-capable sum of `count` uint32 counters; ncclUint32 = 3, ncclSum = 0
     bool all_reduce_sum_u32(const void *send, void *recv, size_t count, cudaStream_t s, std::string *err) {
+        if (local) {
+            h_send.resize(count * 4); h_recv.resize(count * 4);
+            if (!to_host(h_send.data(), send, count * 4, s, err)) return false;
+            if (!local->all_reduce_sum_u32(rank, reinterpret_cast<const uint32_t *>(h_send.data()),
+                                           reinterpret_cast<uint32_t *>(h_recv.data()), count, err)) return false;
+            return to_device(recv, h_recv.data(), count * 4, s, err);
+        }
         int rc = api().AllReduce(send, recv, count, /*ncclUint32*/ 3, /*ncclSum*/ 0, comm, s);
         if (rc != 0) { if (err) *err = "ncclAllReduce: " + estr(rc); return false; }
         return true;
     }
     void destroy() {
         if (comm) api().CommDestroy(comm);
-        comm = nullptr; world = 1; rank = 0;
+        if (local) local->leave(rank);
+        comm = nullptr; local.reset(); world = 1; rank = 0;
+    }
+
+private:
+    // the local transport's staging: the rank's stream is drained first, so its own device work never waits on a peer
+    static bool to_host(void *dst, const void *src, size_t bytes, cudaStream_t s, std::string *err) {
+        cudaError_t e = cudaStreamSynchronize(s);
+        if (e == cudaSuccess && bytes) e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (e != cudaSuccess && err) *err = std::string("local group staging: ") + cudaGetErrorString(e);
+        return e == cudaSuccess;
+    }
+    static bool to_device(void *dst, const void *src, size_t bytes, cudaStream_t s, std::string *err) {
+        cudaError_t e = bytes ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, s) : cudaSuccess;
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (e != cudaSuccess && err) *err = std::string("local group staging: ") + cudaGetErrorString(e);
+        return e == cudaSuccess;
     }
 };

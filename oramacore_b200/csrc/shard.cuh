@@ -252,7 +252,7 @@ __global__ void __launch_bounds__(256) shard_fuse_kernel(const ShardFuseParams p
             for (uint32_t j = 0; j < hdr_of(s)->n_v; j++)
                 if (vl[j].erow == erow) {
                     gv_doc[i] = vl[j].doc; gv_raw[i] = vl[j].score; gv_ft[i] = vl[j].ft; gv_present[i] = vl[j].present;
-                    gv_idx[i] = (has_ft && vl[j].srow != 0xffffffffu) ? base_str[s] + vl[j].srow : (0xfffffffeu - i);
+                    gv_idx[i] = (has_ft && vl[j].srow != 0xffffffffu) ? base_str[s] + vl[j].srow : 0xffffffffu;
                     break;
                 }
         }
@@ -265,6 +265,15 @@ __global__ void __launch_bounds__(256) shard_fuse_kernel(const ShardFuseParams p
             if (head) for (uint32_t i = j; i < gvc; i++) if (gv_doc[i] == gv_doc[j]) sum = __fadd_rn(sum, gv_raw[i]);
             gv_score[j] = sum; gv_first[j] = head ? 1u : 0u;
         }
+        __syncthreads();
+        // K4's tie rule (fuse.cuh): the key index of a unique hit is its doc id's rank among the unique hits, so equal
+        // scores come out in doc id order; in hybrid mode only a hit without a string row takes it, after FUSE_VONLY
+        for (uint32_t j = tid; j < gvc; j += blockDim.x)
+            if (gv_first[j] && !(hybrid && gv_idx[j] != 0xffffffffu)) {
+                uint32_t r = 0;
+                for (uint32_t i = 0; i < gvc; i++) r += (gv_first[i] && gv_doc[i] < gv_doc[j]) ? 1u : 0u;
+                gv_idx[j] = hybrid ? FUSE_VONLY + r : r;
+            }
         __syncthreads();
     }
 
@@ -330,7 +339,7 @@ __global__ void __launch_bounds__(256) shard_fuse_kernel(const ShardFuseParams p
             idx = gv_idx[j];
         } else {
             f = gv_score[j];
-            idx = j;
+            idx = gv_idx[j];
         }
         if (p.n_omc) { bool fd; const float m = omc_of(gv_doc[j], &fd); if (fd) f = __fmul_rn(f, m); }
         return f == f ? make_key(f, idx) : KEY_NONE;
@@ -347,8 +356,7 @@ __global__ void __launch_bounds__(256) shard_fuse_kernel(const ShardFuseParams p
             const uint32_t idx = key_idx(k);
             sc = key_score(k);
             bool found = false;
-            if (!has_ft) { doc = gv_doc[idx]; found = true; }
-            if (!found && has_v)
+            if (has_v)
                 for (uint32_t j = 0; j < gvc; j++) if (gv_first[j] && gv_idx[j] == idx) { doc = gv_doc[j]; found = true; break; }
             if (!found) {
                 uint32_t s = 0;
@@ -402,8 +410,7 @@ static int run_sharded_merge(oc_ctx *c, const oc_search_params *p, const oc::Fus
         }
     }
     const size_t pack_smem = size_t(fp.capb) * 8 + size_t(std::max<uint32_t>(32, next_pow2(fp.n_keep))) * 8 + 64;
-    if (smem_cfg_needed(c->device, (const void *)shard_pack_kernel, pack_smem))
-        CU(cudaFuncSetAttribute(shard_pack_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pack_smem));
+    CU(smem_cfg(c->device, (const void *)shard_pack_kernel, pack_smem));
     shard_pack_kernel<<<B, 256, pack_smem, c->stream>>>(pp);
     launched(c);
     CU(cudaGetLastError());
@@ -429,8 +436,7 @@ static int run_sharded_merge(oc_ctx *c, const oc_search_params *p, const oc::Fus
     sp.out_doc = fp.out_doc; sp.out_score = fp.out_score; sp.out_n = fp.out_n; sp.out_count = fp.out_count; sp.out_min = fp.out_min;
     sp.out_flag = out_flag_dev;
     const size_t fsmem = size_t(sp.capb) * 8 + size_t(fp.v_stride) * 36 + 64;
-    if (smem_cfg_needed(c->device, (const void *)shard_fuse_kernel, fsmem))
-        CU(cudaFuncSetAttribute(shard_fuse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
+    CU(smem_cfg(c->device, (const void *)shard_fuse_kernel, fsmem));
     shard_fuse_kernel<<<B, 256, fsmem, c->stream>>>(sp);
     launched(c);
     CU(cudaGetLastError());

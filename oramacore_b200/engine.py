@@ -81,6 +81,14 @@ class Context:
         buf = (C.c_uint8 * _lib.OC_COMM_ID_BYTES).from_buffer_copy(unique_id)
         check(lib().oc_comm_init(self._h, world_size, rank, buf))
 
+    @staticmethod
+    def comm_init_local(ctxs):
+        """Join contexts of this process (e.g. several on one GPU) as ranks 0..len(ctxs)-1 of one group whose
+        collectives run through host memory (oc_comm_init_local).  Each rank then calls the sharded search on its own
+        thread."""
+        arr = (C.c_void_p * len(ctxs))(*[c._h for c in ctxs])
+        check(lib().oc_comm_init_local(arr, len(ctxs)))
+
     def comm_enable_p2p(self, all_gather):
         """Direct NVLink exchange of the shard records (oc_comm_p2p_*).  `all_gather(blob: bytes) -> list[bytes]`
         is the host runtime's all-gather in rank order (e.g. torch.distributed.all_gather_object)."""

@@ -186,6 +186,7 @@ extern "C" {
     pub fn oc_shutdown(ctx: *mut OcCtx);
     pub fn oc_comm_unique_id(out_id: *mut u8) -> c_int;
     pub fn oc_comm_init(ctx: *mut OcCtx, world: c_int, rank: c_int, id: *const u8) -> c_int;
+    pub fn oc_comm_init_local(ctxs: *const *mut OcCtx, world: c_int) -> c_int;
     pub fn oc_emb_create(ctx: *mut OcCtx, dim: u32, dtype: c_int, rescale_e5: c_int, out: *mut *mut OcEmb) -> c_int;
     pub fn oc_emb_destroy(emb: *mut OcEmb);
     pub fn oc_emb_insert(emb: *mut OcEmb, doc_ids: *const u64, rows: *const c_void, n: u64) -> c_int;
