@@ -695,7 +695,7 @@ int oc_merge_sorted(uint32_t n_indexes, uint32_t n_queries, uint32_t limit, uint
                     uint64_t *out_doc_ids /* B x limit */, float *out_scores, double *out_sort_values,
                     uint32_t *out_n, uint64_t *out_count);
 
-/* ---- term dictionary and query-term resolution (host only; no device needed) ------------------------
+/* ---- term dictionary and query-term resolution (host; oc_dict_resolve_q may expand typos on a device) ------
  * The step the reference performs before the posting walk: TextParser::tokenize_and_stem(term) —
  * originals, plus stems unless `exact`, [""] when nothing is left (token_score.rs:196-209) — and the
  * expansion of every token to index terms inside StringStorage's FST (string_field.rs:208-225): the exact
@@ -729,6 +729,27 @@ int oc_dict_set_stemmer(oc_dict *d, oc_stem_fn fn, void *user);
  * un-vendored oramacore_lib::nlp::TextParser; a host that links it passes its own function instead. */
 size_t oc_stem_english(const char *tok, size_t len, char *out, size_t cap, void *user);
 int oc_dict_resolve(oc_dict *d, const oc_resolve_params *p, oc_resolved **out);
+/* Per-query options for oc_dict_resolve_q. */
+typedef struct oc_resolve_query {
+    int exact;                  /* as oc_resolve_params.exact, for this query                              */
+    int tolerance;              /* < 0: prefix expansion; t >= 0: Levenshtein <= t (bytes)                 */
+    const float *field_boost;   /* n_fields, NULL = 1.0                                                    */
+    const uint8_t *field_mask;  /* n_fields, NULL = all string fields                                      */
+} oc_resolve_query;
+/* oc_dict_resolve with options per query: query b's slice of the output equals oc_dict_resolve of texts[b] alone with
+ * q[b]'s exact / tolerance / field_boost / field_mask and p->exact_match_boost, byte for byte (token ranges, fields,
+ * ids, order, weight bits).  q NULL: every query takes p's options, and the output equals oc_dict_resolve(d, p).
+ * ctx NULL: everything runs on the host.  With a ctx, every (token, field) pair of a query with tolerance >= 1 and a
+ * token of at most 64 bytes is expanded on that ctx's device; tokenising, stemming and the exact, prefix and
+ * tolerance-0 expansions (binary searches) stay on the host.  The ctx keeps a mirror of the dictionary (term bytes,
+ * 8 B of offset and 4 B of sorted permutation per term; oc_dict_device_bytes), refreshed by the next such call after
+ * oc_dict_add_terms: only new terms' bytes are uploaded, the permutation again when it changed.  The mirror of a
+ * destroyed dictionary is freed by the ctx's next device resolve or by oc_shutdown; oc_dict_destroy never touches a
+ * ctx.  Refusals write nothing: OC_ERR_INVALID for what oc_dict_resolve refuses, OC_ERR_UNSUPPORTED for a tolerance
+ * above 8.  Device calls serialise on the ctx lock. */
+int oc_dict_resolve_q(oc_dict *d, oc_ctx *ctx, const oc_resolve_params *p, const oc_resolve_query *q, oc_resolved **out);
+/* device bytes of d's mirror on ctx (0: none yet, or either is NULL) */
+uint64_t oc_dict_device_bytes(oc_dict *d, oc_ctx *ctx);
 void oc_resolved_arrays(const oc_resolved *r, const uint32_t **q_token_offsets, const uint32_t **token_term_offsets,
                         const uint32_t **term_field, const uint32_t **term_id, const float **term_weight,
                         uint32_t *n_tokens, uint32_t *n_terms);

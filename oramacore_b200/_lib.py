@@ -51,7 +51,7 @@ EXPORTED_SYMBOLS = [
     "oc_sort_field_create", "oc_sort_field_destroy", "oc_search_sorted", "oc_search_q_sorted", "oc_search_groups_sorted", "oc_merge_sorted",
     "oc_group_by_n_groups", "oc_search_q_groups", "oc_facets_check", "oc_search_q_facets",
     "oc_dict_create", "oc_dict_destroy", "oc_dict_add_terms", "oc_dict_lookup", "oc_dict_size", "oc_dict_set_stemmer", "oc_stem_english",
-    "oc_dict_resolve", "oc_resolved_arrays", "oc_resolved_fill", "oc_resolved_free",
+    "oc_dict_resolve", "oc_dict_resolve_q", "oc_dict_device_bytes", "oc_resolved_arrays", "oc_resolved_fill", "oc_resolved_free",
 ]
 
 
@@ -126,6 +126,10 @@ class GroupReq(C.Structure):
 class ResolveParams(C.Structure):
     _fields_ = [("texts", C.POINTER(C.c_char_p)), ("n_queries", C.c_uint32), ("exact", C.c_int), ("tolerance", C.c_int),
                 ("field_boost", C.c_void_p), ("field_mask", C.c_void_p), ("exact_match_boost", C.c_float)]
+
+
+class ResolveQuery(C.Structure):   # oc_resolve_query: one query's options for oc_dict_resolve_q
+    _fields_ = [("exact", C.c_int), ("tolerance", C.c_int), ("field_boost", C.c_void_p), ("field_mask", C.c_void_p)]
 
 
 STEM_FN = C.CFUNCTYPE(C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p)
@@ -269,6 +273,9 @@ def lib():
     L.oc_stem_english.argtypes = [C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t, vp]
     L.oc_stem_english.restype = C.c_size_t
     L.oc_dict_resolve.argtypes = [vp, C.POINTER(ResolveParams), C.POINTER(vp)]
+    L.oc_dict_resolve_q.argtypes = [vp, vp, C.POINTER(ResolveParams), vp, C.POINTER(vp)]
+    L.oc_dict_device_bytes.argtypes = [vp, vp]
+    L.oc_dict_device_bytes.restype = u64
     L.oc_resolved_arrays.argtypes = [vp] + [C.POINTER(vp)] * 5 + [C.POINTER(u32)] * 2
     L.oc_resolved_arrays.restype = None
     L.oc_resolved_fill.argtypes = [vp, C.POINTER(SearchParams)]

@@ -22,6 +22,7 @@
 #include "comm.h"
 #include "dense_cache.h"
 #include "dict.h"
+#include "dict_dev.cuh"
 #include "stem_en.h"
 #include "emb_compact.cuh"
 #include "emb_gemm.cuh"
@@ -204,6 +205,10 @@ struct oc_ctx {
     DevBuf cmp_scan, cmp_stage;
     // the dense contribution arrays of hot terms, kept across calls (dense_cache.h)
     DenseCache dense_cache;
+    // oc_dict_resolve_q: the mirror of each dictionary resolved on this ctx, by dictionary serial (dict_dev.cuh), and
+    // the call's pair descriptors, per-chunk counts and output
+    std::unordered_map<uint64_t, std::unique_ptr<ocdd::DictMirror>> dict_mirrors;
+    DevBuf fz_in, fz_cnt, fz_out;
 
     HostBuf h_in, h_out, h_in0;   // h_in0 / in_blob0: query vectors + filter, uploaded before the descriptors
     OcComm comm;
@@ -4916,10 +4921,131 @@ extern "C" int oc_batcher_stats(oc_batcher *b, uint64_t *n_queries, uint64_t *n_
 }
 
 // ------------------------------------------------------------------------------------ term dictionary / query resolution
-// Host only (no device): the step the reference performs before the posting walk — tokenize_and_stem
-// (token_score.rs:196-209) and the FST term expansion inside StringStorage (string_field.rs:208-225).
-struct oc_dict { ocd::Dict d; explicit oc_dict(uint32_t n) : d(n) {} };
+// The step the reference performs before the posting walk — tokenize_and_stem (token_score.rs:196-209) and the FST term
+// expansion inside StringStorage (string_field.rs:208-225).  On the host, except the tolerance >= 1 expansions of
+// oc_dict_resolve_q with a ctx, which run on the device (dict_dev.cuh).
+static std::atomic<uint64_t> g_dict_serial{0};
+struct oc_dict {
+    ocd::Dict d;
+    std::shared_ptr<const uint64_t> token;   // the dictionary's serial; the ctx mirrors of it watch this (dict_dev.cuh)
+    explicit oc_dict(uint32_t n) : d(n), token(std::make_shared<const uint64_t>(++g_dict_serial)) {}
+};
 struct oc_resolved { ocd::Resolved r; };
+
+static void dict_mirror_sweep(oc_ctx *c) {
+    for (auto it = c->dict_mirrors.begin(); it != c->dict_mirrors.end();)
+        it = it->second->owner.expired() ? c->dict_mirrors.erase(it) : std::next(it);
+}
+
+// ocd::FuzzyRun on ctx c: refresh d's mirror, count, scan, emit.  One synchronise for the output size, one for the
+// output.  Runs under the ctx lock on the ctx stream.
+static int dict_fuzzy_device(oc_ctx *c, const oc_dict *d, const std::vector<ocd::FieldDict> &fields, uint64_t gen,
+                             const std::vector<ocd::FuzzyPair> &pairs, ocd::FuzzyLists *out) {
+    using namespace ocdd;
+    std::lock_guard<std::mutex> g(c->mu);
+    CU(cudaSetDevice(c->device));
+    dict_mirror_sweep(c);
+    std::unique_ptr<DictMirror> &mp = c->dict_mirrors[*d->token];
+    if (!mp) { mp.reset(new DictMirror(fields.size())); mp->owner = d->token; }
+    const cudaError_t se = mp->sync(fields, gen, c->stream);
+    if (se != cudaSuccess) {   // a half-refreshed mirror is dropped; the next call builds it again
+        c->dict_mirrors.erase(*d->token);
+        cudaGetLastError();
+        return fail(se == cudaErrorMemoryAllocation ? OC_ERR_OOM : OC_ERR_CUDA, "dictionary mirror upload: %s", cudaGetErrorString(se));
+    }
+    const DictMirror &M = *mp;
+    const uint32_t nf = (uint32_t)fields.size(), np = (uint32_t)pairs.size();
+    std::vector<uint32_t> order(np);   // device pair k = pairs[order[k]]: ordered by field
+    for (uint32_t i = 0; i < np; i++) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return pairs[a].field < pairs[b].field; });
+    std::vector<FzPair> fp(np);
+    uint32_t staged = 8;
+    for (uint32_t k = 0; k < np; k++) {
+        const ocd::FuzzyPair &q = pairs[order[k]];
+        FzPair &P = fp[k];
+        memset(&P, 0, sizeof(P));
+        P.m = (uint32_t)q.tok->size(); P.t = q.t; P.field = q.field;
+        memcpy(P.tok, q.tok->data(), P.m);
+        staged = std::max(staged, P.m + P.t);
+    }
+    const uint32_t stride = ((staged + 7) & ~7u) + 4;   // an odd number of words: the threads of a warp hit distinct banks
+    std::vector<FzField> ff(nf);
+    uint32_t chunks = 0;
+    uint64_t slots = 0;
+    for (uint32_t fi = 0, k = 0; fi < nf; fi++) {
+        FzField &F = ff[fi];
+        const DictMirror::Field &m = M.f[fi];
+        F.bytes = m.bytes.as<uint8_t>(); F.off = m.off.as<uint64_t>(); F.sorted = m.sorted.as<uint32_t>();
+        F.n = (uint32_t)m.n_sorted;
+        F.p0 = k;
+        while (k < np && fp[k].field == fi) k++;
+        F.p1 = k;
+        F.chunk0 = chunks;
+        F.n_chunks = F.p1 > F.p0 ? (F.n + FZ_CHUNK - 1) / FZ_CHUNK : 0;
+        chunks += F.n_chunks;
+        for (uint32_t j = F.p0; j < F.p1; j++) { fp[j].slot = (uint32_t)slots; slots += F.n_chunks + 1; }
+    }
+    if (slots + np > 0xffffffffu) return fail(OC_ERR_UNSUPPORTED, "%u fuzzy pairs over %u chunks", np, chunks);
+    const size_t off_p = (nf * sizeof(FzField) + 255) & ~size_t(255), off_o = off_p + ((np * sizeof(FzPair) + 255) & ~size_t(255));
+    OCTRY(c->fz_in.ensure(off_o + size_t(np) * 4));
+    OCTRY(c->fz_cnt.ensure((slots + np) * 4));
+    std::vector<uint8_t> blob(off_o);
+    memcpy(blob.data(), ff.data(), nf * sizeof(FzField));
+    memcpy(blob.data() + off_p, fp.data(), np * sizeof(FzPair));
+    CU(cudaMemcpyAsync(c->fz_in.p, blob.data(), off_o, cudaMemcpyHostToDevice, c->stream));
+    const FzField *dF = c->fz_in.as<const FzField>();
+    const FzPair *dP = reinterpret_cast<const FzPair *>(c->fz_in.as<uint8_t>() + off_p);
+    uint32_t *dO = reinterpret_cast<uint32_t *>(c->fz_in.as<uint8_t>() + off_o);
+    uint32_t *cnt = c->fz_cnt.as<uint32_t>(), *tot = cnt + slots;
+    const size_t smem = fuzzy_smem(stride);
+    // about four CTAs per SM, without slicing a field's pairs finer than a count-pass group
+    uint32_t max_pairs = 0;
+    for (const FzField &F : ff) max_pairs = std::max(max_pairs, F.p1 - F.p0);
+    const uint32_t want = 4u * (uint32_t)c->prop.multiProcessorCount;
+    const uint32_t split = chunks ? std::max(1u, std::min((want + chunks - 1) / chunks, (max_pairs + FZ_GROUP - 1) / FZ_GROUP)) : 1;
+    if (chunks) {
+        CU(smem_cfg(c->device, (const void *)dict_fuzzy_kernel<false>, smem));
+        CU(smem_cfg(c->device, (const void *)dict_fuzzy_kernel<true>, smem));
+        dict_fuzzy_kernel<false><<<chunks * split, FZ_THREADS, smem, c->stream>>>(dF, nf, dP, stride, split, cnt, nullptr, nullptr, nullptr);
+        CU(cudaGetLastError());
+        launched(c);
+    }
+    dict_fuzzy_scan_kernel<<<np, FZ_THREADS, 0, c->stream>>>(dF, dP, cnt, tot);
+    CU(cudaGetLastError());
+    launched(c);
+    std::vector<uint32_t> total(np), out0(np);
+    CU(cudaMemcpyAsync(total.data(), tot, size_t(np) * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    uint64_t T = 0;
+    for (uint32_t k = 0; k < np; k++) { out0[k] = (uint32_t)T; T += total[k]; }
+    if (T > 0xffffffffu) return fail(OC_ERR_UNSUPPORTED, "%llu expanded terms", (unsigned long long)T);
+    std::vector<uint32_t> ids(T);
+    std::vector<uint8_t> ex(T);
+    if (T) {
+        OCTRY(c->fz_out.ensure(T * 5));
+        uint32_t *d_id = c->fz_out.as<uint32_t>();
+        uint8_t *d_ex = reinterpret_cast<uint8_t *>(d_id + T);
+        CU(cudaMemcpyAsync(dO, out0.data(), size_t(np) * 4, cudaMemcpyHostToDevice, c->stream));
+        dict_fuzzy_kernel<true><<<chunks * split, FZ_THREADS, smem, c->stream>>>(dF, nf, dP, stride, split, cnt, dO, d_id, d_ex);
+        CU(cudaGetLastError());
+        launched(c);
+        CU(cudaMemcpyAsync(ids.data(), d_id, T * 4, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaMemcpyAsync(ex.data(), d_ex, T, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+    }
+    std::vector<uint32_t> at(np);
+    for (uint32_t k = 0; k < np; k++) at[order[k]] = k;
+    out->off.assign(1, 0u);
+    out->id.clear(); out->exact.clear();
+    out->id.reserve(T); out->exact.reserve(T);
+    for (uint32_t i = 0; i < np; i++) {
+        const uint32_t k = at[i];
+        out->id.insert(out->id.end(), ids.begin() + out0[k], ids.begin() + out0[k] + total[k]);
+        out->exact.insert(out->exact.end(), ex.begin() + out0[k], ex.begin() + out0[k] + total[k]);
+        out->off.push_back((uint32_t)out->id.size());
+    }
+    return OC_OK;
+}
 
 extern "C" int oc_dict_create(uint32_t n_fields, oc_dict **out) {
     if (!out || n_fields == 0) return fail(OC_ERR_INVALID, "bad arguments");
@@ -4964,6 +5090,33 @@ extern "C" int oc_dict_resolve(oc_dict *d, const oc_resolve_params *p, oc_resolv
     d->d.resolve(p->texts, p->n_queries, o, &r->r);
     *out = r;
     return OC_OK;
+}
+extern "C" int oc_dict_resolve_q(oc_dict *d, oc_ctx *ctx, const oc_resolve_params *p, const oc_resolve_query *q,
+                                 oc_resolved **out) {
+    if (!d || !p || !out || (p->n_queries && !p->texts)) return fail(OC_ERR_INVALID, "bad arguments");
+    for (uint32_t i = 0; i < p->n_queries; i++) if (!p->texts[i]) return fail(OC_ERR_INVALID, "text %u is NULL", i);
+    if (!q && p->tolerance > 8) return fail(OC_ERR_UNSUPPORTED, "tolerance %d > 8", p->tolerance);
+    if (q) for (uint32_t i = 0; i < p->n_queries; i++)
+        if (q[i].tolerance > 8) return fail(OC_ERR_UNSUPPORTED, "query %u: tolerance %d > 8", i, q[i].tolerance);
+    std::vector<ocd::ResolveOpts> opts(p->n_queries);
+    for (uint32_t i = 0; i < p->n_queries; i++) {
+        ocd::ResolveOpts &o = opts[i];
+        if (q) { o.exact = q[i].exact != 0; o.tolerance = q[i].tolerance; o.field_boost = q[i].field_boost; o.field_mask = q[i].field_mask; }
+        else { o.exact = p->exact != 0; o.tolerance = p->tolerance; o.field_boost = p->field_boost; o.field_mask = p->field_mask; }
+        o.exact_match_boost = p->exact_match_boost > 0.f ? p->exact_match_boost : 2.0f;
+    }
+    const ocd::FuzzyRun run = [&](const std::vector<ocd::FieldDict> &fields, uint64_t gen, const std::vector<ocd::FuzzyPair> &pairs,
+                                  ocd::FuzzyLists *lists) { return dict_fuzzy_device(ctx, d, fields, gen, pairs, lists); };
+    std::unique_ptr<oc_resolved> r(new oc_resolved());
+    OCTRY(d->d.resolve_q(p->texts, p->n_queries, opts, ctx ? &run : nullptr, &r->r));
+    *out = r.release();
+    return OC_OK;
+}
+extern "C" uint64_t oc_dict_device_bytes(oc_dict *d, oc_ctx *ctx) {
+    if (!d || !ctx) return 0;
+    std::lock_guard<std::mutex> g(ctx->mu);
+    auto it = ctx->dict_mirrors.find(*d->token);
+    return it == ctx->dict_mirrors.end() ? 0 : it->second->device_bytes();
 }
 extern "C" void oc_resolved_arrays(const oc_resolved *r, const uint32_t **q_token_offsets, const uint32_t **token_term_offsets,
                                    const uint32_t **term_field, const uint32_t **term_id, const float **term_weight,

@@ -20,6 +20,7 @@
 #include <algorithm>
 #include <cstdint>
 #include <cstring>
+#include <functional>
 #include <mutex>
 #include <shared_mutex>
 #include <string>
@@ -111,6 +112,18 @@ struct ResolveOpts {
     float exact_match_boost = 2.0f;
 };
 
+// A (token, field) expansion with tolerance >= 1 that resolve_q hands to a FuzzyRun (the device): the sorted positions
+// of `field` whose term starts with tok or lies within byte-wise Levenshtein distance t of it, ascending — what
+// Dict::fuzzy emits.  Tokens longer than one 64-bit pattern word stay with the host walk.
+constexpr size_t FUZZY_RUN_MAX_TOK = 64;
+struct FuzzyPair { uint32_t field, t; const std::string *tok; };
+// pair i's terms are id[off[i] .. off[i+1]) in emission order; exact[e]: the term equals the token
+struct FuzzyLists { std::vector<uint32_t> off, id; std::vector<uint8_t> exact; };
+// runs the pairs over fields[] (held under the dictionary's shared lock); gen = Dict::generation().  Returns 0 or an
+// error code, which resolve_q passes on.
+typedef std::function<int(const std::vector<FieldDict> &fields, uint64_t gen, const std::vector<FuzzyPair> &pairs,
+                          FuzzyLists *out)> FuzzyRun;
+
 class Dict {
 public:
     explicit Dict(uint32_t n_fields) : fields_(n_fields) {}
@@ -119,10 +132,12 @@ public:
     void add_terms(uint32_t field, const char *const *terms, uint32_t n, uint32_t *out_ids) {
         std::unique_lock<std::shared_mutex> g(mu_);
         FieldDict &f = fields_[field];
+        const size_t before = f.terms.size();
         for (uint32_t i = 0; i < n; i++) {
             const uint32_t id = f.add(terms[i]);
             if (out_ids) out_ids[i] = id;
         }
+        if (f.terms.size() != before) gen_++;
     }
     bool lookup(uint32_t field, const char *term, uint32_t *id) {
         std::shared_lock<std::shared_mutex> g(mu_);
@@ -138,41 +153,92 @@ public:
     }
     void set_stemmer(StemFn fn, void *user) { std::unique_lock<std::shared_mutex> g(mu_); stem_ = fn; stem_user_ = user; }
 
+    // bumped by add_terms (a new term) and by the reindex of a resolve; read under the shared lock (FuzzyRun)
+    uint64_t generation() const { return gen_; }
+
     void resolve(const char *const *texts, uint32_t n_queries, const ResolveOpts &o, Resolved *out) {
+        resolve_q(texts, n_queries, std::vector<ResolveOpts>(n_queries, o), nullptr, out);
+    }
+    // Query q with its own opts[q].  With `run`, every (token, field) pair of a query with tolerance >= 1 whose token
+    // fits FUZZY_RUN_MAX_TOK is expanded by run, everything else here; the output is the same either way.  A failing
+    // run's code is returned and `out` is left as it was.
+    int resolve_q(const char *const *texts, uint32_t n_queries, const std::vector<ResolveOpts> &opts, const FuzzyRun *run,
+                  Resolved *out) {
         {   // bring the sorted indexes up to date (exclusive), then resolve under the shared lock
             bool need = false;
             { std::shared_lock<std::shared_mutex> g(mu_); for (auto &f : fields_) need = need || f.stale(); }
-            if (need) { std::unique_lock<std::shared_mutex> g(mu_); for (auto &f : fields_) f.reindex(); }
+            if (need) { std::unique_lock<std::shared_mutex> g(mu_); for (auto &f : fields_) f.reindex(); gen_++; }
         }
         std::shared_lock<std::shared_mutex> g(mu_);
-        std::vector<Resolved> per(n_queries);
-        auto work = [&](uint32_t q0, uint32_t q1) { for (uint32_t q = q0; q < q1; q++) resolve_one(texts[q], o, &per[q]); };
-        // the bounded-Levenshtein walk is the only expensive mode: spread its queries over the host cores
+        std::vector<Plan> per(n_queries);
+        auto work = [&](uint32_t q0, uint32_t q1) { for (uint32_t q = q0; q < q1; q++) plan_one(texts[q], opts[q], run != nullptr, &per[q]); };
+        // the bounded-Levenshtein walk is the only expensive mode: without a FuzzyRun, spread its queries over the host cores
+        bool walk = false;
+        for (const ResolveOpts &o : opts) walk = walk || (!o.exact && o.tolerance >= 0);
         unsigned nt = 1;
-        if (!o.exact && o.tolerance >= 0 && n_queries >= 8) nt = std::min<unsigned>(std::max(1u, std::thread::hardware_concurrency()), std::min<unsigned>(n_queries / 4, 32));
+        if (!run && walk && n_queries >= 8) nt = std::min<unsigned>(std::max(1u, std::thread::hardware_concurrency()), std::min<unsigned>(n_queries / 4, 32));
         if (nt <= 1) work(0, n_queries);
         else {
             std::vector<std::thread> th;
             for (unsigned t = 0; t < nt; t++) th.emplace_back(work, uint32_t(uint64_t(n_queries) * t / nt), uint32_t(uint64_t(n_queries) * (t + 1) / nt));
             for (auto &t : th) t.join();
         }
-        size_t n_tok = 0, n_term = 0;
-        for (auto &r : per) { n_tok += r.token_term_offsets.size() - 1; n_term += r.term_id.size(); }
+        std::vector<FuzzyPair> pairs;
+        std::vector<uint32_t> pair0(n_queries);
+        for (uint32_t q = 0; q < n_queries; q++) {
+            pair0[q] = (uint32_t)pairs.size();
+            for (auto &d : per[q].dev) pairs.push_back({d.second, (uint32_t)opts[q].tolerance, &per[q].toks[d.first]});
+        }
+        FuzzyLists dev;
+        if (!pairs.empty()) {
+            const int rc = (*run)(fields_, gen_, pairs, &dev);
+            if (rc) return rc;
+        }
+        size_t n_tok = 0, n_term = dev.id.size();
+        for (auto &p : per) { n_tok += p.toks.size(); n_term += p.id.size(); }
         out->q_token_offsets.assign(1, 0u); out->token_term_offsets.assign(1, 0u);
         out->q_token_offsets.reserve(n_queries + 1); out->token_term_offsets.reserve(n_tok + 1);
         out->term_field.clear(); out->term_id.clear(); out->term_weight.clear();
         out->term_field.reserve(n_term); out->term_id.reserve(n_term); out->term_weight.reserve(n_term);
-        for (auto &r : per) {
-            const uint32_t base = (uint32_t)out->term_id.size();
-            for (size_t t = 1; t < r.token_term_offsets.size(); t++) out->token_term_offsets.push_back(base + r.token_term_offsets[t]);
+        for (uint32_t q = 0; q < n_queries; q++) {
+            const Plan &p = per[q];
+            const ResolveOpts &o = opts[q];
+            size_t s = 0;
+            for (uint32_t k = 0; k < p.toks.size(); k++) {
+                for (; s < p.segs.size() && p.segs[s].tok == k; s++) {
+                    const Plan::Seg &sg = p.segs[s];
+                    const float w = o.field_boost ? o.field_boost[sg.field] : 1.0f;
+                    const uint32_t *ids = p.id.data() + sg.h0;
+                    const uint8_t *ex = p.exact.data() + sg.h0;
+                    size_t n = sg.h1 - sg.h0;
+                    if (sg.dev != Plan::HOST) {
+                        const uint32_t i = pair0[q] + sg.dev;
+                        ids = dev.id.data() + dev.off[i]; ex = dev.exact.data() + dev.off[i]; n = dev.off[i + 1] - dev.off[i];
+                    }
+                    for (size_t e = 0; e < n; e++) {
+                        out->term_field.push_back(sg.field); out->term_id.push_back(ids[e]);
+                        out->term_weight.push_back(ex[e] ? w * o.exact_match_boost : w);
+                    }
+                }
+                out->token_term_offsets.push_back((uint32_t)out->term_id.size());
+            }
             out->q_token_offsets.push_back((uint32_t)out->token_term_offsets.size() - 1);
-            out->term_field.insert(out->term_field.end(), r.term_field.begin(), r.term_field.end());
-            out->term_id.insert(out->term_id.end(), r.term_id.begin(), r.term_id.end());
-            out->term_weight.insert(out->term_weight.end(), r.term_weight.begin(), r.term_weight.end());
         }
+        return 0;
     }
 
 private:
+    // one query's expansion before the FuzzyRun lists are in: per (token, field), in token then field order, either
+    // host-expanded terms or a pair for the run
+    struct Plan {
+        static constexpr uint32_t HOST = 0xffffffffu;
+        struct Seg { uint32_t tok, field, dev, h0, h1; };   // dev: the query's run pair, or HOST: terms [h0, h1) below
+        std::vector<std::string> toks;
+        std::vector<Seg> segs;
+        std::vector<uint32_t> id;
+        std::vector<uint8_t> exact;
+        std::vector<std::pair<uint32_t, uint32_t>> dev;     // run pairs: (token, field)
+    };
     // token_score.rs:196-209: originals (+ stems unless exact); nothing => [""]
     void query_tokens(const char *text, bool exact, std::vector<std::string> &toks) const {
         std::vector<std::string> orig;
@@ -187,18 +253,20 @@ private:
         }
         if (toks.empty()) toks.emplace_back("");
     }
-    void resolve_one(const char *text, const ResolveOpts &o, Resolved *r) const {
-        std::vector<std::string> toks;
-        query_tokens(text, o.exact, toks);
-        for (const std::string &tok : toks) {
+    void plan_one(const char *text, const ResolveOpts &o, bool run, Plan *p) const {
+        query_tokens(text, o.exact, p->toks);
+        for (uint32_t k = 0; k < p->toks.size(); k++) {
+            const std::string &tok = p->toks[k];
             for (uint32_t fi = 0; fi < fields_.size(); fi++) {
                 if (o.field_mask && !o.field_mask[fi]) continue;
+                if (run && !o.exact && o.tolerance >= 1 && tok.size() <= FUZZY_RUN_MAX_TOK) {
+                    p->segs.push_back({k, fi, (uint32_t)p->dev.size(), 0, 0});
+                    p->dev.emplace_back(k, fi);
+                    continue;
+                }
                 const FieldDict &f = fields_[fi];
-                const float w = o.field_boost ? o.field_boost[fi] : 1.0f;
-                auto emit = [&](uint32_t id, bool is_exact) {
-                    r->term_field.push_back(fi); r->term_id.push_back(id);
-                    r->term_weight.push_back(is_exact ? w * o.exact_match_boost : w);
-                };
+                const uint32_t h0 = (uint32_t)p->id.size();
+                auto emit = [&](uint32_t id, bool is_exact) { p->id.push_back(id); p->exact.push_back(is_exact); };
                 if (o.exact) {
                     auto it = f.ids.find(tok);
                     if (it != f.ids.end()) emit(it->second, true);
@@ -209,8 +277,8 @@ private:
                 } else {
                     fuzzy(f, tok, (uint32_t)o.tolerance, emit);
                 }
+                p->segs.push_back({k, fi, Plan::HOST, h0, (uint32_t)p->id.size()});
             }
-            r->token_term_offsets.push_back((uint32_t)r->term_id.size());
         }
     }
     // terms within Levenshtein distance t of tok, plus the terms tok is a prefix of, in lexicographic order.
@@ -269,6 +337,7 @@ private:
     }
 
     std::vector<FieldDict> fields_;
+    uint64_t gen_ = 0;
     std::shared_mutex mu_;
     StemFn stem_ = nullptr;
     void *stem_user_ = nullptr;

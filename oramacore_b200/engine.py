@@ -1014,7 +1014,8 @@ class TermDictionary:
     """Native term dictionaries of the string fields of one Index + batch query resolution (oc_dict_*,
     csrc/dict.h): tokenize (+ stem hook), then per field exact / prefix / Levenshtein expansion — what
     TextParser::tokenize_and_stem and the FST inside StringStorage do in the reference
-    (token_score.rs:196-209, string_field.rs:208-225).  Host only: works without a GPU."""
+    (token_score.rs:196-209, string_field.rs:208-225).  Works without a GPU; resolve_batch(ctx=...) expands typos
+    on that ctx's device."""
 
     def __init__(self, n_fields: int = 1):
         self.n_fields = n_fields
@@ -1067,23 +1068,64 @@ class TermDictionary:
         n = lib().oc_stem_english(b, len(b), out, len(b) + 8, None)
         return out.raw[:n].decode("utf-8") if n else token
 
-    def resolve_batch(self, texts: Sequence[str], exact: bool = False, tolerance: Optional[int] = None,
-                      boost: Optional[Sequence[float]] = None, properties: Optional[Sequence[int]] = None,
-                      exact_match_boost: float = 0.0) -> "TextQueryBatch":
-        """SearchParams{tokens, exact_match, boost, tolerance} for B queries at once (token_score.rs:235-242)
-        -> the packed CSR arrays oc_search takes."""
-        rp = _lib.ResolveParams()
-        arr = (C.c_char_p * len(texts))(*[t.encode("utf-8") for t in texts])
-        rp.texts, rp.n_queries = arr, len(texts)
-        rp.exact, rp.tolerance = int(bool(exact)), -1 if tolerance is None else int(tolerance)
+    def _field_arrays(self, boost, properties):
         fb = None if boost is None else np.ascontiguousarray(boost, np.float32)
+        if fb is not None and fb.size != self.n_fields:
+            raise ValueError(f"boost has {fb.size} entries for {self.n_fields} fields")
         fm = None
         if properties is not None:
             fm = np.zeros(self.n_fields, np.uint8)
             fm[list(properties)] = 1
-        rp.field_boost, rp.field_mask, rp.exact_match_boost = _p(fb), _p(fm), float(exact_match_boost)
+        return fb, fm
+
+    def device_bytes(self, ctx: "Context") -> int:
+        """Device memory of this dictionary's mirror on ctx (0 before the first resolve_batch(ctx=ctx) that needed it)."""
+        return int(lib().oc_dict_device_bytes(self._h, ctx._h))
+
+    def resolve_batch(self, texts: Sequence[str], exact=False, tolerance=None, boost=None, properties=None,
+                      exact_match_boost: float = 0.0, ctx: Optional["Context"] = None) -> "TextQueryBatch":
+        """SearchParams{tokens, exact_match, boost, tolerance} for B queries at once (token_score.rs:235-242)
+        -> the packed CSR arrays oc_search takes.  exact (bool), tolerance (None or int), boost (None or one weight per
+        field) and properties (None or field indexes) each take one value for the batch or a list of one per query.
+        With a ctx, the tolerance >= 1 expansions run on its device (oc_dict_resolve_q); the output is the same."""
+        B = len(texts)
+
+        def per_query(v, single):
+            if single(v):
+                return None
+            v = list(v)
+            if len(v) != B:
+                raise ValueError(f"{len(v)} per-query values for {B} queries")
+            return v
+
+        def flat(v):
+            return v is None or all(isinstance(x, (int, float, np.integer, np.floating)) for x in v)
+        qe = per_query(exact, lambda v: isinstance(v, (bool, int, np.bool_, np.integer)))
+        qt = per_query(tolerance, lambda v: v is None or isinstance(v, (int, np.integer)))
+        qb, qp = per_query(boost, flat), per_query(properties, flat)
+        rp = _lib.ResolveParams()
+        arr = (C.c_char_p * B)(*[t.encode("utf-8") for t in texts])
+        rp.texts, rp.n_queries = arr, B
+        rp.exact_match_boost = float(exact_match_boost)
+        keep, q = [], None
+        if qe is None and qt is None and qb is None and qp is None:
+            rp.exact, rp.tolerance = int(bool(exact)), -1 if tolerance is None else int(tolerance)
+            fb, fm = self._field_arrays(boost, properties)
+            rp.field_boost, rp.field_mask = _p(fb), _p(fm)
+        else:
+            q = (_lib.ResolveQuery * B)()
+            for b in range(B):
+                t = qt[b] if qt is not None else tolerance
+                fb, fm = self._field_arrays(qb[b] if qb is not None else boost, qp[b] if qp is not None else properties)
+                keep += [fb, fm]
+                q[b].exact = int(bool(qe[b] if qe is not None else exact))
+                q[b].tolerance = -1 if t is None else int(t)
+                q[b].field_boost, q[b].field_mask = _p(fb), _p(fm)
         res = C.c_void_p()
-        check(lib().oc_dict_resolve(self._h, C.byref(rp), C.byref(res)))
+        if q is None and ctx is None:
+            check(lib().oc_dict_resolve(self._h, C.byref(rp), C.byref(res)))
+        else:
+            check(lib().oc_dict_resolve_q(self._h, None if ctx is None else ctx._h, C.byref(rp), q, C.byref(res)))
         try:
             ptrs = [C.c_void_p() for _ in range(5)]
             nt, ne = C.c_uint32(), C.c_uint32()

@@ -223,8 +223,9 @@ class IndexLoader:
         return TokenScoreContext(self.ctx, self.emb, self.strs)
 
     def resolve(self, texts: Sequence[str], **kw):
-        """token_score.rs:196-209 + the FST expansion: the packed query arrays oc_search takes."""
-        return self.dict.resolve_batch(list(texts), **kw)
+        """token_score.rs:196-209 + the FST expansion: the packed query arrays oc_search takes.  Typo-tolerant
+        expansions run on this index's device."""
+        return self.dict.resolve_batch(list(texts), ctx=self.ctx, **kw)
 
     def close(self):
         for x in [self.facets, self.emb, self.strs, self.dict, self._live] + list(self.geo.values()) + self._retired:

@@ -177,6 +177,13 @@ pub struct OcResolveParams {
     pub field_mask: *const u8,
     pub exact_match_boost: f32,
 }
+#[repr(C)]
+pub struct OcResolveQuery {
+    pub exact: c_int,
+    pub tolerance: c_int,           // < 0 => None (prefix expansion)
+    pub field_boost: *const f32,
+    pub field_mask: *const u8,
+}
 pub type OcStemFn = unsafe extern "C" fn(tok: *const c_char, len: usize, out: *mut c_char, cap: usize, user: *mut c_void) -> usize;
 
 extern "C" {
@@ -338,6 +345,10 @@ extern "C" {
     pub fn oc_dict_size(d: *mut OcDict, field: u32) -> u32;
     pub fn oc_dict_set_stemmer(d: *mut OcDict, f: Option<OcStemFn>, user: *mut c_void) -> c_int;
     pub fn oc_dict_resolve(d: *mut OcDict, p: *const OcResolveParams, out: *mut *mut OcResolved) -> c_int;
+    /// per query its own exact / tolerance / boost / mask (q NULL: p's); ctx non-NULL: typo tolerance on its device
+    pub fn oc_dict_resolve_q(d: *mut OcDict, ctx: *mut OcCtx, p: *const OcResolveParams, q: *const OcResolveQuery,
+                             out: *mut *mut OcResolved) -> c_int;
+    pub fn oc_dict_device_bytes(d: *mut OcDict, ctx: *mut OcCtx) -> u64;
     pub fn oc_resolved_fill(r: *const OcResolved, p: *mut OcSearchParams);
     pub fn oc_resolved_free(r: *mut OcResolved);
 }
