@@ -200,9 +200,9 @@ def make_filter_bits(allowed_doc_ids: Sequence[int], nbits: int) -> np.ndarray:
 
 
 # ---------------------------------------------------------------- the restated functions
-def fulltext(ix: StrIndex, q, threshold=None, filter_bits=None, filter_nbits=0):
-    """search_full_text: returns (doc_ids sorted, scores) = the whole score map."""
-    tq, tp, m = _TQ(q), _TP(threshold, filter_bits, filter_nbits), _Map()
+def fulltext(ix: StrIndex, q, threshold=None, filter_bits=None, filter_nbits=0, b=0.75, k=1.2):
+    """search_full_text: returns (doc_ids sorted, scores) = the whole score map.  b / k: Bm25Params."""
+    tq, tp, m = _TQ(q), _TP(threshold, filter_bits, filter_nbits, b, k), _Map()
     rc = lib().orc_fulltext(C.byref(ix.c), C.byref(tq.c), C.byref(tp.c), C.byref(m))
     assert rc == 0
     return _take_map(m)
@@ -262,9 +262,9 @@ class SearchBatch:
 
     def add(self, mode: int, limit: int = 10, offset: int = 0, similarity: float = 0.7,
             q_vec: Optional[np.ndarray] = None, text=None, threshold=None,
-            filter_bits=None, filter_nbits=0, omc_doc=None, omc_mult=None):
+            filter_bits=None, filter_nbits=0, omc_doc=None, omc_mult=None, b=0.75, k=1.2):
         tq = _TQ(text) if text is not None else None
-        tp = _TP(threshold, filter_bits, filter_nbits)
+        tp = _TP(threshold, filter_bits, filter_nbits, b, k)
         qv = None if q_vec is None else np.ascontiguousarray(q_vec, np.float32)
         od = None if omc_doc is None else np.ascontiguousarray(omc_doc, np.uint64)
         om = None if omc_mult is None else np.ascontiguousarray(omc_mult, np.float32)

@@ -19,7 +19,8 @@ sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "oracle"))
 import oracle as orc                                   # noqa: E402
 from oramacore_b200.hostindex import HostStringIndex   # noqa: E402
 
-QUERIES = [  # (term, exact, on the GPU test too?)  benches/fulltext_simple.rs:438-458 use the first three strings
+QUERIES = [  # (term, exact, gpu_ok: a flag kept in the fixture, unused: the GPU test runs every query)
+    # benches/fulltext_simple.rs:438-458 use the first three strings
     ("technology", False, False), ("technology software", False, False), ("development", False, False),
     ("fantasy", False, True), ("open world", False, True), ("rpg", True, True), ("adventure", False, True),
     ("elden ring", True, True), ("war", False, True), ("space station", False, True), ("racing cars", False, False),

@@ -41,12 +41,13 @@ def _sorted(docs, scores):
 
 
 def ref_map(orc, ix, q, mode="fulltext", st=None, qv=None, limit=10, similarity=0.0, threshold=None,
-            omc_doc=None, omc_mult=None):
-    """The whole score map of one request, sorted; `limit` is the vector stage's depth (search.rs:330-336)."""
+            omc_doc=None, omc_mult=None, **ft_kw):
+    """The whole score map of one request, sorted; `limit` is the vector stage's depth (search.rs:330-336).
+    ft_kw goes to orc.fulltext: filter_bits / filter_nbits, b, k."""
     if mode == "vector":
         m = orc.vector(st, qv, limit, similarity)
     else:
-        m = orc.fulltext(ix, q, threshold=threshold)
+        m = orc.fulltext(ix, q, threshold=threshold, **ft_kw)
         if mode == "hybrid":
             m = orc.hybrid_combine(orc.vector(st, qv, limit, similarity), m)
     if omc_doc is not None:

@@ -9,7 +9,8 @@ import numpy as np
 import pytest
 
 import oramacore_b200 as ob
-from helpers import assert_topk_equal
+from test_gpu_tile3 import _env
+from test_gpu_topn_paths import ALL, _routes
 
 FIX = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "games_fulltext.npz")
 
@@ -39,13 +40,23 @@ def test_oracle_reproduces_the_committed_answers(orc):
 
 
 @pytest.mark.gpu
-def test_gpu_fulltext_on_the_games_corpus(gpu_ctx, orc):
+def test_gpu_fulltext_on_the_games_corpus(gpu_ctx):
+    """All 13 queries — single-term tokens in one field, two-field tokens, prefix expansions of up to 34 terms, the
+    unknown term and "the" (22 terms, 1468 matches) — as one batch and each query alone, on every scorer route:
+    count, top-10 doc ids and score bits equal the oracle's committed answers."""
     z, data, qs = _load()
-    sel = [i for i in range(len(qs)) if z["gpu_ok"][i]]
     strs = ob.StringFieldStorage(gpu_ctx, data)
-    hits = ob.search(gpu_ctx, None, strs, "fulltext", texts=[qs[i] for i in sel], limit=10)
-    for h, i in zip(hits, sel):
-        n = int(z["exp_n"][i])
-        assert h.count == int(z["exp_count"][i]), (i, h.count, int(z["exp_count"][i]))
-        assert_topk_equal(h.doc_ids, h.scores, z["exp_docs"][i, :n], z["exp_scores"][i, :n], atol=1e-5)
-    strs.close()
+    try:
+        for name, env in _routes(ALL):
+            with _env(**env):
+                batch = ob.search(gpu_ctx, None, strs, "fulltext", texts=qs, limit=10)
+                alone = [ob.search(gpu_ctx, None, strs, "fulltext", texts=[q], limit=10)[0] for q in qs]
+            for i in range(len(qs)):
+                n = int(z["exp_n"][i])
+                for how, h in (("batch", batch[i]), ("alone", alone[i])):
+                    ctx = (name, how, i)
+                    assert h.count == int(z["exp_count"][i]), (ctx, h.count, int(z["exp_count"][i]))
+                    assert np.array_equal(h.doc_ids, z["exp_docs"][i, :n]), (ctx, h.doc_ids, z["exp_docs"][i, :n])
+                    assert np.array_equal(h.scores, z["exp_scores"][i, :n]), (ctx, h.scores, z["exp_scores"][i, :n])
+    finally:
+        strs.close()
