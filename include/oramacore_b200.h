@@ -177,8 +177,32 @@ int oc_str_insert(oc_str *s, uint32_t field, uint64_t doc_id, uint16_t field_len
  * owns the corpus-wide values, see oc_str_set_global) and publishes it with a pointer swap — the reference's
  * CURRENT + versions/<n> scheme (embedding_field.rs:91-95).  The build runs WITHOUT the context lock on the
  * store's own stream: oc_search keeps serving the previous version meanwhile.  A failed commit changes nothing
- * (the pending ops stay queued).  One commit at a time per store. */
+ * (the pending ops stay queued).  One commit at a time per store.  The merge runs on the device: its cost is
+ * O(pending ops) on the host and one pass over the committed postings on the device, and the store keeps no host
+ * copy of its postings.  Same as oc_str_commit_ex(s, NULL). */
 int oc_str_commit(oc_str *s);
+/* Statistics of one oc_str_commit_ex call. */
+typedef struct {
+    uint64_t rows_before, rows_after;          /* rows of the base and of the new snapshot                       */
+    uint64_t postings_before, postings_after;  /* postings of all fields, base / new snapshot                    */
+    uint64_t pending_postings;                 /* pending postings merged (after cancelled and replaced inserts) */
+    uint64_t workspace_bytes;                  /* device memory the call held besides the new snapshot's arrays  */
+    float device_ms;                           /* CUDA-event time of the device work on the store's load stream  */
+    float wall_ms;                             /* the whole call, publishing included                             */
+} oc_str_commit_t;
+/* oc_str_commit, filling *out (may be NULL) when it succeeds.  OC_ERR_INVALID: a term id listed twice in one insert
+ * of a document, or a commit already in flight; OC_ERR_OOM: no room for the new snapshot or the workspace.  Either
+ * way nothing changes. */
+int oc_str_commit_ex(oc_str *s, oc_str_commit_t *out);
+/* Read-back of the published snapshot, the inverse of oc_str_set_rows + oc_str_load_field — what compact()
+ * (string_field.rs:186-191) leaves on disk, so a caller can persist a committed version.  Each call reads one
+ * snapshot; compare `version` across calls.  With NULL arrays they return the sizes; otherwise *n_rows (*n_terms,
+ * *n_postings) is the capacity of the arrays on entry, and a capacity too small fails with OC_ERR_INVALID after
+ * writing the sizes.  row_doc_ids gets the ascending doc id of every row (the identity when the store has no map);
+ * term_offsets takes n_terms + 1 entries. */
+int oc_str_read_rows(oc_str *s, uint64_t *n_rows, uint64_t *row_doc_ids, uint64_t *document_count, uint64_t *version);
+int oc_str_read_field(oc_str *s, uint32_t field, float *avg_field_len, uint32_t *n_terms, uint64_t *n_postings,
+                      uint64_t *term_offsets, uint32_t *post_row, uint16_t *post_tf, uint16_t *post_len);
 /* StringFieldStorage::delete (string_field.rs:180-182).  Ops apply in call order like the reference's compact:
  * the committed rows of the document are tombstoned at once and its still-pending inserts are cancelled; an
  * insert after the delete is a new document. */

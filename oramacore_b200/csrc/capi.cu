@@ -3,8 +3,11 @@
 // No torch, no CPU fallback: every entry point needs a live CUDA device.
 #include <cuda_runtime.h>
 
+#include <cub/device/device_radix_sort.cuh>
+
 #include <algorithm>
 #include <atomic>
+#include <chrono>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
@@ -25,6 +28,7 @@
 #include "dict_dev.cuh"
 #include "stem_en.h"
 #include "emb_compact.cuh"
+#include "str_commit.cuh"
 #include "emb_gemm.cuh"
 #include "emb_scan.cuh"
 #include "fuse.cuh"
@@ -1107,7 +1111,7 @@ extern "C" int oc_emb_search(oc_emb *e, const float *queries, uint32_t B, uint32
 // Snapshot model (the reference keeps `CURRENT` + `versions/<n>` per field and swaps the pointer after
 // compact(), embedding_field.rs:91-95 / string_field.rs:186-191): searches work on the published,
 // immutable StrSnap they grabbed at call entry; oc_str_commit builds the next snapshot WITHOUT the
-// ctx lock (host merge + upload on the store's own stream) and publishes it with a pointer swap, so
+// ctx lock (device merge on the store's own stream, str_commit.cuh) and publishes it with a pointer swap, so
 // searches keep running on the previous version while a commit is in flight.  Ops that arrive during
 // a commit: inserts queue for the next one, deletes hit the old snapshot at once and are replayed on
 // the new one before it is published.
@@ -1120,7 +1124,6 @@ struct StrField {
     Posting *post = nullptr;             // device: (row, tf') derived for b_cached
     float b_cached = -1.f;
     uint64_t n_post = 0;
-    std::vector<PostingRaw> host_post;   // host copy of the committed postings (term-major), kept for oc_str_commit
 };
 // a process-wide identity per snapshot state: a new snapshot takes one, and so does every change made to a published
 // snapshot in place (a field load, corpus-wide values, tombstones).  Keys the dense-array cache (dense_cache.h).
@@ -1168,6 +1171,7 @@ struct oc_str {
     bool global_count = false, global_avg = false;   // document_count / avg_field_len are values owned by the caller (shard of a larger index; an
                                                      // Index whose document_count also counts documents without string fields): commit keeps them
     cudaStream_t load_stream = nullptr;
+    cudaEvent_t ev[4] = {};                          // oc_str_commit_ex: device time of its two device phases
 };
 static std::shared_ptr<StrSnap> str_snapshot(oc_str *s) {
     std::lock_guard<std::mutex> g(s->mu);
@@ -1185,6 +1189,7 @@ extern "C" int oc_str_create(oc_ctx *c, uint32_t n_fields, oc_str **out) {
     s->cur->fields.resize(n_fields);
     s->pending.resize(n_fields);
     CU(cudaStreamCreateWithFlags(&s->load_stream, cudaStreamNonBlocking));
+    for (auto &e : s->ev) CU(cudaEventCreate(&e));
     *out = s;
     return OC_OK;
 }
@@ -1193,6 +1198,7 @@ extern "C" void oc_str_destroy(oc_str *s) {
     cudaSetDevice(s->ctx->device);
     cudaStreamSynchronize(s->ctx->stream);
     if (s->load_stream) { cudaStreamSynchronize(s->load_stream); cudaStreamDestroy(s->load_stream); }
+    for (auto &e : s->ev) if (e) cudaEventDestroy(e);
     s->cur.reset();
     delete s;
 }
@@ -1251,8 +1257,11 @@ extern "C" int oc_str_load_field(oc_str *s, uint32_t field, float avg_field_len,
     oc_ctx *c = s->ctx;
     std::lock_guard<std::mutex> g(c->mu);
     CU(cudaSetDevice(c->device));
-    std::shared_ptr<StrSnap> snap = str_snapshot(s);
-    StrSnap &S = *snap;
+    // held for the whole load: a commit reads the published snapshot's posting arrays on the device, so it may
+    // neither be running now nor start before this field is in place
+    std::lock_guard<std::mutex> g2(s->mu);
+    if (s->committing) return fail(OC_ERR_INVALID, "oc_str_load_field while a commit is in flight");
+    StrSnap &S = *s->cur;
     if (field >= S.fields.size()) return fail(OC_ERR_INVALID, "field %u out of range", field);
     StrField &f = S.fields[field];
     S.ident = next_snap_ident();
@@ -1264,10 +1273,10 @@ extern "C" int oc_str_load_field(oc_str *s, uint32_t field, float avg_field_len,
         if (term_offsets[t + 1] - term_offsets[t] > 0xffffffffull) return fail(OC_ERR_UNSUPPORTED, "posting list too long");
     }
     f.avg_len = avg_field_len; f.n_terms = n_terms; f.n_post = np;
-    f.host_post.resize(np);
+    std::vector<PostingRaw> stage(np);   // interleaved for the upload only: the store keeps no host copy
     for (uint64_t i = 0; i < np; i++) {
         if (post_row[i] >= S.n_rows && S.n_rows) return fail(OC_ERR_INVALID, "posting row %u >= n_rows", post_row[i]);
-        f.host_post[i].row = post_row[i]; f.host_post[i].tf = post_tf[i]; f.host_post[i].len = post_len[i];
+        stage[i].row = post_row[i]; stage[i].tf = post_tf[i]; stage[i].len = post_len[i];
     }
     f.term_offsets.assign(term_offsets, term_offsets + n_terms + 1);
     f.global_df.clear();
@@ -1275,7 +1284,7 @@ extern "C" int oc_str_load_field(oc_str *s, uint32_t field, float avg_field_len,
     if (np) {
         CU(cudaMalloc(&f.post, (np + 4) * sizeof(Posting)));
         CU(cudaMalloc(&f.raw, (np + 4) * sizeof(PostingRaw)));
-        CU(cudaMemcpyAsync(f.raw, f.host_post.data(), np * sizeof(PostingRaw), cudaMemcpyHostToDevice, c->stream));
+        CU(cudaMemcpyAsync(f.raw, stage.data(), np * sizeof(PostingRaw), cudaMemcpyHostToDevice, c->stream));
         CU(cudaStreamSynchronize(c->stream));
     }
     return OC_OK;
@@ -1336,15 +1345,21 @@ extern "C" int oc_str_insert(oc_str *s, uint32_t field, uint64_t doc_id, uint16_
 
 // Merges pending inserts and deletes into the next snapshot: rows are the ascending doc ids, postings
 // term-major / row-ascending, avg_field_len and document_count refreshed (unless the caller owns the
-// corpus-wide values), tombstones dropped.  Everything is built in temporaries; the published snapshot
-// is replaced only after every field validated and uploaded, so a failed commit changes nothing.
-extern "C" int oc_str_commit(oc_str *s) {
+// corpus-wide values), tombstones dropped.  The host filters the pending ops; the merge of the committed postings
+// runs on the device (str_commit.cuh) on the store's own stream, reading the base snapshot's immutable arrays and
+// the alive bitmap as it was when the commit started.  Everything is built in temporaries; the published snapshot
+// is replaced only after every field validated and was built, so a failed commit changes nothing.
+extern "C" int oc_str_commit(oc_str *s) { return oc_str_commit_ex(s, nullptr); }
+
+extern "C" int oc_str_commit_ex(oc_str *s, oc_str_commit_t *out) {
     if (!s) return fail(OC_ERR_INVALID, "str is NULL");
+    const auto wall0 = std::chrono::steady_clock::now();
     oc_ctx *c = s->ctx;
     std::shared_ptr<StrSnap> base;
     std::vector<std::vector<PendingPost>> pend;
     std::unordered_map<uint64_t, uint64_t> pdel;
     std::vector<uint32_t> base_alive;
+    uint64_t base_deleted;
     bool global_count, global_avg;
     {
         std::lock_guard<std::mutex> g(s->mu);
@@ -1356,6 +1371,7 @@ extern "C" int oc_str_commit(oc_str *s) {
         for (size_t i = 0; i < pend.size(); i++) pend[i].swap(s->pending[i]);
         pdel.swap(s->pending_deleted);
         base_alive = base->alive_host;
+        base_deleted = base->n_deleted;
         global_count = s->global_count; global_avg = s->global_avg;
     }
     // on failure: put the taken ops back (in front of whatever arrived meanwhile) and leave `cur` alone
@@ -1389,109 +1405,262 @@ extern "C" int oc_str_commit(oc_str *s) {
         }
         pv.resize(w);
     }
-    // ---- row space of the next snapshot
-    std::vector<uint64_t> docs;
-    std::vector<uint8_t> old_alive(B.n_rows, 1);
-    for (uint64_t r = 0; r < B.n_rows; r++) {
-        const bool alive = base_alive.empty() || ((base_alive[r >> 5] >> (r & 31)) & 1u);
-        old_alive[r] = alive;
-        if (alive) docs.push_back(B.row_doc_host.empty() ? r : B.row_doc_host[r]);
+    // ---- row space of the next snapshot, as far as the pending documents decide it (O(pending)): the new rows are
+    // the alive old documents merged with the pending documents that are not one of them, ascending
+    const uint64_t n_old = B.n_rows;
+    auto old_doc = [&](uint64_t r) { return B.row_doc_host.empty() ? r : B.row_doc_host[r]; };
+    auto old_alive = [&](uint64_t r) { return base_alive.empty() || ((base_alive[r >> 5] >> (r & 31)) & 1u); };
+    std::vector<uint64_t> pdoc;
+    for (auto &pv : pend) for (auto &pn : pv) pdoc.push_back(pn.doc);
+    std::sort(pdoc.begin(), pdoc.end());
+    pdoc.erase(std::unique(pdoc.begin(), pdoc.end()), pdoc.end());
+    if (pdoc.size() > 0xfffffff0ull) return abort_commit(fail(OC_ERR_UNSUPPORTED, "more than 2^32 rows per store"));
+    const uint32_t n_pdoc = (uint32_t)pdoc.size();
+    std::vector<uint32_t> p_lbold(n_pdoc), p_newbelow(size_t(n_pdoc) + 1);
+    uint32_t n_new_p = 0;
+    for (uint32_t j = 0; j < n_pdoc; j++) {
+        const uint64_t d = pdoc[j];
+        const uint64_t lb = B.row_doc_host.empty() ? std::min(d, n_old)
+                                                   : uint64_t(std::lower_bound(B.row_doc_host.begin(), B.row_doc_host.end(), d) - B.row_doc_host.begin());
+        p_lbold[j] = (uint32_t)lb;
+        p_newbelow[j] = n_new_p;
+        if (!(lb < n_old && old_doc(lb) == d && old_alive(lb))) n_new_p++;
     }
-    for (auto &pv : pend) for (auto &pn : pv) docs.push_back(pn.doc);
-    std::sort(docs.begin(), docs.end());
-    docs.erase(std::unique(docs.begin(), docs.end()), docs.end());
-    if (docs.size() > 0xfffffff0ull) return abort_commit(fail(OC_ERR_UNSUPPORTED, "more than 2^32 rows per store"));
-    auto row_of = [&](uint64_t d) { return (uint32_t)(std::lower_bound(docs.begin(), docs.end(), d) - docs.begin()); };
-    std::vector<uint32_t> remap(B.n_rows, 0xffffffffu);
-    for (uint64_t r = 0; r < B.n_rows; r++) if (old_alive[r]) remap[r] = row_of(B.row_doc_host.empty() ? r : B.row_doc_host[r]);
-    auto ns = std::make_shared<StrSnap>();
-    ns->device = c->device;
-    ns->fields.resize(nf);
-    struct Rec { uint32_t term, row; uint16_t tf, len; };
+    p_newbelow[n_pdoc] = n_new_p;
+    const uint64_t n_new = (n_old - base_deleted) + n_new_p;
+    if (n_new > 0xfffffff0ull) return abort_commit(fail(OC_ERR_UNSUPPORTED, "more than 2^32 rows per store"));
+    uint64_t max_doc = n_pdoc ? pdoc.back() : 0;
+    for (uint64_t r = n_old; r-- > 0;)
+        if (old_alive(r)) { max_doc = std::max(max_doc, old_doc(r)); break; }
+    const bool identity = n_new > 0 && max_doc == n_new - 1;   // n_new distinct ascending ids ending at n_new - 1
+
+    // ---- the upload, packed: per-field result slots first (len sums, duplicate flags: their initial values), then
+    // the row-space arrays and the per-field pending postings
+    struct FieldPlan {
+        uint32_t n_terms_old, n_terms, n_pend, n_repl, end_bit;
+        size_t o_off, o_term, o_doc, o_tf, o_len, o_repl;              // in the upload
+        size_t o_keep, o_kpre, o_kblk, o_keys, o_vals, o_newoff, o_tblk, o_slo, o_plo;   // in the workspace
+        uint64_t n_kw, n_kb, n_tb;
+    };
+    struct FieldRes { unsigned long long len_sum, len_cnt; uint32_t dup, dup_term; };
+    std::vector<FieldPlan> plan(nf);
+    std::vector<uint8_t> up;
+    auto put = [&](const void *src, size_t bytes) {
+        const size_t o = up.size();
+        up.resize(o + ((bytes + 15) & ~size_t(15)), 0);
+        if (bytes) memcpy(up.data() + o, src, bytes);
+        return o;
+    };
+    std::vector<FieldRes> res(nf, FieldRes{0, 0, 0, 0xffffffffu});
+    const size_t o_res = put(res.data(), nf * sizeof(FieldRes));
+    const size_t o_pdoc = put(pdoc.data(), pdoc.size() * 8), o_lbold = put(p_lbold.data(), p_lbold.size() * 4),
+                 o_newbelow = put(p_newbelow.data(), p_newbelow.size() * 4);
+    size_t o_alive = 0;
+    const uint64_t n_aw = base_alive.empty() ? 0 : base_alive.size() + 1;   // + a zero word: alive_below(n_old) reads it
+    if (n_aw) { base_alive.push_back(0); o_alive = put(base_alive.data(), n_aw * 4); }
+    uint64_t pend_total = 0, post_before = 0;
     for (size_t fi = 0; fi < nf; fi++) {
         const StrField &of = B.fields[fi];
-        StrField &f = ns->fields[fi];
-        // the committed postings are already term-major / row-ascending and the row remap is monotone, so only the
-        // PENDING postings are sorted; the next CSR is a per-term linear merge of (surviving old list, new list):
-        // O(P_old + p log p) instead of a sort of everything
-        std::vector<uint8_t> replaced(docs.size(), 0);   // a re-inserted document replaces its old postings in this field
-        for (auto &pn : pend[fi]) replaced[row_of(pn.doc)] = 1;
-        std::vector<Rec> add;
-        add.reserve(pend[fi].size());
-        uint32_t max_term = of.n_terms;
-        for (auto &pn : pend[fi]) {
+        FieldPlan &P = plan[fi];
+        std::vector<uint32_t> term, doc, repl;
+        std::vector<uint16_t> tf, len;
+        uint32_t max_term = 0;
+        for (size_t i = 0; i < pend[fi].size(); i++) {
+            const PendingPost &pn = pend[fi][i];
+            const uint32_t j = (uint32_t)(std::lower_bound(pdoc.begin(), pdoc.end(), pn.doc) - pdoc.begin());
+            if (i == 0 || pn.doc != pend[fi][i - 1].doc) repl.push_back(j);   // one insert's postings are adjacent
             if (pn.term == 0xffffffffu) continue;
-            add.push_back({pn.term, row_of(pn.doc), pn.tf, pn.len});
-            max_term = std::max(max_term, pn.term + 1);
+            term.push_back(pn.term); doc.push_back(j); tf.push_back(pn.tf); len.push_back(pn.len);
+            max_term = std::max(max_term, pn.term);
         }
-        std::sort(add.begin(), add.end(), [](const Rec &a, const Rec &b) { return a.term != b.term ? a.term < b.term : a.row < b.row; });
-        for (size_t i = 1; i < add.size(); i++)
-            if (add[i].term == add[i - 1].term && add[i].row == add[i - 1].row)
-                return abort_commit(fail(OC_ERR_INVALID, "field %zu: term %u listed twice in one insert of a document", fi, add[i].term));
-        f.n_terms = max_term;
-        f.term_offsets.assign(size_t(max_term) + 1, 0);
-        f.host_post.clear();
-        f.host_post.reserve(of.host_post.size() + add.size());
-        std::vector<uint16_t> len_of_row(docs.size(), 0);
-        size_t ai = 0;
-        for (uint32_t t = 0; t < max_term; t++) {
-            f.term_offsets[t] = f.host_post.size();
-            uint64_t oi = t < of.n_terms ? of.term_offsets[t] : 0, oe = t < of.n_terms ? of.term_offsets[t + 1] : 0;
-            auto old_next = [&]() -> bool {   // advances oi to the next surviving old posting of this term
-                while (oi < oe) {
-                    const uint32_t nr = remap[of.host_post[oi].row];
-                    if (nr != 0xffffffffu && !replaced[nr]) return true;
-                    oi++;
-                }
-                return false;
-            };
-            for (;;) {
-                const bool ho = old_next(), hn = ai < add.size() && add[ai].term == t;
-                if (!ho && !hn) break;
-                PostingRaw pr;
-                if (ho && (!hn || remap[of.host_post[oi].row] < add[ai].row)) {
-                    pr.row = remap[of.host_post[oi].row]; pr.tf = of.host_post[oi].tf; pr.len = of.host_post[oi].len; oi++;
-                } else {   // (equal rows cannot happen: a row with a pending insert is `replaced`)
-                    pr.row = add[ai].row; pr.tf = add[ai].tf; pr.len = add[ai].len; ai++;
-                }
-                f.host_post.push_back(pr);
-                len_of_row[pr.row] = pr.len;
+        P.n_terms_old = of.n_terms;
+        P.n_pend = (uint32_t)term.size();
+        P.n_repl = (uint32_t)repl.size();
+        P.n_terms = P.n_pend ? std::max(of.n_terms, max_term + 1) : of.n_terms;
+        int tb = 0;
+        while (tb < 32 && (uint64_t(max_term) >> tb)) tb++;
+        P.end_bit = 32 + tb;
+        P.o_off = put(of.term_offsets.data(), of.n_terms ? (size_t(of.n_terms) + 1) * 8 : 0);
+        P.o_term = put(term.data(), term.size() * 4); P.o_doc = put(doc.data(), doc.size() * 4);
+        P.o_tf = put(tf.data(), tf.size() * 2); P.o_len = put(len.data(), len.size() * 2);
+        P.o_repl = put(repl.data(), repl.size() * 4);
+        pend_total += P.n_pend; post_before += of.n_post;
+    }
+    // ---- the workspace, one allocation: upload | alive scan | remap | prow | replaced bits | row keys | CUB temp |
+    // per field: survivor bits + scan, sorted keys / values, term counts and offsets
+    size_t ws = 0;
+    auto take = [&](size_t bytes) { const size_t o = ws; ws += (bytes + 255) & ~size_t(255); return o; };
+    const size_t w_up = take(up.size());
+    const uint64_t n_ab = (n_aw + COMPACT_SCAN_WORDS - 1) / COMPACT_SCAN_WORDS;
+    const size_t w_apre = take(n_aw * 4), w_ablk = take(n_ab * 4);
+    const size_t w_remap = take(n_old * 4), w_prow = take(size_t(n_pdoc) * 4);
+    const uint64_t n_rw = n_new / 32 + 1;
+    const size_t w_repl = take(n_rw * 4);
+    const size_t w_rowkey = take(global_avg ? 0 : n_new * 8);
+    size_t cub_bytes = 0;
+    for (size_t fi = 0; fi < nf; fi++) {
+        FieldPlan &P = plan[fi];
+        const uint64_t np = B.fields[fi].n_post;
+        P.n_kw = np ? np / 32 + 1 : 0;
+        P.n_kb = (P.n_kw + COMPACT_SCAN_WORDS - 1) / COMPACT_SCAN_WORDS;
+        P.n_tb = P.n_terms ? (uint64_t(P.n_terms) + 1 + COMPACT_SCAN_WORDS - 1) / COMPACT_SCAN_WORDS : 0;
+        P.o_keep = take(P.n_kw * 4); P.o_kpre = take(P.n_kw * 4); P.o_kblk = take(P.n_kb * 4);
+        P.o_keys = take(size_t(P.n_pend) * 16); P.o_vals = take(size_t(P.n_pend) * 8);
+        P.o_newoff = take(P.n_terms ? (size_t(P.n_terms) + 1) * 8 : 0); P.o_tblk = take(P.n_tb * 8);
+        P.o_slo = take(size_t(P.n_terms) * 4); P.o_plo = take(P.n_terms ? (size_t(P.n_terms) + 1) * 4 : 0);
+        if (P.n_pend) {
+            size_t b = 0;
+            if (cub::DeviceRadixSort::SortPairs(nullptr, b, (const uint64_t *)nullptr, (uint64_t *)nullptr, (const uint32_t *)nullptr,
+                                                (uint32_t *)nullptr, P.n_pend, 0, P.end_bit, s->load_stream) != cudaSuccess)
+                return abort_commit(fail(OC_ERR_CUDA, "DeviceRadixSort temp size"));
+            cub_bytes = std::max(cub_bytes, b);
+        }
+    }
+    const size_t w_cub = take(cub_bytes);
+    auto ns = std::make_shared<StrSnap>();   // declared before wsp: on failure its arrays are freed after the stream is idle
+    ns->device = c->device;
+    ns->fields.resize(nf);
+    ns->n_rows = n_new;
+    ns->document_count = global_count ? B.document_count : n_new;
+    struct Workspace {   // every way out of the call waits for the load stream, then gives the workspace back
+        oc_str *s; uint8_t *p = nullptr;
+        ~Workspace() { cudaStreamSynchronize(s->load_stream); cudaFree(p); }
+    } wsp{s};
+    auto merge = [&]() -> int {
+        CU(cudaMalloc(&wsp.p, std::max<size_t>(ws, 256)));
+        uint8_t *W = wsp.p;
+        auto at = [&](size_t o) { return static_cast<void *>(W + o); };
+        const uint8_t *U = W + w_up;
+        auto up_at = [&](size_t o) { return static_cast<const void *>(U + o); };
+        FieldRes *d_res = (FieldRes *)(W + w_up + o_res);
+        if (!identity && n_new) CU(cudaMalloc(&ns->row_doc, n_new * 8));
+        cudaStream_t st = s->load_stream;
+        const unsigned max_grid = (unsigned)c->prop.multiProcessorCount * 8;
+        auto blocks = [](uint64_t n, uint64_t per) { return (unsigned)std::max<uint64_t>(1, (n + per - 1) / per); };
+        CU(cudaEventRecord(s->ev[0], st));
+        CU(cudaMemcpyAsync(W + w_up, up.data(), up.size(), cudaMemcpyHostToDevice, st));
+        // 1. row space
+        const uint32_t *alive = n_aw ? (const uint32_t *)up_at(o_alive) : nullptr;
+        uint32_t *a_pre = (uint32_t *)at(w_apre), *a_blk = (uint32_t *)at(w_ablk);
+        if (n_aw) {
+            compact_scan_words_kernel<<<(unsigned)n_ab, COMPACT_SCAN_WORDS, 0, st>>>(alive, n_aw, a_pre, a_blk);
+            compact_scan_blocks_kernel<uint32_t><<<1, COMPACT_SCAN_WORDS, 0, st>>>(a_blk, (uint32_t)n_ab);
+        }
+        uint32_t *remap = (uint32_t *)at(w_remap), *prow = (uint32_t *)at(w_prow);
+        const uint64_t *d_pdoc = (const uint64_t *)up_at(o_pdoc);
+        const uint32_t *d_lbold = (const uint32_t *)up_at(o_lbold), *d_newbelow = (const uint32_t *)up_at(o_newbelow);
+        if (n_old)
+            sc_old_rows_kernel<<<blocks(n_old, SC_THREADS), SC_THREADS, 0, st>>>(n_old, alive, a_pre, a_blk, B.row_doc, d_pdoc,
+                                                                               n_pdoc, d_newbelow, remap, ns->row_doc);
+        if (n_pdoc)
+            sc_pending_rows_kernel<<<blocks(n_pdoc, SC_THREADS), SC_THREADS, 0, st>>>(n_pdoc, d_pdoc, d_lbold, d_newbelow, alive, a_pre,
+                                                                                    a_blk, remap, prow, ns->row_doc);
+        // 2-4. per field: survivors, sorted pending postings, new term offsets
+        uint32_t *repl_bits = (uint32_t *)at(w_repl);
+        for (size_t fi = 0; fi < nf; fi++) {
+            const FieldPlan &P = plan[fi];
+            const StrField &of = B.fields[fi];
+            StrField &f = ns->fields[fi];
+            f.n_terms = P.n_terms;
+            f.term_offsets.assign(size_t(P.n_terms) + 1, 0);
+            CU(cudaMemsetAsync(repl_bits, 0, n_rw * 4, st));
+            if (P.n_repl)
+                sc_replaced_kernel<<<blocks(P.n_repl, SC_THREADS), SC_THREADS, 0, st>>>(P.n_repl, (const uint32_t *)up_at(P.o_repl),
+                                                                                      prow, repl_bits);
+            uint32_t *keep = (uint32_t *)at(P.o_keep), *kpre = (uint32_t *)at(P.o_kpre), *kblk = (uint32_t *)at(P.o_kblk);
+            if (P.n_kw) {
+                sc_survive_kernel<<<blocks(P.n_kw * 32, SC_THREADS), SC_THREADS, 0, st>>>(of.n_post, P.n_kw, of.raw, n_old, remap, repl_bits, keep);
+                compact_scan_words_kernel<<<(unsigned)P.n_kb, COMPACT_SCAN_WORDS, 0, st>>>(keep, P.n_kw, kpre, kblk);
+                compact_scan_blocks_kernel<uint32_t><<<1, COMPACT_SCAN_WORDS, 0, st>>>(kblk, (uint32_t)P.n_kb);
+            }
+            uint64_t *keys = (uint64_t *)at(P.o_keys);
+            uint32_t *vals = (uint32_t *)at(P.o_vals);
+            if (P.n_pend) {
+                sc_pending_keys_kernel<<<blocks(P.n_pend, SC_THREADS), SC_THREADS, 0, st>>>(
+                    P.n_pend, (const uint32_t *)up_at(P.o_term), (const uint32_t *)up_at(P.o_doc), prow, keys + P.n_pend, vals + P.n_pend);
+                size_t b = cub_bytes;
+                CU(cub::DeviceRadixSort::SortPairs(at(w_cub), b, keys + P.n_pend, keys, vals + P.n_pend, vals, P.n_pend, 0,
+                                                   (int)P.end_bit, st));
+                sc_duplicate_kernel<<<blocks(P.n_pend, SC_THREADS), SC_THREADS, 0, st>>>(P.n_pend, keys, &d_res[fi].dup);
+            }
+            if (P.n_terms) {
+                uint64_t *new_off = (uint64_t *)at(P.o_newoff), *tblk = (uint64_t *)at(P.o_tblk);
+                sc_term_counts_kernel<<<(unsigned)P.n_tb, COMPACT_SCAN_WORDS, 0, st>>>(
+                    P.n_terms, of.n_post ? P.n_terms_old : 0, (const uint64_t *)up_at(P.o_off), keep, kpre, kblk, keys, P.n_pend,
+                    (uint32_t *)at(P.o_slo), (uint32_t *)at(P.o_plo), new_off, tblk);
+                compact_scan_blocks_kernel<uint64_t><<<1, COMPACT_SCAN_WORDS, 0, st>>>(tblk, (uint32_t)P.n_tb);
+                sc_add_block_kernel<<<blocks(uint64_t(P.n_terms) + 1, SC_THREADS), SC_THREADS, 0, st>>>(P.n_terms + 1, tblk, new_off);
+                CU(cudaMemcpyAsync(f.term_offsets.data(), new_off, (size_t(P.n_terms) + 1) * 8, cudaMemcpyDeviceToHost, st));
             }
         }
-        f.term_offsets[max_term] = f.host_post.size();
-        const size_t n_recs = f.host_post.size();
-        f.avg_len = of.avg_len;
-        if (!global_avg) {
-            double sum = 0; uint64_t cnt = 0;
-            for (uint16_t l : len_of_row) if (l) { sum += l; cnt++; }
-            if (cnt) f.avg_len = (float)(sum / (double)cnt);   // info().avg_field_length
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(res.data(), d_res, nf * sizeof(FieldRes), cudaMemcpyDeviceToHost, st));
+        CU(cudaEventRecord(s->ev[1], st));
+        CU(cudaStreamSynchronize(st));
+        for (size_t fi = 0; fi < nf; fi++)
+            if (res[fi].dup) return fail(OC_ERR_INVALID, "field %zu: term %u listed twice in one insert of a document", fi, res[fi].dup_term);
+        // 5. the new posting arrays at their exact size, and the scatter-merge into them
+        for (size_t fi = 0; fi < nf; fi++) {
+            StrField &f = ns->fields[fi];
+            f.n_post = f.term_offsets.back();
+            if (!f.n_post) continue;
+            CU(cudaMalloc(&f.post, (f.n_post + 4) * sizeof(Posting)));
+            CU(cudaMalloc(&f.raw, (f.n_post + 4) * sizeof(PostingRaw)));
         }
-        f.n_post = n_recs;
+        CU(cudaEventRecord(s->ev[2], st));
+        unsigned long long *row_key = global_avg ? nullptr : (unsigned long long *)at(w_rowkey);
+        for (size_t fi = 0; fi < nf; fi++) {
+            const FieldPlan &P = plan[fi];
+            const StrField &of = B.fields[fi];
+            StrField &f = ns->fields[fi];
+            if (!f.n_post) continue;
+            if (row_key) CU(cudaMemsetAsync(row_key, 0, n_new * 8, st));
+            const uint32_t *keep = (const uint32_t *)at(P.o_keep), *kpre = (const uint32_t *)at(P.o_kpre), *kblk = (const uint32_t *)at(P.o_kblk);
+            const uint64_t *old_off = (const uint64_t *)up_at(P.o_off), *new_off = (const uint64_t *)at(P.o_newoff), *keys = (const uint64_t *)at(P.o_keys);
+            const uint32_t *slo = (const uint32_t *)at(P.o_slo), *plo = (const uint32_t *)at(P.o_plo);
+            if (of.n_post)
+                sc_scatter_old_kernel<<<blocks(of.n_post, SC_TILE), SC_THREADS, 0, st>>>(of.n_post, of.raw, remap, keep, kpre, kblk,
+                                                                                       P.n_terms_old, old_off, new_off, slo, plo, keys, f.raw, row_key);
+            if (P.n_pend)
+                sc_scatter_pending_kernel<<<blocks(P.n_pend, SC_THREADS), SC_THREADS, 0, st>>>(
+                    P.n_pend, keys, (const uint32_t *)at(P.o_vals), (const uint32_t *)up_at(P.o_doc), (const uint16_t *)up_at(P.o_tf),
+                    (const uint16_t *)up_at(P.o_len), d_lbold, of.raw, of.n_post ? P.n_terms_old : 0, old_off, keep, kpre, kblk, new_off, slo, plo, f.raw, row_key);
+            if (row_key)
+                sc_len_sum_kernel<<<(unsigned)std::min<uint64_t>(max_grid, blocks(n_new, SC_THREADS)), SC_THREADS, 0, st>>>(
+                    (uint32_t)n_new, row_key, &d_res[fi].len_sum);
+        }
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(res.data(), d_res, nf * sizeof(FieldRes), cudaMemcpyDeviceToHost, st));
+        if (ns->row_doc) {
+            ns->row_doc_host.resize(n_new);
+            CU(cudaMemcpyAsync(ns->row_doc_host.data(), ns->row_doc, n_new * 8, cudaMemcpyDeviceToHost, st));
+        }
+        CU(cudaEventRecord(s->ev[3], st));
+        CU(cudaStreamSynchronize(st));
+        return OC_OK;
+    };
+    const int mrc = merge();
+    if (mrc != OC_OK) return abort_commit(mrc);
+    uint64_t post_after = 0;
+    for (size_t fi = 0; fi < nf; fi++) {
+        StrField &f = ns->fields[fi];
+        f.avg_len = B.fields[fi].avg_len;
+        if (!global_avg && res[fi].len_cnt) f.avg_len = (float)((double)res[fi].len_sum / (double)res[fi].len_cnt);   // info().avg_field_length
+        post_after += f.n_post;
         // per-term corpus df of a shard cannot be refreshed locally: sharded searches on this snapshot count
         // df across ranks (OC_SHARD_COUNT_DF) until the caller loads new global tables
     }
-    const bool identity = !docs.empty() && docs.front() == 0 && docs.back() == docs.size() - 1;
-    ns->n_rows = docs.size();
-    ns->document_count = global_count ? B.document_count : docs.size();
-    // ---- upload on the store's own stream (searches keep the ctx stream)
-    auto upload = [&]() -> int {
-        if (!identity && !docs.empty()) {
-            ns->row_doc_host = docs;
-            CU(cudaMalloc(&ns->row_doc, docs.size() * 8));
-            CU(cudaMemcpyAsync(ns->row_doc, docs.data(), docs.size() * 8, cudaMemcpyHostToDevice, s->load_stream));
-        }
-        for (auto &f : ns->fields) {
-            const uint64_t np = f.host_post.size();
-            if (!np) continue;
-            CU(cudaMalloc(&f.post, (np + 4) * sizeof(Posting)));
-            CU(cudaMalloc(&f.raw, (np + 4) * sizeof(PostingRaw)));
-            CU(cudaMemcpyAsync(f.raw, f.host_post.data(), np * sizeof(PostingRaw), cudaMemcpyHostToDevice, s->load_stream));
-        }
-        CU(cudaStreamSynchronize(s->load_stream));
-        return OC_OK;
-    };
-    const int urc = upload();
-    if (urc != OC_OK) return abort_commit(urc);
+    if (out) {
+        float a = 0, b = 0;
+        cudaEventElapsedTime(&a, s->ev[0], s->ev[1]);
+        cudaEventElapsedTime(&b, s->ev[2], s->ev[3]);
+        *out = oc_str_commit_t{};
+        out->rows_before = n_old; out->rows_after = n_new;
+        out->postings_before = post_before; out->postings_after = post_after;
+        out->pending_postings = pend_total;
+        out->workspace_bytes = ws;
+        out->device_ms = a + b;
+    }
     // ---- publish: replay the deletes that arrived while we were building, then swap the pointer
     {
         std::lock_guard<std::mutex> g(s->mu);
@@ -1503,6 +1672,57 @@ extern "C" int oc_str_commit(oc_str *s) {
         s->cur = ns;
         s->deletes_during_commit.clear();
         s->committing = false;
+    }
+    if (out) out->wall_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - wall0).count();
+    return OC_OK;
+}
+
+// Read-back of the published snapshot (the inverse of oc_str_set_rows + oc_str_load_field).
+extern "C" int oc_str_read_rows(oc_str *s, uint64_t *n_rows, uint64_t *row_doc_ids, uint64_t *document_count, uint64_t *version) {
+    if (!s || !n_rows) return fail(OC_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> g(s->mu);
+    const StrSnap &S = *s->cur;
+    const uint64_t cap = *n_rows;
+    *n_rows = S.n_rows;
+    if (document_count) *document_count = S.document_count;
+    if (version) *version = S.version;
+    if (!row_doc_ids) return OC_OK;
+    if (cap < S.n_rows) return fail(OC_ERR_INVALID, "row_doc_ids holds %llu rows, the snapshot has %llu",
+                                    (unsigned long long)cap, (unsigned long long)S.n_rows);
+    if (S.row_doc_host.empty()) for (uint64_t r = 0; r < S.n_rows; r++) row_doc_ids[r] = r;
+    else std::copy(S.row_doc_host.begin(), S.row_doc_host.end(), row_doc_ids);
+    return OC_OK;
+}
+
+extern "C" int oc_str_read_field(oc_str *s, uint32_t field, float *avg_field_len, uint32_t *n_terms, uint64_t *n_postings,
+                                 uint64_t *term_offsets, uint32_t *post_row, uint16_t *post_tf, uint16_t *post_len) {
+    if (!s || !n_terms || !n_postings) return fail(OC_ERR_INVALID, "NULL argument");
+    oc_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> g(c->mu);   // oc_str_load_field replaces a published field's arrays under this lock
+    CU(cudaSetDevice(c->device));
+    std::shared_ptr<StrSnap> snap = str_snapshot(s);
+    if (field >= snap->fields.size()) return fail(OC_ERR_INVALID, "field %u out of range", field);
+    const StrField &f = snap->fields[field];
+    const uint32_t cap_t = *n_terms;
+    const uint64_t cap_p = *n_postings;
+    *n_terms = f.n_terms; *n_postings = f.n_post;
+    if (avg_field_len) *avg_field_len = f.avg_len;
+    if ((term_offsets && cap_t < f.n_terms) || ((post_row || post_tf || post_len) && cap_p < f.n_post))
+        return fail(OC_ERR_INVALID, "arrays too small for field %u (%u terms, %llu postings)", field, f.n_terms,
+                    (unsigned long long)f.n_post);
+    if (term_offsets) {
+        if (f.term_offsets.empty()) term_offsets[0] = 0;
+        else std::copy(f.term_offsets.begin(), f.term_offsets.end(), term_offsets);
+    }
+    if ((post_row || post_tf || post_len) && f.n_post) {
+        std::vector<PostingRaw> h(f.n_post);
+        CU(cudaMemcpyAsync(h.data(), f.raw, f.n_post * sizeof(PostingRaw), cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        for (uint64_t i = 0; i < f.n_post; i++) {
+            if (post_row) post_row[i] = h[i].row;
+            if (post_tf) post_tf[i] = h[i].tf;
+            if (post_len) post_len[i] = h[i].len;
+        }
     }
     return OC_OK;
 }

@@ -25,38 +25,42 @@ namespace oc {
 constexpr uint32_t COMPACT_SCAN_WORDS = 1024;   // words (of 32 rows) per scan block == its threads
 constexpr uint32_t COMPACT_THREADS = 256;
 
-// dead rows below row r; word_pre: per word, within its scan block; block_pre: per scan block
-__device__ __forceinline__ uint32_t compact_dead_below(const uint32_t *dead_bits, const uint32_t *word_pre,
+// set bits below bit r of a bitmap scanned by compact_scan_words_kernel + compact_scan_blocks_kernel (here: dead rows
+// below row r; str_commit.cuh counts alive rows and surviving postings with it); word_pre: per word, within its scan
+// block; block_pre: per scan block.  The sum wraps modulo 2^32, so a difference of two counts is exact whenever the
+// bits between them number fewer than 2^32, however long the bitmap.
+__device__ __forceinline__ uint32_t compact_bits_below(const uint32_t *bits, const uint32_t *word_pre,
                                                        const uint32_t *block_pre, uint64_t r) {
     const uint64_t w = r >> 5;
     return __ldg(block_pre + w / COMPACT_SCAN_WORDS) + __ldg(word_pre + w) +
-           __popc(__ldg(dead_bits + w) & ((1u << (r & 31)) - 1u));
+           __popc(__ldg(bits + w) & ((1u << (r & 31)) - 1u));
 }
 
 // exclusive scan of one value per thread over a block of COMPACT_SCAN_WORDS threads; *total = the block's sum
-__device__ __forceinline__ uint32_t compact_block_exscan(uint32_t v, uint32_t *warp_sums, uint32_t *total) {
+template <typename T>
+__device__ __forceinline__ T compact_block_exscan(T v, T *warp_sums, T *total) {
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t inc = v;
+    T inc = v;
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) {
-        const uint32_t o = __shfl_up_sync(0xffffffffu, inc, d);
+        const T o = __shfl_up_sync(0xffffffffu, inc, d);
         if (lane >= d) inc += o;
     }
     if (lane == 31) warp_sums[warp] = inc;
     __syncthreads();
     if (warp == 0) {
-        const uint32_t s = warp_sums[lane];
-        uint32_t si = s;
+        const T s = warp_sums[lane];
+        T si = s;
 #pragma unroll
         for (int d = 1; d < 32; d <<= 1) {
-            const uint32_t o = __shfl_up_sync(0xffffffffu, si, d);
+            const T o = __shfl_up_sync(0xffffffffu, si, d);
             if (lane >= d) si += o;
         }
         warp_sums[lane] = si - s;
         if (lane == 31) *total = si;
     }
     __syncthreads();
-    const uint32_t r = warp_sums[warp] + inc - v;
+    const T r = warp_sums[warp] + inc - v;
     __syncthreads();   // warp_sums is reused by the caller's next round
     return r;
 }
@@ -67,20 +71,22 @@ compact_scan_words_kernel(const uint32_t *dead_bits, uint64_t n_words, uint32_t 
     __shared__ uint32_t warp_sums[32];
     __shared__ uint32_t total;
     const uint64_t w = uint64_t(blockIdx.x) * COMPACT_SCAN_WORDS + threadIdx.x;
-    const uint32_t ex = compact_block_exscan(w < n_words ? __popc(dead_bits[w]) : 0u, warp_sums, &total);
+    const uint32_t ex = compact_block_exscan<uint32_t>(w < n_words ? __popc(dead_bits[w]) : 0u, warp_sums, &total);
     if (w < n_words) word_pre[w] = ex;
     if (threadIdx.x == 0) block_tot[blockIdx.x] = total;
 }
 
-// in place: block_tot -> dead rows below each scan block (one CTA; n_rows < 2^32 leaves at most 2^17 blocks)
+// in place: block_tot -> exclusive prefix sums, i.e. dead rows below each scan block (one CTA; n_rows < 2^32 leaves at
+// most 2^17 blocks).  T = uint64_t: str_commit.cuh's per-term posting counts.
+template <typename T>
 __global__ void __launch_bounds__(COMPACT_SCAN_WORDS)
-compact_scan_blocks_kernel(uint32_t *block_tot, uint32_t n_blocks) {
-    __shared__ uint32_t warp_sums[32];
-    __shared__ uint32_t total;
-    uint32_t carry = 0;
+compact_scan_blocks_kernel(T *block_tot, uint32_t n_blocks) {
+    __shared__ T warp_sums[32];
+    __shared__ T total;
+    T carry = 0;
     for (uint32_t base = 0; base < n_blocks; base += COMPACT_SCAN_WORDS) {
         const uint32_t i = base + threadIdx.x;
-        const uint32_t ex = compact_block_exscan(i < n_blocks ? block_tot[i] : 0u, warp_sums, &total);
+        const T ex = compact_block_exscan<T>(i < n_blocks ? block_tot[i] : T(0), warp_sums, &total);
         if (i < n_blocks) block_tot[i] = carry + ex;
         carry += total;
         __syncthreads();   // every thread has read `total` before the next round overwrites it
@@ -98,7 +104,7 @@ compact_gather_kernel(const void *rows, uint32_t stride, uint64_t row_begin, uin
     const uint64_t warps = uint64_t(gridDim.x) * (COMPACT_THREADS / 32);
     for (uint64_t r = row_begin + uint64_t(blockIdx.x) * (COMPACT_THREADS / 32) + (threadIdx.x >> 5); r < row_end; r += warps) {
         if ((__ldg(dead_bits + (r >> 5)) >> (r & 31)) & 1u) continue;   // warp-uniform: a dead row is not read
-        const uint64_t d = r - compact_dead_below(dead_bits, word_pre, block_pre, r) - dst_begin;
+        const uint64_t d = r - compact_bits_below(dead_bits, word_pre, block_pre, r) - dst_begin;
         const uint4 *src = static_cast<const uint4 *>(rows) + r * row_vec;
         uint4 *dst = stage + d * row_vec;
         // the source is read once (streaming, evict-first); the staging buffer is read back by the next kernel
@@ -131,7 +137,7 @@ compact_small_gather_kernel(const float *inv_norm, const uint64_t *row_doc, cons
                             const uint32_t *block_pre, uint64_t *st_doc, float *st_inv, float *st_scale) {
     const uint64_t r = row_begin + uint64_t(blockIdx.x) * COMPACT_THREADS + threadIdx.x;
     if (r >= row_end || ((__ldg(dead_bits + (r >> 5)) >> (r & 31)) & 1u)) return;
-    const uint64_t d = r - compact_dead_below(dead_bits, word_pre, block_pre, r) - dst_begin;
+    const uint64_t d = r - compact_bits_below(dead_bits, word_pre, block_pre, r) - dst_begin;
     st_doc[d] = row_doc[r];
     st_inv[d] = inv_norm[r];
     if (row_scale) st_scale[d] = row_scale[r];

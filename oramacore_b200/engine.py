@@ -248,9 +248,31 @@ class StringFieldStorage:
         f = np.asarray([min(v, 65535) for v in terms.values()], np.uint16)
         check(lib().oc_str_insert(self._h, field, int(doc_id), min(int(field_length), 65535), t.shape[0], _p(t), _p(f)))
 
-    def commit(self):
-        """compact(version) (string_field.rs:186-191)."""
-        check(lib().oc_str_commit(self._h))
+    def commit(self) -> dict:
+        """compact(version) (string_field.rs:186-191), merged on the device.  Returns the call's statistics
+        (oc_str_commit_t)."""
+        st = _lib.StrCommit()
+        check(lib().oc_str_commit_ex(self._h, C.byref(st)))
+        return st.as_dict()
+
+    def read_rows(self) -> dict:
+        """The published snapshot's rows: {"row_doc_ids": uint64[n_rows], "document_count", "version"}."""
+        n, dc, ver = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        check(lib().oc_str_read_rows(self._h, C.byref(n), None, None, None))
+        rd = np.zeros(n.value, np.uint64)
+        check(lib().oc_str_read_rows(self._h, C.byref(n), _p(rd), C.byref(dc), C.byref(ver)))
+        return {"row_doc_ids": rd[:n.value], "document_count": dc.value, "version": ver.value}
+
+    def read_field(self, field: int) -> dict:
+        """One field of the published snapshot as oc_str_load_field takes it: {"avg_field_len", "n_terms",
+        "term_offsets": uint64[n_terms + 1], "post_row": uint32[], "post_tf": uint16[], "post_len": uint16[]}."""
+        nt, npost, avg = C.c_uint32(0), C.c_uint64(0), C.c_float(0)
+        check(lib().oc_str_read_field(self._h, field, None, C.byref(nt), C.byref(npost), None, None, None, None))
+        off = np.zeros(nt.value + 1, np.uint64)
+        row, tf, ln = np.zeros(npost.value, np.uint32), np.zeros(npost.value, np.uint16), np.zeros(npost.value, np.uint16)
+        check(lib().oc_str_read_field(self._h, field, C.byref(avg), C.byref(nt), C.byref(npost), _p(off), _p(row), _p(tf), _p(ln)))
+        return {"avg_field_len": np.float32(avg.value), "n_terms": nt.value, "term_offsets": off[:nt.value + 1],
+                "post_row": row[:npost.value], "post_tf": tf[:npost.value], "post_len": ln[:npost.value]}
 
     def delete(self, doc_id):
         """One DocumentId or a sequence of them."""

@@ -39,6 +39,19 @@ pub struct OcEmbCompact {
     pub workspace_bytes: u64,
     pub device_ms: f32,
 }
+/// Statistics of one `oc_str_commit_ex` call (`oc_str_commit_t`).
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct OcStrCommit {
+    pub rows_before: u64,
+    pub rows_after: u64,
+    pub postings_before: u64,
+    pub postings_after: u64,
+    pub pending_postings: u64,
+    pub workspace_bytes: u64,
+    pub device_ms: f32,
+    pub wall_ms: f32,
+}
 /// `OcSearchParams::sharded`: merge across `oc_comm` ranks; add `OC_SHARD_TOMBSTONES` on every rank while
 /// any rank's string store holds uncommitted deletes (the df all-reduce must be entered by all ranks).
 pub const OC_SHARDED: c_int = 1;
@@ -214,6 +227,14 @@ extern "C" {
                          term_ids: *const u32, tfs: *const u16) -> c_int;
     /// compaction (string_field.rs:186-191): merges pending inserts / deletes into the device layout
     pub fn oc_str_commit(s: *mut OcStr) -> c_int;
+    /// `oc_str_commit` that also reports its statistics (`out` may be null)
+    pub fn oc_str_commit_ex(s: *mut OcStr, out: *mut OcStrCommit) -> c_int;
+    /// read-back of the published snapshot (compact(), string_field.rs:186-191): null arrays return the sizes;
+    /// otherwise `*n_rows` / `*n_terms` / `*n_postings` give the arrays' capacity on entry
+    pub fn oc_str_read_rows(s: *mut OcStr, n_rows: *mut u64, row_doc_ids: *mut u64, document_count: *mut u64,
+                            version: *mut u64) -> c_int;
+    pub fn oc_str_read_field(s: *mut OcStr, field: u32, avg_field_len: *mut f32, n_terms: *mut u32, n_postings: *mut u64,
+                             term_offsets: *mut u64, post_row: *mut u32, post_tf: *mut u16, post_len: *mut u16) -> c_int;
     /// page-locked host buffers: query vectors placed here are DMA'd without staging
     pub fn oc_pinned_alloc(bytes: usize, out: *mut *mut c_void) -> c_int;
     /// micro-batching front: one query per call from many threads, coalesced into batched `oc_search`
