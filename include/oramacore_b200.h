@@ -331,6 +331,9 @@ int oc_filter_and(const oc_filter *a, const oc_filter *b, oc_filter **out);   /*
 int oc_filter_or(const oc_filter *a, const oc_filter *b, oc_filter **out);    /* FilterResult::Or  */
 int oc_filter_not(const oc_filter *a, oc_filter **out);                       /* FilterResult::Not (within [0, nbits)) */
 int oc_filter_count(const oc_filter *f, uint64_t *out);                       /* documents that pass */
+/* The DocumentId space [0, nbits) of a handle: a leaf of a facet store or geopoint field takes the nbits of the version
+ * it was built on, which a concurrent commit may grow. */
+int oc_filter_nbits(const oc_filter *f, uint64_t *out);
 int oc_filter_read(const oc_filter *f, uint64_t *out_bits /* (nbits+63)/64 words */);
 void oc_filter_destroy(oc_filter *f);
 
@@ -357,12 +360,32 @@ void oc_filter_destroy(oc_filter *f);
  * negative, fewer than 3 or more than OC_GEO_MAX_VERTICES vertices (the kernel stages them in shared memory). */
 #define OC_GEO_EARTH_RADIUS_M 6371000.0
 #define OC_GEO_MAX_VERTICES 2048u
+/* Statistics of one oc_facets_commit_ex / oc_geo_field_commit_ex call. */
+typedef struct {
+    uint64_t version;                          /* version this call published (1 = the first commit)       */
+    uint64_t rows_kept, rows_dropped, rows_added;   /* entries of all fields: committed kept / removed, inserted */
+    uint64_t workspace_bytes;                  /* largest device workspace of one field                      */
+    float device_ms;                           /* CUDA-event time of the merge kernels, scans and their copies */
+    float wall_ms;                             /* the whole call, publishing included                        */
+} oc_filter_commit_t;
 typedef struct oc_geo_field oc_geo_field;
 /* n entries (doc_ids[i], lat[i], lon[i]); n = 0 gives empty leaves.  Sorted by document id and kept on the device as
- * 48 B per point (unit vector, lat / lon, id).  The handle is immutable: a changed field means a new handle. */
+ * 48 B per point (unit vector, lat / lon, id).  A changed field is committed with oc_geo_field_commit_ex
+ * below. */
 int oc_geo_field_create(oc_ctx *ctx, uint64_t nbits, uint64_t n, const uint64_t *doc_ids, const double *lat,
                         const double *lon, oc_geo_field **out);
 void oc_geo_field_destroy(oc_geo_field *g);
+/* compact() of a geopoint field: oc_geo_field_insert queues points (checked as oc_geo_field_create checks them, before
+ * anything is queued), oc_geo_field_delete removes every point of the documents, in call order as for oc_facets_*, and
+ * oc_geo_field_commit_ex merges them into the next version on the device with the contract, cost and refusals of
+ * oc_facets_commit_ex (48 B per point; workspace 24 B per committed point, about 64 B per queued one).  A document's
+ * points keep their order: committed first, then queued ones in call order.  The unit vectors of the queued points are
+ * computed on the host as oc_geo_field_create computes them, so both give the same bits.  oc_geo_field_read reads the
+ * published points back in their order (NULL arrays: the size; otherwise *n is the capacity on entry). */
+int oc_geo_field_insert(oc_geo_field *g, uint64_t n, const uint64_t *doc_ids, const double *lat, const double *lon);
+int oc_geo_field_delete(oc_geo_field *g, uint64_t n, const uint64_t *doc_ids);
+int oc_geo_field_commit_ex(oc_geo_field *g, uint64_t new_nbits, oc_filter_commit_t *out);
+int oc_geo_field_read(oc_geo_field *g, uint64_t *n, uint64_t *doc_ids, double *lat, double *lon);
 /* GeoFilterOp::Radius / OutsideRadius: inside != 0 => points with d <= radius_m, else points with d > radius_m. */
 int oc_filter_geo_radius(const oc_geo_field *g, double lat, double lon, double radius_m, int inside, oc_filter **out);
 /* GeoFilterOp::Polygon / OutsidePolygon over the vertices (lat[k], lon[k]), k < n_vertices. */
@@ -390,7 +413,52 @@ int oc_facets_create(oc_ctx *ctx, uint64_t nbits, oc_facets **out);
 void oc_facets_destroy(oc_facets *f);
 int oc_facets_add_field(oc_facets *f, uint32_t n_variants, const uint64_t *variant_offsets /* n+1 */, const uint64_t *doc_ids,
                         uint32_t *out_field);
+/* The store keeps each variant's documents ascending, and a number field's entries ascending by value (-0.0 before
+ * +0.0) then by document: input in another order inside a variant or a run of equal values is sorted on the host. */
 int oc_facets_add_number_field(oc_facets *f, uint64_t n, const double *values_sorted, const uint64_t *doc_ids, uint32_t *out_field);
+
+/* ---- filter-field commit -------------------------------------------------------------------------
+ * compact() of the bool, string_filter, number and date fields (read/index/mod.rs:537-580) without a host rebuild:
+ * pending ops queue on the host, in call order, and oc_facets_commit_ex merges them into the next version of every
+ * field's device arrays.  Ops are not visible to searches before the commit.
+ *   - oc_facets_insert_variants: (doc_ids[i], variants[i]) entries of a bool or string_filter field.  OC_FACET_UNIQUE
+ *     gives set semantics: the entry is skipped when the field already holds it (committed and not removed, or queued
+ *     earlier), as for a bool field.  Without it a document may hold a variant several times (array values).
+ *   - oc_facets_add_variant: a new string_filter key; it gets the next variant index.  Variant indices never move, so
+ *     oc_facet_req.variant and where-program nodes stay meaningful across commits.  The variant is empty until a
+ *     commit publishes entries for it.
+ *   - oc_facets_insert_numbers: (doc_ids[i], values[i]) entries of a number or date field; NaN is refused.
+ *   - oc_facets_clear: removes every value of the documents in one field (a replaced value, FilterBool).
+ *   - oc_facets_delete: removes every value of the documents in every field.
+ * A removal applies to the committed entries and to the queued inserts before it, not to later inserts: a delete
+ * followed by an insert of the same document keeps the insert.
+ * oc_facets_commit_ex builds the next version from the previous version's DEVICE arrays on the handle's own stream,
+ * outside the ctx lock: searches, leaves, where programs and oc_group_by_create keep running on the previous version
+ * meanwhile, and the next one is published under the ctx lock once the ctx stream has drained.  new_nbits >= nbits
+ * may grow the DocumentId space; every queued document must be below it.  Order inside a field after a commit:
+ * variant-major with ascending documents (CSR), or ascending value, -0.0 before +0.0, then ascending document (number
+ * and date fields).  A store built by oc_facets_add_* may order equal values differently; every consumer reads a
+ * slice as a set.  The host copy of a number field's values is replaced by a copy of the merge result.
+ * Cost: host O(pending log pending), plus a device-to-host copy of each changed number field's values; device one
+ * pass over each changed field (a field with no queued insert and no removal is left as it is).  Workspace per
+ * changed field, freed before the call returns: 24 B per committed entry, about 40 B per queued insert, 8 B per
+ * removed document and the CUB scan storage.  Limit: fewer than 2^31 - 1 committed + queued entries per field.
+ * OC_ERR_INVALID, changing nothing and keeping every op queued: new_nbits < nbits, a queued document >= new_nbits, a
+ * commit of the handle already in flight; OC_ERR_OOM: no room for the workspace or the next version.  One commit at a
+ * time per handle; oc_facets_add_* is refused while one is in flight. */
+#define OC_FACET_UNIQUE 1u
+int oc_facets_insert_variants(oc_facets *f, uint32_t field, uint64_t n, const uint64_t *doc_ids, const uint32_t *variants, uint32_t flags);
+int oc_facets_add_variant(oc_facets *f, uint32_t field, uint32_t *variant_out);
+int oc_facets_insert_numbers(oc_facets *f, uint32_t field, uint64_t n, const uint64_t *doc_ids, const double *values);
+int oc_facets_clear(oc_facets *f, uint32_t field, uint64_t n, const uint64_t *doc_ids);
+int oc_facets_delete(oc_facets *f, uint64_t n, const uint64_t *doc_ids);
+int oc_facets_commit_ex(oc_facets *f, uint64_t new_nbits, oc_filter_commit_t *out);
+/* Read-back of one field of the published version, as oc_facets_add_field / oc_facets_add_number_field take it.  With
+ * every array NULL it returns the sizes (*n_variants = 0 for a number field).  Otherwise it fills the arrays given, and
+ * *n_entries (doc_ids, values) and *n_variants (offsets) are their capacities on entry; offsets takes n_variants + 1
+ * entries (the host copy: no device read), values (number fields) n_entries. */
+int oc_facets_read_field(oc_facets *f, uint32_t field, uint32_t *n_variants, uint64_t *n_entries, uint64_t *offsets, double *values,
+                         uint64_t *doc_ids);
 
 /* where-filter leaves over a filter field of a facet store (read/index/filter.rs:49-124); the leaf's nbits is the store's.
  * An ordinary oc_filter over the facets' ctx, for oc_filter_and / or / not and any search.  A document is in a leaf

@@ -21,6 +21,7 @@ OC_GEO_EARTH_RADIUS_M = 6371000.0
 OC_GEO_MAX_VERTICES = 2048
 OC_RANGE_LO_OPEN = 1
 OC_RANGE_HI_OPEN = 2
+OC_FACET_UNIQUE = 1   # oc_facets_insert_variants: set semantics (a bool field)
 # Timing.scan_variant: which embedding sweep served the last batch (include/oramacore_b200.h OC_SCAN_*)
 OC_SCAN_EXACT = 0
 OC_SCAN_TC_TF32 = 1
@@ -42,9 +43,12 @@ EXPORTED_SYMBOLS = [
     "oc_batcher_create", "oc_batcher_create2", "oc_batcher_destroy", "oc_batcher_search", "oc_batcher_search_sorted", "oc_batcher_search_groups",
     "oc_batcher_search_faceted", "oc_batcher_stats",
     "oc_filter_from_ids", "oc_filter_from_bits", "oc_filter_and", "oc_filter_or", "oc_filter_not", "oc_filter_count",
-    "oc_filter_read", "oc_filter_destroy", "oc_merge_results",
+    "oc_filter_read", "oc_filter_nbits", "oc_filter_destroy", "oc_merge_results",
     "oc_geo_field_create", "oc_geo_field_destroy", "oc_filter_geo_radius", "oc_filter_geo_polygon",
+    "oc_geo_field_insert", "oc_geo_field_delete", "oc_geo_field_commit_ex", "oc_geo_field_read",
     "oc_facets_create", "oc_facets_destroy", "oc_facets_add_field", "oc_facets_add_number_field", "oc_search_facets",
+    "oc_facets_insert_variants", "oc_facets_add_variant", "oc_facets_insert_numbers", "oc_facets_clear", "oc_facets_delete",
+    "oc_facets_commit_ex", "oc_facets_read_field",
     "oc_filter_facet_variant", "oc_filter_facet_range", "oc_where_check", "oc_filter_from_where",
     "oc_group_by_create", "oc_group_by_destroy", "oc_search_groups",
     "oc_search_pinned", "oc_search_groups_pinned", "oc_merge_pinned",
@@ -79,6 +83,14 @@ class StrCommit(C.Structure):   # oc_str_commit_t
     _fields_ = [("rows_before", C.c_uint64), ("rows_after", C.c_uint64), ("postings_before", C.c_uint64),
                 ("postings_after", C.c_uint64), ("pending_postings", C.c_uint64), ("workspace_bytes", C.c_uint64),
                 ("device_ms", C.c_float), ("wall_ms", C.c_float)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+class FilterCommit(C.Structure):   # oc_filter_commit_t
+    _fields_ = [("version", C.c_uint64), ("rows_kept", C.c_uint64), ("rows_dropped", C.c_uint64), ("rows_added", C.c_uint64),
+                ("workspace_bytes", C.c_uint64), ("device_ms", C.c_float), ("wall_ms", C.c_float)]
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}
@@ -234,6 +246,7 @@ def lib():
     L.oc_filter_not.argtypes = [vp, C.POINTER(vp)]
     L.oc_filter_count.argtypes = [vp, C.POINTER(u64)]
     L.oc_filter_read.argtypes = [vp, vp]
+    L.oc_filter_nbits.argtypes = [vp, C.POINTER(u64)]
     L.oc_filter_destroy.argtypes = [vp]
     L.oc_filter_destroy.restype = None
     L.oc_geo_field_create.argtypes = [vp, u64, u64, vp, vp, vp, C.POINTER(vp)]
@@ -246,6 +259,17 @@ def lib():
     L.oc_facets_destroy.restype = None
     L.oc_facets_add_field.argtypes = [vp, u32, vp, vp, C.POINTER(u32)]
     L.oc_facets_add_number_field.argtypes = [vp, u64, vp, vp, C.POINTER(u32)]
+    L.oc_facets_insert_variants.argtypes = [vp, u32, u64, vp, vp, u32]
+    L.oc_facets_add_variant.argtypes = [vp, u32, C.POINTER(u32)]
+    L.oc_facets_insert_numbers.argtypes = [vp, u32, u64, vp, vp]
+    L.oc_facets_clear.argtypes = [vp, u32, u64, vp]
+    L.oc_facets_delete.argtypes = [vp, u64, vp]
+    L.oc_facets_commit_ex.argtypes = [vp, u64, C.POINTER(FilterCommit)]
+    L.oc_facets_read_field.argtypes = [vp, u32, C.POINTER(u32), C.POINTER(u64), vp, vp, vp]
+    L.oc_geo_field_insert.argtypes = [vp, u64, vp, vp, vp]
+    L.oc_geo_field_delete.argtypes = [vp, u64, vp]
+    L.oc_geo_field_commit_ex.argtypes = [vp, u64, C.POINTER(FilterCommit)]
+    L.oc_geo_field_read.argtypes = [vp, C.POINTER(u64), vp, vp, vp]
     L.oc_filter_facet_variant.argtypes = [vp, u32, u32, C.POINTER(vp)]
     L.oc_filter_facet_range.argtypes = [vp, u32, C.c_double, C.c_double, u32, C.POINTER(vp)]
     L.oc_where_check.argtypes = [C.POINTER(Where), u32]

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 #include <atomic>
@@ -19,6 +20,7 @@
 #include <utility>
 #include <string>
 #include <unordered_map>
+#include <unordered_set>
 #include <vector>
 
 #include "bm25.cuh"
@@ -29,6 +31,7 @@
 #include "stem_en.h"
 #include "emb_compact.cuh"
 #include "str_commit.cuh"
+#include "facet_commit.cuh"
 #include "emb_gemm.cuh"
 #include "emb_scan.cuh"
 #include "fuse.cuh"
@@ -1849,6 +1852,11 @@ extern "C" int oc_filter_count(const oc_filter *f, uint64_t *out) {
     CU(cudaMemcpyAsync(&v, c->work_ctr.p, 8, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     *out = v;
+    return OC_OK;
+}
+extern "C" int oc_filter_nbits(const oc_filter *f, uint64_t *out) {
+    if (!f || !out) return fail(OC_ERR_INVALID, "NULL argument");
+    *out = f->nbits;
     return OC_OK;
 }
 extern "C" int oc_filter_read(const oc_filter *f, uint64_t *out_bits) {
@@ -3755,13 +3763,34 @@ struct FacetField {
     bool number = false;
     uint64_t n_docs = 0;
     uint64_t *docs = nullptr;              // device: variant-major (CSR) or value-sorted (number field)
+    double *d_values = nullptr;            // device: the values of a number field (read by oc_facets_commit_ex)
     std::vector<uint64_t> offsets;         // host: n_variants + 1
     std::vector<double> values;            // host: ascending (number field)
+};
+// The pending ops of a filter-field handle (oc_facets, oc_geo_field), applied in call order by its next commit.
+// Guarded by `mu`; the fields of the handle itself are replaced only by a commit, under the ctx lock.
+struct FcIns { uint64_t doc, seq; double value, lat, lon; uint32_t field, variant; bool unique; };
+struct FcPending {
+    std::mutex mu;
+    bool committing = false;
+    uint64_t seq = 0, version = 0;
+    std::vector<FcIns> ins;
+    std::unordered_map<uint64_t, uint64_t> del;                  // doc -> seq of its last delete (every field)
+    std::map<std::pair<uint32_t, uint64_t>, uint64_t> clr;       // (field, doc) -> seq of its last clear
+    std::vector<uint8_t> number;                                 // per field, as the pending ops see it
+    std::vector<uint32_t> n_var;                                 //   (new string_filter keys count at once)
+    cudaStream_t stream = nullptr;
+    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};   // fc_merge's two device phases
+    ~FcPending() {
+        if (stream) { cudaStreamSynchronize(stream); cudaStreamDestroy(stream); }
+        for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+    }
 };
 struct oc_facets {
     oc_ctx *ctx;
     uint64_t nbits;                        // DocumentId space [0, nbits)
     std::vector<FacetField> fields;
+    FcPending pend;
 };
 
 extern "C" int oc_facets_create(oc_ctx *c, uint64_t nbits, oc_facets **out) {
@@ -3777,18 +3806,28 @@ extern "C" void oc_facets_destroy(oc_facets *f) {
         std::lock_guard<std::mutex> g(f->ctx->mu);
         cudaSetDevice(f->ctx->device);
         cudaStreamSynchronize(f->ctx->stream);
-        for (auto &fl : f->fields) cudaFree(fl.docs);
+        for (auto &fl : f->fields) { cudaFree(fl.docs); cudaFree(fl.d_values); }
     }
     delete f;
 }
 static int facets_add(oc_facets *f, FacetField &&fl, const uint64_t *doc_ids, uint32_t *out_field) {
     oc_ctx *c = f->ctx;
     std::lock_guard<std::mutex> g(c->mu);
+    std::lock_guard<std::mutex> gp(f->pend.mu);
+    if (f->pend.committing) return fail(OC_ERR_INVALID, "a field added while a commit of the store is in flight");
     CU(cudaSetDevice(c->device));
     if (fl.n_docs) {
-        CU(cudaMalloc(&fl.docs, fl.n_docs * 8));
-        CU(cudaMemcpy(fl.docs, doc_ids, fl.n_docs * 8, cudaMemcpyHostToDevice));
+        cudaError_t e = cudaMalloc(&fl.docs, fl.n_docs * 8);
+        if (e == cudaSuccess) e = cudaMemcpy(fl.docs, doc_ids, fl.n_docs * 8, cudaMemcpyHostToDevice);
+        if (e == cudaSuccess && fl.number) e = cudaMalloc(&fl.d_values, fl.n_docs * 8);
+        if (e == cudaSuccess && fl.number) e = cudaMemcpy(fl.d_values, fl.values.data(), fl.n_docs * 8, cudaMemcpyHostToDevice);
+        if (e != cudaSuccess) {
+            cudaFree(fl.docs); cudaFree(fl.d_values);
+            return fail(e == cudaErrorMemoryAllocation ? OC_ERR_OOM : OC_ERR_CUDA, "facet field upload: %s", cudaGetErrorString(e));
+        }
     }
+    f->pend.number.push_back(fl.number);
+    f->pend.n_var.push_back(fl.number ? 0u : uint32_t(fl.offsets.size() - 1));
     f->fields.push_back(std::move(fl));
     if (out_field) *out_field = (uint32_t)f->fields.size() - 1;
     return OC_OK;
@@ -3802,7 +3841,13 @@ extern "C" int oc_facets_add_field(oc_facets *f, uint32_t n_variants, const uint
     FacetField fl;
     fl.n_docs = variant_offsets[n_variants];
     fl.offsets.assign(variant_offsets, variant_offsets + n_variants + 1);
-    return facets_add(f, std::move(fl), doc_ids, out_field);
+    // each variant's documents ascending, the order oc_facets_commit_ex merges into (a slice is read as a set)
+    std::vector<uint64_t> sorted;
+    for (uint32_t v = 0; v < n_variants && sorted.empty(); v++)
+        if (!std::is_sorted(doc_ids + variant_offsets[v], doc_ids + variant_offsets[v + 1])) sorted.assign(doc_ids, doc_ids + fl.n_docs);
+    for (uint32_t v = 0; v < n_variants && !sorted.empty(); v++)
+        std::sort(sorted.begin() + variant_offsets[v], sorted.begin() + variant_offsets[v + 1]);
+    return facets_add(f, std::move(fl), sorted.empty() ? doc_ids : sorted.data(), out_field);
 }
 extern "C" int oc_facets_add_number_field(oc_facets *f, uint64_t n, const double *values_sorted, const uint64_t *doc_ids,
                                           uint32_t *out_field) {
@@ -3811,8 +3856,366 @@ extern "C" int oc_facets_add_number_field(oc_facets *f, uint64_t n, const double
         if (!(values_sorted[i] >= values_sorted[i - 1])) return fail(OC_ERR_INVALID, "values must be ascending (no NaN)");
     FacetField fl;
     fl.number = true; fl.n_docs = n;
-    fl.values.assign(values_sorted, values_sorted + n);
-    return facets_add(f, std::move(fl), doc_ids, out_field);
+    // ascending (value order, document): -0.0 before +0.0 and a run of equal values by document, the order
+    // oc_facets_commit_ex merges into (a range is read as a set)
+    auto key = [&](uint64_t i) { return std::make_pair(oc::fc_order(values_sorted[i]), doc_ids[i]); };
+    bool ordered = true;
+    for (uint64_t i = 1; i < n && ordered; i++) ordered = !(key(i) < key(i - 1));
+    std::vector<uint64_t> docs;
+    if (ordered) {
+        fl.values.assign(values_sorted, values_sorted + n);
+    } else {
+        std::vector<uint64_t> o(n);
+        for (uint64_t i = 0; i < n; i++) o[i] = i;
+        std::sort(o.begin(), o.end(), [&](uint64_t a, uint64_t b) { return key(a) < key(b); });
+        fl.values.resize(n); docs.resize(n);
+        for (uint64_t i = 0; i < n; i++) { fl.values[i] = values_sorted[o[i]]; docs[i] = doc_ids[o[i]]; }
+    }
+    return facets_add(f, std::move(fl), ordered ? doc_ids : docs.data(), out_field);
+}
+
+// ------------------------------------------------------------------------------------ filter-field commit (facet_commit.cuh)
+static void geo_unit(double lat, double lon, double u[3]);
+static bool geo_valid(double lat, double lon);
+
+// One field's merge: the committed entries (kind 0: CSR docs + offsets, 1: number values + docs, 2: geopoint blob) and
+// the surviving pending entries, sorted by (key, call order), into new device arrays of the exact size.  Runs on `st`.
+enum { FC_CSR = 0, FC_NUMBER = 1, FC_GEO = 2 };
+struct FcMergeIn {
+    int kind = FC_CSR;
+    uint64_t n_a = 0;
+    const uint64_t *a_docs = nullptr;          // CSR / number: the committed documents
+    const double *a_vals = nullptr;            // number: the committed values; geo: the committed blob
+    const std::vector<uint64_t> *old_off = nullptr;
+    uint32_t n_var = 0;                        // CSR: variants of the next version (>= old_off->size() - 1)
+    std::vector<uint64_t> kill;                // ascending documents whose committed entries go
+    std::vector<oc::FcKey> kb;                 // pending keys, sorted
+    std::vector<uint32_t> b_keep;              // 1, or 2 for a set-semantics insert
+    std::vector<double> b_cols;                // number: n_b values; geo: x, y, z, lat, lon columns of n_b each
+};
+struct FcMergeOut {
+    uint64_t n = 0, kept = 0, added = 0, ws = 0;
+    float device_ms = 0;                       // the two device phases (keys .. scans, scatter .. copies), by events
+    void *dev = nullptr;                       // CSR / number: docs; geo: the blob
+    double *d_values = nullptr;                // number
+    std::vector<uint64_t> offsets;             // CSR: n_var + 1
+    std::vector<double> values;                // number: the host copy
+};
+static int fc_merge(cudaStream_t st, cudaEvent_t *ev, const FcMergeIn &in, FcMergeOut &o) {
+    using oc::FcKey;
+    const uint64_t n_a = in.n_a, n_b = in.kb.size(), n_kill = in.kill.size();
+    if (n_a + n_b >= uint64_t(INT32_MAX)) return fail(OC_ERR_UNSUPPORTED, "filter-field commit: %llu entries >= 2^31 - 1",
+                                                      (unsigned long long)(n_a + n_b));   // cub::DeviceScan counts in int
+    const uint64_t n_oo = in.kind == FC_CSR ? in.old_off->size() : 0, n_no = in.kind == FC_CSR ? uint64_t(in.n_var) + 1 : 0;
+    size_t scan_a = 0, scan_b = 0;
+    if (cub::DeviceScan::ExclusiveSum(nullptr, scan_a, (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)(n_a + 1), st) != cudaSuccess ||
+        cub::DeviceScan::ExclusiveSum(nullptr, scan_b, (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)(n_b + 1), st) != cudaSuccess)
+        return fail(OC_ERR_CUDA, "filter-field commit: scan size");
+    // workspace: [uploaded: kb | kill | b_cols | old_off | b_keep] [ka | a_keep | a_rank | b_rank | new_off | scan]
+    auto al = [](size_t x) { return (x + 255) & ~size_t(255); };
+    const size_t o_kb = 0, o_kill = o_kb + al(n_b * 16), o_cols = o_kill + al(n_kill * 8), o_oo = o_cols + al(in.b_cols.size() * 8),
+                 o_bk = o_oo + al(n_oo * 8), up = o_bk + al((n_b + 1) * 4);
+    const size_t o_ka = up, o_ak = o_ka + al(n_a * 16), o_ar = o_ak + al((n_a + 1) * 4), o_br = o_ar + al((n_a + 1) * 4),
+                 o_no = o_br + al((n_b + 1) * 4), o_scan = o_no + al(n_no * 8), total = o_scan + al(std::max(scan_a, scan_b));
+    std::vector<uint8_t> h(up, 0);
+    if (n_b) memcpy(h.data() + o_kb, in.kb.data(), n_b * 16);
+    if (n_kill) memcpy(h.data() + o_kill, in.kill.data(), n_kill * 8);
+    if (!in.b_cols.empty()) memcpy(h.data() + o_cols, in.b_cols.data(), in.b_cols.size() * 8);
+    if (n_oo) memcpy(h.data() + o_oo, in.old_off->data(), n_oo * 8);
+    if (n_b) memcpy(h.data() + o_bk, in.b_keep.data(), n_b * 4);   // b_keep[n_b] = 0
+    uint8_t *w = nullptr;
+    if (cudaMallocAsync(&w, total, st) != cudaSuccess) return fail(OC_ERR_OOM, "filter-field commit: %zu B of workspace", total);
+    o.ws = total;
+    int rc = OC_OK;
+    auto done = [&](int r) { cudaFreeAsync(w, st); if (r != OC_OK) { cudaFree(o.dev); cudaFree(o.d_values); o.dev = nullptr; o.d_values = nullptr; } return r; };
+    const FcKey *kb = reinterpret_cast<const FcKey *>(w + o_kb);
+    const uint64_t *kill = reinterpret_cast<const uint64_t *>(w + o_kill);
+    const double *cols = reinterpret_cast<const double *>(w + o_cols);
+    const uint64_t *oo = reinterpret_cast<const uint64_t *>(w + o_oo);
+    uint32_t *bk = reinterpret_cast<uint32_t *>(w + o_bk), *ak = reinterpret_cast<uint32_t *>(w + o_ak);
+    uint32_t *ar = reinterpret_cast<uint32_t *>(w + o_ar), *br = reinterpret_cast<uint32_t *>(w + o_br);
+    FcKey *ka = reinterpret_cast<FcKey *>(w + o_ka);
+    uint64_t *no = reinterpret_cast<uint64_t *>(w + o_no);
+    const unsigned ga = (unsigned)((n_a + oc::FC_THREADS) / oc::FC_THREADS), gb = (unsigned)((n_b + oc::FC_THREADS - 1) / oc::FC_THREADS);
+    cudaError_t e = cudaMemcpyAsync(w, h.data(), up, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaEventRecord(ev[0], st);
+    if (e == cudaSuccess) {
+        if (in.kind == FC_CSR)
+            oc::fc_keys_csr_kernel<<<ga, oc::FC_THREADS, 0, st>>>(in.a_docs, n_a, oo, uint32_t(n_oo - 1), kill, n_kill, ka, ak);
+        else if (in.kind == FC_NUMBER)
+            oc::fc_keys_num_kernel<<<ga, oc::FC_THREADS, 0, st>>>(in.a_vals, in.a_docs, n_a, kill, n_kill, ka, ak);
+        else
+            oc::fc_keys_geo_kernel<<<ga, oc::FC_THREADS, 0, st>>>(reinterpret_cast<const uint64_t *>(in.a_vals + 5 * n_a), n_a, kill, n_kill, ka, ak);
+        if (std::find(in.b_keep.begin(), in.b_keep.end(), 2u) != in.b_keep.end())
+            oc::fc_unique_kernel<<<gb, oc::FC_THREADS, 0, st>>>(ka, ak, n_a, kb, n_b, bk);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(w + o_scan, scan_a, ak, ar, (int)(n_a + 1), st);
+    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(w + o_scan, scan_b, bk, br, (int)(n_b + 1), st);
+    uint32_t tot[2] = {0, 0};
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&tot[0], ar + n_a, 4, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaEventRecord(ev[1], st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&tot[1], br + n_b, 4, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e == cudaSuccess) e = cudaEventElapsedTime(&o.device_ms, ev[0], ev[1]);
+    if (e != cudaSuccess) return done(fail(OC_ERR_CUDA, "filter-field commit: %s", cudaGetErrorString(e)));
+    o.kept = tot[0]; o.added = tot[1]; o.n = o.kept + o.added;
+    const size_t row = in.kind == FC_GEO ? 48 : 8;
+    if (o.n && (e = cudaMalloc(&o.dev, o.n * row)) == cudaSuccess && in.kind == FC_NUMBER) e = cudaMalloc(&o.d_values, o.n * 8);
+    if (e != cudaSuccess) return done(fail(e == cudaErrorMemoryAllocation ? OC_ERR_OOM : OC_ERR_CUDA, "filter-field commit: %llu entries: %s",
+                                          (unsigned long long)o.n, cudaGetErrorString(e)));
+    if ((e = cudaEventRecord(ev[2], st)) != cudaSuccess) return done(fail(OC_ERR_CUDA, "filter-field commit: %s", cudaGetErrorString(e)));
+    auto scatter = [&](auto wr) {
+        if (n_a) oc::fc_scatter_a_kernel<<<(unsigned)((n_a + oc::FC_THREADS - 1) / oc::FC_THREADS), oc::FC_THREADS, 0, st>>>(ka, ak, ar, n_a, kb, br, n_b, wr);
+        if (n_b) oc::fc_scatter_b_kernel<<<gb, oc::FC_THREADS, 0, st>>>(ka, ar, n_a, kb, bk, br, n_b, wr);
+    };
+    if (o.n) {
+        if (in.kind == FC_CSR) scatter(oc::FcCsrW{in.a_docs, kb, static_cast<uint64_t *>(o.dev)});
+        else if (in.kind == FC_NUMBER) scatter(oc::FcNumW{in.a_vals, in.a_docs, cols, kb, o.d_values, static_cast<uint64_t *>(o.dev)});
+        else scatter(oc::FcGeoW{in.a_vals, n_a, cols, n_b, kb, static_cast<double *>(o.dev), o.n});
+    }
+    if (in.kind == FC_CSR) {
+        oc::fc_offsets_kernel<<<(unsigned)((n_no + oc::FC_THREADS - 1) / oc::FC_THREADS), oc::FC_THREADS, 0, st>>>(
+            oo, uint32_t(n_oo - 1), ar, kb, br, n_b, in.n_var, no);
+        o.offsets.resize(n_no);
+    }
+    e = cudaGetLastError();
+    if (e == cudaSuccess && in.kind == FC_CSR) e = cudaMemcpyAsync(o.offsets.data(), no, n_no * 8, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess && in.kind == FC_NUMBER && o.n) {   // the host copy range leaves binary-search, from the merge result
+        o.values.resize(o.n);
+        e = cudaMemcpyAsync(o.values.data(), o.d_values, o.n * 8, cudaMemcpyDeviceToHost, st);
+    }
+    if (e == cudaSuccess) e = cudaEventRecord(ev[3], st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    float ms2 = 0;
+    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms2, ev[2], ev[3]);
+    o.device_ms += ms2;
+    if (e != cudaSuccess) rc = fail(OC_ERR_CUDA, "filter-field commit: %s", cudaGetErrorString(e));
+    return done(rc);
+}
+
+// The pending ops of `P` for field `field`, filtered (an insert survives unless a later delete or clear names its
+// document; a set-semantics insert also unless an earlier survivor has its key) and keyed; `kill` = the documents whose
+// committed entries go.  O(pending log pending).
+static void fc_take(const FcPending &P, const std::vector<FcIns> &ins, const std::unordered_map<uint64_t, uint64_t> &del,
+                    const std::map<std::pair<uint32_t, uint64_t>, uint64_t> &clr, uint32_t field, int kind, FcMergeIn &in) {
+    auto killed_after = [&](uint64_t doc, uint64_t seq) {
+        auto d = del.find(doc);
+        if (d != del.end() && d->second > seq) return true;
+        auto c = clr.find(std::make_pair(field, doc));
+        return c != clr.end() && c->second > seq;
+    };
+    struct KH { size_t operator()(const std::pair<uint64_t, uint64_t> &k) const { return std::hash<uint64_t>()(k.first * 0x9E3779B97F4A7C15ull ^ k.second); } };
+    std::unordered_set<std::pair<uint64_t, uint64_t>, KH> seen;
+    std::vector<std::pair<oc::FcKey, size_t>> keyed;   // (key, index into ins): ins is in call order
+    for (size_t i = 0; i < ins.size(); i++) {
+        const FcIns &x = ins[i];
+        if (x.field != field || killed_after(x.doc, x.seq)) continue;
+        oc::FcKey k = kind == FC_CSR ? oc::FcKey{x.variant, x.doc} : kind == FC_NUMBER ? oc::FcKey{oc::fc_order(x.value), x.doc} : oc::FcKey{x.doc, 0};
+        if (!seen.insert(std::make_pair(k.hi, k.lo)).second && x.unique) continue;
+        keyed.emplace_back(k, i);
+    }
+    std::sort(keyed.begin(), keyed.end(), [](const std::pair<oc::FcKey, size_t> &a, const std::pair<oc::FcKey, size_t> &b) {
+        return oc::fc_less(a.first, b.first) || (oc::fc_equal(a.first, b.first) && a.second < b.second);
+    });
+    const size_t n_b = keyed.size();
+    in.kb.resize(n_b); in.b_keep.resize(n_b);
+    in.b_cols.assign(kind == FC_NUMBER ? n_b : kind == FC_GEO ? 5 * n_b : 0, 0.0);
+    for (size_t j = 0; j < n_b; j++) {
+        const FcIns &x = ins[keyed[j].second];
+        in.kb[j] = keyed[j].first;
+        in.b_keep[j] = x.unique ? 2u : 1u;
+        if (kind == FC_NUMBER) in.b_cols[j] = x.value;
+        if (kind == FC_GEO) {   // the unit vector as oc_geo_field_create computes it, so both give the same bits
+            double u[3];
+            geo_unit(x.lat, x.lon, u);
+            for (int c = 0; c < 3; c++) in.b_cols[c * n_b + j] = u[c];
+            in.b_cols[3 * n_b + j] = x.lat; in.b_cols[4 * n_b + j] = x.lon;
+        }
+    }
+    in.kill.clear();
+    for (const auto &kv : del) in.kill.push_back(kv.first);
+    for (auto it = clr.lower_bound(std::make_pair(field, uint64_t(0))); it != clr.end() && it->first.first == field; ++it)
+        in.kill.push_back(it->first.second);
+    std::sort(in.kill.begin(), in.kill.end());
+    in.kill.erase(std::unique(in.kill.begin(), in.kill.end()), in.kill.end());
+    (void)P;
+}
+
+// Starts a commit: refuses a second one and a pending document >= new_nbits, then copies the ops to merge.
+static int fc_begin(FcPending &P, uint64_t nbits, uint64_t new_nbits, int device, std::vector<FcIns> &ins,
+                    std::unordered_map<uint64_t, uint64_t> &del, std::map<std::pair<uint32_t, uint64_t>, uint64_t> &clr, uint64_t &cut) {
+    std::lock_guard<std::mutex> g(P.mu);
+    if (P.committing) return fail(OC_ERR_INVALID, "a commit of this handle is already in flight");
+    if (new_nbits < nbits) return fail(OC_ERR_INVALID, "new_nbits %llu < nbits %llu: the DocumentId space only grows",
+                                       (unsigned long long)new_nbits, (unsigned long long)nbits);
+    for (const FcIns &x : P.ins)
+        if (x.doc >= new_nbits) return fail(OC_ERR_INVALID, "pending document %llu >= new_nbits %llu", (unsigned long long)x.doc,
+                                            (unsigned long long)new_nbits);
+    if (cudaSetDevice(device) != cudaSuccess) return fail(OC_ERR_CUDA, "cudaSetDevice failed");
+    if (!P.stream) {
+        CU(cudaStreamCreateWithFlags(&P.stream, cudaStreamNonBlocking));
+        for (cudaEvent_t &e : P.ev) CU(cudaEventCreate(&e));
+    }
+    P.committing = true;
+    ins = P.ins; del = P.del; clr = P.clr; cut = P.seq;
+    return OC_OK;
+}
+// Ends a commit: on success the ops it merged leave the queue (ops that arrived meanwhile stay), and the version moves on.
+static uint64_t fc_end(FcPending &P, bool ok, size_t n_ins, uint64_t cut) {
+    std::lock_guard<std::mutex> g(P.mu);
+    P.committing = false;
+    if (!ok) return P.version;
+    P.ins.erase(P.ins.begin(), P.ins.begin() + n_ins);
+    for (auto it = P.del.begin(); it != P.del.end();) it = it->second <= cut ? P.del.erase(it) : std::next(it);
+    for (auto it = P.clr.begin(); it != P.clr.end();) it = it->second <= cut ? P.clr.erase(it) : std::next(it);
+    return ++P.version;
+}
+static int fc_queue_check(const FcPending &P, uint32_t field, bool number, uint64_t n, const uint64_t *doc_ids) {
+    if (n && !doc_ids) return fail(OC_ERR_INVALID, "NULL doc_ids");
+    if (field >= P.number.size()) return fail(OC_ERR_INVALID, "field %u: the store has %zu fields", field, P.number.size());
+    if (bool(P.number[field]) != number) return fail(OC_ERR_INVALID, "field %u is a %s field", field, P.number[field] ? "number" : "bool / string_filter");
+    return OC_OK;
+}
+
+extern "C" int oc_facets_add_variant(oc_facets *f, uint32_t field, uint32_t *variant_out) {
+    if (!f || !variant_out) return fail(OC_ERR_INVALID, "NULL argument");
+    FcPending &P = f->pend;
+    std::lock_guard<std::mutex> g(P.mu);
+    OCTRY(fc_queue_check(P, field, false, 0, nullptr));
+    if (P.n_var[field] == UINT32_MAX - 1) return fail(OC_ERR_UNSUPPORTED, "field %u: 2^32 - 2 variants", field);
+    *variant_out = P.n_var[field]++;
+    return OC_OK;
+}
+extern "C" int oc_facets_insert_variants(oc_facets *f, uint32_t field, uint64_t n, const uint64_t *doc_ids, const uint32_t *variants,
+                                         uint32_t flags) {
+    if (!f || (n && !variants)) return fail(OC_ERR_INVALID, "NULL argument");
+    if (flags & ~OC_FACET_UNIQUE) return fail(OC_ERR_INVALID, "unknown insert flags 0x%x", flags);
+    FcPending &P = f->pend;
+    std::lock_guard<std::mutex> g(P.mu);
+    OCTRY(fc_queue_check(P, field, false, n, doc_ids));
+    for (uint64_t i = 0; i < n; i++)
+        if (variants[i] >= P.n_var[field]) return fail(OC_ERR_INVALID, "entry %llu: variant %u: field %u has %u variants",
+                                                        (unsigned long long)i, variants[i], field, P.n_var[field]);
+    for (uint64_t i = 0; i < n; i++) P.ins.push_back(FcIns{doc_ids[i], ++P.seq, 0.0, 0.0, 0.0, field, variants[i], bool(flags & OC_FACET_UNIQUE)});
+    return OC_OK;
+}
+extern "C" int oc_facets_insert_numbers(oc_facets *f, uint32_t field, uint64_t n, const uint64_t *doc_ids, const double *values) {
+    if (!f || (n && !values)) return fail(OC_ERR_INVALID, "NULL argument");
+    FcPending &P = f->pend;
+    std::lock_guard<std::mutex> g(P.mu);
+    OCTRY(fc_queue_check(P, field, true, n, doc_ids));
+    for (uint64_t i = 0; i < n; i++)
+        if (std::isnan(values[i])) return fail(OC_ERR_INVALID, "entry %llu: NaN value", (unsigned long long)i);
+    for (uint64_t i = 0; i < n; i++) P.ins.push_back(FcIns{doc_ids[i], ++P.seq, values[i], 0.0, 0.0, field, 0, false});
+    return OC_OK;
+}
+extern "C" int oc_facets_clear(oc_facets *f, uint32_t field, uint64_t n, const uint64_t *doc_ids) {
+    if (!f) return fail(OC_ERR_INVALID, "NULL argument");
+    FcPending &P = f->pend;
+    std::lock_guard<std::mutex> g(P.mu);
+    if (n && !doc_ids) return fail(OC_ERR_INVALID, "NULL doc_ids");
+    if (field >= P.number.size()) return fail(OC_ERR_INVALID, "field %u: the store has %zu fields", field, P.number.size());
+    for (uint64_t i = 0; i < n; i++) P.clr[std::make_pair(field, doc_ids[i])] = ++P.seq;
+    return OC_OK;
+}
+extern "C" int oc_facets_delete(oc_facets *f, uint64_t n, const uint64_t *doc_ids) {
+    if (!f || (n && !doc_ids)) return fail(OC_ERR_INVALID, "NULL argument");
+    FcPending &P = f->pend;
+    std::lock_guard<std::mutex> g(P.mu);
+    for (uint64_t i = 0; i < n; i++) P.del[doc_ids[i]] = ++P.seq;
+    return OC_OK;
+}
+
+extern "C" int oc_facets_commit_ex(oc_facets *f, uint64_t new_nbits, oc_filter_commit_t *out) {
+    if (!f) return fail(OC_ERR_INVALID, "NULL argument");
+    const auto wall0 = std::chrono::steady_clock::now();
+    oc_ctx *c = f->ctx;
+    FcPending &P = f->pend;
+    std::vector<FcIns> ins;
+    std::unordered_map<uint64_t, uint64_t> del;
+    std::map<std::pair<uint32_t, uint64_t>, uint64_t> clr;
+    uint64_t cut = 0;
+    std::vector<uint32_t> n_var;
+    {
+        std::lock_guard<std::mutex> g(c->mu);   // nbits and the field list change only under it (and not during a commit)
+        OCTRY(fc_begin(P, f->nbits, new_nbits, c->device, ins, del, clr, cut));
+        std::lock_guard<std::mutex> gp(P.mu);
+        n_var = P.n_var;
+    }
+    // the published fields are not replaced until this commit publishes, so they are read without the ctx lock
+    const size_t nf = f->fields.size();
+    std::vector<FcMergeOut> res(nf);
+    std::vector<bool> fresh(nf, false);
+    oc_filter_commit_t st{};
+    int rc = OC_OK;
+    for (size_t fi = 0; fi < nf && rc == OC_OK; fi++) {
+        const FacetField &fl = f->fields[fi];
+        FcMergeIn in;
+        in.kind = fl.number ? FC_NUMBER : FC_CSR;
+        fc_take(P, ins, del, clr, uint32_t(fi), in.kind, in);
+        if (in.kb.empty() && in.kill.empty()) {   // unchanged (a CSR field may still gain empty variants)
+            st.rows_kept += fl.n_docs;
+            continue;
+        }
+        in.n_a = fl.n_docs; in.a_docs = fl.docs; in.a_vals = fl.d_values; in.old_off = &fl.offsets; in.n_var = n_var[fi];
+        rc = fc_merge(P.stream, P.ev, in, res[fi]);
+        fresh[fi] = rc == OC_OK;
+        st.device_ms += res[fi].device_ms;
+        st.rows_kept += res[fi].kept; st.rows_dropped += fl.n_docs - res[fi].kept; st.rows_added += res[fi].added;
+        st.workspace_bytes = std::max(st.workspace_bytes, res[fi].ws);
+    }
+    if (rc != OC_OK) {
+        for (size_t fi = 0; fi < nf; fi++) if (fresh[fi]) { cudaFree(res[fi].dev); cudaFree(res[fi].d_values); }
+        fc_end(P, false, 0, 0);
+        return rc;
+    }
+    // publish: every reader of the fields holds the ctx lock and works on the ctx stream, so once the stream has
+    // drained nothing refers to the previous arrays
+    std::vector<void *> old;
+    {
+        std::lock_guard<std::mutex> g(c->mu);
+        cudaSetDevice(c->device);
+        for (size_t fi = 0; fi < nf; fi++) {
+            FacetField &fl = f->fields[fi];
+            if (!fresh[fi]) {
+                if (!fl.number) fl.offsets.resize(size_t(n_var[fi]) + 1, fl.offsets.back());
+                continue;
+            }
+            old.push_back(fl.docs); old.push_back(fl.d_values);
+            fl.docs = static_cast<uint64_t *>(res[fi].dev); fl.d_values = res[fi].d_values; fl.n_docs = res[fi].n;
+            if (fl.number) fl.values.swap(res[fi].values); else fl.offsets.swap(res[fi].offsets);
+        }
+        f->nbits = new_nbits;
+        cudaStreamSynchronize(c->stream);
+        for (void *p : old) cudaFree(p);
+    }
+    st.version = fc_end(P, true, ins.size(), cut);
+    st.wall_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - wall0).count();
+    if (out) *out = st;
+    return OC_OK;
+}
+
+extern "C" int oc_facets_read_field(oc_facets *f, uint32_t field, uint32_t *n_variants, uint64_t *n_entries, uint64_t *offsets,
+                                    double *values, uint64_t *doc_ids) {
+    if (!f || !n_variants || !n_entries) return fail(OC_ERR_INVALID, "NULL argument");
+    oc_ctx *c = f->ctx;
+    std::lock_guard<std::mutex> g(c->mu);
+    if (field >= f->fields.size()) return fail(OC_ERR_INVALID, "field %u: the store has %zu fields", field, f->fields.size());
+    const FacetField &fl = f->fields[field];
+    const uint32_t cap_v = *n_variants;
+    const uint64_t cap_n = *n_entries;
+    *n_variants = fl.number ? 0 : uint32_t(fl.offsets.size() - 1);
+    *n_entries = fl.n_docs;
+    if (!doc_ids && !offsets && !values) return OC_OK;
+    if (((doc_ids || (fl.number && values)) && cap_n < fl.n_docs) || (!fl.number && offsets && cap_v < *n_variants))
+        return fail(OC_ERR_INVALID, "arrays hold %llu entries / %u variants, the field has %llu / %u", (unsigned long long)cap_n, cap_v,
+                    (unsigned long long)fl.n_docs, *n_variants);
+    CU(cudaSetDevice(c->device));
+    if (fl.n_docs && doc_ids) CU(cudaMemcpy(doc_ids, fl.docs, fl.n_docs * 8, cudaMemcpyDeviceToHost));
+    if (fl.number && values) std::copy(fl.values.begin(), fl.values.end(), values);
+    if (!fl.number && offsets) std::copy(fl.offsets.begin(), fl.offsets.end(), offsets);
+    return OC_OK;
 }
 
 // where-filter leaves over a filter field (read/index/filter.rs:49-124).  A leaf is one slice [lo, hi) of the field's
@@ -4604,6 +5007,7 @@ struct oc_geo_field {
     oc_ctx *ctx;
     uint64_t nbits, n;
     void *blob = nullptr;   // device: x, y, z, lat, lon (f64) then doc (u64), n entries each
+    FcPending pend;         // one field (0)
     GeoPoints pts() const {
         const double *d = static_cast<const double *>(blob);
         return GeoPoints{d, d + n, d + 2 * n, d + 3 * n, d + 4 * n, reinterpret_cast<const uint64_t *>(d + 5 * n), n};
@@ -4661,6 +5065,83 @@ extern "C" void oc_geo_field_destroy(oc_geo_field *g) {
         if (g->blob) cudaFree(g->blob);
     }
     delete g;
+}
+
+extern "C" int oc_geo_field_insert(oc_geo_field *g, uint64_t n, const uint64_t *doc_ids, const double *lat, const double *lon) {
+    if (!g || (n && (!doc_ids || !lat || !lon))) return fail(OC_ERR_INVALID, "NULL argument");
+    for (uint64_t i = 0; i < n; i++)
+        if (!geo_valid(lat[i], lon[i]))
+            return fail(OC_ERR_INVALID, "geopoint %llu: invalid coordinates (%g, %g)", (unsigned long long)i, lat[i], lon[i]);
+    FcPending &P = g->pend;
+    std::lock_guard<std::mutex> lk(P.mu);
+    for (uint64_t i = 0; i < n; i++) P.ins.push_back(FcIns{doc_ids[i], ++P.seq, 0.0, lat[i], lon[i], 0, 0, false});
+    return OC_OK;
+}
+extern "C" int oc_geo_field_delete(oc_geo_field *g, uint64_t n, const uint64_t *doc_ids) {
+    if (!g || (n && !doc_ids)) return fail(OC_ERR_INVALID, "NULL argument");
+    FcPending &P = g->pend;
+    std::lock_guard<std::mutex> lk(P.mu);
+    for (uint64_t i = 0; i < n; i++) P.del[doc_ids[i]] = ++P.seq;
+    return OC_OK;
+}
+extern "C" int oc_geo_field_commit_ex(oc_geo_field *g, uint64_t new_nbits, oc_filter_commit_t *out) {
+    if (!g) return fail(OC_ERR_INVALID, "NULL argument");
+    const auto wall0 = std::chrono::steady_clock::now();
+    oc_ctx *c = g->ctx;
+    FcPending &P = g->pend;
+    std::vector<FcIns> ins;
+    std::unordered_map<uint64_t, uint64_t> del;
+    std::map<std::pair<uint32_t, uint64_t>, uint64_t> clr;
+    uint64_t cut = 0;
+    {
+        std::lock_guard<std::mutex> lk(c->mu);
+        OCTRY(fc_begin(P, g->nbits, new_nbits, c->device, ins, del, clr, cut));
+    }
+    FcMergeIn in;
+    in.kind = FC_GEO;
+    fc_take(P, ins, del, clr, 0, FC_GEO, in);
+    FcMergeOut res;
+    oc_filter_commit_t st{};
+    const bool changed = !in.kb.empty() || !in.kill.empty();
+    if (changed) {
+        in.n_a = g->n; in.a_vals = static_cast<const double *>(g->blob);
+        const int rc = fc_merge(P.stream, P.ev, in, res);
+        if (rc != OC_OK) { fc_end(P, false, 0, 0); return rc; }
+        st.rows_kept = res.kept; st.rows_dropped = g->n - res.kept; st.rows_added = res.added; st.workspace_bytes = res.ws;
+        st.device_ms = res.device_ms;
+    } else {
+        st.rows_kept = g->n;
+    }
+    {   // publish (see oc_facets_commit_ex)
+        std::lock_guard<std::mutex> lk(c->mu);
+        cudaSetDevice(c->device);
+        g->nbits = new_nbits;
+        if (changed) {
+            void *old = g->blob;
+            g->blob = res.dev; g->n = res.n;
+            cudaStreamSynchronize(c->stream);
+            cudaFree(old);
+        }
+    }
+    st.version = fc_end(P, true, ins.size(), cut);
+    st.wall_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - wall0).count();
+    if (out) *out = st;
+    return OC_OK;
+}
+extern "C" int oc_geo_field_read(oc_geo_field *g, uint64_t *n, uint64_t *doc_ids, double *lat, double *lon) {
+    if (!g || !n) return fail(OC_ERR_INVALID, "NULL argument");
+    oc_ctx *c = g->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);
+    const uint64_t cap = *n;
+    *n = g->n;
+    if (!doc_ids && !lat && !lon) return OC_OK;
+    if (cap < g->n) return fail(OC_ERR_INVALID, "arrays hold %llu points, the field has %llu", (unsigned long long)cap, (unsigned long long)g->n);
+    CU(cudaSetDevice(c->device));
+    const GeoPoints p = g->pts();
+    if (g->n && doc_ids) CU(cudaMemcpy(doc_ids, p.doc, g->n * 8, cudaMemcpyDeviceToHost));
+    if (g->n && lat) CU(cudaMemcpy(lat, p.lat, g->n * 8, cudaMemcpyDeviceToHost));
+    if (g->n && lon) CU(cudaMemcpy(lon, p.lon, g->n * 8, cudaMemcpyDeviceToHost));
+    return OC_OK;
 }
 
 // a zeroed leaf over [0, nbits) of g's ctx, filled by `launch` (called under the ctx lock when g has points)

@@ -301,6 +301,13 @@ class DeviceFilter:
         self.ctx, self._h, self.nbits = ctx, handle, int(nbits)
 
     @classmethod
+    def of_handle(cls, ctx: Context, handle) -> "DeviceFilter":
+        """A handle the library built, with its own nbits (a leaf takes the nbits of the field version it was built on)."""
+        n = C.c_uint64()
+        check(lib().oc_filter_nbits(handle, C.byref(n)))
+        return cls(ctx, handle, n.value)
+
+    @classmethod
     def from_ids(cls, ctx: Context, doc_ids, nbits: int) -> "DeviceFilter":
         ids = np.ascontiguousarray(np.asarray(list(doc_ids) if not isinstance(doc_ids, np.ndarray) else doc_ids, np.uint64))
         h = C.c_void_p()
@@ -389,7 +396,7 @@ def _api_coord(p) -> Tuple[float, float]:
 class GeoPointField:
     """A geopoint filter field laid out for where-filter leaves on the device (oc_geo_field_*): one (doc_id, lat, lon)
     entry per point, degrees, so a document with several points repeats.  The points are taken as f64, as
-    FilterGeoPoint2 carries them.  Ids >= nbits are ignored.  Immutable: build a new one when the field changes.
+    FilterGeoPoint2 carries them.  Ids >= nbits are ignored.  insert() / delete() queue changes that commit() merges.
     radius() / polygon() return a DeviceFilter over [0, nbits) that holds the documents with at least one point inside
     (inside=True) or outside (inside=False); semantics and assumptions in include/oramacore_b200.h."""
 
@@ -412,7 +419,7 @@ class GeoPointField:
         clat, clon, r = self.radius_args(lat, lon, value, unit)
         h = C.c_void_p()
         check(lib().oc_filter_geo_radius(self._h, clat, clon, r, int(bool(inside)), C.byref(h)))
-        return DeviceFilter(self.ctx, h, self.nbits)
+        return DeviceFilter.of_handle(self.ctx, h)
 
     @staticmethod
     def radius_args(lat, lon, value, unit: str = "m"):
@@ -430,7 +437,7 @@ class GeoPointField:
         la, lo = self.polygon_args(coords)
         h = C.c_void_p()
         check(lib().oc_filter_geo_polygon(self._h, _p(la), _p(lo), la.shape[0], int(bool(inside)), C.byref(h)))
-        return DeviceFilter(self.ctx, h, self.nbits)
+        return DeviceFilter.of_handle(self.ctx, h)
 
     @staticmethod
     def polygon_args(coords):
@@ -445,6 +452,41 @@ class GeoPointField:
             k = int(np.flatnonzero(bad)[0])
             _geo_check(la[k], lo[k], f"polygon vertex {k}")
         return la, lo
+
+    def insert(self, doc_ids, lats, lons):
+        """Queue points (doc_ids[i], lats[i], lons[i]), checked as the constructor checks them; visible after commit()."""
+        d = np.ascontiguousarray(np.atleast_1d(np.asarray(doc_ids, np.uint64)).ravel())
+        la = np.ascontiguousarray(np.atleast_1d(np.asarray(lats, np.float64)).ravel())
+        lo = np.ascontiguousarray(np.atleast_1d(np.asarray(lons, np.float64)).ravel())
+        if not (d.shape == la.shape == lo.shape):
+            raise ValueError(f"{d.shape[0]} doc ids for {la.shape[0]} latitudes and {lo.shape[0]} longitudes")
+        bad = ~(np.isfinite(la) & np.isfinite(lo) & (np.abs(la) <= 90.0) & (np.abs(lo) <= 180.0))
+        if bad.any():
+            i = int(np.flatnonzero(bad)[0])
+            _geo_check(la[i], lo[i], f"geopoint {i}")
+        check(lib().oc_geo_field_insert(self._h, d.shape[0], _p(d), _p(la), _p(lo)))
+
+    def delete(self, doc_ids):
+        """Queue the removal of every point of the documents (call order: a later insert stays)."""
+        d = np.ascontiguousarray(np.atleast_1d(np.asarray(doc_ids, np.uint64)).ravel())
+        check(lib().oc_geo_field_delete(self._h, d.shape[0], _p(d)))
+
+    def commit(self, nbits: Optional[int] = None) -> dict:
+        """Merge the queued ops into the next version on the device (oc_geo_field_commit_ex), over [0, nbits) (default:
+        the current nbits; it may only grow).  Returns the call's statistics (oc_filter_commit_t)."""
+        nb = self.nbits if nbits is None else int(nbits)
+        st = _lib.FilterCommit()
+        check(lib().oc_geo_field_commit_ex(self._h, nb, C.byref(st)))
+        self.nbits, self.n = nb, int(st.rows_kept + st.rows_added)
+        return st.as_dict()
+
+    def read(self) -> dict:
+        """The published points in their device order (ascending document): {"doc_ids", "lat", "lon"}."""
+        n = C.c_uint64(0)
+        check(lib().oc_geo_field_read(self._h, C.byref(n), None, None, None))
+        d, la, lo = np.zeros(n.value, np.uint64), np.zeros(n.value, np.float64), np.zeros(n.value, np.float64)
+        check(lib().oc_geo_field_read(self._h, C.byref(n), _p(d), _p(la), _p(lo)))
+        return {"doc_ids": d, "lat": la, "lon": lo}
 
     def close(self):
         if self._h:
@@ -485,7 +527,7 @@ class FacetStore:
             check(lib().oc_filter_facet_variant(self._h, spec[1], spec[2], C.byref(h)))
         else:
             check(lib().oc_filter_facet_range(self._h, spec[1], spec[2], spec[3], spec[4], C.byref(h)))
-        return DeviceFilter(self.ctx, h, self.nbits)
+        return DeviceFilter.of_handle(self.ctx, h)
 
     def leaf_args(self, name: str, flt):
         """What leaf() asks of the library: ("variant", field id, variant), ("range", field id, lo, hi, flags), or None
@@ -536,6 +578,107 @@ class FacetStore:
         self.fields[name] = {"id": fid.value, "kind": "number", "values": np.unique(v)}   # distinct values, ascending
         return fid.value
 
+    @staticmethod
+    def _ids(doc_ids) -> np.ndarray:
+        return np.ascontiguousarray(np.atleast_1d(np.asarray(doc_ids, np.uint64)).ravel())
+
+    def add_key(self, name: str, key) -> int:
+        """The variant of `key` in a bool or string_filter field; a new string_filter key gets the next variant
+        (oc_facets_add_variant), listed in fields[name]["keys"] from the next commit() on."""
+        f = self.fields[name]
+        key = ("true" if key else "false") if f["kind"] == "bool" else key
+        if key in f["variant"]:
+            return f["variant"][key]
+        pend = f.setdefault("pending_keys", {})
+        if key not in pend:
+            if f["kind"] != "string":
+                raise ValueError(f"{name!r} is a {f['kind']} field: it has no key {key!r}")
+            v = C.c_uint32()
+            check(lib().oc_facets_add_variant(self._h, f["id"], C.byref(v)))
+            pend[key] = v.value
+        return pend[key]
+
+    def insert_variants(self, name: str, doc_ids, keys):
+        """Queue one (document, key) entry per pair of a bool (keys True / False, a set per document) or string_filter
+        field (a document may list a key several times); visible after commit()."""
+        f = self.fields[name]
+        d = self._ids(doc_ids)
+        v = np.ascontiguousarray([self.add_key(name, k) for k in keys], np.uint32)
+        if v.shape != d.shape:
+            raise ValueError(f"{d.shape[0]} doc ids for {v.shape[0]} keys")
+        check(lib().oc_facets_insert_variants(self._h, f["id"], d.shape[0], _p(d), _p(v),
+                                              _lib.OC_FACET_UNIQUE if f["kind"] == "bool" else 0))
+
+    def insert_numbers(self, name: str, doc_ids, values):
+        """Queue (document, value) entries of a number field, or of a date field with millisecond timestamps."""
+        f = self.fields[name]
+        d = self._ids(doc_ids)
+        v = np.atleast_1d(np.asarray(values, np.int64 if f["kind"] == "date" else np.float64)).ravel()
+        v = np.ascontiguousarray(v.astype(np.float64))
+        if v.shape != d.shape:
+            raise ValueError(f"{d.shape[0]} doc ids for {v.shape[0]} values")
+        check(lib().oc_facets_insert_numbers(self._h, f["id"], d.shape[0], _p(d), _p(v)))
+
+    def clear(self, name: str, doc_ids):
+        """Queue the removal of every value of the documents in field `name` (a replaced value)."""
+        d = self._ids(doc_ids)
+        check(lib().oc_facets_clear(self._h, self.fields[name]["id"], d.shape[0], _p(d)))
+
+    def delete(self, doc_ids):
+        """Queue the removal of every value of the documents in every field."""
+        d = self._ids(doc_ids)
+        check(lib().oc_facets_delete(self._h, d.shape[0], _p(d)))
+
+    def commit(self, nbits: Optional[int] = None) -> dict:
+        """Merge the queued ops into the next version of every field on the device (oc_facets_commit_ex), over
+        [0, nbits) (default: the current nbits; it may only grow).  Returns the call's statistics (oc_filter_commit_t)."""
+        nb = self.nbits if nbits is None else int(nbits)
+        st = _lib.FilterCommit()
+        check(lib().oc_facets_commit_ex(self._h, nb, C.byref(st)))
+        self.nbits = nb
+        name_of = {f["id"]: n for n, f in self.fields.items()}
+        for f in self.fields.values():
+            for key, v in sorted(f.pop("pending_keys", {}).items(), key=lambda kv: kv[1]):
+                f["keys"].append(key)
+                f["variant"][key] = v
+            if f["kind"] in ("number", "date"):
+                f["values"] = None   # distinct_values() reads the new version back when asked
+            elif f["kind"] == "string":   # the facets list the keys that hold documents, sorted
+                off = self.read_offsets(name_of[f["id"]])
+                f["listed"] = sorted(k for k, v in f["variant"].items() if off[v + 1] > off[v])
+        return st.as_dict()
+
+    def read_offsets(self, name: str) -> np.ndarray:
+        """The published variant offsets of a bool or string_filter field (the host copy; no device read)."""
+        fid = self.fields[name]["id"]
+        nv, n = C.c_uint32(0), C.c_uint64(0)
+        check(lib().oc_facets_read_field(self._h, fid, C.byref(nv), C.byref(n), None, None, None))
+        off = np.zeros(nv.value + 1, np.uint64)
+        check(lib().oc_facets_read_field(self._h, fid, C.byref(nv), C.byref(n), _p(off), None, None))
+        return off
+
+    def distinct_values(self, name: str) -> np.ndarray:
+        """The distinct values of a number or date field, ascending."""
+        f = self.fields[name]
+        if f.get("values") is None:
+            f["values"] = np.unique(self.read_field(name)["values"])
+        return f["values"]
+
+    def read_field(self, name: str) -> dict:
+        """Field `name` of the published version as oc_facets_add_* take it: {"doc_ids"} plus {"offsets"} (bool /
+        string_filter, one entry per variant + 1) or {"values"} (number / date, ascending)."""
+        fid = self.fields[name]["id"]
+        nv, n = C.c_uint32(0), C.c_uint64(0)
+        check(lib().oc_facets_read_field(self._h, fid, C.byref(nv), C.byref(n), None, None, None))
+        d = np.zeros(n.value, np.uint64)
+        if self.fields[name]["kind"] in ("number", "date"):
+            v = np.zeros(n.value, np.float64)
+            check(lib().oc_facets_read_field(self._h, fid, C.byref(nv), C.byref(n), None, _p(v), _p(d)))
+            return {"doc_ids": d, "values": v}
+        off = np.zeros(nv.value + 1, np.uint64)
+        check(lib().oc_facets_read_field(self._h, fid, C.byref(nv), C.byref(n), _p(off), None, _p(d)))
+        return {"doc_ids": d, "offsets": off}
+
     def close(self):
         if self._h:
             lib().oc_facets_destroy(self._h)
@@ -549,7 +692,8 @@ def _number_label(x) -> str:
 def facet_requests(store: FacetStore, facets: Dict[str, dict]):
     """The oc_facet_req tuples (field, variant, from, to) and (field name, label) pairs of one reference-style `facets`
     map: {"field": {"true": bool, "false": bool}} for a bool field, {"field": {"ranges": [{"from": a, "to": b}, ...]}}
-    for a number field (labels "from-to", number_field.rs:382), {"field": {}} for a string_filter field (every key).
+    for a number field (labels "from-to", number_field.rs:382), {"field": {}} for a string_filter field (every key; after
+    a commit() the keys that hold documents, sorted).
     Date fields have no facets, and ranges only apply to number fields."""
     reqs, labels = [], []
     for name, d in facets.items():
@@ -565,10 +709,10 @@ def facet_requests(store: FacetStore, facets: Dict[str, dict]):
         else:
             if "ranges" in d:
                 raise ValueError(f"{name!r} is a {f['kind']} field: ranges apply to number fields")
-            for vi, key in enumerate(f["keys"]):
+            for key in f.get("listed", f["keys"]):
                 if f["kind"] == "bool" and not d.get(key, False):
                     continue
-                reqs.append((f["id"], vi, 0.0, 0.0))
+                reqs.append((f["id"], f["variant"][key], 0.0, 0.0))
                 labels.append((name, key))
     return reqs, labels
 
@@ -614,11 +758,11 @@ class GroupBy:
         check(lib().oc_group_by_create(store._h, _p(ids), ids.shape[0], C.byref(self._h), C.byref(n)))
         self.n_groups = int(n.value)
         per_field = []
-        for f in fs:
+        for p, f in zip(self.properties, fs):
             if f["kind"] == "bool":
                 per_field.append([k == "true" for k in f["keys"]])
             elif f["kind"] == "number":
-                per_field.append([float(x) for x in f["values"]])
+                per_field.append([float(x) for x in store.distinct_values(p)])
             else:
                 per_field.append(list(f["keys"]))
         self.values: List[list] = [[]]

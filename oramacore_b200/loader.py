@@ -15,9 +15,11 @@ and `commit` / `compact` lay the pending data out (`CURRENT` + `versions/<n>`, e
 `IndexLoader.apply(op)` takes the same operations as plain dicts (the JSON shape of the reference's enum), resolves
 terms to stable term ids through the native dictionary (oc_dict_*), and drives the C ABI: oc_str_insert /
 oc_str_delete / oc_str_commit (snapshot swap: searches keep running on the previous version while a commit builds
-the next), oc_emb_insert / oc_emb_delete (live) and oc_emb_compact at commit.  `refresh_facets()` lays the accumulated filter fields out for
-oc_search_facets and rebuilds the geopoint field handles (`geo`, oc_geo_field_*); `where_filter(where)` evaluates a
-where-clause over them (where.py).  tf of a term = number of positions (exact + stemmed), as StringStorage counts them."""
+the next), oc_emb_insert / oc_emb_delete (live) and oc_emb_compact at commit.  Filter values and deletes are queued on
+the facet store and the geopoint fields as apply() sees them (tests/filter_commit_spec.py states the per-kind rules as
+ops); `refresh_facets()` merges them into the next version of every field on the device (oc_facets_commit_ex,
+oc_geo_field_commit_ex), and `where_filter(where)` evaluates a where-clause over them (where.py).  No host copy of the
+filter values is kept.  tf of a term = number of positions (exact + stemmed), as StringStorage counts them."""
 from __future__ import annotations
 
 from typing import Dict, Iterable, List, Optional, Sequence
@@ -51,18 +53,25 @@ class IndexLoader:
         self.dict = TermDictionary(max(len(self.string_fields), 1))
         self.strs = StringFieldStorage.empty(ctx, max(len(self.string_fields), 1))
         self.emb = EmbeddingFieldStorage(ctx, embedding_model or "BGESmall", dim=embedding_dim) if (embedding_model or embedding_dim) else None
-        self._bool = {f: ({}) for f in bool_fields}            # field -> {doc: bool} (FilterBool) or {doc: {bools}}
-        self._num = {f: ({}) for f in number_fields}           # field -> {doc: [numbers]}
-        self._strf = {f: ({}) for f in string_filter_fields}   # field -> {doc: [keys]}
-        self._geo = {f: ({}) for f in geopoint_fields}         # field -> {doc: [(lat, lon)]}
-        self._date = {f: ({}) for f in date_fields}            # field -> {doc: [ms]}
+        self._bool, self._num = list(bool_fields), list(number_fields)
+        self._strf, self._date, self._geo = list(string_filter_fields), list(date_fields), list(geopoint_fields)
         self.document_count = 0
         self.max_doc_id = -1
         self._deleted: set = set()
         self._uncommitted_deleted: set = set()                 # deletes since the last commit (filter.rs:344-392)
-        self.facets: Optional[FacetStore] = None
-        self.geo: Dict[str, GeoPointField] = {}
         self.nbits = 1                                         # DocumentId space of `facets` and `geo`
+        # one store and one geopoint field per field for the life of the loader; values queue until refresh_facets()
+        self.facets: Optional[FacetStore] = None
+        if self._bool or self._num or self._strf or self._date:
+            self.facets = FacetStore(ctx, self.nbits)
+            for f in self._bool:
+                self.facets.add_bool_field(f, [], [])
+            for f in self._num:
+                self.facets.add_number_field(f, [], [])
+            for f in self._date:
+                self.facets.add_date_field(f, [], [])
+            # a string_filter field joins the store with its first key (a field needs one variant)
+        self.geo: Dict[str, GeoPointField] = {f: GeoPointField(ctx, self.nbits, [], [], []) for f in self._geo}
         self._live: Optional[DeviceFilter] = None              # NOT(uncommitted deletes) of where_program, built once
         self._retired: List[DeviceFilter] = []                 # earlier ones, which programs may still point at
 
@@ -86,32 +95,35 @@ class IndexLoader:
                     ids = self.dict.add_terms(fi, names) if names else np.zeros(0, np.uint32)
                     tf = {int(i): max(1, len(terms[n].get("exact_positions", ())) + len(terms[n].get("positions", ()))) for i, n in zip(ids, names)}
                     self.strs.insert(d, fi, int(v["field_length"]), tf)
-                elif t == "FilterBool":
-                    self._bool[v["field"]][d] = bool(v["value"])
+                elif t == "FilterBool":                         # replaces the document's value
+                    f = self._field(self._bool, v["field"])
+                    self.facets.clear(f, [d])
+                    self.facets.insert_variants(f, [d], [bool(v["value"])])
                 elif t == "FilterNumber":
-                    self._num[v["field"]].setdefault(d, []).append(float(v["value"]))
+                    self.facets.insert_numbers(self._field(self._num, v["field"]), [d], [float(v["value"])])
                 elif t == "FilterString":
-                    self._strf[v["field"]].setdefault(d, []).append(str(v["value"]))
+                    self._insert_keys(v["field"], d, [str(v["value"])])
                 elif t == "FilterGeoPoint2":
                     # GeoPointIndexedValue: {"Plain": {"lat", "lon"}} or {"Array": [{"lat", "lon"}, ...]}
                     val = v["value"]
                     pts = [val["Plain"]] if "Plain" in val else list(val["Array"])
-                    self._geo[v["field"]].setdefault(d, []).extend((float(p["lat"]), float(p["lon"])) for p in pts)
-                elif t == "FilterBool2":
-                    bs = self._bool[v["field"]].get(d)
-                    bs = self._bool[v["field"]][d] = {bs} if isinstance(bs, bool) else (bs or set())
-                    bs.update(bool(b) for b in _plain_or_array(v["value"]))
+                    self.geo[self._field(self._geo, v["field"])].insert([d] * len(pts), [float(p["lat"]) for p in pts],
+                                                                        [float(p["lon"]) for p in pts])
+                elif t == "FilterBool2":                        # adds to the document's set of bools
+                    bs = [bool(b) for b in _plain_or_array(v["value"])]
+                    self.facets.insert_variants(self._field(self._bool, v["field"]), [d] * len(bs), bs)
                 elif t == "FilterNumber2":
                     # NumberFieldIndexedValue: {"I64": {"Plain": x} | {"Array": [...]}} or {"F64": ...}
+                    f = self._field(self._num, v["field"])
                     (store, val), = v["value"].items()
                     xs = _plain_or_array(val)
                     xs = [_exact_i64(x, "I64 value") for x in xs] if store == "I64" else [float(x) for x in xs]
-                    self._num[v["field"]].setdefault(d, []).extend(xs)
+                    self.facets.insert_numbers(f, [d] * len(xs), xs)
                 elif t == "FilterString2":
-                    self._strf[v["field"]].setdefault(d, []).extend(str(x) for x in _plain_or_array(v["value"]))
+                    self._insert_keys(v["field"], d, [str(x) for x in _plain_or_array(v["value"])])
                 elif t in ("FilterDate", "FilterDate2"):
-                    xs = [v["value"]] if t == "FilterDate" else _plain_or_array(v["value"])
-                    self._date[v["field"]].setdefault(d, []).extend(int(x) for x in xs)
+                    xs = [int(x) for x in ([v["value"]] if t == "FilterDate" else _plain_or_array(v["value"]))]
+                    self.facets.insert_numbers(self._field(self._date, v["field"]), [d] * len(xs), xs)
                 else:
                     raise ValueError(f"unsupported indexed value {t!r} (outside the search hot path)")
         elif kind == "IndexEmbedding":
@@ -128,11 +140,28 @@ class IndexLoader:
                     self._deleted.add(d)
                     self.document_count -= 1
                 self._uncommitted_deleted.add(d)
-                for m in list(self._bool.values()) + list(self._num.values()) + list(self._strf.values()) + list(self._geo.values()) + list(self._date.values()):
-                    m.pop(d, None)
+            if self.facets is not None:
+                self.facets.delete(ids)
+            for g in self.geo.values():
+                g.delete(ids)
             self._retire_live()
         else:
             raise ValueError(f"unsupported operation {kind!r}")
+
+    @staticmethod
+    def _field(names: List[str], name: str) -> str:
+        if name not in names:
+            raise KeyError(name)
+        return name
+
+    def _insert_keys(self, name: str, d: int, keys: List[str]) -> None:
+        """FilterString / FilterString2 append (a key listed twice is listed twice); a new key gets the next variant."""
+        self._field(self._strf, name)
+        if not keys:
+            return
+        if name not in self.facets.fields:
+            self.facets.add_string_field(name, {keys[0]: []})
+        self.facets.insert_variants(name, [d] * len(keys), keys)
 
     def apply_all(self, ops: Iterable[Dict]) -> None:
         for op in ops:
@@ -150,45 +179,25 @@ class IndexLoader:
         self._uncommitted_deleted.clear()
         self.refresh_facets()
 
-    def refresh_facets(self) -> None:
-        """Lay the filter fields out again: the facet store and one GeoPointField per geopoint field, both over
-        DocumentId [0, max_doc_id + 2).  Handles built earlier are closed."""
-        for g in self.geo.values():
-            g.close()
-        self.geo = {}
+    def refresh_facets(self) -> dict:
+        """Publish every filter value applied so far over DocumentId [0, max_doc_id + 2): the queued values and deletes
+        merge into the next version of the facet store and of every geopoint field on the device; the objects stay
+        the same.  The uncommitted deletes stay uncommitted.  NOT(deletes) handles built earlier are closed (nbits may
+        change).  Returns the commits' statistics by field kind ("facets", and the geopoint field names)."""
         self._retire_live()       # nbits changes: the deletes handle is rebuilt over the new DocumentId space
-        for f in self._retired:   # programs built before now point at the closed facet store and fields as well
+        for f in self._retired:   # programs built before now carry the earlier nbits
             f.close()
         self._retired = []
-        self.nbits = self.max_doc_id + 2
-        for f, m in self._geo.items():
-            docs = [d for d, ps in m.items() for _ in ps]
-            self.geo[f] = GeoPointField(self.ctx, self.max_doc_id + 2, docs, [p[0] for ps in m.values() for p in ps],
-                                        [p[1] for ps in m.values() for p in ps])
-        if not (self._bool or self._num or self._strf or self._date):
-            return
+        self.nbits = max(self.nbits, self.max_doc_id + 2)
+        stats = {}
         if self.facets is not None:
-            self.facets.close()
-        st = FacetStore(self.ctx, self.max_doc_id + 2)
-        for f, m in self._bool.items():
-            has = {d: ({b} if isinstance(b, bool) else b) for d, b in m.items()}
-            st.add_bool_field(f, [d for d, bs in has.items() if True in bs], [d for d, bs in has.items() if False in bs])
-        for f, m in self._num.items():
-            docs = [d for d, vs in m.items() for _ in vs]
-            vals = [x for vs in m.values() for x in vs]
-            st.add_number_field(f, docs, vals)
-        for f, m in self._strf.items():
-            keys: Dict[str, List[int]] = {}
-            for d, ks in m.items():
-                for k in ks:
-                    keys.setdefault(k, []).append(d)
-            st.add_string_field(f, {k: keys[k] for k in sorted(keys)})
-        for f, m in self._date.items():
-            st.add_date_field(f, [d for d, ms in m.items() for _ in ms], [x for ms in m.values() for x in ms])
-        self.facets = st
+            stats["facets"] = self.facets.commit(self.nbits)
+        for name, g in self.geo.items():
+            stats[name] = g.commit(self.nbits)
+        return stats
 
     def filter_fields(self) -> List[str]:
-        return list(self._bool) + list(self._num) + list(self._strf) + list(self._date) + list(self._geo)
+        return self._bool + self._num + self._strf + self._date + self._geo
 
     def where_filter(self, where) -> Optional[DeviceFilter]:
         """The where-clause `where` (a JSON object or a parsed WhereFilter) over this index as execute_filter

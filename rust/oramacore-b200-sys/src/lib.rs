@@ -52,6 +52,20 @@ pub struct OcStrCommit {
     pub device_ms: f32,
     pub wall_ms: f32,
 }
+/// Statistics of one `oc_facets_commit_ex` / `oc_geo_field_commit_ex` call (`oc_filter_commit_t`).
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct OcFilterCommit {
+    pub version: u64,
+    pub rows_kept: u64,
+    pub rows_dropped: u64,
+    pub rows_added: u64,
+    pub workspace_bytes: u64,
+    pub device_ms: f32,
+    pub wall_ms: f32,
+}
+/// `oc_facets_insert_variants` flag: set semantics (a bool field).
+pub const OC_FACET_UNIQUE: u32 = 1;
 /// `OcSearchParams::sharded`: merge across `oc_comm` ranks; add `OC_SHARD_TOMBSTONES` on every rank while
 /// any rank's string store holds uncommitted deletes (the df all-reduce must be entered by all ranks).
 pub const OC_SHARDED: c_int = 1;
@@ -274,12 +288,17 @@ extern "C" {
     pub fn oc_filter_or(a: *const OcFilter, b: *const OcFilter, out: *mut *mut OcFilter) -> c_int;
     pub fn oc_filter_not(a: *const OcFilter, out: *mut *mut OcFilter) -> c_int;
     pub fn oc_filter_count(f: *const OcFilter, out: *mut u64) -> c_int;
+    pub fn oc_filter_nbits(f: *const OcFilter, out: *mut u64) -> c_int;
     pub fn oc_filter_read(f: *const OcFilter, out_bits: *mut u64) -> c_int;
     pub fn oc_filter_destroy(f: *mut OcFilter);
     // geopoint where-filter leaves (GeoPointFieldStorage::filter, geopoint_field.rs:179-229): an oc_filter over [0, nbits)
     pub fn oc_geo_field_create(ctx: *mut OcCtx, nbits: u64, n: u64, doc_ids: *const u64, lat: *const f64, lon: *const f64,
                                out: *mut *mut OcGeoField) -> c_int;
     pub fn oc_geo_field_destroy(g: *mut OcGeoField);
+    pub fn oc_geo_field_insert(g: *mut OcGeoField, n: u64, doc_ids: *const u64, lat: *const f64, lon: *const f64) -> c_int;
+    pub fn oc_geo_field_delete(g: *mut OcGeoField, n: u64, doc_ids: *const u64) -> c_int;
+    pub fn oc_geo_field_commit_ex(g: *mut OcGeoField, new_nbits: u64, out: *mut OcFilterCommit) -> c_int;
+    pub fn oc_geo_field_read(g: *mut OcGeoField, n: *mut u64, doc_ids: *mut u64, lat: *mut f64, lon: *mut f64) -> c_int;
     pub fn oc_filter_geo_radius(g: *const OcGeoField, lat: f64, lon: f64, radius_m: f64, inside: c_int,
                                 out: *mut *mut OcFilter) -> c_int;
     pub fn oc_filter_geo_polygon(g: *const OcGeoField, lat: *const f64, lon: *const f64, n_vertices: u32, inside: c_int,
@@ -291,6 +310,14 @@ extern "C" {
     pub fn oc_facets_create(ctx: *mut OcCtx, nbits: u64, out: *mut *mut OcFacets) -> c_int;
     pub fn oc_facets_destroy(f: *mut OcFacets);
     pub fn oc_facets_add_field(f: *mut OcFacets, n_variants: u32, variant_offsets: *const u64, doc_ids: *const u64, out_field: *mut u32) -> c_int;
+    pub fn oc_facets_insert_variants(f: *mut OcFacets, field: u32, n: u64, doc_ids: *const u64, variants: *const u32, flags: u32) -> c_int;
+    pub fn oc_facets_add_variant(f: *mut OcFacets, field: u32, variant_out: *mut u32) -> c_int;
+    pub fn oc_facets_insert_numbers(f: *mut OcFacets, field: u32, n: u64, doc_ids: *const u64, values: *const f64) -> c_int;
+    pub fn oc_facets_clear(f: *mut OcFacets, field: u32, n: u64, doc_ids: *const u64) -> c_int;
+    pub fn oc_facets_delete(f: *mut OcFacets, n: u64, doc_ids: *const u64) -> c_int;
+    pub fn oc_facets_commit_ex(f: *mut OcFacets, new_nbits: u64, out: *mut OcFilterCommit) -> c_int;
+    pub fn oc_facets_read_field(f: *mut OcFacets, field: u32, n_variants: *mut u32, n_entries: *mut u64, offsets: *mut u64,
+                                values: *mut f64, doc_ids: *mut u64) -> c_int;
     pub fn oc_facets_add_number_field(f: *mut OcFacets, n: u64, values_sorted: *const f64, doc_ids: *const u64, out_field: *mut u32) -> c_int;
     // where-filter leaves over a filter field (filter.rs:49-124): a variant's documents, or a number field's value interval
     pub fn oc_filter_facet_variant(f: *const OcFacets, field: u32, variant: u32, out: *mut *mut OcFilter) -> c_int;
