@@ -1363,7 +1363,7 @@ extern "C" int oc_str_commit_ex(oc_str *s, oc_str_commit_t *out) {
     std::unordered_map<uint64_t, uint64_t> pdel;
     std::vector<uint32_t> base_alive;
     uint64_t base_deleted;
-    bool global_count, global_avg;
+    bool global_avg;
     {
         std::lock_guard<std::mutex> g(s->mu);
         if (s->committing) return fail(OC_ERR_INVALID, "a commit of this store is already in flight");
@@ -1375,7 +1375,7 @@ extern "C" int oc_str_commit_ex(oc_str *s, oc_str_commit_t *out) {
         pdel.swap(s->pending_deleted);
         base_alive = base->alive_host;
         base_deleted = base->n_deleted;
-        global_count = s->global_count; global_avg = s->global_avg;
+        global_avg = s->global_avg;
     }
     // on failure: put the taken ops back (in front of whatever arrived meanwhile) and leave `cur` alone
     auto abort_commit = [&](int rc) {
@@ -1524,7 +1524,7 @@ extern "C" int oc_str_commit_ex(oc_str *s, oc_str_commit_t *out) {
     ns->device = c->device;
     ns->fields.resize(nf);
     ns->n_rows = n_new;
-    ns->document_count = global_count ? B.document_count : n_new;
+    ns->document_count = n_new;             // or the caller's N, taken at the swap below
     struct Workspace {   // every way out of the call waits for the load stream, then gives the workspace back
         oc_str *s; uint8_t *p = nullptr;
         ~Workspace() { cudaStreamSynchronize(s->load_stream); cudaFree(p); }
@@ -1671,6 +1671,12 @@ extern "C" int oc_str_commit_ex(oc_str *s, oc_str_commit_t *out) {
         for (uint64_t d : s->deletes_during_commit) { const uint64_t r = ns->row_of(d); if (r != ~0ull) rows.push_back(r); }
         const int trc = snap_tombstone(*ns, rows, s->load_stream);
         if (trc != OC_OK) { s->committing = false; return trc; }   // (pending ops were consumed; the old snapshot stays published)
+        // the corpus-wide values the caller owns are taken now, not when the commit started, so that an
+        // oc_str_set_global made while the merge ran is not lost with the old snapshot.  They are on `cur`: while a
+        // commit is in flight only oc_str_set_global and tombstones change it (set_rows / load_field are refused).
+        if (s->global_count) ns->document_count = s->cur->document_count;
+        if (s->global_avg)
+            for (size_t fi = 0; fi < nf; fi++) ns->fields[fi].avg_len = s->cur->fields[fi].avg_len;
         ns->version = ++s->version;
         s->cur = ns;
         s->deletes_during_commit.clear();

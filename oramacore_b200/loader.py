@@ -9,7 +9,8 @@ The reference's read side is fed by `Index::update_data(IndexWriteOperation)` (r
       FilterBool2 / FilterString2 / FilterDate / FilterDate2 / FilterNumber2 -> the same filter fields as the write side
                                               emits them today (write/index/fields.rs:312-325, 345-353, 401-423, 467-504)
   * `IndexEmbedding { data: field -> [(doc_id, vectors)] }` -> EmbeddingFieldStorage::insert (mod.rs:1688-1698)
-  * `DeleteDocuments { doc_ids }` — uncommitted deletes, excluded from every search at once (mod.rs:1346-1427)
+  * `DeleteDocuments { doc_ids }` — `document_count -= len(doc_ids)` (saturating), uncommitted deletes, excluded
+      from every search at once (mod.rs:1346-1427)
 and `commit` / `compact` lay the pending data out (`CURRENT` + `versions/<n>`, embedding_field.rs:91-95).
 
 `IndexLoader.apply(op)` takes the same operations as plain dicts (the JSON shape of the reference's enum), resolves
@@ -55,9 +56,8 @@ class IndexLoader:
         self.emb = EmbeddingFieldStorage(ctx, embedding_model or "BGESmall", dim=embedding_dim) if (embedding_model or embedding_dim) else None
         self._bool, self._num = list(bool_fields), list(number_fields)
         self._strf, self._date, self._geo = list(string_filter_fields), list(date_fields), list(geopoint_fields)
-        self.document_count = 0
+        self.document_count = 0                                # N of the idf, live between commits (see _push_count)
         self.max_doc_id = -1
-        self._deleted: set = set()
         self._uncommitted_deleted: set = set()                 # deletes since the last commit (filter.rs:344-392)
         self.nbits = 1                                         # DocumentId space of `facets` and `geo`
         # one store and one geopoint field per field for the life of the loader; values queue until refresh_facets()
@@ -80,9 +80,8 @@ class IndexLoader:
         kind = op["type"]
         if kind == "Index":
             d = int(op["doc_id"])
-            self.document_count += 1
+            self.document_count += 1                            # mod.rs:1460
             self.max_doc_id = max(self.max_doc_id, d)
-            self._deleted.discard(d)
             if d in self._uncommitted_deleted:
                 self._uncommitted_deleted.discard(d)
                 self._retire_live()
@@ -126,6 +125,7 @@ class IndexLoader:
                     self.facets.insert_numbers(self._field(self._date, v["field"]), [d] * len(xs), xs)
                 else:
                     raise ValueError(f"unsupported indexed value {t!r} (outside the search hot path)")
+            self._push_count()
         elif kind == "IndexEmbedding":
             for d, vectors in op["data"]:
                 self.max_doc_id = max(self.max_doc_id, int(d))
@@ -135,11 +135,11 @@ class IndexLoader:
             self.strs.delete(ids)
             if self.emb is not None:
                 self.emb.delete(ids)
-            for d in ids:
-                if d not in self._deleted:
-                    self._deleted.add(d)
-                    self.document_count -= 1
-                self._uncommitted_deleted.add(d)
+            # mod.rs:1417-1423: the count drops by the number of ids in the op, whether or not each was a live
+            # document, and stops at 0
+            self.document_count = max(self.document_count - len(ids), 0)
+            self._push_count()
+            self._uncommitted_deleted.update(ids)
             if self.facets is not None:
                 self.facets.delete(ids)
             for g in self.geo.values():
@@ -147,6 +147,12 @@ class IndexLoader:
             self._retire_live()
         else:
             raise ValueError(f"unsupported operation {kind!r}")
+
+    def _push_count(self) -> None:
+        """N of the idf is Index::document_count (mod.rs:1460: +1 per Index op, also for documents without string
+        fields), read by every search whether or not it was committed (token_score.rs:221, search.rs:305-318).  So the
+        string store gets it after every op that changes it, and again after its commit."""
+        self.strs.set_global(self.document_count)
 
     @staticmethod
     def _field(names: List[str], name: str) -> str:
@@ -174,8 +180,7 @@ class IndexLoader:
         self.strs.commit()
         if self.emb is not None:
             self.emb.compact()
-        # N of the idf is Index::document_count (mod.rs:1460: +1 per Index op, also for documents without string fields)
-        self.strs.set_global(max(self.document_count, 0))
+        self._push_count()
         self._uncommitted_deleted.clear()
         self.refresh_facets()
 
