@@ -670,12 +670,30 @@ int oc_merge_pinned(uint32_t n_indexes, uint32_t n_queries, uint32_t limit, uint
 typedef struct oc_sort_field oc_sort_field;
 /* One (document, value) entry per value: documents may repeat (multi-valued fields).  A bool is 0 / 1, a date its
  * millisecond timestamp; integers beyond 2^53 do not round-trip through the double and are not representable here.
- * Ids >= nbits are ignored.  OC_ERR_INVALID: a NaN value, nbits == 0 or >= 2^32 - 1.  Sorted once on the host (setup,
- * not the hot path); per order the device holds the documents in rank order (8 B each) and a rank per document id
- * (4 x nbits bytes), plus a rank -> string row map rebuilt on the first sorted search after each oc_str_commit.  The
- * handle is immutable: a changed field means a new handle. */
+ * Ids >= nbits are ignored.  OC_ERR_INVALID: a NaN value, nbits == 0 or >= 2^32 - 1; OC_ERR_UNSUPPORTED: 2^31 - 1
+ * entries or more.  Built on the device under the ctx lock, on the ctx stream (radix sorts and a scan, deterministic):
+ * per order the device holds the documents in rank order (8 B each) and a rank per document id (4 x nbits bytes),
+ * plus a rank -> string row map rebuilt on the first sorted search after each oc_str_commit; the host keeps a copy of
+ * the ranks and of each rank's value (+0.0 for a -0.0 entry).  Workspace, freed before the call returns: about 40 B
+ * per entry (16 B more for the upload of oc_sort_field_create's entries), 4 B per document id and the CUB storage.
+ * The handle is immutable: a changed field means a new handle. */
 int oc_sort_field_create(oc_ctx *ctx, uint64_t nbits, uint64_t n, const uint64_t *doc_ids, const double *values,
                          oc_sort_field **out);
+/* The sort field of one field of the facet store's published version, built on the device from the field's device
+ * arrays (nothing is read back to the host first) by the same build as oc_sort_field_create, over nbits = the
+ * version's.  A number or date field: variant_values NULL, each entry's value is its field value.  A bool or
+ * string_filter field: variant_values holds one value per variant (a bool field {1.0, 0.0}: variant 0 is true), and a
+ * document with several variants is placed by the rules above.  It runs under the ctx lock, so it reads one whole
+ * published version even while an oc_facets_commit_ex of the store is in flight; the handle records that version's
+ * number (oc_filter_commit_t.version, 0 before the first commit) and, like a created one, is immutable: build a new
+ * one after a commit of its field.  OC_ERR_INVALID, creating nothing: a NULL argument, an unknown field,
+ * variant_values NULL for a variant field or given for a number field, a NaN variant value, nbits >= 2^32 - 1. */
+int oc_sort_field_from_facets(oc_facets *f, uint32_t field, const double *variant_values, oc_sort_field **out);
+/* Read-back of one order (OC_SORT_ASC / OC_SORT_DESC): *n documents in rank order and the value each was placed by.
+ * With rank_doc and rank_value NULL it returns the sizes; otherwise *n is the arrays' capacity on entry.  nbits and
+ * facets_version (oc_sort_field_from_facets' version, 0 for a created handle) may be NULL. */
+int oc_sort_field_read(const oc_sort_field *f, int order, uint64_t *nbits, uint64_t *n, uint64_t *rank_doc, double *rank_value,
+                       uint64_t *facets_version);
 void oc_sort_field_destroy(oc_sort_field *f);
 #define OC_SORT_ASC 0
 #define OC_SORT_DESC 1

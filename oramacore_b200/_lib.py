@@ -52,7 +52,7 @@ EXPORTED_SYMBOLS = [
     "oc_filter_facet_variant", "oc_filter_facet_range", "oc_where_check", "oc_filter_from_where",
     "oc_group_by_create", "oc_group_by_destroy", "oc_search_groups",
     "oc_search_pinned", "oc_search_groups_pinned", "oc_merge_pinned",
-    "oc_sort_field_create", "oc_sort_field_destroy", "oc_search_sorted", "oc_search_q_sorted", "oc_search_groups_sorted", "oc_merge_sorted",
+    "oc_sort_field_create", "oc_sort_field_from_facets", "oc_sort_field_read", "oc_sort_field_destroy", "oc_search_sorted", "oc_search_q_sorted", "oc_search_groups_sorted", "oc_merge_sorted",
     "oc_group_by_n_groups", "oc_search_q_groups", "oc_facets_check", "oc_search_q_facets",
     "oc_dict_create", "oc_dict_destroy", "oc_dict_add_terms", "oc_dict_lookup", "oc_dict_size", "oc_dict_set_stemmer", "oc_stem_english",
     "oc_dict_resolve", "oc_dict_resolve_q", "oc_dict_device_bytes", "oc_resolved_arrays", "oc_resolved_fill", "oc_resolved_free",
@@ -285,6 +285,8 @@ def lib():
     L.oc_merge_pinned.argtypes = [u32, u32, u32, u32, u32, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(Pins),
                                   C.POINTER(vp), C.POINTER(vp), vp, vp, vp, vp]
     L.oc_sort_field_create.argtypes = [vp, u64, u64, vp, vp, C.POINTER(vp)]
+    L.oc_sort_field_from_facets.argtypes = [vp, u32, vp, C.POINTER(vp)]
+    L.oc_sort_field_read.argtypes = [vp, C.c_int, C.POINTER(u64), C.POINTER(u64), vp, vp, C.POINTER(u64)]
     L.oc_sort_field_destroy.argtypes = [vp]
     L.oc_sort_field_destroy.restype = None
     L.oc_search_sorted.argtypes = [vp, vp, vp, C.POINTER(SearchParams), C.POINTER(Sort), vp, vp, vp, vp, vp, vp, vp, vp]

@@ -39,6 +39,7 @@
 #include "group.cuh"
 #include "pins.cuh"
 #include "sort.cuh"
+#include "sort_build.cuh"
 #include "tmap.cuh"
 #include "where.cuh"
 #include "oramacore_b200.h"
@@ -192,6 +193,7 @@ struct oc_ctx {
     DevBuf row_ft, grp_vdoc, grp_vscore, grp_vn, grp_gmin, grp_den, grp_doc, grp_score, grp_n;   // oc_search_groups
     DevBuf pin_row, pin_ft, pin_ftp, pin_score, pin_present, pin_top_doc, pin_top_score, pin_top_n, pin_gdoc, pin_gscore, pin_gn;   // pins
     DevBuf srt_doc, srt_row, srt_n, srt_ft, srt_ftp, srt_score, srt_present, srt_zero;   // sortBy
+    DevBuf sfb_ws;                    // sort field build (sort_build.cuh), released before the call returns
     DevBuf q_bf16, q_f16, q_scale, q_rho, pre_post, dense_buf, g_thr, g_eps, g_ovf, g_ovfcnt, g_resc, g_cand, g_cnt, g_flag, g_max, r_qpad, r_qinv, r_map, r_doc, r_score, r_row, r_cnt, r_raw;
     // per-query where-filters (q_filters): the embedding rows' bitmap of every distinct handle, and the slots of the
     // queries the exact sweep re-runs; v_qslot / v_rowbits describe the vector stage of the current call (fix_unproven)
@@ -2323,6 +2325,7 @@ struct SortOrder {
 struct oc_sort_field {
     oc_ctx *ctx;
     uint64_t nbits;
+    uint64_t facets_version = 0;           // oc_sort_field_from_facets: the facet-store version it was built from
     SortOrder ord[2];                      // OC_SORT_ASC, OC_SORT_DESC
 };
 static void sort_field_free(oc_sort_field *f) {
@@ -4195,8 +4198,9 @@ extern "C" int oc_facets_commit_ex(oc_facets *f, uint64_t new_nbits, oc_filter_c
         f->nbits = new_nbits;
         cudaStreamSynchronize(c->stream);
         for (void *p : old) cudaFree(p);
+        // the version number moves with the arrays, so a reader under the ctx lock sees them together
+        st.version = fc_end(P, true, ins.size(), cut);
     }
-    st.version = fc_end(P, true, ins.size(), cut);
     st.wall_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - wall0).count();
     if (out) *out = st;
     return OC_OK;
@@ -4808,50 +4812,169 @@ extern "C" int oc_search_groups_pinned(oc_ctx *c, oc_emb *emb, oc_str *str, oc_g
                        nullptr, nullptr, out_group_doc_ids, out_group_scores, nullptr, out_group_n);
 }
 
-// ------------------------------------------------------------------------------------ sortBy (sort.cuh)
+// ------------------------------------------------------------------------------------ sortBy (sort.cuh, sort_build.cuh)
+// The entries of one sort field build: documents and values in device memory, or on the host (uploaded first).
+struct SortBuildIn {
+    uint64_t n = 0;
+    const uint64_t *h_docs = nullptr, *d_docs = nullptr;
+    const double *h_vals = nullptr, *d_vals = nullptr;
+    const std::vector<uint64_t> *off = nullptr;   // or a variant field: its offsets (host copy) and
+    const double *var_vals = nullptr;             //   one value per variant (host)
+};
+// Builds both orders of `f` on the ctx stream (sort_build.cuh).  Called under the ctx lock; on failure `f` is freed.
+static int sort_field_build(oc_ctx *c, const SortBuildIn &in, oc_sort_field *f) {
+    const uint64_t n = in.n, nbits = f->nbits;
+    const uint32_t n_var = in.off ? uint32_t(in.off->size() - 1) : 0;
+    auto bad = [&](int code) { sort_field_free(f); return code; };
+    if (n >= uint64_t(INT32_MAX))   // cub counts in int, and a rank is a uint32
+        return bad(fail(OC_ERR_UNSUPPORTED, "sort field: %llu entries >= 2^31 - 1", (unsigned long long)n));
+    cudaStream_t st = c->stream;
+    const int end_bit = 64 - __builtin_clzll(nbits);   // every kept document is below 2^end_bit
+    size_t b_doc = 0, b_asc = 0, b_desc = 0, b_scan = 0;
+    if (cub::DeviceRadixSort::SortPairs(nullptr, b_doc, (const uint32_t *)nullptr, (uint32_t *)nullptr, (const unsigned long long *)nullptr,
+                                        (unsigned long long *)nullptr, (int)n, 0, end_bit, st) != cudaSuccess ||
+        cub::DeviceRadixSort::SortPairs(nullptr, b_asc, (const unsigned long long *)nullptr, (unsigned long long *)nullptr,
+                                        (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)n, 0, 64, st) != cudaSuccess ||
+        cub::DeviceRadixSort::SortPairsDescending(nullptr, b_desc, (const unsigned long long *)nullptr, (unsigned long long *)nullptr,
+                                                  (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)n, 0, 64, st) != cudaSuccess ||
+        cub::DeviceScan::ExclusiveSum(nullptr, b_scan, (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)(n + 1), st) != cudaSuccess)
+        return bad(fail(OC_ERR_CUDA, "sort field: cub temp size"));
+    // workspace: [uploaded: docs | values | offsets | variant values] doc_a | key_a | doc_b | key_b | first | keep | rank | value | cub
+    auto al = [](size_t x) { return (x + 255) & ~size_t(255); };
+    const size_t o_docs = 0, o_vals = o_docs + al(in.h_docs ? n * 8 : 0), o_off = o_vals + al(in.h_vals ? n * 8 : 0),
+                 o_vv = o_off + al(in.off ? (n_var + 1) * 8 : 0), o_da = o_vv + al(n_var * 8);
+    const size_t o_ka = o_da + al(n * 4), o_db = o_ka + al(n * 8), o_kb = o_db + al(n * 4), o_first = o_kb + al(n * 8),
+                 o_keep = o_first + al(nbits * 4), o_rank = o_keep + al((n + 1) * 4), o_val = o_rank + al((n + 1) * 4),
+                 o_cub = o_val + al(n * 8), total = o_cub + al(std::max(std::max(b_doc, b_scan), std::max(b_asc, b_desc)));
+    struct Release {   // every way out waits for the stream, then gives the workspace back
+        oc_ctx *c;
+        ~Release() { cudaStreamSynchronize(c->stream); c->sfb_ws.release(); }
+    } release{c};
+    if (c->sfb_ws.ensure(total) != OC_OK) return bad(OC_ERR_OOM);
+    uint8_t *w = c->sfb_ws.as<uint8_t>();
+    auto at = [&](size_t o) { return static_cast<void *>(w + o); };
+    const uint64_t *docs = in.d_docs ? in.d_docs : static_cast<const uint64_t *>(at(o_docs));
+    const oc::SfSource src{in.d_vals ? in.d_vals : in.h_vals ? static_cast<const double *>(at(o_vals)) : nullptr,
+                           static_cast<const uint64_t *>(at(o_off)), static_cast<const double *>(at(o_vv)), n_var};
+    uint32_t *da = static_cast<uint32_t *>(at(o_da)), *db = static_cast<uint32_t *>(at(o_db));
+    unsigned long long *ka = static_cast<unsigned long long *>(at(o_ka)), *kb = static_cast<unsigned long long *>(at(o_kb));
+    uint32_t *first = static_cast<uint32_t *>(at(o_first)), *keep = static_cast<uint32_t *>(at(o_keep));
+    uint32_t *rank = static_cast<uint32_t *>(at(o_rank));
+    double *val = static_cast<double *>(at(o_val));
+    const unsigned g = (unsigned)((n + oc::SF_THREADS - 1) / oc::SF_THREADS), g1 = (unsigned)((n + oc::SF_THREADS) / oc::SF_THREADS);
+    cudaError_t e = cudaSuccess;
+    if (n && in.h_docs) e = cudaMemcpyAsync(at(o_docs), in.h_docs, n * 8, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess && n && in.h_vals) e = cudaMemcpyAsync(at(o_vals), in.h_vals, n * 8, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess && in.off) e = cudaMemcpyAsync(at(o_off), in.off->data(), (n_var + 1) * 8, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess && in.off && n_var) e = cudaMemcpyAsync(at(o_vv), in.var_vals, n_var * 8, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess && n) {
+        oc::sf_keys_kernel<<<g, oc::SF_THREADS, 0, st>>>(docs, n, nbits, src, da, ka);
+        launched(c);
+        e = cudaGetLastError();
+        if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(at(o_cub), b_doc, da, db, ka, kb, (int)n, 0, end_bit, st);   // by document
+    }
+    if (e != cudaSuccess) return bad(fail(OC_ERR_CUDA, "sort field build: %s", cudaGetErrorString(e)));
+    for (int ord = OC_SORT_ASC; ord <= OC_SORT_DESC; ord++) {
+        SortOrder &o = f->ord[ord];
+        uint32_t cnt = 0;
+        if (n) {   // entries in rank order with repeats (doc_a, key_a), then the first position of each document
+            e = ord == OC_SORT_ASC ? cub::DeviceRadixSort::SortPairs(at(o_cub), b_asc, kb, ka, db, da, (int)n, 0, 64, st)
+                                   : cub::DeviceRadixSort::SortPairsDescending(at(o_cub), b_desc, kb, ka, db, da, (int)n, 0, 64, st);
+            if (e == cudaSuccess) e = cudaMemsetAsync(first, 0xff, nbits * 4, st);
+            if (e == cudaSuccess) {
+                oc::sf_first_kernel<<<g, oc::SF_THREADS, 0, st>>>(da, n, first);
+                oc::sf_keep_kernel<<<g1, oc::SF_THREADS, 0, st>>>(da, n, first, keep);
+                launched(c); launched(c);
+                e = cudaGetLastError();
+            }
+            if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(at(o_cub), b_scan, keep, rank, (int)(n + 1), st);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(&cnt, rank + n, 4, cudaMemcpyDeviceToHost, st);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        }
+        o.n = cnt;
+        if (e == cudaSuccess) e = cudaMalloc(&o.rank_doc, std::max<size_t>(o.n, 1) * 8);
+        if (e == cudaSuccess) e = cudaMalloc(&o.doc_rank, nbits * 4);
+        if (e == cudaSuccess) e = cudaMalloc(&o.rank_row, (o.n + 1) * 4);
+        if (e == cudaSuccess) e = cudaMemsetAsync(o.doc_rank, 0xff, nbits * 4, st);             // RANK_NONE: no value
+        if (e == cudaSuccess) e = cudaMemsetAsync(o.rank_row + o.n, 0xff, 4, st);               // the sentinel
+        if (e == cudaSuccess && o.n) {
+            oc::sf_scatter_kernel<<<g, oc::SF_THREADS, 0, st>>>(da, ka, rank, n, o.rank_doc, o.doc_rank, val);
+            launched(c);
+            e = cudaGetLastError();
+        }
+        o.h_doc_rank.resize(nbits);
+        o.h_value.resize(o.n);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(o.h_doc_rank.data(), o.doc_rank, nbits * 4, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess && o.n) e = cudaMemcpyAsync(o.h_value.data(), val, o.n * 8, cudaMemcpyDeviceToHost, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess)
+            return bad(fail(e == cudaErrorMemoryAllocation ? OC_ERR_OOM : OC_ERR_CUDA, "sort field build: %s", cudaGetErrorString(e)));
+    }
+    return OC_OK;
+}
+
 extern "C" int oc_sort_field_create(oc_ctx *c, uint64_t nbits, uint64_t n, const uint64_t *doc_ids, const double *values,
                                     oc_sort_field **out) {
     if (!c || !out || nbits == 0 || (n && (!doc_ids || !values))) return fail(OC_ERR_INVALID, "bad arguments");
     if (nbits >= RANK_NONE) return fail(OC_ERR_INVALID, "nbits %llu >= 2^32 - 1", (unsigned long long)nbits);
-    std::vector<std::pair<double, uint64_t>> e;
-    e.reserve(n);
-    for (uint64_t i = 0; i < n; i++) {
+    for (uint64_t i = 0; i < n; i++)
         if (values[i] != values[i]) return fail(OC_ERR_INVALID, "sort value %llu is NaN", (unsigned long long)i);
-        if (doc_ids[i] < nbits) e.emplace_back(values[i] + 0.0, doc_ids[i]);   // -0.0 ties with 0.0
-    }
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (cudaSetDevice(c->device) != cudaSuccess) return fail(OC_ERR_CUDA, "cudaSetDevice failed");
     oc_sort_field *f = new oc_sort_field();
     f->ctx = c; f->nbits = nbits;
-    auto fail_free = [&](int code) { sort_field_free(f); return code; };
-    std::lock_guard<std::mutex> lk(c->mu);
-    if (cudaSetDevice(c->device) != cudaSuccess) return fail_free(fail(OC_ERR_CUDA, "cudaSetDevice failed"));
-    std::vector<uint64_t> rank_doc;
-    for (int ord = OC_SORT_ASC; ord <= OC_SORT_DESC; ord++) {
-        // value in the requested order, ties by ascending id; a document keeps its first position
-        std::sort(e.begin(), e.end(), [ord](const std::pair<double, uint64_t> &a, const std::pair<double, uint64_t> &b) {
-            if (a.first != b.first) return ord == OC_SORT_ASC ? a.first < b.first : a.first > b.first;
-            return a.second < b.second;
-        });
-        SortOrder &o = f->ord[ord];
-        o.h_doc_rank.assign(nbits, RANK_NONE);
-        rank_doc.clear();
-        for (const auto &x : e)
-            if (o.h_doc_rank[x.second] == RANK_NONE) {
-                o.h_doc_rank[x.second] = (uint32_t)rank_doc.size();
-                rank_doc.push_back(x.second);
-                o.h_value.push_back(x.first);
-            }
-        o.n = rank_doc.size();
-        const uint32_t none = RANK_NONE;
-        cudaError_t err = cudaMalloc(&o.rank_doc, std::max<size_t>(o.n, 1) * 8);
-        if (err == cudaSuccess) err = cudaMalloc(&o.doc_rank, nbits * 4);
-        if (err == cudaSuccess) err = cudaMalloc(&o.rank_row, (o.n + 1) * 4);
-        if (err == cudaSuccess && o.n) err = cudaMemcpy(o.rank_doc, rank_doc.data(), o.n * 8, cudaMemcpyHostToDevice);
-        if (err == cudaSuccess) err = cudaMemcpy(o.doc_rank, o.h_doc_rank.data(), nbits * 4, cudaMemcpyHostToDevice);
-        if (err == cudaSuccess) err = cudaMemcpy(o.rank_row + o.n, &none, 4, cudaMemcpyHostToDevice);
-        if (err != cudaSuccess)
-            return fail_free(fail(err == cudaErrorMemoryAllocation ? OC_ERR_OOM : OC_ERR_CUDA, "sort field upload: %s", cudaGetErrorString(err)));
-    }
+    SortBuildIn in;
+    in.n = n; in.h_docs = doc_ids; in.h_vals = values;
+    OCTRY(sort_field_build(c, in, f));
     *out = f;
+    return OC_OK;
+}
+
+extern "C" int oc_sort_field_from_facets(oc_facets *fs, uint32_t field, const double *variant_values, oc_sort_field **out) {
+    if (!fs || !out) return fail(OC_ERR_INVALID, "NULL argument");
+    oc_ctx *c = fs->ctx;
+    std::lock_guard<std::mutex> lk(c->mu);   // one whole published version: a commit publishes under this lock
+    if (field >= fs->fields.size()) return fail(OC_ERR_INVALID, "field %u: the store has %zu fields", field, fs->fields.size());
+    const FacetField &fl = fs->fields[field];
+    if (fl.number && variant_values) return fail(OC_ERR_INVALID, "field %u is a number field: variant_values must be NULL", field);
+    if (!fl.number && !variant_values) return fail(OC_ERR_INVALID, "field %u is a variant field: variant_values is NULL", field);
+    const uint32_t n_var = fl.number ? 0 : uint32_t(fl.offsets.size() - 1);
+    for (uint32_t v = 0; v < n_var; v++)
+        if (variant_values[v] != variant_values[v]) return fail(OC_ERR_INVALID, "variant %u: value is NaN", v);
+    if (fs->nbits >= RANK_NONE) return fail(OC_ERR_INVALID, "nbits %llu >= 2^32 - 1", (unsigned long long)fs->nbits);
+    if (cudaSetDevice(c->device) != cudaSuccess) return fail(OC_ERR_CUDA, "cudaSetDevice failed");
+    oc_sort_field *f = new oc_sort_field();
+    f->ctx = c; f->nbits = fs->nbits;
+    {
+        std::lock_guard<std::mutex> gp(fs->pend.mu);
+        f->facets_version = fs->pend.version;
+    }
+    SortBuildIn in;
+    in.n = fl.n_docs; in.d_docs = fl.docs;
+    if (fl.number) in.d_vals = fl.d_values;
+    else { in.off = &fl.offsets; in.var_vals = variant_values; }
+    OCTRY(sort_field_build(c, in, f));
+    *out = f;
+    return OC_OK;
+}
+
+extern "C" int oc_sort_field_read(const oc_sort_field *f, int order, uint64_t *nbits, uint64_t *n, uint64_t *rank_doc, double *rank_value,
+                                  uint64_t *facets_version) {
+    if (!f || !n) return fail(OC_ERR_INVALID, "NULL argument");
+    if (order != OC_SORT_ASC && order != OC_SORT_DESC) return fail(OC_ERR_INVALID, "sort order %d is neither ASC nor DESC", order);
+    const SortOrder &o = f->ord[order];
+    const uint64_t cap = *n;
+    *n = o.n;
+    if (nbits) *nbits = f->nbits;
+    if (facets_version) *facets_version = f->facets_version;
+    if (!rank_doc && !rank_value) return OC_OK;
+    if (cap < o.n) return fail(OC_ERR_INVALID, "arrays hold %llu entries, the order has %llu", (unsigned long long)cap, (unsigned long long)o.n);
+    if (rank_value) std::copy(o.h_value.begin(), o.h_value.end(), rank_value);
+    if (rank_doc && o.n) {
+        std::lock_guard<std::mutex> lk(f->ctx->mu);
+        CU(cudaSetDevice(f->ctx->device));
+        CU(cudaMemcpy(rank_doc, o.rank_doc, o.n * 8, cudaMemcpyDeviceToHost));
+    }
     return OC_OK;
 }
 

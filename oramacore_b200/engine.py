@@ -906,7 +906,8 @@ class SortField:
     """A number, date or bool filter field laid out for sortBy on the device (oc_sort_field_*): one (doc_id, value)
     entry per value, so a multi-valued document repeats.  kind "number": any real value; "date": millisecond
     timestamps (integers or numpy datetime64); "bool": False / True.  Integers beyond 2^53 and NaN are refused: the
-    values travel as doubles.  Immutable: build a new one when the field changes."""
+    values travel as doubles.  Immutable: build a new one when the field changes (from_facets builds one from a
+    FacetStore field on the device)."""
     KINDS = ("number", "date", "bool")
 
     def __init__(self, ctx: Context, nbits: int, doc_ids, values, kind: str):
@@ -933,6 +934,44 @@ class SortField:
         self._h = C.c_void_p()
         check(lib().oc_sort_field_create(ctx._h, self.nbits, d.shape[0], _p(d), _p(v), C.byref(self._h)))
 
+    @classmethod
+    def from_facets(cls, store: "FacetStore", name: str) -> "SortField":
+        """The sort field of field `name` of the store's published version, built on the device from the field's device
+        arrays (oc_sort_field_from_facets) over the version's nbits: a number or date field sorts by its values, a bool
+        field by true = 1.0, false = 0.0.  A string_filter field raises InvalidSortField(name, "StringFilter") before
+        any device call, as resolve_sort_by does, and a name the store does not hold SortFieldNotFound(name).  The
+        handle keeps the version it was built from: build a new one after the next commit() of the store."""
+        if name not in store.fields:
+            raise SortFieldNotFound(name)
+        f = store.fields[name]
+        vv = None
+        if f["kind"] == "string":
+            raise InvalidSortField(name, _NOT_SORTABLE["string_filter"])
+        if f["kind"] == "bool":
+            vv = np.zeros(len(f["keys"]), np.float64)
+            vv[f["variant"]["true"]] = 1.0
+        self = cls.__new__(cls)
+        self.ctx, self.kind = store.ctx, f["kind"]
+        self._h = C.c_void_p()
+        check(lib().oc_sort_field_from_facets(store._h, f["id"], _p(vv), C.byref(self._h)))
+        self.nbits = self._sizes()["nbits"]   # the version's, which a commit on another thread may have moved on from
+        return self
+
+    def _sizes(self, order: str = "ASC") -> dict:
+        """{"nbits", "n" (documents with a value), "facets_version"} of one order, without reading the arrays."""
+        nb, n, ver = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        check(lib().oc_sort_field_read(self._h, _order(order), C.byref(nb), C.byref(n), None, None, C.byref(ver)))
+        return {"nbits": int(nb.value), "n": int(n.value), "facets_version": int(ver.value)}
+
+    def read(self, order: str = "ASC") -> dict:
+        """One order read back (oc_sort_field_read): {"nbits", "rank_doc" (documents in rank order), "rank_value" (the
+        value each was placed by), "facets_version" (from_facets' store version, 0 for a handle built from values)}."""
+        sz = self._sizes(order)
+        d, v, n = np.zeros(sz["n"], np.uint64), np.zeros(sz["n"], np.float64), C.c_uint64(sz["n"])
+        if sz["n"]:
+            check(lib().oc_sort_field_read(self._h, _order(order), None, C.byref(n), _p(d), _p(v), None))
+        return {"nbits": sz["nbits"], "rank_doc": d, "rank_value": v, "facets_version": sz["facets_version"]}
+
     def close(self):
         if self._h:
             lib().oc_sort_field_destroy(self._h)
@@ -957,10 +996,14 @@ def resolve_sort_by(fields: Mapping[str, object], sort_by: SortBy) -> Tuple[Sort
     return f, sort_by.order
 
 
-def _sort(field: SortField, order: str = "ASC"):
+def _order(order: str) -> int:
     if order not in ("ASC", "DESC"):
         raise ValueError(f"sort order {order!r}: expected 'ASC' or 'DESC'")
-    return _lib.Sort(field._h, 0 if order == "ASC" else 1)
+    return 0 if order == "ASC" else 1
+
+
+def _sort(field: SortField, order: str = "ASC"):
+    return _lib.Sort(field._h, _order(order))
 
 
 def search_sorted_arrays(tsc: "TokenScoreContext", params: "TokenScoreParams", field: SortField, order: str = "ASC", promote=None,

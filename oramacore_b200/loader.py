@@ -19,7 +19,8 @@ oc_str_delete / oc_str_commit (snapshot swap: searches keep running on the previ
 the next), oc_emb_insert / oc_emb_delete (live) and oc_emb_compact at commit.  Filter values and deletes are queued on
 the facet store and the geopoint fields as apply() sees them (tests/filter_commit_spec.py states the per-kind rules as
 ops); `refresh_facets()` merges them into the next version of every field on the device (oc_facets_commit_ex,
-oc_geo_field_commit_ex), and `where_filter(where)` evaluates a where-clause over them (where.py).  No host copy of the
+oc_geo_field_commit_ex), `where_filter(where)` evaluates a where-clause over them (where.py), and `sort_by(SortBy)`
+sorts by a number, date or bool field of the published version (oc_sort_field_from_facets).  No host copy of the
 filter values is kept.  tf of a term = number of positions (exact + stemmed), as StringStorage counts them."""
 from __future__ import annotations
 
@@ -27,8 +28,9 @@ from typing import Dict, Iterable, List, Optional, Sequence
 
 import numpy as np
 
-from .engine import (Context, DeviceFilter, EmbeddingFieldStorage, FacetStore, GeoPointField, StringFieldStorage,
-                     TermDictionary, TokenScoreContext)
+from .engine import (Context, DeviceFilter, EmbeddingFieldStorage, FacetStore, GeoPointField, SortField, StringFieldStorage,
+                     TermDictionary, TokenScoreContext, resolve_sort_by)
+from .types import SortBy
 from .where import WhereFilter, WhereProgram, check_where_keys, compile_where, evaluate_where, parse_where
 
 _F64_INT_MAX = 1 << 53   # I64 values beyond +-2^53 would not survive the trip through a double
@@ -74,6 +76,7 @@ class IndexLoader:
         self.geo: Dict[str, GeoPointField] = {f: GeoPointField(ctx, self.nbits, [], [], []) for f in self._geo}
         self._live: Optional[DeviceFilter] = None              # NOT(uncommitted deletes) of where_program, built once
         self._retired: List[DeviceFilter] = []                 # earlier ones, which programs may still point at
+        self._sorts: Dict[str, SortField] = {}                 # sort fields of the published version, built when asked
 
     # ---- Index::update_data
     def apply(self, op: Dict) -> None:
@@ -193,6 +196,9 @@ class IndexLoader:
         for f in self._retired:   # programs built before now carry the earlier nbits
             f.close()
         self._retired = []
+        for f in self._sorts.values():   # the sorts of the previous version
+            f.close()
+        self._sorts = {}
         self.nbits = max(self.nbits, self.max_doc_id + 2)
         stats = {}
         if self.facets is not None:
@@ -228,6 +234,25 @@ class IndexLoader:
                 dele.close()
         return compile_where(w, self.facets, self.geo, self.nbits, self._live)
 
+    def sort_fields(self) -> Dict[str, object]:
+        """The mapping resolve_sort_by takes: every number, date and bool property to a SortField of the version the
+        last refresh_facets() / commit() published (built on the device the first time it is asked for after a
+        refresh), and every string, string_filter and geopoint property to its kind name.  Values queued since that
+        refresh do not move a sort.  A SortField is valid until the next refresh_facets() / commit(), which closes it."""
+        out: Dict[str, object] = {f: "string" for f in self.string_fields}
+        out.update({f: "string_filter" for f in self._strf})
+        out.update({f: "geopoint" for f in self._geo})
+        for f in self._bool + self._num + self._date:
+            if f not in self._sorts:
+                self._sorts[f] = SortField.from_facets(self.facets, f)
+            out[f] = self._sorts[f]
+        return out
+
+    def sort_by(self, sort_by: SortBy):
+        """resolve_sort_by over sort_fields(): the (SortField, order) pair the sorted searches take.  Raises
+        SortFieldNotFound / InvalidSortField as the reference does (read/index/sort.rs:186-265)."""
+        return resolve_sort_by(self.sort_fields(), sort_by)
+
     def _retire_live(self) -> None:
         if self._live is not None:
             self._retired.append(self._live)
@@ -242,6 +267,6 @@ class IndexLoader:
         return self.dict.resolve_batch(list(texts), ctx=self.ctx, **kw)
 
     def close(self):
-        for x in [self.facets, self.emb, self.strs, self.dict, self._live] + list(self.geo.values()) + self._retired:
+        for x in list(self._sorts.values()) + [self.facets, self.emb, self.strs, self.dict, self._live] + list(self.geo.values()) + self._retired:
             if x is not None:
                 x.close()

@@ -353,6 +353,10 @@ extern "C" {
     // sortBy (sort_token_scores / sort_groups with sort_by, MergeSortedIterator; sort.rs:17-201, 491-559)
     pub fn oc_sort_field_create(ctx: *mut OcCtx, nbits: u64, n: u64, doc_ids: *const u64, values: *const f64,
                                 out: *mut *mut OcSortField) -> c_int;
+    /// the sort field of one field of the facet store's published version, built on the device
+    pub fn oc_sort_field_from_facets(f: *mut OcFacets, field: u32, variant_values: *const f64, out: *mut *mut OcSortField) -> c_int;
+    pub fn oc_sort_field_read(f: *const OcSortField, order: c_int, nbits: *mut u64, n: *mut u64, rank_doc: *mut u64,
+                              rank_value: *mut f64, facets_version: *mut u64) -> c_int;
     pub fn oc_sort_field_destroy(f: *mut OcSortField);
     pub fn oc_search_sorted(ctx: *mut OcCtx, emb: *mut OcEmb, s: *mut OcStr, p: *const OcSearchParams, sort: *const OcSort,
                             pins: *const OcPins, out_doc_ids: *mut u64, out_scores: *mut f32, out_sort_values: *mut f64,
