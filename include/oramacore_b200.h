@@ -44,6 +44,7 @@ typedef struct oc_ctx oc_ctx;   /* one device + stream + workspace (one per proc
 typedef struct oc_emb oc_emb;   /* == one EmbeddingFieldStorage (embedding_field.rs:29-34) */
 typedef struct oc_str oc_str;   /* == the StringFieldStorage set of one Index (string_field.rs:32-36) */
 typedef struct oc_filter oc_filter; /* == a FilterResult<DocumentId> evaluated to a bitmap on the device (filter.rs:344-392) */
+typedef struct oc_omc oc_omc;   /* == the OMC map of one Index (omc_committed + its log, index/mod.rs:604-627, 1720-1739) */
 
 const char *oc_last_error(void);
 int oc_version(void);
@@ -264,6 +265,10 @@ typedef struct {
                                                   threshold and vector_limit (see below)                          */
     const struct oc_where *q_where;            /* NULL, or query b's where-clause as a program, evaluated inside the
                                                   call (see "where programs" below); same meaning as q_filters     */
+    const struct oc_omc *omc;                  /* NULL, or the index's OMC store (oc_omc_*): the call is byte for byte
+                                                  the call with omc_doc_ids / omc_mult / n_omc set to the store's
+                                                  published version, without a per-call upload; not together with
+                                                  n_omc != 0 (see "OMC store" below)                               */
 } oc_search_params;
 
 /* One query's scalar parameters (SearchParams, types.rs:1381-1409, with FulltextMode / VectorMode / HybridMode,
@@ -459,6 +464,45 @@ int oc_facets_commit_ex(oc_facets *f, uint64_t new_nbits, oc_filter_commit_t *ou
  * entries (the host copy: no device read), values (number fields) n_entries. */
 int oc_facets_read_field(oc_facets *f, uint32_t field, uint32_t *n_variants, uint64_t *n_entries, uint64_t *offsets, double *values,
                          uint64_t *doc_ids);
+
+/* ---- OMC store --------------------------------------------------------------------------------------
+ * The OMC ("Orama Custom Multiplier") map of one index (omc_committed, read/index/mod.rs:604-627, 1720-1739): a score
+ * multiplier per document, applied to every score map before count and top-N (read/search.rs:39-48, 340-343).  One
+ * handle per index, on one ctx.  The published version lives on the device as doc[n] (strictly ascending) and
+ * mult[n]; a search with oc_search_params.omc = the handle reads it there.
+ *   - oc_omc_set queues (doc_ids[i], mults[i]) entries, oc_omc_delete queues removals.  Both apply in call order at the
+ *     next commit; the last op for a document wins.  Values: any finite f32 (as the array path takes them); NaN and
+ *     +-inf are refused with OC_ERR_INVALID and nothing of the call is queued.  The store does not drop zero or
+ *     negative values: the reference's write side does that before it emits Index2 (write/index/mod.rs:451-458).
+ *   - oc_omc_commit_ex merges the queue into the next version on the device, with no host copy of the map: the ops
+ *     are radix-sorted by (document, call order), the last op per document is kept, and one pass merges them with the
+ *     previous version.  The merge runs on the handle's own stream outside the ctx lock; the next version is published
+ *     under the ctx lock once the ctx stream has drained, so a search holds one whole version, old or new.  A commit
+ *     with no queued op publishes the same entries under the next version number.  Statistics in oc_filter_commit_t:
+ *     rows_kept (committed entries kept as they were), rows_dropped (committed entries deleted or replaced), rows_added
+ *     (entries written from the queue).  Workspace, freed before the call returns: about 30 B per queued op plus 8 B
+ *     per committed entry and the CUB sort and scan storage.  Limit: fewer than 2^31 - 1 committed + queued entries.
+ *     OC_ERR_INVALID, changing nothing and keeping every op queued: a commit of the handle already in flight;
+ *     OC_ERR_OOM: no room for the workspace or the next version.
+ *   - oc_omc_read reads the published version back.  With doc_ids and mults NULL it returns the size in *n; otherwise
+ *     *n is their capacity on entry (too small: OC_ERR_INVALID after writing the size).  version (may be NULL): 0
+ *     before the first commit, then the number the last commit published.
+ * Searches: every search entry point (oc_search, oc_search_facets, oc_search_groups*, oc_search_pinned,
+ * oc_search_sorted, the q_* calls and the sharded search) takes p->omc.  The ids, score bits, n, count, sort values, pin
+ * outputs, group rows and facet counts are byte for byte those of the same call with omc_doc_ids / omc_mult / n_omc set
+ * to the version oc_omc_read returns.  The tile scorers read the version's documents as string rows: the first search
+ * after a commit of the handle or an oc_str_commit of its string store builds that list on the device and keeps it on
+ * the handle (one device-to-host copy of its length, the only synchronisation this adds); other searches do no host
+ * work and no upload for OMC.  OC_ERR_INVALID, nothing written: p->omc together with n_omc != 0, a handle of another
+ * ctx.  Sharded searches: the shard merge applies the multipliers to every rank's candidates, so each rank's handle
+ * must hold the whole index's map (a caller contract, as for the replicated df tables; not verified).
+ * oc_omc_destroy: no search or commit of the handle may be in flight. */
+int oc_omc_create(oc_ctx *ctx, oc_omc **out);
+void oc_omc_destroy(oc_omc *omc);
+int oc_omc_set(oc_omc *omc, const uint64_t *doc_ids, const float *mults, uint64_t n);
+int oc_omc_delete(oc_omc *omc, const uint64_t *doc_ids, uint64_t n);
+int oc_omc_commit_ex(oc_omc *omc, oc_filter_commit_t *out);
+int oc_omc_read(oc_omc *omc, uint64_t *n, uint64_t *doc_ids, float *mults, uint64_t *version);
 
 /* where-filter leaves over a filter field of a facet store (read/index/filter.rs:49-124); the leaf's nbits is the store's.
  * An ordinary oc_filter over the facets' ctx, for oc_filter_and / or / not and any search.  A document is in a leaf

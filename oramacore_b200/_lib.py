@@ -49,6 +49,7 @@ EXPORTED_SYMBOLS = [
     "oc_facets_create", "oc_facets_destroy", "oc_facets_add_field", "oc_facets_add_number_field", "oc_search_facets",
     "oc_facets_insert_variants", "oc_facets_add_variant", "oc_facets_insert_numbers", "oc_facets_clear", "oc_facets_delete",
     "oc_facets_commit_ex", "oc_facets_read_field",
+    "oc_omc_create", "oc_omc_destroy", "oc_omc_set", "oc_omc_delete", "oc_omc_commit_ex", "oc_omc_read",
     "oc_filter_facet_variant", "oc_filter_facet_range", "oc_where_check", "oc_filter_from_where",
     "oc_group_by_create", "oc_group_by_destroy", "oc_search_groups",
     "oc_search_pinned", "oc_search_groups_pinned", "oc_merge_pinned",
@@ -110,7 +111,7 @@ class SearchParams(C.Structure):
                 ("filter_bits", C.c_void_p), ("filter_nbits", C.c_uint64),
                 ("omc_doc_ids", C.c_void_p), ("omc_mult", C.c_void_p), ("n_omc", C.c_uint64),
                 ("sharded", C.c_int), ("vector_limit", C.c_uint32), ("filter", C.c_void_p),
-                ("q_filters", C.c_void_p), ("q_params", C.c_void_p), ("q_where", C.c_void_p)]
+                ("q_filters", C.c_void_p), ("q_params", C.c_void_p), ("q_where", C.c_void_p), ("omc", C.c_void_p)]
 
 
 class QueryParams(C.Structure):   # oc_query_params: one entry of SearchParams.q_params
@@ -266,6 +267,13 @@ def lib():
     L.oc_facets_delete.argtypes = [vp, u64, vp]
     L.oc_facets_commit_ex.argtypes = [vp, u64, C.POINTER(FilterCommit)]
     L.oc_facets_read_field.argtypes = [vp, u32, C.POINTER(u32), C.POINTER(u64), vp, vp, vp]
+    L.oc_omc_create.argtypes = [vp, C.POINTER(vp)]
+    L.oc_omc_destroy.argtypes = [vp]
+    L.oc_omc_destroy.restype = None
+    L.oc_omc_set.argtypes = [vp, vp, vp, u64]
+    L.oc_omc_delete.argtypes = [vp, vp, u64]
+    L.oc_omc_commit_ex.argtypes = [vp, C.POINTER(FilterCommit)]
+    L.oc_omc_read.argtypes = [vp, C.POINTER(u64), vp, vp, C.POINTER(u64)]
     L.oc_geo_field_insert.argtypes = [vp, u64, vp, vp, vp]
     L.oc_geo_field_delete.argtypes = [vp, u64, vp]
     L.oc_geo_field_commit_ex.argtypes = [vp, u64, C.POINTER(FilterCommit)]

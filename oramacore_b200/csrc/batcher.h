@@ -5,8 +5,8 @@
 // first submitter of a group becomes its leader, waits up to max_wait_us (or until max_batch requests are in), merges
 // the group into ONE Call, runs it through the executor (the library's entry points, a fake in
 // tests/batcher_test.cpp) and scatters each request's outputs back.  A group shares the parameter tuple (mode, limit,
-// offset, similarity, threshold, bm25_k, bm25_b, vector_limit) and a class: flat (PLAIN and SORTED requests), GROUPED,
-// or FACETED on one facet store.  A merged flat call runs as PLAIN unless a request has a sort field or an item; a
+// offset, similarity, threshold, bm25_k, bm25_b, vector_limit), a class: flat (PLAIN and SORTED requests), GROUPED,
+// or FACETED on one facet store, and the OMC store (p->omc, or none).  A merged flat call runs as PLAIN unless a request has a sort field or an item; a
 // merged grouped call runs at the largest need of its requests as the group stride.  Each request's p->filter becomes
 // its q_filters entry.  A request the merged call could not take (batchable and the *_batchable predicates) runs
 // directly, alone; one the library would refuse for its own arguments is refused before it joins.  A merged grouped or
@@ -86,11 +86,12 @@ struct BatchKey {
     // mixed batcher: the scalars above are 0; the route flags and the OMC arrays take their place
     bool thr, deep;
     const uint64_t *omc_doc; const float *omc_mult; uint64_t n_omc;
+    const oc_omc *omc;                   // both batchers: requests batch only on the same OMC store (or none)
     bool operator==(const BatchKey &o) const {
         return mode == o.mode && limit == o.limit && offset == o.offset && vector_limit == o.vector_limit && cls == o.cls &&
                facets == o.facets && memcmp(&similarity, &o.similarity, 4) == 0 && memcmp(&threshold, &o.threshold, 4) == 0 &&
                memcmp(&k, &o.k, 4) == 0 && memcmp(&b, &o.b, 4) == 0 && thr == o.thr && deep == o.deep && omc_doc == o.omc_doc &&
-               omc_mult == o.omc_mult && n_omc == o.n_omc;
+               omc_mult == o.omc_mult && n_omc == o.n_omc && omc == o.omc;
     }
 };
 // The vector depth of a query alone (0 without a vector part): vector_limit, else limit.
@@ -103,9 +104,9 @@ inline BatchKey key_of(const Call &c, bool mixed = false) {
     if (mixed)
         return BatchKey{0, 0, 0, 0.f, 0.f, p->bm25_k, p->bm25_b, 0, cls, c.facets,
                         p->mode != OC_MODE_VECTOR && p->threshold >= 0.0f, vector_depth(p) > TC_MAX_DEPTH,
-                        p->n_omc ? p->omc_doc_ids : nullptr, p->n_omc ? p->omc_mult : nullptr, p->n_omc};
+                        p->n_omc ? p->omc_doc_ids : nullptr, p->n_omc ? p->omc_mult : nullptr, p->n_omc, p->omc};
     return BatchKey{p->mode, p->limit, p->offset, p->similarity, p->threshold, p->bm25_k, p->bm25_b, p->vector_limit,
-                    cls, c.facets, false, false, nullptr, nullptr, 0};
+                    cls, c.facets, false, false, nullptr, nullptr, 0, p->omc};
 }
 // has_emb / has_str: the stores the batcher was created with.  A call that oc_search would reject
 // (unknown mode, missing store, NULL query arrays) is NOT batchable: it goes straight to the
@@ -116,6 +117,7 @@ inline BatchKey key_of(const Call &c, bool mixed = false) {
 inline bool batchable(const oc_search_params *p, bool has_emb = true, bool has_str = true, bool mixed = false) {
     if (p->n_queries != 1 || p->filter_bits || p->q_filters || p->q_params || (p->n_omc != 0 && !mixed) || p->sharded) return false;
     if (p->q_where && p->filter) return false;
+    if (p->omc && p->n_omc) return false;   // refused by the library: alone, so only this request fails
     if (mixed && (uint64_t(p->limit) + p->offset > OC_MAX_TOPK || (p->limit && (p->vector_limit ? p->vector_limit : p->limit) > OC_MAX_TOPK)))
         return false;
     if (mixed && p->n_omc && (!p->omc_doc_ids || !p->omc_mult)) return false;

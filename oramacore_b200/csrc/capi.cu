@@ -40,6 +40,7 @@
 #include "pins.cuh"
 #include "sort.cuh"
 #include "sort_build.cuh"
+#include "omc.cuh"
 #include "tmap.cuh"
 #include "where.cuh"
 #include "oramacore_b200.h"
@@ -2390,6 +2391,259 @@ static int sort_rows_for(oc_ctx *c, SortOrder &o, const std::shared_ptr<StrSnap>
 static int run_groups(oc_ctx *c, const GroupJob &gj, int mode, const StrSnap *S, uint32_t n_tiles, uint32_t vlimit,
                       const uint64_t *omc_doc, const float *omc_mult, uint32_t n_omc, const PinJob &pj, const QueryPlan *q_plan);
 
+// ------------------------------------------------------------------------------------ OMC store (omc.cuh)
+// The published version is replaced only by a commit, under the ctx lock once the ctx stream has drained; every search
+// reads it under the ctx lock.  The queue is guarded by `mu`.  The row-list cache belongs to the searches (ctx lock).
+struct oc_omc {
+    oc_ctx *ctx = nullptr;
+    uint64_t *doc = nullptr;               // device: the published version, doc ascending
+    float *mult = nullptr;
+    uint64_t n = 0, version = 0;
+    std::mutex mu;
+    bool committing = false;
+    std::vector<uint64_t> q_doc;           // the queue, in call order
+    std::vector<float> q_mult;
+    std::vector<uint8_t> q_del;
+    cudaStream_t stream = nullptr;         // the commit's merge
+    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    // the tile scorers' list of the version's string rows, ascending, for (rows_version, rows_snap): a cache the
+    // searches (which see the handle as const) build on their own stream
+    mutable cudaStream_t rows_stream = nullptr;
+    mutable uint64_t rows_version = 0, rows_snap = 0;   // rows_snap: StrSnap::ident (0: none built)
+    mutable uint32_t n_rows = 0;
+    mutable uint64_t rows_cap = 0;
+    mutable uint32_t *row = nullptr;
+    mutable float *row_mult = nullptr;
+};
+
+extern "C" int oc_omc_create(oc_ctx *c, oc_omc **out) {
+    if (!c || !out) return fail(OC_ERR_INVALID, "NULL argument");
+    oc_omc *o = new oc_omc();
+    o->ctx = c;
+    *out = o;
+    return OC_OK;
+}
+extern "C" void oc_omc_destroy(oc_omc *o) {
+    if (!o) return;
+    {
+        std::lock_guard<std::mutex> g(o->ctx->mu);
+        cudaSetDevice(o->ctx->device);
+        cudaStreamSynchronize(o->ctx->stream);
+        if (o->stream) { cudaStreamSynchronize(o->stream); cudaStreamDestroy(o->stream); }
+        if (o->rows_stream) { cudaStreamSynchronize(o->rows_stream); cudaStreamDestroy(o->rows_stream); }
+        for (cudaEvent_t e : o->ev) if (e) cudaEventDestroy(e);
+        cudaFree(o->doc); cudaFree(o->mult); cudaFree(o->row); cudaFree(o->row_mult);
+    }
+    delete o;
+}
+extern "C" int oc_omc_set(oc_omc *o, const uint64_t *doc_ids, const float *mults, uint64_t n) {
+    if (!o || (n && (!doc_ids || !mults))) return fail(OC_ERR_INVALID, "NULL argument");
+    for (uint64_t i = 0; i < n; i++)
+        if (!std::isfinite(mults[i])) return fail(OC_ERR_INVALID, "entry %llu: multiplier is not finite", (unsigned long long)i);
+    std::lock_guard<std::mutex> g(o->mu);
+    o->q_doc.insert(o->q_doc.end(), doc_ids, doc_ids + n);
+    o->q_mult.insert(o->q_mult.end(), mults, mults + n);
+    o->q_del.insert(o->q_del.end(), n, uint8_t(0));
+    return OC_OK;
+}
+extern "C" int oc_omc_delete(oc_omc *o, const uint64_t *doc_ids, uint64_t n) {
+    if (!o || (n && !doc_ids)) return fail(OC_ERR_INVALID, "NULL argument");
+    std::lock_guard<std::mutex> g(o->mu);
+    o->q_doc.insert(o->q_doc.end(), doc_ids, doc_ids + n);
+    o->q_mult.insert(o->q_mult.end(), n, 0.f);
+    o->q_del.insert(o->q_del.end(), n, uint8_t(1));
+    return OC_OK;
+}
+
+// The merge of the n_b queued ops into the version (a_doc, a_mult, n_a), on `st` (omc.cuh).  Two device phases timed by
+// ev[0..1] (upload .. scans) and ev[2..3] (scatter).
+struct OmcMergeOut { uint64_t n = 0, kept = 0, added = 0, ws = 0; float device_ms = 0; uint64_t *doc = nullptr; float *mult = nullptr; };
+static int omc_merge(cudaStream_t st, cudaEvent_t *ev, const uint64_t *a_doc, const float *a_mult, uint64_t n_a,
+                     const std::vector<uint64_t> &q_doc, const std::vector<float> &q_mult, const std::vector<uint8_t> &q_del,
+                     OmcMergeOut &o) {
+    const uint64_t n_b = q_doc.size();
+    if (n_a + n_b >= uint64_t(INT32_MAX)) return fail(OC_ERR_UNSUPPORTED, "OMC commit: %llu entries >= 2^31 - 1",
+                                                      (unsigned long long)(n_a + n_b));   // cub counts in int
+    size_t sort_b = 0, scan_a = 0, scan_b = 0;
+    if (cub::DeviceRadixSort::SortPairs(nullptr, sort_b, (const uint64_t *)nullptr, (uint64_t *)nullptr, (const uint32_t *)nullptr,
+                                        (uint32_t *)nullptr, (int)n_b, 0, 64, st) != cudaSuccess ||
+        cub::DeviceScan::ExclusiveSum(nullptr, scan_a, (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)(n_a + 1), st) != cudaSuccess ||
+        cub::DeviceScan::ExclusiveSum(nullptr, scan_b, (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)(n_b + 1), st) != cudaSuccess)
+        return fail(OC_ERR_CUDA, "OMC commit: temp storage size");
+    // workspace: [uploaded: q_doc | q_mult | q_del | idx] [b_doc | b_idx | a_keep | a_rank | b_keep | b_rank | temp]
+    auto al = [](size_t x) { return (x + 255) & ~size_t(255); };
+    const size_t o_qd = 0, o_qm = o_qd + al(n_b * 8), o_qx = o_qm + al(n_b * 4), o_ix = o_qx + al(n_b), up = o_ix + al(n_b * 4);
+    const size_t o_bd = up, o_bi = o_bd + al(n_b * 8), o_ak = o_bi + al(n_b * 4), o_ar = o_ak + al((n_a + 1) * 4),
+                 o_bk = o_ar + al((n_a + 1) * 4), o_br = o_bk + al((n_b + 1) * 4), o_tmp = o_br + al((n_b + 1) * 4),
+                 total = o_tmp + al(std::max(sort_b, std::max(scan_a, scan_b)));
+    std::vector<uint8_t> h(up, 0);
+    memcpy(h.data() + o_qd, q_doc.data(), n_b * 8);
+    memcpy(h.data() + o_qm, q_mult.data(), n_b * 4);
+    memcpy(h.data() + o_qx, q_del.data(), n_b);
+    uint32_t *idx = reinterpret_cast<uint32_t *>(h.data() + o_ix);
+    for (uint64_t i = 0; i < n_b; i++) idx[i] = uint32_t(i);
+    uint8_t *w = nullptr;
+    if (cudaMallocAsync(&w, total, st) != cudaSuccess) return fail(OC_ERR_OOM, "OMC commit: %zu B of workspace", total);
+    o.ws = total;
+    auto done = [&](int r) { cudaFreeAsync(w, st); if (r != OC_OK) { cudaFree(o.doc); cudaFree(o.mult); o.doc = nullptr; o.mult = nullptr; } return r; };
+    const uint64_t *qd = reinterpret_cast<const uint64_t *>(w + o_qd);
+    const float *qm = reinterpret_cast<const float *>(w + o_qm);
+    const uint8_t *qx = w + o_qx;
+    const uint32_t *ix = reinterpret_cast<const uint32_t *>(w + o_ix);
+    uint64_t *bd = reinterpret_cast<uint64_t *>(w + o_bd);
+    uint32_t *bi = reinterpret_cast<uint32_t *>(w + o_bi), *ak = reinterpret_cast<uint32_t *>(w + o_ak);
+    uint32_t *ar = reinterpret_cast<uint32_t *>(w + o_ar), *bk = reinterpret_cast<uint32_t *>(w + o_bk);
+    uint32_t *br = reinterpret_cast<uint32_t *>(w + o_br);
+    const uint64_t n_max = std::max(n_a, n_b) + 1;
+    cudaError_t e = cudaMemcpyAsync(w, h.data(), up, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaEventRecord(ev[0], st);
+    // stable: each document's ops keep their call order
+    if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(w + o_tmp, sort_b, qd, bd, ix, bi, (int)n_b, 0, 64, st);
+    if (e == cudaSuccess) {
+        om_keep_kernel<<<(unsigned)((n_max + OM_THREADS - 1) / OM_THREADS), OM_THREADS, 0, st>>>(a_doc, n_a, bd, bi, qx, n_b, ak, bk);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(w + o_tmp, scan_a, ak, ar, (int)(n_a + 1), st);
+    if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(w + o_tmp, scan_b, bk, br, (int)(n_b + 1), st);
+    uint32_t tot[2] = {0, 0};
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&tot[0], ar + n_a, 4, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaEventRecord(ev[1], st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&tot[1], br + n_b, 4, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e == cudaSuccess) e = cudaEventElapsedTime(&o.device_ms, ev[0], ev[1]);
+    if (e != cudaSuccess) return done(fail(OC_ERR_CUDA, "OMC commit: %s", cudaGetErrorString(e)));
+    o.kept = tot[0]; o.added = tot[1]; o.n = o.kept + o.added;
+    if (o.n && (e = cudaMalloc(&o.doc, o.n * 8)) == cudaSuccess) e = cudaMalloc(&o.mult, o.n * 4);
+    if (e != cudaSuccess) return done(fail(e == cudaErrorMemoryAllocation ? OC_ERR_OOM : OC_ERR_CUDA, "OMC commit: %llu entries: %s",
+                                          (unsigned long long)o.n, cudaGetErrorString(e)));
+    e = cudaEventRecord(ev[2], st);
+    if (e == cudaSuccess && o.n) {
+        if (n_a) om_scatter_a_kernel<<<(unsigned)((n_a + OM_THREADS - 1) / OM_THREADS), OM_THREADS, 0, st>>>(a_doc, a_mult, n_a, ar, bd, n_b, br, o.doc, o.mult);
+        om_scatter_b_kernel<<<(unsigned)((n_b + OM_THREADS - 1) / OM_THREADS), OM_THREADS, 0, st>>>(bd, bi, qm, n_b, br, a_doc, n_a, ar, o.doc, o.mult);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaEventRecord(ev[3], st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    float ms2 = 0;
+    if (e == cudaSuccess) e = cudaEventElapsedTime(&ms2, ev[2], ev[3]);
+    o.device_ms += ms2;
+    return done(e == cudaSuccess ? OC_OK : fail(OC_ERR_CUDA, "OMC commit: %s", cudaGetErrorString(e)));
+}
+
+extern "C" int oc_omc_commit_ex(oc_omc *o, oc_filter_commit_t *out) {
+    if (!o) return fail(OC_ERR_INVALID, "NULL argument");
+    const auto wall0 = std::chrono::steady_clock::now();
+    oc_ctx *c = o->ctx;
+    std::vector<uint64_t> q_doc;
+    std::vector<float> q_mult;
+    std::vector<uint8_t> q_del;
+    {
+        std::lock_guard<std::mutex> g(o->mu);
+        if (o->committing) return fail(OC_ERR_INVALID, "a commit of this handle is already in flight");
+        if (cudaSetDevice(c->device) != cudaSuccess) return fail(OC_ERR_CUDA, "cudaSetDevice failed");
+        if (!o->stream) {
+            CU(cudaStreamCreateWithFlags(&o->stream, cudaStreamNonBlocking));
+            for (cudaEvent_t &e : o->ev) CU(cudaEventCreate(&e));
+        }
+        o->committing = true;
+        q_doc = o->q_doc; q_mult = o->q_mult; q_del = o->q_del;
+    }
+    // the published version is replaced only by a commit, so it is read without the ctx lock
+    oc_filter_commit_t st{};
+    OmcMergeOut res;
+    int rc = OC_OK;
+    if (!q_doc.empty()) {
+        rc = omc_merge(o->stream, o->ev, o->doc, o->mult, o->n, q_doc, q_mult, q_del, res);
+        st.device_ms = res.device_ms; st.workspace_bytes = res.ws;
+        st.rows_kept = res.kept; st.rows_dropped = o->n - res.kept; st.rows_added = res.added;
+    } else {
+        st.rows_kept = o->n;
+    }
+    if (rc != OC_OK) {
+        std::lock_guard<std::mutex> g(o->mu);
+        o->committing = false;
+        return rc;
+    }
+    {   // publish: every reader holds the ctx lock and works on the ctx stream (see oc_facets_commit_ex)
+        std::lock_guard<std::mutex> g(c->mu);
+        cudaSetDevice(c->device);
+        if (!q_doc.empty()) {
+            cudaStreamSynchronize(c->stream);
+            cudaFree(o->doc); cudaFree(o->mult);
+            o->doc = res.doc; o->mult = res.mult; o->n = res.n;
+        }
+        std::lock_guard<std::mutex> gq(o->mu);
+        o->q_doc.erase(o->q_doc.begin(), o->q_doc.begin() + q_doc.size());
+        o->q_mult.erase(o->q_mult.begin(), o->q_mult.begin() + q_doc.size());
+        o->q_del.erase(o->q_del.begin(), o->q_del.begin() + q_doc.size());
+        o->committing = false;
+        st.version = ++o->version;
+    }
+    st.wall_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - wall0).count();
+    if (out) *out = st;
+    return OC_OK;
+}
+
+extern "C" int oc_omc_read(oc_omc *o, uint64_t *n, uint64_t *doc_ids, float *mults, uint64_t *version) {
+    if (!o || !n) return fail(OC_ERR_INVALID, "NULL argument");
+    oc_ctx *c = o->ctx;
+    std::lock_guard<std::mutex> g(c->mu);
+    const uint64_t cap = *n;
+    *n = o->n;
+    if (version) *version = o->version;
+    if (!doc_ids && !mults) return OC_OK;
+    if (cap < o->n) return fail(OC_ERR_INVALID, "capacity %llu < %llu entries", (unsigned long long)cap, (unsigned long long)o->n);
+    CU(cudaSetDevice(c->device));
+    if (o->n && doc_ids) CU(cudaMemcpy(doc_ids, o->doc, o->n * 8, cudaMemcpyDeviceToHost));
+    if (o->n && mults) CU(cudaMemcpy(mults, o->mult, o->n * 4, cudaMemcpyDeviceToHost));
+    return OC_OK;
+}
+
+// The tile scorers' row list of the published version over snapshot S, built on the device when the version or the
+// snapshot changed since the last build (under the ctx lock).  Ends with the list's length on the host.
+static int omc_rows_for(oc_ctx *c, const oc_omc *o, const StrSnap *S) {
+    if (o->rows_snap == S->ident && o->rows_version == o->version) return OC_OK;
+    const uint64_t n = o->n;
+    o->n_rows = 0;
+    o->rows_snap = 0;
+    if (n) {
+        if (!o->rows_stream) CU(cudaStreamCreateWithFlags(&o->rows_stream, cudaStreamNonBlocking));
+        cudaStream_t st = o->rows_stream;
+        if (n > o->rows_cap) {
+            cudaFree(o->row); cudaFree(o->row_mult);
+            o->row = nullptr; o->row_mult = nullptr; o->rows_cap = 0;
+            CU(cudaMalloc(&o->row, n * 4));
+            CU(cudaMalloc(&o->row_mult, n * 4));
+            o->rows_cap = n;
+        }
+        size_t scan = 0;
+        CU(cub::DeviceScan::ExclusiveSum(nullptr, scan, (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)(n + 1), st));
+        auto al = [](size_t x) { return (x + 255) & ~size_t(255); };
+        const size_t o_has = al(n * 4), o_pos = o_has + al((n + 1) * 4), o_tmp = o_pos + al((n + 1) * 4), total = o_tmp + al(scan);
+        uint8_t *w = nullptr;
+        if (cudaMallocAsync(&w, total, st) != cudaSuccess) return fail(OC_ERR_OOM, "OMC rows: %zu B of workspace", total);
+        uint32_t *row = reinterpret_cast<uint32_t *>(w), *has = reinterpret_cast<uint32_t *>(w + o_has);
+        uint32_t *pos = reinterpret_cast<uint32_t *>(w + o_pos);
+        om_rows_kernel<<<(unsigned)((n + OM_THREADS) / OM_THREADS), OM_THREADS, 0, st>>>(o->doc, n, S->row_doc, S->n_rows, row, has);
+        launched(c);
+        cudaError_t e = cudaGetLastError();
+        if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(w + o_tmp, scan, has, pos, (int)(n + 1), st);
+        if (e == cudaSuccess) {
+            om_rows_scatter_kernel<<<(unsigned)((n + OM_THREADS - 1) / OM_THREADS), OM_THREADS, 0, st>>>(row, o->mult, n, pos, o->row, o->row_mult);
+            launched(c);
+            e = cudaGetLastError();
+        }
+        uint32_t cnt = 0;
+        if (e == cudaSuccess) e = cudaMemcpyAsync(&cnt, pos + n, 4, cudaMemcpyDeviceToHost, st);
+        cudaFreeAsync(w, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) return fail(OC_ERR_CUDA, "OMC rows: %s", cudaGetErrorString(e));
+        o->n_rows = cnt;
+    }
+    o->rows_snap = S->ident; o->rows_version = o->version;
+    return OC_OK;
+}
+
 // One search as an entry point asks for it.  fj: the facet counts.  gj: the grouped calls (always with pj); then
 // limit == 0 is allowed: the hits are not written (out_doc_ids / out_scores / out_n may be NULL), the vector stage gets
 // depth 0 and the fulltext stage runs with one candidate slot per tile.  pj: the pinned calls.  sj: the sorted calls
@@ -2464,11 +2718,17 @@ struct SearchCall {
     std::vector<uint8_t> tok_need_df;
     std::vector<PreDesc> pre_descs;
     std::vector<uint2> pre_items;
-    // OMC rows for the tile kernel (string rows, ascending)
-    uint32_t n_omc = 0;
+    // OMC: the documents and multipliers K4, the shard merge, groups and pins read (n_omc entries), and the tile
+    // kernel's string rows, ascending (n_omc_rows).  Array path: uploaded with the call; store path (p->omc): the
+    // version's device arrays and the handle's row list
+    uint32_t n_omc = 0, n_omc_rows = 0;
     bool omc_tile = false;
     std::vector<uint32_t> omc_rows;
     std::vector<float> omc_row_mult;
+    const uint64_t *omc_doc = nullptr;
+    const float *omc_mult = nullptr;
+    const uint32_t *omc_row_dev = nullptr;
+    const float *omc_row_mult_dev = nullptr;
     // sortBy entries and per-query walks, group handles and spans
     std::vector<SortEntry> s_ents;
     std::vector<SortQuery> s_q;
@@ -2616,6 +2876,8 @@ static int search_check(SearchCall &k) {
     if (!c || !p || !r.out_count) return fail(OC_ERR_INVALID, "NULL argument");
     k.write_hits = !(r.gj || (r.fj && r.fj->hits_optional)) || p->limit > 0;
     if (k.write_hits && (!r.out_doc_ids || !r.out_scores || !r.out_n)) return fail(OC_ERR_INVALID, "NULL argument");
+    if (p->omc && p->n_omc) return fail(OC_ERR_INVALID, "omc together with omc_doc_ids / omc_mult / n_omc");
+    if (p->omc && p->omc->ctx != c) return fail(OC_ERR_INVALID, "omc belongs to another ctx");
     const uint32_t B = k.B = p->n_queries;
     k.qp = p->q_params != nullptr;
     if (k.qp && !r.q_params_ok)
@@ -3098,6 +3360,16 @@ static int ft_share(SearchCall &k) {
 // OMC rows for the tile kernel: the documents' string rows, ascending
 static int omc_plan(SearchCall &k) {
     const oc_search_params *p = k.p; const StrSnap *S = k.S;
+    if (const oc_omc *o = p->omc) {   // the published version (replaced only under the ctx lock this call holds)
+        k.n_omc = (uint32_t)o->n;
+        k.omc_doc = o->doc; k.omc_mult = o->mult;
+        if (k.n_omc && k.has_ft) {
+            OCTRY(omc_rows_for(k.c, o, S));
+            k.n_omc_rows = o->n_rows; k.omc_row_dev = o->row; k.omc_row_mult_dev = o->row_mult;
+        }
+        k.omc_tile = k.n_omc_rows > 0;
+        return OC_OK;
+    }
     const uint32_t n_omc = k.n_omc = (uint32_t)p->n_omc;
     if (n_omc && (!p->omc_doc_ids || !p->omc_mult)) return fail(OC_ERR_INVALID, "omc arrays are NULL");
     if (n_omc && k.has_ft) {
@@ -3113,7 +3385,8 @@ static int omc_plan(SearchCall &k) {
             k.omc_rows.push_back((uint32_t)r); k.omc_row_mult.push_back(p->omc_mult[i]);
         }
     }
-    k.omc_tile = !k.omc_rows.empty();
+    k.n_omc_rows = (uint32_t)k.omc_rows.size();
+    k.omc_tile = k.n_omc_rows > 0;
     return OC_OK;
 }
 
@@ -3175,11 +3448,11 @@ static int main_upload(SearchCall &k) {
     if (!k.pre_descs.empty()) k.s_pre = pk.add(k.pre_descs.data(), k.pre_descs.size());
     if (!k.pre_items.empty()) k.s_pitems = pk.add(k.pre_items.data(), k.pre_items.size());
     if (k.has_ft) k.s_queries = pk.add(k.queries.data(), k.queries.size());
-    if (k.n_omc) {
+    if (k.n_omc && !p->omc) {
         k.s_omcd = pk.add(p->omc_doc_ids, k.n_omc);
         k.s_omcm = pk.add(p->omc_mult, k.n_omc);
     }
-    if (k.omc_tile) {
+    if (k.omc_tile && !p->omc) {
         k.s_omcr = pk.add(k.omc_rows.data(), k.omc_rows.size());
         k.s_omcrm = pk.add(k.omc_row_mult.data(), k.omc_row_mult.size());
     }
@@ -3335,9 +3608,9 @@ static int bm25_stage(SearchCall &k) {
     bp.k = p->bm25_k; bp.b = p->bm25_b;
     bp.row_ok_bits = k.row_ok;
     if (k.per_q) { bp.q_ok_slot = k.qfj.d_q_slot_ft; bp.ok_words = ok_words; }
-    bp.omc_row = k.s_omcr.at(din);
-    bp.omc_mult = k.s_omcrm.at(din);
-    bp.n_omc = (uint32_t)k.omc_rows.size();
+    bp.omc_row = p->omc ? k.omc_row_dev : k.s_omcr.at(din);
+    bp.omc_mult = p->omc ? k.omc_row_mult_dev : k.s_omcrm.at(din);
+    bp.n_omc = k.n_omc_rows;
     bp.v_row = nullptr;            // the hybrid lookups are point lookups (bm25_point_kernel)
     bp.v_stride = k.vlimit;
     bp.v_ft = nullptr; bp.v_present = nullptr;
@@ -3560,8 +3833,8 @@ static int device_tail(SearchCall &k) {
         fp.v_ft = c->v_ft.as<float>(); fp.v_present = c->v_present.as<uint8_t>();
     }
     fp.v_stride = vlimit;
-    fp.omc_doc = k.s_omcd.at(c->in_blob);
-    fp.omc_mult = k.s_omcm.at(c->in_blob);
+    fp.omc_doc = p->omc ? k.omc_doc : k.s_omcd.at(c->in_blob);
+    fp.omc_mult = p->omc ? k.omc_mult : k.s_omcm.at(c->in_blob);
     fp.n_omc = k.n_omc;
     fp.out_doc = k.d_doc; fp.out_score = k.d_score; fp.out_n = k.d_n;
     fp.out_count = reinterpret_cast<unsigned long long *>(k.dout + k.o_cnt);

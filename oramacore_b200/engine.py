@@ -685,6 +685,52 @@ class FacetStore:
             self._h = None
 
 
+class OmcStore:
+    """The OMC map of one Index (omc_committed + its log, index/mod.rs:604-627, 1720-1739) kept on the device
+    (oc_omc_*): a score multiplier per document, applied to every score map before count and top-N (search.rs:39-48).
+    set() / delete() queue ops, which apply in call order at the next commit(); the last op for a document wins.  Pass
+    the store as TokenScoreParams.omc_store: a search reads the published version on the device, with the results of
+    the same search given that version as omc_doc_ids / omc_mult."""
+
+    def __init__(self, ctx: Context):
+        self.ctx = ctx
+        self._h = C.c_void_p()
+        check(lib().oc_omc_create(ctx._h, C.byref(self._h)))
+
+    def set(self, doc_ids, mults):
+        """Queue (doc_ids[i], mults[i]).  Any finite f32 is taken; NaN or +-inf raises and queues nothing."""
+        d = np.ascontiguousarray(doc_ids, np.uint64).reshape(-1)
+        m = np.ascontiguousarray(mults, np.float32).reshape(-1)
+        if d.shape != m.shape:
+            raise ValueError(f"{d.shape[0]} doc_ids for {m.shape[0]} multipliers")
+        check(lib().oc_omc_set(self._h, _p(d), _p(m), d.shape[0]))
+
+    def delete(self, doc_ids):
+        """Queue the removal of the documents' multipliers."""
+        d = np.ascontiguousarray(doc_ids, np.uint64).reshape(-1)
+        check(lib().oc_omc_delete(self._h, _p(d), d.shape[0]))
+
+    def commit(self) -> dict:
+        """Merge the queued ops into the next version on the device (oc_omc_commit_ex).  Returns the call's
+        statistics (oc_filter_commit_t)."""
+        st = _lib.FilterCommit()
+        check(lib().oc_omc_commit_ex(self._h, C.byref(st)))
+        return st.as_dict()
+
+    def read(self):
+        """The published version: (doc_ids ascending, multipliers, version number)."""
+        n, ver = C.c_uint64(0), C.c_uint64(0)
+        check(lib().oc_omc_read(self._h, C.byref(n), None, None, C.byref(ver)))
+        d, m = np.zeros(n.value, np.uint64), np.zeros(n.value, np.float32)
+        check(lib().oc_omc_read(self._h, C.byref(n), _p(d), _p(m), C.byref(ver)))
+        return d, m, int(ver.value)
+
+    def close(self):
+        if self._h:
+            lib().oc_omc_destroy(self._h)
+            self._h = None
+
+
 def _number_label(x) -> str:
     return str(int(x)) if np.isfinite(x) and float(x) == int(x) else repr(float(x))
 
@@ -1418,6 +1464,9 @@ class TokenScoreParams:
     vector_limit: int = 0            # 0 => limit_hint (search.rs:330-336); see oc_search_params.vector_limit
     omc_doc_ids: Optional[np.ndarray] = None   # ascending
     omc_mult: Optional[np.ndarray] = None
+    # the index's OMC map on the device (oc_search_params.omc): the same results as omc_doc_ids / omc_mult set to its
+    # published version (OmcStore.read); not together with them
+    omc_store: Optional["OmcStore"] = None
     sharded: bool = False
     shard_tombstones: bool = False   # OC_SHARD_TOMBSTONES: some rank's string store holds uncommitted deletes
     shard_count_df: bool = False     # OC_SHARD_COUNT_DF: some rank's store lacks the corpus-wide df tables
@@ -1529,6 +1578,9 @@ class TokenScoreContext:
             om = np.ascontiguousarray(params.omc_mult, np.float32)
             keep += [od, om]
             sp.omc_doc_ids, sp.omc_mult, sp.n_omc = _p(od), _p(om), od.shape[0]
+        if params.omc_store is not None:
+            keep.append(params.omc_store)
+            sp.omc = params.omc_store._h
         sp.sharded = (1 | (2 if params.shard_tombstones else 0) | (4 if params.shard_count_df else 0)) if params.sharded else 0
         return sp, keep, B
 
@@ -1550,7 +1602,8 @@ class SearchBatcher:
     coalesces concurrent calls that share (mode, limit, offset, similarity, threshold) into one
     batched oc_search.  A request's device_filter (its where-filter) travels with it into the batch as
     that query's own filter, so filtered and unfiltered requests are coalesced together; requests with
-    filtered_doc_ids (a host bitmap), OMC multipliers or sharding run as their own oc_search.  ctypes
+    filtered_doc_ids (a host bitmap), OMC arrays or sharding run as their own oc_search.  Requests with the
+    same omc_store batch together (in both batchers).  ctypes
     releases the GIL while a caller is blocked in the library.
     mixed=True (OC_BATCHER_MIXED): calls that differ in mode, limit, offset, similarity, threshold or vector_limit
     share a batch too (each request's scalars become its q_params entry), and so do calls with the same OMC arrays;

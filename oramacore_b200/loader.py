@@ -8,6 +8,8 @@ The reference's read side is fed by `Index::update_data(IndexWriteOperation)` (r
       FilterGeoPoint2(field, Plain(point) | Array([points]))  -> the geopoint fields of the where-filter (mod.rs:1556-1565, 1678-1687)
       FilterBool2 / FilterString2 / FilterDate / FilterDate2 / FilterNumber2 -> the same filter fields as the write side
                                               emits them today (write/index/fields.rs:312-325, 345-353, 401-423, 467-504)
+  * `Index2 { doc_id, indexed_values, omc }` — what the write side emits today (write/index/mod.rs:451-472): `Index`,
+      and `omc` (when not None) appended to the index's OMC log (mod.rs:1566-1580)
   * `IndexEmbedding { data: field -> [(doc_id, vectors)] }` -> EmbeddingFieldStorage::insert (mod.rs:1688-1698)
   * `DeleteDocuments { doc_ids }` — `document_count -= len(doc_ids)` (saturating), uncommitted deletes, excluded
       from every search at once (mod.rs:1346-1427)
@@ -21,15 +23,17 @@ the facet store and the geopoint fields as apply() sees them (tests/filter_commi
 ops); `refresh_facets()` merges them into the next version of every field on the device (oc_facets_commit_ex,
 oc_geo_field_commit_ex), `where_filter(where)` evaluates a where-clause over them (where.py), and `sort_by(SortBy)`
 sorts by a number, date or bool field of the published version (oc_sort_field_from_facets).  No host copy of the
-filter values is kept.  tf of a term = number of positions (exact + stemmed), as StringStorage counts them."""
+filter values is kept.  OMC multipliers go to a device-resident OmcStore: `omc()` publishes the ones applied so far
+(get_all_omc, mod.rs:1720-1739: visible before a commit), and `commit()` also removes the uncommitted deletes' entries
+(mod.rs:604-627).  tf of a term = number of positions (exact + stemmed), as StringStorage counts them."""
 from __future__ import annotations
 
 from typing import Dict, Iterable, List, Optional, Sequence
 
 import numpy as np
 
-from .engine import (Context, DeviceFilter, EmbeddingFieldStorage, FacetStore, GeoPointField, SortField, StringFieldStorage,
-                     TermDictionary, TokenScoreContext, resolve_sort_by)
+from .engine import (Context, DeviceFilter, EmbeddingFieldStorage, FacetStore, GeoPointField, OmcStore, SortField,
+                     StringFieldStorage, TermDictionary, TokenScoreContext, resolve_sort_by)
 from .types import SortBy
 from .where import WhereFilter, WhereProgram, check_where_keys, compile_where, evaluate_where, parse_where
 
@@ -77,13 +81,22 @@ class IndexLoader:
         self._live: Optional[DeviceFilter] = None              # NOT(uncommitted deletes) of where_program, built once
         self._retired: List[DeviceFilter] = []                 # earlier ones, which programs may still point at
         self._sorts: Dict[str, SortField] = {}                 # sort fields of the published version, built when asked
+        self.omc_store = OmcStore(ctx)                         # the OMC map; sets queue in _omc_log until omc() / commit()
+        self._omc_log: List[tuple] = []
 
     # ---- Index::update_data
     def apply(self, op: Dict) -> None:
         kind = op["type"]
-        if kind == "Index":
+        if kind in ("Index", "Index2"):
             d = int(op["doc_id"])
+            omc = op.get("omc") if kind == "Index2" else None
+            if omc is not None:
+                omc = np.float32(omc)
+                if not np.isfinite(omc):
+                    raise ValueError(f"document {d}: omc {op['omc']!r} is not a finite f32")
             self.document_count += 1                            # mod.rs:1460
+            if omc is not None:                                 # the uncommitted OMC log (mod.rs:1573-1579)
+                self._omc_log.append((d, omc))
             self.max_doc_id = max(self.max_doc_id, d)
             if d in self._uncommitted_deleted:
                 self._uncommitted_deleted.discard(d)
@@ -184,8 +197,26 @@ class IndexLoader:
         if self.emb is not None:
             self.emb.compact()
         self._push_count()
+        # mod.rs:604-627: the log merges into the committed map, then the uncommitted deletes leave it
+        self._publish_omc(sorted(self._uncommitted_deleted))
         self._uncommitted_deleted.clear()
         self.refresh_facets()
+
+    def omc(self) -> OmcStore:
+        """The OMC store with every multiplier applied so far published (get_all_omc, mod.rs:1720-1739: the log over
+        the committed map, last writer wins), for TokenScoreParams.omc_store.  Deletes leave the map at commit()."""
+        self._publish_omc([])
+        return self.omc_store
+
+    def _publish_omc(self, deleted: List[int]) -> None:
+        if not self._omc_log and not deleted:
+            return
+        if self._omc_log:
+            self.omc_store.set([d for d, _ in self._omc_log], [m for _, m in self._omc_log])
+        if deleted:
+            self.omc_store.delete(deleted)
+        self.omc_store.commit()
+        self._omc_log = []
 
     def refresh_facets(self) -> dict:
         """Publish every filter value applied so far over DocumentId [0, max_doc_id + 2): the queued values and deletes
@@ -267,6 +298,6 @@ class IndexLoader:
         return self.dict.resolve_batch(list(texts), ctx=self.ctx, **kw)
 
     def close(self):
-        for x in list(self._sorts.values()) + [self.facets, self.emb, self.strs, self.dict, self._live] + list(self.geo.values()) + self._retired:
+        for x in list(self._sorts.values()) + [self.facets, self.emb, self.strs, self.dict, self._live, self.omc_store] + list(self.geo.values()) + self._retired:
             if x is not None:
                 x.close()

@@ -17,6 +17,7 @@ use std::ffi::{c_char, c_int, c_void, CStr};
 #[repr(C)] pub struct OcGroupBy { _p: [u8; 0] }
 #[repr(C)] pub struct OcSortField { _p: [u8; 0] }
 #[repr(C)] pub struct OcGeoField { _p: [u8; 0] }
+#[repr(C)] pub struct OcOmc { _p: [u8; 0] }
 #[repr(C)] pub struct OcDict { _p: [u8; 0] }
 #[repr(C)] pub struct OcResolved { _p: [u8; 0] }
 
@@ -114,6 +115,8 @@ pub struct OcSearchParams {
     pub q_params: *const OcQueryParams,     // NULL, or B entries: query b's own mode / limit / offset / similarity /
                                             // threshold / vector_limit; `limit` is then the hit arrays' row stride
     pub q_where: *const OcWhere,            // NULL, or each query's where-clause as a program, evaluated in the call
+    pub omc: *const OcOmc,                  // NULL, or the index's OMC store: the published version, read on the device
+                                            // (not together with n_omc != 0)
 }
 
 /// Where-program node ops (oc_where_node.op) and bounds.
@@ -319,6 +322,13 @@ extern "C" {
     pub fn oc_facets_read_field(f: *mut OcFacets, field: u32, n_variants: *mut u32, n_entries: *mut u64, offsets: *mut u64,
                                 values: *mut f64, doc_ids: *mut u64) -> c_int;
     pub fn oc_facets_add_number_field(f: *mut OcFacets, n: u64, values_sorted: *const f64, doc_ids: *const u64, out_field: *mut u32) -> c_int;
+    // the OMC map of an index (index/mod.rs:604-627, 1720-1739): queued sets / deletes, committed on the device
+    pub fn oc_omc_create(ctx: *mut OcCtx, out: *mut *mut OcOmc) -> c_int;
+    pub fn oc_omc_destroy(omc: *mut OcOmc);
+    pub fn oc_omc_set(omc: *mut OcOmc, doc_ids: *const u64, mults: *const f32, n: u64) -> c_int;
+    pub fn oc_omc_delete(omc: *mut OcOmc, doc_ids: *const u64, n: u64) -> c_int;
+    pub fn oc_omc_commit_ex(omc: *mut OcOmc, out: *mut OcFilterCommit) -> c_int;
+    pub fn oc_omc_read(omc: *mut OcOmc, n: *mut u64, doc_ids: *mut u64, mults: *mut f32, version: *mut u64) -> c_int;
     // where-filter leaves over a filter field (filter.rs:49-124): a variant's documents, or a number field's value interval
     pub fn oc_filter_facet_variant(f: *const OcFacets, field: u32, variant: u32, out: *mut *mut OcFilter) -> c_int;
     pub fn oc_filter_facet_range(f: *const OcFacets, field: u32, lo: f64, hi: f64, flags: u32, out: *mut *mut OcFilter) -> c_int;
