@@ -329,7 +329,10 @@ int oc_search(oc_ctx *ctx, oc_emb *emb, oc_str *str, const oc_search_params *p,
  * [0, nbits) that lives on the device: build the leaves from id lists, combine with And / Or / Not (word-wise
  * kernels), hand the handle to any number of oc_search / oc_search_facets calls (no per-call upload).
  * execute_filter's own rule — AND the where-filter with NOT(uncommitted deletes) — is oc_filter_and +
- * oc_filter_not over an id leaf of the deleted documents. */
+ * oc_filter_not over an id leaf of the deleted documents.
+ * oc_filter_and(a, b) is oc_filter_from_where (below) of the program {FILTER a, FILTER b, AND 2} over a's nbits,
+ * oc_filter_or the same with OR 2, and oc_filter_not(a) that of {FILTER a, NOT}: a handle of another ctx, or b of
+ * another nbits than a, is refused with OC_ERR_INVALID and nothing is created. */
 int oc_filter_from_ids(oc_ctx *ctx, const uint64_t *doc_ids, uint64_t n, uint64_t nbits, oc_filter **out);  /* PlainFilterResult::from_iter; ids >= nbits ignored */
 int oc_filter_from_bits(oc_ctx *ctx, const uint64_t *bits, uint64_t nbits, oc_filter **out);
 int oc_filter_and(const oc_filter *a, const oc_filter *b, oc_filter **out);   /* FilterResult::And */
@@ -346,7 +349,8 @@ void oc_filter_destroy(oc_filter *f);
  * GeoPointFieldStorage::filter (read/index/geopoint_field.rs:179-229) for Filter::GeoPoint (read/index/filter.rs:125-139):
  * the documents of a geopoint field with a point inside (or outside) a radius or a polygon, as an ordinary oc_filter
  * over [0, nbits) of the field's ctx that combines with oc_filter_and / or / not and goes to any search as p->filter.
- * Every query is one scan of the field's points on the device.
+ * Each call is oc_filter_from_where (below) of a program of one OC_WHERE_GEO_RADIUS / OC_WHERE_GEO_POLYGON node over the
+ * field's nbits: one scan of the field's points on the device.
  *   - Coordinates: degrees, latitude in [-90, 90], longitude in [-180, 180], both finite (FieldsGeoPoint::new refuses
  *     anything else).  The reference widens its f32 API values to f64; the caller does the same before calling here.
  *   - A field holds (document, point) entries; a document may have several points (GeoPointIndexedValue::Array).  A
@@ -506,9 +510,9 @@ int oc_omc_read(oc_omc *omc, uint64_t *n, uint64_t *doc_ids, float *mults, uint6
 
 /* where-filter leaves over a filter field of a facet store (read/index/filter.rs:49-124); the leaf's nbits is the store's.
  * An ordinary oc_filter over the facets' ctx, for oc_filter_and / or / not and any search.  A document is in a leaf
- * when AT LEAST ONE of its values passes.  The slice of the field is found by a binary search of the host copy of
- * its values, then the device slice is scattered into a fresh bitmap: nothing is copied from the host, and an empty
- * slice launches nothing.  Ids >= nbits are ignored.
+ * when AT LEAST ONE of its values passes.  Each call is oc_filter_from_where (below) of a program of one
+ * OC_WHERE_VARIANT / OC_WHERE_RANGE node over the store's nbits: the slice of the field is found by a binary search of
+ * the host copy of its values, then the device slice is scattered into a zeroed bitmap.  Ids >= nbits are ignored.
  *   - oc_filter_facet_variant: the documents of variant `variant` of a bool or string_filter field (bool_field.rs:163-166,
  *     string_filter_field.rs:165-167).  Bool variants are 0 = true, 1 = false; a string_filter variant is one key.
  *   - oc_filter_facet_range: the documents of a number field with a value v in the interval [lo, hi], compared as
@@ -528,30 +532,34 @@ int oc_filter_facet_variant(const oc_facets *f, uint32_t field, uint32_t variant
 int oc_filter_facet_range(const oc_facets *f, uint32_t field, double lo, double hi, uint32_t flags, oc_filter **out);
 
 /* ---- where programs ------------------------------------------------------------------------------
- * A where-clause as a postfix program over the leaves above, evaluated inside a search call (oc_search_params.q_where)
- * instead of through one oc_filter_* call per leaf and per And / Or / Not.  Query b's program is
+ * A where-clause as a postfix program, evaluated inside a search call (oc_search_params.q_where) or into a handle
+ * (oc_filter_from_where, which every leaf call above and oc_filter_and / or / not use).  Query b's program is
  * nodes[q_node_offsets[b] .. q_node_offsets[b + 1]); an empty range leaves the query unfiltered.  Each node pushes one
  * bitmap over [0, nbits) or combines the top of the stack:
  *   OC_WHERE_NONE         the empty set
- *   OC_WHERE_VARIANT      oc_filter_facet_variant(src = oc_facets *, field, arg = variant)
- *   OC_WHERE_RANGE        oc_filter_facet_range(src = oc_facets *, field, a = lo, b = hi, arg = OC_RANGE_* flags)
- *   OC_WHERE_GEO_RADIUS   oc_filter_geo_radius(src = oc_geo_field *, a = lat, b = lon, c = radius_m, arg = inside)
- *   OC_WHERE_GEO_POLYGON  oc_filter_geo_polygon(src = oc_geo_field *, vertex_lat / vertex_lon [first_vertex ..
- *                         first_vertex + n_vertices), arg = inside)
+ *   OC_WHERE_VARIANT      src = oc_facets *: the documents of variant arg of the store's bool / string_filter field
+ *   OC_WHERE_RANGE        src = oc_facets *: the documents of the store's number field with a value in [a, b], an end
+ *                         open under the OC_RANGE_* flags in arg (the rules of oc_filter_facet_range above)
+ *   OC_WHERE_GEO_RADIUS   src = oc_geo_field *: the documents with a point within c = radius_m metres of (a = lat,
+ *                         b = lon), or with arg = inside = 0 a point beyond it (geometry: "geopoint where-filter leaves")
+ *   OC_WHERE_GEO_POLYGON  src = oc_geo_field *: the documents with a point inside the polygon of vertices vertex_lat /
+ *                         vertex_lon [first_vertex .. first_vertex + n_vertices), or with arg = inside = 0 outside it
  *   OC_WHERE_FILTER       an existing handle (src = oc_filter *), e.g. NOT(uncommitted deletes), built once per commit
  *   OC_WHERE_AND / OR     pops arg >= 2 values, pushes their And / Or
- *   OC_WHERE_NOT          pops one value, pushes its complement within [0, nbits) (as oc_filter_not)
+ *   OC_WHERE_NOT          pops one value, pushes its complement within [0, nbits)
  * A program ends with exactly one value on the stack.  Query b's outputs are byte for byte those it gets with
- * q_filters[b] = the handle that oc_filter_* build from the same leaves and combinators.
+ * q_filters[b] = oc_filter_from_where of its program.
  * Cost: the call plans on the host (identical leaves and identical programs of the batch are evaluated once; variant and
  * range leaves are resolved to document slices by binary search), then a fixed number of launches on the call's stream:
  * one scatter for every facet leaf, one for every geo leaf, one evaluation of every program, and no synchronise.  The
  * leaf and result bitmaps live in a ctx workspace of (distinct leaves + distinct programs) x nbits / 8 bytes (a program
  * of one leaf or one FILTER takes no result bitmap), kept between calls; OC_ERR_OOM when it cannot be allocated.
- * Checks (OC_ERR_INVALID unless noted; a refused call writes nothing): every check of the leaf call the node stands
- * for; a store or handle of another ctx; a store, or a handle combined with other values, whose nbits differs from
- * oc_where.nbits (a program of one FILTER node takes the handle as it is, as a q_filters entry would); an unknown op;
- * stack underflow; a program that does not end with one value; an arity below 2; more than OC_WHERE_MAX_NODES nodes or
+ * Checks (OC_ERR_INVALID unless noted; a refused call writes nothing): a NULL store or handle; a field or variant out
+ * of range, a VARIANT node on a number field or a RANGE node on a bool / string_filter field, a NaN range bound,
+ * unknown flag bits; invalid coordinates, a radius that is NaN, infinite or negative, fewer than 3 or more than
+ * OC_GEO_MAX_VERTICES vertices, NULL vertex arrays under a polygon; a store or handle of another ctx; a store, or a
+ * handle combined with other values, whose nbits differs from oc_where.nbits (a program of one FILTER node takes the
+ * handle as it is, as a q_filters entry would); an unknown op; stack underflow; a program that does not end with one value; an arity below 2; more than OC_WHERE_MAX_NODES nodes or
  * a stack deeper than OC_WHERE_MAX_DEPTH in one program; q_where together with filter, filter_bits or q_filters.
  * Entry points: those that take q_filters take q_where (a query with a program counts as filtered there); those that
  * refuse q_filters refuse q_where with the same code; a sharded call refuses it with OC_ERR_UNSUPPORTED. */

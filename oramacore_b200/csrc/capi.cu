@@ -1766,14 +1766,6 @@ __global__ void filter_scatter_ids_kernel(const uint64_t *ids, uint64_t n, uint6
     const uint64_t d = ids[i];
     if (d < nbits) atomicOr(bits + (d >> 6), 1ull << (d & 63));
 }
-// op: 0 and, 1 or, 2 not(a); the padding bits of the last word stay clear
-__global__ void filter_combine_kernel(const uint64_t *a, const uint64_t *b, uint64_t words, uint64_t nbits, int op, uint64_t *out) {
-    const uint64_t w = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-    if (w >= words) return;
-    uint64_t v = op == 0 ? (a[w] & b[w]) : op == 1 ? (a[w] | b[w]) : ~a[w];
-    if (w == words - 1 && (nbits & 63)) v &= (1ull << (nbits & 63)) - 1;
-    out[w] = v;
-}
 __global__ void filter_popcount_kernel(const uint64_t *a, uint64_t words, unsigned long long *out) {
     uint64_t c = 0;
     for (uint64_t w = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; w < words; w += uint64_t(gridDim.x) * blockDim.x) c += __popcll(a[w]);
@@ -1825,26 +1817,6 @@ extern "C" int oc_filter_from_bits(oc_ctx *c, const uint64_t *bits, uint64_t nbi
     *out = f;
     return OC_OK;
 }
-static int filter_combine(const oc_filter *a, const oc_filter *b, int op, oc_filter **out) {
-    if (!a || !out || (op != 2 && !b)) return fail(OC_ERR_INVALID, "NULL argument");
-    if (b && (b->ctx != a->ctx || b->nbits != a->nbits)) return fail(OC_ERR_INVALID, "filters of different contexts / sizes");
-    oc_ctx *c = a->ctx;
-    std::lock_guard<std::mutex> g(c->mu);
-    CU(cudaSetDevice(c->device));
-    oc_filter *f = nullptr;
-    OCTRY(filter_alloc(c, a->nbits, &f));
-    if (f->words) {
-        filter_combine_kernel<<<(unsigned)((f->words + 255) / 256), 256, 0, c->stream>>>(a->bits, b ? b->bits : nullptr, f->words, f->nbits, op, f->bits);
-        launched(c);
-        CU(cudaGetLastError());
-        CU(cudaStreamSynchronize(c->stream));
-    }
-    *out = f;
-    return OC_OK;
-}
-extern "C" int oc_filter_and(const oc_filter *a, const oc_filter *b, oc_filter **out) { return filter_combine(a, b, 0, out); }
-extern "C" int oc_filter_or(const oc_filter *a, const oc_filter *b, oc_filter **out) { return filter_combine(a, b, 1, out); }
-extern "C" int oc_filter_not(const oc_filter *a, oc_filter **out) { return filter_combine(a, nullptr, 2, out); }
 extern "C" int oc_filter_count(const oc_filter *f, uint64_t *out) {
     if (!f || !out) return fail(OC_ERR_INVALID, "NULL argument");
     oc_ctx *c = f->ctx;
@@ -4501,65 +4473,6 @@ extern "C" int oc_facets_read_field(oc_facets *f, uint32_t field, uint32_t *n_va
     return OC_OK;
 }
 
-// where-filter leaves over a filter field (read/index/filter.rs:49-124).  A leaf is one slice [lo, hi) of the field's
-// device document array, found on the host by `slice` (called under the ctx lock), scattered into a zeroed bitmap by
-// filter_scatter_ids_kernel: nothing is copied from the host and an empty slice launches nothing.
-template <typename F>
-static int facet_leaf(const oc_facets *f, uint32_t field, bool number, oc_filter **out, F &&slice) {
-    oc_ctx *c = f->ctx;
-    std::lock_guard<std::mutex> g(c->mu);
-    if (field >= f->fields.size()) return fail(OC_ERR_INVALID, "field %u: the store has %zu fields", field, f->fields.size());
-    const FacetField &fl = f->fields[field];
-    if (fl.number != number)
-        return fail(OC_ERR_INVALID, "field %u is a %s field", field, fl.number ? "number" : "bool / string_filter");
-    uint64_t lo = 0, hi = 0;
-    OCTRY(slice(fl, lo, hi));
-    CU(cudaSetDevice(c->device));
-    oc_filter *r = nullptr;
-    OCTRY(filter_alloc(c, f->nbits, &r));
-    cudaError_t e = cudaMemsetAsync(r->bits, 0, std::max<uint64_t>(r->words, 1) * 8, c->stream);
-    if (e == cudaSuccess && hi > lo) {
-        filter_scatter_ids_kernel<<<(unsigned)((hi - lo + 255) / 256), 256, 0, c->stream>>>(
-            fl.docs + lo, hi - lo, f->nbits, reinterpret_cast<unsigned long long *>(r->bits));
-        launched(c);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess) {
-        cudaFree(r->bits);
-        delete r;
-        return fail(OC_ERR_CUDA, "facet filter: %s", cudaGetErrorString(e));
-    }
-    *out = r;
-    return OC_OK;
-}
-
-extern "C" int oc_filter_facet_variant(const oc_facets *f, uint32_t field, uint32_t variant, oc_filter **out) {
-    if (!f || !out) return fail(OC_ERR_INVALID, "NULL argument");
-    return facet_leaf(f, field, false, out, [&](const FacetField &fl, uint64_t &lo, uint64_t &hi) {
-        if (variant + uint64_t(1) >= fl.offsets.size())
-            return fail(OC_ERR_INVALID, "variant %u: field %u has %zu variants", variant, field, fl.offsets.size() - 1);
-        lo = fl.offsets[variant];
-        hi = fl.offsets[variant + 1];
-        return int(OC_OK);
-    });
-}
-
-extern "C" int oc_filter_facet_range(const oc_facets *f, uint32_t field, double lo, double hi, uint32_t flags, oc_filter **out) {
-    if (!f || !out) return fail(OC_ERR_INVALID, "NULL argument");
-    if (std::isnan(lo) || std::isnan(hi)) return fail(OC_ERR_INVALID, "NaN range bound");
-    if (flags & ~(OC_RANGE_LO_OPEN | OC_RANGE_HI_OPEN)) return fail(OC_ERR_INVALID, "unknown range flags 0x%x", flags);
-    return facet_leaf(f, field, true, out, [&](const FacetField &fl, uint64_t &a, uint64_t &b) {
-        const auto &v = fl.values;   // ascending, no NaN
-        a = (flags & OC_RANGE_LO_OPEN) ? std::upper_bound(v.begin(), v.end(), lo) - v.begin()
-                                       : std::lower_bound(v.begin(), v.end(), lo) - v.begin();
-        b = (flags & OC_RANGE_HI_OPEN) ? std::lower_bound(v.begin(), v.end(), hi) - v.begin()
-                                       : std::upper_bound(v.begin(), v.end(), hi) - v.begin();
-        b = std::max(a, b);   // lo > hi: empty
-        return int(OC_OK);
-    });
-}
-
 // row bitmap -> DocumentId bitmap when rows are not document ids
 __global__ void facet_rows_to_docs_kernel(const uint32_t *row_bits, uint64_t row_stride_words, const uint64_t *row_doc, uint64_t n_rows,
                                           uint32_t *doc_bits, uint64_t doc_stride_words, uint64_t nbits) {
@@ -4629,19 +4542,32 @@ __global__ void __launch_bounds__(256) facet_slice_count_kernel(const FacetSlice
     }
 }
 
+// The slice [lo, hi) of a field's device documents that a where leaf or a facet count selects: variant `arg` of a bool /
+// string_filter field, or the values v of a number field with a <= v <= b, an end open under the OC_RANGE_* flags in
+// `arg` (a > b: empty).  False: the field has no variant `arg`.
+static bool facet_slice(const FacetField &fl, uint32_t arg, double a, double b, uint64_t &lo, uint64_t &hi) {
+    if (!fl.number) {
+        if (arg + uint64_t(1) >= fl.offsets.size()) return false;
+        lo = fl.offsets[arg]; hi = fl.offsets[arg + 1];
+        return true;
+    }
+    const auto &v = fl.values;   // ascending, no NaN
+    lo = (arg & OC_RANGE_LO_OPEN) ? std::upper_bound(v.begin(), v.end(), a) - v.begin()
+                                  : std::lower_bound(v.begin(), v.end(), a) - v.begin();
+    hi = (arg & OC_RANGE_HI_OPEN) ? std::lower_bound(v.begin(), v.end(), b) - v.begin()
+                                  : std::upper_bound(v.begin(), v.end(), b) - v.begin();
+    hi = std::max(lo, hi);
+    return true;
+}
+
 // A request's slice [lo, hi) of its field's device documents.  nan: refuse a NaN bound (oc_search_facets passes it on).
 static int facet_resolve(const oc_facets *fc, const oc_facet_req &rq, size_t i, bool nan, uint64_t &lo, uint64_t &hi) {
     if (rq.field >= fc->fields.size()) return fail(OC_ERR_INVALID, "facet request %zu: unknown field %u", i, rq.field);
     const FacetField &fl = fc->fields[rq.field];
-    if (fl.number) {   // NumberFilter::Between = inclusive on both ends (number_field.rs:376, 604-631)
-        if (nan && (std::isnan(rq.from) || std::isnan(rq.to))) return fail(OC_ERR_INVALID, "facet request %zu: NaN range bound", i);
-        lo = uint64_t(std::lower_bound(fl.values.begin(), fl.values.end(), rq.from) - fl.values.begin());
-        hi = uint64_t(std::upper_bound(fl.values.begin(), fl.values.end(), rq.to) - fl.values.begin());
-        if (hi < lo) hi = lo;
-    } else {
-        if (rq.variant + uint64_t(1) >= fl.offsets.size()) return fail(OC_ERR_INVALID, "facet request %zu: unknown variant %u", i, rq.variant);
-        lo = fl.offsets[rq.variant]; hi = fl.offsets[rq.variant + 1];
-    }
+    if (fl.number && nan && (std::isnan(rq.from) || std::isnan(rq.to))) return fail(OC_ERR_INVALID, "facet request %zu: NaN range bound", i);
+    // flags 0: NumberFilter::Between is inclusive on both ends (number_field.rs:376, 604-631)
+    if (!facet_slice(fl, fl.number ? 0 : rq.variant, rq.from, rq.to, lo, hi))
+        return fail(OC_ERR_INVALID, "facet request %zu: unknown variant %u", i, rq.variant);
     return OC_OK;
 }
 
@@ -5546,65 +5472,6 @@ extern "C" int oc_geo_field_read(oc_geo_field *g, uint64_t *n, uint64_t *doc_ids
     return OC_OK;
 }
 
-// a zeroed leaf over [0, nbits) of g's ctx, filled by `launch` (called under the ctx lock when g has points)
-template <typename F>
-static int geo_leaf(const oc_geo_field *g, oc_filter **out, F &&launch) {
-    oc_ctx *c = g->ctx;
-    std::lock_guard<std::mutex> lk(c->mu);
-    CU(cudaSetDevice(c->device));
-    oc_filter *f = nullptr;
-    OCTRY(filter_alloc(c, g->nbits, &f));
-    auto fail_free = [&](int code) { cudaFree(f->bits); delete f; return code; };
-    cudaError_t e = cudaMemsetAsync(f->bits, 0, std::max<uint64_t>(f->words, 1) * 8, c->stream);
-    if (e == cudaSuccess && g->n) {
-        const int r = launch(c, reinterpret_cast<unsigned long long *>(f->bits),
-                             (unsigned)std::min<uint64_t>((g->n + GEO_THREADS - 1) / GEO_THREADS, uint64_t(c->prop.multiProcessorCount) * 8));
-        if (r != OC_OK) return fail_free(r);
-        launched(c);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess) return fail_free(fail(OC_ERR_CUDA, "geo filter: %s", cudaGetErrorString(e)));
-    *out = f;
-    return OC_OK;
-}
-
-extern "C" int oc_filter_geo_radius(const oc_geo_field *g, double lat, double lon, double radius_m, int inside, oc_filter **out) {
-    if (!g || !out) return fail(OC_ERR_INVALID, "NULL argument");
-    if (!geo_valid(lat, lon)) return fail(OC_ERR_INVALID, "radius centre: invalid coordinates (%g, %g)", lat, lon);
-    if (!(std::isfinite(radius_m) && radius_m >= 0.0)) return fail(OC_ERR_INVALID, "radius %g m: not finite and >= 0", radius_m);
-    double u[3];
-    geo_unit(lat, lon, u);
-    const double half = radius_m / (2.0 * OC_GEO_EARTH_RADIUS_M);   // half the central angle
-    const double s = std::sin(half);
-    const double thr = half >= GEO_PI / 2 ? std::numeric_limits<double>::infinity() : 4.0 * s * s;
-    return geo_leaf(g, out, [&](oc_ctx *c, unsigned long long *bits, unsigned grid) {
-        geo_radius_kernel<<<grid, GEO_THREADS, 0, c->stream>>>(g->pts(), u[0], u[1], u[2], thr, inside, bits);
-        return OC_OK;
-    });
-}
-
-extern "C" int oc_filter_geo_polygon(const oc_geo_field *g, const double *lat, const double *lon, uint32_t n_vertices,
-                                     int inside, oc_filter **out) {
-    if (!g || !out || (n_vertices && (!lat || !lon))) return fail(OC_ERR_INVALID, "NULL argument");
-    if (n_vertices < 3 || n_vertices > OC_GEO_MAX_VERTICES)
-        return fail(OC_ERR_INVALID, "polygon of %u vertices: 3 to %u are supported", n_vertices, OC_GEO_MAX_VERTICES);
-    double4 bb = make_double4(lon[0], lon[0], lat[0], lat[0]);
-    for (uint32_t k = 0; k < n_vertices; k++) {
-        if (!geo_valid(lat[k], lon[k])) return fail(OC_ERR_INVALID, "polygon vertex %u: invalid coordinates (%g, %g)", k, lat[k], lon[k]);
-        bb.x = std::min(bb.x, lon[k]); bb.y = std::max(bb.y, lon[k]); bb.z = std::min(bb.z, lat[k]); bb.w = std::max(bb.w, lat[k]);
-    }
-    bb.x -= GEO_BBOX_MARGIN; bb.y += GEO_BBOX_MARGIN;
-    return geo_leaf(g, out, [&](oc_ctx *c, unsigned long long *bits, unsigned grid) {
-        OCTRY(c->in_blob.ensure(size_t(2) * n_vertices * 8));
-        double *v = c->in_blob.as<double>();
-        CU(cudaMemcpyAsync(v, lon, size_t(n_vertices) * 8, cudaMemcpyHostToDevice, c->stream));
-        CU(cudaMemcpyAsync(v + n_vertices, lat, size_t(n_vertices) * 8, cudaMemcpyHostToDevice, c->stream));
-        geo_polygon_kernel<<<grid, GEO_THREADS, 0, c->stream>>>(g->pts(), v, v + n_vertices, n_vertices, bb, inside, bits);
-        return OC_OK;
-    });
-}
-
 // ------------------------------------------------------------------------------------ where programs (where.cuh)
 // The where programs of queries [q0, q0 + n), planned on the host: their distinct leaves (keyed on store, field and
 // parameters, facet leaves on their resolved slice), their distinct programs of more than one node (keyed on content),
@@ -5670,19 +5537,9 @@ static int where_plan(const oc_where *w, uint32_t q0, uint32_t n, const oc_ctx *
                 if (ff->number != number)
                     return fail(OC_ERR_INVALID, "q_where[%u] node %u: field %u is a %s field", b, i, nd.field,
                                 ff->number ? "number" : "bool / string_filter");
-                if (!number) {   // the slices oc_filter_facet_variant / _range take
-                    if (nd.arg + uint64_t(1) >= ff->offsets.size())
-                        return fail(OC_ERR_INVALID, "q_where[%u] node %u: variant %u: field %u has %zu variants", b, i, nd.arg, nd.field,
-                                    ff->offsets.size() - 1);
-                    lo = ff->offsets[nd.arg]; hi = ff->offsets[nd.arg + 1];
-                } else {
-                    const auto &v = ff->values;
-                    lo = (nd.arg & OC_RANGE_LO_OPEN) ? std::upper_bound(v.begin(), v.end(), nd.a) - v.begin()
-                                                     : std::lower_bound(v.begin(), v.end(), nd.a) - v.begin();
-                    hi = (nd.arg & OC_RANGE_HI_OPEN) ? std::lower_bound(v.begin(), v.end(), nd.b) - v.begin()
-                                                     : std::upper_bound(v.begin(), v.end(), nd.b) - v.begin();
-                    hi = std::max(lo, hi);
-                }
+                if (!facet_slice(*ff, nd.arg, nd.a, nd.b, lo, hi))
+                    return fail(OC_ERR_INVALID, "q_where[%u] node %u: variant %u: field %u has %zu variants", b, i, nd.arg, nd.field,
+                                ff->offsets.size() - 1);
                 key = hi > lo ? std::vector<uint64_t>{1, uint64_t(uintptr_t(ff->docs)), lo, hi} : std::vector<uint64_t>{0};
                 break;
             }
@@ -5694,7 +5551,7 @@ static int where_plan(const oc_where *w, uint32_t q0, uint32_t n, const oc_ctx *
                     return fail(OC_ERR_INVALID, "q_where[%u] node %u: geo field nbits %llu != %llu", b, i, (unsigned long long)g->nbits,
                                 (unsigned long long)w->nbits);
                 const uint64_t inside = nd.arg != 0;
-                if (nd.op == OC_WHERE_GEO_RADIUS) {   // oc_filter_geo_radius's checks and threshold
+                if (nd.op == OC_WHERE_GEO_RADIUS) {   // the chord threshold of geo_in_radius
                     if (!geo_valid(nd.a, nd.b)) return fail(OC_ERR_INVALID, "q_where[%u] node %u: radius centre: invalid coordinates (%g, %g)", b, i, nd.a, nd.b);
                     if (!(std::isfinite(nd.c) && nd.c >= 0.0)) return fail(OC_ERR_INVALID, "q_where[%u] node %u: radius %g m: not finite and >= 0", b, i, nd.c);
                     geo_unit(nd.a, nd.b, u);
@@ -5702,7 +5559,7 @@ static int where_plan(const oc_where *w, uint32_t q0, uint32_t n, const oc_ctx *
                     const double s = std::sin(half);
                     thr = half >= GEO_PI / 2 ? std::numeric_limits<double>::infinity() : 4.0 * s * s;
                     key = {2, uint64_t(uintptr_t(g)), dbits(u[0]), dbits(u[1]), dbits(u[2]), dbits(thr), inside};
-                } else {   // oc_filter_geo_polygon's checks and bounding box
+                } else {   // the bounding box of geo_in_polygon's pre-test
                     const uint32_t nv = nd.n_vertices;
                     if (nv < 3 || nv > OC_GEO_MAX_VERTICES)
                         return fail(OC_ERR_INVALID, "q_where[%u] node %u: polygon of %u vertices: 3 to %u are supported", b, i, nv, OC_GEO_MAX_VERTICES);
@@ -5718,7 +5575,7 @@ static int where_plan(const oc_where *w, uint32_t q0, uint32_t n, const oc_ctx *
                     }
                     bb.x -= GEO_BBOX_MARGIN; bb.y += GEO_BBOX_MARGIN;
                 }
-                if (g->n == 0) key = {0};   // no point: an empty leaf, as the leaf call's zeroed bitmap
+                if (g->n == 0) key = {0};   // no point: an empty leaf
                 break;
             }
             case OC_WHERE_FILTER:
@@ -5783,13 +5640,22 @@ static int where_plan(const oc_where *w, uint32_t q0, uint32_t n, const oc_ctx *
 
 // Uploads the plan and materialises every leaf and program on c->stream: one zeroing of the leaf bitmaps, then at most
 // one launch each of where_scatter_kernel, where_geo_kernel and where_eval_kernel.  bits[r] afterwards: the bitmap of
-// result r (a leaf, then the programs) as q_res numbers them.
-static int where_run(oc_ctx *c, WherePlan &pl, std::vector<const uint64_t *> &bits) {
+// result r (a leaf, then the programs) as q_res numbers them.  res_bits (NULL: none) takes the place of result res's
+// workspace slot, so a handle's bitmap is written in place; a FILTER leaf keeps its own bitmap.  The result of a plan
+// of one query is its last slot, which the workspace then leaves out.
+static int where_run(oc_ctx *c, WherePlan &pl, std::vector<const uint64_t *> &bits, uint32_t res = UINT32_MAX,
+                     uint64_t *res_bits = nullptr) {
     const uint64_t words = pl.words;
     const uint32_t n_slots = pl.n_leaf_slots + (uint32_t)pl.progs.size();
-    OCTRY(c->w_bits.ensure(std::max<size_t>(size_t(n_slots) * words * 8, 8)));
+    const uint32_t n_leaves = (uint32_t)pl.leaf_h.size();
+    const uint32_t res_slot = !res_bits || res == UINT32_MAX ? UINT32_MAX
+                              : res >= n_leaves              ? pl.n_leaf_slots + (res - n_leaves)
+                              : pl.leaf_h[res]               ? UINT32_MAX
+                                                             : pl.leaf_slot[res];
+    const uint32_t n_ws = res_slot != UINT32_MAX && res_slot + 1 == n_slots ? n_slots - 1 : n_slots;
+    OCTRY(c->w_bits.ensure(std::max<size_t>(size_t(n_ws) * words * 8, 8)));
     uint64_t *ws = c->w_bits.as<uint64_t>();
-    auto slot_bits = [&](uint32_t s) { return reinterpret_cast<unsigned long long *>(ws + size_t(s) * words); };
+    auto slot_bits = [&](uint32_t s) { return reinterpret_cast<unsigned long long *>(s == res_slot ? res_bits : ws + size_t(s) * words); };
     std::vector<const unsigned long long *> leaf_ptr(pl.leaf_h.size());
     bits.resize(pl.leaf_h.size() + pl.progs.size());
     for (size_t i = 0; i < pl.leaf_h.size(); i++) {
@@ -5816,7 +5682,9 @@ static int where_run(oc_ctx *c, WherePlan &pl, std::vector<const uint64_t *> &bi
         if (L.nv) { L.vlon = dv + uintptr_t(L.vlon); L.vlat = L.vlon + L.nv; }
     }
     OCTRY(upload(pk, c->h_where, c->w_blob, c->stream));
-    if (pl.n_leaf_slots) CU(cudaMemsetAsync(ws, 0, size_t(pl.n_leaf_slots) * words * 8, c->stream));
+    const uint32_t n_ws_leaves = std::min(pl.n_leaf_slots, n_ws);
+    if (n_ws_leaves) CU(cudaMemsetAsync(ws, 0, size_t(n_ws_leaves) * words * 8, c->stream));
+    if (res_slot < pl.n_leaf_slots) CU(cudaMemsetAsync(res_bits, 0, words * 8, c->stream));
     if (pl.total) {
         where_scatter_kernel<<<(unsigned)std::min<uint64_t>((pl.total + 255) / 256, uint64_t(c->prop.multiProcessorCount) * 16), 256, 0,
                                c->stream>>>(s_s.at(c->w_blob), (uint32_t)pl.slices.size(), pl.total, pl.nbits);
@@ -5883,10 +5751,9 @@ extern "C" int oc_where_check(const oc_where *w, uint32_t n_queries) {
     return where_plan(w, 0, n_queries, c, nullptr);
 }
 
-extern "C" int oc_filter_from_where(oc_ctx *c, const oc_where *w, uint32_t query, oc_filter **out) {
-    if (!c || !w || !w->q_node_offsets || !out) return fail(OC_ERR_INVALID, "NULL argument");
-    if (w->q_node_offsets[query + 1] <= w->q_node_offsets[query]) return fail(OC_ERR_INVALID, "q_where[%u]: no program", query);
-    std::lock_guard<std::mutex> g(c->mu);
+// Query `query`'s program of w as a new handle, written in place (a lone FILTER node: copied), with one synchronise.
+// Called with c's lock held.
+static int filter_from_program(oc_ctx *c, const oc_where *w, uint32_t query, oc_filter **out) {
     CU(cudaSetDevice(c->device));
     WherePlan pl;
     OCTRY(where_plan(w, query, 1, c, &pl));
@@ -5895,11 +5762,11 @@ extern "C" int oc_filter_from_where(oc_ctx *c, const oc_where *w, uint32_t query
     oc_filter *f = nullptr;
     OCTRY(filter_alloc(c, h ? h->nbits : pl.nbits, &f));
     std::vector<const uint64_t *> bits;
-    int rc = where_run(c, pl, bits);
+    int rc = where_run(c, pl, bits, r, f->bits);
     cudaError_t e = cudaSuccess;
-    if (rc == OC_OK && f->words) e = cudaMemcpyAsync(f->bits, bits[r], f->words * 8, cudaMemcpyDeviceToDevice, c->stream);
+    if (rc == OC_OK && h && f->words) e = cudaMemcpyAsync(f->bits, h->bits, f->words * 8, cudaMemcpyDeviceToDevice, c->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (rc == OC_OK && e != cudaSuccess) rc = fail(OC_ERR_CUDA, "oc_filter_from_where: %s", cudaGetErrorString(e));
+    if (rc == OC_OK && e != cudaSuccess) rc = fail(OC_ERR_CUDA, "where filter: %s", cudaGetErrorString(e));
     if (rc != OC_OK) {
         cudaFree(f->bits);
         delete f;
@@ -5907,6 +5774,58 @@ extern "C" int oc_filter_from_where(oc_ctx *c, const oc_where *w, uint32_t query
     }
     *out = f;
     return OC_OK;
+}
+
+extern "C" int oc_filter_from_where(oc_ctx *c, const oc_where *w, uint32_t query, oc_filter **out) {
+    if (!c || !w || !w->q_node_offsets || !out) return fail(OC_ERR_INVALID, "NULL argument");
+    if (w->q_node_offsets[query + 1] <= w->q_node_offsets[query]) return fail(OC_ERR_INVALID, "q_where[%u]: no program", query);
+    std::lock_guard<std::mutex> g(c->mu);
+    return filter_from_program(c, w, query, out);
+}
+
+// The leaf and combinator calls: each is the one program nodes[0, n) over [0, *nbits).  *nbits is read under the ctx
+// lock, as a commit of the store publishes a new one under it.
+static int filter_from_nodes(oc_ctx *c, const uint64_t *nbits, const oc_where_node *nodes, uint32_t n, oc_filter **out,
+                             const double *vertex_lat = nullptr, const double *vertex_lon = nullptr) {
+    std::lock_guard<std::mutex> g(c->mu);
+    const uint32_t offsets[2] = {0, n};
+    const oc_where w{*nbits, offsets, nodes, vertex_lat, vertex_lon};
+    return filter_from_program(c, &w, 0, out);
+}
+// Nodes below are {op, field, arg, first_vertex, n_vertices, a, b, c, src} (oc_where_node).
+extern "C" int oc_filter_facet_variant(const oc_facets *f, uint32_t field, uint32_t variant, oc_filter **out) {
+    if (!f || !out) return fail(OC_ERR_INVALID, "NULL argument");
+    const oc_where_node nd{OC_WHERE_VARIANT, field, variant, 0, 0, 0, 0, 0, f};
+    return filter_from_nodes(f->ctx, &f->nbits, &nd, 1, out);
+}
+extern "C" int oc_filter_facet_range(const oc_facets *f, uint32_t field, double lo, double hi, uint32_t flags, oc_filter **out) {
+    if (!f || !out) return fail(OC_ERR_INVALID, "NULL argument");
+    const oc_where_node nd{OC_WHERE_RANGE, field, flags, 0, 0, lo, hi, 0, f};
+    return filter_from_nodes(f->ctx, &f->nbits, &nd, 1, out);
+}
+extern "C" int oc_filter_geo_radius(const oc_geo_field *g, double lat, double lon, double radius_m, int inside, oc_filter **out) {
+    if (!g || !out) return fail(OC_ERR_INVALID, "NULL argument");
+    const oc_where_node nd{OC_WHERE_GEO_RADIUS, 0, uint32_t(inside != 0), 0, 0, lat, lon, radius_m, g};
+    return filter_from_nodes(g->ctx, &g->nbits, &nd, 1, out);
+}
+extern "C" int oc_filter_geo_polygon(const oc_geo_field *g, const double *lat, const double *lon, uint32_t n_vertices,
+                                     int inside, oc_filter **out) {
+    if (!g || !out || (n_vertices && (!lat || !lon))) return fail(OC_ERR_INVALID, "NULL argument");
+    const oc_where_node nd{OC_WHERE_GEO_POLYGON, 0, uint32_t(inside != 0), 0, n_vertices, 0, 0, 0, g};
+    return filter_from_nodes(g->ctx, &g->nbits, &nd, 1, out, lat, lon);
+}
+// where_plan refuses a handle of another ctx, or of another nbits than a's
+static int filter_binary(const oc_filter *a, const oc_filter *b, uint32_t op, oc_filter **out) {
+    if (!a || !b || !out) return fail(OC_ERR_INVALID, "NULL argument");
+    const oc_where_node nd[3] = {{OC_WHERE_FILTER, 0, 0, 0, 0, 0, 0, 0, a}, {OC_WHERE_FILTER, 0, 0, 0, 0, 0, 0, 0, b}, {op, 0, 2}};
+    return filter_from_nodes(a->ctx, &a->nbits, nd, 3, out);
+}
+extern "C" int oc_filter_and(const oc_filter *a, const oc_filter *b, oc_filter **out) { return filter_binary(a, b, OC_WHERE_AND, out); }
+extern "C" int oc_filter_or(const oc_filter *a, const oc_filter *b, oc_filter **out) { return filter_binary(a, b, OC_WHERE_OR, out); }
+extern "C" int oc_filter_not(const oc_filter *a, oc_filter **out) {
+    if (!a || !out) return fail(OC_ERR_INVALID, "NULL argument");
+    const oc_where_node nd[2] = {{OC_WHERE_FILTER, 0, 0, 0, 0, 0, 0, 0, a}, {OC_WHERE_NOT}};
+    return filter_from_nodes(a->ctx, &a->nbits, nd, 2, out);
 }
 
 // ------------------------------------------------------------------------------------ micro-batching front

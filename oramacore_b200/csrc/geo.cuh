@@ -1,17 +1,16 @@
-// geo.cuh — where-filter leaves on a geopoint field: the documents with a point inside / outside a radius or polygon.
+// geo.cuh — the per-point tests of a where-filter leaf on a geopoint field, used by where_geo_kernel (where.cuh).
 //
 // Replaces GeoPointFieldStorage::filter (read/index/geopoint_field.rs:179-229): a full scan of the field's points per
-// query.  A field holds its points sorted by document id, structure of arrays: the unit vector (x, y, z) of each point
-// (computed on the host), its latitude / longitude in degrees and its document id.  Each kernel runs one thread per
-// point, grid-stride, and sets the document's bit in a zeroed oc_filter bitmap when the leaf's predicate holds for that
-// point: a document is in the leaf when at least one of its points satisfies the predicate.
+// leaf.  A field holds its points sorted by document id, structure of arrays: the unit vector (x, y, z) of each point
+// (computed on the host), its latitude / longitude in degrees and its document id.  A document is in the leaf when at
+// least one of its points satisfies the leaf's predicate; geo_set sets its bit.
 //
-//   geo_radius_kernel   great-circle distance d <= r as a chord test: |u_p - u_c|^2 <= thr, thr = 4 sin^2(r / 2R) from
-//                       the host (+inf when r >= pi R).  Three subtractions and three multiply-adds per point.
-//   geo_polygon_kernel  even-odd ray crossing (PNPOLY) in planar (lon, lat) degrees against vertices staged in shared
-//                       memory, after a bounding-box pre-test.  The crossing test is evaluated with explicitly rounded
-//                       f64 operations in the order (xj - xi) * (y - yi) / (yj - yi) + xi, so no FMA contraction can
-//                       change a result.
+//   geo_in_radius   great-circle distance d <= r as a chord test: |u_p - u_c|^2 <= thr, thr = 4 sin^2(r / 2R) from the
+//                   host (+inf when r >= pi R).  Three subtractions and three multiply-adds per point.
+//   geo_in_polygon  even-odd ray crossing (PNPOLY) in planar (lon, lat) degrees against vertices staged in shared memory,
+//                   after a bounding-box pre-test.  The crossing test is evaluated with explicitly rounded f64
+//                   operations in the order (xj - xi) * (y - yi) / (yj - yi) + xi, so no FMA contraction can change a
+//                   result.
 #pragma once
 #include <cstdint>
 
@@ -34,7 +33,6 @@ __device__ __forceinline__ void geo_set(unsigned long long *bits, uint64_t d) {
     atomicOr(bits + (d >> 6), 1ull << (d & 63));
 }
 
-// The per-point tests, shared by these kernels and where_geo_kernel (where.cuh) so both give the same bits.
 __device__ __forceinline__ bool geo_in_radius(double x, double y, double z, double cx, double cy, double cz, double thr) {
     const double dx = x - cx, dy = y - cy, dz = z - cz;
     return dx * dx + dy * dy + dz * dz <= thr;
@@ -54,26 +52,6 @@ __device__ __forceinline__ bool geo_in_polygon(double x, double y, const double 
         }
     }
     return in;
-}
-
-__global__ void __launch_bounds__(GEO_THREADS) geo_radius_kernel(const GeoPoints g, double cx, double cy, double cz,
-                                                                 double thr, int inside, unsigned long long *bits) {
-    for (uint64_t i = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < g.n; i += uint64_t(gridDim.x) * blockDim.x) {
-        const bool in = geo_in_radius(g.x[i], g.y[i], g.z[i], cx, cy, cz, thr);
-        if (in == (inside != 0)) geo_set(bits, g.doc[i]);
-    }
-}
-
-__global__ void __launch_bounds__(GEO_THREADS) geo_polygon_kernel(const GeoPoints g, const double *vlon, const double *vlat,
-                                                                  uint32_t nv, double4 bbox, int inside,
-                                                                  unsigned long long *bits) {
-    __shared__ double sx[GEO_MAX_VERTICES], sy[GEO_MAX_VERTICES];
-    for (uint32_t k = threadIdx.x; k < nv; k += blockDim.x) { sx[k] = vlon[k]; sy[k] = vlat[k]; }
-    __syncthreads();
-    for (uint64_t i = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; i < g.n; i += uint64_t(gridDim.x) * blockDim.x) {
-        const bool in = geo_in_polygon(g.lon[i], g.lat[i], sx, sy, nv, bbox);
-        if (in == (inside != 0)) geo_set(bits, g.doc[i]);
-    }
 }
 
 }  // namespace oc

@@ -1,15 +1,16 @@
-// where.cuh — where-clause programs (oc_search_params.q_where) evaluated inside a search call.
+// where.cuh — where-clause programs, the one evaluator of where filters on the device: inside a search call
+// (oc_search_params.q_where), and for every handle oc_filter_from_where, the leaf calls and And / Or / Not build.
 //
 // The host plan (capi.cu where_plan) deduplicates the leaves and the programs of a batch and lays every bitmap out in one
 // ctx workspace.  Three launches then build every result, however many leaves and queries the batch has:
 //   where_scatter_kernel  the facet leaves: one work list of (document slice, leaf bitmap) items over all leaves, one
-//                         thread per document id, as filter_scatter_ids_kernel does for one slice.
-//   where_geo_kernel      the geo leaves, a fixed number of blocks each: the per-point tests of geo_radius_kernel /
-//                         geo_polygon_kernel (geo.cuh), a polygon's vertices staged in shared memory.
+//                         thread per document id.
+//   where_geo_kernel      the geo leaves, a fixed number of blocks each: the per-point tests of geo.cuh, a polygon's
+//                         vertices staged in shared memory.
 //   where_eval_kernel     every distinct program of more than one node, one per blockIdx.y, one 64-bit word per thread:
 //                         the postfix program runs over that word of its leaves, and the padding bits of the last word
-//                         are cleared in the value it writes.  filter_combine_kernel clears them after every And / Or /
-//                         Not; clearing once at the end gives the same bits, also over a FILTER handle with a dirty tail.
+//                         are cleared in the value it writes, also over a FILTER handle with a dirty tail.  Clearing
+//                         once at the end gives what clearing after every And / Or / Not would.
 #pragma once
 #include <cstdint>
 

@@ -35,7 +35,7 @@ import numpy as np
 from .engine import (Context, DeviceFilter, EmbeddingFieldStorage, FacetStore, GeoPointField, OmcStore, SortField,
                      StringFieldStorage, TermDictionary, TokenScoreContext, resolve_sort_by)
 from .types import SortBy
-from .where import WhereFilter, WhereProgram, check_where_keys, compile_where, evaluate_where, parse_where
+from .where import WhereFilter, WhereProgram, check_where_keys, compile_where, filter_from_program, parse_where
 
 _F64_INT_MAX = 1 << 53   # I64 values beyond +-2^53 would not survive the trip through a double
 
@@ -247,9 +247,8 @@ class IndexLoader:
         TokenScoreParams.device_filter.  Raises FilterFieldNotFound for a key that is not a filter field
         (search.rs:435-449) before any device work, and ValueError for a clause serde would refuse.  The fields are
         the ones laid out by the last refresh_facets() / commit(); the deletes since the last commit are excluded."""
-        w = where if isinstance(where, WhereFilter) else parse_where(where)
-        check_where_keys(w, [self.filter_fields()])
-        return evaluate_where(w, self.facets, self.geo, self.nbits, sorted(self._uncommitted_deleted), ctx=self.ctx)
+        prog = self.where_program(where)
+        return None if prog is None else filter_from_program(self.ctx, prog)
 
     def where_program(self, where) -> Optional[WhereProgram]:
         """The counterpart of where_filter: the same clause as a program for TokenScoreParams.where_programs, which the

@@ -17,13 +17,15 @@ Filter.  Any other pairing is an error.  So `{"not": {"gt": 5}}` is a number fil
   * GeoSearchFilter (types.rs:2175-2221): {"radius": {coordinates, unit = "m", value, inside = true}} or
     {"polygon": {coordinates, inside = true}}, a GeoPoint being {"lat", "lon"}; unknown keys are ignored.
 
-evaluate_where(...) restates calculate_filter + FilterContext::execute_filter (filter.rs:176-287, 344-392) with
-device leaves: FacetStore.leaf for bool / number / date / string_filter fields, GeoPointField radius / polygon for
-geopoint fields, and DeviceFilter and / or / not.  A document is in a leaf when at least one of its values passes.
+compile_where(...) restates calculate_filter + FilterContext::execute_filter (filter.rs:176-287, 344-392) as a postfix
+program (include/oramacore_b200.h "where programs") over device leaves: variant and range leaves of bool / number /
+date / string_filter fields, radius and polygon leaves of geopoint fields, and And / Or / Not.  A search call evaluates
+it itself (oc_search_params.q_where); evaluate_where(...) evaluates it into a DeviceFilter with one call
+(oc_filter_from_where).  A document is in a leaf when at least one of its values passes.
   * A node is the AND of its field leaves, of each `and` child, of the OR of its `or` children and of NOT its `not`
     child.
   * A key of a node that is not a filter field of the index makes the whole node empty.  The keys are checked in
-    order as the leaves are built, so a leaf after such a key (an invalid polygon, say) is never built.
+    order as the leaves are compiled, so a leaf after such a key (an invalid polygon, say) is never checked.
   * A node with `or: []`, and a node with no parts at all (the `{}` of `{"and": [{}]}`), is empty.
   * At the top level an empty filter (`is_empty`, types.rs:1282-1287) means no filter: None, or NOT(deletes) when
     there are uncommitted deletes.  Otherwise the result is the tree AND NOT(uncommitted deletes).
@@ -35,9 +37,7 @@ Assumptions and deliberate differences (the oramacore_fields source is not avail
     (tests/test_where_host.py shows this is the only difference).
   * The reference raises FilterFieldNotFound only when the search found nothing (search.rs:435-449); IndexLoader
     .where_filter checks the keys before any device work, so a clause naming an unknown field is always refused.
-  * Bitmaps are exact, where the reference's sets may be Bloom-backed.
-compile_where(...) applies the same tree rules (one `_node` walk, one `_top_level` rule) to build the postfix program a
-search call evaluates itself (oc_search_params.q_where): no device call per request, and the same bitmap."""
+  * Bitmaps are exact, where the reference's sets may be Bloom-backed."""
 from __future__ import annotations
 
 import math
@@ -298,11 +298,11 @@ def check_where_keys(w: WhereFilter, filter_fields_per_index: Sequence[Sequence[
             raise FilterFieldNotFound(k)
 
 
-# ---------------------------------------------------------------- evaluation
+# ---------------------------------------------------------------- programs (oc_search_params.q_where)
 def _node(b, w: WhereFilter):
-    """The tree rules of calculate_filter (filter.rs:176-287) over a builder `b` (has / leaf / empty / and_ / or_ / not_):
+    """The tree rules of calculate_filter (filter.rs:176-287) over the builder `b` (_Compile):
     the AND of the node's field leaves, of each `and` child, of the OR of its `or` children and of NOT its `not` child.
-    A key that is not a filter field makes the node empty (leaves after it are never built); `or: []` and a node with
+    A key that is not a filter field makes the node empty (leaves after it are never compiled); `or: []` and a node with
     no parts are empty."""
     parts = []
     for k, flt in w.filter_on_fields:
@@ -327,9 +327,23 @@ def _top_level(w: WhereFilter, has_deletes: bool) -> str:
     return "tree_and_live" if has_deletes else "tree"
 
 
-class _Builder:
-    """What both builders of `_node` share: which keys are filter fields of the index, and which leaf a (key, filter)
-    pair is.  A subclass builds its values: facet_leaf, radius, polygon, empty, and_, or_, not_."""
+@dataclass
+class WhereProgram:
+    """A where-clause compiled to the library's postfix program (include/oramacore_b200.h "where programs"): `nodes` are
+    (op, field, arg, a, b, c, src, vertices) tuples, vertices = (lats, lons) for a polygon else None.  `keep` holds the
+    handles the program points at (the deletes handle), `nbits` the DocumentId space of its leaves."""
+    nbits: int
+    nodes: List[tuple] = field(default_factory=list)
+    keep: list = field(default_factory=list)
+
+
+def _n(op, field_=0, arg=0, a=0.0, b=0.0, c=0.0, src=None, verts=None):
+    return (op, field_, arg, a, b, c, src, verts)
+
+
+class _Compile:
+    """The builder `_node` runs over one index: which keys are filter fields, and the node list that pushes each value
+    of the tree (a leaf, the empty set, And / Or / Not)."""
 
     def __init__(self, facets, geo_fields):
         self.facets, self.geo = facets, geo_fields
@@ -346,106 +360,6 @@ class _Builder:
         if isinstance(flt, GeoPolygon):
             return self.polygon(g, flt)
         return self.empty()   # wrong kind for a geopoint field
-
-
-class _Eval(_Builder):
-    """The tree rules building device handles over one index.  Every handle made while a tree is evaluated is kept in
-    `owned` and closed when the evaluation ends, except the result."""
-
-    def __init__(self, ctx, facets, geo_fields, nbits):
-        super().__init__(facets, geo_fields)
-        self.ctx, self.nbits = ctx, nbits
-        self.owned: List[DeviceFilter] = []
-
-    def evaluate(self, w: WhereFilter) -> DeviceFilter:
-        try:
-            res = _node(self, w)
-            self.owned.remove(res)
-            return res
-        finally:
-            for f in self.owned:
-                f.close()
-
-    def keep(self, f: DeviceFilter) -> DeviceFilter:
-        self.owned.append(f)
-        return f
-
-    def facet_leaf(self, key, flt) -> DeviceFilter:
-        return self.keep(self.facets.leaf(key, flt))
-
-    def radius(self, g, flt) -> DeviceFilter:
-        return self.keep(g.radius(flt.lat, flt.lon, flt.value, flt.unit, flt.inside))
-
-    def polygon(self, g, flt) -> DeviceFilter:
-        return self.keep(g.polygon(flt.coordinates, flt.inside))
-
-    def empty(self) -> DeviceFilter:
-        return self.keep(DeviceFilter.from_ids(self.ctx, [], self.nbits))
-
-    def fold(self, parts: List[DeviceFilter], op) -> DeviceFilter:
-        acc = parts[0]
-        for p in parts[1:]:
-            acc = self.keep(op(acc, p))
-        return acc
-
-    def and_(self, parts):
-        return self.fold(parts, DeviceFilter.__and__)
-
-    def or_(self, parts):
-        return self.fold(parts, DeviceFilter.__or__)
-
-    def not_(self, x):
-        return self.keep(~x)
-
-
-def evaluate_where(w: WhereFilter, facets: Optional[FacetStore], geo_fields: Mapping[str, GeoPointField], nbits: int,
-                   uncommitted_deleted: Sequence[int] = (), ctx: Optional[Context] = None) -> Optional[DeviceFilter]:
-    """FilterContext::execute_filter (filter.rs:344-392) over one index: None when nothing is filtered, else a
-    DeviceFilter over [0, nbits).  `ctx` defaults to the context of the facet store or of a geopoint field."""
-    if ctx is None:
-        ctx = facets.ctx if facets is not None else next((g.ctx for g in geo_fields.values()), None)
-    if ctx is None:
-        raise ValueError("evaluate_where: no context (pass ctx= for an index without filter fields)")
-    deleted = sorted({int(d) for d in uncommitted_deleted})
-    top = _top_level(w, bool(deleted))
-    if top == "none":
-        return None
-    live = None
-    if deleted:
-        dele = DeviceFilter.from_ids(ctx, deleted, nbits)
-        try:
-            live = ~dele
-        finally:
-            dele.close()
-    if top == "live":
-        return live
-    tree = _Eval(ctx, facets, dict(geo_fields), int(nbits)).evaluate(w)
-    if live is None:
-        return tree
-    try:
-        return tree & live
-    finally:
-        tree.close()
-        live.close()
-
-
-# ---------------------------------------------------------------- programs (oc_search_params.q_where)
-@dataclass
-class WhereProgram:
-    """A where-clause compiled to the library's postfix program (include/oramacore_b200.h "where programs"): `nodes` are
-    (op, field, arg, a, b, c, src, vertices) tuples, vertices = (lats, lons) for a polygon else None.  `keep` holds the
-    handles the program points at (the deletes handle), `nbits` the DocumentId space of its leaves."""
-    nbits: int
-    nodes: List[tuple] = field(default_factory=list)
-    keep: list = field(default_factory=list)
-
-
-def _n(op, field_=0, arg=0, a=0.0, b=0.0, c=0.0, src=None, verts=None):
-    return (op, field_, arg, a, b, c, src, verts)
-
-
-class _Compile(_Builder):
-    """The tree rules building a postfix program; a value is the node list that pushes it."""
 
     def empty(self):
         return [_n(_lib.OC_WHERE_NONE)]
@@ -484,8 +398,9 @@ class _Compile(_Builder):
 
 def compile_where(w: WhereFilter, facets: Optional[FacetStore], geo_fields: Mapping[str, GeoPointField], nbits: int,
                   live: Optional[DeviceFilter] = None) -> Optional[WhereProgram]:
-    """The program of evaluate_where(w, ...): None when nothing is filtered.  `live` is the NOT(uncommitted deletes)
-    handle (None without deletes), passed as a FILTER node; leaves are checked as their leaf calls check them."""
+    """execute_filter's program over one index: None when nothing is filtered.  `live` is the NOT(uncommitted deletes)
+    handle (None without deletes), passed as a FILTER node; leaves are checked as FacetStore.leaf_args and
+    GeoPointField.radius_args / polygon_args check them."""
     top = _top_level(w, live is not None)
     if top == "none":
         return None
@@ -536,3 +451,33 @@ def filter_from_program(ctx: Context, prog: WhereProgram) -> DeviceFilter:
     if len(prog.nodes) == 1 and prog.nodes[0][0] == _lib.OC_WHERE_FILTER:
         nbits = prog.keep[0].nbits   # a lone handle is taken as it is
     return DeviceFilter(ctx, h, nbits)
+
+
+def evaluate_where(w: WhereFilter, facets: Optional[FacetStore], geo_fields: Mapping[str, GeoPointField], nbits: int,
+                   uncommitted_deleted: Sequence[int] = (), ctx: Optional[Context] = None) -> Optional[DeviceFilter]:
+    """FilterContext::execute_filter (filter.rs:344-392) over one index: None when nothing is filtered, else a
+    DeviceFilter over [0, nbits), the program of compile_where evaluated in one call.  The NOT(uncommitted deletes)
+    handle is built for this call and closed, unless it is the result.  `ctx` defaults to the context of the facet store
+    or of a geopoint field."""
+    if ctx is None:
+        ctx = facets.ctx if facets is not None else next((g.ctx for g in geo_fields.values()), None)
+    if ctx is None:
+        raise ValueError("evaluate_where: no context (pass ctx= for an index without filter fields)")
+    deleted = sorted({int(d) for d in uncommitted_deleted})
+    top = _top_level(w, bool(deleted))
+    if top == "none":
+        return None
+    live = None
+    if deleted:
+        dele = DeviceFilter.from_ids(ctx, deleted, nbits)
+        try:
+            live = ~dele
+        finally:
+            dele.close()
+    if top == "live":
+        return live
+    try:
+        return filter_from_program(ctx, compile_where(w, facets, geo_fields, nbits, live))
+    finally:
+        if live is not None:
+            live.close()

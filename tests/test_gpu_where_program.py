@@ -1,12 +1,13 @@
 """Where clauses as programs evaluated inside the search call (oc_search_params.q_where, TokenScoreParams.where_programs,
 IndexLoader.where_program, oc_filter_from_where, oc_where_check).
 
-The rule: query b's outputs with q_where are byte for byte those it gets with q_filters[b] = the handle evaluate_where
-builds from the same clause.  Checked for the bitmaps themselves (every leaf kind and op, random trees with geo leaves
-and deletes), for oc_search / oc_search_q_sorted / oc_search_q_groups / oc_search_q_facets over fulltext, vector and
-hybrid with mixed per-query parameters, for batches with duplicate programs, unfiltered queries, single leaves and
-FILTER-only programs, for workspace reuse, for every refusal, for the launch count of the where stage and through the
-batcher from many threads."""
+The bitmaps of programs (every leaf kind and op, random trees with geo leaves and deletes, FILTER-only programs, a FILTER
+handle with a dirty tail) are checked against the host restatement of tests/test_where_host.py.  The rule for searches:
+query b's outputs with q_where are byte for byte those it gets with q_filters[b] = the handle evaluate_where builds from
+the same clause.  Checked for oc_search / oc_search_q_sorted / oc_search_q_groups / oc_search_q_facets over fulltext,
+vector and hybrid with mixed per-query parameters, for batches with duplicate programs, unfiltered queries, single
+leaves and FILTER-only programs, for workspace reuse, for every refusal, for the launch count of the where stage and
+through the batcher from many threads."""
 import ctypes as C
 import threading
 
@@ -17,15 +18,15 @@ import oramacore_b200 as ob
 from oramacore_b200 import _lib
 from oramacore_b200.engine import _p
 from oramacore_b200.types import MODE_FULLTEXT, MODE_HYBRID, MODE_VECTOR
-from oramacore_b200.where import (GeoRadius, WhereFilter, compile_where, evaluate_where, filter_from_program, pack_programs,
-                                  parse_where)
+from oramacore_b200.where import WhereProgram, compile_where, evaluate_where, filter_from_program, pack_programs, parse_where
 from test_gpu_q_groups import _facets, _requests
 from test_gpu_q_sorted import _promote, _sorts, _tsc
 from test_gpu_q_sorted import fields  # noqa: F401  (fixture)
 from test_gpu_query_filters import MODES, N, OC_ERR_INVALID, OC_ERR_UNSUPPORTED, _inputs
 from test_gpu_query_filters import corpus  # noqa: F401  (fixture)
-from test_gpu_where import NBITS, _leaf_json, _tree
+from test_gpu_where import NBITS, _ids, _leaf_json, _tree
 from test_gpu_where import store  # noqa: F401  (fixture)
+from test_where_host import host_where
 
 pytestmark = pytest.mark.gpu
 
@@ -45,14 +46,16 @@ def _live(ctx, deleted, nbits):
         d.close()
 
 
-# ---------------------------------------------------------------- bitmaps: oc_filter_from_where == evaluate_where
-def _same_bits(ctx, st, geo, w, deleted, live, nbits=NBITS):
-    ref = evaluate_where(w, st, geo, nbits, deleted, ctx=ctx)
-    prog = compile_where(w, st, geo, nbits, live if deleted else None)
-    assert (ref is None) == (prog is None)
-    if ref is None:
-        return
-    assert _bits(filter_from_program(ctx, prog)).tobytes() == _bits(ref).tobytes()
+# ---------------------------------------------------------------- bitmaps: oc_filter_from_where == the host restatement
+def _check_bits(store, w, deleted, live):  # noqa: F811
+    """The program of w (with the NOT(deletes) handle `live` as a FILTER node when there are deletes) is the set
+    host_where computes."""
+    st, geo, fields_, _, _, _ = store
+    prog = compile_where(w, st, geo, NBITS, live if deleted else None)
+    want = host_where(w, fields_, NBITS, deleted)
+    assert (prog is None) == (want is None)
+    if prog is not None:
+        assert _ids(filter_from_program(st.ctx, prog)) == want
 
 
 @pytest.mark.parametrize("key", ["n", "d", "b", "s", "g"])
@@ -62,25 +65,13 @@ def test_bits_every_leaf_kind(store, key):  # noqa: F811
     try:
         for i in range(30):
             where = {key: _leaf_json(rng, key, nv, fields_)}
-            _same_bits(st.ctx, st, geo, parse_where(where), deleted if i % 3 == 0 else [], live)
+            _check_bits(store, parse_where(where), deleted if i % 3 == 0 else [], live)
         for wrong in (True, "k1", {"gt": 0}):   # the wrong kind of filter for the field: empty
-            _same_bits(st.ctx, st, geo, parse_where({key: wrong}), [], live)
+            _check_bits(store, parse_where({key: wrong}), [], live)
         # each op over two leaves, and the empty top level with deletes (a FILTER-only program)
         a, b = _leaf_json(rng, key, nv, fields_), _leaf_json(rng, key, nv, fields_)
         for where in ({"and": [{key: a}, {key: b}]}, {"or": [{key: a}, {key: b}]}, {"not": {key: a}}, {"or": []}, {}):
-            _same_bits(st.ctx, st, geo, parse_where(where), deleted, live)
-    finally:
-        live.close()
-
-
-def test_bits_geo_radius(store):  # noqa: F811
-    st, geo, _, deleted, rng, _ = store
-    live = _live(st.ctx, deleted, NBITS)
-    try:
-        for i in range(20):
-            w = WhereFilter(filter_on_fields=[("g", GeoRadius(float(rng.uniform(-60, 60)), float(rng.uniform(-120, 120)),
-                                                              float(rng.uniform(1e5, 4e6)), "m", bool(i % 2)))])
-            _same_bits(st.ctx, st, geo, w, deleted if i % 2 else [], live)
+            _check_bits(store, parse_where(where), deleted, live)
     finally:
         live.close()
 
@@ -90,9 +81,18 @@ def test_bits_random_trees(store):  # noqa: F811
     live = _live(st.ctx, deleted, NBITS)
     try:
         for i in range(220):
-            _same_bits(st.ctx, st, geo, parse_where(_tree(rng, 1, nv, fields_)), deleted if i % 2 else [], live)
+            _check_bits(store, parse_where(_tree(rng, 1, nv, fields_)), deleted if i % 2 else [], live)
     finally:
         live.close()
+
+
+def test_leaves_of_another_nbits_are_refused(store):  # noqa: F811
+    """A store whose nbits differs from the nbits asked for is refused, for a tree of one leaf as for more."""
+    st, geo, fields_, _, rng, nv = store
+    for where in ({"b": True}, {"g": _leaf_json(rng, "g", nv, fields_)}, {"b": True, "s": "k1"}):
+        with pytest.raises(_lib.OcError) as e:
+            evaluate_where(parse_where(where), st, geo, NBITS + 1)
+        assert e.value.code == OC_ERR_INVALID, where
 
 
 # ---------------------------------------------------------------- searches: q_where == q_filters of the same handles
@@ -315,7 +315,6 @@ def test_refusals_write_nothing(wcorpus):
                      + [(A, 0, _lib.OC_WHERE_MAX_DEPTH + 1, 0, 0, 0, None, None)],
             "nodes": [(R, num_id, 0, 0, 1, 0, st_h, None)] + [(NO, 0, 0, 0, 0, 0, None, None)] * _lib.OC_WHERE_MAX_NODES,
         }
-        from oramacore_b200.where import WhereProgram
         cases = [(name, [good, WhereProgram(N, nodes)], OC_ERR_INVALID) for name, nodes in bad.items()]
         for name, progs, code in cases:
             w, keep = pack_programs(progs)
@@ -463,21 +462,27 @@ def test_loader_where_program_after_publish_without_commit(gpu_ctx):
 
 def test_filter_node_with_a_dirty_tail(store):  # noqa: F811
     """A FILTER handle whose padding bits are set (oc_filter_from_bits): And / Or / Not in a program clear them in the
-    result as oc_filter_and / or / not do."""
-    st, geo, _, _, _, _ = store
+    result."""
+    st, geo, _, _, rng, _ = store
     assert NBITS % 64
     ctx = st.ctx
-    dirty = ob.DeviceFilter.from_bits(ctx, np.full((NBITS + 63) // 64, ~np.uint64(0), np.uint64), NBITS)
+    words = (NBITS + 63) // 64
+    tail = np.full(words, ~np.uint64(0), np.uint64)
+    tail[-1] = np.uint64((1 << (NBITS % 64)) - 1)
+    d = rng.integers(0, np.iinfo(np.uint64).max, words, dtype=np.uint64, endpoint=True)
+    d[-1] |= ~tail[-1]
+    dirty = ob.DeviceFilter.from_bits(ctx, d, NBITS)
     fid = st.fields["b"]["id"]
     leaf = st.leaf("b", True)
     try:
+        assert (dirty.read() == d).all()
+        lb = leaf.read()
         F, V = (_lib.OC_WHERE_FILTER, 0, 0, 0.0, 0.0, 0.0, dirty._h.value, None), (_lib.OC_WHERE_VARIANT, fid, 0, 0.0, 0.0, 0.0, st._h.value, None)
-        from oramacore_b200.where import WhereProgram
-        for nodes, ref in (([F, V, (_lib.OC_WHERE_OR, 0, 2, 0.0, 0.0, 0.0, None, None)], lambda: dirty | leaf),
-                           ([F, V, (_lib.OC_WHERE_AND, 0, 2, 0.0, 0.0, 0.0, None, None)], lambda: dirty & leaf),
-                           ([F, (_lib.OC_WHERE_NOT, 0, 0, 0.0, 0.0, 0.0, None, None)], lambda: ~dirty)):
+        for nodes, want in (([F, V, (_lib.OC_WHERE_OR, 0, 2, 0.0, 0.0, 0.0, None, None)], (d | lb) & tail),
+                            ([F, V, (_lib.OC_WHERE_AND, 0, 2, 0.0, 0.0, 0.0, None, None)], d & lb & tail),
+                            ([F, (_lib.OC_WHERE_NOT, 0, 0, 0.0, 0.0, 0.0, None, None)], ~d & tail)):
             prog = WhereProgram(NBITS, nodes, [dirty])
-            assert _bits(filter_from_program(ctx, prog)).tobytes() == _bits(ref()).tobytes(), nodes[-1][0]
+            assert _bits(filter_from_program(ctx, prog)).tobytes() == want.tobytes(), nodes[-1][0]
     finally:
         dirty.close(); leaf.close()
 

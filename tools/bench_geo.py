@@ -9,9 +9,9 @@ Runs
     same documents uploaded as a bitmap (what any filter of that size costs the search);
   * the same leaves restated in numpy on the CPU (an f64 haversine, a vectorised PNPOLY), labelled as such: that is a
     CPU restatement, not the reference.
-For every leaf it prints the kernel's device time (torch.profiler, CUDA activity of geo_radius_kernel /
-geo_polygon_kernel, per call) and the host wall time of the whole synchronous call (bitmap allocation, zeroing, the
-kernel, the synchronise); for the searches oc_last_timing.device_ms (CUDA events).  Median / min / max of --calls calls
+For every leaf it prints the kernel's device time (torch.profiler, CUDA activity of where_geo_kernel, per call) and the
+host wall time of the whole synchronous call (bitmap allocation, plan upload, zeroing, the kernel, the copy into the
+handle, the synchronise); for the searches oc_last_timing.device_ms (CUDA events).  Median / min / max of --calls calls
 after one warm-up call.  The card's name and power limit are read in the same process.  Writes nothing into the tree.
 
     python tools/bench_geo.py [--calls 20] [--skip-search]

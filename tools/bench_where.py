@@ -6,7 +6,7 @@ Runs, at 1M and 10M documents (one value per document in each field):
     against what a caller does without them: numpy `searchsorted` over the sorted values (or the variant's id list)
     plus `oc_filter_from_ids` of the same ids, which uploads 8 B per id;
   * one 4-leaf `where` (number range, bool, string, NOT of another range) with 1000 uncommitted deletes, end to end
-    (parse + leaves + and / or / not), through `evaluate_where`;
+    (parse, compile, deletes handle, one oc_filter_from_where), through `evaluate_where`;
   * at 1M only, the h1 oc_search (hybrid, 1M x 768-d fp32 + BM25 over 1M synthetic docs, B = 256, top 10) without a
     filter, under that `where`, and under the same documents built with `from_ids`.
 Leaves and clauses: host wall time of the whole synchronous call, median / min / max of --calls calls after one

@@ -1,13 +1,14 @@
 """Cost of `where` clauses evaluated inside the search call (where programs, oc_search_params.q_where) against the
-handle path (evaluate_where: one oc_filter_* call per leaf and per and / or / not, then q_filters).
+handle path (one handle per clause, then q_filters).
 
 Runs:
   * at 1M and 10M documents, the 4-leaf `where` of tools/bench_where.py with 1000 uncommitted deletes: evaluate_where
-    (which builds NOT(deletes) on every call), the same leaf and combine calls with NOT(deletes) built once, and
-    compile_where + oc_filter_from_where (NOT(deletes) built once, as IndexLoader keeps it per set of deletes).  Host wall time of the whole synchronous work, median / min / max of --calls after one warm-up.
+    (which builds NOT(deletes) on every call, then evaluates the clause's program with oc_filter_from_where) and
+    compile_where + oc_filter_from_where (NOT(deletes) built once, as IndexLoader keeps it per set of deletes).  Host
+    wall time of the whole synchronous work, median / min / max of --calls after one warm-up.
   * the h1 shape (hybrid, 1M x 768-d fp32 + BM25 over 1M synthetic docs, B = 256, top 10) with 256 distinct 4-leaf
-    clauses: building 256 handles + oc_search(q_filters), with NOT(deletes) built per handle and built once, against
-    compiling 256 programs + one oc_search(q_where).
+    clauses: building 256 handles with evaluate_where + oc_search(q_filters), against compiling 256 programs + one
+    oc_search(q_where).
     Wall time of the whole request path; the search's own wall time; and, from one torch.profiler run of each search,
     the summed device time of every kernel of the call and of its where kernels alone.  The outputs of both paths are
     compared byte for byte.
@@ -29,7 +30,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import oramacore_b200 as ob  # noqa: E402
 from oramacore_b200 import synth  # noqa: E402
-from oramacore_b200.where import _Eval, compile_where, filter_from_program  # noqa: E402
+from oramacore_b200.where import compile_where, filter_from_program  # noqa: E402
 from bench_where import WHERE, build_store, card, stats  # noqa: E402
 
 N, DIM, VOCAB, B, LIMIT = 1_000_000, 768, 200_000, 256, 10
@@ -51,16 +52,6 @@ def live_of(ctx, deleted, n):
         return ~d
     finally:
         d.close()
-
-
-def handle_with_live(ctx, st, w, n, live):
-    """The handle path with the NOT(deletes) handle built once, as the program path has it: the tree's leaf and combine
-    calls, then one oc_filter_and with the prebuilt handle."""
-    tree = _Eval(ctx, st, {}, n).evaluate(w)
-    try:
-        return tree & live
-    finally:
-        tree.close()
 
 
 def clauses(rng, k):
@@ -92,7 +83,6 @@ def main():
         ref.close(); got.close()
         row = {"where": WHERE, "documents": n, "deletes": 1000, "bit_identical": same,
                "evaluate_where_ms": wall(lambda: ob.evaluate_where(ob.parse_where(WHERE), st, {}, n, deleted).close(), a.calls),
-               "handles_prebuilt_deletes_ms": wall(lambda: handle_with_live(ctx, st, ob.parse_where(WHERE), n, live).close(), a.calls),
                "compile_where_filter_from_where_ms": wall(
                    lambda: filter_from_program(ctx, compile_where(ob.parse_where(WHERE), st, {}, n, live)).close(), a.calls)}
         print(json.dumps({**row, **info}), flush=True)
@@ -144,20 +134,12 @@ def search_rows(ctx, st, deleted, live, calls, info, rng):
             for h in hs:
                 h.close()
 
-    def handles_prebuilt_path():
-        hs = [handle_with_live(ctx, st, w, N, live) for w in ws]
-        try:
-            return tsc.execute_batch_arrays(ob.TokenScoreParams(device_filters=hs, **kw), texts, qv)
-        finally:
-            for h in hs:
-                h.close()
-
     def program_path():
         ps = [compile_where(w, st, {}, N, live) for w in ws]
         return tsc.execute_batch_arrays(ob.TokenScoreParams(where_programs=ps, **kw), texts, qv)
 
-    a, b, a2 = handles_path(), program_path(), handles_prebuilt_path()
-    same = all(x.tobytes() == y.tobytes() == z.tobytes() for x, y, z in zip(a, b, a2))
+    a, b = handles_path(), program_path()
+    same = all(x.tobytes() == y.tobytes() for x, y in zip(a, b))
     hs = [ob.evaluate_where(w, st, {}, N, deleted) for w in ws]
     ps = [compile_where(w, st, {}, N, live) for w in ws]
     p_h, p_w = ob.TokenScoreParams(device_filters=hs, **kw), ob.TokenScoreParams(where_programs=ps, **kw)
@@ -165,8 +147,6 @@ def search_rows(ctx, st, deleted, live, calls, info, rng):
     search_w = lambda: tsc.execute_batch_arrays(p_w, texts, qv)  # noqa: E731
     for name, path, search, build_note in [
             ("256 handles (evaluate_where) + oc_search(q_filters)", handles_path, search_h, "evaluate_where x 256 inside"),
-            ("256 handles (deletes handle built once) + oc_search(q_filters)", handles_prebuilt_path, search_h,
-             "leaf and combine calls x 256 inside, one prebuilt NOT(deletes)"),
             ("256 programs (compile_where) + oc_search(q_where)", program_path, search_w, "compile_where x 256 inside")]:
         row = {"call": name, "B": B, "limit": LIMIT, "outputs_identical": same,
                "request_path_wall_ms": wall(path, calls), "search_wall_ms": wall(search, calls), "path": build_note}
