@@ -337,6 +337,12 @@ class WhereProgram:
     keep: list = field(default_factory=list)
 
 
+# Operands of one And / Or node that compile_where emits.  A list of parts costs up to _NARY - 1 stack slots above its
+# deepest part, so 8 lets four nested wide lists fit the OC_WHERE_MAX_DEPTH = 32 slots, at one more node per 7 parts
+# beyond the first 8 (a 300-part list: 300 leaves and 43 And / Or nodes).  Lists of up to 8 parts stay one node.
+_NARY = 8
+
+
 def _n(op, field_=0, arg=0, a=0.0, b=0.0, c=0.0, src=None, verts=None):
     return (op, field_, arg, a, b, c, src, verts)
 
@@ -382,9 +388,18 @@ class _Compile:
         return [_n(_lib.OC_WHERE_GEO_POLYGON, 0, int(bool(flt.inside)), src=g._h.value, verts=(la, lo))]
 
     def _nary(self, parts, op):
+        """One And / Or of `parts`, over at most _NARY operands per node: a wider list is folded, the first _NARY parts
+        and then the running value with the next _NARY - 1, so it takes at most _NARY - 1 stack slots more than its
+        deepest part.  Pushing every part before one node refused any list of more than OC_WHERE_MAX_DEPTH parts
+        (tests/test_gpu_where_oracle.py::test_wide_and_or caught it)."""
         if len(parts) == 1:
             return parts[0]
-        return [x for p in parts for x in p] + [_n(op, arg=len(parts))]
+        head, rest = parts[:_NARY], parts[_NARY:]
+        out = [x for p in head for x in p] + [_n(op, arg=len(head))]
+        for i in range(0, len(rest), _NARY - 1):
+            chunk = rest[i:i + _NARY - 1]
+            out += [x for p in chunk for x in p] + [_n(op, arg=len(chunk) + 1)]
+        return out
 
     def and_(self, parts):
         return self._nary(parts, _lib.OC_WHERE_AND)

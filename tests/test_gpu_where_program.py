@@ -1,13 +1,15 @@
 """Where clauses as programs evaluated inside the search call (oc_search_params.q_where, TokenScoreParams.where_programs,
 IndexLoader.where_program, oc_filter_from_where, oc_where_check).
 
-The bitmaps of programs (every leaf kind and op, random trees with geo leaves and deletes, FILTER-only programs, a FILTER
-handle with a dirty tail) are checked against the host restatement of tests/test_where_host.py.  The rule for searches:
-query b's outputs with q_where are byte for byte those it gets with q_filters[b] = the handle evaluate_where builds from
-the same clause.  Checked for oc_search / oc_search_q_sorted / oc_search_q_groups / oc_search_q_facets over fulltext,
-vector and hybrid with mixed per-query parameters, for batches with duplicate programs, unfiltered queries, single
-leaves and FILTER-only programs, for workspace reuse, for every refusal, for the launch count of the where stage and
-through the batcher from many threads."""
+The bitmaps of programs (every leaf kind and op, random trees with geo leaves and deletes, FILTER-only programs, a
+FILTER handle with a dirty tail) are checked against the host restatement of tests/test_where_host.py.  The rule for
+searches: query b's outputs with q_where are byte for byte those it gets with q_filters[b] = the handle evaluate_where
+builds from the same clause.  Both sides of that rule run the same planner and kernels, so it checks the in-call path
+against the handle path only; tests/test_gpu_where_oracle.py checks the in-call programs against bitmaps computed on the
+host.  Checked for oc_search / oc_search_q_sorted / oc_search_q_groups / oc_search_q_facets over fulltext, vector and
+hybrid with mixed per-query parameters, for batches with duplicate programs, unfiltered queries, single leaves and
+FILTER-only programs, for workspace reuse, for every refusal, for the launch count of the where stage and through the
+batcher from many threads."""
 import ctypes as C
 import threading
 
@@ -191,6 +193,9 @@ def _same(a, b, what):
 @pytest.mark.parametrize("B", [1, 48])
 @pytest.mark.parametrize("mode", list(MODES))
 def test_search_identity(wcorpus, fields, mode, B):  # noqa: F811
+    """In-call programs (q_where) give the outputs of q_filters set to the handles evaluate_where builds for the same
+    clauses.  Both come from the same where_plan, so this shows the two paths agree, not that either is right:
+    tests/test_gpu_where_oracle.py compares the in-call programs with independent host bitmaps and the oracle."""
     c = wcorpus
     m = MODES[mode]
     qv, texts = _inputs(B, 700 + B, c["rows"])

@@ -251,7 +251,8 @@ FIELDS = {"b": ("bool", {0: {True}, 1: {False}, 2: {True, False}}), "s": ("strin
           "n": ("number", (np.array([0, 1, 2, 3, 3]), np.array([1.0, 2.0, 3.0, 4.0, -1.0])))}
 
 
-@pytest.mark.parametrize("where, deleted, expected", [
+# (where, deleted, the documents of host_where over FIELDS and 5 documents); also checked against tests/where_spec.py
+TREE_RULE_CASES = [
     ({}, (), None), ({}, (1,), {0, 2, 3, 4}), ({"or": []}, (), None), ({"and": [], "or": []}, (2,), {0, 1, 3, 4}),
     ({"b": True}, (), {0, 2}), ({"b": True}, (2,), {0}), ({"b": False, "s": "x"}, (), set()),
     ({"unknown": True, "b": True}, (), set()), ({"b": True, "unknown": True}, (), set()),
@@ -259,6 +260,9 @@ FIELDS = {"b": ("bool", {0: {True}, 1: {False}, 2: {True, False}}), "s": ("strin
     ({"and": [{}]}, (), set()), ({"not": {}}, (), {0, 1, 2, 3, 4}), ({"b": True, "or": []}, (), set()),
     ({"s": "y", "and": [{"n": {"gt": 1}}], "or": [{"b": False}, {"n": {"lt": 0}}], "not": {"s": "x"}}, (), {1}),
     ({"n": {"between": [3, 2]}}, (), set()), ({"n": True}, (), set()), ({"s": "nope"}, (), set()),
-])
+]
+
+
+@pytest.mark.parametrize("where, deleted, expected", TREE_RULE_CASES)
 def test_tree_rules(where, deleted, expected):
     assert host_where(parse_where(where), FIELDS, 5, deleted) == expected

@@ -10,7 +10,7 @@ import pytest
 
 from oramacore_b200 import _lib
 from oramacore_b200.engine import FacetStore, GeoPointField
-from oramacore_b200.where import compile_where, parse_where
+from oramacore_b200.where import _NARY, compile_where, parse_where
 from test_geo_host import pnpoly
 from test_where_host import FIELDS, host_where
 
@@ -169,3 +169,51 @@ def test_programs_agree_with_the_host_restatement():
             continue
         assert prog.nbits == nbits and len(prog.nodes) <= _lib.OC_WHERE_MAX_NODES
         assert run_program(prog.nodes, sets, geo, nbits, set(range(nbits)) - set(deleted)) == ref, where
+
+
+def _peak(nodes):
+    sp = top = 0
+    for n in nodes:
+        sp += 1 - n[2] if n[0] in (AND, OR) else 0 if n[0] == NOT else 1
+        top = max(top, sp)
+    return top
+
+
+@pytest.mark.parametrize("op", ["and", "or"])
+@pytest.mark.parametrize("n", [2, _NARY, _NARY + 1, 17, 31, 33, 300])
+def test_wide_and_or_lists(op, n):
+    """An And / Or of n parts is folded into nodes of at most _NARY operands: the stack holds at most _NARY - 1 values
+    above the deepest part, and the program is the host restatement's set.  (A list of n > OC_WHERE_MAX_DEPTH parts
+    pushed before one node was refused by the planner.)"""
+    rng = np.random.default_rng(n)
+    nd, nbits = 400, 380
+    fields = _rand_fields(rng, nd)
+    # And over NOT of narrow leaves, Or over narrow leaves: neither result is empty nor everything, and each part matters
+    narrow = [{"n": {"eq": int(v)}} if i % 3 else {"s": f"k{int(v) % 3}"} for i, v in enumerate(rng.integers(-200, 200, n))]
+    narrow[-1] = {"b": True}   # a broad last part, so the last node of the fold changes the result
+    parts = [{"not": p} for p in narrow] if op == "and" else narrow
+    prog, sets, geo = _program({op: parts}, fields, nbits, [])
+    assert all(x[2] <= _NARY for x in prog.nodes if x[0] in (AND, OR))
+    assert _peak(prog.nodes) <= _NARY - 1 + 2   # a part is a leaf, or a leaf and its Not
+    got = run_program(prog.nodes, sets, geo, nbits, set(range(nbits)))
+    assert got == host_where(parse_where({op: parts}), fields, nbits)
+    assert 0 < len(got) < nbits
+    if n > _NARY:   # the parts beyond the first node change the result
+        assert got != host_where(parse_where({op: parts[:_NARY]}), fields, nbits)
+    if n == _NARY:
+        assert [x[0] for x in prog.nodes].count(AND if op == "and" else OR) == 1
+
+
+def test_nested_wide_lists():
+    """Four wide lists nested in each other (the inner one last) fit the stack; each costs _NARY - 1 slots."""
+    rng = np.random.default_rng(4)
+    nd, nbits = 400, 380
+    fields = _rand_fields(rng, nd)
+    leaves = [{"n": {"gt": int(v)}} if i % 2 else {"s": f"k{int(v) % 6}"} for i, v in enumerate(rng.integers(-20, 20, 200))]
+    where = {"or": leaves[:40]}
+    for level, op in enumerate(["and", "or", "and"]):
+        part = leaves[40 * (level + 1): 40 * (level + 2)]
+        where = {op: ([{"not": p} for p in part] if op == "and" else part) + [where]}
+    prog, sets, geo = _program(where, fields, nbits, [])
+    assert _peak(prog.nodes) <= 4 * (_NARY - 1) + 1 <= _lib.OC_WHERE_MAX_DEPTH
+    assert run_program(prog.nodes, sets, geo, nbits, set(range(nbits))) == host_where(parse_where(where), fields, nbits)
