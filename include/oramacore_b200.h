@@ -1025,6 +1025,10 @@ typedef struct {
     float scan_sweep_ms;         /* device time of the sweep launch(es) alone (scan_ms also holds the threshold pass) */
     float rerun_ms;              /* device time of re-running flagged queries (exact sweep + second tail), in device_ms */
     uint32_t scan_rescored;      /* rows re-scored in exact fp32 per query (batch average) by the tensor-core scan */
+    uint32_t bm25_dense_items;   /* dense passes of the register-folded BM25 scorers: one per (query, tile) item with
+                                    hot-term (dense) tokens, one more per re-run after a candidate-buffer overflow  */
+    uint32_t bm25_dense_skipped; /* of those, items whose dense scan was replaced by a count pass: no row scored only by
+                                    hot terms could reach the query's running top-n threshold                      */
 } oc_timing;
 #define OC_SCAN_EXACT 0          /* emb_scan_kernel: exact fp32 sweep (B < 8, limit > 32, tiny stores)          */
 #define OC_SCAN_TC_TF32 1        /* emb_gemm_kernel: wgmma .tf32 on the fp32 rows, one CTA per SM and query group */

@@ -164,7 +164,7 @@ class Timing(C.Structure):
                 ("bm25_postings", C.c_uint64), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64),
                 ("scan_tensor_core", C.c_uint32), ("scan_unproven", C.c_uint32),
                 ("scan_variant", C.c_uint32), ("scan_sweep_ms", C.c_float), ("rerun_ms", C.c_float),
-                ("scan_rescored", C.c_uint32)]
+                ("scan_rescored", C.c_uint32), ("bm25_dense_items", C.c_uint32), ("bm25_dense_skipped", C.c_uint32)]
 
     def as_dict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}

@@ -118,7 +118,7 @@ struct PreDesc {        // one (term, weight) pair shared by several queries of 
     float *dense;       // dense form (hot terms): c scattered into a zeroed float[rows] array, NULL = list form
     uint32_t len;
     float weight, idf;
-    uint32_t pad;
+    uint32_t n_tiles;   // dense form: tiles of the array (where its summary starts, bm25_dense_bits / bm25_dense_bound)
 };
 __device__ __forceinline__ bool f32_is_normal(float x) {
     const uint32_t e = (__float_as_uint(x) >> 23) & 0xffu;
@@ -173,6 +173,9 @@ struct Bm25Params {
     // then holds one bitmap of ok_words words per slot.  Only K3 and K3b read it (such a batch never runs K3c / K3d).
     const uint32_t *q_ok_slot;
     uint64_t ok_words;
+    // NULL, or out: [2] (dense passes, dense passes replaced by a count pass) of the register-folded scorers — summed
+    // over the items, for last_timing()
+    uint32_t *dense_stat;
 };
 // the row bitmap of query q (or of token t in the df pre-pass): the shared one, or its slot's
 __device__ __forceinline__ const uint32_t *row_ok_of(const uint32_t *bits, const uint32_t *slot, uint64_t words, uint32_t q) {
@@ -196,6 +199,24 @@ __host__ __device__ inline size_t bm25_smem_bytes(bool multi, bool threshold, bo
     return b + 64;
 }
 
+// A dense array's summary, in the same allocation right after its float[rows_pad] (rows_pad = n_tiles * TILE):
+//   * a presence bitmap, uint32[rows_pad / 32]: bit r = (c[r] != 0);
+//   * tile_bound, float[n_tiles]: an upper bound of each tile's values — its largest positive c, or 0 (padded to
+//     256 B, so arrays laid end to end keep the alignment of the float4 loads).
+// The register-folded scorers use both to skip the dense scan of an item no dense-only row of which can reach the
+// query's threshold (t3_count).  bm25_precompute_kernel sets them next to each value it stores (the allocation is zeroed
+// first, as the array always was), so they follow every row it leaves at 0 and the "NaN is never stored" rule, and
+// building them costs no launch of its own.
+__host__ __device__ inline uint64_t bm25_dense_bytes(uint32_t n_tiles) {
+    const uint64_t rows_pad = uint64_t(n_tiles) * BM25_TILE;
+    return rows_pad * 4 + rows_pad / 8 + ((uint64_t(n_tiles) * 4 + 255) & ~uint64_t(255));
+}
+__host__ __device__ __forceinline__ const uint32_t *bm25_dense_bits(const float *arr, uint32_t n_tiles) {
+    return reinterpret_cast<const uint32_t *>(arr + size_t(n_tiles) * BM25_TILE);
+}
+__host__ __device__ __forceinline__ const float *bm25_dense_bound(const float *arr, uint32_t n_tiles) {
+    return reinterpret_cast<const float *>(bm25_dense_bits(arr, n_tiles) + size_t(n_tiles) * (BM25_TILE / 32));
+}
 // Zipf query terms repeat across the queries of a batch: the per-posting contribution
 // c = idf*(k+1)*S/(k+S), S = w*tf' of a single-term token depends only on (term, weight), so it is
 // computed ONCE per batch (same rounded ops => bit-identical scores) and the tile kernel only adds:
@@ -214,18 +235,42 @@ __global__ void __launch_bounds__(256) bm25_precompute_kernel(const PreDesc *pre
     const float kp1 = __fadd_rn(k, 1.0f);
     const uint32_t lo = it.y * PRE_CHUNK, hi = min(d.len, lo + PRE_CHUNK);
     const uint2 *src = reinterpret_cast<const uint2 *>(d.src);
-    uint2 *dst = reinterpret_cast<uint2 *>(d.dst);
-    for (uint32_t i = lo + threadIdx.x; i < hi; i += blockDim.x) {
-        const uint2 r = __ldg(src + i);
-        const float ntf = __fmul_rn(d.weight, __uint_as_float(r.y));
-        float c = __int_as_float(0x7fc00000);                  // NaN => skipped (bm25.rs:387,391)
-        if (f32_is_normal(ntf)) c = bm25_sat(ntf, k, kp1, d.idf);
-        if (d.dense) {
-            const bool ok = !row_ok_bits || ((row_ok_bits[r.x >> 5] >> (r.x & 31)) & 1u);
-            if (ok && c == c) d.dense[r.x] = c;
-        } else {
+    if (!d.dense) {
+        uint2 *dst = reinterpret_cast<uint2 *>(d.dst);
+        for (uint32_t i = lo + threadIdx.x; i < hi; i += blockDim.x) {
+            const uint2 r = __ldg(src + i);
+            const float ntf = __fmul_rn(d.weight, __uint_as_float(r.y));
+            float c = __int_as_float(0x7fc00000);              // NaN => skipped (bm25.rs:387,391)
+            if (f32_is_normal(ntf)) c = bm25_sat(ntf, k, kp1, d.idf);
             dst[i] = make_uint2(r.x, __float_as_uint(c));
         }
+        return;
+    }
+    // dense form, warp-uniform trip count (the summary's per-tile maximum is a warp reduction)
+    uint32_t *bits = const_cast<uint32_t *>(bm25_dense_bits(d.dense, d.n_tiles));
+    unsigned int *bound = reinterpret_cast<unsigned int *>(const_cast<float *>(bm25_dense_bound(d.dense, d.n_tiles)));
+    const uint32_t lane = threadIdx.x & 31u;
+    for (uint32_t i0 = lo + (threadIdx.x - lane); i0 < hi; i0 += blockDim.x) {
+        const uint32_t i = i0 + lane;
+        uint32_t row = 0, v = 0;
+        if (i < hi) {
+            const uint2 r = __ldg(src + i);
+            const float ntf = __fmul_rn(d.weight, __uint_as_float(r.y));
+            float c = __int_as_float(0x7fc00000);              // NaN => never stored
+            if (f32_is_normal(ntf)) c = bm25_sat(ntf, k, kp1, d.idf);
+            const bool ok = !row_ok_bits || ((row_ok_bits[r.x >> 5] >> (r.x & 31)) & 1u);
+            row = r.x;
+            if (ok && c == c) {
+                d.dense[row] = c;
+                if (c != 0.f) atomicOr(bits + (row >> 5), 1u << (row & 31u));   // the row's presence bit
+                if (c > 0.f) v = __float_as_uint(c);          // (positive floats order as their bits do)
+            }
+        }
+        // the tile's bound: one atomic per tile the warp's postings fall in (rows ascend: nearly always one)
+        const uint32_t tile = row / BM25_TILE;
+        const uint32_t grp = __match_any_sync(0xffffffffu, tile);
+        const uint32_t m = __reduce_max_sync(grp, v);
+        if (m && lane == uint32_t(__ffs(grp) - 1)) atomicMax(bound + tile, m);
     }
 }
 
@@ -653,7 +698,8 @@ struct ItemTok {            // 32 B
     uint32_t n;             // list: postings in the tile; dense: BM25_TILE (0 = token absent from this tile)
     uint32_t flags;         // TD_PRE / TD_DENSE
     float w, idf;
-    uint32_t bit, pad;
+    uint32_t bit;
+    uint32_t bound;         // dense: float bits of the bound of the tile's contributions (bm25_dense_bound); else unused
 };
 constexpr uint32_t BM25_FLAT_TOK = 4;   // tokens per query the flat descriptors hold (longer queries: in-kernel table build)
 __global__ void __launch_bounds__(256) bm25_flatten_kernel(const Bm25Params p, ItemTok *flat) {
@@ -678,6 +724,7 @@ __global__ void __launch_bounds__(256) bm25_flatten_kernel(const Bm25Params p, I
             if (td.flags & TD_DENSE) {
                 it.ptr = reinterpret_cast<const float *>(td.ptr) + size_t(tile) * BM25_TILE;
                 it.n = td.len ? BM25_TILE : 0;
+                if (td.len) it.bound = __float_as_uint(bm25_dense_bound(reinterpret_cast<const float *>(td.ptr), n_tiles)[tile]);
             } else {
                 const uint32_t *sg = seg + size_t(tk.term_begin) * (n_tiles + 1);
                 const uint32_t lo = sg[tile], hi = sg[tile + 1];
@@ -1081,6 +1128,14 @@ __device__ __noinline__ float t3_fold(const ItemTok *tab, const uint32_t *bm, co
                                          const float k, const float kp1) {
     constexpr uint32_t W = BM25_TILE / 32;
     const uint32_t w = l >> 5, bit = 1u << (l & 31u);
+    // the dense tokens' contributions, loaded together: one memory latency per row, not one per token (when the scan
+    // of the item was skipped, these rows are not in L1)
+    // (registers, picked by selects below: the token loop stays rolled, one copy of t3_find)
+    static_assert(BM25_FLAT_TOK == 4, "t3_fold holds one dense contribution per flat token");
+    auto dense_at = [&](const uint32_t i) {
+        return (tab[i].n && (tab[i].flags & TD_DENSE)) ? __ldg(reinterpret_cast<const float *>(tab[i].ptr) + l) : 0.f;
+    };
+    const float cd0 = dense_at(0), cd1 = dense_at(1), cd2 = dense_at(2), cd3 = dense_at(3);
     float s = 0.f;
 #pragma unroll 1
     for (uint32_t i = 0; i < BM25_FLAT_TOK; i++) {
@@ -1088,7 +1143,7 @@ __device__ __noinline__ float t3_fold(const ItemTok *tab, const uint32_t *bm, co
         if (ni == 0) continue;
         const uint32_t fi = tab[i].flags;
         float ci;
-        if (fi & TD_DENSE) ci = __ldg(reinterpret_cast<const float *>(tab[i].ptr) + l);   // 0.0 = absent
+        if (fi & TD_DENSE) ci = i == 0 ? cd0 : i == 1 ? cd1 : i == 2 ? cd2 : cd3;   // 0.0 = absent
         else {
             uint32_t pay = rec.y;
             if (i != j) {                              // (another non-empty list token: the per-token bitmaps are in use)
@@ -1175,6 +1230,54 @@ __device__ __forceinline__ void t3_scan(const float4 *d0, const float4 *d1, cons
     }
 }
 
+// Skipping the dense part of an item.  A row that no list token holds scores the fold of its dense tokens'
+// contributions in token order, and each contribution is at most its token's tile_bound.  `ub` folds those bounds in
+// the same order with the same rounded adds; round-to-nearest addition is monotone, so ub >= the score of every
+// dense-only row of the item.  When `pos` holds and ub < tau_f, t3_scan would change nothing but the count:
+//   * candidates: every dense-only row fails t3_consider's s >= tau_f, so none is pushed;
+//   * count: under `pos` every stored contribution is > 0 (or a zero, which the bitmap leaves clear) and never NaN,
+//     so a row's fold is != 0 exactly when one of its bits is set — t3_count counts the same rows the scan would;
+//   * maximum: tau only rises, and its final value is attained by n_keep real rows of the query (the seed's rows or
+//     a tile's emitted keys; a key's score is exact).  A skipped row is < the tau_f of its item <= the final tau_f, so
+//     those rows are never skipped, their tiles' tile_max hold them, and the query's maximum over its tiles' tile_max
+//     — all any reader takes from tile_max — is >= the final tau_f > every skipped row;
+//   * minimum: lmin stays 0 under `pos`.
+// The decision must be the same in every thread of the item: t3_count gives thread t whole bitmap words, t3_scan gives
+// it float4 slots, so a mixed decision would count some rows twice and others never.  Hence one threshold per item:
+// K3c shares thread 0's load through shared memory, K3d broadcasts lane 0's (other CTAs raise tau[q] meanwhile, so
+// separate loads could differ).  With a negative weight, idf or k (`pos` false) the item is always scanned.  K3c / K3d never run with matched_bits or
+// row_ft (facets, groups, sortBy), the outputs that would need each row.
+__device__ __forceinline__ float t3_dense_ub(const ItemTok *tab) {
+    float ub = 0.f;
+#pragma unroll
+    for (uint32_t j = 0; j < BM25_FLAT_TOK; j++)
+        if (tab[j].n && (tab[j].flags & TD_DENSE)) ub = __fadd_rn(ub, __uint_as_float(tab[j].bound));
+    return ub;
+}
+// the count pass that replaces t3_scan: rows outside every list token with some dense contribution, from the dense
+// tokens' presence bitmaps (thread t owns the words t, t + STRIDE, ...)
+template <uint32_t STRIDE>
+__device__ __noinline__ uint32_t t3_count(const ItemTok *tab, const uint32_t *touched, const bool any_list, const uint32_t n_tiles,
+                                          const uint32_t tile, const uint32_t tid) {
+    constexpr uint32_t W = BM25_TILE / 32;
+    const uint32_t *bp[BM25_FLAT_TOK];
+#pragma unroll
+    for (uint32_t j = 0; j < BM25_FLAT_TOK; j++)
+        bp[j] = (tab[j].n && (tab[j].flags & TD_DENSE))
+                    ? bm25_dense_bits(reinterpret_cast<const float *>(tab[j].ptr) - size_t(tile) * BM25_TILE, n_tiles) + size_t(tile) * W
+                    : nullptr;
+    uint32_t m = 0;
+#pragma unroll 2
+    for (uint32_t w = tid; w < W; w += STRIDE) {
+        uint32_t u = 0;
+#pragma unroll
+        for (uint32_t j = 0; j < BM25_FLAT_TOK; j++) if (bp[j]) u |= __ldg(bp[j] + w);
+        if (any_list) u &= ~touched[w];
+        m += __popc(u);
+    }
+    return m;
+}
+
 __global__ void __launch_bounds__(BM25_THREADS, 1024 / BM25_THREADS) bm25_tile3_kernel(const Bm25Params p, const ItemTok *flat, unsigned int *work_counter) {
     constexpr uint32_t W = BM25_TILE / 32;                                  // bitmap words per tile
     extern __shared__ __align__(16) uint8_t smem[];
@@ -1187,6 +1290,10 @@ __global__ void __launch_bounds__(BM25_THREADS, 1024 / BM25_THREADS) bm25_tile3_
     __shared__ unsigned int s_maxo2[2], s_mino2[2];
     __shared__ ItemTok s_tab[2][BM25_FLAT_TOK];
     __shared__ uint32_t s_item_cur, s_item_next;
+    __shared__ uint32_t s_dense[2];                        // dense passes, of which skipped (thread 0 only)
+    // the item's running threshold, loaded by thread 0 and double-buffered by item parity: every thread of the CTA
+    // gates by the same value, so the dense-skip decision is block-uniform (t3_count and t3_scan split rows differently)
+    __shared__ unsigned long long s_tau2[2];
 
     const uint32_t tid = threadIdx.x;
     const float kp1 = __fadd_rn(p.k, 1.0f);
@@ -1194,12 +1301,15 @@ __global__ void __launch_bounds__(BM25_THREADS, 1024 / BM25_THREADS) bm25_tile3_
     const uint32_t *okbits = p.row_ok_bits;
 
     for (uint32_t i = tid; i < (BM25_FLAT_TOK + 1) * W; i += BM25_THREADS) touched[i] = 0u;
-    if (tid == 0) { s_item_cur = atomicAdd(work_counter, 1u); s_item_next = atomicAdd(work_counter, 1u); }
+    if (tid == 0) { s_item_cur = atomicAdd(work_counter, 1u); s_item_next = atomicAdd(work_counter, 1u); s_dense[0] = s_dense[1] = 0u; }
     if (tid < 2) { s_cnt2[tid] = 0; s_matched2[tid] = 0; s_maxo2[tid] = f32_ordered(0.f); s_mino2[tid] = f32_ordered(0.f); }
     __syncthreads();
     if (s_item_cur < n_items && tid < BM25_FLAT_TOK) s_tab[0][tid] = flat[size_t(s_item_cur) * BM25_FLAT_TOK + tid];
-    unsigned long long tau_next = 0ull;
-    if (s_item_cur < n_items) { uint32_t t0, q0; bm25_item_decode(p, s_item_cur, t0, q0); tau_next = __ldcg(p.tau + q0); }   // (L2: other CTAs raise it)
+    unsigned long long tau_next = 0ull;                    // (thread 0)
+    if (tid == 0) {
+        s_tau2[0] = 0ull;
+        if (s_item_cur < n_items) { uint32_t t0, q0; bm25_item_decode(p, s_item_cur, t0, q0); s_tau2[0] = __ldcg(p.tau + q0); }   // (L2: other CTAs raise it)
+    }
 
     for (uint32_t par = 0;; par ^= 1u) {
         __syncthreads();                                   // previous item retired: bitmaps clean, table + counters + ids set
@@ -1216,8 +1326,8 @@ __global__ void __launch_bounds__(BM25_THREADS, 1024 / BM25_THREADS) bm25_tile3_
         // in flight during this item: the next item's descriptors and its query's running threshold
         ItemTok nx{};
         if (next < n_items && tid < BM25_FLAT_TOK) nx = flat[size_t(next) * BM25_FLAT_TOK + tid];
-        unsigned long long tau = tau_next;
-        if (next < n_items) { uint32_t tn, qn; bm25_item_decode(p, next, tn, qn); tau_next = __ldcg(p.tau + qn); }
+        unsigned long long tau = s_tau2[par];
+        if (tid == 0 && next < n_items) { uint32_t tn, qn; bm25_item_decode(p, next, tn, qn); tau_next = __ldcg(p.tau + qn); }
 
         // the item's tokens: dense slices in token order; list tokens counted
         const ItemTok *tab = s_tab[par];
@@ -1262,7 +1372,11 @@ __global__ void __launch_bounds__(BM25_THREADS, 1024 / BM25_THREADS) bm25_tile3_
                 __syncthreads();
             }
             // ---------------------------------------- rows outside every list: dense tokens only, folded in registers
-            switch (nd) {
+            // (or only counted, when no such row can reach the threshold)
+            const bool skip = nd && pos && t3_dense_ub(tab) < tau_f;
+            if (nd && tid == 0) { s_dense[0]++; s_dense[1] += skip; }
+            if (skip) matched += t3_count<BM25_THREADS>(tab, touched, any_list, p.n_tiles, tile, tid);
+            else switch (nd) {
                 case 0: break;
                 case 1: t3_scan<1, BM25_THREADS>(d0, d1, d2, d3, touched, any_list, pos, row0, tid, tau, tau_f, s_cnt, tbuf, p.cap, matched, lmax, lmin); break;
                 case 2: t3_scan<2, BM25_THREADS>(d0, d1, d2, d3, touched, any_list, pos, row0, tid, tau, tau_f, s_cnt, tbuf, p.cap, matched, lmax, lmin); break;
@@ -1343,8 +1457,9 @@ __global__ void __launch_bounds__(BM25_THREADS, 1024 / BM25_THREADS) bm25_tile3_
             p.tile_min[slot_base] = f32_unordered(s_mino2[par]);
         }
         if (tid < BM25_FLAT_TOK) s_tab[par ^ 1u][tid] = nx;   // the next item's table
-        if (tid == 0) { s_item_cur = next; s_item_next = next2; }
+        if (tid == 0) { s_item_cur = next; s_item_next = next2; s_tau2[par ^ 1u] = tau_next; }
     }
+    if (tid == 0 && p.dense_stat && s_dense[0]) { atomicAdd(p.dense_stat, s_dense[0]); atomicAdd(p.dense_stat + 1, s_dense[1]); }
 }
 
 // =======================================================================================
@@ -1359,7 +1474,7 @@ struct __align__(16) WarpScratch {
     uint32_t bm[BM25_FLAT_TOK * (BM25_TILE / 32)];
     uint64_t tbuf[BW_CAP];
     ItemTok tab[BM25_FLAT_TOK];
-    uint32_t cnt, pad[3];
+    uint32_t cnt, dense_items, dense_skipped, pad;   // (lane 0: dense passes, of which skipped)
 };
 // the n largest of buf[0, count) (count <= BW_CAP, n <= 32), descending, into buf[0, n); returns the n-th (0 if count < n)
 __device__ __noinline__ unsigned long long warp_keep_top(uint64_t *buf, const uint32_t count, const uint32_t n, const uint32_t lane) {
@@ -1400,7 +1515,7 @@ __global__ void __launch_bounds__(BW_WARPS * 32, 5) bm25_warp_kernel(const Bm25P
 
     for (uint32_t i = lane; i < W; i += 32) touched[i] = 0u;
     for (uint32_t i = lane; i < BM25_FLAT_TOK * W; i += 32) bm[i] = 0u;
-    if (lane == 0) ws.cnt = 0u;
+    if (lane == 0) { ws.cnt = 0u; ws.dense_items = 0u; ws.dense_skipped = 0u; }
     uint32_t item = 0, next = 0;
     if (lane == 0) { item = atomicAdd(work_counter, 1u); next = atomicAdd(work_counter, 1u); }
     item = __shfl_sync(0xffffffffu, item, 0); next = __shfl_sync(0xffffffffu, next, 0);
@@ -1418,7 +1533,9 @@ __global__ void __launch_bounds__(BW_WARPS * 32, 5) bm25_warp_kernel(const Bm25P
         if (lane < BM25_FLAT_TOK) ws.tab[lane] = cur;
         ItemTok nx{};
         if (next < n_items && lane < BM25_FLAT_TOK) nx = flat[size_t(next) * BM25_FLAT_TOK + lane];
-        unsigned long long tau = tau_next;
+        // lane 0's value for every lane: the dense-skip decision must be warp-uniform (t3_count and t3_scan split rows
+        // differently), whatever each lane's load returned
+        unsigned long long tau = __shfl_sync(0xffffffffu, tau_next, 0);
         if (next < n_items) { uint32_t tn, qn; bm25_item_decode(p, next, tn, qn); tau_next = __ldcg(p.tau + qn); }
         __syncwarp();
 
@@ -1459,7 +1576,11 @@ __global__ void __launch_bounds__(BW_WARPS * 32, 5) bm25_warp_kernel(const Bm25P
                 }
                 __syncwarp();
             }
-            switch (nd) {   // rows outside every list: dense tokens only, folded in registers
+            // rows outside every list: dense tokens only, folded in registers (or only counted: see t3_count)
+            const bool skip = nd && pos && t3_dense_ub(tab) < tau_f;
+            if (nd && lane == 0) { ws.dense_items++; ws.dense_skipped += skip; }
+            if (skip) matched += t3_count<32>(tab, touched, any_list, p.n_tiles, tile, lane);
+            else switch (nd) {
                 case 0: break;
                 case 1: t3_scan<1, 32>(d0, d1, d2, d3, touched, any_list, pos, row0, lane, tau, tau_f, &ws.cnt, ws.tbuf, BW_CAP, matched, lmax, lmin); break;
                 case 2: t3_scan<2, 32>(d0, d1, d2, d3, touched, any_list, pos, row0, lane, tau, tau_f, &ws.cnt, ws.tbuf, BW_CAP, matched, lmax, lmin); break;
@@ -1541,6 +1662,7 @@ __global__ void __launch_bounds__(BW_WARPS * 32, 5) bm25_warp_kernel(const Bm25P
         next = __shfl_sync(0xffffffffu, next2, 0);
         __syncwarp();
     }
+    if (lane == 0 && p.dense_stat && ws.dense_items) { atomicAdd(p.dense_stat, ws.dense_items); atomicAdd(p.dense_stat + 1, ws.dense_skipped); }
 }
 
 // ---------------------------------------------------------------------------------------

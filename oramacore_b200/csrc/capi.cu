@@ -2733,7 +2733,7 @@ struct SearchCall {
     unsigned int *tile_counter = nullptr;
     bool did_comm = false;
     // the output blob: [doc B x limit][score B x limit][n B][count B][min B][gflag B]; the host copy adds [g_flag B][rescored B]
-    size_t o_sc = 0, o_n = 0, o_cnt = 0, o_min = 0, o_gflag = 0, out_bytes = 0, o_resc = 0;
+    size_t o_sc = 0, o_n = 0, o_cnt = 0, o_min = 0, o_gflag = 0, out_bytes = 0, o_resc = 0, o_dstat = 0;
     uint8_t *dout = nullptr;
     uint64_t *d_doc = nullptr;
     float *d_score = nullptr;
@@ -3121,13 +3121,13 @@ static int ft_share_dense(SearchCall &k) {
     const char *dense_env = getenv("OC_BM25_DENSE");
     const char *t2_env = getenv("OC_BM25_TILE2");
     const bool dense_on = !k.any_multi && !(dense_env && dense_env[0] == '0') && !share_off && !(t2_env && t2_env[0] == '0');
-    const uint64_t rows_pad = uint64_t(k.n_tiles) * BM25_TILE;
+    const uint64_t dbytes = bm25_dense_bytes(k.n_tiles);   // float[n_tiles * TILE] and its summary (bitmap, tile bounds)
     const uint64_t dense_min = std::max<uint64_t>(512, k.S->n_rows / 16);
     std::vector<uint8_t> u_dense(uniq.size(), 0);
     uint64_t n_dense = 0;
     if (dense_on)
         for (size_t u = 0; u < uniq.size(); u++)
-            if (terms[uniq[u].first_e].len >= dense_min && (n_dense + 1) * rows_pad * 4 <= (size_t(8) << 30)) { u_dense[u] = 1; n_dense++; }
+            if (terms[uniq[u].first_e].len >= dense_min && (n_dense + 1) * dbytes <= (size_t(8) << 30)) { u_dense[u] = 1; n_dense++; }
     uint64_t walked_l = 0, distinct_l = 0;   // what is left for the list form
     for (size_t e = 0; e < terms.size(); e++)
         if (e_to_u[e] != 0xffffffffu && !u_dense[e_to_u[e]]) walked_l += terms[e].len;
@@ -3151,27 +3151,27 @@ static int ft_share_dense(SearchCall &k) {
             }
         std::vector<float *> arr;
         std::vector<uint8_t> build;
-        dense_cache_bind(k, keys, rows_pad * 4, arr, build);
+        dense_cache_bind(k, keys, dbytes, arr, build);
         for (size_t i = 0; i < keys.size(); i++) { u_arr[key_u[i]] = arr[i]; u_kept[key_u[i]] = arr[i] && !build[i]; }
     }
     uint64_t n_buf = 0;
     for (size_t u = 0; u < uniq.size(); u++) n_buf += u_dense[u] && !u_arr[u];
     if (lists) OCTRY(c->pre_post.ensure(distinct_l * 8 + 64));
-    if (n_buf) OCTRY(c->dense_buf.ensure(n_buf * rows_pad * 4));
-    k.dense_bytes = n_buf * rows_pad * 4;
+    if (n_buf) OCTRY(c->dense_buf.ensure(n_buf * dbytes));
+    k.dense_bytes = n_buf * dbytes;
     uint64_t off = 0, doff = 0;
     std::vector<uint64_t> u_off(uniq.size());
     std::vector<uint8_t> u_used(uniq.size(), 0);
     for (size_t u = 0; u < uniq.size(); u++) {
         if (!u_dense[u] && !lists) continue;
         u_used[u] = 1;
-        if (u_dense[u] && !u_arr[u]) { u_arr[u] = c->dense_buf.as<float>() + doff; doff += rows_pad; }
-        if (u_kept[u]) continue;   // a cache hit: nothing to build
+        if (u_dense[u] && !u_arr[u]) { u_arr[u] = c->dense_buf.as<float>() + doff; doff += dbytes / 4; }
+        if (u_kept[u]) continue;   // a cache hit: nothing to build, its summary included
         const TermDesc &td = terms[uniq[u].first_e];
         PreDesc pd{};
         pd.src = td.ptr; pd.len = td.len; pd.weight = td.weight;
         pd.idf = tokens[k.term_token[uniq[u].first_e]].idf;
-        if (u_dense[u]) pd.dense = u_arr[u];
+        if (u_dense[u]) { pd.dense = u_arr[u]; pd.n_tiles = k.n_tiles; }
         else { u_off[u] = off; pd.dst = c->pre_post.as<Posting>() + off; off += td.len; }
         const uint32_t pi = (uint32_t)k.pre_descs.size();
         k.pre_descs.push_back(pd);
@@ -3480,8 +3480,9 @@ static int main_upload(SearchCall &k) {
     k.o_gflag = k.o_min + size_t(B) * 4;                       // sharded: OR over the ranks of the per-query overflow flags
     k.out_bytes = k.o_gflag + ((size_t(B) + 3) & ~size_t(3));
     k.o_resc = k.out_bytes + ((size_t(B) + 3) & ~size_t(3));
+    k.o_dstat = k.o_resc + size_t(B) * 4;
     OCTRY(c->out_blob.ensure(k.out_bytes));
-    OCTRY(c->h_out.ensure(k.o_resc + size_t(B) * 4));
+    OCTRY(c->h_out.ensure(k.o_dstat + 8));
     k.dout = c->out_blob.as<uint8_t>();
     k.d_doc = c->out_blob.as<uint64_t>();
     k.d_score = reinterpret_cast<float *>(k.dout + k.o_sc);
@@ -3593,6 +3594,7 @@ static int bm25_stage(SearchCall &k) {
     bp.cand_cnt = c->cand_cnt.as<uint32_t>(); bp.tile_count = c->tile_cnt.as<uint32_t>();
     bp.tile_max = c->tile_max.as<float>(); bp.tile_min = c->tile_min.as<float>();
     bp.tile_first = 0;
+    bp.dense_stat = k.tile_counter + 2;   // (zeroed with the thresholds)
     if (!k.q_perm.empty()) {
         bp.perm = k.s_perm.at(din);
         uint32_t off = 0, q0 = 0;
@@ -3848,8 +3850,12 @@ static int rerun_checks(SearchCall &k) {
         CU(cudaMemcpyAsync(h + k.out_bytes, c->g_flag.p, k.Bv, cudaMemcpyDeviceToHost, c->stream));
         CU(cudaMemcpyAsync(h + k.o_resc, c->g_resc.p, size_t(k.Bv) * 4, cudaMemcpyDeviceToHost, c->stream));
     }
+    const bool dstat = k.has_ft && k.n_tiles;   // the scorer's dense-pass counters (Bm25Params::dense_stat)
+    if (dstat) CU(cudaMemcpyAsync(h + k.o_dstat, k.tile_counter + 2, 8, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaEventRecord(c->ev[EV_D2H], c->stream));
     CU(cudaStreamSynchronize(c->stream));
+    c->timing.bm25_dense_items = dstat ? reinterpret_cast<const uint32_t *>(h + k.o_dstat)[0] : 0u;
+    c->timing.bm25_dense_skipped = dstat ? reinterpret_cast<const uint32_t *>(h + k.o_dstat)[1] : 0u;
     {   // tensor-core scan: re-run the (rare) queries whose candidate buffers overflowed
         // sharded: every rank must enter the collective the same number of times, so the decision to re-run is
         // taken on the flags all ranks exchanged inside the shard records (no host sync before the collective),

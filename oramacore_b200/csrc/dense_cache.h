@@ -1,7 +1,8 @@
 // dense_cache.h — the dense contribution arrays of hot BM25 terms, kept on the device across search calls.
 //
 // A hot term's array (float[n_tiles * BM25_TILE], the contribution c of each posting scattered to its row, 0 elsewhere;
-// bm25_precompute_kernel) depends only on the string snapshot's postings, the term's field weight and idf, bm25_k
+// bm25_precompute_kernel, followed in the same allocation by its summary, a presence bitmap and per-tile bounds that
+// the same kernel sets: bm25_dense_bytes) depends only on the string snapshot's postings, the term's field weight and idf, bm25_k
 // and bm25_b (the derived postings), and the row bitmap.  Calls without a row bitmap (no filter, no tombstones, no df
 // counted on the device) key the array by those values and reuse it: the same kernel wrote it with the same rounded
 // ops, so a later call reads the bits it would have built.  DESIGN.md §4 "Dense-array cache".

@@ -9,8 +9,10 @@ configuration the script reports
     pass over the 8 batches);
   * from a separate `torch.profiler` run over 8 calls: every kernel, memset and copy by name and stream (count and
     device ms per call), and per call the device time inside the call's window when nothing ran on any stream (idle);
-  * per batch the number of hot terms (a posting in at least every 16th row) and the bytes of their dense arrays,
-    from the corpus, as the library selects them.
+  * per batch the number of hot terms (a posting in at least every 16th row) and the bytes of their dense arrays
+    (with their summaries: presence bitmap and tile maxima), from the corpus, as the library selects them;
+  * per call: the dense passes of the register-folded scorers and the share of them replaced by a count pass
+    (`bm25_dense_items` / `bm25_dense_skipped` of `last_timing()`).
 The card's name, power limit and SM clock limit are read in the same process.  Writes nothing into the tree (the
 traces go to a temporary directory unless --trace-dir names one).
 
@@ -51,7 +53,9 @@ def hot_terms(data, texts, n_rows):
     """Per batch: the distinct hot terms (list length >= max(512, n_rows / 16)) and the bytes of their dense arrays."""
     offs = data.fields[0].term_offsets
     dense_min = max(512, n_rows // 16)
-    rows_pad = (n_rows + TILE - 1) // TILE * TILE
+    n_tiles = (n_rows + TILE - 1) // TILE
+    rows_pad = n_tiles * TILE
+    arr_bytes = rows_pad * 4 + rows_pad // 8 + (n_tiles * 4 + 255) // 256 * 256   # bm25_dense_bytes
     out = []
     for batch in texts:
         ids = set()
@@ -59,7 +63,7 @@ def hot_terms(data, texts, n_rows):
             for t in q.term_id.tolist():
                 if int(offs[t + 1] - offs[t]) >= dense_min:
                     ids.add(t)
-        out.append({"n_dense": len(ids), "dense_bytes": len(ids) * rows_pad * 4})
+        out.append({"n_dense": len(ids), "dense_bytes": len(ids) * arr_bytes})
     return out
 
 
@@ -74,13 +78,19 @@ def set_env(cache, side):
 def timed(ctx, step, calls):
     for k in range(N_BATCHES):   # warm-up: every batch once (the cache, when on, is filled here)
         step(k)
-    t = {}
+    t, items, skipped = {}, 0, 0
     for k in range(calls):
         step(k)
-        for key, v in ctx.last_timing().items():
+        lt = ctx.last_timing()
+        for key, v in lt.items():
             if key.endswith("_ms"):
                 t.setdefault(key, []).append(v)
-    return {k: stats(v) for k, v in t.items() if max(v) > 0}
+        items += lt["bm25_dense_items"]
+        skipped += lt["bm25_dense_skipped"]
+    out = {k: stats(v) for k, v in t.items() if max(v) > 0}
+    out["dense_items_per_call"] = items / calls
+    out["dense_skipped_fraction"] = skipped / items if items else 0.0
+    return out
 
 
 def profiled(step, trace_dir, tag):
