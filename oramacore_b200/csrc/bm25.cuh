@@ -125,26 +125,20 @@ __device__ __forceinline__ bool f32_is_normal(float x) {
     return e != 0u && e != 0xffu;
 }
 
-constexpr uint32_t BM25_CLASSES = 5;   // 4, 3, 2, 1, 0 dense tokens
 struct Bm25Params {
     const TermDesc *terms;
     const TokenDesc *tokens;
     const QueryDesc *queries;
     const uint32_t *term_token;   // [n_term_desc] token index of each expanded term
     const uint32_t *seg;          // [n_term_desc][n_tiles+1]
-    uint32_t n_queries, n_tiles;
+    uint32_t n_queries, n_tiles;  // (tile, query) items are numbered tile-major: item = tile * n_queries + q
     uint64_t n_rows;
-    float k, b;
+    float k;                      // (b is applied by bm25_derive_postings_kernel before the scorers run)
     const uint32_t *row_ok_bits;  // NULL or bitmap over rows (alive AND filter)
     // OMC (search.rs:39-48), sorted by row
     const uint32_t *omc_row;
     const float *omc_mult;
     uint32_t n_omc;
-    // hybrid: vector hits mapped to string rows, [n_queries][v_stride]; 0xffffffff = none
-    const uint32_t *v_row;
-    uint32_t v_stride;
-    float *v_ft;                  // out: fulltext score of each vector hit (0 if absent)
-    uint8_t *v_present;           // out: 1 if the hit's doc is in the fulltext map
     const float *min_hint;        // [n_queries] assumed global min for the rank proxy (0)
     // outputs per (query, tile)
     uint32_t n_keep;              // limit + offset
@@ -155,19 +149,11 @@ struct Bm25Params {
     uint32_t *cand_cnt;           // [n_queries][n_tiles]
     uint32_t *tile_count;         // matched docs
     float *tile_max, *tile_min;   // pre-OMC extrema (fold start 0.0, token_score.rs:398-401)
-    uint32_t tile_first;          // first tile handled by this launch (sharding of launches)
     uint32_t *matched_bits;       // NULL, or out: [n_queries][n_tiles * TILE/32] bitmap of the matched rows (the keys of the
                                   // score map) — what the facet counts run over (read/index/facet.rs:147-209)
-    // item order of the register-folded scorers: queries grouped by their number of dense tokens, most expensive class
-    // first, tile-major inside a class — so the ragged end of the persistent schedule consists of the cheap items.
-    // perm == NULL: natural order (item = tile * n_queries + q)
-    const uint32_t *perm;         // [n_queries] query ids, class by class
-    uint32_t cls_off[BM25_CLASSES];   // first item of each class
-    uint32_t cls_nq[BM25_CLASSES];    // queries in the class
-    uint32_t cls_q0[BM25_CLASSES];    // first perm entry of the class
     // Group mode (the ROWFT instantiations of K3 / K3b; set together with matched_bits): out, [n_queries][n_tiles * TILE]
     // raw fulltext score of every matched row, written where its matched bit is set — slots of unmatched rows are
-    // never written and must be read through the bitmap.  Last member so the other fields keep their offsets.
+    // never written and must be read through the bitmap.
     float *row_ft;
     // per-query where-filters (oc_search_params.q_filters): NULL, or [n_queries] slot of each query in row_ok_bits, which
     // then holds one bitmap of ok_words words per slot.  Only K3 and K3b read it (such a batch never runs K3c / K3d).
@@ -180,14 +166,6 @@ struct Bm25Params {
 // the row bitmap of query q (or of token t in the df pre-pass): the shared one, or its slot's
 __device__ __forceinline__ const uint32_t *row_ok_of(const uint32_t *bits, const uint32_t *slot, uint64_t words, uint32_t q) {
     return (bits && slot) ? bits + size_t(slot[q]) * words : bits;
-}
-__host__ __device__ __forceinline__ void bm25_item_decode(const Bm25Params &p, const uint32_t k, uint32_t &tile, uint32_t &q) {
-    if (!p.perm) { tile = k / p.n_queries; q = k % p.n_queries; return; }
-    uint32_t g = 0;
-    while (g + 1 < BM25_CLASSES && k >= p.cls_off[g + 1]) g++;   // (an empty class has off[g + 1] == off[g]: skipped)
-    const uint32_t local = k - p.cls_off[g], nqg = p.cls_nq[g];
-    tile = local / nqg;
-    q = p.perm[p.cls_q0[g] + local % nqg];
 }
 
 __host__ __device__ inline size_t bm25_smem_bytes(bool multi, bool threshold, bool omc, uint32_t cap) {
@@ -371,7 +349,7 @@ __global__ void __launch_bounds__(BM25_THREADS) bm25_tile_kernel(const Bm25Param
     __shared__ uint32_t s_mbits[BM25_TILE / 32];
 
     const uint32_t q = blockIdx.x % p.n_queries;
-    const uint32_t tile = p.tile_first + blockIdx.x / p.n_queries;
+    const uint32_t tile = blockIdx.x / p.n_queries;
     const uint32_t row0 = tile * BM25_TILE;
     const uint32_t tid = threadIdx.x;
     const QueryDesc qd = p.queries[q];
@@ -527,21 +505,6 @@ __global__ void __launch_bounds__(BM25_THREADS) bm25_tile_kernel(const Bm25Param
         __syncthreads();
         for (uint32_t i = omc_lo + tid; i < omc_hi; i += BM25_THREADS) aux[p.omc_row[i] - row0] = p.omc_mult[i];
         __syncthreads();
-    }
-
-    // ------------------------------------------------ hybrid: report ft of the vector hits
-    if (p.v_row) {
-        for (uint32_t j = tid; j < p.v_stride; j += BM25_THREADS) {
-            const uint32_t vr = p.v_row[size_t(q) * p.v_stride + j];
-            if (vr != 0xffffffffu && vr >= row0 && uint64_t(vr) < uint64_t(row0) + BM25_TILE) {
-                const uint32_t l = vr - row0;
-                bool present;
-                if (THRESH) present = mask[l] != 0u && uint32_t(__popc(mask[l])) >= qd.required;
-                else present = score[l] != 0.f;
-                p.v_ft[size_t(q) * p.v_stride + j] = present ? score[l] : 0.f;
-                p.v_present[size_t(q) * p.v_stride + j] = present ? 1 : 0;
-            }
-        }
     }
 
     // ------------------------------------------------ scan: count, extrema, gated top-n
@@ -710,9 +673,8 @@ __global__ void __launch_bounds__(256) bm25_flatten_kernel(const Bm25Params p, I
     const uint64_t total = uint64_t(n_tiles) * n_queries * BM25_FLAT_TOK;
     if (gid >= total) return;
     const uint32_t j = uint32_t(gid % BM25_FLAT_TOK);
-    const uint64_t item = gid / BM25_FLAT_TOK;
-    uint32_t tile, q;
-    bm25_item_decode(p, uint32_t(item), tile, q);
+    const uint32_t item = uint32_t(gid / BM25_FLAT_TOK);
+    const uint32_t tile = item / n_queries, q = item % n_queries;
     const QueryDesc qd = queries[q];
     ItemTok it{};
     if (j < qd.token_end - qd.token_begin) {
@@ -1308,7 +1270,7 @@ __global__ void __launch_bounds__(BM25_THREADS, 1024 / BM25_THREADS) bm25_tile3_
     unsigned long long tau_next = 0ull;                    // (thread 0)
     if (tid == 0) {
         s_tau2[0] = 0ull;
-        if (s_item_cur < n_items) { uint32_t t0, q0; bm25_item_decode(p, s_item_cur, t0, q0); s_tau2[0] = __ldcg(p.tau + q0); }   // (L2: other CTAs raise it)
+        if (s_item_cur < n_items) s_tau2[0] = __ldcg(p.tau + s_item_cur % p.n_queries);   // (L2: other CTAs raise it)
     }
 
     for (uint32_t par = 0;; par ^= 1u) {
@@ -1318,8 +1280,7 @@ __global__ void __launch_bounds__(BM25_THREADS, 1024 / BM25_THREADS) bm25_tile3_
         const uint32_t next = s_item_next;
         uint32_t next2 = 0;
         if (tid == 0) next2 = atomicAdd(work_counter, 1u);   // consumed at the end of this item
-        uint32_t tile, q;
-        bm25_item_decode(p, item, tile, q);
+        const uint32_t tile = item / p.n_queries, q = item % p.n_queries;
         const uint32_t row0 = tile * BM25_TILE;
         uint32_t *s_cnt = &s_cnt2[par];
         if (tid == 0) { s_cnt2[par ^ 1u] = 0; s_matched2[par ^ 1u] = 0; s_maxo2[par ^ 1u] = f32_ordered(0.f); s_mino2[par ^ 1u] = f32_ordered(0.f); }
@@ -1327,7 +1288,7 @@ __global__ void __launch_bounds__(BM25_THREADS, 1024 / BM25_THREADS) bm25_tile3_
         ItemTok nx{};
         if (next < n_items && tid < BM25_FLAT_TOK) nx = flat[size_t(next) * BM25_FLAT_TOK + tid];
         unsigned long long tau = s_tau2[par];
-        if (tid == 0 && next < n_items) { uint32_t tn, qn; bm25_item_decode(p, next, tn, qn); tau_next = __ldcg(p.tau + qn); }
+        if (tid == 0 && next < n_items) tau_next = __ldcg(p.tau + next % p.n_queries);
 
         // the item's tokens: dense slices in token order; list tokens counted
         const ItemTok *tab = s_tab[par];
@@ -1522,13 +1483,12 @@ __global__ void __launch_bounds__(BW_WARPS * 32, 5) bm25_warp_kernel(const Bm25P
     ItemTok cur{};
     if (item < n_items && lane < BM25_FLAT_TOK) cur = flat[size_t(item) * BM25_FLAT_TOK + lane];
     unsigned long long tau_next = 0ull;
-    if (item < n_items) { uint32_t t0, q0; bm25_item_decode(p, item, t0, q0); tau_next = __ldcg(p.tau + q0); }
+    if (item < n_items) tau_next = __ldcg(p.tau + item % p.n_queries);
 
     while (item < n_items) {
         uint32_t next2 = 0;
         if (lane == 0) next2 = atomicAdd(work_counter, 1u);   // consumed at the end of this item
-        uint32_t tile, q;
-        bm25_item_decode(p, item, tile, q);
+        const uint32_t tile = item / p.n_queries, q = item % p.n_queries;
         const uint32_t row0 = tile * BM25_TILE;
         if (lane < BM25_FLAT_TOK) ws.tab[lane] = cur;
         ItemTok nx{};
@@ -1536,7 +1496,7 @@ __global__ void __launch_bounds__(BW_WARPS * 32, 5) bm25_warp_kernel(const Bm25P
         // lane 0's value for every lane: the dense-skip decision must be warp-uniform (t3_count and t3_scan split rows
         // differently), whatever each lane's load returned
         unsigned long long tau = __shfl_sync(0xffffffffu, tau_next, 0);
-        if (next < n_items) { uint32_t tn, qn; bm25_item_decode(p, next, tn, qn); tau_next = __ldcg(p.tau + qn); }
+        if (next < n_items) tau_next = __ldcg(p.tau + next % p.n_queries);
         __syncwarp();
 
         const float4 *d0 = nullptr, *d1 = nullptr, *d2 = nullptr, *d3 = nullptr;

@@ -19,6 +19,7 @@
 #include <mutex>
 #include <utility>
 #include <string>
+#include <tuple>
 #include <unordered_map>
 #include <unordered_set>
 #include <vector>
@@ -2045,47 +2046,52 @@ static int launch_tile_t(oc_ctx *c, const Bm25Params &bp, uint32_t grid, size_t 
     CU(cudaGetLastError());
     return OC_OK;
 }
-template <bool THRESH, bool OMC, bool ROWFT>
-static int launch_tile2_t(oc_ctx *c, const Bm25Params &bp, size_t smem, cudaStream_t st, const ItemTok *flat, unsigned int *counter) {
-    CU(smem_cfg(c->device, (const void *)bm25_tile2_kernel<THRESH, OMC, ROWFT>, smem));
-    static std::mutex occ_mu;                         // occupancy per (device, shared-memory size): queried once
-    static std::map<std::pair<int, size_t>, int> occ;
+// The grid of a persistent scorer launch, whose blocks pull (tile, query) items from a counter: one block per
+// items_per_block items, but no more blocks than the device holds at once.  Occupancy is queried once per
+// (device, kernel, block size, shared memory).
+static cudaError_t persistent_grid(oc_ctx *c, const void *fn, int threads, size_t smem, uint32_t items_per_block,
+                                   uint64_t items, uint32_t *grid) {
+    static std::mutex mu;
+    static std::map<std::tuple<int, const void *, int, size_t>, int> occ;
+    const auto key = std::make_tuple(c->device, fn, threads, smem);
     int per_sm = 1;
     {
-        std::lock_guard<std::mutex> g(occ_mu);
-        auto it = occ.find(std::make_pair(c->device, smem));
+        std::lock_guard<std::mutex> g(mu);
+        auto it = occ.find(key);
         if (it == occ.end()) {
-            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bm25_tile2_kernel<THRESH, OMC, ROWFT>, BM25_THREADS, smem));
-            occ[std::make_pair(c->device, smem)] = per_sm;
+            const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, threads, smem);
+            if (e != cudaSuccess) return e;
+            occ[key] = per_sm;
         } else per_sm = it->second;
     }
-    const uint64_t items = uint64_t(bp.n_tiles) * bp.n_queries;
-    const uint32_t grid = (uint32_t)std::min<uint64_t>(items, uint64_t(std::max(per_sm, 1)) * c->prop.multiProcessorCount);
+    *grid = (uint32_t)std::min<uint64_t>((items + items_per_block - 1) / items_per_block,
+                                         uint64_t(std::max(per_sm, 1)) * c->prop.multiProcessorCount);
+    return cudaSuccess;
+}
+template <bool THRESH, bool OMC, bool ROWFT>
+static int launch_tile2_t(oc_ctx *c, const Bm25Params &bp, size_t smem, cudaStream_t st, const ItemTok *flat, unsigned int *counter) {
+    const void *fn = (const void *)bm25_tile2_kernel<THRESH, OMC, ROWFT>;
+    CU(smem_cfg(c->device, fn, smem));
+    uint32_t grid;
+    CU(persistent_grid(c, fn, BM25_THREADS, smem, 1, uint64_t(bp.n_tiles) * bp.n_queries, &grid));
     bm25_tile2_kernel<THRESH, OMC, ROWFT><<<grid, BM25_THREADS, smem, st>>>(bp, flat, counter);
     launched(c);
     CU(cudaGetLastError());
     return OC_OK;
 }
 // multi == false (every token resolves to <= 1 term): the posting-centred persistent kernel; else the slot-scan kernel
-static int launch_tile(oc_ctx *c, const Bm25Params &bp_in, uint32_t grid, bool multi, bool thr, bool omc, cudaStream_t st,
+static int launch_tile(oc_ctx *c, const Bm25Params &bp, uint32_t grid, bool multi, bool thr, bool omc, cudaStream_t st,
                        uint32_t max_tokens, unsigned int *counter /* zeroed by the caller */, bool counted_df) {
     const char *env = getenv("OC_BM25_TILE2");
     if (!multi && !(env && env[0] == '0')) {
         // one level of descriptors per (tile, query) item, prefetched by the kernel during the previous item
         const ItemTok *flat = nullptr;
-        const char *fenv = getenv("OC_BM25_FLAT");
         const char *t3e = getenv("OC_BM25_TILE3");
-        const bool can_flat = max_tokens <= BM25_FLAT_TOK && !(fenv && fenv[0] == '0');
+        const bool can_flat = max_tokens <= BM25_FLAT_TOK;
         // counted_df (filter / tombstones / OC_SHARD_COUNT_DF): no token has a host-known idf, so nothing is shared or dense
         // and every hot term arrives as a long posting list — the accumulator kernel walks those at ~10 instructions per
         // posting, the register-folded scorers would fold each posting's row separately
-        const bool use3 = can_flat && !thr && !omc && !counted_df && !bp_in.matched_bits && !(t3e && t3e[0] == '0');
-        Bm25Params bp = bp_in;
-        // OC_BM25_ORDER=1: deal the items of the dense-token queries first and the list-only queries last (a lighter
-        // ragged end of the persistent schedule); measured 1-2 % SLOWER on both bench shapes (the tile-major order of
-        // ALL queries keeps the posting ranges of a tile together in L2), so the natural order is the default
-        const char *oenv = getenv("OC_BM25_ORDER");
-        if (!use3 || !(oenv && oenv[0] == '1')) bp.perm = nullptr;
+        const bool use3 = can_flat && !thr && !omc && !counted_df && !bp.matched_bits && !(t3e && t3e[0] == '0');
         if (can_flat) {
             const uint64_t n_it = uint64_t(bp.n_tiles) * bp.n_queries * BM25_FLAT_TOK;
             OCTRY(c->flat_desc.ensure(n_it * sizeof(ItemTok)));
@@ -2096,21 +2102,7 @@ static int launch_tile(oc_ctx *c, const Bm25Params &bp_in, uint32_t grid, bool m
         }
         if (use3) {
             // plain queries: the register-folded scorer (no accumulator arrays)
-            const size_t smem3 = bm25_tile3_smem_bytes(bp.cap);
-            CU(smem_cfg(c->device, (const void *)bm25_tile3_kernel, smem3));
-            static std::mutex occ3_mu;
-            static std::map<std::pair<int, size_t>, int> occ3;
-            int per_sm = 1;
-            {
-                std::lock_guard<std::mutex> g(occ3_mu);
-                auto it = occ3.find(std::make_pair(c->device, smem3));
-                if (it == occ3.end()) {
-                    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bm25_tile3_kernel, BM25_THREADS, smem3));
-                    occ3[std::make_pair(c->device, smem3)] = per_sm;
-                } else per_sm = it->second;
-            }
             const uint64_t items = uint64_t(bp.n_tiles) * bp.n_queries;
-            const uint32_t g3 = (uint32_t)std::min<uint64_t>(items, uint64_t(std::max(per_sm, 1)) * c->prop.multiProcessorCount);
             const char *seed_env = getenv("OC_BM25_SEED");
             if (bp.n_keep <= 32 && bp.n_tiles > 1 && !(seed_env && seed_env[0] == '0')) {   // warm start of the candidate thresholds
                 bm25_seed_kernel<<<(bp.n_queries * 32 + 255) / 256, 256, 0, st>>>(bp);
@@ -2120,23 +2112,17 @@ static int launch_tile(oc_ctx *c, const Bm25Params &bp_in, uint32_t grid, bool m
             if (bp.n_keep <= 32 && !(wenv && wenv[0] == '0')) {   // a warp per item: no block barriers
                 const size_t smemw = size_t(BW_WARPS) * sizeof(WarpScratch);
                 CU(smem_cfg(c->device, (const void *)bm25_warp_kernel, smemw));
-                static std::mutex occw_mu;
-                static std::map<int, int> occw;
-                int pw = 1;
-                {
-                    std::lock_guard<std::mutex> g(occw_mu);
-                    auto it = occw.find(c->device);
-                    if (it == occw.end()) {
-                        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&pw, bm25_warp_kernel, BW_WARPS * 32, smemw));
-                        occw[c->device] = pw;
-                    } else pw = it->second;
-                }
-                const uint32_t gw = (uint32_t)std::min<uint64_t>((items + BW_WARPS - 1) / BW_WARPS, uint64_t(std::max(pw, 1)) * c->prop.multiProcessorCount);
+                uint32_t gw;
+                CU(persistent_grid(c, (const void *)bm25_warp_kernel, BW_WARPS * 32, smemw, BW_WARPS, items, &gw));
                 bm25_warp_kernel<<<gw, BW_WARPS * 32, smemw, st>>>(bp, flat, counter);
                 launched(c);
                 CU(cudaGetLastError());
                 return OC_OK;
             }
+            const size_t smem3 = bm25_tile3_smem_bytes(bp.cap);
+            CU(smem_cfg(c->device, (const void *)bm25_tile3_kernel, smem3));
+            uint32_t g3;
+            CU(persistent_grid(c, (const void *)bm25_tile3_kernel, BM25_THREADS, smem3, 1, items, &g3));
             bm25_tile3_kernel<<<g3, BM25_THREADS, smem3, st>>>(bp, flat, counter);
             launched(c);
             CU(cudaGetLastError());
@@ -2157,8 +2143,6 @@ static int launch_tile(oc_ctx *c, const Bm25Params &bp_in, uint32_t grid, bool m
             default: return launch_tile2_t<true, true, false>(c, bp, smem, st, flat, counter);
         }
     }
-    Bm25Params bp = bp_in;
-    bp.perm = nullptr;
     const size_t smem = bm25_smem_bytes(multi, thr, omc, bp.cap);
     const int sel = (multi ? 4 : 0) | (thr ? 2 : 0) | (omc ? 1 : 0);
     if (bp.row_ft) switch (sel) {   // group mode: the matched rows' scores too
@@ -2676,9 +2660,9 @@ struct SearchCall {
     // batch in c->dense_buf, dense_new: those built into the ctx's dense-array cache (both zeroed before the precompute
     // kernel fills them); dense_seen: the snapshots the cache's sweep looked at (released after the ctx lock);
     // term_key: (field << 32 | term id) of each expanded term;
-    // tok_slot: per-query filters, the fulltext slot of each token's query; q_perm: the register-folded scorers' item order
+    // tok_slot: per-query filters, the fulltext slot of each token's query
     bool multi_rank = false, tombs = false, thr = false, count_df = false, any_multi = false, need_df = false, derived_now = false;
-    uint32_t n_tiles = 0, max_tokens = 0, cls_nq[BM25_CLASSES] = {0, 0, 0, 0, 0};
+    uint32_t n_tiles = 0, max_tokens = 0;
     uint64_t dense_bytes = 0, postings_walked = 0;
     std::vector<DenseEntry *> dense_new;
     std::vector<std::shared_ptr<StrSnap>> dense_seen;
@@ -2686,7 +2670,7 @@ struct SearchCall {
     std::vector<TokenDesc> tokens;
     std::vector<QueryDesc> queries;
     std::vector<uint64_t> term_key;
-    std::vector<uint32_t> term_token, tok_slot, q_perm;
+    std::vector<uint32_t> term_token, tok_slot;
     std::vector<uint8_t> tok_need_df;
     std::vector<PreDesc> pre_descs;
     std::vector<uint2> pre_items;
@@ -2712,7 +2696,7 @@ struct SearchCall {
     Packer pk0, pk, *first = nullptr;
     DevBuf *first_blob = nullptr;
     Slot<uint64_t> s_flt, s_omcd;
-    Slot<uint32_t> s_qslot, s_qslot_ft, s_ttok, s_tslot, s_perm, s_omcr;
+    Slot<uint32_t> s_qslot, s_qslot_ft, s_ttok, s_tslot, s_omcr;
     Slot<float> s_omcm, s_omcrm;
     Slot<uint2> s_fpairs, s_pitems;
     Slot<RowsOkSlot> s_qslots;
@@ -3186,31 +3170,6 @@ static int ft_share_dense(SearchCall &k) {
     return OC_OK;
 }
 
-// item order of the register-folded scorers (Bm25Params::perm): queries by their number of dense tokens, descending
-static void bm25_item_order(SearchCall &k) {
-    const uint32_t B = k.B;
-    std::vector<uint8_t> nd_q(B, 0);
-    for (uint32_t q = 0; q < B; q++) {
-        uint32_t nd = 0;
-        for (uint32_t t = k.queries[q].token_begin; t < k.queries[q].token_end; t++)
-            if (k.tokens[t].term_end > k.tokens[t].term_begin && (k.terms[k.tokens[t].term_begin].flags & TD_DENSE) &&
-                k.terms[k.tokens[t].term_begin].len)
-                nd++;
-        nd_q[q] = (uint8_t)std::min<uint32_t>(nd, BM25_CLASSES - 1);
-    }
-    // (used with OC_BM25_ORDER=1 only.)  TWO classes: every query with a dense token (one tile-major pass over the dense
-    // arrays: one class per dense-token count re-streamed those arrays once per class and cost the 10M-document
-    // workload 20 %), then the list-only queries, whose items are cheap and touch no dense array.  Inside the first
-    // class the queries are sorted by their number of dense tokens, descending.
-    auto cls_of = [&](uint32_t q) { return nd_q[q] ? 0u : BM25_CLASSES - 1; };
-    for (uint32_t q = 0; q < B; q++) k.cls_nq[cls_of(q)]++;
-    k.q_perm.resize(B);
-    uint32_t at[BM25_CLASSES], acc = 0;
-    for (uint32_t g = 0; g < BM25_CLASSES; g++) { at[g] = acc; acc += k.cls_nq[g]; }
-    for (int nd = BM25_CLASSES - 1; nd >= 0; nd--)
-        for (uint32_t q = 0; q < B; q++) if (nd_q[q] == nd) k.q_perm[at[cls_of(q)]++] = q;
-}
-
 // The fulltext descriptors: terms, tokens and queries, and each token's idf where the host knows it.
 static int ft_descriptors(SearchCall &k) {
     oc_ctx *c = k.c; const oc_search_params *p = k.p;
@@ -3321,14 +3280,6 @@ static int ft_stream(SearchCall &k) {
     return OC_OK;
 }
 
-// The sharing / dense selection and the scorers' item order.
-static int ft_share(SearchCall &k) {
-    if (!k.has_ft) return OC_OK;
-    if (!k.per_q) OCTRY(ft_share_dense(k));
-    if (!k.any_multi && k.max_tokens <= BM25_FLAT_TOK) bm25_item_order(k);
-    return OC_OK;
-}
-
 // OMC rows for the tile kernel: the documents' string rows, ascending
 static int omc_plan(SearchCall &k) {
     const oc_search_params *p = k.p; const StrSnap *S = k.S;
@@ -3430,7 +3381,6 @@ static int main_upload(SearchCall &k) {
     }
     if (!k.has_v) add_first_tables(k);
     if (k.per_q && !k.tok_slot.empty()) k.s_tslot = pk.add(k.tok_slot.data(), k.tok_slot.size());
-    if (!k.q_perm.empty()) k.s_perm = pk.add(k.q_perm.data(), k.q_perm.size());
     Slot<uint64_t> s_pdoc;
     Slot<uint32_t> s_ppos, s_pcnt;
     if (k.pin_items) {
@@ -3578,31 +3528,19 @@ static int bm25_stage(SearchCall &k) {
     bp.term_token = k.s_ttok.at(din);
     bp.seg = c->seg.as<uint32_t>();
     bp.n_queries = B; bp.n_tiles = n_tiles; bp.n_rows = S->n_rows;
-    bp.k = p->bm25_k; bp.b = p->bm25_b;
+    bp.k = p->bm25_k;
     bp.row_ok_bits = k.row_ok;
     if (k.per_q) { bp.q_ok_slot = k.qfj.d_q_slot_ft; bp.ok_words = ok_words; }
     bp.omc_row = p->omc ? k.omc_row_dev : k.s_omcr.at(din);
     bp.omc_mult = p->omc ? k.omc_row_mult_dev : k.s_omcrm.at(din);
     bp.n_omc = k.n_omc_rows;
-    bp.v_row = nullptr;            // the hybrid lookups are point lookups (bm25_point_kernel)
-    bp.v_stride = k.vlimit;
-    bp.v_ft = nullptr; bp.v_present = nullptr;
     bp.min_hint = k.min_hint_dev;
     bp.n_keep = n_keep; bp.cap = k.cap;
     bp.tau = c->tau.as<unsigned long long>();
     bp.cand_key = c->cand_key.as<uint64_t>(); bp.cand_ft = c->cand_ft.as<float>();
     bp.cand_cnt = c->cand_cnt.as<uint32_t>(); bp.tile_count = c->tile_cnt.as<uint32_t>();
     bp.tile_max = c->tile_max.as<float>(); bp.tile_min = c->tile_min.as<float>();
-    bp.tile_first = 0;
     bp.dense_stat = k.tile_counter + 2;   // (zeroed with the thresholds)
-    if (!k.q_perm.empty()) {
-        bp.perm = k.s_perm.at(din);
-        uint32_t off = 0, q0 = 0;
-        for (uint32_t g = 0; g < BM25_CLASSES; g++) {
-            bp.cls_off[g] = off; bp.cls_nq[g] = k.cls_nq[g]; bp.cls_q0[g] = q0;
-            off += k.cls_nq[g] * n_tiles; q0 += k.cls_nq[g];
-        }
-    }
     const SearchReq &r = k.r;
     if (r.fj || r.gj || r.sj) {   // facets / groups / sortBy: the tile kernels also emit the bitmap of matched rows (every (query, tile) item writes its 256 words)
         OCTRY(c->mbits.ensure(size_t(B) * std::max<uint32_t>(n_tiles, 1) * (BM25_TILE / 32) * 4));
@@ -3996,7 +3934,7 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const SearchReq &r) 
     OCTRY(vector_first(k));
     OCTRY(ft_descriptors(k));
     OCTRY(ft_stream(k));
-    OCTRY(ft_share(k));
+    if (k.has_ft && !k.per_q) OCTRY(ft_share_dense(k));
     OCTRY(omc_plan(k));
     sort_group_plan(k);
     OCTRY(main_upload(k));
