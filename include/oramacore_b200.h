@@ -71,7 +71,8 @@ int oc_device_info(oc_ctx *ctx, int *sm_count, size_t *hbm_bytes, char *name, si
 #define OC_SHARD_TOMBSTONES 2
 #define OC_SHARD_COUNT_DF 4      /* count corpus df across ranks (one ncclAllReduce) instead of using the per-term
                                     global_df tables: required, on EVERY rank, while any rank's string store lacks
-                                    them (an oc_str_commit on a shard drops its table) */
+                                    them (an oc_str_commit on a shard drops its table until oc_str_sync_global
+                                    rebuilds it) */
 #define OC_COMM_ID_BYTES 128
 int oc_comm_unique_id(uint8_t out_id[OC_COMM_ID_BYTES]);
 int oc_comm_init(oc_ctx *ctx, int world_size, int rank, const uint8_t id[OC_COMM_ID_BYTES]);
@@ -163,7 +164,9 @@ void oc_str_destroy(oc_str *s);
 int oc_str_set_rows(oc_str *s, uint64_t n_rows, const uint64_t *row_doc_ids, uint64_t document_count);
 /* Postings of one field: term t owns [term_offsets[t], term_offsets[t+1]); rows ascending,
  * unique per term. avg_field_len = info().avg_field_length (string_field.rs:228-235),
- * global when sharded. global_df: NULL, or per-term corpus df across all shards. */
+ * global when sharded. global_df: NULL, or per-term corpus df across all shards (n_terms entries; a table read back
+ * with oc_str_read_global_df may be longer than the field: pad term_offsets with its last entry to that size).
+ * A shard loaded without tables gets them, and the corpus-wide averages, from oc_str_sync_global. */
 int oc_str_load_field(oc_str *s, uint32_t field, float avg_field_len, uint32_t n_terms,
                       const uint64_t *term_offsets, const uint32_t *post_row, const uint16_t *post_tf,
                       const uint16_t *post_len, const uint32_t *global_df);
@@ -175,7 +178,8 @@ int oc_str_insert(oc_str *s, uint32_t field, uint64_t doc_id, uint16_t field_len
                   const uint32_t *term_ids, const uint16_t *tfs);
 /* == compact(version) (string_field.rs:186-191): merges pending inserts / deletes into the NEXT snapshot of the
  * device-resident layout (rows = ascending doc ids; avg_field_len and document_count refreshed unless the caller
- * owns the corpus-wide values, see oc_str_set_global) and publishes it with a pointer swap — the reference's
+ * owns the corpus-wide values, see oc_str_set_global; a shard's corpus-wide df tables are dropped: call
+ * oc_str_sync_global on every rank afterwards) and publishes it with a pointer swap — the reference's
  * CURRENT + versions/<n> scheme (embedding_field.rs:91-95).  The build runs WITHOUT the context lock on the
  * store's own stream: oc_search keeps serving the previous version meanwhile.  A failed commit changes nothing
  * (the pending ops stay queued).  One commit at a time per store.  The merge runs on the device: its cost is
@@ -214,6 +218,36 @@ int oc_str_delete(oc_str *s, const uint64_t *doc_ids, uint64_t n);
  * caller's values instead of recomputing local ones (avg_field_len == NULL: averages stay locally computed).
  * Call again after commits to refresh them. */
 int oc_str_set_global(oc_str *s, uint64_t document_count, const float *avg_field_len);
+/* Rebuilds a shard's corpus-wide df tables and average field lengths from the stores of every rank of the ctx's comm
+ * group (oc_comm_init / oc_comm_init_local): a collective.  Every rank calls it on its store after its own
+ * oc_str_commit returned, at the same point of its sequence of sharded calls.  Under the ctx lock, on the ctx stream:
+ *   1. the ranks all-gather {n_fields, rows, snapshot version}: different n_fields, or 2^32 rows or more in all (df
+ *      is u32), give OC_ERR_INVALID on every rank;
+ *   2. they all-gather each field's n_terms, and T_f = the largest;
+ *   3. each rank writes the list lengths of its published snapshot (tombstoned rows included), zero-padded to T_f,
+ *      and per field the sum and count of its non-zero row lengths (one length per row, read from the postings on
+ *      the device, exact in u64), all-gathers those sums with its allocation / kernel status (a bad one on any rank
+ *      is every rank's return code, OC_ERR_OOM or OC_ERR_CUDA), and all-reduces the df buffer (sum T_f counters);
+ *   4. installs on the snapshot read in 3: each field's df table (T_f entries: a term this shard has no posting of
+ *      counts as an empty list, so every rank takes the same df decisions), avg_field_len = the sums' quotient as
+ *      oc_str_commit computes it (a field without a non-zero length keeps its value), a new snapshot identity.
+ * A rank whose ctx has no comm gets OC_ERR_COMM; a refused call changes nothing and leaves the group usable.
+ * N (document_count) stays the caller's: it also counts documents with no string field.  A later oc_str_commit
+ * drops the tables again (OC_SHARD_COUNT_DF keeps its meaning) and handles the averages as before; a commit in
+ * flight during the sync publishes after it the same way.  oc_str_set_global(N, NULL) keeps tables and averages.
+ * out (may be NULL): */
+typedef struct {
+    uint64_t version;          /* the snapshot the values were installed on                                  */
+    uint64_t rows_global;      /* sum of the ranks' rows                                                     */
+    uint64_t bytes_reduced;    /* this rank's contribution: df table entries x 4 + the length pairs (16 B each) */
+    float device_ms;           /* CUDA-event time of the length sums and of the df all-reduce with its read-back */
+    float wall_ms;             /* the whole call                                                              */
+} oc_str_sync_t;
+int oc_str_sync_global(oc_str *s, oc_str_sync_t *out);
+/* Host read-back of one field's installed df table: df NULL -> *n_terms = its size (0: no table); otherwise *n_terms
+ * is df's capacity on entry (too small: OC_ERR_INVALID after writing the size).  The array oc_str_load_field's
+ * global_df takes, so a persisted shard reloads with it. */
+int oc_str_read_global_df(oc_str *s, uint32_t field, uint32_t *n_terms, uint32_t *df);
 
 typedef struct {
     uint64_t total_documents;  /* rows                              */

@@ -39,7 +39,7 @@ EXPORTED_SYMBOLS = [
     "oc_last_error", "oc_version", "oc_abi_sizes", "oc_init", "oc_shutdown", "oc_device_info", "oc_comm_unique_id",
     "oc_comm_init", "oc_comm_init_local", "oc_comm_p2p_export", "oc_comm_p2p_import", "oc_emb_create", "oc_emb_destroy", "oc_emb_reserve", "oc_emb_insert", "oc_emb_delete", "oc_emb_compact",
     "oc_emb_info", "oc_emb_search", "oc_str_create", "oc_str_destroy", "oc_str_set_rows", "oc_str_load_field",
-    "oc_str_insert", "oc_str_commit", "oc_str_commit_ex", "oc_str_read_rows", "oc_str_read_field", "oc_str_delete", "oc_str_info", "oc_str_set_global", "oc_search", "oc_pinned_alloc", "oc_pinned_free", "oc_last_timing", "oc_launch_count",
+    "oc_str_insert", "oc_str_commit", "oc_str_commit_ex", "oc_str_read_rows", "oc_str_read_field", "oc_str_delete", "oc_str_info", "oc_str_set_global", "oc_str_sync_global", "oc_str_read_global_df", "oc_search", "oc_pinned_alloc", "oc_pinned_free", "oc_last_timing", "oc_launch_count",
     "oc_batcher_create", "oc_batcher_create2", "oc_batcher_destroy", "oc_batcher_search", "oc_batcher_search_sorted", "oc_batcher_search_groups",
     "oc_batcher_search_faceted", "oc_batcher_stats",
     "oc_filter_from_ids", "oc_filter_from_bits", "oc_filter_and", "oc_filter_or", "oc_filter_not", "oc_filter_count",
@@ -83,6 +83,14 @@ class EmbCompact(C.Structure):   # oc_emb_compact_t
 class StrCommit(C.Structure):   # oc_str_commit_t
     _fields_ = [("rows_before", C.c_uint64), ("rows_after", C.c_uint64), ("postings_before", C.c_uint64),
                 ("postings_after", C.c_uint64), ("pending_postings", C.c_uint64), ("workspace_bytes", C.c_uint64),
+                ("device_ms", C.c_float), ("wall_ms", C.c_float)]
+
+    def as_dict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+class StrSync(C.Structure):   # oc_str_sync_t
+    _fields_ = [("version", C.c_uint64), ("rows_global", C.c_uint64), ("bytes_reduced", C.c_uint64),
                 ("device_ms", C.c_float), ("wall_ms", C.c_float)]
 
     def as_dict(self):
@@ -228,6 +236,8 @@ def lib():
     L.oc_str_read_rows.argtypes = [vp, C.POINTER(u64), vp, C.POINTER(u64), C.POINTER(u64)]
     L.oc_str_read_field.argtypes = [vp, u32, C.POINTER(f32), C.POINTER(u32), C.POINTER(u64), vp, vp, vp, vp]
     L.oc_str_set_global.argtypes = [vp, u64, vp]
+    L.oc_str_sync_global.argtypes = [vp, C.POINTER(StrSync)]
+    L.oc_str_read_global_df.argtypes = [vp, u32, C.POINTER(u32), vp]
     L.oc_str_delete.argtypes = [vp, vp, u64]
     L.oc_str_info.argtypes = [vp, C.POINTER(StrInfo)]
     L.oc_search.argtypes = [vp, vp, vp, C.POINTER(SearchParams), vp, vp, vp, vp]

@@ -214,6 +214,8 @@ struct oc_ctx {
     // oc_emb_compact: the dead-row bitmap with its scan, and the staging window the rows move through (held for the
     // call only: a compaction is rare and its window is large)
     DevBuf cmp_scan, cmp_stage;
+    // oc_str_sync_global: the staging of its small gathers (header, term counts, length sums)
+    DevBuf sync_buf;
     // the dense contribution arrays of hot terms, kept across calls (dense_cache.h)
     DenseCache dense_cache;
     // oc_dict_resolve_q: the mirror of each dictionary resolved on this ctx, by dictionary serial (dict_dev.cuh), and
@@ -1754,6 +1756,155 @@ extern "C" int oc_str_info(oc_str *s, oc_str_info_t *out) {
     return OC_OK;
 }
 
+// The corpus-wide df tables and averages of a sharded store, rebuilt by a collective over the ctx's comm group (see the
+// header for the steps).  Every rank decides from gathered facts only, so all ranks return the same code and call the
+// same collectives.  The installed values change host fields of the snapshot a commit in flight may be reading as its
+// base: the df table (no commit reads it), avg_len (as oc_str_set_global does) and the identity; never term_offsets.
+extern "C" int oc_str_sync_global(oc_str *s, oc_str_sync_t *out) {
+    if (!s) return fail(OC_ERR_INVALID, "str is NULL");
+    const auto wall0 = std::chrono::steady_clock::now();
+    oc_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> g(c->mu);
+    if (!c->comm.comm && !c->comm.local) return fail(OC_ERR_COMM, "oc_str_sync_global without oc_comm_init");
+    const int W = c->comm.world;
+    std::shared_ptr<StrSnap> snap = str_snapshot(s);
+    const StrSnap &S = *snap;
+    const uint32_t nf = (uint32_t)S.fields.size();
+    std::string err;
+    auto gather = [&](const void *mine, void *all, size_t bytes) -> int {   // through c->sync_buf: [send | W recv]
+        uint8_t *d = c->sync_buf.as<uint8_t>();
+        CU(cudaMemcpyAsync(d, mine, bytes, cudaMemcpyHostToDevice, c->stream));
+        if (!c->comm.all_gather(d, d + bytes, bytes, c->stream, &err)) return fail(OC_ERR_COMM, "%s", err.c_str());
+        CU(cudaMemcpyAsync(all, d + bytes, bytes * W, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        return OC_OK;
+    };
+    // 1. handshake: the exchange buffer is sized for the largest of the three gathers at this rank's n_fields (a rank
+    // with another n_fields leaves after the handshake, before the gathers that depend on it)
+    struct Hdr { uint32_t n_fields, pad; uint64_t rows, version; };
+    const size_t max_bytes = std::max<size_t>(sizeof(Hdr), 8 + size_t(nf) * 16);
+    CU(cudaSetDevice(c->device));
+    OCTRY(c->sync_buf.ensure(max_bytes * (W + 1)));
+    Hdr me{nf, 0, S.n_rows, S.version};
+    std::vector<Hdr> hdr(W);
+    OCTRY(gather(&me, hdr.data(), sizeof(Hdr)));
+    uint64_t rows_global = 0;
+    bool same_nf = true;
+    for (int r = 0; r < W; r++) {
+        same_nf = same_nf && hdr[r].n_fields == nf;
+        rows_global += hdr[r].rows;
+    }
+    if (!same_nf) return fail(OC_ERR_INVALID, "oc_str_sync_global: the ranks' stores have different numbers of fields");
+    if (rows_global > 0xffffffffull) return fail(OC_ERR_INVALID, "oc_str_sync_global: %llu rows in all: df is 32-bit",
+                                                 (unsigned long long)rows_global);
+    // 2. term spaces
+    std::vector<uint32_t> nt(nf), nt_all(size_t(W) * nf);
+    for (uint32_t fi = 0; fi < nf; fi++) nt[fi] = S.fields[fi].n_terms;
+    if (nf) OCTRY(gather(nt.data(), nt_all.data(), size_t(nf) * 4));
+    std::vector<uint64_t> df_off(size_t(nf) + 1, 0);   // field fi's table in the df buffer
+    for (uint32_t fi = 0; fi < nf; fi++) {
+        uint32_t t = 0;
+        for (int r = 0; r < W; r++) t = std::max(t, nt_all[size_t(r) * nf + fi]);
+        df_off[fi + 1] = df_off[fi] + t;
+    }
+    const uint64_t n_df = df_off[nf];
+    // 3. this rank's list lengths and length sums; the status of this part travels with the sums
+    struct Pair { unsigned long long len_sum, len_cnt; };
+    std::vector<uint32_t> df(n_df, 0);
+    for (uint32_t fi = 0; fi < nf; fi++) {
+        const StrField &f = S.fields[fi];
+        for (uint32_t t = 0; t < f.n_terms; t++) df[df_off[fi] + t] = (uint32_t)(f.term_offsets[t + 1] - f.term_offsets[t]);
+    }
+    std::vector<uint8_t> mine(8 + size_t(nf) * 16, 0);   // {status, pad, Pair[nf]}
+    Pair *pairs = reinterpret_cast<Pair *>(mine.data() + 8);
+    uint8_t *ws = nullptr;   // [df u32 x n_df | Pair x nf | row lengths u64 x n_rows]
+    struct Free { uint8_t *&p; oc_ctx *c; ~Free() { if (p) { cudaStreamSynchronize(c->stream); cudaFree(p); } } } wfree{ws, c};
+    const size_t o_pair = (n_df * 4 + 255) & ~size_t(255), o_row = o_pair + ((size_t(nf) * 16 + 255) & ~size_t(255));
+    auto local = [&]() -> int {
+        CU(cudaMalloc(&ws, o_row + S.n_rows * 8 + 8));
+        unsigned long long *d_pair = reinterpret_cast<unsigned long long *>(ws + o_pair), *row_key = reinterpret_cast<unsigned long long *>(ws + o_row);
+        CU(cudaEventRecord(c->ev[EV_BM0], c->stream));
+        if (n_df) CU(cudaMemcpyAsync(ws, df.data(), n_df * 4, cudaMemcpyHostToDevice, c->stream));
+        CU(cudaMemsetAsync(d_pair, 0, size_t(nf) * 16, c->stream));
+        const unsigned max_grid = (unsigned)c->prop.multiProcessorCount * 8;
+        auto blocks = [&](uint64_t n) { return (unsigned)std::min<uint64_t>(max_grid, std::max<uint64_t>(1, (n + SC_THREADS - 1) / SC_THREADS)); };
+        for (uint32_t fi = 0; fi < nf; fi++) {
+            const StrField &f = S.fields[fi];
+            if (!f.n_post || !S.n_rows) continue;
+            CU(cudaMemsetAsync(row_key, 0, S.n_rows * 8, c->stream));
+            sc_row_len_kernel<<<blocks(f.n_post), SC_THREADS, 0, c->stream>>>(f.n_post, f.raw, row_key);
+            sc_len_sum_kernel<<<blocks(S.n_rows), SC_THREADS, 0, c->stream>>>((uint32_t)S.n_rows, row_key, d_pair + 2 * fi);
+            launched(c); launched(c);
+        }
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(pairs, d_pair, size_t(nf) * 16, cudaMemcpyDeviceToHost, c->stream));
+        CU(cudaEventRecord(c->ev[EV_BM1], c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        return OC_OK;
+    };
+    const int32_t st = local();
+    const std::string local_err = st == OC_OK ? "" : oc_last_error();
+    memcpy(mine.data(), &st, 4);
+    // 4. collectives: the statuses and sums first, so that a failed rank stops every rank before the all-reduce
+    std::vector<uint8_t> all(mine.size() * W);
+    OCTRY(gather(mine.data(), all.data(), mine.size()));
+    std::vector<Pair> tot(nf, Pair{0, 0});
+    for (int r = 0; r < W; r++) {
+        int32_t rs;
+        memcpy(&rs, all.data() + r * mine.size(), 4);
+        if (rs != OC_OK) return fail(rs, "oc_str_sync_global: rank %d: %s", r, r == c->comm.rank ? local_err.c_str() : "its device work failed");
+        const Pair *pr = reinterpret_cast<const Pair *>(all.data() + r * mine.size() + 8);
+        for (uint32_t fi = 0; fi < nf; fi++) { tot[fi].len_sum += pr[fi].len_sum; tot[fi].len_cnt += pr[fi].len_cnt; }
+    }
+    CU(cudaEventRecord(c->ev[EV_COMM0], c->stream));
+    if (n_df) {
+        if (!c->comm.all_reduce_sum_u32(ws, ws, n_df, c->stream, &err)) return fail(OC_ERR_COMM, "%s", err.c_str());
+        CU(cudaMemcpyAsync(df.data(), ws, n_df * 4, cudaMemcpyDeviceToHost, c->stream));
+    }
+    CU(cudaEventRecord(c->ev[EV_COMM1], c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    // 5. install
+    {
+        std::lock_guard<std::mutex> g2(s->mu);
+        StrSnap &D = *snap;
+        D.ident = next_snap_ident();
+        for (uint32_t fi = 0; fi < nf; fi++) {
+            StrField &f = D.fields[fi];
+            f.global_df.assign(df.begin() + df_off[fi], df.begin() + df_off[fi + 1]);
+            if (!tot[fi].len_cnt) continue;
+            const float avg = (float)((double)tot[fi].len_sum / (double)tot[fi].len_cnt);   // as oc_str_commit_ex
+            if (f.avg_len != avg) { f.avg_len = avg; f.b_cached = -1.f; }
+        }
+    }
+    if (out) {
+        float a = 0, b = 0;
+        cudaEventElapsedTime(&a, c->ev[EV_BM0], c->ev[EV_BM1]);
+        cudaEventElapsedTime(&b, c->ev[EV_COMM0], c->ev[EV_COMM1]);
+        *out = oc_str_sync_t{};
+        out->version = S.version;
+        out->rows_global = rows_global;
+        out->bytes_reduced = n_df * 4 + uint64_t(nf) * 16;
+        out->device_ms = a + b;
+        out->wall_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - wall0).count();
+    }
+    return OC_OK;
+}
+
+extern "C" int oc_str_read_global_df(oc_str *s, uint32_t field, uint32_t *n_terms, uint32_t *df) {
+    if (!s || !n_terms) return fail(OC_ERR_INVALID, "NULL argument");
+    oc_ctx *c = s->ctx;
+    std::lock_guard<std::mutex> g(c->mu);   // oc_str_sync_global / oc_str_load_field replace a table under this lock
+    std::shared_ptr<StrSnap> snap = str_snapshot(s);
+    if (field >= snap->fields.size()) return fail(OC_ERR_INVALID, "field %u out of range", field);
+    const std::vector<uint32_t> &t = snap->fields[field].global_df;
+    const uint32_t cap = *n_terms;
+    *n_terms = (uint32_t)t.size();
+    if (!df) return OC_OK;
+    if (cap < t.size()) return fail(OC_ERR_INVALID, "df holds %u entries, the table has %zu", cap, t.size());
+    std::copy(t.begin(), t.end(), df);
+    return OC_OK;
+}
+
 // ------------------------------------------------------------------------------------ device-resident filters
 struct oc_facets;
 struct oc_filter {
@@ -3230,10 +3381,14 @@ static int ft_descriptors(SearchCall &k) {
                 const uint32_t fi = p->term_field[e], ti = p->term_id[e];
                 if (fi >= S->fields.size()) return fail(OC_ERR_INVALID, "term field %u out of range", fi);
                 const StrField &f = S->fields[fi];
-                if (ti >= f.n_terms) continue;  // unknown term: no postings
+                // unknown term: no postings.  A term of the synced df table (oc_str_sync_global) that this shard has
+                // never seen is an empty list, so that every rank takes the same df decisions.
+                const bool local = ti < f.n_terms;
+                if (!local && ti >= f.global_df.size()) continue;
                 TermDesc td{};
-                td.ptr = f.post + f.term_offsets[ti];
-                td.len = (uint32_t)(f.term_offsets[ti + 1] - f.term_offsets[ti]);
+                const uint64_t off = local ? f.term_offsets[ti] : f.n_post;
+                td.ptr = f.post + off;
+                td.len = local ? (uint32_t)(f.term_offsets[ti + 1] - off) : 0u;
                 td.weight = p->term_weight ? p->term_weight[e] : 1.0f;
                 td.avg_len = f.avg_len;
                 df_known = f.global_df.empty() ? td.len : f.global_df[ti];

@@ -23,6 +23,7 @@
 //        pending posting: new_off[t] + its rank among t's pending postings + t's survivors with a lower new row
 //      so the result does not depend on scheduling.  Both keep, per new row, the (term, len) of its posting with the
 //      largest term id (atomicMax); sc_len_sum_kernel sums the non-zero lengths exactly in uint64 for avg_field_len.
+// oc_str_sync_global takes the same sums of a published snapshot from its postings (sc_row_len_kernel).
 //
 // Roofline: HBM.  Algorithmic bytes per old posting: 8 (read for the survivor bit) + 8 (read again by the scatter)
 // + 8 (written) + 4 (the remap entry of its row, mostly from L2) + 2 * 1/8 (survivor bit, written and read); per
@@ -230,6 +231,16 @@ sc_scatter_pending_kernel(uint32_t n_pend, const uint64_t *keys, const uint32_t 
     }
     out[new_off[t] + (k - pend_lo[t]) + below] = {nr, p_tf[v], p_len[v]};
     sc_note_len(row_key, nr, t, p_len[v]);
+}
+
+// row_key[row] = the field length its postings carry (the largest, should they differ): the input sc_len_sum_kernel
+// takes when a snapshot's length sums come from its postings (oc_str_sync_global) rather than from its commit
+__global__ void __launch_bounds__(SC_THREADS)
+sc_row_len_kernel(uint64_t n_post, const PostingRaw *raw, unsigned long long *row_key) {
+    for (uint64_t i = uint64_t(blockIdx.x) * SC_THREADS + threadIdx.x; i < n_post; i += uint64_t(gridDim.x) * SC_THREADS) {
+        const PostingRaw p = raw[i];
+        if (p.len) atomicMax(row_key + p.row, (unsigned long long)p.len);
+    }
 }
 
 // sum[0] += the non-zero lengths in row_key, sum[1] += their count

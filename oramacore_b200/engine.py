@@ -292,6 +292,24 @@ class StringFieldStorage:
         a = None if avg_field_len is None else np.ascontiguousarray(avg_field_len, np.float32)
         check(lib().oc_str_set_global(self._h, int(document_count), _p(a)))
 
+    def sync_global(self) -> dict:
+        """This store is one shard of a group (Context.comm_init / comm_init_local): rebuild the corpus-wide df tables
+        and average field lengths from every rank's published snapshot (oc_str_sync_global).  A collective: every rank
+        calls it, after its own commit() returned.  Returns the call's statistics (oc_str_sync_t)."""
+        st = _lib.StrSync()
+        check(lib().oc_str_sync_global(self._h, C.byref(st)))
+        return st.as_dict()
+
+    def read_global_df(self, field: int) -> Optional[np.ndarray]:
+        """The corpus-wide df table installed for one field (uint32, the array global_df takes), or None."""
+        n = C.c_uint32(0)
+        check(lib().oc_str_read_global_df(self._h, field, C.byref(n), None))
+        if n.value == 0:
+            return None
+        df = np.zeros(n.value, np.uint32)
+        check(lib().oc_str_read_global_df(self._h, field, C.byref(n), _p(df)))
+        return df[:n.value]
+
 
 class DeviceFilter:
     """A FilterResult<DocumentId> evaluated to a bitmap that lives on the device (oc_filter_*): built once from

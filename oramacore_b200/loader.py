@@ -25,10 +25,16 @@ oc_geo_field_commit_ex), `where_filter(where)` evaluates a where-clause over the
 sorts by a number, date or bool field of the published version (oc_sort_field_from_facets).  No host copy of the
 filter values is kept.  OMC multipliers go to a device-resident OmcStore: `omc()` publishes the ones applied so far
 (get_all_omc, mod.rs:1720-1739: visible before a commit), and `commit()` also removes the uncommitted deletes' entries
-(mod.rs:604-627).  tf of a term = number of positions (exact + stemmed), as StringStorage counts them."""
+(mod.rs:604-627).  tf of a term = number of positions (exact + stemmed), as StringStorage counts them.
+
+`IndexLoader(..., shard=(lo, hi))` is one rank of a document-sharded index (sharding.py): every rank applies the whole
+stream but stores only the documents in its doc-id range [lo, hi) (hi None: open-ended; ranges ascend with rank).  The
+dictionary, N, the OMC map, the DocumentId space and the deletes follow every op, so every rank resolves queries to the
+same term ids; `commit()` ends with the collective that rebuilds the corpus-wide df tables and averages
+(StringFieldStorage.sync_global), so it must run on every rank concurrently (one thread or process per rank)."""
 from __future__ import annotations
 
-from typing import Dict, Iterable, List, Optional, Sequence
+from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -52,10 +58,17 @@ def _exact_i64(x, what: str) -> float:
 
 
 class IndexLoader:
+    shard: Optional[Tuple[int, Optional[int]]] = None    # this rank's doc-id range [lo, hi); None: the whole index
+    _deletes_since_commit = False                         # sharded: some rank's store may hold tombstones
+
     def __init__(self, ctx: Context, string_fields: Sequence[str], embedding_model: Optional[str] = None,
                  embedding_dim: Optional[int] = None, bool_fields: Sequence[str] = (), number_fields: Sequence[str] = (),
-                 string_filter_fields: Sequence[str] = (), geopoint_fields: Sequence[str] = (), date_fields: Sequence[str] = ()):
+                 string_filter_fields: Sequence[str] = (), geopoint_fields: Sequence[str] = (), date_fields: Sequence[str] = (),
+                 shard: Optional[Tuple[int, Optional[int]]] = None):
+        if shard is not None and (shard[0] < 0 or (shard[1] is not None and shard[1] < shard[0])):
+            raise ValueError(f"shard {shard!r}: want (lo, hi) with 0 <= lo <= hi, or (lo, None)")
         self.ctx = ctx
+        self.shard = shard
         self.string_fields = list(string_fields)
         self.dict = TermDictionary(max(len(self.string_fields), 1))
         self.strs = StringFieldStorage.empty(ctx, max(len(self.string_fields), 1))
@@ -101,15 +114,20 @@ class IndexLoader:
             if d in self._uncommitted_deleted:
                 self._uncommitted_deleted.discard(d)
                 self._retire_live()
+            own = self.owns(d)
             for v in op["indexed_values"]:
                 t = v["type"]
                 if t == "ScoreString2":
                     fi = self.string_fields.index(v["field"])
                     terms = v["terms"]                                  # {term: {"exact_positions": [...], "positions": [...]}}
                     names = list(terms)
+                    # registered on every rank, stored or not: the ranks' dictionaries hand out the same ids
                     ids = self.dict.add_terms(fi, names) if names else np.zeros(0, np.uint32)
-                    tf = {int(i): max(1, len(terms[n].get("exact_positions", ())) + len(terms[n].get("positions", ()))) for i, n in zip(ids, names)}
-                    self.strs.insert(d, fi, int(v["field_length"]), tf)
+                    if own:
+                        tf = {int(i): max(1, len(terms[n].get("exact_positions", ())) + len(terms[n].get("positions", ()))) for i, n in zip(ids, names)}
+                        self.strs.insert(d, fi, int(v["field_length"]), tf)
+                elif not own:
+                    continue
                 elif t == "FilterBool":                         # replaces the document's value
                     f = self._field(self._bool, v["field"])
                     self.facets.clear(f, [d])
@@ -145,7 +163,8 @@ class IndexLoader:
         elif kind == "IndexEmbedding":
             for d, vectors in op["data"]:
                 self.max_doc_id = max(self.max_doc_id, int(d))
-                self.emb.insert(int(d), vectors)
+                if self.owns(int(d)):
+                    self.emb.insert(int(d), vectors)
         elif kind == "DeleteDocuments":
             ids = [int(x) for x in op["doc_ids"]]
             self.strs.delete(ids)
@@ -156,6 +175,7 @@ class IndexLoader:
             self.document_count = max(self.document_count - len(ids), 0)
             self._push_count()
             self._uncommitted_deleted.update(ids)
+            self._deletes_since_commit = True
             if self.facets is not None:
                 self.facets.delete(ids)
             for g in self.geo.values():
@@ -163,6 +183,19 @@ class IndexLoader:
             self._retire_live()
         else:
             raise ValueError(f"unsupported operation {kind!r}")
+
+    def owns(self, doc_id: int) -> bool:
+        """Whether this loader stores the document (always, unless it is one shard)."""
+        if self.shard is None:
+            return True
+        lo, hi = self.shard
+        return doc_id >= lo and (hi is None or doc_id < hi)
+
+    @property
+    def shard_tombstones(self) -> bool:
+        """The OC_SHARD_TOMBSTONES flag (TokenScoreParams.shard_tombstones) of a sharded search on this loader: a
+        delete since the last commit, which may have tombstoned rows on any rank.  The same on every rank."""
+        return self._deletes_since_commit
 
     def _push_count(self) -> None:
         """N of the idf is Index::document_count (mod.rs:1460: +1 per Index op, also for documents without string
@@ -192,7 +225,8 @@ class IndexLoader:
     def commit(self) -> None:
         """ReadSide::commit -> field compact(): publish the next snapshot of the string store (searches on the
         previous one keep running meanwhile), drop the deleted rows of the embedding store (index/mod.rs:583-590) and
-        refresh the facet layout and the geopoint fields."""
+        refresh the facet layout and the geopoint fields.  A shard then rebuilds the corpus-wide df tables and
+        averages with the other ranks (a collective: every rank's commit() runs concurrently)."""
         self.strs.commit()
         if self.emb is not None:
             self.emb.compact()
@@ -200,7 +234,10 @@ class IndexLoader:
         # mod.rs:604-627: the log merges into the committed map, then the uncommitted deletes leave it
         self._publish_omc(sorted(self._uncommitted_deleted))
         self._uncommitted_deleted.clear()
+        self._deletes_since_commit = False
         self.refresh_facets()
+        if self.shard is not None:
+            self.strs.sync_global()
 
     def omc(self) -> OmcStore:
         """The OMC store with every multiplier applied so far published (get_all_omc, mod.rs:1720-1739: the log over

@@ -2,9 +2,11 @@
 
 Shard g owns the contiguous doc-row range [g*N/G, (g+1)*N/G) of the embedding matrix AND
 the postings restricted to those rows (so BM25 accumulators are shard-local).  The global
-quantities BM25 needs — N (document_count), avg_field_len and per-term df — are static for a
-loaded corpus: they are computed here, at load time, and replicated; there is no per-query
-collective for them.
+quantities BM25 needs — N (document_count), avg_field_len and per-term df — are replicated, so
+there is no per-query collective for them.  For a loaded corpus they are computed here, at load
+time.  A commit on a shard drops its df table: StringFieldStorage.sync_global() on every rank then
+rebuilds the tables and the averages on the devices from all shards (IndexLoader(shard=...) does so
+at the end of each commit); N stays the caller's.
 """
 from __future__ import annotations
 

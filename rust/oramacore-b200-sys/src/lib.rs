@@ -53,6 +53,16 @@ pub struct OcStrCommit {
     pub device_ms: f32,
     pub wall_ms: f32,
 }
+/// Statistics of one `oc_str_sync_global` call (`oc_str_sync_t`).
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct OcStrSync {
+    pub version: u64,
+    pub rows_global: u64,
+    pub bytes_reduced: u64,
+    pub device_ms: f32,
+    pub wall_ms: f32,
+}
 /// Statistics of one `oc_facets_commit_ex` / `oc_geo_field_commit_ex` call (`oc_filter_commit_t`).
 #[repr(C)]
 #[derive(Clone, Copy, Debug, Default)]
@@ -284,6 +294,12 @@ extern "C" {
                      out_doc_ids: *mut u64, out_scores: *mut f32, out_n: *mut u32, out_count: *mut u64) -> c_int;
     /// caller-owned N / average field lengths (shards; Index::document_count), kept across commits
     pub fn oc_str_set_global(s: *mut OcStr, document_count: u64, avg_field_len: *const f32) -> c_int;
+    /// collective over the ctx's comm group: rebuild a shard's corpus-wide df tables and average field lengths
+    /// after every rank's `oc_str_commit` returned (`out` may be null)
+    pub fn oc_str_sync_global(s: *mut OcStr, out: *mut OcStrSync) -> c_int;
+    /// one field's installed df table: null `df` returns its size in `*n_terms` (0: no table); otherwise `*n_terms`
+    /// is the capacity on entry
+    pub fn oc_str_read_global_df(s: *mut OcStr, field: u32, n_terms: *mut u32, df: *mut u32) -> c_int;
     // FilterResult (filter.rs:344-392) evaluated on the device
     pub fn oc_filter_from_ids(ctx: *mut OcCtx, doc_ids: *const u64, n: u64, nbits: u64, out: *mut *mut OcFilter) -> c_int;
     pub fn oc_filter_from_bits(ctx: *mut OcCtx, bits: *const u64, nbits: u64, out: *mut *mut OcFilter) -> c_int;
