@@ -891,6 +891,48 @@ int oc_merge_sorted(uint32_t n_indexes, uint32_t n_queries, uint32_t limit, uint
                     uint64_t *out_doc_ids /* B x limit */, float *out_scores, double *out_sort_values,
                     uint32_t *out_n, uint64_t *out_count);
 
+/* ---- one call over every index of a collection ------------------------------------------------------
+ * search_on_indexes (read/search.rs:283-501) in one call: every index of a collection on this ctx runs into its own top
+ * list on the device, and one kernel merges them (the union, the pins and the field order), so only the merged page
+ * comes back.  Index i is described by ix[i]:
+ *   - request fields, equal on every index (OC_ERR_INVALID otherwise): n_queries, mode, limit, offset, vector_limit (must
+ *     be 0), similarity, threshold, bm25_k, bm25_b and the contents of q_params (each entry's vector_limit must be 0);
+ *   - index fields, that index's own: the token arrays (term ids of its own dictionary), q_vecs, filter / filter_bits /
+ *     q_filters / q_where (over its own filter fields), and omc_doc_ids / omc_mult / n_omc or omc;
+ *   - q_sorts: NULL (score order for every query) or B entries, that index's sort handle.  Query b is in field order
+ *     when every index's q_sorts[b].field is set and all share one order, in score order when every entry is NULL (or
+ *     q_sorts NULL); any other mix is OC_ERR_INVALID.
+ * pins (may be NULL) are the collection's: the items of query b and `apply`, as in oc_pins.
+ * Result, byte for byte: the documented per-index recipe — index i alone through oc_search_q_sorted with limit' =
+ * limit + offset (2 x (limit + offset) for an active pinned query), offset' = 0, vector_limit = limit and pins with
+ * apply = 0, merged by oc_merge_results (score order, no pins), oc_merge_pinned (score order) or oc_merge_sorted
+ * (field order).  With q_params, query b gets that recipe at its own (limit_b, offset_b), as it would alone.
+ *   - out_doc_ids / out_scores / out_sort_values: B x limit; out_n, out_count (the sum of the indexes' counts): B.
+ *   - out_sort_values (may be NULL): the value a hit was placed by; NaN for a promoted item and in score order; 0.0
+ *     past out_n.
+ *   - out_pin_scores / out_pin_present (may be NULL): per item, the score from the first index whose map holds the
+ *     document, else 0.0, and whether one does.
+ * Memory: the indexes' top lists stay in ctx workspaces (about 24 B per (index, query, list slot)); an oc_sort_field
+ * used here gets a device copy of each order's rank values (8 B per ranked document), built the first time and freed
+ * with the handle.  last_timing covers every index and the merge; its d2h_bytes includes the result blobs each index's
+ * re-run checks read back.
+ * Refusals (nothing written): OC_ERR_UNSUPPORTED: p->sharded, a per-index depth (limit' above) over OC_MAX_TOPK;
+ * OC_ERR_INVALID: n_indexes 0 or above OC_MAX_INDEXES, request fields that differ, a store, filter, sort field or OMC
+ * store of another ctx, and everything the per-index call or the host merge would refuse.
+ * Not covered: groupBy and facets across indexes (groups are keyed by value across indexes; facet counts add up by
+ * label on the host), batching in oc_batcher, sharded collections.  Indexes run one after another on the ctx stream.
+ * Callers whose indexes live on different contexts keep using the host merges above. */
+#define OC_MAX_INDEXES 32u
+typedef struct {
+    oc_emb *emb;                     /* NULL: the index has no embedding field              */
+    oc_str *str;                     /* NULL: no string fields                              */
+    const oc_search_params *p;       /* this index's inputs                                 */
+    const oc_sort *q_sorts;          /* NULL: score order for every query; or B entries     */
+} oc_index_query;
+int oc_search_indexes(oc_ctx *ctx, uint32_t n_indexes, const oc_index_query *ix, const oc_pins *pins,
+                      uint64_t *out_doc_ids, float *out_scores, double *out_sort_values, uint32_t *out_n,
+                      uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present);
+
 /* ---- term dictionary and query-term resolution (host; oc_dict_resolve_q may expand typos on a device) ------
  * The step the reference performs before the posting walk: TextParser::tokenize_and_stem(term) —
  * originals, plus stems unless `exact`, [""] when nothing is left (token_score.rs:196-209) — and the

@@ -40,6 +40,7 @@
 #include "group.cuh"
 #include "pins.cuh"
 #include "sort.cuh"
+#include "index_merge.cuh"
 #include "sort_build.cuh"
 #include "omc.cuh"
 #include "tmap.cuh"
@@ -195,6 +196,7 @@ struct oc_ctx {
     DevBuf row_ft, grp_vdoc, grp_vscore, grp_vn, grp_gmin, grp_den, grp_doc, grp_score, grp_n;   // oc_search_groups
     DevBuf pin_row, pin_ft, pin_ftp, pin_score, pin_present, pin_top_doc, pin_top_score, pin_top_n, pin_gdoc, pin_gscore, pin_gn;   // pins
     DevBuf srt_doc, srt_row, srt_n, srt_ft, srt_ftp, srt_score, srt_present, srt_zero;   // sortBy
+    DevBuf mi_doc, mi_score, mi_val, mi_n, mi_cnt, mi_pscore, mi_ppresent, mi_out;   // oc_search_indexes: per-index lists, page
     DevBuf sfb_ws;                    // sort field build (sort_build.cuh), released before the call returns
     DevBuf q_bf16, q_f16, q_scale, q_rho, pre_post, dense_buf, g_thr, g_eps, g_ovf, g_ovfcnt, g_resc, g_cand, g_cnt, g_flag, g_max, r_qpad, r_qinv, r_map, r_doc, r_score, r_row, r_cnt, r_raw;
     // per-query where-filters (q_filters): the embedding rows' bitmap of every distinct handle, and the slots of the
@@ -2429,6 +2431,7 @@ struct SortOrder {
     std::weak_ptr<StrSnap> rows_of;        // the snapshot rank_row maps to
     std::vector<uint32_t> h_doc_rank;      // [nbits]
     std::vector<double> h_value;           // [n] value of each rank
+    double *rank_value = nullptr;          // device [n]: h_value, built by the first oc_search_indexes that needs it
 };
 struct oc_sort_field {
     oc_ctx *ctx;
@@ -2437,7 +2440,7 @@ struct oc_sort_field {
     SortOrder ord[2];                      // OC_SORT_ASC, OC_SORT_DESC
 };
 static void sort_field_free(oc_sort_field *f) {
-    for (SortOrder &o : f->ord) { cudaFree(o.rank_doc); cudaFree(o.doc_rank); cudaFree(o.rank_row); }
+    for (SortOrder &o : f->ord) { cudaFree(o.rank_doc); cudaFree(o.doc_rank); cudaFree(o.rank_row); cudaFree(o.rank_value); }
     delete f;
 }
 // The sorts of one batch: its distinct (field, order) pairs and, per query, the index of its pair or SORT_BY_SCORE
@@ -4072,16 +4075,9 @@ static int copy_out(SearchCall &k) {
 
 static int where_stage(SearchCall &k);
 
-static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const SearchReq &r) {
-    SearchCall k(c, emb, str, r);
-    OCTRY(search_check(k));
-    if (k.B == 0) return OC_OK;
-    // the published snapshot of the string store: grabbed once, immutable for the whole call (a commit may
-    // publish the next version meanwhile); taken before the lock so a last reference dies outside it
-    k.snap = str ? str_snapshot(str) : nullptr;
-    k.S = k.snap.get();
-    std::lock_guard<std::mutex> g(c->mu);
-    CU(cudaSetDevice(c->device));
+// The stages of one search under the ctx lock, up to its results in the ctx's output blob (k.dout) and workspaces.
+static int search_stages(SearchCall &k) {
+    oc_ctx *c = k.c; const SearchReq &r = k.r;
     // facets: the requests resolved to their distinct document slices (the work list goes up with the first upload)
     if (k.facets) OCTRY(facet_plan(*r.fj, k.fpl));
     begin_call(c);
@@ -4095,7 +4091,20 @@ static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const SearchReq &r) 
     OCTRY(main_upload(k));
     if (k.has_ft) OCTRY(bm25_stage(k));
     OCTRY(device_tail(k));
-    OCTRY(rerun_checks(k));
+    return rerun_checks(k);
+}
+
+static int search_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const SearchReq &r) {
+    SearchCall k(c, emb, str, r);
+    OCTRY(search_check(k));
+    if (k.B == 0) return OC_OK;
+    // the published snapshot of the string store: grabbed once, immutable for the whole call (a commit may
+    // publish the next version meanwhile); taken before the lock so a last reference dies outside it
+    k.snap = str ? str_snapshot(str) : nullptr;
+    k.S = k.snap.get();
+    std::lock_guard<std::mutex> g(c->mu);
+    CU(cudaSetDevice(c->device));
+    OCTRY(search_stages(k));
     return copy_out(k);
 }
 
@@ -5321,6 +5330,230 @@ extern "C" int oc_search_q_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_
     for (uint32_t b = 0; b < p->n_queries; b++) OCTRY(sort_job_add(c, q_sorts[b], sj));
     return sorted_impl(c, emb, str, p, sj, pins, true, out_doc_ids, out_scores, out_sort_values, out_n, out_count, out_pin_scores,
                        out_pin_present);
+}
+
+// ------------------------------------------------------------------------------------ one call over the indexes (index_merge.cuh)
+static bool same_f32(float a, float b) { return memcmp(&a, &b, 4) == 0; }
+// the request fields of oc_search_indexes, which every index must share
+static bool same_request(const oc_search_params *a, const oc_search_params *b) {
+    if (a->n_queries != b->n_queries || a->mode != b->mode || a->limit != b->limit || a->offset != b->offset ||
+        a->vector_limit != b->vector_limit || !same_f32(a->similarity, b->similarity) || !same_f32(a->threshold, b->threshold) ||
+        !same_f32(a->bm25_k, b->bm25_k) || !same_f32(a->bm25_b, b->bm25_b) || !a->q_params != !b->q_params)
+        return false;
+    for (uint32_t q = 0; a->q_params && q < a->n_queries; q++) {
+        const oc_query_params &x = a->q_params[q], &y = b->q_params[q];
+        if (x.mode != y.mode || x.limit != y.limit || x.offset != y.offset || !same_f32(x.similarity, y.similarity) ||
+            !same_f32(x.threshold, y.threshold) || x.vector_limit != y.vector_limit)
+            return false;
+    }
+    return true;
+}
+// one index's timing added to the call's
+static void timing_add(oc_timing &t, const oc_timing &a) {
+    t.h2d_ms += a.h2d_ms; t.device_ms += a.device_ms; t.d2h_ms += a.d2h_ms; t.scan_ms += a.scan_ms; t.bm25_ms += a.bm25_ms;
+    t.fuse_ms += a.fuse_ms; t.comm_ms += a.comm_ms; t.kernel_launches += a.kernel_launches; t.scan_launches += a.scan_launches;
+    t.scan_bytes += a.scan_bytes; t.bm25_postings += a.bm25_postings; t.h2d_bytes += a.h2d_bytes; t.d2h_bytes += a.d2h_bytes;
+    t.scan_tensor_core = std::max(t.scan_tensor_core, a.scan_tensor_core); t.scan_unproven += a.scan_unproven;
+    if (a.scan_launches) t.scan_variant = a.scan_variant;
+    t.scan_sweep_ms += a.scan_sweep_ms; t.rerun_ms += a.rerun_ms; t.scan_rescored = std::max(t.scan_rescored, a.scan_rescored);
+    t.bm25_dense_items += a.bm25_dense_items; t.bm25_dense_skipped += a.bm25_dense_skipped;
+}
+
+// search_on_indexes: every index through its own stages into a per-index slot of the ctx's workspaces (under one ctx
+// lock), then index_merge_kernel and one copy of the merged page.  Nothing is written on failure.
+extern "C" int oc_search_indexes(oc_ctx *c, uint32_t n_indexes, const oc_index_query *ix, const oc_pins *pins,
+                                 uint64_t *out_doc_ids, float *out_scores, double *out_sort_values, uint32_t *out_n,
+                                 uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present) {
+    if (!c || !ix || !out_doc_ids || !out_scores || !out_n || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
+    if (n_indexes == 0 || n_indexes > OC_MAX_INDEXES) return fail(OC_ERR_INVALID, "n_indexes %u: expected 1 .. %u", n_indexes, OC_MAX_INDEXES);
+    for (uint32_t i = 0; i < n_indexes; i++) {
+        if (!ix[i].p) return fail(OC_ERR_INVALID, "index %u: NULL params", i);
+        if (ix[i].p->sharded) return fail(OC_ERR_UNSUPPORTED, "index %u: sharded search", i);
+        if (!same_request(ix[i].p, ix[0].p)) return fail(OC_ERR_INVALID, "index %u: its request fields differ from index 0's", i);
+    }
+    const oc_search_params *p0 = ix[0].p;
+    const uint32_t B = p0->n_queries, limit = p0->limit;
+    if (p0->vector_limit) return fail(OC_ERR_INVALID, "vector_limit must be 0: every index runs at vector_limit = limit");
+    if (limit == 0) return fail(OC_ERR_INVALID, "limit must be >= 1");
+    // per query: score order, or one order over every index's sort handle
+    std::vector<uint8_t> q_sort(B, IM_BY_SCORE);
+    bool any_sorted = false;
+    for (uint32_t b = 0; b < B; b++) {
+        uint32_t n_field = 0;
+        int order = -1;
+        bool same = true;
+        for (uint32_t i = 0; i < n_indexes; i++) {
+            if (!ix[i].q_sorts || !ix[i].q_sorts[b].field) continue;
+            same = same && (order < 0 || ix[i].q_sorts[b].order == order);
+            order = ix[i].q_sorts[b].order;
+            n_field++;
+        }
+        if (n_field == 0) continue;
+        if (n_field != n_indexes || !same) return fail(OC_ERR_INVALID, "query %u: a sort on some indexes only, or orders that differ", b);
+        if (order != OC_SORT_ASC && order != OC_SORT_DESC) return fail(OC_ERR_INVALID, "query %u: sort order %d is neither ASC nor DESC", b, order);
+        q_sort[b] = order == OC_SORT_ASC ? IM_ASC : IM_DESC;
+        any_sorted = true;
+    }
+    // pins: every index looks the items up (apply = 0); the merge splices the active queries
+    PinJob pj_all;
+    OCTRY(pin_job_init(pins, B, pj_all));
+    oc_pins pins0{};
+    if (pins) { pins0 = *pins; pins0.apply = 0; }
+    std::vector<uint8_t> q_active(B, 0);
+    bool any_active = false;
+    for (uint32_t b = 0; b < B; b++) { q_active[b] = pj_all.splice && pj_all.cnt[b] > 0; any_active = any_active || q_active[b]; }
+    // each query's page and each index's depth: limit + offset, twice that for an active query
+    std::vector<uint2> q_page(B, make_uint2(p0->offset, limit));
+    std::vector<oc_query_params> qp;
+    uint64_t depth = 0;
+    if (p0->q_params) {
+        qp.assign(p0->q_params, p0->q_params + B);
+        for (uint32_t b = 0; b < B; b++) {
+            const oc_query_params &e = p0->q_params[b];
+            if (e.vector_limit) return fail(OC_ERR_INVALID, "q_params[%u]: vector_limit must be 0", b);
+            if (e.limit == 0) return fail(OC_ERR_INVALID, "q_params[%u]: limit must be >= 1", b);
+            if (e.limit > limit) return fail(OC_ERR_INVALID, "q_params[%u]: limit %u > p->limit %u (the row stride)", b, e.limit, limit);
+            const uint64_t d = (uint64_t(e.limit) + e.offset) * (q_active[b] ? 2 : 1);
+            if (d > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "q_params[%u]: per-index depth %llu > %u", b, (unsigned long long)d, OC_MAX_TOPK);
+            qp[b].limit = (uint32_t)d; qp[b].offset = 0; qp[b].vector_limit = e.limit;
+            q_page[b] = make_uint2(e.offset, e.limit);
+            depth = std::max(depth, d);
+        }
+    } else {
+        depth = (uint64_t(limit) + p0->offset) * (any_active ? 2 : 1);
+        if (depth > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "per-index depth %llu > %u", (unsigned long long)depth, OC_MAX_TOPK);
+    }
+    const uint32_t stride = (uint32_t)std::max<uint64_t>(depth, 1);
+    // every index's call, checked before anything runs
+    std::vector<oc_search_params> ps(n_indexes);
+    std::vector<SortJob> sjs(n_indexes);
+    std::vector<PinJob> pjs(n_indexes);
+    std::vector<std::unique_ptr<SearchReq>> reqs;
+    std::vector<std::unique_ptr<SearchCall>> calls;
+    const bool with_pj = pins || any_sorted;
+    for (uint32_t i = 0; i < n_indexes; i++) {
+        ps[i] = *ix[i].p;
+        ps[i].limit = stride; ps[i].offset = 0; ps[i].vector_limit = limit;
+        ps[i].q_params = qp.empty() ? nullptr : qp.data();
+        for (uint32_t b = 0; any_sorted && b < B; b++)
+            OCTRY(sort_job_add(c, ix[i].q_sorts ? ix[i].q_sorts[b] : oc_sort{nullptr, OC_SORT_ASC}, sjs[i]));
+        if (with_pj) OCTRY(pin_job_init(pins ? &pins0 : nullptr, B, pjs[i]));
+        reqs.emplace_back(new SearchReq(&ps[i], out_doc_ids, out_scores, out_n, out_count));   // (its tail, copy_out, never runs)
+        SearchReq &r = *reqs.back();
+        r.pj = with_pj ? &pjs[i] : nullptr;
+        r.sj = any_sorted ? &sjs[i] : nullptr;
+        r.q_filters_ok = r.q_params_ok = true;
+        calls.emplace_back(new SearchCall(c, ix[i].emb, ix[i].str, r));
+        OCTRY(search_check(*calls.back()));
+    }
+    if (B == 0) return OC_OK;
+    for (uint32_t i = 0; i < n_indexes; i++) {   // each index's string snapshot, before the lock
+        calls[i]->snap = ix[i].str ? str_snapshot(ix[i].str) : nullptr;
+        calls[i]->S = calls[i]->snap.get();
+    }
+    std::lock_guard<std::mutex> g(c->mu);
+    CU(cudaSetDevice(c->device));
+    const uint32_t pstr = pj_all.stride;
+    const size_t per = size_t(B) * stride, nps = size_t(B) * pstr;
+    OCTRY(c->mi_doc.ensure(n_indexes * per * 8));
+    OCTRY(c->mi_score.ensure(n_indexes * per * 4));
+    OCTRY(c->mi_n.ensure(size_t(n_indexes) * B * 4));
+    OCTRY(c->mi_cnt.ensure(size_t(n_indexes) * B * 8));
+    if (any_sorted) OCTRY(c->mi_val.ensure(n_indexes * per * 8));
+    if (pstr) { OCTRY(c->mi_pscore.ensure(n_indexes * nps * 4)); OCTRY(c->mi_ppresent.ensure(n_indexes * nps)); }
+    // where each index's hits find their sort values: the handles' rank values on the device (built once per handle)
+    std::vector<ImSortSrc> src(any_sorted ? size_t(n_indexes) * B : 0, ImSortSrc{nullptr, nullptr, 0});
+    for (uint32_t i = 0; any_sorted && i < n_indexes; i++) {
+        for (uint32_t e = 0; e < sjs[i].f.size(); e++) {
+            SortOrder &o = sjs[i].ord(e);
+            if (o.rank_value || !o.n) continue;
+            CU(cudaMalloc(&o.rank_value, o.n * 8));
+            CU(cudaMemcpyAsync(o.rank_value, o.h_value.data(), o.n * 8, cudaMemcpyHostToDevice, c->stream));
+        }
+        for (uint32_t b = 0; b < B; b++) {
+            const uint32_t e = sjs[i].q_ent[b];
+            if (e != SORT_BY_SCORE) src[size_t(i) * B + b] = ImSortSrc{sjs[i].ord(e).doc_rank, sjs[i].ord(e).rank_value, sjs[i].f[e]->nbits};
+        }
+    }
+    oc_timing total{};
+    for (uint32_t i = 0; i < n_indexes; i++) {
+        SearchCall &k = *calls[i];
+        OCTRY(search_stages(k));
+        OCTRY(finish_timing(c, k.has_v && k.vlimit && k.emb->n_rows > 0, k.has_ft, true, k.did_comm));
+        c->timing.d2h_bytes = k.out_bytes;
+        timing_add(total, c->timing);
+        // the index's top list and item lookups into its slot (the next index's stages reuse the ctx's buffers)
+        CU(cudaMemcpyAsync(c->mi_doc.as<uint64_t>() + i * per, k.d_doc, per * 8, cudaMemcpyDeviceToDevice, c->stream));
+        CU(cudaMemcpyAsync(c->mi_score.as<float>() + i * per, k.d_score, per * 4, cudaMemcpyDeviceToDevice, c->stream));
+        CU(cudaMemcpyAsync(c->mi_n.as<uint32_t>() + size_t(i) * B, k.d_n, size_t(B) * 4, cudaMemcpyDeviceToDevice, c->stream));
+        CU(cudaMemcpyAsync(c->mi_cnt.as<uint64_t>() + size_t(i) * B, k.dout + k.o_cnt, size_t(B) * 8, cudaMemcpyDeviceToDevice, c->stream));
+        if (pstr) {
+            CU(cudaMemcpyAsync(c->mi_pscore.as<float>() + i * nps, c->pin_score.p, nps * 4, cudaMemcpyDeviceToDevice, c->stream));
+            CU(cudaMemcpyAsync(c->mi_ppresent.as<uint8_t>() + i * nps, c->pin_present.p, nps, cudaMemcpyDeviceToDevice, c->stream));
+        }
+    }
+    // the merge: its tables in one upload, one CTA per query, the page in one copy
+    Packer pk;
+    const Slot<uint8_t> s_sort = pk.add(q_sort.data(), B), s_act = pk.add(q_active.data(), B);
+    const Slot<uint2> s_page = pk.add(q_page.data(), B);
+    Slot<ImSortSrc> s_src;
+    Slot<uint64_t> s_pdoc;
+    Slot<uint32_t> s_ppos, s_pcnt;
+    if (any_sorted) s_src = pk.add(src.data(), src.size());
+    if (pstr) { s_pdoc = pk.add(pj_all.doc.data(), nps); s_ppos = pk.add(pj_all.pos.data(), nps); s_pcnt = pk.add(pj_all.cnt.data(), B); }
+    auto al = [](size_t x) { return (x + 255) & ~size_t(255); };
+    const size_t o_sc = al(size_t(B) * limit * 8), o_val = o_sc + al(size_t(B) * limit * 4), o_n = o_val + al(size_t(B) * limit * 8),
+                 o_cnt = o_n + al(size_t(B) * 4), o_ps = o_cnt + al(size_t(B) * 8), o_pp = o_ps + al(nps * 4), out_bytes = o_pp + nps;
+    OCTRY(c->mi_out.ensure(out_bytes));
+    OCTRY(c->h_out.ensure(out_bytes));
+    uint8_t *dout = c->mi_out.as<uint8_t>();
+    CU(cudaEventRecord(c->ev[EV_START], c->stream));
+    OCTRY(upload(pk, c->h_in, c->in_blob, c->stream));
+    CU(cudaEventRecord(c->ev[EV_H2D], c->stream));
+    IndexMergeParams mp{};
+    mp.n_idx = n_indexes; mp.B = B; mp.stride = stride;
+    mp.doc = c->mi_doc.as<uint64_t>(); mp.score = c->mi_score.as<float>(); mp.n = c->mi_n.as<uint32_t>();
+    mp.count = c->mi_cnt.as<unsigned long long>(); mp.value = c->mi_val.as<double>();
+    mp.src = s_src.at(c->in_blob); mp.q_sort = s_sort.at(c->in_blob); mp.q_page = s_page.at(c->in_blob); mp.q_active = s_act.at(c->in_blob);
+    mp.pin_stride = pstr; mp.kp2 = std::max<uint32_t>(32, next_pow2(pstr));
+    mp.pin_doc = s_pdoc.at(c->in_blob); mp.pin_pos = s_ppos.at(c->in_blob); mp.pin_cnt = s_pcnt.at(c->in_blob);
+    mp.pin_score = c->mi_pscore.as<float>(); mp.pin_present = c->mi_ppresent.as<uint8_t>();
+    mp.take_max = stride; mp.limit = limit;
+    mp.out_doc = reinterpret_cast<uint64_t *>(dout); mp.out_score = reinterpret_cast<float *>(dout + o_sc);
+    mp.out_value = reinterpret_cast<double *>(dout + o_val); mp.out_n = reinterpret_cast<uint32_t *>(dout + o_n);
+    mp.out_count = reinterpret_cast<unsigned long long *>(dout + o_cnt);
+    mp.out_pin_score = reinterpret_cast<float *>(dout + o_ps); mp.out_pin_present = dout + o_pp;
+    const size_t smem = index_merge_smem(stride, pstr, mp.kp2, limit);
+    CU(smem_cfg(c->device, (const void *)index_merge_kernel, smem));
+    index_merge_kernel<<<B, IM_THREADS, smem, c->stream>>>(mp);
+    launched(c);
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(c->ev[EV_DEV], c->stream));
+    uint8_t *h = c->h_out.as<uint8_t>();
+    CU(cudaMemcpyAsync(h, dout, out_bytes, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaEventRecord(c->ev[EV_D2H], c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    memcpy(out_doc_ids, h, size_t(B) * limit * 8);
+    memcpy(out_scores, h + o_sc, size_t(B) * limit * 4);
+    if (out_sort_values) memcpy(out_sort_values, h + o_val, size_t(B) * limit * 8);
+    memcpy(out_n, h + o_n, size_t(B) * 4);
+    memcpy(out_count, h + o_cnt, size_t(B) * 8);
+    for (uint32_t q = 0; pstr && q < B; q++)
+        for (uint32_t j = 0; j < pj_all.cnt[q]; j++) {
+            const size_t it = size_t(pins->q_pin_offsets[q]) + j, s = size_t(q) * pstr + j;
+            if (out_pin_scores) memcpy(out_pin_scores + it, h + o_ps + s * 4, 4);
+            if (out_pin_present) out_pin_present[it] = h[o_pp + s];
+        }
+    auto el = [&](int a, int b) { float ms = 0; cudaEventElapsedTime(&ms, c->ev[a], c->ev[b]); return ms; };
+    total.h2d_ms += el(EV_START, EV_H2D);
+    total.device_ms += el(EV_H2D, EV_DEV);
+    total.fuse_ms += el(EV_H2D, EV_DEV);
+    total.d2h_ms += el(EV_DEV, EV_D2H);
+    total.kernel_launches += 1;
+    total.h2d_bytes += pk.total;
+    total.d2h_bytes += out_bytes;
+    c->timing = total;
+    return OC_OK;
 }
 
 // One batch in which every query has its own groups (or none), sort, pins and, with q_filters, filter: query b gets what

@@ -84,7 +84,8 @@ __host__ __device__ inline size_t pin_splice_smem(uint32_t kp2, uint32_t n_top, 
 template <typename Member>
 __device__ uint32_t pin_splice_block(const uint64_t *top_doc, const float *top_score, uint32_t n_top, const uint64_t *doc,
                                      const uint32_t *pos, const float *score, uint32_t k, uint32_t kp2, Member member,
-                                     uint32_t s0, uint32_t n_take, uint64_t *out_doc, float *out_score, uint8_t *smem) {
+                                     uint32_t s0, uint32_t n_take, uint64_t *out_doc, float *out_score, uint8_t *smem,
+                                     uint32_t *out_src = nullptr) {
     uint64_t *ord = reinterpret_cast<uint64_t *>(smem);   // [kp2] ~(position << 32 | j), sorted descending
     uint64_t *ids = ord + kp2;                             // [kp2] ~doc, sorted descending
     uint32_t *ins = reinterpret_cast<uint32_t *>(ids + kp2);   // [kp2] insertion index
@@ -106,7 +107,10 @@ __device__ uint32_t pin_splice_block(const uint64_t *top_doc, const float *top_s
     }
     if (km == 0) {   // nothing to splice (block-uniform): the page of top as it is
         const uint32_t n = n_top > s0 ? min(n_top - s0, n_take) : 0u;
-        for (uint32_t i = tid; i < n; i += nt) { out_doc[i] = top_doc[s0 + i]; out_score[i] = top_score[s0 + i]; }
+        for (uint32_t i = tid; i < n; i += nt) {
+            out_doc[i] = top_doc[s0 + i]; out_score[i] = top_score[s0 + i];
+            if (out_src) out_src[i] = s0 + i;
+        }
         return n;
     }
     group_bitonic_desc(ord, kp2, tid, nt, 0);   // ascending (position, j); non-members last
@@ -148,15 +152,17 @@ __device__ uint32_t pin_splice_block(const uint64_t *top_doc, const float *top_s
         if (s < s_end && s >= s0) {
             uint64_t d;
             float sc;
+            uint32_t src = 0xffffffffu;
             if (is_pin) {
                 const uint32_t j = uint32_t(~ord[slot[s]]);
                 d = doc[j]; sc = score[j];
             } else {
-                const uint32_t t = kidx[s - pb];
-                d = top_doc[t]; sc = top_score[t];
+                src = kidx[s - pb];
+                d = top_doc[src]; sc = top_score[src];
             }
             out_doc[s - s0] = d;
             out_score[s - s0] = sc;
+            if (out_src) out_src[s - s0] = src;
         }
         pins_before += n_p;
     }

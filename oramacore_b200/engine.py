@@ -1283,6 +1283,60 @@ def merge_index_results_sorted(per_index, order: str, limit: int, offset: int = 
     return [SearchHits(od[i, :on[i]].copy(), os_[i, :on[i]].copy(), int(oc[i])) for i in range(B)], ov
 
 
+@dataclass
+class IndexPart:
+    """One index of a search_indexes call: its TokenScoreContext (its embedding and string stores), its own query
+    inputs (texts resolved with its own dictionary, q_vecs) and its index fields as TokenScoreParams fields of those
+    names: device_filter / device_filters / where_programs / filtered_doc_ids + filter_nbits over its own filter fields,
+    and omc_store or omc_doc_ids / omc_mult."""
+    tsc: "TokenScoreContext"
+    texts: object = None
+    q_vecs: Optional[np.ndarray] = None
+    fields: Optional[Mapping[str, object]] = None
+
+
+def search_indexes_arrays(ctx: Context, parts: Sequence[IndexPart], params: "TokenScoreParams", sorts=None, promote=None):
+    """oc_search_indexes: search_on_indexes (read/search.rs:283-501) over the indexes of one collection in one call.
+    `params` holds the request (mode, limit, offset, similarity, threshold, query_params; vector_limit must be 0) and is
+    shared by every index; each part adds its index's inputs.  `sorts`: None (score order), or per index None or per
+    query a (SortField, order) pair or None; query b is sorted when every index gives it a field in one order.
+    `promote` as in search_pinned_arrays.  Returns (docs [B,limit], scores, sort values [B,limit], n [B], count [B],
+    pin scores [items], pin present [items]), byte for byte the per-index searches merged by the host merges."""
+    import dataclasses
+    if not parts:
+        raise ValueError("search_indexes needs at least one index")
+    keep, built = [], []
+    for part in parts:
+        sp, k, B = part.tsc._build_params(dataclasses.replace(params, **dict(part.fields or {})), part.texts, part.q_vecs)
+        keep += [sp, k]
+        built.append((part.tsc, sp))
+    B = built[0][1].n_queries
+    ixs = (_lib.IndexQuery * len(parts))()
+    for i, (tsc, sp) in enumerate(built):
+        srt = None
+        if sorts is not None and sorts[i] is not None:
+            srt = _q_sorts(sorts[i], B)
+            keep.append(srt)
+        ixs[i] = _lib.IndexQuery(tsc.emb._h if tsc.emb else None, tsc.str._h if tsc.str else None, C.pointer(sp),
+                                 None if srt is None else C.cast(srt, C.c_void_p))
+    pins = None if promote is None else _pins(promote, B)[0]
+    n_items = 0 if pins is None else int(pins._keep[0][-1])
+    L = _stride(params)
+    docs, scores, sv = np.zeros((B, L), np.uint64), np.zeros((B, L), np.float32), np.zeros((B, L), np.float64)
+    n, cnt = np.zeros(B, np.uint32), np.zeros(B, np.uint64)
+    ps, pp = np.zeros(max(n_items, 1), np.float32), np.zeros(max(n_items, 1), np.uint8)
+    check(lib().oc_search_indexes(ctx._h, len(parts), ixs, None if pins is None else C.byref(pins), _p(docs), _p(scores),
+                                  _p(sv), _p(n), _p(cnt), _p(ps), _p(pp)))
+    return docs, scores, sv, n, cnt, ps[:n_items], pp[:n_items]
+
+
+def search_indexes(ctx: Context, parts: Sequence[IndexPart], params: "TokenScoreParams", sorts=None,
+                   promote=None) -> List[SearchHits]:
+    """search_indexes_arrays as one SearchHits per query."""
+    docs, scores, _, n, cnt, _, _ = search_indexes_arrays(ctx, parts, params, sorts, promote)
+    return [SearchHits(docs[i, :n[i]].copy(), scores[i, :n[i]].copy(), int(cnt[i])) for i in range(docs.shape[0])]
+
+
 class TermDictionary:
     """Native term dictionaries of the string fields of one Index + batch query resolution (oc_dict_*,
     csrc/dict.h): tokenize (+ stem hook), then per field exact / prefix / Levenshtein expansion — what

@@ -38,8 +38,9 @@ from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from .engine import (Context, DeviceFilter, EmbeddingFieldStorage, FacetStore, GeoPointField, OmcStore, SortField,
-                     StringFieldStorage, TermDictionary, TokenScoreContext, resolve_sort_by)
+from .engine import (Context, DeviceFilter, EmbeddingFieldStorage, FacetStore, GeoPointField, IndexPart, OmcStore, SortField,
+                     StringFieldStorage, TermDictionary, TokenScoreContext, TokenScoreParams, resolve_sort_by, search_indexes_arrays)
+from .types import SearchHits
 from .types import SortBy
 from .where import WhereFilter, WhereProgram, check_where_keys, compile_where, filter_from_program, parse_where
 
@@ -293,6 +294,10 @@ class IndexLoader:
         NOT(deletes) handle the program carries.  A program is valid until the next refresh_facets() / commit()."""
         w = where if isinstance(where, WhereFilter) else parse_where(where)
         check_where_keys(w, [self.filter_fields()])
+        return self._compile_where(w)
+
+    def _compile_where(self, w: WhereFilter) -> Optional[WhereProgram]:
+        """where_program without the key check: a key that is not a filter field of this index filters out everything."""
         if self._uncommitted_deleted and self._live is None:
             dele = DeviceFilter.from_ids(self.ctx, sorted(self._uncommitted_deleted), self.nbits)
             try:
@@ -337,3 +342,28 @@ class IndexLoader:
         for x in list(self._sorts.values()) + [self.facets, self.emb, self.strs, self.dict, self._live, self.omc_store] + list(self.geo.values()) + self._retired:
             if x is not None:
                 x.close()
+
+
+def search_collection(loaders: Sequence[IndexLoader], texts: Optional[Sequence[str]], params: TokenScoreParams, where=None,
+                      sort_by: Optional[SortBy] = None, q_vecs: Optional[np.ndarray] = None, promote=None,
+                      **resolve_kw) -> Tuple[List[SearchHits], np.ndarray]:
+    """search_on_indexes (read/search.rs:283-501) over the indexes of one collection, all on one ctx, in one
+    oc_search_indexes call: each index resolves the texts with its own dictionary, compiles `where` over its own filter
+    fields (a key that is a filter field of no index raises FilterFieldNotFound, search.rs:434-450; a key only some
+    indexes have filters out everything on the others), sorts by its own `sort_by` field and scores with its own OMC
+    map.  `params` holds the request (mode, limit_hint, offset, similarity, threshold, query_params) and is shared by
+    every index.  Returns (one SearchHits per query, the sort values [B, limit])."""
+    B = len(texts) if texts is not None else int(np.asarray(q_vecs).shape[0])
+    w = None if where is None else (where if isinstance(where, WhereFilter) else parse_where(where))
+    if w is not None:
+        check_where_keys(w, [l.filter_fields() for l in loaders])
+    parts, sorts = [], None if sort_by is None else []
+    for l in loaders:
+        fields = {"omc_store": l.omc()}
+        if w is not None:
+            fields["where_programs"] = [l._compile_where(w)] * B
+        parts.append(IndexPart(l.context(), None if texts is None else l.resolve(texts, **resolve_kw), q_vecs, fields))
+        if sorts is not None:
+            sorts.append([l.sort_by(sort_by)] * B)
+    docs, scores, sv, n, cnt, _, _ = search_indexes_arrays(loaders[0].ctx, parts, params, sorts, promote)
+    return [SearchHits(docs[i, :n[i]].copy(), scores[i, :n[i]].copy(), int(cnt[i])) for i in range(B)], sv

@@ -199,6 +199,17 @@ pub struct OcSort {
     pub order: c_int,
 }
 
+/// most indexes of one oc_search_indexes call
+pub const OC_MAX_INDEXES: u32 = 32;
+/// oc_index_query: one index of an oc_search_indexes call (its stores, inputs and per-query sorts; q_sorts may be NULL)
+#[repr(C)]
+pub struct OcIndexQuery {
+    pub emb: *mut OcEmb,
+    pub str_: *mut OcStr,
+    pub p: *const OcSearchParams,
+    pub q_sorts: *const OcSort,
+}
+
 /// one query's groupBy in oc_search_q_groups: its handle (NULL: no groups), max_results and sort (field NULL: score order)
 #[repr(C)]
 pub struct OcGroupReq {
@@ -415,6 +426,10 @@ extern "C" {
                            n: *const *const u32, counts: *const *const u64, pins: *const OcPins,
                            pin_scores: *const *const f32, pin_present: *const *const u8, out_doc_ids: *mut u64,
                            out_scores: *mut f32, out_sort_values: *mut f64, out_n: *mut u32, out_count: *mut u64) -> c_int;
+    /// every index of a collection on one ctx in one call, merged on the device (search_on_indexes)
+    pub fn oc_search_indexes(ctx: *mut OcCtx, n_indexes: u32, ix: *const OcIndexQuery, pins: *const OcPins,
+                             out_doc_ids: *mut u64, out_scores: *mut f32, out_sort_values: *mut f64, out_n: *mut u32,
+                             out_count: *mut u64, out_pin_scores: *mut f32, out_pin_present: *mut u8) -> c_int;
     // term dictionary + batch query resolution (tokenize_and_stem + FST expansion), host only
     pub fn oc_dict_create(n_fields: u32, out: *mut *mut OcDict) -> c_int;
     pub fn oc_dict_destroy(d: *mut OcDict);
