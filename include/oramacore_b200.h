@@ -716,7 +716,7 @@ int oc_search_pinned(oc_ctx *ctx, oc_emb *emb, oc_str *str, const oc_search_para
  * B x n_groups x group_stride; out_group_n: B x n_groups.  group_stride >= 2 x max_results + the most items of one query
  * when some query is active, else >= max_results (OC_ERR_INVALID otherwise).  Refusals as oc_search_pinned and
  * oc_search_groups, plus OC_ERR_UNSUPPORTED for an active query with 2 x max_results > OC_MAX_TOPK.  Multi-index
- * grouped searches with pins are not supported: a promoted document's membership spans indexes. */
+ * grouped searches with pins: oc_search_indexes_ex (a promoted document's membership spans indexes). */
 int oc_search_groups_pinned(oc_ctx *ctx, oc_emb *emb, oc_str *str, oc_group_by *groups, const oc_search_params *p,
                             uint32_t max_results, const oc_pins *pins, uint32_t group_stride, uint64_t *out_doc_ids,
                             float *out_scores, uint32_t *out_n, uint64_t *out_count, uint64_t *out_group_doc_ids,
@@ -919,9 +919,9 @@ int oc_merge_sorted(uint32_t n_indexes, uint32_t n_queries, uint32_t limit, uint
  * Refusals (nothing written): OC_ERR_UNSUPPORTED: p->sharded, a per-index depth (limit' above) over OC_MAX_TOPK;
  * OC_ERR_INVALID: n_indexes 0 or above OC_MAX_INDEXES, request fields that differ, a store, filter, sort field or OMC
  * store of another ctx, and everything the per-index call or the host merge would refuse.
- * Not covered: groupBy and facets across indexes (groups are keyed by value across indexes; facet counts add up by
- * label on the host), batching in oc_batcher, sharded collections.  Indexes run one after another on the ctx stream.
- * Callers whose indexes live on different contexts keep using the host merges above. */
+ * Not covered: batching in oc_batcher, sharded collections.  Indexes run one after another on the ctx stream.
+ * Callers whose indexes live on different contexts keep using the host merges above.  oc_search_indexes is
+ * oc_search_indexes_ex with ex = NULL and no groups or facets. */
 #define OC_MAX_INDEXES 32u
 typedef struct {
     oc_emb *emb;                     /* NULL: the index has no embedding field              */
@@ -932,6 +932,53 @@ typedef struct {
 int oc_search_indexes(oc_ctx *ctx, uint32_t n_indexes, const oc_index_query *ix, const oc_pins *pins,
                       uint64_t *out_doc_ids, float *out_scores, double *out_sort_values, uint32_t *out_n,
                       uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present);
+/* oc_search_indexes with groupBy and facets across the indexes (search_on_indexes with group_by and facets,
+ * read/search.rs:283-501; GroupContext, read/index/group.rs:104-168; FacetContext, read/index/facet.rs:147-209).
+ * Hits, counts and pin outputs are exactly oc_search_indexes' for the same inputs.  ex (NULL: no groups, no facets) has
+ * n_indexes entries, index i's:
+ *   - q_groups (NULL: none) and q_group_keys: B entries each; query b's local groups are those of q_groups[b] (NULL:
+ *     none), and q_group_keys[b] sends local group g to collection key q_group_keys[b][g] < q_n_keys[b].  The caller
+ *     builds the key maps from the group values, so the numbering of oc_group_by need not agree across indexes.
+ *   - facets, facet_reqs[n_facet_reqs] and facet_slots: request r is counted on index i alone, as oc_search_q_facets
+ *     counts it (a query filtered on that index is re-scored without its filter), and added to collection slot
+ *     facet_slots[r].  A slot belongs to the query whose [q_facet_offsets[b], q_facet_offsets[b + 1]) holds it.
+ * Groups: query b's collection group k is the union of the local groups every index maps to k; its rows are
+ * [G_b, G_b + q_n_keys[b]) of out_group_doc_ids / out_group_scores / out_group_sort_values (rows x group_stride) and
+ * out_group_n, G_b = the sum of q_n_keys over the queries before b.  Each row, with m = q_max_results[b]:
+ *   - score order: the top m of the union, score descending, ties by ascending document, NaN dropped (oc_merge_results
+ *     over the indexes' group rows, a missing source has n = 0);
+ *   - field order (query b sorted on every index, as oc_search_indexes requires): oc_merge_sorted over those rows, equal
+ *     values with the lower index first;
+ *   - an active pinned query: the union's top 2 x m in the row's order, with the items whose document is a member of
+ *     the collection group (of any source group) spliced as oc_search_groups_pinned splices them, not truncated; an
+ *     item's score is the first index whose map holds it.
+ * A row's sort value is the value its hit was placed by (NaN for an item and in score order); past n, entries are 0.
+ * group_stride follows oc_search_q_groups (>= m, >= 2 x m + items for an active query).
+ * Facets: out_facet_counts[s] for s in [q_facet_offsets[0], q_facet_offsets[B]) is the sum over the index requests
+ * mapped to s; a slot no index maps to is 0.
+ * Everything runs on the ctx stream under one lock: each index's group lists stay on the device (about 12 B per
+ * (index, local row, list slot)), its facet counts are added on the device, and the groups and counts come back in
+ * the one merged copy.  Refusals (nothing written): everything oc_search_indexes, oc_search_q_groups and
+ * oc_search_q_facets refuse; OC_ERR_INVALID: a key >= q_n_keys[b], two local groups of one index with one key for one
+ * query, a facet slot outside [q_facet_offsets[0], q_facet_offsets[B]), two requests of one index on one slot, facets
+ * or a group_by of another ctx, NULL q_n_keys / q_max_results with groups, NULL q_facet_offsets with facet requests;
+ * OC_ERR_UNSUPPORTED: 2^31 or more collection group rows. */
+typedef struct {
+    const oc_group_by *const *q_groups;       /* NULL: this index adds no groups; else B entries, NULL = none for query b */
+    const uint32_t *const *q_group_keys;      /* B entries: n_groups(q_groups[b]) collection keys, each < q_n_keys[b]   */
+    oc_facets *facets;                        /* NULL: no facet request on this index                                   */
+    uint32_t n_facet_reqs;
+    const oc_facet_req *facet_reqs;
+    const uint32_t *facet_slots;              /* n_facet_reqs: the collection slot each count is added to               */
+} oc_index_extras;
+int oc_search_indexes_ex(oc_ctx *ctx, uint32_t n_indexes, const oc_index_query *ix, const oc_index_extras *ex,
+                         const oc_pins *pins, const uint32_t *q_n_keys /* B, 0 = no groups */,
+                         const uint32_t *q_max_results /* B */, uint32_t group_stride,
+                         const uint32_t *q_facet_offsets /* B+1, may be NULL without facets */, uint64_t *out_doc_ids,
+                         float *out_scores, double *out_sort_values, uint32_t *out_n, uint64_t *out_count,
+                         float *out_pin_scores, uint8_t *out_pin_present, uint64_t *out_group_doc_ids,
+                         float *out_group_scores, double *out_group_sort_values, uint32_t *out_group_n,
+                         uint64_t *out_facet_counts);
 
 /* ---- term dictionary and query-term resolution (host; oc_dict_resolve_q may expand typos on a device) ------
  * The step the reference performs before the posting walk: TextParser::tokenize_and_stem(term) —

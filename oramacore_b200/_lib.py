@@ -54,7 +54,7 @@ EXPORTED_SYMBOLS = [
     "oc_group_by_create", "oc_group_by_destroy", "oc_search_groups",
     "oc_search_pinned", "oc_search_groups_pinned", "oc_merge_pinned",
     "oc_sort_field_create", "oc_sort_field_from_facets", "oc_sort_field_read", "oc_sort_field_destroy", "oc_search_sorted", "oc_search_q_sorted", "oc_search_groups_sorted", "oc_merge_sorted",
-    "oc_search_indexes",
+    "oc_search_indexes", "oc_search_indexes_ex",
     "oc_group_by_n_groups", "oc_search_q_groups", "oc_facets_check", "oc_search_q_facets",
     "oc_dict_create", "oc_dict_destroy", "oc_dict_add_terms", "oc_dict_lookup", "oc_dict_size", "oc_dict_set_stemmer", "oc_stem_english",
     "oc_dict_resolve", "oc_dict_resolve_q", "oc_dict_device_bytes", "oc_resolved_arrays", "oc_resolved_fill", "oc_resolved_free",
@@ -152,6 +152,11 @@ class Sort(C.Structure):
 
 class IndexQuery(C.Structure):   # oc_index_query: one index of an oc_search_indexes call
     _fields_ = [("emb", C.c_void_p), ("str", C.c_void_p), ("p", C.POINTER(SearchParams)), ("q_sorts", C.c_void_p)]
+
+
+class IndexExtras(C.Structure):   # oc_index_extras: one index's groups and facets in an oc_search_indexes_ex call
+    _fields_ = [("q_groups", C.c_void_p), ("q_group_keys", C.c_void_p), ("facets", C.c_void_p), ("n_facet_reqs", C.c_uint32),
+                ("facet_reqs", C.c_void_p), ("facet_slots", C.c_void_p)]
 
 
 class GroupReq(C.Structure):
@@ -324,6 +329,7 @@ def lib():
     L.oc_merge_sorted.argtypes = [u32, u32, u32, u32, u32, C.c_int, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), C.POINTER(vp),
                                   C.POINTER(vp), vp, C.POINTER(vp), C.POINTER(vp), vp, vp, vp, vp, vp]
     L.oc_search_indexes.argtypes = [vp, u32, C.POINTER(IndexQuery), vp] + [vp] * 7
+    L.oc_search_indexes_ex.argtypes = [vp, u32, C.POINTER(IndexQuery), vp, vp, vp, vp, u32, vp] + [vp] * 12
     L.oc_dict_create.argtypes = [u32, C.POINTER(vp)]
     L.oc_dict_destroy.argtypes = [vp]
     L.oc_dict_destroy.restype = None

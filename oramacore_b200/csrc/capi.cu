@@ -197,6 +197,7 @@ struct oc_ctx {
     DevBuf pin_row, pin_ft, pin_ftp, pin_score, pin_present, pin_top_doc, pin_top_score, pin_top_n, pin_gdoc, pin_gscore, pin_gn;   // pins
     DevBuf srt_doc, srt_row, srt_n, srt_ft, srt_ftp, srt_score, srt_present, srt_zero;   // sortBy
     DevBuf mi_doc, mi_score, mi_val, mi_n, mi_cnt, mi_pscore, mi_ppresent, mi_out;   // oc_search_indexes: per-index lists, page
+    DevBuf mg_doc, mg_score, mg_val, mg_n;   // oc_search_indexes_ex: per-index group lists
     DevBuf sfb_ws;                    // sort field build (sort_build.cuh), released before the call returns
     DevBuf q_bf16, q_f16, q_scale, q_rho, pre_post, dense_buf, g_thr, g_eps, g_ovf, g_ovfcnt, g_resc, g_cand, g_cnt, g_flag, g_max, r_qpad, r_qinv, r_map, r_doc, r_score, r_row, r_cnt, r_raw;
     // per-query where-filters (q_filters): the embedding rows' bitmap of every distinct handle, and the slots of the
@@ -2333,6 +2334,8 @@ struct FacetJob {
     uint64_t *out_counts = nullptr;
     const uint32_t *q_off = nullptr;   // oc_search_q_facets: its q_facet_offsets (a query with facets may run at limit 0)
     bool hits_optional = false;        // limit 0 allowed: the hits are not written, the vector stage runs at depth 0
+    unsigned long long *d_out = nullptr;   // oc_search_indexes_ex: device counts at o[k], added to in place (the indexes'
+                                           // counts sum there): no zeroing, no copy, no synchronise
 };
 struct FacetSliceDev {   // one distinct document slice and the counts that want it
     const uint64_t *docs;
@@ -2379,6 +2382,10 @@ struct GroupJob {
     const GroupHandle *d_hand = nullptr;
     const GroupSpan *d_spans = nullptr;
     const SortEntry *d_ents = nullptr;
+    // oc_search_indexes_ex: the top lists stay on the device (c->grp_*, row stride top) for the group merge, with no splice
+    // and no copy; q_deep[q] gives query q depth 2 x max_results without a splice (an active pinned query of the merge)
+    bool keep_top = false;
+    std::vector<uint8_t> q_deep;
 };
 struct PinJob {   // oc_search_pinned / oc_search_groups_pinned: the promote items, padded to `stride` slots per query
     const oc_pins *pins = nullptr;      // the caller's items (NULL: none)
@@ -3504,7 +3511,8 @@ static void sort_group_plan(SearchCall &k) {
             const uint32_t ent = sj ? sj->q_ent[q] : SORT_BY_SCORE;
             if (h == GROUP_NONE || gj->h[h]->n_groups == 0 || (ent != SORT_BY_SCORE) != bool(by_field)) continue;
             // sort_groups with pins takes every group's top 2 * max_results for an active query (sort.rs:137-142)
-            const uint32_t m = gj->q_m[q], depth = m * (pj->splice && pj->cnt[q] > 0 ? 2 : 1);
+            const bool deep = (pj->splice && pj->cnt[q] > 0) || (!gj->q_deep.empty() && gj->q_deep[q]);
+            const uint32_t m = gj->q_m[q], depth = m * (deep ? 2 : 1);
             k.g_spans.push_back(GroupSpan{first, q, h, depth, m, ent, gj->q_row[q]});
             first += gj->h[h]->n_groups;
             gj->top = std::max(gj->top, depth);
@@ -4700,7 +4708,7 @@ static int facet_plan(const FacetJob &fj, FacetPlan &pl) {
             pl.slices.push_back(FacetSliceDev{fl.docs + lo, hi - lo, 0, 0, 0});
             want.emplace_back();
         }
-        want[it->second].push_back(make_uint2(fj.q[k], (uint32_t)k));
+        want[it->second].push_back(make_uint2(fj.q[k], fj.d_out ? (uint32_t)fj.o[k] : (uint32_t)k));
     }
     uint64_t blocks = 0;
     for (size_t s = 0; s < pl.slices.size(); s++) {
@@ -4748,14 +4756,17 @@ static int run_facets(oc_ctx *c, const FacetJob &fj, const FacetPlan &pl, uint32
         }
         bits = c->dbits.as<uint32_t>(); stride = doc_words; cap_bits = fc->nbits;
     }
-    OCTRY(c->facet_out.ensure(n_out * 8));
-    CU(cudaMemsetAsync(c->facet_out.p, 0, n_out * 8, c->stream));
+    if (!fj.d_out) {
+        OCTRY(c->facet_out.ensure(n_out * 8));
+        CU(cudaMemsetAsync(c->facet_out.p, 0, n_out * 8, c->stream));
+    }
     if (pl.n_blocks) {
         facet_slice_count_kernel<<<pl.n_blocks, 256, 0, c->stream>>>(pl.d_slices, (uint32_t)pl.slices.size(), pl.d_pairs, bits, stride,
-                                                                     cap_bits, c->facet_out.as<unsigned long long>());
+                                                                     cap_bits, fj.d_out ? fj.d_out : c->facet_out.as<unsigned long long>());
         launched(c);
         CU(cudaGetLastError());
     }
+    if (fj.d_out) return OC_OK;
     std::vector<uint64_t> counts(n_out);
     CU(cudaMemcpyAsync(counts.data(), c->facet_out.p, n_out * 8, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
@@ -4767,9 +4778,12 @@ static int run_facets(oc_ctx *c, const FacetJob &fj, const FacetPlan &pl, uint32
 // only the uncommitted deletes stay excluded, and stores tombstone deletes at once), so that the counts do not collapse
 // onto the selected category.  The hits of this pass are dropped.
 // q_params_ok: the sub-batch pass of oc_search_q_facets (oc_search_facets takes one set of scalars).
+static void drop_filters(oc_search_params &q) {
+    q.filter_bits = nullptr; q.filter_nbits = 0; q.filter = nullptr; q.q_filters = nullptr; q.q_where = nullptr;
+}
 static int facets_unfiltered(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, FacetJob &fj, bool q_params_ok) {
     oc_search_params q = *p;
-    q.filter_bits = nullptr; q.filter_nbits = 0; q.filter = nullptr; q.q_filters = nullptr; q.q_where = nullptr;
+    drop_filters(q);
     const uint32_t B = p->n_queries;
     std::vector<uint64_t> docs(size_t(B) * p->limit), cnt(B);
     std::vector<float> scores(size_t(B) * p->limit);
@@ -4968,6 +4982,7 @@ static int run_groups(oc_ctx *c, const GroupJob &gj, int mode, const StrSnap *S,
         launched(c);
         CU(cudaGetLastError());
     }
+    if (gj.keep_top) return OC_OK;
     const uint64_t *res_doc = gp.out_doc;
     const float *res_score = gp.out_score;
     const uint32_t *res_n = gp.out_n;
@@ -5332,6 +5347,62 @@ extern "C" int oc_search_q_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_
                        out_pin_present);
 }
 
+// The sub-batch `sub` of p that oc_search_q_facets re-scores for the facets of its filtered queries: their vectors and
+// token CSR, their q_params entries, without groups, sorts or pins (facets_unfiltered drops the filters).
+struct FacetSubBatch {
+    oc_search_params q;
+    std::vector<float> vecs;
+    std::vector<uint32_t> q_tok{0}, tok_term{0}, t_field, t_id;
+    std::vector<float> t_weight;
+    std::vector<oc_query_params> sub_qp;
+};
+static void facet_sub_batch(const oc_search_params *p, const oc_emb *emb, const std::vector<uint32_t> &sub, FacetSubBatch &sb) {
+    const uint32_t S = (uint32_t)sub.size();
+    oc_search_params &q = sb.q;
+    q = *p;
+    q.n_queries = S;
+    std::vector<float> &vecs = sb.vecs, &t_weight = sb.t_weight;
+    std::vector<uint32_t> &q_tok = sb.q_tok, &tok_term = sb.tok_term, &t_field = sb.t_field, &t_id = sb.t_id;
+    // per-query parameters: the sub-batch's entries; a vector entry's row and a text entry's tokens are the ones read
+    std::vector<oc_query_params> &sub_qp = sb.sub_qp;
+    bool sub_v = p->mode != OC_MODE_FULLTEXT, sub_ft = p->mode != OC_MODE_VECTOR;
+    if (p->q_params) {
+        sub_v = sub_ft = false;
+        for (uint32_t b : sub) {
+            sub_qp.push_back(p->q_params[b]);
+            sub_v = sub_v || p->q_params[b].mode != OC_MODE_FULLTEXT;
+            sub_ft = sub_ft || p->q_params[b].mode != OC_MODE_VECTOR;
+        }
+        q.q_params = sub_qp.data();
+    }
+    auto text_of = [&](uint32_t b) { return !p->q_params || p->q_params[b].mode != OC_MODE_VECTOR; };
+    if (sub_v && emb && p->q_vecs) {
+        const size_t dim = emb->dim;
+        vecs.resize(size_t(S) * dim);
+        for (uint32_t s = 0; s < S; s++)
+            if (!p->q_params || p->q_params[sub[s]].mode != OC_MODE_FULLTEXT)
+                memcpy(vecs.data() + size_t(s) * dim, p->q_vecs + size_t(sub[s]) * dim, dim * 4);
+        q.q_vecs = vecs.data();
+    }
+    if (sub_ft && p->q_token_offsets) {
+        for (uint32_t b : sub) {
+            if (!text_of(b)) { q_tok.push_back((uint32_t)tok_term.size() - 1); continue; }
+            for (uint32_t t = p->q_token_offsets[b]; t < p->q_token_offsets[b + 1]; t++) {
+                for (uint32_t e = p->token_term_offsets[t]; e < p->token_term_offsets[t + 1]; e++) {
+                    t_field.push_back(p->term_field[e]);
+                    t_id.push_back(p->term_id[e]);
+                    t_weight.push_back(p->term_weight ? p->term_weight[e] : 1.0f);
+                }
+                tok_term.push_back((uint32_t)t_id.size());
+            }
+            q_tok.push_back((uint32_t)tok_term.size() - 1);
+        }
+        t_field.push_back(0); t_id.push_back(0); t_weight.push_back(1.0f);   // never read: non-NULL arrays for an empty CSR
+        q.q_token_offsets = q_tok.data(); q.token_term_offsets = tok_term.data();
+        q.term_field = t_field.data(); q.term_id = t_id.data(); q.term_weight = t_weight.data();
+    }
+}
+
 // ------------------------------------------------------------------------------------ one call over the indexes (index_merge.cuh)
 static bool same_f32(float a, float b) { return memcmp(&a, &b, 4) == 0; }
 // the request fields of oc_search_indexes, which every index must share
@@ -5359,11 +5430,116 @@ static void timing_add(oc_timing &t, const oc_timing &a) {
     t.bm25_dense_items += a.bm25_dense_items; t.bm25_dense_skipped += a.bm25_dense_skipped;
 }
 
+// The groups of one batch of oc_search_indexes_ex: per index its GroupJob (local rows) and, per distinct combination of
+// (handle, key map) over the indexes, the source table of the collection keys (built once per combination).
+struct MiGroups {
+    uint32_t rows = 0, gtop = 0, sets = 0;   // gtop: the largest depth of a per-index list, also the merge's largest take
+    std::vector<GroupJob> gj;              // [n_idx]
+    std::vector<uint8_t> on;               // [n_idx] the index adds groups to some query
+    std::vector<uint32_t> src_g;           // source tables, concatenated
+    std::vector<GroupHandle> set_h;        // [set][n_idx]
+    std::vector<GroupSpan> spans;          // one per query with collection groups
+    std::vector<uint32_t> q_lrow;          // [n_idx][B]
+};
+// Checks the groups of ex and plans them.  Nothing is written on failure.
+static int mi_groups_plan(oc_ctx *c, uint32_t ni, uint32_t B, const oc_index_extras *ex, const uint32_t *q_n_keys,
+                          const uint32_t *q_max_results, uint32_t group_stride, const std::vector<uint8_t> &q_active,
+                          const PinJob &pj_all, MiGroups &mg) {
+    bool any = false;
+    for (uint32_t i = 0; ex && i < ni; i++) any = any || ex[i].q_groups;
+    for (uint32_t b = 0; q_n_keys && b < B; b++) any = any || q_n_keys[b];
+    if (!any) return OC_OK;
+    if (!q_n_keys || !q_max_results) return fail(OC_ERR_INVALID, "groups: NULL q_n_keys / q_max_results");
+    mg.gj.resize(ni);
+    mg.on.assign(ni, 0);
+    mg.q_lrow.assign(size_t(ni) * B, 0);
+    uint64_t rows = 0;
+    for (uint32_t b = 0; b < B; b++) {
+        const uint32_t m = q_max_results[b];
+        if (!q_n_keys[b]) continue;
+        if (m > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "query %u: max_results %u > %u", b, m, OC_MAX_TOPK);
+        if (q_active[b] && 2 * m > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "query %u: pins: 2 x max_results %u > %u", b, 2 * m, OC_MAX_TOPK);
+        const uint64_t need = q_active[b] ? 2ull * m + pj_all.cnt[b] : m;
+        if (group_stride < need) return fail(OC_ERR_INVALID, "query %u: group_stride %u < %llu", b, group_stride, (unsigned long long)need);
+        rows += q_n_keys[b];
+        mg.gtop = std::max(mg.gtop, m * (q_active[b] ? 2u : 1u));
+    }
+    if (rows > 0x7fffffffull) return fail(OC_ERR_UNSUPPORTED, "groups: %llu collection group rows >= 2^31", (unsigned long long)rows);
+    mg.rows = (uint32_t)rows;
+    // each index's GroupJob, with the depth of an active query although its own pins do not apply
+    for (uint32_t i = 0; i < ni; i++) {
+        GroupJob &gj = mg.gj[i];
+        gj.q_h.assign(B, GROUP_NONE); gj.q_m.assign(B, 0); gj.q_row.assign(B, 0);
+        gj.keep_top = true;
+        gj.q_deep = q_active;
+        const oc_index_extras *e = ex ? &ex[i] : nullptr;
+        if (!e || !e->q_groups) continue;
+        if (!e->q_group_keys) return fail(OC_ERR_INVALID, "index %u: q_groups without q_group_keys", i);
+        uint64_t lrows = 0;
+        for (uint32_t b = 0; b < B; b++) {
+            const oc_group_by *g = e->q_groups[b];
+            if (!g) continue;
+            if (g->ctx != c) return fail(OC_ERR_INVALID, "index %u: group_by of query %u belongs to another ctx", i, b);
+            if (g->n_groups && !e->q_group_keys[b]) return fail(OC_ERR_INVALID, "index %u: query %u has groups and no key map", i, b);
+            if (g->n_groups == 0) continue;
+            uint32_t h = 0;
+            while (h < gj.h.size() && gj.h[h] != g) h++;
+            if (h == gj.h.size()) gj.h.push_back(const_cast<oc_group_by *>(g));
+            gj.q_h[b] = h; gj.q_m[b] = q_max_results[b]; gj.q_row[b] = (uint32_t)lrows;
+            mg.q_lrow[size_t(i) * B + b] = (uint32_t)lrows;
+            lrows += g->n_groups;
+            mg.on[i] = 1;
+        }
+        if (lrows > 0x7fffffffull) return fail(OC_ERR_UNSUPPORTED, "index %u: %llu group rows >= 2^31", i, (unsigned long long)lrows);
+        gj.rows = (uint32_t)lrows;
+    }
+    // the source tables: one per distinct (handle, key map) combination; a query's span points at its combination
+    std::map<std::vector<uintptr_t>, std::pair<uint32_t, uint32_t>> sets;   // combination -> (table offset, set)
+    uint32_t first = 0;
+    for (uint32_t b = 0; b < B; b++) {
+        const uint32_t nk = q_n_keys[b];
+        std::vector<uintptr_t> key(size_t(2) * ni + 1, 0);
+        key[0] = nk;
+        for (uint32_t i = 0; i < ni; i++) {
+            const oc_group_by *g = ex && ex[i].q_groups ? ex[i].q_groups[b] : nullptr;
+            if (!g || !g->n_groups) continue;
+            key[1 + 2 * i] = uintptr_t(g);
+            key[2 + 2 * i] = uintptr_t(ex[i].q_group_keys[b]);
+        }
+        auto it = sets.find(key);
+        if (it == sets.end()) {
+            const uint32_t off = (uint32_t)mg.src_g.size();
+            if (uint64_t(off) + uint64_t(nk) * ni > 0x7fffffffull) return fail(OC_ERR_UNSUPPORTED, "groups: source tables >= 2^31 entries");
+            mg.src_g.resize(size_t(off) + size_t(nk) * ni, IM_NO_SRC);
+            for (uint32_t i = 0; i < ni; i++) {
+                const oc_group_by *g = reinterpret_cast<const oc_group_by *>(key[1 + 2 * i]);
+                const uint32_t *km = reinterpret_cast<const uint32_t *>(key[2 + 2 * i]);
+                mg.set_h.push_back(g ? GroupHandle{g->off, g->docs, nullptr, g->n_groups} : GroupHandle{nullptr, nullptr, nullptr, 0});
+                for (uint32_t l = 0; g && l < g->n_groups; l++) {
+                    if (km[l] >= nk) return fail(OC_ERR_INVALID, "index %u, query %u: group %u has key %u >= q_n_keys %u", i, b, l, km[l], nk);
+                    uint32_t &e = mg.src_g[off + size_t(km[l]) * ni + i];
+                    if (e != IM_NO_SRC) return fail(OC_ERR_INVALID, "index %u, query %u: groups %u and %u have one key %u", i, b, e, l, km[l]);
+                    e = l;
+                }
+            }
+            it = sets.emplace(key, std::make_pair(off, mg.sets++)).first;
+        }
+        if (!nk) continue;
+        mg.spans.push_back(GroupSpan{first, b, it->second.first, 0, q_max_results[b], it->second.second, first});
+        first += nk;
+    }
+    return OC_OK;
+}
+
 // search_on_indexes: every index through its own stages into a per-index slot of the ctx's workspaces (under one ctx
-// lock), then index_merge_kernel and one copy of the merged page.  Nothing is written on failure.
-extern "C" int oc_search_indexes(oc_ctx *c, uint32_t n_indexes, const oc_index_query *ix, const oc_pins *pins,
-                                 uint64_t *out_doc_ids, float *out_scores, double *out_sort_values, uint32_t *out_n,
-                                 uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present) {
+// lock), then its group lists and facet counts, then index_merge_kernel and index_group_merge_kernel and one copy of
+// the merged blob.  Nothing is written on failure.
+extern "C" int oc_search_indexes_ex(oc_ctx *c, uint32_t n_indexes, const oc_index_query *ix, const oc_index_extras *ex,
+                                    const oc_pins *pins, const uint32_t *q_n_keys, const uint32_t *q_max_results,
+                                    uint32_t group_stride, const uint32_t *q_facet_offsets, uint64_t *out_doc_ids, float *out_scores,
+                                    double *out_sort_values, uint32_t *out_n, uint64_t *out_count, float *out_pin_scores,
+                                    uint8_t *out_pin_present, uint64_t *out_group_doc_ids, float *out_group_scores,
+                                    double *out_group_sort_values, uint32_t *out_group_n, uint64_t *out_facet_counts) {
     if (!c || !ix || !out_doc_ids || !out_scores || !out_n || !out_count) return fail(OC_ERR_INVALID, "NULL argument");
     if (n_indexes == 0 || n_indexes > OC_MAX_INDEXES) return fail(OC_ERR_INVALID, "n_indexes %u: expected 1 .. %u", n_indexes, OC_MAX_INDEXES);
     for (uint32_t i = 0; i < n_indexes; i++) {
@@ -5394,7 +5570,7 @@ extern "C" int oc_search_indexes(oc_ctx *c, uint32_t n_indexes, const oc_index_q
         q_sort[b] = order == OC_SORT_ASC ? IM_ASC : IM_DESC;
         any_sorted = true;
     }
-    // pins: every index looks the items up (apply = 0); the merge splices the active queries
+    // pins: every index looks the items up (apply = 0); the merges splice the active queries
     PinJob pj_all;
     OCTRY(pin_job_init(pins, B, pj_all));
     oc_pins pins0{};
@@ -5424,13 +5600,67 @@ extern "C" int oc_search_indexes(oc_ctx *c, uint32_t n_indexes, const oc_index_q
         if (depth > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "per-index depth %llu > %u", (unsigned long long)depth, OC_MAX_TOPK);
     }
     const uint32_t stride = (uint32_t)std::max<uint64_t>(depth, 1);
-    // every index's call, checked before anything runs
+    // groups: each index's local rows and the collection's source tables
+    MiGroups mg;
+    OCTRY(mi_groups_plan(c, n_indexes, B, ex, q_n_keys, q_max_results, group_stride, q_active, pj_all, mg));
+    const bool groups = !mg.gj.empty();
+    if (mg.rows && (!out_group_n || (group_stride && (!out_group_doc_ids || !out_group_scores))))
+        return fail(OC_ERR_INVALID, "NULL group output");
+    // facets: per index, the requests of its unfiltered queries count on its main pass, those of its filtered queries on
+    // an unfiltered pass over their sub-batch; every count is added to its collection slot
+    bool any_facets = false;
+    for (uint32_t i = 0; ex && i < n_indexes; i++) any_facets = any_facets || (ex[i].facets && ex[i].n_facet_reqs);
+    const uint32_t *off = q_facet_offsets;
+    const uint32_t s0 = off ? off[0] : 0, n_slots = off ? off[B] - off[0] : 0;
+    if (off)
+        for (uint32_t b = 0; b < B; b++)
+            if (off[b + 1] < off[b]) return fail(OC_ERR_INVALID, "q_facet_offsets is not monotone at query %u", b);
+    if (any_facets && !off) return fail(OC_ERR_INVALID, "facet requests without q_facet_offsets");
+    if (n_slots && !out_facet_counts) return fail(OC_ERR_INVALID, "NULL facet counts");
+    std::vector<FacetJob> fjm(n_indexes), fjs(n_indexes);
+    std::vector<std::vector<uint32_t>> f_sub(n_indexes);
+    std::vector<std::unique_ptr<FacetSubBatch>> f_sb(n_indexes);
+    for (uint32_t i = 0; any_facets && i < n_indexes; i++) {
+        const oc_index_extras &e = ex[i];
+        if (!e.facets || !e.n_facet_reqs) continue;
+        if (e.facets->ctx != c) return fail(OC_ERR_INVALID, "index %u: facets belong to another ctx", i);
+        if (!e.facet_reqs || !e.facet_slots) return fail(OC_ERR_INVALID, "index %u: NULL facet_reqs / facet_slots", i);
+        OCTRY(oc_facets_check(e.facets, e.facet_reqs, e.n_facet_reqs));
+        const oc_search_params *p = ix[i].p;
+        std::vector<uint8_t> seen(n_slots, 0);
+        std::vector<uint32_t> sub_of(B, 0xffffffffu);
+        FacetJob &mj = fjm[i], &fj = fjs[i];
+        mj.fc = fj.fc = e.facets; mj.reqs = fj.reqs = e.facet_reqs;
+        fj.hits_optional = true;
+        for (uint32_t r = 0; r < e.n_facet_reqs; r++) {
+            const uint32_t s = e.facet_slots[r];
+            if (s < s0 || s - s0 >= n_slots) return fail(OC_ERR_INVALID, "index %u: facet request %u: slot %u outside [%u, %u)", i, r, s, s0, s0 + n_slots);
+            if (seen[s - s0]) return fail(OC_ERR_INVALID, "index %u: two facet requests on slot %u", i, s);
+            seen[s - s0] = 1;
+            const uint32_t b = uint32_t(std::upper_bound(off, off + B + 1, s) - off) - 1;   // the query whose range holds s
+            const bool filtered = p->filter || p->filter_bits || (p->q_filters && p->q_filters[b]) ||
+                                  (p->q_where && p->q_where->q_node_offsets && p->q_where->q_node_offsets[b + 1] > p->q_where->q_node_offsets[b]);
+            uint32_t row = b;
+            if (filtered) {
+                if (sub_of[b] == 0xffffffffu) { sub_of[b] = (uint32_t)f_sub[i].size(); f_sub[i].push_back(b); }
+                row = sub_of[b];
+            }
+            FacetJob &j = filtered ? fj : mj;
+            j.q.push_back(row); j.r.push_back(r); j.o.push_back(s - s0);
+        }
+        if (!f_sub[i].empty()) {
+            f_sb[i].reset(new FacetSubBatch());
+            facet_sub_batch(p, ix[i].emb, f_sub[i], *f_sb[i]);
+            drop_filters(f_sb[i]->q);
+        }
+    }
+    // every index's calls, checked before anything runs
     std::vector<oc_search_params> ps(n_indexes);
     std::vector<SortJob> sjs(n_indexes);
     std::vector<PinJob> pjs(n_indexes);
     std::vector<std::unique_ptr<SearchReq>> reqs;
-    std::vector<std::unique_ptr<SearchCall>> calls;
-    const bool with_pj = pins || any_sorted;
+    std::vector<std::unique_ptr<SearchCall>> calls, fcalls(n_indexes);
+    const bool with_pj = pins || any_sorted || groups;
     for (uint32_t i = 0; i < n_indexes; i++) {
         ps[i] = *ix[i].p;
         ps[i].limit = stride; ps[i].offset = 0; ps[i].vector_limit = limit;
@@ -5442,14 +5672,25 @@ extern "C" int oc_search_indexes(oc_ctx *c, uint32_t n_indexes, const oc_index_q
         SearchReq &r = *reqs.back();
         r.pj = with_pj ? &pjs[i] : nullptr;
         r.sj = any_sorted ? &sjs[i] : nullptr;
+        r.gj = groups && mg.on[i] ? &mg.gj[i] : nullptr;
+        r.fj = fjm[i].q.empty() ? nullptr : &fjm[i];
         r.q_filters_ok = r.q_params_ok = true;
         calls.emplace_back(new SearchCall(c, ix[i].emb, ix[i].str, r));
         OCTRY(search_check(*calls.back()));
+        if (f_sb[i]) {   // the unfiltered facet pass of the index's filtered queries
+            reqs.emplace_back(new SearchReq(&f_sb[i]->q, out_doc_ids, out_scores, out_n, out_count));
+            SearchReq &fr = *reqs.back();
+            fr.fj = &fjs[i];
+            fr.q_filters_ok = fr.q_params_ok = true;
+            fcalls[i].reset(new SearchCall(c, ix[i].emb, ix[i].str, fr));
+            OCTRY(search_check(*fcalls[i]));
+        }
     }
     if (B == 0) return OC_OK;
     for (uint32_t i = 0; i < n_indexes; i++) {   // each index's string snapshot, before the lock
         calls[i]->snap = ix[i].str ? str_snapshot(ix[i].str) : nullptr;
         calls[i]->S = calls[i]->snap.get();
+        if (fcalls[i]) { fcalls[i]->snap = calls[i]->snap; fcalls[i]->S = calls[i]->S; }
     }
     std::lock_guard<std::mutex> g(c->mu);
     CU(cudaSetDevice(c->device));
@@ -5461,6 +5702,28 @@ extern "C" int oc_search_indexes(oc_ctx *c, uint32_t n_indexes, const oc_index_q
     OCTRY(c->mi_cnt.ensure(size_t(n_indexes) * B * 8));
     if (any_sorted) OCTRY(c->mi_val.ensure(n_indexes * per * 8));
     if (pstr) { OCTRY(c->mi_pscore.ensure(n_indexes * nps * 4)); OCTRY(c->mi_ppresent.ensure(n_indexes * nps)); }
+    // the group lists of every index: [n_idx][rows][gtop]
+    uint32_t grows = 0;
+    for (const GroupJob &gj : mg.gj) grows = std::max(grows, gj.rows);
+    const size_t gper = size_t(grows) * mg.gtop;
+    if (groups) {
+        OCTRY(c->mg_doc.ensure(std::max<size_t>(n_indexes * gper, 1) * 8));
+        OCTRY(c->mg_score.ensure(std::max<size_t>(n_indexes * gper, 1) * 4));
+        OCTRY(c->mg_n.ensure(std::max<size_t>(size_t(n_indexes) * grows, 1) * 4));
+        if (any_sorted) OCTRY(c->mg_val.ensure(std::max<size_t>(n_indexes * gper, 1) * 8));
+    }
+    // the merged blob: the page, counts and pin outputs, then the group rows and the facet counts
+    auto al = [](size_t x) { return (x + 255) & ~size_t(255); };
+    const size_t R = mg.rows, gs = group_stride;
+    const size_t o_sc = al(size_t(B) * limit * 8), o_val = o_sc + al(size_t(B) * limit * 4), o_n = o_val + al(size_t(B) * limit * 8),
+                 o_cnt = o_n + al(size_t(B) * 4), o_ps = o_cnt + al(size_t(B) * 8), o_pp = o_ps + al(nps * 4), o_gd = o_pp + al(nps),
+                 o_gs = o_gd + al(R * gs * 8), o_gv = o_gs + al(R * gs * 4), o_gn = o_gv + al(R * gs * 8), o_fc = o_gn + al(R * 4),
+                 out_bytes = o_fc + size_t(n_slots) * 8;
+    OCTRY(c->mi_out.ensure(out_bytes));
+    uint8_t *dout = c->mi_out.as<uint8_t>();
+    unsigned long long *d_fc = reinterpret_cast<unsigned long long *>(dout + o_fc);
+    if (n_slots) CU(cudaMemsetAsync(d_fc, 0, size_t(n_slots) * 8, c->stream));
+    for (uint32_t i = 0; i < n_indexes; i++) { fjm[i].d_out = d_fc; fjs[i].d_out = d_fc; }
     // where each index's hits find their sort values: the handles' rank values on the device (built once per handle)
     std::vector<ImSortSrc> src(any_sorted ? size_t(n_indexes) * B : 0, ImSortSrc{nullptr, nullptr, 0});
     for (uint32_t i = 0; any_sorted && i < n_indexes; i++) {
@@ -5476,9 +5739,20 @@ extern "C" int oc_search_indexes(oc_ctx *c, uint32_t n_indexes, const oc_index_q
         }
     }
     oc_timing total{};
+    // the device time of an index's group and facet stages, read once a later synchronise has passed them
+    bool extra_pending = false;
+    auto extra_time = [&]() -> int {
+        if (!extra_pending) return OC_OK;
+        float ms = 0.f;
+        CU(cudaEventElapsedTime(&ms, c->ev[EV_GRP0], c->ev[EV_GRP1]));
+        total.device_ms += ms;
+        extra_pending = false;
+        return OC_OK;
+    };
     for (uint32_t i = 0; i < n_indexes; i++) {
         SearchCall &k = *calls[i];
         OCTRY(search_stages(k));
+        OCTRY(extra_time());
         OCTRY(finish_timing(c, k.has_v && k.vlimit && k.emb->n_rows > 0, k.has_ft, true, k.did_comm));
         c->timing.d2h_bytes = k.out_bytes;
         timing_add(total, c->timing);
@@ -5491,22 +5765,60 @@ extern "C" int oc_search_indexes(oc_ctx *c, uint32_t n_indexes, const oc_index_q
             CU(cudaMemcpyAsync(c->mi_pscore.as<float>() + i * nps, c->pin_score.p, nps * 4, cudaMemcpyDeviceToDevice, c->stream));
             CU(cudaMemcpyAsync(c->mi_ppresent.as<uint8_t>() + i * nps, c->pin_present.p, nps, cudaMemcpyDeviceToDevice, c->stream));
         }
+        // its facet counts, added into the collection slots, and its group lists into its slot
+        const GroupJob *gj = k.r.gj;
+        const uint32_t l0 = c->call_launches;
+        if (k.facets || (gj && gj->rows)) {
+            CU(cudaEventRecord(c->ev[EV_GRP0], c->stream));
+            if (k.facets) OCTRY(run_facets(c, *k.r.fj, k.fpl, B, k.has_ft, k.has_v, k.S, k.n_tiles, k.vlimit));
+            if (gj && gj->rows) {
+                OCTRY(run_groups(c, *gj, k.mode, k.S, k.n_tiles, k.vlimit, k.fp.omc_doc, k.fp.omc_mult, k.n_omc, *k.r.pj, k.s_plan.at(c->in_blob)));
+                const size_t o = i * gper;
+                if (gj->top) {
+                    CU(cudaMemcpy2DAsync(c->mg_doc.as<uint64_t>() + o, size_t(mg.gtop) * 8, c->grp_doc.p, size_t(gj->top) * 8,
+                                         size_t(gj->top) * 8, gj->rows, cudaMemcpyDeviceToDevice, c->stream));
+                    CU(cudaMemcpy2DAsync(c->mg_score.as<float>() + o, size_t(mg.gtop) * 4, c->grp_score.p, size_t(gj->top) * 4,
+                                         size_t(gj->top) * 4, gj->rows, cudaMemcpyDeviceToDevice, c->stream));
+                }
+                CU(cudaMemcpyAsync(c->mg_n.as<uint32_t>() + size_t(i) * grows, c->grp_n.p, size_t(gj->rows) * 4, cudaMemcpyDeviceToDevice, c->stream));
+            }
+            CU(cudaEventRecord(c->ev[EV_GRP1], c->stream));
+            extra_pending = true;
+            total.kernel_launches += c->call_launches - l0;
+        }
+        if (fcalls[i]) {   // the unfiltered facet pass of its filtered queries
+            SearchCall &f = *fcalls[i];
+            OCTRY(search_stages(f));
+            OCTRY(extra_time());
+            OCTRY(finish_timing(c, f.has_v && f.vlimit && f.emb->n_rows > 0, f.has_ft, true, f.did_comm));
+            c->timing.d2h_bytes = f.out_bytes;
+            timing_add(total, c->timing);
+            CU(cudaEventRecord(c->ev[EV_GRP0], c->stream));
+            const uint32_t l1 = c->call_launches;
+            OCTRY(run_facets(c, *f.r.fj, f.fpl, f.B, f.has_ft, f.has_v, f.S, f.n_tiles, f.vlimit));
+            CU(cudaEventRecord(c->ev[EV_GRP1], c->stream));
+            extra_pending = true;
+            total.kernel_launches += c->call_launches - l1;
+        }
     }
-    // the merge: its tables in one upload, one CTA per query, the page in one copy
+    // the merges: their tables in one upload, one CTA per query (hits) and per (query, collection group), one copy
     Packer pk;
     const Slot<uint8_t> s_sort = pk.add(q_sort.data(), B), s_act = pk.add(q_active.data(), B);
     const Slot<uint2> s_page = pk.add(q_page.data(), B);
     Slot<ImSortSrc> s_src;
     Slot<uint64_t> s_pdoc;
-    Slot<uint32_t> s_ppos, s_pcnt;
+    Slot<uint32_t> s_ppos, s_pcnt, s_srcg, s_lrow;
+    Slot<GroupHandle> s_seth;
+    Slot<GroupSpan> s_spans;
     if (any_sorted) s_src = pk.add(src.data(), src.size());
     if (pstr) { s_pdoc = pk.add(pj_all.doc.data(), nps); s_ppos = pk.add(pj_all.pos.data(), nps); s_pcnt = pk.add(pj_all.cnt.data(), B); }
-    auto al = [](size_t x) { return (x + 255) & ~size_t(255); };
-    const size_t o_sc = al(size_t(B) * limit * 8), o_val = o_sc + al(size_t(B) * limit * 4), o_n = o_val + al(size_t(B) * limit * 8),
-                 o_cnt = o_n + al(size_t(B) * 4), o_ps = o_cnt + al(size_t(B) * 8), o_pp = o_ps + al(nps * 4), out_bytes = o_pp + nps;
-    OCTRY(c->mi_out.ensure(out_bytes));
+    if (mg.rows) {
+        s_srcg = pk.add(mg.src_g.data(), mg.src_g.size());
+        s_lrow = pk.add(mg.q_lrow.data(), mg.q_lrow.size());
+        s_seth = pk.add(mg.set_h.data(), mg.set_h.size());
+        s_spans = pk.add(mg.spans.data(), mg.spans.size());
+    }
     OCTRY(c->h_out.ensure(out_bytes));
-    uint8_t *dout = c->mi_out.as<uint8_t>();
     CU(cudaEventRecord(c->ev[EV_START], c->stream));
     OCTRY(upload(pk, c->h_in, c->in_blob, c->stream));
     CU(cudaEventRecord(c->ev[EV_H2D], c->stream));
@@ -5528,11 +5840,34 @@ extern "C" int oc_search_indexes(oc_ctx *c, uint32_t n_indexes, const oc_index_q
     index_merge_kernel<<<B, IM_THREADS, smem, c->stream>>>(mp);
     launched(c);
     CU(cudaGetLastError());
+    if (mg.rows) {
+        IndexGroupMergeParams gp{};
+        gp.n_idx = n_indexes; gp.B = B;
+        gp.spans = s_spans.at(c->in_blob); gp.n_spans = (uint32_t)mg.spans.size();
+        gp.src_g = s_srcg.at(c->in_blob); gp.set_h = s_seth.at(c->in_blob); gp.q_lrow = s_lrow.at(c->in_blob);
+        gp.rows = grows; gp.gtop = mg.gtop;
+        gp.g_doc = c->mg_doc.as<uint64_t>(); gp.g_score = c->mg_score.as<float>(); gp.g_n = c->mg_n.as<uint32_t>();
+        gp.g_val = c->mg_val.as<double>();
+        gp.src = mp.src; gp.q_sort = mp.q_sort; gp.q_active = mp.q_active;
+        gp.pin_stride = pstr; gp.kp2 = mp.kp2; gp.pin_doc = mp.pin_doc; gp.pin_pos = mp.pin_pos; gp.pin_cnt = mp.pin_cnt;
+        gp.pin_score = mp.pin_score; gp.pin_present = mp.pin_present;
+        gp.take_max = std::max<uint32_t>(mg.gtop, 1);
+        gp.n_slots = (uint32_t)std::min<uint64_t>(group_stride, uint64_t(gp.take_max) + pstr);
+        gp.stride = group_stride;
+        gp.out_doc = reinterpret_cast<uint64_t *>(dout + o_gd); gp.out_score = reinterpret_cast<float *>(dout + o_gs);
+        gp.out_value = reinterpret_cast<double *>(dout + o_gv); gp.out_n = reinterpret_cast<uint32_t *>(dout + o_gn);
+        const size_t gsmem = index_group_merge_smem(gp.take_max, pstr, gp.kp2, gp.n_slots);
+        CU(smem_cfg(c->device, (const void *)index_group_merge_kernel, gsmem));
+        index_group_merge_kernel<<<mg.rows, IM_THREADS, gsmem, c->stream>>>(gp);
+        launched(c);
+        CU(cudaGetLastError());
+    }
     CU(cudaEventRecord(c->ev[EV_DEV], c->stream));
     uint8_t *h = c->h_out.as<uint8_t>();
     CU(cudaMemcpyAsync(h, dout, out_bytes, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaEventRecord(c->ev[EV_D2H], c->stream));
     CU(cudaStreamSynchronize(c->stream));
+    OCTRY(extra_time());
     memcpy(out_doc_ids, h, size_t(B) * limit * 8);
     memcpy(out_scores, h + o_sc, size_t(B) * limit * 4);
     if (out_sort_values) memcpy(out_sort_values, h + o_val, size_t(B) * limit * 8);
@@ -5544,16 +5879,33 @@ extern "C" int oc_search_indexes(oc_ctx *c, uint32_t n_indexes, const oc_index_q
             if (out_pin_scores) memcpy(out_pin_scores + it, h + o_ps + s * 4, 4);
             if (out_pin_present) out_pin_present[it] = h[o_pp + s];
         }
+    if (R) {
+        if (gs) {
+            memcpy(out_group_doc_ids, h + o_gd, R * gs * 8);
+            memcpy(out_group_scores, h + o_gs, R * gs * 4);
+            if (out_group_sort_values) memcpy(out_group_sort_values, h + o_gv, R * gs * 8);
+        }
+        memcpy(out_group_n, h + o_gn, R * 4);
+    }
+    if (n_slots) memcpy(out_facet_counts + s0, h + o_fc, size_t(n_slots) * 8);
     auto el = [&](int a, int b) { float ms = 0; cudaEventElapsedTime(&ms, c->ev[a], c->ev[b]); return ms; };
     total.h2d_ms += el(EV_START, EV_H2D);
     total.device_ms += el(EV_H2D, EV_DEV);
     total.fuse_ms += el(EV_H2D, EV_DEV);
     total.d2h_ms += el(EV_DEV, EV_D2H);
-    total.kernel_launches += 1;
+    total.kernel_launches += mg.rows ? 2 : 1;
     total.h2d_bytes += pk.total;
     total.d2h_bytes += out_bytes;
     c->timing = total;
     return OC_OK;
+}
+
+extern "C" int oc_search_indexes(oc_ctx *c, uint32_t n_indexes, const oc_index_query *ix, const oc_pins *pins,
+                                 uint64_t *out_doc_ids, float *out_scores, double *out_sort_values, uint32_t *out_n,
+                                 uint64_t *out_count, float *out_pin_scores, uint8_t *out_pin_present) {
+    return oc_search_indexes_ex(c, n_indexes, ix, nullptr, pins, nullptr, nullptr, 0, nullptr, out_doc_ids, out_scores,
+                                out_sort_values, out_n, out_count, out_pin_scores, out_pin_present, nullptr, nullptr, nullptr,
+                                nullptr, nullptr);
 }
 
 // One batch in which every query has its own groups (or none), sort, pins and, with q_filters, filter: query b gets what
@@ -5611,52 +5963,9 @@ extern "C" int oc_search_q_facets(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_
     OCTRY(groups_impl(c, emb, str, p, q_groups, pins, group_stride, true, out_doc_ids, out_scores, out_sort_values, out_n, out_count,
                       out_pin_scores, out_pin_present, out_group_doc_ids, out_group_scores, out_group_sort_values, out_group_n, &mj));
     if (sub.empty()) return OC_OK;
-    // the sub-batch of the filtered queries: their vectors and token CSR, without filters, groups, sorts or pins
-    const uint32_t S = (uint32_t)sub.size();
-    oc_search_params q = *p;
-    q.n_queries = S;
-    std::vector<float> vecs;
-    std::vector<uint32_t> q_tok{0}, tok_term{0}, t_field, t_id;
-    std::vector<float> t_weight;
-    // per-query parameters: the sub-batch's entries; a vector entry's row and a text entry's tokens are the ones read
-    std::vector<oc_query_params> sub_qp;
-    bool sub_v = p->mode != OC_MODE_FULLTEXT, sub_ft = p->mode != OC_MODE_VECTOR;
-    if (p->q_params) {
-        sub_v = sub_ft = false;
-        for (uint32_t b : sub) {
-            sub_qp.push_back(p->q_params[b]);
-            sub_v = sub_v || p->q_params[b].mode != OC_MODE_FULLTEXT;
-            sub_ft = sub_ft || p->q_params[b].mode != OC_MODE_VECTOR;
-        }
-        q.q_params = sub_qp.data();
-    }
-    auto text_of = [&](uint32_t b) { return !p->q_params || p->q_params[b].mode != OC_MODE_VECTOR; };
-    if (sub_v && emb && p->q_vecs) {
-        const size_t dim = emb->dim;
-        vecs.resize(size_t(S) * dim);
-        for (uint32_t s = 0; s < S; s++)
-            if (!p->q_params || p->q_params[sub[s]].mode != OC_MODE_FULLTEXT)
-                memcpy(vecs.data() + size_t(s) * dim, p->q_vecs + size_t(sub[s]) * dim, dim * 4);
-        q.q_vecs = vecs.data();
-    }
-    if (sub_ft && p->q_token_offsets) {
-        for (uint32_t b : sub) {
-            if (!text_of(b)) { q_tok.push_back((uint32_t)tok_term.size() - 1); continue; }
-            for (uint32_t t = p->q_token_offsets[b]; t < p->q_token_offsets[b + 1]; t++) {
-                for (uint32_t e = p->token_term_offsets[t]; e < p->token_term_offsets[t + 1]; e++) {
-                    t_field.push_back(p->term_field[e]);
-                    t_id.push_back(p->term_id[e]);
-                    t_weight.push_back(p->term_weight ? p->term_weight[e] : 1.0f);
-                }
-                tok_term.push_back((uint32_t)t_id.size());
-            }
-            q_tok.push_back((uint32_t)tok_term.size() - 1);
-        }
-        t_field.push_back(0); t_id.push_back(0); t_weight.push_back(1.0f);   // never read: non-NULL arrays for an empty CSR
-        q.q_token_offsets = q_tok.data(); q.token_term_offsets = tok_term.data();
-        q.term_field = t_field.data(); q.term_id = t_id.data(); q.term_weight = t_weight.data();
-    }
-    return facets_unfiltered(c, emb, str, &q, fj, true);
+    FacetSubBatch sb;
+    facet_sub_batch(p, emb, sub, sb);
+    return facets_unfiltered(c, emb, str, &sb.q, fj, true);
 }
 
 // ------------------------------------------------------------------------------------ geopoint where-filter leaves (geo.cuh)

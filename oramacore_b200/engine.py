@@ -1288,20 +1288,84 @@ class IndexPart:
     """One index of a search_indexes call: its TokenScoreContext (its embedding and string stores), its own query
     inputs (texts resolved with its own dictionary, q_vecs) and its index fields as TokenScoreParams fields of those
     names: device_filter / device_filters / where_programs / filtered_doc_ids + filter_nbits over its own filter fields,
-    and omc_store or omc_doc_ids / omc_mult."""
+    and omc_store or omc_doc_ids / omc_mult; store: its FacetStore, which facets across the indexes count over."""
     tsc: "TokenScoreContext"
     texts: object = None
     q_vecs: Optional[np.ndarray] = None
     fields: Optional[Mapping[str, object]] = None
+    store: Optional[FacetStore] = None
 
 
-def search_indexes_arrays(ctx: Context, parts: Sequence[IndexPart], params: "TokenScoreParams", sorts=None, promote=None):
-    """oc_search_indexes: search_on_indexes (read/search.rs:283-501) over the indexes of one collection in one call.
+def _group_value_key(v):
+    """A group value as a dict key: a bool, a string or a float compared with == (so -0.0 is +0.0), kinds kept apart."""
+    if isinstance(v, (bool, np.bool_)):
+        return ("b", bool(v))
+    if isinstance(v, str):
+        return ("s", v)
+    return ("f", float(v) + 0.0)
+
+
+def collection_group_keys(group_bys: Sequence[Optional["GroupBy"]]):
+    """The collection's groups over the indexes' GroupBy handles (None: the index adds no groups): the keys in order of
+    first appearance, index by index, each a list of property values (GroupBy.values), and per index the key of each of
+    its local groups (uint32 [n_groups], None without a handle).  Keys are compared as _group_value_key compares values."""
+    index, keys, maps = {}, [], []
+    for gb in group_bys:
+        if gb is None:
+            maps.append(None)
+            continue
+        m = np.zeros(max(gb.n_groups, 1), np.uint32)
+        for g, vals in enumerate(gb.values):
+            k = tuple(_group_value_key(v) for v in vals)
+            if k not in index:
+                index[k] = len(keys)
+                keys.append(list(vals))
+            m[g] = index[k]
+        maps.append(m)
+    return keys, maps
+
+
+def collection_facet_requests(stores: Sequence[Optional[FacetStore]], facets: Dict[str, dict]):
+    """The collection's facet slots of one reference-style `facets` map (see facet_requests) over the indexes' stores
+    (None: an index without filter fields): the slot labels [(field, label)] and per index its (requests, slots).  A slot
+    is labelled as facet_requests labels it; a string_filter field gets the union of the indexes' keys in order of first
+    appearance, index by index.  Fields that no index has raise KeyError([fields]) (the caller's FacetFieldNotFound); a
+    definition of the wrong kind for an index's field, or a date field, raises ValueError."""
+    labels, slot_of, per_index = [], {}, []
+    missing = [name for name in facets if not any(st is not None and name in st.fields for st in stores)]
+    if missing:
+        raise KeyError(missing)
+    for st in stores:
+        reqs, slots = [], []
+        if st is not None:
+            present = {k: v for k, v in facets.items() if k in st.fields}
+            r, lab = facet_requests(st, present)
+            for req, l in zip(r, lab):
+                if l not in slot_of:
+                    slot_of[l] = len(labels)
+                    labels.append(l)
+                reqs.append(req)
+                slots.append(slot_of[l])
+        per_index.append((reqs, slots))
+    # slots in field order of the map, labels in order of first appearance inside a field
+    order = sorted(range(len(labels)), key=lambda j: (list(facets).index(labels[j][0]), j))
+    renum = {old: new for new, old in enumerate(order)}
+    return [labels[j] for j in order], [(r, [renum[x] for x in sl]) for r, sl in per_index]
+
+
+def search_indexes_arrays(ctx: Context, parts: Sequence[IndexPart], params: "TokenScoreParams", sorts=None, promote=None,
+                          groups=None, facets=None, group_stride: Optional[int] = None):
+    """oc_search_indexes_ex: search_on_indexes (read/search.rs:283-501) over the indexes of one collection in one call.
     `params` holds the request (mode, limit, offset, similarity, threshold, query_params; vector_limit must be 0) and is
     shared by every index; each part adds its index's inputs.  `sorts`: None (score order), or per index None or per
     query a (SortField, order) pair or None; query b is sorted when every index gives it a field in one order.
     `promote` as in search_pinned_arrays.  Returns (docs [B,limit], scores, sort values [B,limit], n [B], count [B],
-    pin scores [items], pin present [items]), byte for byte the per-index searches merged by the host merges."""
+    pin scores [items], pin present [items]), byte for byte the per-index searches merged by the host merges.
+    `groups` (per query None or (per index a GroupBy or None, max_results)) and `facets` (per query None or a
+    reference-style map, counted over each part's `store`) add, after those seven, (group docs [rows,stride], group
+    scores, group sort values [rows,stride], group n [rows], rows [B+1], group keys per query (collection_group_keys),
+    facet counts [slots], q_facet_offsets [B+1], slot labels per query (collection_facet_requests)): query b's groups
+    are rows [rows[b], rows[b+1]), its counts counts[off[b]:off[b+1]]."""
     import dataclasses
     if not parts:
         raise ValueError("search_indexes needs at least one index")
@@ -1311,7 +1375,8 @@ def search_indexes_arrays(ctx: Context, parts: Sequence[IndexPart], params: "Tok
         keep += [sp, k]
         built.append((part.tsc, sp))
     B = built[0][1].n_queries
-    ixs = (_lib.IndexQuery * len(parts))()
+    ni = len(parts)
+    ixs = (_lib.IndexQuery * ni)()
     for i, (tsc, sp) in enumerate(built):
         srt = None
         if sorts is not None and sorts[i] is not None:
@@ -1325,9 +1390,74 @@ def search_indexes_arrays(ctx: Context, parts: Sequence[IndexPart], params: "Tok
     docs, scores, sv = np.zeros((B, L), np.uint64), np.zeros((B, L), np.float32), np.zeros((B, L), np.float64)
     n, cnt = np.zeros(B, np.uint32), np.zeros(B, np.uint64)
     ps, pp = np.zeros(max(n_items, 1), np.float32), np.zeros(max(n_items, 1), np.uint8)
-    check(lib().oc_search_indexes(ctx._h, len(parts), ixs, None if pins is None else C.byref(pins), _p(docs), _p(scores),
-                                  _p(sv), _p(n), _p(cnt), _p(ps), _p(pp)))
-    return docs, scores, sv, n, cnt, ps[:n_items], pp[:n_items]
+    if groups is None and facets is None:
+        check(lib().oc_search_indexes(ctx._h, ni, ixs, None if pins is None else C.byref(pins), _p(docs), _p(scores),
+                                      _p(sv), _p(n), _p(cnt), _p(ps), _p(pp)))
+        return docs, scores, sv, n, cnt, ps[:n_items], pp[:n_items]
+    ex = (_lib.IndexExtras * ni)()
+    # groups: one key union per distinct combination of handles, shared by the queries that ask for it
+    groups = groups if groups is not None else [None] * B
+    if len(groups) != B:
+        raise ValueError(f"groups has {len(groups)} entries for {B} queries")
+    n_keys, max_res, q_keys, combos = np.zeros(B, np.uint32), np.zeros(B, np.uint32), [], {}
+    q_gb = [(C.c_void_p * max(B, 1))() for _ in range(ni)]
+    q_km = [(C.c_void_p * max(B, 1))() for _ in range(ni)]
+    for b, g in enumerate(groups):
+        if g is None:
+            q_keys.append(None)
+            continue
+        gbs, m = list(g[0]), int(g[1])
+        if len(gbs) != ni:
+            raise ValueError(f"groups[{b}] has {len(gbs)} handles for {ni} indexes")
+        ck = tuple(id(x) for x in gbs)
+        if ck not in combos:
+            combos[ck] = collection_group_keys(gbs)
+        keys, maps = combos[ck]
+        n_keys[b], max_res[b] = len(keys), m
+        q_keys.append(keys)
+        for i, gb in enumerate(gbs):
+            if gb is not None:
+                q_gb[i][b], q_km[i][b] = gb._h, maps[i].ctypes.data
+    keep += [combos, q_gb, q_km]
+    rows = np.zeros(B + 1, np.int64)
+    rows[1:] = np.cumsum(n_keys)
+    if group_stride is None:
+        k = [0] * B if promote is None else [len(x) for x in promote]
+        group_stride = max([0] + [_group_need((True, max_res[b]), k[b]) for b in range(B) if n_keys[b]])
+    R, S = int(rows[-1]), int(group_stride)
+    gd, gs, gsv = np.zeros((R, S), np.uint64), np.zeros((R, S), np.float32), np.zeros((R, S), np.float64)
+    gn = np.zeros(R, np.uint32)
+    # facets: per query its collection slots, per index its requests and their slots
+    facets = facets if facets is not None else [None] * B
+    if len(facets) != B:
+        raise ValueError(f"facets has {len(facets)} entries for {B} queries")
+    stores = [getattr(p, "store", None) for p in parts]
+    foff, labels, planned = np.zeros(B + 1, np.uint32), [], {}
+    f_reqs, f_slots = [[] for _ in range(ni)], [[] for _ in range(ni)]
+    for b, f in enumerate(facets):
+        if f and id(f) not in planned:   # once per distinct map of the batch
+            planned[id(f)] = collection_facet_requests(stores, f)
+        lab, per = planned[id(f)] if f else ([], [([], [])] * ni)
+        for i, (r, sl) in enumerate(per):
+            f_reqs[i] += r
+            f_slots[i] += [int(foff[b]) + x for x in sl]
+        labels.append(lab)
+        foff[b + 1] = foff[b] + len(lab)
+    fc = np.zeros(max(int(foff[-1]), 1), np.uint64)
+    for i in range(ni):
+        ex[i].q_groups = C.cast(q_gb[i], C.c_void_p) if any(g is not None and g[0][i] is not None for g in groups) else None
+        ex[i].q_group_keys = C.cast(q_km[i], C.c_void_p)
+        if f_reqs[i]:
+            arr = (_lib.FacetReq * len(f_reqs[i]))(*[_lib.FacetReq(*r) for r in f_reqs[i]])
+            sl = np.asarray(f_slots[i], np.uint32)
+            keep += [arr, sl]
+            ex[i].facets, ex[i].n_facet_reqs = stores[i]._h, len(f_reqs[i])
+            ex[i].facet_reqs, ex[i].facet_slots = C.cast(arr, C.c_void_p), sl.ctypes.data
+    check(lib().oc_search_indexes_ex(ctx._h, ni, ixs, ex, None if pins is None else C.byref(pins), _p(n_keys), _p(max_res), S,
+                                     _p(foff), _p(docs), _p(scores), _p(sv), _p(n), _p(cnt), _p(ps), _p(pp), _p(gd), _p(gs),
+                                     _p(gsv), _p(gn), _p(fc)))
+    return (docs, scores, sv, n, cnt, ps[:n_items], pp[:n_items], gd, gs, gsv, gn, rows, q_keys, fc[:int(foff[-1])], foff,
+            labels)
 
 
 def search_indexes(ctx: Context, parts: Sequence[IndexPart], params: "TokenScoreParams", sorts=None,

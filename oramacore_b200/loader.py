@@ -38,9 +38,10 @@ from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from .engine import (Context, DeviceFilter, EmbeddingFieldStorage, FacetStore, GeoPointField, IndexPart, OmcStore, SortField,
-                     StringFieldStorage, TermDictionary, TokenScoreContext, TokenScoreParams, resolve_sort_by, search_indexes_arrays)
-from .types import SearchHits
+from .engine import (Context, DeviceFilter, EmbeddingFieldStorage, FacetStore, GeoPointField, GroupBy, IndexPart, OmcStore, SortField,
+                     StringFieldStorage, TermDictionary, TokenScoreContext, TokenScoreParams, _facet_result, resolve_sort_by,
+                     search_indexes_arrays)
+from .types import FacetFieldNotFound, SearchHits
 from .types import SortBy
 from .where import WhereFilter, WhereProgram, check_where_keys, compile_where, filter_from_program, parse_where
 
@@ -93,8 +94,10 @@ class IndexLoader:
             # a string_filter field joins the store with its first key (a field needs one variant)
         self.geo: Dict[str, GeoPointField] = {f: GeoPointField(ctx, self.nbits, [], [], []) for f in self._geo}
         self._live: Optional[DeviceFilter] = None              # NOT(uncommitted deletes) of where_program, built once
-        self._retired: List[DeviceFilter] = []                 # earlier ones, which programs may still point at
+        self._retired: List[object] = []                       # earlier ones, which programs may still point at, and
+                                                               # this version's group handles
         self._sorts: Dict[str, SortField] = {}                 # sort fields of the published version, built when asked
+        self._groups: Dict[Tuple[str, ...], GroupBy] = {}      # group handles of the published version, built when asked
         self.omc_store = OmcStore(ctx)                         # the OMC map; sets queue in _omc_log until omc() / commit()
         self._omc_log: List[tuple] = []
 
@@ -265,6 +268,7 @@ class IndexLoader:
         for f in self._retired:   # programs built before now carry the earlier nbits
             f.close()
         self._retired = []
+        self._groups = {}         # (their handles were retired with them)
         for f in self._sorts.values():   # the sorts of the previous version
             f.close()
         self._sorts = {}
@@ -320,6 +324,21 @@ class IndexLoader:
             out[f] = self._sorts[f]
         return out
 
+    def group_by(self, properties: Sequence[str]) -> Optional[GroupBy]:
+        """The GroupBy of `properties` over the version the last commit() published (built the first time it is asked
+        for after a commit, closed by the next), or None when the index lacks one of them (it adds no groups,
+        group.rs:104-168).  A date or geopoint property raises ValueError."""
+        for p in properties:
+            if p in self._date or p in self._geo:
+                raise ValueError(f"{p!r} is a {'date' if p in self._date else 'geopoint'} field: it cannot group")
+        key = tuple(properties)
+        if self.facets is None or not all(p in self.facets.fields for p in key):
+            return None
+        if key not in self._groups:   # closed with the retired handles at the next commit
+            self._groups[key] = GroupBy(self.facets, list(key))
+            self._retired.append(self._groups[key])
+        return self._groups[key]
+
     def sort_by(self, sort_by: SortBy):
         """resolve_sort_by over sort_fields(): the (SortField, order) pair the sorted searches take.  Raises
         SortFieldNotFound / InvalidSortField as the reference does (read/index/sort.rs:186-265)."""
@@ -353,6 +372,21 @@ def search_collection(loaders: Sequence[IndexLoader], texts: Optional[Sequence[s
     indexes have filters out everything on the others), sorts by its own `sort_by` field and scores with its own OMC
     map.  `params` holds the request (mode, limit_hint, offset, similarity, threshold, query_params) and is shared by
     every index.  Returns (one SearchHits per query, the sort values [B, limit])."""
+    res = search_collection_ex(loaders, texts, params, where, sort_by, q_vecs, promote, **resolve_kw)
+    return [r["hits"] for r in res], np.stack([r["sort_values"] for r in res]) if res else np.zeros((0, 0))
+
+
+def search_collection_ex(loaders: Sequence[IndexLoader], texts: Optional[Sequence[str]], params: TokenScoreParams, where=None,
+                         sort_by: Optional[SortBy] = None, q_vecs: Optional[np.ndarray] = None, promote=None, facets=None,
+                         group_by=None, **resolve_kw) -> List[dict]:
+    """search_collection with the reference's `facets` and `group_by` (GroupByConfig: {"properties": [...],
+    "max_results": n}), one request for every query, in one oc_search_indexes_ex call.  Per query a dict: "hits"
+    (SearchHits), "sort_values" [limit], "facets" ({field: {"count", "values"}}, None without facets) and "groups" (a
+    list of {"values", "result": [(doc, score), ...]} in key order, None without group_by).
+      - facets: the fields that no index has raise FacetFieldNotFound (search.rs:452-464); a definition of the wrong kind
+        for an index's field, or a date field, raises ValueError (facet.rs:166-178).
+      - group_by: an index that lacks one of the properties adds no groups (group.rs:104-168); a date or geopoint
+        property raises ValueError.  Each index's GroupBy is built once per commit (IndexLoader.group_by)."""
     B = len(texts) if texts is not None else int(np.asarray(q_vecs).shape[0])
     w = None if where is None else (where if isinstance(where, WhereFilter) else parse_where(where))
     if w is not None:
@@ -362,8 +396,30 @@ def search_collection(loaders: Sequence[IndexLoader], texts: Optional[Sequence[s
         fields = {"omc_store": l.omc()}
         if w is not None:
             fields["where_programs"] = [l._compile_where(w)] * B
-        parts.append(IndexPart(l.context(), None if texts is None else l.resolve(texts, **resolve_kw), q_vecs, fields))
+        parts.append(IndexPart(l.context(), None if texts is None else l.resolve(texts, **resolve_kw), q_vecs, fields, l.facets))
         if sorts is not None:
             sorts.append([l.sort_by(sort_by)] * B)
-    docs, scores, sv, n, cnt, _, _ = search_indexes_arrays(loaders[0].ctx, parts, params, sorts, promote)
-    return [SearchHits(docs[i, :n[i]].copy(), scores[i, :n[i]].copy(), int(cnt[i])) for i in range(B)], sv
+    groups = None
+    if group_by is not None:
+        props = list(group_by["properties"])
+        groups = [([l.group_by(props) for l in loaders], int(group_by.get("max_results", 1)))] * B
+    if facets is not None:
+        missing = [f for f in facets if not any(l.facets is not None and f in l.facets.fields for l in loaders)]
+        if missing:
+            raise FacetFieldNotFound(missing)
+    got = search_indexes_arrays(loaders[0].ctx, parts, params, sorts, promote,
+                                groups=groups, facets=None if facets is None else [facets] * B)
+    docs, scores, sv, n, cnt = got[:5]
+    out = []
+    for b in range(B):
+        r = {"hits": SearchHits(docs[b, :n[b]].copy(), scores[b, :n[b]].copy(), int(cnt[b])), "sort_values": sv[b],
+             "facets": None, "groups": None}
+        if len(got) > 7:
+            gd, gs, _, gn, rows, keys, fc, foff, labels = got[7:]
+            if groups is not None:
+                r["groups"] = [{"values": list(keys[b][k]), "result": [(int(gd[row, j]), float(gs[row, j])) for j in range(int(gn[row]))]}
+                               for k, row in enumerate(range(int(rows[b]), int(rows[b + 1])))]
+            if facets is not None:
+                r["facets"] = _facet_result(fc[foff[b]:foff[b + 1]], labels[b])
+        out.append(r)
+    return out

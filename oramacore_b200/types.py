@@ -122,6 +122,14 @@ class FilterFieldNotFound(KeyError):
         self.name = name
 
 
+class FacetFieldNotFound(KeyError):
+    """ReadError::FacetFieldNotFound: the facet fields that are not a filter field of any index (search.rs:452-464)."""
+
+    def __init__(self, names):
+        super().__init__(list(names))
+        self.names = list(names)
+
+
 class InvalidSortField(ValueError):
     """ReadError::InvalidSortField(name, kind): the sortBy property is a field that cannot be sorted by (string,
     string_filter, geopoint); `kind` is the reference's FieldType name, e.g. "GeoPoint"."""

@@ -210,6 +210,18 @@ pub struct OcIndexQuery {
     pub q_sorts: *const OcSort,
 }
 
+/// oc_index_extras: one index's groups (local group -> collection key per query) and facet requests (each added to a
+/// collection slot) in an oc_search_indexes_ex call
+#[repr(C)]
+pub struct OcIndexExtras {
+    pub q_groups: *const *const OcGroupBy,
+    pub q_group_keys: *const *const u32,
+    pub facets: *mut OcFacets,
+    pub n_facet_reqs: u32,
+    pub facet_reqs: *const OcFacetReq,
+    pub facet_slots: *const u32,
+}
+
 /// one query's groupBy in oc_search_q_groups: its handle (NULL: no groups), max_results and sort (field NULL: score order)
 #[repr(C)]
 pub struct OcGroupReq {
@@ -430,6 +442,13 @@ extern "C" {
     pub fn oc_search_indexes(ctx: *mut OcCtx, n_indexes: u32, ix: *const OcIndexQuery, pins: *const OcPins,
                              out_doc_ids: *mut u64, out_scores: *mut f32, out_sort_values: *mut f64, out_n: *mut u32,
                              out_count: *mut u64, out_pin_scores: *mut f32, out_pin_present: *mut u8) -> c_int;
+    /// oc_search_indexes with groups and facets across the indexes; ex NULL or n_indexes entries
+    pub fn oc_search_indexes_ex(ctx: *mut OcCtx, n_indexes: u32, ix: *const OcIndexQuery, ex: *const OcIndexExtras,
+                                pins: *const OcPins, q_n_keys: *const u32, q_max_results: *const u32, group_stride: u32,
+                                q_facet_offsets: *const u32, out_doc_ids: *mut u64, out_scores: *mut f32,
+                                out_sort_values: *mut f64, out_n: *mut u32, out_count: *mut u64, out_pin_scores: *mut f32,
+                                out_pin_present: *mut u8, out_group_doc_ids: *mut u64, out_group_scores: *mut f32,
+                                out_group_sort_values: *mut f64, out_group_n: *mut u32, out_facet_counts: *mut u64) -> c_int;
     // term dictionary + batch query resolution (tokenize_and_stem + FST expansion), host only
     pub fn oc_dict_create(n_fields: u32, out: *mut *mut OcDict) -> c_int;
     pub fn oc_dict_destroy(d: *mut OcDict);
