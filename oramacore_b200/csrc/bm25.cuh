@@ -1185,6 +1185,10 @@ __device__ __forceinline__ void t3_scan(const float4 *d0, const float4 *d1, cons
     load(ca, 0);
 #pragma unroll 1
     for (uint32_t h = 0; h < NB; h += 2) {
+        // the candidate buffer overflowed: the item is redone with a tighter threshold, which recomputes the count and
+        // the extrema, and takes its threshold from keys already in the buffer — the rest of this pass changes nothing
+        // (a cold threshold overflows after a few hundred rows of an 8192-row scan)
+        if (h && *reinterpret_cast<volatile const uint32_t *>(s_cnt) > cap) break;
         load(cb, h + 1);
         fold(ca, h);
         if (h + 2 < NB) load(ca, h + 2);
@@ -1463,6 +1467,28 @@ __device__ __noinline__ unsigned long long warp_keep_top(uint64_t *buf, const ui
     __syncwarp();
     return last;
 }
+// Phase profile of K3d (OC_BM25_PHASE_PROFILE, defined only by `make phaseprof`, which builds a separate library for
+// tools/profile_k3d.py): lane 0 of each warp appends one BwProfItem per item and one BwProfWarp per warp.  The spans
+// are clock64 deltas (per SM clock), the warp times %globaltimer (ns, comparable across SMs).
+enum { BWP_DESC, BWP_MARK, BWP_DENSE, BWP_FOLD, BWP_CLEAR, BWP_KEEP, BWP_EMIT, BWP_N };
+struct BwProfItem {
+    uint32_t item, cls;      // cls: nd | n_list << 4 | skip << 8 | passes << 12 (1 + threshold redos)
+    uint32_t postings, cand; // list postings in the tile (all list tokens), candidates pushed (last pass)
+    uint32_t span[BWP_N];    // cycles per phase
+    uint32_t smid;
+};
+struct BwProfWarp { unsigned long long t0, t1, c0, c1; uint32_t smid, items, pad[2]; };
+struct BwProf { BwProfItem *items; BwProfWarp *warps; unsigned int *n_items, *n_warps; uint32_t cap_items, cap_warps; };
+#ifdef OC_BM25_PHASE_PROFILE
+__device__ BwProf g_bw_prof;
+__device__ __forceinline__ unsigned long long bw_gtime() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
+__device__ __forceinline__ uint32_t bw_smid() { uint32_t s; asm volatile("mov.u32 %0, %%smid;" : "=r"(s)); return s; }
+#define BW_PROF(...) __VA_ARGS__
+#define BW_LAP(ph) do { const long long t_ = clock64(); pspan[ph] += uint32_t(t_ - pclk); pclk = t_; } while (0)
+#else
+#define BW_PROF(...)
+#define BW_LAP(ph) do { } while (0)
+#endif
 __global__ void __launch_bounds__(BW_WARPS * 32, 5) bm25_warp_kernel(const Bm25Params p, const ItemTok *flat, unsigned int *work_counter) {
     constexpr uint32_t W = BM25_TILE / 32;
     extern __shared__ __align__(16) uint8_t smem[];
@@ -1484,8 +1510,10 @@ __global__ void __launch_bounds__(BW_WARPS * 32, 5) bm25_warp_kernel(const Bm25P
     if (item < n_items && lane < BM25_FLAT_TOK) cur = flat[size_t(item) * BM25_FLAT_TOK + lane];
     unsigned long long tau_next = 0ull;
     if (item < n_items) tau_next = __ldcg(p.tau + item % p.n_queries);
+    BW_PROF(const unsigned long long prof_t0 = bw_gtime(), prof_c0 = clock64(); uint32_t prof_items = 0;)
 
     while (item < n_items) {
+        BW_PROF(uint32_t pspan[BWP_N] = {}; long long pclk = clock64(); uint32_t prof_passes = 0, prof_skip = 0, prof_post = 0;)
         uint32_t next2 = 0;
         if (lane == 0) next2 = atomicAdd(work_counter, 1u);   // consumed at the end of this item
         const uint32_t tile = item / p.n_queries, q = item % p.n_queries;
@@ -1511,15 +1539,17 @@ __global__ void __launch_bounds__(BW_WARPS * 32, 5) bm25_warp_kernel(const Bm25P
                 const float4 *dp = reinterpret_cast<const float4 *>(tab[j].ptr);
                 if (nd == 0) d0 = dp; else if (nd == 1) d1 = dp; else if (nd == 2) d2 = dp; else d3 = dp;
                 nd++;
-            } else n_list++;
+            } else { n_list++; BW_PROF(prof_post += n;) }
         }
         const bool any_list = n_list != 0;
         const bool use_bm = n_list > 1 || okbits != nullptr;
         uint32_t matched;
         float lmax, lmin;
+        BW_LAP(BWP_DESC);
         for (;;) {   // (repeats only when a cold threshold overflowed the candidate buffer)
             const float tau_f = tau ? key_score(tau) : -INFINITY;
             matched = 0; lmax = 0.f; lmin = 0.f;
+            BW_PROF(prof_passes++;)
             if (any_list && (nd || use_bm)) {   // mark the rows of the list tokens
 #pragma unroll 1
                 for (uint32_t j = 0; j < BM25_FLAT_TOK; j++) {
@@ -1536,9 +1566,11 @@ __global__ void __launch_bounds__(BW_WARPS * 32, 5) bm25_warp_kernel(const Bm25P
                 }
                 __syncwarp();
             }
+            BW_LAP(BWP_MARK);
             // rows outside every list: dense tokens only, folded in registers (or only counted: see t3_count)
             const bool skip = nd && pos && t3_dense_ub(tab) < tau_f;
             if (nd && lane == 0) { ws.dense_items++; ws.dense_skipped += skip; }
+            BW_PROF(prof_skip = skip;)
             if (skip) matched += t3_count<32>(tab, touched, any_list, p.n_tiles, tile, lane);
             else switch (nd) {
                 case 0: break;
@@ -1547,6 +1579,7 @@ __global__ void __launch_bounds__(BW_WARPS * 32, 5) bm25_warp_kernel(const Bm25P
                 case 3: t3_scan<3, 32>(d0, d1, d2, d3, touched, any_list, pos, row0, lane, tau, tau_f, &ws.cnt, ws.tbuf, BW_CAP, matched, lmax, lmin); break;
                 default: t3_scan<4, 32>(d0, d1, d2, d3, touched, any_list, pos, row0, lane, tau, tau_f, &ws.cnt, ws.tbuf, BW_CAP, matched, lmax, lmin); break;
             }
+            BW_LAP(BWP_DENSE);
             if (any_list) {   // rows of the list tokens: the first list token holding the row folds it
 #pragma unroll 1
                 for (uint32_t j = 0; j < BM25_FLAT_TOK; j++) {
@@ -1573,16 +1606,19 @@ __global__ void __launch_bounds__(BW_WARPS * 32, 5) bm25_warp_kernel(const Bm25P
                 }
             }
             __syncwarp();                                      // candidate pushes and bitmap reads of all lanes are done
+            BW_LAP(BWP_FOLD);
             if (any_list) {
                 if (nd) for (uint32_t i = lane; i < W; i += 32) touched[i] = 0u;
                 if (use_bm) for (uint32_t i = lane; i < BM25_FLAT_TOK * W; i += 32) bm[i] = 0u;
             }
+            BW_LAP(BWP_CLEAR);
             if (ws.cnt <= BW_CAP) break;
             // overflow: the n_keep-th best of the first BW_CAP arrivals bounds the tile's n_keep-th best from below
             const unsigned long long kth = warp_keep_top(ws.tbuf, BW_CAP, p.n_keep, lane) - 1ull;   // "> kth" keeps that row itself
             tau = kth > tau ? kth : tau;
             if (lane == 0) ws.cnt = 0u;
             __syncwarp();
+            BW_LAP(BWP_KEEP);
         }
         matched = __reduce_add_sync(0xffffffffu, matched);
         for (int o = 16; o > 0; o >>= 1) {
@@ -1592,11 +1628,14 @@ __global__ void __launch_bounds__(BW_WARPS * 32, 5) bm25_warp_kernel(const Bm25P
         // ---- emit: best <= n_keep of the buffer
         const size_t slot_base = (size_t(q) * p.n_tiles + tile);
         uint32_t c = ws.cnt;
+        BW_PROF(const uint32_t prof_cand = c;)
+        BW_LAP(BWP_EMIT);
         if (c >= p.n_keep && c > 0) {
             const unsigned long long kth = warp_keep_top(ws.tbuf, c, p.n_keep, lane);
             c = p.n_keep;
             if (lane == 0) atomicMax(p.tau + q, kth);
         }
+        BW_LAP(BWP_KEEP);
         for (uint32_t i = lane; i < c; i += 32) {
             const uint64_t key = ws.tbuf[i];
             p.cand_key[slot_base * p.n_keep + i] = key;
@@ -1617,12 +1656,32 @@ __global__ void __launch_bounds__(BW_WARPS * 32, 5) bm25_warp_kernel(const Bm25P
             const uint32_t bytes = (nx.flags & TD_DENSE) ? 1024u : min(nx.n * 8u, 1024u);
             for (uint32_t o = 0; o < bytes; o += 128u) asm volatile("prefetch.global.L1 [%0];" ::"l"(pf + o));
         }
+        BW_LAP(BWP_EMIT);
+        BW_PROF(if (lane == 0 && g_bw_prof.n_items) {   // (no buffers set: nothing recorded)
+            const BwProf &g = g_bw_prof;
+            const uint32_t s = atomicAdd(g.n_items, 1u);
+            if (s < g.cap_items) {
+                BwProfItem &r = g.items[s];
+                r.item = item; r.cls = nd | n_list << 4 | prof_skip << 8 | prof_passes << 12;
+                r.postings = prof_post; r.cand = prof_cand; r.smid = bw_smid();
+                for (int ph = 0; ph < BWP_N; ph++) r.span[ph] = pspan[ph];
+            }
+            prof_items++;
+        })
         cur = nx;
         item = next;
         next = __shfl_sync(0xffffffffu, next2, 0);
         __syncwarp();
     }
     if (lane == 0 && p.dense_stat && ws.dense_items) { atomicAdd(p.dense_stat, ws.dense_items); atomicAdd(p.dense_stat + 1, ws.dense_skipped); }
+    BW_PROF(if (lane == 0 && g_bw_prof.n_warps) {
+        const BwProf &g = g_bw_prof;
+        const uint32_t s = atomicAdd(g.n_warps, 1u);
+        if (s < g.cap_warps) {
+            BwProfWarp &r = g.warps[s];
+            r.t0 = prof_t0; r.t1 = bw_gtime(); r.c0 = prof_c0; r.c1 = clock64(); r.smid = bw_smid(); r.items = prof_items;
+        }
+    })
 }
 
 // ---------------------------------------------------------------------------------------

@@ -178,7 +178,8 @@ struct oc_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
     cudaStream_t side = nullptr;      // descriptor upload + BM25 plan/precompute while the main stream sweeps the matrix
-    cudaEvent_t ev_side = nullptr;
+    cudaEvent_t ev_side = nullptr;    // the side stream's fulltext stage is complete
+    cudaEvent_t ev_side_in = nullptr; // the side stream has put up what the hybrid point lookups read (see bm25_stage)
     bool sweep_timed = false;         // EV_SWEEP0/1 recorded in this call (tensor-core path)
     bool rerun_timed = false;         // EV_RR0/1 recorded: flagged queries were re-run through the exact sweep
     bool side_dirty = false;          // work was queued on the side stream and not yet joined (an error path returned early)
@@ -245,6 +246,7 @@ struct oc_ctx {
         if (stream) cudaStreamDestroy(stream);
         if (side) cudaStreamDestroy(side);
         if (ev_side) cudaEventDestroy(ev_side);
+        if (ev_side_in) cudaEventDestroy(ev_side_in);
     }
 };
 
@@ -272,10 +274,23 @@ extern "C" int oc_init(int device_id, oc_ctx **out) {
     CU(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
     CU(cudaStreamCreateWithFlags(&c->side, cudaStreamNonBlocking));
     CU(cudaEventCreateWithFlags(&c->ev_side, cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&c->ev_side_in, cudaEventDisableTiming));
     for (int i = 0; i < EV_N; i++) CU(cudaEventCreate(&c->ev[i]));
     *out = c;
     return OC_OK;
 }
+
+#ifdef OC_BM25_PHASE_PROFILE
+// (phase-profile library only: where bm25_warp_kernel appends its records, device pointers; counters NULL: none)
+extern "C" int oc_bm25_phase_profile(void *items, uint32_t cap_items, void *warps, uint32_t cap_warps, void *counters) {
+    BwProf g{};
+    g.items = static_cast<BwProfItem *>(items); g.warps = static_cast<BwProfWarp *>(warps);
+    g.n_items = static_cast<unsigned int *>(counters); g.n_warps = g.n_items + 1;
+    g.cap_items = cap_items; g.cap_warps = cap_warps;
+    CU(cudaMemcpyToSymbol(g_bw_prof, &g, sizeof(g)));
+    return OC_OK;
+}
+#endif
 
 extern "C" void oc_shutdown(oc_ctx *c) {
     if (!c) return;
@@ -3607,8 +3622,8 @@ static int main_upload(SearchCall &k) {
 }
 
 // The fulltext stage.  It does not depend on the vector stage (the vector hits' fulltext scores are point lookups
-// afterwards): in hybrid mode it runs on the side stream, concurrently with the matrix sweep, and is joined before the
-// lookups and the fusion.  It runs ONCE per call; device_tail (lookups + fusion) is re-runnable.
+// afterwards): in hybrid mode it runs on the side stream, concurrently with the matrix sweep; the lookups wait only for
+// its inputs, and the fusion joins it.  It runs ONCE per call; device_tail (lookups + fusion) is re-runnable.
 static int bm25_stage(SearchCall &k) {
     oc_ctx *c = k.c; const oc_search_params *p = k.p;
     const uint32_t B = k.B, n_tiles = k.n_tiles, n_keep = k.n_keep; const StrSnap *S = k.S;
@@ -3641,6 +3656,9 @@ static int bm25_stage(SearchCall &k) {
         CU(cudaGetLastError());
         for (DenseEntry *e : k.dense_new) e->ready = true;   // later calls may read them (after this stream's work)
     }
+    // the hybrid point lookups read the descriptors, the row bitmap and the dense / precomputed contributions, all on
+    // the device from here: device_tail starts them under the tile scorer instead of behind it
+    if (k.side) CU(cudaEventRecord(c->ev_side_in, c->side));
     const size_t n_td = k.terms.size();
     OCTRY(c->seg.ensure((n_td * (size_t(n_tiles) + 1) + 1) * 4));
     if (n_td) {
@@ -3719,11 +3737,7 @@ static int bm25_stage(SearchCall &k) {
     if (n_tiles) OCTRY(launch_tile(c, bp, n_tiles * B, k.any_multi, k.thr, k.omc_tile, ps, k.max_tokens, k.tile_counter, k.need_df));
     CU(cudaEventRecord(c->ev[EV_BM1], ps));
     c->timing.bm25_postings = k.postings_walked;
-    if (k.side) {   // join: the lookups and the fusion need the vector hits (main stream) and the tiles (side stream)
-        CU(cudaEventRecord(c->ev_side, c->side));
-        CU(cudaStreamWaitEvent(c->stream, c->ev_side, 0));
-        c->side_dirty = false;
-    }
+    if (k.side) CU(cudaEventRecord(c->ev_side, c->side));   // (joined in device_tail, after the point lookups)
     return OC_OK;
 }
 
@@ -3882,12 +3896,19 @@ static int device_tail(SearchCall &k) {
         OCTRY(c->v_ft.ensure(size_t(B) * vlimit * 4));
         OCTRY(c->v_present.ensure(size_t(B) * vlimit));
         if (vlimit) {
+            // side stream: the lookups' inputs are up (ev_side_in), the tile scorer may still run; they do not read its
+            // outputs, so they run under it rather than after the join below
+            if (k.side) CU(cudaStreamWaitEvent(c->stream, c->ev_side_in, 0));
             map_docs_to_rows_kernel<<<(B * vlimit + 255) / 256, 256, 0, c->stream>>>(
                 c->v_doc.as<uint64_t>(), c->v_cnt.as<uint32_t>(), vlimit, B, S->row_doc, S->n_rows, c->v_srow.as<uint32_t>());
             launched(c);
             point_lookup(k, c->v_srow.as<uint32_t>(), vlimit, c->v_ft.as<float>(), c->v_present.as<uint8_t>(), uint64_t(B) * vlimit);
             CU(cudaGetLastError());
         }
+    }
+    if (k.side) {   // join: the fusion needs the tiles (side stream); a re-run waits again on the same, complete, record
+        CU(cudaStreamWaitEvent(c->stream, c->ev_side, 0));
+        c->side_dirty = false;
     }
     FuseParams &fp = k.fp;
     fp = FuseParams{};
