@@ -4802,6 +4802,11 @@ static int run_facets(oc_ctx *c, const FacetJob &fj, const FacetPlan &pl, uint32
 static void drop_filters(oc_search_params &q) {
     q.filter_bits = nullptr; q.filter_nbits = 0; q.filter = nullptr; q.q_filters = nullptr; q.q_where = nullptr;
 }
+// Query b of p has a filter that drop_filters removes: its facets count on the unfiltered pass.
+static bool facet_filtered(const oc_search_params *p, uint32_t b) {
+    return p->filter || p->filter_bits || (p->q_filters && p->q_filters[b]) ||
+           (p->q_where && p->q_where->q_node_offsets && p->q_where->q_node_offsets[b + 1] > p->q_where->q_node_offsets[b]);
+}
 static int facets_unfiltered(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_params *p, FacetJob &fj, bool q_params_ok) {
     oc_search_params q = *p;
     drop_filters(q);
@@ -5043,6 +5048,46 @@ static int pins_check_flat(const oc_search_params *p, const PinJob &pj) {
     return OC_OK;
 }
 
+// The group list depth of query b at max_results m: 2 x m for an active query (pins apply and it has items, spliced into
+// its groups; sort.rs:137-142), else m.  group_stride must also hold an active query's items.
+static int group_depth(uint32_t b, uint32_t m, const PinJob &pj, uint32_t group_stride, uint32_t &depth) {
+    if (m > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "query %u: max_results %u > %u", b, m, OC_MAX_TOPK);
+    const bool active = pj.splice && pj.cnt[b] > 0;
+    if (active && 2 * m > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "query %u: pins: 2 x max_results %u > %u", b, 2 * m, OC_MAX_TOPK);
+    const uint64_t need = active ? 2ull * m + pj.cnt[b] : m;
+    if (group_stride < need) return fail(OC_ERR_INVALID, "query %u: group_stride %u < %llu", b, group_stride, (unsigned long long)need);
+    depth = active ? 2 * m : m;
+    return OC_OK;
+}
+
+// One index's GroupJob for a batch: query b groups by q[b] (groups NULL: none) with pj's items.  skip_empty
+// (oc_search_indexes_ex): a handle without groups is left out after its ctx check; its query's depth is checked on the
+// collection's keys, which it may not have.
+static int group_job_plan(oc_ctx *c, uint32_t B, const oc_group_req *q, const PinJob &pj, uint32_t group_stride, bool skip_empty,
+                          GroupJob &gj) {
+    gj.q_h.assign(B, GROUP_NONE);
+    gj.q_m.assign(B, 0);
+    gj.q_row.assign(B, 0);
+    uint64_t rows = 0;
+    for (uint32_t b = 0; b < B; b++) {
+        const oc_group_by *g = q[b].groups;
+        if (!g) continue;
+        if (g->ctx != c) return fail(OC_ERR_INVALID, "group_by of query %u belongs to another ctx", b);
+        if (skip_empty && g->n_groups == 0) continue;
+        uint32_t depth;
+        OCTRY(group_depth(b, q[b].max_results, pj, group_stride, depth));
+        uint32_t h = 0;
+        while (h < gj.h.size() && gj.h[h] != g) h++;
+        if (h == gj.h.size()) gj.h.push_back(const_cast<oc_group_by *>(g));   // only its per-call row map is refreshed, under the ctx lock
+        gj.q_h[b] = h; gj.q_m[b] = q[b].max_results; gj.q_row[b] = (uint32_t)rows;   // refused below past 2^31 rows
+        rows += g->n_groups;
+    }
+    // the work list is a 1-D grid of (query, group) items
+    if (rows > 0x7fffffffull) return fail(OC_ERR_UNSUPPORTED, "groups: %llu (query, group) rows >= 2^31", (unsigned long long)rows);
+    gj.rows = (uint32_t)rows;
+    return OC_OK;
+}
+
 // The one path of the grouped calls: query b takes q[b] (groups NULL: no groups) with its items and, per_query
 // (oc_search_q_groups), its q_filters entry; the flat hits follow oc_search_q_sorted.  The wrappers below pass one
 // request for every query.  Nothing is written on failure.
@@ -5060,39 +5105,18 @@ static int groups_impl(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_search_para
     OCTRY(pins_check_flat(p, pj));
     pj.out_scores = out_pin_scores; pj.out_present = out_pin_present;
     GroupJob gj;
-    gj.q_h.assign(B, GROUP_NONE);
-    gj.q_m.assign(B, 0);
-    gj.q_row.assign(B, 0);
-    uint64_t rows = 0;
+    OCTRY(group_job_plan(c, B, q, pj, group_stride, false, gj));
     bool flat_only = false;   // some query has neither groups nor facets: its hits are oc_search_q_sorted's, which needs limit >= 1
     for (uint32_t b = 0; b < B; b++) {
-        const oc_group_by *g = q[b].groups;
-        if (!g) {
-            const bool flat = !(fj && fj->q_off[b + 1] > fj->q_off[b]);
-            if (flat && p->q_params && p->q_params[b].limit == 0)
-                return fail(OC_ERR_INVALID, "q_params[%u]: limit must be >= 1 when the query has no groups%s", b, fj ? " and no facets" : "");
-            flat_only = flat_only || flat;
-            continue;
-        }
-        if (g->ctx != c) return fail(OC_ERR_INVALID, "group_by of query %u belongs to another ctx", b);
-        const uint32_t m = q[b].max_results;
-        if (m > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "query %u: max_results %u > %u", b, m, OC_MAX_TOPK);
-        const bool active = pj.splice && pj.cnt[b] > 0;
-        if (active && 2 * m > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "query %u: pins: 2 x max_results %u > %u", b, 2 * m, OC_MAX_TOPK);
-        const uint64_t need = active ? 2ull * m + pj.cnt[b] : m;
-        if (group_stride < need)
-            return fail(OC_ERR_INVALID, "query %u: group_stride %u < %llu", b, group_stride, (unsigned long long)need);
-        uint32_t h = 0;
-        while (h < gj.h.size() && gj.h[h] != g) h++;
-        if (h == gj.h.size()) gj.h.push_back(const_cast<oc_group_by *>(g));   // only its per-call row map is refreshed, under the ctx lock
-        gj.q_h[b] = h; gj.q_m[b] = m; gj.q_row[b] = (uint32_t)rows;   // refused below past 2^31 rows
-        rows += g->n_groups;
+        if (q[b].groups) continue;
+        const bool flat = !(fj && fj->q_off[b + 1] > fj->q_off[b]);
+        if (flat && p->q_params && p->q_params[b].limit == 0)
+            return fail(OC_ERR_INVALID, "q_params[%u]: limit must be >= 1 when the query has no groups%s", b, fj ? " and no facets" : "");
+        flat_only = flat_only || flat;
     }
     if (flat_only && p->limit == 0) return fail(OC_ERR_INVALID, "limit must be >= 1 when a query has no groups%s", fj ? " and no facets" : "");
-    // the work list is a 1-D grid of (query, group) items
-    if (rows > 0x7fffffffull) return fail(OC_ERR_UNSUPPORTED, "groups: %llu (query, group) rows >= 2^31", (unsigned long long)rows);
-    if (rows && (!out_group_n || (group_stride && (!out_group_doc_ids || !out_group_scores)))) return fail(OC_ERR_INVALID, "NULL group output");
-    gj.rows = (uint32_t)rows; gj.stride = group_stride;
+    if (gj.rows && (!out_group_n || (group_stride && (!out_group_doc_ids || !out_group_scores)))) return fail(OC_ERR_INVALID, "NULL group output");
+    gj.stride = group_stride;
     gj.out_doc = out_group_doc_ids; gj.out_score = out_group_scores; gj.out_n = out_group_n; gj.out_values = out_group_sort_values;
     SearchReq r(p, out_doc_ids, out_scores, out_n, out_count);
     r.out_sort_values = out_sort_values; r.fj = fj; r.gj = &gj; r.pj = &pj;
@@ -5368,9 +5392,11 @@ extern "C" int oc_search_q_sorted(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_
                        out_pin_present);
 }
 
-// The sub-batch `sub` of p that oc_search_q_facets re-scores for the facets of its filtered queries: their vectors and
-// token CSR, their q_params entries, without groups, sorts or pins (facets_unfiltered drops the filters).
+// The pass that re-scores the sub-batch `sub` of p's filtered queries for their facets (counts fj, rows: places in sub):
+// q holds their vectors and token CSR and their q_params entries, without filters, groups, sorts or pins.
 struct FacetSubBatch {
+    FacetJob fj;
+    std::vector<uint32_t> sub;
     oc_search_params q;
     std::vector<float> vecs;
     std::vector<uint32_t> q_tok{0}, tok_term{0}, t_field, t_id;
@@ -5381,6 +5407,7 @@ static void facet_sub_batch(const oc_search_params *p, const oc_emb *emb, const 
     const uint32_t S = (uint32_t)sub.size();
     oc_search_params &q = sb.q;
     q = *p;
+    drop_filters(q);
     q.n_queries = S;
     std::vector<float> &vecs = sb.vecs, &t_weight = sb.t_weight;
     std::vector<uint32_t> &q_tok = sb.q_tok, &tok_term = sb.tok_term, &t_field = sb.t_field, &t_id = sb.t_id;
@@ -5423,6 +5450,21 @@ static void facet_sub_batch(const oc_search_params *p, const oc_emb *emb, const 
         q.term_field = t_field.data(); q.term_id = t_id.data(); q.term_weight = t_weight.data();
     }
 }
+// Splits the counts (query, request, output slot) of items: an unfiltered query's go to mj, on the main pass, a filtered
+// query's to sb, whose sub-batch takes those queries in the order of their first item.
+static void facet_split(const oc_search_params *p, const oc_emb *emb, oc_facets *fc, const oc_facet_req *reqs,
+                        const std::vector<uint3> &items, FacetJob &mj, FacetSubBatch &sb) {
+    mj.fc = sb.fj.fc = fc; mj.reqs = sb.fj.reqs = reqs;
+    sb.fj.hits_optional = true;
+    std::vector<uint32_t> sub_of(p->n_queries, 0xffffffffu);
+    for (const uint3 &it : items) {
+        const bool filtered = facet_filtered(p, it.x);
+        if (filtered && sub_of[it.x] == 0xffffffffu) { sub_of[it.x] = (uint32_t)sb.sub.size(); sb.sub.push_back(it.x); }
+        FacetJob &j = filtered ? sb.fj : mj;
+        j.q.push_back(filtered ? sub_of[it.x] : it.x); j.r.push_back(it.y); j.o.push_back(it.z);
+    }
+    if (!sb.sub.empty()) facet_sub_batch(p, emb, sb.sub, sb);
+}
 
 // ------------------------------------------------------------------------------------ one call over the indexes (index_merge.cuh)
 static bool same_f32(float a, float b) { return memcmp(&a, &b, 4) == 0; }
@@ -5456,7 +5498,6 @@ static void timing_add(oc_timing &t, const oc_timing &a) {
 struct MiGroups {
     uint32_t rows = 0, gtop = 0, sets = 0;   // gtop: the largest depth of a per-index list, also the merge's largest take
     std::vector<GroupJob> gj;              // [n_idx]
-    std::vector<uint8_t> on;               // [n_idx] the index adds groups to some query
     std::vector<uint32_t> src_g;           // source tables, concatenated
     std::vector<GroupHandle> set_h;        // [set][n_idx]
     std::vector<GroupSpan> spans;          // one per query with collection groups
@@ -5472,47 +5513,29 @@ static int mi_groups_plan(oc_ctx *c, uint32_t ni, uint32_t B, const oc_index_ext
     if (!any) return OC_OK;
     if (!q_n_keys || !q_max_results) return fail(OC_ERR_INVALID, "groups: NULL q_n_keys / q_max_results");
     mg.gj.resize(ni);
-    mg.on.assign(ni, 0);
     mg.q_lrow.assign(size_t(ni) * B, 0);
     uint64_t rows = 0;
     for (uint32_t b = 0; b < B; b++) {
-        const uint32_t m = q_max_results[b];
         if (!q_n_keys[b]) continue;
-        if (m > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "query %u: max_results %u > %u", b, m, OC_MAX_TOPK);
-        if (q_active[b] && 2 * m > OC_MAX_TOPK) return fail(OC_ERR_UNSUPPORTED, "query %u: pins: 2 x max_results %u > %u", b, 2 * m, OC_MAX_TOPK);
-        const uint64_t need = q_active[b] ? 2ull * m + pj_all.cnt[b] : m;
-        if (group_stride < need) return fail(OC_ERR_INVALID, "query %u: group_stride %u < %llu", b, group_stride, (unsigned long long)need);
+        uint32_t depth = 0;
+        OCTRY(group_depth(b, q_max_results[b], pj_all, group_stride, depth));
         rows += q_n_keys[b];
-        mg.gtop = std::max(mg.gtop, m * (q_active[b] ? 2u : 1u));
+        mg.gtop = std::max(mg.gtop, depth);
     }
     if (rows > 0x7fffffffull) return fail(OC_ERR_UNSUPPORTED, "groups: %llu collection group rows >= 2^31", (unsigned long long)rows);
     mg.rows = (uint32_t)rows;
     // each index's GroupJob, with the depth of an active query although its own pins do not apply
+    std::vector<oc_group_req> req(B);
     for (uint32_t i = 0; i < ni; i++) {
         GroupJob &gj = mg.gj[i];
-        gj.q_h.assign(B, GROUP_NONE); gj.q_m.assign(B, 0); gj.q_row.assign(B, 0);
+        const oc_index_extras *e = ex ? &ex[i] : nullptr;
+        if (e && e->q_groups && !e->q_group_keys) return fail(OC_ERR_INVALID, "index %u: q_groups without q_group_keys", i);
+        for (uint32_t b = 0; b < B; b++) req[b] = oc_group_req{e && e->q_groups ? e->q_groups[b] : nullptr, q_max_results[b], oc_sort{}};
+        if (const int rc = group_job_plan(c, B, req.data(), pj_all, group_stride, true, gj))
+            return fail(rc, "index %u: %s", i, std::string(g_err).c_str());
         gj.keep_top = true;
         gj.q_deep = q_active;
-        const oc_index_extras *e = ex ? &ex[i] : nullptr;
-        if (!e || !e->q_groups) continue;
-        if (!e->q_group_keys) return fail(OC_ERR_INVALID, "index %u: q_groups without q_group_keys", i);
-        uint64_t lrows = 0;
-        for (uint32_t b = 0; b < B; b++) {
-            const oc_group_by *g = e->q_groups[b];
-            if (!g) continue;
-            if (g->ctx != c) return fail(OC_ERR_INVALID, "index %u: group_by of query %u belongs to another ctx", i, b);
-            if (g->n_groups && !e->q_group_keys[b]) return fail(OC_ERR_INVALID, "index %u: query %u has groups and no key map", i, b);
-            if (g->n_groups == 0) continue;
-            uint32_t h = 0;
-            while (h < gj.h.size() && gj.h[h] != g) h++;
-            if (h == gj.h.size()) gj.h.push_back(const_cast<oc_group_by *>(g));
-            gj.q_h[b] = h; gj.q_m[b] = q_max_results[b]; gj.q_row[b] = (uint32_t)lrows;
-            mg.q_lrow[size_t(i) * B + b] = (uint32_t)lrows;
-            lrows += g->n_groups;
-            mg.on[i] = 1;
-        }
-        if (lrows > 0x7fffffffull) return fail(OC_ERR_UNSUPPORTED, "index %u: %llu group rows >= 2^31", i, (unsigned long long)lrows);
-        gj.rows = (uint32_t)lrows;
+        std::copy(gj.q_row.begin(), gj.q_row.end(), mg.q_lrow.begin() + size_t(i) * B);
     }
     // the source tables: one per distinct (handle, key map) combination; a query's span points at its combination
     std::map<std::vector<uintptr_t>, std::pair<uint32_t, uint32_t>> sets;   // combination -> (table offset, set)
@@ -5524,6 +5547,7 @@ static int mi_groups_plan(oc_ctx *c, uint32_t ni, uint32_t B, const oc_index_ext
         for (uint32_t i = 0; i < ni; i++) {
             const oc_group_by *g = ex && ex[i].q_groups ? ex[i].q_groups[b] : nullptr;
             if (!g || !g->n_groups) continue;
+            if (!ex[i].q_group_keys[b]) return fail(OC_ERR_INVALID, "index %u: query %u has groups and no key map", i, b);
             key[1 + 2 * i] = uintptr_t(g);
             key[2 + 2 * i] = uintptr_t(ex[i].q_group_keys[b]);
         }
@@ -5638,42 +5662,25 @@ extern "C" int oc_search_indexes_ex(oc_ctx *c, uint32_t n_indexes, const oc_inde
             if (off[b + 1] < off[b]) return fail(OC_ERR_INVALID, "q_facet_offsets is not monotone at query %u", b);
     if (any_facets && !off) return fail(OC_ERR_INVALID, "facet requests without q_facet_offsets");
     if (n_slots && !out_facet_counts) return fail(OC_ERR_INVALID, "NULL facet counts");
-    std::vector<FacetJob> fjm(n_indexes), fjs(n_indexes);
-    std::vector<std::vector<uint32_t>> f_sub(n_indexes);
-    std::vector<std::unique_ptr<FacetSubBatch>> f_sb(n_indexes);
+    std::vector<FacetJob> fjm(n_indexes);
+    std::vector<FacetSubBatch> fsb(n_indexes);
     for (uint32_t i = 0; any_facets && i < n_indexes; i++) {
         const oc_index_extras &e = ex[i];
         if (!e.facets || !e.n_facet_reqs) continue;
         if (e.facets->ctx != c) return fail(OC_ERR_INVALID, "index %u: facets belong to another ctx", i);
         if (!e.facet_reqs || !e.facet_slots) return fail(OC_ERR_INVALID, "index %u: NULL facet_reqs / facet_slots", i);
         OCTRY(oc_facets_check(e.facets, e.facet_reqs, e.n_facet_reqs));
-        const oc_search_params *p = ix[i].p;
         std::vector<uint8_t> seen(n_slots, 0);
-        std::vector<uint32_t> sub_of(B, 0xffffffffu);
-        FacetJob &mj = fjm[i], &fj = fjs[i];
-        mj.fc = fj.fc = e.facets; mj.reqs = fj.reqs = e.facet_reqs;
-        fj.hits_optional = true;
+        std::vector<uint3> items;
         for (uint32_t r = 0; r < e.n_facet_reqs; r++) {
             const uint32_t s = e.facet_slots[r];
             if (s < s0 || s - s0 >= n_slots) return fail(OC_ERR_INVALID, "index %u: facet request %u: slot %u outside [%u, %u)", i, r, s, s0, s0 + n_slots);
             if (seen[s - s0]) return fail(OC_ERR_INVALID, "index %u: two facet requests on slot %u", i, s);
             seen[s - s0] = 1;
             const uint32_t b = uint32_t(std::upper_bound(off, off + B + 1, s) - off) - 1;   // the query whose range holds s
-            const bool filtered = p->filter || p->filter_bits || (p->q_filters && p->q_filters[b]) ||
-                                  (p->q_where && p->q_where->q_node_offsets && p->q_where->q_node_offsets[b + 1] > p->q_where->q_node_offsets[b]);
-            uint32_t row = b;
-            if (filtered) {
-                if (sub_of[b] == 0xffffffffu) { sub_of[b] = (uint32_t)f_sub[i].size(); f_sub[i].push_back(b); }
-                row = sub_of[b];
-            }
-            FacetJob &j = filtered ? fj : mj;
-            j.q.push_back(row); j.r.push_back(r); j.o.push_back(s - s0);
+            items.push_back(make_uint3(b, r, s - s0));
         }
-        if (!f_sub[i].empty()) {
-            f_sb[i].reset(new FacetSubBatch());
-            facet_sub_batch(p, ix[i].emb, f_sub[i], *f_sb[i]);
-            drop_filters(f_sb[i]->q);
-        }
+        facet_split(ix[i].p, ix[i].emb, e.facets, e.facet_reqs, items, fjm[i], fsb[i]);
     }
     // every index's calls, checked before anything runs
     std::vector<oc_search_params> ps(n_indexes);
@@ -5693,15 +5700,15 @@ extern "C" int oc_search_indexes_ex(oc_ctx *c, uint32_t n_indexes, const oc_inde
         SearchReq &r = *reqs.back();
         r.pj = with_pj ? &pjs[i] : nullptr;
         r.sj = any_sorted ? &sjs[i] : nullptr;
-        r.gj = groups && mg.on[i] ? &mg.gj[i] : nullptr;
+        r.gj = groups && mg.gj[i].rows ? &mg.gj[i] : nullptr;
         r.fj = fjm[i].q.empty() ? nullptr : &fjm[i];
         r.q_filters_ok = r.q_params_ok = true;
         calls.emplace_back(new SearchCall(c, ix[i].emb, ix[i].str, r));
         OCTRY(search_check(*calls.back()));
-        if (f_sb[i]) {   // the unfiltered facet pass of the index's filtered queries
-            reqs.emplace_back(new SearchReq(&f_sb[i]->q, out_doc_ids, out_scores, out_n, out_count));
+        if (!fsb[i].sub.empty()) {   // the unfiltered facet pass of the index's filtered queries
+            reqs.emplace_back(new SearchReq(&fsb[i].q, out_doc_ids, out_scores, out_n, out_count));
             SearchReq &fr = *reqs.back();
-            fr.fj = &fjs[i];
+            fr.fj = &fsb[i].fj;
             fr.q_filters_ok = fr.q_params_ok = true;
             fcalls[i].reset(new SearchCall(c, ix[i].emb, ix[i].str, fr));
             OCTRY(search_check(*fcalls[i]));
@@ -5744,7 +5751,7 @@ extern "C" int oc_search_indexes_ex(oc_ctx *c, uint32_t n_indexes, const oc_inde
     uint8_t *dout = c->mi_out.as<uint8_t>();
     unsigned long long *d_fc = reinterpret_cast<unsigned long long *>(dout + o_fc);
     if (n_slots) CU(cudaMemsetAsync(d_fc, 0, size_t(n_slots) * 8, c->stream));
-    for (uint32_t i = 0; i < n_indexes; i++) { fjm[i].d_out = d_fc; fjs[i].d_out = d_fc; }
+    for (uint32_t i = 0; i < n_indexes; i++) { fjm[i].d_out = d_fc; fsb[i].fj.d_out = d_fc; }
     // where each index's hits find their sort values: the handles' rank values on the device (built once per handle)
     std::vector<ImSortSrc> src(any_sorted ? size_t(n_indexes) * B : 0, ImSortSrc{nullptr, nullptr, 0});
     for (uint32_t i = 0; any_sorted && i < n_indexes; i++) {
@@ -5965,28 +5972,18 @@ extern "C" int oc_search_q_facets(oc_ctx *c, oc_emb *emb, oc_str *str, const oc_
         none.assign(B, oc_group_req{nullptr, 0, oc_sort{nullptr, OC_SORT_ASC}});
         q_groups = none.data();
     }
-    // which queries count on the main pass, which are re-scored without their filter
-    const bool all_filtered = p->filter || p->filter_bits;
-    FacetJob mj, fj;
-    mj.fc = fj.fc = facets; mj.reqs = fj.reqs = facet_reqs; mj.out_counts = fj.out_counts = out_facet_counts;
+    std::vector<uint3> items;
+    for (uint32_t b = 0; b < B; b++)
+        for (uint32_t i = off[b]; i < off[b + 1]; i++) items.push_back(make_uint3(b, i, i));
+    FacetJob mj;
+    FacetSubBatch sb;
+    facet_split(p, emb, facets, facet_reqs, items, mj, sb);
+    mj.out_counts = sb.fj.out_counts = out_facet_counts;
     mj.q_off = off;
-    fj.hits_optional = true;
-    std::vector<uint32_t> sub;
-    for (uint32_t b = 0; b < B; b++) {
-        if (off[b + 1] == off[b]) continue;
-        const bool filtered = all_filtered || (p->q_filters && p->q_filters[b]) ||
-                              (p->q_where && p->q_where->q_node_offsets && p->q_where->q_node_offsets[b + 1] > p->q_where->q_node_offsets[b]);
-        if (filtered) sub.push_back(b);
-        FacetJob &j = filtered ? fj : mj;
-        const uint32_t row = filtered ? (uint32_t)sub.size() - 1 : b;
-        for (uint32_t i = off[b]; i < off[b + 1]; i++) { j.q.push_back(row); j.r.push_back(i); j.o.push_back(i); }
-    }
     OCTRY(groups_impl(c, emb, str, p, q_groups, pins, group_stride, true, out_doc_ids, out_scores, out_sort_values, out_n, out_count,
                       out_pin_scores, out_pin_present, out_group_doc_ids, out_group_scores, out_group_sort_values, out_group_n, &mj));
-    if (sub.empty()) return OC_OK;
-    FacetSubBatch sb;
-    facet_sub_batch(p, emb, sub, sb);
-    return facets_unfiltered(c, emb, str, &sb.q, fj, true);
+    if (sb.sub.empty()) return OC_OK;
+    return facets_unfiltered(c, emb, str, &sb.q, sb.fj, true);
 }
 
 // ------------------------------------------------------------------------------------ geopoint where-filter leaves (geo.cuh)

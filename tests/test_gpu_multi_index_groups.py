@@ -475,3 +475,20 @@ def test_refusals_write_nothing(gpu_ctx, cols):
         ogb.close(); ost.close()
     finally:
         other.close()
+
+
+def test_over_deep_pinned_groups_refused_alike(gpu_ctx, cols):
+    """An active pinned query whose group lists would be 2 x max_results > OC_MAX_TOPK deep: oc_search_indexes_ex refuses
+    it with the code and message oc_search_q_groups gives for one of its indexes."""
+    col = cols(2, "mod")
+    p = ob.TokenScoreParams(mode=MODE_FULLTEXT, limit_hint=5)
+    gbs = col.group_by(["cat"])
+    promote, part = [[(1, 0)]] * B, col.parts[0]
+    calls = (lambda: E.search_indexes_arrays(gpu_ctx, col.parts, p, promote=promote, groups=[(gbs, 600)] * B, group_stride=2000),
+             lambda: E.search_q_groups_arrays(part.tsc, dataclasses.replace(p, **dict(part.fields or {})), [(gbs[0], 600)] * B,
+                                              promote, part.texts, part.q_vecs, group_stride=2000))
+    for call in calls:
+        with pytest.raises(ob.OcError) as e:
+            call()
+        assert e.value.code == -4   # OC_ERR_UNSUPPORTED
+        assert "query 0: pins: 2 x max_results 1200 > 1024" in _lib.lib().oc_last_error().decode()
